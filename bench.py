@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 cascaded-regression engine.
+"""bench.py -- headline benchmark of the H100 cascaded-regression engine.
 
 Metric (BASELINE.json): faces/sec, RCR 22-landmark detect with the reference's pre-trained
 face_landmarks_model_rcr_22.bin on 640x480 synthetic 8UC1 frames, batched, one face box per frame
 (config 3, "configs[2]").  A "step" = one pass of the detect cascade (4 levels: HOG -> feature x weight
 GEMM -> IED-scaled update) over one batch of B frames.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl ours|reference] [--dump-outputs DIR]
 
   value        whole-job faces/s with frames + initial landmarks already resident in HBM
   e2e          the same through the reference-facing call detection_model::detect(image, facebox)
@@ -18,6 +18,8 @@ GEMM -> IED-scaled update) over one batch of B frames.
   train        (N=1 only, extra) regressor-train seconds of a reduced RCR training config
 
 --impl reference times the CPU path alone (rank 0), same metric/config.
+--dump-outputs DIR writes what the timed path computed in its last step (landmarks, trained weights) as DIR/<name>.npy;
+the inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -50,7 +52,7 @@ def measured_peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback: H100 SXM HBM3 specification (3.35 TB/s)"
 
 
 def synth_boxes(count, seed):
@@ -90,7 +92,7 @@ def synth_frames_numpy(count, seed):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -195,10 +197,22 @@ def run_reference(args):
     print(json.dumps(line))
 
 
-# static profile facts about the level-0 HOG kernel: NOT measured in the bench run, quoted from the committed ncu summary
-HOG_STATIC_PROFILE = {"source": "profiles/r02_summary.md section 2 (one `ncu --set full` capture of hog_patch_kernel<4,5,11>, 2048 faces)",
-                      "dram_bytes_per_face": (170.898432e6 + 52.981504e6) / 2048, "issue_slots_busy_pct": 61.5,
-                      "warp_instructions_per_patch": 16166, "shared_wavefronts_pct_of_lsu_path": 76}
+DUMP_BYTES = 63 << 20      # --dump-outputs writes at most 64 MB in all (npy headers included)
+
+
+def dump_outputs(dirname, arrays):
+    """Writes name -> array as DIR/<name>.npy (float32, or float64 when the array is).  When the arrays exceed the budget
+    together, each keeps the same fraction of its rows, chosen by a fixed seed, so two runs write the same sample."""
+    os.makedirs(dirname, exist_ok=True)
+    arrs = {k: np.ascontiguousarray(v, dtype=np.float64 if v.dtype == np.float64 else np.float32) for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrs.values())
+    frac = min(1.0, DUMP_BYTES / total) if total else 1.0
+    for name, a in arrs.items():
+        if frac < 1.0 and a.ndim >= 1 and a.shape[0] > 1:
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], max(1, int(a.shape[0] * frac)), replace=False))
+            a = a[rows]
+        np.save(os.path.join(dirname, name + ".npy"), a)
+
 
 TRAIN_CFGS = {
     # SURVEY 8d config 4 / BASELINE configs[3]
@@ -266,16 +280,17 @@ def synth_train_landmarks(sd, mean, cfg, b, e):
 
 
 def syrk_executed_flops(n, D, M, passes=3):
-    """MMA flops the Gram kernel executes: every 128 x 256 tile that touches the upper triangle of [AtA | Atb], three TF32 passes."""
-    TI, TJ = (D + 127) // 128, (D + M + 255) // 256
-    tiles = sum(1 for ti in range(TI) for tj in range(TJ) if tj * 256 + 255 >= ti * 128)
-    return passes * 2.0 * n * tiles * 128 * 256
+    """MMA flops the Gram kernel executes: every 128 x 128 tile that touches the upper triangle of [AtA | Atb], three TF32 passes."""
+    TI, TJ = (D + 127) // 128, (D + M + 127) // 128
+    tiles = sum(1 for ti in range(TI) for tj in range(TJ) if tj * 128 + 127 >= ti * 128)
+    return passes * 2.0 * n * tiles * 128 * 128
 
 
 def run_train(sd, ctx, model, world, rank, dev, barrier, max_over_ranks, comm, cfg=None, steps=1, warmup=1, e2e=False, distributed_solve=None,
-              solver="cholesky"):
+              solver="cholesky", outputs=None):
     """Regressor-train seconds (all S levels: HOG + targets + Gram + exchange + solve + update), strong scaling: the SAME global
-    training set for every number of ranks (samples are generated by global index)."""
+    training set for every number of ranks (samples are generated by global index).  outputs (a dict) receives the trained
+    weights of every level and this rank's final landmarks of the last timed step."""
     import torch
     from superviseddescent_b200 import parallel
     cfg = cfg or TRAIN_CFG
@@ -320,16 +335,20 @@ def run_train(sd, ctx, model, world, rank, dev, barrier, max_over_ranks, comm, c
     res0, res1 = float(torch.sqrt(num[0] / num[2])), float(torch.sqrt(num[1] / num[2]))
     # the trained model's fingerprint: identical data for every N, so these agree across N up to summation order
     checksum = [float(r.x.double().abs().sum()) for r in sdo.regressors]
+    if outputs is not None:
+        for k, r in enumerate(sdo.regressors):
+            outputs[f"train_weights_level{k}"] = r.x.cpu().numpy()
+        outputs["train_landmarks"] = xf.cpu().numpy()
     out = {"metric": "regressor train sec (RCR, all cascade levels)", "value": secs, "unit": "s", "higher_is_better": False, "scaling": "strong",
            "n_gpus": world, "steps": steps, "warmup": max(warmup, 1), "ms_per_step": secs * 1e3, "dtype": "f32", "data": "synthetic", "vs_baseline": None,
            "config": {"workload": cfg["name"], "samples_global": cfg["n"], "samples_this_rank": e - b, "feature_dim": D, "levels": S,
-                      "landmarks": L, "l2": f"per-level operands ({(e - b) * D * 4 / 1e9:.2f} GB of features, {D * (D + 2 * L) * 4 / 1e9:.2f} GB Gram) exceed the 126 MB L2",
+                      "landmarks": L, "l2": f"per-level operands ({(e - b) * D * 4 / 1e9:.2f} GB of features, {D * (D + 2 * L) * 4 / 1e9:.2f} GB Gram) exceed the 50 MB L2",
                       "parallelism": (f"samples sharded over {world} GPU(s); per level one exchange of the upper row bands of [AtA|Atb] "
                                       f"({parallel.band_offsets(D, (D + 2 * L + 3) // 4 * 4)[-1] * 4 / 1e9:.2f} of {D * (D + 2 * L) * 4 / 1e9:.2f} GB): "
                                       + ("all-reduce + conjugate gradients shared by the ranks (one all-reduce of 2L x D floats per iteration)" if ds == "cg"
                                          else "reduce to the block-row-cyclic owners + distributed blocked Cholesky (panel broadcast)" if ds
                                          else "all-reduce + replicated solve" if world > 1 else "single GPU")),
-                      "solver": ("conjugate gradients (tcgen05 3xTF32 products)" if (ds == "cg" or solver == "cg") else "blocked Cholesky"),
+                      "solver": ("conjugate gradients (wgmma 3xTF32 products)" if (ds == "cg" or solver == "cg") else "blocked Cholesky"),
                       "solver_iterations_last_level": ctx.solver_iterations()},
            "gpu_launches": launches,
            "train_residual": {"before": res0, "after": res1},
@@ -341,22 +360,12 @@ def run_train(sd, ctx, model, world, rank, dev, barrier, max_over_ranks, comm, c
     alg = n_loc * D * (D + 1.0) + 2.0 * n_loc * D * 2 * L
     t = solver_ms["At * A"] * 1e-3
     if t > 0:
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        peak = float(peaks.get("bf16_tflops_sustained", 0) or 0) or 1500.0
-        out["roofline"] = {"kernel": "syrk_tc2_kernel ([AtA|Atb] of the last level, tcgen05 3xTF32)", "bound": "tensor", "achieved": alg / t / 1e12, "peak": peak,
-                           "unit": "TFLOP/s", "frac": alg / t / 1e12 / peak,
-                           # DRAM bytes of this launch from the committed ncu capture: only valid for the shape it was taken on
-                           "traffic": 8569163000 + 584547000 if (world == 1 and cfg is TRAIN_CFGS["train"]) else None,
-                           "traffic_source": "profiles/r02_summary.md section 3 (ncu --set full capture of this launch shape on one GPU), not this run",
-                           "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (dense bf16; the kernel runs kind::tf32 at half that rate, three passes)" if peaks else "fallback 1500 (B200_PROFILING.md)",
+        peak = 494.7       # dense TF32 tensor-core peak of the H100 SXM (specification); the kernel runs three TF32 passes
+        out["roofline"] = {"kernel": "syrk_wgmma_kernel ([AtA|Atb] of the last level, wgmma 3xTF32)", "bound": "tensor", "achieved": alg / t / 1e12, "peak": peak,
+                           "unit": "TFLOP/s", "frac": alg / t / 1e12 / peak, "traffic": None,
+                           "peak_source": "H100 SXM dense TF32 specification (494.7 TFLOP/s)",
                            "ms_per_launch": solver_ms["At * A"], "algorithmic_flops_per_launch": alg,
-                           "executed_tf32_tflops": syrk_executed_flops(n_loc, D, 2 * L) / t / 1e12,
-                           "static_profile": {"source": "profiles/r02_summary.md section 3 (ncu --set full capture of the config-4 Gram launch on one GPU: tensor-pipe activity and the DRAM bytes reported as traffic)",
-                                              "tensor_pipe_active_pct": 84.15}}
+                           "executed_tf32_tflops": syrk_executed_flops(n_loc, D, 2 * L) / t / 1e12}
     out["algorithmic_tflop"] = {"gram_syrk": S * (cfg["n"] * D * (D + 1.0) + 2.0 * cfg["n"] * D * 2 * L) / 1e12, "cholesky_and_solve": S * (D ** 3 / 3.0 + 2.0 * D * D * 2 * L) / 1e12}
     if e2e:
         # the same run from HOST buffers: crops and landmark rows in pinned memory, uploads inside the timed region, the trained
@@ -452,8 +461,9 @@ def run_train_workload(args, sd, ctx, model, world, rank, local, dev, barrier, m
     if rank == 0:
         sampler.start()
     ds = {"auto": None, "replicated": False, "distributed": True, "cg": "cg"}[args.solve]
+    outputs = {}
     line = run_train(sd, ctx, model, world, rank, dev, barrier, max_over_ranks, comm, cfg, steps=args.steps, warmup=args.warmup, e2e=True,
-                     distributed_solve=ds, solver="cg" if args.solve == "cg" else "cholesky")
+                     distributed_solve=ds, solver="cg" if args.solve == "cg" else "cholesky", outputs=outputs)
     clocks = sampler.stop() if rank == 0 else None
     if rank != 0:
         return
@@ -472,6 +482,8 @@ def run_train_workload(args, sd, ctx, model, world, rank, local, dev, barrier, m
                                               + f"; x{S} levels (extrapolated); {lvl['kind']}"}
         except Exception as ex:
             line["cpu_baseline"] = {"error": repr(ex)[:200]}
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, outputs)
     print(json.dumps(line))
 
 
@@ -542,6 +554,7 @@ def run_ours(args):
     barrier()
     ms = max_over_ranks(e0.elapsed_time(e1))
     launches = ctx.launches() - l0
+    outputs = {"landmarks": out.cpu().numpy()}             # (B, 2L) of the last timed step
     value = world * B * args.steps / (ms * 1e-3)
 
     # ---------------- end to end through the host-buffer call ----------------
@@ -575,7 +588,7 @@ def run_ours(args):
     for _ in range(3):
         hog0()
     torch.cuda.synchronize()
-    reps = max(5, args.steps)
+    reps = args.steps
     e0.record()
     for _ in range(reps):
         hog0()
@@ -592,23 +605,20 @@ def run_ours(args):
     alg_flops = float(B * L * fs0 * fs0 * (24 + 4 * hp0.num_bins))
     peak, peak_src = measured_peaks()
     achieved = alg_bytes / (hog_ms * 1e-3) / 1e9
-    fp32_peak = 148 * 128 * 2 * 1.965e9 / 1e12      # 148 SMs x 128 FMA lanes x 2 flop x boost clock (B200_PROFILING.md)
+    fp32_peak = 132 * 128 * 2 * 1.98e9 / 1e12       # H100 SXM: 132 SMs x 128 FMA lanes x 2 flop x 1.98 GHz boost clock
     roofline = {"kernel": f"hog_patch_kernel<{hp0.num_bins}> (cascade level 0, fs={fs0})",
                 "bound": "issue", "bound_note": "instruction-issue / fp32-ALU + shared-memory bound (~40 flop per algorithmic byte, SURVEY 8d), not HBM; "
                                                  "achieved/peak/frac are the HBM figures the contract asks for, frac_binding is the fp32 one",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src, "ms_per_launch": hog_ms,
-                # DRAM bytes per launch from the committed `ncu --set full` capture (2048 faces), scaled per face: a capture, not this run
-                "traffic": HOG_STATIC_PROFILE["dram_bytes_per_face"] * B, "traffic_source": HOG_STATIC_PROFILE["source"],
-                "algorithmic_bytes_per_launch": alg_bytes,
+                "traffic": None, "algorithmic_bytes_per_launch": alg_bytes,
                 "achieved_fp32_tflops": alg_flops / (hog_ms * 1e-3) / 1e12, "fp32_peak_tflops": fp32_peak,
-                "frac_binding": alg_flops / (hog_ms * 1e-3) / 1e12 / fp32_peak,
-                "static_profile": dict(HOG_STATIC_PROFILE, dram_bytes_this_batch=HOG_STATIC_PROFILE["dram_bytes_per_face"] * B,
-                                       note="quoted from a committed ncu capture, not measured in this run")}
+                "frac_binding": alg_flops / (hog_ms * 1e-3) / 1e12 / fp32_peak}
 
     train = None
     if not args.no_train:
         try:
-            train = run_train(sd, ctx, model, world, rank, dev, barrier, max_over_ranks, comm)
+            train = run_train(sd, ctx, model, world, rank, dev, barrier, max_over_ranks, comm, steps=args.steps, warmup=args.warmup,
+                              outputs=outputs)
         except Exception as ex:   # the headline line must still be printed
             train = {"error": repr(ex)[:300]}
     if comm is not None:
@@ -623,7 +633,7 @@ def run_ours(args):
         "config": {"workload": "configs[2]: RCR 22-landmark detect, pre-trained face_landmarks_model_rcr_22.bin, 640x480 8UC1 synthetic frames, batched",
                    "frames_per_gpu": B, "global_batch": world * B, "cascade_levels": model.num_levels, "landmarks": L,
                    "parallelism": f"face-batch sharded over {world} GPU(s), no collective",
-                   "l2": f"inputs ({B * W_IMG * H_IMG / 1e6:.0f} MB of frames per GPU) exceed the 126 MB L2"},
+                   "l2": f"inputs ({B * W_IMG * H_IMG / 1e6:.0f} MB of frames per GPU) exceed the 50 MB L2"},
         "e2e": {"value": e2e, "unit": "faces/s", "h2d_bytes_per_step": int(B * W_IMG * H_IMG + B * 2 * L * 4), "d2h_bytes_per_step": int(B * 2 * L * 4),
                 "ms_per_step": ms_e2e / args.steps, "api": "detection_model.detect_batch (sd_detect_batch_host), pinned host frames",
                 "note": "h2d_bytes_per_step counts the host frames handed to the call; the engine's region-of-interest route reads only "
@@ -654,14 +664,17 @@ def run_ours(args):
                                 "single_thread_value": r1}
     if world > 1:
         dist.destroy_process_group()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, outputs)
     print(json.dumps(line))
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=None)
-    ap.add_argument("--warmup", type=int, default=None)
+    ap.add_argument("--steps", type=int, default=None,
+                    help="timed steps of every timed measurement (the headline, e2e, roofline and the extra train leg)")
+    ap.add_argument("--warmup", type=int, default=None, help="untimed steps before each of them (at least one for train)")
     ap.add_argument("--workload", default="detect", choices=["detect", "train", "train5"],
                     help="detect = configs[2] (the default headline line); train = configs[3] and train5 = configs[4]: regressor-train "
                          "seconds as a first-class line (strong scaling over --gpus)")
@@ -671,6 +684,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-train", action="store_true", help="skip the extra regressor-train measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step as DIR/<name>.npy (at most 64 MB in all)")
     args = ap.parse_args()
     if args.steps is None:
         args.steps = {"detect": 10, "train": 3, "train5": 1}[args.workload]

@@ -1,5 +1,5 @@
 /*
- * sd_b200.h -- C ABI of the B200-native cascaded-regression engine.
+ * sd_b200.h -- C ABI of the H100-native cascaded-regression engine.
  *
  * This is the drop-in boundary for the hot path of patrikhuber/superviseddescent
  * (HOG projection -> LinearRegressor::learn -> predict/detect cascade).  Plain C:

@@ -37,7 +37,7 @@ class Context:
 
     def __init__(self, device: int = 0):
         if not torch.cuda.is_available():
-            raise SdError(2, "no CUDA device: the B200 engine has no CPU fallback")
+            raise SdError(2, "no CUDA device: the engine has no CPU fallback")
         self.device = int(device)
         torch.cuda.set_device(self.device)
         self.stream = torch.cuda.current_stream(self.device)

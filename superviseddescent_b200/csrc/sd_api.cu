@@ -90,7 +90,7 @@ int sd_check_hog_status(sd_ctx* ctx, const char* what)
 
 extern "C" {
 
-const char* sd_version(void) { return "superviseddescent_b200 0.1 (sm_100a)"; }
+const char* sd_version(void) { return "superviseddescent_b200 0.1 (sm_90a)"; }
 
 int sd_ctx_create(int device, void* stream, sd_ctx** out)
 {

@@ -4,7 +4,7 @@
 // the CENTRED features plus lambda I.  With the reference's MatrixNorm rule lambda = 1.5 ||A^T A||_F / N is of the size of the
 // largest eigenvalues, so the matrix is very well conditioned: measured condition number 3.5 at N = 900 samples, 10.5 at 3,600
 // (it grows like N: ~30 for config 4, a few hundred for config 5).  CG then needs a few dozen iterations of
-//     Q = S P   (one skinny product with the D x D matrix: 2 D^2 2L flops, the tcgen05 TN-GEMM of sd_gram_tc.cu in its narrow
+//     Q = S P   (one skinny product with the D x D matrix: 2 D^2 2L flops, the wgmma TN-GEMM of sd_gram_tc.cu in its narrow
 //                variant: S is the 128-row operand, P the 64-column one, so the product is bound by the single read of S)
 // instead of the D^3/3 factorisation whose chain of D dependent pivots does not parallelise -- and the product shards over
 // GPUs by rows of S with one small all-reduce (2L x D floats) per iteration, which the factorisation cannot.
@@ -27,7 +27,7 @@ constexpr int CG_MAXCOLS = CG_BX * CG_G;
 // The product streams the symmetric matrix once per iteration, so it gets a copy laid out for that: strip-major,
 //     T[s][k - k0][c] = S[k][128 s + c],   k in [k0, k0 + kp) (this rank's slab of the contraction, zero rows beyond k1), c < 128
 // -- the 128 columns of one CTA's tile are contiguous, a CTA reads its strip front to back (row-major S would give it 512-byte
-// pieces 68 KB apart: measured 2.1 TB/s).  Built from the upper triangle only (S[k][j] = S[j][k] below the diagonal, transposed
+// pieces 68 KB apart).  Built from the upper triangle only (S[k][j] = S[j][k] below the diagonal, transposed
 // through shared memory); G itself is not modified.  One block per 32 x 32 tile of (k, j).
 __global__ void __launch_bounds__(256) cg_pack_kernel(const float* __restrict__ G, long long ldg, int n, int k0, int k1, int kp, float* __restrict__ T)
 {

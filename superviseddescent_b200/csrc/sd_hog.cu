@@ -467,7 +467,7 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const HogArgs a,
     //      device-generated tables (the gradient of an 8-bit patch is a pair of integers in [-255, 255]) ---------
     {
         // linear index over the interior pixels (all lanes busy); four pixels per thread in flight so that the eight table
-        // look-ups overlap (the phase was bound by their latency: profiles/r02_summary.md)
+        // look-ups overlap (the phase is bound by their latency)
         const int iw = fs - 2, npix = iw * iw;
         for (int i0 = tid; i0 < npix; i0 += 4 * kHogThreads) {
             int idx[4], gxs[4], gys[4];
@@ -768,8 +768,8 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
 #undef SD_HOG_PICK
     }
     SD_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
-    // (Measured, profiles/r02_summary.md: forcing six resident CTAs per SM with the whole shared-memory carve-out is SLOWER than
-    // five with the default split -- the orientation / modulus tables live in L1, which the larger carve-out takes away.)
+    // The default shared-memory carve-out is kept on purpose: the orientation / modulus tables live in L1, which a larger
+    // carve-out (more resident CTAs per SM) would take away.
     kern<<<(unsigned)blocks, kHogThreads, lay.total, ctx->stream>>>(a, maps);
     SD_LAUNCH_CHECK(ctx, "hog_patch_kernel");
     return SD_OK;

@@ -39,7 +39,7 @@ struct sd_ctx {
     std::string err;
     std::vector<int2> tile_scratch;       // host side of the tensor-core tile lists
     int64_t launches = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     int gram_mode = 0;
     int solver_mode = 0;           // systems with D > 256: 0 = blocked Cholesky, 1 = conjugate gradients (Cholesky if they stall)
     int cg_iterations = 0;         // of the last solve (0: the factorisation ran)

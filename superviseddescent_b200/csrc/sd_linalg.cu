@@ -754,9 +754,7 @@ __global__ void copy_block_kernel(const float* __restrict__ src, long long lds, 
 // row panel and the trailing update inside the block are small register-tiled GEMMs by all 8 warps.  Outputs:
 // U (in place in G), W = U^-1 and W^T (workspace) -- so that the panel solve U12 = U11^-T G12 and the back
 // substitution X_j = U_jj^-1 Y_j become plain GEMMs.  Blocks narrower than 128 are padded with the identity.
-// Phase timings (clock64, -DSD_PROFILE_POTRF + tools/potrf_prof.py): 369k cycles before the restructuring
-// (4 x 65k in the single-warp phases), ~120k now (load 5k, 4 x 14.6k potrf32, panels 8k, trailing 10k, W 28k, store 7k;
-// the fused rank-128 update of the look-ahead path adds ~30k).
+// -DSD_PROFILE_POTRF records clock64 phase timings of one block in sd_dbg_clk (load, potrf32 steps, panels, trailing, W, store).
 constexpr int PB = 128, PS = 32, PLD = PB + 1;
 #ifdef SD_PROFILE_POTRF
 __device__ long long sd_dbg_clk[64];
@@ -766,7 +764,7 @@ __device__ long long sd_dbg_clk[64];
 #endif
 
 // cp.async staging: all of a CTA's global->shared copies are put in flight at once (the block kernels of the
-// factorisation are latency-bound: measured 37 us per back-substitution step with plain load/store loops).
+// factorisation are latency-bound, so copies must not be issued one load/store loop iteration at a time).
 // valid == false zero-fills the destination (src-size 0; the source pointer is then only required to be mapped).
 __device__ __forceinline__ void cp_async16(float* dst_smem, const float* src, bool valid)
 {
@@ -785,15 +783,13 @@ __device__ __forceinline__ void cp_async_wait_all()
     asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
 }
 
-// Factor and invert the 32 x 32 diagonal sub-block at (k0, k0) of sA.  History (clock64 per sub-block): single warp,
-// right-looking + separate back substitution 65k cycles; single warp, left-looking with the inverse carried along 21k;
-// whole CTA, right-looking on the augmented block (below) 14.6k.  A fully unrolled register/shuffle version was no
-// faster than the first one: ~50 KB of straight-line code thrashes the instruction cache of a lone warp.
+// Factor and invert the 32 x 32 diagonal sub-block at (k0, k0) of sA, by the whole CTA rather than a single warp (the
+// single-warp variants leave most of the SM idle on a chain of dependent pivots).
 //
 // Whole CTA, right-looking on the augmented block M = [A | I]
 // (32 x 64, work copy in sM): per pivot k every thread reads the pivot row, rows k+1.. get their rank-1 update
 // (4 rows x 64 columns per pass), the scaled pivot row goes straight to its destination (U -> sA, U^-T -> sT as T).
-// One __syncthreads per pivot; ~190 cycles per pivot instead of ~660 for the single-warp left-looking version.
+// One __syncthreads per pivot.
 constexpr int MLD = 2 * PS + 1;
 constexpr int ULD = PB + 4;          // row pitch of the panel rows staged for the fused update (float4-aligned)
 __device__ __forceinline__ void potrf32_block(float* sA, float* sT, float* sM, int k0, int tid, bool& bad)
@@ -1506,7 +1502,7 @@ static int solve_gram_impl(sd_ctx* ctx, sd_comm* comm, float* d_G, int64_t ldg, 
     const bool share_norm = dist || (route == 2 && nranks > 1 && D > kLuMaxDim);
     SD_REQUIRE(ctx, !d_mu || D > kLuMaxDim, "centred features are for the factorisation route (D > 256)");
     if (reg->type == 1) {
-        nparts = D < 296 ? D : 296;                                   // 2 x 148 SMs; at most 384 partials fit the scratch
+        nparts = D < 264 ? D : 264;                                   // 2 x 132 SMs; at most 384 partials fit the scratch
         if (d_mu) {
             // s' = bias column of the centred Gram, needed entry by entry for the norm of the uncentred matrix
             double* sv0 = (double*)sd_workspace(ctx, SD_WS_BIAS, (size_t)(D + M) * sizeof(double) + (size_t)(D - 1) * (M + 1) * sizeof(float));

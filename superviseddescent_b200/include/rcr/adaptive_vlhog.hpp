@@ -1,9 +1,9 @@
-// B200 drop-in for include/rcr/adaptive_vlhog.hpp: HoGParam (:41-60) and the projection functor
+// H100 drop-in for include/rcr/adaptive_vlhog.hpp: HoGParam (:41-60) and the projection functor
 // HogTransform (:70-195).  The functor keeps the reference's constructor and call signature
 //     cv::Mat operator()(cv::Mat parameters, size_t regressorLevel, int trainingIndex = 0)
 // (one sample, used by predict(), superviseddescent.hpp:332) and adds project_device(), which the
 // optimiser uses to extract the features of ALL samples of a level with one kernel launch.  The images are
-// uploaded to HBM once, on first use; crop / resize / HOG run in sd_hog_batch (sm_100a).
+// uploaded to HBM once, on first use; crop / resize / HOG run in sd_hog_batch (sm_90a).
 #pragma once
 
 #include <memory>

@@ -1,4 +1,4 @@
-// B200 drop-in for the hot-path part of include/rcr/helpers.hpp: to_row (:45-55),
+// H100 drop-in for the hot-path part of include/rcr/helpers.hpp: to_row (:45-55),
 // to_landmark_collection (:66-75) and get_ied (:136-160).  Drawing / check_face are visualisation and
 // dataset hygiene (out of scope, SURVEY.md 2 #8).
 #pragma once

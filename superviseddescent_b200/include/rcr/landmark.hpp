@@ -1,4 +1,4 @@
-// B200 drop-in for include/rcr/landmark.hpp (:34-64): Landmark<T>, LandmarkCollection<T>, filter().
+// H100 drop-in for include/rcr/landmark.hpp (:34-64): Landmark<T>, LandmarkCollection<T>, filter().
 #pragma once
 
 #include <algorithm>

@@ -1,4 +1,4 @@
-// B200 drop-in for include/rcr/model.hpp: align_mean (:64-76), InterEyeDistanceNormalisation (:84-116),
+// H100 drop-in for include/rcr/model.hpp: align_mean (:64-76), InterEyeDistanceNormalisation (:84-116),
 // detection_model (:122-183) and load/save_detection_model (:192-219).  detect() runs the whole cascade
 // on the GPU through sd_detect_batch_host; the file format is byte compatible with the reference's
 // cereal archives (face_landmarks_model_rcr_22.bin loads unchanged).

@@ -16,7 +16,7 @@ namespace sd_b200 {
 inline void check(sd_ctx* ctx, int rc, const char* what)
 {
     if (rc == SD_OK) return;
-    std::string msg = ctx ? sd_last_error(ctx) : "no CUDA device / context (the B200 engine has no CPU fallback)";
+    std::string msg = ctx ? sd_last_error(ctx) : "no CUDA device / context (the engine has no CPU fallback)";
     throw std::runtime_error(std::string(what) + ": " + msg);
 }
 
@@ -31,7 +31,7 @@ inline sd_ctx* context()
             const char* env = std::getenv("SD_B200_DEVICE");
             const int dev = env ? std::atoi(env) : 0;
             const int rc = sd_ctx_create(dev, nullptr, &ctx);
-            if (rc != SD_OK) throw std::runtime_error("sd_ctx_create failed: no usable CUDA device (the B200 engine has no CPU fallback)");
+            if (rc != SD_OK) throw std::runtime_error("sd_ctx_create failed: no usable CUDA device (the engine has no CPU fallback)");
         }
         ~Holder() { sd_ctx_destroy(ctx); }
     };

@@ -1,9 +1,9 @@
-// B200 drop-in for the reference's include/superviseddescent/regressors.hpp.
+// H100 drop-in for the reference's include/superviseddescent/regressors.hpp.
 //
 // Same names and call signatures: Regressor (regressors.hpp:43-77), Regulariser (:87-169),
 // PartialPivLUSolver (:180-235), ColPivHouseholderQRSolver (:245-306), LinearRegressor<Solver>
 // (:318-400, public member `x`).  The arithmetic is NOT here: Solver::solve forwards to sd_learn and
-// predict/test to sd_predict / sd_test_residual of libsd_b200.so (hand-written sm_100a kernels);
+// predict/test to sd_predict / sd_test_residual of libsd_b200.so (hand-written sm_90a kernels);
 // there is no CPU path.
 #pragma once
 

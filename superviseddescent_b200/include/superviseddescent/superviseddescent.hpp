@@ -1,4 +1,4 @@
-// B200 drop-in for the reference's include/superviseddescent/superviseddescent.hpp.
+// H100 drop-in for the reference's include/superviseddescent/superviseddescent.hpp.
 //
 // SupervisedDescentOptimiser<RegressorType, NormalisationStrategy> keeps train / test / predict with the
 // reference's signatures (superviseddescent.hpp:85-361) and its callback types (:52-54).  Two routes:

@@ -1,4 +1,4 @@
-// B200 drop-in for include/superviseddescent/verbose_solver.hpp: the solver type baked into
+// H100 drop-in for include/superviseddescent/verbose_solver.hpp: the solver type baked into
 // rcr::detection_model::model_type (model.hpp:125).  Prints the same four phase lines as the reference
 // (verbose_solver.hpp:66-103), measured with CUDA events on the device.
 #pragma once

@@ -65,7 +65,7 @@ def _features_like(rng, n, d):
 @pytest.mark.parametrize("mode", [2, 0, 3, 1])
 def test_gram_and_solve_vs_oracle(sd, oracle, mode):
     """[AtA | Atb] and the regularised solve at a size that takes the tensor-core SYRK and the blocked
-    Cholesky.  mode 2 = fp32 SIMT, 0 = 3xTF32 tcgen05 (truncated hi), 3 = unbiased 3xTF32, 1 = single-pass TF32 (looser)."""
+    Cholesky.  mode 2 = fp32 SIMT, 0 = 3xTF32 wgmma (truncated hi), 3 = unbiased 3xTF32, 1 = single-pass TF32 (looser)."""
     import ctypes as C
     import torch
     from superviseddescent_b200 import _capi

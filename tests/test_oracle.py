@@ -37,16 +37,22 @@ def test_hog_core_matches_reference_goldens_bit_exact(oracle, golden):
         assert np.array_equal(got.view(np.uint32), golden.hog[f"out{i}"].view(np.uint32)), f"case {i} K={K_} cs={cs} v={variant}"
 
 
-def test_hog_core_matches_live_reference(oracle):
-    if not oracle.ref_available():
-        pytest.skip("oracle/_ref not built (no /root/reference on this box)")
+def test_hog_core_matches_live_reference(oracle, golden):
+    """hog_core on seeded random patches (K = 4, 9, 6) against the reference's hog.c: its outputs on these inputs are stored in
+    tests/golden/hog_live_ref.npz, and compared live as well when oracle/_ref is built."""
+    g = np.load(os.path.join(golden.dir, "hog_live_ref.npz"))
     rng = np.random.default_rng(7)
+    n = 0
     for K_ in (4, 9, 6):
         for fs, cs in ((55, 11), (30, 6), (48, 8)):
             img = rng.integers(0, 256, (fs, fs)).astype(np.float32)
+            assert np.array_equal(img.astype(np.uint8), g[f"img{n}"]) and list(g[f"cfg{n}"]) == [K_, cs, 1]
             a = oracle.hog_core(img, cs, K_, 1)
-            b = oracle.hog_core(img, cs, K_, 1, use_ref=True)
-            assert np.array_equal(a.view(np.uint32), b.view(np.uint32))
+            assert np.array_equal(a.view(np.uint32), g[f"out{n}"].view(np.uint32)), (K_, fs, cs)
+            if oracle.ref_available():
+                b = oracle.hog_core(img, cs, K_, 1, use_ref=True)
+                assert np.array_equal(a.view(np.uint32), b.view(np.uint32))
+            n += 1
 
 
 def test_orientation_ties_are_resolved_like_the_reference(oracle):
@@ -252,7 +258,7 @@ def test_pose_estimation_example_config2(oracle):
     assert np.all(np.abs(pred[:3] - np.array([11.0, -25.0, -10.0])) < 6.0)      # example's ground truth (:334)
 
 
-def test_fixed_patch_transform_equals_adaptive_one_at_matching_size(oracle):
+def test_fixed_patch_transform_equals_adaptive_one_at_matching_size(oracle, golden):
     """examples/landmark_detection.cpp:195-261 (fixed patch, no resize, no bias) against adaptive_vlhog.hpp:109-185: when
     the inter-eye distance makes the adaptive patch exactly num_cells * cell_size wide, cv::resize is the identity and the
     two functors must agree value for value (the adaptive one appends its bias)."""
@@ -265,12 +271,15 @@ def test_fixed_patch_transform_equals_adaptive_one_at_matching_size(oracle):
     x[0], x[L] = 40.0, 60.0                       # right eye
     x[1], x[L + 1] = 40.0 + nc * cs, 60.0         # left eye: IED = 36 -> half = round(1.0 * 36 / 2) = 18 = nc * (cs / 2)
     x[2], x[L + 2] = 2.0, 118.0                   # near a corner: zero padding on two sides
+    g = np.load(os.path.join(golden.dir, "hog_live_ref.npz"))    # the reference's hog.c on this frame and these landmarks
+    assert np.array_equal(x, g["fixed_x"])
     for variant in (0, 1):
         hp = oracle.HogParam(variant, nc, cs, K, 1.0)
         adaptive = oracle.hog_transform(img, x, hp, [0], [1])
         fixed = oracle.hog_transform_fixed(img, x, hp)
         assert fixed.size == adaptive.size - 1 and adaptive[-1] == 1.0
         assert np.array_equal(fixed, adaptive[:-1])
+        assert np.array_equal(fixed.view(np.uint32), g[f"fixed_v{variant}"].view(np.uint32))
         if oracle.ref_available():
             assert np.array_equal(oracle.hog_transform_fixed(img, x, hp, use_ref=True), fixed)
 
