@@ -16,7 +16,6 @@
 #include "sd_internal.cuh"
 
 #include <cmath>
-#include <cstdlib>
 
 namespace {
 
@@ -285,8 +284,9 @@ int sd_cg_solve(sd_ctx* ctx, sd_comm* comm, float* G, int64_t ldg, int n, int co
     cg_init_finish_kernel<<<1, 1024, 0, ctx->stream>>>(b, M);
     SD_LAUNCH_CHECK(ctx, "cg_init_finish_kernel");
 
-    static const float tol = getenv("SD_B200_CG_TOL") ? (float)atof(getenv("SD_B200_CG_TOL")) : 2e-6f;
-    static const int max_iter = getenv("SD_B200_CG_MAXIT") ? atoi(getenv("SD_B200_CG_MAXIT")) : 600;
+    // fixed, so that every rank of the shared route stops at the same iteration and their all-reduces stay in step
+    constexpr float tol = 2e-6f;
+    constexpr int max_iter = 600;
     // The product is the same launch every iteration: Q[n x M] = S[k0:k1, :]^T P[k0:k1, :]  ( = S P summed over the ranks' slabs of
     // the contraction: S is symmetric ); prepared once (tensor maps, tile list).  S is the 128-row operand: n / 128 tiles keep the
     // SMs busy at any slab size, P is the narrow operand.  Pad columns of Q and the rows of a rank without slab stay zero.

