@@ -284,7 +284,8 @@ SD_API int sd_learn_dist(sd_ctx* ctx, sd_comm* comm, const float* d_A, int64_t l
  *       few dozen products with the D x D matrix replace the D^3 / 3 factorisation; it stops at a relative residual of 2e-6 and
  *       falls back to the Cholesky if the recurrence breaks down or stalls (ill-conditioned systems, tiny lambda).
  * sd_learn_dist: distributed_solve 2 = the ranks share the CG iterations (rows of the matrix sharded, one all-reduce of
- * 2L x D floats per iteration).  sd_solver_iterations: CG iterations of the last solve (0 = the factorisation ran). */
+ * 2L x D floats per iteration).  sd_solver_iterations, of the last solve: +n = CG converged after n iterations and its answer
+ * was used; -n = CG ran n iterations, gave up, and the factorisation answered; 0 = CG was not tried. */
 SD_API int sd_set_solver(sd_ctx* ctx, int mode);
 SD_API int sd_solver_iterations(const sd_ctx* ctx);
 

@@ -70,7 +70,8 @@ class Context:
         _check(self._h, _capi.lib().sd_set_solver(self._h, int(m)))
 
     def solver_iterations(self) -> int:
-        """CG iterations of the last solve (0: the factorisation ran)."""
+        """CG iterations of the last solve: +n = CG converged after n iterations and its answer was used; -n = CG ran n
+        iterations, gave up, and the factorisation answered; 0 = CG was not tried."""
         return int(_capi.lib().sd_solver_iterations(self._h))
 
     def solver_timings(self):

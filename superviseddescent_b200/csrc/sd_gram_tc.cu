@@ -16,7 +16,8 @@
 //
 // Accumulation: the chain of accumulating MMAs is cut every KC = 128 samples: each chunk starts a fresh
 // accumulator (scale-d = 0) and the consumer warps fold the finished chunk into running sums held in registers
-// with round-to-nearest adds, so the error does not grow with the length of the contraction.
+// with round-to-nearest adds, so the MMA chain's error does not grow with the length of the contraction; the fp32 fold over
+// K / 128 chunks does, roughly like the square root of the number of chunks (DESIGN 4.2).
 //
 // Kernel shape (persistent, one CTA per SM, 512 threads): see syrk_wgmma_kernel below.
 #include "sd_internal.cuh"

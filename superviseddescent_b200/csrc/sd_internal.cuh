@@ -42,7 +42,7 @@ struct sd_ctx {
     int sm_count = 132;
     int gram_mode = 0;
     int solver_mode = 0;           // systems with D > 256: 0 = blocked Cholesky, 1 = conjugate gradients (Cholesky if they stall)
-    int cg_iterations = 0;         // of the last solve (0: the factorisation ran)
+    int cg_iterations = 0;         // of the last solve: +n CG converged, -n CG gave up after n (factorisation answered), 0 not tried
     cudaEvent_t cg_ev[8] = {};     // convergence read-backs of the CG loop (the host runs a few iterations ahead of them)
     int64_t roi_fallbacks = 0;     // faces repeated from the full frame because a patch left its ROI
     float timings[4] = {0, 0, 0, 0};

@@ -1467,6 +1467,7 @@ static int solve_gram_impl(sd_ctx* ctx, sd_comm* comm, float* d_G, int64_t ldg, 
     SD_REQUIRE(ctx, d_G && d_X && reg && D >= 1 && M >= 1 && ldg >= D + M, "bad argument");
     SD_REQUIRE(ctx, reg->type == 0 || reg->type == 1, "unknown regularisation type");
     SD_REQUIRE(ctx, n_train_global >= 1, "n_train_global must be >= 1");
+    ctx->cg_iterations = 0;                                           // until CG runs: the small LU and the factorisation
     // the distributed factorisation needs whole panels per rank; small systems were all-reduced and are solved replicated
     const int nranks = sd_comm_size_of(comm);
     const bool dist = route == 1 && nranks > 1 && sd_gram_is_scattered(D, ldg, d_G);
@@ -1548,13 +1549,12 @@ static int solve_gram_impl(sd_ctx* ctx, sd_comm* comm, float* d_G, int64_t ldg, 
         bias_downdate_kernel<<<4 * ctx->sm_count, 256, 0, ctx->stream>>>(d_G, ldg, D, M, sv, 2 * kCholNb, nr, me, partial_downdate ? 1 : 0, k0, k1);
         SD_LAUNCH_CHECK(ctx, "bias_downdate_kernel");
         bool solved = false;
-        ctx->cg_iterations = 0;
         if (try_cg) {
             // conjugate gradients on the (well conditioned) centred system; falls back to the factorisation when it stalls
             float* W = nullptr;
             int ldw = 0, its = 0;
             rc = sd_cg_solve(ctx, route == 2 ? comm : nullptr, d_G, ldg, D - 1, D, M, &W, &ldw, &its);
-            ctx->cg_iterations = its;
+            ctx->cg_iterations = rc == SD_OK ? its : -its;        // negative: CG gave up and the factorisation answers
             if (rc == SD_OK) {
                 SD_CUDA(ctx, cudaEventRecord(ctx->ev[3], ctx->stream));
                 bias_finish_kernel<<<M + 2 * ctx->sm_count, 256, 0, ctx->stream>>>(W, ldw, 0, D, M, sv, d_X, d_mu, d_Xc);

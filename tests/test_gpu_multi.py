@@ -191,14 +191,14 @@ def test_two_ranks_match_one_rank():
             e_single, e_truth = rel_err(X0, Xs), rel_err(X0, Xt)
             print(f"{name} distributed_solve={ds}: X(2 ranks) vs X(1 rank) {e_single:.2e}; vs float64 {e_truth:.2e}; lambda {lam0:.6g} / {lam_s:.6g} / {lam_t:.6g}; "
                   f"CG iterations {r0[(name, ds, 'its')]}")
-            assert (r0[(name, ds, "its")] > 0) == (ds == 2)
+            assert r0[(name, ds, "its")] > 0 if ds == 2 else r0[(name, ds, "its")] == 0    # converged CG / CG not tried
             assert e_single <= (1e-5 if ds < 2 else 2e-5)                   # CG stops at a relative residual of 2e-6
             assert e_truth <= 1e-4
             assert abs(lam0 - lam_s) <= 1e-6 * lam_s
     for r in (r0, r1):
         (Xa, its_a), (Xb, its_b) = r[("fallback", 0)], r[("fallback", 2)]
-        print(f"fall-back: CG gave up after {its_b} iterations; factorisation result identical to route 0: {np.array_equal(Xa, Xb)}")
-        assert its_a == 0 and its_b > 0
+        print(f"fall-back: CG gave up after {-its_b} iterations; factorisation result identical to route 0: {np.array_equal(Xa, Xb)}")
+        assert its_a == 0 and its_b < 0
         assert np.array_equal(Xa, Xb)                                       # the replicated factorisation of the same matrix
     assert np.array_equal(r0[("fallback", 2)][0], r1[("fallback", 2)][0])
     Ws, xs = r0[("cascade", "single")]

@@ -174,11 +174,12 @@ def test_pose_estimation_example_config2(sd, oracle):
 
 
 @pytest.mark.parametrize("D,M,pad", [(257, 1, 0), (300, 8, 0), (384, 44, 0), (385, 44, 1), (513, 3, 2), (640, 70, 0),
-                                     (1000, 44, 3), (1153, 136, 0)])
+                                     (1000, 44, 3), (1153, 136, 0), (2600, 44, 0), (4097, 136, 0), (2600, 44, 1)])
 def test_blocked_cholesky_shapes(sd, D, M, pad):
     """sd_solve_gram on well-conditioned SPD systems of awkward shapes: D just above the LU limit, odd numbers of
     128-blocks (a panel with a single block), ragged last blocks, right-hand sides wider than one column tile, and
-    leading dimensions that are not a multiple of 4 (scalar staging, SIMT trailing updates instead of TMA).  Manual
+    leading dimensions that are not a multiple of 4 (scalar staging, SIMT trailing updates instead of TMA), and early panels
+    whose tail updates have more tiles than the GPU has SMs (tensor cores, and SIMT on a large matrix at an odd pitch).  Manual
     regularisation lambda = 0.5 is added to the diagonal as regressors.hpp:126-148 does (bias row unregularised)."""
     import ctypes as C
     import torch
@@ -243,7 +244,8 @@ def test_colpiv_qr_solver_rank_diagnostic(sd, capsys):
 
 def test_conjugate_gradient_route_matches_the_factorisation(sd):
     """sd_set_solver(1): CG on the tensor cores for the centred, MatrixNorm-regularised system (well conditioned) must give the
-    weights of the blocked Cholesky; an ill-conditioned system (tiny manual lambda) must fall back to the factorisation."""
+    weights of the blocked Cholesky; an ill-conditioned system (tiny manual lambda) must fall back to the factorisation and say so
+    (a negative iteration count)."""
     ctx = sd.default_context()
     A = _features_like(np.random.default_rng(31), 2500, 1800)
     B = (0.05 * np.random.default_rng(32).standard_normal((2500, 44))).astype(np.float32)
@@ -280,11 +282,58 @@ def test_conjugate_gradient_route_matches_the_factorisation(sd):
         ctx.set_solver("cg")
         hard = sd.LinearRegressor(sd.Regulariser(sd.RegularisationType.Manual, 1e-4, True))
         hard.learn(A, B)
+        its_hard = ctx.solver_iterations()
         ctx.set_solver("cholesky")
         ref = sd.LinearRegressor(sd.Regulariser(sd.RegularisationType.Manual, 1e-4, True))
         ref.learn(A, B)
+        print(f"tiny lambda: CG gave up after {-its_hard} iterations")
+        assert its_hard < 0                                 # CG ran, gave up, and the factorisation answered
+        assert ctx.solver_iterations() == 0
+        assert np.array_equal(hard.x.cpu().numpy(), ref.x.cpu().numpy())
         assert np.isfinite(hard.x.cpu().numpy()).all()
         pa, pb = A @ hard.x.cpu().numpy(), A @ ref.x.cpu().numpy()
         assert rel_err(pa, pb) <= 1e-3
     finally:
         ctx.set_solver("cholesky")
+
+
+# (D - 1, M): right-hand sides up to 64 take the narrow (64-column) product, more take 128-column tiles, 192 is the CG cap;
+# D - 1 = 1799 and 3000 leave a padded, partial last strip of the strip-major operand, 2048 fills it exactly
+@pytest.mark.parametrize("n,m", [(1799, 1), (1799, 44), (1799, 64), (1799, 65), (1799, 136), (1799, 192), (1799, 193),
+                                 (2048, 44), (3000, 44), (3000, 136)])
+def test_conjugate_gradient_shapes_match_float64_and_the_factorisation(sd, n, m):
+    """sd_set_solver(1): CG on the tensor cores for the centred, MatrixNorm-regularised system (well conditioned) must converge
+    (a positive iteration count) to the weights of the blocked Cholesky and of float64; more than 192 right-hand sides are the
+    factorisation's job (0: CG not tried)."""
+    ctx = sd.default_context()
+    d = n + 1
+    samples = d + 700
+    A = _features_like(np.random.default_rng(31 + n), samples, d)
+    B = (0.05 * np.random.default_rng(32 + m).standard_normal((samples, m))).astype(np.float32)
+    reg = sd.Regulariser(sd.RegularisationType.MatrixNorm, 1.5, False)
+    chol = sd.LinearRegressor(reg)
+    chol.learn(A, B)
+    assert ctx.solver_iterations() == 0
+    ctx.set_solver("cg")
+    try:
+        cg = sd.LinearRegressor(reg)
+        cg.learn(A, B)
+        its = ctx.solver_iterations()
+    finally:
+        ctx.set_solver("cholesky")
+    A64 = A.astype(np.float64)
+    G = A64.T @ A64
+    lam = 1.5 * np.linalg.norm(G) / samples
+    Rg = np.eye(d) * lam
+    Rg[-1, -1] = 0
+    Xt = np.linalg.solve(G + Rg, A64.T @ B.astype(np.float64))
+    Xcg, Xch = cg.x.cpu().numpy(), chol.x.cpu().numpy()
+    e = rel_err(Xcg, Xch)
+    print(f"D={d} M={m}: CG {its} iterations; weights vs Cholesky {e:.2e}; vs float64 CG {rel_err(Xcg, Xt):.2e} / Cholesky {rel_err(Xch, Xt):.2e}")
+    if m > 192:
+        assert its == 0
+        assert np.array_equal(Xcg, Xch)
+        return
+    assert 3 <= its <= 200
+    assert e <= 2e-5
+    assert rel_err(Xcg, Xt) <= 1e-4
