@@ -178,22 +178,29 @@ __global__ void hog_lut_kernel(const LutArgs t, int8_t* __restrict__ lut)
 
 // shared-memory carve-up (same function on host and device)
 struct HogSmem {
-    int patch, bin, r1, xofs, yofs0, yofs1, xa, yb, wcell, lo, hi, hist, energy, fac, vote, feat, mbar, total;
+    int patch, bin, r1, xofs, yofs0, yofs1, xa, yb, wcell, lo, hi, hist, energy, fac, vote, feat, mbar, stage_end, total;
     int tpad;      // tasks of the horizontal vote pass, padded to a multiple of 32
 };
 
 __host__ __device__ inline int align_up(int v, int a) { return (v + a - 1) / a * a; }
 
+// Regions whose lifetimes do not overlap share storage, so that more CTAs fit on an SM:
+//   patch  (S1-S2)  then  hist, energy, fac (S3-S6)
+//   vote   (S3)     then  feat (S6-S8)
+//   r1: gradient modulus (S2-S3), then the clamped hc values (S6-S7)
+// and [bin | r1 | vote/feat] is dead during S1, so that whole span is the staging area of the source window.
 __host__ __device__ inline HogSmem hog_smem_layout(int fs, int nc, int K, int dd)
 {
     HogSmem s;
     const int cells = nc * nc;
     int o = 0;
-    s.patch = o;  o = align_up(o + fs * fs, 128);
-    s.bin = o;    o = align_up(o + fs * fs, 16);            // [bin | r1] doubles as the staging area of the source window (128-byte
-    int r1 = fs * fs * 4;                                   //  aligned: TMA destination); r1 = gradient modulus, later the clamped
-    if (cells * K * 32 > r1) r1 = cells * K * 32;           //  hc values (double)
-    s.r1 = o;     o = align_up(o + r1, 16);
+    s.patch = o;
+    s.hist = o;
+    s.energy = align_up(s.hist + cells * 2 * K * 4, 16);
+    s.fac = align_up(s.energy + cells * 4, 16);
+    o = s.fac + cells * 4 * 8;
+    if (fs * fs > o) o = fs * fs;
+    o = align_up(o, 16);
     s.xofs = o;   o += fs * 4;
     s.yofs0 = o;  o += fs * 4;
     s.yofs1 = o;  o += fs * 4;
@@ -202,14 +209,19 @@ __host__ __device__ inline HogSmem hog_smem_layout(int fs, int nc, int K, int dd
     s.wcell = o;  o += nc * fs * 4;                         // weight of pixel t for cell index c (0 if it does not vote)
     s.lo = o;     o += nc * 4;
     s.hi = o;     o += nc * 4;
-    s.hist = o;   o += cells * 2 * K * 4;
-    s.energy = o; o = align_up(o + cells * 4, 16);
-    s.fac = o;    o += cells * 4 * 8;
-    s.tpad = align_up((fs - 2) * nc, 32);
-    o = align_up(o, 16);
-    s.vote = o;   o += 2 * K * s.tpad * 4;                  // horizontal pass of the vote: T[bin][(cell column, row)]
-    s.feat = o;   o += cells * dd * 4;
     s.mbar = align_up(o, 8); o = s.mbar + 8;
+    o = align_up(o, 128);
+    s.bin = o;    o = align_up(o + fs * fs, 16);            // staging area from here to stage_end (128-byte aligned: TMA destination)
+    int r1 = fs * fs * 4;                                   // r1 = gradient modulus, later the clamped hc values (double)
+    if (cells * K * 32 > r1) r1 = cells * K * 32;
+    s.r1 = o;     o = align_up(o + r1, 16);
+    s.tpad = align_up((fs - 2) * nc, 32);
+    s.vote = o;                                             // horizontal pass of the vote: T[bin][(cell column, row)]
+    s.feat = o;
+    int vote = 2 * K * s.tpad * 4;
+    if (cells * dd * 4 > vote) vote = cells * dd * 4;
+    o += vote;
+    s.stage_end = o;
     s.total = align_up(o, 16);
     return s;
 }
@@ -292,8 +304,8 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const HogArgs a,
     // ---- S1: zero-padded crop + fixed-point bilinear resize.  The P x P source window is staged in shared memory with its
     //      zero padding materialised, then resampled from there: one output row per warp pass, lanes along x.
     const int x0 = cx - half, y0 = cy - half;
-    uint8_t* s_stage = smem + lay.bin;                             // [bin | r1] are dead until S2
-    const int stage_cap = lay.xofs - lay.bin;
+    uint8_t* s_stage = smem + lay.bin;                             // [bin | r1 | vote] are dead until S2
+    const int stage_cap = lay.stage_end - lay.bin;
     // TMA route: whole frames resident and describable by a tensor map; the smallest box class that covers the window and
     // fits the staging area
     int tma_box = 0;
@@ -332,8 +344,6 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const HogArgs a,
         for (int i = tid; i < nc * fs; i += kHogThreads) s_wcell[i] = __ldg(a.btab + i);
         const int* __restrict__ lohi = reinterpret_cast<const int*>(a.btab + nc * fs);
         if (tid < nc) { s_lo[tid] = __ldg(lohi + tid); s_hi[tid] = __ldg(lohi + nc + tid); }
-        float4* T4 = reinterpret_cast<float4*>(s_T);
-        for (int i = tid; i < K * lay.tpad / 2; i += kHogThreads) T4[i] = make_float4(0.f, 0.f, 0.f, 0.f);     // 2K * tpad floats
     }
     {
         const bool resident = x0 >= rx && y0 >= ry && x0 + P <= rx + rw && y0 + P <= ry + rh && x0 >= 0 && y0 >= 0 && x0 + P <= W && y0 + P <= H;
@@ -517,6 +527,7 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const HogArgs a,
             const float* gp = s_gmag + y * fs + xlo;
             const float* wp = s_wcell + ci * fs + xlo;
             float* T = s_T + task;
+            for (int b = 0; b < 2 * K; ++b) T[b * tpad] = 0.f;        // T shares the staging area of S1: clear this column first
 #pragma unroll 2
             for (int x = xlo; x <= xhi; ++x) {
                 const int b = max((int)*bp++, 0);                     // zero gradient: bin -1, modulus 0 -> adds +0 to bin 0
@@ -525,6 +536,9 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const HogArgs a,
             }
         }
         __syncthreads();
+        // Only the ntask columns that pass 1 cleared and filled are read here: hog_bintab_kernel keeps lo and hi inside the
+        // interior [1, fs - 2], so rows ylo..yhi stay in column block ci.  The padding columns [ntask, tpad) still hold bytes
+        // of the staged window (they were not cleared) and must never be read.
         for (int i = tid; i < 2 * K * cells; i += kHogThreads) {
             const int b = i / cells, c = i - b * cells;
             const int cj = c / nc, ci = c - cj * nc;                  // cell row (y), cell column (x)
