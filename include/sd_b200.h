@@ -230,9 +230,11 @@ SD_API int sd_test_residual(sd_ctx* ctx, const float* d_values, int64_t ldv, con
 /* timings of the last sd_learn / sd_solve_gram: [0] "At * A", [1] "AtA + Reg", [2] "Decomposition",
  * [3] "solve()" in milliseconds (verbose_solver.hpp:66-103) */
 SD_API int sd_solver_timings(sd_ctx* ctx, float ms_out[4]);
-/* precision of the tensor-core Gram: 0 = 3xTF32 split on the truncated operand (default: Gram ~2e-7),
+/* precision of the Gram and of the Cholesky trailing updates (both run the same SYRK kernels):
+ * 0 = 3xTF32 split on the truncated operand (default: Gram ~2e-7),
  * 3 = 3xTF32 split with the hi part rounded in shared memory (unbiased: Gram ~7e-8, ~15 % slower),
- * 1 = single TF32 pass (~7e-5), 2 = force the fp32 SIMT kernel (~3e-7) */
+ * 1 = single TF32 pass (~7e-5), also for the trailing updates, 2 = force the fp32 SIMT kernel (~3e-7) everywhere.
+ * The trailing updates always round the hi part; the product inside conjugate gradients is always 3xTF32 with rounded hi. */
 SD_API int sd_set_gram_mode(sd_ctx* ctx, int mode);
 
 /* ---- multi-GPU training: the exchange at superviseddescent.hpp:207 (SURVEY 8e) ----------------------------------------

@@ -11,8 +11,8 @@
 //
 // All 2L right-hand sides advance in lockstep (independent CG recurrences sharing the product).  Reductions are two-stage with a
 // fixed order, so the result is reproducible.  If the recurrence breaks down (p^T S p <= 0: not positive definite) or does not
-// reach the tolerance, the caller falls back to the blocked Cholesky: the upper triangle of S and the right-hand sides are never
-// modified here (only the unused lower triangle is filled with the mirror image).
+// reach the tolerance, the caller falls back to the blocked Cholesky: G (the matrix S and the right-hand sides) is only read
+// here, never written.
 #include "sd_internal.cuh"
 
 #include <cmath>
@@ -296,7 +296,7 @@ int sd_cg_solve(sd_ctx* ctx, sd_comm* comm, float* G, int64_t ldg, int n, int co
     int rc = SD_OK;
     if (k1 > k0) {
         rc = sd_gemm_tn_tc_prepare(ctx, T, 128, b.P + (size_t)k0 * Mp, Mp, k1 - k0, n, M, b.Q, Mp, 1.0f, 0.0f, 3, true, false,
-                                   nullptr, 1, d_tile_buf, plan, &no_tiles, true, kp);
+                                   nullptr, d_tile_buf, plan, &no_tiles, true, kp);
         if (rc) return rc;
     }
     // convergence read-backs: slot it % 8 holds {max relative residual, breakdown flag} after iteration it; the host looks at the

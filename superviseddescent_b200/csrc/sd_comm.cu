@@ -7,9 +7,9 @@
 // object has no link-time dependency on it and single-GPU users never touch it.
 //
 //   sd_allreduce_gram       every rank gets the summed upper row bands (replicated solve follows)
-//   sd_reduce_scatter_gram  block-row-cyclic owner of each 256-row band gets its sum (distributed factorisation follows)
-// Both move only what the solve reads: each 256-row band from its first diagonal column to the end of the row, packed
-// into one contiguous buffer by an HBM-speed kernel (about half of the D x (D+M) buffer).
+//   sd_reduce_scatter_gram  the owner of each band (sd_panel_owner) gets its sum (distributed factorisation follows)
+// Both move only what the solve reads: each band of SD_PANEL_ROWS rows from its first diagonal column to the end of the row,
+// packed into one contiguous buffer by an HBM-speed kernel (about half of the D x (D+M) buffer).
 #include "sd_internal.cuh"
 
 #include <dlfcn.h>
@@ -67,17 +67,16 @@ NcclApi& nccl()
     return api;
 }
 
-// pack / unpack of the row bands the solve reads: band p = rows [p*band, ...), columns [p*band, W)
-__global__ void band_copy_kernel(float* __restrict__ G, long long ldg, int D, int W, int band, float* __restrict__ flat,
+// pack / unpack of the row bands the solve reads: band p = rows [p*SD_PANEL_ROWS, ...), columns [p*SD_PANEL_ROWS, W)
+__global__ void band_copy_kernel(float* __restrict__ G, long long ldg, int D, int W, float* __restrict__ flat,
                                  const long long* __restrict__ offsets, int nranks, int rank, int unpack)
 {
-    const int p = blockIdx.y;
-    if (nranks > 1 && p % nranks != rank) return;
-    const int r0 = p * band;
-    const int nrows = (D - r0 < band) ? D - r0 : band;
-    const int w = W - r0;                           // multiple of 4 when W and band are
+    const int r0 = blockIdx.y * SD_PANEL_ROWS;
+    if (nranks > 1 && sd_panel_owner(r0, nranks) != rank) return;
+    const int nrows = (D - r0 < SD_PANEL_ROWS) ? D - r0 : SD_PANEL_ROWS;
+    const int w = W - r0;                           // multiple of 4 when W is
     const long long total4 = (long long)nrows * (w >> 2);
-    float* dst = flat + offsets[p];
+    float* dst = flat + offsets[blockIdx.y];
     for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total4; idx += (long long)gridDim.x * blockDim.x) {
         const int r = (int)(idx / (w >> 2));
         const int c = (int)(idx - (long long)r * (w >> 2)) << 2;
@@ -113,7 +112,7 @@ int sd_comm_nccl_check(sd_ctx* ctx, int r, const char* what)
 
 bool sd_gram_is_scattered(int D, int64_t ldg, const float* d_G)
 {
-    return (ldg % 4) == 0 && (reinterpret_cast<uintptr_t>(d_G) & 15) == 0 && D > 2 * 256;
+    return (ldg % 4) == 0 && (reinterpret_cast<uintptr_t>(d_G) & 15) == 0 && D > 2 * SD_PANEL_ROWS;
 }
 
 int sd_comm_rank_of(const sd_comm* c) { return c ? c->rank : 0; }
@@ -143,18 +142,16 @@ int sd_comm_allreduce_f32(sd_ctx* ctx, sd_comm* c, float* d_buf, size_t count, c
 
 namespace {
 
-constexpr int kBand = 256;   // == one Cholesky panel (two 128-blocks): the ownership unit of sd_solve_gram_dist
-
 // offsets of the packed bands; returns the total float count
 long long band_layout(sd_ctx* ctx, sd_comm* c, int D, int W, int* nbands_out)
 {
-    const int nb = sd_div_up(D, kBand);
+    const int nb = sd_div_up(D, SD_PANEL_ROWS);
     *nbands_out = nb;
     if (c->off_D == D && c->off_W == W && c->d_offsets) return c->h_offsets[nb];
     c->h_offsets.assign(nb + 1, 0);
     for (int p = 0; p < nb; ++p) {
-        const int r0 = p * kBand;
-        const int nrows = (D - r0 < kBand) ? D - r0 : kBand;
+        const int r0 = p * SD_PANEL_ROWS;
+        const int nrows = (D - r0 < SD_PANEL_ROWS) ? D - r0 : SD_PANEL_ROWS;
         c->h_offsets[p + 1] = c->h_offsets[p] + (long long)nrows * (W - r0);
     }
     if (c->d_offsets) { cudaStreamSynchronize(ctx->stream); cudaFree(c->d_offsets); c->d_offsets = nullptr; }
@@ -172,8 +169,6 @@ int gram_exchange(sd_ctx* ctx, sd_comm* c, float* d_G, int64_t ldg, int D, int M
     if (c->nranks == 1) return SD_OK;
     NcclApi& n = nccl();
     const int W = (int)ldg;                          // the padding columns travel too (keeps every row a multiple of 4 floats)
-    const bool vec_ok = (ldg % 4) == 0 && (reinterpret_cast<uintptr_t>(d_G) & 15) == 0;
-    (void)vec_ok;
     if (!sd_gram_is_scattered(D, ldg, d_G)) {
         // small or unaligned: the whole buffer in one all-reduce (a superset of what the owners need)
         SD_NCCL(ctx, n.AllReduce(d_G, d_G, (size_t)D * ldg, ncclFloat32, ncclSum, c->comm, ctx->stream));
@@ -185,23 +180,24 @@ int gram_exchange(sd_ctx* ctx, sd_comm* c, float* d_G, int64_t ldg, int D, int M
     float* flat = (float*)sd_workspace(ctx, SD_WS_GRAM_EXT, (size_t)total * sizeof(float));
     if (!flat) return SD_ERR_CUDA;
     const dim3 grid(64, nb);
-    band_copy_kernel<<<grid, 256, 0, ctx->stream>>>(d_G, ldg, D, W, kBand, flat, c->d_offsets, 1, 0, 0);
+    band_copy_kernel<<<grid, 256, 0, ctx->stream>>>(d_G, ldg, D, W, flat, c->d_offsets, 1, 0, 0);
     SD_LAUNCH_CHECK(ctx, "band_copy_kernel(pack)");
     if (!scatter) {
         SD_NCCL(ctx, n.AllReduce(flat, flat, (size_t)total, ncclFloat32, ncclSum, c->comm, ctx->stream));
-        band_copy_kernel<<<grid, 256, 0, ctx->stream>>>(d_G, ldg, D, W, kBand, flat, c->d_offsets, 1, 0, 1);
+        band_copy_kernel<<<grid, 256, 0, ctx->stream>>>(d_G, ldg, D, W, flat, c->d_offsets, 1, 0, 1);
         SD_LAUNCH_CHECK(ctx, "band_copy_kernel(unpack)");
     } else {
-        // one rooted reduce per band, root = its block-row-cyclic owner, all in one group (one launch per rank)
+        // one rooted reduce per band, root = its owner, all in one group (one launch per rank)
         SD_NCCL(ctx, n.GroupStart());
         for (int p = 0; p < nb; ++p) {
             float* b = flat + c->h_offsets[p];
             const size_t cnt = (size_t)(c->h_offsets[p + 1] - c->h_offsets[p]);
-            int r = (int)n.Reduce(b, b, cnt, ncclFloat32, ncclSum, p % c->nranks, c->comm, ctx->stream);
+            const int root = sd_panel_owner((int64_t)p * SD_PANEL_ROWS, c->nranks);
+            int r = (int)n.Reduce(b, b, cnt, ncclFloat32, ncclSum, root, c->comm, ctx->stream);
             if (r != (int)ncclSuccess) { n.GroupEnd(); return sd_comm_nccl_check(ctx, r, "ncclReduce(band)"); }
         }
         SD_NCCL(ctx, n.GroupEnd());
-        band_copy_kernel<<<grid, 256, 0, ctx->stream>>>(d_G, ldg, D, W, kBand, flat, c->d_offsets, c->nranks, c->rank, 1);
+        band_copy_kernel<<<grid, 256, 0, ctx->stream>>>(d_G, ldg, D, W, flat, c->d_offsets, c->nranks, c->rank, 1);
         SD_LAUNCH_CHECK(ctx, "band_copy_kernel(unpack own)");
     }
     return SD_OK;

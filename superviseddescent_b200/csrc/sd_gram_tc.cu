@@ -3,7 +3,7 @@
 // This is LinearRegressor::learn's "At * A" (reference verbose_solver.hpp:67, regressors.hpp:208) with
 // A^T b folded in as extra columns (SA == SB, upper-triangle tiles only), the trailing update of the blocked
 // Cholesky that replaces PartialPivLU (verbose_solver.hpp:89), and -- with two different operands -- the
-// block-row solves P = U_jj^-T B of that factorisation.  S is row-major [K x NJ] -- one sample per row, exactly
+// product S P of the conjugate-gradient route (sd_cg.cu).  S is row-major [K x NJ] -- one sample per row, exactly
 // as the optimiser stacks the feature rows (superviseddescent.hpp:186-189) -- so BOTH operands are "MN-major"
 // (the contraction index K is the slow one).  wgmma reads 32-bit (TF32) operands from shared memory only
 // K-major, so the raw tiles that the TMA brings in are transposed in shared memory by a transform warpgroup,
@@ -191,9 +191,7 @@ struct TcArgs {
     int passes;          // 1 or 3
     int unbiased;        // round hi (slower, unbiased) instead of using the value the tensor core truncates
     const int2* tiles;   // (ti, tj) per tile
-    int num_tiles;       // work items = tiles x ksplit
-    int ksplit, kps;     // the K loop of every tile is cut into ksplit ranges of kps pipeline stages (work item t: tile t / ksplit,
-                         // range t % ksplit); ksplit > 1 needs the reduce-add write-back onto a zeroed C
+    int num_tiles;
     int a_strip;         // > 0: operand A is stored strip-major, [tile row][a_strip contraction rows][128 columns] (sd_cg.cu)
 };
 
@@ -279,10 +277,9 @@ syrk_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
             // ===================== TMA producer =====================
             uint32_t stage = 0, phase = 0;
             for (int t = blockIdx.x; t < a.num_tiles; t += gridDim.x) {
-                const int2 tile = a.tiles[t / a.ksplit];
+                const int2 tile = a.tiles[t];
                 const int i0 = tile.x * BM, j0 = tile.y * BN;
-                const int kb0 = (t % a.ksplit) * a.kps, kb1 = min(num_k, kb0 + a.kps);
-                for (int kb = kb0; kb < kb1; ++kb) {
+                for (int kb = 0; kb < num_k; ++kb) {
                     mbar_wait(&raw_empty[stage], phase ^ 1);
                     mbar_arrive_expect_tx(&raw_full[stage], Cfg::RAW_BYTES);
                     unsigned char* sa = raw_base + stage * Cfg::RAW_BYTES;
@@ -303,8 +300,7 @@ syrk_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         const int tt = threadIdx.x - 128;                 // 0..127
         uint32_t rs = 0, rph = 0, ks = 0, kph = 0;
         for (int t = blockIdx.x; t < a.num_tiles; t += gridDim.x) {
-            const int kb0 = (t % a.ksplit) * a.kps, kb1 = min(num_k, kb0 + a.kps);
-            for (int kb = kb0; kb < kb1; ++kb) {
+            for (int kb = 0; kb < num_k; ++kb) {
                 mbar_wait(&raw_full[rs], rph);
                 mbar_wait(&km_empty[ks], kph ^ 1);
                 const uint32_t raw = smem_u32(raw_base + rs * Cfg::RAW_BYTES);
@@ -331,13 +327,12 @@ syrk_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         float acc[NV];
         float run[NV];
         for (int t = blockIdx.x; t < a.num_tiles; t += gridDim.x) {
-            const int2 tile = a.tiles[t / a.ksplit];
-            const int kb0 = (t % a.ksplit) * a.kps, kb1 = min(num_k, kb0 + a.kps);
+            const int2 tile = a.tiles[t];
 #pragma unroll
             for (int v = 0; v < NV; ++v) { acc[v] = 0.f; run[v] = 0.f; }
-            for (int kb = kb0; kb < kb1; ++kb) {
-                const bool chunk_first = ((kb - kb0) % KC_STAGES) == 0;
-                const bool chunk_last = ((kb - kb0) % KC_STAGES) == KC_STAGES - 1 || kb == kb1 - 1;
+            for (int kb = 0; kb < num_k; ++kb) {
+                const bool chunk_first = (kb % KC_STAGES) == 0;
+                const bool chunk_last = (kb % KC_STAGES) == KC_STAGES - 1 || kb == num_k - 1;
                 mbar_wait(&km_full[ks], kph);
                 const uint32_t a_hi = smem_u32(km_base + ks * Cfg::KM_BYTES) + wg * 64 * 16;
                 const uint32_t b_hi = smem_u32(km_base + ks * Cfg::KM_BYTES) + KM_A_BYTES;
@@ -374,8 +369,8 @@ syrk_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
                 }
             }
             // write-back.  Accumulator fragment: register 4 j + 2 h + e holds row 16 wq + g + 8 h, column 8 j + 2 tq + e.
-            // beta == 1 adds with fire-and-forget reductions (C is not read by the SM); every element is touched once per launch
-            // (or by the two ranges of a split K onto a zeroed C), so the result is the single rounding of old + alpha * sum.
+            // beta == 1 adds with fire-and-forget reductions (C is not read by the SM); every element is touched once per launch,
+            // so the result is the single rounding of old + alpha * sum.
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int i = tile.x * BM + wg * 64 + wq * 16 + g + 8 * h;
@@ -443,9 +438,8 @@ int make_map(sd_ctx* ctx, CUtensorMap* map, const float* base, int64_t ld, int r
 
 }  // namespace
 
-bool sd_syrk_tc_supported(const float* d_S, int64_t lds, int K, int MI, int NJ, const float* d_C, int64_t ldc)
+bool sd_syrk_tc_supported(const float* d_S, int64_t lds, int K)
 {
-    (void)MI; (void)NJ; (void)d_C; (void)ldc;
     // TMA needs a 16-byte aligned base and row pitch
     return K >= 1 && (reinterpret_cast<uintptr_t>(d_S) & 15) == 0 && (lds % 4) == 0;
 }
@@ -461,14 +455,15 @@ struct sd_tc_plan {
 static_assert(sizeof(sd_tc_plan) <= SD_TC_PLAN_BYTES, "sd_tc_plan storage");
 
 // C[i,j] = beta*C[i,j] + alpha * sum_{k<K} SA[k,i] * SB[k,j],  i < MI, j < NJ.   SA: K x MI (lda), SB: K x NJ (ldb), both row-major,
-// i.e. both operands MN-major.  upper_only keeps the tiles that intersect j >= i (SYRK: SA == SB).  `rows` (optional) keeps the
-// tiles whose C rows belong to this rank's block rows (distributed trailing update).  C may alias SB when every CTA's column
-// range of SB is read completely before its tile is written: true for MI <= 128 (one tile row; each tile's operand columns are
-// its own output columns).  d_tiles: device buffer for the tile list (at least sd_tc_max_tiles(MI, NJ) int2), or NULL to use the
-// context's workspace.  *empty is set when no tile survives the filters (nothing to launch).
+// i.e. both operands MN-major.  passes: 3 = 3xTF32 split (unbiased: hi rounded), 1 = one TF32 pass.  upper_only keeps the tiles
+// that intersect j >= i (SYRK: SA == SB).  `rows` (optional) keeps the tiles whose C rows this rank owns (distributed trailing
+// update).  C may alias SB when every CTA's column range of SB is read completely before its tile is written: true for MI <= 128
+// (one tile row; each tile's operand columns are its own output columns).  d_tiles: device buffer for the tile list (at least
+// sd_tc_max_tiles(MI, NJ) int2), or NULL to use the context's workspace.  *empty is set when no tile survives the filters
+// (nothing to launch).
 int sd_gemm_tn_tc_prepare(sd_ctx* ctx, const float* d_SA, int64_t lda, const float* d_SB, int64_t ldb, int K, int MI, int NJ,
-                          float* d_C, int64_t ldc, float alpha, float beta, int passes, bool unbiased_split, bool upper_only,
-                          const sd_row_filter* rows, int ksplit, void* d_tiles_buf, void* plan_storage, bool* empty, bool narrow, int a_strip_rows)
+                          float* d_C, int64_t ldc, float alpha, float beta, int passes, bool unbiased, bool upper_only,
+                          const sd_row_filter* rows, void* d_tiles_buf, void* plan_storage, bool* empty, bool narrow, int a_strip_rows)
 {
     sd_tc_plan* plan = reinterpret_cast<sd_tc_plan*>(plan_storage);
     *empty = true;
@@ -491,30 +486,23 @@ int sd_gemm_tn_tc_prepare(sd_ctx* ctx, const float* d_SA, int64_t lda, const flo
     for (int si = 0; si < TI; si += GI)
         for (int sj = 0; sj < TJ; sj += GJ)
             for (int ti = si; ti < si + GI && ti < TI; ++ti) {
-                if (rows && rows->nranks > 1 && ((rows->first_row + (int64_t)ti * BM) / rows->block) % rows->nranks != rows->rank) continue;
+                if (rows && rows->nranks > 1 && sd_panel_owner(rows->first_row + (int64_t)ti * BM, rows->nranks) != rows->rank) continue;
                 for (int tj = sj; tj < sj + GJ && tj < TJ; ++tj)
                     if (!upper_only || tj * BN + BN - 1 >= ti * BM) tiles.push_back(make_int2(ti, tj));
             }
     if (tiles.empty()) return SD_OK;
     int2* d_tiles = (int2*)d_tiles_buf;
-    if (!d_tiles) d_tiles = (int2*)sd_workspace(ctx, SD_WS_DIAGINV, tiles.size() * sizeof(int2));
+    if (!d_tiles) d_tiles = (int2*)sd_workspace(ctx, SD_WS_TC_TILES, tiles.size() * sizeof(int2));
     if (!d_tiles) return SD_ERR_CUDA;
     SD_CUDA(ctx, cudaMemcpyAsync(d_tiles, tiles.data(), tiles.size() * sizeof(int2), cudaMemcpyHostToDevice, ctx->stream));
 
     TcArgs& a = plan->args;
     a.K = K; a.MI = MI; a.NJ = NJ; a.C = d_C; a.ldc = ldc; a.alpha = alpha; a.beta = beta; a.passes = passes;
-    a.unbiased = (ctx->gram_mode == 3 || unbiased_split) ? 1 : 0;
+    a.unbiased = unbiased ? 1 : 0;
     a.a_strip = a_strip_rows;
-    const int num_k = sd_div_up(K, BK);
-    if (ksplit < 1) ksplit = 1;
-    if (ksplit > num_k) ksplit = num_k;
-    a.kps = sd_div_up(num_k, ksplit);
-    a.ksplit = sd_div_up(num_k, a.kps);                   // every range non-empty
-    a.tiles = d_tiles; a.num_tiles = (int)tiles.size() * a.ksplit;
+    a.tiles = d_tiles; a.num_tiles = (int)tiles.size();
     const int sms = ctx->sm_count - ctx->syrk_sm_reserve > 0 ? ctx->sm_count - ctx->syrk_sm_reserve : 1;
     plan->grid = a.num_tiles < sms ? a.num_tiles : sms;
-    // split K: the ranges of one tile add into C in any order, which is only reproducible for two of them (a + b == b + a)
-    SD_REQUIRE(ctx, a.ksplit == 1 || (beta == 1.f && a.ksplit == 2), "split-K needs beta == 1 (reduce-add write-back) and two ranges");
     plan->bn = BN;
     if (BN == 64) SD_CUDA(ctx, cudaFuncSetAttribute(syrk_wgmma_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<64>::SMEM_BYTES));
     else SD_CUDA(ctx, cudaFuncSetAttribute(syrk_wgmma_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<128>::SMEM_BYTES));
@@ -533,20 +521,13 @@ int sd_gemm_tn_tc_launch(sd_ctx* ctx, const void* plan_storage)
     return SD_OK;
 }
 
-int sd_gemm_tn_tc(sd_ctx* ctx, const float* d_SA, int64_t lda, const float* d_SB, int64_t ldb, int K, int MI, int NJ,
-                  float* d_C, int64_t ldc, float alpha, float beta, int passes, bool unbiased_split, bool upper_only,
-                  const sd_row_filter* rows, int ksplit)
+int sd_syrk_tc(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ, float* d_C, int64_t ldc, float alpha, float beta,
+               int passes, bool unbiased, const sd_row_filter* rows)
 {
     alignas(64) unsigned char storage[SD_TC_PLAN_BYTES];
     bool empty = true;
-    int rc = sd_gemm_tn_tc_prepare(ctx, d_SA, lda, d_SB, ldb, K, MI, NJ, d_C, ldc, alpha, beta, passes, unbiased_split, upper_only, rows, ksplit,
+    int rc = sd_gemm_tn_tc_prepare(ctx, d_S, lds, d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta, passes, unbiased, true, rows,
                                    nullptr, storage, &empty, false, 0);
     if (rc || empty) return rc;
     return sd_gemm_tn_tc_launch(ctx, storage);
-}
-
-int sd_syrk_tc(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ, float* d_C, int64_t ldc,
-               float alpha, float beta, int passes, bool unbiased_split, const sd_row_filter* rows)
-{
-    return sd_gemm_tn_tc(ctx, d_S, lds, d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta, passes, unbiased_split, true, rows);
 }

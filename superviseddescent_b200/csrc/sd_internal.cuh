@@ -15,13 +15,17 @@
 #define SD_MAX_EYES 4
 #define SD_MAX_BINS 16   // undirected orientations K supported by the HOG kernel
 
-enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_DIAGINV,
+enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_PARTIAL, SD_WS_GEOM, SD_WS_GEMM_PARTIAL, SD_WS_DIAGINV2, SD_WS_PANEL, SD_WS_BIAS, SD_WS_CG, SD_WS_CGMAT, SD_WS_COUNT };
 
-// Block-row ownership of a distributed factorisation: global row r of the matrix belongs to rank (r / block) % nranks.
-// first_row = global row of the first row of the C sub-matrix a kernel is launched on.
+// Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row
+// Cholesky blocks), and panel p belongs to rank p % nranks.  The Gram exchange delivers each panel's rows to their owner, and
+// every step of the solve that splits work over the ranks splits it the same way.
+constexpr int SD_PANEL_ROWS = 256;
+__host__ __device__ inline int sd_panel_owner(int64_t row, int nranks) { return (int)(row / SD_PANEL_ROWS) % nranks; }
+
+// The rows of a C sub-matrix that this rank owns; first_row = global row of the sub-matrix's first row.
 struct sd_row_filter {
-    int block;
     int nranks, rank;
     int64_t first_row;
 };
@@ -87,25 +91,13 @@ static inline int sd_div_up(int64_t a, int64_t b) { return (int)((a + b - 1) / b
 
 // ---- internal entry points shared between translation units ---------------------------------
 
-// C[i,j] = beta*C[i,j] + alpha * sum_{k<K} S[k,i] * S[k,j]   for i < MI, j < NJ, restricted to the
-// tiles that intersect j >= i (upper triangle).  S: K x NJ row-major (lds), C: MI x NJ (ldc).
-// Used for the Gram matrix [A^T A | A^T B] and for the Cholesky trailing update.
-// path: 0 = choose by size, 1 = tensor cores whenever the operands allow it, 2 = fp32 SIMT.  A factorisation step
-// passes the same choice for every piece of one rank-k update (mixing the two kernels inside one update was measured
-// to double the error of the solved weights).  unbiased_split: round the hi operand (gram mode 3) for this call.
-int sd_syrk_update(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ,
-                   float* d_C, int64_t ldc, float alpha, float beta, int path = 0, bool unbiased_split = false,
-                   const sd_row_filter* rows = nullptr);
-int sd_syrk_simt(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ,
-                 float* d_C, int64_t ldc, float alpha, float beta);
-int sd_syrk_tc(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ,
-               float* d_C, int64_t ldc, float alpha, float beta, int passes, bool unbiased_split = false,
-               const sd_row_filter* rows = nullptr);
-// C = beta*C + alpha * SA^T SB on the tensor cores (SA: K x MI, SB: K x NJ, row-major); see sd_gram_tc.cu
-int sd_gemm_tn_tc(sd_ctx* ctx, const float* d_SA, int64_t lda, const float* d_SB, int64_t ldb, int K, int MI, int NJ,
-                  float* d_C, int64_t ldc, float alpha, float beta, int passes, bool unbiased_split, bool upper_only,
-                  const sd_row_filter* rows = nullptr, int ksplit = 1);
-bool sd_syrk_tc_supported(const float* d_S, int64_t lds, int K, int MI, int NJ, const float* d_C, int64_t ldc);
+// Tensor-core SYRK (sd_gram_tc.cu): C[i,j] = beta*C[i,j] + alpha * sum_{k<K} S[k,i] * S[k,j] for i < MI, j < NJ, on the
+// tiles that intersect j >= i.  S: K x NJ row-major (lds), C: MI x NJ (ldc).  passes: 3 = 3xTF32 split, 1 = one TF32 pass;
+// unbiased: round the hi part of the split.  rows (optional): only the tiles of rows this rank owns.
+int sd_syrk_tc(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ, float* d_C, int64_t ldc, float alpha, float beta,
+               int passes, bool unbiased, const sd_row_filter* rows);
+// whether the tensor-core kernel can read S (TMA alignment)
+bool sd_syrk_tc_supported(const float* d_S, int64_t lds, int K);
 
 int sd_check_hog_status(sd_ctx* ctx, const char* what);   // sd_api.cu: synchronises, reports and clears the projection's flags
 
@@ -115,8 +107,8 @@ int sd_gram_rank(sd_ctx* ctx, const float* d_G, int64_t ldg, int D, int* rank_ou
 // prepared launches of the tensor-core TN-GEMM (sd_gram_tc.cu): plan_storage = SD_TC_PLAN_BYTES bytes, 64-byte aligned
 #define SD_TC_PLAN_BYTES 640
 int sd_gemm_tn_tc_prepare(sd_ctx* ctx, const float* d_SA, int64_t lda, const float* d_SB, int64_t ldb, int K, int MI, int NJ,
-                          float* d_C, int64_t ldc, float alpha, float beta, int passes, bool unbiased_split, bool upper_only,
-                          const sd_row_filter* rows, int ksplit, void* d_tiles_buf, void* plan_storage, bool* empty,
+                          float* d_C, int64_t ldc, float alpha, float beta, int passes, bool unbiased, bool upper_only,
+                          const sd_row_filter* rows, void* d_tiles_buf, void* plan_storage, bool* empty,
                           bool narrow = false /* a single tile column of <= 192 columns may use the narrow-N kernel variants */,
                           int a_strip_rows = 0 /* > 0: operand A strip-major, see sd_gram_tc.cu */);
 int sd_gemm_tn_tc_launch(sd_ctx* ctx, const void* plan_storage);

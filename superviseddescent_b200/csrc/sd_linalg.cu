@@ -99,8 +99,63 @@ __global__ void syrk_reduce_kernel(const float* __restrict__ partial, int splits
     }
 }
 
+int syrk_simt(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ, float* d_C, int64_t ldc, float alpha, float beta)
+{
+    if (MI <= 0 || NJ <= 0) return SD_OK;
+    dim3 grid(sd_div_up(NJ, ST), sd_div_up(MI, ST), 1);
+    SD_REQUIRE(ctx, grid.y <= 65535, "matrix too large for the SIMT SYRK");
+    const long long tiles = (long long)grid.x * grid.y;
+    int splits = 1;
+    if (tiles < 2LL * ctx->sm_count && K > 2048) {
+        splits = (int)((4LL * ctx->sm_count + tiles - 1) / tiles);
+        const int maxs = sd_div_up(K, 512);
+        if (splits > maxs) splits = maxs;
+        if (splits > 64) splits = 64;
+        if (splits < 1) splits = 1;
+    }
+    if (splits == 1) {
+        syrk_simt_kernel<<<grid, 256, 0, ctx->stream>>>(d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta, nullptr, K);
+        SD_LAUNCH_CHECK(ctx, "syrk_simt_kernel");
+    } else {
+        float* partial = (float*)sd_workspace(ctx, SD_WS_PARTIAL, (size_t)splits * MI * NJ * sizeof(float));
+        if (!partial) return SD_ERR_CUDA;
+        const int kps = sd_div_up(sd_div_up(K, splits), SK) * SK;
+        grid.z = sd_div_up(K, kps);
+        syrk_simt_kernel<<<grid, 256, 0, ctx->stream>>>(d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta, partial, kps);
+        SD_LAUNCH_CHECK(ctx, "syrk_simt_kernel(split)");
+        const int blocks = sd_div_up((int64_t)MI * NJ, 256) > 2048 ? 2048 : sd_div_up((int64_t)MI * NJ, 256);
+        syrk_reduce_kernel<<<blocks, 256, 0, ctx->stream>>>(partial, (int)grid.z, MI, NJ, d_C, ldc, alpha, beta);
+        SD_LAUNCH_CHECK(ctx, "syrk_reduce_kernel");
+    }
+    return SD_OK;
+}
+
+// the size rule of the tensor-core SYRK: below it the SIMT kernel is faster
+bool syrk_is_big(int K, int64_t MI, int64_t NJ)
+{
+    constexpr long long tc_min = 256LL * 256LL;
+    return MI * NJ >= tc_min && K >= 64;
+}
+
+// C[i,j] = beta*C[i,j] + alpha * sum_{k<K} S[k,i] * S[k,j] for i < MI, j < NJ, on the tiles that intersect j >= i: the Gram
+// matrix [A^T A | A^T B] and the trailing updates of the Cholesky.  S: K x NJ row-major (lds), C: MI x NJ (ldc).
+// The one place that reads the gram mode (sd_set_gram_mode):
+//   tensor cores when `big` (the size rule's verdict for the product this call belongs to), mode != 2 and TMA can read S,
+//     3xTF32 (1 pass in mode 1), hi rounded in mode 3 or when the caller asks for the unbiased split;
+//   fp32 SIMT otherwise.
+// rows (optional): the tensor-core route skips the tiles of rows other ranks own.  The SIMT kernel updates every row: rows of
+// other ranks are never read before their owner's broadcast overwrites them.
+int syrk_upper(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ, float* d_C, int64_t ldc, float alpha, float beta,
+               bool big, bool unbiased, const sd_row_filter* rows = nullptr)
+{
+    if (big && ctx->gram_mode != 2 && sd_syrk_tc_supported(d_S, lds, K))
+        return sd_syrk_tc(ctx, d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta, ctx->gram_mode == 1 ? 1 : 3,
+                          unbiased || ctx->gram_mode == 3, rows);
+    return syrk_simt(ctx, d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta);
+}
+
 // =================================================================================================
-// GEMM NN: C[N x M] = beta*C + alpha * A[N x D] * B[D x M], with the cascade-update epilogue
+// GEMM NN: out[N x M] = A[N x D] * B[D x M], with the cascade-update epilogue
 // =================================================================================================
 constexpr int GT = 64, GK = 16;
 
@@ -111,11 +166,20 @@ struct GemmEpilogue {
     sd_eyes_dev eyes;
 };
 
+// 1 / normalisation of row i of x: the model's normalisation is ones / ied (model.hpp:97), and the cascade divides the
+// regressor's output by it (superviseddescent.hpp:213)
+__device__ __forceinline__ float inv_normaliser(const GemmEpilogue& ep, int i, int M)
+{
+    if (ep.eyes.kind != 1) return 1.0f;
+    const double ied = sd_device_ied(ep.x + (long long)i * M, M / 2, ep.eyes);
+    return __fdiv_rn(1.0f, (float)__ddiv_rn(1.0, ied));
+}
+
 // blockIdx.z = split along D; with gridDim.z > 1 every split writes its partial sums (double) to
 // `partial` [split][N][M] and gemm_finalize_kernel reduces them in a fixed order.
 __global__ void __launch_bounds__(256) gemm_nn_kernel(const float* __restrict__ A, long long lda, int N, int D,
                                                       const float* __restrict__ B, long long ldb, int M,
-                                                      float* __restrict__ C, long long ldc, float alpha, float beta,
+                                                      float* __restrict__ C, long long ldc,
                                                       const GemmEpilogue ep, double* __restrict__ partial, int k_per_split)
 {
     __shared__ __align__(16) float As[GK][GT + 4];     // transposed: As[k][row]
@@ -126,16 +190,7 @@ __global__ void __launch_bounds__(256) gemm_nn_kernel(const float* __restrict__ 
     const int r0 = blockIdx.y * GT, c0 = blockIdx.x * GT;
     const int kbeg = blockIdx.z * k_per_split;
     const int kend = min(D, kbeg + k_per_split);
-    if (ep.mode == 1 && !partial && tid < GT) {
-        const int r = r0 + tid;
-        float inv_n = 1.0f;
-        if (r < N && ep.eyes.kind == 1) {
-            const double ied = sd_device_ied(ep.x + (long long)r * M, M / 2, ep.eyes);
-            const float n = (float)__ddiv_rn(1.0, ied);      // ones / ied           (model.hpp:97)
-            inv_n = __fdiv_rn(1.0f, n);                      // 1 / normalisation    (superviseddescent.hpp:213)
-        }
-        s_scale[tid] = inv_n;
-    }
+    if (ep.mode == 1 && !partial && tid < GT) s_scale[tid] = r0 + tid < N ? inv_normaliser(ep, r0 + tid, M) : 1.0f;
     // cv::gemm accumulates float products in double (the reference's predict, regressors.hpp:379).
     // Here: fp32 FMA inside a 16-deep k chunk, chunk sums added into double accumulators.
     double acc[4][4] = {};
@@ -209,8 +264,7 @@ __global__ void __launch_bounds__(256) gemm_nn_kernel(const float* __restrict__ 
                 const float upd = __fmul_rn(accf, s_scale[ty * 4 + r]);
                 ep.x_next[(long long)i * M + j] = __fsub_rn(ep.x[(long long)i * M + j], upd);
             } else {
-                float* p = C + (long long)i * ldc + j;
-                *p = (beta == 0.f) ? alpha * accf : fmaf(alpha, accf, beta * (*p));
+                C[(long long)i * ldc + j] = accf;
             }
         }
     }
@@ -294,15 +348,11 @@ __global__ void __launch_bounds__(PR_ROWS, 1) predict_rows_kernel(const float* _
 
 // sums the split partials in a fixed order (double) and applies the epilogue
 __global__ void gemm_finalize_kernel(const double* __restrict__ partial, int splits, int N, int M,
-                                     float* __restrict__ C, long long ldc, float alpha, float beta, const GemmEpilogue ep)
+                                     float* __restrict__ C, long long ldc, const GemmEpilogue ep)
 {
     const int i = blockIdx.x * blockDim.y + threadIdx.y;
     if (i >= N) return;
-    float inv_n = 1.0f;
-    if (ep.mode == 1 && ep.eyes.kind == 1) {
-        const double ied = sd_device_ied(ep.x + (long long)i * M, M / 2, ep.eyes);
-        inv_n = __fdiv_rn(1.0f, (float)__ddiv_rn(1.0, ied));
-    }
+    const float inv_n = ep.mode == 1 ? inv_normaliser(ep, i, M) : 1.0f;
     for (int j = threadIdx.x; j < M; j += blockDim.x) {
         double s = 0.0;
         for (int z = 0; z < splits; ++z) s += partial[((long long)z * N + i) * M + j];
@@ -310,14 +360,13 @@ __global__ void gemm_finalize_kernel(const double* __restrict__ partial, int spl
         if (ep.mode == 1) {
             ep.x_next[(long long)i * M + j] = __fsub_rn(ep.x[(long long)i * M + j], __fmul_rn(accf, inv_n));
         } else {
-            float* p = C + (long long)i * ldc + j;
-            *p = (beta == 0.f) ? alpha * accf : fmaf(alpha, accf, beta * (*p));
+            C[(long long)i * ldc + j] = accf;
         }
     }
 }
 
 int launch_gemm_nn(sd_ctx* ctx, const float* A, int64_t lda, int N, int D, const float* B, int64_t ldb, int M,
-                   float* C, int64_t ldc, float alpha, float beta, const GemmEpilogue& ep)
+                   float* C, int64_t ldc, const GemmEpilogue& ep)
 {
     if (N <= 0 || M <= 0) return SD_OK;
     // the cascade's shape -- a long contraction, 2L output columns -- goes to the row-per-thread kernel for ANY number of rows: its
@@ -337,7 +386,7 @@ int launch_gemm_nn(sd_ctx* ctx, const float* A, int64_t lda, int N, int D, const
         predict_rows_kernel<<<pgrid, PR_ROWS, 0, ctx->stream>>>(A, lda, N, D, B, ldb, M, partial, kps);
         SD_LAUNCH_CHECK(ctx, "predict_rows_kernel");
         dim3 fblock(32, 8);
-        gemm_finalize_kernel<<<sd_div_up(N, 8), fblock, 0, ctx->stream>>>(partial, splits, N, M, C, ldc, alpha, beta, ep);
+        gemm_finalize_kernel<<<sd_div_up(N, 8), fblock, 0, ctx->stream>>>(partial, splits, N, M, C, ldc, ep);
         SD_LAUNCH_CHECK(ctx, "gemm_finalize_kernel");
         return SD_OK;
     }
@@ -354,7 +403,7 @@ int launch_gemm_nn(sd_ctx* ctx, const float* A, int64_t lda, int N, int D, const
         if (splits < 1) splits = 1;
     }
     if (splits == 1) {
-        gemm_nn_kernel<<<grid, 256, 0, ctx->stream>>>(A, lda, N, D, B, ldb, M, C, ldc, alpha, beta, ep, nullptr, D);
+        gemm_nn_kernel<<<grid, 256, 0, ctx->stream>>>(A, lda, N, D, B, ldb, M, C, ldc, ep, nullptr, D);
         SD_LAUNCH_CHECK(ctx, "gemm_nn_kernel");
         return SD_OK;
     }
@@ -362,10 +411,10 @@ int launch_gemm_nn(sd_ctx* ctx, const float* A, int64_t lda, int N, int D, const
     grid.z = sd_div_up(D, kps);
     double* partial = (double*)sd_workspace(ctx, SD_WS_GEMM_PARTIAL, (size_t)grid.z * N * M * sizeof(double));
     if (!partial) return SD_ERR_CUDA;
-    gemm_nn_kernel<<<grid, 256, 0, ctx->stream>>>(A, lda, N, D, B, ldb, M, C, ldc, alpha, beta, ep, partial, kps);
+    gemm_nn_kernel<<<grid, 256, 0, ctx->stream>>>(A, lda, N, D, B, ldb, M, C, ldc, ep, partial, kps);
     SD_LAUNCH_CHECK(ctx, "gemm_nn_kernel(split)");
     dim3 fblock(32, 8);
-    gemm_finalize_kernel<<<sd_div_up(N, 8), fblock, 0, ctx->stream>>>(partial, (int)grid.z, N, M, C, ldc, alpha, beta, ep);
+    gemm_finalize_kernel<<<sd_div_up(N, 8), fblock, 0, ctx->stream>>>(partial, (int)grid.z, N, M, C, ldc, ep);
     SD_LAUNCH_CHECK(ctx, "gemm_finalize_kernel");
     return SD_OK;
 }
@@ -477,18 +526,17 @@ __global__ void __launch_bounds__(256) centre_kernel(float* __restrict__ A, long
 // sum of squares of the full symmetric D x D matrix from its upper triangle, in double (cv::norm)
 // Rows are dealt round-robin to the blocks (balanced triangle), a block's 1024 threads stride along the row with
 // four independent loads in flight each; fixed grid and fixed order, so the sum is reproducible.
-// own_block/nranks/rank: only the rows of this rank's block rows are summed (distributed solve; the partial sums are then
-// all-reduced).
+// nranks/rank: only the rows this rank owns are summed (distributed solve; the partial sums are then all-reduced).
 // Centred features (mu != NULL): G is the Gram of the rows shifted by mu (bias column unshifted, so G[:, D-1] = s' = A_c^T 1);
 // the norm is taken of the uncentred matrix it stands for,  G[i][j] + s'_i mu_j + mu_i s'_j + n mu_i mu_j  (bias column:
 // G[i][D-1] + n mu_i), entry by entry in double.  sv = s' (bias_extract_kernel), n = global sample count.
 __global__ void __launch_bounds__(1024) frob_upper_centred_kernel(const float* __restrict__ G, long long ldg, int D, double* __restrict__ out,
-                                                                  int own_block, int nranks, int rank, const float* __restrict__ mu,
+                                                                  int nranks, int rank, const float* __restrict__ mu,
                                                                   const double* __restrict__ sv, double n)
 {
     double s0 = 0.0;
     for (int i = blockIdx.x; i < D; i += gridDim.x) {
-        if (nranks > 1 && (i / own_block) % nranks != rank) continue;
+        if (nranks > 1 && sd_panel_owner(i, nranks) != rank) continue;
         const float* row = G + (long long)i * ldg;
         const double mi = (double)mu[i], si = i < D - 1 ? sv[i] : 0.0;
         for (int j = i + threadIdx.x; j < D; j += 1024) {
@@ -509,11 +557,11 @@ __global__ void __launch_bounds__(1024) frob_upper_centred_kernel(const float* _
 }
 
 __global__ void __launch_bounds__(1024) frob_upper_kernel(const float* __restrict__ G, long long ldg, int D, double* __restrict__ out,
-                                                          int own_block, int nranks, int rank)
+                                                          int nranks, int rank)
 {
     double s0 = 0.0, s1 = 0.0;
     for (int i = blockIdx.x; i < D; i += gridDim.x) {
-        if (nranks > 1 && (i / own_block) % nranks != rank) continue;
+        if (nranks > 1 && sd_panel_owner(i, nranks) != rank) continue;
         const float* row = G + (long long)i * ldg;
         if (threadIdx.x == 0) { const double v = (double)row[i]; s0 -= 0.5 * v * v; }  // the diagonal counts once, everything is doubled below
         int j = i + threadIdx.x;
@@ -577,12 +625,12 @@ __global__ void add_diag_kernel(float* __restrict__ G, long long ldg, int D, con
 // would pick that column first as well.
 //   sv[0..D-2] = s (the bias column above the diagonal), sv[D-1] = pivot, sv[D..D+M) = the bias row of the right-hand sides
 __global__ void bias_extract_kernel(const float* __restrict__ G, long long ldg, int D, int M, double* __restrict__ sv,
-                                    int own_block, int nranks, int rank)
+                                    int nranks, int rank)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= D + M) return;
     const int row = i < D ? i : D - 1;
-    const bool mine = nranks <= 1 || (row / own_block) % nranks == rank;       // others contribute zero to the all-reduce
+    const bool mine = nranks <= 1 || sd_panel_owner(row, nranks) == rank;       // others contribute zero to the all-reduce
     double v = 0.0;
     if (mine) v = (double)(i < D ? G[(long long)i * ldg + (D - 1)] : G[(long long)(D - 1) * ldg + i]);
     sv[i] = v;
@@ -593,12 +641,12 @@ __global__ void bias_extract_kernel(const float* __restrict__ G, long long ldg, 
 // part (shared CG route, where a rank only ever reads what its slab [k0, k1) of the product touches): 0 = everything,
 // 1 = the slab's rows, the slab's columns above them and the right-hand sides, 2 = the rest (before a fall-back to the factorisation).
 __global__ void __launch_bounds__(256) bias_downdate_kernel(float* __restrict__ G, long long ldg, int D, int M,
-                                                            const double* __restrict__ sv, int own_block, int nranks, int rank,
+                                                            const double* __restrict__ sv, int nranks, int rank,
                                                             int part, int k0, int k1)
 {
     const double inv_p = 1.0 / sv[D - 1];
     for (int i = blockIdx.x; i < D - 1; i += gridDim.x) {
-        if (nranks > 1 && (i / own_block) % nranks != rank) continue;
+        if (nranks > 1 && sd_panel_owner(i, nranks) != rank) continue;
         const double f = sv[i] * inv_p;
         float* row = G + (long long)i * ldg;
         const bool slab_row = i >= k0 && i < k1;
@@ -1202,14 +1250,10 @@ int launch_trsm_apply(sd_ctx* ctx, cudaStream_t stream, float* B, int64_t ldb, i
     return SD_OK;
 }
 
-bool sd_syrk_is_big(int K, int64_t MI, int64_t NJ)
-{
-    constexpr long long tc_min = 256LL * 256LL;
-    return MI * NJ >= tc_min && K >= 64;
-}
+static_assert(SD_PANEL_ROWS == 2 * kCholNb, "a factorisation panel is two Cholesky blocks");
 
 // comm (optional, more than one rank): DISTRIBUTED factorisation.  Block-row-cyclic ownership in units of one 256-row panel
-// (rank = panel % nranks): on entry every rank holds the summed rows of its own panels (sd_reduce_scatter_gram), the other rows
+// (sd_panel_owner): on entry every rank holds the summed rows of its own panels (sd_reduce_scatter_gram), the other rows
 // are undefined.  The owner factors its panel (chain + block-row solve), broadcasts the finished panel rows [P1;P2] (and the
 // inverses of the two diagonal blocks) over NVLink, and every rank applies the rank-256 update to the block rows it owns.  The
 // look-ahead is kept: the owner of panel p+1 updates that panel first and factors its diagonal blocks on the second stream while
@@ -1237,8 +1281,6 @@ int cholesky_solve(sd_ctx* ctx, float* G, int64_t ldg, int D, int M, float* X, s
     }
     cudaStream_t main_s = ctx->stream, chain_s = ctx->chain_stream;
     cudaEvent_t ev_head = ctx->chain_ev[0], ev_chain = ctx->chain_ev[1];
-    GemmEpilogue ep;
-    memset(&ep, 0, sizeof(ep));
     // ---- factorisation G = U^T U in 256-row panels (two 128-blocks), carrying the right-hand sides along (Y = U^-T R) ----
     //   chain(p)  [one SM]  : A11 = U11^T U11 ; P1a = U11^-T A12 ; A22 - P1a^T P1a = U22^T U22           (diagonal blocks)
     //   bulk(p)             : P1 = U11^-T [rest of block row 1] ; P2 = U22^-T ([rest of block row 2] - P1a^T P1)
@@ -1280,8 +1322,8 @@ int cholesky_solve(sd_ctx* ctx, float* G, int64_t ldg, int D, int M, float* X, s
     for (int b = 0; b < nblocks; b += 2) {
         int j, nb1, nb2;
         panel_dims(b, j, nb1, nb2);
-        const int owner = dist ? (b / 2) % nranks : me;
-        const int next_owner = dist ? (b / 2 + 1) % nranks : me;
+        const int owner = dist ? sd_panel_owner(j, nranks) : me;
+        const int next_owner = dist ? sd_panel_owner(j + SD_PANEL_ROWS, nranks) : me;
         const int j3 = j + nb1 + nb2;                                 // first column right of the panel
         const int cols3 = W_ - j3;
         float* W1 = inv + (size_t)b * 2 * PB * PB;
@@ -1314,14 +1356,15 @@ int cholesky_solve(sd_ctx* ctx, float* G, int64_t ldg, int D, int M, float* X, s
         const int rest = D - j3;                                      // rows (= diagonal columns) below the panel
         if (rest <= 0) continue;
         const int kp = nb1 + nb2;                                     // rows of [P1;P2], contiguous in G
-        const int head = rest < 2 * kCholNb ? rest : 2 * kCholNb;
+        const int head = rest < SD_PANEL_ROWS ? rest : SD_PANEL_ROWS;
         float* C3 = G + (int64_t)j3 * ldg + j3;
-        // one kernel family per rank-kp update, chosen from the size of the whole trailing matrix; the updates use the
-        // unbiased hi/lo split: a truncated hi leaves a one-signed lo*lo term behind, which is harmless in the Gram (it
-        // scales [AtA|Atb] almost uniformly) but is amplified by the cancellation inside Schur complements
-        const int path = sd_syrk_is_big(kp, rest, cols3) ? 1 : 2;
+        // one kernel family per rank-kp update, chosen from the size of the whole trailing matrix (mixing the two kernels inside
+        // one update was measured to double the error of the solved weights); the updates use the unbiased hi/lo split: a
+        // truncated hi leaves a one-signed lo*lo term behind, which is harmless in the Gram (it scales [AtA|Atb] almost
+        // uniformly) but is amplified by the cancellation inside Schur complements
+        const bool big = syrk_is_big(kp, rest, cols3);
         if (me == next_owner) {
-            rc = sd_syrk_update(ctx, row1, ldg, kp, head, cols3, C3, ldg, -1.0f, 1.0f, path, true);
+            rc = syrk_upper(ctx, row1, ldg, kp, head, cols3, C3, ldg, -1.0f, 1.0f, big, true);
             if (rc) return rc;
             SD_CUDA(ctx, cudaEventRecord(ev_head, main_s));
             SD_CUDA(ctx, cudaStreamWaitEvent(chain_s, ev_head, 0));
@@ -1331,10 +1374,10 @@ int cholesky_solve(sd_ctx* ctx, float* G, int64_t ldg, int D, int M, float* X, s
         }
         if (rest > head) {
             sd_row_filter own;
-            own.block = 2 * kCholNb; own.nranks = nranks; own.rank = me; own.first_row = j3 + head;
+            own.nranks = nranks; own.rank = me; own.first_row = j3 + head;
             ctx->syrk_sm_reserve = (me == next_owner) ? 1 : 0;   // leave one SM to the chain running beside it
-            rc = sd_syrk_update(ctx, row1 + head, ldg, kp, rest - head, cols3 - head, C3 + (int64_t)head * ldg + head, ldg, -1.0f, 1.0f, path,
-                                true, dist ? &own : nullptr);
+            rc = syrk_upper(ctx, row1 + head, ldg, kp, rest - head, cols3 - head, C3 + (int64_t)head * ldg + head, ldg, -1.0f, 1.0f, big,
+                            true, dist ? &own : nullptr);
             ctx->syrk_sm_reserve = 0;
             if (rc) return rc;
         }
@@ -1386,51 +1429,6 @@ int check_status(sd_ctx* ctx, const char* what)
 }  // namespace
 
 // =================================================================================================
-// internal dispatch
-// =================================================================================================
-int sd_syrk_simt(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ, float* d_C, int64_t ldc,
-                 float alpha, float beta)
-{
-    if (MI <= 0 || NJ <= 0) return SD_OK;
-    dim3 grid(sd_div_up(NJ, ST), sd_div_up(MI, ST), 1);
-    SD_REQUIRE(ctx, grid.y <= 65535, "matrix too large for the SIMT SYRK");
-    const long long tiles = (long long)grid.x * grid.y;
-    int splits = 1;
-    if (tiles < 2LL * ctx->sm_count && K > 2048) {
-        splits = (int)((4LL * ctx->sm_count + tiles - 1) / tiles);
-        const int maxs = sd_div_up(K, 512);
-        if (splits > maxs) splits = maxs;
-        if (splits > 64) splits = 64;
-        if (splits < 1) splits = 1;
-    }
-    if (splits == 1) {
-        syrk_simt_kernel<<<grid, 256, 0, ctx->stream>>>(d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta, nullptr, K);
-        SD_LAUNCH_CHECK(ctx, "syrk_simt_kernel");
-    } else {
-        float* partial = (float*)sd_workspace(ctx, SD_WS_PARTIAL, (size_t)splits * MI * NJ * sizeof(float));
-        if (!partial) return SD_ERR_CUDA;
-        const int kps = sd_div_up(sd_div_up(K, splits), SK) * SK;
-        grid.z = sd_div_up(K, kps);
-        syrk_simt_kernel<<<grid, 256, 0, ctx->stream>>>(d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta, partial, kps);
-        SD_LAUNCH_CHECK(ctx, "syrk_simt_kernel(split)");
-        const int blocks = sd_div_up((int64_t)MI * NJ, 256) > 2048 ? 2048 : sd_div_up((int64_t)MI * NJ, 256);
-        syrk_reduce_kernel<<<blocks, 256, 0, ctx->stream>>>(partial, (int)grid.z, MI, NJ, d_C, ldc, alpha, beta);
-        SD_LAUNCH_CHECK(ctx, "syrk_reduce_kernel");
-    }
-    return SD_OK;
-}
-
-int sd_syrk_update(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ, float* d_C, int64_t ldc,
-                   float alpha, float beta, int path, bool unbiased_split, const sd_row_filter* rows)
-{
-    const bool want_tc = path == 1 || (path == 0 && sd_syrk_is_big(K, MI, NJ));
-    if (ctx->gram_mode != 2 && path != 2 && want_tc && sd_syrk_tc_supported(d_S, lds, K, MI, NJ, d_C, ldc))
-        return sd_syrk_tc(ctx, d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta, ctx->gram_mode == 1 ? 1 : 3, unbiased_split, rows);
-    // the SIMT kernel updates every row: rows of other ranks are never read before their owner's broadcast overwrites them
-    return sd_syrk_simt(ctx, d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta);
-}
-
-// =================================================================================================
 // C ABI
 // =================================================================================================
 extern "C" {
@@ -1453,7 +1451,7 @@ int sd_gram(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_B, int64_
         SD_LAUNCH_CHECK(ctx, "pack_ext_kernel");
         S = E;
     }
-    return sd_syrk_update(ctx, S, lds, N, D, D + M, d_G, ldg, 1.0f, 0.0f);
+    return syrk_upper(ctx, S, lds, N, D, D + M, d_G, ldg, 1.0f, 0.0f, syrk_is_big(N, D, D + M), false);
 }
 
 // route: 0 = every rank holds the summed G (one GPU, or after sd_allreduce_gram) and solves it alone;
@@ -1487,17 +1485,17 @@ static int solve_gram_impl(sd_ctx* ctx, sd_comm* comm, float* d_G, int64_t ldg, 
             // s' = bias column of the centred Gram, needed entry by entry for the norm of the uncentred matrix
             double* sv0 = (double*)sd_workspace(ctx, SD_WS_BIAS, (size_t)(D + M) * sizeof(double) + (size_t)(D - 1) * (M + 1) * sizeof(float));
             if (!sv0) return SD_ERR_CUDA;
-            bias_extract_kernel<<<sd_div_up(D + M, 256), 256, 0, ctx->stream>>>(d_G, ldg, D, M, sv0, 2 * kCholNb, dist ? nranks : 1, sd_comm_rank_of(comm));
+            bias_extract_kernel<<<sd_div_up(D + M, 256), 256, 0, ctx->stream>>>(d_G, ldg, D, M, sv0, dist ? nranks : 1, sd_comm_rank_of(comm));
             SD_LAUNCH_CHECK(ctx, "bias_extract_kernel");
             if (dist) {
                 int rc0 = sd_comm_allreduce_f64(ctx, comm, sv0, (size_t)(D + M), ctx->stream);
                 if (rc0) return rc0;
             }
-            frob_upper_centred_kernel<<<nparts, 1024, 0, ctx->stream>>>(d_G, ldg, D, partial, 2 * kCholNb, share_norm ? nranks : 1, sd_comm_rank_of(comm),
+            frob_upper_centred_kernel<<<nparts, 1024, 0, ctx->stream>>>(d_G, ldg, D, partial, share_norm ? nranks : 1, sd_comm_rank_of(comm),
                                                                         d_mu, sv0, (double)n_train_global);
             SD_LAUNCH_CHECK(ctx, "frob_upper_centred_kernel");
         } else {
-            frob_upper_kernel<<<nparts, 1024, 0, ctx->stream>>>(d_G, ldg, D, partial, 2 * kCholNb, share_norm ? nranks : 1, sd_comm_rank_of(comm));
+            frob_upper_kernel<<<nparts, 1024, 0, ctx->stream>>>(d_G, ldg, D, partial, share_norm ? nranks : 1, sd_comm_rank_of(comm));
             SD_LAUNCH_CHECK(ctx, "frob_upper_kernel");
         }
         if (share_norm) {
@@ -1534,7 +1532,7 @@ static int solve_gram_impl(sd_ctx* ctx, sd_comm* comm, float* d_G, int64_t ldg, 
         double* sv = (double*)sd_workspace(ctx, SD_WS_BIAS, (size_t)(D + M) * sizeof(double) + (size_t)(D - 1) * (M + 1) * sizeof(float));
         if (!sv) return SD_ERR_CUDA;
         float* Xp = reinterpret_cast<float*>(sv + D + M);
-        bias_extract_kernel<<<sd_div_up(D + M, 256), 256, 0, ctx->stream>>>(d_G, ldg, D, M, sv, 2 * kCholNb, nr, me);
+        bias_extract_kernel<<<sd_div_up(D + M, 256), 256, 0, ctx->stream>>>(d_G, ldg, D, M, sv, nr, me);
         SD_LAUNCH_CHECK(ctx, "bias_extract_kernel");
         if (dist) {
             rc = sd_comm_allreduce_f64(ctx, comm, sv, (size_t)(D + M), ctx->stream);
@@ -1546,7 +1544,7 @@ static int solve_gram_impl(sd_ctx* ctx, sd_comm* comm, float* d_G, int64_t ldg, 
         int k0 = 0, k1 = D - 1;
         const bool partial_downdate = try_cg && route == 2 && nranks > 1;
         if (partial_downdate) sd_cg_slab(D - 1, nranks, me, &k0, &k1);
-        bias_downdate_kernel<<<4 * ctx->sm_count, 256, 0, ctx->stream>>>(d_G, ldg, D, M, sv, 2 * kCholNb, nr, me, partial_downdate ? 1 : 0, k0, k1);
+        bias_downdate_kernel<<<4 * ctx->sm_count, 256, 0, ctx->stream>>>(d_G, ldg, D, M, sv, nr, me, partial_downdate ? 1 : 0, k0, k1);
         SD_LAUNCH_CHECK(ctx, "bias_downdate_kernel");
         bool solved = false;
         if (try_cg) {
@@ -1566,7 +1564,7 @@ static int solve_gram_impl(sd_ctx* ctx, sd_comm* comm, float* d_G, int64_t ldg, 
         }
         if (!solved) {
             if (partial_downdate) {
-                bias_downdate_kernel<<<4 * ctx->sm_count, 256, 0, ctx->stream>>>(d_G, ldg, D, M, sv, 2 * kCholNb, nr, me, 2, k0, k1);
+                bias_downdate_kernel<<<4 * ctx->sm_count, 256, 0, ctx->stream>>>(d_G, ldg, D, M, sv, nr, me, 2, k0, k1);
                 SD_LAUNCH_CHECK(ctx, "bias_downdate_kernel");
             }
             rc = cholesky_solve(ctx, d_G, ldg, D - 1, M + 1, Xp, dist ? comm : nullptr);
@@ -1588,6 +1586,28 @@ static int solve_gram_impl(sd_ctx* ctx, sd_comm* comm, float* d_G, int64_t ldg, 
     return rc;
 }
 
+// LinearRegressor::learn on this rank's rows: [A^T A | A^T B] into the workspace (ev[0] starts "At * A"), summed over the ranks
+// when there is more than one (route 1: each panel to its owner, otherwise to every rank), then solved.  shard: the rows are this
+// rank's share of the samples and may be none (G is zero then); otherwise sd_gram checks N.
+static int learn_impl(sd_ctx* ctx, sd_comm* comm, const float* d_A, int64_t lda, const float* d_B, int64_t ldb, int N, bool shard,
+                      int D, int M, const sd_regulariser* reg, int n_train_global, float* d_X, float* lambda_out, int* rank_out,
+                      int route, const float* d_mu = nullptr, float* d_Xc = nullptr)
+{
+    const int64_t ldg = ((int64_t)(D + M) + 3) / 4 * 4;
+    float* G = (float*)sd_workspace(ctx, SD_WS_SCRATCH, (size_t)D * ldg * sizeof(float));
+    if (!G) return SD_ERR_CUDA;
+    SD_CUDA(ctx, cudaEventRecord(ctx->ev[0], ctx->stream));
+    int rc;
+    if (N > 0 || !shard) rc = sd_gram(ctx, d_A, lda, d_B, ldb, N, D, M, G, ldg);
+    else rc = sd_check_cuda(ctx, cudaMemsetAsync(G, 0, (size_t)D * ldg * sizeof(float), ctx->stream), "memset(G)");
+    if (rc) return rc;
+    if (sd_comm_size_of(comm) > 1) {
+        rc = route == 1 ? sd_reduce_scatter_gram(ctx, comm, G, ldg, D, M) : sd_allreduce_gram(ctx, comm, G, ldg, D, M);
+        if (rc) return rc;
+    }
+    return solve_gram_impl(ctx, comm, G, ldg, D, M, reg, n_train_global, d_X, lambda_out, rank_out, route, d_mu, d_Xc);
+}
+
 int sd_solve_gram(sd_ctx* ctx, float* d_G, int64_t ldg, int D, int M, const sd_regulariser* reg, int n_train_global,
                   float* d_X, float* lambda_out)
 {
@@ -1607,23 +1627,10 @@ int sd_learn_dist(sd_ctx* ctx, sd_comm* comm, const float* d_A, int64_t lda, con
 {
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, comm != nullptr && M >= 1 && N_local >= 0, "bad argument");
-    const int64_t ldg = ((int64_t)(D + M) + 3) / 4 * 4;
-    float* G = (float*)sd_workspace(ctx, SD_WS_SCRATCH, (size_t)D * ldg * sizeof(float));
-    if (!G) return SD_ERR_CUDA;
-    SD_CUDA(ctx, cudaEventRecord(ctx->ev[0], ctx->stream));
-    int rc;
-    if (N_local > 0) rc = sd_gram(ctx, d_A, lda, d_B, ldb, N_local, D, M, G, ldg);
-    else rc = sd_check_cuda(ctx, cudaMemsetAsync(G, 0, (size_t)D * ldg * sizeof(float), ctx->stream), "memset(G)");
-    if (rc) return rc;
-    if (distributed_solve == 1) {
-        rc = sd_reduce_scatter_gram(ctx, comm, G, ldg, D, M);
-        if (rc) return rc;
-        return sd_solve_gram_dist(ctx, comm, G, ldg, D, M, reg, n_train_global, d_X, lambda_out);
-    }
-    rc = sd_allreduce_gram(ctx, comm, G, ldg, D, M);
-    if (rc) return rc;
-    // 2: the ranks share the CG iterations; 0: every rank solves alone (factorisation, or CG if sd_set_solver chose it)
-    return solve_gram_impl(ctx, comm, G, ldg, D, M, reg, n_train_global, d_X, lambda_out, nullptr, distributed_solve == 2 ? 2 : 0);
+    // 1: distributed factorisation; 2: the ranks share the CG iterations; 0: every rank solves alone (factorisation, or CG if
+    // sd_set_solver chose it)
+    const int route = distributed_solve == 1 ? 1 : distributed_solve == 2 ? 2 : 0;
+    return learn_impl(ctx, comm, d_A, lda, d_B, ldb, N_local, true, D, M, reg, n_train_global, d_X, lambda_out, nullptr, route);
 }
 
 int sd_centre_features(sd_ctx* ctx, sd_comm* comm, float* d_A, int64_t lda, int N_local, int D, int n_global,
@@ -1666,21 +1673,10 @@ int sd_learn_centred(sd_ctx* ctx, sd_comm* comm, const float* d_Ac, int64_t lda,
 {
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, M >= 1 && N_local >= 0 && d_mu && d_X, "bad argument");
-    const int64_t ldg = ((int64_t)(D + M) + 3) / 4 * 4;
-    float* G = (float*)sd_workspace(ctx, SD_WS_SCRATCH, (size_t)D * ldg * sizeof(float));
-    if (!G) return SD_ERR_CUDA;
-    SD_CUDA(ctx, cudaEventRecord(ctx->ev[0], ctx->stream));
-    int rc;
-    if (N_local > 0) rc = sd_gram(ctx, d_Ac, lda, d_B, ldb, N_local, D, M, G, ldg);
-    else rc = sd_check_cuda(ctx, cudaMemsetAsync(G, 0, (size_t)D * ldg * sizeof(float), ctx->stream), "memset(G)");
-    if (rc) return rc;
     const bool multi = sd_comm_size_of(comm) > 1;
-    if (multi) {
-        rc = route == 1 ? sd_reduce_scatter_gram(ctx, comm, G, ldg, D, M) : sd_allreduce_gram(ctx, comm, G, ldg, D, M);
-        if (rc) return rc;
-    }
     const float* mu = D > kLuMaxDim ? d_mu : nullptr;       // sd_centre_features leaves the small systems alone
-    rc = solve_gram_impl(ctx, multi ? comm : nullptr, G, ldg, D, M, reg, n_train_global, d_X, lambda_out, nullptr, multi ? route : 0, mu, d_Xc);
+    int rc = learn_impl(ctx, multi ? comm : nullptr, d_Ac, lda, d_B, ldb, N_local, true, D, M, reg, n_train_global, d_X, lambda_out,
+                        nullptr, multi ? route : 0, mu, d_Xc);
     if (rc) return rc;
     if (!mu && d_Xc && d_Xc != d_X) SD_CUDA(ctx, cudaMemcpyAsync(d_Xc, d_X, (size_t)D * M * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
     return SD_OK;
@@ -1691,13 +1687,7 @@ int sd_learn_rank_revealing(sd_ctx* ctx, const float* d_A, int64_t lda, const fl
 {
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, M >= 1 && rank_out, "bad argument");
-    const int64_t ldg = ((int64_t)(D + M) + 3) / 4 * 4;
-    float* G = (float*)sd_workspace(ctx, SD_WS_SCRATCH, (size_t)D * ldg * sizeof(float));
-    if (!G) return SD_ERR_CUDA;
-    SD_CUDA(ctx, cudaEventRecord(ctx->ev[0], ctx->stream));
-    int rc = sd_gram(ctx, d_A, lda, d_B, ldb, N, D, M, G, ldg);
-    if (rc) return rc;
-    return solve_gram_impl(ctx, nullptr, G, ldg, D, M, reg, N, d_X, lambda_out, rank_out);
+    return learn_impl(ctx, nullptr, d_A, lda, d_B, ldb, N, false, D, M, reg, N, d_X, lambda_out, rank_out, 0);
 }
 
 int sd_learn(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_B, int64_t ldb, int N, int D, int M,
@@ -1705,13 +1695,7 @@ int sd_learn(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_B, int64
 {
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, M >= 1, "labels must have at least one column");
-    const int64_t ldg = ((int64_t)(D + M) + 3) / 4 * 4;
-    float* G = (float*)sd_workspace(ctx, SD_WS_SCRATCH, (size_t)D * ldg * sizeof(float));
-    if (!G) return SD_ERR_CUDA;
-    SD_CUDA(ctx, cudaEventRecord(ctx->ev[0], ctx->stream));
-    int rc = sd_gram(ctx, d_A, lda, d_B, ldb, N, D, M, G, ldg);
-    if (rc) return rc;
-    return sd_solve_gram(ctx, G, ldg, D, M, reg, N, d_X, lambda_out);
+    return learn_impl(ctx, nullptr, d_A, lda, d_B, ldb, N, false, D, M, reg, N, d_X, lambda_out, nullptr, 0);
 }
 
 int sd_predict(sd_ctx* ctx, const float* d_values, int64_t ldv, int N, int D, const float* d_X, int M,
@@ -1721,7 +1705,7 @@ int sd_predict(sd_ctx* ctx, const float* d_values, int64_t ldv, int N, int D, co
     SD_REQUIRE(ctx, d_values && d_X && d_out && N >= 0 && D >= 1 && M >= 1 && ldv >= D && ldo >= M, "bad argument");
     GemmEpilogue ep;
     memset(&ep, 0, sizeof(ep));
-    return launch_gemm_nn(ctx, d_values, ldv, N, D, d_X, M, M, d_out, ldo, 1.0f, 0.0f, ep);
+    return launch_gemm_nn(ctx, d_values, ldv, N, D, d_X, M, M, d_out, ldo, ep);
 }
 
 __global__ void residual_kernel(const float* __restrict__ pred, const float* __restrict__ labels, long long ldl, int N, int M,
@@ -1796,7 +1780,7 @@ int sd_cascade_update(sd_ctx* ctx, const float* d_A, int64_t lda, int N, int D, 
     int rc = sd_eyes_to_dev(ctx, norm, P / 2, &ep.eyes);
     if (rc) return rc;
     SD_REQUIRE(ctx, d_x != d_x_next, "x_next must not alias x");
-    return launch_gemm_nn(ctx, d_A, lda, N, D, d_X, P, P, nullptr, 0, 1.0f, 0.0f, ep);
+    return launch_gemm_nn(ctx, d_A, lda, N, D, d_X, P, P, nullptr, 0, ep);
 }
 
 int sd_subtract_templates(sd_ctx* ctx, float* d_A, int64_t lda, const float* d_T, int64_t ldt, int N, int D)
