@@ -109,9 +109,18 @@ typedef struct {
     const sd_roi* d_roi;
     uint8_t* d_roi_miss;
     /* Optional (NULL = equally sized frames): per-frame size / pitch / position; width, height, row_stride and image_stride
-     * above are then ignored.  Not combinable with d_roi. */
+     * above are then ignored.  Together with d_roi, d_frames[i] supplies only the width and height of frame i (where its zero
+     * padding starts): the pixels are where d_roi[i] says. */
     const sd_frame* d_frames;
 } sd_image_batch;
+
+/* One host frame of a detect call: 8UC1, or 8UC3 with interleaved B,G,R (converted exactly as sd_bgr2gray does). */
+typedef struct {
+    const uint8_t* h_data;
+    int32_t width, height;
+    int32_t row_stride;          /* bytes, >= width * channels */
+    int32_t channels;            /* 1 or 3 */
+} sd_host_frame;
 
 /* ---- context --------------------------------------------------------------------------- */
 /* stream: a cudaStream_t owned by the caller (e.g. torch's current stream); NULL is the CUDA default
@@ -125,7 +134,7 @@ SD_API int sd_sync(sd_ctx* ctx);
 SD_API const char* sd_version(void);
 /* number of kernels of THIS library launched on ctx since creation (bench.py's gpu_launches) */
 SD_API int64_t sd_launch_count(const sd_ctx* ctx);
-/* faces that sd_detect_batch_host had to repeat from their full frame (a patch left the uploaded ROI) */
+/* faces that sd_detect_batch_host / sd_detect_faces_host had to repeat from their full frame (a patch left the uploaded ROI) */
 SD_API int64_t sd_roi_fallback_count(const sd_ctx* ctx);
 
 /* device / pinned-host memory for hosts that do not bring their own allocator */
@@ -349,6 +358,27 @@ SD_API int sd_detect_batch_device(sd_ctx* ctx, const sd_model* m, const sd_image
 SD_API int sd_detect_batch_host(sd_ctx* ctx, const sd_model* m, const uint8_t* h_images, int count,
                                 int width, int height, int row_stride, const int32_t* h_boxes,
                                 float* h_landmarks);
+/* detect(image, facebox) / detect(image, initialisation) (model.hpp:132-157) for num_faces faces in num_frames host frames of
+ * any sizes, grey or colour, any number of faces per frame.  Face f lies in frames[h_face_frame[f]].  Exactly one of h_boxes
+ * (num_faces x 4: x, y, w, h -> align_mean) and h_x0 (num_faces x 2L initial landmarks, e.g. the previous video frame's) is
+ * non-NULL.  h_landmarks: num_faces x 2L, in the caller's face order.  Frames that no face refers to are never read.
+ * A face index out of range, channels not 1 or 3, row_stride < width * channels, or both / neither of h_boxes and h_x0 are
+ * SD_ERR_INVALID before any work is queued (h_landmarks is not written); so is a degenerate face, as in sd_detect_batch_device.
+ * Routes:
+ *   - every referenced frame in pinned, device-mapped host memory with a 16-byte aligned base and row_stride: the SMs gather a
+ *     neighbourhood of each face (one per face, also for several faces of one frame) straight from the frame, converting
+ *     colour pixels to grey on the way; a face whose cascade leaves its neighbourhood is repeated from its whole frame
+ *     (sd_roi_fallback_count);
+ *   - otherwise each referenced frame is copied to the device once (colour frames then converted there) in chunks
+ *     overlapped with the cascade.
+ * Both routes give bit-identical landmarks. */
+SD_API int sd_detect_faces_host(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frames, int num_frames,
+                                const int32_t* h_face_frame, int num_faces, const int32_t* h_boxes, const float* h_x0,
+                                float* h_landmarks);
+/* sd_detect_batch_device with a face -> frame index: face i lies in images[d_face_frame[i]] (d_face_frame may be NULL: face i
+ * in frame i), so a frame with several faces is resident once.  An index out of range is SD_ERR_INVALID. */
+SD_API int sd_detect_faces_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_face_frame,
+                                  const float* d_x0, int num_faces, float* d_landmarks);
 
 #ifdef __cplusplus
 }

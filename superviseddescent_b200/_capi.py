@@ -44,6 +44,11 @@ class FrameC(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("row_stride", C.c_int32), ("reserved", C.c_int32), ("offset", C.c_int64)]
 
 
+class HostFrameC(C.Structure):
+    """sd_host_frame: one host frame of a detect call (8UC1, or 8UC3 interleaved B, G, R)."""
+    _fields_ = [("h_data", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32), ("row_stride", C.c_int32), ("channels", C.c_int32)]
+
+
 # every symbol declared in include/sd_b200.h (tests/test_abi.py checks the list against the header)
 EXPORTS = [
     "sd_ctx_create", "sd_ctx_destroy", "sd_last_error", "sd_sync", "sd_version", "sd_launch_count", "sd_roi_fallback_count",
@@ -58,7 +63,7 @@ EXPORTS = [
     "sd_model_num_landmarks", "sd_model_hog_param", "sd_model_regulariser", "sd_model_normalisation",
     "sd_model_get_mean", "sd_model_get_weights", "sd_model_landmark_id", "sd_align_mean",
     "sd_perturb_box", "sd_normalised_landmark_errors",
-    "sd_detect_batch_device", "sd_detect_batch_host",
+    "sd_detect_batch_device", "sd_detect_batch_host", "sd_detect_faces_host", "sd_detect_faces_device",
 ]
 
 _lib = None

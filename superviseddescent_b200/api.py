@@ -23,7 +23,7 @@ import torch
 
 from . import _capi
 from ._capi import HogParam as HoGParam  # same field names as rcr::HoGParam
-from ._capi import ImageBatchC, NormalisationC, RegulariserC, SdError, ptr
+from ._capi import HostFrameC, ImageBatchC, NormalisationC, RegulariserC, SdError, ptr
 
 
 def _check(ctx, rc: int) -> None:
@@ -604,6 +604,24 @@ def calculate_normalised_landmark_errors(predictions, groundtruth, model_landmar
     return out
 
 
+def _np_ptr(a) -> C.c_void_p:
+    return C.c_void_p(0) if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _host_frame(frame):
+    """(H, W) / (H, W, C) uint8 numpy array or CPU tensor -> (sd_host_frame, the array that owns the bytes).  The rows keep
+    their pitch; the pixels of a row must be packed (copied otherwise)."""
+    a = frame.numpy() if isinstance(frame, torch.Tensor) else np.asarray(frame)   # a tensor's numpy() shares (pinned) memory
+    if a.dtype != np.uint8:
+        a = np.ascontiguousarray(a, dtype=np.uint8)
+    if a.ndim not in (2, 3):
+        raise ValueError("every frame must be (H, W) or (H, W, 3) uint8")
+    ch = 1 if a.ndim == 2 else a.shape[2]
+    if a.strides[0] <= 0 or a.strides[1] != ch or (a.ndim == 3 and a.strides[2] != 1):
+        a = np.ascontiguousarray(a)
+    return HostFrameC(a.ctypes.data, a.shape[1], a.shape[0], a.strides[0], ch), a
+
+
 class detection_model:
     """rcr::detection_model (model.hpp:122-183) resident on the GPU."""
 
@@ -652,29 +670,46 @@ class detection_model:
         return out
 
     def detect(self, image, facebox_or_initialisation) -> np.ndarray:
-        """detect(image, facebox) / detect(image, initialisation) (model.hpp:132-157): one frame, returns the 2L row."""
-        image = np.ascontiguousarray(image, dtype=np.uint8)
+        """detect(image, facebox) / detect(image, initialisation) (model.hpp:132-157): one frame, grey or colour, returns the 2L
+        row."""
         arg = np.asarray(facebox_or_initialisation)
         if arg.size == 4:
-            return self.detect_batch(image[None], np.asarray(arg, dtype=np.int32)[None])[0]
-        x0 = _dev(np.asarray(arg, dtype=np.float32).reshape(1, -1), self.ctx)
-        imgs = _dev(image[None], self.ctx, dtype=torch.uint8)
-        return self.detect_batch_device(imgs, x0).cpu().numpy()[0]
+            return self.detect_faces([image], [0], boxes=arg.reshape(1, 4))[0]
+        return self.detect_faces([image], [0], initialisations=arg.reshape(1, -1))[0]
+
+    def detect_faces(self, frames, face_frame, boxes=None, initialisations=None) -> np.ndarray:
+        """detect(image, facebox) / detect(image, initialisation) for any number of faces in host frames of any sizes
+        (sd_detect_faces_host).  frames: a sequence of (H, W) grey or (H, W, 3) B,G,R uint8 numpy arrays or CPU tensors; face i
+        lies in frames[face_frame[i]].  Give exactly one of boxes ((F, 4): x, y, w, h) and initialisations ((F, 2L), e.g. the
+        previous video frame's landmarks).  A row pitch other than the row's bytes (strides[0]) is honoured; pinned frames with
+        16-byte aligned rows take the zero-copy region-of-interest route.  Returns (F, 2L) landmarks in the order of face_frame."""
+        recs, keep = [], []
+        for f in frames:
+            rec, a = _host_frame(f)
+            recs.append(rec)
+            keep.append(a)                                   # the bytes stay alive until the call returns
+        table = (HostFrameC * max(len(recs), 1))(*recs)
+        idx = np.ascontiguousarray(face_frame, dtype=np.int32).ravel()
+        n = idx.size
+        P = 2 * self.num_landmarks
+        b = None if boxes is None else np.ascontiguousarray(boxes, dtype=np.int32).reshape(n, 4)
+        x0 = None if initialisations is None else np.ascontiguousarray(initialisations, dtype=np.float32).reshape(n, P)
+        out = np.empty((n, P), dtype=np.float32)
+        _check(self.ctx.h, _capi.lib().sd_detect_faces_host(self.ctx.h, self._m, table, len(recs), _np_ptr(idx), n, _np_ptr(b),
+                                                            _np_ptr(x0), _np_ptr(out)))
+        return out
 
     def detect_batch(self, images: np.ndarray, boxes: np.ndarray) -> np.ndarray:
-        """Batched detect(image, facebox) with HOST buffers (copies are part of the call).  Colour frames
-        (count, H, W, 3) are converted on the device first (model.hpp:134-145 calls cvtColor through HogTransform)."""
+        """Batched detect(image, facebox) with HOST buffers (copies are part of the call): (count, H, W) grey or
+        (count, H, W, 3) colour frames, one face box each."""
         if isinstance(images, torch.Tensor):
             images_np = images.numpy()
         else:
             images_np = np.ascontiguousarray(images, dtype=np.uint8)
+        n = images_np.shape[0]
         if images_np.ndim == 4:
-            gray = bgr2gray(images_np, self.ctx)
-            n = gray.shape[0]
-            b = np.ascontiguousarray(boxes, dtype=np.int32).reshape(n, 4)
-            x0 = torch.from_numpy(np.stack([align_mean(self.get_mean(), tuple(int(v) for v in b[i])) for i in range(n)]).astype(np.float32))
-            return self.detect_batch_device(gray, x0.to(gray.device)).cpu().numpy()
-        n, h, w = images_np.shape
+            return self.detect_faces(list(images_np), np.arange(n), boxes=boxes)
+        _, h, w = images_np.shape
         boxes = np.ascontiguousarray(boxes, dtype=np.int32).reshape(n, 4)
         out = np.empty((n, 2 * self.num_landmarks), dtype=np.float32)
         _check(self.ctx.h, _capi.lib().sd_detect_batch_host(self.ctx.h, self._m, images_np.ctypes.data_as(C.c_void_p), n, w, h,
@@ -682,12 +717,15 @@ class detection_model:
                                                             out.ctypes.data_as(C.c_void_p)))
         return out
 
-    def detect_batch_device(self, images: torch.Tensor, x0: torch.Tensor) -> torch.Tensor:
-        """Batched detect(image, initialisation), frames and landmarks already resident in HBM."""
-        n, h, w = images.shape
-        ib = ImageBatchC(C.c_void_p(images.data_ptr()), w, h, images.stride(1), images.stride(0), n)
+    def detect_batch_device(self, images: torch.Tensor, x0: torch.Tensor, image_index=None) -> torch.Tensor:
+        """Batched detect(image, initialisation), frames and landmarks already resident in HBM.  Face i starts from x0[i] and
+        lies in images[image_index[i]] (default: images[i]), so a frame with several faces is resident once."""
+        n = x0.shape[0]
+        h, w = images.shape[1], images.shape[2]
+        ib = ImageBatchC(C.c_void_p(images.data_ptr()), w, h, images.stride(1), images.stride(0), images.shape[0])
+        idx = None if image_index is None else torch.as_tensor(image_index, dtype=torch.int32).to(images.device).contiguous()
         out = torch.empty((n, 2 * self.num_landmarks), dtype=torch.float32, device=images.device)
-        _check(self.ctx.h, _capi.lib().sd_detect_batch_device(self.ctx.h, self._m, C.byref(ib), ptr(x0), n, ptr(out)))
+        _check(self.ctx.h, _capi.lib().sd_detect_faces_device(self.ctx.h, self._m, C.byref(ib), ptr(idx), ptr(x0), n, ptr(out)))
         return out
 
     def save(self, filename: str) -> None:

@@ -693,7 +693,6 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
     a.roi = images->d_roi;
     a.roi_miss = images->d_roi_miss;
     a.frames = images->d_frames;
-    SD_REQUIRE(ctx, !(images->d_roi && images->d_frames), "d_roi and d_frames cannot be combined");
     if (!d_image_index) SD_REQUIRE(ctx, images->count >= N, "fewer images than samples and no image index");
     a.x = d_x; a.ldx = ldx; a.N = N; a.L = L;
     a.variant = p->variant; a.nc = p->num_cells; a.cs = p->cell_size; a.K = p->num_bins; a.fs = fs;
@@ -815,14 +814,11 @@ __global__ void bgr2gray_kernel(const uint8_t* __restrict__ bgr, int width, int 
             const uint32_t b0 = w0 & 255, g0 = (w0 >> 8) & 255, r0 = (w0 >> 16) & 255, b1 = w0 >> 24;
             const uint32_t g1 = w1 & 255, r1 = (w1 >> 8) & 255, b2 = (w1 >> 16) & 255, g2 = w1 >> 24;
             const uint32_t r2 = w2 & 255, b3 = (w2 >> 8) & 255, g3 = (w2 >> 16) & 255, r3 = w2 >> 24;
-            const uint32_t y0 = (3735u * b0 + 19235u * g0 + 9798u * r0 + (1u << 14)) >> 15;
-            const uint32_t y1 = (3735u * b1 + 19235u * g1 + 9798u * r1 + (1u << 14)) >> 15;
-            const uint32_t y2 = (3735u * b2 + 19235u * g2 + 9798u * r2 + (1u << 14)) >> 15;
-            const uint32_t y3 = (3735u * b3 + 19235u * g3 + 9798u * r3 + (1u << 14)) >> 15;
+            const uint32_t y0 = sd_bgr_to_gray(b0, g0, r0), y1 = sd_bgr_to_gray(b1, g1, r1);
+            const uint32_t y2 = sd_bgr_to_gray(b2, g2, r2), y3 = sd_bgr_to_gray(b3, g3, r3);
             *reinterpret_cast<uint32_t*>(d) = y0 | (y1 << 8) | (y2 << 16) | (y3 << 24);
         } else {
-            for (int k = 0; k < 4 && x0 + k < width; ++k)
-                d[k] = (uint8_t)((3735u * s[3 * k] + 19235u * s[3 * k + 1] + 9798u * s[3 * k + 2] + (1u << 14)) >> 15);
+            for (int k = 0; k < 4 && x0 + k < width; ++k) d[k] = (uint8_t)sd_bgr_to_gray(s[3 * k], s[3 * k + 1], s[3 * k + 2]);
         }
     }
 }

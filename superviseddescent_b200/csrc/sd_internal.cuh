@@ -36,7 +36,7 @@ struct sd_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    cudaStream_t copy_stream = nullptr;   // host<->device staging for sd_detect_batch_host
+    cudaStream_t copy_stream = nullptr;   // host->device staging for sd_detect_faces_host
     cudaStream_t chain_stream = nullptr;  // Cholesky look-ahead: next panel's diagonal blocks while the trailing update runs
     cudaEvent_t chain_ev[2] = {nullptr, nullptr};
     int syrk_sm_reserve = 0;              // SMs the persistent SYRK leaves free (1 while a look-ahead chain runs beside it)
@@ -57,7 +57,7 @@ struct sd_ctx {
     // pinned scratch for small device->host results (lambda, residual, status flags)
     void* h_scratch = nullptr;
     void* d_scratch = nullptr;   // 4 KB
-    // staging buffers of sd_detect_batch_host
+    // staging buffers of sd_detect_faces_host
     void* d_stage[2] = {nullptr, nullptr};
     size_t stage_bytes[2] = {0, 0};
     cudaEvent_t stage_ev[2] = {nullptr, nullptr};
@@ -169,5 +169,12 @@ __device__ __forceinline__ double sd_device_ied(const float* __restrict__ row, i
     const double dx = (double)__fsub_rn(rx, lx);
     const double dy = (double)__fsub_rn(ry, ly);
     return sqrt(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));
+}
+
+// cv::cvtColor(BGR2GRAY) of one 8-bit pixel, OpenCV >= 3 fixed point (15-bit coefficients, SURVEY.md 8c).  The only spelling of
+// the conversion: bgr2gray_kernel (sd_hog.cu) and the colour ROI gather (sd_model.cu) both call it.
+__device__ __forceinline__ uint32_t sd_bgr_to_gray(uint32_t b, uint32_t g, uint32_t r)
+{
+    return (3735u * b + 19235u * g + 9798u * r + (1u << 14)) >> 15;
 }
 #endif

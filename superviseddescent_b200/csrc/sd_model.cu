@@ -3,9 +3,13 @@
 //
 //   file format    model.hpp:178-182 -> superviseddescent.hpp:356-360 -> regressors.hpp:395-399,164-168
 //                  -> utils/mat_cerealisation.hpp:42-99 ; model.hpp:111-115 ; adaptive_vlhog.hpp:55-59
-//   detect         model.hpp:132-157 -> superviseddescent.hpp:323-344 (predict: sequential over levels)
+//   detect         model.hpp:132-157 -> superviseddescent.hpp:323-344 (predict: sequential over levels), on device frames or
+//                  on host frames of any size, grey or colour, any number of faces each
 #include "sd_internal.cuh"
 
+#include <cuda.h>
+
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <exception>
@@ -140,8 +144,8 @@ int validate_and_upload(sd_ctx* ctx, sd_model* m)
     return SD_OK;
 }
 
-int detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const float* d_x0, int count,
-                  float* d_landmarks)
+int detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x0,
+                  int count, float* d_landmarks)
 {
     const int L = m->num_landmarks, P = 2 * L;
     if (count <= 0) return SD_OK;
@@ -158,7 +162,7 @@ int detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, 
     float* cur = xa;
     float* nxt = xb;
     for (int s = 0; s < m->num_levels; ++s) {               // superviseddescent.hpp:326-342
-        int rc = sd_hog_batch(ctx, images, nullptr, cur, P, count, L, &m->norm, &m->hog[s], A, ld);
+        int rc = sd_hog_batch(ctx, images, d_image_index, cur, P, count, L, &m->norm, &m->hog[s], A, ld);
         if (rc) return rc;
         rc = sd_cascade_update(ctx, A, ld, count, m->rows[s], m->d_weights[s], P, cur, &m->norm, nxt);
         if (rc) return rc;
@@ -169,42 +173,78 @@ int detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, 
 }
 
 
-// ---- region-of-interest upload (sd_detect_batch_host) ------------------------------------------------
-// The cascade only ever reads a neighbourhood of the face, so instead of copying whole 640x480 frames over
-// PCIe a small kernel pulls the ROI rows of every face straight out of the caller's PINNED host buffer
-// (zero-copy loads through the unified address space, 16-byte vectors) into a packed device buffer.  If a
-// patch later needs a frame pixel outside its ROI the HOG kernel raises d_roi_miss[face] and that face is
-// repeated from its full frame, so the result never depends on the ROI heuristic.
-__global__ void __launch_bounds__(256) roi_gather_kernel(const uint8_t* __restrict__ h_frames, long long frame_bytes, int row_stride,
-                                                         const sd_roi* __restrict__ roi, int first, int n, uint8_t* __restrict__ dst)
+// ---- region-of-interest gather (sd_detect_faces_host) -------------------------------------------------
+// The cascade only ever reads a neighbourhood of the face, so instead of copying whole frames over PCIe a small kernel pulls
+// the ROI rows of every face straight out of the caller's PINNED host frame (zero-copy loads through the unified address
+// space, 16-byte vectors) into a packed grey device buffer.  If a patch later needs a frame pixel outside its ROI the HOG
+// kernel raises d_roi_miss[face] and that face is repeated from its full frame, so the result never depends on the ROI
+// heuristic.
+struct GatherRec {
+    const uint8_t* src;          // device-mapped address of the ROI's first pixel in the caller's frame
+    int64_t src_stride;          // bytes between the frame's rows
+    int64_t dst_offset;          // of the grey ROI in the staging buffer; its rows are 16 * vec_per_row bytes apart
+    int32_t vec_per_row, rows;   // ROI size in steps of 16 pixels x rows
+};
+
+// 16 interleaved B,G,R pixels (48 bytes) -> 16 grey bytes
+__device__ __forceinline__ uint4 bgr16_to_gray(const uint4 (&v)[3])
 {
-    for (int f = blockIdx.x; f < n; f += gridDim.x) {
-        const sd_roi r = roi[first + f];
-        const uint8_t* src = h_frames + (long long)(first + f) * frame_bytes + (long long)r.y * row_stride + r.x;
-        uint8_t* d = dst + r.offset;
-        const int vec_per_row = r.row_stride >> 4;
-        const int total = vec_per_row * r.h;
-        // four independent 16-byte reads in flight per thread before the stores: PCIe read latency is ~1 us
-        for (int i0 = threadIdx.x; i0 < total; i0 += 4 * blockDim.x) {
-            uint4 v[4];
-            int row[4], col[4];
+    const uint32_t w[12] = {v[0].x, v[0].y, v[0].z, v[0].w, v[1].x, v[1].y, v[1].z, v[1].w, v[2].x, v[2].y, v[2].z, v[2].w};
+    uint32_t out[4];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
+    for (int q = 0; q < 4; ++q) {
+        uint32_t o = 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const int b = 3 * (4 * q + k);                  // byte index of the pixel's B (little endian words)
+            o |= sd_bgr_to_gray((w[b >> 2] >> (8 * (b & 3))) & 255u, (w[(b + 1) >> 2] >> (8 * ((b + 1) & 3))) & 255u,
+                                (w[(b + 2) >> 2] >> (8 * ((b + 2) & 3))) & 255u) << (8 * k);
+        }
+        out[q] = o;
+    }
+    return make_uint4(out[0], out[1], out[2], out[3]);
+}
+
+// C = channels of the source frames.  One step moves 16 pixels: one uint4 of grey, or three of B,G,R (the ROI's x is a
+// multiple of 16 pixels, so 48 k bytes into a 16-byte aligned row) converted on the way.
+template <int C>
+__global__ void __launch_bounds__(256) roi_gather_kernel(const GatherRec* __restrict__ rec, int n, uint8_t* __restrict__ dst)
+{
+    constexpr int U = 4;                                    // steps in flight per thread before the stores: PCIe read latency is ~1 us
+    for (int f = blockIdx.x; f < n; f += gridDim.x) {
+        const GatherRec r = rec[f];
+        const int total = r.vec_per_row * r.rows;
+        uint8_t* d = dst + r.dst_offset;
+        for (int i0 = threadIdx.x; i0 < total; i0 += U * blockDim.x) {
+            uint4 v[U][C];
+            int row[U], col[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
                 const int i = i0 + u * blockDim.x;
-                row[u] = i / vec_per_row;
-                col[u] = i - row[u] * vec_per_row;
-                if (i < total) v[u] = reinterpret_cast<const uint4*>(src + (long long)row[u] * row_stride)[col[u]];
+                row[u] = i / r.vec_per_row;
+                col[u] = i - row[u] * r.vec_per_row;
+                if (i < total) {
+                    const uint4* s = reinterpret_cast<const uint4*>(r.src + (long long)row[u] * r.src_stride) + C * col[u];
+#pragma unroll
+                    for (int c = 0; c < C; ++c) v[u][c] = s[c];
+                }
             }
 #pragma unroll
-            for (int u = 0; u < 4; ++u)
-                if (i0 + u * blockDim.x < total) reinterpret_cast<uint4*>(d + (long long)row[u] * r.row_stride)[col[u]] = v[u];
+            for (int u = 0; u < U; ++u) {
+                if (i0 + u * blockDim.x >= total) continue;
+                uint4 g;
+                if constexpr (C == 1) g = v[u][0];
+                else g = bgr16_to_gray(v[u]);
+                reinterpret_cast<uint4*>(d + (long long)row[u] * 16 * r.vec_per_row)[col[u]] = g;
+            }
         }
     }
 }
 
-// conservative ROI of one face: landmark bounding box of the initialisation, grown by the largest patch
-// half size of the schedule plus a drift allowance, clipped to the frame, x aligned to 16 bytes
-sd_roi face_roi(const sd_model* m, const float* x0, int width, int height, int row_stride)
+// conservative ROI of one face: landmark bounding box of the initialisation, grown by the largest patch half size of the
+// schedule plus a drift allowance, clipped to the frame, x aligned to 16 pixels; row_pixels = pixels a row of the caller's
+// buffer holds (row_stride / channels), which the ROI never reaches past
+sd_roi face_roi(const sd_model* m, const float* x0, int width, int height, int row_pixels)
 {
     const int L = m->num_landmarks;
     float minx = x0[0], maxx = x0[0], miny = x0[L], maxy = x0[L];
@@ -232,10 +272,285 @@ sd_roi face_roi(const sd_model* m, const float* x0, int width, int height, int r
     if (xb <= xa || yb <= ya) { xa = 0; ya = 0; xb = 16 < width ? 16 : width; yb = 1; }   // face entirely outside the frame
     r.x = xa & ~15;
     int w = ((xb - r.x) + 15) & ~15;
-    const int maxw = (row_stride - r.x) & ~15;
+    const int maxw = (row_pixels - r.x) & ~15;
     if (w > maxw) w = maxw;
     r.w = w; r.y = ya; r.h = yb - ya; r.row_stride = w; r.reserved = 0; r.offset = 0;
     return r;
+}
+
+// Device-mapped address of a pinned host frame, or nullptr.  Frames inside the last pinned allocation seen (every frame of
+// sd_detect_batch_host's batch) are mapped by offset instead of one driver query each.
+struct PinnedRange {
+    uintptr_t lo = 0, hi = 0;    // host addresses of the allocation
+    intptr_t delta = 0;          // device address - host address
+};
+
+typedef CUresult (*PFN_pointerGetAttribute)(void* data, CUpointer_attribute attribute, CUdeviceptr ptr);
+
+const uint8_t* mapped_frame(const uint8_t* p, size_t bytes, PinnedRange& last)
+{
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+    if (a >= last.lo && a + bytes <= last.hi) return reinterpret_cast<const uint8_t*>(a + last.delta);
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, p) != cudaSuccess) { cudaGetLastError(); return nullptr; }
+    if (attr.type != cudaMemoryTypeHost || !attr.devicePointer) return nullptr;
+    static PFN_pointerGetAttribute get = nullptr;
+    if (!get) {
+        void* fn = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuPointerGetAttribute", &fn, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+            get = reinterpret_cast<PFN_pointerGetAttribute>(fn);
+    }
+    CUdeviceptr start = 0;
+    size_t size = 0;
+    if (get && get(&start, CU_POINTER_ATTRIBUTE_RANGE_START_ADDR, (CUdeviceptr)a) == CUDA_SUCCESS &&
+        get(&size, CU_POINTER_ATTRIBUTE_RANGE_SIZE, (CUdeviceptr)a) == CUDA_SUCCESS && start <= a && a + bytes <= start + size) {
+        last.lo = start; last.hi = start + size;
+        last.delta = (intptr_t)reinterpret_cast<uintptr_t>(attr.devicePointer) - (intptr_t)a;
+    }
+    return static_cast<const uint8_t*>(attr.devicePointer);
+}
+
+size_t host_frame_bytes(const sd_host_frame& f) { return (size_t)(f.height - 1) * f.row_stride + (size_t)f.width * f.channels; }
+size_t round16(size_t v) { return (v + 15) & ~(size_t)15; }
+
+// the two staging buffers hold at least `bytes` each
+int ensure_stage(sd_ctx* ctx, size_t bytes)
+{
+    for (int b = 0; b < 2; ++b) {
+        if (ctx->stage_bytes[b] < bytes) {
+            if (ctx->d_stage[b]) { SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); SD_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream)); SD_CUDA(ctx, cudaFree(ctx->d_stage[b])); ctx->d_stage[b] = nullptr; }
+            SD_CUDA(ctx, cudaMalloc(&ctx->d_stage[b], bytes));
+            ctx->stage_bytes[b] = bytes;
+        }
+    }
+    return SD_OK;
+}
+
+// Full route: faces grouped by frame, every referenced frame copied to the device once (grey at a 16-byte pitch; colour as
+// B,G,R behind the chunk's grey frames, converted by bgr2gray_kernel), chunks double-buffered against the cascade.
+// x0 / out: count x 2L in the caller's face order.
+int detect_faces_full(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frames, const int32_t* face_frame, int count,
+                      const float* x0, float* out)
+{
+    const int P = 2 * m->num_landmarks;
+    const size_t chunk_cap = (size_t)128 << 20;              // frame bytes per staging buffer (at least one frame)
+    std::vector<int> order(count);
+    for (int i = 0; i < count; ++i) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return face_frame[a] < face_frame[b]; });
+    std::vector<int> up;                                      // referenced frames in upload order
+    std::vector<int32_t> local(count);                        // per sorted face: its frame's index in `up`, then in its chunk
+    for (int k = 0; k < count; ++k) {
+        if (up.empty() || up.back() != face_frame[order[k]]) up.push_back(face_frame[order[k]]);
+        local[k] = (int32_t)up.size() - 1;
+    }
+    auto gray_bytes = [&](int f) { return (size_t)frames[f].height * round16(frames[f].width); };
+    auto bgr_bytes = [&](int f) { return frames[f].channels == 3 ? (size_t)frames[f].height * round16(3 * (size_t)frames[f].width) : 0; };
+    std::vector<int> chunk_first;                             // first upload of each chunk
+    size_t used = 0, need = 0;
+    for (size_t u = 0; u < up.size(); ++u) {
+        const size_t b = gray_bytes(up[u]) + bgr_bytes(up[u]);
+        if (chunk_first.empty() || used + b > chunk_cap) { chunk_first.push_back((int)u); used = 0; }
+        used += b;
+        need = used > need ? used : need;
+    }
+    chunk_first.push_back((int)up.size());
+    // per upload: its grey frame descriptor (offset from the chunk's buffer) and where its B,G,R bytes land
+    std::vector<sd_frame> desc(up.size());
+    std::vector<int64_t> bgr_off(up.size(), 0);
+    std::vector<int> face_first(chunk_first.size(), count);   // first sorted face of each chunk
+    for (size_t c = 0; c + 1 < chunk_first.size(); ++c) {
+        int64_t g = 0;
+        for (int u = chunk_first[c]; u < chunk_first[c + 1]; ++u) {
+            const sd_host_frame& f = frames[up[u]];
+            desc[u] = sd_frame{f.width, f.height, (int32_t)round16(f.width), 0, g};
+            g += (int64_t)gray_bytes(up[u]);
+        }
+        for (int u = chunk_first[c]; u < chunk_first[c + 1]; ++u) { bgr_off[u] = g; g += (int64_t)bgr_bytes(up[u]); }
+    }
+    std::vector<int> chunk_of(up.size());
+    for (size_t c = 0; c + 1 < chunk_first.size(); ++c)
+        for (int u = chunk_first[c]; u < chunk_first[c + 1]; ++u) chunk_of[u] = (int)c;
+    for (int k = count - 1; k >= 0; --k) {                    // faces of a chunk are contiguous in sorted order
+        const int c = chunk_of[local[k]];
+        face_first[c] = k;
+        local[k] -= chunk_first[c];                           // frame index inside its chunk
+    }
+    int rc = ensure_stage(ctx, need);
+    if (rc) return rc;
+    // device tables: landmarks (in, out) in sorted order, face -> frame index, frame descriptors
+    std::vector<float> xs((size_t)count * P);
+    for (int k = 0; k < count; ++k) memcpy(&xs[(size_t)k * P], x0 + (size_t)order[k] * P, P * sizeof(float));
+    const size_t xbytes = (size_t)count * P * sizeof(float);
+    const size_t ibytes = round16((size_t)count * sizeof(int32_t));
+    unsigned char* tab = (unsigned char*)sd_workspace(ctx, SD_WS_PARTIAL, 2 * xbytes + ibytes + up.size() * sizeof(sd_frame));
+    if (!tab) return SD_ERR_CUDA;
+    float* d_x = (float*)tab;
+    float* d_out = (float*)(tab + xbytes);
+    int32_t* d_idx = (int32_t*)(tab + 2 * xbytes);
+    sd_frame* d_desc = (sd_frame*)(tab + 2 * xbytes + ibytes);
+    SD_CUDA(ctx, cudaMemcpyAsync(d_x, xs.data(), xbytes, cudaMemcpyHostToDevice, ctx->stream));
+    SD_CUDA(ctx, cudaMemcpyAsync(d_idx, local.data(), (size_t)count * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+    SD_CUDA(ctx, cudaMemcpyAsync(d_desc, desc.data(), desc.size() * sizeof(sd_frame), cudaMemcpyHostToDevice, ctx->stream));
+    // the copy stream must not run ahead of work already queued on the compute stream that still reads the staging buffers
+    SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[0], ctx->stream));
+    SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[1], ctx->stream));
+    int buf = 0;
+    for (size_t c = 0; c + 1 < chunk_first.size(); ++c, buf ^= 1) {
+        const int u0 = chunk_first[c], u1 = chunk_first[c + 1];
+        uint8_t* stage = (uint8_t*)ctx->d_stage[buf];
+        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_done[buf], 0));
+        for (int u = u0; u < u1; ++u) {
+            const sd_host_frame& f = frames[up[u]];
+            uint8_t* dst = f.channels == 3 ? stage + bgr_off[u] : stage + desc[u].offset;
+            const size_t pitch = f.channels == 3 ? round16(3 * (size_t)f.width) : (size_t)desc[u].row_stride;
+            if ((size_t)f.row_stride == pitch)
+                SD_CUDA(ctx, cudaMemcpyAsync(dst, f.h_data, host_frame_bytes(f), cudaMemcpyHostToDevice, ctx->copy_stream));
+            else
+                SD_CUDA(ctx, cudaMemcpy2DAsync(dst, pitch, f.h_data, f.row_stride, (size_t)f.width * f.channels, f.height,
+                                               cudaMemcpyHostToDevice, ctx->copy_stream));
+        }
+        SD_CUDA(ctx, cudaEventRecord(ctx->stage_ev[buf], ctx->copy_stream));
+        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->stage_ev[buf], 0));
+        bool uniform = true;
+        for (int u = u0; u < u1; ++u) {
+            const sd_host_frame& f = frames[up[u]];
+            if (f.channels == 3) {
+                rc = sd_bgr2gray(ctx, stage + bgr_off[u], f.width, f.height, (int64_t)round16(3 * (size_t)f.width), 0, 1,
+                                 stage + desc[u].offset, desc[u].row_stride, 0);
+                if (rc) return rc;
+            }
+            uniform = uniform && f.width == frames[up[u0]].width && f.height == frames[up[u0]].height;
+        }
+        // equally sized frames: a plain batch, which the HOG kernel stages by TMA; otherwise one descriptor per frame
+        sd_image_batch ib{};
+        ib.d_data = stage;
+        ib.count = u1 - u0;
+        if (uniform) {
+            ib.width = desc[u0].width; ib.height = desc[u0].height; ib.row_stride = desc[u0].row_stride;
+            ib.image_stride = (int64_t)gray_bytes(up[u0]);
+        } else {
+            ib.d_frames = d_desc + u0;
+        }
+        const int k0 = face_first[c], n = face_first[c + 1] - k0;
+        rc = detect_device(ctx, m, &ib, d_idx + k0, d_x + (size_t)k0 * P, n, d_out + (size_t)k0 * P);
+        if (rc) return rc;
+        SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[buf], ctx->stream));
+    }
+    SD_CUDA(ctx, cudaMemcpyAsync(xs.data(), d_out, xbytes, cudaMemcpyDeviceToHost, ctx->stream));
+    rc = sd_check_hog_status(ctx, "detect");                  // synchronises
+    if (rc) return rc;
+    for (int k = 0; k < count; ++k) memcpy(out + (size_t)order[k] * P, &xs[(size_t)k * P], P * sizeof(float));
+    return SD_OK;
+}
+
+// ROI route: every referenced frame is pinned and device-mapped (mapped[f]), with 16-byte aligned base and rows
+int detect_faces_roi(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frames, const std::vector<const uint8_t*>& mapped,
+                     const int32_t* face_frame, int count, const float* x0, float* out)
+{
+    const int P = 2 * m->num_landmarks;
+    const size_t chunk_cap = (size_t)48 << 20;                // packed grey ROI bytes per staging buffer
+    // the ROI of every face, from its own frame's size; faces are grouped into chunks that fit one staging buffer
+    std::vector<sd_roi> rois(count);
+    std::vector<sd_frame> dims(count);
+    std::vector<int> chunk_first;
+    size_t used = 0;
+    for (int i = 0; i < count; ++i) {
+        const sd_host_frame& f = frames[face_frame[i]];
+        sd_roi r = face_roi(m, x0 + (size_t)i * P, f.width, f.height, f.row_stride / f.channels);
+        const size_t bytes = (size_t)r.row_stride * r.h;
+        if (bytes > chunk_cap)                                // a face window larger than a staging buffer: whole-frame route
+            return detect_faces_full(ctx, m, frames, face_frame, count, x0, out);
+        if (chunk_first.empty() || used + bytes > chunk_cap) { chunk_first.push_back(i); used = 0; }
+        r.offset = (int64_t)used;
+        used += bytes;
+        rois[i] = r;
+        dims[i] = sd_frame{f.width, f.height, 0, 0, 0};      // with d_roi only the frame size is read
+    }
+    chunk_first.push_back(count);
+    // gather records per chunk: grey faces first, then colour faces (one launch each)
+    std::vector<GatherRec> recs(count);
+    std::vector<int> chunk_grey(chunk_first.size(), 0);
+    for (size_t c = 0; c + 1 < chunk_first.size(); ++c) {
+        int k = chunk_first[c];
+        for (int ch = 1; ch <= 3; ch += 2)
+            for (int i = chunk_first[c]; i < chunk_first[c + 1]; ++i) {
+                const sd_host_frame& f = frames[face_frame[i]];
+                if (f.channels != ch) continue;
+                const sd_roi& r = rois[i];
+                recs[k++] = GatherRec{mapped[face_frame[i]] + (int64_t)r.y * f.row_stride + (int64_t)r.x * ch, f.row_stride, r.offset,
+                                      r.w >> 4, r.h};
+                if (ch == 1) ++chunk_grey[c];
+            }
+    }
+    int rc = ensure_stage(ctx, chunk_cap + (1u << 20));
+    if (rc) return rc;
+    // device tables: landmarks (in, out), ROI records, frame sizes, gather records, miss flags
+    const size_t xbytes = (size_t)count * P * sizeof(float);
+    const size_t rbytes = (size_t)count * sizeof(sd_roi);
+    const size_t fbytes = (size_t)count * sizeof(sd_frame);
+    const size_t gbytes = (size_t)count * sizeof(GatherRec);
+    unsigned char* tab = (unsigned char*)sd_workspace(ctx, SD_WS_PARTIAL, 2 * xbytes + rbytes + fbytes + gbytes + count + 64);
+    if (!tab) return SD_ERR_CUDA;
+    float* d_x = (float*)tab;
+    float* d_out = (float*)(tab + xbytes);
+    sd_roi* d_roi = (sd_roi*)(tab + 2 * xbytes);
+    sd_frame* d_dims = (sd_frame*)(tab + 2 * xbytes + rbytes);
+    GatherRec* d_rec = (GatherRec*)(tab + 2 * xbytes + rbytes + fbytes);
+    uint8_t* d_miss = tab + 2 * xbytes + rbytes + fbytes + gbytes;
+    SD_CUDA(ctx, cudaMemcpyAsync(d_x, x0, xbytes, cudaMemcpyHostToDevice, ctx->stream));
+    SD_CUDA(ctx, cudaMemcpyAsync(d_roi, rois.data(), rbytes, cudaMemcpyHostToDevice, ctx->stream));
+    SD_CUDA(ctx, cudaMemcpyAsync(d_dims, dims.data(), fbytes, cudaMemcpyHostToDevice, ctx->stream));
+    SD_CUDA(ctx, cudaMemcpyAsync(d_rec, recs.data(), gbytes, cudaMemcpyHostToDevice, ctx->stream));
+    SD_CUDA(ctx, cudaMemsetAsync(d_miss, 0, count, ctx->stream));
+    SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[0], ctx->stream));
+    SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[1], ctx->stream));
+    int buf = 0;
+    for (size_t c = 0; c + 1 < chunk_first.size(); ++c, buf ^= 1) {
+        const int first = chunk_first[c], n = chunk_first[c + 1] - first, ng = chunk_grey[c];
+        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_done[buf], 0));   // also orders the table uploads before the first gather
+        // the SMs read the chunk's ROI rows zero-copy from the pinned frames: no host cores are spent packing rows at link speed
+        if (ng > 0) {
+            roi_gather_kernel<1><<<ng < 8 * ctx->sm_count ? ng : 8 * ctx->sm_count, 256, 0, ctx->copy_stream>>>(d_rec + first, ng, (uint8_t*)ctx->d_stage[buf]);
+            SD_LAUNCH_CHECK(ctx, "roi_gather_kernel<1>");
+        }
+        if (n - ng > 0) {
+            roi_gather_kernel<3><<<n - ng < 8 * ctx->sm_count ? n - ng : 8 * ctx->sm_count, 256, 0, ctx->copy_stream>>>(d_rec + first + ng, n - ng, (uint8_t*)ctx->d_stage[buf]);
+            SD_LAUNCH_CHECK(ctx, "roi_gather_kernel<3>");
+        }
+        SD_CUDA(ctx, cudaEventRecord(ctx->stage_ev[buf], ctx->copy_stream));
+        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->stage_ev[buf], 0));
+        sd_image_batch ib{};
+        ib.d_data = (const uint8_t*)ctx->d_stage[buf];
+        ib.count = n;
+        ib.d_roi = d_roi + first;
+        ib.d_roi_miss = d_miss + first;
+        ib.d_frames = d_dims + first;
+        rc = detect_device(ctx, m, &ib, nullptr, d_x + (size_t)first * P, n, d_out + (size_t)first * P);
+        if (rc) return rc;
+        SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[buf], ctx->stream));
+    }
+    std::vector<uint8_t> miss(count);
+    SD_CUDA(ctx, cudaMemcpyAsync(out, d_out, xbytes, cudaMemcpyDeviceToHost, ctx->stream));
+    SD_CUDA(ctx, cudaMemcpyAsync(miss.data(), d_miss, count, cudaMemcpyDeviceToHost, ctx->stream));
+    rc = sd_check_hog_status(ctx, "detect");                  // synchronises
+    if (rc) return rc;
+    // faces whose cascade wandered outside the gathered region: repeat them from their full frames
+    std::vector<int> again;
+    for (int i = 0; i < count; ++i) if (miss[i]) again.push_back(i);
+    if (again.empty()) return SD_OK;
+    ctx->roi_fallbacks += (int64_t)again.size();
+    const int na = (int)again.size();
+    std::vector<int32_t> ff(na);
+    std::vector<float> xa((size_t)na * P), xo((size_t)na * P);
+    for (int j = 0; j < na; ++j) {
+        ff[j] = face_frame[again[j]];
+        memcpy(&xa[(size_t)j * P], x0 + (size_t)again[j] * P, P * sizeof(float));
+    }
+    rc = detect_faces_full(ctx, m, frames, ff.data(), na, xa.data(), xo.data());
+    if (rc) return rc;
+    for (int j = 0; j < na; ++j) memcpy(out + (size_t)again[j] * P, &xo[(size_t)j * P], P * sizeof(float));
+    return SD_OK;
 }
 
 }  // namespace
@@ -483,138 +798,67 @@ int sd_detect_batch_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch*
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, m && images && d_x0 && d_landmarks && count >= 0, "bad argument");
     SD_REQUIRE(ctx, images->count >= count, "fewer images than faces");
-    const int rc = detect_device(ctx, m, images, d_x0, count, d_landmarks);
+    const int rc = detect_device(ctx, m, images, nullptr, d_x0, count, d_landmarks);
     if (rc) return rc;
     // a degenerate face (inter-eye distance too small for a patch) or a bad frame index is an error here, as it is in the
     // reference (cv::resize on an empty ROI throws); reading the flag synchronises the stream
     return sd_check_hog_status(ctx, "detect");
 }
 
-static int detect_host_full(sd_ctx* ctx, const sd_model* m, const uint8_t* h_images, int count, int width, int height,
-                            int row_stride, const int32_t* h_boxes, float* h_landmarks)
+int sd_detect_faces_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_face_frame,
+                           const float* d_x0, int num_faces, float* d_landmarks)
 {
-    const int L = m->num_landmarks, P = 2 * L;
-    const size_t frame_bytes = (size_t)height * row_stride;
-    // chunking: ~128 MB of frames per staging buffer, at least 1 face
-    int chunk = (int)((size_t)(128u << 20) / frame_bytes);
-    if (chunk < 1) chunk = 1;
-    if (chunk > count) chunk = count;
-    for (int b = 0; b < 2; ++b) {
-        if (ctx->stage_bytes[b] < (size_t)chunk * frame_bytes) {
-            if (ctx->d_stage[b]) { SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); SD_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream)); SD_CUDA(ctx, cudaFree(ctx->d_stage[b])); ctx->d_stage[b] = nullptr; }
-            SD_CUDA(ctx, cudaMalloc(&ctx->d_stage[b], (size_t)chunk * frame_bytes));
-            ctx->stage_bytes[b] = (size_t)chunk * frame_bytes;
-        }
-    }
-    // initial landmarks for every face: align_mean on the host (model.hpp:135), one small upload
-    std::vector<float> x0((size_t)count * P);
-    for (int i = 0; i < count; ++i)
-        sd_align_mean(m->mean.data(), L, h_boxes[4 * i], h_boxes[4 * i + 1], h_boxes[4 * i + 2], h_boxes[4 * i + 3], 1.f, 1.f, 0.f, 0.f, &x0[(size_t)i * P]);
-    float* d_x = (float*)sd_workspace(ctx, SD_WS_PARTIAL, (size_t)2 * count * P * sizeof(float));
-    if (!d_x) return SD_ERR_CUDA;
-    float* d_out = d_x + (size_t)count * P;
-    SD_CUDA(ctx, cudaMemcpyAsync(d_x, x0.data(), x0.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    // the copy stream must not run ahead of work already queued on the compute stream that still reads the staging buffers
-    SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[0], ctx->stream));
-    SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[1], ctx->stream));
-    int buf = 0;
-    for (int first = 0; first < count; first += chunk, buf ^= 1) {
-        const int n = (count - first < chunk) ? count - first : chunk;
-        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_done[buf], 0));
-        SD_CUDA(ctx, cudaMemcpyAsync(ctx->d_stage[buf], h_images + (size_t)first * frame_bytes, (size_t)n * frame_bytes,
-                                     cudaMemcpyHostToDevice, ctx->copy_stream));
-        SD_CUDA(ctx, cudaEventRecord(ctx->stage_ev[buf], ctx->copy_stream));
-        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->stage_ev[buf], 0));
-        sd_image_batch ib{};
-        ib.d_data = (const uint8_t*)ctx->d_stage[buf];
-        ib.width = width; ib.height = height; ib.row_stride = row_stride; ib.image_stride = (int64_t)frame_bytes; ib.count = n;
-        int rc = detect_device(ctx, m, &ib, d_x + (size_t)first * P, n, d_out + (size_t)first * P);
-        if (rc) return rc;
-        SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[buf], ctx->stream));
-    }
-    SD_CUDA(ctx, cudaMemcpyAsync(h_landmarks, d_out, (size_t)count * P * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-    return sd_check_hog_status(ctx, "detect");                // synchronises
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, m && images && d_x0 && d_landmarks && num_faces >= 0, "bad argument");
+    if (!d_face_frame) SD_REQUIRE(ctx, images->count >= num_faces, "fewer images than faces");
+    const int rc = detect_device(ctx, m, images, d_face_frame, d_x0, num_faces, d_landmarks);
+    if (rc) return rc;
+    return sd_check_hog_status(ctx, "detect");                // also reports a face index out of range
 }
 
-// ROI route: needs the caller's frames in pinned (device-mapped) host memory
-static int detect_host_roi(sd_ctx* ctx, const sd_model* m, const uint8_t* h_images, const uint8_t* d_alias, int count, int width,
-                           int height, int row_stride, const int32_t* h_boxes, float* h_landmarks)
+int sd_detect_faces_host(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frames, int num_frames, const int32_t* h_face_frame,
+                         int num_faces, const int32_t* h_boxes, const float* h_x0, float* h_landmarks)
 {
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, m && num_frames >= 0 && num_faces >= 0, "bad argument");
+    if (num_faces == 0) return SD_OK;
+    SD_REQUIRE(ctx, frames && h_face_frame && h_landmarks, "null argument");
+    SD_REQUIRE(ctx, (h_boxes == nullptr) != (h_x0 == nullptr), "exactly one of h_boxes and h_x0 must be given");
+    std::vector<char> used(num_frames, 0);
+    for (int i = 0; i < num_faces; ++i) {
+        if (h_face_frame[i] < 0 || h_face_frame[i] >= num_frames)
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: face %d refers to frame %d of %d", __func__, i, h_face_frame[i], num_frames);
+        used[h_face_frame[i]] = 1;
+    }
+    for (int f = 0; f < num_frames; ++f) {
+        if (!used[f]) continue;
+        const sd_host_frame& fr = frames[f];
+        if (fr.channels != 1 && fr.channels != 3)
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d has %d channels (1 or 3)", __func__, f, fr.channels);
+        if (!fr.h_data || fr.width <= 0 || fr.height <= 0 || (int64_t)fr.row_stride < (int64_t)fr.width * fr.channels)
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d: bad data pointer, size or row_stride < width * channels", __func__, f);
+    }
     const int L = m->num_landmarks, P = 2 * L;
-    const size_t frame_bytes = (size_t)height * row_stride;
-    const size_t chunk_cap = (size_t)48 << 20;            // packed ROI bytes per staging buffer
-    // initial landmarks and the ROI of every face; faces are grouped into chunks that fit one staging buffer
-    std::vector<float> x0((size_t)count * P);
-    std::vector<sd_roi> rois(count);
-    std::vector<int> chunk_first;
-    size_t used = 0;
-    for (int i = 0; i < count; ++i) {
-        sd_align_mean(m->mean.data(), L, h_boxes[4 * i], h_boxes[4 * i + 1], h_boxes[4 * i + 2], h_boxes[4 * i + 3], 1.f, 1.f, 0.f, 0.f, &x0[(size_t)i * P]);
-        sd_roi r = face_roi(m, &x0[(size_t)i * P], width, height, row_stride);
-        const size_t bytes = (size_t)r.row_stride * r.h;
-        if (bytes > chunk_cap)                                // a face window larger than a staging buffer: whole-frame route
-            return detect_host_full(ctx, m, h_images, count, width, height, row_stride, h_boxes, h_landmarks);
-        if (chunk_first.empty() || used + bytes > chunk_cap) { chunk_first.push_back(i); used = 0; }
-        r.offset = (int64_t)used;
-        used += bytes;
-        rois[i] = r;
+    // initial landmarks: align_mean of each box on the host (model.hpp:135), or the caller's
+    std::vector<float> x0;
+    if (h_boxes) {
+        x0.resize((size_t)num_faces * P);
+        for (int i = 0; i < num_faces; ++i)
+            sd_align_mean(m->mean.data(), L, h_boxes[4 * i], h_boxes[4 * i + 1], h_boxes[4 * i + 2], h_boxes[4 * i + 3], 1.f, 1.f, 0.f, 0.f,
+                          &x0[(size_t)i * P]);
     }
-    chunk_first.push_back(count);
-    for (int b = 0; b < 2; ++b) {
-        if (ctx->stage_bytes[b] < chunk_cap + (1u << 20)) {
-            if (ctx->d_stage[b]) { SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); SD_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream)); SD_CUDA(ctx, cudaFree(ctx->d_stage[b])); ctx->d_stage[b] = nullptr; }
-            SD_CUDA(ctx, cudaMalloc(&ctx->d_stage[b], chunk_cap + (1u << 20)));
-            ctx->stage_bytes[b] = chunk_cap + (1u << 20);
-        }
+    const float* xs = h_boxes ? x0.data() : h_x0;
+    // ROI route when every referenced frame is in pinned, device-mapped host memory with 16-byte aligned rows
+    std::vector<const uint8_t*> mapped(num_frames, nullptr);
+    PinnedRange last;
+    bool roi = true;
+    for (int f = 0; f < num_frames && roi; ++f) {
+        if (!used[f]) continue;
+        mapped[f] = mapped_frame(frames[f].h_data, host_frame_bytes(frames[f]), last);
+        roi = mapped[f] && ((reinterpret_cast<uintptr_t>(mapped[f]) | (uintptr_t)frames[f].row_stride) & 15) == 0;
     }
-    // device tables: landmarks (in, out), ROI records, miss flags
-    const size_t xbytes = (size_t)count * P * sizeof(float);
-    const size_t rbytes = (size_t)count * sizeof(sd_roi);
-    unsigned char* tab = (unsigned char*)sd_workspace(ctx, SD_WS_PARTIAL, 2 * xbytes + rbytes + count + 64);
-    if (!tab) return SD_ERR_CUDA;
-    float* d_x = (float*)tab;
-    float* d_out = (float*)(tab + xbytes);
-    sd_roi* d_roi = (sd_roi*)(tab + 2 * xbytes);
-    uint8_t* d_miss = tab + 2 * xbytes + rbytes;
-    SD_CUDA(ctx, cudaMemcpyAsync(d_x, x0.data(), xbytes, cudaMemcpyHostToDevice, ctx->stream));
-    SD_CUDA(ctx, cudaMemcpyAsync(d_roi, rois.data(), rbytes, cudaMemcpyHostToDevice, ctx->stream));
-    SD_CUDA(ctx, cudaMemsetAsync(d_miss, 0, count, ctx->stream));
-    SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[0], ctx->stream));
-    SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[1], ctx->stream));
-    int buf = 0;
-    for (size_t c = 0; c + 1 < chunk_first.size(); ++c, buf ^= 1) {
-        const int first = chunk_first[c], n = chunk_first[c + 1] - first;
-        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_done[buf], 0));   // also orders the table uploads before the first gather
-        // the SMs read the chunk's ROI rows zero-copy from the pinned frames: no host cores are spent packing rows at link speed
-        const int blocks = n < 8 * ctx->sm_count ? n : 8 * ctx->sm_count;
-        roi_gather_kernel<<<blocks, 256, 0, ctx->copy_stream>>>(d_alias, (long long)frame_bytes, row_stride, d_roi, first, n, (uint8_t*)ctx->d_stage[buf]);
-        SD_LAUNCH_CHECK(ctx, "roi_gather_kernel");
-        SD_CUDA(ctx, cudaEventRecord(ctx->stage_ev[buf], ctx->copy_stream));
-        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->stage_ev[buf], 0));
-        sd_image_batch ib{};
-        ib.d_data = (const uint8_t*)ctx->d_stage[buf];
-        ib.width = width; ib.height = height; ib.row_stride = row_stride; ib.image_stride = 0; ib.count = n;
-        ib.d_roi = d_roi + first;
-        ib.d_roi_miss = d_miss + first;
-        int rc = detect_device(ctx, m, &ib, d_x + (size_t)first * P, n, d_out + (size_t)first * P);
-        if (rc) return rc;
-        SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[buf], ctx->stream));
-    }
-    std::vector<uint8_t> miss(count);
-    SD_CUDA(ctx, cudaMemcpyAsync(h_landmarks, d_out, xbytes, cudaMemcpyDeviceToHost, ctx->stream));
-    SD_CUDA(ctx, cudaMemcpyAsync(miss.data(), d_miss, count, cudaMemcpyDeviceToHost, ctx->stream));
-    {
-        const int rc = sd_check_hog_status(ctx, "detect");    // synchronises
-        if (rc) return rc;
-    }
-    // faces whose cascade wandered outside the uploaded region: repeat them from their full frames
-    for (int i = 0; i < count; ++i) {
-        if (!miss[i]) continue;
-        ctx->roi_fallbacks++;
-        int rc = detect_host_full(ctx, m, h_images + (size_t)i * frame_bytes, 1, width, height, row_stride, h_boxes + 4 * i, h_landmarks + (size_t)i * P);
-        if (rc) return rc;
-    }
-    return SD_OK;
+    if (roi) return detect_faces_roi(ctx, m, frames, mapped, h_face_frame, num_faces, xs, h_landmarks);
+    return detect_faces_full(ctx, m, frames, h_face_frame, num_faces, xs, h_landmarks);
 }
 
 int sd_detect_batch_host(sd_ctx* ctx, const sd_model* m, const uint8_t* h_images, int count, int width, int height,
@@ -622,16 +866,14 @@ int sd_detect_batch_host(sd_ctx* ctx, const sd_model* m, const uint8_t* h_images
 {
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, m && h_images && h_boxes && h_landmarks && count >= 0 && width > 0 && height > 0 && row_stride >= width, "bad argument");
-    if (count == 0) return SD_OK;
-    // ROI route when the frames are in pinned, device-mapped host memory with 16-byte aligned rows
-    const size_t frame_bytes = (size_t)height * row_stride;
-    cudaPointerAttributes attr;
-    const bool pinned = cudaPointerGetAttributes(&attr, h_images) == cudaSuccess && attr.type == cudaMemoryTypeHost && attr.devicePointer;
-    if (!pinned) cudaGetLastError();
-    const bool aligned = pinned && ((reinterpret_cast<uintptr_t>(attr.devicePointer) | (uintptr_t)row_stride | (uintptr_t)frame_bytes) & 15) == 0;
-    if (aligned)
-        return detect_host_roi(ctx, m, h_images, (const uint8_t*)attr.devicePointer, count, width, height, row_stride, h_boxes, h_landmarks);
-    return detect_host_full(ctx, m, h_images, count, width, height, row_stride, h_boxes, h_landmarks);
+    // frame i at h_images + i * height * row_stride, face i in frame i
+    std::vector<sd_host_frame> frames(count);
+    std::vector<int32_t> face_frame(count);
+    for (int i = 0; i < count; ++i) {
+        frames[i] = sd_host_frame{h_images + (size_t)i * height * row_stride, width, height, row_stride, 1};
+        face_frame[i] = i;
+    }
+    return sd_detect_faces_host(ctx, m, frames.data(), count, face_frame.data(), count, h_boxes, nullptr, h_landmarks);
 }
 
 }  // extern "C"

@@ -1,6 +1,6 @@
 // H100 drop-in for include/rcr/model.hpp: align_mean (:64-76), InterEyeDistanceNormalisation (:84-116),
 // detection_model (:122-183) and load/save_detection_model (:192-219).  detect() runs the whole cascade
-// on the GPU through sd_detect_batch_host; the file format is byte compatible with the reference's
+// on the GPU through sd_detect_faces_host; the file format is byte compatible with the reference's
 // cereal archives (face_landmarks_model_rcr_22.bin loads unchanged).
 #pragma once
 
@@ -93,74 +93,44 @@ public:
     // Run the model from a face box: init with the aligned mean, then optimise (model.hpp:132-144)
     LandmarkCollection<cv::Vec2f> detect(cv::Mat image, cv::Rect facebox)
     {
-        std::vector<cv::Mat> out = detect(std::vector<cv::Mat>{image}, std::vector<cv::Rect>{facebox});
-        return to_landmark_collection(out[0], landmark_ids);
+        return to_landmark_collection(detect(std::vector<cv::Mat>{image}, std::vector<int>{0}, std::vector<cv::Rect>{facebox})[0], landmark_ids);
     }
 
     // Run the model from a landmark initialisation, e.g. the previous frame (model.hpp:147-157)
     LandmarkCollection<cv::Vec2f> detect(cv::Mat image, cv::Mat initialisation)
     {
-        sd_ctx* ctx = sd_b200::context();
-        const cv::Mat& gray = image;               // size only; colour frames are converted on the device
-        const size_t frame = static_cast<size_t>(gray.cols) * gray.rows;
-        sd_b200::DeviceBuffer dimg(frame), dx, dout(static_cast<size_t>(initialisation.cols) * sizeof(float)), bgr;
-        upload_gray(ctx, image, dimg.as<unsigned char>(), bgr);
-        sd_b200::upload(initialisation, dx, initialisation.cols);
-        sd_image_batch ib{};
-        ib.d_data = dimg.as<unsigned char>(); ib.width = gray.cols; ib.height = gray.rows; ib.row_stride = gray.cols; ib.image_stride = static_cast<int64_t>(frame); ib.count = 1;
-        sd_b200::check(ctx, sd_detect_batch_device(ctx, handle.get(), &ib, dx.as<float>(), 1, dout.as<float>()), "sd_detect_batch_device");
-        return to_landmark_collection(sd_b200::download(dout.as<float>(), 1, initialisation.cols, initialisation.cols), landmark_ids);
+        return to_landmark_collection(detect(std::vector<cv::Mat>{image}, std::vector<int>{0}, initialisation)[0], landmark_ids);
     }
 
-    // Batched detect: equally sized frames, one face box each; returns one 1 x 2L row per frame.
+    // Batched detect: one face box per frame, frames of any sizes; returns one 1 x 2L row per frame.
     std::vector<cv::Mat> detect(const std::vector<cv::Mat>& images, const std::vector<cv::Rect>& faceboxes)
     {
         if (images.empty() || images.size() != faceboxes.size()) throw std::runtime_error("detect: images / faceboxes size mismatch");
-        sd_ctx* ctx = sd_b200::context();
-        const int n = static_cast<int>(images.size());
-        const int w = images[0].cols, h = images[0].rows;
-        const int P = 2 * sd_model_num_landmarks(handle.get());
-        bool colour = false;
-        for (int i = 0; i < n; ++i) {
-            if (images[i].cols != w || images[i].rows != h) throw std::runtime_error("detect: the batched path needs equally sized images");
-            colour = colour || images[i].channels() == 3;
-        }
-        if (colour) {
-            // colour frames: upload B,G,R, convert on the device (sd_bgr2gray), start from the aligned mean, stay on the device
-            const size_t frame = static_cast<size_t>(w) * h;
-            sd_b200::DeviceBuffer dimg(frame * n), dx(static_cast<size_t>(n) * P * sizeof(float)), dout(static_cast<size_t>(n) * P * sizeof(float)), bgr;
-            std::vector<float> x0(static_cast<size_t>(n) * P);
-            const cv::Mat mean = get_mean();
-            for (int i = 0; i < n; ++i) {
-                upload_gray(ctx, images[i], dimg.as<unsigned char>() + i * frame, bgr);
-                sd_b200::check(ctx, sd_align_mean(mean.ptr<float>(0), P / 2, faceboxes[i].x, faceboxes[i].y, faceboxes[i].width, faceboxes[i].height,
-                                                  1.f, 1.f, 0.f, 0.f, &x0[static_cast<size_t>(i) * P]), "sd_align_mean");
-            }
-            sd_b200::check(ctx, sd_memcpy_h2d(ctx, dx.as<float>(), x0.data(), x0.size() * sizeof(float)), "detect");
-            sd_image_batch ib{};
-            ib.d_data = dimg.as<unsigned char>(); ib.width = w; ib.height = h; ib.row_stride = w; ib.image_stride = static_cast<int64_t>(frame); ib.count = n;
-            sd_b200::check(ctx, sd_detect_batch_device(ctx, handle.get(), &ib, dx.as<float>(), n, dout.as<float>()), "sd_detect_batch_device");
-            const cv::Mat all = sd_b200::download(dout.as<float>(), n, P, P);
-            std::vector<cv::Mat> rows;
-            for (int i = 0; i < n; ++i) rows.push_back(all.row(i).clone());
-            return rows;
-        }
-        std::vector<unsigned char> frames(static_cast<size_t>(n) * w * h);
-        std::vector<int32_t> boxes(static_cast<size_t>(n) * 4);
-        for (int i = 0; i < n; ++i) {
-            const cv::Mat& g = images[i];
-            for (int y = 0; y < h; ++y) std::memcpy(&frames[(static_cast<size_t>(i) * h + y) * w], g.ptr<unsigned char>(y), w);
+        std::vector<int> face_image(images.size());
+        for (size_t i = 0; i < images.size(); ++i) face_image[i] = static_cast<int>(i);
+        return detect(images, face_image, faceboxes);
+    }
+
+    // Several faces per frame: face i lies in images[face_image[i]]; frames 8UC1 or 8UC3 (B,G,R), any sizes and row steps.
+    // Returns one 1 x 2L row per face.
+    std::vector<cv::Mat> detect(const std::vector<cv::Mat>& images, const std::vector<int>& face_image, const std::vector<cv::Rect>& faceboxes)
+    {
+        if (face_image.size() != faceboxes.size()) throw std::runtime_error("detect: face_image / faceboxes size mismatch");
+        std::vector<int32_t> boxes(4 * faceboxes.size());
+        for (size_t i = 0; i < faceboxes.size(); ++i) {
             boxes[4 * i] = faceboxes[i].x; boxes[4 * i + 1] = faceboxes[i].y; boxes[4 * i + 2] = faceboxes[i].width; boxes[4 * i + 3] = faceboxes[i].height;
         }
-        std::vector<float> lms(static_cast<size_t>(n) * P);
-        sd_b200::check(ctx, sd_detect_batch_host(ctx, handle.get(), frames.data(), n, w, h, w, boxes.data(), lms.data()), "sd_detect_batch_host");
-        std::vector<cv::Mat> out;
-        for (int i = 0; i < n; ++i) {
-            cv::Mat row(1, P, CV_32FC1);
-            std::memcpy(row.ptr<float>(0), &lms[static_cast<size_t>(i) * P], sizeof(float) * P);
-            out.push_back(row);
-        }
-        return out;
+        return detect_faces(images, face_image, boxes.data(), nullptr);
+    }
+
+    // Several faces per frame, each from a landmark initialisation (one 1 x 2L row per face, e.g. the previous frame's result).
+    std::vector<cv::Mat> detect(const std::vector<cv::Mat>& images, const std::vector<int>& face_image, cv::Mat initialisations)
+    {
+        const int P = 2 * sd_model_num_landmarks(handle.get());
+        if (initialisations.rows != static_cast<int>(face_image.size()) || initialisations.cols != P)
+            throw std::runtime_error("detect: initialisations must be one 1 x 2L row per face");
+        const cv::Mat x0 = initialisations.isContinuous() ? initialisations : initialisations.clone();
+        return detect_faces(images, face_image, nullptr, x0.ptr<float>(0));
     }
 
     cv::Mat get_mean()
@@ -174,22 +144,27 @@ public:
 
 private:
     friend detection_model load_detection_model(std::string filename);
-    // frame -> device as 8UC1; colour frames go up as B,G,R and are converted there
-    // (cv::cvtColor BGR2GRAY of adaptive_vlhog.hpp:115-117 == sd_bgr2gray)
-    static void upload_gray(sd_ctx* ctx, const cv::Mat& image, unsigned char* d_dst, sd_b200::DeviceBuffer& bgr)
+    // sd_detect_faces_host: frames stay in host memory (Mat::step() is the row stride), landmarks come back in face order
+    std::vector<cv::Mat> detect_faces(const std::vector<cv::Mat>& images, const std::vector<int>& face_image, const int32_t* boxes, const float* x0)
     {
-        const int w = image.cols, h = image.rows;
-        const size_t frame = static_cast<size_t>(w) * h;
-        if (image.channels() == 3) {
-            bgr.allocate(3 * frame);
-            for (int y = 0; y < h; ++y)
-                sd_b200::check(ctx, sd_memcpy_h2d(ctx, bgr.as<unsigned char>() + static_cast<size_t>(y) * 3 * w, image.ptr<unsigned char>(y), 3 * static_cast<size_t>(w)), "detect upload");
-            sd_b200::check(ctx, sd_bgr2gray(ctx, bgr.as<unsigned char>(), w, h, 3 * static_cast<int64_t>(w), 3 * static_cast<int64_t>(frame), 1, d_dst, w,
-                                            static_cast<int64_t>(frame)), "sd_bgr2gray");
-        } else {
-            for (int y = 0; y < h; ++y)
-                sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_dst + static_cast<size_t>(y) * w, image.ptr<unsigned char>(y), w), "detect upload");
+        sd_ctx* ctx = sd_b200::context();
+        const int P = 2 * sd_model_num_landmarks(handle.get());
+        std::vector<sd_host_frame> frames(images.size());
+        for (size_t i = 0; i < images.size(); ++i) {
+            const cv::Mat& im = images[i];
+            frames[i] = sd_host_frame{im.ptr<unsigned char>(0), im.cols, im.rows, static_cast<int32_t>(im.step()), im.channels()};
         }
+        const std::vector<int32_t> idx(face_image.begin(), face_image.end());
+        std::vector<float> lms(face_image.size() * P);
+        sd_b200::check(ctx, sd_detect_faces_host(ctx, handle.get(), frames.data(), static_cast<int>(frames.size()), idx.data(), static_cast<int>(idx.size()),
+                                                 boxes, x0, lms.data()), "sd_detect_faces_host");
+        std::vector<cv::Mat> out;
+        for (size_t i = 0; i < face_image.size(); ++i) {
+            cv::Mat row(1, P, CV_32FC1);
+            std::memcpy(row.ptr<float>(0), &lms[i * P], sizeof(float) * P);
+            out.push_back(row);
+        }
+        return out;
     }
 
     std::shared_ptr<sd_model> handle;
