@@ -12,7 +12,8 @@
  *   - matrices are row-major float32, one sample per row (cv::Mat CV_32FC1 as the
  *     reference uses it, regressors.hpp:202-206); `ld` = row stride in floats.
  *   - landmark rows are [x_0..x_{L-1}, y_0..y_{L-1}] (adaptive_vlhog.hpp:96-97).
- *   - images are 8-bit single channel (adaptive_vlhog.hpp:115-120 grey path).
+ *   - device images are 8-bit single channel (adaptive_vlhog.hpp:115-120 grey path); host frames (sd_host_frame) are
+ *     8UC1 or 8UC3 B,G,R and reach the device as grey frames (sd_upload_frames, sd_detect_faces_host).
  *   - pointers named d_* are DEVICE pointers, h_* are HOST pointers.
  *   - every call is asynchronous on the context's stream unless it returns host
  *     data; sd_sync() waits.  Functions are re-entrant on distinct contexts.
@@ -105,7 +106,7 @@ typedef struct {
     int32_t count;
     /* Optional (NULL = whole frames are resident): only a region of interest of every frame was uploaded.
      * d_roi[i] locates it inside d_data; a patch that needs frame pixels outside its ROI sets d_roi_miss[i]
-     * (sd_detect_batch_host then repeats that face from the full frame). */
+     * (sd_detect_faces_host then repeats that face from the full frame). */
     const sd_roi* d_roi;
     uint8_t* d_roi_miss;
     /* Optional (NULL = equally sized frames): per-frame size / pitch / position; width, height, row_stride and image_stride
@@ -114,7 +115,8 @@ typedef struct {
     const sd_frame* d_frames;
 } sd_image_batch;
 
-/* One host frame of a detect call: 8UC1, or 8UC3 with interleaved B,G,R (converted exactly as sd_bgr2gray does). */
+/* One host frame (sd_detect_faces_host, sd_upload_frames): 8UC1, or 8UC3 with interleaved B,G,R (converted exactly as
+ * sd_bgr2gray does). */
 typedef struct {
     const uint8_t* h_data;
     int32_t width, height;
@@ -134,7 +136,8 @@ SD_API int sd_sync(sd_ctx* ctx);
 SD_API const char* sd_version(void);
 /* number of kernels of THIS library launched on ctx since creation (bench.py's gpu_launches) */
 SD_API int64_t sd_launch_count(const sd_ctx* ctx);
-/* faces that sd_detect_batch_host / sd_detect_faces_host had to repeat from their full frame (a patch left the uploaded ROI) */
+/* faces that sd_detect_faces_host (and sd_detect_batch_host through it) had to repeat from their full frame (a patch left the
+ * uploaded ROI) */
 SD_API int64_t sd_roi_fallback_count(const sd_ctx* ctx);
 
 /* device / pinned-host memory for hosts that do not bring their own allocator */
@@ -184,6 +187,14 @@ SD_API int sd_hog_debug(sd_ctx* ctx, const sd_image_batch* images, const int32_t
 SD_API int sd_bgr2gray(sd_ctx* ctx, const uint8_t* d_bgr, int width, int height, int64_t bgr_row_stride,
                        int64_t bgr_image_stride, int count, uint8_t* d_gray, int64_t gray_row_stride,
                        int64_t gray_image_stride);
+/* Host frames (8UC1 or 8UC3 B,G,R, any sizes and row strides) -> one grey batch for sd_hog_batch, the upload of
+ * HogTransform's images.  d_buf == NULL: *bytes receives the size d_buf needs and nothing else happens.  Otherwise d_buf
+ * (16-byte aligned, *bytes long) receives the grey frames at a 16-byte pitch, followed by the sd_frame table if the sizes
+ * differ; *out describes the batch (plain strided batch when all frames share one size).  Colour is converted as
+ * sd_bgr2gray does, through context-owned scratch (never d_buf).  Returns when the copies are done.
+ * A bad frame (as for sd_detect_faces_host), count < 1, an unaligned d_buf or a *bytes below the size query's are
+ * SD_ERR_INVALID before any work is queued (d_buf is not written). */
+SD_API int sd_upload_frames(sd_ctx* ctx, const sd_host_frame* frames, int count, void* d_buf, size_t* bytes, sd_image_batch* out);
 
 /* ---- regressor: LinearRegressor<Solver> (regressors.hpp:318-400) ------------------------ */
 /* Solver::solve (regressors.hpp:199-234 == verbose_solver.hpp:53-111):

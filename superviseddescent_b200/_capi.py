@@ -54,7 +54,7 @@ EXPORTS = [
     "sd_ctx_create", "sd_ctx_destroy", "sd_last_error", "sd_sync", "sd_version", "sd_launch_count", "sd_roi_fallback_count",
     "sd_malloc", "sd_free", "sd_host_alloc", "sd_host_free", "sd_memcpy_h2d", "sd_memcpy_d2h", "sd_memset",
     "sd_memcpy2d_h2d", "sd_memcpy2d_d2h", "sd_memcpy2d_d2d",
-    "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_bgr2gray",
+    "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_bgr2gray", "sd_upload_frames",
     "sd_learn", "sd_centre_features", "sd_learn_centred", "sd_learn_rank_revealing", "sd_gram", "sd_solve_gram", "sd_predict", "sd_test_residual", "sd_solver_timings", "sd_set_gram_mode", "sd_set_solver", "sd_solver_iterations",
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",
     "sd_comm_sum_int64", "sd_comm_allgather", "sd_allreduce_gram", "sd_reduce_scatter_gram", "sd_solve_gram_dist", "sd_learn_dist",

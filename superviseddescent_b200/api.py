@@ -269,14 +269,7 @@ class FixedHogTransform:
 
     def __init__(self, images, vlhog_variant: int, num_cells: int, cell_size: int, num_bins: int, ctx: Optional["Context"] = None):
         self.ctx = ctx or default_context()
-        imgs = images if isinstance(images, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(images))
-        if imgs.dim() == 2:
-            imgs = imgs.unsqueeze(0)
-        if imgs.dtype == torch.uint8 and imgs.dim() == 4 and imgs.shape[3] == 3:
-            imgs = bgr2gray(imgs, self.ctx)                      # :201-206
-        if imgs.dtype != torch.uint8 or imgs.dim() != 3:
-            raise ValueError("images must be (count, H, W) uint8 or (count, H, W, 3) uint8")
-        self.images = imgs.to(f"cuda:{self.ctx.device}").contiguous()
+        self.images, self._batch = _device_images(images, self.ctx)     # colour: :201-206
         self.param = HoGParam(int(vlhog_variant), num_cells, cell_size, num_bins, 0.0)
 
     def feature_length(self, num_landmarks: int) -> int:
@@ -303,9 +296,7 @@ class FixedHogTransform:
         output: callers overwrite or ignore it)."""
         ctx = self.ctx
         n, L = parameters.shape[0], parameters.shape[1] // 2
-        h, w = self.images.shape[1], self.images.shape[2]
-        ib = ImageBatchC(C.c_void_p(self.images.data_ptr()), w, h, self.images.stride(1), self.images.stride(0), self.images.shape[0])
-        _check(ctx.h, _capi.lib().sd_hog_batch(ctx.h, C.byref(ib), ptr(image_index) if image_index is not None else C.c_void_p(0),
+        _check(ctx.h, _capi.lib().sd_hog_batch(ctx.h, C.byref(self._batch), ptr(image_index) if image_index is not None else C.c_void_p(0),
                                                ptr(parameters), C.c_int64(parameters.stride(0)), n, L, None, C.byref(self.param),
                                                ptr(out), C.c_int64(out.stride(0))))
 
@@ -327,9 +318,46 @@ def bgr2gray(images, ctx: Optional["Context"] = None) -> torch.Tensor:
     return out
 
 
+def _device_images(images, ctx: Context):
+    """The images of a HogTransform -> (the device tensor that owns them, the ImageBatchC sd_hog_batch reads).  A CUDA tensor
+    (count, H, W) is used in place and (count, H, W, 3) converted by bgr2gray; a host (count, H, W) array or tensor is copied
+    in one piece.  Anything else from the host -- a list of (H, W) or (H, W, 3) frames of any sizes, or a (count, H, W, 3)
+    array -- is uploaded by sd_upload_frames."""
+    dev = f"cuda:{ctx.device}"
+    if isinstance(images, (list, tuple)):
+        frames = list(images)
+    else:
+        t = images if isinstance(images, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(images))
+        if t.dim() == 2:
+            t = t.unsqueeze(0)
+        if t.dtype != torch.uint8 or not (t.dim() == 3 or (t.dim() == 4 and t.shape[3] == 3)):
+            raise ValueError("images must be (count, H, W) uint8, (count, H, W, 3) uint8, or a list of such frames of any sizes")
+        if t.is_cuda or t.dim() == 3:
+            t = t.to(dev)
+            t = (bgr2gray(t, ctx) if t.dim() == 4 else t).contiguous()
+            n, h, w = t.shape
+            return t, ImageBatchC(C.c_void_p(t.data_ptr()), w, h, t.stride(1), t.stride(0), n)
+        frames = list(t)
+    recs, keep = [], []
+    for f in frames:
+        rec, a = _host_frame(f)
+        if a.ndim == 3 and a.shape[2] != 3:
+            raise ValueError("every image must be (H, W) uint8 or (H, W, 3) uint8")
+        recs.append(rec)
+        keep.append(a)                                       # the bytes stay alive until the upload returns
+    table = (HostFrameC * len(recs))(*recs)
+    nbytes = C.c_size_t(0)
+    _check(ctx.h, _capi.lib().sd_upload_frames(ctx.h, table, len(recs), None, C.byref(nbytes), None))
+    buf = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    ib = ImageBatchC()
+    _check(ctx.h, _capi.lib().sd_upload_frames(ctx.h, table, len(recs), ptr(buf), C.byref(nbytes), C.byref(ib)))
+    return buf, ib
+
+
 class HogTransform:
     """Projection functor h.  images: (count, H, W) uint8 (8UC1) or (count, H, W, 3) uint8 (8UC3, B G R: converted
-    once on the device as adaptive_vlhog.hpp:114-120 does per call), on host or device.
+    once on the device as adaptive_vlhog.hpp:114-120 does per call), on host or device, or a list of such frames of any
+    sizes.
 
     __call__(parameters, regressor_level, training_index) keeps the reference's meaning
     (adaptive_vlhog.hpp:109) but takes ALL rows at once: parameters is (N, 2L) and training_index an
@@ -340,48 +368,13 @@ class HogTransform:
     def __init__(self, images, hog_params: Sequence[HoGParam], model_landmarks_list: Sequence[str],
                  right_eye_identifiers: Sequence[str], left_eye_identifiers: Sequence[str], ctx: Optional[Context] = None):
         self.ctx = ctx or default_context()
-        self.frames = None
-        if isinstance(images, (list, tuple)) and len({np.asarray(im).shape for im in images}) > 1:
-            # frames of different sizes (the reference takes a std::vector<cv::Mat>): packed back to back, rows 16-byte aligned,
-            # with one sd_frame descriptor each
-            recs, chunks, off = [], [], 0
-            for im in images:
-                a = np.ascontiguousarray(im, dtype=np.uint8)
-                if a.ndim == 3 and a.shape[2] == 3:
-                    a = bgr2gray(a[None], self.ctx)[0].cpu().numpy()
-                if a.ndim != 2:
-                    raise ValueError("every image must be (H, W) uint8 or (H, W, 3) uint8")
-                h, w = a.shape
-                stride = (w + 15) // 16 * 16
-                buf = np.zeros((h, stride), dtype=np.uint8)
-                buf[:, :w] = a
-                recs.append((w, h, stride, 0, off))
-                chunks.append(buf.reshape(-1))
-                off += h * stride
-            self.images = torch.from_numpy(np.concatenate(chunks)).to(f"cuda:{self.ctx.device}")
-            table = np.array(recs, dtype=[("w", "<i4"), ("h", "<i4"), ("s", "<i4"), ("r", "<i4"), ("o", "<i8")])
-            self.frames = torch.from_numpy(table.view(np.uint8).copy()).to(f"cuda:{self.ctx.device}")
-            self.frame_count = len(recs)
-        else:
-            if isinstance(images, (list, tuple)):
-                images = np.stack([np.asarray(im) for im in images])
-            imgs = images if isinstance(images, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(images))
-            if imgs.dim() == 2:
-                imgs = imgs.unsqueeze(0)
-            if imgs.dtype == torch.uint8 and imgs.dim() == 4 and imgs.shape[3] == 3:
-                imgs = bgr2gray(imgs, self.ctx)
-            if imgs.dtype != torch.uint8 or imgs.dim() != 3:
-                raise ValueError("images must be (count, H, W) uint8, (count, H, W, 3) uint8, or a list of such frames of any sizes")
-            self.images = imgs.to(f"cuda:{self.ctx.device}").contiguous()
+        self.images, self._batch = _device_images(images, self.ctx)
         self.hog_params = list(hog_params)
         self.norm = InterEyeDistanceNormalisation(model_landmarks_list, right_eye_identifiers, left_eye_identifiers)
         self.num_landmarks = len(self.norm.model_landmarks_list)
 
     def batch(self) -> ImageBatchC:
-        if self.frames is not None:
-            return ImageBatchC(C.c_void_p(self.images.data_ptr()), 0, 0, 0, 0, self.frame_count, None, None, C.c_void_p(self.frames.data_ptr()))
-        n, h, w = self.images.shape
-        return ImageBatchC(C.c_void_p(self.images.data_ptr()), w, h, self.images.stride(1), self.images.stride(0), n)
+        return self._batch
 
     def feature_length(self, level: int) -> int:
         return _capi.lib().sd_hog_feature_length(self.num_landmarks, C.byref(self.hog_params[level]))

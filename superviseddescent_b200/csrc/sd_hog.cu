@@ -281,7 +281,7 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const HogArgs a,
         img_idx = 0;
         if (tid == 0 && a.status) atomicOr(a.status, 2);
     }
-    // resident region of this frame: the whole frame, or the ROI that sd_detect_batch_host uploaded
+    // resident region of this frame: the whole frame, or the ROI that sd_detect_faces_host gathered
     int W = a.width, H = a.height, rs = a.row_stride;
     const uint8_t* __restrict__ img = a.images + (long long)img_idx * a.image_stride;
     if (a.frames) {

@@ -16,7 +16,8 @@
 #define SD_MAX_BINS 16   // undirected orientations K supported by the HOG kernel
 
 enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
-       SD_WS_PARTIAL, SD_WS_GEOM, SD_WS_GEMM_PARTIAL, SD_WS_DIAGINV2, SD_WS_PANEL, SD_WS_BIAS, SD_WS_CG, SD_WS_CGMAT, SD_WS_COUNT };
+       SD_WS_PARTIAL, SD_WS_GEOM, SD_WS_GEMM_PARTIAL, SD_WS_DIAGINV2, SD_WS_PANEL, SD_WS_BIAS, SD_WS_CG, SD_WS_CGMAT,
+       SD_WS_UPLOAD /* B,G,R scratch of sd_upload_frames */, SD_WS_COUNT };
 
 // Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row
 // Cholesky blocks), and panel p belongs to rank p % nranks.  The Gram exchange delivers each panel's rows to their owner, and
@@ -36,7 +37,7 @@ struct sd_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    cudaStream_t copy_stream = nullptr;   // host->device staging for sd_detect_faces_host
+    cudaStream_t copy_stream = nullptr;   // host->device copies of host frames (sd_detect_faces_host, sd_upload_frames)
     cudaStream_t chain_stream = nullptr;  // Cholesky look-ahead: next panel's diagonal blocks while the trailing update runs
     cudaEvent_t chain_ev[2] = {nullptr, nullptr};
     int syrk_sm_reserve = 0;              // SMs the persistent SYRK leaves free (1 while a look-ahead chain runs beside it)

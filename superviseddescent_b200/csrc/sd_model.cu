@@ -313,6 +313,85 @@ const uint8_t* mapped_frame(const uint8_t* p, size_t bytes, PinnedRange& last)
 
 size_t host_frame_bytes(const sd_host_frame& f) { return (size_t)(f.height - 1) * f.row_stride + (size_t)f.width * f.channels; }
 size_t round16(size_t v) { return (v + 15) & ~(size_t)15; }
+size_t gray_bytes(const sd_host_frame& f) { return (size_t)f.height * round16(f.width); }
+size_t bgr_bytes(const sd_host_frame& f) { return f.channels == 3 ? (size_t)f.height * round16(3 * (size_t)f.width) : 0; }
+
+// what every entry point that reads sd_host_frame requires of frame f; fn names the entry point in the message
+int check_host_frame(sd_ctx* ctx, const char* fn, const sd_host_frame& fr, int f)
+{
+    if (fr.channels != 1 && fr.channels != 3)
+        return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d has %d channels (1 or 3)", fn, f, fr.channels);
+    if (!fr.h_data || fr.width <= 0 || fr.height <= 0 || (int64_t)fr.row_stride < (int64_t)fr.width * fr.channels)
+        return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d: bad data pointer, size or row_stride < width * channels", fn, f);
+    return SD_OK;
+}
+
+// ---- host frames -> grey device frames (sd_detect_faces_host's chunks, sd_upload_frames) --------------------------------
+// The device layout: grey rows at a 16-byte pitch, frames back to back from offset 0.  Equally sized frames are then a plain
+// strided batch, which the HOG kernel stages by TMA; otherwise each frame is read through its sd_frame descriptor.
+// Fills desc[0..n) and returns the grey bytes; *uniform: all frames share one size.
+size_t frame_layout(const sd_host_frame* frames, int n, sd_frame* desc, bool* uniform)
+{
+    size_t off = 0;
+    *uniform = true;
+    for (int i = 0; i < n; ++i) {
+        const sd_host_frame& f = frames[i];
+        desc[i] = sd_frame{f.width, f.height, (int32_t)round16(f.width), 0, (int64_t)off};
+        off += gray_bytes(f);
+        *uniform = *uniform && f.width == frames[0].width && f.height == frames[0].height;
+    }
+    return off;
+}
+
+// The batch sd_hog_batch reads for frames laid out by frame_layout at d_gray; d_desc: the device copy of desc (read only when
+// the sizes differ).
+sd_image_batch gray_batch(const uint8_t* d_gray, const sd_frame* desc, int n, bool uniform, const sd_frame* d_desc)
+{
+    sd_image_batch ib{};
+    ib.d_data = d_gray;
+    ib.count = n;
+    if (uniform) {
+        ib.width = desc[0].width; ib.height = desc[0].height; ib.row_stride = desc[0].row_stride;
+        ib.image_stride = (int64_t)desc[0].row_stride * desc[0].height;
+    } else {
+        ib.d_frames = d_desc;
+    }
+    return ib;
+}
+
+// Copies frames[0..n) to the layout desc describes at d_gray, on the copy stream once free_ev (recorded on the compute stream:
+// nothing still reads the destination or d_bgr) has completed.  Grey frames go straight to their place; colour frames go as
+// B,G,R rows at a 16-byte pitch, back to back from d_bgr (bgr_bytes each), and the compute stream converts them into place
+// (sd_bgr2gray) after ready_ev, which marks the end of the copies.
+int upload_frames(sd_ctx* ctx, const sd_host_frame* frames, const sd_frame* desc, int n, uint8_t* d_gray, uint8_t* d_bgr,
+                  cudaEvent_t free_ev, cudaEvent_t ready_ev)
+{
+    SD_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, free_ev, 0));
+    uint8_t* bgr = d_bgr;
+    for (int i = 0; i < n; ++i) {
+        const sd_host_frame& f = frames[i];
+        uint8_t* dst = f.channels == 3 ? bgr : d_gray + desc[i].offset;
+        const size_t pitch = f.channels == 3 ? round16(3 * (size_t)f.width) : (size_t)desc[i].row_stride;
+        if ((size_t)f.row_stride == pitch)
+            SD_CUDA(ctx, cudaMemcpyAsync(dst, f.h_data, host_frame_bytes(f), cudaMemcpyHostToDevice, ctx->copy_stream));
+        else
+            SD_CUDA(ctx, cudaMemcpy2DAsync(dst, pitch, f.h_data, f.row_stride, (size_t)f.width * f.channels, f.height,
+                                           cudaMemcpyHostToDevice, ctx->copy_stream));
+        bgr += bgr_bytes(f);
+    }
+    SD_CUDA(ctx, cudaEventRecord(ready_ev, ctx->copy_stream));
+    SD_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ready_ev, 0));
+    bgr = d_bgr;
+    for (int i = 0; i < n; ++i) {
+        const sd_host_frame& f = frames[i];
+        if (f.channels != 3) continue;
+        const int rc = sd_bgr2gray(ctx, bgr, f.width, f.height, (int64_t)round16(3 * (size_t)f.width), 0, 1, d_gray + desc[i].offset,
+                                   desc[i].row_stride, 0);
+        if (rc) return rc;
+        bgr += bgr_bytes(f);
+    }
+    return SD_OK;
+}
 
 // the two staging buffers hold at least `bytes` each
 int ensure_stage(sd_ctx* ctx, size_t bytes)
@@ -327,9 +406,8 @@ int ensure_stage(sd_ctx* ctx, size_t bytes)
     return SD_OK;
 }
 
-// Full route: faces grouped by frame, every referenced frame copied to the device once (grey at a 16-byte pitch; colour as
-// B,G,R behind the chunk's grey frames, converted by bgr2gray_kernel), chunks double-buffered against the cascade.
-// x0 / out: count x 2L in the caller's face order.
+// Full route: faces grouped by frame, every referenced frame copied to the device once (upload_frames; a chunk's B,G,R bytes
+// behind its grey frames), chunks double-buffered against the cascade.  x0 / out: count x 2L in the caller's face order.
 int detect_faces_full(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frames, const int32_t* face_frame, int count,
                       const float* x0, float* out)
 {
@@ -344,30 +422,28 @@ int detect_faces_full(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frame
         if (up.empty() || up.back() != face_frame[order[k]]) up.push_back(face_frame[order[k]]);
         local[k] = (int32_t)up.size() - 1;
     }
-    auto gray_bytes = [&](int f) { return (size_t)frames[f].height * round16(frames[f].width); };
-    auto bgr_bytes = [&](int f) { return frames[f].channels == 3 ? (size_t)frames[f].height * round16(3 * (size_t)frames[f].width) : 0; };
+    std::vector<sd_host_frame> fr(up.size());
+    for (size_t u = 0; u < up.size(); ++u) fr[u] = frames[up[u]];
     std::vector<int> chunk_first;                             // first upload of each chunk
     size_t used = 0, need = 0;
-    for (size_t u = 0; u < up.size(); ++u) {
-        const size_t b = gray_bytes(up[u]) + bgr_bytes(up[u]);
+    for (size_t u = 0; u < fr.size(); ++u) {
+        const size_t b = gray_bytes(fr[u]) + bgr_bytes(fr[u]);
         if (chunk_first.empty() || used + b > chunk_cap) { chunk_first.push_back((int)u); used = 0; }
         used += b;
         need = used > need ? used : need;
     }
-    chunk_first.push_back((int)up.size());
-    // per upload: its grey frame descriptor (offset from the chunk's buffer) and where its B,G,R bytes land
-    std::vector<sd_frame> desc(up.size());
-    std::vector<int64_t> bgr_off(up.size(), 0);
-    std::vector<int> face_first(chunk_first.size(), count);   // first sorted face of each chunk
-    for (size_t c = 0; c + 1 < chunk_first.size(); ++c) {
-        int64_t g = 0;
-        for (int u = chunk_first[c]; u < chunk_first[c + 1]; ++u) {
-            const sd_host_frame& f = frames[up[u]];
-            desc[u] = sd_frame{f.width, f.height, (int32_t)round16(f.width), 0, g};
-            g += (int64_t)gray_bytes(up[u]);
-        }
-        for (int u = chunk_first[c]; u < chunk_first[c + 1]; ++u) { bgr_off[u] = g; g += (int64_t)bgr_bytes(up[u]); }
+    chunk_first.push_back((int)fr.size());
+    // per chunk: the grey layout of its frames in its staging buffer (descriptor offsets from the buffer), B,G,R bytes after it
+    const int nc = (int)chunk_first.size() - 1;
+    std::vector<sd_frame> desc(fr.size());
+    std::vector<size_t> bgr_at(nc);
+    std::vector<char> uniform(nc);
+    for (int c = 0; c < nc; ++c) {
+        bool same = true;
+        bgr_at[c] = frame_layout(fr.data() + chunk_first[c], chunk_first[c + 1] - chunk_first[c], desc.data() + chunk_first[c], &same);
+        uniform[c] = same;
     }
+    std::vector<int> face_first(chunk_first.size(), count);   // first sorted face of each chunk
     std::vector<int> chunk_of(up.size());
     for (size_t c = 0; c + 1 < chunk_first.size(); ++c)
         for (int u = chunk_first[c]; u < chunk_first[c + 1]; ++u) chunk_of[u] = (int)c;
@@ -396,42 +472,12 @@ int detect_faces_full(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frame
     SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[0], ctx->stream));
     SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[1], ctx->stream));
     int buf = 0;
-    for (size_t c = 0; c + 1 < chunk_first.size(); ++c, buf ^= 1) {
+    for (int c = 0; c < nc; ++c, buf ^= 1) {
         const int u0 = chunk_first[c], u1 = chunk_first[c + 1];
         uint8_t* stage = (uint8_t*)ctx->d_stage[buf];
-        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_done[buf], 0));
-        for (int u = u0; u < u1; ++u) {
-            const sd_host_frame& f = frames[up[u]];
-            uint8_t* dst = f.channels == 3 ? stage + bgr_off[u] : stage + desc[u].offset;
-            const size_t pitch = f.channels == 3 ? round16(3 * (size_t)f.width) : (size_t)desc[u].row_stride;
-            if ((size_t)f.row_stride == pitch)
-                SD_CUDA(ctx, cudaMemcpyAsync(dst, f.h_data, host_frame_bytes(f), cudaMemcpyHostToDevice, ctx->copy_stream));
-            else
-                SD_CUDA(ctx, cudaMemcpy2DAsync(dst, pitch, f.h_data, f.row_stride, (size_t)f.width * f.channels, f.height,
-                                               cudaMemcpyHostToDevice, ctx->copy_stream));
-        }
-        SD_CUDA(ctx, cudaEventRecord(ctx->stage_ev[buf], ctx->copy_stream));
-        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->stage_ev[buf], 0));
-        bool uniform = true;
-        for (int u = u0; u < u1; ++u) {
-            const sd_host_frame& f = frames[up[u]];
-            if (f.channels == 3) {
-                rc = sd_bgr2gray(ctx, stage + bgr_off[u], f.width, f.height, (int64_t)round16(3 * (size_t)f.width), 0, 1,
-                                 stage + desc[u].offset, desc[u].row_stride, 0);
-                if (rc) return rc;
-            }
-            uniform = uniform && f.width == frames[up[u0]].width && f.height == frames[up[u0]].height;
-        }
-        // equally sized frames: a plain batch, which the HOG kernel stages by TMA; otherwise one descriptor per frame
-        sd_image_batch ib{};
-        ib.d_data = stage;
-        ib.count = u1 - u0;
-        if (uniform) {
-            ib.width = desc[u0].width; ib.height = desc[u0].height; ib.row_stride = desc[u0].row_stride;
-            ib.image_stride = (int64_t)gray_bytes(up[u0]);
-        } else {
-            ib.d_frames = d_desc + u0;
-        }
+        rc = upload_frames(ctx, fr.data() + u0, desc.data() + u0, u1 - u0, stage, stage + bgr_at[c], ctx->stage_done[buf], ctx->stage_ev[buf]);
+        if (rc) return rc;
+        const sd_image_batch ib = gray_batch(stage, desc.data() + u0, u1 - u0, uniform[c], d_desc + u0);
         const int k0 = face_first[c], n = face_first[c + 1] - k0;
         rc = detect_device(ctx, m, &ib, d_idx + k0, d_x + (size_t)k0 * P, n, d_out + (size_t)k0 * P);
         if (rc) return rc;
@@ -831,12 +877,8 @@ int sd_detect_faces_host(sd_ctx* ctx, const sd_model* m, const sd_host_frame* fr
         used[h_face_frame[i]] = 1;
     }
     for (int f = 0; f < num_frames; ++f) {
-        if (!used[f]) continue;
-        const sd_host_frame& fr = frames[f];
-        if (fr.channels != 1 && fr.channels != 3)
-            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d has %d channels (1 or 3)", __func__, f, fr.channels);
-        if (!fr.h_data || fr.width <= 0 || fr.height <= 0 || (int64_t)fr.row_stride < (int64_t)fr.width * fr.channels)
-            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d: bad data pointer, size or row_stride < width * channels", __func__, f);
+        const int rc = used[f] ? check_host_frame(ctx, __func__, frames[f], f) : SD_OK;
+        if (rc) return rc;
     }
     const int L = m->num_landmarks, P = 2 * L;
     // initial landmarks: align_mean of each box on the host (model.hpp:135), or the caller's
@@ -874,6 +916,42 @@ int sd_detect_batch_host(sd_ctx* ctx, const sd_model* m, const uint8_t* h_images
         face_frame[i] = i;
     }
     return sd_detect_faces_host(ctx, m, frames.data(), count, face_frame.data(), count, h_boxes, nullptr, h_landmarks);
+}
+
+int sd_upload_frames(sd_ctx* ctx, const sd_host_frame* frames, int count, void* d_buf, size_t* bytes, sd_image_batch* out)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, frames && count >= 1 && bytes, "bad argument");
+    for (int f = 0; f < count; ++f) {
+        const int rc = check_host_frame(ctx, __func__, frames[f], f);
+        if (rc) return rc;
+    }
+    std::vector<sd_frame> desc(count);
+    bool uniform = true;
+    const size_t gray = frame_layout(frames, count, desc.data(), &uniform);
+    const size_t need = gray + (uniform ? 0 : (size_t)count * sizeof(sd_frame));   // the descriptors follow the grey frames
+    if (!d_buf) { *bytes = need; return SD_OK; }
+    SD_REQUIRE(ctx, out && (reinterpret_cast<uintptr_t>(d_buf) & 15) == 0 && *bytes >= need,
+               "d_buf must be 16-byte aligned and hold the size the query gives; out must not be NULL");
+    uint8_t* base = static_cast<uint8_t*>(d_buf);
+    // Colour frames pass through the B,G,R scratch about 64 MB at a time, so the scratch stays small when a training set is
+    // uploaded.  The staging events are free: sd_detect_faces_host records them anew before it waits on them, and this call
+    // returns only when its own work is done.
+    const size_t chunk_cap = (size_t)64 << 20;
+    for (int i0 = 0, i1; i0 < count; i0 = i1) {
+        size_t b = bgr_bytes(frames[i0]);
+        for (i1 = i0 + 1; i1 < count && b + bgr_bytes(frames[i1]) <= chunk_cap; ++i1) b += bgr_bytes(frames[i1]);
+        uint8_t* bgr = (uint8_t*)sd_workspace(ctx, SD_WS_UPLOAD, b);
+        if (!bgr) return SD_ERR_CUDA;
+        SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[0], ctx->stream));
+        const int rc = upload_frames(ctx, frames + i0, desc.data() + i0, i1 - i0, base, bgr, ctx->stage_done[0], ctx->stage_ev[0]);
+        if (rc) return rc;
+    }
+    if (!uniform)
+        SD_CUDA(ctx, cudaMemcpyAsync(base + gray, desc.data(), (size_t)count * sizeof(sd_frame), cudaMemcpyHostToDevice, ctx->stream));
+    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));        // the caller may free or reuse the host frames
+    *out = gray_batch(base, desc.data(), count, uniform, reinterpret_cast<const sd_frame*>(base + gray));
+    return SD_OK;
 }
 
 }  // extern "C"

@@ -77,59 +77,24 @@ public:
 
 private:
     struct DeviceImages {
-        sd_b200::DeviceBuffer buf, frames;
+        sd_b200::DeviceBuffer buf;
         sd_image_batch batch{};
         bool ready = false;
     };
 
+    // frames of any sizes (the reference's std::vector<cv::Mat>), grey or colour: colour is converted once here, where the
+    // reference converts it in every call (adaptive_vlhog.hpp:114-120)
     void ensure_uploaded()
     {
         if (dev->ready) return;
         if (images.empty()) throw std::runtime_error("HogTransform: no images");
         sd_ctx* ctx = sd_b200::context();
-        // frames may differ in size (the reference's std::vector<cv::Mat>): packed back to back with 16-byte aligned rows and one
-        // sd_frame descriptor each; equally sized frames take the plain strided layout (and the TMA route of the kernel)
-        bool same = true;
-        for (const cv::Mat& im : images) same = same && im.cols == images[0].cols && im.rows == images[0].rows;
-        std::vector<sd_frame> frames(images.size());
-        size_t total = 0;
-        for (size_t i = 0; i < images.size(); ++i) {
-            const int w = images[i].cols, h = images[i].rows;
-            const int stride = same ? w : (w + 15) / 16 * 16;
-            frames[i].width = w; frames[i].height = h; frames[i].row_stride = stride; frames[i].reserved = 0;
-            frames[i].offset = static_cast<int64_t>(total);
-            total += static_cast<size_t>(stride) * h;
-        }
-        dev->buf.allocate(total);
-        sd_b200::check(ctx, sd_memset(ctx, dev->buf.as<unsigned char>(), 0, total), "HogTransform upload");
-        sd_b200::DeviceBuffer bgr;                 // staging for one colour frame
-        for (size_t i = 0; i < images.size(); ++i) {
-            const cv::Mat& im = images[i];
-            const int w = im.cols, h = im.rows;
-            unsigned char* d_frame = dev->buf.as<unsigned char>() + frames[i].offset;
-            if (im.channels() == 3) {
-                // cv::cvtColor(BGR2GRAY), adaptive_vlhog.hpp:115-117: on the device, once per frame (sd_bgr2gray)
-                const size_t frame = static_cast<size_t>(w) * h;
-                bgr.allocate(3 * frame);
-                sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, bgr.as<unsigned char>(), 3 * static_cast<size_t>(w), im.ptr<unsigned char>(0), im.step(), 3 * static_cast<size_t>(w), h), "HogTransform upload");
-                sd_b200::check(ctx, sd_bgr2gray(ctx, bgr.as<unsigned char>(), w, h, 3 * static_cast<int64_t>(w), 3 * static_cast<int64_t>(frame), 1,
-                                                d_frame, frames[i].row_stride, static_cast<int64_t>(frames[i].row_stride) * h), "sd_bgr2gray");
-            } else {
-                sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, d_frame, frames[i].row_stride, im.ptr<unsigned char>(0), im.step(), w, h), "HogTransform upload");
-            }
-        }
-        dev->batch = sd_image_batch{};
-        dev->batch.d_data = dev->buf.as<unsigned char>();
-        dev->batch.count = static_cast<int32_t>(images.size());
-        if (same) {
-            dev->batch.width = images[0].cols; dev->batch.height = images[0].rows; dev->batch.row_stride = images[0].cols;
-            dev->batch.image_stride = static_cast<int64_t>(images[0].cols) * images[0].rows;
-        } else {
-            dev->frames.allocate(frames.size() * sizeof(sd_frame));
-            sd_b200::check(ctx, sd_memcpy_h2d(ctx, dev->frames.as<sd_frame>(), frames.data(), frames.size() * sizeof(sd_frame)), "HogTransform upload");
-            dev->batch.d_frames = dev->frames.as<sd_frame>();
-        }
-        sd_b200::check(ctx, sd_sync(ctx), "HogTransform upload");
+        const std::vector<sd_host_frame> frames = sd_b200::host_frames(images);
+        const int n = static_cast<int>(frames.size());
+        size_t bytes = 0;
+        sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, nullptr, &bytes, nullptr), "HogTransform upload");
+        dev->buf.allocate(bytes);
+        sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, dev->buf.as<void>(), &bytes, &dev->batch), "HogTransform upload");
         dev->ready = true;
     }
 

@@ -149,11 +149,7 @@ private:
     {
         sd_ctx* ctx = sd_b200::context();
         const int P = 2 * sd_model_num_landmarks(handle.get());
-        std::vector<sd_host_frame> frames(images.size());
-        for (size_t i = 0; i < images.size(); ++i) {
-            const cv::Mat& im = images[i];
-            frames[i] = sd_host_frame{im.ptr<unsigned char>(0), im.cols, im.rows, static_cast<int32_t>(im.step()), im.channels()};
-        }
+        const std::vector<sd_host_frame> frames = sd_b200::host_frames(images);
         const std::vector<int32_t> idx(face_image.begin(), face_image.end());
         std::vector<float> lms(face_image.size() * P);
         sd_b200::check(ctx, sd_detect_faces_host(ctx, handle.get(), frames.data(), static_cast<int>(frames.size()), idx.data(), static_cast<int>(idx.size()),

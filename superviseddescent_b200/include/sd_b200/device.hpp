@@ -7,6 +7,7 @@
 #include <stdexcept>
 #include <string>
 #include <utility>
+#include <vector>
 
 #include "sd_b200.h"
 #include "sd_b200/mat.hpp"
@@ -75,6 +76,17 @@ inline void upload(const cv::Mat& m, DeviceBuffer& dst, int64_t ld)
                                    static_cast<size_t>(m.cols) * sizeof(float), static_cast<size_t>(m.rows)), "upload");
     }
     check(ctx, sd_sync(ctx), "upload");   // the host Mat may go away after this call
+}
+
+// 8UC1 / 8UC3 (B,G,R) frames as the C ABI's host frames: the pixels stay where they are, Mat::step() is the row stride
+inline std::vector<sd_host_frame> host_frames(const std::vector<cv::Mat>& images)
+{
+    std::vector<sd_host_frame> frames(images.size());
+    for (size_t i = 0; i < images.size(); ++i) {
+        const cv::Mat& im = images[i];
+        frames[i] = sd_host_frame{im.ptr<unsigned char>(0), im.cols, im.rows, static_cast<int32_t>(im.step()), im.channels()};
+    }
+    return frames;
 }
 
 inline cv::Mat download(const float* d, int rows, int cols, int64_t ld)

@@ -12,22 +12,27 @@ import os
 import numpy as np
 
 
+def bgr_with_gray(gray, db, dr):
+    """A B,G,R frame whose BGR2GRAY is `gray` exactly: B = grey + db, R = grey + dr, G as described above."""
+    g = gray.astype(np.int64)
+    b = np.clip(g + db, 0, 255)
+    r = np.clip(g + dr, 0, 255)
+    lo = g * 32768 - 3735 * b - 9798 * r - 16384           # need 19235 G >= lo
+    gg = np.maximum(-(-lo // 19235), 0)
+    ok = (gg <= 255) & ((3735 * b + 19235 * gg + 9798 * r + 16384) >> 15 == g)
+    bgr = np.where(ok[..., None], np.stack([b, gg, r], axis=-1), g[..., None])
+    return np.ascontiguousarray(bgr.astype(np.uint8))
+
+
 def examples_bgr(golden):
     chroma = np.load(os.path.join(golden.dir, "examples_chroma.npz"))
     frames = []
     for i in range(5):
         gray = golden.examples[f"gray{i}"]
         h, w = gray.shape
-        g = gray.astype(np.int64)
 
         def up(plane):
             f = -(-h // plane.shape[0])
             return np.repeat(np.repeat(plane.astype(np.int64), f, axis=0), f, axis=1)[:h, :w]
-        b = np.clip(g + up(chroma[f"db{i}"]), 0, 255)
-        r = np.clip(g + up(chroma[f"dr{i}"]), 0, 255)
-        lo = g * 32768 - 3735 * b - 9798 * r - 16384           # need 19235 G >= lo
-        gg = np.maximum(-(-lo // 19235), 0)
-        ok = (gg <= 255) & ((3735 * b + 19235 * gg + 9798 * r + 16384) >> 15 == g)
-        bgr = np.where(ok[..., None], np.stack([b, gg, r], axis=-1), g[..., None])
-        frames.append(np.ascontiguousarray(bgr.astype(np.uint8)))
+        frames.append(bgr_with_gray(gray, up(chroma[f"db{i}"]), up(chroma[f"dr{i}"])))
     return frames

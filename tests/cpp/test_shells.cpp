@@ -189,12 +189,51 @@ static void test_rcr_device_route(const char* model_path)
     EXPECT_REL(dev.at<float>(0, 0), lms[0].coordinates[0], 1e-5);
 }
 
+static void test_hog_colour_frames_of_two_sizes(const char* model_path)
+{
+    // HogTransform over a grey frame and a colour frame of another size whose rows are padded (Mat::step() > 3 * cols): the
+    // features must equal those of the same frames converted to grey on the host (OpenCV's BGR2GRAY fixed point)
+    using namespace rcr;
+    detection_model m = load_detection_model(model_path);
+    Mat mean = m.get_mean();
+    std::vector<std::string> ids;
+    for (int i = 0; i < mean.cols / 2; ++i) ids.emplace_back(sd_model_landmark_id(m.native(), i));
+    std::vector<std::string> reye{"37", "40"}, leye{"43", "46"};
+    const int h0 = 70, w0 = 93, h1 = 61, w1 = 110;
+    unsigned s = 777;
+    auto noise = [&](int x, int y) { s = s * 1664525u + 1013904223u; return static_cast<unsigned char>(128 + 50 * std::sin(0.13 * x) * std::cos(0.09 * y) + ((s >> 24) & 31)); };
+    Mat grey0(h0, w0, CV_8UC1);
+    for (int y = 0; y < h0; ++y) for (int x = 0; x < w0; ++x) grey0.at<unsigned char>(y, x) = noise(x, y);
+    Mat padded(h1, w1 + 7, CV_8UC3), grey1(h1, w1, CV_8UC1);
+    for (int y = 0; y < h1; ++y)
+        for (int x = 0; x < w1 + 7; ++x)
+            for (int c = 0; c < 3; ++c) padded.ptr<unsigned char>(y)[3 * x + c] = noise(x + 40 * c, y);
+    Mat colour1 = padded.colRange(0, w1);
+    for (int y = 0; y < h1; ++y)
+        for (int x = 0; x < w1; ++x) {
+            const unsigned char* p = colour1.ptr<unsigned char>(y) + 3 * x;
+            grey1.at<unsigned char>(y, x) = static_cast<unsigned char>((3735 * p[0] + 19235 * p[1] + 9798 * p[2] + (1 << 14)) >> 15);
+        }
+    std::vector<Mat> colour_frames{grey0, colour1}, grey_frames{grey0, grey1};
+    std::vector<HoGParam> hp{{VlHogVariantUoctti, 3, 8, 4, 0.8f}};
+    HogTransform hc(colour_frames, hp, ids, reye, leye), hg(grey_frames, hp, ids, reye, leye);
+    const cv::Rect boxes[2] = {cv::Rect(12, 6, 64, 64), cv::Rect(-10, 4, 70, 70)};
+    for (int i = 0; i < 2; ++i) {
+        Mat x = align_mean(mean, boxes[i]);
+        Mat a = hc(x, 0, i), b = hg(x, 0, i);
+        int differ = a.cols == b.cols ? 0 : 1;
+        for (int j = 0; j < a.cols && j < b.cols; ++j) differ += a.at<float>(0, j) != b.at<float>(0, j);
+        if (differ) { std::printf("FAIL colour frame list: frame %d, %d features differ from the grey list\n", i, differ); ++failures; }
+    }
+}
+
 int main(int argc, char** argv)
 {
     try {
         test_regressors();
         test_optimiser();
         if (argc >= 2) test_rcr_device_route(argv[1]);
+        if (argc >= 2) test_hog_colour_frames_of_two_sizes(argv[1]);
         if (argc >= 10) {
             rcr::detection_model m = rcr::load_detection_model(argv[1]);
             const int w = std::atoi(argv[3]), h = std::atoi(argv[4]);

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import synth
+from colour_examples import bgr_with_gray
 from conftest import rel_err
 
 pytestmark = pytest.mark.gpu
@@ -143,17 +144,28 @@ def test_fixed_patch_hog_transform_vs_oracle(sd, oracle, variant, nc, cs, K):
 def test_hog_frames_of_different_sizes(sd, oracle, golden):
     """The reference's HogTransform takes a std::vector<cv::Mat> of arbitrary sizes (rcr-train reads photographs of different
     resolutions): a list of differently sized frames goes through per-frame descriptors (sd_frame) and must give, frame by
-    frame, what the oracle gives -- including patches that hang over each frame's OWN border."""
+    frame, what the oracle gives -- including patches that hang over each frame's OWN border.  The same frames in B,G,R (one of
+    them with a padded row step) must give the same features and debug taps."""
     m = oracle.Model(golden.model_path)
     sizes = [(120, 160), (97, 131), (200, 150), (64, 64)]
     frames = [synth.smooth_images(1, h, w, seed=40 + i)[0] for i, (h, w) in enumerate(sizes)]
     boxes = [(10, 8, 90, 90), (40, 20, 80, 80), (-20, 60, 120, 120), (5, 5, 50, 50)]
     x = np.stack([oracle.align_mean(m.mean, b) for b in boxes]).astype(np.float32)
+    rng = np.random.default_rng(41)
+    colour = [bgr_with_gray(f, rng.integers(-40, 41, f.shape), rng.integers(-40, 41, f.shape)) for f in frames]
+    h1, w1 = sizes[1]
+    padded = np.zeros((h1, w1 + 5, 3), dtype=np.uint8)
+    padded[:, :w1] = colour[1]
+    colour[1] = padded[:, :w1]
+    assert all(np.array_equal(oracle.bgr2gray_u8(c), f) for c, f in zip(colour, frames))
     for cs, rel, K in ((11, 1.0, 4), (6, 0.25, 9)):
         hp, ohp = sd.HoGParam(1, 5, cs, K, rel), oracle.HogParam(1, 5, cs, K, rel)
         ht = sd.HogTransform(frames, [hp], m.landmark_ids, m.right_ids, m.left_ids)
         A = ht(x, 0).cpu().numpy()
         geo, patches, bins = ht.debug(x, 0)
+        hc = sd.HogTransform(colour, [hp], m.landmark_ids, m.right_ids, m.left_ids)
+        assert np.array_equal(hc(x, 0).cpu().numpy(), A), cs
+        assert all(np.array_equal(c.cpu().numpy(), g.cpu().numpy()) for c, g in zip(hc.debug(x, 0), (geo, patches, bins))), cs
         for i, f in enumerate(frames):
             ref = oracle.hog_transform(f, x[i], ohp, m.right_idx, m.left_idx)
             assert rel_err(A[i], ref) <= TOL, (i, cs)
