@@ -227,9 +227,10 @@ SD_API int sd_learn_centred(sd_ctx* ctx, sd_comm* comm, const float* d_Ac, int64
 /* ColPivHouseholderQRSolver::solve (regressors.hpp:264-305): the same system, plus the one diagnostic that solver exists for --
  * the numerical rank of the regularised A^T A (regressors.hpp:288-293 prints it and asks for a larger lambda).  A^T A + Lambda is
  * symmetric positive semi-definite, so the rank comes from a diagonally pivoted Cholesky (threshold eps * D relative to the
- * largest pivot, Eigen's default rule), D <= 4096; beyond that *rank_out = -1 (not computed).  Like the reference the call goes
- * on to solve when the matrix is rank deficient; if the solve itself then breaks down the status is SD_ERR_NUMERIC and
- * sd_last_error carries the reference's message with the rank. */
+ * largest pivot, Eigen's default rule) at any D.  It factors a copy of the D x D matrix in its own workspace: 1.16 GB at
+ * D = 17,051 and 11.1 GB at D = 52,701, where a one-GPU train then holds about 44 GB (features 21 + Gram 11 + copy 11).  Like
+ * the reference the call goes on to solve when the matrix is rank deficient; if the solve itself then breaks down the status is
+ * SD_ERR_NUMERIC and sd_last_error carries the reference's message with the rank. */
 SD_API int sd_learn_rank_revealing(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_B, int64_t ldb,
                                    int N, int D, int M, const sd_regulariser* reg, float* d_X, float* lambda_out, int* rank_out);
 /* The same, split at the multi-GPU exchange point (superviseddescent.hpp:207 / SURVEY 8e):
@@ -310,6 +311,16 @@ SD_API int sd_learn_dist(sd_ctx* ctx, sd_comm* comm, const float* d_A, int64_t l
  * was used; -n = CG ran n iterations, gave up, and the factorisation answered; 0 = CG was not tried. */
 SD_API int sd_set_solver(sd_ctx* ctx, int mode);
 SD_API int sd_solver_iterations(const sd_ctx* ctx);
+
+/* The rank diagnostic of sd_learn_rank_revealing for every solve: with on != 0, sd_learn, sd_learn_centred, sd_solve_gram and
+ * sd_learn_dist (routes 0 and 2) also compute the numerical rank of the regularised system (what the optimisers' train() needs
+ * for ColPivHouseholderQRSolver levels).  sd_last_rank, of the last solve: the rank, or -1 when it was not computed.  With
+ * centred features the matrix factored is the centred Gram + Lambda; it is congruent to the uncentred one (T^T (A^T A + Lambda) T
+ * with a unit-triangular T, and T^T Lambda T = Lambda because the bias is not regularised), so its exact rank is the same, and
+ * the relative cut is applied to the better-conditioned matrix.  Route 1 (distributed factorisation) holds no rank's whole
+ * matrix: -1 there. */
+SD_API int sd_set_rank_diagnostic(sd_ctx* ctx, int on);
+SD_API int sd_last_rank(const sd_ctx* ctx);
 
 /* ---- cascade steps: SupervisedDescentOptimiser (superviseddescent.hpp:165-344) ---------- */
 /* b_i = (x_i - x_gt_i) (.) norm(x_i)     (superviseddescent.hpp:199-205) */

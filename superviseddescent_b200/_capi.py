@@ -56,6 +56,7 @@ EXPORTS = [
     "sd_memcpy2d_h2d", "sd_memcpy2d_d2h", "sd_memcpy2d_d2d",
     "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_bgr2gray", "sd_upload_frames",
     "sd_learn", "sd_centre_features", "sd_learn_centred", "sd_learn_rank_revealing", "sd_gram", "sd_solve_gram", "sd_predict", "sd_test_residual", "sd_solver_timings", "sd_set_gram_mode", "sd_set_solver", "sd_solver_iterations",
+    "sd_set_rank_diagnostic", "sd_last_rank",
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",
     "sd_comm_sum_int64", "sd_comm_allgather", "sd_allreduce_gram", "sd_reduce_scatter_gram", "sd_solve_gram_dist", "sd_learn_dist",
     "sd_cascade_targets", "sd_cascade_update", "sd_subtract_templates",
@@ -90,6 +91,7 @@ def lib():
         l.sd_model_landmark_id.argtypes = [C.c_void_p, C.c_int]
         l.sd_comm_destroy.argtypes = [C.c_void_p]
         l.sd_solver_iterations.argtypes = [C.c_void_p]
+        l.sd_last_rank.argtypes = [C.c_void_p]
         l.sd_comm_rank.argtypes = [C.c_void_p]
         l.sd_comm_size.argtypes = [C.c_void_p]
         _lib = l

@@ -74,6 +74,16 @@ class Context:
         iterations, gave up, and the factorisation answered; 0 = CG was not tried."""
         return int(_capi.lib().sd_solver_iterations(self._h))
 
+    def set_rank_diagnostic(self, on: bool) -> None:
+        """With on, every solve also computes the numerical rank of its regularised system (ColPivHouseholderQRSolver's
+        diagnostic); last_rank() reads it.  Off by default: it costs a pivoted factorisation of a copy of the D x D matrix."""
+        _check(self._h, _capi.lib().sd_set_rank_diagnostic(self._h, int(bool(on))))
+
+    def last_rank(self) -> int:
+        """Numerical rank of the last solve's regularised system, or -1 when it was not computed (diagnostic off, or the
+        distributed factorisation)."""
+        return int(_capi.lib().sd_last_rank(self._h))
+
     def solver_timings(self):
         out = (C.c_float * 4)()
         _check(self._h, _capi.lib().sd_solver_timings(self._h, out))
@@ -144,6 +154,12 @@ class ColPivHouseholderQRSolver:
     rank_revealing = True
 
 
+def _print_rank_warning(rank: int, D: int) -> None:
+    """regressors.hpp:290-293"""
+    print("The regularised AtA is not invertible. We continued learning, but Eigen may return garbage (their docu is not "
+          f"very specific). (The rank is {rank}, full rank would be {D}). Increase lambda.")
+
+
 class LinearRegressor:
     """superviseddescent::LinearRegressor<Solver> (regressors.hpp:318-400); `solver` plays the template parameter."""
 
@@ -153,7 +169,7 @@ class LinearRegressor:
         self.solver = solver or PartialPivLUSolver()
         self.x: Optional[torch.Tensor] = None   # D x M, device
         self.last_lambda: Optional[float] = None
-        self.last_rank: Optional[int] = None    # ColPivHouseholderQRSolver only
+        self.last_rank: Optional[int] = None    # ColPivHouseholderQRSolver only: rank of the last learn / train level (-1: not computed)
 
     def _ctx(self) -> Context:
         if self.ctx is None:
@@ -187,8 +203,7 @@ class LinearRegressor:
                                                      N, D, M, C.byref(reg), ptr(X), C.byref(lam), C.byref(rank))
             self.last_rank = rank.value
             if 0 <= rank.value < D:
-                print("The regularised AtA is not invertible. We continued learning, but Eigen may return garbage (their docu is not "
-                      f"very specific). (The rank is {rank.value}, full rank would be {D}). Increase lambda.")
+                _print_rank_warning(rank.value, D)
                 if rc == 5:                       # SD_ERR_NUMERIC: the factorisation of the singular matrix stopped; the reference returns garbage here
                     X.fill_(float("nan"))
                     rc = 0
@@ -517,8 +532,18 @@ class SupervisedDescentOptimiser:
                     ds = 2 if distributed_solve == "cg" else int(bool(distributed_solve))
             ch = comm.h if distributed else None
             _check(ctx.h, lib.sd_centre_features(ctx.h, ch, ptr(A), C.c_int64(A.stride(0)), n, D, n_global, C.byref(rc_), ptr(mu)))
-            _check(ctx.h, lib.sd_learn_centred(ctx.h, ch, ptr(A), C.c_int64(A.stride(0)), ptr(Bv), C.c_int64(A.stride(0)), n, D, P,
-                                               C.byref(rc_), n_global, int(ds), ptr(mu), ptr(X), ptr(Xc), C.byref(lam)))
+            qr = getattr(reg.solver, "rank_revealing", False)                # ColPivHouseholderQRSolver: rank of this level's system
+            if qr:
+                ctx.set_rank_diagnostic(True)
+            rc = lib.sd_learn_centred(ctx.h, ch, ptr(A), C.c_int64(A.stride(0)), ptr(Bv), C.c_int64(A.stride(0)), n, D, P,
+                                      C.byref(rc_), n_global, int(ds), ptr(mu), ptr(X), ptr(Xc), C.byref(lam))
+            if qr:
+                ctx.set_rank_diagnostic(False)
+                reg.last_rank = ctx.last_rank()
+                if 0 <= reg.last_rank < D:
+                    _print_rank_warning(reg.last_rank, D)
+            # a factorisation that broke down raises (with the rank in the message): NaN weights would poison the next level
+            _check(ctx.h, rc)
             reg.x, reg.last_lambda = X, lam.value                            #    X: the model (for uncentred features)
             nxt = torch.empty_like(cur)                                      # 4) x <- x - (A X) .* 1/norm(x) (:209-215); A is centred now: Xc
             _check(ctx.h, lib.sd_cascade_update(ctx.h, ptr(A), C.c_int64(A.stride(0)), n, D, ptr(Xc), P, ptr(cur), C.byref(norm), ptr(nxt)))

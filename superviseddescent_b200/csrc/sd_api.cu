@@ -255,6 +255,15 @@ int sd_set_solver(sd_ctx* ctx, int mode)
 
 int sd_solver_iterations(const sd_ctx* ctx) { return ctx ? ctx->cg_iterations : 0; }
 
+int sd_set_rank_diagnostic(sd_ctx* ctx, int on)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    ctx->rank_diagnostic = on != 0;
+    return SD_OK;
+}
+
+int sd_last_rank(const sd_ctx* ctx) { return ctx ? ctx->last_rank : -1; }
+
 int sd_solver_timings(sd_ctx* ctx, float ms_out[4])
 {
     if (!ctx || !ms_out) return SD_ERR_INVALID;

@@ -17,7 +17,8 @@
 
 enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_PARTIAL, SD_WS_GEOM, SD_WS_GEMM_PARTIAL, SD_WS_DIAGINV2, SD_WS_PANEL, SD_WS_BIAS, SD_WS_CG, SD_WS_CGMAT,
-       SD_WS_UPLOAD /* B,G,R scratch of sd_upload_frames */, SD_WS_COUNT };
+       SD_WS_UPLOAD /* B,G,R scratch of sd_upload_frames */,
+       SD_WS_RANK /* the rank diagnostic's working copy of the D x D system, its panel and state (sd_rank.cu) */, SD_WS_COUNT };
 
 // Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row
 // Cholesky blocks), and panel p belongs to rank p % nranks.  The Gram exchange delivers each panel's rows to their owner, and
@@ -48,6 +49,8 @@ struct sd_ctx {
     int gram_mode = 0;
     int solver_mode = 0;           // systems with D > 256: 0 = blocked Cholesky, 1 = conjugate gradients (Cholesky if they stall)
     int cg_iterations = 0;         // of the last solve: +n CG converged, -n CG gave up after n (factorisation answered), 0 not tried
+    bool rank_diagnostic = false;  // sd_set_rank_diagnostic: every solve also computes the rank of its regularised system
+    int last_rank = -1;            // of the last solve: the rank, or -1 when it was not computed
     cudaEvent_t cg_ev[8] = {};     // convergence read-backs of the CG loop (the host runs a few iterations ahead of them)
     int64_t roi_fallbacks = 0;     // faces repeated from the full frame because a patch left its ROI
     float timings[4] = {0, 0, 0, 0};
@@ -99,10 +102,15 @@ int sd_syrk_tc(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ
                int passes, bool unbiased, const sd_row_filter* rows);
 // whether the tensor-core kernel can read S (TMA alignment)
 bool sd_syrk_tc_supported(const float* d_S, int64_t lds, int K);
+// the SYRK dispatcher (sd_linalg.cu): the one place that reads the gram mode and picks the tensor-core or the SIMT kernel.
+// big: the size rule's verdict (syrk_is_big) for the product the call belongs to.
+int syrk_upper(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ, float* d_C, int64_t ldc, float alpha, float beta,
+               bool big, bool unbiased, const sd_row_filter* rows = nullptr);
+bool syrk_is_big(int K, int64_t MI, int64_t NJ);
 
 int sd_check_hog_status(sd_ctx* ctx, const char* what);   // sd_api.cu: synchronises, reports and clears the projection's flags
 
-// numerical rank of the symmetric matrix whose upper triangle is in d_G (pivoted Cholesky, sd_rank.cu); rank -1: not computed
+// numerical rank of the symmetric matrix whose upper triangle is in d_G (blocked pivoted Cholesky on a copy, sd_rank.cu)
 int sd_gram_rank(sd_ctx* ctx, const float* d_G, int64_t ldg, int D, int* rank_out, float* first_pivot, float* last_pivot);
 
 // prepared launches of the tensor-core TN-GEMM (sd_gram_tc.cu): plan_storage = SD_TC_PLAN_BYTES bytes, 64-byte aligned

@@ -130,6 +130,8 @@ int syrk_simt(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ,
     return SD_OK;
 }
 
+}  // namespace
+
 // the size rule of the tensor-core SYRK: below it the SIMT kernel is faster
 bool syrk_is_big(int K, int64_t MI, int64_t NJ)
 {
@@ -146,13 +148,15 @@ bool syrk_is_big(int K, int64_t MI, int64_t NJ)
 // rows (optional): the tensor-core route skips the tiles of rows other ranks own.  The SIMT kernel updates every row: rows of
 // other ranks are never read before their owner's broadcast overwrites them.
 int syrk_upper(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ, float* d_C, int64_t ldc, float alpha, float beta,
-               bool big, bool unbiased, const sd_row_filter* rows = nullptr)
+               bool big, bool unbiased, const sd_row_filter* rows)
 {
     if (big && ctx->gram_mode != 2 && sd_syrk_tc_supported(d_S, lds, K))
         return sd_syrk_tc(ctx, d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta, ctx->gram_mode == 1 ? 1 : 3,
                           unbiased || ctx->gram_mode == 3, rows);
     return syrk_simt(ctx, d_S, lds, K, MI, NJ, d_C, ldc, alpha, beta);
 }
+
+namespace {
 
 // =================================================================================================
 // GEMM NN: out[N x M] = A[N x D] * B[D x M], with the cascade-update epilogue
@@ -1466,6 +1470,7 @@ static int solve_gram_impl(sd_ctx* ctx, sd_comm* comm, float* d_G, int64_t ldg, 
     SD_REQUIRE(ctx, reg->type == 0 || reg->type == 1, "unknown regularisation type");
     SD_REQUIRE(ctx, n_train_global >= 1, "n_train_global must be >= 1");
     ctx->cg_iterations = 0;                                           // until CG runs: the small LU and the factorisation
+    ctx->last_rank = -1;
     // the distributed factorisation needs whole panels per rank; small systems were all-reduced and are solved replicated
     const int nranks = sd_comm_size_of(comm);
     const bool dist = route == 1 && nranks > 1 && sd_gram_is_scattered(D, ldg, d_G);
@@ -1513,11 +1518,15 @@ static int solve_gram_impl(sd_ctx* ctx, sd_comm* comm, float* d_G, int64_t ldg, 
     SD_CUDA(ctx, cudaEventRecord(ctx->ev[2], ctx->stream));
     int rc = SD_OK;
     int rank = -1;
-    if (rank_out) {                                                   // ColPivHouseholderQRSolver's diagnostic (regressors.hpp:288-293)
+    // ColPivHouseholderQRSolver's diagnostic (regressors.hpp:288-293), on the matrix as regularised, before any downdate.  With
+    // centred features (d_mu) that matrix is T^T (A^T A + Lambda) T for a unit-triangular T (the bias is not regularised), so
+    // the exact rank is the same.  Route 1 holds only this rank's panels of G: no rank there.
+    if ((rank_out || ctx->rank_diagnostic) && route != 1) {
         rc = sd_gram_rank(ctx, d_G, ldg, D, &rank, nullptr, nullptr);
         if (rc) return rc;
-        *rank_out = rank;
+        ctx->last_rank = rank;
     }
+    if (rank_out) *rank_out = rank;
     if (D <= kLuMaxDim) {
         lu_small_kernel<<<1, 1024, 0, ctx->stream>>>(d_G, ldg, D, M, reinterpret_cast<int*>(ctx->d_scratch));
         SD_LAUNCH_CHECK(ctx, "lu_small_kernel");

@@ -11,6 +11,7 @@
 #include <limits>
 #include <stdexcept>
 #include <string>
+#include <utility>
 
 #include "sd_b200/device.hpp"
 
@@ -82,7 +83,9 @@ using PartialPivLUSolver = B200Solver;          // regressors.hpp:180-235
 
 // regressors.hpp:245-306: the solver that "can check for invertibility".  Same system and solve as above, plus the numerical
 // rank of the regularised AtA from a diagonally pivoted Cholesky on the device (sd_learn_rank_revealing); a deficient rank is
-// reported with the reference's message (regressors.hpp:290-293) and learning continues, as there.
+// reported with the reference's message (regressors.hpp:290-293) and learning continues, as there.  The optimiser's device
+// route learns through sd_learn_centred instead; it asks the library for the rank (sd_set_rank_diagnostic) and hands it over
+// with report_rank().
 class ColPivHouseholderQRSolver {
 public:
     cv::Mat solve(cv::Mat data, cv::Mat labels, Regulariser regulariser)
@@ -95,11 +98,9 @@ public:
         sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, ext.as<float>(), ld * sizeof(float), data.ptr<float>(0), data.step(), sizeof(float) * D, N), "solve");
         sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, ext.as<float>() + D, ld * sizeof(float), labels.ptr<float>(0), labels.step(), sizeof(float) * M, N), "solve");
         const sd_regulariser reg = regulariser.c();
-        last_rank = -1;
-        const int rc = sd_learn_rank_revealing(ctx, ext.as<float>(), ld, ext.as<float>() + D, ld, N, D, M, &reg, dX.as<float>(), &last_lambda, &last_rank);
-        if (last_rank >= 0 && last_rank < D)
-            std::cout << "The regularised AtA is not invertible. We continued learning, but Eigen may return garbage (their docu is not very specific). (The rank is "
-                      << std::to_string(last_rank) << ", full rank would be " << std::to_string(D) << "). Increase lambda." << std::endl;
+        int rank = -1;
+        const int rc = sd_learn_rank_revealing(ctx, ext.as<float>(), ld, ext.as<float>() + D, ld, N, D, M, &reg, dX.as<float>(), &last_lambda, &rank);
+        report_rank(rank, D);
         if (rc == SD_ERR_NUMERIC && last_rank >= 0 && last_rank < D) {
             // the reference would hand back whatever Eigen's inverse of a singular matrix contains; here the factorisation stops
             cv::Mat nan_x(D, M, CV_32FC1);
@@ -110,8 +111,16 @@ public:
         return sd_b200::download(dX.as<float>(), D, M, M);
     }
     void report() const {}
+    // the rank of a system of D unknowns that was learned; a deficient one prints the reference's message
+    void report_rank(int rank, int D)
+    {
+        last_rank = rank;
+        if (rank >= 0 && rank < D)
+            std::cout << "The regularised AtA is not invertible. We continued learning, but Eigen may return garbage (their docu is not very specific). (The rank is "
+                      << std::to_string(rank) << ", full rank would be " << std::to_string(D) << "). Increase lambda." << std::endl;
+    }
     float last_lambda = 0.0f;
-    int last_rank = -1;       // numerical rank of the last system (-1: not computed, D > 4096)
+    int last_rank = -1;       // numerical rank of the last system learned (-1: not computed, the distributed factorisation)
 };
 
 template <class Solver = PartialPivLUSolver>
@@ -163,6 +172,10 @@ public:
     }
     void set_x(cv::Mat new_x) { x = new_x; dirty = true; }
     void report_solver() { solver.report(); }
+    // only for solvers that report a rank (ColPivHouseholderQRSolver): the optimiser's device route calls it after each level
+    template <class S = Solver>
+    auto report_rank(int rank, int D) -> decltype(std::declval<S&>().report_rank(rank, D)) { return solver.report_rank(rank, D); }
+    const Solver& get_solver() const { return solver; }
     const Regulariser& get_regulariser() const { return regulariser; }
 
 private:

@@ -43,6 +43,12 @@ template <class P> struct is_device_projection<P, void_t<decltype(std::declval<P
 template <class N, class = void> struct has_c_normalisation : std::false_type {};
 template <class N> struct has_c_normalisation<N, void_t<decltype(std::declval<const N&>().c_normalisation())>> : std::true_type {};
 
+// regressors whose solver reports the rank of the system (ColPivHouseholderQRSolver)
+template <class R, class = void> struct reports_rank : std::false_type {};
+template <class R> struct reports_rank<R, void_t<decltype(std::declval<R&>().report_rank(0, 0))>> : std::true_type {};
+template <class R> void report_rank(R& r, int rank, int D, std::true_type) { r.report_rank(rank, D); }
+template <class R> void report_rank(R&, int, int, std::false_type) {}
+
 template <class R, class = void> struct is_device_regressor : std::false_type {};
 template <class R> struct is_device_regressor<R, void_t<decltype(std::declval<R&>().device_x()), decltype(std::declval<R&>().get_regulariser())>> : std::true_type {};
 
@@ -234,8 +240,16 @@ private:
             mu.allocate(static_cast<size_t>(D) * sizeof(float));
             sd_comm* c = nranks > 1 ? comm : nullptr;
             sd_b200::check(ctx, sd_centre_features(ctx, c, A.as<float>(), ld, n, D, static_cast<int>(n_global), &reg, mu.as<float>()), "sd_centre_features");
-            sd_b200::check(ctx, sd_learn_centred(ctx, c, A.as<float>(), ld, B, ld, n, D, Pd, &reg, static_cast<int>(n_global), nranks > 1 ? comm_route : 0,
-                                                 mu.as<float>(), X.as<float>(), Xc.as<float>(), nullptr), "sd_learn_centred");
+            const bool want_rank = detail::reports_rank<RegressorType>::value;
+            if (want_rank) sd_b200::check(ctx, sd_set_rank_diagnostic(ctx, 1), "sd_set_rank_diagnostic");
+            const int rc = sd_learn_centred(ctx, c, A.as<float>(), ld, B, ld, n, D, Pd, &reg, static_cast<int>(n_global), nranks > 1 ? comm_route : 0,
+                                            mu.as<float>(), X.as<float>(), Xc.as<float>(), nullptr);
+            if (want_rank) {
+                sd_set_rank_diagnostic(ctx, 0);
+                detail::report_rank(regressors[level], sd_last_rank(ctx), D, detail::reports_rank<RegressorType>());
+            }
+            // a factorisation that broke down throws (with the rank in the message): NaN weights would poison the next level
+            sd_b200::check(ctx, rc, "sd_learn_centred");
             regressors[level].set_x(sd_b200::download(X.as<float>(), D, Pd, Pd));
             regressors[level].report_solver();
             sd_b200::check(ctx, sd_cascade_update(ctx, A.as<float>(), ld, n, D, Xc.as<float>(), Pd, d_cur.as<float>(), &norm, d_next.as<float>()), "sd_cascade_update");   // 4) :209-215
