@@ -335,6 +335,50 @@ SD_API int sd_cascade_update(sd_ctx* ctx, const float* d_A, int64_t lda, int N, 
 SD_API int sd_subtract_templates(sd_ctx* ctx, float* d_A, int64_t lda, const float* d_T, int64_t ldt,
                                  int N, int D);
 
+/* ---- training and testing in chunks: one HogTransform cascade level per call ---------------------------------------------
+ * A level's feature rows [A | b] (ld = roundup4(D + 2L) floats per sample: 68 KB at D = 17,051, 211 KB at D = 52,701) need not
+ * be resident at once: [A^T A | A^T b] is a sum over rows.  The caller owns one buffer of chunk_rows x ld floats; the level runs
+ * through it chunk by chunk.
+ *
+ * sd_level_chunk_rows: the largest r <= N_local such that r rows of the caller's chunk buffer (r * ld * 4 bytes, with the update's
+ * r * M * 8 bytes of partial sums) fit in free_bytes beside everything the level's solve will still allocate with the context's
+ * current settings -- G (D x ld), the rank copy if the diagnostic is on, CG's copy of the system if CG may run (sd_set_solver 1, or
+ * route 2 on several ranks), the band buffer of the exchange on several ranks, the bias / inverse workspaces -- less what the
+ * context already holds, and a reserve of 512 MB for small workspaces.  free_bytes == 0: cudaMemGetInfo.  Returns N_local (at
+ * least 1) when everything fits; SD_ERR_CUDA, with a message naming D, when not even min(N_local, 256) rows fit.  M = 2L.
+ *
+ * sd_train_level: one training level (superviseddescent.hpp:173-217) for the HOG projection (images, d_image_index and hog_eyes as
+ * in sd_hog_batch; sample i reads frame d_image_index ? d_image_index[i] : i).  d_x, d_x_gt: N_local x 2L current / ground-truth
+ * landmarks; norm: the optimiser's normalisation; d_templates: optional N_local x D (row pitch ldt); reg / route / comm as in
+ * sd_learn_centred (comm may be NULL); n_global: the samples of all ranks.  Writes the model d_X (D x 2L, for uncentred features),
+ * the updated landmarks d_x_next (N_local x 2L) and *lambda_out (may be NULL).
+ *   - one chunk (chunk_rows >= N_local): sd_hog_batch, sd_subtract_templates, sd_cascade_targets, sd_centre_features,
+ *     sd_learn_centred and sd_cascade_update (on the centred rows with their weights) -- bit for bit what those calls give.
+ *   - several chunks: chunk 0 is centred by sd_centre_features over every rank's first chunk; its column means p (the pilot
+ *     shift) are subtracted from every later chunk too, and every chunk's [A - 1 p^T | b] is added onto one Gram.  The solve is
+ *     exact for any shift (DESIGN 4.3); p only has to be close enough to the mean to avoid the float32 cancellation.  The update
+ *     projects and shifts every chunk but the last (still resident) again.
+ *   The rank diagnostic (sd_set_rank_diagnostic), solver, gram mode and sd_solver_timings keep their meaning; with several chunks
+ *   "At * A" spans the whole accumulation, the projection of the later chunks included.  For a fixed chunk_rows and rank count
+ *   the result is reproducible bit for bit.  Every rank makes the same collectives whatever its chunk count.
+ *   SD_ERR_INVALID before any work is queued (outputs unwritten): chunk_rows < 1, ld < D + 2L, templates with
+ *   chunk_rows < N_local (a chunked level would check the all-ones bias column on chunk 0 only, and T is as large as the
+ *   features), d_x_next == d_x, null pointers.
+ *
+ * sd_apply_level: one test / predict level (superviseddescent.hpp:262-306, 323-344) in chunks of chunk_rows rows (ld >= D):
+ * HOG rows, optional templates (N x D, pitch ldt), x_next = x - (A X) (.) 1 / norm(x).  With ld a multiple of 4 and a 16-byte
+ * aligned d_chunk each row's result does not depend on the chunking.  Same argument errors as sd_train_level, with ld >= D. */
+SD_API int sd_level_chunk_rows(sd_ctx* ctx, sd_comm* comm, int64_t N_local, int D, int M, int route, size_t free_bytes, int* rows_out);
+SD_API int sd_train_level(sd_ctx* ctx, sd_comm* comm, const sd_image_batch* images, const int32_t* d_image_index,
+                          const float* d_x, const float* d_x_gt, int N_local, int L, int64_t n_global,
+                          const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
+                          const float* d_templates, int64_t ldt, const sd_regulariser* reg, int route,
+                          float* d_chunk, int64_t ld, int chunk_rows, float* d_X, float* d_x_next, float* lambda_out);
+SD_API int sd_apply_level(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int N, int L,
+                          const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
+                          const float* d_templates, int64_t ldt, const float* d_X,
+                          float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next);
+
 /* ---- rcr::detection_model (model.hpp:122-219) -------------------------------------------- */
 /* load_detection_model / save_detection_model (model.hpp:192-219): cereal binary, byte compatible */
 SD_API int sd_model_load(sd_ctx* ctx, const char* path, sd_model** out);

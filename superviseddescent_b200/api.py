@@ -459,6 +459,7 @@ class SupervisedDescentOptimiser:
         self.regressors = list(regressors)
         self.normalisation_strategy = normalisation or NoNormalisation()
         self.ctx = ctx
+        self.chunk_rows: List[int] = []   # feature rows per chunk of each level of the last train() with a HogTransform
 
     def _ctx(self) -> Context:
         if self.ctx is None:
@@ -492,14 +493,29 @@ class SupervisedDescentOptimiser:
         host[:, :D] = np.stack(rows)
         return _dev(host, ctx), D
 
+    def _chunk_rows(self, rows_per_chunk, n: int, D: int, P: int, comm_h, route: int) -> int:
+        """Rows per chunk of a HogTransform level: rows_per_chunk (at most n), or -- None / 0 -- the most that fit beside the
+        solve (sd_level_chunk_rows; memory torch has reserved but not handed out counts as free, so a warm caching allocator
+        does not split a level that fits)."""
+        if rows_per_chunk:
+            return max(1, min(int(rows_per_chunk), n))
+        ctx = self._ctx()
+        free = torch.cuda.mem_get_info(ctx.device)[0] + torch.cuda.memory_reserved(ctx.device) - torch.cuda.memory_allocated(ctx.device)
+        rows = C.c_int(0)
+        _check(ctx.h, _capi.lib().sd_level_chunk_rows(ctx.h, comm_h, C.c_int64(n), D, P, route, C.c_size_t(free), C.byref(rows)))
+        return rows.value
+
     def train(self, parameters, initialisations, templates, projection, on_training_epoch_callback=None, group=None, comm=None,
-              distributed_solve=None):
+              distributed_solve=None, rows_per_chunk=None):
         """superviseddescent.hpp:165-219.  Multi-GPU: pass `comm` (a parallel.Communicator) or a torch.distributed `group`
         (a communicator is then made from it) -- each rank passes its own shard of rows; per level the C ABI does ONE exchange of
         [AtA | Atb] and the solve (SURVEY 8e).  distributed_solve: None = by size (shared CG below parallel.DIST_SOLVE_MIN_D features,
         the distributed factorisation from there), True = reduce-scatter +
         distributed blocked Cholesky, False = all-reduce + replicated solve, "cg" = all-reduce + conjugate gradients shared by the
-        ranks."""
+        ranks.
+        A HogTransform projection trains each level with sd_train_level, through a buffer of rows_per_chunk feature rows (None:
+        as many as fit on the device, which is all of them whenever the level fits -- then the result is that of one pass over
+        all rows).  Templates need the whole level in one chunk."""
         from . import parallel
         ctx = self._ctx()
         lib = _capi.lib()
@@ -512,31 +528,53 @@ class SupervisedDescentOptimiser:
             comm, own_comm = parallel.Communicator(ctx, group), True
         distributed = comm is not None and comm.size > 1
         n_global = comm.sum_int(n) if distributed else n
+        hog = isinstance(projection, HogTransform)
+        self.chunk_rows = []                                                 # rows per chunk of each HogTransform level
+
+        def route(D):
+            if not distributed:
+                return 0
+            if distributed_solve is None:
+                return 1 if D >= parallel.DIST_SOLVE_MIN_D else 2          # big systems: distributed factorisation; else shared CG
+            return 2 if distributed_solve == "cg" else int(bool(distributed_solve))
+
+        ch = comm.h if distributed else None
         for level, reg in enumerate(self.regressors):
             norm = self.normalisation_strategy.c(P // 2)
-            A, D = self._project(projection, cur, level, extra=P)             # 1) features (:173-189)
-            if tmpl is not None:                                             #    observed = features - templates (:191-197)
-                _check(ctx.h, lib.sd_subtract_templates(ctx.h, ptr(A), C.c_int64(A.stride(0)), ptr(tmpl), C.c_int64(tmpl.stride(0)), n, D))
-            Bv = A[:, D:D + P]                                               # 2) b = (x - x_gt) .* norm(x)  (:199-205)
-            _check(ctx.h, lib.sd_cascade_targets(ctx.h, ptr(cur), ptr(x_gt), n, P, C.byref(norm), ptr(Bv), C.c_int64(A.stride(0))))
-            X = torch.empty((D, P), dtype=torch.float32, device=cur.device)  # 3) learn (:207), on centred rows (sd_centre_features)
-            Xc = torch.empty((D, P), dtype=torch.float32, device=cur.device)
-            mu = torch.empty(D, dtype=torch.float32, device=cur.device)
             lam = C.c_float(0)
             rc_ = reg.regulariser.c()
-            ds = 0
-            if distributed:
-                if distributed_solve is None:
-                    ds = 1 if D >= parallel.DIST_SOLVE_MIN_D else 2     # big systems: distributed factorisation; else shared CG
-                else:
-                    ds = 2 if distributed_solve == "cg" else int(bool(distributed_solve))
-            ch = comm.h if distributed else None
-            _check(ctx.h, lib.sd_centre_features(ctx.h, ch, ptr(A), C.c_int64(A.stride(0)), n, D, n_global, C.byref(rc_), ptr(mu)))
             qr = getattr(reg.solver, "rank_revealing", False)                # ColPivHouseholderQRSolver: rank of this level's system
             if qr:
-                ctx.set_rank_diagnostic(True)
-            rc = lib.sd_learn_centred(ctx.h, ch, ptr(A), C.c_int64(A.stride(0)), ptr(Bv), C.c_int64(A.stride(0)), n, D, P,
-                                      C.byref(rc_), n_global, int(ds), ptr(mu), ptr(X), ptr(Xc), C.byref(lam))
+                ctx.set_rank_diagnostic(True)                                # before the chunk query: the rank copy counts there
+            nxt = torch.empty_like(cur)
+            if hog:                                                          # 1)-4) through a buffer of `rows` feature rows
+                D = projection.feature_length(level)
+                X = torch.empty((D, P), dtype=torch.float32, device=cur.device)
+                ld = (D + P + 3) // 4 * 4
+                rows = max(n, 1) if tmpl is not None else self._chunk_rows(rows_per_chunk, n, D, P, ch, route(D))
+                self.chunk_rows.append(rows)
+                buf = torch.empty((rows, ld), dtype=torch.float32, device=cur.device)
+                eyes = projection.norm.c()
+                rc = lib.sd_train_level(ctx.h, ch, C.byref(projection.batch()), None, ptr(cur), ptr(x_gt), n, P // 2, C.c_int64(n_global),
+                                        C.byref(eyes), C.byref(projection.hog_params[level]), C.byref(norm), ptr(tmpl),
+                                        C.c_int64(tmpl.stride(0) if tmpl is not None else 0), C.byref(rc_), route(D), ptr(buf),
+                                        C.c_int64(ld), rows, ptr(X), ptr(nxt), C.byref(lam))
+                del buf
+            else:
+                A, D = self._project(projection, cur, level, extra=P)         # 1) features (:173-189)
+                if tmpl is not None:                                         #    observed = features - templates (:191-197)
+                    _check(ctx.h, lib.sd_subtract_templates(ctx.h, ptr(A), C.c_int64(A.stride(0)), ptr(tmpl), C.c_int64(tmpl.stride(0)), n, D))
+                Bv = A[:, D:D + P]                                           # 2) b = (x - x_gt) .* norm(x)  (:199-205)
+                _check(ctx.h, lib.sd_cascade_targets(ctx.h, ptr(cur), ptr(x_gt), n, P, C.byref(norm), ptr(Bv), C.c_int64(A.stride(0))))
+                X = torch.empty((D, P), dtype=torch.float32, device=cur.device)  # 3) learn (:207), on centred rows (sd_centre_features)
+                Xc = torch.empty((D, P), dtype=torch.float32, device=cur.device)
+                mu = torch.empty(D, dtype=torch.float32, device=cur.device)
+                _check(ctx.h, lib.sd_centre_features(ctx.h, ch, ptr(A), C.c_int64(A.stride(0)), n, D, n_global, C.byref(rc_), ptr(mu)))
+                rc = lib.sd_learn_centred(ctx.h, ch, ptr(A), C.c_int64(A.stride(0)), ptr(Bv), C.c_int64(A.stride(0)), n, D, P,
+                                          C.byref(rc_), n_global, route(D), ptr(mu), ptr(X), ptr(Xc), C.byref(lam))
+                if rc == 0:                                                  # 4) x <- x - (A X) .* 1/norm(x) (:209-215); A is centred now: Xc
+                    rc = lib.sd_cascade_update(ctx.h, ptr(A), C.c_int64(A.stride(0)), n, D, ptr(Xc), P, ptr(cur), C.byref(norm), ptr(nxt))
+                del A, Bv
             if qr:
                 ctx.set_rank_diagnostic(False)
                 reg.last_rank = ctx.last_rank()
@@ -545,10 +583,7 @@ class SupervisedDescentOptimiser:
             # a factorisation that broke down raises (with the rank in the message): NaN weights would poison the next level
             _check(ctx.h, rc)
             reg.x, reg.last_lambda = X, lam.value                            #    X: the model (for uncentred features)
-            nxt = torch.empty_like(cur)                                      # 4) x <- x - (A X) .* 1/norm(x) (:209-215); A is centred now: Xc
-            _check(ctx.h, lib.sd_cascade_update(ctx.h, ptr(A), C.c_int64(A.stride(0)), n, D, ptr(Xc), P, ptr(cur), C.byref(norm), ptr(nxt)))
             cur = nxt
-            del A, Bv
             if on_training_epoch_callback is not None:                       # 5) callback (:217)
                 on_training_epoch_callback(comm.allgather_rows(cur) if distributed else cur)
         ctx.sync()                                                           # surfaces flags raised by the projection kernels
@@ -556,8 +591,9 @@ class SupervisedDescentOptimiser:
             comm.close()
         return cur
 
-    def test(self, initialisations, templates, projection, on_regressor_iteration_callback=None):
-        """superviseddescent.hpp:262-306."""
+    def test(self, initialisations, templates, projection, on_regressor_iteration_callback=None, rows_per_chunk=None):
+        """superviseddescent.hpp:262-306.  A HogTransform projection runs each level with sd_apply_level through a buffer of
+        rows_per_chunk feature rows (None: as many as fit, as in train())."""
         ctx = self._ctx()
         lib = _capi.lib()
         cur = _dev(initialisations, ctx).clone()
@@ -567,19 +603,31 @@ class SupervisedDescentOptimiser:
         tmpl = _dev(templates, ctx) if templates is not None and np.size(templates) > 0 else None
         for level, reg in enumerate(self.regressors):
             norm = self.normalisation_strategy.c(P // 2)
-            A, D = self._project(projection, cur, level, extra=0)
-            if tmpl is not None:
-                _check(ctx.h, lib.sd_subtract_templates(ctx.h, ptr(A), C.c_int64(A.stride(0)), ptr(tmpl), C.c_int64(tmpl.stride(0)), n, D))
             nxt = torch.empty_like(cur)
-            _check(ctx.h, lib.sd_cascade_update(ctx.h, ptr(A), C.c_int64(A.stride(0)), n, D, ptr(reg.x), P, ptr(cur), C.byref(norm), ptr(nxt)))
+            if isinstance(projection, HogTransform):
+                D = projection.feature_length(level)
+                ld = (D + 3) // 4 * 4
+                rows = self._chunk_rows(rows_per_chunk, n, D, P, None, 0)
+                buf = torch.empty((rows, ld), dtype=torch.float32, device=cur.device)
+                eyes = projection.norm.c()
+                _check(ctx.h, lib.sd_apply_level(ctx.h, C.byref(projection.batch()), None, ptr(cur), n, P // 2, C.byref(eyes),
+                                                 C.byref(projection.hog_params[level]), C.byref(norm), ptr(tmpl),
+                                                 C.c_int64(tmpl.stride(0) if tmpl is not None else 0), ptr(reg.x), ptr(buf), C.c_int64(ld),
+                                                 rows, ptr(nxt)))
+                del buf
+            else:
+                A, D = self._project(projection, cur, level, extra=0)
+                if tmpl is not None:
+                    _check(ctx.h, lib.sd_subtract_templates(ctx.h, ptr(A), C.c_int64(A.stride(0)), ptr(tmpl), C.c_int64(tmpl.stride(0)), n, D))
+                _check(ctx.h, lib.sd_cascade_update(ctx.h, ptr(A), C.c_int64(A.stride(0)), n, D, ptr(reg.x), P, ptr(cur), C.byref(norm), ptr(nxt)))
             cur = nxt
             if on_regressor_iteration_callback is not None:
                 on_regressor_iteration_callback(cur)
         return cur
 
-    def predict(self, initialisations, templates, projection):
+    def predict(self, initialisations, templates, projection, rows_per_chunk=None):
         """superviseddescent.hpp:323-344 (same arithmetic as test(), no callback)."""
-        return self.test(initialisations, templates, projection)
+        return self.test(initialisations, templates, projection, rows_per_chunk=rows_per_chunk)
 
 
 # ------------------------------------------------------------------------------------------------

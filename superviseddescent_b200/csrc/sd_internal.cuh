@@ -18,7 +18,8 @@
 enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_PARTIAL, SD_WS_GEOM, SD_WS_GEMM_PARTIAL, SD_WS_DIAGINV2, SD_WS_PANEL, SD_WS_BIAS, SD_WS_CG, SD_WS_CGMAT,
        SD_WS_UPLOAD /* B,G,R scratch of sd_upload_frames */,
-       SD_WS_RANK /* the rank diagnostic's working copy of the D x D system, its panel and state (sd_rank.cu) */, SD_WS_COUNT };
+       SD_WS_RANK /* the rank diagnostic's working copy of the D x D system, its panel and state (sd_rank.cu) */,
+       SD_WS_LEVEL /* column shift and shifted-row weights of sd_train_level (sd_train.cu) */, SD_WS_COUNT };
 
 // Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row
 // Cholesky blocks), and panel p belongs to rank p % nranks.  The Gram exchange delivers each panel's rows to their owner, and
@@ -109,6 +110,19 @@ int syrk_upper(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ
 bool syrk_is_big(int K, int64_t MI, int64_t NJ);
 
 int sd_check_hog_status(sd_ctx* ctx, const char* what);   // sd_api.cu: synchronises, reports and clears the projection's flags
+
+// The learn path of sd_learn_centred in two steps (sd_linalg.cu), so that a training level can add its rows chunk by chunk
+// (sd_train.cu).  The Gram lives in the context's workspace (D x sd_learn_ldg floats).
+inline int64_t sd_learn_ldg(int D, int M) { return ((int64_t)(D + M) + 3) / 4 * 4; }
+// [A^T A | A^T B] of N rows: started (accumulate == false; records the start of "At * A") or added onto (accumulate == true)
+int sd_learn_gram(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_B, int64_t ldb, int N, bool shard, int D, int M,
+                  bool accumulate);
+// exchange over the ranks and solve with the column shift d_mu, as sd_learn_centred does after its Gram
+int sd_learn_centred_solve(sd_ctx* ctx, sd_comm* comm, int D, int M, const sd_regulariser* reg, int n_train_global, int route,
+                           const float* d_mu, float* d_X, float* d_Xc, float* lambda_out);
+// d_A[:, c] -= d_mu[c] for c < D - 1 on N rows (the centring pass of sd_centre_features)
+int sd_shift_rows(sd_ctx* ctx, float* d_A, int64_t lda, int N, int D, const float* d_mu);
+constexpr int SD_LU_MAX_DIM = 256;   // systems up to this D keep the reference-order LU on uncentred rows
 
 // numerical rank of the symmetric matrix whose upper triangle is in d_G (blocked pivoted Cholesky on a copy, sd_rank.cu)
 int sd_gram_rank(sd_ctx* ctx, const float* d_G, int64_t ldg, int D, int* rank_out, float* first_pivot, float* last_pivot);

@@ -21,7 +21,7 @@
 
 namespace {
 
-constexpr int kLuMaxDim = 256;   // D up to which the faithful partial-pivot LU is used
+constexpr int kLuMaxDim = SD_LU_MAX_DIM;   // D up to which the faithful partial-pivot LU is used
 constexpr int kCholNb = 128;     // Cholesky block size
 
 // =================================================================================================
@@ -1430,15 +1430,9 @@ int check_status(sd_ctx* ctx, const char* what)
     return SD_OK;
 }
 
-}  // namespace
-
-// =================================================================================================
-// C ABI
-// =================================================================================================
-extern "C" {
-
-int sd_gram(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_B, int64_t ldb, int N, int D, int M,
-            float* d_G, int64_t ldg)
+// [A^T A | A^T B] of N rows written to d_G (beta 0), or added onto it (beta 1: the chunks of a training level, sd_train.cu)
+int gram_impl(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_B, int64_t ldb, int N, int D, int M,
+              float* d_G, int64_t ldg, float beta)
 {
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, d_A && d_G && N >= 1 && D >= 1 && M >= 0, "bad argument");
@@ -1455,7 +1449,20 @@ int sd_gram(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_B, int64_
         SD_LAUNCH_CHECK(ctx, "pack_ext_kernel");
         S = E;
     }
-    return syrk_upper(ctx, S, lds, N, D, D + M, d_G, ldg, 1.0f, 0.0f, syrk_is_big(N, D, D + M), false);
+    return syrk_upper(ctx, S, lds, N, D, D + M, d_G, ldg, 1.0f, beta, syrk_is_big(N, D, D + M), false);
+}
+
+}  // namespace
+
+// =================================================================================================
+// C ABI
+// =================================================================================================
+extern "C" {
+
+int sd_gram(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_B, int64_t ldb, int N, int D, int M,
+            float* d_G, int64_t ldg)
+{
+    return gram_impl(ctx, d_A, lda, d_B, ldb, N, D, M, d_G, ldg, 0.0f);
 }
 
 // route: 0 = every rank holds the summed G (one GPU, or after sd_allreduce_gram) and solves it alone;
@@ -1595,27 +1602,73 @@ static int solve_gram_impl(sd_ctx* ctx, sd_comm* comm, float* d_G, int64_t ldg, 
     return rc;
 }
 
-// LinearRegressor::learn on this rank's rows: [A^T A | A^T B] into the workspace (ev[0] starts "At * A"), summed over the ranks
-// when there is more than one (route 1: each panel to its owner, otherwise to every rank), then solved.  shard: the rows are this
-// rank's share of the samples and may be none (G is zero then); otherwise sd_gram checks N.
-static int learn_impl(sd_ctx* ctx, sd_comm* comm, const float* d_A, int64_t lda, const float* d_B, int64_t ldb, int N, bool shard,
-                      int D, int M, const sd_regulariser* reg, int n_train_global, float* d_X, float* lambda_out, int* rank_out,
-                      int route, const float* d_mu = nullptr, float* d_Xc = nullptr)
+}  // extern "C"
+
+// The learn path's Gram [A^T A | A^T B] of this rank's rows, in the workspace.  accumulate == false starts it (ev[0] starts
+// "At * A"); accumulate == true adds more rows onto it (the later chunks of a training level).  shard: the rows are this rank's
+// share of the samples and may be none (G is zero then); otherwise sd_gram checks N.
+int sd_learn_gram(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_B, int64_t ldb, int N, bool shard, int D, int M,
+                  bool accumulate)
 {
-    const int64_t ldg = ((int64_t)(D + M) + 3) / 4 * 4;
+    const int64_t ldg = sd_learn_ldg(D, M);
     float* G = (float*)sd_workspace(ctx, SD_WS_SCRATCH, (size_t)D * ldg * sizeof(float));
     if (!G) return SD_ERR_CUDA;
-    SD_CUDA(ctx, cudaEventRecord(ctx->ev[0], ctx->stream));
-    int rc;
-    if (N > 0 || !shard) rc = sd_gram(ctx, d_A, lda, d_B, ldb, N, D, M, G, ldg);
-    else rc = sd_check_cuda(ctx, cudaMemsetAsync(G, 0, (size_t)D * ldg * sizeof(float), ctx->stream), "memset(G)");
-    if (rc) return rc;
+    if (!accumulate) SD_CUDA(ctx, cudaEventRecord(ctx->ev[0], ctx->stream));
+    if (N > 0 || !shard) return gram_impl(ctx, d_A, lda, d_B, ldb, N, D, M, G, ldg, accumulate ? 1.0f : 0.0f);
+    if (accumulate) return SD_OK;
+    return sd_check_cuda(ctx, cudaMemsetAsync(G, 0, (size_t)D * ldg * sizeof(float), ctx->stream), "memset(G)");
+}
+
+// The rest of LinearRegressor::learn on the Gram sd_learn_gram left: summed over the ranks when there is more than one (route 1:
+// each panel to its owner, otherwise to every rank), then solved.
+static int learn_solve(sd_ctx* ctx, sd_comm* comm, int D, int M, const sd_regulariser* reg, int n_train_global, float* d_X,
+                       float* lambda_out, int* rank_out, int route, const float* d_mu = nullptr, float* d_Xc = nullptr)
+{
+    const int64_t ldg = sd_learn_ldg(D, M);
+    float* G = (float*)sd_workspace(ctx, SD_WS_SCRATCH, (size_t)D * ldg * sizeof(float));
+    if (!G) return SD_ERR_CUDA;
     if (sd_comm_size_of(comm) > 1) {
-        rc = route == 1 ? sd_reduce_scatter_gram(ctx, comm, G, ldg, D, M) : sd_allreduce_gram(ctx, comm, G, ldg, D, M);
+        const int rc = route == 1 ? sd_reduce_scatter_gram(ctx, comm, G, ldg, D, M) : sd_allreduce_gram(ctx, comm, G, ldg, D, M);
         if (rc) return rc;
     }
     return solve_gram_impl(ctx, comm, G, ldg, D, M, reg, n_train_global, d_X, lambda_out, rank_out, route, d_mu, d_Xc);
 }
+
+// LinearRegressor::learn on this rank's rows: Gram, exchange, solve
+static int learn_impl(sd_ctx* ctx, sd_comm* comm, const float* d_A, int64_t lda, const float* d_B, int64_t ldb, int N, bool shard,
+                      int D, int M, const sd_regulariser* reg, int n_train_global, float* d_X, float* lambda_out, int* rank_out,
+                      int route)
+{
+    const int rc = sd_learn_gram(ctx, d_A, lda, d_B, ldb, N, shard, D, M, false);
+    if (rc) return rc;
+    return learn_solve(ctx, comm, D, M, reg, n_train_global, d_X, lambda_out, rank_out, route);
+}
+
+// sd_learn_centred after its Gram: exchange and solve with the shift d_mu (D > 256 only: sd_centre_features leaves the small
+// systems alone); d_Xc receives the weights for the shifted rows
+int sd_learn_centred_solve(sd_ctx* ctx, sd_comm* comm, int D, int M, const sd_regulariser* reg, int n_train_global, int route,
+                           const float* d_mu, float* d_X, float* d_Xc, float* lambda_out)
+{
+    const bool multi = sd_comm_size_of(comm) > 1;
+    const float* mu = D > kLuMaxDim ? d_mu : nullptr;
+    int rc = learn_solve(ctx, multi ? comm : nullptr, D, M, reg, n_train_global, d_X, lambda_out, nullptr, multi ? route : 0, mu, d_Xc);
+    if (rc) return rc;
+    if (!mu && d_Xc && d_Xc != d_X) SD_CUDA(ctx, cudaMemcpyAsync(d_Xc, d_X, (size_t)D * M * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+    return SD_OK;
+}
+
+// A[:, c] -= mu[c] for the feature columns of N rows (the bias column stays all ones)
+int sd_shift_rows(sd_ctx* ctx, float* d_A, int64_t lda, int N, int D, const float* d_mu)
+{
+    if (N <= 0) return SD_OK;
+    const long long total = (long long)N * (D - 1);
+    const int blocks = (int)(sd_div_up(total, 256) < 32LL * ctx->sm_count ? sd_div_up(total, 256) : 32LL * ctx->sm_count);
+    centre_kernel<<<blocks, 256, 0, ctx->stream>>>(d_A, lda, N, D, d_mu);
+    SD_LAUNCH_CHECK(ctx, "centre_kernel");
+    return SD_OK;
+}
+
+extern "C" {
 
 int sd_solve_gram(sd_ctx* ctx, float* d_G, int64_t ldg, int D, int M, const sd_regulariser* reg, int n_train_global,
                   float* d_X, float* lambda_out)
@@ -1668,13 +1721,7 @@ int sd_centre_features(sd_ctx* ctx, sd_comm* comm, float* d_A, int64_t lda, int 
     if (rc) return rc;
     colmean_kernel<<<sd_div_up(D, 256), 256, 0, ctx->stream>>>(part, D, n_global, 1, d_mu);
     SD_LAUNCH_CHECK(ctx, "colmean_kernel");
-    if (N_local > 0) {
-        const long long total = (long long)N_local * (D - 1);
-        const int blocks = (int)(sd_div_up(total, 256) < 32LL * ctx->sm_count ? sd_div_up(total, 256) : 32LL * ctx->sm_count);
-        centre_kernel<<<blocks, 256, 0, ctx->stream>>>(d_A, lda, N_local, D, d_mu);
-        SD_LAUNCH_CHECK(ctx, "centre_kernel");
-    }
-    return SD_OK;
+    return sd_shift_rows(ctx, d_A, lda, N_local, D, d_mu);
 }
 
 int sd_learn_centred(sd_ctx* ctx, sd_comm* comm, const float* d_Ac, int64_t lda, const float* d_B, int64_t ldb, int N_local, int D, int M,
@@ -1682,13 +1729,9 @@ int sd_learn_centred(sd_ctx* ctx, sd_comm* comm, const float* d_Ac, int64_t lda,
 {
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, M >= 1 && N_local >= 0 && d_mu && d_X, "bad argument");
-    const bool multi = sd_comm_size_of(comm) > 1;
-    const float* mu = D > kLuMaxDim ? d_mu : nullptr;       // sd_centre_features leaves the small systems alone
-    int rc = learn_impl(ctx, multi ? comm : nullptr, d_Ac, lda, d_B, ldb, N_local, true, D, M, reg, n_train_global, d_X, lambda_out,
-                        nullptr, multi ? route : 0, mu, d_Xc);
+    const int rc = sd_learn_gram(ctx, d_Ac, lda, d_B, ldb, N_local, true, D, M, false);
     if (rc) return rc;
-    if (!mu && d_Xc && d_Xc != d_X) SD_CUDA(ctx, cudaMemcpyAsync(d_Xc, d_X, (size_t)D * M * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
-    return SD_OK;
+    return sd_learn_centred_solve(ctx, comm, D, M, reg, n_train_global, route, d_mu, d_X, d_Xc, lambda_out);
 }
 
 int sd_learn_rank_revealing(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_B, int64_t ldb, int N, int D, int M,

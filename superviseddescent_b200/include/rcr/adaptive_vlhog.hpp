@@ -1,9 +1,9 @@
 // H100 drop-in for include/rcr/adaptive_vlhog.hpp: HoGParam (:41-60) and the projection functor
 // HogTransform (:70-195).  The functor keeps the reference's constructor and call signature
 //     cv::Mat operator()(cv::Mat parameters, size_t regressorLevel, int trainingIndex = 0)
-// (one sample, used by predict(), superviseddescent.hpp:332) and adds project_device(), which the
-// optimiser uses to extract the features of ALL samples of a level with one kernel launch.  The images are
-// uploaded to HBM once, on first use; crop / resize / HOG run in sd_hog_batch (sm_90a).
+// (one sample, used by predict(), superviseddescent.hpp:332) and exposes its device images, eyes and per-level
+// HOG parameters, with which the optimiser projects ALL samples of a level on the device (sd_train_level,
+// sd_apply_level).  The images are uploaded to HBM once, on first use; crop / resize / HOG run in sd_hog_batch (sm_90a).
 #pragma once
 
 #include <memory>
@@ -54,12 +54,14 @@ public:
         return sd_b200::download(dA.as<float>(), 1, D, D);
     }
 
-    // Features of samples 0..n-1 (sample i reads image i), straight into a device matrix with row stride ld.
-    void project_device(const float* d_x, int64_t ldx, int n, size_t level, float* d_A, int64_t ld)
+    // What the optimiser's device route hands to sd_train_level / sd_apply_level: the images resident on the device (uploaded
+    // on first use; sample i reads image i), the eye landmarks (eyes()) and the HOG parameters of a level.
+    const sd_image_batch& device_batch()
     {
         ensure_uploaded();
-        launch(d_x, ldx, n, level, d_A, ld, nullptr);
+        return dev->batch;
     }
+    sd_hog_param hog_param(size_t level) const { return hog_params[level].c(); }
 
     sd_normalisation eyes() const
     {

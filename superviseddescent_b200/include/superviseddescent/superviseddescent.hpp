@@ -5,8 +5,9 @@
 //
 //   device route   RegressorType is this package's LinearRegressor<>, the projection is a device
 //                  projection (rcr::HogTransform) and the normalisation maps to sd_normalisation:
-//                  features, targets, Gram, solve and update all stay in HBM (sd_hog_batch ->
-//                  sd_cascade_targets -> sd_gram -> sd_solve_gram -> sd_cascade_update).
+//                  features, targets, Gram, solve and update all stay in HBM, one sd_train_level /
+//                  sd_apply_level call per level through a buffer of feature rows that holds the whole
+//                  level when it fits, and chunks of it otherwise (set_rows_per_chunk).
 //   functor route  any other projection functor h(row, level, idx) -> Mat | float is USER host code; it is
 //                  evaluated on a pool of host threads exactly as the reference does (:173-189) and the
 //                  stacked feature matrix goes through RegressorType::learn / predict (which are GPU calls
@@ -36,9 +37,9 @@ namespace detail {
 template <class...> struct voider { using type = void; };
 template <class... T> using void_t = typename voider<T...>::type;
 
-// projection that can fill a device matrix for all rows at once (rcr::HogTransform)
+// projection whose images are resident on the device, projected there for all rows at once (rcr::HogTransform)
 template <class P, class = void> struct is_device_projection : std::false_type {};
-template <class P> struct is_device_projection<P, void_t<decltype(std::declval<P&>().project_device(static_cast<const float*>(nullptr), int64_t(0), 0, size_t(0), static_cast<float*>(nullptr), int64_t(0)))>> : std::true_type {};
+template <class P> struct is_device_projection<P, void_t<decltype(std::declval<P&>().device_batch()), decltype(std::declval<P&>().hog_param(size_t(0)))>> : std::true_type {};
 
 template <class N, class = void> struct has_c_normalisation : std::false_type {};
 template <class N> struct has_c_normalisation<N, void_t<decltype(std::declval<const N&>().c_normalisation())>> : std::true_type {};
@@ -152,10 +153,15 @@ public:
     std::vector<RegressorType>& get_regressors() { return regressors; }
     NormalisationStrategy& get_normalisation() { return normalisation_strategy; }
 
+    // Device route: feature rows per chunk of a level in train() / test() / predict().  0 (the default): as many as fit on the
+    // device beside the solve (sd_level_chunk_rows) -- the whole level whenever it fits.  Templates always take one chunk.
+    void set_rows_per_chunk(int rows) { rows_per_chunk = rows < 0 ? 0 : rows; }
+
 private:
     std::vector<RegressorType> regressors;
     NormalisationStrategy normalisation_strategy;
     bool want_callback = true;
+    int rows_per_chunk = 0;
 
     // ------------------------------------------------------------------ functor route (host projection)
     template <class P, class CB>
@@ -207,6 +213,15 @@ private:
     sd_comm* comm = nullptr;     // set for the duration of a multi-GPU train()
     int comm_route = 0;
 
+    // feature rows per chunk of a device-route level: set_rows_per_chunk's (at most n), or as many as fit
+    int chunk_rows(sd_ctx* ctx, sd_comm* c, int n, int D, int Pd, int route) const
+    {
+        if (rows_per_chunk > 0) return rows_per_chunk < n ? rows_per_chunk : (n > 0 ? n : 1);
+        int rows = 0;
+        sd_b200::check(ctx, sd_level_chunk_rows(ctx, c, n, D, Pd, route, 0, &rows), "sd_level_chunk_rows");
+        return rows;
+    }
+
     // ------------------------------------------------------------------ device route
     template <class P, class CB>
     void train_impl(cv::Mat parameters, cv::Mat initialisations, cv::Mat templates, P projection, CB cb, std::true_type)
@@ -217,42 +232,37 @@ private:
         sd_b200::upload(parameters, d_gt, Pd);
         sd_b200::upload(initialisations, d_cur, Pd);
         const sd_normalisation norm = normalisation_strategy.c_normalisation();
-        sd_b200::DeviceBuffer A, G, X, Xc, mu;
+        const sd_normalisation eyes = projection.eyes();
+        const sd_image_batch& images = projection.device_batch();
+        if (!templates.empty()) sd_b200::upload(templates, d_tmpl, templates.cols);
+        sd_b200::DeviceBuffer X;
         int64_t n_global = n;
         const int nranks = comm ? sd_comm_size(comm) : 1;
         if (nranks > 1) sd_b200::check(ctx, sd_comm_sum_int64(ctx, comm, &n_global), "sd_comm_sum_int64");
+        sd_comm* c = nranks > 1 ? comm : nullptr;
+        const int route = nranks > 1 ? comm_route : 0;
         for (size_t level = 0; level < regressors.size(); ++level) {
             const int D = projection.feature_length(level);
             const int64_t ld = (static_cast<int64_t>(D) + Pd + 3) / 4 * 4;
-            A.allocate(static_cast<size_t>(n) * ld * sizeof(float));
-            projection.project_device(d_cur.as<float>(), Pd, n, level, A.as<float>(), ld);                    // 1) :173-189
-            if (!templates.empty()) {
-                sd_b200::upload(templates, d_tmpl, templates.cols);
-                sd_b200::check(ctx, sd_subtract_templates(ctx, A.as<float>(), ld, d_tmpl.as<float>(), templates.cols, n, D), "sd_subtract_templates");
-            }
-            float* B = A.as<float>() + D;                                                                    // 2) :199-205
-            sd_b200::check(ctx, sd_cascade_targets(ctx, d_cur.as<float>(), d_gt.as<float>(), n, Pd, &norm, B, ld), "sd_cascade_targets");
-            X.allocate(static_cast<size_t>(D) * Pd * sizeof(float));                                          // 3) :207
+            const sd_hog_param hp = projection.hog_param(level);
             const sd_regulariser reg = regressors[level].get_regulariser().c();
-            // learn on centred rows (sd_centre_features: column means over all ranks, subtracted in place; no-op for D <= 256);
-            // X is the model, Xc the weights that go with the centred buffer
-            Xc.allocate(static_cast<size_t>(D) * Pd * sizeof(float));
-            mu.allocate(static_cast<size_t>(D) * sizeof(float));
-            sd_comm* c = nranks > 1 ? comm : nullptr;
-            sd_b200::check(ctx, sd_centre_features(ctx, c, A.as<float>(), ld, n, D, static_cast<int>(n_global), &reg, mu.as<float>()), "sd_centre_features");
             const bool want_rank = detail::reports_rank<RegressorType>::value;
-            if (want_rank) sd_b200::check(ctx, sd_set_rank_diagnostic(ctx, 1), "sd_set_rank_diagnostic");
-            const int rc = sd_learn_centred(ctx, c, A.as<float>(), ld, B, ld, n, D, Pd, &reg, static_cast<int>(n_global), nranks > 1 ? comm_route : 0,
-                                            mu.as<float>(), X.as<float>(), Xc.as<float>(), nullptr);
+            if (want_rank) sd_b200::check(ctx, sd_set_rank_diagnostic(ctx, 1), "sd_set_rank_diagnostic");   // counted by the chunk query
+            // 1)-4) :173-215 -- features, targets, Gram, exchange, solve and update through a buffer of `rows` feature rows
+            const int rows = templates.empty() ? chunk_rows(ctx, c, n, D, Pd, route) : (n > 0 ? n : 1);
+            sd_b200::DeviceBuffer chunk(static_cast<size_t>(rows) * ld * sizeof(float));
+            X.allocate(static_cast<size_t>(D) * Pd * sizeof(float));
+            const int rc = sd_train_level(ctx, c, &images, nullptr, d_cur.as<float>(), d_gt.as<float>(), n, Pd / 2, n_global, &eyes, &hp, &norm,
+                                          templates.empty() ? nullptr : d_tmpl.as<float>(), templates.cols, &reg, route, chunk.as<float>(), ld,
+                                          rows, X.as<float>(), d_next.as<float>(), nullptr);
             if (want_rank) {
                 sd_set_rank_diagnostic(ctx, 0);
                 detail::report_rank(regressors[level], sd_last_rank(ctx), D, detail::reports_rank<RegressorType>());
             }
             // a factorisation that broke down throws (with the rank in the message): NaN weights would poison the next level
-            sd_b200::check(ctx, rc, "sd_learn_centred");
+            sd_b200::check(ctx, rc, "sd_train_level");
             regressors[level].set_x(sd_b200::download(X.as<float>(), D, Pd, Pd));
             regressors[level].report_solver();
-            sd_b200::check(ctx, sd_cascade_update(ctx, A.as<float>(), ld, n, D, Xc.as<float>(), Pd, d_cur.as<float>(), &norm, d_next.as<float>()), "sd_cascade_update");   // 4) :209-215
             std::swap(d_cur, d_next);
             if (want_callback) {                                                                             // 5) :217
                 if (nranks > 1) {
@@ -286,19 +296,21 @@ private:
     {
         sd_ctx* ctx = sd_b200::context();
         const int n = initialisations.rows, Pd = initialisations.cols;
-        sd_b200::DeviceBuffer d_cur, d_next(static_cast<size_t>(n) * Pd * sizeof(float)), d_tmpl, A;
+        sd_b200::DeviceBuffer d_cur, d_next(static_cast<size_t>(n) * Pd * sizeof(float)), d_tmpl;
         sd_b200::upload(initialisations, d_cur, Pd);
         const sd_normalisation norm = normalisation_strategy.c_normalisation();
+        const sd_normalisation eyes = projection.eyes();
+        const sd_image_batch& images = projection.device_batch();
+        if (!templates.empty()) sd_b200::upload(templates, d_tmpl, templates.cols);
         for (size_t level = 0; level < regressors.size(); ++level) {
             const int D = projection.feature_length(level);
             const int64_t ld = (static_cast<int64_t>(D) + 3) / 4 * 4;
-            A.allocate(static_cast<size_t>(n) * ld * sizeof(float));
-            projection.project_device(d_cur.as<float>(), Pd, n, level, A.as<float>(), ld);
-            if (!templates.empty()) {
-                sd_b200::upload(templates, d_tmpl, templates.cols);
-                sd_b200::check(ctx, sd_subtract_templates(ctx, A.as<float>(), ld, d_tmpl.as<float>(), templates.cols, n, D), "sd_subtract_templates");
-            }
-            sd_b200::check(ctx, sd_cascade_update(ctx, A.as<float>(), ld, n, D, regressors[level].device_x(), Pd, d_cur.as<float>(), &norm, d_next.as<float>()), "sd_cascade_update");
+            const sd_hog_param hp = projection.hog_param(level);
+            const int rows = chunk_rows(ctx, nullptr, n, D, Pd, 0);
+            sd_b200::DeviceBuffer chunk(static_cast<size_t>(rows) * ld * sizeof(float));
+            sd_b200::check(ctx, sd_apply_level(ctx, &images, nullptr, d_cur.as<float>(), n, Pd / 2, &eyes, &hp, &norm,
+                                               templates.empty() ? nullptr : d_tmpl.as<float>(), templates.cols, regressors[level].device_x(),
+                                               chunk.as<float>(), ld, rows, d_next.as<float>()), "sd_apply_level");
             std::swap(d_cur, d_next);
             if (want_callback) cb(sd_b200::download(d_cur.as<float>(), n, Pd, Pd));                          // :303
         }
