@@ -379,6 +379,41 @@ SD_API int sd_apply_level(sd_ctx* ctx, const sd_image_batch* images, const int32
                           const float* d_templates, int64_t ldt, const float* d_X,
                           float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next);
 
+/* ---- the same levels on frames that stay in host memory (DESIGN 4.6) ------------------------------------------------------
+ * sd_train_level_host / sd_apply_level_host: the contract of sd_train_level / sd_apply_level, bit for bit the same X, lambda and
+ * x_next as those calls on the same frames uploaded by sd_upload_frames, with three differences:
+ *   - frames: num_frames host frames (sd_host_frame: grey or B,G,R, any sizes), each in pinned, device-mapped memory with a 16-byte
+ *     aligned base and row_stride (the ROI route of sd_detect_faces_host), and row_stride >= channels * (width rounded up to 16).
+ *     Only frames a sample refers to are read or checked.  They are read in place while the call runs.
+ *   - d_sample_frame (device, N ints, required): sample i reads frames[d_sample_frame[i]].  An index out of range raises the
+ *     projection's status flag (reported by the next synchronising call, as for sd_hog_batch) and the sample reads frame 0.
+ *   - d_stage / stage_bytes: a device staging buffer the caller owns (16-byte aligned), used as two halves.  Each half must hold the
+ *     largest frame a sample refers to as grey bytes at a 16-byte pitch (height * roundup16(width)): no region is larger.
+ * Per chunk of rows the HOG rows are produced in gather batches that fit one staging half: the exact union of the windows of the
+ * batch's patches is planned per frame on the device (samples of one frame in one batch share one region), gathered zero-copy
+ * over PCIe (colour converted to grey on the way) on the context's copy stream while the previous batch's HOG runs, and read by
+ * the unchanged HOG kernel.  One small read-back per batch is the only synchronisation the plan adds.
+ * Frames that break these rules, or a staging half that is too small, are SD_ERR_INVALID before any work is queued (the outputs are
+ * not written).  The call reads d_sample_frame back once before it queues work.  Every rank passes its own frames. */
+SD_API int sd_train_level_host(sd_ctx* ctx, sd_comm* comm, const sd_host_frame* frames, int num_frames, const int32_t* d_sample_frame,
+                               const float* d_x, const float* d_x_gt, int N_local, int L, int64_t n_global,
+                               const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
+                               const float* d_templates, int64_t ldt, const sd_regulariser* reg, int route,
+                               float* d_chunk, int64_t ld, int chunk_rows, void* d_stage, size_t stage_bytes,
+                               float* d_X, float* d_x_next, float* lambda_out);
+SD_API int sd_apply_level_host(sd_ctx* ctx, const sd_host_frame* frames, int num_frames, const int32_t* d_sample_frame,
+                               const float* d_x, int N, int L, const sd_normalisation* hog_eyes, const sd_hog_param* p,
+                               const sd_normalisation* norm, const float* d_templates, int64_t ldt, const float* d_X,
+                               float* d_chunk, int64_t ld, int chunk_rows, void* d_stage, size_t stage_bytes, float* d_x_next);
+/* host-frame bytes (region bytes x channels) the _host levels have read over PCIe on ctx since creation */
+SD_API int64_t sd_gathered_bytes(const sd_ctx* ctx);
+/* *in_place = 1 when the _host levels can read the frame where it is (pinned and device-mapped, 16-byte aligned base and
+ * row_stride, row_stride >= channels * roundup16(width)), else 0; a bad frame (as for sd_upload_frames) is SD_ERR_INVALID.  The
+ * HogTransform front ends pack the other frames once into pinned memory. */
+SD_API int sd_host_frame_in_place(sd_ctx* ctx, const sd_host_frame* frame, int* in_place);
+/* free and total memory of the context's device (cudaMemGetInfo): what the HogTransform front ends choose their route by */
+SD_API int sd_device_memory(sd_ctx* ctx, size_t* free_bytes, size_t* total_bytes);
+
 /* ---- rcr::detection_model (model.hpp:122-219) -------------------------------------------- */
 /* load_detection_model / save_detection_model (model.hpp:192-219): cereal binary, byte compatible */
 SD_API int sd_model_load(sd_ctx* ctx, const char* path, sd_model** out);

@@ -60,6 +60,7 @@ EXPORTS = [
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",
     "sd_comm_sum_int64", "sd_comm_allgather", "sd_allreduce_gram", "sd_reduce_scatter_gram", "sd_solve_gram_dist", "sd_learn_dist",
     "sd_cascade_targets", "sd_cascade_update", "sd_subtract_templates", "sd_level_chunk_rows", "sd_train_level", "sd_apply_level",
+    "sd_train_level_host", "sd_apply_level_host", "sd_gathered_bytes", "sd_host_frame_in_place", "sd_device_memory",
     "sd_model_load", "sd_model_save", "sd_model_create", "sd_model_destroy", "sd_model_num_levels",
     "sd_model_num_landmarks", "sd_model_hog_param", "sd_model_regulariser", "sd_model_normalisation",
     "sd_model_get_mean", "sd_model_get_weights", "sd_model_landmark_id", "sd_align_mean",
@@ -83,6 +84,8 @@ def lib():
         l.sd_launch_count.restype = C.c_int64
         l.sd_roi_fallback_count.restype = C.c_int64
         l.sd_roi_fallback_count.argtypes = [C.c_void_p]
+        l.sd_gathered_bytes.restype = C.c_int64
+        l.sd_gathered_bytes.argtypes = [C.c_void_p]
         l.sd_model_landmark_id.restype = C.c_char_p
         l.sd_last_error.argtypes = [C.c_void_p]
         l.sd_launch_count.argtypes = [C.c_void_p]

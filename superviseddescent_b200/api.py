@@ -360,6 +360,12 @@ def _device_images(images, ctx: Context):
             raise ValueError("every image must be (H, W) uint8 or (H, W, 3) uint8")
         recs.append(rec)
         keep.append(a)                                       # the bytes stay alive until the upload returns
+    return _upload_host_frames(recs, ctx)
+
+
+def _upload_host_frames(recs, ctx: Context):
+    """sd_host_frame records -> (the device tensor that owns the grey frames, the ImageBatchC sd_hog_batch reads)."""
+    dev = f"cuda:{ctx.device}"
     table = (HostFrameC * len(recs))(*recs)
     nbytes = C.c_size_t(0)
     _check(ctx.h, _capi.lib().sd_upload_frames(ctx.h, table, len(recs), None, C.byref(nbytes), None))
@@ -369,55 +375,198 @@ def _device_images(images, ctx: Context):
     return buf, ib
 
 
+# The distinct frames of a HogTransform are uploaded when their grey bytes fit in this share of the device's free memory (read when
+# the transform is first used); otherwise they stay in host memory and train() / test() gather them per level
+# (sd_train_level_host / sd_apply_level_host).
+DEVICE_FRAME_SHARE = 0.5
+# bytes of one half of the staging buffer of the host route (at least the largest frame's grey bytes)
+HOST_STAGE_HALF = 48 << 20
+
+
+def _round16(v: int) -> int:
+    return (v + 15) // 16 * 16
+
+
+def _free_device_bytes(device: int) -> int:
+    """Free device memory, counting what torch has reserved but not handed out."""
+    return torch.cuda.mem_get_info(device)[0] + torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
+
+
+class _PinnedBuffer:
+    """bytes of pinned host memory from sd_host_alloc (exactly that size), as a numpy uint8 array; freed with the object"""
+
+    def __init__(self, ctx: Context, nbytes: int):
+        self.ctx, self._p = ctx, C.c_void_p()
+        _check(ctx.h, _capi.lib().sd_host_alloc(ctx.h, C.c_size_t(nbytes), C.byref(self._p)))
+        self.array = np.ctypeslib.as_array((C.c_uint8 * nbytes).from_address(self._p.value))
+
+    def __del__(self):
+        try:
+            if self._p:
+                _capi.lib().sd_host_free(self.ctx.h, self._p)
+                self._p = C.c_void_p()
+        except Exception:
+            pass
+
+
 class HogTransform:
     """Projection functor h.  images: (count, H, W) uint8 (8UC1) or (count, H, W, 3) uint8 (8UC3, B G R: converted
     once on the device as adaptive_vlhog.hpp:114-120 does per call), on host or device, or a list of such frames of any
     sizes.
 
+    A list may name one frame several times (rcr-train makes 11 samples per photo): entries that are the same object or share
+    data pointer, shape and strides are one frame, held once.  image_index (optional, N ints): sample i reads images[image_index[i]]
+    (default: sample i reads images[i]).  Host frames whose grey bytes fit in DEVICE_FRAME_SHARE of the free device memory are
+    uploaded when the transform is first used; larger sets stay in host memory and the optimiser gathers them level by level.
+    Frames the levels can read in place (pinned and aligned, sd_host_frame_in_place) are read at every level, so changing them
+    after the first use changes the result; the others are copied once, on first use, into one pinned buffer.  Until the first
+    use the transform holds references to the arrays of a list: do not change them before it.
+
     __call__(parameters, regressor_level, training_index) keeps the reference's meaning
     (adaptive_vlhog.hpp:109) but takes ALL rows at once: parameters is (N, 2L) and training_index an
-    optional (N,) int array (default: row i uses image i, as train()/test() do).  A single (2L,) row
+    optional (N,) int array of indices into images (default: the sample -> frame map above).  A single (2L,) row
     with an int training_index is accepted too (predict()'s call shape, superviseddescent.hpp:332).
     """
 
     def __init__(self, images, hog_params: Sequence[HoGParam], model_landmarks_list: Sequence[str],
-                 right_eye_identifiers: Sequence[str], left_eye_identifiers: Sequence[str], ctx: Optional[Context] = None):
+                 right_eye_identifiers: Sequence[str], left_eye_identifiers: Sequence[str], ctx: Optional[Context] = None,
+                 image_index=None):
         self.ctx = ctx or default_context()
-        self.images, self._batch = _device_images(images, self.ctx)
         self.hog_params = list(hog_params)
         self.norm = InterEyeDistanceNormalisation(model_landmarks_list, right_eye_identifiers, left_eye_identifiers)
         self.num_landmarks = len(self.norm.model_landmarks_list)
+        self.images = None            # device bytes that hold the frames (device route)
+        self._batch = None
+        self._host = None             # (HostFrameC table, arrays that own the bytes) on the host route
+        self._frames = None           # distinct host frames, until the route is chosen
+        self._list_frame = None       # list entry -> distinct frame (None: entry i is frame i)
+        if isinstance(images, (list, tuple)):
+            self._frames, self._list_frame = self._distinct(images)
+        else:
+            self.images, self._batch = _device_images(images, self.ctx)
+        n_list = len(images)
+        if image_index is not None:
+            idx = np.ascontiguousarray(image_index, dtype=np.int64).ravel()
+            if idx.size and (idx.min() < 0 or idx.max() >= n_list):
+                raise ValueError("image_index refers to an image that is not in the list")
+            sample = (self._list_frame[idx] if self._list_frame is not None else idx).astype(np.int32)
+        else:
+            sample = self._list_frame
+        self._sample_frame = None if sample is None else torch.from_numpy(np.ascontiguousarray(sample, dtype=np.int32)).to(f"cuda:{self.ctx.device}")
+
+    @staticmethod
+    def _distinct(images):
+        """(list of (sd_host_frame, owning array) of the distinct frames, list entry -> frame index)"""
+        frames, index, seen = [], np.empty(len(images), dtype=np.int32), {}
+        for i, f in enumerate(images):
+            rec, a = _host_frame(f)
+            if a.ndim == 3 and a.shape[2] != 3:
+                raise ValueError("every image must be (H, W) uint8 or (H, W, 3) uint8")
+            key = (a.ctypes.data, a.shape, a.strides)
+            if key not in seen:
+                seen[key] = len(frames)
+                frames.append((rec, a))
+            index[i] = seen[key]
+        return frames, index
+
+    def _choose_route(self):
+        """Once, on first use: upload the distinct frames when their grey bytes fit in DEVICE_FRAME_SHARE of the free device
+        memory, else keep them in host memory."""
+        if self._frames is None:
+            return
+        frames, self._frames = self._frames, None
+        recs = [r for r, _ in frames]
+        grey = sum(r.height * _round16(r.width) for r in recs)
+        if grey <= DEVICE_FRAME_SHARE * _free_device_bytes(self.ctx.device):
+            self.images, self._batch = _upload_host_frames(recs, self.ctx)
+            return
+        # host route: pinned frames with 16-byte aligned rows (and every 16-pixel step of a row inside it) are read in place; the
+        # others are packed once into one pinned buffer at such a pitch
+        lib = _capi.lib()
+
+        def in_place(r):
+            ok = C.c_int(0)
+            _check(self.ctx.h, lib.sd_host_frame_in_place(self.ctx.h, C.byref(r), C.byref(ok)))
+            return bool(ok.value)
+        pack = [not in_place(r) for r, _ in frames]
+        pitch = [r.channels * _round16(r.width) for r, _ in frames]
+        total = sum(p * r.height for (r, _), p, k in zip(frames, pitch, pack) if k)
+        buf = _PinnedBuffer(self.ctx, total) if total else None
+        out, keep, off = [], [a for _, a in frames], 0
+        for (r, a), p, k in zip(frames, pitch, pack):
+            if k:
+                dst = buf.array[off:off + p * r.height].reshape(r.height, p)
+                dst[:, :r.width * r.channels] = a.reshape(r.height, r.width * r.channels)
+                off += p * r.height
+                r = HostFrameC(dst.ctypes.data, r.width, r.height, p, r.channels)
+            out.append(r)
+        self._host = ((HostFrameC * len(out))(*out), keep, buf)
+
+    def on_device(self) -> bool:
+        """Whether the frames are resident on the device (False: they stay in host memory and are gathered per level)."""
+        self._choose_route()
+        return self._host is None
 
     def batch(self) -> ImageBatchC:
+        self._choose_route()
+        if self._host is not None:
+            raise SdError(1, "HogTransform: the frames stay in host memory (they do not fit on the device); only the optimiser's "
+                             "train() / test() / predict() read them")
         return self._batch
+
+    def sample_frame(self, n: int) -> Optional[torch.Tensor]:
+        """Device (n,) int32 index: sample i reads frame sample_frame[i] of batch() (None: frame i)."""
+        if self._sample_frame is None:
+            return None
+        if n > self._sample_frame.numel():
+            raise ValueError(f"{n} samples but the image list / image_index has {self._sample_frame.numel()}")
+        return self._sample_frame[:n]
+
+    def host_frames(self):
+        """(sd_host_frame table, number of frames) on the host route."""
+        self._choose_route()
+        return self._host[0], len(self._host[0])
+
+    def stage_bytes(self) -> int:
+        """Staging buffer of the host route: two halves of HOST_STAGE_HALF bytes, or of the largest frame's grey bytes."""
+        table, n = self.host_frames()
+        largest = max(table[i].height * _round16(table[i].width) for i in range(n))
+        return 2 * _round16(max(HOST_STAGE_HALF, largest))
 
     def feature_length(self, level: int) -> int:
         return _capi.lib().sd_hog_feature_length(self.num_landmarks, C.byref(self.hog_params[level]))
 
     def into(self, parameters: torch.Tensor, level: int, out: torch.Tensor, image_index: Optional[torch.Tensor] = None):
-        """Writes the feature rows into out[:, :D] (out may be wider: extended [A | b] operand)."""
+        """Writes the feature rows into out[:, :D] (out may be wider: extended [A | b] operand).  image_index: frames of batch()
+        (default: sample_frame)."""
         ctx = self.ctx
         n = parameters.shape[0]
         eyes = self.norm.c()
         ib = self.batch()
+        if image_index is None:
+            image_index = self.sample_frame(n)
         idx_ptr = ptr(image_index) if image_index is not None else C.c_void_p(0)
         _check(ctx.h, _capi.lib().sd_hog_batch(ctx.h, C.byref(ib), idx_ptr, ptr(parameters), C.c_int64(parameters.stride(0)),
                                                n, self.num_landmarks, C.byref(eyes), C.byref(self.hog_params[level]),
                                                ptr(out), C.c_int64(out.stride(0))))
 
+    def _frame_index(self, training_index, n: int, single: bool, device) -> Optional[torch.Tensor]:
+        """training_index (indices into images) -> frames of batch()"""
+        if training_index is None:
+            return torch.zeros(1, dtype=torch.int32, device=device) if single else self.sample_frame(n)
+        if np.isscalar(training_index):
+            training_index = [int(training_index)] * n
+        idx = np.asarray(training_index, dtype=np.int64)
+        if self._list_frame is not None:
+            idx = self._list_frame[idx]
+        return torch.from_numpy(np.ascontiguousarray(idx, dtype=np.int32)).to(device)
+
     def __call__(self, parameters, regressor_level: int, training_index=None) -> torch.Tensor:
-        ctx = self.ctx
-        x = _dev(parameters, ctx)
+        x = _dev(parameters, self.ctx)
         single = x.dim() == 1
         if single:
             x = x.reshape(1, -1)
-        idx = None
-        if training_index is not None:
-            if np.isscalar(training_index):
-                training_index = [int(training_index)] * x.shape[0]
-            idx = _dev(np.asarray(training_index, dtype=np.int32), ctx, dtype=torch.int32)
-        elif single:
-            idx = torch.zeros(1, dtype=torch.int32, device=x.device)
+        idx = self._frame_index(training_index, x.shape[0], single, x.device)
         D = self.feature_length(regressor_level)
         out = torch.empty((x.shape[0], D), dtype=torch.float32, device=x.device)
         self.into(x, regressor_level, out, idx)
@@ -434,9 +583,7 @@ class HogTransform:
         geo = torch.empty((n, L, 3), dtype=torch.int32, device=x.device)
         patches = torch.empty((n, L, fs, fs), dtype=torch.uint8, device=x.device)
         bins = torch.empty((n, L, fs, fs), dtype=torch.int8, device=x.device)
-        idx = None
-        if training_index is not None:
-            idx = _dev(np.asarray(training_index, dtype=np.int32), ctx, dtype=torch.int32)
+        idx = self._frame_index(training_index, n, False, x.device)
         eyes = self.norm.c()
         ib = self.batch()
         _check(ctx.h, _capi.lib().sd_hog_debug(ctx.h, C.byref(ib), ptr(idx), ptr(x), C.c_int64(x.stride(0)), n, L,
@@ -493,6 +640,26 @@ class SupervisedDescentOptimiser:
         host[:, :D] = np.stack(rows)
         return _dev(host, ctx), D
 
+    class _Frames:
+        """What a HogTransform level reads: the device batch, or the host frames and a staging buffer; and the sample -> frame
+        index (None: sample i reads frame i)."""
+        batch = table = stage = None
+        count = 0
+        index = None
+
+    def _frame_source(self, h: "HogTransform", n: int, device) -> "_Frames":
+        f = self._Frames()
+        f.index = h.sample_frame(n)
+        if h.on_device():
+            f.batch = h.batch()
+            return f
+        f.table, f.count = h.host_frames()
+        if f.index is None:
+            f.index = torch.arange(n, dtype=torch.int32, device=device)
+        # allocated before the chunk query, so that the chunk buffer is sized on the free memory beside it
+        f.stage = torch.empty(h.stage_bytes(), dtype=torch.uint8, device=device)
+        return f
+
     def _chunk_rows(self, rows_per_chunk, n: int, D: int, P: int, comm_h, route: int) -> int:
         """Rows per chunk of a HogTransform level: rows_per_chunk (at most n), or -- None / 0 -- the most that fit beside the
         solve (sd_level_chunk_rows; memory torch has reserved but not handed out counts as free, so a warm caching allocator
@@ -500,7 +667,7 @@ class SupervisedDescentOptimiser:
         if rows_per_chunk:
             return max(1, min(int(rows_per_chunk), n))
         ctx = self._ctx()
-        free = torch.cuda.mem_get_info(ctx.device)[0] + torch.cuda.memory_reserved(ctx.device) - torch.cuda.memory_allocated(ctx.device)
+        free = _free_device_bytes(ctx.device)
         rows = C.c_int(0)
         _check(ctx.h, _capi.lib().sd_level_chunk_rows(ctx.h, comm_h, C.c_int64(n), D, P, route, C.c_size_t(free), C.byref(rows)))
         return rows.value
@@ -515,7 +682,8 @@ class SupervisedDescentOptimiser:
         ranks.
         A HogTransform projection trains each level with sd_train_level, through a buffer of rows_per_chunk feature rows (None:
         as many as fit on the device, which is all of them whenever the level fits -- then the result is that of one pass over
-        all rows).  Templates need the whole level in one chunk."""
+        all rows).  Templates need the whole level in one chunk.  A HogTransform whose frames stay in host memory trains with
+        sd_train_level_host instead (same results), the chunk buffer sized beside its staging buffer."""
         from . import parallel
         ctx = self._ctx()
         lib = _capi.lib()
@@ -539,6 +707,7 @@ class SupervisedDescentOptimiser:
             return 2 if distributed_solve == "cg" else int(bool(distributed_solve))
 
         ch = comm.h if distributed else None
+        frames = self._frame_source(projection, n, cur.device) if hog else None
         for level, reg in enumerate(self.regressors):
             norm = self.normalisation_strategy.c(P // 2)
             lam = C.c_float(0)
@@ -555,10 +724,14 @@ class SupervisedDescentOptimiser:
                 self.chunk_rows.append(rows)
                 buf = torch.empty((rows, ld), dtype=torch.float32, device=cur.device)
                 eyes = projection.norm.c()
-                rc = lib.sd_train_level(ctx.h, ch, C.byref(projection.batch()), None, ptr(cur), ptr(x_gt), n, P // 2, C.c_int64(n_global),
-                                        C.byref(eyes), C.byref(projection.hog_params[level]), C.byref(norm), ptr(tmpl),
-                                        C.c_int64(tmpl.stride(0) if tmpl is not None else 0), C.byref(rc_), route(D), ptr(buf),
-                                        C.c_int64(ld), rows, ptr(X), ptr(nxt), C.byref(lam))
+                args = (ptr(cur), ptr(x_gt), n, P // 2, C.c_int64(n_global), C.byref(eyes), C.byref(projection.hog_params[level]),
+                        C.byref(norm), ptr(tmpl), C.c_int64(tmpl.stride(0) if tmpl is not None else 0), C.byref(rc_), route(D), ptr(buf),
+                        C.c_int64(ld), rows)
+                if frames.stage is not None:
+                    rc = lib.sd_train_level_host(ctx.h, ch, frames.table, frames.count, ptr(frames.index), *args, ptr(frames.stage),
+                                                 C.c_size_t(frames.stage.numel()), ptr(X), ptr(nxt), C.byref(lam))
+                else:
+                    rc = lib.sd_train_level(ctx.h, ch, C.byref(frames.batch), ptr(frames.index), *args, ptr(X), ptr(nxt), C.byref(lam))
                 del buf
             else:
                 A, D = self._project(projection, cur, level, extra=P)         # 1) features (:173-189)
@@ -601,6 +774,7 @@ class SupervisedDescentOptimiser:
             cur = cur.reshape(1, -1)
         n, P = cur.shape
         tmpl = _dev(templates, ctx) if templates is not None and np.size(templates) > 0 else None
+        frames = self._frame_source(projection, n, cur.device) if isinstance(projection, HogTransform) else None
         for level, reg in enumerate(self.regressors):
             norm = self.normalisation_strategy.c(P // 2)
             nxt = torch.empty_like(cur)
@@ -610,10 +784,13 @@ class SupervisedDescentOptimiser:
                 rows = self._chunk_rows(rows_per_chunk, n, D, P, None, 0)
                 buf = torch.empty((rows, ld), dtype=torch.float32, device=cur.device)
                 eyes = projection.norm.c()
-                _check(ctx.h, lib.sd_apply_level(ctx.h, C.byref(projection.batch()), None, ptr(cur), n, P // 2, C.byref(eyes),
-                                                 C.byref(projection.hog_params[level]), C.byref(norm), ptr(tmpl),
-                                                 C.c_int64(tmpl.stride(0) if tmpl is not None else 0), ptr(reg.x), ptr(buf), C.c_int64(ld),
-                                                 rows, ptr(nxt)))
+                args = (ptr(cur), n, P // 2, C.byref(eyes), C.byref(projection.hog_params[level]), C.byref(norm), ptr(tmpl),
+                        C.c_int64(tmpl.stride(0) if tmpl is not None else 0), ptr(reg.x), ptr(buf), C.c_int64(ld), rows)
+                if frames.stage is not None:
+                    _check(ctx.h, lib.sd_apply_level_host(ctx.h, frames.table, frames.count, ptr(frames.index), *args, ptr(frames.stage),
+                                                          C.c_size_t(frames.stage.numel()), ptr(nxt)))
+                else:
+                    _check(ctx.h, lib.sd_apply_level(ctx.h, C.byref(frames.batch), ptr(frames.index), *args, ptr(nxt)))
                 del buf
             else:
                 A, D = self._project(projection, cur, level, extra=0)

@@ -19,7 +19,8 @@ enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_PARTIAL, SD_WS_GEOM, SD_WS_GEMM_PARTIAL, SD_WS_DIAGINV2, SD_WS_PANEL, SD_WS_BIAS, SD_WS_CG, SD_WS_CGMAT,
        SD_WS_UPLOAD /* B,G,R scratch of sd_upload_frames */,
        SD_WS_RANK /* the rank diagnostic's working copy of the D x D system, its panel and state (sd_rank.cu) */,
-       SD_WS_LEVEL /* column shift and shifted-row weights of sd_train_level (sd_train.cu) */, SD_WS_COUNT };
+       SD_WS_LEVEL /* column shift and shifted-row weights of sd_train_level (sd_train.cu) */,
+       SD_WS_GATHER /* frame, union, region and record tables of the host-frame levels (sd_train.cu) */, SD_WS_COUNT };
 
 // Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row
 // Cholesky blocks), and panel p belongs to rank p % nranks.  The Gram exchange delivers each panel's rows to their owner, and
@@ -54,6 +55,7 @@ struct sd_ctx {
     int last_rank = -1;            // of the last solve: the rank, or -1 when it was not computed
     cudaEvent_t cg_ev[8] = {};     // convergence read-backs of the CG loop (the host runs a few iterations ahead of them)
     int64_t roi_fallbacks = 0;     // faces repeated from the full frame because a patch left its ROI
+    int64_t gathered_bytes = 0;    // host-frame bytes the levels of sd_train_level_host / sd_apply_level_host read over PCIe
     float timings[4] = {0, 0, 0, 0};
     cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     void* hog_lut[SD_MAX_BINS + 1] = {};   // per K: (gx,gy) -> orientation bin table (sd_hog.cu)
@@ -168,6 +170,33 @@ struct sd_eyes_dev {
 };
 int sd_eyes_to_dev(sd_ctx* ctx, const sd_normalisation* n, int num_landmarks, sd_eyes_dev* out);
 
+// ---- host frames read in place (sd_model.cu) ---------------------------------------------------------------------------------
+// One region of a pinned host frame for roi_gather_kernel: the SMs pull its rows zero-copy into a packed grey device buffer
+// (16-byte vectors; colour pixels converted on the way).  The region's x is a multiple of 16 pixels and its rows lie inside the
+// frame's row_stride.
+struct GatherRec {
+    const uint8_t* src;          // device-mapped address of the region's first pixel in the caller's frame
+    int64_t src_stride;          // bytes between the frame's rows
+    int64_t dst_offset;          // of the grey region in the staging buffer; its rows are 16 * vec_per_row bytes apart
+    int32_t vec_per_row, rows;   // region size in steps of 16 pixels x rows
+};
+// the one gather: n_grey records of grey frames, then n_colour records of B,G,R frames, into dst, on `stream`
+int sd_roi_gather(sd_ctx* ctx, const GatherRec* d_grey, int n_grey, const GatherRec* d_colour, int n_colour, uint8_t* dst,
+                  cudaStream_t stream);
+// Device-mapped address of a pinned host frame, or nullptr.  Frames inside the last pinned allocation seen are mapped by
+// offset instead of one driver query each.
+struct PinnedRange {
+    uintptr_t lo = 0, hi = 0;    // host addresses of the allocation
+    intptr_t delta = 0;          // device address - host address
+};
+const uint8_t* sd_mapped_frame(const uint8_t* p, size_t bytes, PinnedRange& last);
+// what every entry point that reads sd_host_frame requires of frame f; fn names the entry point in the message
+int sd_check_host_frame(sd_ctx* ctx, const char* fn, const sd_host_frame& fr, int f);
+inline size_t sd_host_frame_bytes(const sd_host_frame& f) { return (size_t)(f.height - 1) * f.row_stride + (size_t)f.width * f.channels; }
+inline size_t sd_round16(size_t v) { return (v + 15) & ~(size_t)15; }
+// grey bytes of a frame at a 16-byte pitch: no region of it is larger
+inline size_t sd_gray_bytes(const sd_host_frame& f) { return (size_t)f.height * sd_round16(f.width); }
+
 #ifdef __CUDACC__
 // Inter-eye distance exactly as helpers.hpp:136-160 evaluates it: eye centres are float sums
 // scaled by the float reciprocal of the count (cv::Vec /= float), the difference is taken in float,
@@ -192,6 +221,24 @@ __device__ __forceinline__ double sd_device_ied(const float* __restrict__ row, i
     const double dx = (double)__fsub_rn(rx, lx);
     const double dy = (double)__fsub_rn(ry, ly);
     return sqrt(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));
+}
+
+// Half patch size of one sample (adaptive_vlhog.hpp:123): std::round(float rel * double IED / 2), or fixed_half > 0 for the
+// non-adaptive HogTransform (examples/landmark_detection.cpp:213).  A half below 1 (cv::resize would throw on the empty ROI)
+// becomes 1 and sets *degenerate.  hog_geometry_kernel (sd_hog.cu) and roi_plan_kernel (sd_train.cu) both call it, so the
+// window a training gather plans is the window the HOG kernel reads.
+__device__ __forceinline__ int sd_patch_half(const float* __restrict__ row, int L, const sd_eyes_dev& eyes, float rel, int fixed_half,
+                                             bool* degenerate)
+{
+    *degenerate = false;
+    if (fixed_half > 0) return fixed_half;
+    const double ied = sd_device_ied(row, L, eyes);
+    int half = (int)round(__dmul_rn(__dmul_rn((double)rel, ied), 0.5));
+    if (half < 1) {
+        half = 1;
+        *degenerate = true;
+    }
+    return half;
 }
 
 // cv::cvtColor(BGR2GRAY) of one 8-bit pixel, OpenCV >= 3 fixed point (15-bit coefficients, SURVEY.md 8c).  The only spelling of

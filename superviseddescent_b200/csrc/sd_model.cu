@@ -173,18 +173,12 @@ int detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, 
 }
 
 
-// ---- region-of-interest gather (sd_detect_faces_host) -------------------------------------------------
+// ---- region-of-interest gather (sd_detect_faces_host, sd_train_level_host, sd_apply_level_host) ----------------------------
 // The cascade only ever reads a neighbourhood of the face, so instead of copying whole frames over PCIe a small kernel pulls
 // the ROI rows of every face straight out of the caller's PINNED host frame (zero-copy loads through the unified address
-// space, 16-byte vectors) into a packed grey device buffer.  If a patch later needs a frame pixel outside its ROI the HOG
-// kernel raises d_roi_miss[face] and that face is repeated from its full frame, so the result never depends on the ROI
-// heuristic.
-struct GatherRec {
-    const uint8_t* src;          // device-mapped address of the ROI's first pixel in the caller's frame
-    int64_t src_stride;          // bytes between the frame's rows
-    int64_t dst_offset;          // of the grey ROI in the staging buffer; its rows are 16 * vec_per_row bytes apart
-    int32_t vec_per_row, rows;   // ROI size in steps of 16 pixels x rows
-};
+// space, 16-byte vectors) into a packed grey device buffer.  In detect, if a patch later needs a frame pixel outside its ROI
+// the HOG kernel raises d_roi_miss[face] and that face is repeated from its full frame, so the result never depends on the
+// ROI heuristic; a training level plans its regions exactly (sd_train.cu).
 
 // 16 interleaved B,G,R pixels (48 bytes) -> 16 grey bytes
 __device__ __forceinline__ uint4 bgr16_to_gray(const uint4 (&v)[3])
@@ -278,16 +272,26 @@ sd_roi face_roi(const sd_model* m, const float* x0, int width, int height, int r
     return r;
 }
 
-// Device-mapped address of a pinned host frame, or nullptr.  Frames inside the last pinned allocation seen (every frame of
-// sd_detect_batch_host's batch) are mapped by offset instead of one driver query each.
-struct PinnedRange {
-    uintptr_t lo = 0, hi = 0;    // host addresses of the allocation
-    intptr_t delta = 0;          // device address - host address
-};
-
 typedef CUresult (*PFN_pointerGetAttribute)(void* data, CUpointer_attribute attribute, CUdeviceptr ptr);
 
-const uint8_t* mapped_frame(const uint8_t* p, size_t bytes, PinnedRange& last)
+}  // namespace
+
+int sd_roi_gather(sd_ctx* ctx, const GatherRec* d_grey, int n_grey, const GatherRec* d_colour, int n_colour, uint8_t* dst, cudaStream_t stream)
+{
+    const int most = 8 * ctx->sm_count;
+    if (n_grey > 0) {
+        roi_gather_kernel<1><<<n_grey < most ? n_grey : most, 256, 0, stream>>>(d_grey, n_grey, dst);
+        SD_LAUNCH_CHECK(ctx, "roi_gather_kernel<1>");
+    }
+    if (n_colour > 0) {
+        roi_gather_kernel<3><<<n_colour < most ? n_colour : most, 256, 0, stream>>>(d_colour, n_colour, dst);
+        SD_LAUNCH_CHECK(ctx, "roi_gather_kernel<3>");
+    }
+    return SD_OK;
+}
+
+// Frames inside the last pinned allocation seen (every frame of sd_detect_batch_host's batch) are mapped by offset.
+const uint8_t* sd_mapped_frame(const uint8_t* p, size_t bytes, PinnedRange& last)
 {
     const uintptr_t a = reinterpret_cast<uintptr_t>(p);
     if (a >= last.lo && a + bytes <= last.hi) return reinterpret_cast<const uint8_t*>(a + last.delta);
@@ -311,13 +315,7 @@ const uint8_t* mapped_frame(const uint8_t* p, size_t bytes, PinnedRange& last)
     return static_cast<const uint8_t*>(attr.devicePointer);
 }
 
-size_t host_frame_bytes(const sd_host_frame& f) { return (size_t)(f.height - 1) * f.row_stride + (size_t)f.width * f.channels; }
-size_t round16(size_t v) { return (v + 15) & ~(size_t)15; }
-size_t gray_bytes(const sd_host_frame& f) { return (size_t)f.height * round16(f.width); }
-size_t bgr_bytes(const sd_host_frame& f) { return f.channels == 3 ? (size_t)f.height * round16(3 * (size_t)f.width) : 0; }
-
-// what every entry point that reads sd_host_frame requires of frame f; fn names the entry point in the message
-int check_host_frame(sd_ctx* ctx, const char* fn, const sd_host_frame& fr, int f)
+int sd_check_host_frame(sd_ctx* ctx, const char* fn, const sd_host_frame& fr, int f)
 {
     if (fr.channels != 1 && fr.channels != 3)
         return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d has %d channels (1 or 3)", fn, f, fr.channels);
@@ -325,6 +323,10 @@ int check_host_frame(sd_ctx* ctx, const char* fn, const sd_host_frame& fr, int f
         return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d: bad data pointer, size or row_stride < width * channels", fn, f);
     return SD_OK;
 }
+
+namespace {
+
+size_t bgr_bytes(const sd_host_frame& f) { return f.channels == 3 ? (size_t)f.height * sd_round16(3 * (size_t)f.width) : 0; }
 
 // ---- host frames -> grey device frames (sd_detect_faces_host's chunks, sd_upload_frames) --------------------------------
 // The device layout: grey rows at a 16-byte pitch, frames back to back from offset 0.  Equally sized frames are then a plain
@@ -336,8 +338,8 @@ size_t frame_layout(const sd_host_frame* frames, int n, sd_frame* desc, bool* un
     *uniform = true;
     for (int i = 0; i < n; ++i) {
         const sd_host_frame& f = frames[i];
-        desc[i] = sd_frame{f.width, f.height, (int32_t)round16(f.width), 0, (int64_t)off};
-        off += gray_bytes(f);
+        desc[i] = sd_frame{f.width, f.height, (int32_t)sd_round16(f.width), 0, (int64_t)off};
+        off += sd_gray_bytes(f);
         *uniform = *uniform && f.width == frames[0].width && f.height == frames[0].height;
     }
     return off;
@@ -371,9 +373,9 @@ int upload_frames(sd_ctx* ctx, const sd_host_frame* frames, const sd_frame* desc
     for (int i = 0; i < n; ++i) {
         const sd_host_frame& f = frames[i];
         uint8_t* dst = f.channels == 3 ? bgr : d_gray + desc[i].offset;
-        const size_t pitch = f.channels == 3 ? round16(3 * (size_t)f.width) : (size_t)desc[i].row_stride;
+        const size_t pitch = f.channels == 3 ? sd_round16(3 * (size_t)f.width) : (size_t)desc[i].row_stride;
         if ((size_t)f.row_stride == pitch)
-            SD_CUDA(ctx, cudaMemcpyAsync(dst, f.h_data, host_frame_bytes(f), cudaMemcpyHostToDevice, ctx->copy_stream));
+            SD_CUDA(ctx, cudaMemcpyAsync(dst, f.h_data, sd_host_frame_bytes(f), cudaMemcpyHostToDevice, ctx->copy_stream));
         else
             SD_CUDA(ctx, cudaMemcpy2DAsync(dst, pitch, f.h_data, f.row_stride, (size_t)f.width * f.channels, f.height,
                                            cudaMemcpyHostToDevice, ctx->copy_stream));
@@ -385,7 +387,7 @@ int upload_frames(sd_ctx* ctx, const sd_host_frame* frames, const sd_frame* desc
     for (int i = 0; i < n; ++i) {
         const sd_host_frame& f = frames[i];
         if (f.channels != 3) continue;
-        const int rc = sd_bgr2gray(ctx, bgr, f.width, f.height, (int64_t)round16(3 * (size_t)f.width), 0, 1, d_gray + desc[i].offset,
+        const int rc = sd_bgr2gray(ctx, bgr, f.width, f.height, (int64_t)sd_round16(3 * (size_t)f.width), 0, 1, d_gray + desc[i].offset,
                                    desc[i].row_stride, 0);
         if (rc) return rc;
         bgr += bgr_bytes(f);
@@ -427,7 +429,7 @@ int detect_faces_full(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frame
     std::vector<int> chunk_first;                             // first upload of each chunk
     size_t used = 0, need = 0;
     for (size_t u = 0; u < fr.size(); ++u) {
-        const size_t b = gray_bytes(fr[u]) + bgr_bytes(fr[u]);
+        const size_t b = sd_gray_bytes(fr[u]) + bgr_bytes(fr[u]);
         if (chunk_first.empty() || used + b > chunk_cap) { chunk_first.push_back((int)u); used = 0; }
         used += b;
         need = used > need ? used : need;
@@ -458,7 +460,7 @@ int detect_faces_full(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frame
     std::vector<float> xs((size_t)count * P);
     for (int k = 0; k < count; ++k) memcpy(&xs[(size_t)k * P], x0 + (size_t)order[k] * P, P * sizeof(float));
     const size_t xbytes = (size_t)count * P * sizeof(float);
-    const size_t ibytes = round16((size_t)count * sizeof(int32_t));
+    const size_t ibytes = sd_round16((size_t)count * sizeof(int32_t));
     unsigned char* tab = (unsigned char*)sd_workspace(ctx, SD_WS_PARTIAL, 2 * xbytes + ibytes + up.size() * sizeof(sd_frame));
     if (!tab) return SD_ERR_CUDA;
     float* d_x = (float*)tab;
@@ -556,14 +558,8 @@ int detect_faces_roi(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frames
         const int first = chunk_first[c], n = chunk_first[c + 1] - first, ng = chunk_grey[c];
         SD_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_done[buf], 0));   // also orders the table uploads before the first gather
         // the SMs read the chunk's ROI rows zero-copy from the pinned frames: no host cores are spent packing rows at link speed
-        if (ng > 0) {
-            roi_gather_kernel<1><<<ng < 8 * ctx->sm_count ? ng : 8 * ctx->sm_count, 256, 0, ctx->copy_stream>>>(d_rec + first, ng, (uint8_t*)ctx->d_stage[buf]);
-            SD_LAUNCH_CHECK(ctx, "roi_gather_kernel<1>");
-        }
-        if (n - ng > 0) {
-            roi_gather_kernel<3><<<n - ng < 8 * ctx->sm_count ? n - ng : 8 * ctx->sm_count, 256, 0, ctx->copy_stream>>>(d_rec + first + ng, n - ng, (uint8_t*)ctx->d_stage[buf]);
-            SD_LAUNCH_CHECK(ctx, "roi_gather_kernel<3>");
-        }
+        rc = sd_roi_gather(ctx, d_rec + first, ng, d_rec + first + ng, n - ng, (uint8_t*)ctx->d_stage[buf], ctx->copy_stream);
+        if (rc) return rc;
         SD_CUDA(ctx, cudaEventRecord(ctx->stage_ev[buf], ctx->copy_stream));
         SD_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->stage_ev[buf], 0));
         sd_image_batch ib{};
@@ -877,7 +873,7 @@ int sd_detect_faces_host(sd_ctx* ctx, const sd_model* m, const sd_host_frame* fr
         used[h_face_frame[i]] = 1;
     }
     for (int f = 0; f < num_frames; ++f) {
-        const int rc = used[f] ? check_host_frame(ctx, __func__, frames[f], f) : SD_OK;
+        const int rc = used[f] ? sd_check_host_frame(ctx, __func__, frames[f], f) : SD_OK;
         if (rc) return rc;
     }
     const int L = m->num_landmarks, P = 2 * L;
@@ -896,7 +892,7 @@ int sd_detect_faces_host(sd_ctx* ctx, const sd_model* m, const sd_host_frame* fr
     bool roi = true;
     for (int f = 0; f < num_frames && roi; ++f) {
         if (!used[f]) continue;
-        mapped[f] = mapped_frame(frames[f].h_data, host_frame_bytes(frames[f]), last);
+        mapped[f] = sd_mapped_frame(frames[f].h_data, sd_host_frame_bytes(frames[f]), last);
         roi = mapped[f] && ((reinterpret_cast<uintptr_t>(mapped[f]) | (uintptr_t)frames[f].row_stride) & 15) == 0;
     }
     if (roi) return detect_faces_roi(ctx, m, frames, mapped, h_face_frame, num_faces, xs, h_landmarks);
@@ -923,7 +919,7 @@ int sd_upload_frames(sd_ctx* ctx, const sd_host_frame* frames, int count, void* 
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, frames && count >= 1 && bytes, "bad argument");
     for (int f = 0; f < count; ++f) {
-        const int rc = check_host_frame(ctx, __func__, frames[f], f);
+        const int rc = sd_check_host_frame(ctx, __func__, frames[f], f);
         if (rc) return rc;
     }
     std::vector<sd_frame> desc(count);

@@ -10,9 +10,13 @@
 // (solve_gram_impl) is exact for any shift -- it rebuilds the norm of the unshifted matrix from the shift, eliminates the bias
 // column first (the exact centring of any shifted Gram) and shifts the bias back.  With one chunk p IS the mean and the call
 // sequence is sd_train's one-shot sequence, kernel for kernel.
+//
+// sd_train_level_host / sd_apply_level_host run the same loop; only the HOG rows come from another source: frames that stay in
+// pinned host memory, gathered batch by batch (gather_hog_rows).
 #include "sd_internal.cuh"
 
 #include <climits>
+#include <cstring>
 
 namespace {
 
@@ -32,17 +36,404 @@ sd_image_batch batch_from(const sd_image_batch& b, int r0)
     return v;
 }
 
-// HOG rows of samples [r0, r0 + rows) into the chunk buffer
-int hog_rows(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int r0, int rows, int L,
-             const sd_normalisation* eyes, const sd_hog_param* p, float* d_chunk, int64_t ld)
+// ---- host frames: the training gather (DESIGN 4.6) ----------------------------------------------------------------------------
+// At the start of a level every sample's landmarks are known, so the window each of its patches reads is known exactly.  Per
+// gather batch, roi_plan_kernel merges the windows of a sample's L patches into the union slot of its frame, gather_layout_kernel
+// clips every touched union to its frame, lays the unions out back to back in one staging half and writes the gather records;
+// roi_gather_kernel pulls them over PCIe (samples of one frame in one batch share one region), and the unchanged HOG kernel reads
+// them through per-sample sd_roi records.  The window a sample's patch reads always lies in its frame's region: a region miss
+// is a bug, reported as such, never a retry.
+struct FrameDev {
+    const uint8_t* src;                   // device-mapped address of the frame's first pixel
+    int32_t width, height, row_stride, channels;
+};
+
+struct GatherTotals {
+    long long bytes;                      // grey bytes of the batch's regions in the staging half
+    long long pcie;                       // bytes read from host memory (x channels)
+    int n_grey, n_colour;                 // gather records of grey / colour frames
+};
+
+// The state of one host-frame level call (sd_train_level_host, sd_apply_level_host)
+struct HostGather {
+    const sd_host_frame* frames;
+    int num_frames;
+    const int32_t* d_sample_frame;
+    uint8_t* stage[2];
+    size_t half;                          // bytes of one staging half
+    // device tables (SD_WS_GATHER)
+    FrameDev* d_fr;
+    int2* d_lo;                           // per frame: union of the planned windows, min corner (INT_MAX = none) ...
+    int2* d_hi;                           // ... and max corner, exclusive
+    sd_roi* d_froi;                       // per frame: its region in the current batch
+    GatherRec* d_rec;                     // grey records [0, F), colour records [F, 2F)
+    sd_roi* d_roi;                        // per sample: its frame's region
+    sd_frame* d_dims;                     // per sample: its frame's size
+    uint8_t* d_miss;                      // per sample: a patch read outside the region (must never be raised)
+    GatherTotals* d_tot;
+    int guess = 0;                        // samples the next batch starts from (gather_hog_rows)
+    int buf = 0;
+};
+
+constexpr int kPlanThreads = 128;
+constexpr int kLayoutThreads = 1024;
+
+// frame of sample s, as the HOG kernel resolves an image index: an index out of range raises the status flag and reads frame 0
+__device__ __forceinline__ int sample_frame(const int32_t* __restrict__ idx, int s, int F, int* status)
+{
+    int f = idx[s];
+    if (f < 0 || f >= F) {
+        if (status) atomicOr(status, 2);
+        f = 0;
+    }
+    return f;
+}
+
+// One block per sample: the union of [cvRound(x_l) - half, cvRound(x_l) + half) over its L patches, merged into its frame's slot.
+__global__ void __launch_bounds__(kPlanThreads) roi_plan_kernel(const float* __restrict__ x, int L, const int32_t* __restrict__ idx,
+                                                                int F, const sd_eyes_dev eyes, float rel, int fixed_half,
+                                                                int2* __restrict__ lo, int2* __restrict__ hi, int* status)
+{
+    const int s = blockIdx.x;
+    const float* __restrict__ row = x + (long long)s * 2 * L;
+    __shared__ int s_half;
+    __shared__ int s_box[4][kPlanThreads / 32];
+    if (threadIdx.x == 0) {
+        bool degenerate;
+        s_half = sd_patch_half(row, L, eyes, rel, fixed_half, &degenerate);   // the HOG kernel flags a degenerate sample itself
+    }
+    __syncthreads();
+    int x0 = INT_MAX, y0 = INT_MAX, x1 = INT_MIN, y1 = INT_MIN;
+    for (int l = threadIdx.x; l < L; l += kPlanThreads) {
+        const int cx = __float2int_rn(row[l]), cy = __float2int_rn(row[l + L]);
+        x0 = min(x0, cx - s_half); y0 = min(y0, cy - s_half);
+        x1 = max(x1, cx + s_half); y1 = max(y1, cy + s_half);
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        x0 = min(x0, __shfl_xor_sync(0xffffffffu, x0, o)); y0 = min(y0, __shfl_xor_sync(0xffffffffu, y0, o));
+        x1 = max(x1, __shfl_xor_sync(0xffffffffu, x1, o)); y1 = max(y1, __shfl_xor_sync(0xffffffffu, y1, o));
+    }
+    const int w = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0) { s_box[0][w] = x0; s_box[1][w] = y0; s_box[2][w] = x1; s_box[3][w] = y1; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int k = 1; k < kPlanThreads / 32; ++k) {
+            x0 = min(x0, s_box[0][k]); y0 = min(y0, s_box[1][k]); x1 = max(x1, s_box[2][k]); y1 = max(y1, s_box[3][k]);
+        }
+        const int f = sample_frame(idx, s, F, status);
+        atomicMin(&lo[f].x, x0); atomicMin(&lo[f].y, y0);
+        atomicMax(&hi[f].x, x1); atomicMax(&hi[f].y, y1);
+    }
+}
+
+// One block over all frames: every touched union is clipped to its frame, its x aligned down to 16 pixels and its width bounded by
+// row_stride / channels (as detect's face_roi does), laid out at an exclusive scan of the region bytes, given a gather record, and
+// its slot emptied for the next batch.  Then each of the batch's n samples receives its frame's region and size.
+__global__ void __launch_bounds__(kLayoutThreads) gather_layout_kernel(const FrameDev* __restrict__ fr, int F, int2* __restrict__ lo,
+                                                                       int2* __restrict__ hi, sd_roi* __restrict__ froi,
+                                                                       GatherRec* __restrict__ rec, const int32_t* __restrict__ idx, int n,
+                                                                       sd_roi* __restrict__ roi, sd_frame* __restrict__ dims,
+                                                                       GatherTotals* __restrict__ tot)
+{
+    __shared__ long long s_scan[kLayoutThreads / 32];
+    __shared__ long long s_base, s_pcie;
+    __shared__ int s_ng, s_nc;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) { s_base = 0; s_pcie = 0; s_ng = 0; s_nc = 0; }
+    __syncthreads();
+    for (int f0 = 0; f0 < F; f0 += kLayoutThreads) {
+        const int f = f0 + tid;
+        long long bytes = 0;
+        sd_roi r{};
+        if (f < F) {
+            const int2 a = lo[f], b = hi[f];
+            if (a.x <= b.x) {                                  // touched by this batch
+                lo[f] = make_int2(INT_MAX, INT_MAX);
+                hi[f] = make_int2(INT_MIN, INT_MIN);
+                const FrameDev d = fr[f];
+                const int xa = max(a.x, 0), ya = max(a.y, 0), xb = min(b.x, d.width), yb = min(b.y, d.height);
+                if (xa < xb && ya < yb) {                      // otherwise every patch lies outside the frame: zeros, no pixel read
+                    r.x = xa & ~15;
+                    int w = (xb - r.x + 15) & ~15;
+                    const int maxw = (d.row_stride / d.channels - r.x) & ~15;
+                    r.w = w < maxw ? w : maxw;
+                    r.y = ya;
+                    r.h = yb - ya;
+                    r.row_stride = r.w;
+                    bytes = (long long)r.w * r.h;
+                }
+            }
+        }
+        // block-wide exclusive scan of the region bytes
+        long long v = bytes;
+        for (int o = 1; o < 32; o <<= 1) {
+            const long long t = __shfl_up_sync(0xffffffffu, v, o);
+            if (lane >= o) v += t;
+        }
+        if (lane == 31) s_scan[warp] = v;
+        __syncthreads();
+        if (warp == 0) {
+            long long w = lane < kLayoutThreads / 32 ? s_scan[lane] : 0;
+            for (int o = 1; o < 32; o <<= 1) {
+                const long long t = __shfl_up_sync(0xffffffffu, w, o);
+                if (lane >= o) w += t;
+            }
+            if (lane < kLayoutThreads / 32) s_scan[lane] = w;   // inclusive per warp
+        }
+        __syncthreads();
+        const long long excl = s_base + (warp > 0 ? s_scan[warp - 1] : 0) + v - bytes;
+        if (f < F) {
+            r.offset = excl;
+            froi[f] = r;
+            if (bytes > 0) {
+                const FrameDev d = fr[f];
+                const int k = d.channels == 1 ? atomicAdd(&s_ng, 1) : F + atomicAdd(&s_nc, 1);
+                rec[k] = GatherRec{d.src + (long long)r.y * d.row_stride + (long long)r.x * d.channels, d.row_stride, excl, r.w >> 4, r.h};
+                atomicAdd((unsigned long long*)&s_pcie, (unsigned long long)(bytes * d.channels));
+            }
+        }
+        __syncthreads();
+        if (tid == 0) s_base += s_scan[kLayoutThreads / 32 - 1];
+        __syncthreads();
+    }
+    for (int s = tid; s < n; s += kLayoutThreads) {
+        const int f = sample_frame(idx, s, F, nullptr);        // roi_plan_kernel has flagged a bad index
+        roi[s] = froi[f];
+        dims[s] = sd_frame{fr[f].width, fr[f].height, 0, 0, 0};
+    }
+    if (tid == 0) *tot = GatherTotals{s_base, s_pcie, s_ng, s_nc};
+}
+
+// Checks the frames and the staging buffer (SD_ERR_INVALID before any work is queued) and sets up the device tables.
+int gather_prepare(sd_ctx* ctx, HostGather& g, int N, void* d_stage, size_t stage_bytes)
+{
+    const int F = g.num_frames;
+    SD_REQUIRE(ctx, g.frames && F >= 1 && g.d_sample_frame && d_stage, "null frames, sample -> frame index or staging buffer");
+    SD_REQUIRE(ctx, (reinterpret_cast<uintptr_t>(d_stage) & 15) == 0, "d_stage must be 16-byte aligned");
+    // the frames the samples refer to (an index out of range reads frame 0 and is reported by the projection's status flag)
+    std::vector<int32_t> idx(N);
+    if (N > 0) {
+        SD_CUDA(ctx, cudaMemcpyAsync(idx.data(), g.d_sample_frame, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+        SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    }
+    std::vector<char> used(F, 0);
+    for (int s = 0; s < N; ++s) used[idx[s] >= 0 && idx[s] < F ? idx[s] : 0] = 1;
+    std::vector<FrameDev> fr(F);
+    PinnedRange last;
+    size_t largest = 0;
+    for (int f = 0; f < F; ++f) {
+        if (!used[f]) { fr[f] = FrameDev{nullptr, 1, 1, 16, 1}; continue; }
+        const sd_host_frame& h = g.frames[f];
+        int rc = sd_check_host_frame(ctx, __func__, h, f);
+        if (rc) return rc;
+        const uint8_t* m = sd_mapped_frame(h.h_data, sd_host_frame_bytes(h), last);
+        if (!m || ((reinterpret_cast<uintptr_t>(m) | (uintptr_t)h.row_stride) & 15))
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d is not pinned and device-mapped with a 16-byte aligned base and row_stride", __func__, f);
+        // the gather moves 16 pixels at a time: every 16-pixel step of a row must lie inside the row
+        if ((size_t)h.row_stride < (size_t)h.channels * sd_round16(h.width))
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d: row_stride < channels * (width rounded up to 16)", __func__, f);
+        fr[f] = FrameDev{m, h.width, h.height, h.row_stride, h.channels};
+        largest = sd_gray_bytes(h) > largest ? sd_gray_bytes(h) : largest;
+    }
+    g.half = (stage_bytes / 2) & ~(size_t)15;
+    if (g.half < largest)
+        return sd_fail(ctx, SD_ERR_INVALID, "%s: a staging half of %zu bytes is smaller than the largest frame a sample refers to (%zu grey bytes)",
+                       __func__, g.half, largest);
+    g.stage[0] = static_cast<uint8_t*>(d_stage);
+    g.stage[1] = g.stage[0] + g.half;
+    // device tables
+    const size_t n = N > 0 ? N : 1;
+    const size_t b_fr = sd_round16(F * sizeof(FrameDev)), b_lo = sd_round16(F * sizeof(int2)), b_froi = sd_round16(F * sizeof(sd_roi));
+    const size_t b_rec = sd_round16(2 * F * sizeof(GatherRec)), b_roi = sd_round16(n * sizeof(sd_roi)), b_dims = sd_round16(n * sizeof(sd_frame));
+    uint8_t* t = (uint8_t*)sd_workspace(ctx, SD_WS_GATHER, b_fr + 2 * b_lo + b_froi + b_rec + b_roi + b_dims + sd_round16(n) + sizeof(GatherTotals));
+    if (!t) return SD_ERR_CUDA;
+    g.d_fr = (FrameDev*)t;                      t += b_fr;
+    g.d_lo = (int2*)t;                          t += b_lo;
+    g.d_hi = (int2*)t;                          t += b_lo;
+    g.d_froi = (sd_roi*)t;                      t += b_froi;
+    g.d_rec = (GatherRec*)t;                    t += b_rec;
+    g.d_roi = (sd_roi*)t;                       t += b_roi;
+    g.d_dims = (sd_frame*)t;                    t += b_dims;
+    g.d_miss = t;                               t += sd_round16(n);
+    g.d_tot = (GatherTotals*)t;
+    SD_CUDA(ctx, cudaMemcpyAsync(g.d_fr, fr.data(), F * sizeof(FrameDev), cudaMemcpyHostToDevice, ctx->stream));
+    SD_CUDA(ctx, cudaMemsetAsync(g.d_lo, 0x7f, F * sizeof(int2), ctx->stream));          // 0x7f7f7f7f: above any coordinate
+    SD_CUDA(ctx, cudaMemsetAsync(g.d_hi, 0x80, F * sizeof(int2), ctx->stream));          // 0x80808080: below any coordinate
+    SD_CUDA(ctx, cudaMemsetAsync(g.d_miss, 0, n, ctx->stream));
+    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));                                      // fr goes out of scope
+    g.guess = N > 0 ? N : 1;
+    return SD_OK;
+}
+
+// A patch that read outside its planned region would mean rows computed from a partial window: fail the call.
+int gather_finish(sd_ctx* ctx, const HostGather& g, int N)
+{
+    if (N == 0) return SD_OK;
+    std::vector<uint8_t> miss(N);
+    SD_CUDA(ctx, cudaMemcpyAsync(miss.data(), g.d_miss, N, cudaMemcpyDeviceToHost, ctx->stream));
+    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    for (int s = 0; s < N; ++s)
+        if (miss[s]) return sd_fail(ctx, SD_ERR_CUDA, "internal error: sample %d read a pixel outside its planned gather region", s);
+    return SD_OK;
+}
+
+// HOG rows of samples [r0, r0 + rows) from host frames, in gather batches that fit one staging half: plan, layout and gather on
+// the copy stream (the gather of batch k+1 runs while the HOG of batch k does), HOG on the compute stream.
+int gather_hog_rows(sd_ctx* ctx, HostGather& g, const float* d_x, int r0, int rows, int L, const sd_normalisation* eyes,
+                    const sd_hog_param* p, float* d_chunk, int64_t ld)
 {
     const int P = 2 * L;
-    const sd_image_batch view = d_image_index ? *images : batch_from(*images, r0);
-    return sd_hog_batch(ctx, &view, d_image_index ? d_image_index + r0 : nullptr, d_x + (int64_t)r0 * P, P, rows, L, eyes, p,
+    const bool fixed = !eyes || eyes->kind == 0;
+    sd_eyes_dev eyes_dev;
+    memset(&eyes_dev, 0, sizeof(eyes_dev));
+    int rc = fixed ? SD_OK : sd_eyes_to_dev(ctx, eyes, L, &eyes_dev);
+    if (rc) return rc;
+    const int fixed_half = fixed ? p->num_cells * (p->cell_size / 2) : 0;
+    int* status = reinterpret_cast<int*>(ctx->d_scratch) + 1;
+    // the copy stream starts after everything queued so far on the compute stream: the landmarks, and every earlier reader of the
+    // per-sample tables and of both staging halves
+    SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[0], ctx->stream));
+    SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[1], ctx->stream));
+    SD_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_done[0], 0));
+    for (int b0 = 0; b0 < rows;) {
+        const int s0 = r0 + b0;
+        int nb = g.guess < rows - b0 ? g.guess : rows - b0;
+        GatherTotals t;
+        for (;;) {
+            roi_plan_kernel<<<nb, kPlanThreads, 0, ctx->copy_stream>>>(d_x + (int64_t)s0 * P, L, g.d_sample_frame + s0, g.num_frames, eyes_dev,
+                                                                       p->relative_patch_size, fixed_half, g.d_lo, g.d_hi, status);
+            SD_LAUNCH_CHECK(ctx, "roi_plan_kernel");
+            gather_layout_kernel<<<1, kLayoutThreads, 0, ctx->copy_stream>>>(g.d_fr, g.num_frames, g.d_lo, g.d_hi, g.d_froi, g.d_rec,
+                                                                            g.d_sample_frame + s0, nb, g.d_roi + s0, g.d_dims + s0, g.d_tot);
+            SD_LAUNCH_CHECK(ctx, "gather_layout_kernel");
+            SD_CUDA(ctx, cudaMemcpyAsync(&t, g.d_tot, sizeof(t), cudaMemcpyDeviceToHost, ctx->copy_stream));
+            SD_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
+            if ((size_t)t.bytes <= g.half) break;
+            // too large for one staging half: fewer samples (one always fits: no region exceeds its frame's grey bytes)
+            const int scaled = (int)((double)nb * (double)g.half / (double)t.bytes * 0.9);
+            nb = scaled < nb - 1 ? (scaled > 1 ? scaled : 1) : nb - 1;
+        }
+        // the next batch starts from this size, twice it when this one filled less than half a staging half
+        g.guess = (size_t)t.bytes * 2 <= g.half && nb <= INT_MAX / 2 ? 2 * nb : nb;
+        const int buf = g.buf;
+        g.buf ^= 1;
+        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_done[buf], 0));   // the HOG that last read this half is done
+        rc = sd_roi_gather(ctx, g.d_rec, t.n_grey, g.d_rec + g.num_frames, t.n_colour, g.stage[buf], ctx->copy_stream);
+        if (rc) return rc;
+        SD_CUDA(ctx, cudaEventRecord(ctx->stage_ev[buf], ctx->copy_stream));
+        SD_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->stage_ev[buf], 0));
+        sd_image_batch ib{};
+        ib.d_data = g.stage[buf];
+        ib.count = nb;
+        ib.d_roi = g.d_roi + s0;
+        ib.d_roi_miss = g.d_miss + s0;
+        ib.d_frames = g.d_dims + s0;
+        rc = sd_hog_batch(ctx, &ib, nullptr, d_x + (int64_t)s0 * P, P, nb, L, eyes, p, d_chunk + (int64_t)b0 * ld, ld);
+        if (rc) return rc;
+        SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[buf], ctx->stream));
+        ctx->gathered_bytes += t.pcie;
+        b0 += nb;
+    }
+    return SD_OK;
+}
+
+// Where a level's HOG rows come from: frames resident on the device (images, d_image_index) or host frames (host).
+struct HogSource {
+    const sd_image_batch* images;
+    const int32_t* d_image_index;
+    HostGather* host;
+};
+
+// HOG rows of samples [r0, r0 + rows) into the chunk buffer
+int hog_rows(sd_ctx* ctx, const HogSource& src, const float* d_x, int r0, int rows, int L, const sd_normalisation* eyes,
+             const sd_hog_param* p, float* d_chunk, int64_t ld)
+{
+    if (src.host) return gather_hog_rows(ctx, *src.host, d_x, r0, rows, L, eyes, p, d_chunk, ld);
+    const int P = 2 * L;
+    const sd_image_batch view = src.d_image_index ? *src.images : batch_from(*src.images, r0);
+    return sd_hog_batch(ctx, &view, src.d_image_index ? src.d_image_index + r0 : nullptr, d_x + (int64_t)r0 * P, P, rows, L, eyes, p,
                         d_chunk, ld);
 }
 
 size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
+
+// superviseddescent.hpp:173-217 for either source of HOG rows (see sd_train_level)
+int train_level(sd_ctx* ctx, sd_comm* comm, const HogSource& src, const float* d_x, const float* d_x_gt, int N_local, int L,
+                int64_t n_global, const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
+                const float* d_templates, int64_t ldt, const sd_regulariser* reg, int route, float* d_chunk, int64_t ld, int chunk_rows,
+                float* d_X, float* d_x_next, float* lambda_out, void* d_stage, size_t stage_bytes)
+{
+    SD_REQUIRE(ctx, d_x && d_x_gt && p && reg && d_chunk && d_X && d_x_next, "null argument");
+    SD_REQUIRE(ctx, N_local >= 0 && L >= 1 && n_global >= 1 && n_global <= INT_MAX, "bad sample / landmark count");
+    SD_REQUIRE(ctx, chunk_rows >= 1, "chunk_rows must be >= 1");
+    SD_REQUIRE(ctx, reg->type == 0 || reg->type == 1, "unknown regularisation type");
+    const int D = sd_hog_feature_length(L, p), P = 2 * L;
+    SD_REQUIRE(ctx, D >= 2, "bad HOG parameters");
+    SD_REQUIRE(ctx, ld >= (int64_t)D + P, "ld < D + 2L");
+    SD_REQUIRE(ctx, !d_templates || (chunk_rows >= N_local && ldt >= D), "templates need one chunk (chunk_rows >= N_local) and ldt >= D");
+    SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
+    int rc = src.host ? gather_prepare(ctx, *src.host, N_local, d_stage, stage_bytes) : SD_OK;
+    if (rc) return rc;
+    float* mu = (float*)sd_workspace(ctx, SD_WS_LEVEL, (size_t)D * (P + 1) * sizeof(float));
+    if (!mu) return SD_ERR_CUDA;
+    float* Xc = mu + D;                                   // weights for the shifted rows: what the update multiplies them with
+    sd_comm* c = sd_comm_size_of(comm) > 1 ? comm : nullptr;
+    float* B = d_chunk + D;                               // [A | b] side by side: the Gram reads both in one pass
+    const int chunks = N_local > 0 ? sd_div_up(N_local, chunk_rows) : 1;
+    // the pilot shift is the mean of every rank's first chunk (sd_centre_features also checks the all-ones bias column there)
+    int64_t n0 = N_local < chunk_rows ? N_local : chunk_rows;
+    rc = c ? sd_comm_sum_int64(ctx, c, &n0) : SD_OK;
+    if (rc) return rc;
+    if (n0 < 1) return sd_fail(ctx, SD_ERR_INVALID, "sd_train_level: no samples on any rank");
+    const bool shifted = D > SD_LU_MAX_DIM && !reg->regularise_last_row;     // otherwise sd_centre_features leaves mu = 0
+    for (int k = 0; k < chunks; ++k) {
+        const int r0 = k * chunk_rows, rows = N_local - r0 < chunk_rows ? N_local - r0 : chunk_rows;
+        rc = hog_rows(ctx, src, d_x, r0, rows, L, hog_eyes, p, d_chunk, ld);                                           // :173-189
+        if (!rc && d_templates) rc = sd_subtract_templates(ctx, d_chunk, ld, d_templates, ldt, rows, D);             // :191-197
+        if (!rc) rc = sd_cascade_targets(ctx, d_x + (int64_t)r0 * P, d_x_gt + (int64_t)r0 * P, rows, P, norm, B, ld); // :199-205
+        if (!rc) rc = k == 0 ? sd_centre_features(ctx, c, d_chunk, ld, rows, D, (int)n0, reg, mu)
+                             : (shifted ? sd_shift_rows(ctx, d_chunk, ld, rows, D, mu) : SD_OK);
+        if (!rc) rc = sd_learn_gram(ctx, d_chunk, ld, B, ld, rows, true, D, P, k > 0);
+        if (rc) return rc;
+    }
+    rc = sd_learn_centred_solve(ctx, c, D, P, reg, (int)n_global, route, mu, d_X, Xc, lambda_out);                    // :207
+    if (rc) return rc;
+    // :209-215 -- the last chunk is still in the buffer; the others are projected and shifted again
+    const int last = (chunks - 1) * chunk_rows;
+    rc = sd_cascade_update(ctx, d_chunk, ld, N_local - last, D, Xc, P, d_x + (int64_t)last * P, norm, d_x_next + (int64_t)last * P);
+    for (int k = 0; !rc && k + 1 < chunks; ++k) {
+        const int r0 = k * chunk_rows;
+        rc = hog_rows(ctx, src, d_x, r0, chunk_rows, L, hog_eyes, p, d_chunk, ld);
+        if (!rc && shifted) rc = sd_shift_rows(ctx, d_chunk, ld, chunk_rows, D, mu);
+        if (!rc) rc = sd_cascade_update(ctx, d_chunk, ld, chunk_rows, D, Xc, P, d_x + (int64_t)r0 * P, norm, d_x_next + (int64_t)r0 * P);
+    }
+    if (!rc && src.host) rc = gather_finish(ctx, *src.host, N_local);
+    return rc;
+}
+
+// superviseddescent.hpp:262-306, 323-344 for either source of HOG rows (see sd_apply_level)
+int apply_level(sd_ctx* ctx, const HogSource& src, const float* d_x, int N, int L, const sd_normalisation* hog_eyes,
+                const sd_hog_param* p, const sd_normalisation* norm, const float* d_templates, int64_t ldt, const float* d_X,
+                float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next, void* d_stage, size_t stage_bytes)
+{
+    SD_REQUIRE(ctx, d_x && p && d_X && d_chunk && d_x_next, "null argument");
+    SD_REQUIRE(ctx, N >= 0 && L >= 1, "bad sample / landmark count");
+    SD_REQUIRE(ctx, chunk_rows >= 1, "chunk_rows must be >= 1");
+    const int D = sd_hog_feature_length(L, p), P = 2 * L;
+    SD_REQUIRE(ctx, D >= 2, "bad HOG parameters");
+    SD_REQUIRE(ctx, ld >= D, "ld < D");
+    SD_REQUIRE(ctx, !d_templates || ldt >= D, "ldt < D");
+    SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
+    int rc = src.host ? gather_prepare(ctx, *src.host, N, d_stage, stage_bytes) : SD_OK;
+    for (int r0 = 0; !rc && r0 < N; r0 += chunk_rows) {
+        const int rows = N - r0 < chunk_rows ? N - r0 : chunk_rows;
+        rc = hog_rows(ctx, src, d_x, r0, rows, L, hog_eyes, p, d_chunk, ld);
+        if (!rc && d_templates) rc = sd_subtract_templates(ctx, d_chunk, ld, d_templates + (int64_t)r0 * ldt, ldt, rows, D);
+        if (!rc) rc = sd_cascade_update(ctx, d_chunk, ld, rows, D, d_X, P, d_x + (int64_t)r0 * P, norm, d_x_next + (int64_t)r0 * P);
+    }
+    if (!rc && src.host) rc = gather_finish(ctx, *src.host, N);
+    return rc;
+}
 
 }  // namespace
 
@@ -95,49 +486,21 @@ int sd_train_level(sd_ctx* ctx, sd_comm* comm, const sd_image_batch* images, con
                    float* d_chunk, int64_t ld, int chunk_rows, float* d_X, float* d_x_next, float* lambda_out)
 {
     if (!ctx) return SD_ERR_INVALID;
-    SD_REQUIRE(ctx, images && d_x && d_x_gt && p && reg && d_chunk && d_X && d_x_next, "null argument");
-    SD_REQUIRE(ctx, N_local >= 0 && L >= 1 && n_global >= 1 && n_global <= INT_MAX, "bad sample / landmark count");
-    SD_REQUIRE(ctx, chunk_rows >= 1, "chunk_rows must be >= 1");
-    SD_REQUIRE(ctx, reg->type == 0 || reg->type == 1, "unknown regularisation type");
-    const int D = sd_hog_feature_length(L, p), P = 2 * L;
-    SD_REQUIRE(ctx, D >= 2, "bad HOG parameters");
-    SD_REQUIRE(ctx, ld >= (int64_t)D + P, "ld < D + 2L");
-    SD_REQUIRE(ctx, !d_templates || (chunk_rows >= N_local && ldt >= D), "templates need one chunk (chunk_rows >= N_local) and ldt >= D");
-    SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
-    float* mu = (float*)sd_workspace(ctx, SD_WS_LEVEL, (size_t)D * (P + 1) * sizeof(float));
-    if (!mu) return SD_ERR_CUDA;
-    float* Xc = mu + D;                                   // weights for the shifted rows: what the update multiplies them with
-    sd_comm* c = sd_comm_size_of(comm) > 1 ? comm : nullptr;
-    float* B = d_chunk + D;                               // [A | b] side by side: the Gram reads both in one pass
-    const int chunks = N_local > 0 ? sd_div_up(N_local, chunk_rows) : 1;
-    // the pilot shift is the mean of every rank's first chunk (sd_centre_features also checks the all-ones bias column there)
-    int64_t n0 = N_local < chunk_rows ? N_local : chunk_rows;
-    int rc = c ? sd_comm_sum_int64(ctx, c, &n0) : SD_OK;
-    if (rc) return rc;
-    if (n0 < 1) return sd_fail(ctx, SD_ERR_INVALID, "sd_train_level: no samples on any rank");
-    const bool shifted = D > SD_LU_MAX_DIM && !reg->regularise_last_row;     // otherwise sd_centre_features leaves mu = 0
-    for (int k = 0; k < chunks; ++k) {
-        const int r0 = k * chunk_rows, rows = N_local - r0 < chunk_rows ? N_local - r0 : chunk_rows;
-        rc = hog_rows(ctx, images, d_image_index, d_x, r0, rows, L, hog_eyes, p, d_chunk, ld);                         // :173-189
-        if (!rc && d_templates) rc = sd_subtract_templates(ctx, d_chunk, ld, d_templates, ldt, rows, D);             // :191-197
-        if (!rc) rc = sd_cascade_targets(ctx, d_x + (int64_t)r0 * P, d_x_gt + (int64_t)r0 * P, rows, P, norm, B, ld); // :199-205
-        if (!rc) rc = k == 0 ? sd_centre_features(ctx, c, d_chunk, ld, rows, D, (int)n0, reg, mu)
-                             : (shifted ? sd_shift_rows(ctx, d_chunk, ld, rows, D, mu) : SD_OK);
-        if (!rc) rc = sd_learn_gram(ctx, d_chunk, ld, B, ld, rows, true, D, P, k > 0);
-        if (rc) return rc;
-    }
-    rc = sd_learn_centred_solve(ctx, c, D, P, reg, (int)n_global, route, mu, d_X, Xc, lambda_out);                    // :207
-    if (rc) return rc;
-    // :209-215 -- the last chunk is still in the buffer; the others are projected and shifted again
-    const int last = (chunks - 1) * chunk_rows;
-    rc = sd_cascade_update(ctx, d_chunk, ld, N_local - last, D, Xc, P, d_x + (int64_t)last * P, norm, d_x_next + (int64_t)last * P);
-    for (int k = 0; !rc && k + 1 < chunks; ++k) {
-        const int r0 = k * chunk_rows;
-        rc = hog_rows(ctx, images, d_image_index, d_x, r0, chunk_rows, L, hog_eyes, p, d_chunk, ld);
-        if (!rc && shifted) rc = sd_shift_rows(ctx, d_chunk, ld, chunk_rows, D, mu);
-        if (!rc) rc = sd_cascade_update(ctx, d_chunk, ld, chunk_rows, D, Xc, P, d_x + (int64_t)r0 * P, norm, d_x_next + (int64_t)r0 * P);
-    }
-    return rc;
+    SD_REQUIRE(ctx, images, "null argument");
+    return train_level(ctx, comm, HogSource{images, d_image_index, nullptr}, d_x, d_x_gt, N_local, L, n_global, hog_eyes, p, norm,
+                       d_templates, ldt, reg, route, d_chunk, ld, chunk_rows, d_X, d_x_next, lambda_out, nullptr, 0);
+}
+
+int sd_train_level_host(sd_ctx* ctx, sd_comm* comm, const sd_host_frame* frames, int num_frames, const int32_t* d_sample_frame,
+                        const float* d_x, const float* d_x_gt, int N_local, int L, int64_t n_global, const sd_normalisation* hog_eyes,
+                        const sd_hog_param* p, const sd_normalisation* norm, const float* d_templates, int64_t ldt,
+                        const sd_regulariser* reg, int route, float* d_chunk, int64_t ld, int chunk_rows, void* d_stage,
+                        size_t stage_bytes, float* d_X, float* d_x_next, float* lambda_out)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    HostGather g{frames, num_frames, d_sample_frame};
+    return train_level(ctx, comm, HogSource{nullptr, nullptr, &g}, d_x, d_x_gt, N_local, L, n_global, hog_eyes, p, norm, d_templates,
+                       ldt, reg, route, d_chunk, ld, chunk_rows, d_X, d_x_next, lambda_out, d_stage, stage_bytes);
 }
 
 int sd_apply_level(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int N, int L,
@@ -145,22 +508,44 @@ int sd_apply_level(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_i
                    int64_t ldt, const float* d_X, float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next)
 {
     if (!ctx) return SD_ERR_INVALID;
-    SD_REQUIRE(ctx, images && d_x && p && d_X && d_chunk && d_x_next, "null argument");
-    SD_REQUIRE(ctx, N >= 0 && L >= 1, "bad sample / landmark count");
-    SD_REQUIRE(ctx, chunk_rows >= 1, "chunk_rows must be >= 1");
-    const int D = sd_hog_feature_length(L, p), P = 2 * L;
-    SD_REQUIRE(ctx, D >= 2, "bad HOG parameters");
-    SD_REQUIRE(ctx, ld >= D, "ld < D");
-    SD_REQUIRE(ctx, !d_templates || ldt >= D, "ldt < D");
-    SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
-    int rc = SD_OK;
-    for (int r0 = 0; !rc && r0 < N; r0 += chunk_rows) {
-        const int rows = N - r0 < chunk_rows ? N - r0 : chunk_rows;
-        rc = hog_rows(ctx, images, d_image_index, d_x, r0, rows, L, hog_eyes, p, d_chunk, ld);
-        if (!rc && d_templates) rc = sd_subtract_templates(ctx, d_chunk, ld, d_templates + (int64_t)r0 * ldt, ldt, rows, D);
-        if (!rc) rc = sd_cascade_update(ctx, d_chunk, ld, rows, D, d_X, P, d_x + (int64_t)r0 * P, norm, d_x_next + (int64_t)r0 * P);
-    }
-    return rc;
+    SD_REQUIRE(ctx, images, "null argument");
+    return apply_level(ctx, HogSource{images, d_image_index, nullptr}, d_x, N, L, hog_eyes, p, norm, d_templates, ldt, d_X, d_chunk, ld,
+                       chunk_rows, d_x_next, nullptr, 0);
+}
+
+int sd_apply_level_host(sd_ctx* ctx, const sd_host_frame* frames, int num_frames, const int32_t* d_sample_frame, const float* d_x, int N,
+                        int L, const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
+                        const float* d_templates, int64_t ldt, const float* d_X, float* d_chunk, int64_t ld, int chunk_rows, void* d_stage,
+                        size_t stage_bytes, float* d_x_next)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    HostGather g{frames, num_frames, d_sample_frame};
+    return apply_level(ctx, HogSource{nullptr, nullptr, &g}, d_x, N, L, hog_eyes, p, norm, d_templates, ldt, d_X, d_chunk, ld, chunk_rows,
+                       d_x_next, d_stage, stage_bytes);
+}
+
+int64_t sd_gathered_bytes(const sd_ctx* ctx) { return ctx ? ctx->gathered_bytes : 0; }
+
+int sd_host_frame_in_place(sd_ctx* ctx, const sd_host_frame* frame, int* in_place)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, frame && in_place, "null argument");
+    const int rc = sd_check_host_frame(ctx, __func__, *frame, 0);
+    if (rc) return rc;
+    PinnedRange last;
+    const uint8_t* m = sd_mapped_frame(frame->h_data, sd_host_frame_bytes(*frame), last);
+    *in_place = m && ((reinterpret_cast<uintptr_t>(m) | (uintptr_t)frame->row_stride) & 15) == 0 &&
+                (size_t)frame->row_stride >= (size_t)frame->channels * sd_round16(frame->width);
+    return SD_OK;
+}
+
+int sd_device_memory(sd_ctx* ctx, size_t* free_bytes, size_t* total_bytes)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, free_bytes && total_bytes, "null argument");
+    SD_CUDA(ctx, cudaSetDevice(ctx->device));
+    SD_CUDA(ctx, cudaMemGetInfo(free_bytes, total_bytes));
+    return SD_OK;
 }
 
 }  // extern "C"

@@ -3,11 +3,15 @@
 //     cv::Mat operator()(cv::Mat parameters, size_t regressorLevel, int trainingIndex = 0)
 // (one sample, used by predict(), superviseddescent.hpp:332) and exposes its device images, eyes and per-level
 // HOG parameters, with which the optimiser projects ALL samples of a level on the device (sd_train_level,
-// sd_apply_level).  The images are uploaded to HBM once, on first use; crop / resize / HOG run in sd_hog_batch (sm_90a).
+// sd_apply_level, or their _host twins when the frames do not fit on the device).  Each distinct image is held once: uploaded to HBM
+// on first use, or kept in host memory; crop / resize / HOG run in sd_hog_batch (sm_90a).
 #pragma once
 
+#include <cstring>
+#include <map>
 #include <memory>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "rcr/helpers.hpp"
@@ -44,22 +48,74 @@ public:
     cv::Mat operator()(cv::Mat parameters, size_t regressorLevel, int trainingIndex = 0)
     {
         sd_ctx* ctx = sd_b200::context();
-        ensure_uploaded();
+        const sd_image_batch& batch = device_batch();
         const int D = feature_length(regressorLevel);
         sd_b200::DeviceBuffer dx, dA(static_cast<size_t>(D) * sizeof(float)), didx(sizeof(int32_t));
         sd_b200::upload(parameters, dx, parameters.cols);
-        const int32_t idx = trainingIndex;
+        // an index outside images stays out of range, and the projection reports it
+        const int32_t idx = trainingIndex >= 0 && trainingIndex < static_cast<int>(dev->frame_of.size()) ? dev->frame_of[trainingIndex] : -1;
         sd_b200::check(ctx, sd_memcpy_h2d(ctx, didx.as<int32_t>(), &idx, sizeof(idx)), "HogTransform");
-        launch(dx.as<float>(), parameters.cols, 1, regressorLevel, dA.as<float>(), D, didx.as<int32_t>());
+        const sd_normalisation nrm = eyes();
+        const sd_hog_param p = hog_params[regressorLevel].c();
+        sd_b200::check(ctx, sd_hog_batch(ctx, &batch, didx.as<int32_t>(), dx.as<float>(), parameters.cols, 1, static_cast<int>(modelLandmarksList.size()),
+                                         &nrm, &p, dA.as<float>(), D), "sd_hog_batch");
         return sd_b200::download(dA.as<float>(), 1, D, D);
     }
 
-    // What the optimiser's device route hands to sd_train_level / sd_apply_level: the images resident on the device (uploaded
-    // on first use; sample i reads image i), the eye landmarks (eyes()) and the HOG parameters of a level.
+    // The route, chosen once on first use: the distinct frames are uploaded when their grey bytes fit in device_frame_share() of
+    // the free device memory; otherwise they stay in host memory and the optimiser's train() / test() read them level by level
+    // (sd_train_level_host / sd_apply_level_host).  Uploaded frames are copied when the transform is first used; frames kept on the
+    // host are read in place at every level when they are pinned and aligned (sd_host_frame_in_place), and copied once into one
+    // pinned buffer otherwise.
+    static double& device_frame_share()
+    {
+        static double share = 0.5;
+        return share;
+    }
+    bool on_device()
+    {
+        ensure_ready();
+        return !dev->host;
+    }
+
+    // What the optimiser hands to sd_train_level / sd_apply_level on the device route: the distinct images resident on the device
+    // (uploaded on first use), the sample -> image index (device_sample_frame), the eye landmarks (eyes()) and the HOG parameters of
+    // a level.
     const sd_image_batch& device_batch()
     {
-        ensure_uploaded();
+        ensure_ready();
+        if (dev->host) throw std::runtime_error("HogTransform: the frames stay in host memory (they do not fit on the device); only the optimiser's train() / test() / predict() read them");
         return dev->batch;
+    }
+    // On the host route: the distinct frames for sd_train_level_host / sd_apply_level_host, and the size of the staging buffer they
+    // need (two halves of at least 48 MB, and of the largest frame's grey bytes)
+    const std::vector<sd_host_frame>& host_frames()
+    {
+        ensure_ready();
+        return dev->frames;
+    }
+    size_t stage_bytes()
+    {
+        size_t half = static_cast<size_t>(48) << 20;
+        for (const sd_host_frame& f : host_frames()) {
+            const size_t grey = static_cast<size_t>(f.height) * ((static_cast<size_t>(f.width) + 15) / 16 * 16);
+            half = grey > half ? grey : half;
+        }
+        return 2 * half;
+    }
+    // Device index of n samples: sample i reads distinct frame device_sample_frame(n)[i], the frame of images[i].  Entries of
+    // `images` with equal data, size and step (rcr-train's shallow copies of one photo) are one frame, held once.
+    const int32_t* device_sample_frame(int n)
+    {
+        ensure_ready();
+        if (n > static_cast<int>(images.size())) throw std::runtime_error("HogTransform: more samples than images");
+        return dev->index.as<int32_t>();
+    }
+    // number of distinct frames
+    int num_frames()
+    {
+        ensure_ready();
+        return static_cast<int>(dev->frames.size());
     }
     sd_hog_param hog_param(size_t level) const { return hog_params[level].c(); }
 
@@ -79,33 +135,74 @@ public:
 
 private:
     struct DeviceImages {
-        sd_b200::DeviceBuffer buf;
+        std::vector<sd_host_frame> frames;   // the distinct frames (on the host route: where the levels read them)
+        std::vector<int32_t> frame_of;        // images[i] -> distinct frame
+        sd_b200::DeviceBuffer index;          // frame_of on the device
+        sd_b200::DeviceBuffer buf;            // device route: the grey frames
         sd_image_batch batch{};
+        sd_b200::HostBuffer packed;           // host route: the frames that could not be read in place
+        bool host = false;
         bool ready = false;
     };
 
-    // frames of any sizes (the reference's std::vector<cv::Mat>), grey or colour: colour is converted once here, where the
-    // reference converts it in every call (adaptive_vlhog.hpp:114-120)
-    void ensure_uploaded()
+    // frames of any sizes (the reference's std::vector<cv::Mat>), grey or colour: colour is converted once on the device, where the
+    // reference converts it in every call (adaptive_vlhog.hpp:114-120).  Each distinct frame is held once.
+    void ensure_ready()
     {
         if (dev->ready) return;
         if (images.empty()) throw std::runtime_error("HogTransform: no images");
         sd_ctx* ctx = sd_b200::context();
-        const std::vector<sd_host_frame> frames = sd_b200::host_frames(images);
+        const std::vector<sd_host_frame> all = sd_b200::host_frames(images);
+        std::vector<sd_host_frame>& frames = dev->frames;
+        std::map<std::tuple<const void*, int, int, int, int>, int32_t> seen;
+        dev->frame_of.resize(all.size());
+        size_t grey = 0;
+        for (size_t i = 0; i < all.size(); ++i) {
+            const sd_host_frame& f = all[i];
+            const auto key = std::make_tuple(static_cast<const void*>(f.h_data), f.width, f.height, f.row_stride, f.channels);
+            const auto it = seen.find(key);
+            if (it != seen.end()) { dev->frame_of[i] = it->second; continue; }
+            dev->frame_of[i] = seen[key] = static_cast<int32_t>(frames.size());
+            frames.push_back(f);
+            grey += static_cast<size_t>(f.height) * ((static_cast<size_t>(f.width) + 15) / 16 * 16);
+        }
+        dev->index.allocate(all.size() * sizeof(int32_t));
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, dev->index.as<int32_t>(), dev->frame_of.data(), all.size() * sizeof(int32_t)), "HogTransform upload");
+        sd_b200::check(ctx, sd_sync(ctx), "HogTransform upload");
+        size_t free_bytes = 0, total = 0;
+        sd_b200::check(ctx, sd_device_memory(ctx, &free_bytes, &total), "sd_device_memory");
         const int n = static_cast<int>(frames.size());
-        size_t bytes = 0;
-        sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, nullptr, &bytes, nullptr), "HogTransform upload");
-        dev->buf.allocate(bytes);
-        sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, dev->buf.as<void>(), &bytes, &dev->batch), "HogTransform upload");
+        if (static_cast<double>(grey) <= device_frame_share() * static_cast<double>(free_bytes)) {
+            size_t bytes = 0;
+            sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, nullptr, &bytes, nullptr), "HogTransform upload");
+            dev->buf.allocate(bytes);
+            sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, dev->buf.as<void>(), &bytes, &dev->batch), "HogTransform upload");
+        } else {
+            // host route: frames the levels cannot read in place are packed once into one pinned buffer, rows at a pitch of
+            // channels * (width rounded up to 16) bytes
+            std::vector<char> pack(frames.size());
+            size_t packed = 0;
+            for (size_t f = 0; f < frames.size(); ++f) {
+                int in_place = 0;
+                sd_b200::check(ctx, sd_host_frame_in_place(ctx, &frames[f], &in_place), "HogTransform");
+                pack[f] = !in_place;
+                if (pack[f]) packed += static_cast<size_t>(frames[f].height) * frames[f].channels * ((static_cast<size_t>(frames[f].width) + 15) / 16 * 16);
+            }
+            if (packed) dev->packed.allocate(packed);
+            unsigned char* dst = dev->packed.as<unsigned char>();
+            for (size_t f = 0; f < frames.size(); ++f) {
+                if (!pack[f]) continue;
+                sd_host_frame& fr = frames[f];
+                const size_t pitch = static_cast<size_t>(fr.channels) * ((static_cast<size_t>(fr.width) + 15) / 16 * 16);
+                for (int y = 0; y < fr.height; ++y)
+                    std::memcpy(dst + y * pitch, fr.h_data + static_cast<size_t>(y) * fr.row_stride, static_cast<size_t>(fr.width) * fr.channels);
+                fr.h_data = dst;
+                fr.row_stride = static_cast<int32_t>(pitch);
+                dst += pitch * fr.height;
+            }
+            dev->host = true;
+        }
         dev->ready = true;
-    }
-
-    void launch(const float* d_x, int64_t ldx, int n, size_t level, float* d_A, int64_t ld, const int32_t* d_index)
-    {
-        sd_ctx* ctx = sd_b200::context();
-        const sd_normalisation nrm = eyes();
-        const sd_hog_param p = hog_params[level].c();
-        sd_b200::check(ctx, sd_hog_batch(ctx, &dev->batch, d_index, d_x, ldx, n, static_cast<int>(modelLandmarksList.size()), &nrm, &p, d_A, ld), "sd_hog_batch");
     }
 
     const std::vector<cv::Mat>& images;

@@ -64,6 +64,24 @@ private:
     size_t bytes_ = 0;
 };
 
+// pinned host memory (sd_host_alloc), e.g. frames the HogTransform keeps in host memory
+class HostBuffer {
+public:
+    HostBuffer() = default;
+    HostBuffer(const HostBuffer&) = delete;
+    HostBuffer& operator=(const HostBuffer&) = delete;
+    ~HostBuffer() { if (ptr_) sd_host_free(context(), ptr_); }
+    void allocate(size_t bytes)
+    {
+        if (ptr_) { sd_host_free(context(), ptr_); ptr_ = nullptr; }
+        check(context(), sd_host_alloc(context(), bytes, &ptr_), "sd_host_alloc");
+    }
+    template <class T> T* as() const { return static_cast<T*>(ptr_); }
+
+private:
+    void* ptr_ = nullptr;
+};
+
 // packed float32 cv::Mat -> device (row stride ld floats, ld >= cols)
 inline void upload(const cv::Mat& m, DeviceBuffer& dst, int64_t ld)
 {

@@ -233,7 +233,10 @@ private:
         sd_b200::upload(initialisations, d_cur, Pd);
         const sd_normalisation norm = normalisation_strategy.c_normalisation();
         const sd_normalisation eyes = projection.eyes();
-        const sd_image_batch& images = projection.device_batch();
+        const int32_t* d_frame = projection.device_sample_frame(n);
+        // frames on the device, or host frames read through a staging buffer (allocated before the chunk query sizes the chunk)
+        const bool on_device = projection.on_device();
+        sd_b200::DeviceBuffer stage(on_device ? 0 : projection.stage_bytes());
         if (!templates.empty()) sd_b200::upload(templates, d_tmpl, templates.cols);
         sd_b200::DeviceBuffer X;
         int64_t n_global = n;
@@ -252,9 +255,13 @@ private:
             const int rows = templates.empty() ? chunk_rows(ctx, c, n, D, Pd, route) : (n > 0 ? n : 1);
             sd_b200::DeviceBuffer chunk(static_cast<size_t>(rows) * ld * sizeof(float));
             X.allocate(static_cast<size_t>(D) * Pd * sizeof(float));
-            const int rc = sd_train_level(ctx, c, &images, nullptr, d_cur.as<float>(), d_gt.as<float>(), n, Pd / 2, n_global, &eyes, &hp, &norm,
-                                          templates.empty() ? nullptr : d_tmpl.as<float>(), templates.cols, &reg, route, chunk.as<float>(), ld,
-                                          rows, X.as<float>(), d_next.as<float>(), nullptr);
+            const float* tmpl = templates.empty() ? nullptr : d_tmpl.as<float>();
+            const int rc = on_device
+                ? sd_train_level(ctx, c, &projection.device_batch(), d_frame, d_cur.as<float>(), d_gt.as<float>(), n, Pd / 2, n_global, &eyes, &hp,
+                                 &norm, tmpl, templates.cols, &reg, route, chunk.as<float>(), ld, rows, X.as<float>(), d_next.as<float>(), nullptr)
+                : sd_train_level_host(ctx, c, projection.host_frames().data(), static_cast<int>(projection.host_frames().size()), d_frame,
+                                      d_cur.as<float>(), d_gt.as<float>(), n, Pd / 2, n_global, &eyes, &hp, &norm, tmpl, templates.cols, &reg, route,
+                                      chunk.as<float>(), ld, rows, stage.as<void>(), stage.bytes(), X.as<float>(), d_next.as<float>(), nullptr);
             if (want_rank) {
                 sd_set_rank_diagnostic(ctx, 0);
                 detail::report_rank(regressors[level], sd_last_rank(ctx), D, detail::reports_rank<RegressorType>());
@@ -300,7 +307,9 @@ private:
         sd_b200::upload(initialisations, d_cur, Pd);
         const sd_normalisation norm = normalisation_strategy.c_normalisation();
         const sd_normalisation eyes = projection.eyes();
-        const sd_image_batch& images = projection.device_batch();
+        const int32_t* d_frame = projection.device_sample_frame(n);
+        const bool on_device = projection.on_device();
+        sd_b200::DeviceBuffer stage(on_device ? 0 : projection.stage_bytes());
         if (!templates.empty()) sd_b200::upload(templates, d_tmpl, templates.cols);
         for (size_t level = 0; level < regressors.size(); ++level) {
             const int D = projection.feature_length(level);
@@ -308,9 +317,17 @@ private:
             const sd_hog_param hp = projection.hog_param(level);
             const int rows = chunk_rows(ctx, nullptr, n, D, Pd, 0);
             sd_b200::DeviceBuffer chunk(static_cast<size_t>(rows) * ld * sizeof(float));
-            sd_b200::check(ctx, sd_apply_level(ctx, &images, nullptr, d_cur.as<float>(), n, Pd / 2, &eyes, &hp, &norm,
-                                               templates.empty() ? nullptr : d_tmpl.as<float>(), templates.cols, regressors[level].device_x(),
-                                               chunk.as<float>(), ld, rows, d_next.as<float>()), "sd_apply_level");
+            const float* tmpl = templates.empty() ? nullptr : d_tmpl.as<float>();
+            if (on_device)
+                sd_b200::check(ctx, sd_apply_level(ctx, &projection.device_batch(), d_frame, d_cur.as<float>(), n, Pd / 2, &eyes, &hp, &norm, tmpl,
+                                                   templates.cols, regressors[level].device_x(), chunk.as<float>(), ld, rows, d_next.as<float>()),
+                               "sd_apply_level");
+            else
+                sd_b200::check(ctx, sd_apply_level_host(ctx, projection.host_frames().data(), static_cast<int>(projection.host_frames().size()), d_frame,
+                                                        d_cur.as<float>(), n, Pd / 2, &eyes, &hp, &norm, tmpl, templates.cols,
+                                                        regressors[level].device_x(), chunk.as<float>(), ld, rows, stage.as<void>(), stage.bytes(),
+                                                        d_next.as<float>()),
+                               "sd_apply_level_host");
             std::swap(d_cur, d_next);
             if (want_callback) cb(sd_b200::download(d_cur.as<float>(), n, Pd, Pd));                          // :303
         }
