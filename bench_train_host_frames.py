@@ -1,5 +1,5 @@
 """Training on frames that stay in host memory: the device route (frames uploaded once) against the host route (frames gathered
-level by level from pinned host memory, sd_train_level_host), on an rcr-train-shaped set.
+level by level from pinned host memory through sd_train_level), on an rcr-train-shaped set.
 
     python bench_train_host_frames.py [--photos 800] [--levels 5] [--big]
 

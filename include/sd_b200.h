@@ -335,23 +335,48 @@ SD_API int sd_cascade_update(sd_ctx* ctx, const float* d_A, int64_t lda, int N, 
 SD_API int sd_subtract_templates(sd_ctx* ctx, float* d_A, int64_t lda, const float* d_T, int64_t ldt,
                                  int N, int D);
 
-/* ---- training and testing in chunks: one HogTransform cascade level per call ---------------------------------------------
+/* ---- cascade levels: one HogTransform cascade level per call, in chunks of rows ---------------------------------------------
  * A level's feature rows [A | b] (ld = roundup4(D + 2L) floats per sample: 68 KB at D = 17,051, 211 KB at D = 52,701) need not
  * be resident at once: [A^T A | A^T b] is a sum over rows.  The caller owns one buffer of chunk_rows x ld floats; the level runs
  * through it chunk by chunk.
  *
- * sd_level_chunk_rows: the largest r <= N_local such that r rows of the caller's chunk buffer (r * ld * 4 bytes, with the update's
- * r * M * 8 bytes of partial sums) fit in free_bytes beside everything the level's solve will still allocate with the context's
- * current settings -- G (D x ld), the rank copy if the diagnostic is on, CG's copy of the system if CG may run (sd_set_solver 1, or
- * route 2 on several ranks), the band buffer of the exchange on several ranks, the bias / inverse workspaces -- less what the
- * context already holds, and a reserve of 512 MB for small workspaces.  free_bytes == 0: cudaMemGetInfo.  Returns N_local (at
- * least 1) when everything fits; SD_ERR_CUDA, with a message naming D, when not even min(N_local, 256) rows fit.  M = 2L.
+ * Where a level's frames are (sd_level_frames): exactly one of images and host_frames is non-NULL, anything else is SD_ERR_INVALID
+ * before any work is queued.
+ *   - images: frames resident on the device, as for sd_hog_batch.
+ *   - host_frames: num_host_frames host frames (sd_host_frame: grey or B,G,R, any sizes), each in pinned, device-mapped memory with
+ *     a 16-byte aligned base and row_stride (the ROI route of sd_detect_faces_host), and row_stride >= channels * (width rounded up
+ *     to 16).  Only frames a sample refers to are read or checked; they are read in place while the call runs.  Per chunk of rows
+ *     the HOG rows are produced in gather batches that fit one half of the context's staging pair: the exact union of the windows
+ *     of the batch's patches is planned per frame on the device (samples of one frame in one batch share one region), gathered
+ *     zero-copy over PCIe (colour converted to grey on the way) on the context's copy stream while the previous batch's HOG runs,
+ *     and read by the unchanged HOG kernel.  One small read-back per batch is the only synchronisation the plan adds, and the call
+ *     reads d_sample_frame back once before it queues work.  Each half holds max(stage_half_bytes, the largest referenced frame's
+ *     grey bytes at a 16-byte pitch) rounded up to 16; the context keeps the pair (it is the pair sd_detect_faces_host uses) and
+ *     grows it when a call needs more.  X, lambda and x_next are bit for bit what the same frames uploaded by sd_upload_frames give.
+ *     Frames that break these rules are SD_ERR_INVALID before any work is queued.  Every rank passes its own frames.
+ *   - d_sample_frame (device, N ints, may be NULL = frame i): sample i reads frame d_sample_frame[i].  An index out of range raises
+ *     the projection's status flag (reported by the next synchronising call, as for sd_hog_batch); on the host route the sample
+ *     then reads frame 0. */
+typedef struct {
+    const sd_image_batch* images;      /* frames resident on the device, or NULL */
+    const sd_host_frame* host_frames;  /* frames in pinned host memory, or NULL */
+    int32_t num_host_frames;
+    const int32_t* d_sample_frame;     /* sample i reads frame d_sample_frame[i]; NULL = frame i, on either route */
+    size_t stage_half_bytes;           /* host route: bytes per staging half; 0 = the library's default (48 MB) */
+} sd_level_frames;
+/* sd_level_chunk_rows: the largest r <= N_local such that r rows of the caller's chunk buffer (r * ld * 4 bytes, with the update's
+ * r * M * 8 bytes of partial sums) fit in free_bytes beside everything the level will still allocate with the context's current
+ * settings -- G (D x ld), the rank copy if the diagnostic is on, CG's copy of the system if CG may run (sd_set_solver 1, or route 2
+ * on several ranks), the band buffer of the exchange on several ranks, the bias / inverse workspaces and, for host frames, the
+ * staging pair (sized by the largest frame of the table) -- less what the context already holds, and a reserve of 512 MB for small
+ * workspaces.  frames may be NULL (no staging).  free_bytes == 0: cudaMemGetInfo.  Returns N_local (at least 1) when everything
+ * fits; SD_ERR_CUDA, with a message naming D, when not even min(N_local, 256) rows fit.  M = 2L.
  *
- * sd_train_level: one training level (superviseddescent.hpp:173-217) for the HOG projection (images, d_image_index and hog_eyes as
- * in sd_hog_batch; sample i reads frame d_image_index ? d_image_index[i] : i).  d_x, d_x_gt: N_local x 2L current / ground-truth
- * landmarks; norm: the optimiser's normalisation; d_templates: optional N_local x D (row pitch ldt); reg / route / comm as in
- * sd_learn_centred (comm may be NULL); n_global: the samples of all ranks.  Writes the model d_X (D x 2L, for uncentred features),
- * the updated landmarks d_x_next (N_local x 2L) and *lambda_out (may be NULL).
+ * sd_train_level: one training level (superviseddescent.hpp:173-217) for the HOG projection (frames as above, hog_eyes as in
+ * sd_hog_batch).  d_x, d_x_gt: N_local x 2L current / ground-truth landmarks; norm: the optimiser's normalisation; d_templates:
+ * optional N_local x D (row pitch ldt); reg / route / comm as in sd_learn_centred (comm may be NULL); n_global: the samples of all
+ * ranks.  Writes the model d_X (D x 2L, for uncentred features), the updated landmarks d_x_next (N_local x 2L) and *lambda_out (may
+ * be NULL).
  *   - one chunk (chunk_rows >= N_local): sd_hog_batch, sd_subtract_templates, sd_cascade_targets, sd_centre_features,
  *     sd_learn_centred and sd_cascade_update (on the centred rows with their weights) -- bit for bit what those calls give.
  *   - several chunks: chunk 0 is centred by sd_centre_features over every rank's first chunk; its column means p (the pilot
@@ -363,51 +388,25 @@ SD_API int sd_subtract_templates(sd_ctx* ctx, float* d_A, int64_t lda, const flo
  *   the result is reproducible bit for bit.  Every rank makes the same collectives whatever its chunk count.
  *   SD_ERR_INVALID before any work is queued (outputs unwritten): chunk_rows < 1, ld < D + 2L, templates with
  *   chunk_rows < N_local (a chunked level would check the all-ones bias column on chunk 0 only, and T is as large as the
- *   features), d_x_next == d_x, null pointers.
+ *   features), d_x_next == d_x, null pointers, bad frames.
  *
  * sd_apply_level: one test / predict level (superviseddescent.hpp:262-306, 323-344) in chunks of chunk_rows rows (ld >= D):
  * HOG rows, optional templates (N x D, pitch ldt), x_next = x - (A X) (.) 1 / norm(x).  With ld a multiple of 4 and a 16-byte
  * aligned d_chunk each row's result does not depend on the chunking.  Same argument errors as sd_train_level, with ld >= D. */
-SD_API int sd_level_chunk_rows(sd_ctx* ctx, sd_comm* comm, int64_t N_local, int D, int M, int route, size_t free_bytes, int* rows_out);
-SD_API int sd_train_level(sd_ctx* ctx, sd_comm* comm, const sd_image_batch* images, const int32_t* d_image_index,
+SD_API int sd_level_chunk_rows(sd_ctx* ctx, sd_comm* comm, const sd_level_frames* frames, int64_t N_local, int D, int M, int route,
+                               size_t free_bytes, int* rows_out);
+SD_API int sd_train_level(sd_ctx* ctx, sd_comm* comm, const sd_level_frames* frames,
                           const float* d_x, const float* d_x_gt, int N_local, int L, int64_t n_global,
                           const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
                           const float* d_templates, int64_t ldt, const sd_regulariser* reg, int route,
                           float* d_chunk, int64_t ld, int chunk_rows, float* d_X, float* d_x_next, float* lambda_out);
-SD_API int sd_apply_level(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int N, int L,
+SD_API int sd_apply_level(sd_ctx* ctx, const sd_level_frames* frames, const float* d_x, int N, int L,
                           const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
                           const float* d_templates, int64_t ldt, const float* d_X,
                           float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next);
-
-/* ---- the same levels on frames that stay in host memory (DESIGN 4.6) ------------------------------------------------------
- * sd_train_level_host / sd_apply_level_host: the contract of sd_train_level / sd_apply_level, bit for bit the same X, lambda and
- * x_next as those calls on the same frames uploaded by sd_upload_frames, with three differences:
- *   - frames: num_frames host frames (sd_host_frame: grey or B,G,R, any sizes), each in pinned, device-mapped memory with a 16-byte
- *     aligned base and row_stride (the ROI route of sd_detect_faces_host), and row_stride >= channels * (width rounded up to 16).
- *     Only frames a sample refers to are read or checked.  They are read in place while the call runs.
- *   - d_sample_frame (device, N ints, required): sample i reads frames[d_sample_frame[i]].  An index out of range raises the
- *     projection's status flag (reported by the next synchronising call, as for sd_hog_batch) and the sample reads frame 0.
- *   - d_stage / stage_bytes: a device staging buffer the caller owns (16-byte aligned), used as two halves.  Each half must hold the
- *     largest frame a sample refers to as grey bytes at a 16-byte pitch (height * roundup16(width)): no region is larger.
- * Per chunk of rows the HOG rows are produced in gather batches that fit one staging half: the exact union of the windows of the
- * batch's patches is planned per frame on the device (samples of one frame in one batch share one region), gathered zero-copy
- * over PCIe (colour converted to grey on the way) on the context's copy stream while the previous batch's HOG runs, and read by
- * the unchanged HOG kernel.  One small read-back per batch is the only synchronisation the plan adds.
- * Frames that break these rules, or a staging half that is too small, are SD_ERR_INVALID before any work is queued (the outputs are
- * not written).  The call reads d_sample_frame back once before it queues work.  Every rank passes its own frames. */
-SD_API int sd_train_level_host(sd_ctx* ctx, sd_comm* comm, const sd_host_frame* frames, int num_frames, const int32_t* d_sample_frame,
-                               const float* d_x, const float* d_x_gt, int N_local, int L, int64_t n_global,
-                               const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
-                               const float* d_templates, int64_t ldt, const sd_regulariser* reg, int route,
-                               float* d_chunk, int64_t ld, int chunk_rows, void* d_stage, size_t stage_bytes,
-                               float* d_X, float* d_x_next, float* lambda_out);
-SD_API int sd_apply_level_host(sd_ctx* ctx, const sd_host_frame* frames, int num_frames, const int32_t* d_sample_frame,
-                               const float* d_x, int N, int L, const sd_normalisation* hog_eyes, const sd_hog_param* p,
-                               const sd_normalisation* norm, const float* d_templates, int64_t ldt, const float* d_X,
-                               float* d_chunk, int64_t ld, int chunk_rows, void* d_stage, size_t stage_bytes, float* d_x_next);
-/* host-frame bytes (region bytes x channels) the _host levels have read over PCIe on ctx since creation */
+/* host-frame bytes (region bytes x channels) the levels on host frames have read over PCIe on ctx since creation */
 SD_API int64_t sd_gathered_bytes(const sd_ctx* ctx);
-/* *in_place = 1 when the _host levels can read the frame where it is (pinned and device-mapped, 16-byte aligned base and
+/* *in_place = 1 when the levels can read a host frame where it is (pinned and device-mapped, 16-byte aligned base and
  * row_stride, row_stride >= channels * roundup16(width)), else 0; a bad frame (as for sd_upload_frames) is SD_ERR_INVALID.  The
  * HogTransform front ends pack the other frames once into pinned memory. */
 SD_API int sd_host_frame_in_place(sd_ctx* ctx, const sd_host_frame* frame, int* in_place);

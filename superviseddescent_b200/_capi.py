@@ -49,6 +49,12 @@ class HostFrameC(C.Structure):
     _fields_ = [("h_data", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32), ("row_stride", C.c_int32), ("channels", C.c_int32)]
 
 
+class LevelFramesC(C.Structure):
+    """sd_level_frames: where a cascade level's frames are (a device batch or host frames) and which frame each sample reads."""
+    _fields_ = [("images", C.POINTER(ImageBatchC)), ("host_frames", C.POINTER(HostFrameC)), ("num_host_frames", C.c_int32),
+                ("d_sample_frame", C.c_void_p), ("stage_half_bytes", C.c_size_t)]
+
+
 # every symbol declared in include/sd_b200.h (tests/test_abi.py checks the list against the header)
 EXPORTS = [
     "sd_ctx_create", "sd_ctx_destroy", "sd_last_error", "sd_sync", "sd_version", "sd_launch_count", "sd_roi_fallback_count",
@@ -60,7 +66,7 @@ EXPORTS = [
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",
     "sd_comm_sum_int64", "sd_comm_allgather", "sd_allreduce_gram", "sd_reduce_scatter_gram", "sd_solve_gram_dist", "sd_learn_dist",
     "sd_cascade_targets", "sd_cascade_update", "sd_subtract_templates", "sd_level_chunk_rows", "sd_train_level", "sd_apply_level",
-    "sd_train_level_host", "sd_apply_level_host", "sd_gathered_bytes", "sd_host_frame_in_place", "sd_device_memory",
+    "sd_gathered_bytes", "sd_host_frame_in_place", "sd_device_memory",
     "sd_model_load", "sd_model_save", "sd_model_create", "sd_model_destroy", "sd_model_num_levels",
     "sd_model_num_landmarks", "sd_model_hog_param", "sd_model_regulariser", "sd_model_normalisation",
     "sd_model_get_mean", "sd_model_get_weights", "sd_model_landmark_id", "sd_align_mean",

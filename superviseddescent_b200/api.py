@@ -23,7 +23,7 @@ import torch
 
 from . import _capi
 from ._capi import HogParam as HoGParam  # same field names as rcr::HoGParam
-from ._capi import HostFrameC, ImageBatchC, NormalisationC, RegulariserC, SdError, ptr
+from ._capi import HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, ptr
 
 
 def _check(ctx, rc: int) -> None:
@@ -376,11 +376,10 @@ def _upload_host_frames(recs, ctx: Context):
 
 
 # The distinct frames of a HogTransform are uploaded when their grey bytes fit in this share of the device's free memory (read when
-# the transform is first used); otherwise they stay in host memory and train() / test() gather them per level
-# (sd_train_level_host / sd_apply_level_host).
+# the transform is first used); otherwise they stay in host memory and train() / test() gather them per level.
 DEVICE_FRAME_SHARE = 0.5
-# bytes of one half of the staging buffer of the host route (at least the largest frame's grey bytes)
-HOST_STAGE_HALF = 48 << 20
+# bytes of one staging half of the host route (sd_level_frames.stage_half_bytes); 0: the library's default
+HOST_STAGE_HALF = 0
 
 
 def _round16(v: int) -> int:
@@ -522,16 +521,17 @@ class HogTransform:
             raise ValueError(f"{n} samples but the image list / image_index has {self._sample_frame.numel()}")
         return self._sample_frame[:n]
 
-    def host_frames(self):
-        """(sd_host_frame table, number of frames) on the host route."""
-        self._choose_route()
-        return self._host[0], len(self._host[0])
-
-    def stage_bytes(self) -> int:
-        """Staging buffer of the host route: two halves of HOST_STAGE_HALF bytes, or of the largest frame's grey bytes."""
-        table, n = self.host_frames()
-        largest = max(table[i].height * _round16(table[i].width) for i in range(n))
-        return 2 * _round16(max(HOST_STAGE_HALF, largest))
+    def level_frames(self, n: int) -> LevelFramesC:
+        """The sd_level_frames of n samples for sd_train_level / sd_apply_level: the device batch or the host frames, and the
+        sample -> frame index.  It holds references to what it points at."""
+        index = self.sample_frame(n)
+        f = LevelFramesC(d_sample_frame=ptr(index), stage_half_bytes=HOST_STAGE_HALF)
+        if self.on_device():
+            f.images = C.pointer(self._batch)
+        else:
+            f.host_frames, f.num_host_frames = self._host[0], len(self._host[0])
+        f.keep = (index, self._batch, self._host)
+        return f
 
     def feature_length(self, level: int) -> int:
         return _capi.lib().sd_hog_feature_length(self.num_landmarks, C.byref(self.hog_params[level]))
@@ -640,36 +640,17 @@ class SupervisedDescentOptimiser:
         host[:, :D] = np.stack(rows)
         return _dev(host, ctx), D
 
-    class _Frames:
-        """What a HogTransform level reads: the device batch, or the host frames and a staging buffer; and the sample -> frame
-        index (None: sample i reads frame i)."""
-        batch = table = stage = None
-        count = 0
-        index = None
-
-    def _frame_source(self, h: "HogTransform", n: int, device) -> "_Frames":
-        f = self._Frames()
-        f.index = h.sample_frame(n)
-        if h.on_device():
-            f.batch = h.batch()
-            return f
-        f.table, f.count = h.host_frames()
-        if f.index is None:
-            f.index = torch.arange(n, dtype=torch.int32, device=device)
-        # allocated before the chunk query, so that the chunk buffer is sized on the free memory beside it
-        f.stage = torch.empty(h.stage_bytes(), dtype=torch.uint8, device=device)
-        return f
-
-    def _chunk_rows(self, rows_per_chunk, n: int, D: int, P: int, comm_h, route: int) -> int:
+    def _chunk_rows(self, rows_per_chunk, frames: LevelFramesC, n: int, D: int, P: int, comm_h, route: int) -> int:
         """Rows per chunk of a HogTransform level: rows_per_chunk (at most n), or -- None / 0 -- the most that fit beside the
-        solve (sd_level_chunk_rows; memory torch has reserved but not handed out counts as free, so a warm caching allocator
-        does not split a level that fits)."""
+        solve and the staging of host frames (sd_level_chunk_rows; memory torch has reserved but not handed out counts as free,
+        so a warm caching allocator does not split a level that fits)."""
         if rows_per_chunk:
             return max(1, min(int(rows_per_chunk), n))
         ctx = self._ctx()
         free = _free_device_bytes(ctx.device)
         rows = C.c_int(0)
-        _check(ctx.h, _capi.lib().sd_level_chunk_rows(ctx.h, comm_h, C.c_int64(n), D, P, route, C.c_size_t(free), C.byref(rows)))
+        _check(ctx.h, _capi.lib().sd_level_chunk_rows(ctx.h, comm_h, C.byref(frames), C.c_int64(n), D, P, route, C.c_size_t(free),
+                                                      C.byref(rows)))
         return rows.value
 
     def train(self, parameters, initialisations, templates, projection, on_training_epoch_callback=None, group=None, comm=None,
@@ -682,8 +663,8 @@ class SupervisedDescentOptimiser:
         ranks.
         A HogTransform projection trains each level with sd_train_level, through a buffer of rows_per_chunk feature rows (None:
         as many as fit on the device, which is all of them whenever the level fits -- then the result is that of one pass over
-        all rows).  Templates need the whole level in one chunk.  A HogTransform whose frames stay in host memory trains with
-        sd_train_level_host instead (same results), the chunk buffer sized beside its staging buffer."""
+        all rows).  Templates need the whole level in one chunk.  Frames that stay in host memory are gathered level by level
+        (same results), the chunk buffer sized beside the staging they need."""
         from . import parallel
         ctx = self._ctx()
         lib = _capi.lib()
@@ -707,7 +688,7 @@ class SupervisedDescentOptimiser:
             return 2 if distributed_solve == "cg" else int(bool(distributed_solve))
 
         ch = comm.h if distributed else None
-        frames = self._frame_source(projection, n, cur.device) if hog else None
+        frames = projection.level_frames(n) if hog else None
         for level, reg in enumerate(self.regressors):
             norm = self.normalisation_strategy.c(P // 2)
             lam = C.c_float(0)
@@ -720,18 +701,14 @@ class SupervisedDescentOptimiser:
                 D = projection.feature_length(level)
                 X = torch.empty((D, P), dtype=torch.float32, device=cur.device)
                 ld = (D + P + 3) // 4 * 4
-                rows = max(n, 1) if tmpl is not None else self._chunk_rows(rows_per_chunk, n, D, P, ch, route(D))
+                rows = max(n, 1) if tmpl is not None else self._chunk_rows(rows_per_chunk, frames, n, D, P, ch, route(D))
                 self.chunk_rows.append(rows)
                 buf = torch.empty((rows, ld), dtype=torch.float32, device=cur.device)
                 eyes = projection.norm.c()
-                args = (ptr(cur), ptr(x_gt), n, P // 2, C.c_int64(n_global), C.byref(eyes), C.byref(projection.hog_params[level]),
-                        C.byref(norm), ptr(tmpl), C.c_int64(tmpl.stride(0) if tmpl is not None else 0), C.byref(rc_), route(D), ptr(buf),
-                        C.c_int64(ld), rows)
-                if frames.stage is not None:
-                    rc = lib.sd_train_level_host(ctx.h, ch, frames.table, frames.count, ptr(frames.index), *args, ptr(frames.stage),
-                                                 C.c_size_t(frames.stage.numel()), ptr(X), ptr(nxt), C.byref(lam))
-                else:
-                    rc = lib.sd_train_level(ctx.h, ch, C.byref(frames.batch), ptr(frames.index), *args, ptr(X), ptr(nxt), C.byref(lam))
+                rc = lib.sd_train_level(ctx.h, ch, C.byref(frames), ptr(cur), ptr(x_gt), n, P // 2, C.c_int64(n_global), C.byref(eyes),
+                                        C.byref(projection.hog_params[level]), C.byref(norm), ptr(tmpl),
+                                        C.c_int64(tmpl.stride(0) if tmpl is not None else 0), C.byref(rc_), route(D), ptr(buf),
+                                        C.c_int64(ld), rows, ptr(X), ptr(nxt), C.byref(lam))
                 del buf
             else:
                 A, D = self._project(projection, cur, level, extra=P)         # 1) features (:173-189)
@@ -774,23 +751,19 @@ class SupervisedDescentOptimiser:
             cur = cur.reshape(1, -1)
         n, P = cur.shape
         tmpl = _dev(templates, ctx) if templates is not None and np.size(templates) > 0 else None
-        frames = self._frame_source(projection, n, cur.device) if isinstance(projection, HogTransform) else None
+        frames = projection.level_frames(n) if isinstance(projection, HogTransform) else None
         for level, reg in enumerate(self.regressors):
             norm = self.normalisation_strategy.c(P // 2)
             nxt = torch.empty_like(cur)
             if isinstance(projection, HogTransform):
                 D = projection.feature_length(level)
                 ld = (D + 3) // 4 * 4
-                rows = self._chunk_rows(rows_per_chunk, n, D, P, None, 0)
+                rows = self._chunk_rows(rows_per_chunk, frames, n, D, P, None, 0)
                 buf = torch.empty((rows, ld), dtype=torch.float32, device=cur.device)
                 eyes = projection.norm.c()
-                args = (ptr(cur), n, P // 2, C.byref(eyes), C.byref(projection.hog_params[level]), C.byref(norm), ptr(tmpl),
-                        C.c_int64(tmpl.stride(0) if tmpl is not None else 0), ptr(reg.x), ptr(buf), C.c_int64(ld), rows)
-                if frames.stage is not None:
-                    _check(ctx.h, lib.sd_apply_level_host(ctx.h, frames.table, frames.count, ptr(frames.index), *args, ptr(frames.stage),
-                                                          C.c_size_t(frames.stage.numel()), ptr(nxt)))
-                else:
-                    _check(ctx.h, lib.sd_apply_level(ctx.h, C.byref(frames.batch), ptr(frames.index), *args, ptr(nxt)))
+                _check(ctx.h, lib.sd_apply_level(ctx.h, C.byref(frames), ptr(cur), n, P // 2, C.byref(eyes), C.byref(projection.hog_params[level]),
+                                                 C.byref(norm), ptr(tmpl), C.c_int64(tmpl.stride(0) if tmpl is not None else 0), ptr(reg.x),
+                                                 ptr(buf), C.c_int64(ld), rows, ptr(nxt)))
                 del buf
             else:
                 A, D = self._project(projection, cur, level, extra=0)

@@ -20,7 +20,7 @@ enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_UPLOAD /* B,G,R scratch of sd_upload_frames */,
        SD_WS_RANK /* the rank diagnostic's working copy of the D x D system, its panel and state (sd_rank.cu) */,
        SD_WS_LEVEL /* column shift and shifted-row weights of sd_train_level (sd_train.cu) */,
-       SD_WS_GATHER /* frame, union, region and record tables of the host-frame levels (sd_train.cu) */, SD_WS_COUNT };
+       SD_WS_GATHER /* frame, union, region, record and index tables of the levels on host frames (sd_train.cu) */, SD_WS_COUNT };
 
 // Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row
 // Cholesky blocks), and panel p belongs to rank p % nranks.  The Gram exchange delivers each panel's rows to their owner, and
@@ -55,7 +55,7 @@ struct sd_ctx {
     int last_rank = -1;            // of the last solve: the rank, or -1 when it was not computed
     cudaEvent_t cg_ev[8] = {};     // convergence read-backs of the CG loop (the host runs a few iterations ahead of them)
     int64_t roi_fallbacks = 0;     // faces repeated from the full frame because a patch left its ROI
-    int64_t gathered_bytes = 0;    // host-frame bytes the levels of sd_train_level_host / sd_apply_level_host read over PCIe
+    int64_t gathered_bytes = 0;    // host-frame bytes sd_train_level / sd_apply_level read over PCIe
     float timings[4] = {0, 0, 0, 0};
     cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     void* hog_lut[SD_MAX_BINS + 1] = {};   // per K: (gx,gy) -> orientation bin table (sd_hog.cu)
@@ -64,7 +64,7 @@ struct sd_ctx {
     // pinned scratch for small device->host results (lambda, residual, status flags)
     void* h_scratch = nullptr;
     void* d_scratch = nullptr;   // 4 KB
-    // staging buffers of sd_detect_faces_host
+    // staging pair of sd_detect_faces_host and of the levels on host frames (sd_ensure_stage)
     void* d_stage[2] = {nullptr, nullptr};
     size_t stage_bytes[2] = {0, 0};
     cudaEvent_t stage_ev[2] = {nullptr, nullptr};
@@ -192,6 +192,10 @@ struct PinnedRange {
 const uint8_t* sd_mapped_frame(const uint8_t* p, size_t bytes, PinnedRange& last);
 // what every entry point that reads sd_host_frame requires of frame f; fn names the entry point in the message
 int sd_check_host_frame(sd_ctx* ctx, const char* fn, const sd_host_frame& fr, int f);
+// grey bytes per staging half by default: detect's ROI chunks and the levels' gather batches
+constexpr size_t SD_STAGE_HALF_BYTES = size_t(48) << 20;
+// the context's staging pair (d_stage) holds at least `bytes` each (grow-only; a buffer that grows is freed after both streams drain)
+int sd_ensure_stage(sd_ctx* ctx, size_t bytes);
 inline size_t sd_host_frame_bytes(const sd_host_frame& f) { return (size_t)(f.height - 1) * f.row_stride + (size_t)f.width * f.channels; }
 inline size_t sd_round16(size_t v) { return (v + 15) & ~(size_t)15; }
 // grey bytes of a frame at a 16-byte pitch: no region of it is larger

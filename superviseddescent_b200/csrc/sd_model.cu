@@ -173,7 +173,7 @@ int detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, 
 }
 
 
-// ---- region-of-interest gather (sd_detect_faces_host, sd_train_level_host, sd_apply_level_host) ----------------------------
+// ---- region-of-interest gather (sd_detect_faces_host, and sd_train_level / sd_apply_level on host frames) -------------------
 // The cascade only ever reads a neighbourhood of the face, so instead of copying whole frames over PCIe a small kernel pulls
 // the ROI rows of every face straight out of the caller's PINNED host frame (zero-copy loads through the unified address
 // space, 16-byte vectors) into a packed grey device buffer.  In detect, if a patch later needs a frame pixel outside its ROI
@@ -324,6 +324,18 @@ int sd_check_host_frame(sd_ctx* ctx, const char* fn, const sd_host_frame& fr, in
     return SD_OK;
 }
 
+int sd_ensure_stage(sd_ctx* ctx, size_t bytes)
+{
+    for (int b = 0; b < 2; ++b) {
+        if (ctx->stage_bytes[b] < bytes) {
+            if (ctx->d_stage[b]) { SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); SD_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream)); SD_CUDA(ctx, cudaFree(ctx->d_stage[b])); ctx->d_stage[b] = nullptr; }
+            SD_CUDA(ctx, cudaMalloc(&ctx->d_stage[b], bytes));
+            ctx->stage_bytes[b] = bytes;
+        }
+    }
+    return SD_OK;
+}
+
 namespace {
 
 size_t bgr_bytes(const sd_host_frame& f) { return f.channels == 3 ? (size_t)f.height * sd_round16(3 * (size_t)f.width) : 0; }
@@ -395,19 +407,6 @@ int upload_frames(sd_ctx* ctx, const sd_host_frame* frames, const sd_frame* desc
     return SD_OK;
 }
 
-// the two staging buffers hold at least `bytes` each
-int ensure_stage(sd_ctx* ctx, size_t bytes)
-{
-    for (int b = 0; b < 2; ++b) {
-        if (ctx->stage_bytes[b] < bytes) {
-            if (ctx->d_stage[b]) { SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); SD_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream)); SD_CUDA(ctx, cudaFree(ctx->d_stage[b])); ctx->d_stage[b] = nullptr; }
-            SD_CUDA(ctx, cudaMalloc(&ctx->d_stage[b], bytes));
-            ctx->stage_bytes[b] = bytes;
-        }
-    }
-    return SD_OK;
-}
-
 // Full route: faces grouped by frame, every referenced frame copied to the device once (upload_frames; a chunk's B,G,R bytes
 // behind its grey frames), chunks double-buffered against the cascade.  x0 / out: count x 2L in the caller's face order.
 int detect_faces_full(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frames, const int32_t* face_frame, int count,
@@ -454,7 +453,7 @@ int detect_faces_full(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frame
         face_first[c] = k;
         local[k] -= chunk_first[c];                           // frame index inside its chunk
     }
-    int rc = ensure_stage(ctx, need);
+    int rc = sd_ensure_stage(ctx, need);
     if (rc) return rc;
     // device tables: landmarks (in, out) in sorted order, face -> frame index, frame descriptors
     std::vector<float> xs((size_t)count * P);
@@ -497,7 +496,7 @@ int detect_faces_roi(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frames
                      const int32_t* face_frame, int count, const float* x0, float* out)
 {
     const int P = 2 * m->num_landmarks;
-    const size_t chunk_cap = (size_t)48 << 20;                // packed grey ROI bytes per staging buffer
+    const size_t chunk_cap = SD_STAGE_HALF_BYTES;             // packed grey ROI bytes per staging buffer
     // the ROI of every face, from its own frame's size; faces are grouped into chunks that fit one staging buffer
     std::vector<sd_roi> rois(count);
     std::vector<sd_frame> dims(count);
@@ -531,7 +530,7 @@ int detect_faces_roi(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frames
                 if (ch == 1) ++chunk_grey[c];
             }
     }
-    int rc = ensure_stage(ctx, chunk_cap + (1u << 20));
+    int rc = sd_ensure_stage(ctx, chunk_cap + (1u << 20));
     if (rc) return rc;
     // device tables: landmarks (in, out), ROI records, frame sizes, gather records, miss flags
     const size_t xbytes = (size_t)count * P * sizeof(float);

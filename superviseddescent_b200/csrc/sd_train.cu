@@ -1,4 +1,4 @@
-// Cascade levels of the HOG optimiser in chunks of rows (include/sd_b200.h, "training and testing in chunks").
+// Cascade levels of the HOG optimiser in chunks of rows (include/sd_b200.h, "cascade levels").
 //
 //   sd_level_chunk_rows  rows of one chunk that fit beside what the level's solve allocates
 //   sd_train_level       superviseddescent.hpp:173-217: HOG, targets, shift, Gram accumulation, exchange, solve, update
@@ -11,8 +11,8 @@
 // column first (the exact centring of any shifted Gram) and shifts the bias back.  With one chunk p IS the mean and the call
 // sequence is sd_train's one-shot sequence, kernel for kernel.
 //
-// sd_train_level_host / sd_apply_level_host run the same loop; only the HOG rows come from another source: frames that stay in
-// pinned host memory, gathered batch by batch (gather_hog_rows).
+// The HOG rows come from frames resident on the device, or from frames that stay in pinned host memory, gathered batch by batch
+// (gather_hog_rows); sd_level_frames says which.
 #include "sd_internal.cuh"
 
 #include <climits>
@@ -54,13 +54,11 @@ struct GatherTotals {
     int n_grey, n_colour;                 // gather records of grey / colour frames
 };
 
-// The state of one host-frame level call (sd_train_level_host, sd_apply_level_host)
+// The state of one level call on host frames
 struct HostGather {
-    const sd_host_frame* frames;
     int num_frames;
-    const int32_t* d_sample_frame;
-    uint8_t* stage[2];
-    size_t half;                          // bytes of one staging half
+    const int32_t* d_sample_frame;        // the caller's index, or the identity in SD_WS_GATHER
+    size_t half;                          // bytes of one staging half (the context's d_stage pair)
     // device tables (SD_WS_GATHER)
     FrameDev* d_fr;
     int2* d_lo;                           // per frame: union of the planned windows, min corner (INT_MAX = none) ...
@@ -204,16 +202,23 @@ __global__ void __launch_bounds__(kLayoutThreads) gather_layout_kernel(const Fra
     if (tid == 0) *tot = GatherTotals{s_base, s_pcie, s_ng, s_nc};
 }
 
-// Checks the frames and the staging buffer (SD_ERR_INVALID before any work is queued) and sets up the device tables.
-int gather_prepare(sd_ctx* ctx, HostGather& g, int N, void* d_stage, size_t stage_bytes)
+// bytes of one staging half: the caller's size (0 = the default), at least the largest frame's grey bytes (no region is larger)
+size_t stage_half(const sd_level_frames& src, size_t largest)
 {
-    const int F = g.num_frames;
-    SD_REQUIRE(ctx, g.frames && F >= 1 && g.d_sample_frame && d_stage, "null frames, sample -> frame index or staging buffer");
-    SD_REQUIRE(ctx, (reinterpret_cast<uintptr_t>(d_stage) & 15) == 0, "d_stage must be 16-byte aligned");
+    const size_t want = src.stage_half_bytes ? src.stage_half_bytes : SD_STAGE_HALF_BYTES;
+    return sd_round16(want > largest ? want : largest);
+}
+
+// Checks the frames (SD_ERR_INVALID before any work is queued), sizes the context's staging pair and sets up the device tables.
+int gather_prepare(sd_ctx* ctx, HostGather& g, const sd_level_frames& src, int N)
+{
+    const int F = src.num_host_frames;
     // the frames the samples refer to (an index out of range reads frame 0 and is reported by the projection's status flag)
     std::vector<int32_t> idx(N);
-    if (N > 0) {
-        SD_CUDA(ctx, cudaMemcpyAsync(idx.data(), g.d_sample_frame, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    if (!src.d_sample_frame)
+        for (int s = 0; s < N; ++s) idx[s] = s;
+    else if (N > 0) {
+        SD_CUDA(ctx, cudaMemcpyAsync(idx.data(), src.d_sample_frame, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
         SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     }
     std::vector<char> used(F, 0);
@@ -223,7 +228,7 @@ int gather_prepare(sd_ctx* ctx, HostGather& g, int N, void* d_stage, size_t stag
     size_t largest = 0;
     for (int f = 0; f < F; ++f) {
         if (!used[f]) { fr[f] = FrameDev{nullptr, 1, 1, 16, 1}; continue; }
-        const sd_host_frame& h = g.frames[f];
+        const sd_host_frame& h = src.host_frames[f];
         int rc = sd_check_host_frame(ctx, __func__, h, f);
         if (rc) return rc;
         const uint8_t* m = sd_mapped_frame(h.h_data, sd_host_frame_bytes(h), last);
@@ -235,17 +240,16 @@ int gather_prepare(sd_ctx* ctx, HostGather& g, int N, void* d_stage, size_t stag
         fr[f] = FrameDev{m, h.width, h.height, h.row_stride, h.channels};
         largest = sd_gray_bytes(h) > largest ? sd_gray_bytes(h) : largest;
     }
-    g.half = (stage_bytes / 2) & ~(size_t)15;
-    if (g.half < largest)
-        return sd_fail(ctx, SD_ERR_INVALID, "%s: a staging half of %zu bytes is smaller than the largest frame a sample refers to (%zu grey bytes)",
-                       __func__, g.half, largest);
-    g.stage[0] = static_cast<uint8_t*>(d_stage);
-    g.stage[1] = g.stage[0] + g.half;
+    g.half = stage_half(src, largest);
+    int rc = sd_ensure_stage(ctx, g.half);
+    if (rc) return rc;
     // device tables
     const size_t n = N > 0 ? N : 1;
     const size_t b_fr = sd_round16(F * sizeof(FrameDev)), b_lo = sd_round16(F * sizeof(int2)), b_froi = sd_round16(F * sizeof(sd_roi));
     const size_t b_rec = sd_round16(2 * F * sizeof(GatherRec)), b_roi = sd_round16(n * sizeof(sd_roi)), b_dims = sd_round16(n * sizeof(sd_frame));
-    uint8_t* t = (uint8_t*)sd_workspace(ctx, SD_WS_GATHER, b_fr + 2 * b_lo + b_froi + b_rec + b_roi + b_dims + sd_round16(n) + sizeof(GatherTotals));
+    const size_t b_idx = src.d_sample_frame ? 0 : sd_round16(n * sizeof(int32_t));
+    uint8_t* t = (uint8_t*)sd_workspace(ctx, SD_WS_GATHER,
+                                        b_fr + 2 * b_lo + b_froi + b_rec + b_roi + b_dims + b_idx + sd_round16(n) + sizeof(GatherTotals));
     if (!t) return SD_ERR_CUDA;
     g.d_fr = (FrameDev*)t;                      t += b_fr;
     g.d_lo = (int2*)t;                          t += b_lo;
@@ -254,13 +258,18 @@ int gather_prepare(sd_ctx* ctx, HostGather& g, int N, void* d_stage, size_t stag
     g.d_rec = (GatherRec*)t;                    t += b_rec;
     g.d_roi = (sd_roi*)t;                       t += b_roi;
     g.d_dims = (sd_frame*)t;                    t += b_dims;
+    int32_t* d_idx = (int32_t*)t;               t += b_idx;
     g.d_miss = t;                               t += sd_round16(n);
     g.d_tot = (GatherTotals*)t;
+    g.num_frames = F;
+    g.d_sample_frame = b_idx ? d_idx : src.d_sample_frame;
+    if (b_idx && N > 0)                                                                    // no index: sample i reads frame i
+        SD_CUDA(ctx, cudaMemcpyAsync(d_idx, idx.data(), (size_t)N * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
     SD_CUDA(ctx, cudaMemcpyAsync(g.d_fr, fr.data(), F * sizeof(FrameDev), cudaMemcpyHostToDevice, ctx->stream));
     SD_CUDA(ctx, cudaMemsetAsync(g.d_lo, 0x7f, F * sizeof(int2), ctx->stream));          // 0x7f7f7f7f: above any coordinate
     SD_CUDA(ctx, cudaMemsetAsync(g.d_hi, 0x80, F * sizeof(int2), ctx->stream));          // 0x80808080: below any coordinate
     SD_CUDA(ctx, cudaMemsetAsync(g.d_miss, 0, n, ctx->stream));
-    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));                                      // fr goes out of scope
+    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));                                      // fr and idx go out of scope
     g.guess = N > 0 ? N : 1;
     return SD_OK;
 }
@@ -317,13 +326,14 @@ int gather_hog_rows(sd_ctx* ctx, HostGather& g, const float* d_x, int r0, int ro
         g.guess = (size_t)t.bytes * 2 <= g.half && nb <= INT_MAX / 2 ? 2 * nb : nb;
         const int buf = g.buf;
         g.buf ^= 1;
+        uint8_t* stage = static_cast<uint8_t*>(ctx->d_stage[buf]);
         SD_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_done[buf], 0));   // the HOG that last read this half is done
-        rc = sd_roi_gather(ctx, g.d_rec, t.n_grey, g.d_rec + g.num_frames, t.n_colour, g.stage[buf], ctx->copy_stream);
+        rc = sd_roi_gather(ctx, g.d_rec, t.n_grey, g.d_rec + g.num_frames, t.n_colour, stage, ctx->copy_stream);
         if (rc) return rc;
         SD_CUDA(ctx, cudaEventRecord(ctx->stage_ev[buf], ctx->copy_stream));
         SD_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->stage_ev[buf], 0));
         sd_image_batch ib{};
-        ib.d_data = g.stage[buf];
+        ib.d_data = stage;
         ib.count = nb;
         ib.d_roi = g.d_roi + s0;
         ib.d_roi_miss = g.d_miss + s0;
@@ -337,32 +347,45 @@ int gather_hog_rows(sd_ctx* ctx, HostGather& g, const float* d_x, int r0, int ro
     return SD_OK;
 }
 
-// Where a level's HOG rows come from: frames resident on the device (images, d_image_index) or host frames (host).
-struct HogSource {
-    const sd_image_batch* images;
-    const int32_t* d_image_index;
-    HostGather* host;
-};
+// exactly one source of frames (SD_ERR_INVALID otherwise)
+int check_frames(sd_ctx* ctx, const sd_level_frames* src)
+{
+    SD_REQUIRE(ctx, src && !src->images != !src->host_frames, "exactly one of frames->images and frames->host_frames");
+    SD_REQUIRE(ctx, src->images || src->num_host_frames >= 1, "num_host_frames < 1");
+    return SD_OK;
+}
+
+// On the host route: checks the frames and sets up the gather (SD_ERR_INVALID before any work is queued).
+int frames_prepare(sd_ctx* ctx, const sd_level_frames* src, HostGather& g, int N)
+{
+    const int rc = check_frames(ctx, src);
+    if (rc || src->images) return rc;
+    return gather_prepare(ctx, g, *src, N);
+}
 
 // HOG rows of samples [r0, r0 + rows) into the chunk buffer
-int hog_rows(sd_ctx* ctx, const HogSource& src, const float* d_x, int r0, int rows, int L, const sd_normalisation* eyes,
-             const sd_hog_param* p, float* d_chunk, int64_t ld)
+int hog_rows(sd_ctx* ctx, const sd_level_frames& src, HostGather& g, const float* d_x, int r0, int rows, int L,
+             const sd_normalisation* eyes, const sd_hog_param* p, float* d_chunk, int64_t ld)
 {
-    if (src.host) return gather_hog_rows(ctx, *src.host, d_x, r0, rows, L, eyes, p, d_chunk, ld);
+    if (!src.images) return gather_hog_rows(ctx, g, d_x, r0, rows, L, eyes, p, d_chunk, ld);
     const int P = 2 * L;
-    const sd_image_batch view = src.d_image_index ? *src.images : batch_from(*src.images, r0);
-    return sd_hog_batch(ctx, &view, src.d_image_index ? src.d_image_index + r0 : nullptr, d_x + (int64_t)r0 * P, P, rows, L, eyes, p,
-                        d_chunk, ld);
+    const int32_t* idx = src.d_sample_frame;
+    const sd_image_batch view = idx ? *src.images : batch_from(*src.images, r0);
+    return sd_hog_batch(ctx, &view, idx ? idx + r0 : nullptr, d_x + (int64_t)r0 * P, P, rows, L, eyes, p, d_chunk, ld);
 }
 
 size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
 
-// superviseddescent.hpp:173-217 for either source of HOG rows (see sd_train_level)
-int train_level(sd_ctx* ctx, sd_comm* comm, const HogSource& src, const float* d_x, const float* d_x_gt, int N_local, int L,
-                int64_t n_global, const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
-                const float* d_templates, int64_t ldt, const sd_regulariser* reg, int route, float* d_chunk, int64_t ld, int chunk_rows,
-                float* d_X, float* d_x_next, float* lambda_out, void* d_stage, size_t stage_bytes)
+}  // namespace
+
+extern "C" {
+
+int sd_train_level(sd_ctx* ctx, sd_comm* comm, const sd_level_frames* frames, const float* d_x, const float* d_x_gt, int N_local, int L,
+                   int64_t n_global, const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
+                   const float* d_templates, int64_t ldt, const sd_regulariser* reg, int route, float* d_chunk, int64_t ld, int chunk_rows,
+                   float* d_X, float* d_x_next, float* lambda_out)
 {
+    if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, d_x && d_x_gt && p && reg && d_chunk && d_X && d_x_next, "null argument");
     SD_REQUIRE(ctx, N_local >= 0 && L >= 1 && n_global >= 1 && n_global <= INT_MAX, "bad sample / landmark count");
     SD_REQUIRE(ctx, chunk_rows >= 1, "chunk_rows must be >= 1");
@@ -372,7 +395,8 @@ int train_level(sd_ctx* ctx, sd_comm* comm, const HogSource& src, const float* d
     SD_REQUIRE(ctx, ld >= (int64_t)D + P, "ld < D + 2L");
     SD_REQUIRE(ctx, !d_templates || (chunk_rows >= N_local && ldt >= D), "templates need one chunk (chunk_rows >= N_local) and ldt >= D");
     SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
-    int rc = src.host ? gather_prepare(ctx, *src.host, N_local, d_stage, stage_bytes) : SD_OK;
+    HostGather g{};
+    int rc = frames_prepare(ctx, frames, g, N_local);
     if (rc) return rc;
     float* mu = (float*)sd_workspace(ctx, SD_WS_LEVEL, (size_t)D * (P + 1) * sizeof(float));
     if (!mu) return SD_ERR_CUDA;
@@ -388,7 +412,7 @@ int train_level(sd_ctx* ctx, sd_comm* comm, const HogSource& src, const float* d
     const bool shifted = D > SD_LU_MAX_DIM && !reg->regularise_last_row;     // otherwise sd_centre_features leaves mu = 0
     for (int k = 0; k < chunks; ++k) {
         const int r0 = k * chunk_rows, rows = N_local - r0 < chunk_rows ? N_local - r0 : chunk_rows;
-        rc = hog_rows(ctx, src, d_x, r0, rows, L, hog_eyes, p, d_chunk, ld);                                           // :173-189
+        rc = hog_rows(ctx, *frames, g, d_x, r0, rows, L, hog_eyes, p, d_chunk, ld);                                    // :173-189
         if (!rc && d_templates) rc = sd_subtract_templates(ctx, d_chunk, ld, d_templates, ldt, rows, D);             // :191-197
         if (!rc) rc = sd_cascade_targets(ctx, d_x + (int64_t)r0 * P, d_x_gt + (int64_t)r0 * P, rows, P, norm, B, ld); // :199-205
         if (!rc) rc = k == 0 ? sd_centre_features(ctx, c, d_chunk, ld, rows, D, (int)n0, reg, mu)
@@ -403,19 +427,19 @@ int train_level(sd_ctx* ctx, sd_comm* comm, const HogSource& src, const float* d
     rc = sd_cascade_update(ctx, d_chunk, ld, N_local - last, D, Xc, P, d_x + (int64_t)last * P, norm, d_x_next + (int64_t)last * P);
     for (int k = 0; !rc && k + 1 < chunks; ++k) {
         const int r0 = k * chunk_rows;
-        rc = hog_rows(ctx, src, d_x, r0, chunk_rows, L, hog_eyes, p, d_chunk, ld);
+        rc = hog_rows(ctx, *frames, g, d_x, r0, chunk_rows, L, hog_eyes, p, d_chunk, ld);
         if (!rc && shifted) rc = sd_shift_rows(ctx, d_chunk, ld, chunk_rows, D, mu);
         if (!rc) rc = sd_cascade_update(ctx, d_chunk, ld, chunk_rows, D, Xc, P, d_x + (int64_t)r0 * P, norm, d_x_next + (int64_t)r0 * P);
     }
-    if (!rc && src.host) rc = gather_finish(ctx, *src.host, N_local);
+    if (!rc && !frames->images) rc = gather_finish(ctx, g, N_local);
     return rc;
 }
 
-// superviseddescent.hpp:262-306, 323-344 for either source of HOG rows (see sd_apply_level)
-int apply_level(sd_ctx* ctx, const HogSource& src, const float* d_x, int N, int L, const sd_normalisation* hog_eyes,
-                const sd_hog_param* p, const sd_normalisation* norm, const float* d_templates, int64_t ldt, const float* d_X,
-                float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next, void* d_stage, size_t stage_bytes)
+int sd_apply_level(sd_ctx* ctx, const sd_level_frames* frames, const float* d_x, int N, int L, const sd_normalisation* hog_eyes,
+                   const sd_hog_param* p, const sd_normalisation* norm, const float* d_templates, int64_t ldt, const float* d_X,
+                   float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next)
 {
+    if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, d_x && p && d_X && d_chunk && d_x_next, "null argument");
     SD_REQUIRE(ctx, N >= 0 && L >= 1, "bad sample / landmark count");
     SD_REQUIRE(ctx, chunk_rows >= 1, "chunk_rows must be >= 1");
@@ -424,25 +448,25 @@ int apply_level(sd_ctx* ctx, const HogSource& src, const float* d_x, int N, int 
     SD_REQUIRE(ctx, ld >= D, "ld < D");
     SD_REQUIRE(ctx, !d_templates || ldt >= D, "ldt < D");
     SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
-    int rc = src.host ? gather_prepare(ctx, *src.host, N, d_stage, stage_bytes) : SD_OK;
+    HostGather g{};
+    int rc = frames_prepare(ctx, frames, g, N);
     for (int r0 = 0; !rc && r0 < N; r0 += chunk_rows) {
         const int rows = N - r0 < chunk_rows ? N - r0 : chunk_rows;
-        rc = hog_rows(ctx, src, d_x, r0, rows, L, hog_eyes, p, d_chunk, ld);
+        rc = hog_rows(ctx, *frames, g, d_x, r0, rows, L, hog_eyes, p, d_chunk, ld);
         if (!rc && d_templates) rc = sd_subtract_templates(ctx, d_chunk, ld, d_templates + (int64_t)r0 * ldt, ldt, rows, D);
         if (!rc) rc = sd_cascade_update(ctx, d_chunk, ld, rows, D, d_X, P, d_x + (int64_t)r0 * P, norm, d_x_next + (int64_t)r0 * P);
     }
-    if (!rc && src.host) rc = gather_finish(ctx, *src.host, N);
+    if (!rc && !frames->images) rc = gather_finish(ctx, g, N);
     return rc;
 }
 
-}  // namespace
-
-extern "C" {
-
-int sd_level_chunk_rows(sd_ctx* ctx, sd_comm* comm, int64_t N_local, int D, int M, int route, size_t free_bytes, int* rows_out)
+int sd_level_chunk_rows(sd_ctx* ctx, sd_comm* comm, const sd_level_frames* frames, int64_t N_local, int D, int M, int route,
+                        size_t free_bytes, int* rows_out)
 {
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, rows_out && N_local >= 0 && D >= 1 && M >= 1, "bad argument");
+    int rc = frames ? check_frames(ctx, frames) : SD_OK;
+    if (rc) return rc;
     if (free_bytes == 0) {
         size_t total = 0;
         SD_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -466,6 +490,14 @@ int sd_level_chunk_rows(sd_ctx* ctx, sd_comm* comm, int64_t N_local, int D, int 
         if (ctx->solver_mode == 1 || (nranks > 1 && route == 2))                        // CG's strip-major copy of the system
             add(SD_WS_CGMAT, round_up(n, 128) * round_up(n, 16) * sizeof(float));
     }
+    if (frames && frames->host_frames) {                                                // the staging pair of the gather
+        size_t largest = 0;
+        for (int f = 0; f < frames->num_host_frames; ++f)
+            largest = sd_gray_bytes(frames->host_frames[f]) > largest ? sd_gray_bytes(frames->host_frames[f]) : largest;
+        const size_t half = stage_half(*frames, largest);
+        for (int b = 0; b < 2; ++b)
+            if (half > ctx->stage_bytes[b]) need += half - ctx->stage_bytes[b];
+    }
     // per row: the caller's chunk row and the update's partial sums (sd_cascade_update)
     const size_t per_row = (size_t)ld * sizeof(float) + (size_t)M * sizeof(double);
     const size_t fixed = need + kReserveBytes;
@@ -478,50 +510,6 @@ int sd_level_chunk_rows(sd_ctx* ctx, sd_comm* comm, int64_t N_local, int D, int 
     if (rows > INT_MAX) rows = INT_MAX;
     *rows_out = rows < 1 ? 1 : (int)rows;
     return SD_OK;
-}
-
-int sd_train_level(sd_ctx* ctx, sd_comm* comm, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x,
-                   const float* d_x_gt, int N_local, int L, int64_t n_global, const sd_normalisation* hog_eyes, const sd_hog_param* p,
-                   const sd_normalisation* norm, const float* d_templates, int64_t ldt, const sd_regulariser* reg, int route,
-                   float* d_chunk, int64_t ld, int chunk_rows, float* d_X, float* d_x_next, float* lambda_out)
-{
-    if (!ctx) return SD_ERR_INVALID;
-    SD_REQUIRE(ctx, images, "null argument");
-    return train_level(ctx, comm, HogSource{images, d_image_index, nullptr}, d_x, d_x_gt, N_local, L, n_global, hog_eyes, p, norm,
-                       d_templates, ldt, reg, route, d_chunk, ld, chunk_rows, d_X, d_x_next, lambda_out, nullptr, 0);
-}
-
-int sd_train_level_host(sd_ctx* ctx, sd_comm* comm, const sd_host_frame* frames, int num_frames, const int32_t* d_sample_frame,
-                        const float* d_x, const float* d_x_gt, int N_local, int L, int64_t n_global, const sd_normalisation* hog_eyes,
-                        const sd_hog_param* p, const sd_normalisation* norm, const float* d_templates, int64_t ldt,
-                        const sd_regulariser* reg, int route, float* d_chunk, int64_t ld, int chunk_rows, void* d_stage,
-                        size_t stage_bytes, float* d_X, float* d_x_next, float* lambda_out)
-{
-    if (!ctx) return SD_ERR_INVALID;
-    HostGather g{frames, num_frames, d_sample_frame};
-    return train_level(ctx, comm, HogSource{nullptr, nullptr, &g}, d_x, d_x_gt, N_local, L, n_global, hog_eyes, p, norm, d_templates,
-                       ldt, reg, route, d_chunk, ld, chunk_rows, d_X, d_x_next, lambda_out, d_stage, stage_bytes);
-}
-
-int sd_apply_level(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int N, int L,
-                   const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm, const float* d_templates,
-                   int64_t ldt, const float* d_X, float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next)
-{
-    if (!ctx) return SD_ERR_INVALID;
-    SD_REQUIRE(ctx, images, "null argument");
-    return apply_level(ctx, HogSource{images, d_image_index, nullptr}, d_x, N, L, hog_eyes, p, norm, d_templates, ldt, d_X, d_chunk, ld,
-                       chunk_rows, d_x_next, nullptr, 0);
-}
-
-int sd_apply_level_host(sd_ctx* ctx, const sd_host_frame* frames, int num_frames, const int32_t* d_sample_frame, const float* d_x, int N,
-                        int L, const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
-                        const float* d_templates, int64_t ldt, const float* d_X, float* d_chunk, int64_t ld, int chunk_rows, void* d_stage,
-                        size_t stage_bytes, float* d_x_next)
-{
-    if (!ctx) return SD_ERR_INVALID;
-    HostGather g{frames, num_frames, d_sample_frame};
-    return apply_level(ctx, HogSource{nullptr, nullptr, &g}, d_x, N, L, hog_eyes, p, norm, d_templates, ldt, d_X, d_chunk, ld, chunk_rows,
-                       d_x_next, d_stage, stage_bytes);
 }
 
 int64_t sd_gathered_bytes(const sd_ctx* ctx) { return ctx ? ctx->gathered_bytes : 0; }

@@ -2,9 +2,9 @@
 // HogTransform (:70-195).  The functor keeps the reference's constructor and call signature
 //     cv::Mat operator()(cv::Mat parameters, size_t regressorLevel, int trainingIndex = 0)
 // (one sample, used by predict(), superviseddescent.hpp:332) and exposes its device images, eyes and per-level
-// HOG parameters, with which the optimiser projects ALL samples of a level on the device (sd_train_level,
-// sd_apply_level, or their _host twins when the frames do not fit on the device).  Each distinct image is held once: uploaded to HBM
-// on first use, or kept in host memory; crop / resize / HOG run in sd_hog_batch (sm_90a).
+// HOG parameters, with which the optimiser projects ALL samples of a level on the device (sd_train_level, sd_apply_level).
+// Each distinct image is held once: uploaded to HBM on first use, or kept in host memory when it does not fit; crop / resize /
+// HOG run in sd_hog_batch (sm_90a).
 #pragma once
 
 #include <cstring>
@@ -63,8 +63,8 @@ public:
     }
 
     // The route, chosen once on first use: the distinct frames are uploaded when their grey bytes fit in device_frame_share() of
-    // the free device memory; otherwise they stay in host memory and the optimiser's train() / test() read them level by level
-    // (sd_train_level_host / sd_apply_level_host).  Uploaded frames are copied when the transform is first used; frames kept on the
+    // the free device memory; otherwise they stay in host memory and the optimiser's train() / test() read them level by level.
+    // Uploaded frames are copied when the transform is first used; frames kept on the
     // host are read in place at every level when they are pinned and aligned (sd_host_frame_in_place), and copied once into one
     // pinned buffer otherwise.
     static double& device_frame_share()
@@ -78,38 +78,29 @@ public:
         return !dev->host;
     }
 
-    // What the optimiser hands to sd_train_level / sd_apply_level on the device route: the distinct images resident on the device
-    // (uploaded on first use), the sample -> image index (device_sample_frame), the eye landmarks (eyes()) and the HOG parameters of
-    // a level.
+    // The distinct images resident on the device (uploaded on first use), for the one-sample operator()
     const sd_image_batch& device_batch()
     {
         ensure_ready();
         if (dev->host) throw std::runtime_error("HogTransform: the frames stay in host memory (they do not fit on the device); only the optimiser's train() / test() / predict() read them");
         return dev->batch;
     }
-    // On the host route: the distinct frames for sd_train_level_host / sd_apply_level_host, and the size of the staging buffer they
-    // need (two halves of at least 48 MB, and of the largest frame's grey bytes)
-    const std::vector<sd_host_frame>& host_frames()
-    {
-        ensure_ready();
-        return dev->frames;
-    }
-    size_t stage_bytes()
-    {
-        size_t half = static_cast<size_t>(48) << 20;
-        for (const sd_host_frame& f : host_frames()) {
-            const size_t grey = static_cast<size_t>(f.height) * ((static_cast<size_t>(f.width) + 15) / 16 * 16);
-            half = grey > half ? grey : half;
-        }
-        return 2 * half;
-    }
-    // Device index of n samples: sample i reads distinct frame device_sample_frame(n)[i], the frame of images[i].  Entries of
-    // `images` with equal data, size and step (rcr-train's shallow copies of one photo) are one frame, held once.
-    const int32_t* device_sample_frame(int n)
+    // What the optimiser hands to sd_train_level / sd_apply_level with the eye landmarks (eyes()) and a level's HOG parameters: the
+    // distinct frames -- on the device, or in host memory -- and the index by which sample i reads the frame of images[i].  Entries
+    // of `images` with equal data, size and step (rcr-train's shallow copies of one photo) are one frame, held once.
+    sd_level_frames level_frames(int n)
     {
         ensure_ready();
         if (n > static_cast<int>(images.size())) throw std::runtime_error("HogTransform: more samples than images");
-        return dev->index.as<int32_t>();
+        sd_level_frames f{};
+        if (dev->host) {
+            f.host_frames = dev->frames.data();
+            f.num_host_frames = static_cast<int32_t>(dev->frames.size());
+        } else {
+            f.images = &dev->batch;
+        }
+        f.d_sample_frame = dev->index.as<int32_t>();
+        return f;
     }
     // number of distinct frames
     int num_frames()

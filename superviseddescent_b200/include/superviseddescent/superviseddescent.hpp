@@ -37,9 +37,9 @@ namespace detail {
 template <class...> struct voider { using type = void; };
 template <class... T> using void_t = typename voider<T...>::type;
 
-// projection whose images are resident on the device, projected there for all rows at once (rcr::HogTransform)
+// projection whose frames a level call reads, projected on the device for all rows at once (rcr::HogTransform)
 template <class P, class = void> struct is_device_projection : std::false_type {};
-template <class P> struct is_device_projection<P, void_t<decltype(std::declval<P&>().device_batch()), decltype(std::declval<P&>().hog_param(size_t(0)))>> : std::true_type {};
+template <class P> struct is_device_projection<P, void_t<decltype(std::declval<P&>().level_frames(0)), decltype(std::declval<P&>().hog_param(size_t(0)))>> : std::true_type {};
 
 template <class N, class = void> struct has_c_normalisation : std::false_type {};
 template <class N> struct has_c_normalisation<N, void_t<decltype(std::declval<const N&>().c_normalisation())>> : std::true_type {};
@@ -179,7 +179,7 @@ private:
                     b.at<float>(i, j) = (current_x.at<float>(i, j) - parameters.at<float>(i, j)) * n.at<float>(0, j);
             }
             regressors[level].learn(observed, b);                                                // :207
-            current_x = apply_level_host(level, observed, current_x);                            // :209-215
+            current_x = update_on_host(level, observed, current_x);                              // :209-215
             cb(current_x);                                                                       // :217
         }
     }
@@ -192,13 +192,13 @@ private:
         for (size_t level = 0; level < regressors.size(); ++level) {
             Mat features = detail::project_on_host(current_x, level, projection);
             Mat observed = templates.empty() ? features : Mat(features - templates);
-            current_x = apply_level_host(level, observed, current_x);
+            current_x = update_on_host(level, observed, current_x);
             cb(current_x);                                                                       // :303
         }
         return current_x;
     }
 
-    cv::Mat apply_level_host(size_t level, const cv::Mat& observed, const cv::Mat& current_x)
+    cv::Mat update_on_host(size_t level, const cv::Mat& observed, const cv::Mat& current_x)
     {
         cv::Mat update = regressors[level].predict(observed);      // one batched GPU GEMM instead of N GEMVs
         cv::Mat x_k(current_x.rows, current_x.cols, CV_32FC1);
@@ -214,11 +214,11 @@ private:
     int comm_route = 0;
 
     // feature rows per chunk of a device-route level: set_rows_per_chunk's (at most n), or as many as fit
-    int chunk_rows(sd_ctx* ctx, sd_comm* c, int n, int D, int Pd, int route) const
+    int chunk_rows(sd_ctx* ctx, sd_comm* c, const sd_level_frames& frames, int n, int D, int Pd, int route) const
     {
         if (rows_per_chunk > 0) return rows_per_chunk < n ? rows_per_chunk : (n > 0 ? n : 1);
         int rows = 0;
-        sd_b200::check(ctx, sd_level_chunk_rows(ctx, c, n, D, Pd, route, 0, &rows), "sd_level_chunk_rows");
+        sd_b200::check(ctx, sd_level_chunk_rows(ctx, c, &frames, n, D, Pd, route, 0, &rows), "sd_level_chunk_rows");
         return rows;
     }
 
@@ -233,10 +233,7 @@ private:
         sd_b200::upload(initialisations, d_cur, Pd);
         const sd_normalisation norm = normalisation_strategy.c_normalisation();
         const sd_normalisation eyes = projection.eyes();
-        const int32_t* d_frame = projection.device_sample_frame(n);
-        // frames on the device, or host frames read through a staging buffer (allocated before the chunk query sizes the chunk)
-        const bool on_device = projection.on_device();
-        sd_b200::DeviceBuffer stage(on_device ? 0 : projection.stage_bytes());
+        const sd_level_frames frames = projection.level_frames(n);
         if (!templates.empty()) sd_b200::upload(templates, d_tmpl, templates.cols);
         sd_b200::DeviceBuffer X;
         int64_t n_global = n;
@@ -252,16 +249,12 @@ private:
             const bool want_rank = detail::reports_rank<RegressorType>::value;
             if (want_rank) sd_b200::check(ctx, sd_set_rank_diagnostic(ctx, 1), "sd_set_rank_diagnostic");   // counted by the chunk query
             // 1)-4) :173-215 -- features, targets, Gram, exchange, solve and update through a buffer of `rows` feature rows
-            const int rows = templates.empty() ? chunk_rows(ctx, c, n, D, Pd, route) : (n > 0 ? n : 1);
+            const int rows = templates.empty() ? chunk_rows(ctx, c, frames, n, D, Pd, route) : (n > 0 ? n : 1);
             sd_b200::DeviceBuffer chunk(static_cast<size_t>(rows) * ld * sizeof(float));
             X.allocate(static_cast<size_t>(D) * Pd * sizeof(float));
             const float* tmpl = templates.empty() ? nullptr : d_tmpl.as<float>();
-            const int rc = on_device
-                ? sd_train_level(ctx, c, &projection.device_batch(), d_frame, d_cur.as<float>(), d_gt.as<float>(), n, Pd / 2, n_global, &eyes, &hp,
-                                 &norm, tmpl, templates.cols, &reg, route, chunk.as<float>(), ld, rows, X.as<float>(), d_next.as<float>(), nullptr)
-                : sd_train_level_host(ctx, c, projection.host_frames().data(), static_cast<int>(projection.host_frames().size()), d_frame,
-                                      d_cur.as<float>(), d_gt.as<float>(), n, Pd / 2, n_global, &eyes, &hp, &norm, tmpl, templates.cols, &reg, route,
-                                      chunk.as<float>(), ld, rows, stage.as<void>(), stage.bytes(), X.as<float>(), d_next.as<float>(), nullptr);
+            const int rc = sd_train_level(ctx, c, &frames, d_cur.as<float>(), d_gt.as<float>(), n, Pd / 2, n_global, &eyes, &hp, &norm, tmpl,
+                                          templates.cols, &reg, route, chunk.as<float>(), ld, rows, X.as<float>(), d_next.as<float>(), nullptr);
             if (want_rank) {
                 sd_set_rank_diagnostic(ctx, 0);
                 detail::report_rank(regressors[level], sd_last_rank(ctx), D, detail::reports_rank<RegressorType>());
@@ -307,27 +300,18 @@ private:
         sd_b200::upload(initialisations, d_cur, Pd);
         const sd_normalisation norm = normalisation_strategy.c_normalisation();
         const sd_normalisation eyes = projection.eyes();
-        const int32_t* d_frame = projection.device_sample_frame(n);
-        const bool on_device = projection.on_device();
-        sd_b200::DeviceBuffer stage(on_device ? 0 : projection.stage_bytes());
+        const sd_level_frames frames = projection.level_frames(n);
         if (!templates.empty()) sd_b200::upload(templates, d_tmpl, templates.cols);
         for (size_t level = 0; level < regressors.size(); ++level) {
             const int D = projection.feature_length(level);
             const int64_t ld = (static_cast<int64_t>(D) + 3) / 4 * 4;
             const sd_hog_param hp = projection.hog_param(level);
-            const int rows = chunk_rows(ctx, nullptr, n, D, Pd, 0);
+            const int rows = chunk_rows(ctx, nullptr, frames, n, D, Pd, 0);
             sd_b200::DeviceBuffer chunk(static_cast<size_t>(rows) * ld * sizeof(float));
             const float* tmpl = templates.empty() ? nullptr : d_tmpl.as<float>();
-            if (on_device)
-                sd_b200::check(ctx, sd_apply_level(ctx, &projection.device_batch(), d_frame, d_cur.as<float>(), n, Pd / 2, &eyes, &hp, &norm, tmpl,
-                                                   templates.cols, regressors[level].device_x(), chunk.as<float>(), ld, rows, d_next.as<float>()),
-                               "sd_apply_level");
-            else
-                sd_b200::check(ctx, sd_apply_level_host(ctx, projection.host_frames().data(), static_cast<int>(projection.host_frames().size()), d_frame,
-                                                        d_cur.as<float>(), n, Pd / 2, &eyes, &hp, &norm, tmpl, templates.cols,
-                                                        regressors[level].device_x(), chunk.as<float>(), ld, rows, stage.as<void>(), stage.bytes(),
-                                                        d_next.as<float>()),
-                               "sd_apply_level_host");
+            sd_b200::check(ctx, sd_apply_level(ctx, &frames, d_cur.as<float>(), n, Pd / 2, &eyes, &hp, &norm, tmpl, templates.cols,
+                                               regressors[level].device_x(), chunk.as<float>(), ld, rows, d_next.as<float>()),
+                           "sd_apply_level");
             std::swap(d_cur, d_next);
             if (want_callback) cb(sd_b200::download(d_cur.as<float>(), n, Pd, Pd));                          // :303
         }

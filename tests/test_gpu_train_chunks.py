@@ -212,14 +212,15 @@ def test_invalid_arguments_leave_the_outputs_unwritten(sd, setup):
     X = torch.full((D, P), 7.0, device="cuda")
     nxt = torch.full((n, P), 7.0, device="cuda")
     eyes, reg = ht.norm.c(), sd.Regulariser(sd.RegularisationType.MatrixNorm, 1.5, False).c()
+    frames = ht.level_frames(n)
 
     def train(chunk_rows=n, ld_=ld, t=None, x_next=nxt):
-        return lib.sd_train_level(ctx.h, None, C.byref(ht.batch()), None, ptr(cur), ptr(gt), n, P // 2, C.c_int64(n), C.byref(eyes),
+        return lib.sd_train_level(ctx.h, None, C.byref(frames), ptr(cur), ptr(gt), n, P // 2, C.c_int64(n), C.byref(eyes),
                                   C.byref(ht.hog_params[0]), C.byref(eyes), ptr(t), C.c_int64(D), C.byref(reg), 0, ptr(buf),
                                   C.c_int64(ld_), chunk_rows, ptr(X), ptr(x_next), None)
 
     def apply(chunk_rows=n, ld_=ld, x_next=nxt):
-        return lib.sd_apply_level(ctx.h, C.byref(ht.batch()), None, ptr(cur), n, P // 2, C.byref(eyes), C.byref(ht.hog_params[0]),
+        return lib.sd_apply_level(ctx.h, C.byref(frames), ptr(cur), n, P // 2, C.byref(eyes), C.byref(ht.hog_params[0]),
                                   C.byref(eyes), None, C.c_int64(0), ptr(X), ptr(buf), C.c_int64(ld_), chunk_rows, ptr(x_next))
 
     launches = ctx.launches()
@@ -233,7 +234,7 @@ def test_invalid_arguments_leave_the_outputs_unwritten(sd, setup):
     assert np.array_equal(cur.cpu().numpy(), x0)
 
 
-def test_chunk_query(sd):
+def test_chunk_query_counts_host_staging(sd):
     ctx = sd.default_context()
     lib = sd._capi.lib()
     import torch
@@ -243,16 +244,26 @@ def test_chunk_query(sd):
     P = 44
     ld = (D + P + 3) // 4 * 4
     rows = C.c_int(0)
-    assert lib.sd_level_chunk_rows(ctx.h, None, C.c_int64(10000), D, P, 0, C.c_size_t(0), C.byref(rows)) == 0
+    assert lib.sd_level_chunk_rows(ctx.h, None, None, C.c_int64(10000), D, P, 0, C.c_size_t(0), C.byref(rows)) == 0
     assert rows.value == 10000
     free = torch.cuda.mem_get_info()[0]
-    assert lib.sd_level_chunk_rows(ctx.h, None, C.c_int64(4000000), D, P, 0, C.c_size_t(free), C.byref(rows)) == 0
+    assert lib.sd_level_chunk_rows(ctx.h, None, None, C.c_int64(4000000), D, P, 0, C.c_size_t(free), C.byref(rows)) == 0
     print(f"D = {D}: {rows.value} rows of {ld * 4} bytes fit in {free / 1e9:.1f} GB")
     assert 0 < rows.value < 4000000
     assert rows.value * ld * 4 + (512 << 20) <= free
     # not even the minimal chunk fits (256 MB is below the reserve, whatever the context already holds): an error naming D
-    assert lib.sd_level_chunk_rows(ctx.h, None, C.c_int64(4000000), D, P, 0, C.c_size_t(256 << 20), C.byref(rows)) == 2
+    assert lib.sd_level_chunk_rows(ctx.h, None, None, C.c_int64(4000000), D, P, 0, C.c_size_t(256 << 20), C.byref(rows)) == 2
     assert "17051" in lib.sd_last_error(ctx.h).decode()
+    # host frames: the staging pair the level will hold is counted too (a fresh context holds none of it yet)
+    fresh = sd.Context(ctx.device)
+    img = np.zeros((16, 16), dtype=np.uint8)
+    frames = sd.LevelFramesC(num_host_frames=1, stage_half_bytes=1 << 30)
+    frames.host_frames = C.pointer(sd._host_frame(img)[0])
+    dev_rows, host_rows = C.c_int(0), C.c_int(0)
+    assert lib.sd_level_chunk_rows(fresh.h, None, None, C.c_int64(4000000), D, P, 0, C.c_size_t(free), C.byref(dev_rows)) == 0
+    assert lib.sd_level_chunk_rows(fresh.h, None, C.byref(frames), C.c_int64(4000000), D, P, 0, C.c_size_t(free), C.byref(host_rows)) == 0
+    pair_rows = (2 << 30) // (ld * 4 + P * 8)
+    assert dev_rows.value - host_rows.value in (pair_rows, pair_rows + 1)
 
 
 def _free_port():

@@ -1,8 +1,8 @@
-"""Cascade levels on frames that stay in host memory (sd_train_level_host, sd_apply_level_host) and HogTransform's frames shared by
-several samples.
+"""Cascade levels on frames that stay in host memory (sd_train_level, sd_apply_level with sd_level_frames.host_frames) and
+HogTransform's frames shared by several samples.
 
-The host route must give bit for bit what sd_train_level / sd_apply_level give on the same frames uploaded by sd_upload_frames:
-the HOG kernel reads the same bytes, gathered from the planned regions instead of whole resident frames."""
+The host route must give bit for bit what the device route gives on the same frames uploaded by sd_upload_frames: the HOG kernel
+reads the same bytes, gathered from the planned regions instead of whole resident frames."""
 import ctypes as C
 
 import numpy as np
@@ -90,11 +90,23 @@ def _eyes(sd, ids):
     return sd.InterEyeDistanceNormalisation(ids, REYE, LEYE).c()
 
 
-def _train(sd, S, hp, host, chunk_rows, stage_bytes=None, eyes_on=True):
+def _frames(sd, S, host, idx, stage_half=0, table=None):
+    """the sd_level_frames of the setup's frames: host frames (table, default the setup's) or the uploaded batch"""
+    f = sd.LevelFramesC(d_sample_frame=sd._capi.ptr(idx), stage_half_bytes=stage_half)
+    if host:
+        f.host_frames, f.num_host_frames = table if table is not None else S["table"], S["nf"]
+    else:
+        f.images = C.pointer(S["ib"])
+    return f
+
+
+def _train(sd, S, hp, host, chunk_rows, stage_half=0, eyes_on=True, rows=None):
+    """one training level on the samples `rows` (default all) of the setup; rows given: sample i reads frame i (index NULL)"""
     import torch
     ctx, lib, ptr = S["ctx"], sd._capi.lib(), sd._capi.ptr
-    x0, xg = torch.from_numpy(S["x0"]).cuda(), torch.from_numpy(S["x_gt"]).cuda()
-    idx = torch.from_numpy(S["frames"]).cuda()
+    sel = slice(None) if rows is None else rows
+    x0, xg = torch.from_numpy(S["x0"][sel]).cuda(), torch.from_numpy(S["x_gt"][sel]).cuda()
+    idx = torch.from_numpy(S["frames"]).cuda() if rows is None else None
     n, P = x0.shape
     p = sd.HoGParam(*hp)
     D = lib.sd_hog_feature_length(P // 2, C.byref(p))
@@ -106,25 +118,19 @@ def _train(sd, S, hp, host, chunk_rows, stage_bytes=None, eyes_on=True):
     norm = _eyes(sd, S["ids"])
     eyes = C.byref(norm) if eyes_on else None
     reg = sd.Regulariser(sd.RegularisationType.MatrixNorm, 1.5, False).c()
-    if host:
-        stage = torch.empty(stage_bytes, dtype=torch.uint8, device="cuda")
-        rc = lib.sd_train_level_host(ctx.h, None, S["table"], S["nf"], ptr(idx), ptr(x0), ptr(xg), n, P // 2, C.c_int64(n), eyes, C.byref(p),
-                                     C.byref(norm), None, C.c_int64(0), C.byref(reg), 0, ptr(buf), C.c_int64(ld), chunk_rows, ptr(stage),
-                                     C.c_size_t(stage_bytes), ptr(X), ptr(nxt), C.byref(lam))
-    else:
-        rc = lib.sd_train_level(ctx.h, None, C.byref(S["ib"]), ptr(idx), ptr(x0), ptr(xg), n, P // 2, C.c_int64(n), eyes, C.byref(p),
-                                C.byref(norm), None, C.c_int64(0), C.byref(reg), 0, ptr(buf), C.c_int64(ld), chunk_rows, ptr(X), ptr(nxt),
-                                C.byref(lam))
+    frames = _frames(sd, S, host, idx, stage_half)
+    rc = lib.sd_train_level(ctx.h, None, C.byref(frames), ptr(x0), ptr(xg), n, P // 2, C.c_int64(n), eyes, C.byref(p), C.byref(norm), None,
+                            C.c_int64(0), C.byref(reg), 0, ptr(buf), C.c_int64(ld), chunk_rows, ptr(X), ptr(nxt), C.byref(lam))
     assert rc == 0, lib.sd_last_error(ctx.h).decode()
     ctx.sync()
     return X.cpu().numpy(), lam.value, nxt.cpu().numpy()
 
 
-def _apply(sd, S, hp, X, host, chunk_rows, stage_bytes=None, eyes_on=True):
+def _apply(sd, S, hp, X, host, chunk_rows, stage_half=0, eyes_on=True, rows=None):
     import torch
     ctx, lib, ptr = S["ctx"], sd._capi.lib(), sd._capi.ptr
-    x0 = torch.from_numpy(S["x0"]).cuda()
-    idx = torch.from_numpy(S["frames"]).cuda()
+    x0 = torch.from_numpy(S["x0"][slice(None) if rows is None else rows]).cuda()
+    idx = torch.from_numpy(S["frames"]).cuda() if rows is None else None
     n, P = x0.shape
     p = sd.HoGParam(*hp)
     D = lib.sd_hog_feature_length(P // 2, C.byref(p))
@@ -134,13 +140,9 @@ def _apply(sd, S, hp, X, host, chunk_rows, stage_bytes=None, eyes_on=True):
     nxt = torch.full((n, P), 7.0, device="cuda")
     norm = _eyes(sd, S["ids"])
     eyes = C.byref(norm) if eyes_on else None
-    if host:
-        stage = torch.empty(stage_bytes, dtype=torch.uint8, device="cuda")
-        rc = lib.sd_apply_level_host(ctx.h, S["table"], S["nf"], ptr(idx), ptr(x0), n, P // 2, eyes, C.byref(p), C.byref(norm), None,
-                                     C.c_int64(0), ptr(Xd), ptr(buf), C.c_int64(ld), chunk_rows, ptr(stage), C.c_size_t(stage_bytes), ptr(nxt))
-    else:
-        rc = lib.sd_apply_level(ctx.h, C.byref(S["ib"]), ptr(idx), ptr(x0), n, P // 2, eyes, C.byref(p), C.byref(norm), None, C.c_int64(0),
-                                ptr(Xd), ptr(buf), C.c_int64(ld), chunk_rows, ptr(nxt))
+    frames = _frames(sd, S, host, idx, stage_half)
+    rc = lib.sd_apply_level(ctx.h, C.byref(frames), ptr(x0), n, P // 2, eyes, C.byref(p), C.byref(norm), None, C.c_int64(0), ptr(Xd),
+                            ptr(buf), C.c_int64(ld), chunk_rows, ptr(nxt))
     assert rc == 0, lib.sd_last_error(ctx.h).decode()
     ctx.sync()
     return nxt.cpu().numpy()
@@ -153,25 +155,35 @@ def _largest_grey():
 @pytest.mark.parametrize("hp", [ADAPTIVE, FIXED], ids=["adaptive", "fixed"])
 @pytest.mark.parametrize("chunk", ["one", "several"])
 @pytest.mark.parametrize("stage", ["roomy", "tight"])
-def test_host_level_is_the_device_level(sd, setup, hp, chunk, stage):
+def test_host_route_level_is_the_device_level(sd, setup, hp, chunk, stage):
     S = setup
     n = S["x0"].shape[0]
     rows = n if chunk == "one" else 29
-    stage_bytes = (64 << 20) if stage == "roomy" else 2 * _largest_grey()     # tight: a batch holds about one frame's regions
+    stage_half = (32 << 20) if stage == "roomy" else _largest_grey()          # tight: a batch holds about one frame's regions
     eyes_on = hp is ADAPTIVE
     gathered = sd._capi.lib().sd_gathered_bytes(S["ctx"].h)
     want = _train(sd, S, hp, False, rows, eyes_on=eyes_on)
-    got = _train(sd, S, hp, True, rows, stage_bytes, eyes_on=eyes_on)
+    got = _train(sd, S, hp, True, rows, stage_half, eyes_on=eyes_on)
     assert sd._capi.lib().sd_gathered_bytes(S["ctx"].h) > gathered
     assert np.array_equal(got[0], want[0]) and got[1] == want[1] and np.array_equal(got[2], want[2])
     # the sample outside its frame moved like every other (its HOG rows are the zero rows the device route gives)
     assert np.isfinite(got[2]).all()
     a_want = _apply(sd, S, hp, want[0], False, rows, eyes_on=eyes_on)
-    a_got = _apply(sd, S, hp, want[0], True, rows, stage_bytes, eyes_on=eyes_on)
+    a_got = _apply(sd, S, hp, want[0], True, rows, stage_half, eyes_on=eyes_on)
     assert np.array_equal(a_got, a_want)
 
 
-def test_bad_frames_and_staging_are_refused_before_any_work(sd, setup):
+def test_host_level_without_an_index_reads_frame_i(sd, setup):
+    """d_sample_frame NULL on the host route: sample i reads frame i, as with the identity index"""
+    S = setup
+    first = [int(np.flatnonzero(S["frames"] == f)[0]) for f in range(S["nf"])]   # one sample of each frame, in frame order
+    want = _train(sd, S, ADAPTIVE, False, len(first), rows=first)
+    got = _train(sd, S, ADAPTIVE, True, len(first), rows=first)
+    assert np.array_equal(got[0], want[0]) and got[1] == want[1] and np.array_equal(got[2], want[2])
+    assert np.array_equal(_apply(sd, S, ADAPTIVE, want[0], True, 4, rows=first), _apply(sd, S, ADAPTIVE, want[0], False, 4, rows=first))
+
+
+def test_bad_frames_are_refused_before_any_work(sd, setup):
     import torch
     S = setup
     ctx, lib, ptr = S["ctx"], sd._capi.lib(), sd._capi.ptr
@@ -186,14 +198,12 @@ def test_bad_frames_and_staging_are_refused_before_any_work(sd, setup):
     nxt = torch.full((n, P), 7.0, device="cuda")
     norm = _eyes(sd, S["ids"])
     reg = sd.Regulariser(sd.RegularisationType.MatrixNorm, 1.5, False).c()
-    stage = torch.empty(64 << 20, dtype=torch.uint8, device="cuda")
 
-    def calls(table, stage_bytes):
-        t = lib.sd_train_level_host(ctx.h, None, table, S["nf"], ptr(idx), ptr(x0), ptr(xg), n, P // 2, C.c_int64(n), C.byref(norm),
-                                    C.byref(p), C.byref(norm), None, C.c_int64(0), C.byref(reg), 0, ptr(buf), C.c_int64(ld), n, ptr(stage),
-                                    C.c_size_t(stage_bytes), ptr(X), ptr(nxt), None)
-        a = lib.sd_apply_level_host(ctx.h, table, S["nf"], ptr(idx), ptr(x0), n, P // 2, C.byref(norm), C.byref(p), C.byref(norm), None,
-                                    C.c_int64(0), ptr(X), ptr(buf), C.c_int64(D + 3 & ~3), n, ptr(stage), C.c_size_t(stage_bytes), ptr(nxt))
+    def calls(frames):
+        t = lib.sd_train_level(ctx.h, None, C.byref(frames), ptr(x0), ptr(xg), n, P // 2, C.c_int64(n), C.byref(norm), C.byref(p),
+                               C.byref(norm), None, C.c_int64(0), C.byref(reg), 0, ptr(buf), C.c_int64(ld), n, ptr(X), ptr(nxt), None)
+        a = lib.sd_apply_level(ctx.h, C.byref(frames), ptr(x0), n, P // 2, C.byref(norm), C.byref(p), C.byref(norm), None, C.c_int64(0),
+                               ptr(X), ptr(buf), C.c_int64(D + 3 & ~3), n, ptr(nxt))
         return t, a
 
     recs = [S["table"][i] for i in range(S["nf"])]
@@ -205,14 +215,16 @@ def test_bad_frames_and_staging_are_refused_before_any_work(sd, setup):
     bad_stride[0] = sd.HostFrameC(r.h_data, r.width - 8, r.height, r.row_stride - 8, r.channels)   # pitch 152: not a multiple of 16
     launches = ctx.launches()
     for table in (bad_pin, bad_stride):
-        assert calls((sd.HostFrameC * len(table))(*table), 64 << 20) == (1, 1)
-    assert calls(S["table"], 2 * _largest_grey() - 32) == (1, 1)          # a staging half below the largest frame
+        assert calls(_frames(sd, S, True, idx, table=(sd.HostFrameC * len(table))(*table))) == (1, 1)
+    both = _frames(sd, S, True, idx)
+    both.images = C.pointer(S["ib"])
+    assert calls(both) == (1, 1) and calls(sd.LevelFramesC(d_sample_frame=ptr(idx))) == (1, 1)   # exactly one source of frames
     assert ctx.launches() == launches
     ctx.sync()
     assert bool((X == 7.0).all()) and bool((nxt == 7.0).all())
     # an index out of range is the projection's status flag, reported by the next synchronising call
     idx[5] = 99
-    assert calls(S["table"], 64 << 20) == (0, 0)
+    assert calls(_frames(sd, S, True, idx)) == (0, 0)
     with pytest.raises(sd.SdError) as e:
         ctx.sync()
     assert e.value.code == 1 and "out of range" in str(e.value)
