@@ -133,6 +133,8 @@ SD_API int sd_ctx_create(int device, void* stream, sd_ctx** out);
 SD_API void sd_ctx_destroy(sd_ctx* ctx);
 SD_API const char* sd_last_error(const sd_ctx* ctx);
 SD_API int sd_sync(sd_ctx* ctx);
+/* the cudaStream_t the context runs on (what sd_ctx_create was given, or the stream it created) */
+SD_API void* sd_ctx_stream(const sd_ctx* ctx);
 SD_API const char* sd_version(void);
 /* number of kernels of THIS library launched on ctx since creation (bench.py's gpu_launches) */
 SD_API int64_t sd_launch_count(const sd_ctx* ctx);
@@ -370,7 +372,8 @@ typedef struct {
  * on several ranks), the band buffer of the exchange on several ranks, the bias / inverse workspaces and, for host frames, the
  * staging pair (sized by the largest frame of the table) -- less what the context already holds, and a reserve of 512 MB for small
  * workspaces.  frames may be NULL (no staging).  free_bytes == 0: cudaMemGetInfo.  Returns N_local (at least 1) when everything
- * fits; SD_ERR_CUDA, with a message naming D, when not even min(N_local, 256) rows fit.  M = 2L.
+ * fits; SD_ERR_CUDA, with a message naming D, when not even min(N_local, 256) rows fit.  M = the parameter width P (2L for HOG
+ * levels).  It serves the projected levels below unchanged: D = feature_length, M = P, frames = NULL.
  *
  * sd_train_level: one training level (superviseddescent.hpp:173-217) for the HOG projection (frames as above, hog_eyes as in
  * sd_hog_batch).  d_x, d_x_gt: N_local x 2L current / ground-truth landmarks; norm: the optimiser's normalisation; d_templates:
@@ -404,6 +407,54 @@ SD_API int sd_apply_level(sd_ctx* ctx, const sd_level_frames* frames, const floa
                           const sd_normalisation* hog_eyes, const sd_hog_param* p, const sd_normalisation* norm,
                           const float* d_templates, int64_t ldt, const float* d_X,
                           float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next);
+
+/* ---- cascade levels on the caller's projection ------------------------------------------------------------------------------
+ * The reference's ProjectionFunction is any h(x_row, level, index) (examples/simple_function.cpp, pose_estimation.cpp).  A
+ * projection that can run on the device hands the level its feature rows through a callback; everything after the rows --
+ * templates, targets, the pilot shift, the Gram in chunks, the exchange, the solve and the update -- is the loop of sd_train_level /
+ * sd_apply_level, with the same rules:
+ *   - targets go in columns [D, D + P) of the chunk buffer (ld >= D + P in training, ld >= D in apply);
+ *   - centring and the pilot shift apply only when D > 256, the last column is exactly ones and the bias is not regularised;
+ *   - templates need one chunk; route and comm as in sd_train_level, and every rank makes the same collectives (on several ranks
+ *     two more than sd_train_level: the failure agreement below);
+ *   - for a fixed chunk_rows and rank count the result is reproducible bit for bit (given a deterministic callback).
+ * P is any parameter width (6 for the pose example).  norm->kind == 1 (inter-eye distance) needs an even P and eye indices below
+ * P / 2.
+ *
+ * The callback writes the features of parameter rows [first_row, first_row + rows) of this rank into columns [0, feature_length)
+ * of d_out (row pitch ld floats); d_x points at row first_row (pitch ldx floats).  It returns 0, or non-zero to fail the level.
+ *   - Its work must be ordered on sd_ctx_stream(ctx): it enqueues there, or synchronises its own stream before it returns.
+ *   - It must not write outside columns [0, feature_length) of its `rows` rows of d_out.
+ *   - It may call sd_hog_batch, sd_bgr2gray and the memcpy / memset entry points on ctx.  It must not call any learn, solve, level
+ *     or detect entry point on ctx: those share the level's workspaces.
+ *   - In training it is called twice for every chunk but the last (once for the Gram, once for the update), so it must be
+ *     deterministic.  It is never called with rows == 0.
+ *   - Its own device memory is not counted by sd_level_chunk_rows, which leaves it only the 512 MB reserve: a callback that
+ *     needs scratch per row should pass free_bytes less that scratch to the query, or choose chunk_rows itself.
+ * Errors: a non-zero return fails the level with SD_ERR_INVALID and the message "projection callback returned N".  On several
+ * ranks a callback that fails on one rank fails the level on every rank (the others report "the projection callback failed on
+ * another rank"): the failing rank still takes part in the collectives up to the exchange, and the ranks agree on failures
+ * before the exchange and at the end of the level (one host integer each).  Any other error on one rank is, as for
+ * sd_train_level, not agreed on: the other ranks may wait in a collective.  A NULL fn,
+ * feature_length < 1, P < 1, a normalisation P cannot carry, ld below the rule above, and the argument errors of sd_train_level /
+ * sd_apply_level are SD_ERR_INVALID before any work is queued (outputs unwritten, the callback not called). */
+typedef int (*sd_project_fn)(void* user, sd_ctx* ctx, int level, const float* d_x, int64_t ldx, int64_t first_row, int rows,
+                             float* d_out, int64_t ld);
+typedef struct {
+    sd_project_fn fn;
+    void* user;                  /* passed to fn unchanged */
+    int32_t level;               /* passed to fn: the reference's regressorLevel */
+    int32_t feature_length;      /* D */
+} sd_level_projection;
+SD_API int sd_train_level_projected(sd_ctx* ctx, sd_comm* comm, const sd_level_projection* proj,
+                                    const float* d_x, const float* d_x_gt, int N_local, int P, int64_t n_global,
+                                    const sd_normalisation* norm, const float* d_templates, int64_t ldt,
+                                    const sd_regulariser* reg, int route, float* d_chunk, int64_t ld, int chunk_rows,
+                                    float* d_X, float* d_x_next, float* lambda_out);
+SD_API int sd_apply_level_projected(sd_ctx* ctx, const sd_level_projection* proj, const float* d_x, int N, int P,
+                                    const sd_normalisation* norm, const float* d_templates, int64_t ldt, const float* d_X,
+                                    float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next);
+
 /* host-frame bytes (region bytes x channels) the levels on host frames have read over PCIe on ctx since creation */
 SD_API int64_t sd_gathered_bytes(const sd_ctx* ctx);
 /* *in_place = 1 when the levels can read a host frame where it is (pinned and device-mapped, 16-byte aligned base and

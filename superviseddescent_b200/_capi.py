@@ -55,9 +55,18 @@ class LevelFramesC(C.Structure):
                 ("d_sample_frame", C.c_void_p), ("stage_half_bytes", C.c_size_t)]
 
 
+# sd_project_fn(user, ctx, level, d_x, ldx, first_row, rows, d_out, ld) -> 0 or non-zero
+ProjectFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int64)
+
+
+class LevelProjectionC(C.Structure):
+    """sd_level_projection: the callback that writes a level's feature rows on the device, and its feature length."""
+    _fields_ = [("fn", ProjectFn), ("user", C.c_void_p), ("level", C.c_int32), ("feature_length", C.c_int32)]
+
+
 # every symbol declared in include/sd_b200.h (tests/test_abi.py checks the list against the header)
 EXPORTS = [
-    "sd_ctx_create", "sd_ctx_destroy", "sd_last_error", "sd_sync", "sd_version", "sd_launch_count", "sd_roi_fallback_count",
+    "sd_ctx_create", "sd_ctx_destroy", "sd_last_error", "sd_sync", "sd_ctx_stream", "sd_version", "sd_launch_count", "sd_roi_fallback_count",
     "sd_malloc", "sd_free", "sd_host_alloc", "sd_host_free", "sd_memcpy_h2d", "sd_memcpy_d2h", "sd_memset",
     "sd_memcpy2d_h2d", "sd_memcpy2d_d2h", "sd_memcpy2d_d2d",
     "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_bgr2gray", "sd_upload_frames",
@@ -66,7 +75,7 @@ EXPORTS = [
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",
     "sd_comm_sum_int64", "sd_comm_allgather", "sd_allreduce_gram", "sd_reduce_scatter_gram", "sd_solve_gram_dist", "sd_learn_dist",
     "sd_cascade_targets", "sd_cascade_update", "sd_subtract_templates", "sd_level_chunk_rows", "sd_train_level", "sd_apply_level",
-    "sd_gathered_bytes", "sd_host_frame_in_place", "sd_device_memory",
+    "sd_train_level_projected", "sd_apply_level_projected", "sd_gathered_bytes", "sd_host_frame_in_place", "sd_device_memory",
     "sd_model_load", "sd_model_save", "sd_model_create", "sd_model_destroy", "sd_model_num_levels",
     "sd_model_num_landmarks", "sd_model_hog_param", "sd_model_regulariser", "sd_model_normalisation",
     "sd_model_get_mean", "sd_model_get_weights", "sd_model_landmark_id", "sd_align_mean",
@@ -103,6 +112,13 @@ def lib():
         l.sd_last_rank.argtypes = [C.c_void_p]
         l.sd_comm_rank.argtypes = [C.c_void_p]
         l.sd_comm_size.argtypes = [C.c_void_p]
+        l.sd_ctx_stream.restype = C.c_void_p
+        l.sd_ctx_stream.argtypes = [C.c_void_p]
+        l.sd_train_level_projected.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(LevelProjectionC), C.c_void_p, C.c_void_p, C.c_int,
+                                               C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p,
+                                               C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        l.sd_apply_level_projected.argtypes = [C.c_void_p, C.POINTER(LevelProjectionC), C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                               C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]
         _lib = l
     return _lib
 

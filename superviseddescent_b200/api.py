@@ -592,12 +592,78 @@ class HogTransform:
 
 
 # ------------------------------------------------------------------------------------------------
+# projections that run on the device
+# ------------------------------------------------------------------------------------------------
+class DeviceProjection:
+    """A projection h that writes the feature rows of many samples at once on the device (a pose model's 3-D projection, random
+    or pixel features, a torch module).  The optimiser runs its levels through sd_train_level_projected /
+    sd_apply_level_projected: in chunks (rows_per_chunk), on several ranks (comm / group / distributed_solve), with the rank
+    diagnostic -- everything a HogTransform level has.  Subclass it, or provide the two methods:
+
+      feature_length(level) -> int                  D of the level
+      project(x, level, first_row, out) -> None     x: (rows, P) CUDA tensor view of this rank's parameter rows
+                                                    [first_row, first_row + rows); out: (rows, D) view into the chunk buffer
+                                                    (rows are further apart than D): write the features into it
+
+    project runs with the library's stream as torch's current stream and must queue its work there.  In training it is called
+    twice for every chunk but the last (once for the Gram, once for the update), so it must be deterministic.  An exception it
+    raises fails the level and is re-raised from train() / test()."""
+
+    def feature_length(self, level: int) -> int:
+        raise NotImplementedError
+
+    def project(self, x: torch.Tensor, level: int, first_row: int, out: torch.Tensor) -> None:
+        raise NotImplementedError
+
+
+def _is_device_projection(h) -> bool:
+    return callable(getattr(h, "project", None)) and callable(getattr(h, "feature_length", None))
+
+
+class _LevelProjection:
+    """The sd_level_projection of a DeviceProjection on one level.  The callback hands project() views of the optimiser's own
+    parameter tensor x and chunk buffer buf (the library passes pointers into exactly those), under the context's stream; an
+    exception is kept for raise_error().  close() right after the C call drops the callback and with it every reference to x and
+    buf, so the chunk buffer is freed with the optimiser's own reference (the callback does not refer back to this object: no
+    cycle waits for the garbage collector)."""
+
+    def __init__(self, ctx: Context, h, level: int, x: torch.Tensor, buf: torch.Tensor):
+        errors = self._errors = []
+        D = int(h.feature_length(level))
+        sp = _capi.lib().sd_ctx_stream(ctx.h) or 0
+        current = torch.cuda.current_stream(ctx.device)
+        stream = current if current.cuda_stream == sp else torch.cuda.ExternalStream(sp, device=torch.device("cuda", ctx.device))
+
+        def fn(user, c, lvl, d_x, ldx, first_row, rows, d_out, ld):
+            try:
+                xs, out = x[first_row:first_row + rows], buf[:rows, :D]
+                if (d_x or 0) != xs.data_ptr() or ldx != x.stride(0) or (d_out or 0) != out.data_ptr() or ld != buf.stride(0):
+                    raise RuntimeError("projection callback: the level passed rows outside the optimiser's tensors")
+                with torch.cuda.stream(stream):
+                    h.project(xs, lvl, first_row, out)
+                return 0
+            except BaseException as e:   # noqa: B902 -- nothing may unwind through the C frames; re-raised by raise_error
+                errors.append(e)
+                return 1
+
+        self._fn = _capi.ProjectFn(fn)                                      # alive as long as the descriptor
+        self.c = _capi.LevelProjectionC(self._fn, None, level, D)
+
+    def close(self) -> None:
+        self._fn = self.c = None
+
+    def raise_error(self) -> None:
+        if self._errors:
+            raise self._errors.pop()
+
+
+# ------------------------------------------------------------------------------------------------
 # superviseddescent.hpp: the cascade
 # ------------------------------------------------------------------------------------------------
 class SupervisedDescentOptimiser:
     """superviseddescent::SupervisedDescentOptimiser<LinearRegressor, Normalisation> (superviseddescent.hpp:85-361).
 
-    projection: either a HogTransform (stays on the device) or any callable
+    projection: a HogTransform or a DeviceProjection (both stay on the device), or any callable
     h(x_row: np.ndarray, regressor_level: int, sample_index: int) -> row / float, evaluated on the host
     exactly as the reference evaluates user functors (superviseddescent.hpp:178-189).
     """
@@ -606,7 +672,7 @@ class SupervisedDescentOptimiser:
         self.regressors = list(regressors)
         self.normalisation_strategy = normalisation or NoNormalisation()
         self.ctx = ctx
-        self.chunk_rows: List[int] = []   # feature rows per chunk of each level of the last train() with a HogTransform
+        self.chunk_rows: List[int] = []   # feature rows per chunk of each level of the last train() on the device route
 
     def _ctx(self) -> Context:
         if self.ctx is None:
@@ -640,17 +706,17 @@ class SupervisedDescentOptimiser:
         host[:, :D] = np.stack(rows)
         return _dev(host, ctx), D
 
-    def _chunk_rows(self, rows_per_chunk, frames: LevelFramesC, n: int, D: int, P: int, comm_h, route: int) -> int:
-        """Rows per chunk of a HogTransform level: rows_per_chunk (at most n), or -- None / 0 -- the most that fit beside the
-        solve and the staging of host frames (sd_level_chunk_rows; memory torch has reserved but not handed out counts as free,
-        so a warm caching allocator does not split a level that fits)."""
+    def _chunk_rows(self, rows_per_chunk, frames: Optional[LevelFramesC], n: int, D: int, P: int, comm_h, route: int) -> int:
+        """Rows per chunk of a HogTransform or DeviceProjection level (frames None): rows_per_chunk (at most n), or -- None / 0
+        -- the most that fit beside the solve and the staging of host frames (sd_level_chunk_rows; memory torch has reserved but
+        not handed out counts as free, so a warm caching allocator does not split a level that fits)."""
         if rows_per_chunk:
             return max(1, min(int(rows_per_chunk), n))
         ctx = self._ctx()
         free = _free_device_bytes(ctx.device)
         rows = C.c_int(0)
-        _check(ctx.h, _capi.lib().sd_level_chunk_rows(ctx.h, comm_h, C.byref(frames), C.c_int64(n), D, P, route, C.c_size_t(free),
-                                                      C.byref(rows)))
+        _check(ctx.h, _capi.lib().sd_level_chunk_rows(ctx.h, comm_h, C.byref(frames) if frames is not None else None, C.c_int64(n), D, P,
+                                                      route, C.c_size_t(free), C.byref(rows)))
         return rows.value
 
     def train(self, parameters, initialisations, templates, projection, on_training_epoch_callback=None, group=None, comm=None,
@@ -664,7 +730,10 @@ class SupervisedDescentOptimiser:
         A HogTransform projection trains each level with sd_train_level, through a buffer of rows_per_chunk feature rows (None:
         as many as fit on the device, which is all of them whenever the level fits -- then the result is that of one pass over
         all rows).  Templates need the whole level in one chunk.  Frames that stay in host memory are gathered level by level
-        (same results), the chunk buffer sized beside the staging they need."""
+        (same results), the chunk buffer sized beside the staging they need.  A DeviceProjection trains the same way through
+        sd_train_level_projected; an exception its project() raises is re-raised here (on several ranks the other ranks raise
+        SdError: the level fails on every rank).  The automatic chunk leaves a DeviceProjection only the library's 512 MB reserve
+        for its own temporaries: one that needs more per row passes rows_per_chunk."""
         from . import parallel
         ctx = self._ctx()
         lib = _capi.lib()
@@ -678,7 +747,8 @@ class SupervisedDescentOptimiser:
         distributed = comm is not None and comm.size > 1
         n_global = comm.sum_int(n) if distributed else n
         hog = isinstance(projection, HogTransform)
-        self.chunk_rows = []                                                 # rows per chunk of each HogTransform level
+        batched = not hog and _is_device_projection(projection)             # a DeviceProjection
+        self.chunk_rows = []                                                 # rows per chunk of each device-route level
 
         def route(D):
             if not distributed:
@@ -697,18 +767,26 @@ class SupervisedDescentOptimiser:
             if qr:
                 ctx.set_rank_diagnostic(True)                                # before the chunk query: the rank copy counts there
             nxt = torch.empty_like(cur)
-            if hog:                                                          # 1)-4) through a buffer of `rows` feature rows
+            proj = None
+            if hog or batched:                                               # 1)-4) through a buffer of `rows` feature rows
                 D = projection.feature_length(level)
                 X = torch.empty((D, P), dtype=torch.float32, device=cur.device)
                 ld = (D + P + 3) // 4 * 4
                 rows = max(n, 1) if tmpl is not None else self._chunk_rows(rows_per_chunk, frames, n, D, P, ch, route(D))
                 self.chunk_rows.append(rows)
                 buf = torch.empty((rows, ld), dtype=torch.float32, device=cur.device)
-                eyes = projection.norm.c()
-                rc = lib.sd_train_level(ctx.h, ch, C.byref(frames), ptr(cur), ptr(x_gt), n, P // 2, C.c_int64(n_global), C.byref(eyes),
-                                        C.byref(projection.hog_params[level]), C.byref(norm), ptr(tmpl),
-                                        C.c_int64(tmpl.stride(0) if tmpl is not None else 0), C.byref(rc_), route(D), ptr(buf),
-                                        C.c_int64(ld), rows, ptr(X), ptr(nxt), C.byref(lam))
+                ldt = C.c_int64(tmpl.stride(0) if tmpl is not None else 0)
+                if hog:
+                    eyes = projection.norm.c()
+                    rc = lib.sd_train_level(ctx.h, ch, C.byref(frames), ptr(cur), ptr(x_gt), n, P // 2, C.c_int64(n_global), C.byref(eyes),
+                                            C.byref(projection.hog_params[level]), C.byref(norm), ptr(tmpl), ldt, C.byref(rc_), route(D),
+                                            ptr(buf), C.c_int64(ld), rows, ptr(X), ptr(nxt), C.byref(lam))
+                else:
+                    proj = _LevelProjection(ctx, projection, level, cur, buf)
+                    rc = lib.sd_train_level_projected(ctx.h, ch, C.byref(proj.c), ptr(cur), ptr(x_gt), n, P, n_global, C.byref(norm),
+                                                      ptr(tmpl), ldt, C.byref(rc_), route(D), ptr(buf), ld, rows, ptr(X), ptr(nxt),
+                                                      C.byref(lam))
+                    proj.close()
                 del buf
             else:
                 A, D = self._project(projection, cur, level, extra=P)         # 1) features (:173-189)
@@ -730,6 +808,8 @@ class SupervisedDescentOptimiser:
                 reg.last_rank = ctx.last_rank()
                 if 0 <= reg.last_rank < D:
                     _print_rank_warning(reg.last_rank, D)
+            if proj is not None:
+                proj.raise_error()
             # a factorisation that broke down raises (with the rank in the message): NaN weights would poison the next level
             _check(ctx.h, rc)
             reg.x, reg.last_lambda = X, lam.value                            #    X: the model (for uncentred features)
@@ -742,8 +822,8 @@ class SupervisedDescentOptimiser:
         return cur
 
     def test(self, initialisations, templates, projection, on_regressor_iteration_callback=None, rows_per_chunk=None):
-        """superviseddescent.hpp:262-306.  A HogTransform projection runs each level with sd_apply_level through a buffer of
-        rows_per_chunk feature rows (None: as many as fit, as in train())."""
+        """superviseddescent.hpp:262-306.  A HogTransform projection runs each level with sd_apply_level, a DeviceProjection
+        with sd_apply_level_projected, through a buffer of rows_per_chunk feature rows (None: as many as fit, as in train())."""
         ctx = self._ctx()
         lib = _capi.lib()
         cur = _dev(initialisations, ctx).clone()
@@ -751,19 +831,29 @@ class SupervisedDescentOptimiser:
             cur = cur.reshape(1, -1)
         n, P = cur.shape
         tmpl = _dev(templates, ctx) if templates is not None and np.size(templates) > 0 else None
-        frames = projection.level_frames(n) if isinstance(projection, HogTransform) else None
+        hog = isinstance(projection, HogTransform)
+        batched = not hog and _is_device_projection(projection)
+        frames = projection.level_frames(n) if hog else None
         for level, reg in enumerate(self.regressors):
             norm = self.normalisation_strategy.c(P // 2)
             nxt = torch.empty_like(cur)
-            if isinstance(projection, HogTransform):
+            if hog or batched:
                 D = projection.feature_length(level)
                 ld = (D + 3) // 4 * 4
                 rows = self._chunk_rows(rows_per_chunk, frames, n, D, P, None, 0)
                 buf = torch.empty((rows, ld), dtype=torch.float32, device=cur.device)
-                eyes = projection.norm.c()
-                _check(ctx.h, lib.sd_apply_level(ctx.h, C.byref(frames), ptr(cur), n, P // 2, C.byref(eyes), C.byref(projection.hog_params[level]),
-                                                 C.byref(norm), ptr(tmpl), C.c_int64(tmpl.stride(0) if tmpl is not None else 0), ptr(reg.x),
-                                                 ptr(buf), C.c_int64(ld), rows, ptr(nxt)))
+                ldt = C.c_int64(tmpl.stride(0) if tmpl is not None else 0)
+                if hog:
+                    eyes = projection.norm.c()
+                    _check(ctx.h, lib.sd_apply_level(ctx.h, C.byref(frames), ptr(cur), n, P // 2, C.byref(eyes), C.byref(projection.hog_params[level]),
+                                                     C.byref(norm), ptr(tmpl), ldt, ptr(reg.x), ptr(buf), C.c_int64(ld), rows, ptr(nxt)))
+                else:
+                    proj = _LevelProjection(ctx, projection, level, cur, buf)
+                    rc = lib.sd_apply_level_projected(ctx.h, C.byref(proj.c), ptr(cur), n, P, C.byref(norm), ptr(tmpl), ldt, ptr(reg.x),
+                                                      ptr(buf), ld, rows, ptr(nxt))
+                    proj.close()
+                    proj.raise_error()
+                    _check(ctx.h, rc)
                 del buf
             else:
                 A, D = self._project(projection, cur, level, extra=0)

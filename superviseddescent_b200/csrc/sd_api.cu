@@ -162,6 +162,8 @@ int sd_sync(sd_ctx* ctx)
     return sd_check_hog_status(ctx, "sync");                  // synchronises the stream; reports flags raised by sd_hog_batch
 }
 
+void* sd_ctx_stream(const sd_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
+
 int64_t sd_launch_count(const sd_ctx* ctx) { return ctx ? ctx->launches : 0; }
 int64_t sd_roi_fallback_count(const sd_ctx* ctx) { return ctx ? ctx->roi_fallbacks : 0; }
 

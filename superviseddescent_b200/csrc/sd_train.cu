@@ -1,8 +1,9 @@
-// Cascade levels of the HOG optimiser in chunks of rows (include/sd_b200.h, "cascade levels").
+// Cascade levels of the optimiser in chunks of rows (include/sd_b200.h, "cascade levels").
 //
-//   sd_level_chunk_rows  rows of one chunk that fit beside what the level's solve allocates
-//   sd_train_level       superviseddescent.hpp:173-217: HOG, targets, shift, Gram accumulation, exchange, solve, update
-//   sd_apply_level       superviseddescent.hpp:262-306, 323-344: HOG, templates, update
+//   sd_level_chunk_rows       rows of one chunk that fit beside what the level's solve allocates
+//   sd_train_level            superviseddescent.hpp:173-217: HOG, targets, shift, Gram accumulation, exchange, solve, update
+//   sd_apply_level            superviseddescent.hpp:262-306, 323-344: HOG, templates, update
+//   sd_*_level_projected      the same two levels with the feature rows from the caller's projection callback (RowSource)
 //
 // [A^T A | A^T b] is a sum over rows, so a level never needs all of its feature rows at once.  The rows are shifted by the column
 // means of the first chunk (the pilot p, over all ranks) before they enter the Gram: with n0 rows in that chunk p is within about
@@ -374,7 +375,141 @@ int hog_rows(sd_ctx* ctx, const sd_level_frames& src, HostGather& g, const float
     return sd_hog_batch(ctx, &view, idx ? idx + r0 : nullptr, d_x + (int64_t)r0 * P, P, rows, L, eyes, p, d_chunk, ld);
 }
 
+// ---- the row source of a level (DESIGN 4.7) -----------------------------------------------------------------------------------
+// A level's feature rows come from the HOG of its frames (sd_train_level / sd_apply_level) or from the caller's projection
+// (sd_train_level_projected / sd_apply_level_projected).  Everything after the rows -- templates, targets, shift, Gram, exchange,
+// solve, update -- is one loop (train_rows, apply_rows) whichever the source.
+struct RowSource {
+    const sd_level_projection* proj = nullptr;   // the caller's projection; NULL: HOG of the frames below
+    const sd_level_frames* frames = nullptr;
+    HostGather g{};
+    int L = 0;
+    const sd_normalisation* hog_eyes = nullptr;
+    const sd_hog_param* p = nullptr;
+};
+
+// On the HOG source: checks the frames and sets up a host-frame gather (SD_ERR_INVALID before any work is queued).
+int source_prepare(sd_ctx* ctx, RowSource& s, int N)
+{
+    return s.proj ? SD_OK : frames_prepare(ctx, s.frames, s.g, N);
+}
+
+// feature rows of samples [r0, r0 + rows) into columns [0, D) of the chunk buffer; P = the parameter width
+int source_rows(sd_ctx* ctx, RowSource& s, const float* d_x, int P, int r0, int rows, float* d_chunk, int64_t ld)
+{
+    if (!s.proj) return hog_rows(ctx, *s.frames, s.g, d_x, r0, rows, s.L, s.hog_eyes, s.p, d_chunk, ld);
+    if (rows == 0) return SD_OK;                                     // a rank without samples
+    const int rc = s.proj->fn(s.proj->user, ctx, s.proj->level, d_x + (int64_t)r0 * P, P, r0, rows, d_chunk, ld);
+    return rc ? sd_fail(ctx, SD_ERR_INVALID, "projection callback returned %d", rc) : SD_OK;
+}
+
+// the end of a level on host frames: no patch may have read outside its planned region
+int source_finish(sd_ctx* ctx, const RowSource& s, int N)
+{
+    return s.proj || s.frames->images ? SD_OK : gather_finish(ctx, s.g, N);
+}
+
+// The rules of a caller's projection (SD_ERR_INVALID before any work is queued): a callback, D >= 1, and a normalisation that can
+// read the parameter rows -- inter-eye distance needs [x.., y..] rows (even P) with its eye indices below P / 2.
+int check_projection(sd_ctx* ctx, const char* fn, const sd_level_projection* proj, int P, const sd_normalisation* norm)
+{
+    if (!proj || !proj->fn || proj->feature_length < 1)
+        return sd_fail(ctx, SD_ERR_INVALID, "%s: the projection needs a callback and feature_length >= 1", fn);
+    if (P < 1) return sd_fail(ctx, SD_ERR_INVALID, "%s: P < 1", fn);
+    if (norm && norm->kind == 1) {
+        sd_eyes_dev eyes;
+        if (P % 2 || sd_eyes_to_dev(ctx, norm, P / 2, &eyes))
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: inter-eye distance normalisation needs an even P and eye indices below P / 2", fn);
+    } else if (norm && norm->kind != 0) {
+        return sd_fail(ctx, SD_ERR_INVALID, "%s: unknown normalisation kind %d", fn, norm->kind);
+    }
+    return SD_OK;
+}
+
 size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
+
+// Several ranks on a caller's projection: a callback that fails on one rank must not leave the others waiting in a collective.  The
+// failing rank still takes part in every collective up to the exchange (the centring's without rows), and the ranks agree on a
+// failure -- one host integer -- before the exchange and at the end of the level, so either every rank fails the level or none.
+int agree_on_failure(sd_ctx* ctx, const char* fn, const RowSource& s, sd_comm* c, int failed)
+{
+    if (!s.proj || !c) return failed;
+    int64_t any = failed != 0;
+    const int rc = sd_comm_sum_int64(ctx, c, &any);
+    if (failed) return failed;                                       // keeps its own message
+    if (rc) return rc;
+    return any ? sd_fail(ctx, SD_ERR_INVALID, "%s: the projection callback failed on another rank", fn) : SD_OK;
+}
+
+// One training level of D features on P parameters from the row source s (sd_train_level, sd_train_level_projected); the caller
+// has checked the arguments.
+int train_rows(sd_ctx* ctx, const char* fn, sd_comm* comm, RowSource& s, int D, const float* d_x, const float* d_x_gt, int N_local,
+               int P, int64_t n_global, const sd_normalisation* norm, const float* d_templates, int64_t ldt, const sd_regulariser* reg,
+               int route, float* d_chunk, int64_t ld, int chunk_rows, float* d_X, float* d_x_next, float* lambda_out)
+{
+    int rc = source_prepare(ctx, s, N_local);
+    if (rc) return rc;
+    float* mu = (float*)sd_workspace(ctx, SD_WS_LEVEL, (size_t)D * (P + 1) * sizeof(float));
+    if (!mu) return SD_ERR_CUDA;
+    float* Xc = mu + D;                                   // weights for the shifted rows: what the update multiplies them with
+    sd_comm* c = sd_comm_size_of(comm) > 1 ? comm : nullptr;
+    float* B = d_chunk + D;                               // [A | b] side by side: the Gram reads both in one pass
+    const int chunks = N_local > 0 ? sd_div_up(N_local, chunk_rows) : 1;
+    // the pilot shift is the mean of every rank's first chunk (sd_centre_features also checks the all-ones bias column there)
+    int64_t n0 = N_local < chunk_rows ? N_local : chunk_rows;
+    rc = c ? sd_comm_sum_int64(ctx, c, &n0) : SD_OK;
+    if (rc) return rc;
+    if (n0 < 1) return sd_fail(ctx, SD_ERR_INVALID, "%s: no samples on any rank", fn);
+    const bool shifted = D > SD_LU_MAX_DIM && !reg->regularise_last_row;     // otherwise sd_centre_features leaves mu = 0
+    int failed = SD_OK;
+    for (int k = 0; k < chunks; ++k) {
+        const int r0 = k * chunk_rows, rows = N_local - r0 < chunk_rows ? N_local - r0 : chunk_rows;
+        rc = source_rows(ctx, s, d_x, P, r0, rows, d_chunk, ld);                                                      // :173-189
+        if (rc && s.proj && c) {                          // agree_on_failure: the centring's collective without rows, then stop
+            failed = rc;
+            rc = k == 0 ? sd_centre_features(ctx, c, d_chunk, ld, 0, D, (int)n0, reg, mu) : SD_OK;
+            if (rc) return rc;
+            break;
+        }
+        if (!rc && d_templates) rc = sd_subtract_templates(ctx, d_chunk, ld, d_templates, ldt, rows, D);             // :191-197
+        if (!rc) rc = sd_cascade_targets(ctx, d_x + (int64_t)r0 * P, d_x_gt + (int64_t)r0 * P, rows, P, norm, B, ld); // :199-205
+        if (!rc) rc = k == 0 ? sd_centre_features(ctx, c, d_chunk, ld, rows, D, (int)n0, reg, mu)
+                             : (shifted ? sd_shift_rows(ctx, d_chunk, ld, rows, D, mu) : SD_OK);
+        if (!rc) rc = sd_learn_gram(ctx, d_chunk, ld, B, ld, rows, true, D, P, k > 0);
+        if (rc) return rc;
+    }
+    rc = agree_on_failure(ctx, fn, s, c, failed);
+    if (rc) return rc;
+    rc = sd_learn_centred_solve(ctx, c, D, P, reg, (int)n_global, route, mu, d_X, Xc, lambda_out);                    // :207
+    if (rc) return rc;
+    // :209-215 -- the last chunk is still in the buffer; the others are projected and shifted again
+    const int last = (chunks - 1) * chunk_rows;
+    rc = sd_cascade_update(ctx, d_chunk, ld, N_local - last, D, Xc, P, d_x + (int64_t)last * P, norm, d_x_next + (int64_t)last * P);
+    for (int k = 0; !rc && k + 1 < chunks; ++k) {
+        const int r0 = k * chunk_rows;
+        rc = source_rows(ctx, s, d_x, P, r0, chunk_rows, d_chunk, ld);
+        if (!rc && shifted) rc = sd_shift_rows(ctx, d_chunk, ld, chunk_rows, D, mu);
+        if (!rc) rc = sd_cascade_update(ctx, d_chunk, ld, chunk_rows, D, Xc, P, d_x + (int64_t)r0 * P, norm, d_x_next + (int64_t)r0 * P);
+    }
+    if (!rc) rc = source_finish(ctx, s, N_local);
+    return agree_on_failure(ctx, fn, s, c, rc);
+}
+
+// One test / predict level of D features on P parameters from the row source s (sd_apply_level, sd_apply_level_projected); the
+// caller has checked the arguments.
+int apply_rows(sd_ctx* ctx, RowSource& s, int D, const float* d_x, int N, int P, const sd_normalisation* norm, const float* d_templates,
+               int64_t ldt, const float* d_X, float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next)
+{
+    int rc = source_prepare(ctx, s, N);
+    for (int r0 = 0; !rc && r0 < N; r0 += chunk_rows) {
+        const int rows = N - r0 < chunk_rows ? N - r0 : chunk_rows;
+        rc = source_rows(ctx, s, d_x, P, r0, rows, d_chunk, ld);
+        if (!rc && d_templates) rc = sd_subtract_templates(ctx, d_chunk, ld, d_templates + (int64_t)r0 * ldt, ldt, rows, D);
+        if (!rc) rc = sd_cascade_update(ctx, d_chunk, ld, rows, D, d_X, P, d_x + (int64_t)r0 * P, norm, d_x_next + (int64_t)r0 * P);
+    }
+    if (!rc) rc = source_finish(ctx, s, N);
+    return rc;
+}
 
 }  // namespace
 
@@ -395,44 +530,13 @@ int sd_train_level(sd_ctx* ctx, sd_comm* comm, const sd_level_frames* frames, co
     SD_REQUIRE(ctx, ld >= (int64_t)D + P, "ld < D + 2L");
     SD_REQUIRE(ctx, !d_templates || (chunk_rows >= N_local && ldt >= D), "templates need one chunk (chunk_rows >= N_local) and ldt >= D");
     SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
-    HostGather g{};
-    int rc = frames_prepare(ctx, frames, g, N_local);
-    if (rc) return rc;
-    float* mu = (float*)sd_workspace(ctx, SD_WS_LEVEL, (size_t)D * (P + 1) * sizeof(float));
-    if (!mu) return SD_ERR_CUDA;
-    float* Xc = mu + D;                                   // weights for the shifted rows: what the update multiplies them with
-    sd_comm* c = sd_comm_size_of(comm) > 1 ? comm : nullptr;
-    float* B = d_chunk + D;                               // [A | b] side by side: the Gram reads both in one pass
-    const int chunks = N_local > 0 ? sd_div_up(N_local, chunk_rows) : 1;
-    // the pilot shift is the mean of every rank's first chunk (sd_centre_features also checks the all-ones bias column there)
-    int64_t n0 = N_local < chunk_rows ? N_local : chunk_rows;
-    rc = c ? sd_comm_sum_int64(ctx, c, &n0) : SD_OK;
-    if (rc) return rc;
-    if (n0 < 1) return sd_fail(ctx, SD_ERR_INVALID, "sd_train_level: no samples on any rank");
-    const bool shifted = D > SD_LU_MAX_DIM && !reg->regularise_last_row;     // otherwise sd_centre_features leaves mu = 0
-    for (int k = 0; k < chunks; ++k) {
-        const int r0 = k * chunk_rows, rows = N_local - r0 < chunk_rows ? N_local - r0 : chunk_rows;
-        rc = hog_rows(ctx, *frames, g, d_x, r0, rows, L, hog_eyes, p, d_chunk, ld);                                    // :173-189
-        if (!rc && d_templates) rc = sd_subtract_templates(ctx, d_chunk, ld, d_templates, ldt, rows, D);             // :191-197
-        if (!rc) rc = sd_cascade_targets(ctx, d_x + (int64_t)r0 * P, d_x_gt + (int64_t)r0 * P, rows, P, norm, B, ld); // :199-205
-        if (!rc) rc = k == 0 ? sd_centre_features(ctx, c, d_chunk, ld, rows, D, (int)n0, reg, mu)
-                             : (shifted ? sd_shift_rows(ctx, d_chunk, ld, rows, D, mu) : SD_OK);
-        if (!rc) rc = sd_learn_gram(ctx, d_chunk, ld, B, ld, rows, true, D, P, k > 0);
-        if (rc) return rc;
-    }
-    rc = sd_learn_centred_solve(ctx, c, D, P, reg, (int)n_global, route, mu, d_X, Xc, lambda_out);                    // :207
-    if (rc) return rc;
-    // :209-215 -- the last chunk is still in the buffer; the others are projected and shifted again
-    const int last = (chunks - 1) * chunk_rows;
-    rc = sd_cascade_update(ctx, d_chunk, ld, N_local - last, D, Xc, P, d_x + (int64_t)last * P, norm, d_x_next + (int64_t)last * P);
-    for (int k = 0; !rc && k + 1 < chunks; ++k) {
-        const int r0 = k * chunk_rows;
-        rc = hog_rows(ctx, *frames, g, d_x, r0, chunk_rows, L, hog_eyes, p, d_chunk, ld);
-        if (!rc && shifted) rc = sd_shift_rows(ctx, d_chunk, ld, chunk_rows, D, mu);
-        if (!rc) rc = sd_cascade_update(ctx, d_chunk, ld, chunk_rows, D, Xc, P, d_x + (int64_t)r0 * P, norm, d_x_next + (int64_t)r0 * P);
-    }
-    if (!rc && !frames->images) rc = gather_finish(ctx, g, N_local);
-    return rc;
+    RowSource s;
+    s.frames = frames;
+    s.L = L;
+    s.hog_eyes = hog_eyes;
+    s.p = p;
+    return train_rows(ctx, __func__, comm, s, D, d_x, d_x_gt, N_local, P, n_global, norm, d_templates, ldt, reg, route, d_chunk, ld,
+                      chunk_rows, d_X, d_x_next, lambda_out);
 }
 
 int sd_apply_level(sd_ctx* ctx, const sd_level_frames* frames, const float* d_x, int N, int L, const sd_normalisation* hog_eyes,
@@ -448,16 +552,53 @@ int sd_apply_level(sd_ctx* ctx, const sd_level_frames* frames, const float* d_x,
     SD_REQUIRE(ctx, ld >= D, "ld < D");
     SD_REQUIRE(ctx, !d_templates || ldt >= D, "ldt < D");
     SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
-    HostGather g{};
-    int rc = frames_prepare(ctx, frames, g, N);
-    for (int r0 = 0; !rc && r0 < N; r0 += chunk_rows) {
-        const int rows = N - r0 < chunk_rows ? N - r0 : chunk_rows;
-        rc = hog_rows(ctx, *frames, g, d_x, r0, rows, L, hog_eyes, p, d_chunk, ld);
-        if (!rc && d_templates) rc = sd_subtract_templates(ctx, d_chunk, ld, d_templates + (int64_t)r0 * ldt, ldt, rows, D);
-        if (!rc) rc = sd_cascade_update(ctx, d_chunk, ld, rows, D, d_X, P, d_x + (int64_t)r0 * P, norm, d_x_next + (int64_t)r0 * P);
-    }
-    if (!rc && !frames->images) rc = gather_finish(ctx, g, N);
-    return rc;
+    RowSource s;
+    s.frames = frames;
+    s.L = L;
+    s.hog_eyes = hog_eyes;
+    s.p = p;
+    return apply_rows(ctx, s, D, d_x, N, P, norm, d_templates, ldt, d_X, d_chunk, ld, chunk_rows, d_x_next);
+}
+
+int sd_train_level_projected(sd_ctx* ctx, sd_comm* comm, const sd_level_projection* proj, const float* d_x, const float* d_x_gt,
+                             int N_local, int P, int64_t n_global, const sd_normalisation* norm, const float* d_templates, int64_t ldt,
+                             const sd_regulariser* reg, int route, float* d_chunk, int64_t ld, int chunk_rows, float* d_X,
+                             float* d_x_next, float* lambda_out)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, d_x && d_x_gt && reg && d_chunk && d_X && d_x_next, "null argument");
+    SD_REQUIRE(ctx, N_local >= 0 && n_global >= 1 && n_global <= INT_MAX, "bad sample count");
+    SD_REQUIRE(ctx, chunk_rows >= 1, "chunk_rows must be >= 1");
+    SD_REQUIRE(ctx, reg->type == 0 || reg->type == 1, "unknown regularisation type");
+    const int rc = check_projection(ctx, __func__, proj, P, norm);
+    if (rc) return rc;
+    const int D = proj->feature_length;
+    SD_REQUIRE(ctx, ld >= (int64_t)D + P, "ld < D + P");
+    SD_REQUIRE(ctx, !d_templates || (chunk_rows >= N_local && ldt >= D), "templates need one chunk (chunk_rows >= N_local) and ldt >= D");
+    SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
+    RowSource s;
+    s.proj = proj;
+    return train_rows(ctx, __func__, comm, s, D, d_x, d_x_gt, N_local, P, n_global, norm, d_templates, ldt, reg, route, d_chunk, ld,
+                      chunk_rows, d_X, d_x_next, lambda_out);
+}
+
+int sd_apply_level_projected(sd_ctx* ctx, const sd_level_projection* proj, const float* d_x, int N, int P, const sd_normalisation* norm,
+                             const float* d_templates, int64_t ldt, const float* d_X, float* d_chunk, int64_t ld, int chunk_rows,
+                             float* d_x_next)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, d_x && d_X && d_chunk && d_x_next, "null argument");
+    SD_REQUIRE(ctx, N >= 0, "bad sample count");
+    SD_REQUIRE(ctx, chunk_rows >= 1, "chunk_rows must be >= 1");
+    const int rc = check_projection(ctx, __func__, proj, P, norm);
+    if (rc) return rc;
+    const int D = proj->feature_length;
+    SD_REQUIRE(ctx, ld >= D, "ld < D");
+    SD_REQUIRE(ctx, !d_templates || ldt >= D, "ldt < D");
+    SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
+    RowSource s;
+    s.proj = proj;
+    return apply_rows(ctx, s, D, d_x, N, P, norm, d_templates, ldt, d_X, d_chunk, ld, chunk_rows, d_x_next);
 }
 
 int sd_level_chunk_rows(sd_ctx* ctx, sd_comm* comm, const sd_level_frames* frames, int64_t N_local, int D, int M, int route,

@@ -4,16 +4,19 @@
 // reference's signatures (superviseddescent.hpp:85-361) and its callback types (:52-54).  Two routes:
 //
 //   device route   RegressorType is this package's LinearRegressor<>, the projection is a device
-//                  projection (rcr::HogTransform) and the normalisation maps to sd_normalisation:
+//                  projection (rcr::HogTransform, or a batch projection with feature_length / project_device,
+//                  see is_device_batch_projection) and the normalisation maps to sd_normalisation:
 //                  features, targets, Gram, solve and update all stay in HBM, one sd_train_level /
-//                  sd_apply_level call per level through a buffer of feature rows that holds the whole
-//                  level when it fits, and chunks of it otherwise (set_rows_per_chunk).
+//                  sd_apply_level call (sd_*_level_projected for a batch projection) per level through a
+//                  buffer of feature rows that holds the whole level when it fits, and chunks of it
+//                  otherwise (set_rows_per_chunk).
 //   functor route  any other projection functor h(row, level, idx) -> Mat | float is USER host code; it is
 //                  evaluated on a pool of host threads exactly as the reference does (:173-189) and the
 //                  stacked feature matrix goes through RegressorType::learn / predict (which are GPU calls
 //                  for LinearRegressor<>).  That is the reference's API for user functors, not a fallback.
 #pragma once
 
+#include <exception>
 #include <functional>
 #include <thread>
 #include <type_traits>
@@ -40,6 +43,101 @@ template <class... T> using void_t = typename voider<T...>::type;
 // projection whose frames a level call reads, projected on the device for all rows at once (rcr::HogTransform)
 template <class P, class = void> struct is_device_projection : std::false_type {};
 template <class P> struct is_device_projection<P, void_t<decltype(std::declval<P&>().level_frames(0)), decltype(std::declval<P&>().hog_param(size_t(0)))>> : std::true_type {};
+
+// projection that writes the feature rows of a chunk on the device itself (sd_level_projection):
+//   int feature_length(size_t level);
+//   int project_device(sd_ctx* ctx, size_t level, const float* d_x, int64_t ldx, int64_t first_row, int rows, float* d_out, int64_t ld);
+// project_device follows the callback contract of include/sd_b200.h (work ordered on sd_ctx_stream(ctx), columns [0, D) only,
+// deterministic); a non-zero return or an exception fails the level, and the exception is rethrown from train() / test().
+template <class P, class = void> struct is_device_batch_projection : std::false_type {};
+template <class P> struct is_device_batch_projection<P, void_t<
+    decltype(static_cast<int>(std::declval<P&>().feature_length(size_t(0)))),
+    decltype(static_cast<int>(std::declval<P&>().project_device(std::declval<sd_ctx*>(), size_t(0), std::declval<const float*>(), int64_t(0),
+                                                                int64_t(0), 0, std::declval<float*>(), int64_t(0))))>> : std::true_type {};
+
+template <class P> struct takes_device_route
+    : std::integral_constant<bool, is_device_projection<P>::value || is_device_batch_projection<P>::value> {};
+
+// Where the device route's levels get their feature rows: a HogTransform's frames (sd_train_level / sd_apply_level), or a batch
+// projection's callback (sd_train_level_projected / sd_apply_level_projected).
+template <class P, bool Hog = is_device_projection<P>::value> class LevelSource;
+
+template <class P> class LevelSource<P, true> {
+public:
+    LevelSource(P& projection, int n) : h(projection), eyes(projection.eyes()), frames(projection.level_frames(n)) {}
+    const sd_level_frames* level_frames() const { return &frames; }
+    int train(sd_ctx* ctx, sd_comm* c, size_t level, const float* d_x, const float* d_gt, int n, int Pd, int64_t n_global,
+              const sd_normalisation& norm, const float* tmpl, int64_t ldt, const sd_regulariser& reg, int route, float* chunk,
+              int64_t ld, int rows, float* X, float* x_next)
+    {
+        const sd_hog_param hp = h.hog_param(level);
+        return sd_train_level(ctx, c, &frames, d_x, d_gt, n, Pd / 2, n_global, &eyes, &hp, &norm, tmpl, ldt, &reg, route, chunk, ld, rows,
+                              X, x_next, nullptr);
+    }
+    int apply(sd_ctx* ctx, size_t level, const float* d_x, int n, int Pd, const sd_normalisation& norm, const float* tmpl, int64_t ldt,
+              const float* X, float* chunk, int64_t ld, int rows, float* x_next)
+    {
+        const sd_hog_param hp = h.hog_param(level);
+        return sd_apply_level(ctx, &frames, d_x, n, Pd / 2, &eyes, &hp, &norm, tmpl, ldt, X, chunk, ld, rows, x_next);
+    }
+    void rethrow() {}
+
+private:
+    P& h;
+    sd_normalisation eyes;
+    sd_level_frames frames;
+};
+
+template <class P> class LevelSource<P, false> {
+public:
+    LevelSource(P& projection, int /*n*/) : h(projection) {}
+    const sd_level_frames* level_frames() const { return nullptr; }
+    int train(sd_ctx* ctx, sd_comm* c, size_t level, const float* d_x, const float* d_gt, int n, int Pd, int64_t n_global,
+              const sd_normalisation& norm, const float* tmpl, int64_t ldt, const sd_regulariser& reg, int route, float* chunk,
+              int64_t ld, int rows, float* X, float* x_next)
+    {
+        const sd_level_projection proj = descriptor(level);
+        return sd_train_level_projected(ctx, c, &proj, d_x, d_gt, n, Pd, n_global, &norm, tmpl, ldt, &reg, route, chunk, ld, rows, X,
+                                        x_next, nullptr);
+    }
+    int apply(sd_ctx* ctx, size_t level, const float* d_x, int n, int Pd, const sd_normalisation& norm, const float* tmpl, int64_t ldt,
+              const float* X, float* chunk, int64_t ld, int rows, float* x_next)
+    {
+        const sd_level_projection proj = descriptor(level);
+        return sd_apply_level_projected(ctx, &proj, d_x, n, Pd, &norm, tmpl, ldt, X, chunk, ld, rows, x_next);
+    }
+    // an exception of project_device, kept while the C call unwound normally, is rethrown here
+    void rethrow()
+    {
+        if (!error) return;
+        std::exception_ptr e = error;
+        error = nullptr;
+        std::rethrow_exception(e);
+    }
+
+private:
+    sd_level_projection descriptor(size_t level)
+    {
+        sd_level_projection proj{};
+        proj.fn = &LevelSource::call;
+        proj.user = this;
+        proj.level = static_cast<int32_t>(level);
+        proj.feature_length = h.feature_length(level);
+        return proj;
+    }
+    static int call(void* user, sd_ctx* ctx, int level, const float* d_x, int64_t ldx, int64_t first_row, int rows, float* d_out, int64_t ld)
+    {
+        LevelSource* self = static_cast<LevelSource*>(user);
+        try {
+            return self->h.project_device(ctx, static_cast<size_t>(level), d_x, ldx, first_row, rows, d_out, ld);
+        } catch (...) {                          // nothing may unwind through the library's frames
+            self->error = std::current_exception();
+            return -1;
+        }
+    }
+    P& h;
+    std::exception_ptr error;
+};
 
 template <class N, class = void> struct has_c_normalisation : std::false_type {};
 template <class N> struct has_c_normalisation<N, void_t<decltype(std::declval<const N&>().c_normalisation())>> : std::true_type {};
@@ -103,9 +201,9 @@ public:
     void train(cv::Mat parameters, cv::Mat initialisations, cv::Mat templates, ProjectionFunction projection,
                OnTrainingEpochCallback on_training_epoch_callback, sd_comm* communicator, int route = 0)
     {
-        static_assert(detail::is_device_projection<ProjectionFunction>::value && detail::has_c_normalisation<NormalisationStrategy>::value &&
+        static_assert(detail::takes_device_route<ProjectionFunction>::value && detail::has_c_normalisation<NormalisationStrategy>::value &&
                           detail::is_device_regressor<RegressorType>::value,
-                      "multi-GPU training needs the device route (HogTransform projection, device regressors)");
+                      "multi-GPU training needs the device route (HogTransform or device batch projection, device regressors)");
         comm = communicator;
         comm_route = route;
         train_impl(parameters, initialisations, templates, projection, on_training_epoch_callback, std::true_type());
@@ -118,7 +216,7 @@ public:
                OnTrainingEpochCallback on_training_epoch_callback)
     {
         train_impl(parameters, initialisations, templates, projection, on_training_epoch_callback,
-                   std::integral_constant<bool, detail::is_device_projection<ProjectionFunction>::value &&
+                   std::integral_constant<bool, detail::takes_device_route<ProjectionFunction>::value &&
                                                     detail::has_c_normalisation<NormalisationStrategy>::value &&
                                                     detail::is_device_regressor<RegressorType>::value>());
     }
@@ -138,7 +236,7 @@ public:
                  OnRegressorIterationCallback on_regressor_iteration_callback)
     {
         return test_impl(initialisations, templates, projection, on_regressor_iteration_callback,
-                         std::integral_constant<bool, detail::is_device_projection<ProjectionFunction>::value &&
+                         std::integral_constant<bool, detail::takes_device_route<ProjectionFunction>::value &&
                                                           detail::has_c_normalisation<NormalisationStrategy>::value &&
                                                           detail::is_device_regressor<RegressorType>::value>());
     }
@@ -154,7 +252,9 @@ public:
     NormalisationStrategy& get_normalisation() { return normalisation_strategy; }
 
     // Device route: feature rows per chunk of a level in train() / test() / predict().  0 (the default): as many as fit on the
-    // device beside the solve (sd_level_chunk_rows) -- the whole level whenever it fits.  Templates always take one chunk.
+    // device beside the solve (sd_level_chunk_rows) -- the whole level whenever it fits.  Templates always take one chunk.  The
+    // automatic chunk leaves a batch projection's project_device only the library's 512 MB reserve for its own temporaries: one
+    // that needs more per row sets the chunk here.
     void set_rows_per_chunk(int rows) { rows_per_chunk = rows < 0 ? 0 : rows; }
 
 private:
@@ -214,11 +314,11 @@ private:
     int comm_route = 0;
 
     // feature rows per chunk of a device-route level: set_rows_per_chunk's (at most n), or as many as fit
-    int chunk_rows(sd_ctx* ctx, sd_comm* c, const sd_level_frames& frames, int n, int D, int Pd, int route) const
+    int chunk_rows(sd_ctx* ctx, sd_comm* c, const sd_level_frames* frames, int n, int D, int Pd, int route) const
     {
         if (rows_per_chunk > 0) return rows_per_chunk < n ? rows_per_chunk : (n > 0 ? n : 1);
         int rows = 0;
-        sd_b200::check(ctx, sd_level_chunk_rows(ctx, c, &frames, n, D, Pd, route, 0, &rows), "sd_level_chunk_rows");
+        sd_b200::check(ctx, sd_level_chunk_rows(ctx, c, frames, n, D, Pd, route, 0, &rows), "sd_level_chunk_rows");
         return rows;
     }
 
@@ -232,8 +332,7 @@ private:
         sd_b200::upload(parameters, d_gt, Pd);
         sd_b200::upload(initialisations, d_cur, Pd);
         const sd_normalisation norm = normalisation_strategy.c_normalisation();
-        const sd_normalisation eyes = projection.eyes();
-        const sd_level_frames frames = projection.level_frames(n);
+        detail::LevelSource<P> src(projection, n);
         if (!templates.empty()) sd_b200::upload(templates, d_tmpl, templates.cols);
         sd_b200::DeviceBuffer X;
         int64_t n_global = n;
@@ -244,21 +343,21 @@ private:
         for (size_t level = 0; level < regressors.size(); ++level) {
             const int D = projection.feature_length(level);
             const int64_t ld = (static_cast<int64_t>(D) + Pd + 3) / 4 * 4;
-            const sd_hog_param hp = projection.hog_param(level);
             const sd_regulariser reg = regressors[level].get_regulariser().c();
             const bool want_rank = detail::reports_rank<RegressorType>::value;
             if (want_rank) sd_b200::check(ctx, sd_set_rank_diagnostic(ctx, 1), "sd_set_rank_diagnostic");   // counted by the chunk query
             // 1)-4) :173-215 -- features, targets, Gram, exchange, solve and update through a buffer of `rows` feature rows
-            const int rows = templates.empty() ? chunk_rows(ctx, c, frames, n, D, Pd, route) : (n > 0 ? n : 1);
+            const int rows = templates.empty() ? chunk_rows(ctx, c, src.level_frames(), n, D, Pd, route) : (n > 0 ? n : 1);
             sd_b200::DeviceBuffer chunk(static_cast<size_t>(rows) * ld * sizeof(float));
             X.allocate(static_cast<size_t>(D) * Pd * sizeof(float));
             const float* tmpl = templates.empty() ? nullptr : d_tmpl.as<float>();
-            const int rc = sd_train_level(ctx, c, &frames, d_cur.as<float>(), d_gt.as<float>(), n, Pd / 2, n_global, &eyes, &hp, &norm, tmpl,
-                                          templates.cols, &reg, route, chunk.as<float>(), ld, rows, X.as<float>(), d_next.as<float>(), nullptr);
+            const int rc = src.train(ctx, c, level, d_cur.as<float>(), d_gt.as<float>(), n, Pd, n_global, norm, tmpl, templates.cols, reg, route,
+                                     chunk.as<float>(), ld, rows, X.as<float>(), d_next.as<float>());
             if (want_rank) {
                 sd_set_rank_diagnostic(ctx, 0);
                 detail::report_rank(regressors[level], sd_last_rank(ctx), D, detail::reports_rank<RegressorType>());
             }
+            src.rethrow();
             // a factorisation that broke down throws (with the rank in the message): NaN weights would poison the next level
             sd_b200::check(ctx, rc, "sd_train_level");
             regressors[level].set_x(sd_b200::download(X.as<float>(), D, Pd, Pd));
@@ -299,19 +398,18 @@ private:
         sd_b200::DeviceBuffer d_cur, d_next(static_cast<size_t>(n) * Pd * sizeof(float)), d_tmpl;
         sd_b200::upload(initialisations, d_cur, Pd);
         const sd_normalisation norm = normalisation_strategy.c_normalisation();
-        const sd_normalisation eyes = projection.eyes();
-        const sd_level_frames frames = projection.level_frames(n);
+        detail::LevelSource<P> src(projection, n);
         if (!templates.empty()) sd_b200::upload(templates, d_tmpl, templates.cols);
         for (size_t level = 0; level < regressors.size(); ++level) {
             const int D = projection.feature_length(level);
             const int64_t ld = (static_cast<int64_t>(D) + 3) / 4 * 4;
-            const sd_hog_param hp = projection.hog_param(level);
-            const int rows = chunk_rows(ctx, nullptr, frames, n, D, Pd, 0);
+            const int rows = chunk_rows(ctx, nullptr, src.level_frames(), n, D, Pd, 0);
             sd_b200::DeviceBuffer chunk(static_cast<size_t>(rows) * ld * sizeof(float));
             const float* tmpl = templates.empty() ? nullptr : d_tmpl.as<float>();
-            sd_b200::check(ctx, sd_apply_level(ctx, &frames, d_cur.as<float>(), n, Pd / 2, &eyes, &hp, &norm, tmpl, templates.cols,
-                                               regressors[level].device_x(), chunk.as<float>(), ld, rows, d_next.as<float>()),
-                           "sd_apply_level");
+            const int rc = src.apply(ctx, level, d_cur.as<float>(), n, Pd, norm, tmpl, templates.cols, regressors[level].device_x(),
+                                     chunk.as<float>(), ld, rows, d_next.as<float>());
+            src.rethrow();
+            sd_b200::check(ctx, rc, "sd_apply_level");
             std::swap(d_cur, d_next);
             if (want_callback) cb(sd_b200::download(d_cur.as<float>(), n, Pd, Pd));                          // :303
         }
