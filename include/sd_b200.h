@@ -455,6 +455,53 @@ SD_API int sd_apply_level_projected(sd_ctx* ctx, const sd_level_projection* proj
                                     const sd_normalisation* norm, const float* d_templates, int64_t ldt, const float* d_X,
                                     float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next);
 
+/* ---- cascade levels on the caller's host projection -------------------------------------------------------------------------
+ * The reference's own projections (examples/simple_function.cpp, pose_estimation.cpp, the hello-world HogTransform) and CPU
+ * descriptors run on the host.  Such a projection hands the level its feature rows through a host callback; the library copies
+ * them up in a pipeline and everything after the rows is the loop of sd_train_level_projected / sd_apply_level_projected, with
+ * the same rules (targets in [D, D + P), the pilot shift, templates in one chunk, the exchange and the failure agreement on
+ * several ranks, the rank diagnostic, reproducibility for a fixed chunk_rows and rank count).
+ *
+ * Inputs of the callback:
+ *   - h_x points at row first_row of a pinned host copy of this rank's d_x (pitch ldx = P floats).  The library makes that copy
+ *     once per level call, before the first callback; the callback must not write it.
+ *   - it writes columns [0, feature_length) of `rows` rows into h_out, a pinned staging half (pitch ld_out = roundup4(D) floats),
+ *     and returns 0, or non-zero to fail the level.
+ * Batches: within a chunk the callback is called in ascending row order, each call for min(rows left in the chunk, rows that fit
+ * one staging half) rows and never for 0 rows.  A half holds stage_half_bytes (0 = 48 MB), at least one row.
+ * The pipeline: each filled half goes up on the context's copy stream (one 2-D copy of columns [0, D) into the chunk buffer at the
+ * batch's row offset) while the callback fills the other half; the host waits on a half's copy before it refills it.  The first
+ * copy of a chunk waits for the previous chunk's last reader on the context's stream, and the stream waits for the chunk's last
+ * copy before templates, targets, centring and the Gram.  So the host fills chunk k + 1 while the GPU works on chunk k.  The
+ * context keeps the pinned staging pair and the pinned copy of x (grow-only, freed by sd_ctx_destroy); sd_level_chunk_rows is
+ * unchanged (frames = NULL): the staging is host memory.
+ * The contract:
+ *   - in training the callback is called twice for every chunk but the last, so it must be deterministic;
+ *   - it runs on the calling thread, and must not call into ctx;
+ *   - when it writes the rows a device callback (sd_level_projection) writes, X, lambda and x_next are bit for bit those of
+ *     sd_train_level_projected / sd_apply_level_projected for the same chunk_rows, whatever the staging-half size.
+ * Errors: a non-zero return fails the level with SD_ERR_INVALID and the message "projection callback returned N"; on several
+ * ranks the failure is agreed on as for sd_level_projection.  A NULL fn, feature_length < 1 and the argument errors of
+ * sd_train_level_projected / sd_apply_level_projected are SD_ERR_INVALID before any work is queued (outputs unwritten, the
+ * callback not called). */
+typedef int (*sd_host_project_fn)(void* user, int level, const float* h_x, int64_t ldx, int64_t first_row, int rows,
+                                  float* h_out, int64_t ld_out);
+typedef struct {
+    sd_host_project_fn fn;
+    void* user;                  /* passed to fn unchanged */
+    int32_t level;               /* passed to fn: the reference's regressorLevel */
+    int32_t feature_length;      /* D */
+    size_t stage_half_bytes;     /* bytes per pinned staging half; 0 = the library's default (48 MB) */
+} sd_level_host_projection;
+SD_API int sd_train_level_host_projected(sd_ctx* ctx, sd_comm* comm, const sd_level_host_projection* proj,
+                                         const float* d_x, const float* d_x_gt, int N_local, int P, int64_t n_global,
+                                         const sd_normalisation* norm, const float* d_templates, int64_t ldt,
+                                         const sd_regulariser* reg, int route, float* d_chunk, int64_t ld, int chunk_rows,
+                                         float* d_X, float* d_x_next, float* lambda_out);
+SD_API int sd_apply_level_host_projected(sd_ctx* ctx, const sd_level_host_projection* proj, const float* d_x, int N, int P,
+                                         const sd_normalisation* norm, const float* d_templates, int64_t ldt, const float* d_X,
+                                         float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next);
+
 /* host-frame bytes (region bytes x channels) the levels on host frames have read over PCIe on ctx since creation */
 SD_API int64_t sd_gathered_bytes(const sd_ctx* ctx);
 /* *in_place = 1 when the levels can read a host frame where it is (pinned and device-mapped, 16-byte aligned base and

@@ -64,6 +64,17 @@ class LevelProjectionC(C.Structure):
     _fields_ = [("fn", ProjectFn), ("user", C.c_void_p), ("level", C.c_int32), ("feature_length", C.c_int32)]
 
 
+# sd_host_project_fn(user, level, h_x, ldx, first_row, rows, h_out, ld_out) -> 0 or non-zero
+HostProjectFn = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int64)
+
+
+class LevelHostProjectionC(C.Structure):
+    """sd_level_host_projection: the host callback that fills a level's feature rows in pinned staging, its feature length and
+    the staging-half size (0: the library's default)."""
+    _fields_ = [("fn", HostProjectFn), ("user", C.c_void_p), ("level", C.c_int32), ("feature_length", C.c_int32),
+                ("stage_half_bytes", C.c_size_t)]
+
+
 # every symbol declared in include/sd_b200.h (tests/test_abi.py checks the list against the header)
 EXPORTS = [
     "sd_ctx_create", "sd_ctx_destroy", "sd_last_error", "sd_sync", "sd_ctx_stream", "sd_version", "sd_launch_count", "sd_roi_fallback_count",
@@ -75,7 +86,8 @@ EXPORTS = [
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",
     "sd_comm_sum_int64", "sd_comm_allgather", "sd_allreduce_gram", "sd_reduce_scatter_gram", "sd_solve_gram_dist", "sd_learn_dist",
     "sd_cascade_targets", "sd_cascade_update", "sd_subtract_templates", "sd_level_chunk_rows", "sd_train_level", "sd_apply_level",
-    "sd_train_level_projected", "sd_apply_level_projected", "sd_gathered_bytes", "sd_host_frame_in_place", "sd_device_memory",
+    "sd_train_level_projected", "sd_apply_level_projected", "sd_train_level_host_projected", "sd_apply_level_host_projected",
+    "sd_gathered_bytes", "sd_host_frame_in_place", "sd_device_memory",
     "sd_model_load", "sd_model_save", "sd_model_create", "sd_model_destroy", "sd_model_num_levels",
     "sd_model_num_landmarks", "sd_model_hog_param", "sd_model_regulariser", "sd_model_normalisation",
     "sd_model_get_mean", "sd_model_get_weights", "sd_model_landmark_id", "sd_align_mean",
@@ -119,6 +131,12 @@ def lib():
                                                C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         l.sd_apply_level_projected.argtypes = [C.c_void_p, C.POINTER(LevelProjectionC), C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                                C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]
+        l.sd_train_level_host_projected.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(LevelHostProjectionC), C.c_void_p, C.c_void_p,
+                                                    C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int,
+                                                    C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        l.sd_apply_level_host_projected.argtypes = [C.c_void_p, C.POINTER(LevelHostProjectionC), C.c_void_p, C.c_int, C.c_int,
+                                                    C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int,
+                                                    C.c_void_p]
         _lib = l
     return _lib
 

@@ -658,14 +658,104 @@ class _LevelProjection:
 
 
 # ------------------------------------------------------------------------------------------------
+# projections that run on the host
+# ------------------------------------------------------------------------------------------------
+class HostProjection:
+    """A projection h that writes the feature rows of many samples at once on the host (numpy features, CPU descriptors, the
+    reference's own functors through RowwiseProjection).  The optimiser runs its levels through sd_train_level_host_projected /
+    sd_apply_level_host_projected: the library calls project_host batch by batch into pinned staging and uploads each batch
+    while the next one is filled, so the host works while the GPU does; in chunks (rows_per_chunk), on several ranks (comm /
+    group / distributed_solve), with the rank diagnostic -- everything a DeviceProjection level has.  Subclass it, or provide the
+    two methods:
+
+      feature_length(level) -> int                  D of the level
+      project_host(x, level, first_row, out) -> None
+                                                    x: (rows, P) read-only float32 numpy view of this rank's parameter rows
+                                                    [first_row, first_row + rows); out: (rows, D) float32 numpy view into a
+                                                    pinned staging half (rows are further apart than D): write the features into it
+
+    stage_half_bytes (optional attribute): bytes of one staging half, 0 = the library's default (48 MB); a batch is as many rows
+    as fit one half, at least one.  In training project_host is called twice for every chunk but the last (once for the Gram,
+    once for the update), so it must be deterministic.  It runs on the thread that called train() / test().  An exception it
+    raises fails the level and is re-raised from train() / test()."""
+
+    stage_half_bytes = 0
+
+    def feature_length(self, level: int) -> int:
+        raise NotImplementedError
+
+    def project_host(self, x: np.ndarray, level: int, first_row: int, out: np.ndarray) -> None:
+        raise NotImplementedError
+
+
+class RowwiseProjection(HostProjection):
+    """A per-row projection functor h(x_row, level, index) -> row / float (the reference's ProjectionFunction, e.g. the pose
+    example's) as a HostProjection: project_host calls h row by row, exactly as the plain-functor route does, so the level gets
+    the same feature rows -- but through the level pipeline (chunks, several ranks, the host filling rows while the GPU works).
+    feature_length: D of every level, or a sequence with one D per level."""
+
+    def __init__(self, h: Callable, feature_length):
+        self.h = h
+        self.lengths = feature_length
+
+    def feature_length(self, level: int) -> int:
+        return int(self.lengths if np.isscalar(self.lengths) else self.lengths[level])
+
+    def project_host(self, x: np.ndarray, level: int, first_row: int, out: np.ndarray) -> None:
+        D = out.shape[1]
+        for i in range(x.shape[0]):
+            row = np.atleast_1d(np.asarray(self.h(x[i].copy(), level, first_row + i), dtype=np.float32)).ravel()
+            if row.size != D:
+                raise ValueError(f"RowwiseProjection: h returned {row.size} values for row {first_row + i}, feature_length is {D}")
+            out[i] = row
+
+
+def _is_host_projection(h) -> bool:
+    return callable(getattr(h, "project_host", None)) and callable(getattr(h, "feature_length", None))
+
+
+class _LevelHostProjection:
+    """The sd_level_host_projection of a HostProjection on one level.  The callback hands project_host() numpy views of the
+    pinned copy of the parameter rows and of the staging half; an exception is kept for raise_error().  As for
+    _LevelProjection, close() right after the C call drops the callback, and the callback does not refer back to this object."""
+
+    def __init__(self, h, level: int):
+        errors = self._errors = []
+        D = int(h.feature_length(level))
+
+        def fn(user, lvl, h_x, ldx, first_row, rows, h_out, ld_out):
+            try:
+                x = np.ctypeslib.as_array((C.c_float * (rows * ldx)).from_address(h_x)).reshape(rows, ldx)
+                x.flags.writeable = False                                   # the second pass of training reads it again
+                out = np.ctypeslib.as_array((C.c_float * (rows * ld_out)).from_address(h_out)).reshape(rows, ld_out)[:, :D]
+                h.project_host(x, lvl, first_row, out)
+                return 0
+            except BaseException as e:   # noqa: B902 -- nothing may unwind through the C frames; re-raised by raise_error
+                errors.append(e)
+                return 1
+
+        self._fn = _capi.HostProjectFn(fn)                                  # alive as long as the descriptor
+        self.c = _capi.LevelHostProjectionC(self._fn, None, level, D, int(getattr(h, "stage_half_bytes", 0) or 0))
+
+    def close(self) -> None:
+        self._fn = self.c = None
+
+    def raise_error(self) -> None:
+        if self._errors:
+            raise self._errors.pop()
+
+
+# ------------------------------------------------------------------------------------------------
 # superviseddescent.hpp: the cascade
 # ------------------------------------------------------------------------------------------------
 class SupervisedDescentOptimiser:
     """superviseddescent::SupervisedDescentOptimiser<LinearRegressor, Normalisation> (superviseddescent.hpp:85-361).
 
-    projection: a HogTransform or a DeviceProjection (both stay on the device), or any callable
+    projection: a HogTransform or a DeviceProjection (both stay on the device), a HostProjection (rows filled on the host and
+    uploaded in a pipeline; RowwiseProjection wraps a per-row functor), or any callable
     h(x_row: np.ndarray, regressor_level: int, sample_index: int) -> row / float, evaluated on the host
-    exactly as the reference evaluates user functors (superviseddescent.hpp:178-189).
+    exactly as the reference evaluates user functors (superviseddescent.hpp:178-189).  train / test / predict try them in that
+    order: HogTransform, an object with project(), an object with project_host(), a callable.
     """
 
     def __init__(self, regressors: List[LinearRegressor], normalisation=None, ctx: Optional[Context] = None):
@@ -707,7 +797,8 @@ class SupervisedDescentOptimiser:
         return _dev(host, ctx), D
 
     def _chunk_rows(self, rows_per_chunk, frames: Optional[LevelFramesC], n: int, D: int, P: int, comm_h, route: int) -> int:
-        """Rows per chunk of a HogTransform or DeviceProjection level (frames None): rows_per_chunk (at most n), or -- None / 0
+        """Rows per chunk of a HogTransform, DeviceProjection or HostProjection level (frames None for the last two):
+        rows_per_chunk (at most n), or -- None / 0
         -- the most that fit beside the solve and the staging of host frames (sd_level_chunk_rows; memory torch has reserved but
         not handed out counts as free, so a warm caching allocator does not split a level that fits)."""
         if rows_per_chunk:
@@ -733,7 +824,8 @@ class SupervisedDescentOptimiser:
         (same results), the chunk buffer sized beside the staging they need.  A DeviceProjection trains the same way through
         sd_train_level_projected; an exception its project() raises is re-raised here (on several ranks the other ranks raise
         SdError: the level fails on every rank).  The automatic chunk leaves a DeviceProjection only the library's 512 MB reserve
-        for its own temporaries: one that needs more per row passes rows_per_chunk."""
+        for its own temporaries: one that needs more per row passes rows_per_chunk.  A HostProjection trains the same way through
+        sd_train_level_host_projected, with the same chunking, ranks and error rules."""
         from . import parallel
         ctx = self._ctx()
         lib = _capi.lib()
@@ -748,7 +840,8 @@ class SupervisedDescentOptimiser:
         n_global = comm.sum_int(n) if distributed else n
         hog = isinstance(projection, HogTransform)
         batched = not hog and _is_device_projection(projection)             # a DeviceProjection
-        self.chunk_rows = []                                                 # rows per chunk of each device-route level
+        hosted = not hog and not batched and _is_host_projection(projection)  # a HostProjection
+        self.chunk_rows = []                                                 # rows per chunk of each level-call level
 
         def route(D):
             if not distributed:
@@ -768,7 +861,7 @@ class SupervisedDescentOptimiser:
                 ctx.set_rank_diagnostic(True)                                # before the chunk query: the rank copy counts there
             nxt = torch.empty_like(cur)
             proj = None
-            if hog or batched:                                               # 1)-4) through a buffer of `rows` feature rows
+            if hog or batched or hosted:                                     # 1)-4) through a buffer of `rows` feature rows
                 D = projection.feature_length(level)
                 X = torch.empty((D, P), dtype=torch.float32, device=cur.device)
                 ld = (D + P + 3) // 4 * 4
@@ -781,11 +874,17 @@ class SupervisedDescentOptimiser:
                     rc = lib.sd_train_level(ctx.h, ch, C.byref(frames), ptr(cur), ptr(x_gt), n, P // 2, C.c_int64(n_global), C.byref(eyes),
                                             C.byref(projection.hog_params[level]), C.byref(norm), ptr(tmpl), ldt, C.byref(rc_), route(D),
                                             ptr(buf), C.c_int64(ld), rows, ptr(X), ptr(nxt), C.byref(lam))
-                else:
+                elif batched:
                     proj = _LevelProjection(ctx, projection, level, cur, buf)
                     rc = lib.sd_train_level_projected(ctx.h, ch, C.byref(proj.c), ptr(cur), ptr(x_gt), n, P, n_global, C.byref(norm),
                                                       ptr(tmpl), ldt, C.byref(rc_), route(D), ptr(buf), ld, rows, ptr(X), ptr(nxt),
                                                       C.byref(lam))
+                    proj.close()
+                else:
+                    proj = _LevelHostProjection(projection, level)
+                    rc = lib.sd_train_level_host_projected(ctx.h, ch, C.byref(proj.c), ptr(cur), ptr(x_gt), n, P, n_global, C.byref(norm),
+                                                           ptr(tmpl), ldt, C.byref(rc_), route(D), ptr(buf), ld, rows, ptr(X), ptr(nxt),
+                                                           C.byref(lam))
                     proj.close()
                 del buf
             else:
@@ -823,7 +922,8 @@ class SupervisedDescentOptimiser:
 
     def test(self, initialisations, templates, projection, on_regressor_iteration_callback=None, rows_per_chunk=None):
         """superviseddescent.hpp:262-306.  A HogTransform projection runs each level with sd_apply_level, a DeviceProjection
-        with sd_apply_level_projected, through a buffer of rows_per_chunk feature rows (None: as many as fit, as in train())."""
+        with sd_apply_level_projected, a HostProjection with sd_apply_level_host_projected, through a buffer of rows_per_chunk
+        feature rows (None: as many as fit, as in train())."""
         ctx = self._ctx()
         lib = _capi.lib()
         cur = _dev(initialisations, ctx).clone()
@@ -833,11 +933,12 @@ class SupervisedDescentOptimiser:
         tmpl = _dev(templates, ctx) if templates is not None and np.size(templates) > 0 else None
         hog = isinstance(projection, HogTransform)
         batched = not hog and _is_device_projection(projection)
+        hosted = not hog and not batched and _is_host_projection(projection)
         frames = projection.level_frames(n) if hog else None
         for level, reg in enumerate(self.regressors):
             norm = self.normalisation_strategy.c(P // 2)
             nxt = torch.empty_like(cur)
-            if hog or batched:
+            if hog or batched or hosted:
                 D = projection.feature_length(level)
                 ld = (D + 3) // 4 * 4
                 rows = self._chunk_rows(rows_per_chunk, frames, n, D, P, None, 0)
@@ -848,9 +949,14 @@ class SupervisedDescentOptimiser:
                     _check(ctx.h, lib.sd_apply_level(ctx.h, C.byref(frames), ptr(cur), n, P // 2, C.byref(eyes), C.byref(projection.hog_params[level]),
                                                      C.byref(norm), ptr(tmpl), ldt, ptr(reg.x), ptr(buf), C.c_int64(ld), rows, ptr(nxt)))
                 else:
-                    proj = _LevelProjection(ctx, projection, level, cur, buf)
-                    rc = lib.sd_apply_level_projected(ctx.h, C.byref(proj.c), ptr(cur), n, P, C.byref(norm), ptr(tmpl), ldt, ptr(reg.x),
-                                                      ptr(buf), ld, rows, ptr(nxt))
+                    if batched:
+                        proj = _LevelProjection(ctx, projection, level, cur, buf)
+                        rc = lib.sd_apply_level_projected(ctx.h, C.byref(proj.c), ptr(cur), n, P, C.byref(norm), ptr(tmpl), ldt,
+                                                          ptr(reg.x), ptr(buf), ld, rows, ptr(nxt))
+                    else:
+                        proj = _LevelHostProjection(projection, level)
+                        rc = lib.sd_apply_level_host_projected(ctx.h, C.byref(proj.c), ptr(cur), n, P, C.byref(norm), ptr(tmpl), ldt,
+                                                               ptr(reg.x), ptr(buf), ld, rows, ptr(nxt))
                     proj.close()
                     proj.raise_error()
                     _check(ctx.h, rc)

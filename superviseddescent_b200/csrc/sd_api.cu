@@ -121,8 +121,10 @@ int sd_ctx_create(int device, void* stream, sd_ctx** out)
     for (int i = 0; i < 6 && ok; ++i) ok = cudaEventCreate(&ctx->ev[i]) == cudaSuccess;
     for (int i = 0; i < 2 && ok; ++i) {
         ok = cudaEventCreateWithFlags(&ctx->stage_ev[i], cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&ctx->stage_done[i], cudaEventDisableTiming) == cudaSuccess;
+             cudaEventCreateWithFlags(&ctx->stage_done[i], cudaEventDisableTiming) == cudaSuccess &&
+             cudaEventCreateWithFlags(&ctx->host_stage_ev[i], cudaEventDisableTiming) == cudaSuccess;
     }
+    ok = ok && cudaEventCreateWithFlags(&ctx->host_chunk_free, cudaEventDisableTiming) == cudaSuccess;
     ok = ok && cudaMallocHost(&ctx->h_scratch, 4096) == cudaSuccess && cudaMalloc(&ctx->d_scratch, 4096) == cudaSuccess &&
          cudaMemset(ctx->d_scratch, 0, 4096) == cudaSuccess;
     if (!ok) { sd_ctx_destroy(ctx); return SD_ERR_CUDA; }
@@ -142,7 +144,11 @@ void sd_ctx_destroy(sd_ctx* ctx)
         if (ctx->d_stage[i]) cudaFree(ctx->d_stage[i]);
         if (ctx->stage_ev[i]) cudaEventDestroy(ctx->stage_ev[i]);
         if (ctx->stage_done[i]) cudaEventDestroy(ctx->stage_done[i]);
+        if (ctx->host_stage[i]) cudaFreeHost(ctx->host_stage[i]);
+        if (ctx->host_stage_ev[i]) cudaEventDestroy(ctx->host_stage_ev[i]);
     }
+    if (ctx->host_chunk_free) cudaEventDestroy(ctx->host_chunk_free);
+    if (ctx->host_x) cudaFreeHost(ctx->host_x);
     for (int i = 0; i < 6; ++i) if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
     for (int i = 0; i < 8; ++i) if (ctx->cg_ev[i]) cudaEventDestroy(ctx->cg_ev[i]);
     if (ctx->h_scratch) cudaFreeHost(ctx->h_scratch);

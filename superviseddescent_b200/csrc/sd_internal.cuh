@@ -69,6 +69,14 @@ struct sd_ctx {
     size_t stage_bytes[2] = {0, 0};
     cudaEvent_t stage_ev[2] = {nullptr, nullptr};
     cudaEvent_t stage_done[2] = {nullptr, nullptr};
+    // the levels on a host projection (sd_train.cu): pinned staging pair the callback fills, one event per half (its upload is
+    // done), the chunk buffer's last reader on the stream, and the pinned copy of the level's parameter rows
+    void* host_stage[2] = {nullptr, nullptr};
+    size_t host_stage_bytes[2] = {0, 0};
+    cudaEvent_t host_stage_ev[2] = {nullptr, nullptr};
+    cudaEvent_t host_chunk_free = nullptr;
+    void* host_x = nullptr;
+    size_t host_x_bytes = 0;
 };
 
 int sd_fail(sd_ctx* ctx, int code, const char* fmt, ...);

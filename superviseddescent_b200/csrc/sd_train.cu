@@ -4,6 +4,7 @@
 //   sd_train_level            superviseddescent.hpp:173-217: HOG, targets, shift, Gram accumulation, exchange, solve, update
 //   sd_apply_level            superviseddescent.hpp:262-306, 323-344: HOG, templates, update
 //   sd_*_level_projected      the same two levels with the feature rows from the caller's projection callback (RowSource)
+//   sd_*_level_host_projected the same with a host callback, its rows uploaded through a pinned staging pair (host_rows)
 //
 // [A^T A | A^T b] is a sum over rows, so a level never needs all of its feature rows at once.  The rows are shifted by the column
 // means of the first chunk (the pilot p, over all ranks) before they enter the Gram: with n0 rows in that chunk p is within about
@@ -375,30 +376,120 @@ int hog_rows(sd_ctx* ctx, const sd_level_frames& src, HostGather& g, const float
     return sd_hog_batch(ctx, &view, idx ? idx + r0 : nullptr, d_x + (int64_t)r0 * P, P, rows, L, eyes, p, d_chunk, ld);
 }
 
-// ---- the row source of a level (DESIGN 4.7) -----------------------------------------------------------------------------------
-// A level's feature rows come from the HOG of its frames (sd_train_level / sd_apply_level) or from the caller's projection
-// (sd_train_level_projected / sd_apply_level_projected).  Everything after the rows -- templates, targets, shift, Gram, exchange,
-// solve, update -- is one loop (train_rows, apply_rows) whichever the source.
+size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
+
+// ---- rows from a host projection: the copy pipeline (DESIGN 4.8) --------------------------------------------------------------
+// The callback fills one pinned staging half on the calling thread while the other half's rows go up on the copy stream; one event
+// per half tells the host when it may refill that half.  The first upload of a chunk waits for the chunk buffer's last reader on
+// the stream, and the stream waits for the chunk's last upload, so the host fills chunk k + 1 while the GPU works on chunk k.
+struct HostRows {
+    const float* h_x = nullptr;          // pinned copy of this rank's parameter rows (the context's host_x)
+    int64_t ld_out = 0;                  // floats between staged rows: roundup4(D)
+    int per_half = 1;                    // rows of one batch: what the requested staging half holds, at least one
+    int buf = 0;                         // the half the next batch fills
+};
+
+// the context's pinned buffer *p holds at least `bytes` (grow-only; the old one is freed once no upload reads it)
+int ensure_pinned(sd_ctx* ctx, void** p, size_t* have, size_t bytes)
+{
+    if (*have >= bytes) return SD_OK;
+    if (*p) {
+        SD_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
+        SD_CUDA(ctx, cudaFreeHost(*p));
+        *p = nullptr;
+        *have = 0;
+    }
+    SD_CUDA(ctx, cudaMallocHost(p, bytes));
+    *have = bytes;
+    return SD_OK;
+}
+
+// Sizes the staging pair from the descriptor and copies d_x (N x P) into pinned memory once for the level call.
+int host_prepare(sd_ctx* ctx, const sd_level_host_projection& hp, HostRows& h, const float* d_x, int N, int P)
+{
+    h.ld_out = (int64_t)round_up(hp.feature_length, 4);
+    const size_t row = (size_t)h.ld_out * sizeof(float);
+    const size_t fit = (hp.stage_half_bytes ? hp.stage_half_bytes : SD_STAGE_HALF_BYTES) / row;
+    h.per_half = fit < 1 ? 1 : (fit > INT_MAX ? INT_MAX : (int)fit);
+    h.buf = 0;
+    if (N == 0) return SD_OK;                                        // a rank without samples: no callback, no copy
+    const size_t half = (size_t)(h.per_half < N ? h.per_half : N) * row;    // no batch is longer than the level
+    for (int b = 0; b < 2; ++b) {
+        const int rc = ensure_pinned(ctx, &ctx->host_stage[b], &ctx->host_stage_bytes[b], half);
+        if (rc) return rc;
+    }
+    const size_t xbytes = (size_t)N * P * sizeof(float);
+    const int rc = ensure_pinned(ctx, &ctx->host_x, &ctx->host_x_bytes, xbytes);
+    if (rc) return rc;
+    SD_CUDA(ctx, cudaMemcpyAsync(ctx->host_x, d_x, xbytes, cudaMemcpyDeviceToHost, ctx->stream));
+    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    h.h_x = static_cast<const float*>(ctx->host_x);
+    return SD_OK;
+}
+
+// feature rows of samples [r0, r0 + rows) into columns [0, D) of the chunk buffer, batch by batch through the staging pair
+int host_rows(sd_ctx* ctx, const sd_level_host_projection& hp, HostRows& h, int P, int r0, int rows, float* d_chunk, int64_t ld)
+{
+    SD_CUDA(ctx, cudaEventRecord(ctx->host_chunk_free, ctx->stream));                 // after the previous chunk's last reader
+    SD_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->host_chunk_free, 0));
+    int rc = SD_OK, last = -1;
+    for (int b0 = 0; b0 < rows;) {
+        const int nb = rows - b0 < h.per_half ? rows - b0 : h.per_half;
+        const int buf = h.buf;
+        h.buf ^= 1;
+        SD_CUDA(ctx, cudaEventSynchronize(ctx->host_stage_ev[buf]));                  // the upload that last read this half is done
+        float* out = static_cast<float*>(ctx->host_stage[buf]);
+        const int64_t first = (int64_t)r0 + b0;
+        const int cb = hp.fn(hp.user, hp.level, h.h_x + first * P, P, first, nb, out, h.ld_out);
+        if (cb) {
+            rc = sd_fail(ctx, SD_ERR_INVALID, "projection callback returned %d", cb);
+            break;
+        }
+        SD_CUDA(ctx, cudaMemcpy2DAsync(d_chunk + (int64_t)b0 * ld, (size_t)ld * sizeof(float), out, (size_t)h.ld_out * sizeof(float),
+                                       (size_t)hp.feature_length * sizeof(float), nb, cudaMemcpyHostToDevice, ctx->copy_stream));
+        SD_CUDA(ctx, cudaEventRecord(ctx->host_stage_ev[buf], ctx->copy_stream));
+        last = buf;
+        b0 += nb;
+    }
+    // what reads the chunk (templates, targets, centring, Gram, update) waits for its uploads; after a failure too, so that the
+    // caller may free the buffer in stream order
+    if (last >= 0) SD_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->host_stage_ev[last], 0));
+    return rc;
+}
+
+// ---- the row source of a level (DESIGN 4.7, 4.8) ------------------------------------------------------------------------------
+// A level's feature rows come from the HOG of its frames (sd_train_level / sd_apply_level), from the caller's device projection
+// (sd_train_level_projected / sd_apply_level_projected) or from the caller's host projection (sd_*_level_host_projected).
+// Everything after the rows -- templates, targets, shift, Gram, exchange, solve, update -- is one loop (train_rows, apply_rows)
+// whichever the source.
 struct RowSource {
-    const sd_level_projection* proj = nullptr;   // the caller's projection; NULL: HOG of the frames below
+    const sd_level_projection* proj = nullptr;        // the caller's device projection ...
+    const sd_level_host_projection* hproj = nullptr;  // ... or host projection; both NULL: HOG of the frames below
+    HostRows h{};
     const sd_level_frames* frames = nullptr;
     HostGather g{};
     int L = 0;
     const sd_normalisation* hog_eyes = nullptr;
     const sd_hog_param* p = nullptr;
+    void use(const sd_level_projection* d) { proj = d; }
+    void use(const sd_level_host_projection* d) { hproj = d; }
+    bool callback() const { return proj || hproj; }
 };
 
-// On the HOG source: checks the frames and sets up a host-frame gather (SD_ERR_INVALID before any work is queued).
-int source_prepare(sd_ctx* ctx, RowSource& s, int N)
+// On the HOG source: checks the frames and sets up a host-frame gather (SD_ERR_INVALID before any work is queued).  On a host
+// projection: the staging pair and the pinned copy of d_x.
+int source_prepare(sd_ctx* ctx, RowSource& s, const float* d_x, int P, int N)
 {
+    if (s.hproj) return host_prepare(ctx, *s.hproj, s.h, d_x, N, P);
     return s.proj ? SD_OK : frames_prepare(ctx, s.frames, s.g, N);
 }
 
 // feature rows of samples [r0, r0 + rows) into columns [0, D) of the chunk buffer; P = the parameter width
 int source_rows(sd_ctx* ctx, RowSource& s, const float* d_x, int P, int r0, int rows, float* d_chunk, int64_t ld)
 {
-    if (!s.proj) return hog_rows(ctx, *s.frames, s.g, d_x, r0, rows, s.L, s.hog_eyes, s.p, d_chunk, ld);
+    if (!s.callback()) return hog_rows(ctx, *s.frames, s.g, d_x, r0, rows, s.L, s.hog_eyes, s.p, d_chunk, ld);
     if (rows == 0) return SD_OK;                                     // a rank without samples
+    if (s.hproj) return host_rows(ctx, *s.hproj, s.h, P, r0, rows, d_chunk, ld);
     const int rc = s.proj->fn(s.proj->user, ctx, s.proj->level, d_x + (int64_t)r0 * P, P, r0, rows, d_chunk, ld);
     return rc ? sd_fail(ctx, SD_ERR_INVALID, "projection callback returned %d", rc) : SD_OK;
 }
@@ -406,12 +497,14 @@ int source_rows(sd_ctx* ctx, RowSource& s, const float* d_x, int P, int r0, int 
 // the end of a level on host frames: no patch may have read outside its planned region
 int source_finish(sd_ctx* ctx, const RowSource& s, int N)
 {
-    return s.proj || s.frames->images ? SD_OK : gather_finish(ctx, s.g, N);
+    return s.callback() || s.frames->images ? SD_OK : gather_finish(ctx, s.g, N);
 }
 
-// The rules of a caller's projection (SD_ERR_INVALID before any work is queued): a callback, D >= 1, and a normalisation that can
-// read the parameter rows -- inter-eye distance needs [x.., y..] rows (even P) with its eye indices below P / 2.
-int check_projection(sd_ctx* ctx, const char* fn, const sd_level_projection* proj, int P, const sd_normalisation* norm)
+// The rules of a caller's projection, device or host (SD_ERR_INVALID before any work is queued): a callback, D >= 1, and a
+// normalisation that can read the parameter rows -- inter-eye distance needs [x.., y..] rows (even P) with its eye indices below
+// P / 2.
+template <class Desc>
+int check_projection(sd_ctx* ctx, const char* fn, const Desc* proj, int P, const sd_normalisation* norm)
 {
     if (!proj || !proj->fn || proj->feature_length < 1)
         return sd_fail(ctx, SD_ERR_INVALID, "%s: the projection needs a callback and feature_length >= 1", fn);
@@ -426,14 +519,12 @@ int check_projection(sd_ctx* ctx, const char* fn, const sd_level_projection* pro
     return SD_OK;
 }
 
-size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
-
 // Several ranks on a caller's projection: a callback that fails on one rank must not leave the others waiting in a collective.  The
 // failing rank still takes part in every collective up to the exchange (the centring's without rows), and the ranks agree on a
 // failure -- one host integer -- before the exchange and at the end of the level, so either every rank fails the level or none.
 int agree_on_failure(sd_ctx* ctx, const char* fn, const RowSource& s, sd_comm* c, int failed)
 {
-    if (!s.proj || !c) return failed;
+    if (!s.callback() || !c) return failed;
     int64_t any = failed != 0;
     const int rc = sd_comm_sum_int64(ctx, c, &any);
     if (failed) return failed;                                       // keeps its own message
@@ -441,13 +532,13 @@ int agree_on_failure(sd_ctx* ctx, const char* fn, const RowSource& s, sd_comm* c
     return any ? sd_fail(ctx, SD_ERR_INVALID, "%s: the projection callback failed on another rank", fn) : SD_OK;
 }
 
-// One training level of D features on P parameters from the row source s (sd_train_level, sd_train_level_projected); the caller
+// One training level of D features on P parameters from the row source s (sd_train_level, sd_train_level_*projected); the caller
 // has checked the arguments.
 int train_rows(sd_ctx* ctx, const char* fn, sd_comm* comm, RowSource& s, int D, const float* d_x, const float* d_x_gt, int N_local,
                int P, int64_t n_global, const sd_normalisation* norm, const float* d_templates, int64_t ldt, const sd_regulariser* reg,
                int route, float* d_chunk, int64_t ld, int chunk_rows, float* d_X, float* d_x_next, float* lambda_out)
 {
-    int rc = source_prepare(ctx, s, N_local);
+    int rc = source_prepare(ctx, s, d_x, P, N_local);
     if (rc) return rc;
     float* mu = (float*)sd_workspace(ctx, SD_WS_LEVEL, (size_t)D * (P + 1) * sizeof(float));
     if (!mu) return SD_ERR_CUDA;
@@ -465,7 +556,7 @@ int train_rows(sd_ctx* ctx, const char* fn, sd_comm* comm, RowSource& s, int D, 
     for (int k = 0; k < chunks; ++k) {
         const int r0 = k * chunk_rows, rows = N_local - r0 < chunk_rows ? N_local - r0 : chunk_rows;
         rc = source_rows(ctx, s, d_x, P, r0, rows, d_chunk, ld);                                                      // :173-189
-        if (rc && s.proj && c) {                          // agree_on_failure: the centring's collective without rows, then stop
+        if (rc && s.callback() && c) {                    // agree_on_failure: the centring's collective without rows, then stop
             failed = rc;
             rc = k == 0 ? sd_centre_features(ctx, c, d_chunk, ld, 0, D, (int)n0, reg, mu) : SD_OK;
             if (rc) return rc;
@@ -495,12 +586,12 @@ int train_rows(sd_ctx* ctx, const char* fn, sd_comm* comm, RowSource& s, int D, 
     return agree_on_failure(ctx, fn, s, c, rc);
 }
 
-// One test / predict level of D features on P parameters from the row source s (sd_apply_level, sd_apply_level_projected); the
+// One test / predict level of D features on P parameters from the row source s (sd_apply_level, sd_apply_level_*projected); the
 // caller has checked the arguments.
 int apply_rows(sd_ctx* ctx, RowSource& s, int D, const float* d_x, int N, int P, const sd_normalisation* norm, const float* d_templates,
                int64_t ldt, const float* d_X, float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next)
 {
-    int rc = source_prepare(ctx, s, N);
+    int rc = source_prepare(ctx, s, d_x, P, N);
     for (int r0 = 0; !rc && r0 < N; r0 += chunk_rows) {
         const int rows = N - r0 < chunk_rows ? N - r0 : chunk_rows;
         rc = source_rows(ctx, s, d_x, P, r0, rows, d_chunk, ld);
@@ -510,6 +601,57 @@ int apply_rows(sd_ctx* ctx, RowSource& s, int D, const float* d_x, int N, int P,
     if (!rc) rc = source_finish(ctx, s, N);
     return rc;
 }
+
+// SD_REQUIRE for the projected levels, which name the entry point `fn` in their messages
+#define SD_REQUIRE_IN(ctx, fn, cond, msg)                                                      \
+    do {                                                                                       \
+        if (!(cond)) return sd_fail((ctx), SD_ERR_INVALID, "%s: %s", (fn), msg);               \
+    } while (0)
+
+// sd_train_level_projected / sd_train_level_host_projected: the argument checks, then the level from the caller's projection
+template <class Desc>
+int train_projected(sd_ctx* ctx, const char* fn, sd_comm* comm, const Desc* proj, const float* d_x, const float* d_x_gt, int N_local,
+                    int P, int64_t n_global, const sd_normalisation* norm, const float* d_templates, int64_t ldt, const sd_regulariser* reg,
+                    int route, float* d_chunk, int64_t ld, int chunk_rows, float* d_X, float* d_x_next, float* lambda_out)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE_IN(ctx, fn, d_x && d_x_gt && reg && d_chunk && d_X && d_x_next, "null argument");
+    SD_REQUIRE_IN(ctx, fn, N_local >= 0 && n_global >= 1 && n_global <= INT_MAX, "bad sample count");
+    SD_REQUIRE_IN(ctx, fn, chunk_rows >= 1, "chunk_rows must be >= 1");
+    SD_REQUIRE_IN(ctx, fn, reg->type == 0 || reg->type == 1, "unknown regularisation type");
+    const int rc = check_projection(ctx, fn, proj, P, norm);
+    if (rc) return rc;
+    const int D = proj->feature_length;
+    SD_REQUIRE_IN(ctx, fn, ld >= (int64_t)D + P, "ld < D + P");
+    SD_REQUIRE_IN(ctx, fn, !d_templates || (chunk_rows >= N_local && ldt >= D), "templates need one chunk (chunk_rows >= N_local) and ldt >= D");
+    SD_REQUIRE_IN(ctx, fn, d_x_next != d_x, "x_next must not alias x");
+    RowSource s;
+    s.use(proj);
+    return train_rows(ctx, fn, comm, s, D, d_x, d_x_gt, N_local, P, n_global, norm, d_templates, ldt, reg, route, d_chunk, ld,
+                      chunk_rows, d_X, d_x_next, lambda_out);
+}
+
+// sd_apply_level_projected / sd_apply_level_host_projected
+template <class Desc>
+int apply_projected(sd_ctx* ctx, const char* fn, const Desc* proj, const float* d_x, int N, int P, const sd_normalisation* norm,
+                    const float* d_templates, int64_t ldt, const float* d_X, float* d_chunk, int64_t ld, int chunk_rows, float* d_x_next)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE_IN(ctx, fn, d_x && d_X && d_chunk && d_x_next, "null argument");
+    SD_REQUIRE_IN(ctx, fn, N >= 0, "bad sample count");
+    SD_REQUIRE_IN(ctx, fn, chunk_rows >= 1, "chunk_rows must be >= 1");
+    const int rc = check_projection(ctx, fn, proj, P, norm);
+    if (rc) return rc;
+    const int D = proj->feature_length;
+    SD_REQUIRE_IN(ctx, fn, ld >= D, "ld < D");
+    SD_REQUIRE_IN(ctx, fn, !d_templates || ldt >= D, "ldt < D");
+    SD_REQUIRE_IN(ctx, fn, d_x_next != d_x, "x_next must not alias x");
+    RowSource s;
+    s.use(proj);
+    return apply_rows(ctx, s, D, d_x, N, P, norm, d_templates, ldt, d_X, d_chunk, ld, chunk_rows, d_x_next);
+}
+
+#undef SD_REQUIRE_IN
 
 }  // namespace
 
@@ -565,40 +707,31 @@ int sd_train_level_projected(sd_ctx* ctx, sd_comm* comm, const sd_level_projecti
                              const sd_regulariser* reg, int route, float* d_chunk, int64_t ld, int chunk_rows, float* d_X,
                              float* d_x_next, float* lambda_out)
 {
-    if (!ctx) return SD_ERR_INVALID;
-    SD_REQUIRE(ctx, d_x && d_x_gt && reg && d_chunk && d_X && d_x_next, "null argument");
-    SD_REQUIRE(ctx, N_local >= 0 && n_global >= 1 && n_global <= INT_MAX, "bad sample count");
-    SD_REQUIRE(ctx, chunk_rows >= 1, "chunk_rows must be >= 1");
-    SD_REQUIRE(ctx, reg->type == 0 || reg->type == 1, "unknown regularisation type");
-    const int rc = check_projection(ctx, __func__, proj, P, norm);
-    if (rc) return rc;
-    const int D = proj->feature_length;
-    SD_REQUIRE(ctx, ld >= (int64_t)D + P, "ld < D + P");
-    SD_REQUIRE(ctx, !d_templates || (chunk_rows >= N_local && ldt >= D), "templates need one chunk (chunk_rows >= N_local) and ldt >= D");
-    SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
-    RowSource s;
-    s.proj = proj;
-    return train_rows(ctx, __func__, comm, s, D, d_x, d_x_gt, N_local, P, n_global, norm, d_templates, ldt, reg, route, d_chunk, ld,
-                      chunk_rows, d_X, d_x_next, lambda_out);
+    return train_projected(ctx, __func__, comm, proj, d_x, d_x_gt, N_local, P, n_global, norm, d_templates, ldt, reg, route, d_chunk, ld,
+                           chunk_rows, d_X, d_x_next, lambda_out);
 }
 
 int sd_apply_level_projected(sd_ctx* ctx, const sd_level_projection* proj, const float* d_x, int N, int P, const sd_normalisation* norm,
                              const float* d_templates, int64_t ldt, const float* d_X, float* d_chunk, int64_t ld, int chunk_rows,
                              float* d_x_next)
 {
-    if (!ctx) return SD_ERR_INVALID;
-    SD_REQUIRE(ctx, d_x && d_X && d_chunk && d_x_next, "null argument");
-    SD_REQUIRE(ctx, N >= 0, "bad sample count");
-    SD_REQUIRE(ctx, chunk_rows >= 1, "chunk_rows must be >= 1");
-    const int rc = check_projection(ctx, __func__, proj, P, norm);
-    if (rc) return rc;
-    const int D = proj->feature_length;
-    SD_REQUIRE(ctx, ld >= D, "ld < D");
-    SD_REQUIRE(ctx, !d_templates || ldt >= D, "ldt < D");
-    SD_REQUIRE(ctx, d_x_next != d_x, "x_next must not alias x");
-    RowSource s;
-    s.proj = proj;
-    return apply_rows(ctx, s, D, d_x, N, P, norm, d_templates, ldt, d_X, d_chunk, ld, chunk_rows, d_x_next);
+    return apply_projected(ctx, __func__, proj, d_x, N, P, norm, d_templates, ldt, d_X, d_chunk, ld, chunk_rows, d_x_next);
+}
+
+int sd_train_level_host_projected(sd_ctx* ctx, sd_comm* comm, const sd_level_host_projection* proj, const float* d_x, const float* d_x_gt,
+                                  int N_local, int P, int64_t n_global, const sd_normalisation* norm, const float* d_templates,
+                                  int64_t ldt, const sd_regulariser* reg, int route, float* d_chunk, int64_t ld, int chunk_rows,
+                                  float* d_X, float* d_x_next, float* lambda_out)
+{
+    return train_projected(ctx, __func__, comm, proj, d_x, d_x_gt, N_local, P, n_global, norm, d_templates, ldt, reg, route, d_chunk, ld,
+                           chunk_rows, d_X, d_x_next, lambda_out);
+}
+
+int sd_apply_level_host_projected(sd_ctx* ctx, const sd_level_host_projection* proj, const float* d_x, int N, int P,
+                                  const sd_normalisation* norm, const float* d_templates, int64_t ldt, const float* d_X, float* d_chunk,
+                                  int64_t ld, int chunk_rows, float* d_x_next)
+{
+    return apply_projected(ctx, __func__, proj, d_x, N, P, norm, d_templates, ldt, d_X, d_chunk, ld, chunk_rows, d_x_next);
 }
 
 int sd_level_chunk_rows(sd_ctx* ctx, sd_comm* comm, const sd_level_frames* frames, int64_t N_local, int D, int M, int route,

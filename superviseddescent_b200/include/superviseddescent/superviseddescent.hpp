@@ -5,11 +5,12 @@
 //
 //   device route   RegressorType is this package's LinearRegressor<>, the projection is a device
 //                  projection (rcr::HogTransform, or a batch projection with feature_length / project_device,
-//                  see is_device_batch_projection) and the normalisation maps to sd_normalisation:
-//                  features, targets, Gram, solve and update all stay in HBM, one sd_train_level /
-//                  sd_apply_level call (sd_*_level_projected for a batch projection) per level through a
-//                  buffer of feature rows that holds the whole level when it fits, and chunks of it
-//                  otherwise (set_rows_per_chunk).
+//                  see is_device_batch_projection) or a host batch projection (feature_length / project_host,
+//                  see is_host_batch_projection; RowwiseProjection wraps a per-row functor) and the
+//                  normalisation maps to sd_normalisation: targets, Gram, solve and update all stay in HBM,
+//                  one sd_train_level / sd_apply_level call (sd_*_level_projected, sd_*_level_host_projected for
+//                  a batch projection) per level through a buffer of feature rows that holds the whole level
+//                  when it fits, and chunks of it otherwise (set_rows_per_chunk).
 //   functor route  any other projection functor h(row, level, idx) -> Mat | float is USER host code; it is
 //                  evaluated on a pool of host threads exactly as the reference does (:173-189) and the
 //                  stacked feature matrix goes through RegressorType::learn / predict (which are GPU calls
@@ -55,14 +56,48 @@ template <class P> struct is_device_batch_projection<P, void_t<
     decltype(static_cast<int>(std::declval<P&>().project_device(std::declval<sd_ctx*>(), size_t(0), std::declval<const float*>(), int64_t(0),
                                                                 int64_t(0), 0, std::declval<float*>(), int64_t(0))))>> : std::true_type {};
 
+// projection that writes the feature rows of a batch on the host (sd_level_host_projection):
+//   int feature_length(size_t level);
+//   int project_host(size_t level, const float* x, int64_t ldx, int64_t first_row, int rows, float* out, int64_t ld);
+// x: the batch's parameter rows (pitch ldx = P); out: a pinned staging half (pitch ld), columns [0, D) of `rows` rows to write.
+// project_host follows the host callback contract of include/sd_b200.h (deterministic, no calls into the library's context); a
+// non-zero return or an exception fails the level, and the exception is rethrown from train() / test().  RowwiseProjection makes
+// one from a per-row functor.
+template <class P, class = void> struct is_host_batch_projection : std::false_type {};
+template <class P> struct is_host_batch_projection<P, void_t<
+    decltype(static_cast<int>(std::declval<P&>().feature_length(size_t(0)))),
+    decltype(static_cast<int>(std::declval<P&>().project_host(size_t(0), std::declval<const float*>(), int64_t(0), int64_t(0), 0,
+                                                              std::declval<float*>(), int64_t(0))))>> : std::true_type {};
+
 template <class P> struct takes_device_route
-    : std::integral_constant<bool, is_device_projection<P>::value || is_device_batch_projection<P>::value> {};
+    : std::integral_constant<bool, is_device_projection<P>::value || is_device_batch_projection<P>::value ||
+                                       is_host_batch_projection<P>::value> {};
 
-// Where the device route's levels get their feature rows: a HogTransform's frames (sd_train_level / sd_apply_level), or a batch
-// projection's callback (sd_train_level_projected / sd_apply_level_projected).
-template <class P, bool Hog = is_device_projection<P>::value> class LevelSource;
+// Where the device route's levels get their feature rows: a HogTransform's frames (sd_train_level / sd_apply_level), a device
+// batch projection's callback (sd_train_level_projected / sd_apply_level_projected) or a host batch projection's callback
+// (sd_train_level_host_projected / sd_apply_level_host_projected), tried in that order.
+enum { kHogSource, kDeviceSource, kHostSource };
+template <class P> struct source_kind
+    : std::integral_constant<int, is_device_projection<P>::value ? kHogSource : (is_device_batch_projection<P>::value ? kDeviceSource : kHostSource)> {};
 
-template <class P> class LevelSource<P, true> {
+template <class P, int Kind = source_kind<P>::value> class LevelSource;
+
+// an exception of the projection, kept while the C call unwound normally, for rethrow() after the call
+class CallbackError {
+public:
+    void rethrow()
+    {
+        if (!error) return;
+        std::exception_ptr e = error;
+        error = nullptr;
+        std::rethrow_exception(e);
+    }
+
+protected:
+    std::exception_ptr error;
+};
+
+template <class P> class LevelSource<P, kHogSource> {
 public:
     LevelSource(P& projection, int n) : h(projection), eyes(projection.eyes()), frames(projection.level_frames(n)) {}
     const sd_level_frames* level_frames() const { return &frames; }
@@ -88,7 +123,7 @@ private:
     sd_level_frames frames;
 };
 
-template <class P> class LevelSource<P, false> {
+template <class P> class LevelSource<P, kDeviceSource> : public CallbackError {
 public:
     LevelSource(P& projection, int /*n*/) : h(projection) {}
     const sd_level_frames* level_frames() const { return nullptr; }
@@ -105,14 +140,6 @@ public:
     {
         const sd_level_projection proj = descriptor(level);
         return sd_apply_level_projected(ctx, &proj, d_x, n, Pd, &norm, tmpl, ldt, X, chunk, ld, rows, x_next);
-    }
-    // an exception of project_device, kept while the C call unwound normally, is rethrown here
-    void rethrow()
-    {
-        if (!error) return;
-        std::exception_ptr e = error;
-        error = nullptr;
-        std::rethrow_exception(e);
     }
 
 private:
@@ -136,7 +163,49 @@ private:
         }
     }
     P& h;
-    std::exception_ptr error;
+};
+
+template <class P> class LevelSource<P, kHostSource> : public CallbackError {
+public:
+    LevelSource(P& projection, int /*n*/) : h(projection) {}
+    const sd_level_frames* level_frames() const { return nullptr; }
+    int train(sd_ctx* ctx, sd_comm* c, size_t level, const float* d_x, const float* d_gt, int n, int Pd, int64_t n_global,
+              const sd_normalisation& norm, const float* tmpl, int64_t ldt, const sd_regulariser& reg, int route, float* chunk,
+              int64_t ld, int rows, float* X, float* x_next)
+    {
+        const sd_level_host_projection proj = descriptor(level);
+        return sd_train_level_host_projected(ctx, c, &proj, d_x, d_gt, n, Pd, n_global, &norm, tmpl, ldt, &reg, route, chunk, ld, rows, X,
+                                             x_next, nullptr);
+    }
+    int apply(sd_ctx* ctx, size_t level, const float* d_x, int n, int Pd, const sd_normalisation& norm, const float* tmpl, int64_t ldt,
+              const float* X, float* chunk, int64_t ld, int rows, float* x_next)
+    {
+        const sd_level_host_projection proj = descriptor(level);
+        return sd_apply_level_host_projected(ctx, &proj, d_x, n, Pd, &norm, tmpl, ldt, X, chunk, ld, rows, x_next);
+    }
+
+private:
+    sd_level_host_projection descriptor(size_t level)
+    {
+        sd_level_host_projection proj{};
+        proj.fn = &LevelSource::call;
+        proj.user = this;
+        proj.level = static_cast<int32_t>(level);
+        proj.feature_length = h.feature_length(level);
+        proj.stage_half_bytes = 0;               // the library's default
+        return proj;
+    }
+    static int call(void* user, int level, const float* x, int64_t ldx, int64_t first_row, int rows, float* out, int64_t ld)
+    {
+        LevelSource* self = static_cast<LevelSource*>(user);
+        try {
+            return self->h.project_host(static_cast<size_t>(level), x, ldx, first_row, rows, out, ld);
+        } catch (...) {                          // nothing may unwind through the library's frames
+            self->error = std::current_exception();
+            return -1;
+        }
+    }
+    P& h;
 };
 
 template <class N, class = void> struct has_c_normalisation : std::false_type {};
@@ -178,6 +247,65 @@ cv::Mat project_on_host(const cv::Mat& current_x, size_t level, ProjectionFuncti
 
 }  // namespace detail
 
+// A reference-style projection functor h(cv::Mat row, size_t level, int index) -> Mat | float as a host batch projection, so that
+// the optimiser runs it through the level pipeline (chunks, several ranks, the host filling rows while the GPU works) instead of
+// the functor route.  project_host evaluates a batch's rows on hardware_concurrency() threads, each worker with its own copy of
+// the functor, as the functor route does; the rows h sees are views of the library's pinned copy of the parameters.
+// feature_length: one D for every level, or one per level.
+template <class H>
+class RowwiseProjection {
+public:
+    RowwiseProjection(H h, int feature_length) : h(std::move(h)), lengths(1, feature_length) {}
+    RowwiseProjection(H h, std::vector<int> feature_lengths) : h(std::move(h)), lengths(std::move(feature_lengths)) {}
+
+    int feature_length(size_t level) const { return lengths.size() == 1 ? lengths[0] : lengths.at(level); }
+
+    int project_host(size_t level, const float* x, int64_t ldx, int64_t first_row, int rows, float* out, int64_t ld)
+    {
+        const int D = feature_length(level);
+        unsigned threads = std::thread::hardware_concurrency();
+        if (threads == 0) threads = 4;
+        if (threads > static_cast<unsigned>(rows)) threads = rows > 0 ? rows : 1;
+        std::vector<std::exception_ptr> errors(threads);
+        auto work = [&](unsigned t, H& projection) {
+            try {
+                for (int i = static_cast<int>(t); i < rows; i += static_cast<int>(threads)) {
+                    const cv::Mat row(1, static_cast<int>(ldx), CV_32FC1, const_cast<float*>(x + static_cast<int64_t>(i) * ldx));
+                    const cv::Mat f = detail::as_row(projection(row, level, static_cast<int>(first_row + i)));
+                    if (f.type() != CV_32FC1 || f.rows * f.cols != D)
+                        throw std::runtime_error("RowwiseProjection: the functor returned " + std::to_string(f.rows * f.cols) + " values for row " +
+                                                 std::to_string(first_row + i) + ", feature_length is " + std::to_string(D));
+                    float* dst = out + static_cast<int64_t>(i) * ld;
+                    for (int k = 0; k < D; ++k) dst[k] = f.at<float>(k);
+                }
+            } catch (...) {
+                errors[t] = std::current_exception();
+            }
+        };
+        if (threads == 1) {
+            work(0, h);
+        } else {
+            std::vector<std::thread> pool;
+            for (unsigned t = 0; t < threads; ++t)
+                pool.emplace_back([&work, t, projection = h]() mutable { work(t, projection); });   // each worker owns a copy
+            for (auto& th : pool) th.join();
+        }
+        for (auto& e : errors)
+            if (e) std::rethrow_exception(e);
+        return 0;
+    }
+
+private:
+    H h;
+    std::vector<int> lengths;
+};
+
+template <class H> RowwiseProjection<H> rowwise(H h, int feature_length) { return RowwiseProjection<H>(std::move(h), feature_length); }
+template <class H> RowwiseProjection<H> rowwise(H h, std::vector<int> feature_lengths)
+{
+    return RowwiseProjection<H>(std::move(h), std::move(feature_lengths));
+}
+
 template <class RegressorType, class NormalisationStrategy = NoNormalisation>
 class SupervisedDescentOptimiser {
 public:
@@ -203,7 +331,7 @@ public:
     {
         static_assert(detail::takes_device_route<ProjectionFunction>::value && detail::has_c_normalisation<NormalisationStrategy>::value &&
                           detail::is_device_regressor<RegressorType>::value,
-                      "multi-GPU training needs the device route (HogTransform or device batch projection, device regressors)");
+                      "multi-GPU training needs the device route (HogTransform, device or host batch projection, device regressors)");
         comm = communicator;
         comm_route = route;
         train_impl(parameters, initialisations, templates, projection, on_training_epoch_callback, std::true_type());
