@@ -139,7 +139,6 @@ void sd_ctx_destroy(sd_ctx* ctx)
     cudaStreamSynchronize(ctx->stream);
     if (ctx->copy_stream) cudaStreamSynchronize(ctx->copy_stream);
     for (int i = 0; i < SD_WS_COUNT; ++i) if (ctx->ws[i]) cudaFree(ctx->ws[i]);
-    for (int i = 0; i <= SD_MAX_BINS; ++i) if (ctx->hog_lut[i]) cudaFree(ctx->hog_lut[i]);
     for (int i = 0; i < 2; ++i) {
         if (ctx->d_stage[i]) cudaFree(ctx->d_stage[i]);
         if (ctx->stage_ev[i]) cudaEventDestroy(ctx->stage_ev[i]);

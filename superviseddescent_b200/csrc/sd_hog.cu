@@ -8,14 +8,15 @@
 //   zero-padded crop: ONE TMA tile load per patch (3-D tensor map over the frame batch; out-of-frame
 //     bytes are zero-filled by the TMA = copyMakeBorder(BORDER_CONSTANT 0))   adaptive_vlhog.hpp:135-151
 //   cv::resize INTER_LINEAR (fixed point), tables precomputed once per face   adaptive_vlhog.hpp:154-155
-//   gradient, orientation arg-max and modulus from device-generated tables (integer results, bit exact)  hog.c:631-672
+//   gradient, orientation arg-max and modulus in registers (bit exact: margin-checked arg-max, exact fallback)  hog.c:631-672
 //   bilinear spatial vote as two separable passes (rows x cell columns, then cell rows; no atomics)      hog.c:697-724
 //   cell energy, 2x2-block normalisation in double, clamp 0.2    hog.c:875-1053
 //   per-dimension transpose + landmark concatenation + bias      adaptive_vlhog.hpp:166-183
 //
 // Arithmetic that decides an INTEGER result (crop centre, half size, resize taps, orientation bin)
 // is written with explicit round-to-nearest intrinsics so that no FMA contraction can change it;
-// the reference is built for baseline x86-64 (mul then add).  The only deviation from the
+// the reference is built for baseline x86-64 (mul then add).  The orientation bin's margin test (hog_bin) is the exception:
+// its error bound allows FMA, and the pixels it cannot decide take the reference expression.  The only deviation from the
 // reference's value stream is the summation ORDER of the float votes inside a cell histogram
 // (fixed, deterministic tree here; raster order there): ~1e-7 relative.
 #include "sd_internal.cuh"
@@ -28,7 +29,6 @@ namespace {
 
 constexpr int kHogThreads = 256;
 constexpr int kHogWarps = kHogThreads / 32;
-constexpr int kLutDim = 511;                       // gx, gy in [-255, 255]
 
 struct HogArgs {
     const uint8_t* images;
@@ -44,8 +44,8 @@ struct HogArgs {
     int N, L;
     int variant, nc, cs, K, fs, dd;
     const int* half;            // per sample: half patch size (hog_geometry_kernel)
-    const int8_t* lut;          // (gy+255)*511 + (gx+255) -> directed orientation bin, -1 for a zero gradient
-    const float* mag_lut;       // gx*gx + gy*gy -> sqrtf of it (the exact integer's correctly rounded root)
+    float ox[SD_MAX_BINS], oy[SD_MAX_BINS];   // orientation k: (cos, sin)(k pi / K) in float, host libm (hog.c:195-204)
+    int vbin[2];                // reference bin of a gradient (0, gy): [0] gy > 0, [1] gy < 0
     const int* rtab;            // per sample: resize tables [5][fs] (hog_geometry_kernel)
     const float* btab;          // per launch: spatial binning weights [nc][fs], then lo[nc], hi[nc] (hog_bintab_kernel)
     int tma_count;              // number of usable tensor-map size classes (0: the window is staged by load loops)
@@ -130,44 +130,57 @@ __global__ void hog_bintab_kernel(int fs, int nc, int cs, float* __restrict__ bt
     }
 }
 
-// sqrtf of every possible squared gradient modulus of an 8-bit patch (gx, gy in [-255, 255]): hog.c:645 takes sqrtf of the
-// float gx*gx + gy*gy, which is an exactly representable integer here
-__global__ void hog_maglut_kernel(float* __restrict__ lut, int n)
+// ---- orientation bin of a pixel with a non-zero gradient (gx, gy), the reference's float expression verbatim
+//      (hog.c:645-672): modulus, normalised gradient, then the first maximum of |<u, o_k>| in ascending k -------------
+__device__ __forceinline__ int hog_bin_reference(const HogArgs& a, int K, float gx, float gy, float g)
 {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) lut[i] = __fsqrt_rn((float)i);
+    // (float)((double)gx / max((double)g, 1e-10)) == gx / g in float: double rounding is innocuous for
+    // division when the wide format has >= 2p+2 bits (53 >= 50).
+    const float ux = __fdiv_rn(gx, g);
+    const float uy = __fdiv_rn(gy, g);
+    float best = 0.f;
+    int bin = -1;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        float s = __fadd_rn(__fmul_rn(ux, a.ox[k]), __fmul_rn(uy, a.oy[k]));
+        int b = k;
+        if (s < 0.f) { s = -s; b += K; }
+        if (s > best) { best = s; bin = b; }   // strict >, ascending k
+    }
+    return bin;
 }
 
-// ---- (gx, gy) -> orientation bin table, generated ON THE DEVICE with the reference's float expression
-//      (hog.c:645-672): gradients of an 8-bit patch are integers in [-255, 255], so the arg-max is a pure
-//      function of the pair and can be tabulated exactly. ---------------------------------------------
-struct LutArgs {
-    int K;
-    float ox[SD_MAX_BINS], oy[SD_MAX_BINS];
-};
+// ---- orientation bin of an interior pixel without a division.  t_k = gx ox_k + gy oy_k on the integer gradient decides the
+//      arg-max whenever its winner leads the runner-up by more than eps |g|; only the other lanes need the exact answer below.
+//      Why that is exact (u = 2^-24, r = |g| exact, e_k = gx ox_k + gy oy_k exact, ox_k^2 + oy_k^2 = 1 + O(u)):
+//        |t_k - e_k|     <= 2u r                           (one product, one FMA)
+//        |s_k - e_k / r| <= 4u                              (s_k: the reference's float dot product of gx/g, gy/g)
+//      so t_b leading every other |t_j| by eps r makes |s_b| lead every |s_j| by (eps - 12u) > 0, and |t_b| > eps r fixes
+//      the sign of s_b: the reference's first strict maximum is the same k and the same half-plane.  eps = 4e-6 is ~33u;
+//      the slack also covers the rounding of the test itself (squared, against eps^2 g2, to avoid the root).
+//      tests/test_gpu_hog_orientation.py checks every (gx, gy) in [-255, 255]^2 at every K in 1..16. ------------------------
+constexpr float kBinMargin2 = 4e-6f * 4e-6f;
 
-__global__ void hog_lut_kernel(const LutArgs t, int8_t* __restrict__ lut)
+__device__ __forceinline__ int hog_bin(const HogArgs& a, int K, int gx, int gy, int g2, float g)
 {
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= kLutDim * kLutDim) return;
-    const float gx = (float)(idx % kLutDim - 255), gy = (float)(idx / kLutDim - 255);
-    const float g2 = __fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy));
-    int bin = -1;
-    if (g2 > 0.f) {
-        const float g = __fsqrt_rn(g2);
-        // (float)((double)gx / max((double)g, 1e-10)) == gx / g in float: double rounding is innocuous for
-        // division when the wide format has >= 2p+2 bits (53 >= 50).
-        const float ux = __fdiv_rn(gx, g);
-        const float uy = __fdiv_rn(gy, g);
-        float best = 0.f;
-        for (int k = 0; k < t.K; ++k) {
-            float s = __fadd_rn(__fmul_rn(ux, t.ox[k]), __fmul_rn(uy, t.oy[k]));
-            int b = k;
-            if (s < 0.f) { s = -s; b += t.K; }
-            if (s > best) { best = s; bin = b; }   // strict >, ascending k
-        }
+    if (g2 == 0) return -1;
+    const float fx = (float)gx, fy = (float)gy;
+    float m1 = 0.f, m2 = 0.f;            // largest and second largest |t_k| (a tie leaves m1 == m2: no margin)
+    int best = 0;
+    bool neg = false;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        const float t = fmaf(fx, a.ox[k], fy * a.oy[k]);
+        const float m = fabsf(t);
+        if (m > m1) { m2 = m1; m1 = m; best = k; neg = t < 0.f; }
+        else if (m > m2) m2 = m;
     }
-    lut[idx] = (int8_t)bin;
+    const float d = m1 - m2;
+    if (d * d > kBinMargin2 * (float)g2) return neg ? best + K : best;
+    // the gx = 0 axis is a bin boundary for odd K and common in real patches; the reference's unit vector there is exactly
+    // (0, +-1), so its bin is a function of K and the sign of gy alone (launch_hog)
+    if (gx == 0) return a.vbin[gy < 0];
+    return hog_bin_reference(a, K, fx, fy, g);
 }
 
 // shared-memory carve-up (same function on host and device)
@@ -230,7 +243,7 @@ __host__ __device__ constexpr int hog_tma_box(int c) { return c == 0 ? 32 : c ==
 struct HogMaps { CUtensorMap m[kTmaClasses]; };
 
 template <int KT, int NCT, int CST>
-__global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const HogArgs a, const __grid_constant__ HogMaps maps)
+__global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const __grid_constant__ HogArgs a, const __grid_constant__ HogMaps maps)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     const int K = KT > 0 ? KT : a.K;
@@ -467,34 +480,21 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const HogArgs a,
     }
     __syncthreads();
 
-    // ---- S2: gradient + orientation arg-max per interior pixel (hog.c:631-672): arg-max and modulus come from the
-    //      device-generated tables (the gradient of an 8-bit patch is a pair of integers in [-255, 255]) ---------
+    // ---- S2: gradient + orientation arg-max per interior pixel (hog.c:631-672), in registers: the gradient of an 8-bit
+    //      patch is a pair of integers in [-255, 255], its squared modulus an exact float integer whose correctly rounded
+    //      root is the reference's sqrtf, and hog_bin decides the reference's arg-max -----------------------------------
     {
-        // linear index over the interior pixels (all lanes busy); four pixels per thread in flight so that the eight table
-        // look-ups overlap (the phase is bound by their latency)
+        // linear index over the interior pixels (all lanes busy)
         const int iw = fs - 2, npix = iw * iw;
-        for (int i0 = tid; i0 < npix; i0 += 4 * kHogThreads) {
-            int idx[4], gxs[4], gys[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const int i = i0 + k * kHogThreads;
-                const int y = i / iw, x = i - y * iw;
-                idx[k] = (y + 1) * fs + (x + 1);
-                if (i < npix) {
-                    gxs[k] = (int)s_patch[idx[k] + 1] - (int)s_patch[idx[k] - 1];
-                    gys[k] = (int)s_patch[idx[k] + fs] - (int)s_patch[idx[k] - fs];
-                } else { gxs[k] = 0; gys[k] = 0; }
-            }
-            int8_t bn[4];
-            float mg[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                bn[k] = __ldg(a.lut + (gys[k] + 255) * kLutDim + (gxs[k] + 255));
-                mg[k] = __ldg(a.mag_lut + (gxs[k] * gxs[k] + gys[k] * gys[k]));
-            }
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                if (i0 + k * kHogThreads < npix) { s_bin[idx[k]] = bn[k]; s_gmag[idx[k]] = mg[k]; }
+        for (int i = tid; i < npix; i += kHogThreads) {
+            const int y = i / iw, x = i - y * iw;
+            const int idx = (y + 1) * fs + (x + 1);
+            const int gx = (int)s_patch[idx + 1] - (int)s_patch[idx - 1];
+            const int gy = (int)s_patch[idx + fs] - (int)s_patch[idx - fs];
+            const int g2 = gx * gx + gy * gy;
+            const float g = __fsqrt_rn((float)g2);
+            s_bin[idx] = (int8_t)hog_bin(a, K, gx, gy, g2, g);
+            s_gmag[idx] = g;
         }
     }
     if (a.bins) {
@@ -696,32 +696,22 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
     a.geometry = d_geometry; a.patches = d_patches; a.bins = d_bins;
     a.status = reinterpret_cast<int*>(ctx->d_scratch) + 1;   // the projection's own status word: bit 0 empty patch, bit 1 bad image index
 
-    // orientation table for this K, built once per context (hog.c:195-204: host libm cos/sin, as the reference)
-    if (!ctx->hog_lut[a.K]) {
-        LutArgs t;
-        t.K = a.K;
-        for (int k = 0; k < SD_MAX_BINS; ++k) { t.ox[k] = 0.f; t.oy[k] = 0.f; }
-        for (int k = 0; k < a.K; ++k) {
-            const double angle = k * 3.141592653589793 / a.K;
-            t.ox[k] = (float)cos(angle);
-            t.oy[k] = (float)sin(angle);
-        }
-        void* lut = nullptr;
-        SD_CUDA(ctx, cudaMalloc(&lut, (size_t)kLutDim * kLutDim));
-        hog_lut_kernel<<<sd_div_up(kLutDim * kLutDim, 256), 256, 0, ctx->stream>>>(t, (int8_t*)lut);
-        SD_LAUNCH_CHECK(ctx, "hog_lut_kernel");
-        ctx->hog_lut[a.K] = lut;
+    // orientation directions (hog.c:195-204: host libm cos/sin, as the reference)
+    for (int k = 0; k < SD_MAX_BINS; ++k) { a.ox[k] = 0.f; a.oy[k] = 0.f; }
+    for (int k = 0; k < a.K; ++k) {
+        const double angle = k * 3.141592653589793 / a.K;
+        a.ox[k] = (float)cos(angle);
+        a.oy[k] = (float)sin(angle);
     }
-    a.lut = (const int8_t*)ctx->hog_lut[a.K];
-    if (!ctx->hog_lut[0]) {              // slot 0 (K >= 1 always): modulus table, shared by every K
-        const int n = 2 * 255 * 255 + 1;
-        void* lut = nullptr;
-        SD_CUDA(ctx, cudaMalloc(&lut, (size_t)n * sizeof(float)));
-        hog_maglut_kernel<<<sd_div_up(n, 256), 256, 0, ctx->stream>>>((float*)lut, n);
-        SD_LAUNCH_CHECK(ctx, "hog_maglut_kernel");
-        ctx->hog_lut[0] = lut;
+    // hog.c:645-672 at gx = 0: ux = +0 and uy = +-1 exactly (the root of gy^2 is exact), so s_k = +-oy_k exactly; the first
+    // strict maximum of oy_k > 0 wins, in the lower half-plane when gy < 0 (K = 1: no k has oy_k > 0, bin -1)
+    {
+        float best = 0.f;
+        int bin = -1;
+        for (int k = 0; k < a.K; ++k) if (a.oy[k] > best) { best = a.oy[k]; bin = k; }
+        a.vbin[0] = bin;
+        a.vbin[1] = bin < 0 ? -1 : bin + a.K;
     }
-    a.mag_lut = (const float*)ctx->hog_lut[0];
 
     // per-sample tables (half size, cv::resize taps) and the per-launch spatial binning table
     const size_t geom_bytes = (size_t)N * sizeof(int) + (size_t)N * 5 * fs * sizeof(int) + (size_t)(a.nc * fs + 2 * a.nc) * sizeof(float);
@@ -775,8 +765,8 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
 #undef SD_HOG_PICK
     }
     SD_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
-    // The default shared-memory carve-out is kept on purpose: the orientation / modulus tables live in L1, which a larger
-    // carve-out (more resident CTAs per SM) would take away.
+    // Default shared-memory carve-out: the maximum one ran the four detect levels no faster (5.84 ms both, 4096 faces, one
+    // H100 80GB HBM3 at a 400 W power limit), since registers, not shared memory, bound the CTAs per SM at fs = 55 / 50 / 40.
     kern<<<(unsigned)blocks, kHogThreads, lay.total, ctx->stream>>>(a, maps);
     SD_LAUNCH_CHECK(ctx, "hog_patch_kernel");
     return SD_OK;

@@ -58,7 +58,6 @@ struct sd_ctx {
     int64_t gathered_bytes = 0;    // host-frame bytes sd_train_level / sd_apply_level read over PCIe
     float timings[4] = {0, 0, 0, 0};
     cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    void* hog_lut[SD_MAX_BINS + 1] = {};   // per K: (gx,gy) -> orientation bin table (sd_hog.cu)
     void* ws[SD_WS_COUNT] = {};
     size_t ws_bytes[SD_WS_COUNT] = {};
     // pinned scratch for small device->host results (lambda, residual, status flags)
