@@ -275,78 +275,153 @@ __global__ void __launch_bounds__(256) gemm_nn_kernel(const float* __restrict__ 
 }
 
 
-// ---- skinny-output GEMM of the cascade (LinearRegressor::predict, regressors.hpp:377-381: values * x with 2L output columns) ----
-// One THREAD per sample row: it streams its own feature row from HBM (128-bit loads, each 128-byte line is consumed by the
-// same thread over 8 loads) and keeps up to 48 output columns in registers; the weight chunk [32 x 48] sits in shared memory
-// and every read of it is a broadcast (all lanes the same address: one wavefront), so the inner loop is FFMA-bound: 48 FFMA
-// per 12 LDS.128 + 0.25 LDG.128.  (The 64 x 64 smem-tiled kernel below spends its time on shared-memory traffic when only 44
-// of its 64 tile columns exist.)  Split over D across blockIdx.y; products are summed in fp32 inside a 32-deep chunk and the
-// chunk sums in double -- cv::gemm accumulates float products in double -- then gemm_finalize_kernel adds the splits in a
-// fixed order.  blockIdx.z walks column groups of 48 (2L = 136 for the 68-point model).
-constexpr int PR_ROWS = 256, PR_KC = 32, PR_COLS = 48;
-
-__global__ void __launch_bounds__(PR_ROWS, 1) predict_rows_kernel(const float* __restrict__ A, long long lda, int N, int D,
-                                                                  const float* __restrict__ X, long long ldb, int M,
-                                                                  double* __restrict__ partial, int k_per_split)
+// cp.async staging.  A source-size below the copy size zero-fills the rest of the destination; at source-size 0 the source
+// pointer is only required to be mapped.
+__device__ __forceinline__ void cp_async16_part(float* dst_smem, const float* src, int bytes)
 {
-    __shared__ __align__(16) float Xs[PR_KC][PR_COLS];
-    const int tid = threadIdx.x;
-    const int row = blockIdx.x * PR_ROWS + tid;
-    const int c0 = blockIdx.z * PR_COLS;
+    const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst_smem);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async16(float* dst_smem, const float* src, bool valid)
+{
+    cp_async16_part(dst_smem, src, valid ? 16 : 0);
+}
+__device__ __forceinline__ void cp_async4(float* dst_smem, const float* src, bool valid)
+{
+    const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst_smem);
+    const int n = valid ? 4 : 0;
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(d), "l"(src), "r"(n) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit()
+{
+    asm volatile("cp.async.commit_group;" ::: "memory");
+}
+template <int PENDING>
+__device__ __forceinline__ void cp_async_wait()
+{
+    asm volatile("cp.async.wait_group %0;" ::"n"(PENDING) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all()
+{
+    asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
+}
+
+// ---- skinny-output GEMM of the cascade (LinearRegressor::predict, regressors.hpp:377-381: values * x with 2L output columns) ----
+// A CTA computes 256 sample rows x one group of 48 output columns over its split of D, in 32-deep chunks.  Thread mapping:
+// warp w owns the 12 columns 12 (w % 4) .. + 11 of the group and the rows 128 (w / 4) + lane + 32 r, r = 0..3, and keeps
+// those 4 x 12 sums in registers.  Per k step a thread reads its 4 feature values (one LDS.128 of a row covers 4 k steps,
+// and 8 lanes' rows 144 B apart hit distinct banks) and 12 weights (3 warp-uniform LDS.128 broadcasts), for 48 FFMA.  A
+// broadcast still moves 16 B to each of 32 lanes through the SM's shared-memory data path; one row x 48 columns per thread
+// needed 12 of them per 48 FFMA, and that path, not the FFMA pipes, set the pace (DESIGN 4.4).  Each chunk of A [256 x 32]
+// and of the weights [32 x 48] is copied to shared memory with cp.async, PR_STAGES - 1 chunks ahead of the one being
+// multiplied, so that at one CTA per SM a chunk's HBM latency overlaps the FFMA work of the chunks before it.
+// Arithmetic: products are summed in fp32 (fmaf, ascending k) inside a 32-deep chunk aligned to a global multiple of 32, and
+// the chunk sums in double in ascending chunk order -- cv::gemm accumulates float products in double -- then
+// gemm_finalize_kernel adds the splits (blockIdx.y, along D) in a fixed order.  blockIdx.z walks column groups of 48
+// (2L = 136 for the 68-point model).
+constexpr int PR_ROWS = 256, PR_KC = 32, PR_COLS = 48;
+constexpr int PR_TR = 4, PR_TC = 12;                                   // rows x columns of one thread
+constexpr int PR_THREADS = PR_ROWS * PR_COLS / (PR_TR * PR_TC);
+constexpr int PR_ALD = PR_KC + 4;                                      // pitch of a staged A row (floats)
+constexpr int PR_STAGES = 3;
+constexpr int PR_SMEM = PR_STAGES * (PR_ROWS * PR_ALD + PR_KC * PR_COLS) * (int)sizeof(float);
+static_assert(PR_THREADS == 256 && PR_ROWS == (PR_THREADS / 32) / (PR_COLS / PR_TC) * 32 * PR_TR, "warp tiling");
+
+__global__ void __launch_bounds__(PR_THREADS, 1) predict_rows_kernel(const float* __restrict__ A, long long lda, int N, int D,
+                                                                     const float* __restrict__ X, long long ldb, int M,
+                                                                     double* __restrict__ partial, int k_per_split)
+{
+    extern __shared__ __align__(16) float pr_smem[];
+    float* const As = pr_smem;                                         // [stage][row][PR_ALD]
+    float* const Xs = pr_smem + PR_STAGES * PR_ROWS * PR_ALD;          // [stage][k][PR_COLS]
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int r0 = blockIdx.x * PR_ROWS, c0 = blockIdx.z * PR_COLS;
     const int kbeg = blockIdx.y * k_per_split;
     const int kend = min(D, kbeg + k_per_split);
-    const bool live = row < N;
-    const float* __restrict__ arow = A + (long long)(live ? row : 0) * lda;
-    double dacc[PR_COLS];
+    const int chunks = (kend - kbeg + PR_KC - 1) / PR_KC;
+    const int tc = (warp % (PR_COLS / PR_TC)) * PR_TC;                 // first column of this thread in the group
+    const int tr = (warp / (PR_COLS / PR_TC)) * 32 * PR_TR + lane;     // first row of this thread in the block
+
+    // A's rows beyond N and features at or beyond kend are zero-filled, and so are the weights beyond kend or M
+    auto stage_chunk = [&](int chunk) {
+        const int k0 = kbeg + chunk * PR_KC, s = chunk % PR_STAGES;
+        float* as = As + s * PR_ROWS * PR_ALD;
 #pragma unroll
-    for (int c = 0; c < PR_COLS; ++c) dacc[c] = 0.0;
-    for (int k0 = kbeg; k0 < kend; k0 += PR_KC) {
-        // this thread's 32 feature values of the chunk (columns at or beyond kend may hold anything: masked to zero)
-        float4 av[PR_KC / 4];
-#pragma unroll
-        for (int q = 0; q < PR_KC / 4; ++q) {
+        for (int j = 0; j < PR_ROWS * PR_KC / 4 / PR_THREADS; ++j) {
+            const int i = tid + j * PR_THREADS;
+            const int r = i / (PR_KC / 4), q = i % (PR_KC / 4);
             const int k = k0 + 4 * q;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (live && k < kend) {
-                v = __ldg(reinterpret_cast<const float4*>(arow + k));       // lda and kbeg are multiples of 4, the base is 16-byte aligned
-                if (k + 1 >= kend) v.y = 0.f;
-                if (k + 2 >= kend) v.z = 0.f;
-                if (k + 3 >= kend) v.w = 0.f;
-            }
-            av[q] = v;
+            const int bytes = r0 + r < N ? 4 * max(0, min(4, kend - k)) : 0;
+            // lda and kbeg are multiples of 4 and A is 16-byte aligned
+            cp_async16_part(as + r * PR_ALD + 4 * q, bytes ? A + (long long)(r0 + r) * lda + k : A, bytes);
         }
-        __syncthreads();                                                    // the previous chunk's weights are no longer read
-        for (int i = tid; i < PR_KC * PR_COLS; i += PR_ROWS) {
-            const int kk = i / PR_COLS, c = i - kk * PR_COLS;
-            const int k = k0 + kk;
-            Xs[kk][c] = (k < kend && c0 + c < M) ? __ldg(X + (long long)k * ldb + c0 + c) : 0.f;
-        }
-        __syncthreads();
-        float acc[PR_COLS];
+        float* xs = Xs + s * PR_KC * PR_COLS;
 #pragma unroll
-        for (int c = 0; c < PR_COLS; ++c) acc[c] = 0.f;
+        for (int j = 0; j < PR_KC * PR_COLS / PR_THREADS; ++j) {
+            const int i = tid + j * PR_THREADS;
+            const int kk = i / PR_COLS, c = i % PR_COLS;
+            const bool valid = k0 + kk < kend && c0 + c < M;
+            cp_async4(xs + i, valid ? X + (long long)(k0 + kk) * ldb + c0 + c : X, valid);
+        }
+    };
+
+    double dacc[PR_TR][PR_TC];
+#pragma unroll
+    for (int r = 0; r < PR_TR; ++r)
+#pragma unroll
+        for (int c = 0; c < PR_TC; ++c) dacc[r][c] = 0.0;
+#pragma unroll
+    for (int s = 0; s < PR_STAGES - 1; ++s) {
+        if (s < chunks) stage_chunk(s);
+        cp_async_commit();                                             // one group per chunk, empty ones included
+    }
+    for (int ch = 0; ch < chunks; ++ch) {
+        cp_async_wait<PR_STAGES - 2>();                                // this thread's copies of chunk ch have landed
+        __syncthreads();                                               // everyone's have, and chunk ch - 1's stage is free
+        if (ch + PR_STAGES - 1 < chunks) stage_chunk(ch + PR_STAGES - 1);
+        cp_async_commit();
+        const float* as = As + (ch % PR_STAGES) * PR_ROWS * PR_ALD + tr * PR_ALD;
+        const float* xs = Xs + (ch % PR_STAGES) * PR_KC * PR_COLS + tc;
+        float acc[PR_TR][PR_TC];
+#pragma unroll
+        for (int r = 0; r < PR_TR; ++r)
+#pragma unroll
+            for (int c = 0; c < PR_TC; ++c) acc[r][c] = 0.f;
 #pragma unroll
         for (int q = 0; q < PR_KC / 4; ++q) {
-            const float a4[4] = {av[q].x, av[q].y, av[q].z, av[q].w};
+            float a[PR_TR][4];
+#pragma unroll
+            for (int r = 0; r < PR_TR; ++r) {
+                const float4 v = *reinterpret_cast<const float4*>(as + r * 32 * PR_ALD + 4 * q);
+                a[r][0] = v.x; a[r][1] = v.y; a[r][2] = v.z; a[r][3] = v.w;
+            }
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const float a = a4[e];
+                float w[PR_TC];
 #pragma unroll
-                for (int c = 0; c < PR_COLS; c += 4) {
-                    const float4 w = *reinterpret_cast<const float4*>(&Xs[4 * q + e][c]);
-                    acc[c] = fmaf(a, w.x, acc[c]); acc[c + 1] = fmaf(a, w.y, acc[c + 1]);
-                    acc[c + 2] = fmaf(a, w.z, acc[c + 2]); acc[c + 3] = fmaf(a, w.w, acc[c + 3]);
+                for (int c = 0; c < PR_TC; c += 4) {
+                    const float4 v = *reinterpret_cast<const float4*>(xs + (4 * q + e) * PR_COLS + c);
+                    w[c] = v.x; w[c + 1] = v.y; w[c + 2] = v.z; w[c + 3] = v.w;
                 }
+#pragma unroll
+                for (int r = 0; r < PR_TR; ++r)
+#pragma unroll
+                    for (int c = 0; c < PR_TC; ++c) acc[r][c] = fmaf(a[r][e], w[c], acc[r][c]);
             }
         }
 #pragma unroll
-        for (int c = 0; c < PR_COLS; ++c) dacc[c] += (double)acc[c];
-    }
-    if (live) {
-        double* out = partial + ((long long)blockIdx.y * N + row) * M + c0;
+        for (int r = 0; r < PR_TR; ++r)
 #pragma unroll
-        for (int c = 0; c < PR_COLS; ++c)
-            if (c0 + c < M) out[c] = dacc[c];
+            for (int c = 0; c < PR_TC; ++c) dacc[r][c] += (double)acc[r][c];
+    }
+#pragma unroll
+    for (int r = 0; r < PR_TR; ++r) {
+        const int row = r0 + tr + 32 * r;
+        if (row >= N) continue;
+        double* out = partial + ((long long)blockIdx.y * N + row) * M + c0 + tc;
+#pragma unroll
+        for (int c = 0; c < PR_TC; ++c)
+            if (c0 + tc + c < M) out[c] = dacc[r][c];
     }
 }
 
@@ -377,8 +452,10 @@ int launch_gemm_nn(sd_ctx* ctx, const float* A, int64_t lda, int N, int D, const
     // chunk boundaries are global multiples of 32, so a row's result does not depend on the batch it is computed in
     if (D >= 1024 && M <= 4 * PR_COLS && (lda % 4) == 0 && (reinterpret_cast<uintptr_t>(A) & 15) == 0) {
         const int row_blocks = sd_div_up(N, PR_ROWS), col_groups = sd_div_up(M, PR_COLS);
-        int splits = (int)(2LL * ctx->sm_count / ((long long)row_blocks * col_groups));     // two CTAs' worth of work per SM, whole waves
-        if (N < PR_ROWS) splits = splits * N / PR_ROWS + 1;                                 // few rows: few threads per CTA are live anyway
+        const long long ctas = (long long)row_blocks * col_groups;
+        // one wave: a CTA's registers fill an SM, and every further split adds N x M doubles for gemm_finalize_kernel to read
+        int splits = (int)(ctx->sm_count / ctas);
+        if (N < PR_ROWS) splits = (int)(2LL * ctx->sm_count / ctas) * N / PR_ROWS + 1;     // few rows: few threads per CTA are live anyway
         const int maxs = sd_div_up(D, 4 * PR_KC);
         if (splits > maxs) splits = maxs;
         if (splits < 1) splits = 1;
@@ -387,7 +464,8 @@ int launch_gemm_nn(sd_ctx* ctx, const float* A, int64_t lda, int N, int D, const
         double* partial = (double*)sd_workspace(ctx, SD_WS_GEMM_PARTIAL, (size_t)splits * N * M * sizeof(double));
         if (!partial) return SD_ERR_CUDA;
         const dim3 pgrid(row_blocks, splits, col_groups);
-        predict_rows_kernel<<<pgrid, PR_ROWS, 0, ctx->stream>>>(A, lda, N, D, B, ldb, M, partial, kps);
+        SD_CUDA(ctx, cudaFuncSetAttribute(predict_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PR_SMEM));
+        predict_rows_kernel<<<pgrid, PR_THREADS, PR_SMEM, ctx->stream>>>(A, lda, N, D, B, ldb, M, partial, kps);
         SD_LAUNCH_CHECK(ctx, "predict_rows_kernel");
         dim3 fblock(32, 8);
         gemm_finalize_kernel<<<sd_div_up(N, 8), fblock, 0, ctx->stream>>>(partial, splits, N, M, C, ldc, ep);
@@ -806,26 +884,6 @@ __global__ void copy_block_kernel(const float* __restrict__ src, long long lds, 
 // U (in place in G), W = U^-1 and W^T (workspace) -- so that the panel solve U12 = U11^-T G12 and the back
 // substitution X_j = U_jj^-1 Y_j become plain GEMMs.  Blocks narrower than 128 are padded with the identity.
 constexpr int PB = 128, PS = 32, PLD = PB + 1;
-
-// cp.async staging: all of a CTA's global->shared copies are put in flight at once (the block kernels of the
-// factorisation are latency-bound, so copies must not be issued one load/store loop iteration at a time).
-// valid == false zero-fills the destination (src-size 0; the source pointer is then only required to be mapped).
-__device__ __forceinline__ void cp_async16(float* dst_smem, const float* src, bool valid)
-{
-    const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst_smem);
-    const int n = valid ? 16 : 0;
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(src), "r"(n) : "memory");
-}
-__device__ __forceinline__ void cp_async4(float* dst_smem, const float* src, bool valid)
-{
-    const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst_smem);
-    const int n = valid ? 4 : 0;
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(d), "l"(src), "r"(n) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all()
-{
-    asm volatile("cp.async.commit_group;\n\tcp.async.wait_group 0;" ::: "memory");
-}
 
 // Factor and invert the 32 x 32 diagonal sub-block at (k0, k0) of sA, by the whole CTA rather than a single warp (the
 // single-warp variants leave most of the SM idle on a chain of dependent pivots).
