@@ -198,6 +198,27 @@ SD_API int sd_bgr2gray(sd_ctx* ctx, const uint8_t* d_bgr, int width, int height,
  * SD_ERR_INVALID before any work is queued (d_buf is not written). */
 SD_API int sd_upload_frames(sd_ctx* ctx, const sd_host_frame* frames, int count, void* d_buf, size_t* bytes, sd_image_batch* out);
 
+/* ---- dense HOG of whole frames: vl_hog_put_image (one channel) + vl_hog_extract (hog.c:595-728, :857-1062) -------------
+ * The general HOG API the reference ships (hog.h:104-139) on every 8-bit grey frame of a batch, e.g. the input of a
+ * sliding-window detector.  Output per frame: VLFeat's planar layout [dd][hogH][hogW], x fastest, with
+ *   hogW = (width + cell_size / 2) / cell_size, hogH = (height + cell_size / 2) / cell_size     (hog.c:542-543)
+ *   dd   = 3 * num_bins + 4 (variant 1, UoCTTI) or 4 * num_bins (variant 0, Dalal-Triggs).
+ * Valid arguments: width and height > 3 with hogW, hogH > 0 (hog.c:545-548), num_bins in [1, 16], cell_size in [1, 32],
+ * variant 0 or 1.  Orientations are assigned to the nearest bin (no bilinear orientation assignment), as rcr::HogTransform
+ * uses vl_hog.  Features agree with hog.c to ~1e-7 relative (the votes of a cell are summed in a different, fixed order); a
+ * frame of num_cells * cell_size pixels square gives bit for bit the features sd_hog_batch computes for the same fixed patch.
+ *
+ * sd_hog_dense_shape: host only.  Writes hogW, hogH and dd, or returns SD_ERR_INVALID for an invalid configuration. */
+SD_API int sd_hog_dense_shape(int width, int height, int cell_size, int num_bins, int variant, int* hog_w, int* hog_h, int* dd);
+/* sd_hog_dense: asynchronous on the context's stream.  Frame i's features start at d_out + d_out_offset[i] (offsets in floats,
+ * a device array of images->count int64), or, with d_out_offset == NULL (allowed only when all frames have one size), at
+ * d_out + i * dd * hogH * hogW.  Frames of different sizes (images->d_frames) need the offsets, computed with
+ * sd_hog_dense_shape; the call then reads the frame table back once before it queues work.  Each frame's features depend on
+ * that frame alone: the same in any batch, and the same in every run.  A batch with d_roi, an invalid configuration, or a
+ * frame that breaks the size rule is SD_ERR_INVALID before any work is queued (d_out is not written). */
+SD_API int sd_hog_dense(sd_ctx* ctx, const sd_image_batch* images, int cell_size, int num_bins, int variant, float* d_out,
+                        const int64_t* d_out_offset);
+
 /* ---- regressor: LinearRegressor<Solver> (regressors.hpp:318-400) ------------------------ */
 /* Solver::solve (regressors.hpp:199-234 == verbose_solver.hpp:53-111):
  *   X = (A^T A + Lambda)^-1 A^T B ;  A: N x D, B: N x M, X: D x M (ldx_out = M).

@@ -375,6 +375,80 @@ def _upload_host_frames(recs, ctx: Context):
     return buf, ib
 
 
+# ------------------------------------------------------------------------------------------------
+# dense HOG of whole frames: vl_hog_put_image + vl_hog_extract (hog.h:104-139)
+# ------------------------------------------------------------------------------------------------
+def hog_dense_shape(width: int, height: int, cell_size: int, num_bins: int, variant: int = 1):
+    """(dd, hogH, hogW) of the dense HOG of a width x height frame (hog.c:542-548); SdError for an invalid configuration."""
+    w, h, d = C.c_int(), C.c_int(), C.c_int()
+    rc = _capi.lib().sd_hog_dense_shape(int(width), int(height), int(cell_size), int(num_bins), int(variant), C.byref(w), C.byref(h),
+                                        C.byref(d))
+    if rc:
+        raise SdError(rc, f"invalid dense HOG configuration: {width} x {height} px, cell_size {cell_size}, num_bins {num_bins}, "
+                          f"variant {variant} (frames > 3 px and at least half a cell, cell_size 1..32, num_bins 1..16)")
+    return d.value, h.value, w.value
+
+
+def hog_dense(frames, cell_size: int, num_bins: int, variant: int = 1, ctx: Optional[Context] = None):
+    """VLFeat HOG of whole 8-bit frames (vl_hog_new(variant, num_bins) + vl_hog_put_image(frame, 1 channel, cell_size) +
+    vl_hog_extract) on the device, in VLFeat's planar layout [dd][hogH][hogW] with x fastest.
+
+    frames: a CUDA uint8 tensor (count, H, W), used in place; or host frames -- a (count, H, W) or (count, H, W, 3) uint8 array,
+    or a list of (H, W) / (H, W, 3) uint8 frames of any sizes -- uploaded by sd_upload_frames (B,G,R colour converted to grey
+    there, as HogTransform does).  variant: 1 = UoCTTI (dd = 3K + 4), 0 = Dalal-Triggs (dd = 4K).
+    Returns one (count, dd, hogH, hogW) float32 CUDA tensor when all frames have one size, else a list of (dd, hogH, hogW)
+    tensors."""
+    ctx = ctx or default_context()
+    lib = _capi.lib()
+    keep = None
+    if isinstance(frames, torch.Tensor) and frames.is_cuda:
+        if frames.dtype != torch.uint8 or frames.dim() != 3:
+            raise ValueError("a device tensor of frames must be (count, H, W) uint8")
+        t = frames.to(f"cuda:{ctx.device}")
+        if t.stride(2) != 1:
+            t = t.contiguous()
+        n, h, w = t.shape
+        keep, ib = t, ImageBatchC(C.c_void_p(t.data_ptr()), w, h, t.stride(1), t.stride(0), n)
+        sizes = [(h, w)] * n
+    else:
+        if isinstance(frames, (list, tuple)):
+            frames = list(frames)
+        else:
+            a = frames.numpy() if isinstance(frames, torch.Tensor) else np.asarray(frames)
+            if a.dtype != np.uint8 or not (a.ndim == 3 or (a.ndim == 4 and a.shape[3] == 3)):
+                raise ValueError("frames must be (count, H, W) uint8, (count, H, W, 3) uint8, or a list of such frames of any sizes")
+            frames = list(a)
+        recs, arrays = [], []
+        for f in frames:
+            rec, a = _host_frame(f)
+            if a.ndim == 3 and a.shape[2] != 3:
+                raise ValueError("every frame must be (H, W) uint8 or (H, W, 3) uint8")
+            recs.append(rec)
+            arrays.append(a)                                  # the bytes stay alive until the upload returns
+        sizes = [(r.height, r.width) for r in recs]
+        if not recs:
+            return []
+        for h, w in set(sizes):
+            hog_dense_shape(w, h, cell_size, num_bins, variant)   # refuse before the upload
+        keep, ib = _upload_host_frames(recs, ctx)
+    n = len(sizes)
+    dev = f"cuda:{ctx.device}"
+    if n == 0:
+        return torch.empty((0,) + hog_dense_shape(keep.shape[2], keep.shape[1], cell_size, num_bins, variant), dtype=torch.float32,
+                           device=dev)
+    shapes = [hog_dense_shape(w, h, cell_size, num_bins, variant) for h, w in sizes]
+    if len(set(shapes)) == 1:
+        out = torch.empty((n,) + shapes[0], dtype=torch.float32, device=dev)
+        _check(ctx.h, lib.sd_hog_dense(ctx.h, C.byref(ib), int(cell_size), int(num_bins), int(variant), ptr(out), None))
+        return out
+    counts = [d * h * w for d, h, w in shapes]
+    starts = np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.int64)
+    offsets = torch.from_numpy(starts).to(dev)
+    out = torch.empty(int(sum(counts)), dtype=torch.float32, device=dev)
+    _check(ctx.h, lib.sd_hog_dense(ctx.h, C.byref(ib), int(cell_size), int(num_bins), int(variant), ptr(out), ptr(offsets)))
+    return [out[s:s + c].view(shape) for s, c, shape in zip(starts.tolist(), counts, shapes)]
+
+
 # The distinct frames of a HogTransform are uploaded when their grey bytes fit in this share of the device's free memory (read when
 # the transform is first used); otherwise they stay in host memory and train() / test() gather them per level.
 DEVICE_FRAME_SHARE = 0.5

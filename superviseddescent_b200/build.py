@@ -20,7 +20,7 @@ LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libsd_b200.so")
 
-SOURCES = ["sd_api.cu", "sd_hog.cu", "sd_linalg.cu", "sd_gram_tc.cu", "sd_model.cu", "sd_comm.cu", "sd_rank.cu", "sd_cg.cu", "sd_train.cu"]
+SOURCES = ["sd_api.cu", "sd_hog.cu", "sd_hog_dense.cu", "sd_linalg.cu", "sd_gram_tc.cu", "sd_model.cu", "sd_comm.cu", "sd_rank.cu", "sd_cg.cu", "sd_train.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo",
          "-Xcompiler", "-fPIC,-fvisibility=hidden", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
@@ -36,7 +36,7 @@ def _stale(target: str, deps) -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(LIBDIR, exist_ok=True)
     os.makedirs(OBJDIR, exist_ok=True)
-    headers = [os.path.join(CSRC, "sd_internal.cuh"), os.path.join(ROOT, "include", "sd_b200.h")]
+    headers = [os.path.join(CSRC, "sd_internal.cuh"), os.path.join(CSRC, "sd_hog_common.cuh"), os.path.join(ROOT, "include", "sd_b200.h")]
     jobs = []
     objs = []
     for src in SOURCES:

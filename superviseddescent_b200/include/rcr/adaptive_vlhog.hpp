@@ -204,4 +204,41 @@ private:
     std::shared_ptr<DeviceImages> dev;   // shared between the copies the optimiser makes of this functor
 };
 
+// VLFeat HOG of whole frames (hog.h:104-139: vl_hog_new(variant, num_bins), vl_hog_put_image(frame, 1 channel, cell_size),
+// vl_hog_extract), for frames of any sizes, 8UC1 or 8UC3 (B,G,R, converted to grey as HogTransform does), in one batched call
+// on the device (sd_hog_dense).  Returns one CV_32FC1 Mat per frame with dd * hogH rows and hogW columns: VLFeat's planar
+// [dd][hogH][hogW] order, so row d * hogH + y holds dimension d of cell row y.  Throws std::runtime_error for a frame or a
+// configuration that sd_hog_dense_shape refuses.
+inline std::vector<cv::Mat> hog_dense(const std::vector<cv::Mat>& images, VlHogVariant variant, int cell_size, int num_bins)
+{
+    std::vector<cv::Mat> out;
+    if (images.empty()) return out;
+    sd_ctx* ctx = sd_b200::context();
+    const std::vector<sd_host_frame> frames = sd_b200::host_frames(images);
+    const int n = static_cast<int>(frames.size());
+    std::vector<int64_t> offset(n);
+    std::vector<int> rows(n), cols(n);
+    int64_t total = 0;
+    for (int i = 0; i < n; ++i) {
+        int w = 0, h = 0, dd = 0;
+        if (sd_hog_dense_shape(frames[i].width, frames[i].height, cell_size, num_bins, variant, &w, &h, &dd) != SD_OK)
+            throw std::runtime_error("hog_dense: frame " + std::to_string(i) + " (" + std::to_string(frames[i].width) + " x " +
+                                     std::to_string(frames[i].height) + ") or the configuration is invalid: frames wider and taller "
+                                     "than 3 px and at least half a cell, cell_size 1..32, num_bins 1..16");
+        offset[i] = total;
+        rows[i] = dd * h;
+        cols[i] = w;
+        total += static_cast<int64_t>(dd) * h * w;
+    }
+    size_t bytes = 0;
+    sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, nullptr, &bytes, nullptr), "hog_dense upload");
+    sd_b200::DeviceBuffer buf(bytes), d_out(static_cast<size_t>(total) * sizeof(float)), d_offset(static_cast<size_t>(n) * sizeof(int64_t));
+    sd_image_batch batch{};
+    sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, buf.as<void>(), &bytes, &batch), "hog_dense upload");
+    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_offset.as<int64_t>(), offset.data(), static_cast<size_t>(n) * sizeof(int64_t)), "hog_dense");
+    sd_b200::check(ctx, sd_hog_dense(ctx, &batch, cell_size, num_bins, variant, d_out.as<float>(), d_offset.as<int64_t>()), "sd_hog_dense");
+    for (int i = 0; i < n; ++i) out.push_back(sd_b200::download(d_out.as<float>() + offset[i], rows[i], cols[i], cols[i]));
+    return out;
+}
+
 }  // namespace rcr
