@@ -205,7 +205,7 @@ SD_API int sd_upload_frames(sd_ctx* ctx, const sd_host_frame* frames, int count,
  *   dd   = 3 * num_bins + 4 (variant 1, UoCTTI) or 4 * num_bins (variant 0, Dalal-Triggs).
  * Valid arguments: width and height > 3 with hogW, hogH > 0 (hog.c:545-548), num_bins in [1, 16], cell_size in [1, 32],
  * variant 0 or 1.  Orientations are assigned to the nearest bin (no bilinear orientation assignment), as rcr::HogTransform
- * uses vl_hog.  Features agree with hog.c to ~1e-7 relative (the votes of a cell are summed in a different, fixed order); a
+ * uses vl_hog; sd_hog_dense_images below adds float and multi-channel frames and bilinear assignment.  Features agree with hog.c to ~1e-7 relative (the votes of a cell are summed in a different, fixed order); a
  * frame of num_cells * cell_size pixels square gives bit for bit the features sd_hog_batch computes for the same fixed patch.
  *
  * sd_hog_dense_shape: host only.  Writes hogW, hogH and dd, or returns SD_ERR_INVALID for an invalid configuration. */
@@ -218,6 +218,39 @@ SD_API int sd_hog_dense_shape(int width, int height, int cell_size, int num_bins
  * frame that breaks the size rule is SD_ERR_INVALID before any work is queued (d_out is not written). */
 SD_API int sd_hog_dense(sd_ctx* ctx, const sd_image_batch* images, int cell_size, int num_bins, int variant, float* d_out,
                         const int64_t* d_out_offset);
+
+/* ---- dense HOG of 8-bit or float frames with 1..16 channels: every input of vl_hog_put_image (hog.c:595-728) ----------------
+ * One frame: element (x, y, c) at offset + y * row_stride + x * pixel_stride + c * channel_stride, in ELEMENTS of the batch's
+ * dtype.  VLFeat's planar layout is pixel_stride = 1, channel_stride = height * row_stride; the interleaved layout of OpenCV
+ * and numpy (H, W, C) is pixel_stride = C, channel_stride = 1.  Offset and strides are non-negative. */
+typedef struct {
+    int32_t width, height;
+    int64_t offset, row_stride, pixel_stride, channel_stride;
+} sd_hog_image;
+#define SD_HOG_U8 0
+#define SD_HOG_F32 1
+/* A batch of frames resident on the device: equally sized (frame i at frame.offset + i * image_stride elements), or --
+ * d_frames != NULL -- one device descriptor per frame (frame and image_stride are then ignored). */
+typedef struct {
+    const void* d_data;          /* SD_HOG_F32: 4-byte aligned */
+    int32_t dtype;               /* SD_HOG_U8 or SD_HOG_F32 */
+    int32_t channels;            /* 1..16, the same for every frame */
+    int32_t count;
+    sd_hog_image frame;
+    int64_t image_stride;        /* elements */
+    const sd_hog_image* d_frames;
+} sd_hog_images;
+/* sd_hog_dense_images: vl_hog_new(variant, num_bins) + vl_hog_set_use_bilinear_orientation_assignments(bilinear_orientations)
+ * + vl_hog_put_image(frame, channels, cell_size) + vl_hog_extract on every frame, asynchronous on the context's stream.  At each
+ * pixel the gradient comes from the channel with the largest squared modulus (the first on a tie; hog.c:631-644); channels are
+ * taken as given (no colour conversion).  bilinear_orientations = 1: each pixel votes into its two nearest orientation bins
+ * (hog.c:674-678), each vote weighted by the orientation weight squared, as hog.c:706-714 does.  Output, offsets, size rule
+ * and frame independence as sd_hog_dense (sd_hog_dense_shape gives the shape).  Nearest-bin features of 8-bit frames are bit
+ * for bit those of sd_hog_dense on the same pixels, and those of float frames holding the same values.  An unknown dtype,
+ * channels outside [1, 16], an unaligned float buffer, a negative offset or stride, a frame that breaks the size rule, or an
+ * invalid configuration is SD_ERR_INVALID before any work is queued (d_out is not written). */
+SD_API int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size, int num_bins, int variant,
+                               int bilinear_orientations, float* d_out, const int64_t* d_out_offset);
 
 /* ---- regressor: LinearRegressor<Solver> (regressors.hpp:318-400) ------------------------ */
 /* Solver::solve (regressors.hpp:199-234 == verbose_solver.hpp:53-111):

@@ -44,6 +44,18 @@ class FrameC(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("row_stride", C.c_int32), ("reserved", C.c_int32), ("offset", C.c_int64)]
 
 
+class HogImageC(C.Structure):
+    """sd_hog_image: one frame of sd_hog_dense_images; offset and strides in elements."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("offset", C.c_int64), ("row_stride", C.c_int64),
+                ("pixel_stride", C.c_int64), ("channel_stride", C.c_int64)]
+
+
+class HogImagesC(C.Structure):
+    """sd_hog_images: u8 or f32 frames of 1..16 channels on the device, equally sized or one descriptor per frame."""
+    _fields_ = [("d_data", C.c_void_p), ("dtype", C.c_int32), ("channels", C.c_int32), ("count", C.c_int32),
+                ("frame", HogImageC), ("image_stride", C.c_int64), ("d_frames", C.c_void_p)]
+
+
 class HostFrameC(C.Structure):
     """sd_host_frame: one host frame of a detect call (8UC1, or 8UC3 interleaved B, G, R)."""
     _fields_ = [("h_data", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32), ("row_stride", C.c_int32), ("channels", C.c_int32)]
@@ -81,6 +93,7 @@ EXPORTS = [
     "sd_malloc", "sd_free", "sd_host_alloc", "sd_host_free", "sd_memcpy_h2d", "sd_memcpy_d2h", "sd_memset",
     "sd_memcpy2d_h2d", "sd_memcpy2d_d2h", "sd_memcpy2d_d2d",
     "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_bgr2gray", "sd_upload_frames", "sd_hog_dense_shape", "sd_hog_dense",
+    "sd_hog_dense_images",
     "sd_learn", "sd_centre_features", "sd_learn_centred", "sd_learn_rank_revealing", "sd_gram", "sd_solve_gram", "sd_predict", "sd_test_residual", "sd_solver_timings", "sd_set_gram_mode", "sd_set_solver", "sd_solver_iterations",
     "sd_set_rank_diagnostic", "sd_last_rank",
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",

@@ -23,7 +23,7 @@ import torch
 
 from . import _capi
 from ._capi import HogParam as HoGParam  # same field names as rcr::HoGParam
-from ._capi import HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, ptr
+from ._capi import HogImageC, HogImagesC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, ptr
 
 
 def _check(ctx, rc: int) -> None:
@@ -446,6 +446,105 @@ def hog_dense(frames, cell_size: int, num_bins: int, variant: int = 1, ctx: Opti
     offsets = torch.from_numpy(starts).to(dev)
     out = torch.empty(int(sum(counts)), dtype=torch.float32, device=dev)
     _check(ctx.h, lib.sd_hog_dense(ctx.h, C.byref(ib), int(cell_size), int(num_bins), int(variant), ptr(out), ptr(offsets)))
+    return [out[s:s + c].view(shape) for s, c, shape in zip(starts.tolist(), counts, shapes)]
+
+
+_VL_HOG_DTYPES = {torch.uint8: 0, torch.float32: 1}    # SD_HOG_U8, SD_HOG_F32
+
+
+def _vl_hog_frame(t: torch.Tensor, channels_last: bool, batched: bool):
+    """(channels, sd_hog_image fields) of one frame, or of the first frame of a batch, read through t's strides."""
+    s = t.stride()[1:] if batched else t.stride()
+    shape = t.shape[1:] if batched else t.shape
+    if len(shape) == 2:
+        (h, w), (rs, ps), c, cst = shape, s, 1, 0
+    elif channels_last:
+        (h, w, c), (rs, ps, cst) = shape, s
+    else:
+        (c, h, w), (cst, rs, ps) = shape, s
+    return c, HogImageC(w, h, 0, rs, ps, cst)
+
+
+def vl_hog(images, cell_size: int, num_bins: int, variant: int = 1, bilinear_orientations: bool = False, channels_last: bool = False,
+           ctx: Optional[Context] = None):
+    """VLFeat HOG of whole uint8 or float32 frames of one or more channels (vl_hog_new(variant, num_bins) +
+    vl_hog_set_use_bilinear_orientation_assignments(bilinear_orientations) + vl_hog_put_image(frame, channels, cell_size) +
+    vl_hog_extract) on the device, in VLFeat's planar layout [dd][hogH][hogW] with x fastest.
+
+    images: a batch -- an array or tensor (count, H, W), (count, C, H, W), or (count, H, W, C) with channels_last=True -- or a
+    list of frames of any sizes, (H, W), (C, H, W) or (H, W, C), all of one dtype and one C.  CUDA tensors are read in place
+    through their strides; host frames are copied into one device buffer.  At each pixel the gradient comes from the channel
+    with the largest gradient; channels are used as given (for OpenCV frames channel 0 is B).  bilinear_orientations: every
+    pixel votes into its two nearest orientation bins.  variant: 1 = UoCTTI (dd = 3K + 4), 0 = Dalal-Triggs (dd = 4K).
+    Returns one (count, dd, hogH, hogW) float32 CUDA tensor when all frames have one size, else a list of (dd, hogH, hogW)
+    tensors."""
+    ctx = ctx or default_context()
+    dev = f"cuda:{ctx.device}"
+    lib = _capi.lib()
+
+    def tensor(a):
+        return a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))
+
+    def dtype_of(t):
+        if t.dtype not in _VL_HOG_DTYPES:
+            raise ValueError("frames must be uint8 or float32")
+        return _VL_HOG_DTYPES[t.dtype]
+
+    ib = HogImagesC()
+    ib.d_frames = None
+    if isinstance(images, (list, tuple)):
+        frames = [tensor(f) for f in images]
+        if not frames:
+            return []
+        if any(f.dim() not in (2, 3) for f in frames):
+            raise ValueError("every frame of a list must be (H, W), (C, H, W), or (H, W, C) with channels_last=True")
+        if len({f.dtype for f in frames}) != 1:
+            raise ValueError("all frames must have one dtype")
+        dt = dtype_of(frames[0])
+        frames = [f.contiguous() for f in frames]
+        descs = [_vl_hog_frame(f, channels_last, False) for f in frames]
+        if len({c for c, _ in descs}) != 1:
+            raise ValueError("all frames must have one number of channels")
+        sizes = [(d.height, d.width) for _, d in descs]
+        for h, w in set(sizes):
+            hog_dense_shape(w, h, cell_size, num_bins, variant)   # refuse before the upload
+        pos = 0
+        for f, (_, d) in zip(frames, descs):
+            d.offset = pos
+            pos += f.numel()
+        keep = torch.cat([f.reshape(-1) for f in frames]).to(dev)
+        ib.channels, ib.count = descs[0][0], len(frames)
+        if len(set(sizes)) == 1:
+            ib.frame, ib.image_stride = descs[0][1], frames[0].numel()
+        else:
+            table = (HogImageC * len(descs))(*[d for _, d in descs])
+            keep_table = torch.from_numpy(np.frombuffer(bytes(table), dtype=np.uint8).copy()).to(dev)
+            ib.d_frames = keep_table.data_ptr()
+    else:
+        t = tensor(images)
+        if t.dim() not in (3, 4):
+            raise ValueError("a batch of frames must be (count, H, W), (count, C, H, W), or (count, H, W, C) with channels_last=True")
+        dt = dtype_of(t)
+        keep = t.to(dev)
+        ib.channels, ib.frame = _vl_hog_frame(keep, channels_last, True)
+        ib.count, ib.image_stride = keep.shape[0], keep.stride(0)
+        sizes = [(ib.frame.height, ib.frame.width)] * ib.count
+    ib.d_data, ib.dtype = keep.data_ptr(), dt
+    n = len(sizes)
+    if n == 0:
+        return torch.empty((0,) + hog_dense_shape(ib.frame.width, ib.frame.height, cell_size, num_bins, variant), dtype=torch.float32,
+                           device=dev)
+    shapes = [hog_dense_shape(w, h, cell_size, num_bins, variant) for h, w in sizes]
+    bil = int(bool(bilinear_orientations))
+    if len(set(shapes)) == 1:
+        out = torch.empty((n,) + shapes[0], dtype=torch.float32, device=dev)
+        _check(ctx.h, lib.sd_hog_dense_images(ctx.h, C.byref(ib), int(cell_size), int(num_bins), int(variant), bil, ptr(out), None))
+        return out
+    counts = [d * h * w for d, h, w in shapes]
+    starts = np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.int64)
+    offsets = torch.from_numpy(starts).to(dev)
+    out = torch.empty(int(sum(counts)), dtype=torch.float32, device=dev)
+    _check(ctx.h, lib.sd_hog_dense_images(ctx.h, C.byref(ib), int(cell_size), int(num_bins), int(variant), bil, ptr(out), ptr(offsets)))
     return [out[s:s + c].view(shape) for s, c, shape in zip(starts.tolist(), counts, shapes)]
 
 

@@ -33,16 +33,19 @@ inline void hog_orientations(int K, float* ox, float* oy, int* vbin)
     }
 }
 
-// ---- orientation bin of a pixel with a non-zero gradient (gx, gy), the reference's float expression verbatim
-//      (hog.c:645-672): modulus, normalised gradient, then the first maximum of |<u, o_k>| in ascending k -------------
+// ---- one component of the reference's unit gradient (hog.c:645-647): (float)((double)v / max((double)g, 1e-10)).  For
+//      g > 1e-10 that is v / g in float: double rounding is innocuous for division when the wide format has >= 2p+2 bits
+//      (53 >= 50).  Below, the floor divides in double (tiny float images; g itself may come from a subnormal square).
+__device__ __forceinline__ float hog_unit(float v, float g)
+{
+    return (double)g > 1e-10 ? __fdiv_rn(v, g) : (float)__ddiv_rn((double)v, 1e-10);
+}
+
+// ---- the first maximum of |<u, o_k>| in ascending k for a unit gradient u (hog.c:656-672, nearest-bin assignment) ----
 //      Args: any kernel argument block with the members ox, oy and vbin that hog_orientations fills.
 template <class Args>
-__device__ __forceinline__ int hog_bin_reference(const Args& a, int K, float gx, float gy, float g)
+__device__ __forceinline__ int hog_bin_unit(const Args& a, int K, float ux, float uy)
 {
-    // (float)((double)gx / max((double)g, 1e-10)) == gx / g in float: double rounding is innocuous for
-    // division when the wide format has >= 2p+2 bits (53 >= 50).
-    const float ux = __fdiv_rn(gx, g);
-    const float uy = __fdiv_rn(gy, g);
     float best = 0.f;
     int bin = -1;
 #pragma unroll
@@ -53,6 +56,37 @@ __device__ __forceinline__ int hog_bin_reference(const Args& a, int K, float gx,
         if (s > best) { best = s; bin = b; }   // strict >, ascending k
     }
     return bin;
+}
+
+// ---- orientation bin of a pixel with a non-zero integer-valued gradient (gx, gy), the reference's float expression
+//      verbatim (hog.c:645-672): modulus, normalised gradient (g >= 1, so hog_unit is a float division), then the bin ------
+template <class Args>
+__device__ __forceinline__ int hog_bin_reference(const Args& a, int K, float gx, float gy, float g)
+{
+    return hog_bin_unit(a, K, __fdiv_rn(gx, g), __fdiv_rn(gy, g));
+}
+
+// ---- bilinear orientation assignment (hog.c:656-678): the reference's top-two tracking of |<u, o_k>| verbatim (a score
+//      replaces the first only when strictly larger, else the second when strictly larger), then
+//        w1 = (float)((double)acosf(min(s0, 1)) / (pi / K)),  w0 = 1 - w1.
+//      b1 = -1 when no second score is positive (K = 1 among others); b0 = -1 for a zero gradient.  pi_k is pi / K in double.
+//      acos in double rounded to float stays within an ulp of the reference's acosf. ------------------------------------
+template <class Args>
+__device__ __forceinline__ void hog_bins_bilinear(const Args& a, int K, float ux, float uy, int& b0, int& b1, float& w1)
+{
+    float s0 = 0.f, s1 = 0.f;
+    b0 = -1;
+    b1 = -1;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        float s = __fadd_rn(__fmul_rn(ux, a.ox[k]), __fmul_rn(uy, a.oy[k]));
+        int b = k;
+        if (s < 0.f) { s = -s; b += K; }
+        if (s > s0) { b1 = b0; s1 = s0; b0 = b; s0 = s; }
+        else if (s > s1) { b1 = b; s1 = s; }
+    }
+    const float angle0 = (float)acos((double)fminf(s0, 1.f));
+    w1 = (float)__ddiv_rn((double)angle0, a.pi_k);
 }
 
 // ---- orientation bin of an interior pixel without a division.  t_k = gx ox_k + gy oy_k on the integer gradient decides the

@@ -241,4 +241,74 @@ inline std::vector<cv::Mat> hog_dense(const std::vector<cv::Mat>& images, VlHogV
     return out;
 }
 
+// VLFeat HOG of whole frames of one or more channels, 8-bit or float (vl_hog_new(variant, num_bins),
+// vl_hog_set_use_bilinear_orientation_assignments(bilinear_orientations), vl_hog_put_image(frame, channels, cell_size),
+// vl_hog_extract), in one batched call on the device (sd_hog_dense_images).  Each frame is the list of its channel planes --
+// what cv::split gives, VLFeat's planar layout -- all CV_8UC1 or all CV_32FC1, of one size per frame; every frame has the same
+// number of planes and the same type.  Channels are used as given: at each pixel the one with the largest gradient wins.
+// Returns what rcr::hog_dense returns: one CV_32FC1 Mat per frame with dd * hogH rows and hogW columns.  Throws
+// std::runtime_error for frames or a configuration that sd_hog_dense_images refuses.
+inline std::vector<cv::Mat> vl_hog(const std::vector<std::vector<cv::Mat>>& frames, VlHogVariant variant, int cell_size, int num_bins,
+                                   bool bilinear_orientations = false)
+{
+    std::vector<cv::Mat> out;
+    if (frames.empty()) return out;
+    const int n = static_cast<int>(frames.size());
+    const int channels = static_cast<int>(frames[0].size());
+    if (channels < 1 || channels > 16) throw std::runtime_error("vl_hog: frames must have 1..16 channel planes");
+    const int type = frames[0][0].type();
+    if (type != CV_8UC1 && type != CV_32FC1) throw std::runtime_error("vl_hog: channel planes must be CV_8UC1 or CV_32FC1");
+    const size_t es = type == CV_8UC1 ? 1 : 4;
+    std::vector<sd_hog_image> desc(n);
+    std::vector<int64_t> offset(n);
+    std::vector<int> rows(n), cols(n);
+    int64_t elems = 0, total = 0;
+    for (int i = 0; i < n; ++i) {
+        const std::vector<cv::Mat>& f = frames[i];
+        if (static_cast<int>(f.size()) != channels) throw std::runtime_error("vl_hog: frame " + std::to_string(i) + " has a different number of planes");
+        for (const cv::Mat& p : f)
+            if (p.type() != type || p.cols != f[0].cols || p.rows != f[0].rows)
+                throw std::runtime_error("vl_hog: the planes of frame " + std::to_string(i) + " differ in type or size from the first frame's");
+        const int W = f[0].cols, H = f[0].rows;
+        int w = 0, h = 0, dd = 0;
+        if (sd_hog_dense_shape(W, H, cell_size, num_bins, variant, &w, &h, &dd) != SD_OK)
+            throw std::runtime_error("vl_hog: frame " + std::to_string(i) + " (" + std::to_string(W) + " x " + std::to_string(H) +
+                                     ") or the configuration is invalid: frames wider and taller than 3 px and at least half a cell, "
+                                     "cell_size 1..32, num_bins 1..16");
+        desc[i].width = W;
+        desc[i].height = H;
+        desc[i].offset = elems;
+        desc[i].row_stride = W;
+        desc[i].pixel_stride = 1;
+        desc[i].channel_stride = static_cast<int64_t>(W) * H;
+        elems += static_cast<int64_t>(W) * H * channels;
+        offset[i] = total;
+        rows[i] = dd * h;
+        cols[i] = w;
+        total += static_cast<int64_t>(dd) * h * w;
+    }
+    sd_ctx* ctx = sd_b200::context();
+    sd_b200::DeviceBuffer buf(static_cast<size_t>(elems) * es), d_desc(static_cast<size_t>(n) * sizeof(sd_hog_image)),
+        d_out(static_cast<size_t>(total) * sizeof(float)), d_offset(static_cast<size_t>(n) * sizeof(int64_t));
+    for (int i = 0; i < n; ++i)
+        for (int c = 0; c < channels; ++c) {
+            const cv::Mat& p = frames[i][c];
+            unsigned char* dst = buf.as<unsigned char>() + static_cast<size_t>(desc[i].offset + c * desc[i].channel_stride) * es;
+            sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, dst, static_cast<size_t>(p.cols) * es, p.ptr<unsigned char>(0), p.step(), static_cast<size_t>(p.cols) * es,
+                                                static_cast<size_t>(p.rows)), "vl_hog upload");
+        }
+    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_desc.as<sd_hog_image>(), desc.data(), static_cast<size_t>(n) * sizeof(sd_hog_image)), "vl_hog upload");
+    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_offset.as<int64_t>(), offset.data(), static_cast<size_t>(n) * sizeof(int64_t)), "vl_hog");
+    sd_hog_images images{};
+    images.d_data = buf.as<void>();
+    images.dtype = type == CV_8UC1 ? SD_HOG_U8 : SD_HOG_F32;
+    images.channels = channels;
+    images.count = n;
+    images.d_frames = d_desc.as<sd_hog_image>();
+    sd_b200::check(ctx, sd_hog_dense_images(ctx, &images, cell_size, num_bins, variant, bilinear_orientations ? 1 : 0, d_out.as<float>(),
+                                            d_offset.as<int64_t>()), "sd_hog_dense_images");
+    for (int i = 0; i < n; ++i) out.push_back(sd_b200::download(d_out.as<float>() + offset[i], rows[i], cols[i], cols[i]));
+    return out;
+}
+
 }  // namespace rcr
