@@ -47,6 +47,7 @@ struct HogArgs {
     const int* half;            // per sample: half patch size (hog_geometry_kernel)
     float ox[SD_MAX_BINS], oy[SD_MAX_BINS];   // orientation k: (cos, sin)(k pi / K) in float, host libm (hog.c:195-204)
     int vbin[2];                // reference bin of a gradient (0, gy): [0] gy > 0, [1] gy < 0
+    float bx[SD_MAX_BINS / 2], by[SD_MAX_BINS / 2], bin_margin;   // hog_bin's sector boundaries and margin (hog_orientations)
     const int* rtab;            // per sample: resize tables [5][fs] (hog_geometry_kernel)
     const float* btab;          // per launch: spatial binning weights [nc][fs], then lo[nc], hi[nc] (hog_bintab_kernel)
     int tma_count;              // number of usable tensor-map size classes (0: the window is staged by load loops)
@@ -441,7 +442,7 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const __grid_con
             const int gy = (int)s_patch[idx + fs] - (int)s_patch[idx - fs];
             const int g2 = gx * gx + gy * gy;
             const float g = __fsqrt_rn((float)g2);
-            s_bin[idx] = (int8_t)hog_bin(a, K, gx, gy, g2, g);
+            s_bin[idx] = (int8_t)hog_bin(a, K, gx, gy, g);
             s_gmag[idx] = g;
         }
     }
@@ -628,7 +629,7 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
     a.geometry = d_geometry; a.patches = d_patches; a.bins = d_bins;
     a.status = reinterpret_cast<int*>(ctx->d_scratch) + 1;   // the projection's own status word: bit 0 empty patch, bit 1 bad image index
 
-    hog_orientations(a.K, a.ox, a.oy, a.vbin);   // hog.c:195-204
+    hog_orientations(a.K, a);   // hog.c:195-204
 
     // per-sample tables (half size, cv::resize taps) and the per-launch spatial binning table
     const size_t geom_bytes = (size_t)N * sizeof(int) + (size_t)N * 5 * fs * sizeof(int) + (size_t)(a.nc * fs + 2 * a.nc) * sizeof(float);

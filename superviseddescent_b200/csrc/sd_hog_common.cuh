@@ -12,16 +12,33 @@
 
 namespace {
 
+// Margin of hog_bin's sector test against the reference's first-maximum rule: a lead of the winning |<g, o_k>| over every other
+// one of more than eps |g| cannot change the reference's arg-max or its sign (derivation at hog_bin).
+constexpr double kBinLead = 4e-6;
+
 // Orientation directions (hog.c:195-204: host libm cos/sin, as the reference) and the reference bin of a gradient (0, gy):
-// vbin[0] for gy > 0, vbin[1] for gy < 0.  ox / oy hold SD_MAX_BINS entries; those past K are zero.
-inline void hog_orientations(int K, float* ox, float* oy, int* vbin)
+// vbin[0] for gy > 0, vbin[1] for gy < 0.  ox / oy hold SD_MAX_BINS entries; those past K are zero.  For hog_bin's sector
+// search: the directions (bx_j, by_j) = (cos, sin)((2j + 1) pi / 2K) of the sector boundaries inside the open first quadrant
+// (j < K / 2), and the margin eps / (2 sin(pi / 2K)) on |cross(b, g)| / |g| that gives a lead of eps.
+//   Args: any kernel argument block with the members ox, oy, vbin, bx, by and bin_margin.
+template <class Args>
+inline void hog_orientations(int K, Args& a)
 {
+    float* ox = a.ox;
+    float* oy = a.oy;
+    int* vbin = a.vbin;
     for (int k = 0; k < SD_MAX_BINS; ++k) { ox[k] = 0.f; oy[k] = 0.f; }
     for (int k = 0; k < K; ++k) {
         const double angle = k * 3.141592653589793 / K;
         ox[k] = (float)cos(angle);
         oy[k] = (float)sin(angle);
     }
+    for (int j = 0; j < SD_MAX_BINS / 2; ++j) {
+        const double angle = (2 * j + 1) * 3.141592653589793 / (2 * K);
+        a.bx[j] = j < K / 2 ? (float)cos(angle) : 0.f;
+        a.by[j] = j < K / 2 ? (float)sin(angle) : 0.f;
+    }
+    a.bin_margin = (float)(kBinLead / (2.0 * sin(3.141592653589793 / (2 * K))));
     // hog.c:645-672 at gx = 0: ux = +0 and uy = +-1 exactly (the root of gy^2 is exact), so s_k = +-oy_k exactly; the first
     // strict maximum of oy_k > 0 wins, in the lower half-plane when gy < 0 (K = 1: no k has oy_k > 0, bin -1)
     {
@@ -89,38 +106,48 @@ __device__ __forceinline__ void hog_bins_bilinear(const Args& a, int K, float ux
     w1 = (float)__ddiv_rn((double)angle0, a.pi_k);
 }
 
-// ---- orientation bin of an interior pixel without a division.  t_k = gx ox_k + gy oy_k on the integer gradient decides the
-//      arg-max whenever its winner leads the runner-up by more than eps |g|; only the other lanes need the exact answer below.
-//      Why that is exact (u = 2^-24, r = |g| exact, e_k = gx ox_k + gy oy_k exact, ox_k^2 + oy_k^2 = 1 + O(u)):
-//        |t_k - e_k|     <= 2u r                           (one product, one FMA)
-//        |s_k - e_k / r| <= 4u                              (s_k: the reference's float dot product of gx/g, gy/g)
-//      so t_b leading every other |t_j| by eps r makes |s_b| lead every |s_j| by (eps - 12u) > 0, and |t_b| > eps r fixes
-//      the sign of s_b: the reference's first strict maximum is the same k and the same half-plane.  eps = 4e-6 is ~33u;
-//      the slack also covers the rounding of the test itself (squared, against eps^2 g2, to avoid the root).
-//      tests/test_gpu_hog_orientation.py checks every (gx, gy) in [-255, 255]^2 at every K in 1..16. ------------------------
-constexpr float kBinMargin2 = 4e-6f * 4e-6f;
-
+// ---- orientation bin of an interior pixel without a division, by sector search.  Exactly, the reference's bin (the first
+//      strict maximum of |<u, o_k>|, k or k + K by its sign) is the index of the one of 2K angular sectors centred on k pi / K
+//      that holds theta = arg g; the sector boundaries are the bisectors (2j + 1) pi / 2K.  Two exact folds on the integers
+//      bring g into the quadrant gx >= 0, gy >= 0: the point reflection g -> -g maps bin k to k + K (mod 2K), and the mirror
+//      gx -> -gx maps the half-plane sector s (centre s pi / K, s = 0..K) to K - s.  There only the K / 2 boundaries
+//      b_j = (cos, sin)((2j + 1) pi / 2K) are left (and pi / 2 for odd K, the gx = 0 axis), so the sector is the count of
+//      positive cross products c_j = cross(b_j, g) = r sin(theta - beta_j), r = |g|: at most 8 of them, no indexed loads.
+//      Accepting it is exact when the nearest boundary, at angle delta, has |c| > C r, C = eps / (2 sin(pi / 2K)):
+//        - the winner's exact |cos(theta - k pi / K)| leads every other one by 2 sin(pi / 2K) sin delta, and is >= sin delta;
+//        - u = 2^-24.  s_k (the reference's float dot product of gx/g, gy/g) is within 4u of the exact dot product with the
+//          float o_k, which is within u of cos(theta - k pi / K).  c_j (one product, one FMA, float b_j) is within 3u r of
+//          r sin(theta - beta_j).  The test m > fl(C g) carries another ~3u relative;
+//        - so sin delta > C - 4u, the exact lead exceeds eps - 8u and the reference's lead exceeds eps - 18u > 0
+//          (eps = 4e-6 is ~67u).  The winner's |s_k| > sin delta - 5u > 0 fixes the sign, and every c_j, whose |c_j| is at
+//          least r sin delta > 3u r, has the right sign: the count is the exact sector.
+//      The folds need no symmetry of the float tables, since the exact sectors have it.  m is the least |c_j|: the other
+//      boundaries (outside the quadrant) are mirror images at the same or a larger angle.  Pixels that miss the margin, nearly
+//      all exactly on a boundary, take the reference expression.  gx = 0 stays in the quadrant: at even K it is the centre of
+//      sector K / 2 and the count decides it; at odd K it is a boundary (m = |gx| = 0), common in real patches, and the
+//      reference's unit vector there is exactly (0, +-1), so its bin is a function of K and the sign of gy alone
+//      (hog_orientations).  g = 0 makes every c_j zero and also misses the margin (bin -1).  tests/test_gpu_hog_orientation.py and tests/test_gpu_hog_sector.py check every (gx, gy) in
+//      [-255, 255]^2 at every K in 1..16. -------------------------------------------------------------------------------
 template <class Args>
-__device__ __forceinline__ int hog_bin(const Args& a, int K, int gx, int gy, int g2, float g)
+__device__ __forceinline__ int hog_bin(const Args& a, int K, int gx, int gy, float g)
 {
-    if (g2 == 0) return -1;
-    const float fx = (float)gx, fy = (float)gy;
-    float m1 = 0.f, m2 = 0.f;            // largest and second largest |t_k| (a tie leaves m1 == m2: no margin)
-    int best = 0;
-    bool neg = false;
+    const float fx = (float)abs(gx), fy = (float)abs(gy);
+    float m = (K & 1) ? fx : INFINITY;   // odd K: |cross((0, 1), g)| against the boundary pi / 2
+    int s = 0;
 #pragma unroll
-    for (int k = 0; k < K; ++k) {
-        const float t = fmaf(fx, a.ox[k], fy * a.oy[k]);
-        const float m = fabsf(t);
-        if (m > m1) { m2 = m1; m1 = m; best = k; neg = t < 0.f; }
-        else if (m > m2) m2 = m;
+    for (int j = 0; j < K / 2; ++j) {
+        const float c = fmaf(a.bx[j], fy, -(a.by[j] * fx));
+        s += c > 0.f;
+        m = fminf(m, fabsf(c));
     }
-    const float d = m1 - m2;
-    if (d * d > kBinMargin2 * (float)g2) return neg ? best + K : best;
-    // the gx = 0 axis is a bin boundary for odd K and common in real patches; the reference's unit vector there is exactly
-    // (0, +-1), so its bin is a function of K and the sign of gy alone (hog_orientations)
-    if (gx == 0) return a.vbin[gy < 0];
-    return hog_bin_reference(a, K, fx, fy, g);
+    if (m > a.bin_margin * g) {
+        const bool neg = gy < 0;
+        if ((gx < 0) != neg) s = K - s;
+        if (neg) s += K;
+        return s < 2 * K ? s : 0;
+    }
+    if (gx == 0) return gy == 0 ? -1 : a.vbin[gy < 0];
+    return hog_bin_reference(a, K, (float)gx, (float)gy, g);
 }
 
 typedef CUresult (*PFN_hogEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,

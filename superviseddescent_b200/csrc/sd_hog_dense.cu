@@ -52,6 +52,7 @@ struct DenseArgs {
     int tma;                             // the staging is one TMA tile
     float ox[SD_MAX_BINS], oy[SD_MAX_BINS];
     int vbin[2];
+    float bx[SD_MAX_BINS / 2], by[SD_MAX_BINS / 2], bin_margin;   // hog_bin's sector boundaries and margin
 };
 
 struct ImageArgs {
@@ -70,6 +71,7 @@ struct ImageArgs {
     double pi_k;                         // pi / K (hog.c:677)
     float ox[SD_MAX_BINS], oy[SD_MAX_BINS];
     int vbin[2];
+    float bx[SD_MAX_BINS / 2], by[SD_MAX_BINS / 2], bin_margin;   // hog_bin's sector boundaries and margin
 };
 
 // tile side in cells for a cell size: the staged region cs * (T + 4) + 2 stays near kDenseSpanBudget pixels
@@ -254,7 +256,7 @@ __device__ __forceinline__ void hog_dense_cta(const Args& a, const CUtensorMap* 
                     const int gy = (int)p[pitch] - (int)p[-pitch];
                     const int g2 = gx * gx + gy * gy;
                     const float g = __fsqrt_rn((float)g2);
-                    s_bin[y * span + x] = (int8_t)hog_bin(a, K, gx, gy, g2, g);
+                    s_bin[y * span + x] = (int8_t)hog_bin(a, K, gx, gy, g);
                     s_g[y * span + x] = g;
                 }
         }
@@ -290,7 +292,7 @@ __device__ __forceinline__ void hog_dense_cta(const Args& a, const CUtensorMap* 
                     s_bin1[y * span + x] = (int8_t)b1;
                     s_w1[y * span + x] = w1;
                 } else if constexpr (std::is_same<Pix, uint8_t>::value) {
-                    b0 = hog_bin(a, K, (int)gx, (int)gy, (int)g2, g);
+                    b0 = hog_bin(a, K, (int)gx, (int)gy, g);
                 } else {
                     b0 = hog_bin_unit(a, K, hog_unit(gx, g), hog_unit(gy, g));
                 }
@@ -547,7 +549,7 @@ int sd_hog_dense(sd_ctx* ctx, const sd_image_batch* images, int cell_size, int n
     a.tile = dense_tile(cell_size);
     a.span = cell_size * (a.tile + 4) + 2;
     a.pitch = dense_align(a.span + 15, 16);
-    hog_orientations(num_bins, a.ox, a.oy, a.vbin);   // hog.c:195-204
+    hog_orientations(num_bins, a);   // hog.c:195-204
 
     // TMA staging: equally sized frames with 16-byte aligned base and pitches (a box of pitch x span bytes per CTA; bytes past
     // the frame's edge are zero-filled and never read)
@@ -654,7 +656,7 @@ int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size,
     a.tile = images_tile(kern, cell_size, num_bins, bil);
     a.span = cell_size * (a.tile + 3) + 4;
     a.pi_k = 3.141592653589793 / (double)num_bins;    // VL_PI / numOrientations (hog.c:677)
-    hog_orientations(num_bins, a.ox, a.oy, a.vbin);
+    hog_orientations(num_bins, a);
 
     const DenseSmem lay = dense_smem_layout(a.span, 0, num_bins, dense_cells(a.tile), bil);
     SD_REQUIRE(ctx, lay.total <= 227 * 1024, "dense HOG configuration needs more than 227 KB of shared memory");
