@@ -405,25 +405,9 @@ syrk_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     }
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-PFN_encodeTiled get_encode_fn()
-{
-    static PFN_encodeTiled fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<PFN_encodeTiled>(p);
-    }
-    return fn;
-}
-
 int make_map(sd_ctx* ctx, CUtensorMap* map, const float* base, int64_t ld, int rows, int cols)
 {
-    PFN_encodeTiled enc = get_encode_fn();
+    sd_encode_tiled_fn enc = sd_encode_tiled();
     if (!enc) return sd_fail(ctx, SD_ERR_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
     cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
     cuuint64_t gstride[1] = {(cuuint64_t)ld * sizeof(float)};
@@ -437,6 +421,18 @@ int make_map(sd_ctx* ctx, CUtensorMap* map, const float* base, int64_t ld, int r
 }
 
 }  // namespace
+
+sd_encode_tiled_fn sd_encode_tiled()
+{
+    static sd_encode_tiled_fn fn = nullptr;
+    if (!fn) {
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
+            fn = reinterpret_cast<sd_encode_tiled_fn>(p);
+    }
+    return fn;
+}
 
 bool sd_syrk_tc_supported(const float* d_S, int64_t lds, int K)
 {

@@ -1,10 +1,6 @@
-// Pieces of VLFeat's HOG shared by the landmark-patch kernel (sd_hog.cu) and the dense whole-frame kernel (sd_hog_dense.cu):
-// the orientation bin of an 8-bit gradient, the orientation table it reads, and the driver entry point of the TMA tensor maps.
-// Both kernels call the same functions, so tests/test_gpu_hog_orientation.py covers the bin rule of both.
+// VLFeat's HOG arithmetic, the TMA staging and the frame tensor map, shared by the landmark-patch kernel (sd_hog.cu) and the
+// dense whole-frame kernel (sd_hog_dense.cu): one copy, so an fs x fs frame gives bit for bit the features of an fs x fs patch.
 #pragma once
-
-#include <cuda.h>
-#include <cuda_runtime.h>
 
 #include <cmath>
 
@@ -19,34 +15,36 @@ constexpr double kBinLead = 4e-6;
 // Orientation directions (hog.c:195-204: host libm cos/sin, as the reference) and the reference bin of a gradient (0, gy):
 // vbin[0] for gy > 0, vbin[1] for gy < 0.  ox / oy hold SD_MAX_BINS entries; those past K are zero.  For hog_bin's sector
 // search: the directions (bx_j, by_j) = (cos, sin)((2j + 1) pi / 2K) of the sector boundaries inside the open first quadrant
-// (j < K / 2), and the margin eps / (2 sin(pi / 2K)) on |cross(b, g)| / |g| that gives a lead of eps.
-//   Args: any kernel argument block with the members ox, oy, vbin, bx, by and bin_margin.
-template <class Args>
-inline void hog_orientations(int K, Args& a)
+// (j < K / 2), and the margin eps / (2 sin(pi / 2K)) on |cross(b, g)| / |g| that gives a lead of eps.  Every kernel argument
+// block carries one (hog_orientations fills it).
+struct HogOrient {
+    float ox[SD_MAX_BINS], oy[SD_MAX_BINS];   // orientation k: (cos, sin)(k pi / K) in float
+    int vbin[2];                              // reference bin of a gradient (0, gy): [0] gy > 0, [1] gy < 0
+    float bx[SD_MAX_BINS / 2], by[SD_MAX_BINS / 2], bin_margin;   // hog_bin's sector boundaries and margin
+};
+
+inline void hog_orientations(int K, HogOrient& o)
 {
-    float* ox = a.ox;
-    float* oy = a.oy;
-    int* vbin = a.vbin;
-    for (int k = 0; k < SD_MAX_BINS; ++k) { ox[k] = 0.f; oy[k] = 0.f; }
+    for (int k = 0; k < SD_MAX_BINS; ++k) { o.ox[k] = 0.f; o.oy[k] = 0.f; }
     for (int k = 0; k < K; ++k) {
         const double angle = k * 3.141592653589793 / K;
-        ox[k] = (float)cos(angle);
-        oy[k] = (float)sin(angle);
+        o.ox[k] = (float)cos(angle);
+        o.oy[k] = (float)sin(angle);
     }
     for (int j = 0; j < SD_MAX_BINS / 2; ++j) {
         const double angle = (2 * j + 1) * 3.141592653589793 / (2 * K);
-        a.bx[j] = j < K / 2 ? (float)cos(angle) : 0.f;
-        a.by[j] = j < K / 2 ? (float)sin(angle) : 0.f;
+        o.bx[j] = j < K / 2 ? (float)cos(angle) : 0.f;
+        o.by[j] = j < K / 2 ? (float)sin(angle) : 0.f;
     }
-    a.bin_margin = (float)(kBinLead / (2.0 * sin(3.141592653589793 / (2 * K))));
+    o.bin_margin = (float)(kBinLead / (2.0 * sin(3.141592653589793 / (2 * K))));
     // hog.c:645-672 at gx = 0: ux = +0 and uy = +-1 exactly (the root of gy^2 is exact), so s_k = +-oy_k exactly; the first
     // strict maximum of oy_k > 0 wins, in the lower half-plane when gy < 0 (K = 1: no k has oy_k > 0, bin -1)
     {
         float best = 0.f;
         int bin = -1;
-        for (int k = 0; k < K; ++k) if (oy[k] > best) { best = oy[k]; bin = k; }
-        vbin[0] = bin;
-        vbin[1] = bin < 0 ? -1 : bin + K;
+        for (int k = 0; k < K; ++k) if (o.oy[k] > best) { best = o.oy[k]; bin = k; }
+        o.vbin[0] = bin;
+        o.vbin[1] = bin < 0 ? -1 : bin + K;
     }
 }
 
@@ -59,15 +57,13 @@ __device__ __forceinline__ float hog_unit(float v, float g)
 }
 
 // ---- the first maximum of |<u, o_k>| in ascending k for a unit gradient u (hog.c:656-672, nearest-bin assignment) ----
-//      Args: any kernel argument block with the members ox, oy and vbin that hog_orientations fills.
-template <class Args>
-__device__ __forceinline__ int hog_bin_unit(const Args& a, int K, float ux, float uy)
+__device__ __forceinline__ int hog_bin_unit(const HogOrient& o, int K, float ux, float uy)
 {
     float best = 0.f;
     int bin = -1;
 #pragma unroll
     for (int k = 0; k < K; ++k) {
-        float s = __fadd_rn(__fmul_rn(ux, a.ox[k]), __fmul_rn(uy, a.oy[k]));
+        float s = __fadd_rn(__fmul_rn(ux, o.ox[k]), __fmul_rn(uy, o.oy[k]));
         int b = k;
         if (s < 0.f) { s = -s; b += K; }
         if (s > best) { best = s; bin = b; }   // strict >, ascending k
@@ -77,10 +73,9 @@ __device__ __forceinline__ int hog_bin_unit(const Args& a, int K, float ux, floa
 
 // ---- orientation bin of a pixel with a non-zero integer-valued gradient (gx, gy), the reference's float expression
 //      verbatim (hog.c:645-672): modulus, normalised gradient (g >= 1, so hog_unit is a float division), then the bin ------
-template <class Args>
-__device__ __forceinline__ int hog_bin_reference(const Args& a, int K, float gx, float gy, float g)
+__device__ __forceinline__ int hog_bin_reference(const HogOrient& o, int K, float gx, float gy, float g)
 {
-    return hog_bin_unit(a, K, __fdiv_rn(gx, g), __fdiv_rn(gy, g));
+    return hog_bin_unit(o, K, __fdiv_rn(gx, g), __fdiv_rn(gy, g));
 }
 
 // ---- bilinear orientation assignment (hog.c:656-678): the reference's top-two tracking of |<u, o_k>| verbatim (a score
@@ -88,22 +83,22 @@ __device__ __forceinline__ int hog_bin_reference(const Args& a, int K, float gx,
 //        w1 = (float)((double)acosf(min(s0, 1)) / (pi / K)),  w0 = 1 - w1.
 //      b1 = -1 when no second score is positive (K = 1 among others); b0 = -1 for a zero gradient.  pi_k is pi / K in double.
 //      acos in double rounded to float stays within an ulp of the reference's acosf. ------------------------------------
-template <class Args>
-__device__ __forceinline__ void hog_bins_bilinear(const Args& a, int K, float ux, float uy, int& b0, int& b1, float& w1)
+__device__ __forceinline__ void hog_bins_bilinear(const HogOrient& o, double pi_k, int K, float ux, float uy, int& b0, int& b1,
+                                                  float& w1)
 {
     float s0 = 0.f, s1 = 0.f;
     b0 = -1;
     b1 = -1;
 #pragma unroll
     for (int k = 0; k < K; ++k) {
-        float s = __fadd_rn(__fmul_rn(ux, a.ox[k]), __fmul_rn(uy, a.oy[k]));
+        float s = __fadd_rn(__fmul_rn(ux, o.ox[k]), __fmul_rn(uy, o.oy[k]));
         int b = k;
         if (s < 0.f) { s = -s; b += K; }
         if (s > s0) { b1 = b0; s1 = s0; b0 = b; s0 = s; }
         else if (s > s1) { b1 = b; s1 = s; }
     }
     const float angle0 = (float)acos((double)fminf(s0, 1.f));
-    w1 = (float)__ddiv_rn((double)angle0, a.pi_k);
+    w1 = (float)__ddiv_rn((double)angle0, pi_k);
 }
 
 // ---- orientation bin of an interior pixel without a division, by sector search.  Exactly, the reference's bin (the first
@@ -128,42 +123,136 @@ __device__ __forceinline__ void hog_bins_bilinear(const Args& a, int K, float ux
 //      reference's unit vector there is exactly (0, +-1), so its bin is a function of K and the sign of gy alone
 //      (hog_orientations).  g = 0 makes every c_j zero and also misses the margin (bin -1).  tests/test_gpu_hog_orientation.py and tests/test_gpu_hog_sector.py check every (gx, gy) in
 //      [-255, 255]^2 at every K in 1..16. -------------------------------------------------------------------------------
-template <class Args>
-__device__ __forceinline__ int hog_bin(const Args& a, int K, int gx, int gy, float g)
+__device__ __forceinline__ int hog_bin(const HogOrient& o, int K, int gx, int gy, float g)
 {
     const float fx = (float)abs(gx), fy = (float)abs(gy);
     float m = (K & 1) ? fx : INFINITY;   // odd K: |cross((0, 1), g)| against the boundary pi / 2
     int s = 0;
 #pragma unroll
     for (int j = 0; j < K / 2; ++j) {
-        const float c = fmaf(a.bx[j], fy, -(a.by[j] * fx));
+        const float c = fmaf(o.bx[j], fy, -(o.by[j] * fx));
         s += c > 0.f;
         m = fminf(m, fabsf(c));
     }
-    if (m > a.bin_margin * g) {
+    if (m > o.bin_margin * g) {
         const bool neg = gy < 0;
         if ((gx < 0) != neg) s = K - s;
         if (neg) s += K;
         return s < 2 * K ? s : 0;
     }
-    if (gx == 0) return gy == 0 ? -1 : a.vbin[gy < 0];
-    return hog_bin_reference(a, K, (float)gx, (float)gy, g);
+    if (gx == 0) return gy == 0 ? -1 : o.vbin[gy < 0];
+    return hog_bin_reference(o, K, (float)gx, (float)gy, g);
 }
 
-typedef CUresult (*PFN_hogEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                       const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                       CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-PFN_hogEncodeTiled hog_encode_fn()
+// ---- spatial binning of pixel coordinate t (hog.c:697-709, rounded as there): h = (t + 0.5) / cs - 0.5, b = floor(h),
+//      w2 = h - b, w1 = (float)(1.0 - w2); the pixel adds w1 to cell b and w2 to cell b + 1 ------------------------------
+__device__ __forceinline__ void hog_spatial_weight(int t, int cs, int* b, float* w1, float* w2)
 {
-    static PFN_hogEncodeTiled fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<PFN_hogEncodeTiled>(p);
+    const float h = (float)__dadd_rn(__ddiv_rn((double)t + 0.5, (double)cs), -0.5);
+    int bb = (int)h;                                  // vl_floor_f, hog.h:52-58
+    if (!(h >= 0.f || (float)bb == h)) bb -= 1;
+    *b = bb;
+    *w2 = __fsub_rn(h, (float)bb);
+    *w1 = (float)__dadd_rn(1.0, -(double)*w2);
+}
+
+// ---- undirected cell energy (hog.c:875-890) in float: sum over k of (h_k + h_{k+K})^2, h_b = hist[b * stride] -----------
+__device__ __forceinline__ float hog_cell_energy(const float* hist, int stride, int K)
+{
+    float e = 0.f;
+    for (int k = 0; k < K; ++k) {
+        const float h = __fadd_rn(hist[k * stride], hist[(k + K) * stride]);
+        e = __fadd_rn(e, __fmul_rn(h, h));
     }
-    return fn;
+    return e;
+}
+
+// ---- block factor in double (hog.c:930-982) of the 2 x 2 cells at columns xa, xb and rows ya, yb of the energies E (row
+//      stride ld).  factor1: n1+n2+n4+n5, factor2: n2+n3+n5+n6, factor3: n4+n5+n7+n8, factor4: n5+n6+n8+n9 --------------
+__device__ __forceinline__ double hog_block_factor(const float* E, int ld, int xa, int xb, int ya, int yb)
+{
+    double s = (double)E[xa + ya * ld];
+    s = __dadd_rn(s, (double)E[xb + ya * ld]);
+    s = __dadd_rn(s, (double)E[xa + yb * ld]);
+    s = __dadd_rn(s, (double)E[xb + yb * ld]);
+    s = __dadd_rn(s, 1e-4);
+    return __ddiv_rn(1.0, sqrt(s));
+}
+
+// ---- normalise bins k and k + K of a cell (ha, hb) by its four block factors, clamp at 0.2 and project (hog.c:985-1044).
+//      keep(f, hc) takes block f's clamped sum, which the texture dims add up over k (hog.c:1046-1053); store(d, v) writes
+//      feature dimension d of the cell.
+template <class Keep, class Store>
+__device__ __forceinline__ void hog_project(const double* fac, double ha, double hb, int k, int K, int variant, Keep keep, Store store)
+{
+    double sa = 0.0, sb = 0.0, sc = 0.0;
+    double hcv[4];
+#pragma unroll
+    for (int f = 0; f < 4; ++f) {
+        double haf = __dmul_rn(fac[f], ha);
+        double hbf = __dmul_rn(fac[f], hb);
+        double hcf = __dadd_rn(haf, hbf);
+        haf = (0.2 < haf) ? 0.2 : haf;
+        hbf = (0.2 < hbf) ? 0.2 : hbf;
+        hcf = (0.2 < hcf) ? 0.2 : hcf;
+        hcv[f] = hcf;
+        sa = (f == 0) ? haf : __dadd_rn(sa, haf);
+        sb = (f == 0) ? hbf : __dadd_rn(sb, hbf);
+        sc = (f == 0) ? hcf : __dadd_rn(sc, hcf);
+        keep(f, hcf);
+    }
+    if (variant == 1) {                                 // UoCTTI
+        store(k, (float)__dmul_rn(0.5, sa));
+        store(k + K, (float)__dmul_rn(0.5, sb));
+        store(k + 2 * K, (float)__dmul_rn(0.5, sc));
+    } else {                                            // Dalal-Triggs
+#pragma unroll
+        for (int f = 0; f < 4; ++f) store(k + f * K, (float)hcv[f]);
+    }
+}
+
+// ---- TMA staging: one thread copies the box at (x, y, z) of a 3-D tensor map (`bytes` bytes; x a multiple of 16, bytes
+//      outside the tensor zero-filled) to dst on the mbarrier at mbar, and every thread waits in hog_tma_wait ----------------
+__device__ __forceinline__ void hog_tma_load(uint64_t* mbar, void* dst, const CUtensorMap* map, int x, int y, int z, int bytes)
+{
+    const uint32_t bar = (uint32_t)__cvta_generic_to_shared(mbar);
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+                 ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(map), "r"(bar), "r"(x), "r"(y), "r"(z) : "memory");
+}
+
+__device__ __forceinline__ void hog_tma_wait(uint64_t* mbar)
+{
+    const uint32_t bar = (uint32_t)__cvta_generic_to_shared(mbar);
+    uint32_t ok = 0;
+    const long long t0 = clock64();
+    while (!ok) {                                      // bounded: a protocol bug must trap, never hang the GPU
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                     : "=r"(ok) : "r"(bar) : "memory");
+        if (!ok && clock64() - t0 > 4000000000LL) __trap();
+    }
+}
+
+// ---- the 3-D u8 tensor map {width, height, count} of equally sized frames with a box_w x box_h x 1 box; false for per-frame
+//      descriptors, a base or pitch that is not 16-byte aligned, or a box the driver refuses
+inline bool hog_frame_map(const sd_image_batch* images, int box_w, int box_h, CUtensorMap* map)
+{
+    if (images->d_frames || (reinterpret_cast<uintptr_t>(images->d_data) & 15) || images->row_stride % 16 ||
+        (images->count > 1 && images->image_stride % 16))
+        return false;
+    const sd_encode_tiled_fn enc = sd_encode_tiled();
+    if (!enc) return false;
+    cuuint64_t gdim[3] = {(cuuint64_t)images->width, (cuuint64_t)images->height, (cuuint64_t)images->count};
+    cuuint64_t gstride[2] = {(cuuint64_t)images->row_stride,
+                             (cuuint64_t)(images->count > 1 ? images->image_stride : (int64_t)images->row_stride * images->height)};
+    if (gstride[1] % 16) gstride[1] = (gstride[1] + 15) / 16 * 16;
+    cuuint32_t box[3] = {(cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    return enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<uint8_t*>(images->d_data), gdim, gstride, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 }  // namespace

@@ -2,6 +2,7 @@
 // Nothing here is part of the C ABI (include/sd_b200.h).
 #pragma once
 
+#include <cuda.h>
 #include <cuda_runtime.h>
 
 #include <cstdarg>
@@ -112,6 +113,11 @@ int sd_syrk_tc(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ
                int passes, bool unbiased, const sd_row_filter* rows);
 // whether the tensor-core kernel can read S (TMA alignment)
 bool sd_syrk_tc_supported(const float* d_S, int64_t lds, int K);
+// the driver's cuTensorMapEncodeTiled, looked up once (sd_gram_tc.cu); nullptr when the driver does not provide it
+typedef CUresult (*sd_encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                       const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                       CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+sd_encode_tiled_fn sd_encode_tiled();
 // the SYRK dispatcher (sd_linalg.cu): the one place that reads the gram mode and picks the tensor-core or the SIMT kernel.
 // big: the size rule's verdict (syrk_is_big) for the product the call belongs to.
 int syrk_upper(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ, float* d_C, int64_t ldc, float alpha, float beta,
