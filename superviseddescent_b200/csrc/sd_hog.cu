@@ -421,8 +421,9 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const __grid_con
             const int gy = (int)s_patch[idx + fs] - (int)s_patch[idx - fs];
             const int g2 = gx * gx + gy * gy;
             const float g = __fsqrt_rn((float)g2);
-            s_bin[idx] = (int8_t)hog_bin(a.orient, K, gx, gy, g);
-            s_gmag[idx] = g;
+            const int b = hog_bin(a.orient, K, gx, gy, g);
+            s_bin[idx] = (int8_t)b;
+            s_gmag[idx] = b < 0 ? 0.f : g;                         // no bin, no vote (hog.c:694): g = 0, or gx = 0 at K = 1
         }
     }
     if (a.bins) {
@@ -452,7 +453,7 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const __grid_con
             for (int b = 0; b < 2 * K; ++b) T[b * tpad] = 0.f;        // T shares the staging area of S1: clear this column first
 #pragma unroll 2
             for (int x = xlo; x <= xhi; ++x) {
-                const int b = max((int)*bp++, 0);                     // zero gradient: bin -1, modulus 0 -> adds +0 to bin 0
+                const int b = max((int)*bp++, 0);                     // no bin: bin -1, modulus stored as 0 -> adds +0 to bin 0
                 float* q = T + b * tpad;
                 *q = __fadd_rn(*q, __fmul_rn(*gp++, *wp++));
             }
@@ -568,6 +569,11 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
     a.dd = p->variant == 1 ? 3 * p->num_bins + 4 : 4 * p->num_bins;
     a.A = d_A; a.ld = ld;
     if (d_A) SD_REQUIRE(ctx, ld >= (int64_t)L * a.nc * a.nc * a.dd + 1, "ld < feature length");
+    // every argument check before the first launch: a rejected configuration queues no work
+    const HogSmem lay = hog_smem_layout(fs, a.nc, a.K, a.dd);
+    SD_REQUIRE(ctx, lay.total <= 227 * 1024, "HOG configuration needs more than 227 KB of shared memory");
+    const long long blocks = (long long)N * L;
+    SD_REQUIRE(ctx, blocks < 2147483647LL, "too many patches for one launch");
     a.geometry = d_geometry; a.patches = d_patches; a.bins = d_bins;
     a.status = reinterpret_cast<int*>(ctx->d_scratch) + 1;   // the projection's own status word: bit 0 empty patch, bit 1 bad image index
 
@@ -599,10 +605,6 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
         }
     }
 
-    const HogSmem lay = hog_smem_layout(fs, a.nc, a.K, a.dd);
-    SD_REQUIRE(ctx, lay.total <= 227 * 1024, "HOG configuration needs more than 227 KB of shared memory");
-    const long long blocks = (long long)N * L;
-    SD_REQUIRE(ctx, blocks < 2147483647LL, "too many patches for one launch");
     auto kern = hog_patch_kernel<0, 0, 0>;
     if (a.K == 4) kern = hog_patch_kernel<4, 0, 0>;
     else if (a.K == 9) kern = hog_patch_kernel<9, 0, 0>;

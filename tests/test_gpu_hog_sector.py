@@ -66,9 +66,7 @@ def test_sector_margin_on_the_host(oracle):
 @pytest.mark.gpu
 def test_sector_bins_every_gradient_landmark_and_dense(sd, oracle):
     """Every gradient at every K: the landmark kernel's bins against the reference, and the dense kernel's features of the same
-    frames against the landmark kernel's, bit for bit (the dense HOG of an fs x fs frame is the fixed-patch row).  At K = 1 the
-    features are not compared: there the gx = 0 axis has no bin, and the landmark kernel's vote adds such a pixel's modulus to
-    bin 0 while the dense kernel leaves it out, as hog.c does."""
+    frames against the landmark kernel's, bit for bit (the dense HOG of an fs x fs frame is the fixed-patch row)."""
     import torch
     from superviseddescent_b200 import _capi
     frames, gx, gy = _frames()
@@ -87,8 +85,6 @@ def test_sector_bins_every_gradient_landmark_and_dense(sd, oracle):
         got = bins[:, 0].cpu().numpy().astype(np.int32)[:, cy, cx]
         ref = _centre_bins(oracle, frames, K)
         assert np.array_equal(got, ref), f"K={K}: {int(np.sum(got != ref))} gradients differ"
-        if K == 1:
-            continue
         row = h(x.cpu().numpy(), 0).cpu().numpy()
         dd = 3 * K + 4
         dense = sd.hog_dense(dframes, CS, K, 1).cpu().numpy()

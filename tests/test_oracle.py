@@ -24,6 +24,23 @@ def test_resize_matches_cv2_goldens(oracle, golden):
         assert np.array_equal(got, dst), f"case {i}: {src.shape}->{dst.shape}"
 
 
+def test_resize_matches_cv2_goldens_wide(oracle, golden):
+    """resize_linear_u8 against cv2.resize at the windows and destinations (up to 192 px) of the landmark HOG configuration
+    sweep (tests/golden/gen_resize_wide.py): P = 2, P < fs, P = fs, P = 2 fs (cv2's INTER_AREA) and P far above fs."""
+    import importlib.util
+    spec = importlib.util.spec_from_file_location("gen_resize_wide", os.path.join(golden.dir, "gen_resize_wide.py"))
+    gen = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(gen)
+    g = np.load(os.path.join(golden.dir, "resize_cv2_wide.npz"))
+    want = {(P, fs) for P, dests in gen.pairs().items() for fs in dests}
+    have = {tuple(int(v) for v in k.split("_")[1:]) for k in g.files if k.startswith("dst_")}
+    assert have == want
+    for P, fs in sorted(have):
+        src = g[f"blur_{P}"] if f"blur_{P}" in g.files else gen.noise_source(P)
+        got = oracle.resize_linear_u8(src, fs, fs)
+        assert np.array_equal(got, g[f"dst_{P}_{fs}"]), f"{P} -> {fs}: {int(np.sum(got != g[f'dst_{P}_{fs}']))} pixels differ"
+
+
 def test_bgr2gray_matches_cv2_golden(oracle, golden):
     assert np.array_equal(oracle.bgr2gray_u8(golden.examples["bgr_crop"]), golden.examples["bgr_crop_gray"])
 
