@@ -252,6 +252,34 @@ typedef struct {
 SD_API int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size, int num_bins, int variant,
                                int bilinear_orientations, float* d_out, const int64_t* d_out_offset);
 
+/* ---- dense HOG of a caller's gradient fields: vl_hog_put_polar_field + vl_hog_extract (hog.c:746-845, :857-1062) ----------
+ * Each field is a modulus and an angle per pixel, e.g. the gradient of another operator, colour gradients combined by the
+ * caller, or an optical flow's magnitude and direction (histograms of flow).  One sd_hog_image places element (x, y) at
+ * offset + y * row_stride + x * pixel_stride of BOTH buffers: two separate planes, or an interleaved (H, W, 2) array with
+ * d_angle = d_modulus + 1 and pixel_stride = 2.  channel_stride is not read (it must not be negative, as everywhere). */
+typedef struct {
+    const float* d_modulus;          /* 4-byte aligned */
+    const float* d_angle;            /* 4-byte aligned; same element layout as d_modulus */
+    int32_t count;
+    sd_hog_image frame;              /* equally sized fields: field i at frame.offset + i * image_stride */
+    int64_t image_stride;            /* elements */
+    const sd_hog_image* d_frames;    /* optional: one descriptor per field, as in sd_hog_images */
+} sd_hog_polar_fields;
+/* sd_hog_dense_polar: vl_hog_new(variant, num_bins) + vl_hog_set_use_bilinear_orientation_assignments(bilinear_orientations)
+ * + vl_hog_put_polar_field(modulus, angle, directed, width, height, cell_size) + vl_hog_extract on every field, asynchronous on
+ * the context's stream.  Every pixel votes, the border rows and columns included; a modulus <= 0 does not (a NaN modulus
+ * does, as in hog.c).  ho = angle / (pi / num_bins) selects the bin floor(ho) or floor(ho) + 1 (nearest, a tie to the second),
+ * or both, weighted 1 - frac(ho) and frac(ho) (bilinear), each taken modulo 2 * num_bins (directed = 1) or num_bins
+ * (directed = 0); a vote carries modulus * wx * wy * w_o^2 as in hog.c.  Two cases hog.c leaves undefined have a defined
+ * result: a pixel whose ho is not a finite float (a NaN or infinite angle, or a quotient that overflows float) does not vote,
+ * and the residue is computed exactly without hog.c's loop, so angles of any magnitude (|ho| >= 2^63 included) vote into
+ * the exact bin.  Output, offsets, size rule and frame independence as sd_hog_dense_images (sd_hog_dense_shape gives the
+ * shape).  Null or unaligned field pointers, directed or bilinear_orientations outside {0, 1}, a negative offset or stride, a
+ * field that breaks the size rule, an invalid configuration, or fields of different sizes without d_out_offset is
+ * SD_ERR_INVALID before any work is queued (d_out is not written). */
+SD_API int sd_hog_dense_polar(sd_ctx* ctx, const sd_hog_polar_fields* fields, int cell_size, int num_bins, int variant,
+                              int directed, int bilinear_orientations, float* d_out, const int64_t* d_out_offset);
+
 /* ---- regressor: LinearRegressor<Solver> (regressors.hpp:318-400) ------------------------ */
 /* Solver::solve (regressors.hpp:199-234 == verbose_solver.hpp:53-111):
  *   X = (A^T A + Lambda)^-1 A^T B ;  A: N x D, B: N x M, X: D x M (ldx_out = M).

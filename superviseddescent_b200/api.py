@@ -23,7 +23,7 @@ import torch
 
 from . import _capi
 from ._capi import HogParam as HoGParam  # same field names as rcr::HoGParam
-from ._capi import HogImageC, HogImagesC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, ptr
+from ._capi import HogImageC, HogImagesC, HogPolarFieldsC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, ptr
 
 
 def _check(ctx, rc: int) -> None:
@@ -1336,3 +1336,82 @@ def load_detection_model(filename: str, ctx: Optional[Context] = None) -> detect
 def save_detection_model(model: detection_model, filename: str) -> None:
     """rcr::save_detection_model (model.hpp:214-219)."""
     model.save(filename)
+
+
+def vl_hog_polar(modulus, angle, cell_size: int, num_bins: int, variant: int = 1, directed: bool = True,
+                 bilinear_orientations: bool = False, ctx: Optional[Context] = None):
+    """VLFeat HOG of gradient fields the caller computed (vl_hog_new(variant, num_bins) +
+    vl_hog_set_use_bilinear_orientation_assignments(bilinear_orientations) + vl_hog_put_polar_field(modulus, angle, directed,
+    cell_size) + vl_hog_extract) on the device, in VLFeat's planar layout [dd][hogH][hogW] with x fastest.
+
+    modulus, angle: float32 fields, paired element by element -- two arrays or tensors (count, H, W) of one shape, or two lists
+    of (H, W) fields of any sizes.  angle is in radians, measured from the x axis towards y (rows grow downwards); it is taken
+    modulo 2 pi (directed) or pi.  Every pixel votes, the border included; a modulus <= 0 or a non-finite angle does not.
+    CUDA tensors of one device and equal strides are read in place; anything else is made contiguous and uploaded.
+    bilinear_orientations: every pixel votes into its two nearest orientation bins.  variant: 1 = UoCTTI (dd = 3K + 4),
+    0 = Dalal-Triggs (dd = 4K).  Returns one (count, dd, hogH, hogW) float32 CUDA tensor when all fields have one size, else a
+    list of (dd, hogH, hogW) tensors.  ValueError for fields that are not float32, not of the shapes above, or not paired."""
+    ctx = ctx or default_context()
+    dev = torch.device(f"cuda:{ctx.device}")
+    lib = _capi.lib()
+
+    def tensor(a):
+        return a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))
+
+    def checked(m, a, dims):
+        m, a = tensor(m), tensor(a)
+        if m.dtype != torch.float32 or a.dtype != torch.float32:
+            raise ValueError("modulus and angle must be float32")
+        if m.dim() != dims or tuple(m.shape) != tuple(a.shape):
+            raise ValueError(f"modulus and angle must be {'(count, H, W)' if dims == 3 else '(H, W)'} fields of one shape")
+        return m, a
+
+    fb = HogPolarFieldsC()
+    fb.d_frames = None
+    if isinstance(modulus, (list, tuple)) or isinstance(angle, (list, tuple)):
+        if not (isinstance(modulus, (list, tuple)) and isinstance(angle, (list, tuple))) or len(modulus) != len(angle):
+            raise ValueError("modulus and angle must both be lists of one length")
+        pairs = [checked(m, a, 2) for m, a in zip(modulus, angle)]
+        if not pairs:
+            return []
+        sizes = [tuple(m.shape) for m, _ in pairs]
+        for h, w in set(sizes):
+            hog_dense_shape(w, h, cell_size, num_bins, variant)   # refuse before the upload
+        descs, pos = [], 0
+        for h, w in sizes:
+            descs.append(HogImageC(w, h, pos, w, 1, 0))
+            pos += h * w
+        keep_m = torch.cat([m.reshape(-1) for m, _ in pairs]).to(dev)
+        keep_a = torch.cat([a.reshape(-1) for _, a in pairs]).to(dev)
+        fb.count = len(pairs)
+        if len(set(sizes)) == 1:
+            fb.frame, fb.image_stride = descs[0], sizes[0][0] * sizes[0][1]
+        else:
+            table = (HogImageC * len(descs))(*descs)
+            keep_table = torch.from_numpy(np.frombuffer(bytes(table), dtype=np.uint8).copy()).to(dev)
+            fb.d_frames = keep_table.data_ptr()
+    else:
+        m, a = checked(modulus, angle, 3)
+        if not (m.device == dev and a.device == dev and m.stride() == a.stride()):
+            m, a = m.contiguous().to(dev), a.contiguous().to(dev)
+        keep_m, keep_a = m, a
+        n, h, w = m.shape
+        fb.count, fb.frame, fb.image_stride = n, HogImageC(w, h, 0, m.stride(1), m.stride(2), 0), m.stride(0)
+        sizes = [(h, w)] * n
+    fb.d_modulus, fb.d_angle = keep_m.data_ptr(), keep_a.data_ptr()
+    n = len(sizes)
+    if n == 0:
+        return torch.empty((0,) + hog_dense_shape(fb.frame.width, fb.frame.height, cell_size, num_bins, variant), dtype=torch.float32,
+                           device=dev)
+    shapes = [hog_dense_shape(w, h, cell_size, num_bins, variant) for h, w in sizes]
+    flags = (int(cell_size), int(num_bins), int(variant), int(bool(directed)), int(bool(bilinear_orientations)))
+    if len(set(sizes)) == 1:
+        out = torch.empty((n,) + shapes[0], dtype=torch.float32, device=dev)
+        _check(ctx.h, lib.sd_hog_dense_polar(ctx.h, C.byref(fb), *flags, ptr(out), None))
+        return out
+    counts = [d * h * w for d, h, w in shapes]
+    starts = np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.int64)
+    offsets = torch.from_numpy(starts).to(dev)
+    out = torch.empty(int(sum(counts)), dtype=torch.float32, device=dev)
+    _check(ctx.h, lib.sd_hog_dense_polar(ctx.h, C.byref(fb), *flags, ptr(out), ptr(offsets)))
+    return [out[s:s + c].view(shape) for s, c, shape in zip(starts.tolist(), counts, shapes)]

@@ -9,11 +9,14 @@
 //      spatial weights per absolute coordinate, as the reference rounds them                                     hog.c:697-709
 //   S3 bilinear vote, separable: per cell, per row a sum over the row's pixels, then a sum over the rows          hog.c:713-724
 //   S4-S7 cell energy in float, the four block factors, clamp and projection in double                          hog.c:875-1053
-// Two kernels run the same CTA body (hog_dense_cta), which differs only in S1-S2:
+// Three kernels run the same CTA body (hog_dense_cta), which differs only in S1-S2:
 //   hog_dense_kernel   8-bit grey frames, nearest-bin orientations (sd_hog_dense): staged pixels, the integer bin rule
 //   hog_images_kernel  u8 or f32 frames of 1..16 strided channels, nearest-bin or bilinear orientations (sd_hog_dense_images):
 //                      each pixel's gradient is read straight from the frame, channel by channel, and the channel with the
 //                      largest squared modulus wins (hog.c:631-644); bilinear pixels keep two bins and a second weight
+//   hog_polar_kernel   a caller's gradient field, modulus and angle per pixel (sd_hog_dense_polar, vl_hog_put_polar_field,
+//                      hog.c:746-845): two f32 fields read in place through element strides; every pixel of the frame
+//                      votes, the border included, and the bins come from the angle alone (polar_bins)
 // Every histogram depends only on the frame's pixels and is summed in a fixed order (the order of the landmark-patch
 // kernel's two vote passes), so the result does not depend on the tiling, on the batch, or on the run.  A frame of
 // fs x fs pixels gives, bit for bit, the features the patch kernel computes from the same fs x fs patch.
@@ -66,6 +69,23 @@ struct ImageArgs {
     int span;                            // pixels per side of the region that votes: cs * (tile + 3) + 4
     double pi_k;                         // pi / K (hog.c:677)
     HogOrient orient;
+};
+
+struct PolarArgs {
+    const float* modulus;                // one descriptor places element e at modulus[e] and angle[e]
+    const float* angle;
+    sd_hog_image frame;                  // equally sized fields (frames == nullptr): field i at frame.offset + i * image_stride
+    long long image_stride;
+    const sd_hog_image* frames;          // optional: one descriptor per field
+    int directed;                        // the bin period is 2K (directed) or K
+    int frame0;
+    float* out;
+    const int64_t* out_offset;
+    long long out_stride;
+    int variant, cs, K, dd;
+    int tile;
+    int span;                            // pixels per side of the region that votes: cs * (tile + 3) + 4
+    double pi_k;                         // pi / K (hog.c:756)
 };
 
 // tile side in cells for a cell size: the staged region cs * (T + 4) + 2 stays near kDenseSpanBudget pixels
@@ -127,13 +147,47 @@ __device__ __forceinline__ void dense_weights(int tid, int cs, int span, int ox0
 // the staged pitch of a configuration: 8-bit grey frames are staged in shared memory, strided frames are read in place
 __device__ __forceinline__ int dense_pitch(const DenseArgs& a) { return a.pitch; }
 __device__ __forceinline__ int dense_pitch(const ImageArgs&) { return 0; }
+__device__ __forceinline__ int dense_pitch(const PolarArgs&) { return 0; }
 
-// One CTA of either kernel.  STAGED (DenseArgs): 8-bit grey frames, staged by TMA or a load loop, nearest-bin orientations from
-// the integer rule.  Otherwise (ImageArgs): Pix frames of C strided channels read in place, nearest-bin or (BIL) bilinear
-// orientations.  The weights and S3-S7 are the same code for both.
+// ---- orientation bins of a polar-field pixel (hog.c:784-800) without the reference's loop.  ho = (float)(angle / (pi / K)) in
+//      double as there, bino = floor(ho), wo2 = ho - bino and wo1 = 1 - wo2 in float.  hog.c adds 2K to bino until it is
+//      non-negative and then takes it modulo period (K, or 2K when directed); period divides 2K, so that is the Euclidean
+//      residue of bino, which floorf and fmodf give exactly for every finite ho, with no bound on |ho|.  Nearest-bin: bino + 1
+//      when wo1 > wo2 fails (a tie included), modulo period; bilinear: bins bino and bino + 1 modulo period, *w1 = wo2 the
+//      weight of the second (S3 forms wo1 = 1 - wo2 as hog.c does).  A pixel whose ho is not finite (a non-finite angle, or
+//      one whose quotient overflows float; hog.c's floor is undefined there) gets bin -1 and does not vote.  Every other bin
+//      is in [0, period).
+template <bool BIL>
+__device__ __forceinline__ int polar_bins(float angle, double pi_k, int period, int* b1, float* w1)
+{
+    const float ho = (float)__ddiv_rn((double)angle, pi_k);
+    if (!isfinite(ho)) return -1;
+    const float bino = floorf(ho);
+    const float wo2 = __fsub_rn(ho, bino), wo1 = __fsub_rn(1.f, wo2);
+    float r = fmodf(bino, (float)period);            // exact: an integer in (-period, period)
+    if (r < 0.f) r += (float)period;
+    const int b = (int)r;
+    if constexpr (BIL) {
+        *b1 = b + 1 == period ? 0 : b + 1;
+        *w1 = wo2;
+        return b;
+    } else {
+        const int n = b + (wo1 > wo2 ? 0 : 1);
+        return n == period ? 0 : n;
+    }
+}
+
+// One CTA of any of the three kernels.  STAGED (DenseArgs): 8-bit grey frames, staged by TMA or a load loop, nearest-bin
+// orientations from the integer rule.  POLAR (PolarArgs): a modulus and an angle field read in place, nearest-bin or (BIL)
+// bilinear bins from the angle.  Otherwise (ImageArgs): Pix frames of C strided channels read in place, nearest-bin or (BIL)
+// bilinear orientations.  The weights and S3-S7 are the same code for all three.
 template <int KT, bool STAGED, class Pix, bool BIL, class Args>
 __device__ __forceinline__ void hog_dense_cta(const Args& a, const CUtensorMap* map)
 {
+    // The pixels that vote: those in [E, W - 1 - E] x [E, H - 1 - E].  A gradient needs its neighbours, so only interior pixels
+    // vote (hog.c:616-617); a polar field votes at every pixel of the frame (hog.c:770-780).
+    constexpr bool POLAR = std::is_same<Args, PolarArgs>::value;
+    constexpr int E = POLAR ? 0 : 1;
     extern __shared__ __align__(128) unsigned char smem[];
     const int K = KT > 0 ? KT : a.K;
     const int cs = a.cs, tile = a.tile, span = a.span, pitch = dense_pitch(a);
@@ -161,7 +215,15 @@ __device__ __forceinline__ void hog_dense_cta(const Args& a, const CUtensorMap* 
     const uint8_t* __restrict__ img;
     sd_hog_image fr;                                 // otherwise: the frame's descriptor
     const Pix* __restrict__ pimg;
-    if constexpr (STAGED) {
+    const float* __restrict__ pmod;                  // POLAR: the frame's modulus and angle fields
+    const float* __restrict__ pang;
+    if constexpr (POLAR) {
+        fr = a.frames ? a.frames[f] : a.frame;
+        const long long e0 = a.frames ? fr.offset : fr.offset + (long long)f * a.image_stride;
+        pmod = a.modulus + e0;
+        pang = a.angle + e0;
+        W = fr.width; H = fr.height;
+    } else if constexpr (STAGED) {
         W = a.width; H = a.height; rs = a.row_stride;
         img = a.images + (long long)f * a.image_stride;
         if (a.frames) {
@@ -187,6 +249,10 @@ __device__ __forceinline__ void hog_dense_cta(const Args& a, const CUtensorMap* 
     // [cs hx0 - cs / 2 - 3 / 2, cs hx1 + 3 cs / 2 + 1 / 2].  STAGED stages [cs hx0 - cs - 1, cs hx1 + 2 cs] (span
     // cs (tile + 4) + 2); staged column i is frame column ox0 + i, at byte shift + i of its row.  Frames read in place keep per-pixel
     // values for the tightest region, ox0 = cs hx0 - floor(cs / 2) - 2 with span cs (tile + 3) + 4: 132 wide at cs 32.
+    // A polar field needs no neighbours, so the same region holds every pixel that votes into hx0..hx1, border pixels included:
+    // since hx1 <= hx0 + tile + 1, the voting pixels lie in [cs hx0 - cs / 2 - 1 / 2, cs hx0 + cs tile + 5 cs / 2 - 1 / 2), and
+    // [ox0, ox0 + span - 1] = [cs hx0 - floor(cs / 2) - 2, cs hx0 + cs tile + 3 cs - floor(cs / 2) + 1] contains it with at least
+    // one pixel to spare on each side.  Region columns outside the frame (x < 0 or x > W - 1) are left out by the voting range.
     const int ox0 = STAGED ? cs * hx0 - cs - 1 : cs * hx0 - cs / 2 - 2, oy0 = STAGED ? cs * hy0 - cs - 1 : cs * hy0 - cs / 2 - 2;
 
     if constexpr (STAGED) {
@@ -232,6 +298,31 @@ __device__ __forceinline__ void hog_dense_cta(const Args& a, const CUtensorMap* 
                     s_g[y * span + x] = g;
                 }
         }
+    } else if constexpr (POLAR) {
+        dense_weights(tid, cs, span, ox0, oy0, s_bx, s_wx1, s_wx2, s_by, s_wy1, s_wy2);
+        // ---- S2 (hog.c:770-800): per pixel of the frame, the modulus and the bin(s) of the angle (polar_bins); a modulus <= 0
+        //      does not vote (a NaN modulus does, as in hog.c)
+        const long long prs = fr.row_stride, pps = fr.pixel_stride;
+        const int period = a.directed ? 2 * K : K;
+        const int xa = max(E, E - ox0), xb = min(span - 1 - E, W - 1 - E - ox0);
+        const int ya = max(E, E - oy0), yb = min(span - 1 - E, H - 1 - E - oy0);
+        const int nx = xb - xa + 1;
+        if (nx > 0)
+            for (int i = tid; i < nx * (yb - ya + 1); i += kDenseThreads) {
+                const int r = i / nx;
+                const int y = ya + r, x = xa + i - r * nx;
+                const long long e = (long long)(oy0 + y) * prs + (long long)(ox0 + x) * pps;
+                const float m = __ldg(pmod + e);
+                int b1 = -1;
+                float w1 = 0.f;
+                const int b0 = polar_bins<BIL>(__ldg(pang + e), a.pi_k, period, &b1, &w1);
+                s_bin[y * span + x] = (int8_t)(m <= 0.f ? -1 : b0);
+                if constexpr (BIL) {
+                    s_bin1[y * span + x] = (int8_t)b1;
+                    s_w1[y * span + x] = w1;
+                }
+                s_g[y * span + x] = m;
+            }
     } else {
         dense_weights(tid, cs, span, ox0, oy0, s_bx, s_wx1, s_wx2, s_by, s_wy1, s_wy2);
         // ---- S2 (hog.c:631-682): per interior pixel, the gradient of every channel in ascending order, in float; a channel
@@ -283,11 +374,12 @@ __device__ __forceinline__ void hog_dense_cta(const Args& a, const CUtensorMap* 
     if (tid < ncell) {
         const int cyl = tid / nhx, cxl = tid - cyl * nhx;
         const int ci = hx0 + cxl, cj = hy0 + cyl;
-        // the interior pixels of the frame that vote into column ci / row cj: a contiguous run of staged coordinates
+        // the pixels of the frame that vote (interior, or every one for POLAR) into column ci / row cj: a contiguous run of
+        // staged coordinates
         int xlo = span, xhi = -1, ylo = span, yhi = -1;
-        for (int i = max(1, 1 - ox0); i <= min(span - 2, W - 2 - ox0); ++i)
+        for (int i = max(E, E - ox0); i <= min(span - 1 - E, W - 1 - E - ox0); ++i)
             if (s_bx[i] == ci || s_bx[i] == ci - 1) { xlo = min(xlo, i); xhi = i; }
-        for (int i = max(1, 1 - oy0); i <= min(span - 2, H - 2 - oy0); ++i)
+        for (int i = max(E, E - oy0); i <= min(span - 1 - E, H - 1 - E - oy0); ++i)
             if (s_by[i] == cj || s_by[i] == cj - 1) { ylo = min(ylo, i); yhi = i; }
         float* T = s_T + tid;
         float* hist = s_hist + tid;
@@ -299,7 +391,7 @@ __device__ __forceinline__ void hog_dense_cta(const Args& a, const CUtensorMap* 
             for (int x = xlo; x <= xhi; ++x) {
                 const int b = bp[x];
                 // b < 0: zero gradient (the patch kernel adds its +0 to bin 0, which changes nothing), or K = 1 on the gx = 0
-                // axis, which the reference does not vote
+                // axis, which the reference does not vote; or a polar pixel with a modulus <= 0 or a non-finite ho
                 if (b < 0) continue;
                 const float w = s_bx[x] == ci ? s_wx1[x] : s_wx2[x];
                 float* q = T + b * hs;
@@ -369,7 +461,14 @@ __global__ void __launch_bounds__(kDenseThreads, 2) hog_images_kernel(const __gr
     hog_dense_cta<KT, false, Pix, BIL>(a, nullptr);
 }
 
+template <int KT, bool BIL>
+__global__ void __launch_bounds__(kDenseThreads, 2) hog_polar_kernel(const __grid_constant__ PolarArgs a)
+{
+    hog_dense_cta<KT, false, float, BIL>(a, nullptr);
+}
+
 typedef void (*ImagesKernel)(ImageArgs);
+typedef void (*PolarKernel)(PolarArgs);
 
 template <class Pix, bool BIL>
 ImagesKernel images_kernel(int K)
@@ -377,13 +476,20 @@ ImagesKernel images_kernel(int K)
     return K == 4 ? hog_images_kernel<4, Pix, BIL> : K == 9 ? hog_images_kernel<9, Pix, BIL> : hog_images_kernel<0, Pix, BIL>;
 }
 
+template <bool BIL>
+PolarKernel polar_kernel(int K)
+{
+    return K == 4 ? hog_polar_kernel<4, BIL> : K == 9 ? hog_polar_kernel<9, BIL> : hog_polar_kernel<0, BIL>;
+}
+
 // Tile side of hog_images_kernel.  Nearest-bin: dense_tile's, as the 8-bit grey kernel.  Bilinear orientations hold 10 B per
 // pixel, twice the nearest-bin figure, so at dense_tile's side a CTA of cs 8 takes 120 KB and only one fits on an SM, with
 // (T + 2)^2 = 121 threads busy in S3.  There the tile with the most output cells in flight per SM, resident CTAs x T^2, wins
 // (one thread per histogram cell walks all of its cell's pixels in S3, so a CTA takes about as long at any T): measured 25-35 %
 // faster at cs 4 and 8 (DESIGN 4.9).  The same rule for nearest-bin frames chose T = 12 at two CTAs over T = 9 at three at
-// cs 8, which measured 8-13 % slower.
-int images_tile(ImagesKernel kern, int cs, int K, bool bil)
+// cs 8, which measured 8-13 % slower.  hog_polar_kernel keeps the same per-pixel state and takes the same rule.
+template <class Args>
+int images_tile(void (*kern)(Args), int cs, int K, bool bil)
 {
     if (!bil) return dense_tile(cs);
     int best = 1, most = 0;
@@ -598,6 +704,55 @@ int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size,
 
     const DenseSmem lay = dense_smem_layout(a.span, 0, num_bins, dense_cells(a.tile), bil);
     return launch_dense(ctx, __func__, "hog_images_kernel", kern, a, count, max_w, max_h, lay.total);
+}
+
+int sd_hog_dense_polar(sd_ctx* ctx, const sd_hog_polar_fields* fields, int cell_size, int num_bins, int variant, int directed,
+                       int bilinear_orientations, float* d_out, const int64_t* d_out_offset)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, fields && d_out, "null argument");
+    SD_REQUIRE(ctx, directed == 0 || directed == 1, "directed must be 0 or 1");
+    SD_REQUIRE(ctx, bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
+    SD_REQUIRE(ctx, variant == 0 || variant == 1, "unknown HOG variant");
+    SD_REQUIRE(ctx, num_bins >= 1 && num_bins <= SD_MAX_BINS, "num_bins must be in [1,16]");
+    SD_REQUIRE(ctx, cell_size >= 1 && cell_size <= kDenseMaxCell, "cell_size must be in [1,32]");
+    SD_REQUIRE(ctx, fields->count >= 0, "negative field count");
+    const int count = fields->count;
+    if (count == 0) return SD_OK;
+    SD_REQUIRE(ctx, fields->d_modulus && fields->d_angle, "null argument");
+    SD_REQUIRE(ctx, ((reinterpret_cast<uintptr_t>(fields->d_modulus) | reinterpret_cast<uintptr_t>(fields->d_angle)) & 3) == 0,
+               "fields must be 4-byte aligned");
+
+    int max_w = 0, max_h = 0, dd = 0;
+    if (fields->d_frames) {
+        const int rc = read_frames(ctx, __func__, fields->d_frames, count, cell_size, num_bins, variant, d_out_offset, &max_w,
+                                   &max_h, &dd);
+        if (rc) return rc;
+    } else {
+        SD_REQUIRE(ctx, image_ok(fields->frame, cell_size, num_bins, variant, &max_w, &max_h, &dd) && fields->image_stride >= 0,
+                   "fields must be wider and taller than 3 px and at least half a cell, with non-negative offset and strides");
+    }
+
+    PolarArgs a;
+    memset(&a, 0, sizeof(a));
+    a.modulus = fields->d_modulus;
+    a.angle = fields->d_angle;
+    a.frame = fields->frame;
+    a.image_stride = fields->image_stride;
+    a.frames = fields->d_frames;
+    a.directed = directed;
+    a.out = d_out;
+    a.out_offset = d_out_offset;
+    a.out_stride = (long long)dd * max_w * max_h;
+    a.variant = variant; a.cs = cell_size; a.K = num_bins; a.dd = dd;
+    const bool bil = bilinear_orientations != 0;
+    const PolarKernel kern = bil ? polar_kernel<true>(num_bins) : polar_kernel<false>(num_bins);
+    a.tile = images_tile(kern, cell_size, num_bins, bil);
+    a.span = cell_size * (a.tile + 3) + 4;
+    a.pi_k = 3.141592653589793 / (double)num_bins;    // angleStep = VL_PI / numOrientations (hog.c:756)
+
+    const DenseSmem lay = dense_smem_layout(a.span, 0, num_bins, dense_cells(a.tile), bil);
+    return launch_dense(ctx, __func__, "hog_polar_kernel", kern, a, count, max_w, max_h, lay.total);
 }
 
 }  // extern "C"

@@ -311,4 +311,71 @@ inline std::vector<cv::Mat> vl_hog(const std::vector<std::vector<cv::Mat>>& fram
     return out;
 }
 
+// VLFeat HOG of gradient fields the caller computed (vl_hog_new(variant, num_bins),
+// vl_hog_set_use_bilinear_orientation_assignments(bilinear_orientations), vl_hog_put_polar_field(modulus, angle, directed,
+// cell_size), vl_hog_extract), in one batched call on the device (sd_hog_dense_polar): e.g. the gradient of another operator, or
+// the magnitude and direction of an optical flow.  modulus[i] and angle[i] are CV_32FC1 planes of one size (row steps allowed);
+// fields may differ in size.  Angles in radians, taken modulo 2 pi (directed) or pi; every pixel votes, the border included,
+// except where the modulus is <= 0 or the angle is not finite.  Returns what rcr::vl_hog returns: one CV_32FC1 Mat per field with
+// dd * hogH rows and hogW columns.  Throws std::runtime_error for pairs of different sizes, other types, or fields or a
+// configuration that sd_hog_dense_polar refuses.
+inline std::vector<cv::Mat> vl_hog_polar(const std::vector<cv::Mat>& modulus, const std::vector<cv::Mat>& angle, VlHogVariant variant,
+                                         int cell_size, int num_bins, bool directed = true, bool bilinear_orientations = false)
+{
+    std::vector<cv::Mat> out;
+    if (modulus.size() != angle.size()) throw std::runtime_error("vl_hog_polar: modulus and angle must hold the same number of fields");
+    if (modulus.empty()) return out;
+    const int n = static_cast<int>(modulus.size());
+    std::vector<sd_hog_image> desc(n);
+    std::vector<int64_t> offset(n);
+    std::vector<int> rows(n), cols(n);
+    int64_t elems = 0, total = 0;
+    for (int i = 0; i < n; ++i) {
+        const cv::Mat& m = modulus[i];
+        const cv::Mat& a = angle[i];
+        if (m.type() != CV_32FC1 || a.type() != CV_32FC1) throw std::runtime_error("vl_hog_polar: fields must be CV_32FC1");
+        if (m.cols != a.cols || m.rows != a.rows)
+            throw std::runtime_error("vl_hog_polar: the modulus and angle of field " + std::to_string(i) + " differ in size");
+        const int W = m.cols, H = m.rows;
+        int w = 0, h = 0, dd = 0;
+        if (sd_hog_dense_shape(W, H, cell_size, num_bins, variant, &w, &h, &dd) != SD_OK)
+            throw std::runtime_error("vl_hog_polar: field " + std::to_string(i) + " (" + std::to_string(W) + " x " + std::to_string(H) +
+                                     ") or the configuration is invalid: fields wider and taller than 3 px and at least half a cell, "
+                                     "cell_size 1..32, num_bins 1..16");
+        desc[i].width = W;
+        desc[i].height = H;
+        desc[i].offset = elems;
+        desc[i].row_stride = W;
+        desc[i].pixel_stride = 1;
+        desc[i].channel_stride = 0;
+        elems += static_cast<int64_t>(W) * H;
+        offset[i] = total;
+        rows[i] = dd * h;
+        cols[i] = w;
+        total += static_cast<int64_t>(dd) * h * w;
+    }
+    sd_ctx* ctx = sd_b200::context();
+    sd_b200::DeviceBuffer d_mod(static_cast<size_t>(elems) * sizeof(float)), d_ang(static_cast<size_t>(elems) * sizeof(float)),
+        d_desc(static_cast<size_t>(n) * sizeof(sd_hog_image)), d_out(static_cast<size_t>(total) * sizeof(float)),
+        d_offset(static_cast<size_t>(n) * sizeof(int64_t));
+    for (int i = 0; i < n; ++i) {
+        const size_t row_bytes = static_cast<size_t>(desc[i].width) * sizeof(float);
+        sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, d_mod.as<float>() + desc[i].offset, row_bytes, modulus[i].ptr<unsigned char>(0),
+                                            modulus[i].step(), row_bytes, static_cast<size_t>(desc[i].height)), "vl_hog_polar upload");
+        sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, d_ang.as<float>() + desc[i].offset, row_bytes, angle[i].ptr<unsigned char>(0),
+                                            angle[i].step(), row_bytes, static_cast<size_t>(desc[i].height)), "vl_hog_polar upload");
+    }
+    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_desc.as<sd_hog_image>(), desc.data(), static_cast<size_t>(n) * sizeof(sd_hog_image)), "vl_hog_polar upload");
+    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_offset.as<int64_t>(), offset.data(), static_cast<size_t>(n) * sizeof(int64_t)), "vl_hog_polar");
+    sd_hog_polar_fields fields{};
+    fields.d_modulus = d_mod.as<float>();
+    fields.d_angle = d_ang.as<float>();
+    fields.count = n;
+    fields.d_frames = d_desc.as<sd_hog_image>();
+    sd_b200::check(ctx, sd_hog_dense_polar(ctx, &fields, cell_size, num_bins, variant, directed ? 1 : 0, bilinear_orientations ? 1 : 0,
+                                           d_out.as<float>(), d_offset.as<int64_t>()), "sd_hog_dense_polar");
+    for (int i = 0; i < n; ++i) out.push_back(sd_b200::download(d_out.as<float>() + offset[i], rows[i], cols[i], cols[i]));
+    return out;
+}
+
 }  // namespace rcr
