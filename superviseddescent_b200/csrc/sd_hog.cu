@@ -2,8 +2,9 @@
 // (reference include/rcr/adaptive_vlhog.hpp:109-185) fused with VLFeat's vl_hog_put_image /
 // vl_hog_extract (reference include/rcr/hog.c:595-728, :857-1062).
 //
-// One CTA per (sample, landmark) patch.  Everything between the 8-bit source image in HBM and the
-// feature row in HBM lives in shared memory:
+// hog_patch_kernel: one CTA per (sample, landmark) patch, from the 8-bit source image in HBM to the patch's cell histograms,
+// which it leaves in its slice of the feature row; hog_normalise_kernel, several patches per CTA, turns them into the
+// features in place (the last four steps below):
 //   geometry (IED -> half patch size, cvRound centre)            adaptive_vlhog.hpp:123,132-133
 //   zero-padded crop: ONE TMA tile load per patch (3-D tensor map over the frame batch; out-of-frame
 //     bytes are zero-filled by the TMA = copyMakeBorder(BORDER_CONSTANT 0))   adaptive_vlhog.hpp:135-151
@@ -23,6 +24,7 @@
 #include "sd_hog_common.cuh"
 
 #include <cmath>
+#include <cuda_pipeline.h>
 
 namespace {
 
@@ -128,29 +130,20 @@ __global__ void hog_bintab_kernel(int fs, int nc, int cs, float* __restrict__ bt
 
 // shared-memory carve-up (same function on host and device)
 struct HogSmem {
-    int patch, bin, r1, xofs, yofs0, yofs1, xa, yb, wcell, lo, hi, hist, energy, fac, vote, feat, mbar, stage_end, total;
+    int patch, bin, r1, xofs, yofs0, yofs1, xa, yb, wcell, lo, hi, vote, mbar, stage_end, total;
     int tpad;      // tasks of the horizontal vote pass, padded to a multiple of 32
 };
 
 __host__ __device__ inline int align_up(int v, int a) { return (v + a - 1) / a * a; }
 
-// Regions whose lifetimes do not overlap share storage, so that more CTAs fit on an SM:
-//   patch  (S1-S2)  then  hist, energy, fac (S3-S6)
-//   vote   (S3)     then  feat (S6-S8)
-//   r1: gradient modulus (S2-S3), then the clamped hc values (S6-S7)
-// and [bin | r1 | vote/feat] is dead during S1, so that whole span is the staging area of the source window.
-__host__ __device__ inline HogSmem hog_smem_layout(int fs, int nc, int K, int dd)
+// [bin | r1 | vote] is dead during S1, so that whole span is the staging area of the source window.  The cell histograms
+// go from the vote's second pass straight to global memory (hog_normalise_kernel takes them from there).
+__host__ __device__ inline HogSmem hog_smem_layout(int fs, int nc, int K)
 {
     HogSmem s;
-    const int cells = nc * nc;
     int o = 0;
     s.patch = o;
-    s.hist = o;
-    s.energy = align_up(s.hist + cells * 2 * K * 4, 16);
-    s.fac = align_up(s.energy + cells * 4, 16);
-    o = s.fac + cells * 4 * 8;
-    if (fs * fs > o) o = fs * fs;
-    o = align_up(o, 16);
+    o = align_up(fs * fs, 16);
     s.xofs = o;   o += fs * 4;
     s.yofs0 = o;  o += fs * 4;
     s.yofs1 = o;  o += fs * 4;
@@ -162,15 +155,10 @@ __host__ __device__ inline HogSmem hog_smem_layout(int fs, int nc, int K, int dd
     s.mbar = align_up(o, 8); o = s.mbar + 8;
     o = align_up(o, 128);
     s.bin = o;    o = align_up(o + fs * fs, 16);            // staging area from here to stage_end (128-byte aligned: TMA destination)
-    int r1 = fs * fs * 4;                                   // r1 = gradient modulus, later the clamped hc values (double)
-    if (cells * K * 32 > r1) r1 = cells * K * 32;
-    s.r1 = o;     o = align_up(o + r1, 16);
+    s.r1 = o;     o = align_up(o + fs * fs * 4, 16);        // r1 = gradient modulus
     s.tpad = align_up((fs - 2) * nc, 32);
     s.vote = o;                                             // horizontal pass of the vote: T[bin][(cell column, row)]
-    s.feat = o;
-    int vote = 2 * K * s.tpad * 4;
-    if (cells * dd * 4 > vote) vote = cells * dd * 4;
-    o += vote;
+    o += 2 * K * s.tpad * 4;
     s.stage_end = o;
     s.total = align_up(o, 16);
     return s;
@@ -185,20 +173,20 @@ constexpr int kTmaClasses = 8;
 __host__ __device__ constexpr int hog_tma_box(int c) { return c == 0 ? 32 : c == 1 ? 48 : c == 2 ? 64 : c == 3 ? 80 : c == 4 ? 96 : c == 5 ? 112 : c == 6 ? 128 : 160; }
 struct HogMaps { CUtensorMap m[kTmaClasses]; };
 
+// The compiled-in schedules fit 32 registers without spills, so an SM holds 8 CTAs where shared memory allows; the run-time
+// ones spill at that bound and keep the compiler's choice (a minimum of 0 CTAs per SM sets no bound).
 template <int KT, int NCT, int CST>
-__global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const __grid_constant__ HogArgs a, const __grid_constant__ HogMaps maps)
+__global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel(const __grid_constant__ HogArgs a, const __grid_constant__ HogMaps maps)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     const int K = KT > 0 ? KT : a.K;
     const int nc = NCT > 0 ? NCT : a.nc;
     const int fs = (NCT > 0 && CST > 0) ? NCT * CST : a.fs;
-    const int dd = a.dd;
     const int cells = nc * nc;
-    const HogSmem lay = hog_smem_layout(fs, nc, K, dd);
+    const HogSmem lay = hog_smem_layout(fs, nc, K);
     uint8_t* s_patch = smem + lay.patch;
     int8_t* s_bin = reinterpret_cast<int8_t*>(smem + lay.bin);
     float* s_gmag = reinterpret_cast<float*>(smem + lay.r1);
-    double* s_hc = reinterpret_cast<double*>(smem + lay.r1);
     int* s_xofs = reinterpret_cast<int*>(smem + lay.xofs);
     int* s_yofs0 = reinterpret_cast<int*>(smem + lay.yofs0);
     int* s_yofs1 = reinterpret_cast<int*>(smem + lay.yofs1);
@@ -207,11 +195,7 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const __grid_con
     float* s_wcell = reinterpret_cast<float*>(smem + lay.wcell);
     int* s_lo = reinterpret_cast<int*>(smem + lay.lo);
     int* s_hi = reinterpret_cast<int*>(smem + lay.hi);
-    float* s_hist = reinterpret_cast<float*>(smem + lay.hist);
-    float* s_energy = reinterpret_cast<float*>(smem + lay.energy);
-    double* s_fac = reinterpret_cast<double*>(smem + lay.fac);
     float* s_T = reinterpret_cast<float*>(smem + lay.vote);
-    float* s_feat = reinterpret_cast<float*>(smem + lay.feat);
     uint64_t* s_mbar = reinterpret_cast<uint64_t*>(smem + lay.mbar);
 
     const int tid = threadIdx.x;
@@ -434,6 +418,7 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const __grid_con
             a.bins[patch_id * fs * fs + idx] = interior ? s_bin[idx] : (int8_t)-1;
         }
     }
+    if (!a.A) return;                                             // sd_hog_debug: geometry, patches and bins only
     __syncthreads();
 
     // ---- S3: bilinear spatial vote (hog.c:697-724), separable:  hist[b][cj][ci] = sum_y wy[cj][y] * ( sum_x wx[ci][x] * g[y][x] * [bin[y][x] == b] ).
@@ -462,6 +447,9 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const __grid_con
         // Only the ntask columns that pass 1 cleared and filled are read here: hog_bintab_kernel keeps lo and hi inside the
         // interior [1, fs - 2], so rows ylo..yhi stay in column block ci.  The padding columns [ntask, tpad) still hold bytes
         // of the staged window (they were not cleared) and must never be read.
+        // The histogram hist[b * cells + c] goes to the first 2K cells floats of this landmark's slice of the feature row
+        // (which holds cells * dd >= 3K cells floats), where hog_normalise_kernel turns it into the features.
+        float* __restrict__ out = a.A + (long long)sample * a.ld + (long long)lm * cells * a.dd;
         for (int i = tid; i < 2 * K * cells; i += kHogThreads) {
             const int b = i / cells, c = i - b * cells;
             const int cj = c / nc, ci = c - cj * nc;                  // cell row (y), cell column (x)
@@ -470,57 +458,80 @@ __global__ void __launch_bounds__(kHogThreads) hog_patch_kernel(const __grid_con
             const float* wy = s_wcell + cj * fs + ylo;
             float acc = 0.f;
             for (int y = ylo; y <= yhi; ++y) acc = __fadd_rn(acc, __fmul_rn(*Tp++, *wy++));
-            s_hist[b * cells + c] = acc;
+            out[i] = acc;
         }
     }
-    __syncthreads();
+}
 
-    // ---- S4: undirected cell energy (hog.c:875-890) -------------------------------------------
-    for (int c = tid; c < cells; c += kHogThreads) s_energy[c] = hog_cell_energy(s_hist + c, cells, K);
-    __syncthreads();
+// ---- S4-S8 of a batch of patches whose cell histograms hog_patch_kernel left in their feature slices: undirected cell
+//      energy (hog.c:875-890), the block factors in double (hog.c:930-982), then per cell normalise, clamp at 0.2, project
+//      and texture sums (hog_cell_features, hog.c:985-1053), stored per dimension transposed (adaptive_vlhog.hpp:168-174)
+//      over the same slice, and the bias (:182-183).  `per_cta` patches per CTA, one thread per (patch, cell).  The factor
+//      of a block (a square root and a division in double) is computed once per block, (nc + 1)^2 of them per patch, not
+//      once for each of the up to four cells that use it, and the energies are widened to double once per cell.  Each CTA reads its
+//      patches' whole histograms into shared memory before a barrier and writes features only after it, so the in-place
+//      update is safe; slices start at any float offset (ld is any value >= D), so the loads and stores are scalar.
+struct NormArgs {
+    float* A;
+    long long ld;
+    int N, L, nc, K, dd, variant, per_cta;
+};
 
-    // ---- S5: the four block factors of each cell, in double (hog.c:930-982) ------------------
-    for (int i = tid; i < cells * 4; i += kHogThreads) {
-        const int c = i >> 2, f = i & 3;
-        const int y = c / nc, x = c - y * nc;
-        const int xm = max(x - 1, 0), xp = min(x + 1, nc - 1);
-        const int ym = max(y - 1, 0), yp = min(y + 1, nc - 1);
-        const int xa = (f & 1) ? x : xm, xb = (f & 1) ? xp : x;
-        const int ya = (f & 2) ? y : ym, yb = (f & 2) ? yp : y;
-        s_fac[i] = hog_block_factor(s_energy, nc, xa, xb, ya, yb);
+// per patch: slice offset, histograms, energies (double), block factors (double)
+__host__ __device__ inline int hog_norm_smem(int nc, int K, int per_cta)
+{
+    const int cells = nc * nc;
+    return per_cta * (8 + 2 * K * cells * 4 + cells * 8 + (nc + 1) * (nc + 1) * 8);
+}
+
+template <int KT>
+__global__ void __launch_bounds__(kHogThreads) hog_normalise_kernel(const NormArgs a)
+{
+    extern __shared__ __align__(16) unsigned char s_norm[];
+    const int K = KT > 0 ? KT : a.K;
+    const int nc = a.nc, nb = nc + 1, cells = nc * nc, blocks = nb * nb, hsz = 2 * K * cells, per_lm = cells * a.dd;
+    const long long first = (long long)blockIdx.x * a.per_cta;
+    const int np = (int)min((long long)a.per_cta, (long long)a.N * a.L - first);
+    long long* s_slice = reinterpret_cast<long long*>(s_norm);   // [patch] offset of its slice in A
+    double* s_energy = reinterpret_cast<double*>(s_slice + a.per_cta);   // [patch][cells]
+    double* s_fac = s_energy + a.per_cta * cells;                 // [patch][block row jy][block column jx]
+    float* s_hist = reinterpret_cast<float*>(s_fac + a.per_cta * blocks);   // [patch][2K][cells]
+    for (int p = threadIdx.x; p < np; p += kHogThreads) {
+        const long long id = first + p;
+        const int sample = (int)(id / a.L), lm = (int)(id - (long long)sample * a.L);
+        s_slice[p] = (long long)sample * a.ld + (long long)lm * per_lm;
+        if (lm == 0) a.A[(long long)sample * a.ld + (long long)a.L * per_lm] = 1.0f;   // bias, outside every slice
     }
     __syncthreads();
-
-    // ---- S6: normalise, clamp at 0.2, project (hog.c:985-1044); s_gmag is dead, reuse as s_hc -
-    for (int i = tid; i < cells * K; i += kHogThreads) {
-        const int k = i / cells, c = i - k * cells;
-        const int cj = c / nc, ci = c - cj * nc;
-        const int oc = ci * nc + cj;                        // per-dimension transpose, adaptive_vlhog.hpp:168-174
-        hog_project(s_fac + c * 4, (double)s_hist[k * cells + c], (double)s_hist[(k + K) * cells + c], k, K, a.variant,
-                    [=](int f, double hc) { s_hc[(c * K + k) * 4 + f] = hc; },
-                    [=](int d, float v) { s_feat[d * cells + oc] = v; });
+    // asynchronous copies: every load of a thread is in flight at once (a load-then-store loop waits out the latency of
+    // each one in turn, which took most of this kernel's time)
+    for (int i = threadIdx.x; i < np * hsz; i += kHogThreads) {
+        const int p = i / hsz;
+        __pipeline_memcpy_async(s_hist + i, a.A + s_slice[p] + (i - p * hsz), sizeof(float));
+    }
+    __pipeline_commit();
+    __pipeline_wait_prior(0);
+    __syncthreads();
+    for (int i = threadIdx.x; i < np * cells; i += kHogThreads) {
+        const int p = i / cells, c = i - p * cells;
+        s_energy[i] = (double)hog_cell_energy(s_hist + p * hsz + c, cells, K);
     }
     __syncthreads();
-
-    // ---- S7: texture dims = 1/sqrt(18) * sum_k hc_f, summed in ascending k (hog.c:1046-1053) -
-    if (a.variant == 1) {
-        for (int i = tid; i < cells * 4; i += kHogThreads) {
-            const int c = i >> 2, f = i & 3;
-            const int cj = c / nc, ci = c - cj * nc;
-            double t = 0.0;
-            for (int k = 0; k < K; ++k) t = __dadd_rn(t, s_hc[(c * K + k) * 4 + f]);
-            const float c18 = __fdiv_rn(1.0f, __fsqrt_rn(18.0f));
-            s_feat[(3 * K + f) * cells + ci * nc + cj] = (float)__dmul_rn((double)c18, t);
-        }
-        __syncthreads();
+    // block (jx, jy): cell columns max(jx - 1, 0) and min(jx, nc - 1), rows likewise.  Factor q of cell (x, y) is block
+    // (x + (q & 1), y + (q >> 1)), the block hog_cell_factors forms for it.
+    for (int i = threadIdx.x; i < np * blocks; i += kHogThreads) {
+        const int p = i / blocks, j = i - p * blocks;
+        const int jy = j / nb, jx = j - jy * nb;
+        s_fac[i] = hog_block_factor(s_energy + p * cells, nc, max(jx - 1, 0), min(jx, nc - 1), max(jy - 1, 0), min(jy, nc - 1));
     }
-
-    // ---- S8: coalesced write of this landmark's slice of the feature row ---------------------
-    if (a.A) {
-        const int per_lm = cells * dd;
-        float* __restrict__ out = a.A + (long long)sample * a.ld + (long long)lm * per_lm;
-        for (int i = tid; i < per_lm; i += kHogThreads) out[i] = s_feat[i];
-        if (lm == 0 && tid == 0) a.A[(long long)sample * a.ld + (long long)a.L * per_lm] = 1.0f;   // bias, :182-183
+    __syncthreads();
+    for (int i = threadIdx.x; i < np * cells; i += kHogThreads) {
+        const int p = i / cells, c = i - p * cells;
+        const int cj = c / nc, ci = c - cj * nc;                 // cell row (y), cell column (x)
+        const double* F = s_fac + p * blocks + cj * nb + ci;
+        const double fac[4] = {F[0], F[1], F[nb], F[nb + 1]};
+        float* __restrict__ out = a.A + s_slice[p] + ci * nc + cj;   // per-dimension transpose
+        hog_cell_features(fac, s_hist + p * hsz + c, cells, K, a.variant, [=](int d, float v) { out[d * cells] = v; });
     }
 }
 
@@ -570,8 +581,13 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
     a.A = d_A; a.ld = ld;
     if (d_A) SD_REQUIRE(ctx, ld >= (int64_t)L * a.nc * a.nc * a.dd + 1, "ld < feature length");
     // every argument check before the first launch: a rejected configuration queues no work
-    const HogSmem lay = hog_smem_layout(fs, a.nc, a.K, a.dd);
-    SD_REQUIRE(ctx, lay.total <= 227 * 1024, "HOG configuration needs more than 227 KB of shared memory");
+    const HogSmem lay = hog_smem_layout(fs, a.nc, a.K);
+    const int cells = a.nc * a.nc;
+    NormArgs na;
+    na.A = d_A; na.ld = ld; na.N = N; na.L = L; na.nc = a.nc; na.K = a.K; na.dd = a.dd; na.variant = a.variant;
+    na.per_cta = cells < kHogThreads ? kHogThreads / cells : 1;  // one thread per cell of the CTA's patches
+    const int norm_smem = hog_norm_smem(a.nc, a.K, na.per_cta);
+    SD_REQUIRE(ctx, lay.total <= 227 * 1024 && norm_smem <= 227 * 1024, "HOG configuration needs more than 227 KB of shared memory");
     const long long blocks = (long long)N * L;
     SD_REQUIRE(ctx, blocks < 2147483647LL, "too many patches for one launch");
     a.geometry = d_geometry; a.patches = d_patches; a.bins = d_bins;
@@ -619,6 +635,11 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
     // H100 80GB HBM3 at a 400 W power limit), since registers, not shared memory, bound the CTAs per SM at fs = 55 / 50 / 40.
     kern<<<(unsigned)blocks, kHogThreads, lay.total, ctx->stream>>>(a, maps);
     SD_LAUNCH_CHECK(ctx, "hog_patch_kernel");
+    if (!d_A) return SD_OK;
+    auto norm = a.K == 4 ? hog_normalise_kernel<4> : a.K == 9 ? hog_normalise_kernel<9> : hog_normalise_kernel<0>;
+    SD_CUDA(ctx, cudaFuncSetAttribute(norm, cudaFuncAttributeMaxDynamicSharedMemorySize, norm_smem));
+    norm<<<(unsigned)sd_div_up(blocks, na.per_cta), kHogThreads, norm_smem, ctx->stream>>>(na);
+    SD_LAUNCH_CHECK(ctx, "hog_normalise_kernel");
     return SD_OK;
 }
 

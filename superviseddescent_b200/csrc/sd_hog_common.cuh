@@ -168,8 +168,10 @@ __device__ __forceinline__ float hog_cell_energy(const float* hist, int stride, 
 }
 
 // ---- block factor in double (hog.c:930-982) of the 2 x 2 cells at columns xa, xb and rows ya, yb of the energies E (row
-//      stride ld).  factor1: n1+n2+n4+n5, factor2: n2+n3+n5+n6, factor3: n4+n5+n7+n8, factor4: n5+n6+n8+n9 --------------
-__device__ __forceinline__ double hog_block_factor(const float* E, int ld, int xa, int xb, int ya, int yb)
+//      stride ld; float, or the same values already widened to double).  factor1: n1+n2+n4+n5, factor2: n2+n3+n5+n6,
+//      factor3: n4+n5+n7+n8, factor4: n5+n6+n8+n9 ------------------------------------------------------------------------
+template <class T>
+__device__ __forceinline__ double hog_block_factor(const T* E, int ld, int xa, int xb, int ya, int yb)
 {
     double s = (double)E[xa + ya * ld];
     s = __dadd_rn(s, (double)E[xb + ya * ld]);
@@ -208,6 +210,40 @@ __device__ __forceinline__ void hog_project(const double* fac, double ha, double
     } else {                                            // Dalal-Triggs
 #pragma unroll
         for (int f = 0; f < 4; ++f) store(k + f * K, (float)hcv[f]);
+    }
+}
+
+// ---- the four block factors of the cell at column x, row y of a gw x gh cell grid (hog.c:930-982), from the energies E
+//      (E[(x - ex0) + (y - ey0) * lde]: a window of the grid that holds the cell's neighbours).  Factor q covers the block
+//      whose columns are (x - 1, x) for even q, (x, x + 1) for odd q, and rows (y - 1, y) for q < 2, (y, y + 1) above,
+//      clamped to the grid.
+__device__ __forceinline__ void hog_cell_factors(const float* E, int lde, int ex0, int ey0, int gw, int gh, int x, int y,
+                                                 double fac[4])
+{
+    const int xm = max(x - 1, 0), xp = min(x + 1, gw - 1);
+    const int ym = max(y - 1, 0), yp = min(y + 1, gh - 1);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const int xa = ((q & 1) ? x : xm) - ex0, xb = ((q & 1) ? xp : x) - ex0;
+        const int ya = ((q & 2) ? y : ym) - ey0, yb = ((q & 2) ? yp : y) - ey0;
+        fac[q] = hog_block_factor(E, lde, xa, xb, ya, yb);
+    }
+}
+
+// ---- the features of a cell from its four block factors (hog.c:985-1053): hog_project for k = 0..K-1 on its bins
+//      h[b * hs], and the texture dims 1/sqrt(18) * sum_k hc_f summed in ascending k (UoCTTI).  store(d, v) writes feature
+//      dimension d of the cell.
+template <class Store>
+__device__ __forceinline__ void hog_cell_features(const double* fac, const float* h, int hs, int K, int variant, Store store)
+{
+    double t[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int k = 0; k < K; ++k)
+        hog_project(fac, (double)h[k * hs], (double)h[(k + K) * hs], k, K, variant,
+                    [&](int q, double hc) { t[q] = __dadd_rn(t[q], hc); }, store);
+    if (variant == 1) {
+        const float c18 = __fdiv_rn(1.0f, __fsqrt_rn(18.0f));
+#pragma unroll
+        for (int q = 0; q < 4; ++q) store(3 * K + q, (float)__dmul_rn((double)c18, t[q]));
     }
 }
 

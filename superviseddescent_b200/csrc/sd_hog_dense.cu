@@ -424,28 +424,12 @@ __device__ __forceinline__ void hog_dense_cta(const Args& a, const CUtensorMap* 
     if (tid < tw * th) {
         const int yl = tid / tw;
         const int x = tx0 + tid - yl * tw, y = ty0 + yl;
-        const int xm = max(x - 1, 0), xp = min(x + 1, hogW - 1);
-        const int ym = max(y - 1, 0), yp = min(y + 1, hogH - 1);
-        double fac[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const int xa = ((q & 1) ? x : xm) - hx0, xb = ((q & 1) ? xp : x) - hx0;
-            const int ya = ((q & 2) ? y : ym) - hy0, yb = ((q & 2) ? yp : y) - hy0;
-            fac[q] = hog_block_factor(s_energy, nhx, xa, xb, ya, yb);
-        }
         const int c = (x - hx0) + (y - hy0) * nhx;
         const long long plane = (long long)hogW * hogH;
         float* __restrict__ out = a.out + (a.out_offset ? a.out_offset[f] : (long long)f * a.out_stride) + (long long)y * hogW + x;
-        double t[4] = {0.0, 0.0, 0.0, 0.0};
-        for (int k = 0; k < K; ++k)
-            hog_project(fac, (double)s_hist[k * hs + c], (double)s_hist[(k + K) * hs + c], k, K, a.variant,
-                        [&](int q, double hc) { t[q] = __dadd_rn(t[q], hc); },
-                        [=](int d, float v) { out[d * plane] = v; });
-        if (a.variant == 1) {
-            const float c18 = __fdiv_rn(1.0f, __fsqrt_rn(18.0f));
-#pragma unroll
-            for (int q = 0; q < 4; ++q) out[(3 * K + q) * plane] = (float)__dmul_rn((double)c18, t[q]);
-        }
+        double fac[4];
+        hog_cell_factors(s_energy, nhx, hx0, hy0, hogW, hogH, x, y, fac);
+        hog_cell_features(fac, s_hist + c, hs, K, a.variant, [=](int d, float v) { out[d * plane] = v; });
     }
 }
 
