@@ -280,6 +280,45 @@ typedef struct {
 SD_API int sd_hog_dense_polar(sd_ctx* ctx, const sd_hog_polar_fields* fields, int cell_size, int num_bins, int variant,
                               int directed, int bilinear_orientations, float* d_out, const int64_t* d_out_offset);
 
+/* ---- render, flip and transpose of planar HOG features: vl_hog_render, vl_hog_get_permutation (hog.c:225-312, :428-495) ----
+ * Features are VLFeat's planar layout [dd][h][w] of a grid of w x h cells (what the dense HOG calls above write), with dd and
+ * the variant as there.  A rendered grid is an image of h * 21 rows of w * 21 floats, row-major: cell (x, y) owns the 21 x 21
+ * tile at column 21 x, row 21 y.  sd_hog_permutation and sd_hog_glyphs are host only: the tables vl_hog_new builds. */
+#define SD_HOG_GLYPH_SIZE 21
+/* One grid of a batch: its features at d_features + offset, its result at d_out + out_offset (floats, non-negative). */
+typedef struct {
+    int32_t width, height;           /* cells, >= 1 */
+    int64_t offset, out_offset;
+} sd_hog_grid;
+/* A batch of grids on the device: equally sized (width x height cells; grid i's features at d_features + i * dd * h * w, its
+ * result packed the same way: i * h * w * 441 floats for a render, i * dd * h * w for a relayout), or -- d_grids != NULL --
+ * one device descriptor per grid (width and height are then ignored; the call reads the table back once). */
+typedef struct {
+    const float* d_features;
+    int32_t count;
+    int32_t width, height;
+    const sd_hog_grid* d_grids;
+} sd_hog_grids;
+/* sd_hog_permutation: writes the dd entries of vl_hog_get_permutation: the features of a left-right mirrored image are
+ * flipped[i] = features[perm[i]] at the mirrored cell.  sd_hog_glyphs: writes the num_bins x 21 x 21 glyphs of vl_hog_new
+ * (each value 0 or 1, glyph k row-major; transposed = 1 gives the column-major glyphs of a transposed VlHog).  Either returns
+ * SD_ERR_INVALID for a null pointer, num_bins outside [1, 16], or variant / transposed outside {0, 1}. */
+SD_API int sd_hog_permutation(int num_bins, int variant, int64_t* perm);
+SD_API int sd_hog_glyphs(int num_bins, int transposed, float* glyphs);
+/* sd_hog_render: vl_hog_render of every grid into d_image, asynchronous on the context's stream.  Read-modify-write, as hog.c
+ * adds into the caller's buffer: zero the image first for a fresh render.  Per cell, weight k is the sum of the orientation's 3
+ * (UoCTTI) or 4 (Dalal-Triggs) planes in hog.c's order; each pixel adds weight_k * glyph_k for k ascending in float without
+ * FMA and is then clamped to [min(0, weights), max(0, weights)] with hog.c's comparisons, so the image is bit for bit hog.c's
+ * (NaN included) for the same features and starting image.  transposed selects the glyphs of a transposed VlHog.  Null
+ * pointers, an invalid configuration, or a grid smaller than 1 x 1 or with a negative offset is SD_ERR_INVALID before any work
+ * is queued (d_image is not written). */
+SD_API int sd_hog_render(sd_ctx* ctx, const sd_hog_grids* grids, int num_bins, int variant, int transposed, float* d_image);
+/* sd_hog_relayout: a gather of every grid's planes into d_out, asynchronous on the context's stream, out of place (d_out must
+ * not overlap the input).  flip = 1: plane i of the result is plane perm[i] (sd_hog_permutation) with its columns mirrored,
+ * out[i][y][x] = in[perm[i]][y][w - 1 - x] -- the features of the left-right mirrored image.  transpose = 1: each (flipped)
+ * plane is then stored transposed, [w][h] -- the features of a transposed VlHog.  Validation as sd_hog_render. */
+SD_API int sd_hog_relayout(sd_ctx* ctx, const sd_hog_grids* grids, int num_bins, int variant, int flip, int transpose, float* d_out);
+
 /* ---- regressor: LinearRegressor<Solver> (regressors.hpp:318-400) ------------------------ */
 /* Solver::solve (regressors.hpp:199-234 == verbose_solver.hpp:53-111):
  *   X = (A^T A + Lambda)^-1 A^T B ;  A: N x D, B: N x M, X: D x M (ldx_out = M).

@@ -62,6 +62,17 @@ class HogPolarFieldsC(C.Structure):
                 ("image_stride", C.c_int64), ("d_frames", C.c_void_p)]
 
 
+class HogGridC(C.Structure):
+    """sd_hog_grid: one grid of planar features; offsets in floats."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("offset", C.c_int64), ("out_offset", C.c_int64)]
+
+
+class HogGridsC(C.Structure):
+    """sd_hog_grids: planar feature grids on the device, equally sized or one descriptor per grid."""
+    _fields_ = [("d_features", C.c_void_p), ("count", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
+                ("d_grids", C.c_void_p)]
+
+
 class HostFrameC(C.Structure):
     """sd_host_frame: one host frame of a detect call (8UC1, or 8UC3 interleaved B, G, R)."""
     _fields_ = [("h_data", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32), ("row_stride", C.c_int32), ("channels", C.c_int32)]
@@ -99,7 +110,7 @@ EXPORTS = [
     "sd_malloc", "sd_free", "sd_host_alloc", "sd_host_free", "sd_memcpy_h2d", "sd_memcpy_d2h", "sd_memset",
     "sd_memcpy2d_h2d", "sd_memcpy2d_d2h", "sd_memcpy2d_d2d",
     "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_bgr2gray", "sd_upload_frames", "sd_hog_dense_shape", "sd_hog_dense",
-    "sd_hog_dense_images", "sd_hog_dense_polar",
+    "sd_hog_dense_images", "sd_hog_dense_polar", "sd_hog_permutation", "sd_hog_glyphs", "sd_hog_render", "sd_hog_relayout",
     "sd_learn", "sd_centre_features", "sd_learn_centred", "sd_learn_rank_revealing", "sd_gram", "sd_solve_gram", "sd_predict", "sd_test_residual", "sd_solver_timings", "sd_set_gram_mode", "sd_set_solver", "sd_solver_iterations",
     "sd_set_rank_diagnostic", "sd_last_rank",
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",

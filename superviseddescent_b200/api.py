@@ -23,7 +23,7 @@ import torch
 
 from . import _capi
 from ._capi import HogParam as HoGParam  # same field names as rcr::HoGParam
-from ._capi import HogImageC, HogImagesC, HogPolarFieldsC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, ptr
+from ._capi import HogGridC, HogGridsC, HogImageC, HogImagesC, HogPolarFieldsC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, ptr
 
 
 def _check(ctx, rc: int) -> None:
@@ -1415,3 +1415,112 @@ def vl_hog_polar(modulus, angle, cell_size: int, num_bins: int, variant: int = 1
     out = torch.empty(int(sum(counts)), dtype=torch.float32, device=dev)
     _check(ctx.h, lib.sd_hog_dense_polar(ctx.h, C.byref(fb), *flags, ptr(out), ptr(offsets)))
     return [out[s:s + c].view(shape) for s, c, shape in zip(starts.tolist(), counts, shapes)]
+
+
+GLYPH_SIZE = 21     # SD_HOG_GLYPH_SIZE: pixels per side of a rendered cell (hog.c:183)
+
+
+def _hog_dims(num_bins: int, variant: int) -> int:
+    if variant not in (0, 1) or not 1 <= int(num_bins) <= 16:
+        raise ValueError(f"num_bins must be in 1..16 and variant 0 or 1 (got {num_bins}, {variant})")
+    return 3 * int(num_bins) + 4 if variant == 1 else 4 * int(num_bins)
+
+
+def vl_hog_permutation(variant: int, num_bins: int) -> np.ndarray:
+    """vl_hog_get_permutation of vl_hog_new(variant, num_bins): int64 array of dd entries with
+    flipped[i] = features[perm[i]] for the features of the left-right mirrored image.  Host only."""
+    dd = _hog_dims(num_bins, variant)
+    out = np.zeros(dd, np.int64)
+    _check(None, _capi.lib().sd_hog_permutation(int(num_bins), int(variant), C.c_void_p(out.ctypes.data)))
+    return out
+
+
+def vl_hog_glyphs(num_bins: int, transposed: bool = False) -> np.ndarray:
+    """The glyphs of vl_hog_new(.., num_bins, transposed): a (num_bins, 21, 21) float32 array of 0 and 1, glyph k at [k]
+    (row-major; transposed=True gives hog.c's column-major glyphs).  Host only."""
+    _hog_dims(num_bins, 1)
+    out = np.zeros((int(num_bins), GLYPH_SIZE, GLYPH_SIZE), np.float32)
+    _check(None, _capi.lib().sd_hog_glyphs(int(num_bins), int(bool(transposed)), C.c_void_p(out.ctypes.data)))
+    return out
+
+
+def _hog_grids(features, num_bins: int, variant: int, out_size, ctx: Context):
+    """(grids struct, device features kept alive, result shapes, result offsets or None, batched) for the planar features of
+    vl_hog_render / vl_hog_flip: a (B, dd, h, w) batch or a list of (dd, h, w) grids."""
+    dd = _hog_dims(num_bins, variant)
+    dev = f"cuda:{ctx.device}"
+
+    def tensor(a):
+        t = a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))
+        if t.dtype != torch.float32:
+            raise ValueError("features must be float32")
+        return t
+
+    g = HogGridsC()
+    g.d_grids = None
+    if isinstance(features, (list, tuple)):
+        grids = [tensor(f) for f in features]
+        if any(f.dim() != 3 or f.shape[0] != dd for f in grids):
+            raise ValueError(f"every grid must be (dd, h, w) with dd = {dd}")
+        sizes = [tuple(f.shape[1:]) for f in grids]
+        keep = torch.cat([f.reshape(-1) for f in grids]).to(dev) if grids else None
+        descs, pos, opos, offsets = [], 0, 0, []
+        for h, w in sizes:
+            descs.append(HogGridC(w, h, pos, opos))
+            offsets.append(opos)
+            pos += dd * h * w
+            opos += int(np.prod(out_size(h, w)))
+        g.count = len(grids)
+        table = (HogGridC * max(len(descs), 1))(*descs)
+        keep_table = torch.from_numpy(np.frombuffer(bytes(table), dtype=np.uint8).copy()).to(dev)
+        g.d_grids = keep_table.data_ptr()
+        g.d_features = keep.data_ptr() if keep is not None else None
+        return g, (keep, keep_table), [out_size(h, w) for h, w in sizes], offsets, False
+    t = tensor(features)
+    if t.dim() != 4 or t.shape[1] != dd:
+        raise ValueError(f"features must be (B, dd, h, w) with dd = {dd}, or a list of (dd, h, w) grids")
+    keep = t.to(dev).contiguous()
+    b, _, h, w = keep.shape
+    g.d_features, g.count, g.width, g.height = keep.data_ptr(), b, w, h
+    return g, (keep,), [(b,) + tuple(out_size(h, w))], None, True
+
+
+def _hog_result(ctx, shapes, offsets, batched, run, zero: bool):
+    """Allocates the results (one batch tensor, or one buffer viewed as the grids' shapes), runs run(buffer) and returns them."""
+    dev = f"cuda:{ctx.device}"
+    alloc = torch.zeros if zero else torch.empty
+    if batched:
+        out = alloc(shapes[0], dtype=torch.float32, device=dev)
+        if out.shape[0]:
+            run(out)
+        return out
+    if not shapes:
+        return []
+    total = offsets[-1] + int(np.prod(shapes[-1]))
+    out = alloc(total, dtype=torch.float32, device=dev)
+    run(out)
+    return [out[o:o + int(np.prod(s))].view(s) for o, s in zip(offsets, shapes)]
+
+
+def vl_hog_render(features, num_bins: int, variant: int = 1, ctx: Optional[Context] = None):
+    """vl_hog_render of planar HOG features on the device (sd_hog_render): a (B, dd, h, w) batch, or a list of (dd, h, w)
+    grids of any sizes, each rendered into a fresh zeroed image of (h * 21, w * 21) floats -- cell (x, y) as the 21 x 21 glyph
+    tile at (21 y, 21 x), every orientation's bar weighted by the sum of its planes, clamped to the cell's weight range.
+    Returns a (B, h * 21, w * 21) float32 CUDA tensor, or a list of (h * 21, w * 21) tensors."""
+    ctx = ctx or default_context()
+    g, keep, shapes, offsets, batched = _hog_grids(features, num_bins, variant, lambda h, w: (h * GLYPH_SIZE, w * GLYPH_SIZE), ctx)
+    lib = _capi.lib()
+    return _hog_result(ctx, shapes, offsets, batched, lambda out: _check(ctx.h, lib.sd_hog_render(
+        ctx.h, C.byref(g), int(num_bins), int(variant), 0, ptr(out))), zero=True)
+
+
+def vl_hog_flip(features, num_bins: int, variant: int = 1, ctx: Optional[Context] = None):
+    """Left-right flip of planar HOG features on the device (sd_hog_relayout): the features of the mirrored image,
+    out[i][y][x] = features[perm[i]][y][w - 1 - x] with perm = vl_hog_permutation(variant, num_bins).  features: a
+    (B, dd, h, w) batch or a list of (dd, h, w) grids; returns the same shapes as fresh CUDA tensors."""
+    ctx = ctx or default_context()
+    g, keep, shapes, offsets, batched = _hog_grids(features, num_bins, variant,
+                                                   lambda h, w: (_hog_dims(num_bins, variant), h, w), ctx)
+    lib = _capi.lib()
+    return _hog_result(ctx, shapes, offsets, batched, lambda out: _check(ctx.h, lib.sd_hog_relayout(
+        ctx.h, C.byref(g), int(num_bins), int(variant), 1, 0, ptr(out))), zero=False)
