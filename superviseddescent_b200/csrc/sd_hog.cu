@@ -28,8 +28,9 @@
 
 namespace {
 
+// CTA size of hog_normalise_kernel and of the run-time hog_patch_kernel schedules; the compiled-in schedules pick their
+// own (launch_hog)
 constexpr int kHogThreads = 256;
-constexpr int kHogWarps = kHogThreads / 32;
 
 struct HogArgs {
     const uint8_t* images;
@@ -173,11 +174,15 @@ constexpr int kTmaClasses = 8;
 __host__ __device__ constexpr int hog_tma_box(int c) { return c == 0 ? 32 : c == 1 ? 48 : c == 2 ? 64 : c == 3 ? 80 : c == 4 ? 96 : c == 5 ? 112 : c == 6 ? 128 : 160; }
 struct HogMaps { CUtensorMap m[kTmaClasses]; };
 
-// The compiled-in schedules fit 32 registers without spills, so an SM holds 8 CTAs where shared memory allows; the run-time
-// ones spill at that bound and keep the compiler's choice (a minimum of 0 CTAs per SM sets no bound).
-template <int KT, int NCT, int CST>
-__global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel(const __grid_constant__ HogArgs a, const __grid_constant__ HogMaps maps)
+// NT threads per CTA.  The compiled-in schedules fit 32 registers without spills, so an SM holds 2048 / NT CTAs where shared
+// memory allows; the run-time ones (NT = 256) spill at that bound and keep the compiler's choice (a minimum of 0 CTAs per SM
+// sets no bound).
+template <int KT, int NCT, int CST, int NT>
+__global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(const __grid_constant__ HogArgs a, const __grid_constant__ HogMaps maps)
 {
+    // whole warps, and at least one row group of the fs <= 64 resize (NT / fs >= 1)
+    static_assert(NT % 32 == 0 && NT >= 64, "hog_patch_kernel needs whole warps and at least 64 threads");
+    constexpr int kWarps = NT / 32;
     extern __shared__ __align__(128) unsigned char smem[];
     const int K = KT > 0 ? KT : a.K;
     const int nc = NCT > 0 ? NCT : a.nc;
@@ -261,7 +266,7 @@ __global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel
     // tables: cv::resize taps of this sample (hog_geometry_kernel), spatial binning weights of this launch (hog_bintab_kernel)
     {
         const int* __restrict__ rt = a.rtab + (long long)sample * 5 * fs;
-        for (int t = tid; t < fs; t += kHogThreads) {
+        for (int t = tid; t < fs; t += NT) {
             s_xofs[t] = __ldg(rt + t);
             const int xa = __ldg(rt + fs + t), yb = __ldg(rt + 4 * fs + t);
             s_xa[t] = *reinterpret_cast<const short2*>(&xa);
@@ -269,7 +274,7 @@ __global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel
             s_yofs1[t] = __ldg(rt + 3 * fs + t);
             s_yb[t] = *reinterpret_cast<const short2*>(&yb);
         }
-        for (int i = tid; i < nc * fs; i += kHogThreads) s_wcell[i] = __ldg(a.btab + i);
+        for (int i = tid; i < nc * fs; i += NT) s_wcell[i] = __ldg(a.btab + i);
         const int* __restrict__ lohi = reinterpret_cast<const int*>(a.btab + nc * fs);
         if (tid < nc) { s_lo[tid] = __ldg(lohi + tid); s_hi[tid] = __ldg(lohi + nc + tid); }
     }
@@ -292,19 +297,19 @@ __global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel
                 const int gs = nvec <= 8 ? 3 : (nvec <= 16 ? 4 : 5);
                 const int lv = lane & ((1 << gs) - 1), lr = lane >> gs, rows_per_pass = 32 >> gs;
                 const uint8_t* wrow = img + (long long)(y0 - ry) * rs + (x0 - rx - shiftb);
-                for (int r = warp * rows_per_pass + lr; r < P; r += kHogWarps * rows_per_pass)
+                for (int r = warp * rows_per_pass + lr; r < P; r += kWarps * rows_per_pass)
                     for (int v = lv; v < nvec; v += (1 << gs))
                         reinterpret_cast<uint4*>(s_stage + r * pitch)[v] = __ldg(reinterpret_cast<const uint4*>(wrow + (long long)r * rs) + v);
             } else if (words) {
                 const int nwords = (shiftb + P + 3) >> 2;
                 const uint8_t* wrow = img + (long long)(y0 - ry) * rs + (x0 - rx - shiftb);
-                for (int r = warp; r < P; r += kHogWarps) {
+                for (int r = warp; r < P; r += kWarps) {
                     const uint32_t* src = reinterpret_cast<const uint32_t*>(wrow + (long long)r * rs);
                     uint32_t* dst = reinterpret_cast<uint32_t*>(s_stage + r * pitch);
                     for (int w = lane; w < nwords; w += 32) dst[w] = __ldg(src + w);
                 }
             } else {
-                for (int r = warp; r < P; r += kHogWarps) {
+                for (int r = warp; r < P; r += kWarps) {
                     const int iy = y0 + r;
                     const bool rowin = (unsigned)iy < (unsigned)H;
                     const bool rowres = iy >= ry && iy < ry + rh;
@@ -322,15 +327,17 @@ __global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel
             __syncthreads();                                       // tables (and the load loops' stores) visible
             if (tma_box) hog_tma_wait(s_mbar);
             if (fs <= 64) {
-                // a thread keeps ONE output column (its two source taps and weights stay in registers) and walks down the rows
-                const int dx = tid & 63, g = tid >> 6;
-                if (dx < fs) {
+                // a thread keeps ONE output column (its two source taps and weights stay in registers) and walks down the rows:
+                // NT / fs row groups of fs threads, NT mod fs threads idle
+                const int groups = NT / fs;
+                const int dx = tid % fs, g = tid / fs;
+                if (g < groups) {
                     const int sx = s_xofs[dx];
                     const int sx1 = min(sx + 1, P - 1);            // clamped tap has zero weight
                     const int ax = s_xa[dx].x, bx = s_xa[dx].y;
                     const uint8_t* base = s_stage + shiftb;
 #pragma unroll 4
-                    for (int dy = g; dy < fs; dy += kHogThreads / 64) {
+                    for (int dy = g; dy < fs; dy += groups) {
                         const short2 yb = s_yb[dy];
                         const uint8_t* r0 = base + s_yofs0[dy] * pitch;
                         const uint8_t* r1 = base + s_yofs1[dy] * pitch;
@@ -341,7 +348,7 @@ __global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel
                     }
                 }
             } else {
-                for (int dy = warp; dy < fs; dy += kHogWarps) {
+                for (int dy = warp; dy < fs; dy += kWarps) {
                     const short2 yb = s_yb[dy];
                     const uint8_t* r0 = s_stage + s_yofs0[dy] * pitch + shiftb;
                     const uint8_t* r1 = s_stage + s_yofs1[dy] * pitch + shiftb;
@@ -359,7 +366,7 @@ __global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel
         } else {
             // window too large for the staging area: sample straight from global memory with full checks
             __syncthreads();                                       // tables visible
-            for (int dy = warp; dy < fs; dy += kHogWarps) {
+            for (int dy = warp; dy < fs; dy += kWarps) {
                 const short2 yb = s_yb[dy];
                 const int iy0 = y0 + s_yofs0[dy], iy1 = y0 + s_yofs1[dy];
                 for (int dx = lane; dx < fs; dx += 32) {
@@ -387,7 +394,7 @@ __global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel
         if (miss && a.roi_miss) a.roi_miss[img_idx] = 1;
         if (a.patches) {
             __syncthreads();
-            for (int i = tid; i < fs * fs; i += kHogThreads) a.patches[patch_id * fs * fs + i] = s_patch[i];
+            for (int i = tid; i < fs * fs; i += NT) a.patches[patch_id * fs * fs + i] = s_patch[i];
         }
     }
     __syncthreads();
@@ -398,7 +405,7 @@ __global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel
     {
         // linear index over the interior pixels (all lanes busy)
         const int iw = fs - 2, npix = iw * iw;
-        for (int i = tid; i < npix; i += kHogThreads) {
+        for (int i = tid; i < npix; i += NT) {
             const int y = i / iw, x = i - y * iw;
             const int idx = (y + 1) * fs + (x + 1);
             const int gx = (int)s_patch[idx + 1] - (int)s_patch[idx - 1];
@@ -412,7 +419,7 @@ __global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel
     }
     if (a.bins) {
         __syncthreads();
-        for (int idx = tid; idx < fs * fs; idx += kHogThreads) {
+        for (int idx = tid; idx < fs * fs; idx += NT) {
             const int y = idx / fs, x = idx - y * fs;
             const bool interior = x >= 1 && x <= fs - 2 && y >= 1 && y <= fs - 2;
             a.bins[patch_id * fs * fs + idx] = interior ? s_bin[idx] : (int8_t)-1;
@@ -428,7 +435,7 @@ __global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel
     //      order; this is the same sum associated differently (~1e-7 relative), deterministic.
     {
         const int nrow = fs - 2, ntask = nrow * nc, tpad = lay.tpad;
-        for (int task = tid; task < ntask; task += kHogThreads) {
+        for (int task = tid; task < ntask; task += NT) {
             const int ci = task / nrow, y = 1 + task - ci * nrow;
             const int xlo = s_lo[ci], xhi = s_hi[ci];
             const int8_t* bp = s_bin + y * fs + xlo;
@@ -450,7 +457,7 @@ __global__ void __launch_bounds__(kHogThreads, NCT > 0 ? 8 : 0) hog_patch_kernel
         // The histogram hist[b * cells + c] goes to the first 2K cells floats of this landmark's slice of the feature row
         // (which holds cells * dd >= 3K cells floats), where hog_normalise_kernel turns it into the features.
         float* __restrict__ out = a.A + (long long)sample * a.ld + (long long)lm * cells * a.dd;
-        for (int i = tid; i < 2 * K * cells; i += kHogThreads) {
+        for (int i = tid; i < 2 * K * cells; i += NT) {
             const int b = i / cells, c = i - b * cells;
             const int cj = c / nc, ci = c - cj * nc;                  // cell row (y), cell column (x)
             const int ylo = s_lo[cj], yhi = s_hi[cj];
@@ -621,19 +628,23 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
         }
     }
 
-    auto kern = hog_patch_kernel<0, 0, 0>;
-    if (a.K == 4) kern = hog_patch_kernel<4, 0, 0>;
-    else if (a.K == 9) kern = hog_patch_kernel<9, 0, 0>;
+    auto kern = hog_patch_kernel<0, 0, 0, kHogThreads>;
+    int threads = kHogThreads;
+    if (a.K == 4) kern = hog_patch_kernel<4, 0, 0, kHogThreads>;
+    else if (a.K == 9) kern = hog_patch_kernel<9, 0, 0, kHogThreads>;
     if (a.nc == 5 && (a.K == 4 || a.K == 9)) {
-#define SD_HOG_PICK(KK, CC) if (a.K == KK && a.cs == CC) kern = hog_patch_kernel<KK, 5, CC>;
-        SD_HOG_PICK(4, 11) SD_HOG_PICK(4, 10) SD_HOG_PICK(4, 8) SD_HOG_PICK(4, 6)
-        SD_HOG_PICK(9, 11) SD_HOG_PICK(9, 10) SD_HOG_PICK(9, 8) SD_HOG_PICK(9, 6)
+        // the compiled-in schedules and their threads per CTA (DESIGN §4.1)
+#define SD_HOG_PICK(KK, CC, TT) if (a.K == KK && a.cs == CC) { kern = hog_patch_kernel<KK, 5, CC, TT>; threads = TT; }
+        SD_HOG_PICK(4, 11, 224) SD_HOG_PICK(4, 10, 160) SD_HOG_PICK(4, 8, 160) SD_HOG_PICK(4, 6, 128)
+        SD_HOG_PICK(9, 11, 256) SD_HOG_PICK(9, 10, 160) SD_HOG_PICK(9, 8, 160) SD_HOG_PICK(9, 6, 128)
 #undef SD_HOG_PICK
     }
     SD_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
     // Default shared-memory carve-out: the maximum one ran the four detect levels no faster (5.84 ms both, 4096 faces, one
-    // H100 80GB HBM3 at a 400 W power limit), since registers, not shared memory, bound the CTAs per SM at fs = 55 / 50 / 40.
-    kern<<<(unsigned)blocks, kHogThreads, lay.total, ctx->stream>>>(a, maps);
+    // H100 80GB HBM3 at a 400 W power limit; measured at 256 threads, when registers, not shared memory, bounded the CTAs per
+    // SM at fs = 55 / 50 / 40).  With the default, every compiled schedule reaches the CTAs per SM that the thread and
+    // shared-memory limits allow (DESIGN §4.1; counted per SM on an H100 and equal to cudaOccupancyMaxActiveBlocksPerMultiprocessor).
+    kern<<<(unsigned)blocks, threads, lay.total, ctx->stream>>>(a, maps);
     SD_LAUNCH_CHECK(ctx, "hog_patch_kernel");
     if (!d_A) return SD_OK;
     auto norm = a.K == 4 ? hog_normalise_kernel<4> : a.K == 9 ? hog_normalise_kernel<9> : hog_normalise_kernel<0>;
