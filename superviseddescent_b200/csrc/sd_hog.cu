@@ -129,27 +129,45 @@ __global__ void hog_bintab_kernel(int fs, int nc, int cs, float* __restrict__ bt
     }
 }
 
+// cv::resize's vertical step of one output pixel from its horizontal sums t0, t1 of source rows 0 and 1 and the y weights
+// yb = weight 0 | weight 1 << 16 (int16 each): (b * (t >> 4)) >> 16 per row, then + 2 >> 2
+__device__ __forceinline__ int hog_resize_out(int yb, int t0, int t1)
+{
+    return (((((int)(short)yb) * (t0 >> 4)) >> 16) + (((yb >> 16) * (t1 >> 4)) >> 16) + 2) >> 2;
+}
+
+// byte n (0..7) of the 8 bytes lo, hi (little endian)
+__device__ __forceinline__ int byte_of(unsigned lo, unsigned hi, int n) { return (int)(((n < 4 ? lo : hi) >> (8 * (n & 3))) & 0xffu); }
+
 // shared-memory carve-up (same function on host and device)
 struct HogSmem {
-    int patch, bin, r1, xofs, yofs0, yofs1, xa, yb, wcell, lo, hi, vote, mbar, stage_end, total;
+    int patch, bin, r1, tab, xa, wcell, lo, hi, vote, mbar, stage_end, total;
+    int pp;        // row pitch of the resized patch: fs rounded up to a multiple of 4
+    int pb, pm;    // row pitches of the interior bins (bytes, a multiple of 4) and moduli (floats, odd)
     int tpad;      // tasks of the horizontal vote pass, padded to a multiple of 32
 };
 
 __host__ __device__ inline int align_up(int v, int a) { return (v + a - 1) / a * a; }
 
 // [bin | r1 | vote] is dead during S1, so that whole span is the staging area of the source window.  The cell histograms
-// go from the vote's second pass straight to global memory (hog_normalise_kernel takes them from there).
+// go from the vote's second pass straight to global memory (hog_normalise_kernel takes them from there).  The patch rows
+// are word aligned (pitch pp) so that S1 stores and S2 loads whole words.  Bins and moduli hold the interior pixels only,
+// pixel (y, x) at (y - 1) * pitch + x - 1, so that S2's runs of four start on a word of bins.  Pass 1 of the vote reads
+// one row per lane: an odd pitch (moduli) keeps those reads free of bank conflicts, and so does an odd number of words
+// between rows of bins where that fits in fs * fs bytes.  Both regions hold fs * fs pixels, as before: the staging area
+// and the largest configuration are the same.
 __host__ __device__ inline HogSmem hog_smem_layout(int fs, int nc, int K)
 {
     HogSmem s;
+    s.pp = align_up(fs, 4);
+    s.pm = align_up(fs - 2, 4) + 1;                         // a row's runs of four, odd: (fs - 2) * pm < fs * fs
+    s.pb = s.pm - 1;
+    if ((s.pb & 7) == 0 && (fs - 2) * (s.pb + 4) <= fs * fs) s.pb += 4;
     int o = 0;
     s.patch = o;
-    o = align_up(fs * fs, 16);
-    s.xofs = o;   o += fs * 4;
-    s.yofs0 = o;  o += fs * 4;
-    s.yofs1 = o;  o += fs * 4;
-    s.xa = o;     o += fs * 4;                              // 2 x int16
-    s.yb = o;     o += fs * 4;
+    o = align_up(s.pp * fs, 16);
+    s.tab = o;    o += fs * 16;                             // int4 {x source index, y source index 0 / 1, y weights (2 x int16)}
+    s.xa = o;     o += fs * 4;                              // x weights, 2 x int16
     s.wcell = o;  o += nc * fs * 4;                         // weight of pixel t for cell index c (0 if it does not vote)
     s.lo = o;     o += nc * 4;
     s.hi = o;     o += nc * 4;
@@ -161,7 +179,7 @@ __host__ __device__ inline HogSmem hog_smem_layout(int fs, int nc, int K)
     s.vote = o;                                             // horizontal pass of the vote: T[bin][(cell column, row)]
     o += 2 * K * s.tpad * 4;
     s.stage_end = o;
-    s.total = align_up(o, 16);
+    s.total = align_up(o + 8, 16);                          // S1's word loads read up to 7 bytes past the staged window
     return s;
 }
 
@@ -189,14 +207,12 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
     const int fs = (NCT > 0 && CST > 0) ? NCT * CST : a.fs;
     const int cells = nc * nc;
     const HogSmem lay = hog_smem_layout(fs, nc, K);
+    const int pp = lay.pp, pb = lay.pb, pm = lay.pm;
     uint8_t* s_patch = smem + lay.patch;
     int8_t* s_bin = reinterpret_cast<int8_t*>(smem + lay.bin);
     float* s_gmag = reinterpret_cast<float*>(smem + lay.r1);
-    int* s_xofs = reinterpret_cast<int*>(smem + lay.xofs);
-    int* s_yofs0 = reinterpret_cast<int*>(smem + lay.yofs0);
-    int* s_yofs1 = reinterpret_cast<int*>(smem + lay.yofs1);
+    int4* s_tab = reinterpret_cast<int4*>(smem + lay.tab);
     short2* s_xa = reinterpret_cast<short2*>(smem + lay.xa);
-    short2* s_yb = reinterpret_cast<short2*>(smem + lay.yb);
     float* s_wcell = reinterpret_cast<float*>(smem + lay.wcell);
     int* s_lo = reinterpret_cast<int*>(smem + lay.lo);
     int* s_hi = reinterpret_cast<int*>(smem + lay.hi);
@@ -267,12 +283,9 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
     {
         const int* __restrict__ rt = a.rtab + (long long)sample * 5 * fs;
         for (int t = tid; t < fs; t += NT) {
-            s_xofs[t] = __ldg(rt + t);
-            const int xa = __ldg(rt + fs + t), yb = __ldg(rt + 4 * fs + t);
+            const int xa = __ldg(rt + fs + t);
             s_xa[t] = *reinterpret_cast<const short2*>(&xa);
-            s_yofs0[t] = __ldg(rt + 2 * fs + t);
-            s_yofs1[t] = __ldg(rt + 3 * fs + t);
-            s_yb[t] = *reinterpret_cast<const short2*>(&yb);
+            s_tab[t] = make_int4(__ldg(rt + t), __ldg(rt + 2 * fs + t), __ldg(rt + 3 * fs + t), __ldg(rt + 4 * fs + t));
         }
         for (int i = tid; i < nc * fs; i += NT) s_wcell[i] = __ldg(a.btab + i);
         const int* __restrict__ lohi = reinterpret_cast<const int*>(a.btab + nc * fs);
@@ -297,7 +310,9 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
                 const int gs = nvec <= 8 ? 3 : (nvec <= 16 ? 4 : 5);
                 const int lv = lane & ((1 << gs) - 1), lr = lane >> gs, rows_per_pass = 32 >> gs;
                 const uint8_t* wrow = img + (long long)(y0 - ry) * rs + (x0 - rx - shiftb);
+                // not unrolled (here and in the word loop): unrolled, they spill at 32 registers at fs = 30, K = 4
                 for (int r = warp * rows_per_pass + lr; r < P; r += kWarps * rows_per_pass)
+#pragma unroll 1
                     for (int v = lv; v < nvec; v += (1 << gs))
                         reinterpret_cast<uint4*>(s_stage + r * pitch)[v] = __ldg(reinterpret_cast<const uint4*>(wrow + (long long)r * rs) + v);
             } else if (words) {
@@ -306,6 +321,7 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
                 for (int r = warp; r < P; r += kWarps) {
                     const uint32_t* src = reinterpret_cast<const uint32_t*>(wrow + (long long)r * rs);
                     uint32_t* dst = reinterpret_cast<uint32_t*>(s_stage + r * pitch);
+#pragma unroll 1
                     for (int w = lane; w < nwords; w += 32) dst[w] = __ldg(src + w);
                 }
             } else {
@@ -327,39 +343,61 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
             __syncthreads();                                       // tables (and the load loops' stores) visible
             if (tma_box) hog_tma_wait(s_mbar);
             if (fs <= 64) {
-                // a thread keeps ONE output column (its two source taps and weights stay in registers) and walks down the rows:
-                // NT / fs row groups of fs threads, NT mod fs threads idle
-                const int groups = NT / fs;
-                const int dx = tid % fs, g = tid / fs;
+                // a thread keeps TWO adjacent output columns (their taps and weights stay in registers) and walks down the
+                // rows: NT / ceil(fs / 2) row groups, the rest of the threads idle.  When the four taps of the pair lie in the
+                // 8 bytes from the word at q (any window up to about 3x the patch), a row costs one table load, two word loads
+                // per source row and one 16-bit store for both outputs; a byte permute puts a tap pair in the low half of a
+                // word and dp2a forms its weighted sum, the same integer as the scalar products.  Odd fs: the last thread's
+                // second output repeats its first into the padding column.
+                const int np = (fs + 1) >> 1, groups = NT / np;
+                const int j = tid % np, g = tid / np;
                 if (g < groups) {
-                    const int sx = s_xofs[dx];
-                    const int sx1 = min(sx + 1, P - 1);            // clamped tap has zero weight
-                    const int ax = s_xa[dx].x, bx = s_xa[dx].y;
-                    const uint8_t* base = s_stage + shiftb;
-#pragma unroll 4
-                    for (int dy = g; dy < fs; dy += groups) {
-                        const short2 yb = s_yb[dy];
-                        const uint8_t* r0 = base + s_yofs0[dy] * pitch;
-                        const uint8_t* r1 = base + s_yofs1[dy] * pitch;
-                        const int t0 = (int)r0[sx] * ax + (int)r0[sx1] * bx;
-                        const int t1 = (int)r1[sx] * ax + (int)r1[sx1] * bx;
-                        const int v = ((((int)yb.x * (t0 >> 4)) >> 16) + (((int)yb.y * (t1 >> 4)) >> 16) + 2) >> 2;
-                        s_patch[dy * fs + dx] = (uint8_t)v;        // s_patch precedes the staging area: no overlap
+                    const int dxa = 2 * j, dxb = min(dxa + 1, fs - 1);
+                    const int sxa = s_tab[dxa].x, sxb = s_tab[dxb].x;
+                    const unsigned xa = *reinterpret_cast<const unsigned*>(s_xa + dxa), xb = *reinterpret_cast<const unsigned*>(s_xa + dxb);
+                    const int q = (shiftb + sxa) & ~3;
+                    const int oa = shiftb + sxa - q, ob = shiftb + sxb - q;
+                    uint8_t* out = s_patch + dxa;                  // s_patch precedes the staging area: no overlap
+                    if (ob <= 6) {
+                        // tap sx + 1 of a clamped column (sx = P - 1) may lie past the window: its weight is 0
+                        const unsigned sa = oa | (oa + 1) << 4, sb = ob | (ob + 1) << 4;
+                        const uint8_t* base = s_stage + q;
+#pragma unroll 2
+                        for (int dy = g; dy < fs; dy += groups) {
+                            const int4 yt = s_tab[dy];
+                            const unsigned* r0 = reinterpret_cast<const unsigned*>(base + yt.y * pitch);
+                            const unsigned* r1 = reinterpret_cast<const unsigned*>(base + yt.z * pitch);
+                            const unsigned a0 = r0[0], a1 = r0[1], b0 = r1[0], b1 = r1[1];
+                            const int va = hog_resize_out(yt.w, __dp2a_lo(xa, __byte_perm(a0, a1, sa), 0u), __dp2a_lo(xa, __byte_perm(b0, b1, sa), 0u));
+                            const int vb = hog_resize_out(yt.w, __dp2a_lo(xb, __byte_perm(a0, a1, sb), 0u), __dp2a_lo(xb, __byte_perm(b0, b1, sb), 0u));
+                            *reinterpret_cast<uint16_t*>(out + dy * pp) = (uint16_t)(va | vb << 8);
+                        }
+                    } else {
+                        const int ax = s_xa[dxa].x, bx = s_xa[dxa].y, cx = s_xa[dxb].x, dx = s_xa[dxb].y;
+                        const int sxa1 = min(sxa + 1, P - 1), sxb1 = min(sxb + 1, P - 1);   // clamped tap has zero weight
+                        const uint8_t* base = s_stage + shiftb;
+                        for (int dy = g; dy < fs; dy += groups) {
+                            const int4 yt = s_tab[dy];
+                            const uint8_t* r0 = base + yt.y * pitch;
+                            const uint8_t* r1 = base + yt.z * pitch;
+                            const int va = hog_resize_out(yt.w, (int)r0[sxa] * ax + (int)r0[sxa1] * bx, (int)r1[sxa] * ax + (int)r1[sxa1] * bx);
+                            const int vb = hog_resize_out(yt.w, (int)r0[sxb] * cx + (int)r0[sxb1] * dx, (int)r1[sxb] * cx + (int)r1[sxb1] * dx);
+                            *reinterpret_cast<uint16_t*>(out + dy * pp) = (uint16_t)(va | vb << 8);
+                        }
                     }
                 }
             } else {
                 for (int dy = warp; dy < fs; dy += kWarps) {
-                    const short2 yb = s_yb[dy];
-                    const uint8_t* r0 = s_stage + s_yofs0[dy] * pitch + shiftb;
-                    const uint8_t* r1 = s_stage + s_yofs1[dy] * pitch + shiftb;
+                    const int4 yt = s_tab[dy];
+                    const uint8_t* r0 = s_stage + yt.y * pitch + shiftb;
+                    const uint8_t* r1 = s_stage + yt.z * pitch + shiftb;
                     for (int dx = lane; dx < fs; dx += 32) {
-                        const int sx = s_xofs[dx];
+                        const int sx = s_tab[dx].x;
                         const int sx1 = min(sx + 1, P - 1);
                         const short2 xa = s_xa[dx];
                         const int t0 = (int)r0[sx] * xa.x + (int)r0[sx1] * xa.y;
                         const int t1 = (int)r1[sx] * xa.x + (int)r1[sx1] * xa.y;
-                        const int v = ((((int)yb.x * (t0 >> 4)) >> 16) + (((int)yb.y * (t1 >> 4)) >> 16) + 2) >> 2;
-                        s_patch[dy * fs + dx] = (uint8_t)v;
+                        s_patch[dy * pp + dx] = (uint8_t)hog_resize_out(yt.w, t0, t1);
                     }
                 }
             }
@@ -367,10 +405,10 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
             // window too large for the staging area: sample straight from global memory with full checks
             __syncthreads();                                       // tables visible
             for (int dy = warp; dy < fs; dy += kWarps) {
-                const short2 yb = s_yb[dy];
-                const int iy0 = y0 + s_yofs0[dy], iy1 = y0 + s_yofs1[dy];
+                const int4 yt = s_tab[dy];
+                const int iy0 = y0 + yt.y, iy1 = y0 + yt.z;
                 for (int dx = lane; dx < fs; dx += 32) {
-                    const int sx = s_xofs[dx];
+                    const int sx = s_tab[dx].x;
                     const short2 xa = s_xa[dx];
                     int p[4];
 #pragma unroll
@@ -386,15 +424,17 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
                     }
                     const int t0 = p[0] * xa.x + p[1] * xa.y;
                     const int t1 = p[2] * xa.x + p[3] * xa.y;
-                    const int v = ((((int)yb.x * (t0 >> 4)) >> 16) + (((int)yb.y * (t1 >> 4)) >> 16) + 2) >> 2;
-                    s_patch[dy * fs + dx] = (uint8_t)v;
+                    s_patch[dy * pp + dx] = (uint8_t)hog_resize_out(yt.w, t0, t1);
                 }
             }
         }
         if (miss && a.roi_miss) a.roi_miss[img_idx] = 1;
         if (a.patches) {
             __syncthreads();
-            for (int i = tid; i < fs * fs; i += NT) a.patches[patch_id * fs * fs + i] = s_patch[i];
+            for (int i = tid; i < fs * fs; i += NT) {
+                const int y = i / fs;
+                a.patches[patch_id * fs * fs + i] = s_patch[y * pp + (i - y * fs)];
+            }
         }
     }
     __syncthreads();
@@ -403,18 +443,29 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
     //      patch is a pair of integers in [-255, 255], its squared modulus an exact float integer whose correctly rounded
     //      root is the reference's sqrtf, and hog_bin decides the reference's arg-max -----------------------------------
     {
-        // linear index over the interior pixels (all lanes busy)
-        const int iw = fs - 2, npix = iw * iw;
-        for (int i = tid; i < npix; i += NT) {
-            const int y = i / iw, x = i - y * iw;
-            const int idx = (y + 1) * fs + (x + 1);
-            const int gx = (int)s_patch[idx + 1] - (int)s_patch[idx - 1];
-            const int gy = (int)s_patch[idx + fs] - (int)s_patch[idx - fs];
-            const int g2 = gx * gx + gy * gy;
-            const float g = __fsqrt_rn((float)g2);
-            const int b = hog_bin(a.orient, K, gx, gy, g);
-            s_bin[idx] = (int8_t)b;
-            s_gmag[idx] = b < 0 ? 0.f : g;                         // no bin, no vote (hog.c:694): g = 0, or gx = 0 at K = 1
+        // linear index over (interior row, run of 4 pixels): the run's three source rows come in as two words each and its
+        // bins go out in one 32-bit store.  A row's last run may reach up to 3 pixels past the interior: they land in the
+        // padding columns (x - 1 < pb), which nothing reads.
+        const int iw = fs - 2, runs = (iw + 3) >> 2, nitem = iw * runs;
+        const int pw = pp >> 2;                                    // row pitch in words
+        for (int i = tid; i < nitem; i += NT) {
+            const int y = i / runs, r = i - y * runs;              // pixels (y + 1, 4r + 1 .. 4r + 4)
+            const unsigned* c = reinterpret_cast<const unsigned*>(s_patch) + (y + 1) * pw + r;
+            const unsigned c0 = c[0], c1 = c[1], u0 = c[-pw], u1 = c[1 - pw], d0 = c[pw], d1 = c[pw + 1];
+            unsigned bins = 0;
+            float* gm = s_gmag + y * pm + 4 * r;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                // bytes k .. k + 2 of the centre row's 8, byte k + 1 of the rows above and below
+                const int gx = byte_of(c0, c1, k + 2) - byte_of(c0, c1, k);
+                const int gy = byte_of(d0, d1, k + 1) - byte_of(u0, u1, k + 1);
+                const int g2 = gx * gx + gy * gy;
+                const float g = __fsqrt_rn((float)g2);
+                const int b = hog_bin(a.orient, K, gx, gy, g);
+                bins |= (unsigned)(b & 0xff) << (8 * k);
+                gm[k] = b < 0 ? 0.f : g;                           // no bin, no vote (hog.c:694): g = 0, or gx = 0 at K = 1
+            }
+            *reinterpret_cast<unsigned*>(s_bin + y * pb + 4 * r) = bins;
         }
     }
     if (a.bins) {
@@ -422,7 +473,7 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
         for (int idx = tid; idx < fs * fs; idx += NT) {
             const int y = idx / fs, x = idx - y * fs;
             const bool interior = x >= 1 && x <= fs - 2 && y >= 1 && y <= fs - 2;
-            a.bins[patch_id * fs * fs + idx] = interior ? s_bin[idx] : (int8_t)-1;
+            a.bins[patch_id * fs * fs + idx] = interior ? s_bin[(y - 1) * pb + x - 1] : (int8_t)-1;
         }
     }
     if (!a.A) return;                                             // sd_hog_debug: geometry, patches and bins only
@@ -438,8 +489,8 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
         for (int task = tid; task < ntask; task += NT) {
             const int ci = task / nrow, y = 1 + task - ci * nrow;
             const int xlo = s_lo[ci], xhi = s_hi[ci];
-            const int8_t* bp = s_bin + y * fs + xlo;
-            const float* gp = s_gmag + y * fs + xlo;
+            const int8_t* bp = s_bin + (y - 1) * pb + (xlo - 1);
+            const float* gp = s_gmag + (y - 1) * pm + (xlo - 1);
             const float* wp = s_wcell + ci * fs + xlo;
             float* T = s_T + task;
             for (int b = 0; b < 2 * K; ++b) T[b * tpad] = 0.f;        // T shares the staging area of S1: clear this column first
