@@ -221,6 +221,29 @@ SD_API int sd_hog_dense_shape(int width, int height, int cell_size, int num_bins
 SD_API int sd_hog_dense(sd_ctx* ctx, const sd_image_batch* images, int cell_size, int num_bins, int variant, float* d_out,
                         const int64_t* d_out_offset);
 
+/* ---- dense HOG pyramid: every frame of a batch at every scale, in one call --------------------------------------------------
+ * The level of a width x height frame at scale s is level_w x level_h px with level_w = floor(width * s + 0.5) and
+ * level_h = floor(height * s + 0.5), in double.  Each level is resized from the frame itself (not from another level) by
+ * cv::resize INTER_LINEAR's 8-bit fixed-point rule, the resize of sd_hog_batch's patches, with the per-axis scale
+ * 1 / (level_w / width) in double; a level of the frame's own size is the frame.  Its features are bit for bit sd_hog_dense's
+ * of the resized frame, [dd][hog_h][hog_w] at d_out + d_out_offset[frame * num_scales + s] (floats; a device array of
+ * count * num_scales int64).  A level narrower or lower than 4 px, or whose cell grid is empty, is empty: hog_w = hog_h = 0,
+ * nothing is written and its offset is not read.  Scales must be finite and in (0, 4], and levels at most 2^28 px per side.
+ * Cell (x, y) of a level starts at pixel (x * cell_size * width / level_w, y * cell_size * height / level_h) of the frame.
+ *
+ * sd_hog_pyramid_shape: host only.  Writes the level's size, its hog_w, hog_h (0 for an empty level) and dd, or returns
+ * SD_ERR_INVALID for a frame smaller than 1 x 1, an invalid scale or an invalid configuration. */
+SD_API int sd_hog_pyramid_shape(int width, int height, double scale, int cell_size, int num_bins, int variant,
+                                int* level_w, int* level_h, int* hog_w, int* hog_h, int* dd);
+/* sd_hog_pyramid: asynchronous on the context's stream; h_scales is a host array of num_scales scales.  Frames are an
+ * sd_image_batch as for sd_hog_dense: equally sized, or per-frame d_frames (the call then reads the table back once); host
+ * and colour frames reach the device through sd_upload_frames.  The resized levels go through context scratch, one slice of
+ * the batch at a time (about 64 MB of levels per slice), so the scratch does not grow with the batch.  Each level's features
+ * depend on its frame and scale alone.  Null pointers, a batch with d_roi, num_scales < 1, an invalid scale or configuration,
+ * or a frame smaller than 1 x 1 is SD_ERR_INVALID before any work is queued (d_out is not written). */
+SD_API int sd_hog_pyramid(sd_ctx* ctx, const sd_image_batch* images, const double* h_scales, int num_scales,
+                          int cell_size, int num_bins, int variant, float* d_out, const int64_t* d_out_offset);
+
 /* ---- dense HOG of 8-bit or float frames with 1..16 channels: every input of vl_hog_put_image (hog.c:595-728) ----------------
  * One frame: element (x, y, c) at offset + y * row_stride + x * pixel_stride + c * channel_stride, in ELEMENTS of the batch's
  * dtype.  VLFeat's planar layout is pixel_stride = 1, channel_stride = height * row_stride; the interleaved layout of OpenCV
@@ -320,6 +343,27 @@ SD_API int sd_hog_render(sd_ctx* ctx, const sd_hog_grids* grids, int num_bins, i
  * out[i][y][x] = in[perm[i]][y][w - 1 - x] -- the features of the left-right mirrored image.  transpose = 1: each (flipped)
  * plane is then stored transposed, [w][h] -- the features of a transposed VlHog.  Validation as sd_hog_render. */
 SD_API int sd_hog_relayout(sd_ctx* ctx, const sd_hog_grids* grids, int num_bins, int variant, int flip, int transpose, float* d_out);
+
+/* ---- HOG filters: a bank of templates scored over a batch of HOG grids (the score maps of a sliding-window detector) ---------
+ * Filters are [Q][dd][fh][fw], the layout of the features of a grid of fw x fh cells: sd_hog_dense of a template image gives a
+ * filter, sd_hog_render draws one and sd_hog_relayout(flip = 1) mirrors one.  For grid g ([dd][h][w] as in sd_hog_grids),
+ * filter q and output (y, x):
+ *   S = bias[q] + sum_{c < dd} sum_{dy < fh} sum_{dx < fw} F[q][c][dy][dx] * M[c][y + dy - pad_y][x + dx - pad_x]
+ * with M = 0 outside the grid, over oh = h + 2 pad_y - fh + 1 rows and ow = w + 2 pad_x - fw + 1 columns, written [Q][oh][ow] at
+ * d_scores + out_offset of the grid's descriptor, or at d_scores + i * Q * oh * ow for equally sized grids.  A grid with
+ * oh <= 0 or ow <= 0 (smaller than the filter) has no scores and is valid.  Arithmetic: float32 FMAs (no TF32) in one fixed
+ * order -- per (channel, dy) ascending, dx ascending, a chain from 0; the bias added last -- so each score depends on its grid,
+ * filter and bias alone: the same in any batch and in every run.  Score (x, y) of a pyramid level covers the cells from
+ * (x - pad_x, y - pad_y), which start at pixel (x - pad_x) * cell_size * width / level_w of the frame (rows alike).
+ * Limits: fw, fh in [1, SD_HOG_FILTER_MAX_SIDE], num_filters in [1, SD_HOG_FILTER_MAX_BANK], pad_x in [0, fw - 1] and pad_y
+ * in [0, fh - 1].  Null pointers (d_bias may be NULL: no bias), pointers that are not 4-byte aligned, an invalid configuration,
+ * a grid smaller than 1 x 1 or with a negative offset, or anything outside the limits is SD_ERR_INVALID before any work is
+ * queued (d_scores is not written). */
+#define SD_HOG_FILTER_MAX_SIDE 32
+#define SD_HOG_FILTER_MAX_BANK 256
+SD_API int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int variant,
+                            const float* d_filters, int num_filters, int filter_w, int filter_h,
+                            const float* d_bias /* num_filters floats or NULL */, int pad_x, int pad_y, float* d_scores);
 
 /* ---- regressor: LinearRegressor<Solver> (regressors.hpp:318-400) ------------------------ */
 /* Solver::solve (regressors.hpp:199-234 == verbose_solver.hpp:53-111):

@@ -111,6 +111,7 @@ EXPORTS = [
     "sd_memcpy2d_h2d", "sd_memcpy2d_d2h", "sd_memcpy2d_d2d",
     "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_bgr2gray", "sd_upload_frames", "sd_hog_dense_shape", "sd_hog_dense",
     "sd_hog_dense_images", "sd_hog_dense_polar", "sd_hog_permutation", "sd_hog_glyphs", "sd_hog_render", "sd_hog_relayout",
+    "sd_hog_pyramid_shape", "sd_hog_pyramid", "sd_hog_correlate",
     "sd_learn", "sd_centre_features", "sd_learn_centred", "sd_learn_rank_revealing", "sd_gram", "sd_solve_gram", "sd_predict", "sd_test_residual", "sd_solver_timings", "sd_set_gram_mode", "sd_set_solver", "sd_solver_iterations",
     "sd_set_rank_diagnostic", "sd_last_rank",
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",
@@ -167,6 +168,11 @@ def lib():
         l.sd_apply_level_host_projected.argtypes = [C.c_void_p, C.POINTER(LevelHostProjectionC), C.c_void_p, C.c_int, C.c_int,
                                                     C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int,
                                                     C.c_void_p]
+        _i = C.c_int
+        _ip = C.POINTER(C.c_int)
+        l.sd_hog_pyramid_shape.argtypes = [_i, _i, C.c_double, _i, _i, _i, _ip, _ip, _ip, _ip, _ip]
+        l.sd_hog_pyramid.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_double), _i, _i, _i, _i, C.c_void_p, C.c_void_p]
+        l.sd_hog_correlate.argtypes = [C.c_void_p, C.c_void_p, _i, _i, C.c_void_p, _i, _i, _i, C.c_void_p, _i, _i, C.c_void_p]
         _lib = l
     return _lib
 

@@ -389,6 +389,41 @@ def hog_dense_shape(width: int, height: int, cell_size: int, num_bins: int, vari
     return d.value, h.value, w.value
 
 
+def _grey_frames(frames, ctx: Context, check):
+    """The 8-bit frames of hog_dense / vl_hog_pyramid -> (the device tensor that owns them, their ImageBatchC, [(H, W)] per frame).
+    A CUDA (count, H, W) uint8 tensor is used in place; host frames are uploaded by sd_upload_frames after check(W, H) has
+    accepted every size.  An empty list of host frames gives (None, None, [])."""
+    if isinstance(frames, torch.Tensor) and frames.is_cuda:
+        if frames.dtype != torch.uint8 or frames.dim() != 3:
+            raise ValueError("a device tensor of frames must be (count, H, W) uint8")
+        t = frames.to(f"cuda:{ctx.device}")
+        if t.stride(2) != 1:
+            t = t.contiguous()
+        n, h, w = t.shape
+        return t, ImageBatchC(C.c_void_p(t.data_ptr()), w, h, t.stride(1), t.stride(0), n), [(h, w)] * n
+    if isinstance(frames, (list, tuple)):
+        frames = list(frames)
+    else:
+        a = frames.numpy() if isinstance(frames, torch.Tensor) else np.asarray(frames)
+        if a.dtype != np.uint8 or not (a.ndim == 3 or (a.ndim == 4 and a.shape[3] == 3)):
+            raise ValueError("frames must be (count, H, W) uint8, (count, H, W, 3) uint8, or a list of such frames of any sizes")
+        frames = list(a)
+    recs, arrays = [], []
+    for f in frames:
+        rec, a = _host_frame(f)
+        if a.ndim == 3 and a.shape[2] != 3:
+            raise ValueError("every frame must be (H, W) uint8 or (H, W, 3) uint8")
+        recs.append(rec)
+        arrays.append(a)                                  # the bytes stay alive until the upload returns
+    sizes = [(r.height, r.width) for r in recs]
+    if not recs:
+        return None, None, []
+    for h, w in set(sizes):
+        check(w, h)                                       # refuse before the upload
+    keep, ib = _upload_host_frames(recs, ctx)
+    return keep, ib, sizes
+
+
 def hog_dense(frames, cell_size: int, num_bins: int, variant: int = 1, ctx: Optional[Context] = None):
     """VLFeat HOG of whole 8-bit frames (vl_hog_new(variant, num_bins) + vl_hog_put_image(frame, 1 channel, cell_size) +
     vl_hog_extract) on the device, in VLFeat's planar layout [dd][hogH][hogW] with x fastest.
@@ -400,37 +435,9 @@ def hog_dense(frames, cell_size: int, num_bins: int, variant: int = 1, ctx: Opti
     tensors."""
     ctx = ctx or default_context()
     lib = _capi.lib()
-    keep = None
-    if isinstance(frames, torch.Tensor) and frames.is_cuda:
-        if frames.dtype != torch.uint8 or frames.dim() != 3:
-            raise ValueError("a device tensor of frames must be (count, H, W) uint8")
-        t = frames.to(f"cuda:{ctx.device}")
-        if t.stride(2) != 1:
-            t = t.contiguous()
-        n, h, w = t.shape
-        keep, ib = t, ImageBatchC(C.c_void_p(t.data_ptr()), w, h, t.stride(1), t.stride(0), n)
-        sizes = [(h, w)] * n
-    else:
-        if isinstance(frames, (list, tuple)):
-            frames = list(frames)
-        else:
-            a = frames.numpy() if isinstance(frames, torch.Tensor) else np.asarray(frames)
-            if a.dtype != np.uint8 or not (a.ndim == 3 or (a.ndim == 4 and a.shape[3] == 3)):
-                raise ValueError("frames must be (count, H, W) uint8, (count, H, W, 3) uint8, or a list of such frames of any sizes")
-            frames = list(a)
-        recs, arrays = [], []
-        for f in frames:
-            rec, a = _host_frame(f)
-            if a.ndim == 3 and a.shape[2] != 3:
-                raise ValueError("every frame must be (H, W) uint8 or (H, W, 3) uint8")
-            recs.append(rec)
-            arrays.append(a)                                  # the bytes stay alive until the upload returns
-        sizes = [(r.height, r.width) for r in recs]
-        if not recs:
-            return []
-        for h, w in set(sizes):
-            hog_dense_shape(w, h, cell_size, num_bins, variant)   # refuse before the upload
-        keep, ib = _upload_host_frames(recs, ctx)
+    keep, ib, sizes = _grey_frames(frames, ctx, lambda w, h: hog_dense_shape(w, h, cell_size, num_bins, variant))
+    if ib is None:
+        return []
     n = len(sizes)
     dev = f"cuda:{ctx.device}"
     if n == 0:
@@ -1524,3 +1531,115 @@ def vl_hog_flip(features, num_bins: int, variant: int = 1, ctx: Optional[Context
     lib = _capi.lib()
     return _hog_result(ctx, shapes, offsets, batched, lambda out: _check(ctx.h, lib.sd_hog_relayout(
         ctx.h, C.byref(g), int(num_bins), int(variant), 1, 0, ptr(out))), zero=False)
+
+
+# ------------------------------------------------------------------------------------------------
+# HOG pyramids and filters: the two batched primitives of a sliding-window detector
+# ------------------------------------------------------------------------------------------------
+def hog_pyramid_shape(width: int, height: int, scale: float, cell_size: int, num_bins: int, variant: int = 1):
+    """((level_w, level_h), (dd, hogH, hogW)) of a width x height frame at scale (sd_hog_pyramid_shape); hogH = hogW = 0 for an
+    empty level.  SdError for an invalid scale or configuration."""
+    o = [C.c_int() for _ in range(5)]
+    rc = _capi.lib().sd_hog_pyramid_shape(int(width), int(height), float(scale), int(cell_size), int(num_bins), int(variant),
+                                          *[C.byref(v) for v in o])
+    if rc:
+        raise SdError(rc, f"invalid HOG pyramid level: {width} x {height} px at scale {scale}, cell_size {cell_size}, num_bins "
+                          f"{num_bins}, variant {variant} (scales finite and in (0, 4], cell_size 1..32, num_bins 1..16)")
+    lw, lh, w, h, d = (v.value for v in o)
+    return (lw, lh), (d, h, w)
+
+
+def vl_hog_pyramid(frames, scales, cell_size: int, num_bins: int, variant: int = 1, ctx: Optional[Context] = None):
+    """Dense HOG of every frame at every scale in one call (sd_hog_pyramid): level s of a W x H frame is the frame resized by
+    cv::resize INTER_LINEAR to floor(W * s + 0.5) x floor(H * s + 0.5), and its features are hog_dense's of that level.
+
+    frames: as hog_dense takes them.  Returns (features, sizes): features[f][s] is a (dd, hogH, hogW) float32 CUDA view into
+    one buffer, or None for an empty level (smaller than 4 px or than half a cell); sizes[f][s] = (level_w, level_h)."""
+    ctx = ctx or default_context()
+    scales = [float(s) for s in scales]
+    if not scales:
+        raise ValueError("vl_hog_pyramid needs at least one scale")
+
+    def check(w, h):
+        for s in scales:
+            hog_pyramid_shape(w, h, s, cell_size, num_bins, variant)
+
+    keep, ib, sizes = _grey_frames(frames, ctx, check)
+    if not sizes:
+        return [], []
+    levels = [[hog_pyramid_shape(w, h, s, cell_size, num_bins, variant) for s in scales] for h, w in sizes]
+    offsets, pos = [], 0
+    for row in levels:
+        for _, (d, h, w) in row:
+            offsets.append(pos)
+            pos += d * h * w
+    dev = f"cuda:{ctx.device}"
+    out = torch.empty(max(pos, 1), dtype=torch.float32, device=dev)
+    d_off = torch.tensor(offsets, dtype=torch.int64, device=dev)
+    h_scales = (C.c_double * len(scales))(*scales)
+    _check(ctx.h, _capi.lib().sd_hog_pyramid(ctx.h, C.byref(ib), h_scales, len(scales), int(cell_size), int(num_bins), int(variant),
+                                             ptr(out), ptr(d_off)))
+    feats, i = [], 0
+    for row in levels:
+        fr = []
+        for _, shape in row:
+            fr.append(out[offsets[i]:offsets[i] + int(np.prod(shape))].view(shape) if shape[1] else None)
+            i += 1
+        feats.append(fr)
+    return feats, [[lv for lv, _ in row] for row in levels]
+
+
+def vl_hog_correlate(maps, filters, num_bins: int, variant: int = 1, bias=None, pad=(0, 0), ctx: Optional[Context] = None):
+    """Scores of a bank of HOG filters over a list of HOG grids (sd_hog_correlate):
+        S[q, y, x] = bias[q] + sum_{c, dy, dx} filters[q, c, dy, dx] * M[c, y + dy - pad_y, x + dx - pad_x],   M = 0 outside,
+    float32 FMAs in a fixed order (no TF32).  maps: a list of (dd, h, w) float32 CUDA tensors; maps that are contiguous views
+    of one storage (as vl_hog_pyramid returns them) are read in place, others are packed first.  filters: (Q, dd, fh, fw);
+    bias: (Q,) or None; pad = (pad_x, pad_y), each in [0, filter side - 1].  Returns one (Q, oh, ow) tensor per map,
+    oh = h + 2 pad_y - fh + 1 and ow = w + 2 pad_x - fw + 1 (an empty tensor where either is <= 0)."""
+    ctx = ctx or default_context()
+    dd = _hog_dims(num_bins, variant)
+    dev = f"cuda:{ctx.device}"
+    f = filters if isinstance(filters, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(filters))
+    if f.dtype != torch.float32 or f.dim() != 4 or f.shape[1] != dd:
+        raise ValueError(f"filters must be a float32 (Q, dd, fh, fw) tensor with dd = {dd}")
+    f = f.to(dev).contiguous()
+    q, _, fh, fw = f.shape
+    b = None
+    if bias is not None:
+        b = (bias if isinstance(bias, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(bias))).to(dev, torch.float32).contiguous()
+        if b.shape != (q,):
+            raise ValueError(f"bias must have one value per filter ({q})")
+    pad_x, pad_y = (int(p) for p in pad)
+    maps = list(maps)
+    if any(not isinstance(m, torch.Tensor) or not m.is_cuda or m.dtype != torch.float32 or m.dim() != 3 or m.shape[0] != dd
+           for m in maps):
+        raise ValueError(f"every map must be a float32 CUDA tensor (dd, h, w) with dd = {dd}")
+    if not maps:
+        return []
+    maps = [m.to(dev) for m in maps]
+    sizes = [tuple(m.shape[1:]) for m in maps]
+    outs = [(q, h + 2 * pad_y - fh + 1, w + 2 * pad_x - fw + 1) for h, w in sizes]
+    # in place: contiguous maps of one storage, 4-byte aligned; else one packed copy
+    stor = maps[0].untyped_storage().data_ptr()
+    if all(m.is_contiguous() and m.untyped_storage().data_ptr() == stor for m in maps):
+        base, keep = stor, maps
+        offs = [(m.data_ptr() - base) // 4 for m in maps]
+    else:
+        keep = torch.cat([m.reshape(-1) for m in maps])
+        base = keep.data_ptr()
+        offs = np.concatenate([[0], np.cumsum([m.numel() for m in maps])[:-1]]).astype(np.int64).tolist()
+    descs, out_offs, pos = [], [], 0
+    for (h, w), o, (_, oh, ow) in zip(sizes, offs, outs):
+        descs.append(HogGridC(w, h, int(o), pos))
+        out_offs.append(pos)
+        if oh > 0 and ow > 0:
+            pos += q * oh * ow
+    table = (HogGridC * len(descs))(*descs)
+    d_table = torch.from_numpy(np.frombuffer(bytes(table), dtype=np.uint8).copy()).to(dev)
+    g = HogGridsC()
+    g.d_features, g.count, g.width, g.height, g.d_grids = base, len(maps), 0, 0, d_table.data_ptr()
+    out = torch.empty(max(pos, 1), dtype=torch.float32, device=dev)
+    _check(ctx.h, _capi.lib().sd_hog_correlate(ctx.h, C.byref(g), int(num_bins), int(variant), ptr(f), int(q), int(fw), int(fh),
+                                               ptr(b), pad_x, pad_y, ptr(out)))
+    return [out[o:o + q * oh * ow].view(q, oh, ow) if oh > 0 and ow > 0 else out.new_empty((q, max(oh, 0), max(ow, 0)))
+            for o, (_, oh, ow) in zip(out_offs, outs)]

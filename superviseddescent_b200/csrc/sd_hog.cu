@@ -61,10 +61,7 @@ struct HogArgs {
 // ---- per-sample geometry: IED -> half patch size (adaptive_vlhog.hpp:123) and the interpolation tables of cv::resize
 //      (INTER_LINEAR, 8U, 11-bit fixed point) for a P x P -> fs x fs resize, once per sample instead of once per thread of
 //      every one of its L patches.  One CTA per sample.  rtab[sample][0..4][fs]: x source index, x weights (2 x int16),
-//      y source index 0 / 1 (clamped), y weights. -------------------------------------------------------------------------
-__device__ __forceinline__ int clip_index(int x, int a, int b) { return x >= a ? (x < b ? x : b - 1) : a; }
-__device__ __forceinline__ short sat_short(int v) { return (short)(v > 32767 ? 32767 : (v < -32768 ? -32768 : v)); }
-
+//      y source index 0 / 1 (clamped), y weights (hog_resize_tap). ------------------------------------------------------
 __global__ void hog_geometry_kernel(const float* __restrict__ x, long long ldx, int N, int L, const sd_eyes_dev eyes, float rel,
                                     int fixed_half, int fs, int* __restrict__ half_out, int* __restrict__ rtab, int* __restrict__ status)
 {
@@ -82,24 +79,12 @@ __global__ void hog_geometry_kernel(const float* __restrict__ x, long long ldx, 
     const int P = 2 * s_half;
     int* rt = rtab + (long long)i * 5 * fs;
     for (int t = threadIdx.x; t < fs; t += blockDim.x) {
-        const double inv_scale = __ddiv_rn((double)fs, (double)P);
-        const double scale = __ddiv_rn(1.0, inv_scale);
-        float f = (float)__dadd_rn(__dmul_rn((double)t + 0.5, scale), -0.5);
-        const int s = (int)floorf(f);
-        f = __fsub_rn(f, (float)s);
-        int sx = s;
-        float fx = f;
-        if (sx < 0) { fx = 0.f; sx = 0; }
-        if (sx >= P - 1) { fx = 0.f; sx = P - 1; }
-        const short2 xa = make_short2(sat_short(__float2int_rn(__fmul_rn(__fsub_rn(1.f, fx), 2048.f))),
-                                      sat_short(__float2int_rn(__fmul_rn(fx, 2048.f))));
-        const short2 yb = make_short2(sat_short(__float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f))),
-                                      sat_short(__float2int_rn(__fmul_rn(f, 2048.f))));
-        rt[t] = sx;
-        rt[fs + t] = *reinterpret_cast<const int*>(&xa);
-        rt[2 * fs + t] = clip_index(s, 0, P);
-        rt[3 * fs + t] = clip_index(s + 1, 0, P);
-        rt[4 * fs + t] = *reinterpret_cast<const int*>(&yb);
+        const HogResizeTap r = hog_resize_tap(t, fs, P);
+        rt[t] = r.sx;
+        rt[fs + t] = r.xw;
+        rt[2 * fs + t] = r.y0;
+        rt[3 * fs + t] = r.y1;
+        rt[4 * fs + t] = r.yw;
     }
 }
 
@@ -127,13 +112,6 @@ __global__ void hog_bintab_kernel(int fs, int nc, int cs, float* __restrict__ bt
         lohi[c] = lo;
         lohi[nc + c] = hi;
     }
-}
-
-// cv::resize's vertical step of one output pixel from its horizontal sums t0, t1 of source rows 0 and 1 and the y weights
-// yb = weight 0 | weight 1 << 16 (int16 each): (b * (t >> 4)) >> 16 per row, then + 2 >> 2
-__device__ __forceinline__ int hog_resize_out(int yb, int t0, int t1)
-{
-    return (((((int)(short)yb) * (t0 >> 4)) >> 16) + (((yb >> 16) * (t1 >> 4)) >> 16) + 2) >> 2;
 }
 
 // byte n (0..7) of the 8 bytes lo, hi (little endian)

@@ -247,6 +247,49 @@ __device__ __forceinline__ void hog_cell_features(const double* fac, const float
     }
 }
 
+// ---- cv::resize INTER_LINEAR of 8-bit pixels (11-bit fixed point), the landmark patches' resize (sd_hog.cu) and the pyramid
+//      levels' (sd_hog_dense.cu).  The taps of output coordinate t of a src -> dst px axis, in OpenCV's arithmetic: scale =
+//      1 / (dst / src) in double, f = (t + 0.5) scale - 0.5 rounded to float, s = floor(f).  Column taps: source index sx (s
+//      clamped to [0, src - 1], where its fraction becomes 0) and the weights xw = (1 - fx) | fx << 16, each 2048 x rounded
+//      to int16; row taps: source rows y0, y1 (s and s + 1 clamped) and the weights yw of the unclamped fraction. ------------
+struct HogResizeTap {
+    int sx, xw, y0, y1, yw;
+};
+
+__device__ __forceinline__ int clip_index(int x, int a, int b) { return x >= a ? (x < b ? x : b - 1) : a; }
+__device__ __forceinline__ short sat_short(int v) { return (short)(v > 32767 ? 32767 : (v < -32768 ? -32768 : v)); }
+
+__device__ __forceinline__ HogResizeTap hog_resize_tap(int t, int dst, int src)
+{
+    const double inv_scale = __ddiv_rn((double)dst, (double)src);
+    const double scale = __ddiv_rn(1.0, inv_scale);
+    float f = (float)__dadd_rn(__dmul_rn((double)t + 0.5, scale), -0.5);
+    const int s = (int)floorf(f);
+    f = __fsub_rn(f, (float)s);
+    int sx = s;
+    float fx = f;
+    if (sx < 0) { fx = 0.f; sx = 0; }
+    if (sx >= src - 1) { fx = 0.f; sx = src - 1; }
+    const short2 xa = make_short2(sat_short(__float2int_rn(__fmul_rn(__fsub_rn(1.f, fx), 2048.f))),
+                                  sat_short(__float2int_rn(__fmul_rn(fx, 2048.f))));
+    const short2 yb = make_short2(sat_short(__float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f))),
+                                  sat_short(__float2int_rn(__fmul_rn(f, 2048.f))));
+    HogResizeTap r;
+    r.sx = sx;
+    r.xw = *reinterpret_cast<const int*>(&xa);
+    r.y0 = clip_index(s, 0, src);
+    r.y1 = clip_index(s + 1, 0, src);
+    r.yw = *reinterpret_cast<const int*>(&yb);
+    return r;
+}
+
+// cv::resize's vertical step of one output pixel from its horizontal sums t0, t1 of source rows 0 and 1 and the y weights
+// yb = weight 0 | weight 1 << 16 (int16 each): (b * (t >> 4)) >> 16 per row, then + 2 >> 2
+__device__ __forceinline__ int hog_resize_out(int yb, int t0, int t1)
+{
+    return (((((int)(short)yb) * (t0 >> 4)) >> 16) + (((yb >> 16) * (t1 >> 4)) >> 16) + 2) >> 2;
+}
+
 // ---- TMA staging: one thread copies the box at (x, y, z) of a 3-D tensor map (`bytes` bytes; x a multiple of 16, bytes
 //      outside the tensor zero-filled) to dst on the mbarrier at mbar, and every thread waits in hog_tma_wait ----------------
 __device__ __forceinline__ void hog_tma_load(uint64_t* mbar, void* dst, const CUtensorMap* map, int x, int y, int z, int bytes)

@@ -503,11 +503,46 @@ bool dense_shape(int width, int height, int cs, int K, int variant, int* hog_w, 
     return true;
 }
 
+// the configuration of hog_dense_kernel (sd_hog_dense, sd_hog_pyramid): tile, staged region and orientation table
+DenseArgs dense_args(const uint8_t* images, const sd_frame* frames, int cs, int K, int variant, int dd, float* out,
+                     const int64_t* out_offset)
+{
+    DenseArgs a;
+    memset(&a, 0, sizeof(a));
+    a.images = images;
+    a.frames = frames;
+    a.out = out;
+    a.out_offset = out_offset;
+    a.variant = variant; a.cs = cs; a.K = K; a.dd = dd;
+    a.tile = dense_tile(cs);
+    a.span = cs * (a.tile + 4) + 2;
+    a.pitch = dense_align(a.span + 15, 16);
+    hog_orientations(K, a.orient);   // hog.c:195-204
+    return a;
+}
+
+typedef void (*DenseKernel)(DenseArgs, CUtensorMap);
+
+DenseKernel dense_kernel(int K)
+{
+    return K == 4 ? hog_dense_kernel<4> : K == 9 ? hog_dense_kernel<9> : hog_dense_kernel<0>;
+}
+
 // a frame descriptor of sd_hog_dense_images: the size rule and non-negative offset and strides
 bool image_ok(const sd_hog_image& d, int cs, int K, int variant, int* hog_w, int* hog_h, int* dd)
 {
     return dense_shape(d.width, d.height, cs, K, variant, hog_w, hog_h, dd) && d.offset >= 0 && d.row_stride >= 0 &&
            d.pixel_stride >= 0 && d.channel_stride >= 0;
+}
+
+// a device descriptor table on the host, read back once
+template <class Frame>
+int fetch_frames(sd_ctx* ctx, const Frame* d_frames, int count, std::vector<Frame>& fr)
+{
+    fr.resize(count);
+    SD_CUDA(ctx, cudaMemcpyAsync(fr.data(), d_frames, sizeof(Frame) * count, cudaMemcpyDeviceToHost, ctx->stream));
+    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return SD_OK;
 }
 
 // The descriptor table of a batch, read back once: every frame passes the rules of its entry point (fn, for the messages),
@@ -516,9 +551,8 @@ template <class Frame>
 int read_frames(sd_ctx* ctx, const char* fn, const Frame* d_frames, int count, int cs, int K, int variant, bool offsets,
                 int* max_w, int* max_h, int* dd)
 {
-    std::vector<Frame> fr(count);
-    SD_CUDA(ctx, cudaMemcpyAsync(fr.data(), d_frames, sizeof(Frame) * count, cudaMemcpyDeviceToHost, ctx->stream));
-    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    std::vector<Frame> fr;
+    if (const int rc = fetch_frames(ctx, d_frames, count, fr)) return rc;
     bool uniform = true;
     for (int i = 0; i < count; ++i) {
         const Frame& d = fr[i];
@@ -556,6 +590,99 @@ int launch_dense(sd_ctx* ctx, const char* fn, const char* name, void (*kern)(Arg
         SD_LAUNCH_CHECK(ctx, name);
     }
     return SD_OK;
+}
+
+// ---- the pyramid (sd_hog_pyramid): every level of every frame resized into scratch (hog_pyramid_resize_kernel), then all of
+//      them through hog_dense_kernel as one batch of sd_frame descriptors (the load-loop route: the levels differ in size).
+//      The batch is cut into slices whose levels fit kPyramidSliceBytes (one frame at least), so the scratch is bounded by
+//      the slice, not by the batch.
+constexpr int kResizeW = 64, kResizeH = 16, kResizeThreads = 256;   // output pixels of a resize CTA
+constexpr size_t kPyramidSliceBytes = size_t(64) << 20;
+constexpr double kPyramidMaxSide = 1 << 28;                          // px per side of a level
+
+// level size of a width x height frame at scale (both in double, as cv::Size(round(width * scale))): false for a scale that
+// is not finite or lies outside (0, 4], or a frame or level outside [1, 2^28] px per side
+bool pyramid_level(int width, int height, double scale, int* lw, int* lh)
+{
+    if (!(scale > 0.0 && scale <= 4.0) || width < 1 || height < 1) return false;   // NaN fails the first test
+    const double w = floor((double)width * scale + 0.5), h = floor((double)height * scale + 0.5);
+    if (w > kPyramidMaxSide || h > kPyramidMaxSide) return false;
+    *lw = (int)w;
+    *lh = (int)h;
+    return true;
+}
+
+struct PyrLevel {
+    long long src, dst;          // byte offsets of the frame's first pixel from the batch's data, of the level's from the scratch
+    int W, H, rs;                // the frame: size and row stride
+    int w, h, pitch;             // the level: size and row stride
+    int tile0, tiles_x;          // the level's first CTA of the resize launch, and its CTAs per row of tiles
+    int slot;                    // frame * num_scales + scale: the caller's output offset of the level
+};
+
+struct ResizeArgs {
+    const uint8_t* images;
+    uint8_t* scratch;
+    const PyrLevel* levels;
+    int count;
+    const int64_t* out_offset;   // the caller's, per slot
+    int64_t* level_offset;       // per level: the caller's offset of its slot (the dense kernel's out_offset)
+};
+
+// One CTA per kResizeW x kResizeH tile of one level: the taps of its columns and rows (hog_resize_tap), then cv::resize's two
+// fixed-point passes per pixel, the source read through L1.  A level of the frame's own size is copied.
+__global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_kernel(const __grid_constant__ ResizeArgs a)
+{
+    __shared__ int s_sx[kResizeW], s_xw[kResizeW], s_y0[kResizeH], s_y1[kResizeH], s_yw[kResizeH];
+    const int b = blockIdx.x, tid = threadIdx.x;
+    int lo = 0, hi = a.count - 1;                    // the last level whose first tile is <= b
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (a.levels[mid].tile0 <= b) lo = mid;
+        else hi = mid - 1;
+    }
+    const PyrLevel L = a.levels[lo];
+    const int t = b - L.tile0, ty = t / L.tiles_x;
+    const int x0 = (t - ty * L.tiles_x) * kResizeW, y0 = ty * kResizeH;
+    if (t == 0 && tid == 0) a.level_offset[lo] = a.out_offset[L.slot];
+    const uint8_t* __restrict__ src = a.images + L.src;
+    uint8_t* __restrict__ dst = a.scratch + L.dst;
+    const bool copy = L.w == L.W && L.h == L.H;
+    if (!copy) {
+        if (tid < kResizeW) {
+            if (x0 + tid < L.w) {
+                const HogResizeTap r = hog_resize_tap(x0 + tid, L.w, L.W);
+                s_sx[tid] = r.sx;
+                s_xw[tid] = r.xw;
+            }
+        } else if (tid < kResizeW + kResizeH) {
+            const int i = tid - kResizeW;
+            if (y0 + i < L.h) {
+                const HogResizeTap r = hog_resize_tap(y0 + i, L.h, L.H);
+                s_y0[i] = r.y0;
+                s_y1[i] = r.y1;
+                s_yw[i] = r.yw;
+            }
+        }
+        __syncthreads();
+    }
+    for (int i = tid; i < kResizeW * kResizeH; i += kResizeThreads) {
+        const int r = i / kResizeW, c = i - r * kResizeW;
+        const int x = x0 + c, y = y0 + r;
+        if (x >= L.w || y >= L.h) continue;
+        int v;
+        if (copy) {
+            v = __ldg(src + (long long)y * L.rs + x);
+        } else {
+            const int sx = s_sx[c], sx1 = min(sx + 1, L.W - 1);   // a clamped tap has zero weight
+            const int ax = (short)s_xw[c], bx = s_xw[c] >> 16;
+            const uint8_t* r0 = src + (long long)s_y0[r] * L.rs;
+            const uint8_t* r1 = src + (long long)s_y1[r] * L.rs;
+            v = hog_resize_out(s_yw[r], (int)__ldg(r0 + sx) * ax + (int)__ldg(r0 + sx1) * bx,
+                               (int)__ldg(r1 + sx) * ax + (int)__ldg(r1 + sx1) * bx);
+        }
+        dst[(long long)y * L.pitch + x] = (uint8_t)v;
+    }
 }
 
 }  // namespace
@@ -599,20 +726,10 @@ int sd_hog_dense(sd_ctx* ctx, const sd_image_batch* images, int cell_size, int n
         SD_REQUIRE(ctx, images->row_stride >= images->width && (count == 1 || images->image_stride > 0), "bad strides");
     }
 
-    DenseArgs a;
-    memset(&a, 0, sizeof(a));
-    a.images = images->d_data;
+    DenseArgs a = dense_args(images->d_data, images->d_frames, cell_size, num_bins, variant, dd, d_out, d_out_offset);
     a.width = images->width; a.height = images->height; a.row_stride = images->row_stride;
     a.image_stride = images->image_stride;
-    a.frames = images->d_frames;
-    a.out = d_out;
-    a.out_offset = d_out_offset;
     a.out_stride = (long long)dd * max_w * max_h;
-    a.variant = variant; a.cs = cell_size; a.K = num_bins; a.dd = dd;
-    a.tile = dense_tile(cell_size);
-    a.span = cell_size * (a.tile + 4) + 2;
-    a.pitch = dense_align(a.span + 15, 16);
-    hog_orientations(num_bins, a.orient);   // hog.c:195-204
 
     // TMA staging: equally sized frames with 16-byte aligned base and pitches (a box of pitch x span bytes per CTA; bytes past
     // the frame's edge are zero-filled and never read)
@@ -620,11 +737,141 @@ int sd_hog_dense(sd_ctx* ctx, const sd_image_batch* images, int cell_size, int n
     memset(&map, 0, sizeof(map));
     a.tma = hog_frame_map(images, a.pitch, a.span, &map);
 
-    auto kern = hog_dense_kernel<0>;
-    if (num_bins == 4) kern = hog_dense_kernel<4>;
-    else if (num_bins == 9) kern = hog_dense_kernel<9>;
     const DenseSmem lay = dense_smem_layout(a.span, a.pitch, num_bins, dense_cells(a.tile));
-    return launch_dense(ctx, __func__, "hog_dense_kernel", kern, a, count, max_w, max_h, lay.total, map);
+    return launch_dense(ctx, __func__, "hog_dense_kernel", dense_kernel(num_bins), a, count, max_w, max_h, lay.total, map);
+}
+
+int sd_hog_pyramid_shape(int width, int height, double scale, int cell_size, int num_bins, int variant, int* level_w, int* level_h,
+                         int* hog_w, int* hog_h, int* dd)
+{
+    if (!level_w || !level_h || !hog_w || !hog_h || !dd) return SD_ERR_INVALID;
+    if (variant != 0 && variant != 1) return SD_ERR_INVALID;
+    if (num_bins < 1 || num_bins > SD_MAX_BINS || cell_size < 1 || cell_size > kDenseMaxCell) return SD_ERR_INVALID;
+    int lw, lh;
+    if (!pyramid_level(width, height, scale, &lw, &lh)) return SD_ERR_INVALID;
+    int w = 0, h = 0, d = variant == 1 ? 3 * num_bins + 4 : 4 * num_bins;
+    if (!dense_shape(lw, lh, cell_size, num_bins, variant, &w, &h, &d)) w = h = 0;   // an empty level
+    *level_w = lw;
+    *level_h = lh;
+    *hog_w = w;
+    *hog_h = h;
+    *dd = d;
+    return SD_OK;
+}
+
+int sd_hog_pyramid(sd_ctx* ctx, const sd_image_batch* images, const double* h_scales, int num_scales, int cell_size, int num_bins,
+                   int variant, float* d_out, const int64_t* d_out_offset)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, images && h_scales && d_out && d_out_offset, "null argument");
+    SD_REQUIRE(ctx, !images->d_roi, "a batch with regions of interest has no whole frames");
+    SD_REQUIRE(ctx, variant == 0 || variant == 1, "unknown HOG variant");
+    SD_REQUIRE(ctx, num_bins >= 1 && num_bins <= SD_MAX_BINS, "num_bins must be in [1,16]");
+    SD_REQUIRE(ctx, cell_size >= 1 && cell_size <= kDenseMaxCell, "cell_size must be in [1,32]");
+    SD_REQUIRE(ctx, num_scales >= 1, "num_scales must be at least 1");
+    for (int s = 0; s < num_scales; ++s)
+        SD_REQUIRE(ctx, h_scales[s] > 0.0 && h_scales[s] <= 4.0, "every scale must be finite and in (0, 4]");
+    SD_REQUIRE(ctx, images->count >= 0, "negative frame count");
+    const int count = images->count;
+    if (count == 0) return SD_OK;
+    SD_REQUIRE(ctx, images->d_data, "null argument");
+    SD_REQUIRE(ctx, (long long)count * num_scales <= INT_MAX, "too many levels");
+
+    // the frames: the batch's, or the descriptor table read back once
+    std::vector<sd_frame> fr;
+    if (images->d_frames) {
+        if (const int rc = fetch_frames(ctx, images->d_frames, count, fr)) return rc;
+    } else {
+        SD_REQUIRE(ctx, count == 1 || images->image_stride > 0, "bad strides");
+        fr.assign(count, sd_frame{images->width, images->height, images->row_stride, 0, 0});
+        for (int i = 0; i < count; ++i) fr[i].offset = (int64_t)i * images->image_stride;
+    }
+    // every level of every frame, in the order of the caller's slots; empty levels are left out
+    std::vector<PyrLevel> lv;
+    std::vector<int> first(count + 1, 0);           // frame f's levels are lv[first[f] .. first[f + 1])
+    for (int f = 0; f < count; ++f) {
+        const sd_frame& d = fr[f];
+        if (d.width < 1 || d.height < 1 || d.row_stride < d.width || d.offset < 0)
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d (%d x %d, row stride %d, offset %lld) is not a frame", __func__, f,
+                           d.width, d.height, d.row_stride, (long long)d.offset);
+        first[f] = (int)lv.size();
+        for (int s = 0; s < num_scales; ++s) {
+            PyrLevel L{};
+            int hw, hh, dd;
+            if (!pyramid_level(d.width, d.height, h_scales[s], &L.w, &L.h))
+                return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d at scale %g is larger than 2^28 px per side", __func__, f, h_scales[s]);
+            if (!dense_shape(L.w, L.h, cell_size, num_bins, variant, &hw, &hh, &dd)) continue;
+            L.src = d.offset;
+            L.W = d.width; L.H = d.height; L.rs = d.row_stride;
+            L.pitch = dense_align(L.w, 16);
+            L.tiles_x = sd_div_up(L.w, kResizeW);
+            L.slot = f * num_scales + s;
+            lv.push_back(L);
+        }
+    }
+    first[count] = (int)lv.size();
+    if (lv.empty()) return SD_OK;
+
+    const int dd = variant == 1 ? 3 * num_bins + 4 : 4 * num_bins;
+    DenseArgs a = dense_args(nullptr, nullptr, cell_size, num_bins, variant, dd, d_out, nullptr);
+    const DenseSmem lay = dense_smem_layout(a.span, a.pitch, num_bins, dense_cells(a.tile));
+    CUtensorMap map;                                 // not read: levels of different sizes are staged by the load loop
+    memset(&map, 0, sizeof(map));
+
+    // slices of whole frames whose levels fit kPyramidSliceBytes (one frame at least)
+    for (int f0 = 0; f0 < count;) {
+        size_t bytes = 0;
+        int f1 = f0;
+        for (; f1 < count; ++f1) {
+            size_t fb = 0;
+            for (int l = first[f1]; l < first[f1 + 1]; ++l) fb += (size_t)lv[l].pitch * lv[l].h;
+            if (f1 > f0 && bytes + fb > kPyramidSliceBytes) break;
+            bytes += fb;
+        }
+        const int l0 = first[f0], n = first[f1] - l0;
+        f0 = f1;
+        if (n == 0) continue;
+        // level positions in the scratch, the resize tiles, the dense kernel's descriptors and the grid that covers them
+        std::vector<sd_frame> desc(n);
+        long long pos = 0;
+        int tiles = 0, max_w = 0, max_h = 0;
+        for (int i = 0; i < n; ++i) {
+            PyrLevel& L = lv[l0 + i];
+            L.dst = pos;
+            L.tile0 = tiles;
+            SD_REQUIRE(ctx, (long long)tiles + (long long)L.tiles_x * sd_div_up(L.h, kResizeH) <= INT_MAX, "level too large");
+            tiles += L.tiles_x * sd_div_up(L.h, kResizeH);
+            desc[i] = sd_frame{L.w, L.h, L.pitch, 0, pos};
+            pos += (long long)L.pitch * L.h;
+            max_w = std::max(max_w, (L.w + cell_size / 2) / cell_size);
+            max_h = std::max(max_h, (L.h + cell_size / 2) / cell_size);
+        }
+        const size_t pix = sd_round16((size_t)pos), lv_bytes = sizeof(PyrLevel) * n, desc_bytes = sizeof(sd_frame) * n;
+        uint8_t* ws = static_cast<uint8_t*>(sd_workspace(ctx, SD_WS_PYRAMID, pix + lv_bytes + desc_bytes + sizeof(int64_t) * n));
+        if (!ws) return SD_ERR_CUDA;
+        PyrLevel* d_lv = reinterpret_cast<PyrLevel*>(ws + pix);
+        sd_frame* d_desc = reinterpret_cast<sd_frame*>(ws + pix + lv_bytes);
+        int64_t* d_off = reinterpret_cast<int64_t*>(ws + pix + lv_bytes + desc_bytes);
+        SD_CUDA(ctx, cudaMemcpyAsync(d_lv, lv.data() + l0, lv_bytes, cudaMemcpyHostToDevice, ctx->stream));
+        SD_CUDA(ctx, cudaMemcpyAsync(d_desc, desc.data(), desc_bytes, cudaMemcpyHostToDevice, ctx->stream));
+
+        ResizeArgs r;
+        r.images = images->d_data;
+        r.scratch = ws;
+        r.levels = d_lv;
+        r.count = n;
+        r.out_offset = d_out_offset;
+        r.level_offset = d_off;
+        hog_pyramid_resize_kernel<<<(unsigned)tiles, kResizeThreads, 0, ctx->stream>>>(r);
+        SD_LAUNCH_CHECK(ctx, "hog_pyramid_resize_kernel");
+
+        a.images = ws;
+        a.frames = d_desc;
+        a.out_offset = d_off;
+        if (const int rc = launch_dense(ctx, __func__, "hog_dense_kernel", dense_kernel(num_bins), a, n, max_w, max_h, lay.total, map))
+            return rc;
+    }
+    return SD_OK;
 }
 
 int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size, int num_bins, int variant,

@@ -210,9 +210,20 @@ __global__ void __launch_bounds__(kTile * 8) hog_relayout_kernel(const __grid_co
 
 // ---- shared by both entry points ----------------------------------------------------------------------------------------------
 
+int check_config(sd_ctx* ctx, const sd_hog_grids* grids, int num_bins, int variant)
+{
+    SD_REQUIRE(ctx, grids, "null argument");
+    SD_REQUIRE(ctx, variant == 0 || variant == 1, "unknown HOG variant");
+    SD_REQUIRE(ctx, num_bins >= 1 && num_bins <= SD_MAX_BINS, "num_bins must be in [1,16]");
+    SD_REQUIRE(ctx, grids->count >= 0, "negative grid count");
+    return SD_OK;
+}
+
+}  // namespace
+
 // The grids of a call: equally sized (packed, max_w x max_h cells), or the descriptor table read back once (the launch covers
-// the largest grid).  Returns SD_OK, or an sd_fail status before anything is queued.
-int read_grids(sd_ctx* ctx, const char* fn, const sd_hog_grids* grids, int* max_w, int* max_h)
+// the largest grid; *table, if given, receives it).  Returns SD_OK, or an sd_fail status before anything is queued.
+int sd_read_hog_grids(sd_ctx* ctx, const char* fn, const sd_hog_grids* grids, int* max_w, int* max_h, std::vector<sd_hog_grid>* table)
 {
     const int count = grids->count;
     if (!grids->d_grids) {
@@ -233,19 +244,9 @@ int read_grids(sd_ctx* ctx, const char* fn, const sd_hog_grids* grids, int* max_
         *max_w = std::max(*max_w, (int)d.width);
         *max_h = std::max(*max_h, (int)d.height);
     }
+    if (table) table->swap(t);
     return SD_OK;
 }
-
-int check_config(sd_ctx* ctx, const sd_hog_grids* grids, int num_bins, int variant)
-{
-    SD_REQUIRE(ctx, grids, "null argument");
-    SD_REQUIRE(ctx, variant == 0 || variant == 1, "unknown HOG variant");
-    SD_REQUIRE(ctx, num_bins >= 1 && num_bins <= SD_MAX_BINS, "num_bins must be in [1,16]");
-    SD_REQUIRE(ctx, grids->count >= 0, "negative grid count");
-    return SD_OK;
-}
-
-}  // namespace
 
 extern "C" {
 
@@ -273,7 +274,7 @@ int sd_hog_render(sd_ctx* ctx, const sd_hog_grids* grids, int num_bins, int vari
     if (count == 0) return SD_OK;
     SD_REQUIRE(ctx, grids->d_features, "null argument");
     int max_w = 0, max_h = 0;
-    if (const int rc = read_grids(ctx, __func__, grids, &max_w, &max_h)) return rc;
+    if (const int rc = sd_read_hog_grids(ctx, __func__, grids, &max_w, &max_h, nullptr)) return rc;
     const int tiles_x = sd_div_up(max_w, kRenderCells);
     SD_REQUIRE(ctx, (long long)tiles_x * max_h <= INT_MAX, "grid too large");
 
@@ -312,7 +313,7 @@ int sd_hog_relayout(sd_ctx* ctx, const sd_hog_grids* grids, int num_bins, int va
     SD_REQUIRE(ctx, grids->d_features, "null argument");
     SD_REQUIRE(ctx, grids->d_features != d_out, "the relayout is out of place: d_out must not be the input");
     int max_w = 0, max_h = 0;
-    if (const int rc = read_grids(ctx, __func__, grids, &max_w, &max_h)) return rc;
+    if (const int rc = sd_read_hog_grids(ctx, __func__, grids, &max_w, &max_h, nullptr)) return rc;
     const int dd = dims_of(num_bins, variant);
     const int tiles_x = sd_div_up(max_w, kTile);
     SD_REQUIRE(ctx, (long long)tiles_x * sd_div_up(max_h, kTile) <= INT_MAX, "grid too large");

@@ -21,7 +21,9 @@ enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_UPLOAD /* B,G,R scratch of sd_upload_frames */,
        SD_WS_RANK /* the rank diagnostic's working copy of the D x D system, its panel and state (sd_rank.cu) */,
        SD_WS_LEVEL /* column shift and shifted-row weights of sd_train_level (sd_train.cu) */,
-       SD_WS_GATHER /* frame, union, region, record and index tables of the levels on host frames (sd_train.cu) */, SD_WS_COUNT };
+       SD_WS_GATHER /* frame, union, region, record and index tables of the levels on host frames (sd_train.cu) */,
+       SD_WS_PYRAMID /* resized levels and level tables of one slice of sd_hog_pyramid (sd_hog_dense.cu) */,
+       SD_WS_FILTERS /* first CTA of every grid of sd_hog_correlate (sd_hog_filters.cu) */, SD_WS_COUNT };
 
 // Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row
 // Cholesky blocks), and panel p belongs to rank p % nranks.  The Gram exchange delivers each panel's rows to their owner, and
@@ -125,6 +127,8 @@ int syrk_upper(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ
 bool syrk_is_big(int K, int64_t MI, int64_t NJ);
 
 int sd_check_hog_status(sd_ctx* ctx, const char* what);   // sd_api.cu: synchronises, reports and clears the projection's flags
+// the grids of an sd_hog_grids call, validated; per-grid descriptors are read back once into *table (if given) (sd_hog_render.cu)
+int sd_read_hog_grids(sd_ctx* ctx, const char* fn, const sd_hog_grids* grids, int* max_w, int* max_h, std::vector<sd_hog_grid>* table);
 
 // The learn path of sd_learn_centred in two steps (sd_linalg.cu), so that a training level can add its rows chunk by chunk
 // (sd_train.cu).  The Gram lives in the context's workspace (D x sd_learn_ldg floats).

@@ -7,6 +7,7 @@
 // HOG run in sd_hog_batch (sm_90a).
 #pragma once
 
+#include <algorithm>
 #include <cstring>
 #include <map>
 #include <memory>
@@ -237,6 +238,111 @@ inline std::vector<cv::Mat> hog_dense(const std::vector<cv::Mat>& images, VlHogV
     sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_offset.as<int64_t>(), offset.data(), static_cast<size_t>(n) * sizeof(int64_t)), "hog_dense");
     sd_b200::check(ctx, sd_hog_dense(ctx, &batch, cell_size, num_bins, variant, d_out.as<float>(), d_offset.as<int64_t>()), "sd_hog_dense");
     for (int i = 0; i < n; ++i) out.push_back(sd_b200::download(d_out.as<float>() + offset[i], rows[i], cols[i], cols[i]));
+    return out;
+}
+
+// Dense HOG of every frame at every scale, in one batched call on the device (sd_hog_pyramid): level s of a W x H frame is the
+// frame resized by cv::resize INTER_LINEAR to floor(W * s + 0.5) x floor(H * s + 0.5), and its features are hog_dense's of that
+// level.  Returns, per frame, one Mat per scale as hog_dense returns it (dd * hogH rows of hogW columns), or an empty Mat for
+// an empty level (smaller than 4 px or than half a cell).  Throws std::runtime_error for no scales, a scale outside (0, 4], or
+// a configuration that sd_hog_pyramid_shape refuses.
+inline std::vector<std::vector<cv::Mat>> vl_hog_pyramid(const std::vector<cv::Mat>& images, const std::vector<double>& scales,
+                                                        VlHogVariant variant, int cell_size, int num_bins)
+{
+    std::vector<std::vector<cv::Mat>> out;
+    if (images.empty()) return out;
+    if (scales.empty()) throw std::runtime_error("vl_hog_pyramid: no scales");
+    sd_ctx* ctx = sd_b200::context();
+    const std::vector<sd_host_frame> frames = sd_b200::host_frames(images);
+    const int n = static_cast<int>(frames.size()), S = static_cast<int>(scales.size());
+    std::vector<int64_t> offset(static_cast<size_t>(n) * S);
+    std::vector<int> rows(offset.size()), cols(offset.size());
+    int64_t total = 0;
+    for (int i = 0; i < n; ++i)
+        for (int s = 0; s < S; ++s) {
+            int lw = 0, lh = 0, w = 0, h = 0, dd = 0;
+            if (sd_hog_pyramid_shape(frames[i].width, frames[i].height, scales[s], cell_size, num_bins, variant, &lw, &lh, &w, &h, &dd) != SD_OK)
+                throw std::runtime_error("vl_hog_pyramid: frame " + std::to_string(i) + " at scale " + std::to_string(scales[s]) +
+                                         " or the configuration is invalid: scales in (0, 4], cell_size 1..32, num_bins 1..16");
+            const size_t l = static_cast<size_t>(i) * S + s;
+            offset[l] = total;
+            rows[l] = dd * h;
+            cols[l] = w;
+            total += static_cast<int64_t>(dd) * h * w;
+        }
+    size_t bytes = 0;
+    sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, nullptr, &bytes, nullptr), "vl_hog_pyramid upload");
+    sd_b200::DeviceBuffer buf(bytes), d_out(static_cast<size_t>(std::max<int64_t>(total, 1)) * sizeof(float)),
+        d_offset(offset.size() * sizeof(int64_t));
+    sd_image_batch batch{};
+    sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, buf.as<void>(), &bytes, &batch), "vl_hog_pyramid upload");
+    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_offset.as<int64_t>(), offset.data(), offset.size() * sizeof(int64_t)), "vl_hog_pyramid");
+    sd_b200::check(ctx, sd_hog_pyramid(ctx, &batch, scales.data(), S, cell_size, num_bins, variant, d_out.as<float>(),
+                                       d_offset.as<int64_t>()), "sd_hog_pyramid");
+    for (int i = 0; i < n; ++i) {
+        std::vector<cv::Mat> levels;
+        for (int s = 0; s < S; ++s) {
+            const size_t l = static_cast<size_t>(i) * S + s;
+            levels.push_back(cols[l] ? sd_b200::download(d_out.as<float>() + offset[l], rows[l], cols[l], cols[l]) : cv::Mat());
+        }
+        out.push_back(levels);
+    }
+    return out;
+}
+
+// Scores of a bank of HOG filters over HOG grids, in one batched call on the device (sd_hog_correlate).  maps: grids as
+// hog_dense returns them (CV_32FC1, dd * h rows of w columns); filters: Q filters in the same layout, dd * fh rows of fw
+// columns each (hog_dense of a template image is one); bias: Q values, or empty for none.  Returns one CV_32FC1 Mat per map of
+// Q * oh rows and ow columns, filter q's score map in rows q * oh .. q * oh + oh - 1, with oh = h + 2 pad_y - fh + 1 and
+// ow = w + 2 pad_x - fw + 1 (an empty Mat when either is <= 0).  Throws std::runtime_error for maps or filters of the wrong
+// shape, and for a configuration that sd_hog_correlate refuses.
+inline std::vector<cv::Mat> vl_hog_correlate(const std::vector<cv::Mat>& maps, const std::vector<cv::Mat>& filters, VlHogVariant variant,
+                                             int num_bins, const std::vector<float>& bias, int pad_x, int pad_y)
+{
+    std::vector<cv::Mat> out;
+    if (maps.empty()) return out;
+    sd_ctx* ctx = sd_b200::context();
+    const int dd = variant == VlHogVariantUoctti ? 3 * num_bins + 4 : 4 * num_bins;
+    const int Q = static_cast<int>(filters.size());
+    if (Q < 1 || dd < 1 || filters[0].rows % dd) throw std::runtime_error("vl_hog_correlate: no filters, or filters not dd * fh rows");
+    const int fh = filters[0].rows / dd, fw = filters[0].cols;
+    if (!bias.empty() && static_cast<int>(bias.size()) != Q) throw std::runtime_error("vl_hog_correlate: one bias per filter");
+    // filters and maps packed on the host, then one upload each
+    std::vector<float> hf;
+    for (const cv::Mat& f : filters) {
+        if (f.type() != CV_32FC1 || f.rows != dd * fh || f.cols != fw) throw std::runtime_error("vl_hog_correlate: filters differ in shape");
+        for (int r = 0; r < f.rows; ++r) hf.insert(hf.end(), f.ptr<float>(r), f.ptr<float>(r) + f.cols);
+    }
+    std::vector<float> hm;
+    std::vector<sd_hog_grid> grids;
+    std::vector<int> oh(maps.size()), ow(maps.size());
+    int64_t pos = 0;
+    for (size_t i = 0; i < maps.size(); ++i) {
+        const cv::Mat& m = maps[i];
+        if (m.type() != CV_32FC1 || m.rows < dd || m.rows % dd || m.cols < 1)
+            throw std::runtime_error("vl_hog_correlate: map " + std::to_string(i) + " is not dd * h rows of w columns");
+        const int h = m.rows / dd, w = m.cols;
+        oh[i] = h + 2 * pad_y - fh + 1;
+        ow[i] = w + 2 * pad_x - fw + 1;
+        grids.push_back(sd_hog_grid{w, h, static_cast<int64_t>(hm.size()), pos});
+        for (int r = 0; r < m.rows; ++r) hm.insert(hm.end(), m.ptr<float>(r), m.ptr<float>(r) + m.cols);
+        if (oh[i] > 0 && ow[i] > 0) pos += static_cast<int64_t>(Q) * oh[i] * ow[i];
+    }
+    sd_b200::DeviceBuffer d_maps(hm.size() * sizeof(float)), d_filters(hf.size() * sizeof(float)),
+        d_bias(std::max<size_t>(bias.size(), 1) * sizeof(float)), d_grids(grids.size() * sizeof(sd_hog_grid)),
+        d_scores(static_cast<size_t>(std::max<int64_t>(pos, 1)) * sizeof(float));
+    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_maps.as<float>(), hm.data(), hm.size() * sizeof(float)), "vl_hog_correlate");
+    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_filters.as<float>(), hf.data(), hf.size() * sizeof(float)), "vl_hog_correlate");
+    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_grids.as<sd_hog_grid>(), grids.data(), grids.size() * sizeof(sd_hog_grid)), "vl_hog_correlate");
+    if (!bias.empty()) sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_bias.as<float>(), bias.data(), bias.size() * sizeof(float)), "vl_hog_correlate");
+    sd_hog_grids g{};
+    g.d_features = d_maps.as<float>();
+    g.count = static_cast<int32_t>(maps.size());
+    g.d_grids = d_grids.as<sd_hog_grid>();
+    sd_b200::check(ctx, sd_hog_correlate(ctx, &g, num_bins, variant, d_filters.as<float>(), Q, fw, fh, bias.empty() ? nullptr : d_bias.as<float>(),
+                                         pad_x, pad_y, d_scores.as<float>()), "sd_hog_correlate");
+    for (size_t i = 0; i < maps.size(); ++i)
+        out.push_back(oh[i] > 0 && ow[i] > 0 ? sd_b200::download(d_scores.as<float>() + grids[i].out_offset, Q * oh[i], ow[i], ow[i]) : cv::Mat());
     return out;
 }
 
