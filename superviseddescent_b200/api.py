@@ -16,6 +16,8 @@ from __future__ import annotations
 
 import ctypes as C
 import enum
+import itertools
+import math
 from typing import Callable, List, Optional, Sequence
 
 import numpy as np
@@ -112,12 +114,13 @@ def default_context() -> Context:
     return _default_ctx
 
 
+def _tensor(a) -> torch.Tensor:
+    """A tensor as given; an array (or anything numpy takes) as a tensor over a contiguous copy of it."""
+    return a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))
+
+
 def _dev(a, ctx: Context, dtype=torch.float32) -> torch.Tensor:
-    if isinstance(a, torch.Tensor):
-        t = a.to(device=f"cuda:{ctx.device}", dtype=dtype)
-    else:
-        t = torch.from_numpy(np.ascontiguousarray(a)).to(device=f"cuda:{ctx.device}", dtype=dtype)
-    return t.contiguous()
+    return _tensor(a).to(device=f"cuda:{ctx.device}", dtype=dtype).contiguous()
 
 
 # ------------------------------------------------------------------------------------------------
@@ -320,7 +323,7 @@ def bgr2gray(images, ctx: Optional["Context"] = None) -> torch.Tensor:
     """cv::cvtColor(BGR2GRAY) on the device (adaptive_vlhog.hpp:114-120): (count, H, W, 3) uint8 -> (count, H, W) uint8.
     Host arrays are uploaded first; the result stays in HBM."""
     ctx = ctx or default_context()
-    t = images if isinstance(images, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(images))
+    t = _tensor(images)
     if t.dim() == 3:
         t = t.unsqueeze(0)
     if t.dtype != torch.uint8 or t.dim() != 4 or t.shape[3] != 3:
@@ -342,7 +345,7 @@ def _device_images(images, ctx: Context):
     if isinstance(images, (list, tuple)):
         frames = list(images)
     else:
-        t = images if isinstance(images, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(images))
+        t = _tensor(images)
         if t.dim() == 2:
             t = t.unsqueeze(0)
         if t.dtype != torch.uint8 or not (t.dim() == 3 or (t.dim() == 4 and t.shape[3] == 3)):
@@ -353,13 +356,7 @@ def _device_images(images, ctx: Context):
             n, h, w = t.shape
             return t, ImageBatchC(C.c_void_p(t.data_ptr()), w, h, t.stride(1), t.stride(0), n)
         frames = list(t)
-    recs, keep = [], []
-    for f in frames:
-        rec, a = _host_frame(f)
-        if a.ndim == 3 and a.shape[2] != 3:
-            raise ValueError("every image must be (H, W) uint8 or (H, W, 3) uint8")
-        recs.append(rec)
-        keep.append(a)                                       # the bytes stay alive until the upload returns
+    recs, keep = _host_frames(frames)                       # keep: the bytes stay alive until the upload returns
     return _upload_host_frames(recs, ctx)
 
 
@@ -373,6 +370,58 @@ def _upload_host_frames(recs, ctx: Context):
     ib = ImageBatchC()
     _check(ctx.h, _capi.lib().sd_upload_frames(ctx.h, table, len(recs), ptr(buf), C.byref(nbytes), C.byref(ib)))
     return buf, ib
+
+
+# ------------------------------------------------------------------------------------------------
+# batches of the dense-HOG calls: items packed end to end, descriptor tables, result buffers
+# ------------------------------------------------------------------------------------------------
+def _starts(counts):
+    """The offset of each item when items of these element counts lie end to end."""
+    return list(itertools.accumulate(counts, initial=0))[:-1]
+
+
+def _pack(items, dev):
+    """Tensors -> (one device buffer of their elements, end to end, in one copy; the element offset of each)."""
+    return torch.cat([t.reshape(-1) for t in items]).to(dev), _starts([t.numel() for t in items])
+
+
+def _device_table(descs, dev) -> torch.Tensor:
+    """A non-empty list of descriptors of one ctypes Structure type, as one table in a device tensor that owns its bytes."""
+    table = (type(descs[0]) * len(descs))(*descs)
+    return torch.from_numpy(np.frombuffer(bytes(table), dtype=np.uint8).copy()).to(dev)
+
+
+def _results(shapes, dev, zero: bool = False):
+    """The float32 results of a call, in one new device buffer -> (buffer, element offsets, results).
+
+    shapes: one tuple, the shape of a batch tensor, which is the buffer itself (offsets None); or a list of per-item shapes,
+    laid end to end and returned as a list of views, None for an item whose shape is None.  The buffer of a list has at least
+    one element, so that a call whose items are all empty still gets a valid pointer.  zero: the buffer starts zeroed."""
+    alloc = torch.zeros if zero else torch.empty
+    if isinstance(shapes, tuple):
+        out = alloc(shapes, dtype=torch.float32, device=dev)
+        return out, None, out
+    counts = [0 if s is None else math.prod(s) for s in shapes]
+    offsets = _starts(counts)
+    out = alloc(max(sum(counts), 1), dtype=torch.float32, device=dev)
+    return out, offsets, [None if s is None else out[o:o + c].view(s) for o, c, s in zip(offsets, counts, shapes)]
+
+
+def _dense_results(ctx, sizes, frame, cell_size: int, num_bins: int, variant: int, run):
+    """The dense HOG of frames of sizes [(H, W)], written by run(out, offsets).  frame: the (H, W) of every frame when the call
+    describes its frames as one batch, without a descriptor table; the result is then one (count, dd, hogH, hogW) tensor
+    (offsets None), and for no frames run is not called.  Otherwise it is a list of (dd, hogH, hogW) views of one buffer, at
+    the int64 element offsets that offsets holds on the device."""
+    dev = f"cuda:{ctx.device}"
+    if frame is not None:
+        h, w = frame
+        out, _, res = _results((len(sizes),) + hog_dense_shape(w, h, cell_size, num_bins, variant), dev)
+        if sizes:
+            run(out, None)
+        return res
+    out, offsets, res = _results([hog_dense_shape(w, h, cell_size, num_bins, variant) for h, w in sizes], dev)
+    run(out, torch.tensor(offsets, dtype=torch.int64, device=dev))
+    return res
 
 
 # ------------------------------------------------------------------------------------------------
@@ -408,13 +457,7 @@ def _grey_frames(frames, ctx: Context, check):
         if a.dtype != np.uint8 or not (a.ndim == 3 or (a.ndim == 4 and a.shape[3] == 3)):
             raise ValueError("frames must be (count, H, W) uint8, (count, H, W, 3) uint8, or a list of such frames of any sizes")
         frames = list(a)
-    recs, arrays = [], []
-    for f in frames:
-        rec, a = _host_frame(f)
-        if a.ndim == 3 and a.shape[2] != 3:
-            raise ValueError("every frame must be (H, W) uint8 or (H, W, 3) uint8")
-        recs.append(rec)
-        arrays.append(a)                                  # the bytes stay alive until the upload returns
+    recs, arrays = _host_frames(frames)                   # arrays: the bytes stay alive until the upload returns
     sizes = [(r.height, r.width) for r in recs]
     if not recs:
         return None, None, []
@@ -438,22 +481,9 @@ def hog_dense(frames, cell_size: int, num_bins: int, variant: int = 1, ctx: Opti
     keep, ib, sizes = _grey_frames(frames, ctx, lambda w, h: hog_dense_shape(w, h, cell_size, num_bins, variant))
     if ib is None:
         return []
-    n = len(sizes)
-    dev = f"cuda:{ctx.device}"
-    if n == 0:
-        return torch.empty((0,) + hog_dense_shape(keep.shape[2], keep.shape[1], cell_size, num_bins, variant), dtype=torch.float32,
-                           device=dev)
-    shapes = [hog_dense_shape(w, h, cell_size, num_bins, variant) for h, w in sizes]
-    if len(set(shapes)) == 1:
-        out = torch.empty((n,) + shapes[0], dtype=torch.float32, device=dev)
-        _check(ctx.h, lib.sd_hog_dense(ctx.h, C.byref(ib), int(cell_size), int(num_bins), int(variant), ptr(out), None))
-        return out
-    counts = [d * h * w for d, h, w in shapes]
-    starts = np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.int64)
-    offsets = torch.from_numpy(starts).to(dev)
-    out = torch.empty(int(sum(counts)), dtype=torch.float32, device=dev)
-    _check(ctx.h, lib.sd_hog_dense(ctx.h, C.byref(ib), int(cell_size), int(num_bins), int(variant), ptr(out), ptr(offsets)))
-    return [out[s:s + c].view(shape) for s, c, shape in zip(starts.tolist(), counts, shapes)]
+    return _dense_results(ctx, sizes, None if ib.d_frames else (ib.height, ib.width), cell_size, num_bins, variant,
+                          lambda out, offsets: _check(ctx.h, lib.sd_hog_dense(ctx.h, C.byref(ib), int(cell_size), int(num_bins),
+                                                                              int(variant), ptr(out), ptr(offsets))))
 
 
 _VL_HOG_DTYPES = {torch.uint8: 0, torch.float32: 1}    # SD_HOG_U8, SD_HOG_F32
@@ -489,9 +519,6 @@ def vl_hog(images, cell_size: int, num_bins: int, variant: int = 1, bilinear_ori
     dev = f"cuda:{ctx.device}"
     lib = _capi.lib()
 
-    def tensor(a):
-        return a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))
-
     def dtype_of(t):
         if t.dtype not in _VL_HOG_DTYPES:
             raise ValueError("frames must be uint8 or float32")
@@ -500,7 +527,7 @@ def vl_hog(images, cell_size: int, num_bins: int, variant: int = 1, bilinear_ori
     ib = HogImagesC()
     ib.d_frames = None
     if isinstance(images, (list, tuple)):
-        frames = [tensor(f) for f in images]
+        frames = [_tensor(f) for f in images]
         if not frames:
             return []
         if any(f.dim() not in (2, 3) for f in frames):
@@ -515,20 +542,17 @@ def vl_hog(images, cell_size: int, num_bins: int, variant: int = 1, bilinear_ori
         sizes = [(d.height, d.width) for _, d in descs]
         for h, w in set(sizes):
             hog_dense_shape(w, h, cell_size, num_bins, variant)   # refuse before the upload
-        pos = 0
-        for f, (_, d) in zip(frames, descs):
-            d.offset = pos
-            pos += f.numel()
-        keep = torch.cat([f.reshape(-1) for f in frames]).to(dev)
+        keep, offsets = _pack(frames, dev)
+        for (_, d), o in zip(descs, offsets):
+            d.offset = o
         ib.channels, ib.count = descs[0][0], len(frames)
         if len(set(sizes)) == 1:
             ib.frame, ib.image_stride = descs[0][1], frames[0].numel()
         else:
-            table = (HogImageC * len(descs))(*[d for _, d in descs])
-            keep_table = torch.from_numpy(np.frombuffer(bytes(table), dtype=np.uint8).copy()).to(dev)
+            keep_table = _device_table([d for _, d in descs], dev)
             ib.d_frames = keep_table.data_ptr()
     else:
-        t = tensor(images)
+        t = _tensor(images)
         if t.dim() not in (3, 4):
             raise ValueError("a batch of frames must be (count, H, W), (count, C, H, W), or (count, H, W, C) with channels_last=True")
         dt = dtype_of(t)
@@ -537,22 +561,10 @@ def vl_hog(images, cell_size: int, num_bins: int, variant: int = 1, bilinear_ori
         ib.count, ib.image_stride = keep.shape[0], keep.stride(0)
         sizes = [(ib.frame.height, ib.frame.width)] * ib.count
     ib.d_data, ib.dtype = keep.data_ptr(), dt
-    n = len(sizes)
-    if n == 0:
-        return torch.empty((0,) + hog_dense_shape(ib.frame.width, ib.frame.height, cell_size, num_bins, variant), dtype=torch.float32,
-                           device=dev)
-    shapes = [hog_dense_shape(w, h, cell_size, num_bins, variant) for h, w in sizes]
     bil = int(bool(bilinear_orientations))
-    if len(set(shapes)) == 1:
-        out = torch.empty((n,) + shapes[0], dtype=torch.float32, device=dev)
-        _check(ctx.h, lib.sd_hog_dense_images(ctx.h, C.byref(ib), int(cell_size), int(num_bins), int(variant), bil, ptr(out), None))
-        return out
-    counts = [d * h * w for d, h, w in shapes]
-    starts = np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.int64)
-    offsets = torch.from_numpy(starts).to(dev)
-    out = torch.empty(int(sum(counts)), dtype=torch.float32, device=dev)
-    _check(ctx.h, lib.sd_hog_dense_images(ctx.h, C.byref(ib), int(cell_size), int(num_bins), int(variant), bil, ptr(out), ptr(offsets)))
-    return [out[s:s + c].view(shape) for s, c, shape in zip(starts.tolist(), counts, shapes)]
+    return _dense_results(ctx, sizes, None if ib.d_frames else (ib.frame.height, ib.frame.width), cell_size, num_bins, variant,
+                          lambda out, offsets: _check(ctx.h, lib.sd_hog_dense_images(ctx.h, C.byref(ib), int(cell_size), int(num_bins),
+                                                                                     int(variant), bil, ptr(out), ptr(offsets))))
 
 
 # The distinct frames of a HogTransform are uploaded when their grey bytes fit in this share of the device's free memory (read when
@@ -637,10 +649,7 @@ class HogTransform:
     def _distinct(images):
         """(list of (sd_host_frame, owning array) of the distinct frames, list entry -> frame index)"""
         frames, index, seen = [], np.empty(len(images), dtype=np.int32), {}
-        for i, f in enumerate(images):
-            rec, a = _host_frame(f)
-            if a.ndim == 3 and a.shape[2] != 3:
-                raise ValueError("every image must be (H, W) uint8 or (H, W, 3) uint8")
+        for i, (rec, a) in enumerate(zip(*_host_frames(images))):
             key = (a.ctypes.data, a.shape, a.strides)
             if key not in seen:
                 seen[key] = len(frames)
@@ -1214,6 +1223,19 @@ def _host_frame(frame):
     return HostFrameC(a.ctypes.data, a.shape[1], a.shape[0], a.strides[0], ch), a
 
 
+def _host_frames(frames):
+    """(H, W) / (H, W, 3) uint8 host frames -> (their sd_host_frame records, the arrays that own the bytes the records point
+    to)."""
+    recs, arrays = [], []
+    for f in frames:
+        rec, a = _host_frame(f)
+        if a.ndim == 3 and a.shape[2] != 3:
+            raise ValueError("every frame must be (H, W) uint8 or (H, W, 3) uint8")
+        recs.append(rec)
+        arrays.append(a)
+    return recs, arrays
+
+
 class detection_model:
     """rcr::detection_model (model.hpp:122-183) resident on the GPU."""
 
@@ -1362,11 +1384,8 @@ def vl_hog_polar(modulus, angle, cell_size: int, num_bins: int, variant: int = 1
     dev = torch.device(f"cuda:{ctx.device}")
     lib = _capi.lib()
 
-    def tensor(a):
-        return a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))
-
     def checked(m, a, dims):
-        m, a = tensor(m), tensor(a)
+        m, a = _tensor(m), _tensor(a)
         if m.dtype != torch.float32 or a.dtype != torch.float32:
             raise ValueError("modulus and angle must be float32")
         if m.dim() != dims or tuple(m.shape) != tuple(a.shape):
@@ -1384,18 +1403,14 @@ def vl_hog_polar(modulus, angle, cell_size: int, num_bins: int, variant: int = 1
         sizes = [tuple(m.shape) for m, _ in pairs]
         for h, w in set(sizes):
             hog_dense_shape(w, h, cell_size, num_bins, variant)   # refuse before the upload
-        descs, pos = [], 0
-        for h, w in sizes:
-            descs.append(HogImageC(w, h, pos, w, 1, 0))
-            pos += h * w
-        keep_m = torch.cat([m.reshape(-1) for m, _ in pairs]).to(dev)
-        keep_a = torch.cat([a.reshape(-1) for _, a in pairs]).to(dev)
+        keep_m, offsets = _pack([m for m, _ in pairs], dev)
+        keep_a, _ = _pack([a for _, a in pairs], dev)
+        descs = [HogImageC(w, h, o, w, 1, 0) for (h, w), o in zip(sizes, offsets)]
         fb.count = len(pairs)
         if len(set(sizes)) == 1:
             fb.frame, fb.image_stride = descs[0], sizes[0][0] * sizes[0][1]
         else:
-            table = (HogImageC * len(descs))(*descs)
-            keep_table = torch.from_numpy(np.frombuffer(bytes(table), dtype=np.uint8).copy()).to(dev)
+            keep_table = _device_table(descs, dev)
             fb.d_frames = keep_table.data_ptr()
     else:
         m, a = checked(modulus, angle, 3)
@@ -1406,22 +1421,9 @@ def vl_hog_polar(modulus, angle, cell_size: int, num_bins: int, variant: int = 1
         fb.count, fb.frame, fb.image_stride = n, HogImageC(w, h, 0, m.stride(1), m.stride(2), 0), m.stride(0)
         sizes = [(h, w)] * n
     fb.d_modulus, fb.d_angle = keep_m.data_ptr(), keep_a.data_ptr()
-    n = len(sizes)
-    if n == 0:
-        return torch.empty((0,) + hog_dense_shape(fb.frame.width, fb.frame.height, cell_size, num_bins, variant), dtype=torch.float32,
-                           device=dev)
-    shapes = [hog_dense_shape(w, h, cell_size, num_bins, variant) for h, w in sizes]
     flags = (int(cell_size), int(num_bins), int(variant), int(bool(directed)), int(bool(bilinear_orientations)))
-    if len(set(sizes)) == 1:
-        out = torch.empty((n,) + shapes[0], dtype=torch.float32, device=dev)
-        _check(ctx.h, lib.sd_hog_dense_polar(ctx.h, C.byref(fb), *flags, ptr(out), None))
-        return out
-    counts = [d * h * w for d, h, w in shapes]
-    starts = np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.int64)
-    offsets = torch.from_numpy(starts).to(dev)
-    out = torch.empty(int(sum(counts)), dtype=torch.float32, device=dev)
-    _check(ctx.h, lib.sd_hog_dense_polar(ctx.h, C.byref(fb), *flags, ptr(out), ptr(offsets)))
-    return [out[s:s + c].view(shape) for s, c, shape in zip(starts.tolist(), counts, shapes)]
+    return _dense_results(ctx, sizes, None if fb.d_frames else (fb.frame.height, fb.frame.width), cell_size, num_bins, variant,
+                          lambda out, offsets: _check(ctx.h, lib.sd_hog_dense_polar(ctx.h, C.byref(fb), *flags, ptr(out), ptr(offsets))))
 
 
 GLYPH_SIZE = 21     # SD_HOG_GLYPH_SIZE: pixels per side of a rendered cell (hog.c:183)
@@ -1451,62 +1453,39 @@ def vl_hog_glyphs(num_bins: int, transposed: bool = False) -> np.ndarray:
     return out
 
 
-def _hog_grids(features, num_bins: int, variant: int, out_size, ctx: Context):
-    """(grids struct, device features kept alive, result shapes, result offsets or None, batched) for the planar features of
-    vl_hog_render / vl_hog_flip: a (B, dd, h, w) batch or a list of (dd, h, w) grids."""
+def _hog_grids(features, num_bins: int, variant: int, out_size, ctx: Context, zero: bool):
+    """The planar features of vl_hog_render / vl_hog_flip -- a (B, dd, h, w) batch or a list of (dd, h, w) grids -> (grids
+    struct, device tensors it points to, result buffer, results): a (B,) + out_size(h, w) tensor, or a list of out_size(h, w)
+    tensors, whose descriptors hold their offsets.  An empty list gives a count of 0 and no results."""
     dd = _hog_dims(num_bins, variant)
     dev = f"cuda:{ctx.device}"
-
-    def tensor(a):
-        t = a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))
-        if t.dtype != torch.float32:
-            raise ValueError("features must be float32")
-        return t
-
     g = HogGridsC()
     g.d_grids = None
     if isinstance(features, (list, tuple)):
-        grids = [tensor(f) for f in features]
+        grids = [_tensor(f) for f in features]
+        if any(f.dtype != torch.float32 for f in grids):
+            raise ValueError("features must be float32")
         if any(f.dim() != 3 or f.shape[0] != dd for f in grids):
             raise ValueError(f"every grid must be (dd, h, w) with dd = {dd}")
-        sizes = [tuple(f.shape[1:]) for f in grids]
-        keep = torch.cat([f.reshape(-1) for f in grids]).to(dev) if grids else None
-        descs, pos, opos, offsets = [], 0, 0, []
-        for h, w in sizes:
-            descs.append(HogGridC(w, h, pos, opos))
-            offsets.append(opos)
-            pos += dd * h * w
-            opos += int(np.prod(out_size(h, w)))
         g.count = len(grids)
-        table = (HogGridC * max(len(descs), 1))(*descs)
-        keep_table = torch.from_numpy(np.frombuffer(bytes(table), dtype=np.uint8).copy()).to(dev)
-        g.d_grids = keep_table.data_ptr()
-        g.d_features = keep.data_ptr() if keep is not None else None
-        return g, (keep, keep_table), [out_size(h, w) for h, w in sizes], offsets, False
-    t = tensor(features)
+        if not grids:
+            return g, (), None, []
+        sizes = [tuple(f.shape[1:]) for f in grids]
+        keep, offsets = _pack(grids, dev)
+        out, out_offsets, results = _results([out_size(h, w) for h, w in sizes], dev, zero)
+        keep_table = _device_table([HogGridC(w, h, o, oo) for (h, w), o, oo in zip(sizes, offsets, out_offsets)], dev)
+        g.d_features, g.d_grids = keep.data_ptr(), keep_table.data_ptr()
+        return g, (keep, keep_table), out, results
+    t = _tensor(features)
+    if t.dtype != torch.float32:
+        raise ValueError("features must be float32")
     if t.dim() != 4 or t.shape[1] != dd:
         raise ValueError(f"features must be (B, dd, h, w) with dd = {dd}, or a list of (dd, h, w) grids")
     keep = t.to(dev).contiguous()
     b, _, h, w = keep.shape
     g.d_features, g.count, g.width, g.height = keep.data_ptr(), b, w, h
-    return g, (keep,), [(b,) + tuple(out_size(h, w))], None, True
-
-
-def _hog_result(ctx, shapes, offsets, batched, run, zero: bool):
-    """Allocates the results (one batch tensor, or one buffer viewed as the grids' shapes), runs run(buffer) and returns them."""
-    dev = f"cuda:{ctx.device}"
-    alloc = torch.zeros if zero else torch.empty
-    if batched:
-        out = alloc(shapes[0], dtype=torch.float32, device=dev)
-        if out.shape[0]:
-            run(out)
-        return out
-    if not shapes:
-        return []
-    total = offsets[-1] + int(np.prod(shapes[-1]))
-    out = alloc(total, dtype=torch.float32, device=dev)
-    run(out)
-    return [out[o:o + int(np.prod(s))].view(s) for o, s in zip(offsets, shapes)]
+    out, _, results = _results((b,) + tuple(out_size(h, w)), dev, zero)
+    return g, (keep,), out, results
 
 
 def vl_hog_render(features, num_bins: int, variant: int = 1, ctx: Optional[Context] = None):
@@ -1515,10 +1494,10 @@ def vl_hog_render(features, num_bins: int, variant: int = 1, ctx: Optional[Conte
     tile at (21 y, 21 x), every orientation's bar weighted by the sum of its planes, clamped to the cell's weight range.
     Returns a (B, h * 21, w * 21) float32 CUDA tensor, or a list of (h * 21, w * 21) tensors."""
     ctx = ctx or default_context()
-    g, keep, shapes, offsets, batched = _hog_grids(features, num_bins, variant, lambda h, w: (h * GLYPH_SIZE, w * GLYPH_SIZE), ctx)
-    lib = _capi.lib()
-    return _hog_result(ctx, shapes, offsets, batched, lambda out: _check(ctx.h, lib.sd_hog_render(
-        ctx.h, C.byref(g), int(num_bins), int(variant), 0, ptr(out))), zero=True)
+    g, keep, out, results = _hog_grids(features, num_bins, variant, lambda h, w: (h * GLYPH_SIZE, w * GLYPH_SIZE), ctx, zero=True)
+    if g.count:
+        _check(ctx.h, _capi.lib().sd_hog_render(ctx.h, C.byref(g), int(num_bins), int(variant), 0, ptr(out)))
+    return results
 
 
 def vl_hog_flip(features, num_bins: int, variant: int = 1, ctx: Optional[Context] = None):
@@ -1526,11 +1505,11 @@ def vl_hog_flip(features, num_bins: int, variant: int = 1, ctx: Optional[Context
     out[i][y][x] = features[perm[i]][y][w - 1 - x] with perm = vl_hog_permutation(variant, num_bins).  features: a
     (B, dd, h, w) batch or a list of (dd, h, w) grids; returns the same shapes as fresh CUDA tensors."""
     ctx = ctx or default_context()
-    g, keep, shapes, offsets, batched = _hog_grids(features, num_bins, variant,
-                                                   lambda h, w: (_hog_dims(num_bins, variant), h, w), ctx)
-    lib = _capi.lib()
-    return _hog_result(ctx, shapes, offsets, batched, lambda out: _check(ctx.h, lib.sd_hog_relayout(
-        ctx.h, C.byref(g), int(num_bins), int(variant), 1, 0, ptr(out))), zero=False)
+    g, keep, out, results = _hog_grids(features, num_bins, variant, lambda h, w: (_hog_dims(num_bins, variant), h, w), ctx,
+                                       zero=False)
+    if g.count:
+        _check(ctx.h, _capi.lib().sd_hog_relayout(ctx.h, C.byref(g), int(num_bins), int(variant), 1, 0, ptr(out)))
+    return results
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1568,25 +1547,14 @@ def vl_hog_pyramid(frames, scales, cell_size: int, num_bins: int, variant: int =
     if not sizes:
         return [], []
     levels = [[hog_pyramid_shape(w, h, s, cell_size, num_bins, variant) for s in scales] for h, w in sizes]
-    offsets, pos = [], 0
-    for row in levels:
-        for _, (d, h, w) in row:
-            offsets.append(pos)
-            pos += d * h * w
     dev = f"cuda:{ctx.device}"
-    out = torch.empty(max(pos, 1), dtype=torch.float32, device=dev)
+    out, offsets, feats = _results([shape if shape[1] else None for row in levels for _, shape in row], dev)
     d_off = torch.tensor(offsets, dtype=torch.int64, device=dev)
     h_scales = (C.c_double * len(scales))(*scales)
     _check(ctx.h, _capi.lib().sd_hog_pyramid(ctx.h, C.byref(ib), h_scales, len(scales), int(cell_size), int(num_bins), int(variant),
                                              ptr(out), ptr(d_off)))
-    feats, i = [], 0
-    for row in levels:
-        fr = []
-        for _, shape in row:
-            fr.append(out[offsets[i]:offsets[i] + int(np.prod(shape))].view(shape) if shape[1] else None)
-            i += 1
-        feats.append(fr)
-    return feats, [[lv for lv, _ in row] for row in levels]
+    S = len(scales)
+    return [feats[i:i + S] for i in range(0, len(feats), S)], [[lv for lv, _ in row] for row in levels]
 
 
 def vl_hog_correlate(maps, filters, num_bins: int, variant: int = 1, bias=None, pad=(0, 0), ctx: Optional[Context] = None):
@@ -1599,14 +1567,14 @@ def vl_hog_correlate(maps, filters, num_bins: int, variant: int = 1, bias=None, 
     ctx = ctx or default_context()
     dd = _hog_dims(num_bins, variant)
     dev = f"cuda:{ctx.device}"
-    f = filters if isinstance(filters, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(filters))
+    f = _tensor(filters)
     if f.dtype != torch.float32 or f.dim() != 4 or f.shape[1] != dd:
         raise ValueError(f"filters must be a float32 (Q, dd, fh, fw) tensor with dd = {dd}")
     f = f.to(dev).contiguous()
     q, _, fh, fw = f.shape
     b = None
     if bias is not None:
-        b = (bias if isinstance(bias, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(bias))).to(dev, torch.float32).contiguous()
+        b = _tensor(bias).to(dev, torch.float32).contiguous()
         if b.shape != (q,):
             raise ValueError(f"bias must have one value per filter ({q})")
     pad_x, pad_y = (int(p) for p in pad)
@@ -1618,28 +1586,19 @@ def vl_hog_correlate(maps, filters, num_bins: int, variant: int = 1, bias=None, 
         return []
     maps = [m.to(dev) for m in maps]
     sizes = [tuple(m.shape[1:]) for m in maps]
-    outs = [(q, h + 2 * pad_y - fh + 1, w + 2 * pad_x - fw + 1) for h, w in sizes]
     # in place: contiguous maps of one storage, 4-byte aligned; else one packed copy
     stor = maps[0].untyped_storage().data_ptr()
     if all(m.is_contiguous() and m.untyped_storage().data_ptr() == stor for m in maps):
         base, keep = stor, maps
         offs = [(m.data_ptr() - base) // 4 for m in maps]
     else:
-        keep = torch.cat([m.reshape(-1) for m in maps])
+        keep, offs = _pack(maps, dev)
         base = keep.data_ptr()
-        offs = np.concatenate([[0], np.cumsum([m.numel() for m in maps])[:-1]]).astype(np.int64).tolist()
-    descs, out_offs, pos = [], [], 0
-    for (h, w), o, (_, oh, ow) in zip(sizes, offs, outs):
-        descs.append(HogGridC(w, h, int(o), pos))
-        out_offs.append(pos)
-        if oh > 0 and ow > 0:
-            pos += q * oh * ow
-    table = (HogGridC * len(descs))(*descs)
-    d_table = torch.from_numpy(np.frombuffer(bytes(table), dtype=np.uint8).copy()).to(dev)
+    # a map smaller than the filter scores nothing: an empty (Q, oh, ow) tensor
+    out, out_offs, scores = _results([(q, max(h + 2 * pad_y - fh + 1, 0), max(w + 2 * pad_x - fw + 1, 0)) for h, w in sizes], dev)
+    d_table = _device_table([HogGridC(w, h, o, oo) for (h, w), o, oo in zip(sizes, offs, out_offs)], dev)
     g = HogGridsC()
     g.d_features, g.count, g.width, g.height, g.d_grids = base, len(maps), 0, 0, d_table.data_ptr()
-    out = torch.empty(max(pos, 1), dtype=torch.float32, device=dev)
     _check(ctx.h, _capi.lib().sd_hog_correlate(ctx.h, C.byref(g), int(num_bins), int(variant), ptr(f), int(q), int(fw), int(fh),
                                                ptr(b), pad_x, pad_y, ptr(out)))
-    return [out[o:o + q * oh * ow].view(q, oh, ow) if oh > 0 and ow > 0 else out.new_empty((q, max(oh, 0), max(ow, 0)))
-            for o, (_, oh, ow) in zip(out_offs, outs)]
+    return scores

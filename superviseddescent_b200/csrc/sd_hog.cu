@@ -577,8 +577,7 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
 {
     SD_REQUIRE(ctx, images && images->d_data && d_x && p, "null argument");
     SD_REQUIRE(ctx, N >= 0 && L >= 1, "bad sample / landmark count");
-    SD_REQUIRE(ctx, p->variant == 0 || p->variant == 1, "unknown HOG variant");
-    SD_REQUIRE(ctx, p->num_bins >= 1 && p->num_bins <= SD_MAX_BINS, "num_bins must be in [1,16]");
+    if (const int rc = sd_hog_check_config(ctx, __func__, p->variant, p->num_bins)) return rc;
     SD_REQUIRE(ctx, p->num_cells >= 1 && p->cell_size >= 1, "bad cell configuration");
     const int fs = p->num_cells * p->cell_size;
     SD_REQUIRE(ctx, fs > 3 && fs <= 256, "resized patch must be 4..256 px (hog.c:545-546 asserts > 3)");
@@ -613,7 +612,7 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
     if (!d_image_index) SD_REQUIRE(ctx, images->count >= N, "fewer images than samples and no image index");
     a.x = d_x; a.ldx = ldx; a.N = N; a.L = L;
     a.variant = p->variant; a.nc = p->num_cells; a.cs = p->cell_size; a.K = p->num_bins; a.fs = fs;
-    a.dd = p->variant == 1 ? 3 * p->num_bins + 4 : 4 * p->num_bins;
+    a.dd = sd_hog_dd(p->num_bins, p->variant);
     a.A = d_A; a.ld = ld;
     if (d_A) SD_REQUIRE(ctx, ld >= (int64_t)L * a.nc * a.nc * a.dd + 1, "ld < feature length");
     // every argument check before the first launch: a rejected configuration queues no work
@@ -724,7 +723,7 @@ extern "C" {
 int sd_hog_feature_length(int num_landmarks, const sd_hog_param* p)
 {
     if (!p) return -1;
-    const int dd = p->variant == 1 ? 3 * p->num_bins + 4 : 4 * p->num_bins;
+    const int dd = sd_hog_dd(p->num_bins, p->variant);
     return num_landmarks * p->num_cells * p->num_cells * dd + 1;
 }
 

@@ -32,7 +32,6 @@
 namespace {
 
 constexpr int kDenseThreads = 256;
-constexpr int kDenseMaxCell = 32;   // largest cell size: one cell with its halo stays below 227 KB of shared memory at K = 16
 constexpr int kDenseMaxTile = 14;   // (T + 2)^2 histogram cells <= kDenseThreads: one thread per histogram cell
 constexpr int kDenseSpanBudget = 112;
 constexpr int kDenseMaxChannels = 16;
@@ -492,14 +491,13 @@ int images_tile(void (*kern)(Args), int cs, int K, bool bil)
 // the rules of vl_hog_prepare_buffers (hog.c:542-548) and of this implementation's range, shared by both entry points
 bool dense_shape(int width, int height, int cs, int K, int variant, int* hog_w, int* hog_h, int* dd)
 {
-    if (variant != 0 && variant != 1) return false;
-    if (K < 1 || K > SD_MAX_BINS || cs < 1 || cs > kDenseMaxCell) return false;
+    if (sd_hog_check_config(nullptr, __func__, variant, K, cs)) return false;
     if (width <= 3 || height <= 3) return false;
     const int w = (width + cs / 2) / cs, h = (height + cs / 2) / cs;
     if (w <= 0 || h <= 0) return false;
     *hog_w = w;
     *hog_h = h;
-    *dd = variant == 1 ? 3 * K + 4 : 4 * K;
+    *dd = sd_hog_dd(K, variant);
     return true;
 }
 
@@ -535,16 +533,6 @@ bool image_ok(const sd_hog_image& d, int cs, int K, int variant, int* hog_w, int
            d.pixel_stride >= 0 && d.channel_stride >= 0;
 }
 
-// a device descriptor table on the host, read back once
-template <class Frame>
-int fetch_frames(sd_ctx* ctx, const Frame* d_frames, int count, std::vector<Frame>& fr)
-{
-    fr.resize(count);
-    SD_CUDA(ctx, cudaMemcpyAsync(fr.data(), d_frames, sizeof(Frame) * count, cudaMemcpyDeviceToHost, ctx->stream));
-    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return SD_OK;
-}
-
 // The descriptor table of a batch, read back once: every frame passes the rules of its entry point (fn, for the messages),
 // *max_w x *max_h cells cover the largest frame, and frames of different sizes need one output offset per frame (offsets).
 template <class Frame>
@@ -552,7 +540,7 @@ int read_frames(sd_ctx* ctx, const char* fn, const Frame* d_frames, int count, i
                 int* max_w, int* max_h, int* dd)
 {
     std::vector<Frame> fr;
-    if (const int rc = fetch_frames(ctx, d_frames, count, fr)) return rc;
+    if (const int rc = sd_fetch_table(ctx, d_frames, count, fr)) return rc;
     bool uniform = true;
     for (int i = 0; i < count; ++i) {
         const Frame& d = fr[i];
@@ -706,9 +694,7 @@ int sd_hog_dense(sd_ctx* ctx, const sd_image_batch* images, int cell_size, int n
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, images && d_out, "null argument");
     SD_REQUIRE(ctx, !images->d_roi, "a batch with regions of interest has no whole frames");
-    SD_REQUIRE(ctx, variant == 0 || variant == 1, "unknown HOG variant");
-    SD_REQUIRE(ctx, num_bins >= 1 && num_bins <= SD_MAX_BINS, "num_bins must be in [1,16]");
-    SD_REQUIRE(ctx, cell_size >= 1 && cell_size <= kDenseMaxCell, "cell_size must be in [1,32]");
+    if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins, cell_size)) return rc;
     SD_REQUIRE(ctx, images->count >= 0, "negative frame count");
     const int count = images->count;
     if (count == 0) return SD_OK;
@@ -745,11 +731,10 @@ int sd_hog_pyramid_shape(int width, int height, double scale, int cell_size, int
                          int* hog_w, int* hog_h, int* dd)
 {
     if (!level_w || !level_h || !hog_w || !hog_h || !dd) return SD_ERR_INVALID;
-    if (variant != 0 && variant != 1) return SD_ERR_INVALID;
-    if (num_bins < 1 || num_bins > SD_MAX_BINS || cell_size < 1 || cell_size > kDenseMaxCell) return SD_ERR_INVALID;
+    if (sd_hog_check_config(nullptr, __func__, variant, num_bins, cell_size)) return SD_ERR_INVALID;
     int lw, lh;
     if (!pyramid_level(width, height, scale, &lw, &lh)) return SD_ERR_INVALID;
-    int w = 0, h = 0, d = variant == 1 ? 3 * num_bins + 4 : 4 * num_bins;
+    int w = 0, h = 0, d = sd_hog_dd(num_bins, variant);
     if (!dense_shape(lw, lh, cell_size, num_bins, variant, &w, &h, &d)) w = h = 0;   // an empty level
     *level_w = lw;
     *level_h = lh;
@@ -765,9 +750,7 @@ int sd_hog_pyramid(sd_ctx* ctx, const sd_image_batch* images, const double* h_sc
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, images && h_scales && d_out && d_out_offset, "null argument");
     SD_REQUIRE(ctx, !images->d_roi, "a batch with regions of interest has no whole frames");
-    SD_REQUIRE(ctx, variant == 0 || variant == 1, "unknown HOG variant");
-    SD_REQUIRE(ctx, num_bins >= 1 && num_bins <= SD_MAX_BINS, "num_bins must be in [1,16]");
-    SD_REQUIRE(ctx, cell_size >= 1 && cell_size <= kDenseMaxCell, "cell_size must be in [1,32]");
+    if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins, cell_size)) return rc;
     SD_REQUIRE(ctx, num_scales >= 1, "num_scales must be at least 1");
     for (int s = 0; s < num_scales; ++s)
         SD_REQUIRE(ctx, h_scales[s] > 0.0 && h_scales[s] <= 4.0, "every scale must be finite and in (0, 4]");
@@ -780,7 +763,7 @@ int sd_hog_pyramid(sd_ctx* ctx, const sd_image_batch* images, const double* h_sc
     // the frames: the batch's, or the descriptor table read back once
     std::vector<sd_frame> fr;
     if (images->d_frames) {
-        if (const int rc = fetch_frames(ctx, images->d_frames, count, fr)) return rc;
+        if (const int rc = sd_fetch_table(ctx, images->d_frames, count, fr)) return rc;
     } else {
         SD_REQUIRE(ctx, count == 1 || images->image_stride > 0, "bad strides");
         fr.assign(count, sd_frame{images->width, images->height, images->row_stride, 0, 0});
@@ -812,7 +795,7 @@ int sd_hog_pyramid(sd_ctx* ctx, const sd_image_batch* images, const double* h_sc
     first[count] = (int)lv.size();
     if (lv.empty()) return SD_OK;
 
-    const int dd = variant == 1 ? 3 * num_bins + 4 : 4 * num_bins;
+    const int dd = sd_hog_dd(num_bins, variant);
     DenseArgs a = dense_args(nullptr, nullptr, cell_size, num_bins, variant, dd, d_out, nullptr);
     const DenseSmem lay = dense_smem_layout(a.span, a.pitch, num_bins, dense_cells(a.tile));
     CUtensorMap map;                                 // not read: levels of different sizes are staged by the load loop
@@ -882,9 +865,7 @@ int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size,
     SD_REQUIRE(ctx, images->dtype == SD_HOG_U8 || images->dtype == SD_HOG_F32, "dtype must be SD_HOG_U8 or SD_HOG_F32");
     SD_REQUIRE(ctx, images->channels >= 1 && images->channels <= kDenseMaxChannels, "channels must be in [1,16]");
     SD_REQUIRE(ctx, bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
-    SD_REQUIRE(ctx, variant == 0 || variant == 1, "unknown HOG variant");
-    SD_REQUIRE(ctx, num_bins >= 1 && num_bins <= SD_MAX_BINS, "num_bins must be in [1,16]");
-    SD_REQUIRE(ctx, cell_size >= 1 && cell_size <= kDenseMaxCell, "cell_size must be in [1,32]");
+    if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins, cell_size)) return rc;
     SD_REQUIRE(ctx, images->count >= 0, "negative frame count");
     const int count = images->count;
     if (count == 0) return SD_OK;
@@ -944,9 +925,7 @@ int sd_hog_dense_polar(sd_ctx* ctx, const sd_hog_polar_fields* fields, int cell_
     SD_REQUIRE(ctx, fields && d_out, "null argument");
     SD_REQUIRE(ctx, directed == 0 || directed == 1, "directed must be 0 or 1");
     SD_REQUIRE(ctx, bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
-    SD_REQUIRE(ctx, variant == 0 || variant == 1, "unknown HOG variant");
-    SD_REQUIRE(ctx, num_bins >= 1 && num_bins <= SD_MAX_BINS, "num_bins must be in [1,16]");
-    SD_REQUIRE(ctx, cell_size >= 1 && cell_size <= kDenseMaxCell, "cell_size must be in [1,32]");
+    if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins, cell_size)) return rc;
     SD_REQUIRE(ctx, fields->count >= 0, "negative field count");
     const int count = fields->count;
     if (count == 0) return SD_OK;

@@ -202,8 +202,7 @@ int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int va
 {
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, maps && d_filters && d_scores, "null argument");
-    SD_REQUIRE(ctx, variant == 0 || variant == 1, "unknown HOG variant");
-    SD_REQUIRE(ctx, num_bins >= 1 && num_bins <= SD_MAX_BINS, "num_bins must be in [1,16]");
+    if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins)) return rc;
     SD_REQUIRE(ctx, num_filters >= 1 && num_filters <= SD_HOG_FILTER_MAX_BANK, "num_filters must be in [1, SD_HOG_FILTER_MAX_BANK]");
     SD_REQUIRE(ctx, filter_w >= 1 && filter_w <= SD_HOG_FILTER_MAX_SIDE && filter_h >= 1 && filter_h <= SD_HOG_FILTER_MAX_SIDE,
                "filter sides must be in [1, SD_HOG_FILTER_MAX_SIDE]");
@@ -217,7 +216,7 @@ int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int va
     int max_w = 0, max_h = 0;
     std::vector<sd_hog_grid> table;
     if (const int rc = sd_read_hog_grids(ctx, __func__, maps, &max_w, &max_h, &table)) return rc;
-    const int dd = variant == 1 ? 3 * num_bins + 4 : 4 * num_bins;
+    const int dd = sd_hog_dd(num_bins, variant);
     const int QF = group_of(num_filters);
 
     CorrArgs a;

@@ -21,8 +21,6 @@ constexpr int kTile = 32;                         // relayout: 32 x 32 elements 
 
 // ---- host tables ------------------------------------------------------------------------------------------------------------
 
-int dims_of(int K, int variant) { return variant == 1 ? 3 * K + 4 : 4 * K; }
-
 // vl_hog_new's permutation (hog.c:225-268): flipped[i] = features[perm[i]].  Orientation o (pointing at angle o pi / K) maps to
 // K - o, the mirror image about the vertical axis; the directed half adds K modulo 2K; the undirected and Dalal-Triggs blocks
 // fold modulo K.  The four blocks around a cell (x offset bx, y offset by, index bx + 2 by) swap left and right.
@@ -213,8 +211,7 @@ __global__ void __launch_bounds__(kTile * 8) hog_relayout_kernel(const __grid_co
 int check_config(sd_ctx* ctx, const sd_hog_grids* grids, int num_bins, int variant)
 {
     SD_REQUIRE(ctx, grids, "null argument");
-    SD_REQUIRE(ctx, variant == 0 || variant == 1, "unknown HOG variant");
-    SD_REQUIRE(ctx, num_bins >= 1 && num_bins <= SD_MAX_BINS, "num_bins must be in [1,16]");
+    if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins)) return rc;
     SD_REQUIRE(ctx, grids->count >= 0, "negative grid count");
     return SD_OK;
 }
@@ -233,9 +230,8 @@ int sd_read_hog_grids(sd_ctx* ctx, const char* fn, const sd_hog_grids* grids, in
         *max_h = grids->height;
         return SD_OK;
     }
-    std::vector<sd_hog_grid> t(count);
-    SD_CUDA(ctx, cudaMemcpyAsync(t.data(), grids->d_grids, sizeof(sd_hog_grid) * count, cudaMemcpyDeviceToHost, ctx->stream));
-    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    std::vector<sd_hog_grid> t;
+    if (const int rc = sd_fetch_table(ctx, grids->d_grids, count, t)) return rc;
     for (int i = 0; i < count; ++i) {
         const sd_hog_grid& d = t[i];
         if (d.width < 1 || d.height < 1 || d.offset < 0 || d.out_offset < 0)
@@ -252,7 +248,7 @@ extern "C" {
 
 int sd_hog_permutation(int num_bins, int variant, int64_t* perm)
 {
-    if (!perm || num_bins < 1 || num_bins > SD_MAX_BINS || (variant != 0 && variant != 1)) return SD_ERR_INVALID;
+    if (!perm || sd_hog_check_config(nullptr, __func__, variant, num_bins)) return SD_ERR_INVALID;
     permutation(num_bins, variant, perm);
     return SD_OK;
 }
@@ -283,7 +279,7 @@ int sd_hog_render(sd_ctx* ctx, const sd_hog_grids* grids, int num_bins, int vari
     a.features = grids->d_features;
     a.image = d_image;
     a.width = grids->width; a.height = grids->height;
-    a.in_stride = (long long)dims_of(num_bins, variant) * a.width * a.height;
+    a.in_stride = (long long)sd_hog_dd(num_bins, variant) * a.width * a.height;
     a.out_stride = (long long)a.width * a.height * kGlyphPixels;
     a.grids = grids->d_grids;
     a.K = num_bins;
@@ -314,7 +310,7 @@ int sd_hog_relayout(sd_ctx* ctx, const sd_hog_grids* grids, int num_bins, int va
     SD_REQUIRE(ctx, grids->d_features != d_out, "the relayout is out of place: d_out must not be the input");
     int max_w = 0, max_h = 0;
     if (const int rc = sd_read_hog_grids(ctx, __func__, grids, &max_w, &max_h, nullptr)) return rc;
-    const int dd = dims_of(num_bins, variant);
+    const int dd = sd_hog_dd(num_bins, variant);
     const int tiles_x = sd_div_up(max_w, kTile);
     SD_REQUIRE(ctx, (long long)tiles_x * sd_div_up(max_h, kTile) <= INT_MAX, "grid too large");
     if (!grids->d_grids) {

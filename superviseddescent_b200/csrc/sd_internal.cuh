@@ -15,6 +15,7 @@
 
 #define SD_MAX_EYES 4
 #define SD_MAX_BINS 16   // undirected orientations K supported by the HOG kernel
+constexpr int kDenseMaxCell = 32;   // largest dense cell size: one cell with its halo stays below 227 KB of shared memory at K = 16
 
 enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_PARTIAL, SD_WS_GEOM, SD_WS_GEMM_PARTIAL, SD_WS_DIAGINV2, SD_WS_PANEL, SD_WS_BIAS, SD_WS_CG, SD_WS_CGMAT,
@@ -105,6 +106,37 @@ void* sd_workspace(sd_ctx* ctx, int slot, size_t bytes);
     } while (0)
 
 static inline int sd_div_up(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
+
+// ---- HOG configurations ------------------------------------------------------------------------
+
+// dd, the features per cell of vl_hog_new(variant, num_bins): 3K + 4 for UoCTTI (variant 1), 4K for Dalal-Triggs (variant 0)
+inline int sd_hog_dd(int num_bins, int variant) { return variant == 1 ? 3 * num_bins + 4 : 4 * num_bins; }
+
+// The configuration rule of the HOG entry points: variant 0 or 1 and num_bins in [1, SD_MAX_BINS], and for the dense ones, which
+// take a cell size, cell_size in [1, kDenseMaxCell].  Returns SD_OK, or SD_ERR_INVALID with the message "fn: ..." in ctx (none
+// for ctx == nullptr: the host-only functions report a status only).
+inline int sd_hog_check_config(sd_ctx* ctx, const char* fn, int variant, int num_bins)
+{
+    if (variant != 0 && variant != 1) return sd_fail(ctx, SD_ERR_INVALID, "%s: unknown HOG variant", fn);
+    if (num_bins < 1 || num_bins > SD_MAX_BINS) return sd_fail(ctx, SD_ERR_INVALID, "%s: num_bins must be in [1,16]", fn);
+    return SD_OK;
+}
+inline int sd_hog_check_config(sd_ctx* ctx, const char* fn, int variant, int num_bins, int cell_size)
+{
+    if (const int rc = sd_hog_check_config(ctx, fn, variant, num_bins)) return rc;
+    if (cell_size < 1 || cell_size > kDenseMaxCell) return sd_fail(ctx, SD_ERR_INVALID, "%s: cell_size must be in [1,32]", fn);
+    return SD_OK;
+}
+
+// a device descriptor table of count entries, read back to the host once
+template <class T>
+int sd_fetch_table(sd_ctx* ctx, const T* d_table, int count, std::vector<T>& table)
+{
+    table.resize(count);
+    SD_CUDA(ctx, cudaMemcpyAsync(table.data(), d_table, sizeof(T) * count, cudaMemcpyDeviceToHost, ctx->stream));
+    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return SD_OK;
+}
 
 // ---- internal entry points shared between translation units ---------------------------------
 

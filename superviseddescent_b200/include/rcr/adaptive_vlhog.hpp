@@ -30,6 +30,81 @@ struct HoGParam {
     sd_hog_param c() const { sd_hog_param p; p.variant = vlhog_variant; p.num_cells = num_cells; p.cell_size = cell_size; p.num_bins = num_bins; p.relative_patch_size = relative_patch_size; return p; }
 };
 
+namespace hog_batch {
+
+// The results of one batched call, end to end in one device buffer: item i is a CV_32FC1 Mat of rows[i] x cols[i] floats at
+// offset[i].  An item without rows or columns is empty: it holds nothing and downloads as an empty Mat.
+struct Results {
+    std::vector<int64_t> offset;
+    std::vector<int> rows, cols;
+    int64_t total = 0;
+    sd_b200::DeviceBuffer d_out, d_offset;
+
+    void add(int r, int c)
+    {
+        if (r <= 0 || c <= 0) r = c = 0;
+        offset.push_back(total);
+        rows.push_back(r);
+        cols.push_back(c);
+        total += static_cast<int64_t>(r) * c;
+    }
+    // the buffer, one float at least, so that a call whose items are all empty gets a valid pointer
+    float* out()
+    {
+        d_out.allocate(static_cast<size_t>(std::max<int64_t>(total, 1)) * sizeof(float));
+        return d_out.as<float>();
+    }
+    // the items' offsets, uploaded for the calls that take one int64 offset per item
+    const int64_t* offsets(sd_ctx* ctx, const char* what)
+    {
+        d_offset.allocate(offset.size() * sizeof(int64_t));
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_offset.as<int64_t>(), offset.data(), offset.size() * sizeof(int64_t)), what);
+        return d_offset.as<int64_t>();
+    }
+    std::vector<cv::Mat> download() const
+    {
+        std::vector<cv::Mat> items;
+        for (size_t i = 0; i < offset.size(); ++i)
+            items.push_back(cols[i] ? sd_b200::download(d_out.as<float>() + offset[i], rows[i], cols[i], cols[i]) : cv::Mat());
+        return items;
+    }
+};
+
+// 8UC1 / 8UC3 (B,G,R) frames on the device as one grey batch (sd_upload_frames), in buf
+inline sd_image_batch upload_grey(sd_ctx* ctx, const std::vector<sd_host_frame>& frames, sd_b200::DeviceBuffer& buf, const char* what)
+{
+    const int n = static_cast<int>(frames.size());
+    size_t bytes = 0;
+    sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, nullptr, &bytes, nullptr), what);
+    buf.allocate(bytes);
+    sd_image_batch batch{};
+    sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, buf.as<void>(), &bytes, &batch), what);
+    return batch;
+}
+
+// CV_8UC1 or CV_32FC1 planes of elem_size bytes per element (row steps allowed) packed end to end into buf, in the order
+// given; returns where each plane starts, in elements
+inline std::vector<int64_t> pack_planes(sd_ctx* ctx, const std::vector<cv::Mat>& planes, size_t elem_size, sd_b200::DeviceBuffer& buf,
+                                        const char* what)
+{
+    std::vector<int64_t> start(planes.size());
+    int64_t elems = 0;
+    for (size_t i = 0; i < planes.size(); ++i) {
+        start[i] = elems;
+        elems += static_cast<int64_t>(planes[i].rows) * planes[i].cols;
+    }
+    buf.allocate(static_cast<size_t>(elems) * elem_size);
+    for (size_t i = 0; i < planes.size(); ++i) {
+        const cv::Mat& p = planes[i];
+        const size_t row_bytes = static_cast<size_t>(p.cols) * elem_size;
+        sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, buf.as<unsigned char>() + static_cast<size_t>(start[i]) * elem_size, row_bytes,
+                                            p.ptr<unsigned char>(0), p.step(), row_bytes, static_cast<size_t>(p.rows)), what);
+    }
+    return start;
+}
+
+}  // namespace hog_batch
+
 class HogTransform {
 public:
     // Do not call with `images` that are temporaries (the reference holds a const&, adaptive_vlhog.hpp:188).
@@ -162,12 +237,8 @@ private:
         sd_b200::check(ctx, sd_sync(ctx), "HogTransform upload");
         size_t free_bytes = 0, total = 0;
         sd_b200::check(ctx, sd_device_memory(ctx, &free_bytes, &total), "sd_device_memory");
-        const int n = static_cast<int>(frames.size());
         if (static_cast<double>(grey) <= device_frame_share() * static_cast<double>(free_bytes)) {
-            size_t bytes = 0;
-            sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, nullptr, &bytes, nullptr), "HogTransform upload");
-            dev->buf.allocate(bytes);
-            sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, dev->buf.as<void>(), &bytes, &dev->batch), "HogTransform upload");
+            dev->batch = hog_batch::upload_grey(ctx, frames, dev->buf, "HogTransform upload");
         } else {
             // host route: frames the levels cannot read in place are packed once into one pinned buffer, rows at a pitch of
             // channels * (width rounded up to 16) bytes
@@ -211,34 +282,22 @@ private:
 // configuration that sd_hog_dense_shape refuses.
 inline std::vector<cv::Mat> hog_dense(const std::vector<cv::Mat>& images, VlHogVariant variant, int cell_size, int num_bins)
 {
-    std::vector<cv::Mat> out;
-    if (images.empty()) return out;
+    if (images.empty()) return {};
     sd_ctx* ctx = sd_b200::context();
     const std::vector<sd_host_frame> frames = sd_b200::host_frames(images);
-    const int n = static_cast<int>(frames.size());
-    std::vector<int64_t> offset(n);
-    std::vector<int> rows(n), cols(n);
-    int64_t total = 0;
-    for (int i = 0; i < n; ++i) {
+    hog_batch::Results res;
+    for (size_t i = 0; i < frames.size(); ++i) {
         int w = 0, h = 0, dd = 0;
         if (sd_hog_dense_shape(frames[i].width, frames[i].height, cell_size, num_bins, variant, &w, &h, &dd) != SD_OK)
             throw std::runtime_error("hog_dense: frame " + std::to_string(i) + " (" + std::to_string(frames[i].width) + " x " +
                                      std::to_string(frames[i].height) + ") or the configuration is invalid: frames wider and taller "
                                      "than 3 px and at least half a cell, cell_size 1..32, num_bins 1..16");
-        offset[i] = total;
-        rows[i] = dd * h;
-        cols[i] = w;
-        total += static_cast<int64_t>(dd) * h * w;
+        res.add(dd * h, w);
     }
-    size_t bytes = 0;
-    sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, nullptr, &bytes, nullptr), "hog_dense upload");
-    sd_b200::DeviceBuffer buf(bytes), d_out(static_cast<size_t>(total) * sizeof(float)), d_offset(static_cast<size_t>(n) * sizeof(int64_t));
-    sd_image_batch batch{};
-    sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, buf.as<void>(), &bytes, &batch), "hog_dense upload");
-    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_offset.as<int64_t>(), offset.data(), static_cast<size_t>(n) * sizeof(int64_t)), "hog_dense");
-    sd_b200::check(ctx, sd_hog_dense(ctx, &batch, cell_size, num_bins, variant, d_out.as<float>(), d_offset.as<int64_t>()), "sd_hog_dense");
-    for (int i = 0; i < n; ++i) out.push_back(sd_b200::download(d_out.as<float>() + offset[i], rows[i], cols[i], cols[i]));
-    return out;
+    sd_b200::DeviceBuffer buf;
+    const sd_image_batch batch = hog_batch::upload_grey(ctx, frames, buf, "hog_dense upload");
+    sd_b200::check(ctx, sd_hog_dense(ctx, &batch, cell_size, num_bins, variant, res.out(), res.offsets(ctx, "hog_dense")), "sd_hog_dense");
+    return res.download();
 }
 
 // Dense HOG of every frame at every scale, in one batched call on the device (sd_hog_pyramid): level s of a W x H frame is the
@@ -249,44 +308,27 @@ inline std::vector<cv::Mat> hog_dense(const std::vector<cv::Mat>& images, VlHogV
 inline std::vector<std::vector<cv::Mat>> vl_hog_pyramid(const std::vector<cv::Mat>& images, const std::vector<double>& scales,
                                                         VlHogVariant variant, int cell_size, int num_bins)
 {
-    std::vector<std::vector<cv::Mat>> out;
-    if (images.empty()) return out;
+    if (images.empty()) return {};
     if (scales.empty()) throw std::runtime_error("vl_hog_pyramid: no scales");
     sd_ctx* ctx = sd_b200::context();
     const std::vector<sd_host_frame> frames = sd_b200::host_frames(images);
     const int n = static_cast<int>(frames.size()), S = static_cast<int>(scales.size());
-    std::vector<int64_t> offset(static_cast<size_t>(n) * S);
-    std::vector<int> rows(offset.size()), cols(offset.size());
-    int64_t total = 0;
+    hog_batch::Results res;
     for (int i = 0; i < n; ++i)
         for (int s = 0; s < S; ++s) {
             int lw = 0, lh = 0, w = 0, h = 0, dd = 0;
             if (sd_hog_pyramid_shape(frames[i].width, frames[i].height, scales[s], cell_size, num_bins, variant, &lw, &lh, &w, &h, &dd) != SD_OK)
                 throw std::runtime_error("vl_hog_pyramid: frame " + std::to_string(i) + " at scale " + std::to_string(scales[s]) +
                                          " or the configuration is invalid: scales in (0, 4], cell_size 1..32, num_bins 1..16");
-            const size_t l = static_cast<size_t>(i) * S + s;
-            offset[l] = total;
-            rows[l] = dd * h;
-            cols[l] = w;
-            total += static_cast<int64_t>(dd) * h * w;
+            res.add(dd * h, w);
         }
-    size_t bytes = 0;
-    sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, nullptr, &bytes, nullptr), "vl_hog_pyramid upload");
-    sd_b200::DeviceBuffer buf(bytes), d_out(static_cast<size_t>(std::max<int64_t>(total, 1)) * sizeof(float)),
-        d_offset(offset.size() * sizeof(int64_t));
-    sd_image_batch batch{};
-    sd_b200::check(ctx, sd_upload_frames(ctx, frames.data(), n, buf.as<void>(), &bytes, &batch), "vl_hog_pyramid upload");
-    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_offset.as<int64_t>(), offset.data(), offset.size() * sizeof(int64_t)), "vl_hog_pyramid");
-    sd_b200::check(ctx, sd_hog_pyramid(ctx, &batch, scales.data(), S, cell_size, num_bins, variant, d_out.as<float>(),
-                                       d_offset.as<int64_t>()), "sd_hog_pyramid");
-    for (int i = 0; i < n; ++i) {
-        std::vector<cv::Mat> levels;
-        for (int s = 0; s < S; ++s) {
-            const size_t l = static_cast<size_t>(i) * S + s;
-            levels.push_back(cols[l] ? sd_b200::download(d_out.as<float>() + offset[l], rows[l], cols[l], cols[l]) : cv::Mat());
-        }
-        out.push_back(levels);
-    }
+    sd_b200::DeviceBuffer buf;
+    const sd_image_batch batch = hog_batch::upload_grey(ctx, frames, buf, "vl_hog_pyramid upload");
+    sd_b200::check(ctx, sd_hog_pyramid(ctx, &batch, scales.data(), S, cell_size, num_bins, variant, res.out(),
+                                       res.offsets(ctx, "vl_hog_pyramid")), "sd_hog_pyramid");
+    const std::vector<cv::Mat> levels = res.download();
+    std::vector<std::vector<cv::Mat>> out;
+    for (int i = 0; i < n; ++i) out.emplace_back(levels.begin() + static_cast<size_t>(i) * S, levels.begin() + static_cast<size_t>(i + 1) * S);
     return out;
 }
 
@@ -299,10 +341,9 @@ inline std::vector<std::vector<cv::Mat>> vl_hog_pyramid(const std::vector<cv::Ma
 inline std::vector<cv::Mat> vl_hog_correlate(const std::vector<cv::Mat>& maps, const std::vector<cv::Mat>& filters, VlHogVariant variant,
                                              int num_bins, const std::vector<float>& bias, int pad_x, int pad_y)
 {
-    std::vector<cv::Mat> out;
-    if (maps.empty()) return out;
+    if (maps.empty()) return {};
     sd_ctx* ctx = sd_b200::context();
-    const int dd = variant == VlHogVariantUoctti ? 3 * num_bins + 4 : 4 * num_bins;
+    const int dd = sd_b200::hog_dimension(variant, num_bins);
     const int Q = static_cast<int>(filters.size());
     if (Q < 1 || dd < 1 || filters[0].rows % dd) throw std::runtime_error("vl_hog_correlate: no filters, or filters not dd * fh rows");
     const int fh = filters[0].rows / dd, fw = filters[0].cols;
@@ -315,22 +356,19 @@ inline std::vector<cv::Mat> vl_hog_correlate(const std::vector<cv::Mat>& maps, c
     }
     std::vector<float> hm;
     std::vector<sd_hog_grid> grids;
-    std::vector<int> oh(maps.size()), ow(maps.size());
-    int64_t pos = 0;
+    hog_batch::Results res;
     for (size_t i = 0; i < maps.size(); ++i) {
         const cv::Mat& m = maps[i];
         if (m.type() != CV_32FC1 || m.rows < dd || m.rows % dd || m.cols < 1)
             throw std::runtime_error("vl_hog_correlate: map " + std::to_string(i) + " is not dd * h rows of w columns");
         const int h = m.rows / dd, w = m.cols;
-        oh[i] = h + 2 * pad_y - fh + 1;
-        ow[i] = w + 2 * pad_x - fw + 1;
-        grids.push_back(sd_hog_grid{w, h, static_cast<int64_t>(hm.size()), pos});
+        const int oh = h + 2 * pad_y - fh + 1, ow = w + 2 * pad_x - fw + 1;
+        res.add(Q * oh, ow);
+        grids.push_back(sd_hog_grid{w, h, static_cast<int64_t>(hm.size()), res.offset[i]});
         for (int r = 0; r < m.rows; ++r) hm.insert(hm.end(), m.ptr<float>(r), m.ptr<float>(r) + m.cols);
-        if (oh[i] > 0 && ow[i] > 0) pos += static_cast<int64_t>(Q) * oh[i] * ow[i];
     }
     sd_b200::DeviceBuffer d_maps(hm.size() * sizeof(float)), d_filters(hf.size() * sizeof(float)),
-        d_bias(std::max<size_t>(bias.size(), 1) * sizeof(float)), d_grids(grids.size() * sizeof(sd_hog_grid)),
-        d_scores(static_cast<size_t>(std::max<int64_t>(pos, 1)) * sizeof(float));
+        d_bias(std::max<size_t>(bias.size(), 1) * sizeof(float)), d_grids(grids.size() * sizeof(sd_hog_grid));
     sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_maps.as<float>(), hm.data(), hm.size() * sizeof(float)), "vl_hog_correlate");
     sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_filters.as<float>(), hf.data(), hf.size() * sizeof(float)), "vl_hog_correlate");
     sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_grids.as<sd_hog_grid>(), grids.data(), grids.size() * sizeof(sd_hog_grid)), "vl_hog_correlate");
@@ -340,10 +378,8 @@ inline std::vector<cv::Mat> vl_hog_correlate(const std::vector<cv::Mat>& maps, c
     g.count = static_cast<int32_t>(maps.size());
     g.d_grids = d_grids.as<sd_hog_grid>();
     sd_b200::check(ctx, sd_hog_correlate(ctx, &g, num_bins, variant, d_filters.as<float>(), Q, fw, fh, bias.empty() ? nullptr : d_bias.as<float>(),
-                                         pad_x, pad_y, d_scores.as<float>()), "sd_hog_correlate");
-    for (size_t i = 0; i < maps.size(); ++i)
-        out.push_back(oh[i] > 0 && ow[i] > 0 ? sd_b200::download(d_scores.as<float>() + grids[i].out_offset, Q * oh[i], ow[i], ow[i]) : cv::Mat());
-    return out;
+                                         pad_x, pad_y, res.out()), "sd_hog_correlate");
+    return res.download();
 }
 
 // VLFeat HOG of whole frames of one or more channels, 8-bit or float (vl_hog_new(variant, num_bins),
@@ -356,18 +392,15 @@ inline std::vector<cv::Mat> vl_hog_correlate(const std::vector<cv::Mat>& maps, c
 inline std::vector<cv::Mat> vl_hog(const std::vector<std::vector<cv::Mat>>& frames, VlHogVariant variant, int cell_size, int num_bins,
                                    bool bilinear_orientations = false)
 {
-    std::vector<cv::Mat> out;
-    if (frames.empty()) return out;
+    if (frames.empty()) return {};
     const int n = static_cast<int>(frames.size());
     const int channels = static_cast<int>(frames[0].size());
     if (channels < 1 || channels > 16) throw std::runtime_error("vl_hog: frames must have 1..16 channel planes");
     const int type = frames[0][0].type();
     if (type != CV_8UC1 && type != CV_32FC1) throw std::runtime_error("vl_hog: channel planes must be CV_8UC1 or CV_32FC1");
-    const size_t es = type == CV_8UC1 ? 1 : 4;
     std::vector<sd_hog_image> desc(n);
-    std::vector<int64_t> offset(n);
-    std::vector<int> rows(n), cols(n);
-    int64_t elems = 0, total = 0;
+    std::vector<cv::Mat> planes;
+    hog_batch::Results res;
     for (int i = 0; i < n; ++i) {
         const std::vector<cv::Mat>& f = frames[i];
         if (static_cast<int>(f.size()) != channels) throw std::runtime_error("vl_hog: frame " + std::to_string(i) + " has a different number of planes");
@@ -380,40 +413,24 @@ inline std::vector<cv::Mat> vl_hog(const std::vector<std::vector<cv::Mat>>& fram
             throw std::runtime_error("vl_hog: frame " + std::to_string(i) + " (" + std::to_string(W) + " x " + std::to_string(H) +
                                      ") or the configuration is invalid: frames wider and taller than 3 px and at least half a cell, "
                                      "cell_size 1..32, num_bins 1..16");
-        desc[i].width = W;
-        desc[i].height = H;
-        desc[i].offset = elems;
-        desc[i].row_stride = W;
-        desc[i].pixel_stride = 1;
-        desc[i].channel_stride = static_cast<int64_t>(W) * H;
-        elems += static_cast<int64_t>(W) * H * channels;
-        offset[i] = total;
-        rows[i] = dd * h;
-        cols[i] = w;
-        total += static_cast<int64_t>(dd) * h * w;
+        desc[i] = sd_hog_image{W, H, 0, W, 1, static_cast<int64_t>(W) * H};   // offset: where the planes are packed
+        planes.insert(planes.end(), f.begin(), f.end());
+        res.add(dd * h, w);
     }
     sd_ctx* ctx = sd_b200::context();
-    sd_b200::DeviceBuffer buf(static_cast<size_t>(elems) * es), d_desc(static_cast<size_t>(n) * sizeof(sd_hog_image)),
-        d_out(static_cast<size_t>(total) * sizeof(float)), d_offset(static_cast<size_t>(n) * sizeof(int64_t));
-    for (int i = 0; i < n; ++i)
-        for (int c = 0; c < channels; ++c) {
-            const cv::Mat& p = frames[i][c];
-            unsigned char* dst = buf.as<unsigned char>() + static_cast<size_t>(desc[i].offset + c * desc[i].channel_stride) * es;
-            sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, dst, static_cast<size_t>(p.cols) * es, p.ptr<unsigned char>(0), p.step(), static_cast<size_t>(p.cols) * es,
-                                                static_cast<size_t>(p.rows)), "vl_hog upload");
-        }
+    sd_b200::DeviceBuffer buf, d_desc(static_cast<size_t>(n) * sizeof(sd_hog_image));
+    const std::vector<int64_t> start = hog_batch::pack_planes(ctx, planes, type == CV_8UC1 ? 1 : 4, buf, "vl_hog upload");
+    for (int i = 0; i < n; ++i) desc[i].offset = start[static_cast<size_t>(i) * channels];
     sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_desc.as<sd_hog_image>(), desc.data(), static_cast<size_t>(n) * sizeof(sd_hog_image)), "vl_hog upload");
-    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_offset.as<int64_t>(), offset.data(), static_cast<size_t>(n) * sizeof(int64_t)), "vl_hog");
     sd_hog_images images{};
     images.d_data = buf.as<void>();
     images.dtype = type == CV_8UC1 ? SD_HOG_U8 : SD_HOG_F32;
     images.channels = channels;
     images.count = n;
     images.d_frames = d_desc.as<sd_hog_image>();
-    sd_b200::check(ctx, sd_hog_dense_images(ctx, &images, cell_size, num_bins, variant, bilinear_orientations ? 1 : 0, d_out.as<float>(),
-                                            d_offset.as<int64_t>()), "sd_hog_dense_images");
-    for (int i = 0; i < n; ++i) out.push_back(sd_b200::download(d_out.as<float>() + offset[i], rows[i], cols[i], cols[i]));
-    return out;
+    sd_b200::check(ctx, sd_hog_dense_images(ctx, &images, cell_size, num_bins, variant, bilinear_orientations ? 1 : 0, res.out(),
+                                            res.offsets(ctx, "vl_hog")), "sd_hog_dense_images");
+    return res.download();
 }
 
 // VLFeat HOG of gradient fields the caller computed (vl_hog_new(variant, num_bins),
@@ -427,14 +444,11 @@ inline std::vector<cv::Mat> vl_hog(const std::vector<std::vector<cv::Mat>>& fram
 inline std::vector<cv::Mat> vl_hog_polar(const std::vector<cv::Mat>& modulus, const std::vector<cv::Mat>& angle, VlHogVariant variant,
                                          int cell_size, int num_bins, bool directed = true, bool bilinear_orientations = false)
 {
-    std::vector<cv::Mat> out;
     if (modulus.size() != angle.size()) throw std::runtime_error("vl_hog_polar: modulus and angle must hold the same number of fields");
-    if (modulus.empty()) return out;
+    if (modulus.empty()) return {};
     const int n = static_cast<int>(modulus.size());
     std::vector<sd_hog_image> desc(n);
-    std::vector<int64_t> offset(n);
-    std::vector<int> rows(n), cols(n);
-    int64_t elems = 0, total = 0;
+    hog_batch::Results res;
     for (int i = 0; i < n; ++i) {
         const cv::Mat& m = modulus[i];
         const cv::Mat& a = angle[i];
@@ -447,40 +461,23 @@ inline std::vector<cv::Mat> vl_hog_polar(const std::vector<cv::Mat>& modulus, co
             throw std::runtime_error("vl_hog_polar: field " + std::to_string(i) + " (" + std::to_string(W) + " x " + std::to_string(H) +
                                      ") or the configuration is invalid: fields wider and taller than 3 px and at least half a cell, "
                                      "cell_size 1..32, num_bins 1..16");
-        desc[i].width = W;
-        desc[i].height = H;
-        desc[i].offset = elems;
-        desc[i].row_stride = W;
-        desc[i].pixel_stride = 1;
-        desc[i].channel_stride = 0;
-        elems += static_cast<int64_t>(W) * H;
-        offset[i] = total;
-        rows[i] = dd * h;
-        cols[i] = w;
-        total += static_cast<int64_t>(dd) * h * w;
+        desc[i] = sd_hog_image{W, H, 0, W, 1, 0};   // offset: where the field is packed
+        res.add(dd * h, w);
     }
     sd_ctx* ctx = sd_b200::context();
-    sd_b200::DeviceBuffer d_mod(static_cast<size_t>(elems) * sizeof(float)), d_ang(static_cast<size_t>(elems) * sizeof(float)),
-        d_desc(static_cast<size_t>(n) * sizeof(sd_hog_image)), d_out(static_cast<size_t>(total) * sizeof(float)),
-        d_offset(static_cast<size_t>(n) * sizeof(int64_t));
-    for (int i = 0; i < n; ++i) {
-        const size_t row_bytes = static_cast<size_t>(desc[i].width) * sizeof(float);
-        sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, d_mod.as<float>() + desc[i].offset, row_bytes, modulus[i].ptr<unsigned char>(0),
-                                            modulus[i].step(), row_bytes, static_cast<size_t>(desc[i].height)), "vl_hog_polar upload");
-        sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, d_ang.as<float>() + desc[i].offset, row_bytes, angle[i].ptr<unsigned char>(0),
-                                            angle[i].step(), row_bytes, static_cast<size_t>(desc[i].height)), "vl_hog_polar upload");
-    }
+    sd_b200::DeviceBuffer d_mod, d_ang, d_desc(static_cast<size_t>(n) * sizeof(sd_hog_image));
+    const std::vector<int64_t> start = hog_batch::pack_planes(ctx, modulus, sizeof(float), d_mod, "vl_hog_polar upload");
+    hog_batch::pack_planes(ctx, angle, sizeof(float), d_ang, "vl_hog_polar upload");   // the same starts: each pair is one size
+    for (int i = 0; i < n; ++i) desc[i].offset = start[i];
     sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_desc.as<sd_hog_image>(), desc.data(), static_cast<size_t>(n) * sizeof(sd_hog_image)), "vl_hog_polar upload");
-    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_offset.as<int64_t>(), offset.data(), static_cast<size_t>(n) * sizeof(int64_t)), "vl_hog_polar");
     sd_hog_polar_fields fields{};
     fields.d_modulus = d_mod.as<float>();
     fields.d_angle = d_ang.as<float>();
     fields.count = n;
     fields.d_frames = d_desc.as<sd_hog_image>();
     sd_b200::check(ctx, sd_hog_dense_polar(ctx, &fields, cell_size, num_bins, variant, directed ? 1 : 0, bilinear_orientations ? 1 : 0,
-                                           d_out.as<float>(), d_offset.as<int64_t>()), "sd_hog_dense_polar");
-    for (int i = 0; i < n; ++i) out.push_back(sd_b200::download(d_out.as<float>() + offset[i], rows[i], cols[i], cols[i]));
-    return out;
+                                           res.out(), res.offsets(ctx, "vl_hog_polar")), "sd_hog_dense_polar");
+    return res.download();
 }
 
 }  // namespace rcr

@@ -148,7 +148,7 @@ inline VlHog* vl_hog_new(VlHogVariant variant, vl_size numOrientations, vl_bool 
     VlHog* self = new VlHog();
     self->variant = variant;
     self->numOrientations = numOrientations;
-    self->dimension = variant == VlHogVariantUoctti ? 3 * numOrientations + 4 : 4 * numOrientations;
+    self->dimension = static_cast<vl_size>(sd_b200::hog_dimension(variant, K));
     self->transposed = transposed ? VL_TRUE : VL_FALSE;
     self->bilinear = VL_FALSE;
     self->hogWidth = self->hogHeight = 0;

@@ -107,6 +107,9 @@ inline std::vector<sd_host_frame> host_frames(const std::vector<cv::Mat>& images
     return frames;
 }
 
+// dd, the features per HOG cell of vl_hog_new(variant, num_bins): 3K + 4 for UoCTTI (variant 1), 4K for Dalal-Triggs
+inline int hog_dimension(int variant, int num_bins) { return variant == 1 ? 3 * num_bins + 4 : 4 * num_bins; }
+
 inline cv::Mat download(const float* d, int rows, int cols, int64_t ld)
 {
     cv::Mat m(rows, cols, CV_32FC1);
