@@ -365,6 +365,56 @@ SD_API int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins,
                             const float* d_filters, int num_filters, int filter_w, int filter_h,
                             const float* d_bias /* num_filters floats or NULL */, int pad_x, int pad_y, float* d_scores);
 
+/* ---- detections from HOG filter scores: thresholded boxes in frame pixels and greedy non-maximum suppression ----------------
+ * One score map of sd_hog_correlate's output: the [Q][height][width] scores of one pyramid level of one frame. */
+typedef struct {
+    int32_t frame;              /* in [0, num_frames): the frame whose detection list receives the map's detections */
+    int32_t level;              /* reported with each detection; not otherwise interpreted */
+    int32_t frame_w, frame_h;   /* the frame, px */
+    int32_t level_w, level_h;   /* the level, px (sd_hog_pyramid_shape); level_w == frame_w for an unscaled map */
+    int32_t width, height;      /* ow x oh score positions (either may be 0: no scores) */
+    int64_t offset;             /* floats: the map's scores at d_scores + offset */
+} sd_hog_score_map;
+typedef struct {
+    int32_t x, y, w, h;         /* box in frame pixels, the argument layout of sd_detect_faces_* */
+    float score;
+    int32_t filter, level;      /* filter index q, the map's level */
+    int32_t cell_x, cell_y;     /* score position in the map */
+} sd_hog_detection;
+/* sd_hog_detections: the detections of every frame of a batch, asynchronous on the context's stream.
+ *   Candidates.  Score (x, y) of filter q in a map is a candidate of the map's frame when score > threshold (a NaN score never
+ *     is).  d_above[f] (d_above may be NULL) receives frame f's candidate count before any cap.
+ *   Box.  Exact integer arithmetic in int64, rh(n, d) = floor((2n + d) / (2d)) (round half up, floor division),
+ *     sx = cell_size * frame_w, sy = cell_size * frame_h:
+ *       x0 = rh((x - pad_x) * sx, level_w),  x1 = rh((x - pad_x + filter_w) * sx, level_w),  rows alike with sy and level_h;
+ *     the box is (x0, y0, x1 - x0, y1 - y0), not clipped to the frame.  This is sd_hog_correlate's mapping of a score to pixels,
+ *     (x - pad_x) * cell_size * width / level_w, rounded.
+ *   Order.  A frame's candidates by score descending (scores compare as floats: -0 == +0), then in enumeration order: the map's
+ *     index in the table, then q, y, x.  The order is total.
+ *   Cap.  Only the first max_candidates candidates of a frame, in that order, go on to suppression.
+ *   Suppression.  Greedy over the capped list in order: a candidate is kept unless a kept candidate overlaps it with
+ *     (double)inter > overlap * (double)union, inter and union int64 pixel areas (torchvision's nms rule on these boxes); a box
+ *     of zero area never suppresses and is never suppressed.  overlap = 1 keeps every candidate.  Suppression stops when
+ *     max_detections candidates are kept.
+ *   Output.  Frame f's kept detections, in order, at d_out + f * max_detections; d_count[f] says how many.  Slots past the count
+ *     are not written.
+ *   Classes.  All filters of one call form one class (a filter and its mirror, mixture components).  Per-class suppression is one
+ *     call per class: a map's offset may point at filter q0's plane, with num_filters that class's filter count.
+ * A frame's result depends only on its own maps, in their table order: bit for bit the same in any batch and in every run.  The
+ * call reads the map table back once and queues its work; scratch is num_frames x max_candidates 8-byte keys, a small state per
+ * frame and three int32 per map.  Null pointers (d_scores and d_maps may be NULL when num_maps = 0), d_scores, d_out or d_count
+ * not 4-byte aligned, d_maps or d_above not 8-byte aligned, num_frames < 1, num_maps < 0, a map whose frame is out of range,
+ * whose offset is negative, whose frame or level is smaller than 1 x 1, whose size is negative or whose boxes do not fit in int32,
+ * more than 2^32 - 1 scores in one frame, overlap outside [0, 1], a NaN threshold, num_filters, cell_size (1..32), filter sides or
+ * pads outside sd_hog_correlate's limits, max_candidates outside [1, SD_HOG_DETECT_MAX_CANDIDATES], or max_detections outside
+ * [1, max_candidates] is SD_ERR_INVALID before any work is queued (nothing is written).  num_maps = 0 writes zero counts. */
+#define SD_HOG_DETECT_MAX_CANDIDATES 8192
+SD_API int sd_hog_detections(sd_ctx* ctx, const float* d_scores, const sd_hog_score_map* d_maps, int num_maps,
+                             int num_frames, int num_filters, int cell_size, int filter_w, int filter_h, int pad_x, int pad_y,
+                             float threshold, double overlap, int max_candidates, int max_detections,
+                             sd_hog_detection* d_out /* num_frames x max_detections */, int32_t* d_count /* num_frames */,
+                             int64_t* d_above /* num_frames, or NULL */);
+
 /* ---- regressor: LinearRegressor<Solver> (regressors.hpp:318-400) ------------------------ */
 /* Solver::solve (regressors.hpp:199-234 == verbose_solver.hpp:53-111):
  *   X = (A^T A + Lambda)^-1 A^T B ;  A: N x D, B: N x M, X: D x M (ldx_out = M).

@@ -73,6 +73,18 @@ class HogGridsC(C.Structure):
                 ("d_grids", C.c_void_p)]
 
 
+class HogScoreMapC(C.Structure):
+    """sd_hog_score_map: the [Q][height][width] scores of one pyramid level of one frame, at d_scores + offset (floats)."""
+    _fields_ = [("frame", C.c_int32), ("level", C.c_int32), ("frame_w", C.c_int32), ("frame_h", C.c_int32), ("level_w", C.c_int32),
+                ("level_h", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("offset", C.c_int64)]
+
+
+class HogDetectionC(C.Structure):
+    """sd_hog_detection: a box in frame pixels (x, y, w, h), its score, filter, level and score position."""
+    _fields_ = [("x", C.c_int32), ("y", C.c_int32), ("w", C.c_int32), ("h", C.c_int32), ("score", C.c_float),
+                ("filter", C.c_int32), ("level", C.c_int32), ("cell_x", C.c_int32), ("cell_y", C.c_int32)]
+
+
 class HostFrameC(C.Structure):
     """sd_host_frame: one host frame of a detect call (8UC1, or 8UC3 interleaved B, G, R)."""
     _fields_ = [("h_data", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32), ("row_stride", C.c_int32), ("channels", C.c_int32)]
@@ -111,7 +123,7 @@ EXPORTS = [
     "sd_memcpy2d_h2d", "sd_memcpy2d_d2h", "sd_memcpy2d_d2d",
     "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_bgr2gray", "sd_upload_frames", "sd_hog_dense_shape", "sd_hog_dense",
     "sd_hog_dense_images", "sd_hog_dense_polar", "sd_hog_permutation", "sd_hog_glyphs", "sd_hog_render", "sd_hog_relayout",
-    "sd_hog_pyramid_shape", "sd_hog_pyramid", "sd_hog_correlate",
+    "sd_hog_pyramid_shape", "sd_hog_pyramid", "sd_hog_correlate", "sd_hog_detections",
     "sd_learn", "sd_centre_features", "sd_learn_centred", "sd_learn_rank_revealing", "sd_gram", "sd_solve_gram", "sd_predict", "sd_test_residual", "sd_solver_timings", "sd_set_gram_mode", "sd_set_solver", "sd_solver_iterations",
     "sd_set_rank_diagnostic", "sd_last_rank",
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",
@@ -173,6 +185,8 @@ def lib():
         l.sd_hog_pyramid_shape.argtypes = [_i, _i, C.c_double, _i, _i, _i, _ip, _ip, _ip, _ip, _ip]
         l.sd_hog_pyramid.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_double), _i, _i, _i, _i, C.c_void_p, C.c_void_p]
         l.sd_hog_correlate.argtypes = [C.c_void_p, C.c_void_p, _i, _i, C.c_void_p, _i, _i, _i, C.c_void_p, _i, _i, C.c_void_p]
+        l.sd_hog_detections.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, _i, _i, _i, _i, _i, _i, _i, _i, C.c_float, C.c_double,
+                                        _i, _i, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = l
     return _lib
 

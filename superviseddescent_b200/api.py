@@ -14,6 +14,7 @@ plumbing only -- every computation below is a kernel of libsd_b200.so).
 """
 from __future__ import annotations
 
+import collections
 import ctypes as C
 import enum
 import itertools
@@ -25,7 +26,7 @@ import torch
 
 from . import _capi
 from ._capi import HogParam as HoGParam  # same field names as rcr::HoGParam
-from ._capi import HogGridC, HogGridsC, HogImageC, HogImagesC, HogPolarFieldsC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, ptr
+from ._capi import HogDetectionC, HogGridC, HogGridsC, HogImageC, HogImagesC, HogPolarFieldsC, HogScoreMapC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, ptr
 
 
 def _check(ctx, rc: int) -> None:
@@ -1602,3 +1603,57 @@ def vl_hog_correlate(maps, filters, num_bins: int, variant: int = 1, bias=None, 
     _check(ctx.h, _capi.lib().sd_hog_correlate(ctx.h, C.byref(g), int(num_bins), int(variant), ptr(f), int(q), int(fw), int(fh),
                                                ptr(b), pad_x, pad_y, ptr(out)))
     return scores
+
+
+HogDetections = collections.namedtuple("HogDetections", "frame boxes scores filter level cell above")
+HogDetections.__doc__ = """Detections of vl_hog_detect, in frame order and then in the rule's order within each frame: frame (n,) int32,
+boxes (n, 4) int32 (x, y, w, h in frame pixels), scores (n,) float32, filter (n,) int32, level (n,) int32 (the scale index),
+cell (n, 2) int32 (the score position x, y in its level), and above (num_frames,) int64, each frame's candidate count."""
+
+
+def vl_hog_detect(frames, scales, filters, cell_size: int, num_bins: int, threshold: float, variant: int = 1, bias=None, pad=(0, 0),
+                  overlap: float = 0.5, max_candidates: int = 4096, max_detections: int = 256,
+                  ctx: Optional[Context] = None) -> HogDetections:
+    """A sliding-window detector over image pyramids: vl_hog_pyramid of every frame at every scale, vl_hog_correlate of the
+    filter bank on every level (read in place), and one sd_hog_detections call over all score maps: the scores above threshold,
+    their boxes in frame pixels, the first max_candidates of each frame by score, and greedy non-maximum suppression at IoU
+    overlap over all filters as one class, up to max_detections per frame.  frames, scales, filters, bias and pad as
+    vl_hog_pyramid and vl_hog_correlate take them.  Returns HogDetections; detect_faces(frames, d.frame, boxes=d.boxes) takes
+    the result as it is."""
+    ctx = ctx or default_context()
+    f = _tensor(filters)
+    if f.dim() != 4:
+        raise ValueError("filters must be a (Q, dd, fh, fw) tensor")
+    q, _, fh, fw = f.shape
+    pad_x, pad_y = (int(p) for p in pad)
+    feats, levels = vl_hog_pyramid(frames, scales, cell_size, num_bins, variant, ctx=ctx)
+    n = len(feats)
+    if n == 0:
+        z = np.zeros(0, np.int32)
+        return HogDetections(z, np.zeros((0, 4), np.int32), np.zeros(0, np.float32), z, z, np.zeros((0, 2), np.int32),
+                             np.zeros(0, np.int64))
+    if isinstance(frames, (list, tuple)):
+        sizes = [(int(fr.shape[1]), int(fr.shape[0])) for fr in frames]
+    else:
+        sizes = [(int(frames.shape[2]), int(frames.shape[1]))] * n
+    which = [(i, s) for i in range(n) for s in range(len(scales)) if feats[i][s] is not None]
+    scores = vl_hog_correlate([feats[i][s] for i, s in which], f, num_bins, variant, bias=bias, pad=(pad_x, pad_y), ctx=ctx)
+    dev = f"cuda:{ctx.device}"
+    md = int(max_detections)
+    out = torch.empty((max(n, 1), max(md, 1), len(HogDetectionC._fields_)), dtype=torch.int32, device=dev)
+    count = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    above = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+    table, base = None, None
+    if which:
+        base = scores[0].untyped_storage().data_ptr()    # the maps' scores are views of one buffer
+        table = _device_table([HogScoreMapC(i, s, sizes[i][0], sizes[i][1], levels[i][s][0], levels[i][s][1], sc.shape[2], sc.shape[1],
+                                            sc.storage_offset()) for (i, s), sc in zip(which, scores)], dev)
+    _check(ctx.h, _capi.lib().sd_hog_detections(ctx.h, ptr(base), ptr(table), len(which), n, int(q), int(cell_size), int(fw), int(fh),
+                                                pad_x, pad_y, float(threshold), float(overlap), int(max_candidates), md, ptr(out),
+                                                ptr(count), ptr(above)))
+    counts = count.cpu().numpy()[:n].astype(np.int64)
+    rows = out.cpu().numpy()
+    r = np.concatenate([rows[i, :c] for i, c in enumerate(counts)] + [np.zeros((0, rows.shape[2]), np.int32)])
+    return HogDetections(np.repeat(np.arange(n, dtype=np.int32), counts), np.ascontiguousarray(r[:, 0:4]),
+                         np.ascontiguousarray(r[:, 4]).view(np.float32), np.ascontiguousarray(r[:, 5]), np.ascontiguousarray(r[:, 6]),
+                         np.ascontiguousarray(r[:, 7:9]), above.cpu().numpy()[:n].copy())

@@ -24,7 +24,9 @@ enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_LEVEL /* column shift and shifted-row weights of sd_train_level (sd_train.cu) */,
        SD_WS_GATHER /* frame, union, region, record and index tables of the levels on host frames (sd_train.cu) */,
        SD_WS_PYRAMID /* resized levels and level tables of one slice of sd_hog_pyramid (sd_hog_dense.cu) */,
-       SD_WS_FILTERS /* first CTA of every grid of sd_hog_correlate (sd_hog_filters.cu) */, SD_WS_COUNT };
+       SD_WS_FILTERS /* first CTA of every grid of sd_hog_correlate (sd_hog_filters.cu) */,
+       SD_WS_DETECT /* candidate keys, frame states, histograms and map tables of sd_hog_detections (sd_hog_detect.cu) */,
+       SD_WS_COUNT };
 
 // Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row
 // Cholesky blocks), and panel p belongs to rank p % nranks.  The Gram exchange delivers each panel's rows to their owner, and

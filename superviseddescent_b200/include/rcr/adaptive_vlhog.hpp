@@ -382,6 +382,79 @@ inline std::vector<cv::Mat> vl_hog_correlate(const std::vector<cv::Mat>& maps, c
     return res.download();
 }
 
+// One detection of vl_hog_detect: the box in frame pixels (not clipped to the frame), the score, the filter index q, the level
+// (the scale's index) and the score position in that level.
+struct hog_detection {
+    cv::Rect box;
+    float score;
+    int filter, level;
+    int cell_x, cell_y;
+};
+
+// A sliding-window detector over image pyramids: vl_hog_pyramid of every frame, vl_hog_correlate of the filter bank on every
+// level, then sd_hog_detections over all score maps (the scores above threshold, their boxes in frame pixels, the first
+// max_candidates of each frame by score, and greedy non-maximum suppression at IoU overlap over all filters as one class).
+// Arguments as vl_hog_pyramid and vl_hog_correlate take them.  Returns one list per frame, in the rule's order (include/sd_b200.h);
+// each box is what detect_faces takes.  Throws std::runtime_error where those calls or sd_hog_detections refuse.
+inline std::vector<std::vector<hog_detection>> vl_hog_detect(const std::vector<cv::Mat>& images, const std::vector<double>& scales,
+                                                             const std::vector<cv::Mat>& filters, VlHogVariant variant, int cell_size,
+                                                             int num_bins, const std::vector<float>& bias, int pad_x, int pad_y,
+                                                             float threshold, double overlap, int max_candidates, int max_detections)
+{
+    if (images.empty()) return {};
+    const std::vector<std::vector<cv::Mat>> pyr = vl_hog_pyramid(images, scales, variant, cell_size, num_bins);
+    const int dd = sd_b200::hog_dimension(variant, num_bins);
+    const int Q = static_cast<int>(filters.size());
+    if (Q < 1 || filters[0].rows % dd) throw std::runtime_error("vl_hog_detect: no filters, or filters not dd * fh rows");
+    const int fh = filters[0].rows / dd, fw = filters[0].cols;
+    const int n = static_cast<int>(images.size());
+    std::vector<cv::Mat> maps;
+    std::vector<sd_hog_score_map> descs;
+    for (int i = 0; i < n; ++i)
+        for (size_t s = 0; s < scales.size(); ++s) {
+            if (pyr[i][s].empty()) continue;
+            int lw = 0, lh = 0, w = 0, h = 0, d = 0;
+            sd_hog_pyramid_shape(images[i].cols, images[i].rows, scales[s], cell_size, num_bins, variant, &lw, &lh, &w, &h, &d);
+            maps.push_back(pyr[i][s]);
+            descs.push_back(sd_hog_score_map{i, static_cast<int32_t>(s), images[i].cols, images[i].rows, lw, lh, 0, 0, 0});
+        }
+    // the score maps with scores, packed end to end: a map smaller than the filter has no candidates
+    const std::vector<cv::Mat> scores = vl_hog_correlate(maps, filters, variant, num_bins, bias, pad_x, pad_y);
+    std::vector<cv::Mat> planes;
+    std::vector<sd_hog_score_map> table;
+    for (size_t k = 0; k < scores.size(); ++k)
+        if (!scores[k].empty()) {
+            planes.push_back(scores[k]);
+            table.push_back(descs[k]);
+            table.back().width = scores[k].cols;
+            table.back().height = scores[k].rows / Q;
+        }
+    sd_ctx* ctx = sd_b200::context();
+    sd_b200::DeviceBuffer d_scores, d_table(table.size() * sizeof(sd_hog_score_map));
+    const std::vector<int64_t> start = hog_batch::pack_planes(ctx, planes, sizeof(float), d_scores, "vl_hog_detect upload");
+    for (size_t k = 0; k < table.size(); ++k) table[k].offset = start[k];
+    if (!table.empty())
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_table.as<sd_hog_score_map>(), table.data(), table.size() * sizeof(sd_hog_score_map)),
+                       "vl_hog_detect upload");
+    const size_t slots = static_cast<size_t>(n) * static_cast<size_t>(std::max(max_detections, 1));
+    sd_b200::DeviceBuffer d_out(slots * sizeof(sd_hog_detection)), d_count(static_cast<size_t>(n) * sizeof(int32_t));
+    sd_b200::check(ctx, sd_hog_detections(ctx, d_scores.as<float>(), d_table.as<sd_hog_score_map>(), static_cast<int>(table.size()), n, Q,
+                                          cell_size, fw, fh, pad_x, pad_y, threshold, overlap, max_candidates, max_detections,
+                                          d_out.as<sd_hog_detection>(), d_count.as<int32_t>(), nullptr), "sd_hog_detections");
+    std::vector<sd_hog_detection> out(slots);
+    std::vector<int32_t> count(n);
+    sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.data(), d_out.as<void>(), slots * sizeof(sd_hog_detection)), "vl_hog_detect download");
+    sd_b200::check(ctx, sd_memcpy_d2h(ctx, count.data(), d_count.as<void>(), count.size() * sizeof(int32_t)), "vl_hog_detect download");
+    sd_b200::check(ctx, sd_sync(ctx), "vl_hog_detect download");
+    std::vector<std::vector<hog_detection>> result(n);
+    for (int i = 0; i < n; ++i)
+        for (int k = 0; k < count[i]; ++k) {
+            const sd_hog_detection& r = out[static_cast<size_t>(i) * max_detections + k];
+            result[i].push_back(hog_detection{cv::Rect(r.x, r.y, r.w, r.h), r.score, r.filter, r.level, r.cell_x, r.cell_y});
+        }
+    return result;
+}
+
 // VLFeat HOG of whole frames of one or more channels, 8-bit or float (vl_hog_new(variant, num_bins),
 // vl_hog_set_use_bilinear_orientation_assignments(bilinear_orientations), vl_hog_put_image(frame, channels, cell_size),
 // vl_hog_extract), in one batched call on the device (sd_hog_dense_images).  Each frame is the list of its channel planes --
