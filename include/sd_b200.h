@@ -415,6 +415,127 @@ SD_API int sd_hog_detections(sd_ctx* ctx, const float* d_scores, const sd_hog_sc
                              sd_hog_detection* d_out /* num_frames x max_detections */, int32_t* d_count /* num_frames */,
                              int64_t* d_above /* num_frames, or NULL */);
 
+/* ---- training HOG filters: window rows, a squared-hinge linear SVM and hard-negative mining ---------------------------------
+ * One window of a batch of grids: score position (x, y) of sd_hog_correlate on grid `grid`; flip = 1 reads the window of the
+ * left-right mirrored image. */
+typedef struct {
+    int32_t grid, x, y, flip;
+} sd_hog_window;
+/* sd_hog_windows: the feature row of every window, asynchronous on the context's stream.  With D = dd * fh * fw + 1, row r holds
+ * what score (x, y) of sd_hog_correlate reads, in the filter layout:
+ *   rows[r * ldr + (c * fh + dy) * fw + dx] = M[c][y + dy - pad_y][x + dx - pad_x]      (M = 0 outside the grid)
+ * and rows[r * ldr + D - 1] = 1.0, the bias column of the centred learn path; columns D .. ldr - 1 are not written.  A flipped
+ * window is sd_hog_relayout(flip = 1) of the fh x fw block it reads: plane perm[c] (sd_hog_permutation), columns mirrored.  A
+ * pure gather: row . [F | b] in float64 is sd_hog_correlate's score of [F | b] within that call's float32 rounding.  The call
+ * reads the grid table (if any) and the window table back once.  Null or unaligned pointers (4 bytes), an invalid configuration,
+ * filter sides or pads outside sd_hog_correlate's limits, ldr < D, a window whose grid is out of range, whose (x, y) is not a
+ * score position of its grid, or whose flip is not 0 or 1 is SD_ERR_INVALID before any work is queued (d_rows is not written). */
+SD_API int sd_hog_windows(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int variant, int filter_w, int filter_h, int pad_x,
+                          int pad_y, const sd_hog_window* d_windows, int count, float* d_rows, int64_t ldr);
+/* sd_hog_box_windows: host only.  For each ground-truth box (boxes[4 b ..] = x, y, w, h in pixels of a frame_w x frame_h frame)
+ * the window that covers it best over the frame's pyramid at the given scales: the candidates are every score position of every
+ * non-empty level (sd_hog_pyramid_shape), each with the exact integer box sd_hog_detections reports for it; the best has the
+ * largest IoU over int64 areas, compared exactly as rationals, ties to the lower level, then y, then x.  out[b] = (level, x, y,
+ * 0) and iou[b] = its IoU as a double; a box whose best window fails (double) inter >= positive_overlap * (double) union gets
+ * grid = -1.  SD_ERR_INVALID for null pointers, a frame smaller than 1 x 1, an invalid scale or configuration, filter sides or
+ * pads outside sd_hog_correlate's limits, positive_overlap outside [0, 1], or a box with w or h < 1. */
+SD_API int sd_hog_box_windows(int frame_w, int frame_h, const double* scales, int num_scales, int cell_size, int num_bins,
+                              int variant, int filter_w, int filter_h, int pad_x, int pad_y, double positive_overlap,
+                              const int32_t* boxes, int num_boxes, sd_hog_window* out, double* iou);
+/* sd_learn_squared_hinge: the linear SVM with squared hinge loss,
+ *   minimise f(w) = lambda / 2 * sum_{j < D-1} w_j^2 + 1/2 * sum_i max(0, 1 - y_i a_i . w)^2,
+ * rows a_i of A (N x D, the last column the all-ones bias, which is not regularised), labels y_i = +1 or -1.  The primal finite
+ * Newton method (Keerthi & DeCoste 2005): from w = 0 (every row active), each step solves the ridge system on the active rows
+ * S = {i : y_i a_i . w < 1}, (lambda I' + A_S^T A_S) w = A_S^T y_S, with sd_learn_centred (Manual lambda, bias unregularised) on
+ * rows shifted by one column mean fixed for the whole solve (sd_centre_features on the first step's rows, which are all of them).
+ * The margins of the Newton point are computed in float64 on the device; if its active set is S it is the optimum, otherwise an
+ * exact line search on the host (phi(t) = f(w + t d) is a convex piecewise quadratic, minimised in float64 over its sorted
+ * breakpoints) gives the next point.  It stops when the active set after a step equals the set the step was solved on
+ * (SD_SVM_CONVERGED), when f does not decrease (SD_SVM_NO_DECREASE: the last point that decreased f is kept), or after
+ * max_iterations steps.  The context's solver and Gram settings apply as for sd_learn_centred.  d_A is not modified; the scratch
+ * is N x roundup4(D + 1) floats of compacted rows and N doubles of margins, plus the learn path's own workspace.  Each step reads
+ * back the N margins and synchronises.  The result is the same in every run.  Null or unaligned (4 bytes) pointers, a label
+ * other than +1 or -1, lambda <= 0 or not finite, N < 1, D < 2, lda < D or max_iterations < 1 is SD_ERR_INVALID before any work
+ * is queued (d_w is not written). */
+#define SD_SVM_CONVERGED 0
+#define SD_SVM_NO_DECREASE 1
+#define SD_SVM_ITERATION_CAP 2
+typedef struct {
+    int32_t iterations;          /* Newton steps taken */
+    int32_t active;              /* |S| at the returned w */
+    int32_t stop;                /* SD_SVM_* */
+    int32_t reserved;
+    double objective;            /* f at the returned w, float64 */
+} sd_svm_report;
+SD_API int sd_learn_squared_hinge(sd_ctx* ctx, const float* d_A, int64_t lda, const float* d_y, int N, int D, float lambda,
+                                  int max_iterations, float* d_w /* D */, sd_svm_report* report /* may be NULL */);
+/* sd_hog_train_filter: a HOG filter for the sliding-window detector (sd_hog_pyramid + sd_hog_correlate + sd_hog_detections),
+ * trained by a squared-hinge SVM with hard-negative mining.  The rule:
+ *   Positives.  Each box is assigned its window by sd_hog_box_windows with positive_overlap = (double) p->positive_overlap (the
+ *     float widened, so a threshold such as 0.7 is the float nearest to it); with flip_positives each assigned box
+ *     also adds its mirrored window.  Rows are in box order, each unflipped row followed by its mirror.  Unassigned boxes are
+ *     counted and skipped.  The positive set is fixed across rounds.
+ *   Round 0.  The filter is the mean of the unflipped positive rows (feature columns, float64 sums rounded to float) minus its
+ *     own scalar mean (float64, rounded to float), bias 0.  Each frame gives its detections under this filter: sd_hog_detections
+ *     over all its levels with threshold -FLT_MAX, max_candidates SD_HOG_DETECT_MAX_CANDIDATES, overlap mine_overlap and
+ *     max_detections negatives_per_frame; a window whose box overlaps a box of its frame with (double) inter > negative_overlap *
+ *     (double) union is excluded.  Then the first solve runs.
+ *   Rounds 1 .. rounds.  The same mining with the current filter and bias at threshold -1 (the windows that violate the margin).
+ *   Cache.  Windows already cached, by (frame, level, x, y), are not new.  New windows take the next empty slot of the cache;
+ *     when it is full, the slots of cached negatives that are inactive under the round's filter (margin >= 1), in slot order;
+ *     when those are used up, the round's remaining new windows are truncated.  New windows come in frame order and, within a
+ *     frame, in the detection order.  A round after round 0 that adds no window ends the training, and its solve is skipped.
+ *   Solve.  sd_learn_squared_hinge (lambda, max_iterations) on the positive rows (+1) followed by the cache in slot order (-1).
+ *   Frames without boxes are pure negative frames.  The pyramids are computed a slice of frames at a time (about 256 MB of
+ *   features each) and each slice is mined and gathered while it is resident; the scratch does not grow with the number of
+ *   frames, apart from per-frame and per-box tables and the (positives + max_negatives) x D rows.  The result depends only on the
+ *   frames, boxes and parameters, bit for bit the same in every run.
+ * Output: d_filter (device, dd * fh * fw floats, the [dd][fh][fw] layout of sd_hog_correlate), *h_bias, one report per round in
+ * h_rounds[0 .. rounds] (entries after an early stop are zero), the cache in slot order in h_negatives (max_negatives entries, or
+ * NULL; grid = frame * num_scales + level, flip 0) and its size in *h_num_negatives.  The frames are an sd_image_batch as for
+ * sd_hog_pyramid (no d_roi).  Null pointers, an invalid configuration, scale, filter side or pad, a box whose frame is out of
+ * range or whose w or h < 1, lambda <= 0, overlaps outside [0, 1], flip_positives outside {0, 1}, rounds < 0, negatives_per_frame
+ * outside [1, SD_HOG_DETECT_MAX_CANDIDATES], max_negatives < 1, max_iterations < 1, D above SD_HOG_TRAIN_MAX_DIM or no assigned
+ * box is SD_ERR_INVALID, and rows, Gram and one slice that would not fit in device memory SD_ERR_CUDA, before any work is
+ * queued. */
+#define SD_HOG_TRAIN_MAX_DIM 8192   /* D = dd * fh * fw + 1: 31 x 16 x 16 + 1 = 7937 fits; the Gram is 256 MB at the cap */
+typedef struct {
+    int32_t frame, x, y, w, h;
+} sd_hog_box;
+typedef struct {
+    float lambda;                 /* on the filter, not the bias */
+    float positive_overlap;       /* e.g. 0.5: minimum IoU of a box's window (sd_hog_box_windows) */
+    float negative_overlap;       /* e.g. 0.3: a mined window overlapping a box of its frame by more is not a negative */
+    int32_t flip_positives;       /* 1: every positive also as its mirrored window */
+    int32_t rounds;               /* mining rounds after round 0 */
+    int32_t negatives_per_frame;  /* per frame and round (sd_hog_detections' max_detections) */
+    float mine_overlap;           /* suppression among one frame's mined windows; 1 = none */
+    int32_t max_negatives;        /* rows of the negative cache */
+    int32_t max_iterations;       /* Newton iterations per solve */
+} sd_hog_train_param;
+typedef struct {
+    int32_t positives;            /* positive rows (mirrors included) */
+    int32_t unassigned;           /* boxes no window covers at positive_overlap */
+    int32_t cache;                /* cached negatives after the round's mining */
+    int32_t mined;                /* windows the round's detections gave, after the box exclusion */
+    int32_t excluded;             /* windows excluded for overlapping a box */
+    int32_t added;                /* new windows that entered the cache */
+    int32_t evicted;              /* inactive cached negatives whose slots new windows took */
+    int32_t truncated;            /* new windows dropped because the cache was full */
+    int32_t solved;               /* 1: the round's solve ran */
+    int32_t reserved;
+    sd_svm_report solve;
+    /* the round's phases: CUDA events around the pyramids, the scores, the detections and the window gathers (kernel only; its
+     * tables are uploaded before), the host clock around the host filtering (the detections' download and the box exclusion)
+     * and around the solve (which ends synchronised); round 0 includes the pass that gathers the positives */
+    float pyramid_ms, scores_ms, detect_ms, host_ms, gather_ms, solve_ms;
+    double gathered_bytes;        /* rows read and written by the round's gathers: 2 x rows x D x 4 */
+} sd_hog_train_report;
+SD_API int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_box* h_boxes, int num_boxes,
+                               const double* h_scales, int num_scales, int cell_size, int num_bins, int variant, int filter_w,
+                               int filter_h, int pad_x, int pad_y, const sd_hog_train_param* p, float* d_filter, float* h_bias,
+                               sd_hog_train_report* h_rounds, sd_hog_window* h_negatives, int* h_num_negatives);
+
 /* ---- regressor: LinearRegressor<Solver> (regressors.hpp:318-400) ------------------------ */
 /* Solver::solve (regressors.hpp:199-234 == verbose_solver.hpp:53-111):
  *   X = (A^T A + Lambda)^-1 A^T B ;  A: N x D, B: N x M, X: D x M (ldx_out = M).

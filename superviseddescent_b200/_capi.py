@@ -85,6 +85,38 @@ class HogDetectionC(C.Structure):
                 ("filter", C.c_int32), ("level", C.c_int32), ("cell_x", C.c_int32), ("cell_y", C.c_int32)]
 
 
+class HogWindowC(C.Structure):
+    """sd_hog_window: score position (x, y) of grid `grid`; flip = 1 reads the window of the mirrored image."""
+    _fields_ = [("grid", C.c_int32), ("x", C.c_int32), ("y", C.c_int32), ("flip", C.c_int32)]
+
+
+class SvmReportC(C.Structure):
+    """sd_svm_report: Newton steps, final |S|, stop reason (0 converged, 1 no decrease, 2 iteration cap) and f in float64."""
+    _fields_ = [("iterations", C.c_int32), ("active", C.c_int32), ("stop", C.c_int32), ("reserved", C.c_int32),
+                ("objective", C.c_double)]
+
+
+class HogBoxC(C.Structure):
+    """sd_hog_box: a ground-truth box (x, y, w, h) in pixels of frame `frame`."""
+    _fields_ = [("frame", C.c_int32), ("x", C.c_int32), ("y", C.c_int32), ("w", C.c_int32), ("h", C.c_int32)]
+
+
+class HogTrainParamC(C.Structure):
+    """sd_hog_train_param: the training rule's parameters (include/sd_b200.h, sd_hog_train_filter)."""
+    _fields_ = [("lambda_", C.c_float), ("positive_overlap", C.c_float), ("negative_overlap", C.c_float),
+                ("flip_positives", C.c_int32), ("rounds", C.c_int32), ("negatives_per_frame", C.c_int32),
+                ("mine_overlap", C.c_float), ("max_negatives", C.c_int32), ("max_iterations", C.c_int32)]
+
+
+class HogTrainReportC(C.Structure):
+    """sd_hog_train_report: one mining round and its solve."""
+    _fields_ = [("positives", C.c_int32), ("unassigned", C.c_int32), ("cache", C.c_int32), ("mined", C.c_int32),
+                ("excluded", C.c_int32), ("added", C.c_int32), ("evicted", C.c_int32), ("truncated", C.c_int32),
+                ("solved", C.c_int32), ("reserved", C.c_int32), ("solve", SvmReportC), ("pyramid_ms", C.c_float),
+                ("scores_ms", C.c_float), ("detect_ms", C.c_float), ("host_ms", C.c_float), ("gather_ms", C.c_float),
+                ("solve_ms", C.c_float), ("gathered_bytes", C.c_double)]
+
+
 class HostFrameC(C.Structure):
     """sd_host_frame: one host frame of a detect call (8UC1, or 8UC3 interleaved B, G, R)."""
     _fields_ = [("h_data", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32), ("row_stride", C.c_int32), ("channels", C.c_int32)]
@@ -124,6 +156,7 @@ EXPORTS = [
     "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_bgr2gray", "sd_upload_frames", "sd_hog_dense_shape", "sd_hog_dense",
     "sd_hog_dense_images", "sd_hog_dense_polar", "sd_hog_permutation", "sd_hog_glyphs", "sd_hog_render", "sd_hog_relayout",
     "sd_hog_pyramid_shape", "sd_hog_pyramid", "sd_hog_correlate", "sd_hog_detections",
+    "sd_hog_windows", "sd_hog_box_windows", "sd_learn_squared_hinge", "sd_hog_train_filter",
     "sd_learn", "sd_centre_features", "sd_learn_centred", "sd_learn_rank_revealing", "sd_gram", "sd_solve_gram", "sd_predict", "sd_test_residual", "sd_solver_timings", "sd_set_gram_mode", "sd_set_solver", "sd_solver_iterations",
     "sd_set_rank_diagnostic", "sd_last_rank",
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",
@@ -187,6 +220,13 @@ def lib():
         l.sd_hog_correlate.argtypes = [C.c_void_p, C.c_void_p, _i, _i, C.c_void_p, _i, _i, _i, C.c_void_p, _i, _i, C.c_void_p]
         l.sd_hog_detections.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, _i, _i, _i, _i, _i, _i, _i, _i, C.c_float, C.c_double,
                                         _i, _i, C.c_void_p, C.c_void_p, C.c_void_p]
+        l.sd_hog_windows.argtypes = [C.c_void_p, C.c_void_p, _i, _i, _i, _i, _i, _i, C.c_void_p, _i, C.c_void_p, C.c_int64]
+        l.sd_hog_box_windows.argtypes = [_i, _i, C.c_void_p, _i, _i, _i, _i, _i, _i, _i, _i, C.c_double, C.c_void_p, _i,
+                                         C.c_void_p, C.c_void_p]
+        l.sd_learn_squared_hinge.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, _i, _i, C.c_float, _i, C.c_void_p,
+                                             C.c_void_p]
+        l.sd_hog_train_filter.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, _i, C.c_void_p, _i, _i, _i, _i, _i, _i, _i, _i,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = l
     return _lib
 

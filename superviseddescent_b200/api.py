@@ -26,7 +26,7 @@ import torch
 
 from . import _capi
 from ._capi import HogParam as HoGParam  # same field names as rcr::HoGParam
-from ._capi import HogDetectionC, HogGridC, HogGridsC, HogImageC, HogImagesC, HogPolarFieldsC, HogScoreMapC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, ptr
+from ._capi import HogBoxC, HogDetectionC, HogGridC, HogGridsC, HogImageC, HogImagesC, HogPolarFieldsC, HogScoreMapC, HogTrainParamC, HogTrainReportC, HogWindowC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, SvmReportC, ptr
 
 
 def _check(ctx, rc: int) -> None:
@@ -1657,3 +1657,163 @@ def vl_hog_detect(frames, scales, filters, cell_size: int, num_bins: int, thresh
     return HogDetections(np.repeat(np.arange(n, dtype=np.int32), counts), np.ascontiguousarray(r[:, 0:4]),
                          np.ascontiguousarray(r[:, 4]).view(np.float32), np.ascontiguousarray(r[:, 5]), np.ascontiguousarray(r[:, 6]),
                          np.ascontiguousarray(r[:, 7:9]), above.cpu().numpy()[:n].copy())
+
+
+# ------------------------------------------------------------------------------------------------
+# training HOG filters: window rows, a squared-hinge SVM and hard-negative mining
+# ------------------------------------------------------------------------------------------------
+def _maps_table(maps, dd: int, dev):
+    """A list of (dd, h, w) float32 CUDA maps -> (HogGridsC, tensors it points to): read in place when they are contiguous views
+    of one storage (as vl_hog_pyramid returns them), packed otherwise -- vl_hog_correlate's rule."""
+    if any(not isinstance(m, torch.Tensor) or not m.is_cuda or m.dtype != torch.float32 or m.dim() != 3 or m.shape[0] != dd
+           for m in maps):
+        raise ValueError(f"every map must be a float32 CUDA tensor (dd, h, w) with dd = {dd}")
+    maps = [m.to(dev) for m in maps]
+    stor = maps[0].untyped_storage().data_ptr()
+    if all(m.is_contiguous() and m.untyped_storage().data_ptr() == stor for m in maps):
+        base, keep = stor, maps
+        offs = [(m.data_ptr() - base) // 4 for m in maps]
+    else:
+        keep, offs = _pack(maps, dev)
+        base = keep.data_ptr()
+    table = _device_table([HogGridC(m.shape[2], m.shape[1], o, 0) for m, o in zip(maps, offs)], dev)
+    g = HogGridsC()
+    g.d_features, g.count, g.width, g.height, g.d_grids = base, len(maps), 0, 0, table.data_ptr()
+    return g, (keep, table)
+
+
+def vl_hog_windows(maps, windows, filter_size, num_bins: int, variant: int = 1, pad=(0, 0), ctx: Optional[Context] = None):
+    """The feature rows of score positions (sd_hog_windows): row r is the window that score (x, y) of vl_hog_correlate on map
+    `grid` reads, in the filter layout [dd][fh][fw] flattened, then a 1.0 bias column -- D = dd * fh * fw + 1 floats.  flip = 1
+    gives the window of the mirrored image (vl_hog_flip of the block).  maps: a list of (dd, h, w) float32 CUDA tensors as
+    vl_hog_correlate takes them; windows: an (n, 4) int array of (grid, x, y, flip); filter_size = (fw, fh).  Returns an (n, D)
+    float32 CUDA tensor."""
+    ctx = ctx or default_context()
+    dd = _hog_dims(num_bins, variant)
+    dev = f"cuda:{ctx.device}"
+    fw, fh = (int(v) for v in filter_size)
+    pad_x, pad_y = (int(v) for v in pad)
+    w = np.ascontiguousarray(np.asarray(windows, np.int32).reshape(-1, 4))
+    n, D = w.shape[0], dd * fw * fh + 1
+    rows = torch.empty((max(n, 1), D), dtype=torch.float32, device=dev)
+    maps = list(maps)
+    if not maps:
+        raise ValueError("vl_hog_windows needs at least one map")
+    g, keep = _maps_table(maps, dd, dev)
+    d_w = torch.from_numpy(w if n else np.zeros((1, 4), np.int32)).to(dev)
+    _check(ctx.h, _capi.lib().sd_hog_windows(ctx.h, C.byref(g), int(num_bins), int(variant), fw, fh, pad_x, pad_y, ptr(d_w), n,
+                                             ptr(rows), C.c_int64(D)))
+    return rows[:n]
+
+
+def hog_box_windows(width: int, height: int, boxes, scales, filter_size, cell_size: int, num_bins: int, variant: int = 1,
+                    pad=(0, 0), positive_overlap: float = 0.5):
+    """For each ground-truth box (x, y, w, h) of one width x height frame, the window of the frame's pyramid that covers it best
+    (sd_hog_box_windows, host only): the largest exact IoU between the box and the integer box sd_hog_detections reports for a
+    score position, ties to the lower level, then y, then x.  Returns (windows, iou): an (n, 3) int32 array of (level, x, y),
+    level -1 where the best IoU is below positive_overlap, and the (n,) float64 IoU of each box's best window."""
+    b = np.ascontiguousarray(np.asarray(boxes, np.int32).reshape(-1, 4))
+    n = b.shape[0]
+    sc = (C.c_double * max(len(scales), 1))(*[float(s) for s in scales])
+    out = (HogWindowC * max(n, 1))()
+    iou = np.zeros(max(n, 1), np.float64)
+    fw, fh = (int(v) for v in filter_size)
+    pad_x, pad_y = (int(v) for v in pad)
+    rc = _capi.lib().sd_hog_box_windows(int(width), int(height), sc, len(scales), int(cell_size), int(num_bins), int(variant), fw, fh,
+                                        pad_x, pad_y, float(positive_overlap), C.c_void_p(b.ctypes.data), n, out,
+                                        C.c_void_p(iou.ctypes.data))
+    if rc:
+        raise SdError(rc, f"invalid hog_box_windows arguments: frame {width} x {height}, scales {list(scales)}, filter {fw} x {fh}, "
+                          f"pad ({pad_x}, {pad_y}), cell_size {cell_size}, positive_overlap {positive_overlap}, or a box with w or h < 1")
+    win = np.array([(out[i].grid, out[i].x, out[i].y) for i in range(n)], np.int32).reshape(n, 3)
+    return win, iou[:n].copy()
+
+
+SvmReport = collections.namedtuple("SvmReport", "iterations active stop objective")
+SvmReport.__doc__ = """Report of learn_squared_hinge: Newton steps, the final active-set size, the stop reason ("converged",
+"no decrease" or "iteration cap") and the objective f in float64."""
+_SVM_STOP = {0: "converged", 1: "no decrease", 2: "iteration cap"}
+
+
+def _svm_report(r) -> SvmReport:
+    return SvmReport(int(r.iterations), int(r.active), _SVM_STOP[int(r.stop)], float(r.objective))
+
+
+def learn_squared_hinge(A, y, lam: float, max_iterations: int = 50, ctx: Optional[Context] = None):
+    """Linear SVM with squared hinge loss on the device (sd_learn_squared_hinge): w minimising
+        lam / 2 * sum_{j < D-1} w_j^2 + 1/2 * sum_i max(0, 1 - y_i a_i . w)^2
+    over the rows of A (N x D; the last column all ones: the unregularised bias), y_i = +1 or -1, by the primal finite Newton
+    method on the learn path.  Returns (w, SvmReport): w a (D,) float32 CUDA tensor."""
+    ctx = ctx or default_context()
+    A = _dev(A, ctx)
+    yy = _dev(y, ctx).reshape(-1)
+    if A.dim() != 2 or yy.shape[0] != A.shape[0]:
+        raise ValueError("A must be (N, D) and y (N,)")
+    N, D = A.shape
+    w = torch.empty(D, dtype=torch.float32, device=A.device)
+    rep = SvmReportC()
+    _check(ctx.h, _capi.lib().sd_learn_squared_hinge(ctx.h, ptr(A), C.c_int64(A.stride(0)), ptr(yy), N, D, float(lam),
+                                                     int(max_iterations), ptr(w), C.byref(rep)))
+    return w, _svm_report(rep)
+
+
+HogFilter = collections.namedtuple("HogFilter", "filter bias negatives report")
+HogFilter.__doc__ = """Result of train_hog_filter: filter (dd, fh, fw) float32 CUDA tensor, bias (float), negatives (n, 4) int32
+array of the negative cache in slot order (frame, level, x, y), and report, one dict per mining round (the fields of
+sd_hog_train_report, the solve as an SvmReport, or None when the round's solve was skipped; times_ms, the round's phases in
+milliseconds, and gathered_bytes).  positive_overlap reaches the library as a float: the positives are hog_box_windows(...,
+positive_overlap=float(np.float32(positive_overlap)))."""
+
+
+def train_hog_filter(frames, box_frame, boxes, scales, filter_size, cell_size: int, num_bins: int, variant: int = 1, pad=(0, 0),
+                     lam: float = 0.01, positive_overlap: float = 0.5, negative_overlap: float = 0.3, flip_positives: bool = False,
+                     rounds: int = 3, negatives_per_frame: int = 32, mine_overlap: float = 0.5, max_negatives: int = 8192,
+                     max_iterations: int = 50, ctx: Optional[Context] = None) -> HogFilter:
+    """Train a HOG filter for vl_hog_detect (sd_hog_train_filter): each box's best window as a positive (hog_box_windows, with
+    its mirror if flip_positives), round 0 with the mean positive minus its mean as the filter, then `rounds` rounds of
+    hard-negative mining at the margin (threshold -1) and a squared-hinge SVM (learn_squared_hinge) each.  frames as
+    vl_hog_pyramid takes them; box_frame (n,) and boxes (n, 4) (x, y, w, h) in the layout of HogDetections.
+    vl_hog_detect(frames, scales, hf.filter[None], ..., bias=[hf.bias]) takes the result as it is."""
+    ctx = ctx or default_context()
+    dd = _hog_dims(num_bins, variant)
+    fw, fh = (int(v) for v in filter_size)
+    pad_x, pad_y = (int(v) for v in pad)
+    scales = [float(s) for s in scales]
+    if not scales:
+        raise ValueError("train_hog_filter needs at least one scale")
+
+    def check(w, h):
+        for s in scales:
+            hog_pyramid_shape(w, h, s, cell_size, num_bins, variant)
+
+    keep, ib, sizes = _grey_frames(frames, ctx, check)
+    if not sizes:
+        raise ValueError("train_hog_filter needs at least one frame")
+    bf = np.asarray(box_frame, np.int64).reshape(-1)
+    bx = np.asarray(boxes, np.int64).reshape(-1, 4)
+    if bf.shape[0] != bx.shape[0]:
+        raise ValueError("box_frame and boxes must have one entry per box")
+    nb = bx.shape[0]
+    hb = (HogBoxC * max(nb, 1))(*[HogBoxC(int(f), *(int(v) for v in b)) for f, b in zip(bf, bx)])
+    prm = HogTrainParamC(float(lam), float(positive_overlap), float(negative_overlap), int(bool(flip_positives)), int(rounds),
+                         int(negatives_per_frame), float(mine_overlap), int(max_negatives), int(max_iterations))
+    dev = f"cuda:{ctx.device}"
+    filt = torch.empty((dd, fh, fw), dtype=torch.float32, device=dev)
+    bias = C.c_float(0)
+    reps = (HogTrainReportC * (int(rounds) + 1))() if rounds >= 0 else None
+    negs = (HogWindowC * max(int(max_negatives), 1))()
+    nn = C.c_int(0)
+    sc = (C.c_double * len(scales))(*scales)
+    _check(ctx.h, _capi.lib().sd_hog_train_filter(ctx.h, C.byref(ib), hb, nb, sc, len(scales), int(cell_size), int(num_bins),
+                                                  int(variant), fw, fh, pad_x, pad_y, C.byref(prm), ptr(filt), C.byref(bias), reps,
+                                                  negs, C.byref(nn)))
+    S = len(scales)
+    neg = np.array([(negs[k].grid // S, negs[k].grid % S, negs[k].x, negs[k].y) for k in range(nn.value)], np.int32).reshape(-1, 4)
+    report = []
+    for r in reps:
+        d = {f: int(getattr(r, f)) for f, _ in HogTrainReportC._fields_[:10] if f != "reserved"}
+        d["solve"] = _svm_report(r.solve) if r.solved else None
+        d["times_ms"] = {f[:-3]: float(getattr(r, f)) for f in ("pyramid_ms", "scores_ms", "detect_ms", "host_ms", "gather_ms", "solve_ms")}
+        d["gathered_bytes"] = float(r.gathered_bytes)
+        report.append(d)
+    return HogFilter(filt, float(bias.value), neg, report)

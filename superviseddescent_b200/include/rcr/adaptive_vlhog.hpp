@@ -455,6 +455,47 @@ inline std::vector<std::vector<hog_detection>> vl_hog_detect(const std::vector<c
     return result;
 }
 
+// A HOG filter trained by train_hog_filter: the filter in the shell's filter layout (dd * fh rows of fw floats, as vl_hog_correlate
+// and vl_hog_detect take filters), its bias, one report per round (sd_hog_train_report; rounds after an early stop are zero) and
+// the negative cache in slot order (grid = frame * scales.size() + level).
+struct hog_filter {
+    cv::Mat filter;
+    float bias;
+    std::vector<sd_hog_train_report> rounds;
+    std::vector<sd_hog_window> negatives;
+};
+
+// Trains a HOG filter for vl_hog_detect with a squared-hinge SVM and hard-negative mining (sd_hog_train_filter; the rule is in
+// include/sd_b200.h).  images: 8UC1 or 8UC3 (B,G,R) frames of any sizes; box k, boxes[k] in frame pixels, belongs to frame
+// box_frame[k]; frames without a box are pure negative frames.  Throws std::runtime_error where sd_hog_train_filter refuses.
+inline hog_filter train_hog_filter(const std::vector<cv::Mat>& images, const std::vector<int>& box_frame, const std::vector<cv::Rect>& boxes,
+                                   const std::vector<double>& scales, VlHogVariant variant, int cell_size, int num_bins, int filter_w,
+                                   int filter_h, int pad_x, int pad_y, const sd_hog_train_param& params)
+{
+    if (images.empty()) throw std::runtime_error("train_hog_filter: no frames");
+    if (box_frame.size() != boxes.size()) throw std::runtime_error("train_hog_filter: box_frame and boxes differ in length");
+    if (params.rounds < 0 || params.max_negatives < 1) throw std::runtime_error("train_hog_filter: rounds < 0 or max_negatives < 1");
+    sd_ctx* ctx = sd_b200::context();
+    const std::vector<sd_host_frame> frames = sd_b200::host_frames(images);
+    sd_b200::DeviceBuffer buf;
+    const sd_image_batch batch = hog_batch::upload_grey(ctx, frames, buf, "train_hog_filter upload");
+    std::vector<sd_hog_box> hb;
+    for (size_t k = 0; k < boxes.size(); ++k)
+        hb.push_back(sd_hog_box{box_frame[k], boxes[k].x, boxes[k].y, boxes[k].width, boxes[k].height});
+    const int dd = sd_b200::hog_dimension(variant, num_bins);
+    sd_b200::DeviceBuffer d_filter(static_cast<size_t>(dd) * filter_h * filter_w * sizeof(float));
+    hog_filter out;
+    out.rounds.resize(static_cast<size_t>(params.rounds) + 1);
+    out.negatives.resize(static_cast<size_t>(params.max_negatives));
+    int num_negatives = 0;
+    sd_b200::check(ctx, sd_hog_train_filter(ctx, &batch, hb.data(), static_cast<int>(hb.size()), scales.data(), static_cast<int>(scales.size()),
+                                            cell_size, num_bins, variant, filter_w, filter_h, pad_x, pad_y, &params, d_filter.as<float>(),
+                                            &out.bias, out.rounds.data(), out.negatives.data(), &num_negatives), "sd_hog_train_filter");
+    out.negatives.resize(static_cast<size_t>(num_negatives));
+    out.filter = sd_b200::download(d_filter.as<float>(), dd * filter_h, filter_w, filter_w);
+    return out;
+}
+
 // VLFeat HOG of whole frames of one or more channels, 8-bit or float (vl_hog_new(variant, num_bins),
 // vl_hog_set_use_bilinear_orientation_assignments(bilinear_orientations), vl_hog_put_image(frame, channels, cell_size),
 // vl_hog_extract), in one batched call on the device (sd_hog_dense_images).  Each frame is the list of its channel planes --
