@@ -88,10 +88,11 @@ __global__ void hog_geometry_kernel(const float* __restrict__ x, long long ldx, 
     }
 }
 
-// ---- spatial binning tables of vl_hog_put_image (hog.c:697-709), once per launch: btab[c * fs + t] = weight with which pixel
-//      coordinate t votes into cell index c (w1 for its own bin, w2 for the next one, 0 otherwise); then, as ints, the first and
-//      last interior coordinate that votes into cell c (same tables for rows and columns: square patch, square cells) ---------
-__global__ void hog_bintab_kernel(int fs, int nc, int cs, float* __restrict__ btab)
+// ---- spatial binning tables of vl_hog_put_image (hog.c:697-709), once per launch: btab[c * pw + t - 1] = weight with which
+//      interior pixel coordinate t (1 .. fs - 2) votes into cell index c (w1 for its own bin, w2 for the next one, 0 otherwise;
+//      pw = fs - 2 rounded up to even, the padding entry 0); then, as ints, the first and last interior coordinate that votes
+//      into cell c (same tables for rows and columns: square patch, square cells) ------------------------------------------
+__global__ void hog_bintab_kernel(int fs, int nc, int cs, int pw, float* __restrict__ btab)
 {
     __shared__ int s_sbin[256];
     for (int t = threadIdx.x; t < fs; t += blockDim.x) {
@@ -99,10 +100,13 @@ __global__ void hog_bintab_kernel(int fs, int nc, int cs, float* __restrict__ bt
         float w1, w2;
         hog_spatial_weight(t, cs, &b, &w1, &w2);
         s_sbin[t] = b;
-        for (int c = 0; c < nc; ++c) btab[c * fs + t] = (b == c) ? w1 : ((b == c - 1) ? w2 : 0.f);
+        if (t >= 1 && t <= fs - 2)
+            for (int c = 0; c < nc; ++c) btab[c * pw + t - 1] = (b == c) ? w1 : ((b == c - 1) ? w2 : 0.f);
+        else if (t == fs - 1 && pw > fs - 2)
+            for (int c = 0; c < nc; ++c) btab[c * pw + pw - 1] = 0.f;
     }
     __syncthreads();
-    int* lohi = reinterpret_cast<int*>(btab + nc * fs);
+    int* lohi = reinterpret_cast<int*>(btab + nc * pw);
     for (int c = threadIdx.x; c < nc; c += blockDim.x) {
         int lo = fs, hi = -1;
         for (int t = 1; t <= fs - 2; ++t) {
@@ -122,6 +126,7 @@ struct HogSmem {
     int patch, bin, r1, tab, xa, wcell, lo, hi, vote, mbar, stage_end, total;
     int pp;        // row pitch of the resized patch: fs rounded up to a multiple of 4
     int pb, pm;    // row pitches of the interior bins (bytes, a multiple of 4) and moduli (floats, odd)
+    int pw;        // row pitch of the binning weights (floats, even)
     int tpad;      // tasks of the horizontal vote pass, padded to a multiple of 32
 };
 
@@ -133,7 +138,8 @@ __host__ __device__ inline int align_up(int v, int a) { return (v + a - 1) / a *
 // pixel (y, x) at (y - 1) * pitch + x - 1, so that S2's runs of four start on a word of bins.  Pass 1 of the vote reads
 // one row per lane: an odd pitch (moduli) keeps those reads free of bank conflicts, and so does an odd number of words
 // between rows of bins where that fits in fs * fs bytes.  Both regions hold fs * fs pixels, as before: the staging area
-// and the largest configuration are the same.
+// and the largest configuration are the same.  The binning weights hold the interior coordinates only, t at c * pw + t - 1
+// with an even pitch, so that a pair (t, t + 1) with t odd is one aligned 8-byte word of weights and one 16-bit word of bins.
 __host__ __device__ inline HogSmem hog_smem_layout(int fs, int nc, int K)
 {
     HogSmem s;
@@ -146,7 +152,8 @@ __host__ __device__ inline HogSmem hog_smem_layout(int fs, int nc, int K)
     o = align_up(s.pp * fs, 16);
     s.tab = o;    o += fs * 16;                             // int4 {x source index, y source index 0 / 1, y weights (2 x int16)}
     s.xa = o;     o += fs * 4;                              // x weights, 2 x int16
-    s.wcell = o;  o += nc * fs * 4;                         // weight of pixel t for cell index c (0 if it does not vote)
+    s.pw = align_up(fs - 2, 2);
+    s.wcell = align_up(o, 8); o = s.wcell + nc * s.pw * 4; // weight of pixel t for cell index c (0 if it does not vote)
     s.lo = o;     o += nc * 4;
     s.hi = o;     o += nc * 4;
     s.mbar = align_up(o, 8); o = s.mbar + 8;
@@ -185,7 +192,7 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
     const int fs = (NCT > 0 && CST > 0) ? NCT * CST : a.fs;
     const int cells = nc * nc;
     const HogSmem lay = hog_smem_layout(fs, nc, K);
-    const int pp = lay.pp, pb = lay.pb, pm = lay.pm;
+    const int pp = lay.pp, pb = lay.pb, pm = lay.pm, pw = lay.pw;
     uint8_t* s_patch = smem + lay.patch;
     int8_t* s_bin = reinterpret_cast<int8_t*>(smem + lay.bin);
     float* s_gmag = reinterpret_cast<float*>(smem + lay.r1);
@@ -265,8 +272,8 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
             s_xa[t] = *reinterpret_cast<const short2*>(&xa);
             s_tab[t] = make_int4(__ldg(rt + t), __ldg(rt + 2 * fs + t), __ldg(rt + 3 * fs + t), __ldg(rt + 4 * fs + t));
         }
-        for (int i = tid; i < nc * fs; i += NT) s_wcell[i] = __ldg(a.btab + i);
-        const int* __restrict__ lohi = reinterpret_cast<const int*>(a.btab + nc * fs);
+        for (int i = tid; i < nc * pw; i += NT) s_wcell[i] = __ldg(a.btab + i);
+        const int* __restrict__ lohi = reinterpret_cast<const int*>(a.btab + nc * pw);
         if (tid < nc) { s_lo[tid] = __ldg(lohi + tid); s_hi[tid] = __ldg(lohi + nc + tid); }
     }
     {
@@ -459,25 +466,35 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
 
     // ---- S3: bilinear spatial vote (hog.c:697-724), separable:  hist[b][cj][ci] = sum_y wy[cj][y] * ( sum_x wx[ci][x] * g[y][x] * [bin[y][x] == b] ).
     //      Pass 1: one thread per (cell column ci, interior row y) walks the <= 2*cs pixels of that row that vote into ci and adds
-    //      g * wx into ITS OWN column of T[bin][task] (bank == task mod 32: conflict free, no atomics, fixed order).
-    //      Pass 2: one thread per (bin, cell) folds the rows with wy.  The reference adds (g * wx) * wy per pixel in raster
-    //      order; this is the same sum associated differently (~1e-7 relative), deterministic.
+    //      g * wx into ITS OWN column of T[bin][task] (bank == task mod 32: conflict free, no atomics, fixed order).  It takes
+    //      the pixels in aligned pairs (x, x + 1), x odd: one 16-bit load of their bins and one 8-byte load of their weights.
+    //      Pass 2: one thread per (bin b < K, cell) folds the rows with wy for bins b and b + K, one weight load for both.  The
+    //      reference adds (g * wx) * wy per pixel in raster order; this is the same sum associated differently (~1e-7
+    //      relative), deterministic, and every product and add is the dense kernel's (sd_hog_dense.cu) in its order.
     {
         const int nrow = fs - 2, ntask = nrow * nc, tpad = lay.tpad;
         for (int task = tid; task < ntask; task += NT) {
             const int ci = task / nrow, y = 1 + task - ci * nrow;
             const int xlo = s_lo[ci], xhi = s_hi[ci];
-            const int8_t* bp = s_bin + (y - 1) * pb + (xlo - 1);
-            const float* gp = s_gmag + (y - 1) * pm + (xlo - 1);
-            const float* wp = s_wcell + ci * fs + xlo;
+            // pixel x of this row and cell column: bin bp[x], modulus gp[x], weight wp[x]
+            const int8_t* bp = s_bin + (y - 1) * pb - 1;
+            const float* gp = s_gmag + (y - 1) * pm - 1;
+            const float* wp = s_wcell + ci * pw - 1;
             float* T = s_T + task;
             for (int b = 0; b < 2 * K; ++b) T[b * tpad] = 0.f;        // T shares the staging area of S1: clear this column first
-#pragma unroll 2
-            for (int x = xlo; x <= xhi; ++x) {
-                const int b = max((int)*bp++, 0);                     // no bin: bin -1, modulus stored as 0 -> adds +0 to bin 0
-                float* q = T + b * tpad;
-                *q = __fadd_rn(*q, __fmul_rn(*gp++, *wp++));
+            // no bin: bin -1, modulus stored as 0 -> adds +0 to bin 0
+            const auto vote = [&](int b, float p) { float* q = T + max(b, 0) * tpad; *q = __fadd_rn(*q, p); };
+            int x = xlo;
+            if (!(x & 1) && x <= xhi) { vote(bp[x], __fmul_rn(gp[x], wp[x])); ++x; }
+            // both vote loops rolled: unrolled, they push S1's cold load loops of some schedules past 32 registers
+#pragma unroll 1
+            for (; x < xhi; x += 2) {
+                const unsigned bb = *reinterpret_cast<const unsigned short*>(bp + x);
+                const float2 w = *reinterpret_cast<const float2*>(wp + x);
+                vote((int)(int8_t)bb, __fmul_rn(gp[x], w.x));
+                vote((int)(int8_t)(bb >> 8), __fmul_rn(gp[x + 1], w.y));
             }
+            if (x == xhi) vote(bp[x], __fmul_rn(gp[x], wp[x]));
         }
         __syncthreads();
         // Only the ntask columns that pass 1 cleared and filled are read here: hog_bintab_kernel keeps lo and hi inside the
@@ -486,15 +503,22 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
         // The histogram hist[b * cells + c] goes to the first 2K cells floats of this landmark's slice of the feature row
         // (which holds cells * dd >= 3K cells floats), where hog_normalise_kernel turns it into the features.
         float* __restrict__ out = a.A + (long long)sample * a.ld + (long long)lm * cells * a.dd;
-        for (int i = tid; i < 2 * K * cells; i += NT) {
+        for (int i = tid; i < K * cells; i += NT) {
             const int b = i / cells, c = i - b * cells;
             const int cj = c / nc, ci = c - cj * nc;                  // cell row (y), cell column (x)
             const int ylo = s_lo[cj], yhi = s_hi[cj];
             const float* Tp = s_T + b * tpad + ci * nrow + (ylo - 1);
-            const float* wy = s_wcell + cj * fs + ylo;
-            float acc = 0.f;
-            for (int y = ylo; y <= yhi; ++y) acc = __fadd_rn(acc, __fmul_rn(*Tp++, *wy++));
+            const float* wy = s_wcell + cj * pw + (ylo - 1);
+            float acc = 0.f, acc2 = 0.f;                              // bins b and b + K
+#pragma unroll 1
+            for (int y = ylo; y <= yhi; ++y) {
+                const float w = *wy++;
+                acc = __fadd_rn(acc, __fmul_rn(Tp[0], w));
+                acc2 = __fadd_rn(acc2, __fmul_rn(Tp[K * tpad], w));
+                ++Tp;
+            }
             out[i] = acc;
+            out[i + K * cells] = acc2;
         }
     }
 }
@@ -638,7 +662,7 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
     float* d_btab = reinterpret_cast<float*>(d_rtab + (size_t)N * 5 * fs);
     hog_geometry_kernel<<<N, 64, 0, ctx->stream>>>(d_x, ldx, N, L, eyes_dev, p->relative_patch_size, fixed_half, fs, d_half, d_rtab, a.status);
     SD_LAUNCH_CHECK(ctx, "hog_geometry_kernel");
-    hog_bintab_kernel<<<1, 256, 0, ctx->stream>>>(fs, a.nc, a.cs, d_btab);
+    hog_bintab_kernel<<<1, 256, 0, ctx->stream>>>(fs, a.nc, a.cs, lay.pw, d_btab);
     SD_LAUNCH_CHECK(ctx, "hog_bintab_kernel");
     a.half = d_half;
     a.rtab = d_rtab;
