@@ -169,6 +169,41 @@ def test_descriptor_gaps_keep_canaries(sd):
     assert len(spans) == 3
 
 
+@pytest.mark.parametrize("Q", [1, 2, 3, 9, 256])
+def test_equally_sized_grids_without_a_table(sd, Q):
+    """A batch tensor of grids with d_grids = NULL: grid i's scores at d_scores + i Q oh ow, within the bars and bit for bit the
+    scores of the same maps passed with a table; one call per grid size (the route has one size per call)."""
+    from superviseddescent_b200 import _capi
+    from superviseddescent_b200._capi import HogGridsC
+    K, variant, fh, fw, count, lead, tail = 9, 1, 6, 6, 3, 13, 29
+    dd = _dd(K, variant)
+    rng = np.random.default_rng(300 + Q)
+    f = torch.from_numpy(rng.normal(0, 1, (Q, dd, fh, fw)).astype(np.float32)).cuda()
+    bias = torch.from_numpy(rng.normal(0, 3, Q).astype(np.float32)).cuda()
+    ctx = sd.default_context()
+    # partial tiles in both directions, a 1 x 1 grid (scored through the pads), and a grid smaller than the filter
+    for (h, w), pad in [((33, 65), (0, 0)), ((17, 31), (2, 3)), ((1, 1), (5, 5)), ((4, 5), (0, 0))]:
+        batch = torch.from_numpy(rng.uniform(0, 0.4, (count, dd, h, w)).astype(np.float32)).cuda()
+        oh, ow = h + 2 * pad[1] - fh + 1, w + 2 * pad[0] - fw + 1
+        n = Q * max(oh, 0) * max(ow, 0)
+        out = torch.full((lead + count * n + tail,), CANARY, dtype=torch.float32, device="cuda")
+        g = HogGridsC()
+        g.d_features, g.count, g.width, g.height, g.d_grids = batch.data_ptr(), count, w, h, None
+        rc = _capi.lib().sd_hog_correlate(ctx.h, C.byref(g), K, variant, _capi.ptr(f), Q, fw, fh, _capi.ptr(bias), pad[0], pad[1],
+                                          _capi.ptr(out[lead:]))
+        assert rc == 0
+        torch.cuda.synchronize()
+        assert bool((out[:lead] == CANARY).all()) and bool((out[lead + count * n:] == CANARY).all()), (h, w)
+        if n == 0:
+            print(f"Q {Q} grid {h}x{w}: smaller than the filter, nothing written")
+            continue
+        got = out[lead:lead + count * n].view(count, Q, oh, ow)
+        table = sd.vl_hog_correlate(list(batch), f, K, variant, bias=bias, pad=pad)
+        for i in range(count):
+            _check(got[i], batch[i], f, bias, pad, f"Q {Q} equally sized grid {i} {h}x{w} pad {pad}")
+            assert torch.equal(got[i].view(torch.int32), table[i].view(torch.int32)), (Q, h, w, i)
+
+
 def test_refusals_leave_scores_untouched(sd):
     from superviseddescent_b200 import _capi
     from superviseddescent_b200._capi import HogGridsC

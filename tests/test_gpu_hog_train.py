@@ -1,11 +1,13 @@
 """Training HOG filters on the device: sd_hog_windows, sd_learn_squared_hinge and sd_hog_train_filter (api.vl_hog_windows,
 api.learn_squared_hinge, api.train_hog_filter).
 
-- Window rows are numpy slicing of the maps bit for bit, with pads, flips and grids of different sizes; canaries around the rows
+- Window rows are numpy slicing of the maps bit for bit, with pads, flips, grids of different sizes and a batch of equally sized
+  grids without a descriptor table; canaries around the rows
   and in the ldr gap survive; a flipped row is the unflipped row of the mirrored position in vl_hog_flip's grid; row . [F | b]
   in float64 is vl_hog_correlate's score within the float32 bound of its FMA chain; every refusal writes nothing.
 - The SVM's w is within tests/chol_ref.py's per-element bars of the float64 ridge solution on its final active set, at D <= 256
-  (the LU route) and D > 256 (the centred Cholesky), on random rows and on HOG rows from the gather; every row's float64 margin
+  (the LU route) and D > 256 (the centred Cholesky) up to D = 4,093 with fewer rows than features, on random rows and on HOG
+  rows from the gather; every row's float64 margin
   agrees with that set except rows within the margin bar of 1; f decreases at every step.
 - The trainer's filter and bias are learn_squared_hinge on the rows rebuilt from its negatives and the assigned positives with
   the public primitives, bit for bit; two runs are identical.
@@ -76,6 +78,38 @@ def test_windows_are_slices_of_the_maps(sd, K, variant, fw, fh, px, py):
     assert (got[0] == CANARY).all() and (got[-1] == CANARY).all() and (got[1:-1, D:] == CANARY).all()
     # the public wrapper gives the same rows
     assert torch.equal(sd.vl_hog_windows(maps, win, (fw, fh), K, variant, pad=(px, py)), rows[1:-1, :D])
+
+
+def test_windows_of_equally_sized_grids(sd):
+    """A batch tensor of grids with d_grids = NULL: window (grid, x, y) reads grid * dd * h * w floats in."""
+    rng = np.random.default_rng(17)
+    K, variant, fw, fh, px, py, B, h, w = 9, 1, 5, 4, 2, 1, 6, 11, 17
+    dd = sd._hog_dims(K, variant)
+    batch = torch.from_numpy(rng.uniform(0, 0.4, (B, dd, h, w)).astype(np.float32)).cuda()
+    win = _random_windows(rng, [(h, w)] * B, fw, fh, px, py, 400)
+    assert set(win[:, 0].tolist()) == set(range(B))
+    D = dd * fw * fh + 1
+    ldr = D + 3
+    rows = torch.full((len(win) + 2, ldr), float(CANARY), device="cuda")
+    g = _capi.HogGridsC()
+    g.d_features, g.count, g.width, g.height, g.d_grids = batch.data_ptr(), B, w, h, None
+    d_w = torch.from_numpy(win).cuda()
+    ctx = sd.default_context()
+    rc = _capi.lib().sd_hog_windows(ctx.h, sd.C.byref(g), K, variant, fw, fh, px, py, _capi.ptr(d_w), len(win),
+                                    _capi.ptr(rows[1:]), ldr)
+    assert rc == 0
+    got = rows.cpu().numpy()
+    perm = sd.vl_hog_permutation(variant, K)
+    maps = batch.cpu().numpy()
+    for r, (gi, x, y, fl) in enumerate(win):
+        blk = _window_ref(maps[gi], x, y, fw, fh, px, py)
+        if fl:
+            blk = blk[perm][:, :, ::-1]
+        ref = np.concatenate([blk.ravel(), [1.0]]).astype(np.float32)
+        assert np.array_equal(got[1 + r, :D].view(np.uint32), ref.view(np.uint32)), (r, gi, x, y, fl)
+    assert (got[0] == CANARY).all() and (got[-1] == CANARY).all() and (got[1:-1, D:] == CANARY).all()
+    # the same maps through a table give the same rows
+    assert torch.equal(sd.vl_hog_windows(list(batch), win, (fw, fh), K, variant, pad=(px, py)), rows[1:-1, :D])
 
 
 def test_flip_identity_through_relayout(sd):
@@ -212,7 +246,7 @@ def _check_svm(sd, A, y, lam, name):
 
 
 @pytest.mark.parametrize("N,D,lam,hog_like", [(400, 40, 0.5, False), (900, 200, 2.0, True), (1500, 300, 1.0, True),
-                                              (2000, 513, 4.0, True)])
+                                              (2000, 513, 4.0, True), (4000, 1117, 4.0, True), (2500, 4093, 4.0, True)])
 def test_svm_within_the_bars_of_its_active_set(sd, N, D, lam, hog_like):
     A, y = _svm_problem(np.random.default_rng(N + D), N, D, hog_like)
     _check_svm(sd, A, y, lam, "random" if not hog_like else "hog-like")
