@@ -536,6 +536,99 @@ SD_API int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const 
                                int filter_h, int pad_x, int pad_y, const sd_hog_train_param* p, float* d_filter, float* h_bias,
                                sd_hog_train_report* h_rounds, sd_hog_window* h_negatives, int* h_num_negatives);
 
+/* ---- deformable part models: bounded distance transforms, star-model scores and the part boxes of each detection -----------
+ * A star model has Q components.  Component q is a root filter (filter_w x filter_h cells) scored on a level of scale s, and P
+ * part filters (part_w x part_h cells) scored on the level of scale 2 s, each allowed to move from its anchor at a quadratic
+ * cost.  The part score maps are one sd_hog_correlate call with the Q * P part filters as one bank ([Q * P][ph][pw] per part
+ * level, part q * P + p at plane q * P + p).
+ *
+ * sd_hog_distance_transform: the bounded generalised distance transform of every plane of a batch of maps, asynchronous on the
+ * context's stream.  maps is an sd_hog_grids of maps of num_planes planes each, [num_planes][h][w] score positions (planes of
+ * sd_hog_correlate with num_filters = num_planes; the grid descriptor's width and height are the planes' w and h).  Plane k of
+ * every map uses h_deformation[4 k .. 4 k + 3] = (w0, w1, w2, w3): a displacement (dx, dy) costs w0 dx^2 + w1 dx + w2 dy^2 + w3 dy
+ * score positions of its level.  R = max_displacement bounds |dx| and |dy|; R >= max(w, h) makes the transform unbounded in
+ * effect (the transform of DPM is unbounded).  The rule, in float32 where it says fl():
+ *   Cost tables (host): cx[d] = (float)((double) w0 d d + (double) w1 d) and cy[e] = (float)((double) w2 e e + (double) w3 e) for
+ *     d, e in [-R, R]; every entry must be finite.
+ *   Pass X: t(y, u) is the best of fl(s(y, u + d) - cx[d]) over d = -R .. R ascending with 0 <= u + d < w, where a non-NaN
+ *     candidate replaces the current best when there is none yet or when it is strictly greater; dx(y, u) is the chosen d.  With
+ *     no non-NaN candidate t = -inf and there is no choice.
+ *   Pass Y: D(v, u) is the best of fl(t(v + e, u) - cy[e]) over e = -R .. R ascending with 0 <= v + e < h, by the same rule.  The
+ *     placement is (u + dx(v + e*, u), v + e*) for the chosen e*, or (-1, -1) when pass Y chose nothing or the chosen row's pass
+ *     X chose nothing.
+ * The value equals the brute-force maximum of fl(fl(s - cx) - cy) over (dx, dy) (fl(a - c) is monotone in a).  The placement
+ * follows the separable tie rule -- the smallest e, then the smallest d within that row -- which differs from a lexicographic
+ * brute force in rare rounding cases.  Output: the values of plane k of map i at d_values + out_offset + k * h * w (equally
+ * sized maps: (i * num_planes + k) * h * w), and, when d_place is not NULL, int32 (u, v) pairs at d_place + 2 * (the same
+ * offset).  Each value depends on its plane, deformation and R alone: the same in any batch and in every run.  Null pointers,
+ * d_values not 4-byte or d_place not 8-byte aligned, num_planes outside [1, SD_HOG_FILTER_MAX_BANK], max_displacement outside
+ * [0, SD_HOG_PART_MAX_DISPLACEMENT], a cost entry that is not finite, or a grid smaller than 1 x 1 or with a negative offset is
+ * SD_ERR_INVALID before any work is queued (nothing is written). */
+#define SD_HOG_PART_MAX_DISPLACEMENT 32
+#define SD_HOG_PART_MAX_PARTS 32
+SD_API int sd_hog_distance_transform(sd_ctx* ctx, const sd_hog_grids* maps, int num_planes, const float* h_deformation,
+                                     int max_displacement, float* d_values, int32_t* d_place /* or NULL */);
+/* A star model's geometry; its filters and deformations are the caller's (the correlate and transform calls take them). */
+typedef struct {
+    int32_t num_components, num_parts;   /* Q >= 1, P in [1, SD_HOG_PART_MAX_PARTS], Q * P <= SD_HOG_FILTER_MAX_BANK */
+    int32_t filter_w, filter_h;          /* root filter, cells */
+    int32_t part_w, part_h;              /* part filters, cells of the part level */
+    int32_t pad_x, pad_y;                /* the root correlate's pad, in [0, filter side - 1] */
+    int32_t part_pad_x, part_pad_y;      /* the part correlate's pad, in [0, part side - 1] */
+    const int32_t* d_anchors;            /* device, 8-byte aligned: [Q][P][2] (ax, ay) part-level cells relative to twice the
+                                          * root window's top-left cell */
+} sd_hog_part_model;
+/* One root map (one frame at one root level) and its paired part level. */
+typedef struct {
+    int32_t frame, level;                /* as the root map's sd_hog_score_map: detections report them */
+    int32_t frame_w, frame_h;            /* the frame, px */
+    int32_t part_level_w, part_level_h;  /* the part level, px (sd_hog_pyramid_shape) */
+    int32_t width, height;               /* root score positions, ow x oh */
+    int32_t part_width, part_height;     /* part score positions, pw x ph (either may be 0: every anchor is outside) */
+    int64_t root_offset;                 /* floats: the root scores [Q][oh][ow] (bias included) at d_root + root_offset */
+    int64_t part_offset;                 /* floats: the part maps [Q * P][ph][pw] at d_parts + part_offset */
+    int64_t out_offset;                  /* floats: the star model's scores [Q][oh][ow] at d_out + out_offset */
+} sd_hog_part_map;
+/* sd_hog_part_scores: the star model's score maps, asynchronous on the context's stream.  d_parts holds the transformed part
+ * maps (sd_hog_distance_transform's values).  For root position (x, y) of component q, parts p = 0 .. P - 1 in order:
+ *   u0 = 2 (x - pad_x) + ax[q][p] + part_pad_x,  v0 = 2 (y - pad_y) + ay[q][p] + part_pad_y
+ *   total = root[q][y][x];  total = fl(total + D[q P + p][v0][u0])
+ * and the total is -inf when any anchor lies outside [0, pw) x [0, ph).  The output has the root map's geometry, so
+ * sd_hog_detections takes it unchanged with num_filters = Q and the root's filter size and pad: its boxes are the root boxes and
+ * the components compete in one suppression; a -inf total is never a candidate.  The call reads the map table back once.  Null
+ * or unaligned pointers (4 bytes; the table and anchors 8), a model outside its limits (sd_hog_part_model), num_maps < 0, or a
+ * map with a negative size or offset is SD_ERR_INVALID before any work is queued (nothing is written). */
+SD_API int sd_hog_part_scores(sd_ctx* ctx, const float* d_root, const float* d_parts, const sd_hog_part_map* d_maps, int num_maps,
+                              const sd_hog_part_model* model, float* d_out);
+/* One part of one detection: its placement (u, v) in part score positions, its term D (the transformed part score at the
+ * anchor), and its box in frame pixels (x, y, w, h). */
+typedef struct {
+    int32_t u, v;
+    float term;
+    int32_t x, y, w, h;
+} sd_hog_part_placement;
+/* sd_hog_part_placements: the parts of every detection of sd_hog_detections on sd_hog_part_scores' maps.  d_det and d_count are
+ * that call's output as it is (frame f's detections at d_det + f * max_detections, d_count[f] of them); each detection's
+ * (frame, level) selects its table entry, and its filter is the component q.  d_parts holds the part score maps BEFORE the
+ * transform, at the table's part_offset (the transform writes its values at the same offsets when out_offset = offset).  At
+ * the anchor (u0, v0) of each part the transform's rule is recomputed from those maps with h_deformation (Q * P entries of 4)
+ * and max_displacement, so the placement and term are bit for bit sd_hog_distance_transform's there.  Box, by sd_hog_detections'
+ * rule at the part level, sx = cell_size * frame_w, sy = cell_size * frame_h:
+ *   x0 = rh((u - part_pad_x) sx, part_level_w),  x1 = rh((u - part_pad_x + part_w) sx, part_level_w),  rows alike;
+ * the box is (x0, y0, x1 - x0, y1 - y0).  A part whose anchor lies outside the part map, or that has no placement, gets
+ * (-1, -1), term -inf (outside) or the transform's value, and a zero box.  Output: detection k of frame f, part p at
+ * d_out + (f * max_detections + k) * P + p; slots past the count are not written.  The call reads the table, the counts and the
+ * detections back once.  Null or unaligned pointers, a model outside its limits, max_displacement or a cost entry as
+ * sd_hog_distance_transform refuses them, cell_size outside [1, 32], num_frames < 1, max_detections outside
+ * [1, SD_HOG_DETECT_MAX_CANDIDATES], a map with a negative size or offset, a frame out of range, a frame or part level smaller
+ * than 1 x 1 or part boxes that do not fit in int32, two maps with one (frame, level), a count outside [0, max_detections], or a
+ * detection whose (frame, level) is not in the table or whose filter or score position is not one of its map is SD_ERR_INVALID
+ * before any work is queued (nothing is written). */
+SD_API int sd_hog_part_placements(sd_ctx* ctx, const float* d_parts, const sd_hog_part_map* d_maps, int num_maps,
+                                  const sd_hog_part_model* model, const float* h_deformation, int max_displacement, int cell_size,
+                                  const sd_hog_detection* d_det, const int32_t* d_count, int num_frames, int max_detections,
+                                  sd_hog_part_placement* d_out /* num_frames x max_detections x P */);
+
 /* ---- regressor: LinearRegressor<Solver> (regressors.hpp:318-400) ------------------------ */
 /* Solver::solve (regressors.hpp:199-234 == verbose_solver.hpp:53-111):
  *   X = (A^T A + Lambda)^-1 A^T B ;  A: N x D, B: N x M, X: D x M (ldx_out = M).

@@ -90,6 +90,27 @@ class HogWindowC(C.Structure):
     _fields_ = [("grid", C.c_int32), ("x", C.c_int32), ("y", C.c_int32), ("flip", C.c_int32)]
 
 
+class HogPartModelC(C.Structure):
+    """sd_hog_part_model: a star model's geometry (Q components of P parts) and its device anchors [Q][P][2]."""
+    _fields_ = [("num_components", C.c_int32), ("num_parts", C.c_int32), ("filter_w", C.c_int32), ("filter_h", C.c_int32),
+                ("part_w", C.c_int32), ("part_h", C.c_int32), ("pad_x", C.c_int32), ("pad_y", C.c_int32), ("part_pad_x", C.c_int32),
+                ("part_pad_y", C.c_int32), ("d_anchors", C.c_void_p)]
+
+
+class HogPartMapC(C.Structure):
+    """sd_hog_part_map: one root map (frame, level) and its paired part level; offsets in floats."""
+    _fields_ = [("frame", C.c_int32), ("level", C.c_int32), ("frame_w", C.c_int32), ("frame_h", C.c_int32),
+                ("part_level_w", C.c_int32), ("part_level_h", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
+                ("part_width", C.c_int32), ("part_height", C.c_int32), ("root_offset", C.c_int64), ("part_offset", C.c_int64),
+                ("out_offset", C.c_int64)]
+
+
+class HogPartPlacementC(C.Structure):
+    """sd_hog_part_placement: a part's placement (u, v), its term and its box (x, y, w, h) in frame pixels."""
+    _fields_ = [("u", C.c_int32), ("v", C.c_int32), ("term", C.c_float), ("x", C.c_int32), ("y", C.c_int32), ("w", C.c_int32),
+                ("h", C.c_int32)]
+
+
 class SvmReportC(C.Structure):
     """sd_svm_report: Newton steps, final |S|, stop reason (0 converged, 1 no decrease, 2 iteration cap) and f in float64."""
     _fields_ = [("iterations", C.c_int32), ("active", C.c_int32), ("stop", C.c_int32), ("reserved", C.c_int32),
@@ -157,6 +178,7 @@ EXPORTS = [
     "sd_hog_dense_images", "sd_hog_dense_polar", "sd_hog_permutation", "sd_hog_glyphs", "sd_hog_render", "sd_hog_relayout",
     "sd_hog_pyramid_shape", "sd_hog_pyramid", "sd_hog_correlate", "sd_hog_detections",
     "sd_hog_windows", "sd_hog_box_windows", "sd_learn_squared_hinge", "sd_hog_train_filter",
+    "sd_hog_distance_transform", "sd_hog_part_scores", "sd_hog_part_placements",
     "sd_learn", "sd_centre_features", "sd_learn_centred", "sd_learn_rank_revealing", "sd_gram", "sd_solve_gram", "sd_predict", "sd_test_residual", "sd_solver_timings", "sd_set_gram_mode", "sd_set_solver", "sd_solver_iterations",
     "sd_set_rank_diagnostic", "sd_last_rank",
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",
@@ -227,6 +249,10 @@ def lib():
                                              C.c_void_p]
         l.sd_hog_train_filter.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, _i, C.c_void_p, _i, _i, _i, _i, _i, _i, _i, _i,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        l.sd_hog_distance_transform.argtypes = [C.c_void_p, C.c_void_p, _i, C.c_void_p, _i, C.c_void_p, C.c_void_p]
+        l.sd_hog_part_scores.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _i, C.c_void_p, C.c_void_p]
+        l.sd_hog_part_placements.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, _i, C.c_void_p, C.c_void_p, _i, _i, C.c_void_p,
+                                             C.c_void_p, _i, _i, C.c_void_p]
         _lib = l
     return _lib
 

@@ -26,7 +26,7 @@ import torch
 
 from . import _capi
 from ._capi import HogParam as HoGParam  # same field names as rcr::HoGParam
-from ._capi import HogBoxC, HogDetectionC, HogGridC, HogGridsC, HogImageC, HogImagesC, HogPolarFieldsC, HogScoreMapC, HogTrainParamC, HogTrainReportC, HogWindowC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, SvmReportC, ptr
+from ._capi import HogBoxC, HogDetectionC, HogGridC, HogGridsC, HogImageC, HogImagesC, HogPartMapC, HogPartModelC, HogPartPlacementC, HogPolarFieldsC, HogScoreMapC, HogTrainParamC, HogTrainReportC, HogWindowC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, SvmReportC, ptr
 
 
 def _check(ctx, rc: int) -> None:
@@ -1817,3 +1817,248 @@ def train_hog_filter(frames, box_frame, boxes, scales, filter_size, cell_size: i
         d["gathered_bytes"] = float(r.gathered_bytes)
         report.append(d)
     return HogFilter(filt, float(bias.value), neg, report)
+
+
+# ------------------------------------------------------------------------------------------------
+# deformable part models: bounded distance transforms, star-model scores and part placements
+# ------------------------------------------------------------------------------------------------
+PART_MAX_DISPLACEMENT = 32   # SD_HOG_PART_MAX_DISPLACEMENT
+PART_MAX_PARTS = 32          # SD_HOG_PART_MAX_PARTS
+
+
+class HogPartModel:
+    """A star model of Q components for vl_hog_part_detect: root (Q, dd, fh, fw) filters with bias (Q,), parts (Q, P, dd, pfh, pfw)
+    filters scored at twice the root's resolution, anchors (Q, P, 2) int (ax, ay) in part-level cells relative to twice the root
+    window's top-left cell, deformation (Q, P, 4) (w0, w1, w2, w3): a displacement (dx, dy) costs w0 dx^2 + w1 dx + w2 dy^2 + w3 dy,
+    pad = (pad_x, pad_y) of the root correlate, part_pad of the part correlate, and max_displacement R bounding |dx| and |dy|."""
+
+    def __init__(self, root, bias, parts, anchors, deformation, pad=(0, 0), part_pad=(0, 0), max_displacement: int = 4):
+        self.root = _tensor(root).to(torch.float32).contiguous()
+        self.bias = _tensor(bias).to(torch.float32).reshape(-1).contiguous()
+        self.parts = _tensor(parts).to(torch.float32).contiguous()
+        self.anchors = np.ascontiguousarray(np.asarray(anchors, np.int64)).astype(np.int32)
+        self.deformation = np.ascontiguousarray(np.asarray(deformation, np.float32))
+        self.pad = tuple(int(v) for v in pad)
+        self.part_pad = tuple(int(v) for v in part_pad)
+        self.max_displacement = int(max_displacement)
+        if self.root.dim() != 4 or self.parts.dim() != 5:
+            raise ValueError("root must be (Q, dd, fh, fw) and parts (Q, P, dd, pfh, pfw)")
+        q, dd = self.root.shape[:2]
+        if self.parts.shape[0] != q or self.parts.shape[2] != dd:
+            raise ValueError("parts must be (Q, P, dd, pfh, pfw) with the root's Q and dd")
+        p = self.parts.shape[1]
+        if self.bias.shape != (q,) or self.anchors.shape != (q, p, 2) or self.deformation.shape != (q, p, 4):
+            raise ValueError(f"bias must be ({q},), anchors ({q}, {p}, 2) and deformation ({q}, {p}, 4)")
+
+    @property
+    def num_components(self) -> int:
+        return self.root.shape[0]
+
+    @property
+    def num_parts(self) -> int:
+        return self.parts.shape[1]
+
+    def flipped(self, num_bins: int, variant: int = 1, ctx: Optional[Context] = None) -> "HogPartModel":
+        """The model of the left-right mirrored image: vl_hog_flip of the root and every part, anchors ax' = 2 fw - ax - pfw, and
+        w1 negated (a displacement dx becomes -dx).  Pads and R are kept."""
+        q, p, dd, pfh, pfw = self.parts.shape
+        fw = self.root.shape[3]
+        root = vl_hog_flip(self.root, num_bins, variant, ctx=ctx)
+        parts = vl_hog_flip(self.parts.reshape(q * p, dd, pfh, pfw), num_bins, variant, ctx=ctx).reshape(q, p, dd, pfh, pfw)
+        anchors = self.anchors.copy()
+        anchors[..., 0] = 2 * fw - anchors[..., 0] - pfw
+        deformation = self.deformation.copy()
+        deformation[..., 1] = -deformation[..., 1]
+        return HogPartModel(root, self.bias.clone(), parts, anchors, deformation, self.pad, self.part_pad, self.max_displacement)
+
+    def _c(self, dev):
+        """(HogPartModelC, the device anchors it points to)."""
+        q, p, _, pfh, pfw = self.parts.shape
+        _, _, fh, fw = self.root.shape
+        anchors = torch.from_numpy(self.anchors).to(dev)
+        return HogPartModelC(q, p, fw, fh, pfw, pfh, self.pad[0], self.pad[1], self.part_pad[0], self.part_pad[1],
+                             anchors.data_ptr()), anchors
+
+
+def _deformation(deformation, planes: int):
+    d = np.ascontiguousarray(np.asarray(deformation, np.float32).reshape(-1))
+    if d.size != 4 * planes:
+        raise ValueError(f"deformation must hold 4 values per plane ({planes} planes)")
+    return d, C.c_void_p(d.ctypes.data)
+
+
+def vl_hog_distance_transform(maps, deformation, max_displacement: int, ctx: Optional[Context] = None):
+    """The bounded generalised distance transform of score maps on the device (sd_hog_distance_transform):
+        D(v, u) = max over |dx|, |dy| <= R of s(v + dy, u + dx) - (w0 dx^2 + w1 dx + w2 dy^2 + w3 dy),
+    separably in float32 with the tie rule of include/sd_b200.h, and where that maximum is, (u + dx, v + dy).  maps: a
+    (N, P, h, w) float32 tensor, or a list of (P, h, w) maps of any sizes; deformation: (P, 4), plane k's (w0, w1, w2, w3);
+    R = max_displacement in [0, 32].  Returns (values, placements) in the shapes of maps, placements with a trailing (u, v)
+    axis of int32 ((-1, -1) where the rule places nothing)."""
+    ctx = ctx or default_context()
+    dev = f"cuda:{ctx.device}"
+    single = not isinstance(maps, (list, tuple))
+    items = [_tensor(maps)] if single else [_tensor(m) for m in maps]
+    if any(t.dtype != torch.float32 or t.dim() != (4 if single else 3) for t in items):
+        raise ValueError("maps must be a float32 (N, P, h, w) tensor or a list of (P, h, w) tensors")
+    if not items or (single and items[0].shape[0] == 0):
+        return (items[0].clone(), torch.zeros(tuple(items[0].shape) + (2,), dtype=torch.int32, device=items[0].device)) if single else ([], [])
+    planes = items[0].shape[-3]
+    if any(t.shape[-3] != planes for t in items):
+        raise ValueError("every map must have the same number of planes")
+    d, d_ptr = _deformation(deformation, planes)
+    g = HogGridsC()
+    g.d_grids = None
+    if single:
+        keep = items[0].to(dev).contiguous()
+        n, _, h, w = keep.shape
+        g.d_features, g.count, g.width, g.height = keep.data_ptr(), n, w, h
+        values = torch.empty_like(keep)
+        place = torch.empty(tuple(keep.shape) + (2,), dtype=torch.int32, device=dev)
+        table = None
+    else:
+        keep, offs = _pack(items, dev)
+        values = torch.empty_like(keep)
+        place = torch.empty((keep.numel(), 2), dtype=torch.int32, device=dev)
+        table = _device_table([HogGridC(t.shape[2], t.shape[1], o, o) for t, o in zip(items, offs)], dev)
+        g.d_features, g.count, g.width, g.height, g.d_grids = keep.data_ptr(), len(items), 0, 0, table.data_ptr()
+    _check(ctx.h, _capi.lib().sd_hog_distance_transform(ctx.h, C.byref(g), int(planes), d_ptr, int(max_displacement), ptr(values),
+                                                        ptr(place)))
+    if single:
+        return values, place
+    return ([values[o:o + t.numel()].view(t.shape) for t, o in zip(items, offs)],
+            [place[o:o + t.numel()].view(tuple(t.shape) + (2,)) for t, o in zip(items, offs)])
+
+
+def vl_hog_part_scores(root_scores, part_values, model: HogPartModel, ctx: Optional[Context] = None):
+    """The star model's score maps (sd_hog_part_scores): for each root map (Q, oh, ow) of vl_hog_correlate with the model's root
+    filters, and its transformed part maps (Q * P, ph, pw) of vl_hog_distance_transform (or None: every anchor is outside),
+        total = root[q, y, x] + D[q P + p, v0, u0] for p = 0 .. P - 1 in order, in float32,
+    at u0 = 2 (x - pad_x) + ax + part_pad_x, v0 alike, and -inf where any anchor lies outside the part map.  Returns one
+    (Q, oh, ow) float32 CUDA tensor per root map."""
+    ctx = ctx or default_context()
+    dev = f"cuda:{ctx.device}"
+    roots = [_tensor(r) for r in root_scores]
+    parts = [None if v is None else _tensor(v) for v in part_values]
+    if len(roots) != len(parts):
+        raise ValueError("one part map (or None) per root map")
+    q, p = model.num_components, model.num_parts
+    if any(r.dtype != torch.float32 or r.dim() != 3 or r.shape[0] != q for r in roots):
+        raise ValueError(f"root maps must be float32 (Q, oh, ow) with Q = {q}")
+    if any(v is not None and (v.dtype != torch.float32 or v.dim() != 3 or v.shape[0] != q * p) for v in parts):
+        raise ValueError(f"part maps must be float32 (Q * P, ph, pw) with Q * P = {q * p}")
+    if not roots:
+        return []
+    keep_r, roff = _pack(roots, dev)
+    present = [v for v in parts if v is not None]
+    keep_p, poff = _pack(present, dev) if present else (torch.zeros(1, device=dev), [])
+    poff = iter(poff)
+    descs, out_shapes = [], []
+    for r, v in zip(roots, parts):
+        pw, ph, po = (v.shape[2], v.shape[1], next(poff)) if v is not None else (0, 0, 0)
+        descs.append((r.shape[2], r.shape[1], pw, ph, po))
+        out_shapes.append(tuple(r.shape))
+    out, ooff, res = _results(out_shapes, dev)
+    table = _device_table([HogPartMapC(0, k, 1, 1, 1, 1, w, h, pw, ph, ro, po, oo)
+                           for k, ((w, h, pw, ph, po), ro, oo) in enumerate(zip(descs, roff, ooff))], dev)
+    mc, anchors = model._c(dev)
+    _check(ctx.h, _capi.lib().sd_hog_part_scores(ctx.h, ptr(keep_r), ptr(keep_p), ptr(table), len(roots), C.byref(mc), ptr(out)))
+    return res
+
+
+HogPartDetections = collections.namedtuple("HogPartDetections", HogDetections._fields + ("parts", "placement", "part_scores"))
+HogPartDetections.__doc__ = """Detections of vl_hog_part_detect: the fields of HogDetections (filter is the component q), plus parts
+(n, P, 4) int32 part boxes (x, y, w, h in frame pixels, zero where a part has no placement), placement (n, P, 2) int32 (u, v) part
+score positions ((-1, -1) for none) and part_scores (n, P) float32, each part's transformed score D at its anchor."""
+
+
+def vl_hog_part_detect(frames, scales, model: HogPartModel, cell_size: int, num_bins: int, threshold: float, variant: int = 1,
+                       overlap: float = 0.5, max_candidates: int = 4096, max_detections: int = 256,
+                       ctx: Optional[Context] = None) -> HogPartDetections:
+    """A star-model detector over image pyramids: one vl_hog_pyramid over the root scales and their doubles (a scale present in
+    both is computed once; root scales must be <= 2), vl_hog_correlate of the root filters (bias included) on the root levels and
+    of all Q * P part filters on the part levels, each read in place; vl_hog_distance_transform of the part maps; the star
+    model's scores (vl_hog_part_scores); sd_hog_detections over them with the root's filter size and pad, all components as one
+    class; and the part placements of every detection (sd_hog_part_placements).  One host read-back at the end.  Returns
+    HogPartDetections; detect_faces(frames, d.frame, boxes=d.boxes) takes the result as it is."""
+    ctx = ctx or default_context()
+    dev = f"cuda:{ctx.device}"
+    q, p, dd, pfh, pfw = model.parts.shape
+    _, _, fh, fw = model.root.shape
+    if dd != _hog_dims(num_bins, variant):
+        raise ValueError(f"the model's dd ({dd}) is not that of num_bins {num_bins}, variant {variant}")
+    scales = [float(s) for s in scales]
+    if not scales or any(not 0 < s <= 2 for s in scales):
+        raise ValueError("vl_hog_part_detect needs root scales in (0, 2]")
+    every = list(dict.fromkeys(scales + [2 * s for s in scales]))
+    ri, pi = [every.index(s) for s in scales], [every.index(2 * s) for s in scales]
+    feats, levels = vl_hog_pyramid(frames, every, cell_size, num_bins, variant, ctx=ctx)
+    n = len(feats)
+    if n == 0:
+        z = np.zeros(0, np.int32)
+        return HogPartDetections(z, np.zeros((0, 4), np.int32), np.zeros(0, np.float32), z, z, np.zeros((0, 2), np.int32),
+                                 np.zeros(0, np.int64), np.zeros((0, p, 4), np.int32), np.zeros((0, p, 2), np.int32),
+                                 np.zeros((0, p), np.float32))
+    if isinstance(frames, (list, tuple)):
+        sizes = [(int(fr.shape[1]), int(fr.shape[0])) for fr in frames]
+    else:
+        sizes = [(int(frames.shape[2]), int(frames.shape[1]))] * n
+    which = [(i, s) for i in range(n) for s in range(len(scales)) if feats[i][ri[s]] is not None]
+    roots = vl_hog_correlate([feats[i][ri[s]] for i, s in which], model.root, num_bins, variant, bias=model.bias, pad=model.pad,
+                             ctx=ctx) if which else []
+    kept = [(i, s, r) for (i, s), r in zip(which, roots) if r.numel()]
+    # every part level of a kept root map, once
+    plevels = list(dict.fromkeys((i, pi[s]) for i, s, _ in kept if feats[i][pi[s]] is not None))
+    pscores = vl_hog_correlate([feats[i][l] for i, l in plevels], model.parts.reshape(q * p, dd, pfh, pfw), num_bins, variant,
+                               pad=model.part_pad, ctx=ctx) if plevels else []
+    pmap = {key: sc for key, sc in zip(plevels, pscores) if sc.numel()}
+    d, d_ptr = _deformation(model.deformation, q * p)
+    R = int(model.max_displacement)
+    lib = _capi.lib()
+    if pmap:
+        stor = next(iter(pmap.values())).untyped_storage()
+        raw = torch.empty(0, dtype=torch.float32, device=dev).set_(stor)
+        values = torch.empty_like(raw)
+        g = HogGridsC()
+        gt = _device_table([HogGridC(sc.shape[2], sc.shape[1], sc.storage_offset(), sc.storage_offset()) for sc in pmap.values()], dev)
+        g.d_features, g.count, g.width, g.height, g.d_grids = raw.data_ptr(), len(pmap), 0, 0, gt.data_ptr()
+        _check(ctx.h, lib.sd_hog_distance_transform(ctx.h, C.byref(g), q * p, d_ptr, R, ptr(values), None))
+    else:
+        raw = values = torch.zeros(1, dtype=torch.float32, device=dev)
+    mc, anchors = model._c(dev)
+    md = int(max_detections)
+    out = torch.empty((n, max(md, 1), len(HogDetectionC._fields_)), dtype=torch.int32, device=dev)
+    count = torch.empty(n, dtype=torch.int32, device=dev)
+    above = torch.empty(n, dtype=torch.int64, device=dev)
+    place = torch.empty((n, max(md, 1), p, len(HogPartPlacementC._fields_)), dtype=torch.int32, device=dev)
+    table = score_table = total = None
+    if kept:
+        rbase = kept[0][2].untyped_storage()
+        total = torch.empty(rbase.nbytes() // 4, dtype=torch.float32, device=dev)
+        descs, sdescs = [], []
+        for i, s, r in kept:
+            sc = pmap.get((i, pi[s]))
+            plw, plh = levels[i][pi[s]]
+            pw, ph, po = (sc.shape[2], sc.shape[1], sc.storage_offset()) if sc is not None else (0, 0, 0)
+            off = r.storage_offset()
+            descs.append(HogPartMapC(i, s, sizes[i][0], sizes[i][1], plw, plh, r.shape[2], r.shape[1], pw, ph, off, po, off))
+            sdescs.append(HogScoreMapC(i, s, sizes[i][0], sizes[i][1], levels[i][ri[s]][0], levels[i][ri[s]][1], r.shape[2], r.shape[1],
+                                       off))
+        table = _device_table(descs, dev)
+        score_table = _device_table(sdescs, dev)
+        _check(ctx.h, lib.sd_hog_part_scores(ctx.h, ptr(kept[0][2].untyped_storage().data_ptr()), ptr(values), ptr(table), len(kept),
+                                             C.byref(mc), ptr(total)))
+    _check(ctx.h, lib.sd_hog_detections(ctx.h, ptr(total), ptr(score_table), len(kept), n, int(q), int(cell_size), int(fw), int(fh),
+                                        model.pad[0], model.pad[1], float(threshold), float(overlap), int(max_candidates), md,
+                                        ptr(out), ptr(count), ptr(above)))
+    _check(ctx.h, lib.sd_hog_part_placements(ctx.h, ptr(raw), ptr(table), len(kept), C.byref(mc), d_ptr, R, int(cell_size), ptr(out),
+                                             ptr(count), n, md, ptr(place)))
+    counts = count.cpu().numpy().astype(np.int64)
+    rows = out.cpu().numpy()
+    pl = place.cpu().numpy()
+    r = np.concatenate([rows[i, :c] for i, c in enumerate(counts)] + [np.zeros((0, rows.shape[2]), np.int32)])
+    pr = np.concatenate([pl[i, :c] for i, c in enumerate(counts)] + [np.zeros((0, p, pl.shape[3]), np.int32)])
+    return HogPartDetections(np.repeat(np.arange(n, dtype=np.int32), counts), np.ascontiguousarray(r[:, 0:4]),
+                             np.ascontiguousarray(r[:, 4]).view(np.float32), np.ascontiguousarray(r[:, 5]),
+                             np.ascontiguousarray(r[:, 6]), np.ascontiguousarray(r[:, 7:9]), above.cpu().numpy().copy(),
+                             np.ascontiguousarray(pr[:, :, 3:7]), np.ascontiguousarray(pr[:, :, 0:2]),
+                             np.ascontiguousarray(pr[:, :, 2]).view(np.float32))

@@ -1,0 +1,530 @@
+// Deformable part models over HOG pyramids (sd_hog_distance_transform, sd_hog_part_scores, sd_hog_part_placements): the bounded
+// generalised distance transform of part score maps, the star model's score maps, and the part boxes of each detection.
+//
+//   dt_tile_kernel        one CTA per 32 x 32 output tile of one plane: the tile's rows with R rows of halo above and below and
+//                         R columns either side are staged in shared memory, pass X runs over every staged row (32 columns),
+//                         pass Y over the tile.  Both passes take candidates in ascending displacement through dt_take.
+//   part_scores_kernel    one thread per root score: the root score plus each part's transformed score at its anchor.
+//   part_place_kernel     one warp per (detection, part): the rule of dt_tile_kernel at the one anchor, through dt_take again,
+//                         so that the placement is bit for bit the transform's.
+//
+// Every kernel walks a flat list of work items with a grid-stride loop over blockIdx.x; no count is bound by gridDim.y / z.
+// There are no atomics: each output element is written by one thread.
+//
+// Scratch (SD_WS_PARTS): the cost tables, the per-map first tiles of a table route, and the placements' per-detection map index.
+#include "sd_internal.cuh"
+
+#include <algorithm>
+#include <climits>
+#include <cmath>
+#include <cstring>
+#include <map>
+#include <vector>
+
+namespace {
+
+constexpr int kT = 32;                 // output tile side of the transform
+constexpr int kThreads = 256;
+constexpr int kNone = INT_MIN;         // "no candidate chosen"
+constexpr int kScoreTile = kThreads * 4;
+constexpr int kPlaceWarps = 4;
+
+// The rule's update, shared by every kernel: a non-NaN candidate replaces the current best when there is none yet or when it
+// is strictly greater.  Called in ascending displacement order, the choice is the smallest displacement that reaches the max.
+__device__ __forceinline__ void dt_take(float cand, int k, float& best, int& arg)
+{
+    if (!isnan(cand) && (arg == kNone || cand > best)) {
+        best = cand;
+        arg = k;
+    }
+}
+
+__device__ __forceinline__ int find_last_le(const long long* first, int n, long long t)
+{
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (__ldg(first + mid) <= t) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// ---- the transform ----------------------------------------------------------------------------------------------------------
+
+struct DtArgs {
+    const float* in;
+    float* out;
+    int2* place;                  // may be null
+    const sd_hog_grid* grids;     // null: equally sized maps
+    int width, height;            // equally sized maps
+    int num_maps, P, R;
+    const float* costs;           // [P][2][2R + 1]: cx then cy
+    const long long* tile0;       // table route: each map's first tile
+    long long total_tiles;
+};
+
+__global__ void __launch_bounds__(kThreads) dt_tile_kernel(const __grid_constant__ DtArgs a)
+{
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int R = a.R, span = kT + 2 * R, taps = 2 * R + 1;
+    float* s_in = reinterpret_cast<float*>(smem);                 // [span][span]
+    float* s_t = s_in + span * span;                              // [span][kT]
+    float* s_c = s_t + span * kT;                                 // [2][taps]
+    signed char* s_dx = reinterpret_cast<signed char*>(s_c + 2 * taps);   // [span][kT]; -128: none
+    const int tid = threadIdx.x;
+
+    for (long long t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
+        int m, w, h;
+        long long base, obase, local;
+        if (a.grids) {
+            m = find_last_le(a.tile0, a.num_maps, t);
+            const sd_hog_grid g = a.grids[m];
+            w = g.width; h = g.height; base = g.offset; obase = g.out_offset;
+            local = t - __ldg(a.tile0 + m);
+        } else {
+            w = a.width; h = a.height;
+            const long long per = (long long)a.P * ((w + kT - 1) / kT) * ((h + kT - 1) / kT);
+            m = (int)(t / per);
+            local = t - (long long)m * per;
+            base = obase = (long long)m * a.P * w * h;
+        }
+        const int tx = (w + kT - 1) / kT, ty = (h + kT - 1) / kT;
+        const int k = (int)(local / ((long long)tx * ty));
+        const int r = (int)(local - (long long)k * tx * ty);
+        const int x0 = (r % tx) * kT, y0 = (r / tx) * kT;
+        const long long plane = (long long)k * w * h;
+        const float* in = a.in + base + plane;
+
+        __syncthreads();                                          // the previous tile is done with shared memory
+        for (int i = tid; i < 2 * taps; i += kThreads) s_c[i] = __ldg(a.costs + (size_t)k * 2 * taps + i);
+        const int ylo = max(0, y0 - R), yhi = min(h, y0 + kT + R);
+        const int xlo = max(0, x0 - R), xhi = min(w, x0 + kT + R);
+        const int cols = xhi - xlo;
+        for (int i = tid; i < (yhi - ylo) * cols; i += kThreads) {
+            const int y = ylo + i / cols, x = xlo + i % cols;
+            s_in[(y - y0 + R) * span + (x - x0 + R)] = __ldg(in + (long long)y * w + x);
+        }
+        __syncthreads();
+
+        // pass X over every staged row, the tile's columns
+        const int xe = min(kT, w - x0);
+        for (int i = tid; i < (yhi - ylo) * kT; i += kThreads) {
+            const int c = i & (kT - 1), y = ylo + i / kT;
+            if (c >= xe) continue;
+            const int u = x0 + c;
+            const float* row = s_in + (y - y0 + R) * span + (c + R);
+            float best = -INFINITY;
+            int arg = kNone;
+            for (int d = -R; d <= R; ++d)
+                if (u + d >= 0 && u + d < w) dt_take(__fsub_rn(row[d], s_c[d + R]), d, best, arg);
+            s_t[(y - y0 + R) * kT + c] = best;
+            s_dx[(y - y0 + R) * kT + c] = arg == kNone ? (signed char)-128 : (signed char)arg;
+        }
+        __syncthreads();
+
+        // pass Y over the tile
+        const int ye = min(kT, h - y0);
+        for (int i = tid; i < ye * kT; i += kThreads) {
+            const int c = i & (kT - 1), rr = i / kT;
+            if (c >= xe) continue;
+            const int u = x0 + c, v = y0 + rr;
+            float best = -INFINITY;
+            int arg = kNone;
+            for (int e = -R; e <= R; ++e)
+                if (v + e >= 0 && v + e < h) dt_take(__fsub_rn(s_t[(rr + e + R) * kT + c], s_c[taps + e + R]), e, best, arg);
+            const long long o = obase + plane + (long long)v * w + u;
+            a.out[o] = best;
+            if (a.place) {
+                int2 p = make_int2(-1, -1);
+                if (arg != kNone) {
+                    const int dx = s_dx[(rr + arg + R) * kT + c];
+                    if (dx != -128) p = make_int2(u + dx, v + arg);
+                }
+                a.place[o] = p;
+            }
+        }
+    }
+}
+
+// ---- the star model's scores --------------------------------------------------------------------------------------------------
+
+struct ScoreArgs {
+    const float* root;
+    const float* parts;
+    float* out;
+    const sd_hog_part_map* maps;
+    const int32_t* anchors;       // [Q][P][2]
+    const long long* tile0;
+    int num_maps, Q, P, pad_x, pad_y, part_pad_x, part_pad_y;
+    long long total_tiles;
+};
+
+__global__ void __launch_bounds__(kThreads) part_scores_kernel(const __grid_constant__ ScoreArgs a)
+{
+    for (long long t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
+        const int m = find_last_le(a.tile0, a.num_maps, t);
+        const sd_hog_part_map d = a.maps[m];
+        const long long plane = (long long)d.width * d.height, n = a.Q * plane;
+        const long long e0 = (t - __ldg(a.tile0 + m)) * kScoreTile, e1 = min(e0 + kScoreTile, n);
+        const long long pplane = (long long)d.part_width * d.part_height;
+        for (long long e = e0 + threadIdx.x; e < e1; e += kThreads) {
+            const int q = (int)(e / plane);
+            const long long rem = e - q * plane;
+            const int y = (int)(rem / d.width), x = (int)(rem - (long long)y * d.width);
+            float total = __ldg(a.root + d.root_offset + e);
+            bool outside = false;
+            for (int p = 0; p < a.P; ++p) {
+                const int2 an = __ldg(reinterpret_cast<const int2*>(a.anchors) + q * a.P + p);
+                const long long u0 = 2LL * (x - a.pad_x) + an.x + a.part_pad_x, v0 = 2LL * (y - a.pad_y) + an.y + a.part_pad_y;
+                if (u0 < 0 || u0 >= d.part_width || v0 < 0 || v0 >= d.part_height) {
+                    outside = true;
+                    continue;
+                }
+                total = __fadd_rn(total, __ldg(a.parts + d.part_offset + (long long)(q * a.P + p) * pplane + v0 * d.part_width + u0));
+            }
+            a.out[d.out_offset + e] = outside ? -INFINITY : total;
+        }
+    }
+}
+
+// ---- the part placements of detections ---------------------------------------------------------------------------------------
+
+struct PlaceArgs {
+    const float* parts;           // the part score maps (before the transform)
+    const sd_hog_part_map* maps;
+    const int32_t* anchors;
+    const float* costs;           // [Q * P][2][2R + 1]
+    const sd_hog_detection* det;
+    const int32_t* count;
+    const int32_t* slot_map;      // num_frames x max_det: the table entry of each detection
+    sd_hog_part_placement* out;
+    int num_frames, max_det, P, R, cell, pfw, pfh, pad_x, pad_y, part_pad_x, part_pad_y;
+};
+
+__host__ __device__ __forceinline__ long long round_half_up(long long n, long long d)
+{
+    const long long num = 2 * n + d, den = 2 * d;
+    long long q = num / den;
+    if (num % den != 0 && num < 0) --q;
+    return q;
+}
+
+__global__ void __launch_bounds__(kPlaceWarps * 32) part_place_kernel(const __grid_constant__ PlaceArgs a)
+{
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int taps = 2 * a.R + 1, lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    float* s_t = reinterpret_cast<float*>(smem) + wid * 2 * taps;  // [taps] row values, then [taps] their dx
+    int* s_dx = reinterpret_cast<int*>(s_t + taps);
+    const long long items = (long long)a.num_frames * a.max_det * a.P;
+    for (long long it = (long long)blockIdx.x * kPlaceWarps + wid; it < items; it += (long long)gridDim.x * kPlaceWarps) {
+        const long long slot = it / a.P;
+        const int p = (int)(it - slot * a.P);
+        const int f = (int)(slot / a.max_det), k = (int)(slot - (long long)f * a.max_det);
+        if (k >= __ldg(a.count + f)) continue;                    // uniform over the warp
+        const sd_hog_detection det = a.det[slot];
+        const sd_hog_part_map d = a.maps[__ldg(a.slot_map + slot)];
+        const int q = det.filter, kp = q * a.P + p;
+        const int2 an = __ldg(reinterpret_cast<const int2*>(a.anchors) + kp);
+        const long long u0 = 2LL * (det.cell_x - a.pad_x) + an.x + a.part_pad_x, v0 = 2LL * (det.cell_y - a.pad_y) + an.y + a.part_pad_y;
+        sd_hog_part_placement r;
+        r.u = r.v = -1;
+        r.term = -INFINITY;
+        r.x = r.y = r.w = r.h = 0;
+        if (u0 >= 0 && u0 < d.part_width && v0 >= 0 && v0 < d.part_height) {
+            const int w = d.part_width, h = d.part_height, u = (int)u0, v = (int)v0;
+            const float* plane = a.parts + d.part_offset + (long long)kp * w * h;
+            const float* cx = a.costs + (size_t)kp * 2 * taps;
+            const float* cy = cx + taps;
+            // pass X at column u of each row v + e that the rule reads
+            for (int i = lane; i < taps; i += 32) {
+                const int y = v + i - a.R;
+                if (y < 0 || y >= h) continue;
+                const float* row = plane + (long long)y * w + u;
+                float best = -INFINITY;
+                int arg = kNone;
+                for (int dd = -a.R; dd <= a.R; ++dd)
+                    if (u + dd >= 0 && u + dd < w) dt_take(__fsub_rn(__ldg(row + dd), __ldg(cx + dd + a.R)), dd, best, arg);
+                s_t[i] = best;
+                s_dx[i] = arg;
+            }
+            __syncwarp();
+            if (lane == 0) {
+                float best = -INFINITY;
+                int arg = kNone;
+                for (int e = -a.R; e <= a.R; ++e)
+                    if (v + e >= 0 && v + e < h) dt_take(__fsub_rn(s_t[e + a.R], __ldg(cy + e + a.R)), e, best, arg);
+                r.term = best;
+                if (arg != kNone && s_dx[arg + a.R] != kNone) {
+                    r.u = u + s_dx[arg + a.R];
+                    r.v = v + arg;
+                    const long long sx = (long long)a.cell * d.frame_w, sy = (long long)a.cell * d.frame_h;
+                    const long long bx0 = round_half_up((long long)(r.u - a.part_pad_x) * sx, d.part_level_w);
+                    const long long bx1 = round_half_up((long long)(r.u - a.part_pad_x + a.pfw) * sx, d.part_level_w);
+                    const long long by0 = round_half_up((long long)(r.v - a.part_pad_y) * sy, d.part_level_h);
+                    const long long by1 = round_half_up((long long)(r.v - a.part_pad_y + a.pfh) * sy, d.part_level_h);
+                    r.x = (int)bx0; r.y = (int)by0; r.w = (int)(bx1 - bx0); r.h = (int)(by1 - by0);
+                }
+            }
+            __syncwarp();
+        }
+        if (lane == 0) a.out[it] = r;
+    }
+}
+
+bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+// cost tables of num_planes deformations: cx[d] = (float)((double)w0 d^2 + (double)w1 d), cy alike with w2, w3
+bool cost_tables(const float* h_def, int num_planes, int R, std::vector<float>& costs)
+{
+    const int taps = 2 * R + 1;
+    costs.resize((size_t)num_planes * 2 * taps);
+    for (int k = 0; k < num_planes; ++k)
+        for (int axis = 0; axis < 2; ++axis)
+            for (int d = -R; d <= R; ++d) {
+                const double c = (double)h_def[4 * k + 2 * axis] * d * d + (double)h_def[4 * k + 2 * axis + 1] * d;
+                const float f = (float)c;
+                if (!std::isfinite(f)) return false;
+                costs[((size_t)k * 2 + axis) * taps + d + R] = f;
+            }
+    return true;
+}
+
+int check_model(sd_ctx* ctx, const sd_hog_part_model* m)
+{
+    SD_REQUIRE(ctx, m && m->d_anchors && aligned(m->d_anchors, 8), "null model or anchors not 8-byte aligned");
+    SD_REQUIRE(ctx, m->num_parts >= 1 && m->num_parts <= SD_HOG_PART_MAX_PARTS, "num_parts must be in [1, SD_HOG_PART_MAX_PARTS]");
+    SD_REQUIRE(ctx, m->num_components >= 1 && (long long)m->num_components * m->num_parts <= SD_HOG_FILTER_MAX_BANK,
+               "num_components must be >= 1 with num_components * num_parts <= SD_HOG_FILTER_MAX_BANK");
+    SD_REQUIRE(ctx, m->filter_w >= 1 && m->filter_w <= SD_HOG_FILTER_MAX_SIDE && m->filter_h >= 1 && m->filter_h <= SD_HOG_FILTER_MAX_SIDE &&
+                        m->part_w >= 1 && m->part_w <= SD_HOG_FILTER_MAX_SIDE && m->part_h >= 1 && m->part_h <= SD_HOG_FILTER_MAX_SIDE,
+               "filter and part sides must be in [1, SD_HOG_FILTER_MAX_SIDE]");
+    SD_REQUIRE(ctx, m->pad_x >= 0 && m->pad_x < m->filter_w && m->pad_y >= 0 && m->pad_y < m->filter_h && m->part_pad_x >= 0 &&
+                        m->part_pad_x < m->part_w && m->part_pad_y >= 0 && m->part_pad_y < m->part_h,
+               "pads must be in [0, side - 1]");
+    return SD_OK;
+}
+
+// the score tiles of each map of a part table (first tile per map) and the check every call makes of the table's sizes
+int part_tiles(sd_ctx* ctx, const std::vector<sd_hog_part_map>& table, int Q, std::vector<long long>& tile0, long long* total)
+{
+    tile0.resize(table.size());
+    long long tiles = 0;
+    for (size_t i = 0; i < table.size(); ++i) {
+        const sd_hog_part_map& d = table[i];
+        SD_REQUIRE(ctx, d.width >= 0 && d.height >= 0 && d.part_width >= 0 && d.part_height >= 0, "a map's size is negative");
+        SD_REQUIRE(ctx, d.root_offset >= 0 && d.part_offset >= 0 && d.out_offset >= 0, "a map's offset is negative");
+        tile0[i] = tiles;
+        tiles += ((long long)Q * d.width * d.height + kScoreTile - 1) / kScoreTile;
+    }
+    *total = tiles;
+    return SD_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sd_hog_distance_transform(sd_ctx* ctx, const sd_hog_grids* maps, int num_planes, const float* h_deformation, int max_displacement,
+                              float* d_values, int32_t* d_place)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, maps && h_deformation && d_values, "null argument");
+    SD_REQUIRE(ctx, maps->count >= 0, "negative map count");
+    SD_REQUIRE(ctx, maps->count == 0 || (maps->d_features && aligned(maps->d_features, 4)), "maps must be non-null and 4-byte aligned");
+    SD_REQUIRE(ctx, aligned(d_values, 4) && aligned(d_place, 8), "values must be 4-byte aligned and placements 8-byte aligned");
+    SD_REQUIRE(ctx, num_planes >= 1 && num_planes <= SD_HOG_FILTER_MAX_BANK, "num_planes must be in [1, SD_HOG_FILTER_MAX_BANK]");
+    SD_REQUIRE(ctx, max_displacement >= 0 && max_displacement <= SD_HOG_PART_MAX_DISPLACEMENT,
+               "max_displacement must be in [0, SD_HOG_PART_MAX_DISPLACEMENT]");
+    const int R = max_displacement, taps = 2 * R + 1;
+    std::vector<float> costs;
+    SD_REQUIRE(ctx, cost_tables(h_deformation, num_planes, R, costs), "a cost table entry is not finite");
+    if (maps->count == 0) return SD_OK;
+    int max_w = 0, max_h = 0;
+    std::vector<sd_hog_grid> table;
+    if (const int rc = sd_read_hog_grids(ctx, __func__, maps, &max_w, &max_h, maps->d_grids ? &table : nullptr)) return rc;
+    std::vector<long long> tile0;
+    long long tiles = 0;
+    if (maps->d_grids) {
+        tile0.resize(table.size());
+        for (size_t i = 0; i < table.size(); ++i) {
+            tile0[i] = tiles;
+            tiles += (long long)num_planes * sd_div_up(table[i].width, kT) * sd_div_up(table[i].height, kT);
+        }
+    } else {
+        tiles = (long long)maps->count * num_planes * sd_div_up(maps->width, kT) * sd_div_up(maps->height, kT);
+    }
+
+    const size_t cost_bytes = sd_round16(sizeof(float) * costs.size());
+    unsigned char* ws = static_cast<unsigned char*>(sd_workspace(ctx, SD_WS_PARTS, cost_bytes + sizeof(long long) * tile0.size()));
+    if (!ws) return SD_ERR_CUDA;
+    DtArgs a;
+    memset(&a, 0, sizeof(a));
+    a.in = maps->d_features;
+    a.out = d_values;
+    a.place = reinterpret_cast<int2*>(d_place);
+    a.grids = maps->d_grids;
+    a.width = maps->width;
+    a.height = maps->height;
+    a.num_maps = maps->count;
+    a.P = num_planes;
+    a.R = R;
+    a.costs = reinterpret_cast<const float*>(ws);
+    a.tile0 = reinterpret_cast<const long long*>(ws + cost_bytes);
+    a.total_tiles = tiles;
+    SD_CUDA(ctx, cudaMemcpyAsync(ws, costs.data(), sizeof(float) * costs.size(), cudaMemcpyHostToDevice, ctx->stream));
+    if (!tile0.empty())
+        SD_CUDA(ctx, cudaMemcpyAsync(ws + cost_bytes, tile0.data(), sizeof(long long) * tile0.size(), cudaMemcpyHostToDevice, ctx->stream));
+    const int span = kT + 2 * R;
+    const int smem = (span * span + span * kT + 2 * taps) * (int)sizeof(float) + span * kT;
+    SD_CUDA(ctx, cudaFuncSetAttribute(dt_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    const int grid = (int)std::min<long long>(tiles, 16LL * ctx->sm_count);
+    dt_tile_kernel<<<grid, kThreads, smem, ctx->stream>>>(a);
+    SD_LAUNCH_CHECK(ctx, "dt_tile_kernel");
+    return SD_OK;
+}
+
+int sd_hog_part_scores(sd_ctx* ctx, const float* d_root, const float* d_parts, const sd_hog_part_map* d_maps, int num_maps,
+                       const sd_hog_part_model* model, float* d_out)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    if (const int rc = check_model(ctx, model)) return rc;
+    SD_REQUIRE(ctx, num_maps >= 0, "negative map count");
+    SD_REQUIRE(ctx, num_maps == 0 || (d_root && d_parts && d_maps && d_out), "null argument");
+    SD_REQUIRE(ctx, aligned(d_root, 4) && aligned(d_parts, 4) && aligned(d_out, 4) && aligned(d_maps, 8),
+               "scores must be 4-byte aligned and the map table 8-byte aligned");
+    if (num_maps == 0) return SD_OK;
+    std::vector<sd_hog_part_map> table;
+    if (const int rc = sd_fetch_table(ctx, d_maps, num_maps, table)) return rc;
+    std::vector<long long> tile0;
+    long long tiles = 0;
+    if (const int rc = part_tiles(ctx, table, model->num_components, tile0, &tiles)) return rc;
+    if (tiles == 0) return SD_OK;
+    long long* ws = static_cast<long long*>(sd_workspace(ctx, SD_WS_PARTS, sizeof(long long) * tile0.size()));
+    if (!ws) return SD_ERR_CUDA;
+    SD_CUDA(ctx, cudaMemcpyAsync(ws, tile0.data(), sizeof(long long) * tile0.size(), cudaMemcpyHostToDevice, ctx->stream));
+    ScoreArgs a;
+    memset(&a, 0, sizeof(a));
+    a.root = d_root;
+    a.parts = d_parts;
+    a.out = d_out;
+    a.maps = d_maps;
+    a.anchors = model->d_anchors;
+    a.tile0 = ws;
+    a.num_maps = num_maps;
+    a.Q = model->num_components;
+    a.P = model->num_parts;
+    a.pad_x = model->pad_x; a.pad_y = model->pad_y;
+    a.part_pad_x = model->part_pad_x; a.part_pad_y = model->part_pad_y;
+    a.total_tiles = tiles;
+    const int grid = (int)std::min<long long>(tiles, 16LL * ctx->sm_count);
+    part_scores_kernel<<<grid, kThreads, 0, ctx->stream>>>(a);
+    SD_LAUNCH_CHECK(ctx, "part_scores_kernel");
+    return SD_OK;
+}
+
+int sd_hog_part_placements(sd_ctx* ctx, const float* d_parts, const sd_hog_part_map* d_maps, int num_maps, const sd_hog_part_model* model,
+                           const float* h_deformation, int max_displacement, int cell_size, const sd_hog_detection* d_det,
+                           const int32_t* d_count, int num_frames, int max_detections, sd_hog_part_placement* d_out)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    if (const int rc = check_model(ctx, model)) return rc;
+    SD_REQUIRE(ctx, h_deformation && d_det && d_count && d_out && (num_maps == 0 || (d_parts && d_maps)), "null argument");
+    SD_REQUIRE(ctx, aligned(d_parts, 4) && aligned(d_maps, 8) && aligned(d_det, 4) && aligned(d_count, 4) && aligned(d_out, 4),
+               "scores, detections, counts and output must be 4-byte aligned, the map table 8-byte aligned");
+    SD_REQUIRE(ctx, num_maps >= 0, "negative map count");
+    SD_REQUIRE(ctx, num_frames >= 1, "num_frames must be >= 1");
+    SD_REQUIRE(ctx, max_detections >= 1 && max_detections <= SD_HOG_DETECT_MAX_CANDIDATES,
+               "max_detections must be in [1, SD_HOG_DETECT_MAX_CANDIDATES]");
+    SD_REQUIRE(ctx, cell_size >= 1 && cell_size <= kDenseMaxCell, "cell_size must be in [1,32]");
+    SD_REQUIRE(ctx, max_displacement >= 0 && max_displacement <= SD_HOG_PART_MAX_DISPLACEMENT,
+               "max_displacement must be in [0, SD_HOG_PART_MAX_DISPLACEMENT]");
+    const int Q = model->num_components, P = model->num_parts, R = max_displacement;
+    std::vector<float> costs;
+    SD_REQUIRE(ctx, cost_tables(h_deformation, Q * P, R, costs), "a cost table entry is not finite");
+
+    std::vector<sd_hog_part_map> table;
+    if (num_maps > 0)
+        if (const int rc = sd_fetch_table(ctx, d_maps, num_maps, table)) return rc;
+    std::vector<long long> tile0;
+    long long tiles = 0;
+    if (const int rc = part_tiles(ctx, table, Q, tile0, &tiles)) return rc;
+    std::map<std::pair<int, int>, int> index;
+    const __int128 limit = (__int128)1 << 62;
+    for (int i = 0; i < num_maps; ++i) {
+        const sd_hog_part_map& d = table[i];
+        SD_REQUIRE(ctx, d.frame >= 0 && d.frame < num_frames, "a map's frame is out of range");
+        SD_REQUIRE(ctx, d.frame_w >= 1 && d.frame_h >= 1 && d.part_level_w >= 1 && d.part_level_h >= 1,
+                   "a map's frame or part level is smaller than 1 x 1");
+        SD_REQUIRE(ctx, index.emplace(std::make_pair(d.frame, d.level), i).second, "two maps share one (frame, level)");
+        if (d.part_width > 0 && d.part_height > 0) {   // the part boxes of the extreme positions fit in int32
+            const __int128 sx = (__int128)cell_size * d.frame_w, sy = (__int128)cell_size * d.frame_h;
+            const __int128 nx[2] = {(__int128)(-model->part_pad_x) * sx, (__int128)(d.part_width - 1 - model->part_pad_x + model->part_w) * sx};
+            const __int128 ny[2] = {(__int128)(-model->part_pad_y) * sy, (__int128)(d.part_height - 1 - model->part_pad_y + model->part_h) * sy};
+            bool ok = true;
+            for (int k = 0; k < 2; ++k) {
+                ok = ok && nx[k] < limit && nx[k] > -limit && ny[k] < limit && ny[k] > -limit;
+                if (ok) {
+                    const long long bx = round_half_up((long long)nx[k], d.part_level_w), by = round_half_up((long long)ny[k], d.part_level_h);
+                    ok = bx >= INT_MIN && bx <= INT_MAX && by >= INT_MIN && by <= INT_MAX;
+                }
+            }
+            SD_REQUIRE(ctx, ok, "a map's part boxes do not fit in int32");
+        }
+    }
+    // the detections, read back once: each must come from a map of the table
+    const size_t slots = (size_t)num_frames * max_detections;
+    std::vector<int32_t> count(num_frames);
+    std::vector<sd_hog_detection> det(slots);
+    SD_CUDA(ctx, cudaMemcpyAsync(count.data(), d_count, sizeof(int32_t) * num_frames, cudaMemcpyDeviceToHost, ctx->stream));
+    SD_CUDA(ctx, cudaMemcpyAsync(det.data(), d_det, sizeof(sd_hog_detection) * slots, cudaMemcpyDeviceToHost, ctx->stream));
+    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    std::vector<int32_t> slot_map(slots, 0);
+    long long work = 0;
+    for (int f = 0; f < num_frames; ++f) {
+        SD_REQUIRE(ctx, count[f] >= 0 && count[f] <= max_detections, "a frame's detection count is outside [0, max_detections]");
+        for (int k = 0; k < count[f]; ++k) {
+            const sd_hog_detection& r = det[(size_t)f * max_detections + k];
+            const auto it = index.find(std::make_pair(f, (int)r.level));
+            SD_REQUIRE(ctx, it != index.end(), "a detection's (frame, level) is not in the table");
+            const sd_hog_part_map& d = table[it->second];
+            SD_REQUIRE(ctx, r.filter >= 0 && r.filter < Q && r.cell_x >= 0 && r.cell_x < d.width && r.cell_y >= 0 && r.cell_y < d.height,
+                       "a detection's filter or score position is not one of its map");
+            slot_map[(size_t)f * max_detections + k] = it->second;
+            ++work;
+        }
+    }
+    if (work == 0) return SD_OK;
+
+    const size_t cost_bytes = sd_round16(sizeof(float) * costs.size());
+    unsigned char* ws = static_cast<unsigned char*>(sd_workspace(ctx, SD_WS_PARTS, cost_bytes + sizeof(int32_t) * slots));
+    if (!ws) return SD_ERR_CUDA;
+    SD_CUDA(ctx, cudaMemcpyAsync(ws, costs.data(), sizeof(float) * costs.size(), cudaMemcpyHostToDevice, ctx->stream));
+    SD_CUDA(ctx, cudaMemcpyAsync(ws + cost_bytes, slot_map.data(), sizeof(int32_t) * slots, cudaMemcpyHostToDevice, ctx->stream));
+    PlaceArgs a;
+    memset(&a, 0, sizeof(a));
+    a.parts = d_parts;
+    a.maps = d_maps;
+    a.anchors = model->d_anchors;
+    a.costs = reinterpret_cast<const float*>(ws);
+    a.det = d_det;
+    a.count = d_count;
+    a.slot_map = reinterpret_cast<const int32_t*>(ws + cost_bytes);
+    a.out = d_out;
+    a.num_frames = num_frames;
+    a.max_det = max_detections;
+    a.P = P;
+    a.R = R;
+    a.cell = cell_size;
+    a.pfw = model->part_w; a.pfh = model->part_h;
+    a.pad_x = model->pad_x; a.pad_y = model->pad_y;
+    a.part_pad_x = model->part_pad_x; a.part_pad_y = model->part_pad_y;
+    const long long items = (long long)slots * P;
+    const int grid = (int)std::min<long long>((items + kPlaceWarps - 1) / kPlaceWarps, 16LL * ctx->sm_count);
+    const int smem = kPlaceWarps * 2 * (2 * R + 1) * (int)sizeof(float);
+    part_place_kernel<<<grid, kPlaceWarps * 32, smem, ctx->stream>>>(a);
+    SD_LAUNCH_CHECK(ctx, "part_place_kernel");
+    return SD_OK;
+}
+
+}  // extern "C"

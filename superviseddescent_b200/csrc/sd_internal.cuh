@@ -29,6 +29,7 @@ enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_SVM /* compacted active rows, margins, column shift and index of sd_learn_squared_hinge (sd_hog_train.cu) */,
        SD_WS_TRAIN_ROWS /* positive rows, negative cache and labels of sd_hog_train_filter (sd_hog_train.cu) */,
        SD_WS_TRAIN_SLICE /* one slice's pyramid, scores, tables and detections of sd_hog_train_filter (sd_hog_train.cu) */,
+       SD_WS_PARTS /* cost tables, first tiles and detection map indices of the part-model calls (sd_hog_parts.cu) */,
        SD_WS_COUNT };
 
 // Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row

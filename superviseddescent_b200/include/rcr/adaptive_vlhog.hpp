@@ -8,6 +8,7 @@
 #pragma once
 
 #include <algorithm>
+#include <array>
 #include <cstring>
 #include <map>
 #include <memory>
@@ -451,6 +452,212 @@ inline std::vector<std::vector<hog_detection>> vl_hog_detect(const std::vector<c
         for (int k = 0; k < count[i]; ++k) {
             const sd_hog_detection& r = out[static_cast<size_t>(i) * max_detections + k];
             result[i].push_back(hog_detection{cv::Rect(r.x, r.y, r.w, r.h), r.score, r.filter, r.level, r.cell_x, r.cell_y});
+        }
+    return result;
+}
+
+// A star model for vl_hog_part_detect (include/sd_b200.h, sd_hog_part_model): Q root filters with their bias, and per component
+// P part filters scored at twice the root's resolution, in the shell's filter layout (dd * fh rows of fw floats); anchors[q][p]
+// = (ax, ay) in part-level cells relative to twice the root window's top-left cell; deformation[q][p] = (w0, w1, w2, w3), a
+// displacement (dx, dy) costing w0 dx^2 + w1 dx + w2 dy^2 + w3 dy; the root and part pads; R = max_displacement.
+struct hog_part_model {
+    std::vector<cv::Mat> root;
+    std::vector<float> bias;
+    std::vector<std::vector<cv::Mat>> parts;
+    std::vector<std::vector<std::array<int, 2>>> anchors;
+    std::vector<std::vector<std::array<float, 4>>> deformation;
+    int pad_x = 0, pad_y = 0, part_pad_x = 0, part_pad_y = 0;
+    int max_displacement = 4;
+};
+
+// One part of a detection: its box in frame pixels (empty where it has no placement), its placement (u, v) in part score
+// positions ((-1, -1) for none) and its transformed score D at the anchor.
+struct hog_part {
+    cv::Rect box;
+    int u, v;
+    float score;
+};
+struct hog_part_detection {
+    hog_detection detection;      // the root box, the star model's score, the component as the filter
+    std::vector<hog_part> parts;
+};
+
+// A star-model detector over image pyramids: vl_hog_pyramid over the root scales and their doubles (a scale present in both is
+// computed once; root scales must be in (0, 2]), vl_hog_correlate of the roots and of all Q * P parts, then on the device
+// sd_hog_distance_transform, sd_hog_part_scores, sd_hog_detections (the root's filter size and pad, all components as one
+// class) and sd_hog_part_placements.  Returns one list per frame, in the rule's order; each detection's box is what
+// detect_faces takes.  Throws std::runtime_error for a model of inconsistent shapes and where those calls refuse.
+inline std::vector<std::vector<hog_part_detection>> vl_hog_part_detect(const std::vector<cv::Mat>& images, const std::vector<double>& scales,
+                                                                       const hog_part_model& model, VlHogVariant variant, int cell_size,
+                                                                       int num_bins, float threshold, double overlap, int max_candidates,
+                                                                       int max_detections)
+{
+    if (images.empty()) return {};
+    const int dd = sd_b200::hog_dimension(variant, num_bins);
+    const int Q = static_cast<int>(model.root.size());
+    if (Q < 1 || model.parts.size() != model.root.size() || model.parts[0].empty() || model.anchors.size() != model.root.size() ||
+        model.deformation.size() != model.root.size() || model.root[0].rows % dd || model.parts[0][0].rows % dd)
+        throw std::runtime_error("vl_hog_part_detect: the model needs Q roots, parts, anchors and deformations of dd * side rows");
+    const int P = static_cast<int>(model.parts[0].size());
+    std::vector<cv::Mat> part_filters;
+    std::vector<int32_t> anchors;
+    std::vector<float> deformation;
+    for (int q = 0; q < Q; ++q) {
+        if (static_cast<int>(model.parts[q].size()) != P || static_cast<int>(model.anchors[q].size()) != P ||
+            static_cast<int>(model.deformation[q].size()) != P)
+            throw std::runtime_error("vl_hog_part_detect: every component needs P parts, anchors and deformations");
+        for (int p = 0; p < P; ++p) {
+            part_filters.push_back(model.parts[q][p]);
+            anchors.insert(anchors.end(), model.anchors[q][p].begin(), model.anchors[q][p].end());
+            deformation.insert(deformation.end(), model.deformation[q][p].begin(), model.deformation[q][p].end());
+        }
+    }
+    std::vector<double> every;
+    for (double s : scales) {
+        if (!(s > 0 && s <= 2)) throw std::runtime_error("vl_hog_part_detect: root scales must be in (0, 2]");
+        if (std::find(every.begin(), every.end(), s) == every.end()) every.push_back(s);
+    }
+    for (double s : scales)
+        if (std::find(every.begin(), every.end(), 2 * s) == every.end()) every.push_back(2 * s);
+    auto index = [&every](double s) { return static_cast<int>(std::find(every.begin(), every.end(), s) - every.begin()); };
+    const std::vector<std::vector<cv::Mat>> pyr = vl_hog_pyramid(images, every, variant, cell_size, num_bins);
+    const int n = static_cast<int>(images.size());
+    std::vector<cv::Mat> root_maps;
+    std::vector<std::array<int, 2>> root_of;   // (frame, scale index)
+    for (int i = 0; i < n; ++i)
+        for (size_t s = 0; s < scales.size(); ++s)
+            if (!pyr[i][index(scales[s])].empty()) {
+                root_maps.push_back(pyr[i][index(scales[s])]);
+                root_of.push_back({{i, static_cast<int>(s)}});
+            }
+    const std::vector<cv::Mat> roots = vl_hog_correlate(root_maps, model.root, variant, num_bins, model.bias, model.pad_x, model.pad_y);
+    // the part levels of the root maps with scores, each once
+    std::vector<std::array<int, 2>> plevels;
+    std::vector<cv::Mat> part_maps;
+    std::vector<int> part_of(roots.size(), -1);
+    for (size_t k = 0; k < roots.size(); ++k) {
+        if (roots[k].empty()) continue;
+        const std::array<int, 2> key{{root_of[k][0], index(2 * scales[root_of[k][1]])}};
+        if (pyr[key[0]][key[1]].empty()) continue;
+        auto it = std::find(plevels.begin(), plevels.end(), key);
+        if (it == plevels.end()) {
+            plevels.push_back(key);
+            part_maps.push_back(pyr[key[0]][key[1]]);
+            it = plevels.end() - 1;
+        }
+        part_of[k] = static_cast<int>(it - plevels.begin());
+    }
+    const std::vector<cv::Mat> part_scores =
+        part_maps.empty() ? std::vector<cv::Mat>() : vl_hog_correlate(part_maps, part_filters, variant, num_bins, {}, model.part_pad_x, model.part_pad_y);
+    sd_ctx* ctx = sd_b200::context();
+    // the part score maps on the device, their transform at the same offsets
+    sd_b200::DeviceBuffer d_raw, d_values, d_grids;
+    std::vector<cv::Mat> pplanes;
+    std::vector<int> pslot(part_scores.size(), -1);   // each part level's place among the maps with scores
+    for (size_t k = 0; k < part_scores.size(); ++k)
+        if (!part_scores[k].empty()) {
+            pslot[k] = static_cast<int>(pplanes.size());
+            pplanes.push_back(part_scores[k]);
+        }
+    const std::vector<int64_t> pstart = hog_batch::pack_planes(ctx, pplanes, sizeof(float), d_raw, "vl_hog_part_detect upload");
+    std::vector<sd_hog_grid> grids;
+    int64_t raw_floats = 0;
+    for (size_t j = 0; j < pplanes.size(); ++j) {
+        grids.push_back(sd_hog_grid{pplanes[j].cols, pplanes[j].rows / (Q * P), pstart[j], pstart[j]});
+        raw_floats += static_cast<int64_t>(pplanes[j].rows) * pplanes[j].cols;
+    }
+    d_raw.allocate(static_cast<size_t>(std::max<int64_t>(raw_floats, 1)) * sizeof(float));
+    d_values.allocate(static_cast<size_t>(std::max<int64_t>(raw_floats, 1)) * sizeof(float));
+    if (!grids.empty()) {
+        d_grids.allocate(grids.size() * sizeof(sd_hog_grid));
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_grids.as<sd_hog_grid>(), grids.data(), grids.size() * sizeof(sd_hog_grid)), "vl_hog_part_detect upload");
+        sd_hog_grids g{};
+        g.d_features = d_raw.as<float>();
+        g.count = static_cast<int32_t>(grids.size());
+        g.d_grids = d_grids.as<sd_hog_grid>();
+        sd_b200::check(ctx, sd_hog_distance_transform(ctx, &g, Q * P, deformation.data(), model.max_displacement, d_values.as<float>(), nullptr),
+                       "sd_hog_distance_transform");
+    }
+    // the root scores and the star model's scores at the same offsets
+    std::vector<cv::Mat> planes;
+    std::vector<size_t> kept;
+    for (size_t k = 0; k < roots.size(); ++k)
+        if (!roots[k].empty()) {
+            planes.push_back(roots[k]);
+            kept.push_back(k);
+        }
+    sd_b200::DeviceBuffer d_root, d_total, d_table, d_maps, d_anchors(anchors.size() * sizeof(int32_t));
+    const std::vector<int64_t> rstart = hog_batch::pack_planes(ctx, planes, sizeof(float), d_root, "vl_hog_part_detect upload");
+    int64_t root_floats = 1;
+    for (const cv::Mat& m : planes) root_floats += static_cast<int64_t>(m.rows) * m.cols;
+    d_total.allocate(static_cast<size_t>(root_floats) * sizeof(float));
+    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_anchors.as<int32_t>(), anchors.data(), anchors.size() * sizeof(int32_t)), "vl_hog_part_detect upload");
+    std::vector<sd_hog_part_map> table;
+    std::vector<sd_hog_score_map> maps;
+    for (size_t j = 0; j < kept.size(); ++j) {
+        const size_t k = kept[j];
+        const int i = root_of[k][0], s = root_of[k][1];
+        int lw = 0, lh = 0, w = 0, h = 0, d = 0, plw = 0, plh = 0;
+        sd_hog_pyramid_shape(images[i].cols, images[i].rows, scales[s], cell_size, num_bins, variant, &lw, &lh, &w, &h, &d);
+        sd_hog_pyramid_shape(images[i].cols, images[i].rows, 2 * scales[s], cell_size, num_bins, variant, &plw, &plh, &w, &h, &d);
+        const int oh = roots[k].rows / Q, ow = roots[k].cols;
+        int pw = 0, ph = 0;
+        int64_t po = 0;
+        if (part_of[k] >= 0 && pslot[part_of[k]] >= 0) {
+            const int j = pslot[part_of[k]];
+            pw = pplanes[j].cols;
+            ph = pplanes[j].rows / (Q * P);
+            po = pstart[j];
+        }
+        table.push_back(sd_hog_part_map{i, s, images[i].cols, images[i].rows, plw, plh, ow, oh, pw, ph, rstart[j], po, rstart[j]});
+        maps.push_back(sd_hog_score_map{i, s, images[i].cols, images[i].rows, lw, lh, ow, oh, rstart[j]});
+    }
+    sd_hog_part_model m{};
+    m.num_components = Q;
+    m.num_parts = P;
+    m.filter_w = model.root[0].cols;
+    m.filter_h = model.root[0].rows / dd;
+    m.part_w = model.parts[0][0].cols;
+    m.part_h = model.parts[0][0].rows / dd;
+    m.pad_x = model.pad_x; m.pad_y = model.pad_y;
+    m.part_pad_x = model.part_pad_x; m.part_pad_y = model.part_pad_y;
+    m.d_anchors = d_anchors.as<int32_t>();
+    const int nm = static_cast<int>(table.size());
+    if (nm > 0) {
+        d_table.allocate(table.size() * sizeof(sd_hog_part_map));
+        d_maps.allocate(maps.size() * sizeof(sd_hog_score_map));
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_table.as<sd_hog_part_map>(), table.data(), table.size() * sizeof(sd_hog_part_map)), "vl_hog_part_detect upload");
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_maps.as<sd_hog_score_map>(), maps.data(), maps.size() * sizeof(sd_hog_score_map)), "vl_hog_part_detect upload");
+        sd_b200::check(ctx, sd_hog_part_scores(ctx, d_root.as<float>(), d_values.as<float>(), d_table.as<sd_hog_part_map>(), nm, &m, d_total.as<float>()),
+                       "sd_hog_part_scores");
+    }
+    const size_t slots = static_cast<size_t>(n) * static_cast<size_t>(std::max(max_detections, 1));
+    sd_b200::DeviceBuffer d_out(slots * sizeof(sd_hog_detection)), d_count(static_cast<size_t>(n) * sizeof(int32_t)),
+        d_parts(slots * P * sizeof(sd_hog_part_placement));
+    sd_b200::check(ctx, sd_hog_detections(ctx, d_total.as<float>(), d_maps.as<sd_hog_score_map>(), nm, n, Q, cell_size, m.filter_w, m.filter_h,
+                                          m.pad_x, m.pad_y, threshold, overlap, max_candidates, max_detections, d_out.as<sd_hog_detection>(),
+                                          d_count.as<int32_t>(), nullptr), "sd_hog_detections");
+    sd_b200::check(ctx, sd_hog_part_placements(ctx, d_raw.as<float>(), d_table.as<sd_hog_part_map>(), nm, &m, deformation.data(),
+                                               model.max_displacement, cell_size, d_out.as<sd_hog_detection>(), d_count.as<int32_t>(), n,
+                                               max_detections, d_parts.as<sd_hog_part_placement>()), "sd_hog_part_placements");
+    std::vector<sd_hog_detection> out(slots);
+    std::vector<sd_hog_part_placement> parts(slots * P);
+    std::vector<int32_t> count(n);
+    sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.data(), d_out.as<void>(), slots * sizeof(sd_hog_detection)), "vl_hog_part_detect download");
+    sd_b200::check(ctx, sd_memcpy_d2h(ctx, parts.data(), d_parts.as<void>(), parts.size() * sizeof(sd_hog_part_placement)), "vl_hog_part_detect download");
+    sd_b200::check(ctx, sd_memcpy_d2h(ctx, count.data(), d_count.as<void>(), count.size() * sizeof(int32_t)), "vl_hog_part_detect download");
+    sd_b200::check(ctx, sd_sync(ctx), "vl_hog_part_detect download");
+    std::vector<std::vector<hog_part_detection>> result(n);
+    for (int i = 0; i < n; ++i)
+        for (int k = 0; k < count[i]; ++k) {
+            const size_t slot = static_cast<size_t>(i) * max_detections + k;
+            const sd_hog_detection& r = out[slot];
+            hog_part_detection det{hog_detection{cv::Rect(r.x, r.y, r.w, r.h), r.score, r.filter, r.level, r.cell_x, r.cell_y}, {}};
+            for (int p = 0; p < P; ++p) {
+                const sd_hog_part_placement& pp = parts[slot * P + p];
+                det.parts.push_back(hog_part{cv::Rect(pp.x, pp.y, pp.w, pp.h), pp.u, pp.v, pp.term});
+            }
+            result[i].push_back(det);
         }
     return result;
 }
