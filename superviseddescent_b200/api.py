@@ -1580,26 +1580,13 @@ def vl_hog_correlate(maps, filters, num_bins: int, variant: int = 1, bias=None, 
             raise ValueError(f"bias must have one value per filter ({q})")
     pad_x, pad_y = (int(p) for p in pad)
     maps = list(maps)
-    if any(not isinstance(m, torch.Tensor) or not m.is_cuda or m.dtype != torch.float32 or m.dim() != 3 or m.shape[0] != dd
-           for m in maps):
-        raise ValueError(f"every map must be a float32 CUDA tensor (dd, h, w) with dd = {dd}")
+    _check_maps(maps, dd)
     if not maps:
         return []
-    maps = [m.to(dev) for m in maps]
-    sizes = [tuple(m.shape[1:]) for m in maps]
-    # in place: contiguous maps of one storage, 4-byte aligned; else one packed copy
-    stor = maps[0].untyped_storage().data_ptr()
-    if all(m.is_contiguous() and m.untyped_storage().data_ptr() == stor for m in maps):
-        base, keep = stor, maps
-        offs = [(m.data_ptr() - base) // 4 for m in maps]
-    else:
-        keep, offs = _pack(maps, dev)
-        base = keep.data_ptr()
     # a map smaller than the filter scores nothing: an empty (Q, oh, ow) tensor
-    out, out_offs, scores = _results([(q, max(h + 2 * pad_y - fh + 1, 0), max(w + 2 * pad_x - fw + 1, 0)) for h, w in sizes], dev)
-    d_table = _device_table([HogGridC(w, h, o, oo) for (h, w), o, oo in zip(sizes, offs, out_offs)], dev)
-    g = HogGridsC()
-    g.d_features, g.count, g.width, g.height, g.d_grids = base, len(maps), 0, 0, d_table.data_ptr()
+    out, out_offs, scores = _results([(q, max(m.shape[1] + 2 * pad_y - fh + 1, 0), max(m.shape[2] + 2 * pad_x - fw + 1, 0))
+                                      for m in maps], dev)
+    g, keep = _maps_table(maps, dd, dev, out_offs)
     _check(ctx.h, _capi.lib().sd_hog_correlate(ctx.h, C.byref(g), int(num_bins), int(variant), ptr(f), int(q), int(fw), int(fh),
                                                ptr(b), pad_x, pad_y, ptr(out)))
     return scores
@@ -1629,20 +1616,15 @@ def vl_hog_detect(frames, scales, filters, cell_size: int, num_bins: int, thresh
     feats, levels = vl_hog_pyramid(frames, scales, cell_size, num_bins, variant, ctx=ctx)
     n = len(feats)
     if n == 0:
-        z = np.zeros(0, np.int32)
-        return HogDetections(z, np.zeros((0, 4), np.int32), np.zeros(0, np.float32), z, z, np.zeros((0, 2), np.int32),
-                             np.zeros(0, np.int64))
-    if isinstance(frames, (list, tuple)):
-        sizes = [(int(fr.shape[1]), int(fr.shape[0])) for fr in frames]
-    else:
-        sizes = [(int(frames.shape[2]), int(frames.shape[1]))] * n
+        return _detections(None, None, None)[0]
+    sizes = _frame_sizes(frames, n)
     which = [(i, s) for i in range(n) for s in range(len(scales)) if feats[i][s] is not None]
     scores = vl_hog_correlate([feats[i][s] for i, s in which], f, num_bins, variant, bias=bias, pad=(pad_x, pad_y), ctx=ctx)
     dev = f"cuda:{ctx.device}"
     md = int(max_detections)
-    out = torch.empty((max(n, 1), max(md, 1), len(HogDetectionC._fields_)), dtype=torch.int32, device=dev)
-    count = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
-    above = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+    out = torch.empty((n, max(md, 1), len(HogDetectionC._fields_)), dtype=torch.int32, device=dev)
+    count = torch.empty(n, dtype=torch.int32, device=dev)
+    above = torch.empty(n, dtype=torch.int64, device=dev)
     table, base = None, None
     if which:
         base = scores[0].untyped_storage().data_ptr()    # the maps' scores are views of one buffer
@@ -1651,23 +1633,48 @@ def vl_hog_detect(frames, scales, filters, cell_size: int, num_bins: int, thresh
     _check(ctx.h, _capi.lib().sd_hog_detections(ctx.h, ptr(base), ptr(table), len(which), n, int(q), int(cell_size), int(fw), int(fh),
                                                 pad_x, pad_y, float(threshold), float(overlap), int(max_candidates), md, ptr(out),
                                                 ptr(count), ptr(above)))
-    counts = count.cpu().numpy()[:n].astype(np.int64)
-    rows = out.cpu().numpy()
-    r = np.concatenate([rows[i, :c] for i, c in enumerate(counts)] + [np.zeros((0, rows.shape[2]), np.int32)])
-    return HogDetections(np.repeat(np.arange(n, dtype=np.int32), counts), np.ascontiguousarray(r[:, 0:4]),
+    return _detections(out, count, above)[0]
+
+
+def _frame_sizes(frames, n: int):
+    """(width, height) of each of the n frames of a frames argument as vl_hog_pyramid takes it."""
+    if isinstance(frames, (list, tuple)):
+        return [(int(fr.shape[1]), int(fr.shape[0])) for fr in frames]
+    return [(int(frames.shape[2]), int(frames.shape[1]))] * n
+
+
+def _frame_rows(rows, counts):
+    """rows[i, :counts[i]] of every frame i, end to end."""
+    return np.concatenate([rows[i, :c] for i, c in enumerate(counts)] + [np.zeros((0,) + rows.shape[2:], rows.dtype)])
+
+
+def _detections(out, count, above):
+    """The output of one sd_hog_detections call on the host -> (HogDetections, each frame's detection count).  out, count,
+    above: its (n, max_detections, 9) int32, (n,) int32 and (n,) int64 device tensors, or None for a call without frames."""
+    if out is None:
+        rows, counts, above = np.zeros((0, 1, len(HogDetectionC._fields_)), np.int32), np.zeros(0, np.int64), np.zeros(0, np.int64)
+    else:
+        rows, counts, above = out.cpu().numpy(), count.cpu().numpy().astype(np.int64), above.cpu().numpy()
+    r = _frame_rows(rows, counts)
+    return HogDetections(np.repeat(np.arange(len(counts), dtype=np.int32), counts), np.ascontiguousarray(r[:, 0:4]),
                          np.ascontiguousarray(r[:, 4]).view(np.float32), np.ascontiguousarray(r[:, 5]), np.ascontiguousarray(r[:, 6]),
-                         np.ascontiguousarray(r[:, 7:9]), above.cpu().numpy()[:n].copy())
+                         np.ascontiguousarray(r[:, 7:9]), above), counts
 
 
 # ------------------------------------------------------------------------------------------------
 # training HOG filters: window rows, a squared-hinge SVM and hard-negative mining
 # ------------------------------------------------------------------------------------------------
-def _maps_table(maps, dd: int, dev):
-    """A list of (dd, h, w) float32 CUDA maps -> (HogGridsC, tensors it points to): read in place when they are contiguous views
-    of one storage (as vl_hog_pyramid returns them), packed otherwise -- vl_hog_correlate's rule."""
+def _check_maps(maps, dd: int) -> None:
     if any(not isinstance(m, torch.Tensor) or not m.is_cuda or m.dtype != torch.float32 or m.dim() != 3 or m.shape[0] != dd
            for m in maps):
         raise ValueError(f"every map must be a float32 CUDA tensor (dd, h, w) with dd = {dd}")
+
+
+def _maps_table(maps, dd: int, dev, out_offsets=None):
+    """A non-empty list of (dd, h, w) float32 CUDA maps -> (HogGridsC, tensors it points to): read in place when they are
+    contiguous views of one storage (as vl_hog_pyramid returns them), packed otherwise.  out_offsets: each map's element offset
+    in the call's output, 0 for every map when None."""
+    _check_maps(maps, dd)
     maps = [m.to(dev) for m in maps]
     stor = maps[0].untyped_storage().data_ptr()
     if all(m.is_contiguous() and m.untyped_storage().data_ptr() == stor for m in maps):
@@ -1676,7 +1683,8 @@ def _maps_table(maps, dd: int, dev):
     else:
         keep, offs = _pack(maps, dev)
         base = keep.data_ptr()
-    table = _device_table([HogGridC(m.shape[2], m.shape[1], o, 0) for m, o in zip(maps, offs)], dev)
+    out_offsets = out_offsets or [0] * len(maps)
+    table = _device_table([HogGridC(m.shape[2], m.shape[1], o, oo) for m, o, oo in zip(maps, offs, out_offsets)], dev)
     g = HogGridsC()
     g.d_features, g.count, g.width, g.height, g.d_grids = base, len(maps), 0, 0, table.data_ptr()
     return g, (keep, table)
@@ -1994,14 +2002,8 @@ def vl_hog_part_detect(frames, scales, model: HogPartModel, cell_size: int, num_
     feats, levels = vl_hog_pyramid(frames, every, cell_size, num_bins, variant, ctx=ctx)
     n = len(feats)
     if n == 0:
-        z = np.zeros(0, np.int32)
-        return HogPartDetections(z, np.zeros((0, 4), np.int32), np.zeros(0, np.float32), z, z, np.zeros((0, 2), np.int32),
-                                 np.zeros(0, np.int64), np.zeros((0, p, 4), np.int32), np.zeros((0, p, 2), np.int32),
-                                 np.zeros((0, p), np.float32))
-    if isinstance(frames, (list, tuple)):
-        sizes = [(int(fr.shape[1]), int(fr.shape[0])) for fr in frames]
-    else:
-        sizes = [(int(frames.shape[2]), int(frames.shape[1]))] * n
+        return _part_detections(_detections(None, None, None), np.zeros((0, 1, p, len(HogPartPlacementC._fields_)), np.int32))
+    sizes = _frame_sizes(frames, n)
     which = [(i, s) for i in range(n) for s in range(len(scales)) if feats[i][ri[s]] is not None]
     roots = vl_hog_correlate([feats[i][ri[s]] for i, s in which], model.root, num_bins, variant, bias=model.bias, pad=model.pad,
                              ctx=ctx) if which else []
@@ -2052,13 +2054,12 @@ def vl_hog_part_detect(frames, scales, model: HogPartModel, cell_size: int, num_
                                         ptr(out), ptr(count), ptr(above)))
     _check(ctx.h, lib.sd_hog_part_placements(ctx.h, ptr(raw), ptr(table), len(kept), C.byref(mc), d_ptr, R, int(cell_size), ptr(out),
                                              ptr(count), n, md, ptr(place)))
-    counts = count.cpu().numpy().astype(np.int64)
-    rows = out.cpu().numpy()
-    pl = place.cpu().numpy()
-    r = np.concatenate([rows[i, :c] for i, c in enumerate(counts)] + [np.zeros((0, rows.shape[2]), np.int32)])
-    pr = np.concatenate([pl[i, :c] for i, c in enumerate(counts)] + [np.zeros((0, p, pl.shape[3]), np.int32)])
-    return HogPartDetections(np.repeat(np.arange(n, dtype=np.int32), counts), np.ascontiguousarray(r[:, 0:4]),
-                             np.ascontiguousarray(r[:, 4]).view(np.float32), np.ascontiguousarray(r[:, 5]),
-                             np.ascontiguousarray(r[:, 6]), np.ascontiguousarray(r[:, 7:9]), above.cpu().numpy().copy(),
-                             np.ascontiguousarray(pr[:, :, 3:7]), np.ascontiguousarray(pr[:, :, 0:2]),
+    return _part_detections(_detections(out, count, above), place.cpu().numpy())
+
+
+def _part_detections(detections, place):
+    """HogPartDetections from _detections' result and the (n, max_detections, P, 7) int32 sd_hog_part_placement rows."""
+    d, counts = detections
+    pr = _frame_rows(place, counts)
+    return HogPartDetections(*d, np.ascontiguousarray(pr[:, :, 3:7]), np.ascontiguousarray(pr[:, :, 0:2]),
                              np.ascontiguousarray(pr[:, :, 2]).view(np.float32))

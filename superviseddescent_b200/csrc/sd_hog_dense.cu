@@ -623,12 +623,7 @@ __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_kernel(cons
 {
     __shared__ int s_sx[kResizeW], s_xw[kResizeW], s_y0[kResizeH], s_y1[kResizeH], s_yw[kResizeH];
     const int b = blockIdx.x, tid = threadIdx.x;
-    int lo = 0, hi = a.count - 1;                    // the last level whose first tile is <= b
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (a.levels[mid].tile0 <= b) lo = mid;
-        else hi = mid - 1;
-    }
+    const int lo = sd_find_last_le(0, a.count - 1, b, [&](int i) { return a.levels[i].tile0; });   // the level of tile b
     const PyrLevel L = a.levels[lo];
     const int t = b - L.tile0, ty = t / L.tiles_x;
     const int x0 = (t - ty * L.tiles_x) * kResizeW, y0 = ty * kResizeH;

@@ -74,27 +74,6 @@ __device__ __forceinline__ unsigned long long cand_key(float s, unsigned rank)
     return ((unsigned long long)score_key(s) << 32) | (0xFFFFFFFFu - rank);
 }
 
-// the map of tile t: the last map whose first tile is <= t
-__device__ __forceinline__ int map_of_tile(const DetArgs& a, int t)
-{
-    int lo = 0, hi = a.num_maps - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (__ldg(a.tile0 + mid) <= t) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
-}
-
-// round half up of n / d, d > 0, with floor division
-__host__ __device__ __forceinline__ long long round_half_up(long long n, long long d)
-{
-    const long long num = 2 * n + d, den = 2 * d;
-    long long q = num / den;
-    if (num % den != 0 && num < 0) --q;
-    return q;
-}
-
 // the tile's map and its range of scores [e0, e1) in the map
 struct TileSpan {
     int m;
@@ -105,7 +84,7 @@ struct TileSpan {
 __device__ __forceinline__ TileSpan tile_span(const DetArgs& a, int t)
 {
     TileSpan s;
-    s.m = map_of_tile(a, t);
+    s.m = sd_find_last_le(0, a.num_maps - 1, t, [&](int i) { return __ldg(a.tile0 + i); });   // the last map whose first tile is <= t
     s.d = a.maps[s.m];
     const long long n = (long long)a.Q * s.d.width * s.d.height;
     s.e0 = (long long)(t - __ldg(a.tile0 + s.m)) * kTile;
@@ -231,14 +210,9 @@ struct Decoded {
 __device__ Decoded decode(const DetArgs& a, int f, unsigned long long k)
 {
     const unsigned rank = 0xFFFFFFFFu - (unsigned)(k & 0xFFFFFFFFu);
-    int lo = a.fmap0[f], hi = a.fmap0[f + 1] - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (a.rank0[a.fmaps[mid]] <= rank) lo = mid;
-        else hi = mid - 1;
-    }
+    const int i = sd_find_last_le(a.fmap0[f], a.fmap0[f + 1] - 1, rank, [&](int j) { return a.rank0[a.fmaps[j]]; });
     Decoded r;
-    r.m = a.fmaps[lo];
+    r.m = a.fmaps[i];
     const sd_hog_score_map& d = a.maps[r.m];
     r.e = rank - a.rank0[r.m];
     const long long row = r.e / d.width;
@@ -248,16 +222,11 @@ __device__ Decoded decode(const DetArgs& a, int f, unsigned long long k)
     return r;
 }
 
-// {x0, y0, x1, y1} of a score position: the rule's exact integer mapping
+// {x0, y0, x1, y1} of a score position in int32 (sd_hog_detections checks that they fit)
 __device__ int4 box_of(const DetArgs& a, const sd_hog_score_map& d, int x, int y)
 {
-    const long long sx = (long long)a.cell * d.frame_w, sy = (long long)a.cell * d.frame_h;
-    int4 b;
-    b.x = (int)round_half_up((long long)(x - a.pad_x) * sx, d.level_w);
-    b.z = (int)round_half_up((long long)(x - a.pad_x + a.fw) * sx, d.level_w);
-    b.y = (int)round_half_up((long long)(y - a.pad_y) * sy, d.level_h);
-    b.w = (int)round_half_up((long long)(y - a.pad_y + a.fh) * sy, d.level_h);
-    return b;
+    const sd_box64 b = sd_window_box(x, y, a.pad_x, a.pad_y, a.fw, a.fh, a.cell, d.frame_w, d.frame_h, d.level_w, d.level_h);
+    return make_int4((int)b.x0, (int)b.y0, (int)b.x1, (int)b.y1);
 }
 
 __device__ __forceinline__ long long box_area(int4 b) { return (long long)(b.z - b.x) * (b.w - b.y); }
@@ -346,9 +315,24 @@ __global__ void __launch_bounds__(kNmsThreads, 1) det_nms_kernel(const __grid_co
     if (tid == 0) a.count[f] = kept;
 }
 
-bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
-
 }  // namespace
+
+bool sd_window_boxes_fit_int32(int width, int height, int pad_x, int pad_y, int fw, int fh, int cell, int frame_w, int frame_h,
+                               int level_w, int level_h)
+{
+    if (width <= 0 || height <= 0) return true;
+    // the extreme numerators, those of positions 0 and width - 1 (height - 1), exactly
+    const __int128 limit = (__int128)1 << 62;
+    const __int128 sx = (__int128)cell * frame_w, sy = (__int128)cell * frame_h;
+    const __int128 nx[2] = {(__int128)(-pad_x) * sx, (__int128)(width - 1 - pad_x + fw) * sx};
+    const __int128 ny[2] = {(__int128)(-pad_y) * sy, (__int128)(height - 1 - pad_y + fh) * sy};
+    for (int k = 0; k < 2; ++k) {
+        if (!(nx[k] < limit && nx[k] > -limit && ny[k] < limit && ny[k] > -limit)) return false;
+        const long long bx = sd_round_half_up((long long)nx[k], level_w), by = sd_round_half_up((long long)ny[k], level_h);
+        if (bx < INT_MIN || bx > INT_MAX || by < INT_MIN || by > INT_MAX) return false;
+    }
+    return true;
+}
 
 extern "C" {
 
@@ -359,15 +343,14 @@ int sd_hog_detections(sd_ctx* ctx, const float* d_scores, const sd_hog_score_map
 {
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, d_out && d_count && (num_maps == 0 || (d_scores && d_maps)), "null argument");
-    SD_REQUIRE(ctx, aligned(d_scores, 4) && aligned(d_maps, 8) && aligned(d_out, 4) && aligned(d_count, 4) && aligned(d_above, 8),
+    SD_REQUIRE(ctx, sd_aligned(d_scores, 4) && sd_aligned(d_maps, 8) && sd_aligned(d_out, 4) && sd_aligned(d_count, 4) &&
+                        sd_aligned(d_above, 8),
                "scores, output and counts must be 4-byte aligned, the map table and d_above 8-byte aligned");
     SD_REQUIRE(ctx, num_frames >= 1, "num_frames must be >= 1");
     SD_REQUIRE(ctx, num_maps >= 0, "negative map count");
     SD_REQUIRE(ctx, num_filters >= 1 && num_filters <= SD_HOG_FILTER_MAX_BANK, "num_filters must be in [1, SD_HOG_FILTER_MAX_BANK]");
     SD_REQUIRE(ctx, cell_size >= 1 && cell_size <= kDenseMaxCell, "cell_size must be in [1,32]");
-    SD_REQUIRE(ctx, filter_w >= 1 && filter_w <= SD_HOG_FILTER_MAX_SIDE && filter_h >= 1 && filter_h <= SD_HOG_FILTER_MAX_SIDE,
-               "filter sides must be in [1, SD_HOG_FILTER_MAX_SIDE]");
-    SD_REQUIRE(ctx, pad_x >= 0 && pad_x < filter_w && pad_y >= 0 && pad_y < filter_h, "pads must be in [0, filter side - 1]");
+    if (const int rc = sd_hog_check_filter(ctx, __func__, filter_w, filter_h, pad_x, pad_y)) return rc;
     SD_REQUIRE(ctx, !std::isnan(threshold), "threshold is NaN");
     SD_REQUIRE(ctx, overlap >= 0.0 && overlap <= 1.0, "overlap must be in [0, 1]");
     SD_REQUIRE(ctx, max_candidates >= 1 && max_candidates <= SD_HOG_DETECT_MAX_CANDIDATES,
@@ -385,7 +368,6 @@ int sd_hog_detections(sd_ctx* ctx, const float* d_scores, const sd_hog_score_map
     int* fmap0 = fmaps + num_maps;
     std::vector<long long> frame_scores(num_frames, 0);
     long long tiles = 0;
-    const __int128 limit = (__int128)1 << 62;
     for (int i = 0; i < num_maps; ++i) {
         const sd_hog_score_map& m = table[i];
         SD_REQUIRE(ctx, m.frame >= 0 && m.frame < num_frames, "a map's frame is out of range");
@@ -399,20 +381,9 @@ int sd_hog_detections(sd_ctx* ctx, const float* d_scores, const sd_hog_score_map
         rank0[i] = (unsigned)frame_scores[m.frame];
         frame_scores[m.frame] += n;
         SD_REQUIRE(ctx, frame_scores[m.frame] <= (long long)UINT_MAX, "more than 2^32 - 1 scores in one frame");
-        if (n > 0) {        // the boxes of the extreme positions fit in int32 (and their numerators in int64 with room)
-            const __int128 sx = (__int128)cell_size * m.frame_w, sy = (__int128)cell_size * m.frame_h;
-            const __int128 nx[2] = {(__int128)(-pad_x) * sx, (__int128)(m.width - 1 - pad_x + filter_w) * sx};
-            const __int128 ny[2] = {(__int128)(-pad_y) * sy, (__int128)(m.height - 1 - pad_y + filter_h) * sy};
-            bool ok = true;
-            for (int k = 0; k < 2; ++k) {
-                ok = ok && nx[k] < limit && nx[k] > -limit && ny[k] < limit && ny[k] > -limit;
-                if (ok) {
-                    const long long bx = round_half_up((long long)nx[k], m.level_w), by = round_half_up((long long)ny[k], m.level_h);
-                    ok = bx >= INT_MIN && bx <= INT_MAX && by >= INT_MIN && by <= INT_MAX;
-                }
-            }
-            SD_REQUIRE(ctx, ok, "a map's boxes do not fit in int32");
-        }
+        SD_REQUIRE(ctx, sd_window_boxes_fit_int32(m.width, m.height, pad_x, pad_y, filter_w, filter_h, cell_size, m.frame_w, m.frame_h,
+                                                  m.level_w, m.level_h),
+                   "a map's boxes do not fit in int32");
     }
     {
         std::vector<int> per(num_frames + 1, 0);

@@ -79,18 +79,13 @@ __global__ void __launch_bounds__(kThreads, 4) hog_correlate_kernel(const __grid
     float* __restrict__ out;
     const int fw = a.fw, fh = a.fh;
     if (a.grids) {
-        int lo = 0, hi = a.count - 1;                // the last grid whose first CTA is <= b
-        while (lo < hi) {
-            const int mid = (lo + hi + 1) >> 1;
-            if (a.tile0[mid] <= b) lo = mid;
-            else hi = mid - 1;
-        }
-        const sd_hog_grid d = a.grids[lo];
+        const int g = sd_find_last_le(0, a.count - 1, b, [&](int i) { return a.tile0[i]; });   // the grid of CTA b
+        const sd_hog_grid d = a.grids[g];
         W = d.width; H = d.height;
         M = a.maps + d.offset;
         out = a.scores + d.out_offset;
-        tiles_x = (W + 2 * a.pad_x - fw + 1 + kTileW - 1) / kTileW;
-        t = b - a.tile0[lo];
+        tiles_x = (sd_score_extent(W, a.pad_x, fw) + kTileW - 1) / kTileW;
+        t = b - a.tile0[g];
     } else {
         const int g = b / a.tiles;
         W = a.width; H = a.height;
@@ -99,7 +94,7 @@ __global__ void __launch_bounds__(kThreads, 4) hog_correlate_kernel(const __grid
         tiles_x = a.tiles_x;
         t = b - g * a.tiles;
     }
-    const int oh = H + 2 * a.pad_y - fh + 1, ow = W + 2 * a.pad_x - fw + 1;
+    const int oh = sd_score_extent(H, a.pad_y, fh), ow = sd_score_extent(W, a.pad_x, fw);
     const int tr = t / tiles_x;
     const int x0 = (t - tr * tiles_x) * kTileW, y0 = tr * kTileH;
     const int q0 = blockIdx.y * QF;
@@ -191,8 +186,6 @@ CorrKernel corr_kernel(int QF)
     return QF == 1 ? hog_correlate_kernel<1> : QF == 2 ? hog_correlate_kernel<2> : QF == 4 ? hog_correlate_kernel<4> : hog_correlate_kernel<8>;
 }
 
-bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
-
 }  // namespace
 
 extern "C" {
@@ -204,14 +197,13 @@ int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int va
     SD_REQUIRE(ctx, maps && d_filters && d_scores, "null argument");
     if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins)) return rc;
     SD_REQUIRE(ctx, num_filters >= 1 && num_filters <= SD_HOG_FILTER_MAX_BANK, "num_filters must be in [1, SD_HOG_FILTER_MAX_BANK]");
-    SD_REQUIRE(ctx, filter_w >= 1 && filter_w <= SD_HOG_FILTER_MAX_SIDE && filter_h >= 1 && filter_h <= SD_HOG_FILTER_MAX_SIDE,
-               "filter sides must be in [1, SD_HOG_FILTER_MAX_SIDE]");
-    SD_REQUIRE(ctx, pad_x >= 0 && pad_x < filter_w && pad_y >= 0 && pad_y < filter_h, "pads must be in [0, filter side - 1]");
-    SD_REQUIRE(ctx, aligned4(d_filters) && aligned4(d_scores) && aligned4(d_bias), "filters, bias and scores must be 4-byte aligned");
+    if (const int rc = sd_hog_check_filter(ctx, __func__, filter_w, filter_h, pad_x, pad_y)) return rc;
+    SD_REQUIRE(ctx, sd_aligned(d_filters, 4) && sd_aligned(d_scores, 4) && sd_aligned(d_bias, 4),
+               "filters, bias and scores must be 4-byte aligned");
     SD_REQUIRE(ctx, maps->count >= 0, "negative grid count");
     const int count = maps->count;
     if (count == 0) return SD_OK;
-    SD_REQUIRE(ctx, maps->d_features && aligned4(maps->d_features), "maps must be non-null and 4-byte aligned");
+    SD_REQUIRE(ctx, maps->d_features && sd_aligned(maps->d_features, 4), "maps must be non-null and 4-byte aligned");
 
     int max_w = 0, max_h = 0;
     std::vector<sd_hog_grid> table;
@@ -239,7 +231,7 @@ int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int va
         std::vector<int> tile0(count);
         for (int i = 0; i < count; ++i) {
             tile0[i] = (int)total;
-            const int oh = table[i].height + 2 * pad_y - filter_h + 1, ow = table[i].width + 2 * pad_x - filter_w + 1;
+            const int oh = sd_score_extent(table[i].height, pad_y, filter_h), ow = sd_score_extent(table[i].width, pad_x, filter_w);
             if (oh > 0 && ow > 0) total += (long long)sd_div_up(ow, kTileW) * sd_div_up(oh, kTileH);
             SD_REQUIRE(ctx, total <= INT_MAX, "too many score tiles");
         }
@@ -249,7 +241,7 @@ int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int va
         SD_CUDA(ctx, cudaMemcpyAsync(d_tile0, tile0.data(), sizeof(int) * count, cudaMemcpyHostToDevice, ctx->stream));
         a.tile0 = d_tile0;
     } else {
-        const int oh = max_h + 2 * pad_y - filter_h + 1, ow = max_w + 2 * pad_x - filter_w + 1;
+        const int oh = sd_score_extent(max_h, pad_y, filter_h), ow = sd_score_extent(max_w, pad_x, filter_w);
         if (oh <= 0 || ow <= 0) return SD_OK;
         a.width = max_w; a.height = max_h;
         a.in_stride = (long long)dd * max_w * max_h;

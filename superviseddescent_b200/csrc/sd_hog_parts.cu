@@ -39,17 +39,6 @@ __device__ __forceinline__ void dt_take(float cand, int k, float& best, int& arg
     }
 }
 
-__device__ __forceinline__ int find_last_le(const long long* first, int n, long long t)
-{
-    int lo = 0, hi = n - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (__ldg(first + mid) <= t) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
-}
-
 // ---- the transform ----------------------------------------------------------------------------------------------------------
 
 struct DtArgs {
@@ -78,7 +67,7 @@ __global__ void __launch_bounds__(kThreads) dt_tile_kernel(const __grid_constant
         int m, w, h;
         long long base, obase, local;
         if (a.grids) {
-            m = find_last_le(a.tile0, a.num_maps, t);
+            m = sd_find_last_le(0, a.num_maps - 1, t, [&](int i) { return __ldg(a.tile0 + i); });
             const sd_hog_grid g = a.grids[m];
             w = g.width; h = g.height; base = g.offset; obase = g.out_offset;
             local = t - __ldg(a.tile0 + m);
@@ -163,7 +152,7 @@ struct ScoreArgs {
 __global__ void __launch_bounds__(kThreads) part_scores_kernel(const __grid_constant__ ScoreArgs a)
 {
     for (long long t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
-        const int m = find_last_le(a.tile0, a.num_maps, t);
+        const int m = sd_find_last_le(0, a.num_maps - 1, t, [&](int i) { return __ldg(a.tile0 + i); });
         const sd_hog_part_map d = a.maps[m];
         const long long plane = (long long)d.width * d.height, n = a.Q * plane;
         const long long e0 = (t - __ldg(a.tile0 + m)) * kScoreTile, e1 = min(e0 + kScoreTile, n);
@@ -201,14 +190,6 @@ struct PlaceArgs {
     sd_hog_part_placement* out;
     int num_frames, max_det, P, R, cell, pfw, pfh, pad_x, pad_y, part_pad_x, part_pad_y;
 };
-
-__host__ __device__ __forceinline__ long long round_half_up(long long n, long long d)
-{
-    const long long num = 2 * n + d, den = 2 * d;
-    long long q = num / den;
-    if (num % den != 0 && num < 0) --q;
-    return q;
-}
 
 __global__ void __launch_bounds__(kPlaceWarps * 32) part_place_kernel(const __grid_constant__ PlaceArgs a)
 {
@@ -258,12 +239,9 @@ __global__ void __launch_bounds__(kPlaceWarps * 32) part_place_kernel(const __gr
                 if (arg != kNone && s_dx[arg + a.R] != kNone) {
                     r.u = u + s_dx[arg + a.R];
                     r.v = v + arg;
-                    const long long sx = (long long)a.cell * d.frame_w, sy = (long long)a.cell * d.frame_h;
-                    const long long bx0 = round_half_up((long long)(r.u - a.part_pad_x) * sx, d.part_level_w);
-                    const long long bx1 = round_half_up((long long)(r.u - a.part_pad_x + a.pfw) * sx, d.part_level_w);
-                    const long long by0 = round_half_up((long long)(r.v - a.part_pad_y) * sy, d.part_level_h);
-                    const long long by1 = round_half_up((long long)(r.v - a.part_pad_y + a.pfh) * sy, d.part_level_h);
-                    r.x = (int)bx0; r.y = (int)by0; r.w = (int)(bx1 - bx0); r.h = (int)(by1 - by0);
+                    const sd_box64 b = sd_window_box(r.u, r.v, a.part_pad_x, a.part_pad_y, a.pfw, a.pfh, a.cell, d.frame_w, d.frame_h,
+                                                     d.part_level_w, d.part_level_h);
+                    r.x = (int)b.x0; r.y = (int)b.y0; r.w = (int)(b.x1 - b.x0); r.h = (int)(b.y1 - b.y0);
                 }
             }
             __syncwarp();
@@ -271,8 +249,6 @@ __global__ void __launch_bounds__(kPlaceWarps * 32) part_place_kernel(const __gr
         if (lane == 0) a.out[it] = r;
     }
 }
-
-bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
 
 // cost tables of num_planes deformations: cx[d] = (float)((double)w0 d^2 + (double)w1 d), cy alike with w2, w3
 bool cost_tables(const float* h_def, int num_planes, int R, std::vector<float>& costs)
@@ -292,17 +268,12 @@ bool cost_tables(const float* h_def, int num_planes, int R, std::vector<float>& 
 
 int check_model(sd_ctx* ctx, const sd_hog_part_model* m)
 {
-    SD_REQUIRE(ctx, m && m->d_anchors && aligned(m->d_anchors, 8), "null model or anchors not 8-byte aligned");
+    SD_REQUIRE(ctx, m && m->d_anchors && sd_aligned(m->d_anchors, 8), "null model or anchors not 8-byte aligned");
     SD_REQUIRE(ctx, m->num_parts >= 1 && m->num_parts <= SD_HOG_PART_MAX_PARTS, "num_parts must be in [1, SD_HOG_PART_MAX_PARTS]");
     SD_REQUIRE(ctx, m->num_components >= 1 && (long long)m->num_components * m->num_parts <= SD_HOG_FILTER_MAX_BANK,
                "num_components must be >= 1 with num_components * num_parts <= SD_HOG_FILTER_MAX_BANK");
-    SD_REQUIRE(ctx, m->filter_w >= 1 && m->filter_w <= SD_HOG_FILTER_MAX_SIDE && m->filter_h >= 1 && m->filter_h <= SD_HOG_FILTER_MAX_SIDE &&
-                        m->part_w >= 1 && m->part_w <= SD_HOG_FILTER_MAX_SIDE && m->part_h >= 1 && m->part_h <= SD_HOG_FILTER_MAX_SIDE,
-               "filter and part sides must be in [1, SD_HOG_FILTER_MAX_SIDE]");
-    SD_REQUIRE(ctx, m->pad_x >= 0 && m->pad_x < m->filter_w && m->pad_y >= 0 && m->pad_y < m->filter_h && m->part_pad_x >= 0 &&
-                        m->part_pad_x < m->part_w && m->part_pad_y >= 0 && m->part_pad_y < m->part_h,
-               "pads must be in [0, side - 1]");
-    return SD_OK;
+    if (const int rc = sd_hog_check_filter(ctx, __func__, m->filter_w, m->filter_h, m->pad_x, m->pad_y)) return rc;
+    return sd_hog_check_filter(ctx, __func__, m->part_w, m->part_h, m->part_pad_x, m->part_pad_y);
 }
 
 // the score tiles of each map of a part table (first tile per map) and the check every call makes of the table's sizes
@@ -331,8 +302,8 @@ int sd_hog_distance_transform(sd_ctx* ctx, const sd_hog_grids* maps, int num_pla
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, maps && h_deformation && d_values, "null argument");
     SD_REQUIRE(ctx, maps->count >= 0, "negative map count");
-    SD_REQUIRE(ctx, maps->count == 0 || (maps->d_features && aligned(maps->d_features, 4)), "maps must be non-null and 4-byte aligned");
-    SD_REQUIRE(ctx, aligned(d_values, 4) && aligned(d_place, 8), "values must be 4-byte aligned and placements 8-byte aligned");
+    SD_REQUIRE(ctx, maps->count == 0 || (maps->d_features && sd_aligned(maps->d_features, 4)), "maps must be non-null and 4-byte aligned");
+    SD_REQUIRE(ctx, sd_aligned(d_values, 4) && sd_aligned(d_place, 8), "values must be 4-byte aligned and placements 8-byte aligned");
     SD_REQUIRE(ctx, num_planes >= 1 && num_planes <= SD_HOG_FILTER_MAX_BANK, "num_planes must be in [1, SD_HOG_FILTER_MAX_BANK]");
     SD_REQUIRE(ctx, max_displacement >= 0 && max_displacement <= SD_HOG_PART_MAX_DISPLACEMENT,
                "max_displacement must be in [0, SD_HOG_PART_MAX_DISPLACEMENT]");
@@ -391,7 +362,7 @@ int sd_hog_part_scores(sd_ctx* ctx, const float* d_root, const float* d_parts, c
     if (const int rc = check_model(ctx, model)) return rc;
     SD_REQUIRE(ctx, num_maps >= 0, "negative map count");
     SD_REQUIRE(ctx, num_maps == 0 || (d_root && d_parts && d_maps && d_out), "null argument");
-    SD_REQUIRE(ctx, aligned(d_root, 4) && aligned(d_parts, 4) && aligned(d_out, 4) && aligned(d_maps, 8),
+    SD_REQUIRE(ctx, sd_aligned(d_root, 4) && sd_aligned(d_parts, 4) && sd_aligned(d_out, 4) && sd_aligned(d_maps, 8),
                "scores must be 4-byte aligned and the map table 8-byte aligned");
     if (num_maps == 0) return SD_OK;
     std::vector<sd_hog_part_map> table;
@@ -430,7 +401,8 @@ int sd_hog_part_placements(sd_ctx* ctx, const float* d_parts, const sd_hog_part_
     if (!ctx) return SD_ERR_INVALID;
     if (const int rc = check_model(ctx, model)) return rc;
     SD_REQUIRE(ctx, h_deformation && d_det && d_count && d_out && (num_maps == 0 || (d_parts && d_maps)), "null argument");
-    SD_REQUIRE(ctx, aligned(d_parts, 4) && aligned(d_maps, 8) && aligned(d_det, 4) && aligned(d_count, 4) && aligned(d_out, 4),
+    SD_REQUIRE(ctx, sd_aligned(d_parts, 4) && sd_aligned(d_maps, 8) && sd_aligned(d_det, 4) && sd_aligned(d_count, 4) &&
+                        sd_aligned(d_out, 4),
                "scores, detections, counts and output must be 4-byte aligned, the map table 8-byte aligned");
     SD_REQUIRE(ctx, num_maps >= 0, "negative map count");
     SD_REQUIRE(ctx, num_frames >= 1, "num_frames must be >= 1");
@@ -450,27 +422,15 @@ int sd_hog_part_placements(sd_ctx* ctx, const float* d_parts, const sd_hog_part_
     long long tiles = 0;
     if (const int rc = part_tiles(ctx, table, Q, tile0, &tiles)) return rc;
     std::map<std::pair<int, int>, int> index;
-    const __int128 limit = (__int128)1 << 62;
     for (int i = 0; i < num_maps; ++i) {
         const sd_hog_part_map& d = table[i];
         SD_REQUIRE(ctx, d.frame >= 0 && d.frame < num_frames, "a map's frame is out of range");
         SD_REQUIRE(ctx, d.frame_w >= 1 && d.frame_h >= 1 && d.part_level_w >= 1 && d.part_level_h >= 1,
                    "a map's frame or part level is smaller than 1 x 1");
         SD_REQUIRE(ctx, index.emplace(std::make_pair(d.frame, d.level), i).second, "two maps share one (frame, level)");
-        if (d.part_width > 0 && d.part_height > 0) {   // the part boxes of the extreme positions fit in int32
-            const __int128 sx = (__int128)cell_size * d.frame_w, sy = (__int128)cell_size * d.frame_h;
-            const __int128 nx[2] = {(__int128)(-model->part_pad_x) * sx, (__int128)(d.part_width - 1 - model->part_pad_x + model->part_w) * sx};
-            const __int128 ny[2] = {(__int128)(-model->part_pad_y) * sy, (__int128)(d.part_height - 1 - model->part_pad_y + model->part_h) * sy};
-            bool ok = true;
-            for (int k = 0; k < 2; ++k) {
-                ok = ok && nx[k] < limit && nx[k] > -limit && ny[k] < limit && ny[k] > -limit;
-                if (ok) {
-                    const long long bx = round_half_up((long long)nx[k], d.part_level_w), by = round_half_up((long long)ny[k], d.part_level_h);
-                    ok = bx >= INT_MIN && bx <= INT_MAX && by >= INT_MIN && by <= INT_MAX;
-                }
-            }
-            SD_REQUIRE(ctx, ok, "a map's part boxes do not fit in int32");
-        }
+        SD_REQUIRE(ctx, sd_window_boxes_fit_int32(d.part_width, d.part_height, model->part_pad_x, model->part_pad_y, model->part_w,
+                                                  model->part_h, cell_size, d.frame_w, d.frame_h, d.part_level_w, d.part_level_h),
+                   "a map's part boxes do not fit in int32");
     }
     // the detections, read back once: each must come from a map of the table
     const size_t slots = (size_t)num_frames * max_detections;

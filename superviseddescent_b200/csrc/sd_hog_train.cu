@@ -100,8 +100,6 @@ __global__ void __launch_bounds__(256) svm_compact_kernel(const float* __restric
     }
 }
 
-bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
-
 int launch_windows(sd_ctx* ctx, const float* maps, const sd_hog_grid* d_grids, int width, int height, int num_bins, int variant,
                    int fw, int fh, int pad_x, int pad_y, const sd_hog_window* d_windows, const int* d_dest, int count, float* d_rows,
                    int64_t ldr)
@@ -125,30 +123,9 @@ int launch_windows(sd_ctx* ctx, const float* maps, const sd_hog_grid* d_grids, i
     return SD_OK;
 }
 
-// the filter limits of sd_hog_correlate
-int check_filter(sd_ctx* ctx, const char* fn, int fw, int fh, int pad_x, int pad_y)
-{
-    if (fw < 1 || fw > SD_HOG_FILTER_MAX_SIDE || fh < 1 || fh > SD_HOG_FILTER_MAX_SIDE)
-        return sd_fail(ctx, SD_ERR_INVALID, "%s: filter sides must be in [1, SD_HOG_FILTER_MAX_SIDE]", fn);
-    if (pad_x < 0 || pad_x >= fw || pad_y < 0 || pad_y >= fh)
-        return sd_fail(ctx, SD_ERR_INVALID, "%s: pads must be in [0, filter side - 1]", fn);
-    return SD_OK;
-}
-
-// ---- the box rule of sd_hog_detections and exact IoU ---------------------------------------------------------------------
-int64_t rh(int64_t n, int64_t d) { int64_t q = (2 * n + d) / (2 * d); if ((2 * n + d) % (2 * d) < 0) --q; return q; }
-
-struct Box64 { int64_t x0, y0, x1, y1; };
-
-Box64 window_box(int x, int y, int frame_w, int frame_h, int level_w, int level_h, int cell_size, int fw, int fh, int pad_x, int pad_y)
-{
-    const int64_t sx = (int64_t)cell_size * frame_w, sy = (int64_t)cell_size * frame_h;
-    return {rh((int64_t)(x - pad_x) * sx, level_w), rh((int64_t)(y - pad_y) * sy, level_h),
-            rh((int64_t)(x - pad_x + fw) * sx, level_w), rh((int64_t)(y - pad_y + fh) * sy, level_h)};
-}
-
+// ---- exact IoU of detection boxes ------------------------------------------------------------------------------------------
 // intersection and union of two boxes in int64 pixel areas
-void inter_union(const Box64& a, const Box64& b, int64_t* inter, int64_t* uni)
+void inter_union(const sd_box64& a, const sd_box64& b, int64_t* inter, int64_t* uni)
 {
     const int64_t iw = std::min(a.x1, b.x1) - std::max(a.x0, b.x0), ih = std::min(a.y1, b.y1) - std::max(a.y0, b.y0);
     *inter = iw > 0 && ih > 0 ? iw * ih : 0;
@@ -159,17 +136,17 @@ struct Level { int level_w, level_h, hog_w, hog_h; };
 
 // sd_hog_box_windows for one box over a frame's level table (levels with hog_w = 0 are empty)
 void best_window(const std::vector<Level>& lv, int frame_w, int frame_h, int cell_size, int fw, int fh, int pad_x, int pad_y,
-                 double positive_overlap, const Box64& box, sd_hog_window* out, double* iou)
+                 double positive_overlap, const sd_box64& box, sd_hog_window* out, double* iou)
 {
     int64_t bi = 0, bu = 1;                           // best IoU so far as a rational, -1 / 1 before the first candidate
     bool any = false;
     sd_hog_window best = {-1, 0, 0, 0};
     for (int s = 0; s < (int)lv.size(); ++s) {
         if (!lv[s].hog_w) continue;
-        const int oh = lv[s].hog_h + 2 * pad_y - fh + 1, ow = lv[s].hog_w + 2 * pad_x - fw + 1;
+        const int oh = sd_score_extent(lv[s].hog_h, pad_y, fh), ow = sd_score_extent(lv[s].hog_w, pad_x, fw);
         for (int y = 0; y < oh; ++y)
             for (int x = 0; x < ow; ++x) {
-                const Box64 b = window_box(x, y, frame_w, frame_h, lv[s].level_w, lv[s].level_h, cell_size, fw, fh, pad_x, pad_y);
+                const sd_box64 b = sd_window_box(x, y, pad_x, pad_y, fw, fh, cell_size, frame_w, frame_h, lv[s].level_w, lv[s].level_h);
                 int64_t in, un;
                 inter_union(box, b, &in, &un);
                 // in / un > bi / bu, exactly (both unions are positive)
@@ -370,13 +347,13 @@ int sd_hog_windows(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int vari
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, maps && d_windows && d_rows, "null argument");
     if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins)) return rc;
-    if (const int rc = check_filter(ctx, __func__, filter_w, filter_h, pad_x, pad_y)) return rc;
-    SD_REQUIRE(ctx, aligned4(d_windows) && aligned4(d_rows), "windows and rows must be 4-byte aligned");
+    if (const int rc = sd_hog_check_filter(ctx, __func__, filter_w, filter_h, pad_x, pad_y)) return rc;
+    SD_REQUIRE(ctx, sd_aligned(d_windows, 4) && sd_aligned(d_rows, 4), "windows and rows must be 4-byte aligned");
     SD_REQUIRE(ctx, count >= 0 && maps->count >= 0, "negative count");
     const int64_t D = (int64_t)sd_hog_dd(num_bins, variant) * filter_w * filter_h + 1;
     SD_REQUIRE(ctx, ldr >= D, "ldr must be at least dd * filter_h * filter_w + 1");
     if (count == 0) return SD_OK;
-    SD_REQUIRE(ctx, maps->count >= 1 && maps->d_features && aligned4(maps->d_features), "maps must be non-null and 4-byte aligned");
+    SD_REQUIRE(ctx, maps->count >= 1 && maps->d_features && sd_aligned(maps->d_features, 4), "maps must be non-null and 4-byte aligned");
     int max_w = 0, max_h = 0;
     std::vector<sd_hog_grid> table;
     if (const int rc = sd_read_hog_grids(ctx, __func__, maps, &max_w, &max_h, &table)) return rc;
@@ -388,7 +365,7 @@ int sd_hog_windows(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int vari
             return sd_fail(ctx, SD_ERR_INVALID, "%s: window %d: grid %d out of [0, %d) or flip %d not 0 or 1", __func__, r, v.grid,
                            maps->count, v.flip);
         const int w = maps->d_grids ? table[v.grid].width : max_w, h = maps->d_grids ? table[v.grid].height : max_h;
-        const int ow = w + 2 * pad_x - filter_w + 1, oh = h + 2 * pad_y - filter_h + 1;
+        const int ow = sd_score_extent(w, pad_x, filter_w), oh = sd_score_extent(h, pad_y, filter_h);
         if (v.x < 0 || v.x >= ow || v.y < 0 || v.y >= oh)
             return sd_fail(ctx, SD_ERR_INVALID, "%s: window %d: (%d, %d) is not a score position of grid %d (%d x %d)", __func__, r, v.x,
                            v.y, v.grid, ow > 0 ? ow : 0, oh > 0 ? oh : 0);
@@ -403,14 +380,14 @@ int sd_hog_box_windows(int frame_w, int frame_h, const double* scales, int num_s
 {
     if (!scales || num_scales < 1 || num_boxes < 0 || (num_boxes > 0 && (!boxes || !out || !iou))) return SD_ERR_INVALID;
     if (frame_w < 1 || frame_h < 1 || !(positive_overlap >= 0.0 && positive_overlap <= 1.0)) return SD_ERR_INVALID;
-    if (check_filter(nullptr, __func__, filter_w, filter_h, pad_x, pad_y)) return SD_ERR_INVALID;
+    if (sd_hog_check_filter(nullptr, __func__, filter_w, filter_h, pad_x, pad_y)) return SD_ERR_INVALID;
     std::vector<Level> lv;
     if (level_table(frame_w, frame_h, scales, num_scales, cell_size, num_bins, variant, &lv)) return SD_ERR_INVALID;
     for (int b = 0; b < num_boxes; ++b)
         if (boxes[4 * b + 2] < 1 || boxes[4 * b + 3] < 1) return SD_ERR_INVALID;
     for (int b = 0; b < num_boxes; ++b) {
         const int32_t* q = boxes + 4 * b;
-        const Box64 box = {q[0], q[1], (int64_t)q[0] + q[2], (int64_t)q[1] + q[3]};
+        const sd_box64 box = {q[0], q[1], (int64_t)q[0] + q[2], (int64_t)q[1] + q[3]};
         best_window(lv, frame_w, frame_h, cell_size, filter_w, filter_h, pad_x, pad_y, positive_overlap, box, out + b, iou + b);
     }
     return SD_OK;
@@ -424,7 +401,7 @@ int sd_learn_squared_hinge(sd_ctx* ctx, const float* d_A, int64_t lda, const flo
     SD_REQUIRE(ctx, N >= 1 && D >= 2 && lda >= D, "N must be >= 1, D >= 2 and lda >= D");
     SD_REQUIRE(ctx, lambda > 0.f && std::isfinite(lambda), "lambda must be positive and finite");
     SD_REQUIRE(ctx, max_iterations >= 1, "max_iterations must be >= 1");
-    SD_REQUIRE(ctx, aligned4(d_A) && aligned4(d_y) && aligned4(d_w), "A, y and w must be 4-byte aligned");
+    SD_REQUIRE(ctx, sd_aligned(d_A, 4) && sd_aligned(d_y, 4) && sd_aligned(d_w, 4), "A, y and w must be 4-byte aligned");
     std::vector<float> y(N);
     SD_CUDA(ctx, cudaMemcpyAsync(y.data(), d_y, sizeof(float) * N, cudaMemcpyDeviceToHost, ctx->stream));
     SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -443,8 +420,8 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
                "null argument");
     SD_REQUIRE(ctx, !images->d_roi, "a batch with regions of interest has no whole frames");
     if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins, cell_size)) return rc;
-    if (const int rc = check_filter(ctx, __func__, filter_w, filter_h, pad_x, pad_y)) return rc;
-    SD_REQUIRE(ctx, aligned4(d_filter), "the filter must be 4-byte aligned");
+    if (const int rc = sd_hog_check_filter(ctx, __func__, filter_w, filter_h, pad_x, pad_y)) return rc;
+    SD_REQUIRE(ctx, sd_aligned(d_filter, 4), "the filter must be 4-byte aligned");
     SD_REQUIRE(ctx, num_scales >= 1 && images->count >= 1 && num_boxes >= 0, "need at least one scale and one frame");
     for (int s = 0; s < num_scales; ++s)
         SD_REQUIRE(ctx, h_scales[s] > 0.0 && h_scales[s] <= 4.0, "every scale must be finite and in (0, 4]");
@@ -491,7 +468,7 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
         sd_hog_window wv;
         double iou;
         best_window(lv[q.frame], fr.width, fr.height, cell_size, filter_w, filter_h, pad_x, pad_y, p->positive_overlap,
-                    Box64{q.x, q.y, (int64_t)q.x + q.w, (int64_t)q.y + q.h}, &wv, &iou);
+                    sd_box64{q.x, q.y, (int64_t)q.x + q.w, (int64_t)q.y + q.h}, &wv, &iou);
         if (wv.grid < 0) {
             ++unassigned;
             continue;
@@ -550,7 +527,7 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
         for (int f = slice0[i]; f < slice0[i + 1]; ++f)
             for (int s = 0; s < S; ++s)
                 if (lv[f][s].hog_w) {
-                    const int64_t oh = lv[f][s].hog_h + 2 * pad_y - filter_h + 1, ow = lv[f][s].hog_w + 2 * pad_x - filter_w + 1;
+                    const int64_t oh = sd_score_extent(lv[f][s].hog_h, pad_y, filter_h), ow = sd_score_extent(lv[f][s].hog_w, pad_x, filter_w);
                     if (oh > 0 && ow > 0) sc += (size_t)(oh * ow);
                 }
         max_scores = std::max(max_scores, sc);
@@ -719,7 +696,8 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
                 for (int s = 0; s < S; ++s) {
                     const int gi = grid_of[(size_t)(f - f0) * S + s];
                     if (gi < 0) continue;
-                    const int oh = std::max(0, lv[f][s].hog_h + 2 * pad_y - filter_h + 1), ow = std::max(0, lv[f][s].hog_w + 2 * pad_x - filter_w + 1);
+                    const int oh = std::max(0, sd_score_extent(lv[f][s].hog_h, pad_y, filter_h)),
+                              ow = std::max(0, sd_score_extent(lv[f][s].hog_w, pad_x, filter_w));
                     g[gi].out_offset = acc;
                     maps.push_back(sd_hog_score_map{f - f0, s, frames[f].width, frames[f].height, lv[f][s].level_w, lv[f][s].level_h, ow, oh, acc});
                     acc += (int64_t)oh * ow;
@@ -749,12 +727,12 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
             for (int f = f0; f < f1; ++f)
                 for (int k = 0; k < cnt[f - f0]; ++k) {
                     const sd_hog_detection& d = det[(size_t)(f - f0) * p->negatives_per_frame + k];
-                    const Box64 db = {d.x, d.y, (int64_t)d.x + d.w, (int64_t)d.y + d.h};
+                    const sd_box64 db = {d.x, d.y, (int64_t)d.x + d.w, (int64_t)d.y + d.h};
                     bool near_box = false;
                     for (int b : frame_boxes[f]) {
                         const sd_hog_box& q = h_boxes[b];
                         int64_t in, un;
-                        inter_union(db, Box64{q.x, q.y, (int64_t)q.x + q.w, (int64_t)q.y + q.h}, &in, &un);
+                        inter_union(db, sd_box64{q.x, q.y, (int64_t)q.x + q.w, (int64_t)q.y + q.h}, &in, &un);
                         if ((double)in > (double)p->negative_overlap * (double)un) near_box = true;
                     }
                     if (near_box) {

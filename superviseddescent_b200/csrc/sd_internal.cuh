@@ -113,6 +113,9 @@ void* sd_workspace(sd_ctx* ctx, int slot, size_t bytes);
 
 static inline int sd_div_up(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
+// whether p is a multiple of bytes (a power of two); a null pointer is aligned
+inline bool sd_aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 // ---- HOG configurations ------------------------------------------------------------------------
 
 // dd, the features per cell of vl_hog_new(variant, num_bins): 3K + 4 for UoCTTI (variant 1), 4K for Dalal-Triggs (variant 0)
@@ -133,6 +136,55 @@ inline int sd_hog_check_config(sd_ctx* ctx, const char* fn, int variant, int num
     if (cell_size < 1 || cell_size > kDenseMaxCell) return sd_fail(ctx, SD_ERR_INVALID, "%s: cell_size must be in [1,32]", fn);
     return SD_OK;
 }
+
+// The filter rule of the sliding-window calls: filter sides in [1, SD_HOG_FILTER_MAX_SIDE] and pads in [0, side - 1].  Reports
+// as sd_hog_check_config does.
+inline int sd_hog_check_filter(sd_ctx* ctx, const char* fn, int fw, int fh, int pad_x, int pad_y)
+{
+    if (fw < 1 || fw > SD_HOG_FILTER_MAX_SIDE || fh < 1 || fh > SD_HOG_FILTER_MAX_SIDE)
+        return sd_fail(ctx, SD_ERR_INVALID, "%s: filter sides must be in [1, SD_HOG_FILTER_MAX_SIDE]", fn);
+    if (pad_x < 0 || pad_x >= fw || pad_y < 0 || pad_y >= fh)
+        return sd_fail(ctx, SD_ERR_INVALID, "%s: pads must be in [0, filter side - 1]", fn);
+    return SD_OK;
+}
+
+// score positions along one axis of a grid of n cells under a filter of side f padded by pad cells: n + 2 pad - f + 1
+// (<= 0: none)
+__host__ __device__ inline int sd_score_extent(int n, int pad, int f) { return n + 2 * pad - f + 1; }
+
+// the detection box rule (include/sd_b200.h): rh(n, d) = floor((2n + d) / (2d)), n / d rounded half up, for d > 0
+__host__ __device__ inline long long sd_round_half_up(long long n, long long d)
+{
+    const long long num = 2 * n + d, den = 2 * d;
+    long long q = num / den;
+    if (num % den < 0) --q;
+    return q;
+}
+
+struct sd_box64 {
+    int64_t x0, y0, x1, y1;
+};
+
+// The pixel box of score position (x, y) of a filter of fw x fh cells, padded by (pad_x, pad_y), at a level of level_w x level_h
+// px of a frame_w x frame_h frame: the cells' pixels scaled back to the frame, x0 = rh((x - pad_x) cell frame_w, level_w),
+// x1 = rh((x - pad_x + fw) cell frame_w, level_w), y alike.  The boxes of sd_hog_detections, of the part placements and of
+// sd_hog_box_windows are all this one.
+__host__ __device__ inline sd_box64 sd_window_box(int x, int y, int pad_x, int pad_y, int fw, int fh, int cell, int frame_w, int frame_h,
+                                                  int level_w, int level_h)
+{
+    const long long sx = (long long)cell * frame_w, sy = (long long)cell * frame_h;
+    sd_box64 b;
+    b.x0 = sd_round_half_up((long long)(x - pad_x) * sx, level_w);
+    b.x1 = sd_round_half_up((long long)(x - pad_x + fw) * sx, level_w);
+    b.y0 = sd_round_half_up((long long)(y - pad_y) * sy, level_h);
+    b.y1 = sd_round_half_up((long long)(y - pad_y + fh) * sy, level_h);
+    return b;
+}
+
+// whether every box sd_window_box gives a map of width x height score positions fits in int32, its numerators in int64 with
+// room to spare (sd_hog_detect.cu); a map without positions has no boxes
+bool sd_window_boxes_fit_int32(int width, int height, int pad_x, int pad_y, int fw, int fh, int cell, int frame_w, int frame_h,
+                               int level_w, int level_h);
 
 // a device descriptor table of count entries, read back to the host once
 template <class T>
@@ -257,6 +309,19 @@ inline size_t sd_round16(size_t v) { return (v + 15) & ~(size_t)15; }
 inline size_t sd_gray_bytes(const sd_host_frame& f) { return (size_t)f.height * sd_round16(f.width); }
 
 #ifdef __CUDACC__
+// The last index i in [lo, hi] whose start(i) <= t, for starts that ascend with i and start(lo) <= t: the grid, map or level that
+// work item t of a flattened launch belongs to.  start is the caller's load of a table entry.
+template <class T, class Start>
+__device__ __forceinline__ int sd_find_last_le(int lo, int hi, T t, Start start)
+{
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (start(mid) <= t) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
 // Inter-eye distance exactly as helpers.hpp:136-160 evaluates it: eye centres are float sums
 // scaled by the float reciprocal of the count (cv::Vec /= float), the difference is taken in float,
 // squares are accumulated in double (cv::norm NORM_L2) and the root is a double sqrt.

@@ -83,6 +83,19 @@ inline sd_image_batch upload_grey(sd_ctx* ctx, const std::vector<sd_host_frame>&
     return batch;
 }
 
+// The output of one sd_hog_detections call on the host: the n frames' max(max_detections, 1) slots each into out; returns each
+// frame's detection count.  Copies queued on the stream before the call are complete when it returns.
+inline std::vector<int32_t> download_detections(sd_ctx* ctx, const sd_b200::DeviceBuffer& d_out, const sd_b200::DeviceBuffer& d_count,
+                                                int n, int max_detections, std::vector<sd_hog_detection>& out, const char* what)
+{
+    out.resize(static_cast<size_t>(n) * static_cast<size_t>(std::max(max_detections, 1)));
+    std::vector<int32_t> count(n);
+    sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.data(), d_out.as<void>(), out.size() * sizeof(sd_hog_detection)), what);
+    sd_b200::check(ctx, sd_memcpy_d2h(ctx, count.data(), d_count.as<void>(), count.size() * sizeof(int32_t)), what);
+    sd_b200::check(ctx, sd_sync(ctx), what);
+    return count;
+}
+
 // CV_8UC1 or CV_32FC1 planes of elem_size bytes per element (row steps allowed) packed end to end into buf, in the order
 // given; returns where each plane starts, in elements
 inline std::vector<int64_t> pack_planes(sd_ctx* ctx, const std::vector<cv::Mat>& planes, size_t elem_size, sd_b200::DeviceBuffer& buf,
@@ -392,6 +405,8 @@ struct hog_detection {
     int cell_x, cell_y;
 };
 
+inline hog_detection to_hog_detection(const sd_hog_detection& r) { return {cv::Rect(r.x, r.y, r.w, r.h), r.score, r.filter, r.level, r.cell_x, r.cell_y}; }
+
 // A sliding-window detector over image pyramids: vl_hog_pyramid of every frame, vl_hog_correlate of the filter bank on every
 // level, then sd_hog_detections over all score maps (the scores above threshold, their boxes in frame pixels, the first
 // max_candidates of each frame by score, and greedy non-maximum suppression at IoU overlap over all filters as one class).
@@ -442,17 +457,11 @@ inline std::vector<std::vector<hog_detection>> vl_hog_detect(const std::vector<c
     sd_b200::check(ctx, sd_hog_detections(ctx, d_scores.as<float>(), d_table.as<sd_hog_score_map>(), static_cast<int>(table.size()), n, Q,
                                           cell_size, fw, fh, pad_x, pad_y, threshold, overlap, max_candidates, max_detections,
                                           d_out.as<sd_hog_detection>(), d_count.as<int32_t>(), nullptr), "sd_hog_detections");
-    std::vector<sd_hog_detection> out(slots);
-    std::vector<int32_t> count(n);
-    sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.data(), d_out.as<void>(), slots * sizeof(sd_hog_detection)), "vl_hog_detect download");
-    sd_b200::check(ctx, sd_memcpy_d2h(ctx, count.data(), d_count.as<void>(), count.size() * sizeof(int32_t)), "vl_hog_detect download");
-    sd_b200::check(ctx, sd_sync(ctx), "vl_hog_detect download");
+    std::vector<sd_hog_detection> out;
+    const std::vector<int32_t> count = hog_batch::download_detections(ctx, d_out, d_count, n, max_detections, out, "vl_hog_detect download");
     std::vector<std::vector<hog_detection>> result(n);
     for (int i = 0; i < n; ++i)
-        for (int k = 0; k < count[i]; ++k) {
-            const sd_hog_detection& r = out[static_cast<size_t>(i) * max_detections + k];
-            result[i].push_back(hog_detection{cv::Rect(r.x, r.y, r.w, r.h), r.score, r.filter, r.level, r.cell_x, r.cell_y});
-        }
+        for (int k = 0; k < count[i]; ++k) result[i].push_back(to_hog_detection(out[static_cast<size_t>(i) * max_detections + k]));
     return result;
 }
 
@@ -640,19 +649,15 @@ inline std::vector<std::vector<hog_part_detection>> vl_hog_part_detect(const std
     sd_b200::check(ctx, sd_hog_part_placements(ctx, d_raw.as<float>(), d_table.as<sd_hog_part_map>(), nm, &m, deformation.data(),
                                                model.max_displacement, cell_size, d_out.as<sd_hog_detection>(), d_count.as<int32_t>(), n,
                                                max_detections, d_parts.as<sd_hog_part_placement>()), "sd_hog_part_placements");
-    std::vector<sd_hog_detection> out(slots);
     std::vector<sd_hog_part_placement> parts(slots * P);
-    std::vector<int32_t> count(n);
-    sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.data(), d_out.as<void>(), slots * sizeof(sd_hog_detection)), "vl_hog_part_detect download");
     sd_b200::check(ctx, sd_memcpy_d2h(ctx, parts.data(), d_parts.as<void>(), parts.size() * sizeof(sd_hog_part_placement)), "vl_hog_part_detect download");
-    sd_b200::check(ctx, sd_memcpy_d2h(ctx, count.data(), d_count.as<void>(), count.size() * sizeof(int32_t)), "vl_hog_part_detect download");
-    sd_b200::check(ctx, sd_sync(ctx), "vl_hog_part_detect download");
+    std::vector<sd_hog_detection> out;
+    const std::vector<int32_t> count = hog_batch::download_detections(ctx, d_out, d_count, n, max_detections, out, "vl_hog_part_detect download");
     std::vector<std::vector<hog_part_detection>> result(n);
     for (int i = 0; i < n; ++i)
         for (int k = 0; k < count[i]; ++k) {
             const size_t slot = static_cast<size_t>(i) * max_detections + k;
-            const sd_hog_detection& r = out[slot];
-            hog_part_detection det{hog_detection{cv::Rect(r.x, r.y, r.w, r.h), r.score, r.filter, r.level, r.cell_x, r.cell_y}, {}};
+            hog_part_detection det{to_hog_detection(out[slot]), {}};
             for (int p = 0; p < P; ++p) {
                 const sd_hog_part_placement& pp = parts[slot * P + p];
                 det.parts.push_back(hog_part{cv::Rect(pp.x, pp.y, pp.w, pp.h), pp.u, pp.v, pp.term});

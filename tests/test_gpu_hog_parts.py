@@ -254,6 +254,7 @@ def test_refusals_write_nothing(sd):
     table = sd._device_table([row], "cuda:0")
     dup = sd._device_table([row, row], "cuda:0")
     neg = sd._device_table([HogPartMapC(0, 0, 64, 64, 64, 64, 3, -1, 8, 8, 0, 0, 0)], "cuda:0")
+    wide = sd._device_table([HogPartMapC(0, 0, 1 << 30, 64, 1, 64, 3, 3, 8, 8, 0, 0, 0)], "cuda:0")   # part boxes past int32
 
     def ps(m, t=table, n=1):
         return lib.sd_hog_part_scores(ctx.h, ptr(root), ptr(parts), ptr(t), n, C.byref(m), ptr(total))
@@ -278,7 +279,8 @@ def test_refusals_write_nothing(sd):
         return lib.sd_hog_part_placements(ctx.h, ptr(parts), ptr(t), n, C.byref(m), C.c_void_p(dp.ctypes.data), R, CS, ptr(det),
                                           ptr(cnt), 1, md, ptr(out_p))
 
-    for rc in (pp(t=dup, n=2), pp(cnt=count2), pp(R=33), pp(d=np.full((6, 4), np.nan)), pp(m=model(P=0)), pp(md=0), pp(t=neg)):
+    for rc in (pp(t=dup, n=2), pp(cnt=count2), pp(R=33), pp(d=np.full((6, 4), np.nan)), pp(m=model(P=0)), pp(md=0), pp(t=neg),
+               pp(t=wide)):
         assert rc != 0
     torch.cuda.synchronize()
     assert torch.all(out_p == -99)
