@@ -240,7 +240,8 @@ SD_API int sd_hog_pyramid_shape(int width, int height, double scale, int cell_si
  * and colour frames reach the device through sd_upload_frames.  The resized levels go through context scratch, one slice of
  * the batch at a time (about 64 MB of levels per slice), so the scratch does not grow with the batch.  Each level's features
  * depend on its frame and scale alone.  Null pointers, a batch with d_roi, num_scales < 1, an invalid scale or configuration,
- * or a frame smaller than 1 x 1 is SD_ERR_INVALID before any work is queued (d_out is not written). */
+ * or a frame smaller than 1 x 1 is SD_ERR_INVALID before any work is queued (d_out is not written).  sd_hog_pyramid_images
+ * (below sd_hog_dense_images) keeps a frame's channels instead of taking grey frames. */
 SD_API int sd_hog_pyramid(sd_ctx* ctx, const sd_image_batch* images, const double* h_scales, int num_scales,
                           int cell_size, int num_bins, int variant, float* d_out, const int64_t* d_out_offset);
 
@@ -276,6 +277,20 @@ typedef struct {
  * invalid configuration is SD_ERR_INVALID before any work is queued (d_out is not written). */
 SD_API int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size, int num_bins, int variant,
                                int bilinear_orientations, float* d_out, const int64_t* d_out_offset);
+/* sd_hog_pyramid_images: sd_hog_pyramid of 8-bit frames with 1..16 channels, asynchronous on the context's stream.  Frames are an
+ * sd_hog_images with dtype SD_HOG_U8, in any layout it describes (planar, interleaved, strided; equally sized or per-frame
+ * d_frames, whose table the call reads back once).  Level sizes, empty levels, scale limits, output layout and offsets are
+ * exactly sd_hog_pyramid's (sd_hog_pyramid_shape gives the shape; channels do not change it).  Each channel is resized on its
+ * own by sd_hog_pyramid's 8-bit INTER_LINEAR rule; for 1, 3 and 4 channels that is cv::resize of the whole frame, for other
+ * counts cv::resize may differ by 1 at exact 2x downscales.  Each level's features are bit for bit sd_hog_dense_images' of
+ * the resized level with the same channels and bilinear_orientations: at each pixel the channel with the largest gradient
+ * votes, the first on a tie.  The levels go through context scratch one slice of the batch at a time, as in sd_hog_pyramid.
+ * Null pointers, a dtype other than SD_HOG_U8, channels outside [1, 16], bilinear_orientations outside {0, 1}, num_scales < 1,
+ * an invalid scale or configuration, a frame smaller than 1 x 1, or a negative offset or stride is SD_ERR_INVALID before any
+ * work is queued (d_out is not written). */
+SD_API int sd_hog_pyramid_images(sd_ctx* ctx, const sd_hog_images* images, const double* h_scales, int num_scales,
+                                 int cell_size, int num_bins, int variant, int bilinear_orientations,
+                                 float* d_out, const int64_t* d_out_offset);
 
 /* ---- dense HOG of a caller's gradient fields: vl_hog_put_polar_field + vl_hog_extract (hog.c:746-845, :857-1062) ----------
  * Each field is a modulus and an angle per pixel, e.g. the gradient of another operator, colour gradients combined by the
@@ -497,7 +512,7 @@ SD_API int sd_learn_squared_hinge(sd_ctx* ctx, const float* d_A, int64_t lda, co
  * range or whose w or h < 1, lambda <= 0, overlaps outside [0, 1], flip_positives outside {0, 1}, rounds < 0, negatives_per_frame
  * outside [1, SD_HOG_DETECT_MAX_CANDIDATES], max_negatives < 1, max_iterations < 1, D above SD_HOG_TRAIN_MAX_DIM or no assigned
  * box is SD_ERR_INVALID, and rows, Gram and one slice that would not fit in device memory SD_ERR_CUDA, before any work is
- * queued. */
+ * queued.  sd_hog_train_filter_images (below) trains on frames that keep their channels. */
 #define SD_HOG_TRAIN_MAX_DIM 8192   /* D = dd * fh * fw + 1: 31 x 16 x 16 + 1 = 7937 fits; the Gram is 256 MB at the cap */
 typedef struct {
     int32_t frame, x, y, w, h;
@@ -535,6 +550,15 @@ SD_API int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const 
                                const double* h_scales, int num_scales, int cell_size, int num_bins, int variant, int filter_w,
                                int filter_h, int pad_x, int pad_y, const sd_hog_train_param* p, float* d_filter, float* h_bias,
                                sd_hog_train_report* h_rounds, sd_hog_window* h_negatives, int* h_num_negatives);
+/* sd_hog_train_filter_images: sd_hog_train_filter with the same arguments, rule, report and output, on frames that keep their
+ * channels: an sd_hog_images of 8-bit frames with 1..16 channels, whose pyramids are sd_hog_pyramid_images' with
+ * bilinear_orientations.  A filter trained so is scored on the same features: sd_hog_pyramid_images with the same channels and
+ * bilinear_orientations.  A dtype other than SD_HOG_U8, channels outside [1, 16], bilinear_orientations outside {0, 1} or a
+ * negative offset or stride is SD_ERR_INVALID as well. */
+SD_API int sd_hog_train_filter_images(sd_ctx* ctx, const sd_hog_images* images, int bilinear_orientations, const sd_hog_box* h_boxes,
+                                      int num_boxes, const double* h_scales, int num_scales, int cell_size, int num_bins, int variant,
+                                      int filter_w, int filter_h, int pad_x, int pad_y, const sd_hog_train_param* p, float* d_filter,
+                                      float* h_bias, sd_hog_train_report* h_rounds, sd_hog_window* h_negatives, int* h_num_negatives);
 
 /* ---- deformable part models: bounded distance transforms, star-model scores and the part boxes of each detection -----------
  * A star model has Q components.  Component q is a root filter (filter_w x filter_h cells) scored on a level of scale s, and P

@@ -517,8 +517,22 @@ def vl_hog(images, cell_size: int, num_bins: int, variant: int = 1, bilinear_ori
     Returns one (count, dd, hogH, hogW) float32 CUDA tensor when all frames have one size, else a list of (dd, hogH, hogW)
     tensors."""
     ctx = ctx or default_context()
-    dev = f"cuda:{ctx.device}"
     lib = _capi.lib()
+    keep, ib, sizes = _hog_images(images, channels_last, ctx, lambda w, h: hog_dense_shape(w, h, cell_size, num_bins, variant))
+    if ib is None:
+        return []
+    bil = int(bool(bilinear_orientations))
+    return _dense_results(ctx, sizes, None if ib.d_frames else (ib.frame.height, ib.frame.width), cell_size, num_bins, variant,
+                          lambda out, offsets: _check(ctx.h, lib.sd_hog_dense_images(ctx.h, C.byref(ib), int(cell_size), int(num_bins),
+                                                                                     int(variant), bil, ptr(out), ptr(offsets))))
+
+
+def _hog_images(images, channels_last: bool, ctx: Context, check):
+    """The frames of vl_hog, or of the multichannel=True route of the sliding-window calls -> (what owns their device bytes,
+    their HogImagesC, [(H, W)] per frame).  A batch is read through its strides (a CUDA tensor in place, a host one after one
+    copy); a list of frames is packed end to end in one device buffer after check(W, H) has accepted every size, with a
+    descriptor table when the sizes differ.  An empty list gives (None, None, [])."""
+    dev = f"cuda:{ctx.device}"
 
     def dtype_of(t):
         if t.dtype not in _VL_HOG_DTYPES:
@@ -530,7 +544,7 @@ def vl_hog(images, cell_size: int, num_bins: int, variant: int = 1, bilinear_ori
     if isinstance(images, (list, tuple)):
         frames = [_tensor(f) for f in images]
         if not frames:
-            return []
+            return None, None, []
         if any(f.dim() not in (2, 3) for f in frames):
             raise ValueError("every frame of a list must be (H, W), (C, H, W), or (H, W, C) with channels_last=True")
         if len({f.dtype for f in frames}) != 1:
@@ -542,30 +556,29 @@ def vl_hog(images, cell_size: int, num_bins: int, variant: int = 1, bilinear_ori
             raise ValueError("all frames must have one number of channels")
         sizes = [(d.height, d.width) for _, d in descs]
         for h, w in set(sizes):
-            hog_dense_shape(w, h, cell_size, num_bins, variant)   # refuse before the upload
-        keep, offsets = _pack(frames, dev)
+            check(w, h)                                       # refuse before the upload
+        data, offsets = _pack(frames, dev)
         for (_, d), o in zip(descs, offsets):
             d.offset = o
         ib.channels, ib.count = descs[0][0], len(frames)
+        keep = data
         if len(set(sizes)) == 1:
             ib.frame, ib.image_stride = descs[0][1], frames[0].numel()
         else:
-            keep_table = _device_table([d for _, d in descs], dev)
-            ib.d_frames = keep_table.data_ptr()
+            table = _device_table([d for _, d in descs], dev)
+            ib.d_frames = table.data_ptr()
+            keep = (data, table)
     else:
         t = _tensor(images)
         if t.dim() not in (3, 4):
             raise ValueError("a batch of frames must be (count, H, W), (count, C, H, W), or (count, H, W, C) with channels_last=True")
         dt = dtype_of(t)
-        keep = t.to(dev)
-        ib.channels, ib.frame = _vl_hog_frame(keep, channels_last, True)
-        ib.count, ib.image_stride = keep.shape[0], keep.stride(0)
+        data = keep = t.to(dev)
+        ib.channels, ib.frame = _vl_hog_frame(data, channels_last, True)
+        ib.count, ib.image_stride = data.shape[0], data.stride(0)
         sizes = [(ib.frame.height, ib.frame.width)] * ib.count
-    ib.d_data, ib.dtype = keep.data_ptr(), dt
-    bil = int(bool(bilinear_orientations))
-    return _dense_results(ctx, sizes, None if ib.d_frames else (ib.frame.height, ib.frame.width), cell_size, num_bins, variant,
-                          lambda out, offsets: _check(ctx.h, lib.sd_hog_dense_images(ctx.h, C.byref(ib), int(cell_size), int(num_bins),
-                                                                                     int(variant), bil, ptr(out), ptr(offsets))))
+    ib.d_data, ib.dtype = data.data_ptr(), dt
+    return keep, ib, sizes
 
 
 # The distinct frames of a HogTransform are uploaded when their grey bytes fit in this share of the device's free memory (read when
@@ -1529,22 +1542,30 @@ def hog_pyramid_shape(width: int, height: int, scale: float, cell_size: int, num
     return (lw, lh), (d, h, w)
 
 
-def vl_hog_pyramid(frames, scales, cell_size: int, num_bins: int, variant: int = 1, ctx: Optional[Context] = None):
+def vl_hog_pyramid(frames, scales, cell_size: int, num_bins: int, variant: int = 1, ctx: Optional[Context] = None,
+                   multichannel: bool = False, bilinear_orientations: bool = False):
     """Dense HOG of every frame at every scale in one call (sd_hog_pyramid): level s of a W x H frame is the frame resized by
     cv::resize INTER_LINEAR to floor(W * s + 0.5) x floor(H * s + 0.5), and its features are hog_dense's of that level.
 
-    frames: as hog_dense takes them.  Returns (features, sizes): features[f][s] is a (dd, hogH, hogW) float32 CUDA view into
-    one buffer, or None for an empty level (smaller than 4 px or than half a cell); sizes[f][s] = (level_w, level_h)."""
+    frames: as hog_dense takes them: colour frames are converted to grey.  multichannel=True keeps the channels
+    (sd_hog_pyramid_images): frames are uint8, channels last -- a host or CUDA (count, H, W) or (count, H, W, C) array or tensor
+    (CUDA tensors read in place through their strides), or a list of (H, W) or (H, W, C) frames of any sizes with one C -- each
+    channel is resized on its own, and at each pixel the channel with the largest gradient votes, as vl_hog does;
+    bilinear_orientations (multichannel only): every pixel votes into its two nearest orientation bins.  Returns (features,
+    sizes): features[f][s] is a (dd, hogH, hogW) float32 CUDA view into one buffer, or None for an empty level (smaller than
+    4 px or than half a cell); sizes[f][s] = (level_w, level_h)."""
     ctx = ctx or default_context()
     scales = [float(s) for s in scales]
     if not scales:
         raise ValueError("vl_hog_pyramid needs at least one scale")
+    if bilinear_orientations and not multichannel:
+        raise ValueError("bilinear_orientations needs multichannel=True (grey frames pass as they are)")
 
     def check(w, h):
         for s in scales:
             hog_pyramid_shape(w, h, s, cell_size, num_bins, variant)
 
-    keep, ib, sizes = _grey_frames(frames, ctx, check)
+    keep, ib, sizes = _hog_images(frames, True, ctx, check) if multichannel else _grey_frames(frames, ctx, check)
     if not sizes:
         return [], []
     levels = [[hog_pyramid_shape(w, h, s, cell_size, num_bins, variant) for s in scales] for h, w in sizes]
@@ -1552,8 +1573,12 @@ def vl_hog_pyramid(frames, scales, cell_size: int, num_bins: int, variant: int =
     out, offsets, feats = _results([shape if shape[1] else None for row in levels for _, shape in row], dev)
     d_off = torch.tensor(offsets, dtype=torch.int64, device=dev)
     h_scales = (C.c_double * len(scales))(*scales)
-    _check(ctx.h, _capi.lib().sd_hog_pyramid(ctx.h, C.byref(ib), h_scales, len(scales), int(cell_size), int(num_bins), int(variant),
-                                             ptr(out), ptr(d_off)))
+    if multichannel:
+        _check(ctx.h, _capi.lib().sd_hog_pyramid_images(ctx.h, C.byref(ib), h_scales, len(scales), int(cell_size), int(num_bins),
+                                                        int(variant), int(bool(bilinear_orientations)), ptr(out), ptr(d_off)))
+    else:
+        _check(ctx.h, _capi.lib().sd_hog_pyramid(ctx.h, C.byref(ib), h_scales, len(scales), int(cell_size), int(num_bins),
+                                                 int(variant), ptr(out), ptr(d_off)))
     S = len(scales)
     return [feats[i:i + S] for i in range(0, len(feats), S)], [[lv for lv, _ in row] for row in levels]
 
@@ -1600,12 +1625,13 @@ cell (n, 2) int32 (the score position x, y in its level), and above (num_frames,
 
 def vl_hog_detect(frames, scales, filters, cell_size: int, num_bins: int, threshold: float, variant: int = 1, bias=None, pad=(0, 0),
                   overlap: float = 0.5, max_candidates: int = 4096, max_detections: int = 256,
-                  ctx: Optional[Context] = None) -> HogDetections:
+                  ctx: Optional[Context] = None, multichannel: bool = False, bilinear_orientations: bool = False) -> HogDetections:
     """A sliding-window detector over image pyramids: vl_hog_pyramid of every frame at every scale, vl_hog_correlate of the
     filter bank on every level (read in place), and one sd_hog_detections call over all score maps: the scores above threshold,
     their boxes in frame pixels, the first max_candidates of each frame by score, and greedy non-maximum suppression at IoU
-    overlap over all filters as one class, up to max_detections per frame.  frames, scales, filters, bias and pad as
-    vl_hog_pyramid and vl_hog_correlate take them.  Returns HogDetections; detect_faces(frames, d.frame, boxes=d.boxes) takes
+    overlap over all filters as one class, up to max_detections per frame.  frames, scales, filters, bias, pad, multichannel
+    and bilinear_orientations as vl_hog_pyramid and vl_hog_correlate take them; filters trained with multichannel or
+    bilinear_orientations are scored with the same.  Returns HogDetections; detect_faces(frames, d.frame, boxes=d.boxes) takes
     the result as it is."""
     ctx = ctx or default_context()
     f = _tensor(filters)
@@ -1613,7 +1639,8 @@ def vl_hog_detect(frames, scales, filters, cell_size: int, num_bins: int, thresh
         raise ValueError("filters must be a (Q, dd, fh, fw) tensor")
     q, _, fh, fw = f.shape
     pad_x, pad_y = (int(p) for p in pad)
-    feats, levels = vl_hog_pyramid(frames, scales, cell_size, num_bins, variant, ctx=ctx)
+    feats, levels = vl_hog_pyramid(frames, scales, cell_size, num_bins, variant, ctx=ctx, multichannel=multichannel,
+                                   bilinear_orientations=bilinear_orientations)
     n = len(feats)
     if n == 0:
         return _detections(None, None, None)[0]
@@ -1770,18 +1797,21 @@ HogFilter.__doc__ = """Result of train_hog_filter: filter (dd, fh, fw) float32 C
 array of the negative cache in slot order (frame, level, x, y), and report, one dict per mining round (the fields of
 sd_hog_train_report, the solve as an SvmReport, or None when the round's solve was skipped; times_ms, the round's phases in
 milliseconds, and gathered_bytes).  positive_overlap reaches the library as a float: the positives are hog_box_windows(...,
-positive_overlap=float(np.float32(positive_overlap)))."""
+positive_overlap=float(np.float32(positive_overlap))).  The filter is one for the features it was trained on: one trained with
+multichannel or bilinear_orientations is scored by vl_hog_detect with the same values."""
 
 
 def train_hog_filter(frames, box_frame, boxes, scales, filter_size, cell_size: int, num_bins: int, variant: int = 1, pad=(0, 0),
                      lam: float = 0.01, positive_overlap: float = 0.5, negative_overlap: float = 0.3, flip_positives: bool = False,
                      rounds: int = 3, negatives_per_frame: int = 32, mine_overlap: float = 0.5, max_negatives: int = 8192,
-                     max_iterations: int = 50, ctx: Optional[Context] = None) -> HogFilter:
+                     max_iterations: int = 50, ctx: Optional[Context] = None, multichannel: bool = False,
+                     bilinear_orientations: bool = False) -> HogFilter:
     """Train a HOG filter for vl_hog_detect (sd_hog_train_filter): each box's best window as a positive (hog_box_windows, with
     its mirror if flip_positives), round 0 with the mean positive minus its mean as the filter, then `rounds` rounds of
-    hard-negative mining at the margin (threshold -1) and a squared-hinge SVM (learn_squared_hinge) each.  frames as
-    vl_hog_pyramid takes them; box_frame (n,) and boxes (n, 4) (x, y, w, h) in the layout of HogDetections.
-    vl_hog_detect(frames, scales, hf.filter[None], ..., bias=[hf.bias]) takes the result as it is."""
+    hard-negative mining at the margin (threshold -1) and a squared-hinge SVM (learn_squared_hinge) each.  frames,
+    multichannel and bilinear_orientations as vl_hog_pyramid takes them (multichannel: sd_hog_train_filter_images); box_frame
+    (n,) and boxes (n, 4) (x, y, w, h) in the layout of HogDetections.  vl_hog_detect(frames, scales, hf.filter[None], ...,
+    bias=[hf.bias]) with the same multichannel and bilinear_orientations takes the result as it is."""
     ctx = ctx or default_context()
     dd = _hog_dims(num_bins, variant)
     fw, fh = (int(v) for v in filter_size)
@@ -1789,12 +1819,14 @@ def train_hog_filter(frames, box_frame, boxes, scales, filter_size, cell_size: i
     scales = [float(s) for s in scales]
     if not scales:
         raise ValueError("train_hog_filter needs at least one scale")
+    if bilinear_orientations and not multichannel:
+        raise ValueError("bilinear_orientations needs multichannel=True (grey frames pass as they are)")
 
     def check(w, h):
         for s in scales:
             hog_pyramid_shape(w, h, s, cell_size, num_bins, variant)
 
-    keep, ib, sizes = _grey_frames(frames, ctx, check)
+    keep, ib, sizes = _hog_images(frames, True, ctx, check) if multichannel else _grey_frames(frames, ctx, check)
     if not sizes:
         raise ValueError("train_hog_filter needs at least one frame")
     bf = np.asarray(box_frame, np.int64).reshape(-1)
@@ -1812,9 +1844,13 @@ def train_hog_filter(frames, box_frame, boxes, scales, filter_size, cell_size: i
     negs = (HogWindowC * max(int(max_negatives), 1))()
     nn = C.c_int(0)
     sc = (C.c_double * len(scales))(*scales)
-    _check(ctx.h, _capi.lib().sd_hog_train_filter(ctx.h, C.byref(ib), hb, nb, sc, len(scales), int(cell_size), int(num_bins),
-                                                  int(variant), fw, fh, pad_x, pad_y, C.byref(prm), ptr(filt), C.byref(bias), reps,
-                                                  negs, C.byref(nn)))
+    lib = _capi.lib()
+    rest = (hb, nb, sc, len(scales), int(cell_size), int(num_bins), int(variant), fw, fh, pad_x, pad_y, C.byref(prm), ptr(filt),
+            C.byref(bias), reps, negs, C.byref(nn))
+    if multichannel:
+        _check(ctx.h, lib.sd_hog_train_filter_images(ctx.h, C.byref(ib), int(bool(bilinear_orientations)), *rest))
+    else:
+        _check(ctx.h, lib.sd_hog_train_filter(ctx.h, C.byref(ib), *rest))
     S = len(scales)
     neg = np.array([(negs[k].grid // S, negs[k].grid % S, negs[k].x, negs[k].y) for k in range(nn.value)], np.int32).reshape(-1, 4)
     report = []
@@ -1838,7 +1874,9 @@ class HogPartModel:
     """A star model of Q components for vl_hog_part_detect: root (Q, dd, fh, fw) filters with bias (Q,), parts (Q, P, dd, pfh, pfw)
     filters scored at twice the root's resolution, anchors (Q, P, 2) int (ax, ay) in part-level cells relative to twice the root
     window's top-left cell, deformation (Q, P, 4) (w0, w1, w2, w3): a displacement (dx, dy) costs w0 dx^2 + w1 dx + w2 dy^2 + w3 dy,
-    pad = (pad_x, pad_y) of the root correlate, part_pad of the part correlate, and max_displacement R bounding |dx| and |dy|."""
+    pad = (pad_x, pad_y) of the root correlate, part_pad of the part correlate, and max_displacement R bounding |dx| and |dy|.
+    The filters are ones for the features they were trained on: a model of colour HOG (vl_hog_pyramid's multichannel and
+    bilinear_orientations) is scored by vl_hog_part_detect with the same values."""
 
     def __init__(self, root, bias, parts, anchors, deformation, pad=(0, 0), part_pad=(0, 0), max_displacement: int = 4):
         self.root = _tensor(root).to(torch.float32).contiguous()
@@ -1981,13 +2019,15 @@ score positions ((-1, -1) for none) and part_scores (n, P) float32, each part's 
 
 def vl_hog_part_detect(frames, scales, model: HogPartModel, cell_size: int, num_bins: int, threshold: float, variant: int = 1,
                        overlap: float = 0.5, max_candidates: int = 4096, max_detections: int = 256,
-                       ctx: Optional[Context] = None) -> HogPartDetections:
+                       ctx: Optional[Context] = None, multichannel: bool = False,
+                       bilinear_orientations: bool = False) -> HogPartDetections:
     """A star-model detector over image pyramids: one vl_hog_pyramid over the root scales and their doubles (a scale present in
     both is computed once; root scales must be <= 2), vl_hog_correlate of the root filters (bias included) on the root levels and
     of all Q * P part filters on the part levels, each read in place; vl_hog_distance_transform of the part maps; the star
     model's scores (vl_hog_part_scores); sd_hog_detections over them with the root's filter size and pad, all components as one
-    class; and the part placements of every detection (sd_hog_part_placements).  One host read-back at the end.  Returns
-    HogPartDetections; detect_faces(frames, d.frame, boxes=d.boxes) takes the result as it is."""
+    class; and the part placements of every detection (sd_hog_part_placements).  One host read-back at the end.  frames,
+    multichannel and bilinear_orientations as vl_hog_pyramid takes them.  Returns HogPartDetections; detect_faces(frames,
+    d.frame, boxes=d.boxes) takes the result as it is."""
     ctx = ctx or default_context()
     dev = f"cuda:{ctx.device}"
     q, p, dd, pfh, pfw = model.parts.shape
@@ -1999,7 +2039,8 @@ def vl_hog_part_detect(frames, scales, model: HogPartModel, cell_size: int, num_
         raise ValueError("vl_hog_part_detect needs root scales in (0, 2]")
     every = list(dict.fromkeys(scales + [2 * s for s in scales]))
     ri, pi = [every.index(s) for s in scales], [every.index(2 * s) for s in scales]
-    feats, levels = vl_hog_pyramid(frames, every, cell_size, num_bins, variant, ctx=ctx)
+    feats, levels = vl_hog_pyramid(frames, every, cell_size, num_bins, variant, ctx=ctx, multichannel=multichannel,
+                                   bilinear_orientations=bilinear_orientations)
     n = len(feats)
     if n == 0:
         return _part_detections(_detections(None, None, None), np.zeros((0, 1, p, len(HogPartPlacementC._fields_)), np.int32))

@@ -668,6 +668,138 @@ __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_kernel(cons
     }
 }
 
+// ---- the pyramid of 8-bit frames with C channels (sd_hog_pyramid_images): each channel resized on its own by the rule above,
+//      every level written interleaved ((H, W, C), rows at a pitch of C * w rounded up to 16 bytes) into scratch, then all of
+//      them through hog_images_kernel as one batch of sd_hog_image descriptors
+struct PyrImageLevel {
+    long long src;               // element offset of the frame's pixel (0, 0, 0) from the batch's data
+    long long rs, ps, chs;       // the frame's row, pixel and channel strides in elements
+    long long dst;               // byte offset of the level from the scratch
+    int W, H;                    // the frame
+    int w, h, pitch;             // the level: size and row stride in bytes
+    int tile0, tiles_x;
+    int slot;
+};
+
+struct ResizeImagesArgs {
+    const uint8_t* images;
+    uint8_t* scratch;
+    const PyrImageLevel* levels;
+    int count, channels;
+    const int64_t* out_offset;
+    int64_t* level_offset;
+};
+
+// One CTA per kResizeW x kResizeH pixel tile of one level, as hog_pyramid_resize_kernel: the taps of its columns and rows once,
+// then every channel of every pixel with the channel fastest, so that a warp writes consecutive bytes of the level.
+__global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kernel(const __grid_constant__ ResizeImagesArgs a)
+{
+    __shared__ int s_sx[kResizeW], s_xw[kResizeW], s_y0[kResizeH], s_y1[kResizeH], s_yw[kResizeH];
+    const int b = blockIdx.x, tid = threadIdx.x, C = a.channels;
+    const int lo = sd_find_last_le(0, a.count - 1, b, [&](int i) { return a.levels[i].tile0; });
+    const PyrImageLevel L = a.levels[lo];
+    const int t = b - L.tile0, ty = t / L.tiles_x;
+    const int x0 = (t - ty * L.tiles_x) * kResizeW, y0 = ty * kResizeH;
+    if (t == 0 && tid == 0) a.level_offset[lo] = a.out_offset[L.slot];
+    const uint8_t* __restrict__ src = a.images + L.src;
+    uint8_t* __restrict__ dst = a.scratch + L.dst;
+    const bool copy = L.w == L.W && L.h == L.H;
+    if (!copy) {
+        if (tid < kResizeW) {
+            if (x0 + tid < L.w) {
+                const HogResizeTap r = hog_resize_tap(x0 + tid, L.w, L.W);
+                s_sx[tid] = r.sx;
+                s_xw[tid] = r.xw;
+            }
+        } else if (tid < kResizeW + kResizeH) {
+            const int i = tid - kResizeW;
+            if (y0 + i < L.h) {
+                const HogResizeTap r = hog_resize_tap(y0 + i, L.h, L.H);
+                s_y0[i] = r.y0;
+                s_y1[i] = r.y1;
+                s_yw[i] = r.yw;
+            }
+        }
+        __syncthreads();
+    }
+    const int row = kResizeW * C;
+    for (int i = tid; i < row * kResizeH; i += kResizeThreads) {
+        const int r = i / row, j = i - r * row;
+        const int c = j / C, ch = j - c * C;
+        const int x = x0 + c, y = y0 + r;
+        if (x >= L.w || y >= L.h) continue;
+        const uint8_t* s = src + ch * L.chs;
+        int v;
+        if (copy) {
+            v = __ldg(s + y * L.rs + x * L.ps);
+        } else {
+            const int sx = s_sx[c], sx1 = min(sx + 1, L.W - 1);   // a clamped tap has zero weight
+            const int ax = (short)s_xw[c], bx = s_xw[c] >> 16;
+            const uint8_t* r0 = s + s_y0[r] * L.rs;
+            const uint8_t* r1 = s + s_y1[r] * L.rs;
+            v = hog_resize_out(s_yw[r], (int)__ldg(r0 + sx * L.ps) * ax + (int)__ldg(r0 + sx1 * L.ps) * bx,
+                               (int)__ldg(r1 + sx * L.ps) * ax + (int)__ldg(r1 + sx1 * L.ps) * bx);
+        }
+        dst[(long long)y * L.pitch + x * C + ch] = (uint8_t)v;
+    }
+}
+
+// Queues the levels of a pyramid one slice of whole frames at a time, the frames' levels fitting kPyramidSliceBytes (one
+// frame at least), so the scratch is bounded by the slice and not by the batch.  lv: every non-empty level (PyrLevel or
+// PyrImageLevel), frame f's at lv[first[f] .. first[f + 1]).  Per slice it places the levels in scratch (dst, tile0) and calls
+// run(l0, n, bytes, tiles, max_w, max_h): its first level, level count, scratch bytes, resize CTAs and largest cell grid.
+template <class Level, class Run>
+int pyramid_slices(sd_ctx* ctx, const char* fn, std::vector<Level>& lv, const std::vector<int>& first, int count, int cell_size, Run run)
+{
+    for (int f0 = 0; f0 < count;) {
+        size_t bytes = 0;
+        int f1 = f0;
+        for (; f1 < count; ++f1) {
+            size_t fb = 0;
+            for (int l = first[f1]; l < first[f1 + 1]; ++l) fb += (size_t)lv[l].pitch * lv[l].h;
+            if (f1 > f0 && bytes + fb > kPyramidSliceBytes) break;
+            bytes += fb;
+        }
+        const int l0 = first[f0], n = first[f1] - l0;
+        f0 = f1;
+        if (n == 0) continue;
+        long long pos = 0;
+        int tiles = 0, max_w = 0, max_h = 0;
+        for (int i = 0; i < n; ++i) {
+            Level& L = lv[l0 + i];
+            L.dst = pos;
+            L.tile0 = tiles;
+            if ((long long)tiles + (long long)L.tiles_x * sd_div_up(L.h, kResizeH) > INT_MAX)
+                return sd_fail(ctx, SD_ERR_INVALID, "%s: level too large", fn);
+            tiles += L.tiles_x * sd_div_up(L.h, kResizeH);
+            pos += (long long)L.pitch * L.h;
+            max_w = std::max(max_w, (L.w + cell_size / 2) / cell_size);
+            max_h = std::max(max_h, (L.h + cell_size / 2) / cell_size);
+        }
+        if (const int rc = run(l0, n, pos, tiles, max_w, max_h)) return rc;
+    }
+    return SD_OK;
+}
+
+// The scratch of one slice: [levels (bytes, 16-byte aligned) | level table | the dense kernel's descriptors | per-level
+// output offsets], the two tables uploaded.  Returns the scratch, or nullptr (the context holds the error).
+template <class Level, class Desc>
+uint8_t* pyramid_scratch(sd_ctx* ctx, long long bytes, const Level* levels, const std::vector<Desc>& desc, Level** d_lv,
+                         Desc** d_desc, int64_t** d_off)
+{
+    const size_t n = desc.size();
+    const size_t pix = sd_round16((size_t)bytes), lv_bytes = sizeof(Level) * n, desc_bytes = sizeof(Desc) * n;
+    uint8_t* ws = static_cast<uint8_t*>(sd_workspace(ctx, SD_WS_PYRAMID, pix + lv_bytes + desc_bytes + sizeof(int64_t) * n));
+    if (!ws) return nullptr;
+    *d_lv = reinterpret_cast<Level*>(ws + pix);
+    *d_desc = reinterpret_cast<Desc*>(ws + pix + lv_bytes);
+    *d_off = reinterpret_cast<int64_t*>(ws + pix + lv_bytes + desc_bytes);
+    if (sd_check_cuda(ctx, cudaMemcpyAsync(*d_lv, levels, lv_bytes, cudaMemcpyHostToDevice, ctx->stream), "pyramid levels") ||
+        sd_check_cuda(ctx, cudaMemcpyAsync(*d_desc, desc.data(), desc_bytes, cudaMemcpyHostToDevice, ctx->stream), "pyramid levels"))
+        return nullptr;
+    return ws;
+}
+
 }  // namespace
 
 extern "C" {
@@ -795,43 +927,17 @@ int sd_hog_pyramid(sd_ctx* ctx, const sd_image_batch* images, const double* h_sc
     const DenseSmem lay = dense_smem_layout(a.span, a.pitch, num_bins, dense_cells(a.tile));
     CUtensorMap map;                                 // not read: levels of different sizes are staged by the load loop
     memset(&map, 0, sizeof(map));
-
-    // slices of whole frames whose levels fit kPyramidSliceBytes (one frame at least)
-    for (int f0 = 0; f0 < count;) {
-        size_t bytes = 0;
-        int f1 = f0;
-        for (; f1 < count; ++f1) {
-            size_t fb = 0;
-            for (int l = first[f1]; l < first[f1 + 1]; ++l) fb += (size_t)lv[l].pitch * lv[l].h;
-            if (f1 > f0 && bytes + fb > kPyramidSliceBytes) break;
-            bytes += fb;
-        }
-        const int l0 = first[f0], n = first[f1] - l0;
-        f0 = f1;
-        if (n == 0) continue;
-        // level positions in the scratch, the resize tiles, the dense kernel's descriptors and the grid that covers them
+    return pyramid_slices(ctx, __func__, lv, first, count, cell_size, [&](int l0, int n, long long bytes, int tiles, int max_w, int max_h) -> int {
         std::vector<sd_frame> desc(n);
-        long long pos = 0;
-        int tiles = 0, max_w = 0, max_h = 0;
         for (int i = 0; i < n; ++i) {
-            PyrLevel& L = lv[l0 + i];
-            L.dst = pos;
-            L.tile0 = tiles;
-            SD_REQUIRE(ctx, (long long)tiles + (long long)L.tiles_x * sd_div_up(L.h, kResizeH) <= INT_MAX, "level too large");
-            tiles += L.tiles_x * sd_div_up(L.h, kResizeH);
-            desc[i] = sd_frame{L.w, L.h, L.pitch, 0, pos};
-            pos += (long long)L.pitch * L.h;
-            max_w = std::max(max_w, (L.w + cell_size / 2) / cell_size);
-            max_h = std::max(max_h, (L.h + cell_size / 2) / cell_size);
+            const PyrLevel& L = lv[l0 + i];
+            desc[i] = sd_frame{L.w, L.h, L.pitch, 0, L.dst};
         }
-        const size_t pix = sd_round16((size_t)pos), lv_bytes = sizeof(PyrLevel) * n, desc_bytes = sizeof(sd_frame) * n;
-        uint8_t* ws = static_cast<uint8_t*>(sd_workspace(ctx, SD_WS_PYRAMID, pix + lv_bytes + desc_bytes + sizeof(int64_t) * n));
+        PyrLevel* d_lv;
+        sd_frame* d_desc;
+        int64_t* d_off;
+        uint8_t* ws = pyramid_scratch(ctx, bytes, lv.data() + l0, desc, &d_lv, &d_desc, &d_off);
         if (!ws) return SD_ERR_CUDA;
-        PyrLevel* d_lv = reinterpret_cast<PyrLevel*>(ws + pix);
-        sd_frame* d_desc = reinterpret_cast<sd_frame*>(ws + pix + lv_bytes);
-        int64_t* d_off = reinterpret_cast<int64_t*>(ws + pix + lv_bytes + desc_bytes);
-        SD_CUDA(ctx, cudaMemcpyAsync(d_lv, lv.data() + l0, lv_bytes, cudaMemcpyHostToDevice, ctx->stream));
-        SD_CUDA(ctx, cudaMemcpyAsync(d_desc, desc.data(), desc_bytes, cudaMemcpyHostToDevice, ctx->stream));
 
         ResizeArgs r;
         r.images = images->d_data;
@@ -846,10 +952,118 @@ int sd_hog_pyramid(sd_ctx* ctx, const sd_image_batch* images, const double* h_sc
         a.images = ws;
         a.frames = d_desc;
         a.out_offset = d_off;
-        if (const int rc = launch_dense(ctx, __func__, "hog_dense_kernel", dense_kernel(num_bins), a, n, max_w, max_h, lay.total, map))
-            return rc;
+        return launch_dense(ctx, "sd_hog_pyramid", "hog_dense_kernel", dense_kernel(num_bins), a, n, max_w, max_h, lay.total, map);
+    });
+}
+
+int sd_hog_pyramid_images(sd_ctx* ctx, const sd_hog_images* images, const double* h_scales, int num_scales, int cell_size,
+                          int num_bins, int variant, int bilinear_orientations, float* d_out, const int64_t* d_out_offset)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, images && h_scales && d_out && d_out_offset, "null argument");
+    SD_REQUIRE(ctx, images->dtype == SD_HOG_U8, "dtype must be SD_HOG_U8: the levels are resized by the 8-bit rule");
+    SD_REQUIRE(ctx, images->channels >= 1 && images->channels <= kDenseMaxChannels, "channels must be in [1,16]");
+    SD_REQUIRE(ctx, bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
+    if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins, cell_size)) return rc;
+    SD_REQUIRE(ctx, num_scales >= 1, "num_scales must be at least 1");
+    for (int s = 0; s < num_scales; ++s)
+        SD_REQUIRE(ctx, h_scales[s] > 0.0 && h_scales[s] <= 4.0, "every scale must be finite and in (0, 4]");
+    SD_REQUIRE(ctx, images->count >= 0, "negative frame count");
+    const int count = images->count, C = images->channels;
+    if (count == 0) return SD_OK;
+    SD_REQUIRE(ctx, images->d_data, "null argument");
+    SD_REQUIRE(ctx, (long long)count * num_scales <= INT_MAX, "too many levels");
+
+    // the frames: the batch's, or the descriptor table read back once
+    std::vector<sd_hog_image> fr;
+    if (images->d_frames) {
+        if (const int rc = sd_fetch_table(ctx, images->d_frames, count, fr)) return rc;
+    } else {
+        SD_REQUIRE(ctx, images->image_stride >= 0, "negative image stride");
+        fr.assign(count, images->frame);
+        for (int i = 0; i < count; ++i) fr[i].offset += (int64_t)i * images->image_stride;
     }
-    return SD_OK;
+    // every non-empty level of every frame, in the order of the caller's slots
+    std::vector<PyrImageLevel> lv;
+    std::vector<int> first(count + 1, 0);
+    for (int f = 0; f < count; ++f) {
+        const sd_hog_image& d = fr[f];
+        if (d.width < 1 || d.height < 1 || d.offset < 0 || d.row_stride < 0 || d.pixel_stride < 0 || d.channel_stride < 0)
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d (%d x %d) is smaller than 1 x 1 or has a negative offset or stride",
+                           __func__, f, d.width, d.height);
+        first[f] = (int)lv.size();
+        for (int s = 0; s < num_scales; ++s) {
+            PyrImageLevel L{};
+            int hw, hh, dd;
+            if (!pyramid_level(d.width, d.height, h_scales[s], &L.w, &L.h))
+                return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d at scale %g is larger than 2^28 px per side", __func__, f, h_scales[s]);
+            if (!dense_shape(L.w, L.h, cell_size, num_bins, variant, &hw, &hh, &dd)) continue;
+            if ((long long)L.w * C > INT_MAX - 15) return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d: level too large", __func__, f);
+            L.src = d.offset;
+            L.rs = d.row_stride; L.ps = d.pixel_stride; L.chs = d.channel_stride;
+            L.W = d.width; L.H = d.height;
+            L.pitch = dense_align(L.w * C, 16);
+            L.tiles_x = sd_div_up(L.w, kResizeW);
+            L.slot = f * num_scales + s;
+            lv.push_back(L);
+        }
+    }
+    first[count] = (int)lv.size();
+    if (lv.empty()) return SD_OK;
+
+    // one channel, nearest bins, contiguous rows: sd_hog_pyramid computes the same levels (as sd_hog_dense_images routes to
+    // sd_hog_dense)
+    const sd_hog_image& f0 = images->frame;
+    if (C == 1 && !bilinear_orientations && !images->d_frames && f0.pixel_stride == 1 && f0.row_stride >= f0.width &&
+        f0.row_stride <= INT_MAX && (count == 1 || images->image_stride > 0)) {
+        sd_image_batch ib{};
+        ib.d_data = static_cast<const uint8_t*>(images->d_data) + f0.offset;
+        ib.width = f0.width; ib.height = f0.height; ib.row_stride = (int32_t)f0.row_stride;
+        ib.image_stride = images->image_stride;
+        ib.count = count;
+        return sd_hog_pyramid(ctx, &ib, h_scales, num_scales, cell_size, num_bins, variant, d_out, d_out_offset);
+    }
+
+    const bool bil = bilinear_orientations != 0;
+    const ImagesKernel kern = bil ? images_kernel<uint8_t, true>(num_bins) : images_kernel<uint8_t, false>(num_bins);
+    ImageArgs a;
+    memset(&a, 0, sizeof(a));
+    a.channels = C;
+    a.out = d_out;
+    a.variant = variant; a.cs = cell_size; a.K = num_bins; a.dd = sd_hog_dd(num_bins, variant);
+    a.tile = images_tile(kern, cell_size, num_bins, bil);
+    a.span = cell_size * (a.tile + 3) + 4;
+    a.pi_k = 3.141592653589793 / (double)num_bins;    // VL_PI / numOrientations (hog.c:677)
+    hog_orientations(num_bins, a.orient);
+    const DenseSmem lay = dense_smem_layout(a.span, 0, num_bins, dense_cells(a.tile), bil);
+    return pyramid_slices(ctx, __func__, lv, first, count, cell_size, [&](int l0, int n, long long bytes, int tiles, int max_w, int max_h) -> int {
+        std::vector<sd_hog_image> desc(n);
+        for (int i = 0; i < n; ++i) {
+            const PyrImageLevel& L = lv[l0 + i];
+            desc[i] = sd_hog_image{L.w, L.h, L.dst, L.pitch, C, 1};
+        }
+        PyrImageLevel* d_lv;
+        sd_hog_image* d_desc;
+        int64_t* d_off;
+        uint8_t* ws = pyramid_scratch(ctx, bytes, lv.data() + l0, desc, &d_lv, &d_desc, &d_off);
+        if (!ws) return SD_ERR_CUDA;
+
+        ResizeImagesArgs r;
+        r.images = static_cast<const uint8_t*>(images->d_data);
+        r.scratch = ws;
+        r.levels = d_lv;
+        r.count = n;
+        r.channels = C;
+        r.out_offset = d_out_offset;
+        r.level_offset = d_off;
+        hog_pyramid_resize_images_kernel<<<(unsigned)tiles, kResizeThreads, 0, ctx->stream>>>(r);
+        SD_LAUNCH_CHECK(ctx, "hog_pyramid_resize_images_kernel");
+
+        a.data = ws;
+        a.frames = d_desc;
+        a.out_offset = d_off;
+        return launch_dense(ctx, "sd_hog_pyramid_images", "hog_images_kernel", kern, a, n, max_w, max_h, lay.total);
+    });
 }
 
 int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size, int num_bins, int variant,

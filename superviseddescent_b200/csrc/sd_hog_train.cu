@@ -14,6 +14,7 @@
 #include <cfloat>
 #include <cmath>
 #include <cstring>
+#include <functional>
 #include <set>
 #include <tuple>
 #include <vector>
@@ -410,51 +411,62 @@ int sd_learn_squared_hinge(sd_ctx* ctx, const float* d_A, int64_t lda, const flo
     return squared_hinge(ctx, d_A, lda, d_y, y, N, D, lambda, max_iterations, d_w, report);
 }
 
-int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_box* h_boxes, int num_boxes, const double* h_scales,
-                        int num_scales, int cell_size, int num_bins, int variant, int filter_w, int filter_h, int pad_x, int pad_y,
-                        const sd_hog_train_param* p, float* d_filter, float* h_bias, sd_hog_train_report* h_rounds,
-                        sd_hog_window* h_negatives, int* h_num_negatives)
+}  // extern "C"
+
+namespace {
+
+// The trainer's frames, the one thing its two entry points differ in: their count, each one's size (read once, after the
+// arguments are checked) and the pyramids of frames [f0, f1) into d_out at sd_hog_pyramid's per-level offsets d_off.
+struct FrameSize { int width, height; };
+struct TrainFrames {
+    int count;
+    std::function<int(std::vector<FrameSize>&)> sizes;
+    std::function<int(int f0, int f1, float* d_out, const int64_t* d_off)> pyramid;
+};
+
+#define TRAIN_REQUIRE(cond, msg)                                                   \
+    do {                                                                           \
+        if (!(cond)) return sd_fail(ctx, SD_ERR_INVALID, "%s: %s", fn, msg);       \
+    } while (0)
+
+// sd_hog_train_filter's rule (include/sd_b200.h) on the frames of src; fn names the entry point in messages
+int train_filter(sd_ctx* ctx, const char* fn, const TrainFrames& src, const sd_hog_box* h_boxes, int num_boxes, const double* h_scales,
+                 int num_scales, int cell_size, int num_bins, int variant, int filter_w, int filter_h, int pad_x, int pad_y,
+                 const sd_hog_train_param* p, float* d_filter, float* h_bias, sd_hog_train_report* h_rounds, sd_hog_window* h_negatives,
+                 int* h_num_negatives)
 {
-    if (!ctx) return SD_ERR_INVALID;
-    SD_REQUIRE(ctx, images && h_scales && p && d_filter && h_bias && h_rounds && h_num_negatives && (num_boxes == 0 || h_boxes),
-               "null argument");
-    SD_REQUIRE(ctx, !images->d_roi, "a batch with regions of interest has no whole frames");
-    if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins, cell_size)) return rc;
-    if (const int rc = sd_hog_check_filter(ctx, __func__, filter_w, filter_h, pad_x, pad_y)) return rc;
-    SD_REQUIRE(ctx, sd_aligned(d_filter, 4), "the filter must be 4-byte aligned");
-    SD_REQUIRE(ctx, num_scales >= 1 && images->count >= 1 && num_boxes >= 0, "need at least one scale and one frame");
+    if (const int rc = sd_hog_check_config(ctx, fn, variant, num_bins, cell_size)) return rc;
+    if (const int rc = sd_hog_check_filter(ctx, fn, filter_w, filter_h, pad_x, pad_y)) return rc;
+    TRAIN_REQUIRE(sd_aligned(d_filter, 4), "the filter must be 4-byte aligned");
+    TRAIN_REQUIRE(num_scales >= 1 && src.count >= 1 && num_boxes >= 0, "need at least one scale and one frame");
     for (int s = 0; s < num_scales; ++s)
-        SD_REQUIRE(ctx, h_scales[s] > 0.0 && h_scales[s] <= 4.0, "every scale must be finite and in (0, 4]");
-    SD_REQUIRE(ctx, p->lambda > 0.f && std::isfinite(p->lambda), "lambda must be positive and finite");
-    SD_REQUIRE(ctx, p->positive_overlap >= 0.f && p->positive_overlap <= 1.f && p->negative_overlap >= 0.f && p->negative_overlap <= 1.f &&
-                    p->mine_overlap >= 0.f && p->mine_overlap <= 1.f, "overlaps must be in [0, 1]");
-    SD_REQUIRE(ctx, p->flip_positives == 0 || p->flip_positives == 1, "flip_positives must be 0 or 1");
-    SD_REQUIRE(ctx, p->rounds >= 0 && p->max_iterations >= 1 && p->max_negatives >= 1, "rounds >= 0, max_iterations >= 1, max_negatives >= 1");
-    SD_REQUIRE(ctx, p->negatives_per_frame >= 1 && p->negatives_per_frame <= SD_HOG_DETECT_MAX_CANDIDATES,
-               "negatives_per_frame must be in [1, SD_HOG_DETECT_MAX_CANDIDATES]");
+        TRAIN_REQUIRE(h_scales[s] > 0.0 && h_scales[s] <= 4.0, "every scale must be finite and in (0, 4]");
+    TRAIN_REQUIRE(p->lambda > 0.f && std::isfinite(p->lambda), "lambda must be positive and finite");
+    TRAIN_REQUIRE(p->positive_overlap >= 0.f && p->positive_overlap <= 1.f && p->negative_overlap >= 0.f && p->negative_overlap <= 1.f &&
+                      p->mine_overlap >= 0.f && p->mine_overlap <= 1.f, "overlaps must be in [0, 1]");
+    TRAIN_REQUIRE(p->flip_positives == 0 || p->flip_positives == 1, "flip_positives must be 0 or 1");
+    TRAIN_REQUIRE(p->rounds >= 0 && p->max_iterations >= 1 && p->max_negatives >= 1, "rounds >= 0, max_iterations >= 1, max_negatives >= 1");
+    TRAIN_REQUIRE(p->negatives_per_frame >= 1 && p->negatives_per_frame <= SD_HOG_DETECT_MAX_CANDIDATES,
+                  "negatives_per_frame must be in [1, SD_HOG_DETECT_MAX_CANDIDATES]");
     const int dd = sd_hog_dd(num_bins, variant);
     const int D = dd * filter_w * filter_h + 1;
-    SD_REQUIRE(ctx, D <= SD_HOG_TRAIN_MAX_DIM, "dd * filter_h * filter_w + 1 exceeds SD_HOG_TRAIN_MAX_DIM");
-    const int F = images->count, S = num_scales;
+    TRAIN_REQUIRE(D <= SD_HOG_TRAIN_MAX_DIM, "dd * filter_h * filter_w + 1 exceeds SD_HOG_TRAIN_MAX_DIM");
+    const int F = src.count, S = num_scales;
 
     // the frames' sizes and level tables
-    std::vector<sd_frame> frames;
-    if (images->d_frames) {
-        if (const int rc = sd_fetch_table(ctx, images->d_frames, F, frames)) return rc;
-    } else {
-        frames.assign(F, sd_frame{images->width, images->height, images->row_stride, 0, 0});
-    }
+    std::vector<FrameSize> frames;
+    if (const int rc = src.sizes(frames)) return rc;
     std::vector<std::vector<Level>> lv(F);
     for (int f = 0; f < F; ++f) {
-        SD_REQUIRE(ctx, frames[f].width >= 1 && frames[f].height >= 1, "every frame must be at least 1 x 1");
+        TRAIN_REQUIRE(frames[f].width >= 1 && frames[f].height >= 1, "every frame must be at least 1 x 1");
         if (level_table(frames[f].width, frames[f].height, h_scales, S, cell_size, num_bins, variant, &lv[f]))
-            return sd_fail(ctx, SD_ERR_INVALID, "%s: invalid pyramid level", __func__);
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: invalid pyramid level", fn);
     }
     std::vector<std::vector<int>> frame_boxes(F);
     for (int b = 0; b < num_boxes; ++b) {
         const sd_hog_box& q = h_boxes[b];
         if (q.frame < 0 || q.frame >= F || q.w < 1 || q.h < 1)
-            return sd_fail(ctx, SD_ERR_INVALID, "%s: box %d: frame %d out of [0, %d) or an empty box", __func__, b, q.frame, F);
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: box %d: frame %d out of [0, %d) or an empty box", fn, b, q.frame, F);
         frame_boxes[q.frame].push_back(b);
     }
 
@@ -464,7 +476,7 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
     int unassigned = 0;
     for (int b = 0; b < num_boxes; ++b) {
         const sd_hog_box& q = h_boxes[b];
-        const sd_frame& fr = frames[q.frame];
+        const FrameSize& fr = frames[q.frame];
         sd_hog_window wv;
         double iou;
         best_window(lv[q.frame], fr.width, fr.height, cell_size, filter_w, filter_h, pad_x, pad_y, p->positive_overlap,
@@ -479,12 +491,12 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
         }
     }
     const int npos = (int)pos.size();
-    SD_REQUIRE(ctx, npos >= 1, "no box is covered by a window at positive_overlap: nothing to train on");
+    TRAIN_REQUIRE(npos >= 1, "no box is covered by a window at positive_overlap: nothing to train on");
 
     // memory: the rows of the solve, the SVM's compacted copy, the Gram, one slice of pyramid features
     const int64_t ld = ((int64_t)D + 3) / 4 * 4;
     const int64_t nrows = (int64_t)npos + p->max_negatives;
-    SD_REQUIRE(ctx, nrows <= INT32_MAX / 2, "too many rows");
+    TRAIN_REQUIRE(nrows <= INT32_MAX / 2, "too many rows");
     const size_t rows_bytes = (size_t)nrows * ld * sizeof(float) + (size_t)nrows * sizeof(float);
     const size_t need = 2 * rows_bytes + (size_t)D * sd_learn_ldg(D, 1) * sizeof(float) + kSliceFloats * sizeof(float) * 2;
     size_t free_b = 0, total_b = 0;
@@ -492,7 +504,7 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
     size_t held = 0;
     for (int s = 0; s < SD_WS_COUNT; ++s) held += ctx->ws_bytes[s];
     if (need > free_b + held)
-        return sd_fail(ctx, SD_ERR_CUDA, "%s: D = %d with %lld rows needs about %zu MB of device memory, %zu MB available", __func__, D,
+        return sd_fail(ctx, SD_ERR_CUDA, "%s: D = %d with %lld rows needs about %zu MB of device memory, %zu MB available", fn, D,
                        (long long)nrows, need >> 20, (free_b + held) >> 20);
 
     // slices of frames whose pyramids fit kSliceFloats (at least one frame each)
@@ -534,7 +546,7 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
     }
     const int max_levels = max_slice_frames * S;
     const int64_t slice_dets = (int64_t)max_slice_frames * p->negatives_per_frame;
-    SD_REQUIRE(ctx, slice_dets <= INT32_MAX / (int64_t)sizeof(sd_hog_detection), "too many detections per slice: lower negatives_per_frame");
+    TRAIN_REQUIRE(slice_dets <= INT32_MAX / (int64_t)sizeof(sd_hog_detection), "too many detections per slice: lower negatives_per_frame");
     const int max_win = (int)std::max<int64_t>(npos, std::max<int64_t>(p->max_negatives, slice_dets));
     const size_t feat_b = sd_round16(max_slice * sizeof(float)), score_b = sd_round16(max_scores * sizeof(float) + 4);
     const size_t off_b = sd_round16(sizeof(int64_t) * max_levels), grid_b = sd_round16(sizeof(sd_hog_grid) * max_levels);
@@ -598,12 +610,7 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
             }
         if (grids.empty()) return SD_OK;
         SD_CUDA(ctx, cudaMemcpyAsync(d_off, off.data(), sizeof(int64_t) * off.size(), cudaMemcpyHostToDevice, ctx->stream));
-        sd_image_batch sub = *images;
-        sub.count = f1 - f0;
-        if (images->d_frames) sub.d_frames = images->d_frames + f0;
-        else sub.d_data = images->d_data + (int64_t)f0 * images->image_stride;
-        return timed(&sd_hog_train_report::pyramid_ms,
-                     [&] { return sd_hog_pyramid(ctx, &sub, h_scales, S, cell_size, num_bins, variant, d_feat, d_off); });
+        return timed(&sd_hog_train_report::pyramid_ms, [&] { return src.pyramid(f0, f1, d_feat, d_off); });
     };
     // gather windows (frame, level, x, y, flip) of the resident slice into rows dest[i] of d_rows
     auto gather = [&](int f0, const std::vector<sd_hog_window>& w, const std::vector<int>& dest) -> int {
@@ -782,6 +789,85 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
     if (h_negatives)
         for (size_t k = 0; k < cache.size(); ++k) h_negatives[k] = {cache[k].frame * S + cache[k].level, cache[k].x, cache[k].y, 0};
     return SD_OK;
+}
+
+#undef TRAIN_REQUIRE
+
+}  // namespace
+
+extern "C" {
+
+int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_box* h_boxes, int num_boxes, const double* h_scales,
+                        int num_scales, int cell_size, int num_bins, int variant, int filter_w, int filter_h, int pad_x, int pad_y,
+                        const sd_hog_train_param* p, float* d_filter, float* h_bias, sd_hog_train_report* h_rounds,
+                        sd_hog_window* h_negatives, int* h_num_negatives)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, images && h_scales && p && d_filter && h_bias && h_rounds && h_num_negatives && (num_boxes == 0 || h_boxes),
+               "null argument");
+    SD_REQUIRE(ctx, !images->d_roi, "a batch with regions of interest has no whole frames");
+    TrainFrames src;
+    src.count = images->count;
+    src.sizes = [&](std::vector<FrameSize>& sizes) -> int {
+        std::vector<sd_frame> fr;
+        if (images->d_frames) {
+            if (const int rc = sd_fetch_table(ctx, images->d_frames, images->count, fr)) return rc;
+        } else {
+            fr.assign(images->count, sd_frame{images->width, images->height, images->row_stride, 0, 0});
+        }
+        for (const sd_frame& d : fr) sizes.push_back({d.width, d.height});
+        return SD_OK;
+    };
+    src.pyramid = [&](int f0, int f1, float* d_out, const int64_t* d_off) {
+        sd_image_batch sub = *images;
+        sub.count = f1 - f0;
+        if (images->d_frames) sub.d_frames = images->d_frames + f0;
+        else sub.d_data = images->d_data + (int64_t)f0 * images->image_stride;
+        return sd_hog_pyramid(ctx, &sub, h_scales, num_scales, cell_size, num_bins, variant, d_out, d_off);
+    };
+    return train_filter(ctx, __func__, src, h_boxes, num_boxes, h_scales, num_scales, cell_size, num_bins, variant, filter_w, filter_h,
+                        pad_x, pad_y, p, d_filter, h_bias, h_rounds, h_negatives, h_num_negatives);
+}
+
+int sd_hog_train_filter_images(sd_ctx* ctx, const sd_hog_images* images, int bilinear_orientations, const sd_hog_box* h_boxes,
+                               int num_boxes, const double* h_scales, int num_scales, int cell_size, int num_bins, int variant,
+                               int filter_w, int filter_h, int pad_x, int pad_y, const sd_hog_train_param* p, float* d_filter,
+                               float* h_bias, sd_hog_train_report* h_rounds, sd_hog_window* h_negatives, int* h_num_negatives)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, images && h_scales && p && d_filter && h_bias && h_rounds && h_num_negatives && (num_boxes == 0 || h_boxes),
+               "null argument");
+    SD_REQUIRE(ctx, images->dtype == SD_HOG_U8, "dtype must be SD_HOG_U8: the levels are resized by the 8-bit rule");
+    SD_REQUIRE(ctx, images->channels >= 1 && images->channels <= 16, "channels must be in [1,16]");
+    SD_REQUIRE(ctx, bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
+    SD_REQUIRE(ctx, images->count < 1 || images->d_data, "null argument");
+    TrainFrames src;
+    src.count = images->count;
+    src.sizes = [&](std::vector<FrameSize>& sizes) -> int {
+        std::vector<sd_hog_image> fr;
+        if (images->d_frames) {
+            if (const int rc = sd_fetch_table(ctx, images->d_frames, images->count, fr)) return rc;
+        } else {
+            if (images->image_stride < 0) return sd_fail(ctx, SD_ERR_INVALID, "sd_hog_train_filter_images: negative image stride");
+            fr.assign(images->count, images->frame);
+        }
+        for (int f = 0; f < images->count; ++f) {
+            const sd_hog_image& d = fr[f];
+            if (d.offset < 0 || d.row_stride < 0 || d.pixel_stride < 0 || d.channel_stride < 0)
+                return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d has a negative offset or stride", "sd_hog_train_filter_images", f);
+            sizes.push_back({d.width, d.height});
+        }
+        return SD_OK;
+    };
+    src.pyramid = [&](int f0, int f1, float* d_out, const int64_t* d_off) {
+        sd_hog_images sub = *images;
+        sub.count = f1 - f0;
+        if (images->d_frames) sub.d_frames = images->d_frames + f0;
+        else sub.frame.offset += (int64_t)f0 * images->image_stride;
+        return sd_hog_pyramid_images(ctx, &sub, h_scales, num_scales, cell_size, num_bins, variant, bilinear_orientations, d_out, d_off);
+    };
+    return train_filter(ctx, __func__, src, h_boxes, num_boxes, h_scales, num_scales, cell_size, num_bins, variant, filter_w, filter_h,
+                        pad_x, pad_y, p, d_filter, h_bias, h_rounds, h_negatives, h_num_negatives);
 }
 
 }  // extern "C"
