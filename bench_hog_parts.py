@@ -3,15 +3,17 @@
     python bench_hog_parts.py [--frames 64] [--reps 10] [--out FILE]
 
 Workload: the 64-frame 1280x720 set of bench_hog_filters.py, cell size 8, K = 9, UoCTTI.  Q = 2 components (a random model
-and its mirror), root filters of 6 x 6 cells, P = 8 parts of 6 x 6 part-level cells, R = 4 and R = 16.  Root scales
+and its mirror), root filters of 6 x 6 cells, P = 8 parts of 6 x 6 part-level cells, R = 4, R = 16 and the exact transform
+(R null: sd_hog_distance_transform_exact, which writes placement maps, and sd_hog_part_placements_mapped).  Root scales
 0.5 * 2^(-l/5) while the root level holds the root filter; the parts are scored at twice each root scale, so the pyramid is
 2^(-l/5) from 1 down.  Threshold 0 on random filters: every frame fills max_candidates = 4096 and keeps max_detections = 256,
 the placements' largest load at these caps.
 
 For every stage -- pyramid, root scores, part scores, transform, assembly, detections, placements -- the time per frame from
 CUDA events around --reps calls of that stage alone, on inputs the chain produced.  The transform's algorithmic bytes are one
-read and one write of every part score (8 bytes per score); its achieved rate is compared with the H100's 3.35 TB/s.  The card
-name and power limit are read in the same run.  One JSON line per R."""
+read and one write of every part score (8 bytes per score), plus 8 bytes of placement per score where it writes placements
+(the exact route); its achieved rate is compared with the H100's 3.35 TB/s.  The card name, power limit and max SM clock are
+read in the same run.  One JSON line per R."""
 from __future__ import annotations
 
 import argparse
@@ -99,6 +101,7 @@ def main():
     rscores = torch.empty(max(rsize, 1), dtype=torch.float32, device=dev)
     pscores = torch.empty(max(psize, 1), dtype=torch.float32, device=dev)
     values = torch.empty_like(pscores)
+    pplace = torch.empty((max(psize, 1), 2), dtype=torch.int32, device=dev)
     total = torch.empty_like(rscores)
     pat = {(f, i): (oh, ow, pos) for f, i, oh, ow, pos in pmaps}
     descs, sdescs = [], []
@@ -125,20 +128,33 @@ def main():
     chk = api._check
     R_now = [4]
 
+    def transform():
+        if R_now[0] is None:
+            chk(ctx.h, lib.sd_hog_distance_transform_exact(ctx.h, C.byref(gv), Q * P, C.c_void_p(mc_d.ctypes.data), ptr(values),
+                                                           ptr(pplace)))
+        else:
+            chk(ctx.h, lib.sd_hog_distance_transform(ctx.h, C.byref(gv), Q * P, C.c_void_p(mc_d.ctypes.data), R_now[0], ptr(values),
+                                                     None))
+
+    def placements():
+        if R_now[0] is None:
+            chk(ctx.h, lib.sd_hog_part_placements_mapped(ctx.h, ptr(values), ptr(pplace), ptr(ptab), len(descs), C.byref(mc), CS,
+                                                         ptr(out), ptr(count), n, MD, ptr(place)))
+        else:
+            chk(ctx.h, lib.sd_hog_part_placements(ctx.h, ptr(pscores), ptr(ptab), len(descs), C.byref(mc), C.c_void_p(mc_d.ctypes.data),
+                                                  R_now[0], CS, ptr(out), ptr(count), n, MD, ptr(place)))
+
     stages = {
         "pyramid": lambda: chk(ctx.h, lib.sd_hog_pyramid(ctx.h, C.byref(ib), h_scales, len(every), CS, K, VARIANT, ptr(feats), ptr(d_off))),
         "root_scores": lambda: chk(ctx.h, lib.sd_hog_correlate(ctx.h, C.byref(gr), K, VARIANT, ptr(rf), Q, FW, FH, None, 0, 0, ptr(rscores))),
         "part_scores": lambda: chk(ctx.h, lib.sd_hog_correlate(ctx.h, C.byref(gp), K, VARIANT, ptr(pf), Q * P, PFW, PFH, None, 0, 0,
                                                                ptr(pscores))),
-        "transform": lambda: chk(ctx.h, lib.sd_hog_distance_transform(ctx.h, C.byref(gv), Q * P, C.c_void_p(mc_d.ctypes.data), R_now[0],
-                                                                      ptr(values), None)),
+        "transform": transform,
         "assembly": lambda: chk(ctx.h, lib.sd_hog_part_scores(ctx.h, ptr(rscores), ptr(values), ptr(ptab), len(descs), C.byref(mc),
                                                               ptr(total))),
         "detections": lambda: chk(ctx.h, lib.sd_hog_detections(ctx.h, ptr(total), ptr(stab), len(sdescs), n, Q, CS, FW, FH, 0, 0, 0.0, 0.5,
                                                                MC, MD, ptr(out), ptr(count), None)),
-        "placements": lambda: chk(ctx.h, lib.sd_hog_part_placements(ctx.h, ptr(pscores), ptr(ptab), len(descs), C.byref(mc),
-                                                                    C.c_void_p(mc_d.ctypes.data), R_now[0], CS, ptr(out), ptr(count), n,
-                                                                    MD, ptr(place))),
+        "placements": placements,
     }
 
     def timed(fn, reps):
@@ -154,14 +170,14 @@ def main():
 
     part_elems = psize
     lines = []
-    for R in (4, 16):
+    for R in (4, 16, None):
         R_now[0] = R
         for fn in stages.values():                              # the chain once, in order: every stage's inputs exist
             fn()
         torch.cuda.synchronize()
         t = {name: timed(fn, args.reps) for name, fn in stages.items()}
         us = {k: v / n * 1e6 for k, v in t.items()}
-        tr_bytes = 8.0 * part_elems
+        tr_bytes = (8.0 if R is not None else 16.0) * part_elems
         rec = {"R": R, "frames": n, "Q": Q, "P": P, "root_scales": len(roots), "pyramid_levels": len(every),
                "part_scores_per_frame": part_elems // n, "detections_per_frame": float(count.float().mean()),
                "us_per_frame": {k: round(v, 2) for k, v in us.items()},

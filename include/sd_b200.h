@@ -571,7 +571,7 @@ SD_API int sd_hog_train_filter_images(sd_ctx* ctx, const sd_hog_images* images, 
  * sd_hog_correlate with num_filters = num_planes; the grid descriptor's width and height are the planes' w and h).  Plane k of
  * every map uses h_deformation[4 k .. 4 k + 3] = (w0, w1, w2, w3): a displacement (dx, dy) costs w0 dx^2 + w1 dx + w2 dy^2 + w3 dy
  * score positions of its level.  R = max_displacement bounds |dx| and |dy|; R >= max(w, h) makes the transform unbounded in
- * effect (the transform of DPM is unbounded).  The rule, in float32 where it says fl():
+ * effect (the transform of DPM is unbounded: sd_hog_distance_transform_exact computes it at any map size).  The rule, in float32 where it says fl():
  *   Cost tables (host): cx[d] = (float)((double) w0 d d + (double) w1 d) and cy[e] = (float)((double) w2 e e + (double) w3 e) for
  *     d, e in [-R, R]; every entry must be finite.
  *   Pass X: t(y, u) is the best of fl(s(y, u + d) - cx[d]) over d = -R .. R ascending with 0 <= u + d < w, where a non-NaN
@@ -592,6 +592,30 @@ SD_API int sd_hog_train_filter_images(sd_ctx* ctx, const sd_hog_images* images, 
 #define SD_HOG_PART_MAX_PARTS 32
 SD_API int sd_hog_distance_transform(sd_ctx* ctx, const sd_hog_grids* maps, int num_planes, const float* h_deformation,
                                      int max_displacement, float* d_values, int32_t* d_place /* or NULL */);
+/* sd_hog_distance_transform_exact: the unbounded generalised distance transform of DPM (Felzenszwalb & Huttenlocher's lower
+ * envelope, "Distance transforms of sampled functions"), exact at any map size, asynchronous on the context's stream.  Maps,
+ * planes, deformations, output layout and alignment as sd_hog_distance_transform, with no bound on the displacement; the
+ * displacement d of a candidate q for position p is q - p, as there.  Each of pass X (along every row, on the scores) and then
+ * pass Y (along every column, on pass X's float32 output) applies to each line f(0 .. n - 1) with weights (a, b) = (w0, w1) in
+ * pass X and (w2, w3) in pass Y, as doubles:
+ *   Candidates: the positions q whose f(q) is finite, in ascending order.
+ *   Envelope (float64): position r > q owns p against q when p > s(q, r), where, in this operation order,
+ *     s(q, r) = (((f(q) - f(r)) + a * (double)((r - q)(r + q))) + b * (double)(r - q)) / ((a + a) * (double)(r - q))
+ *     ((r - q)(r + q) in int64; no operation fused).  The envelope is a stack of (q, z): each new candidate r pops the top
+ *     (q, z) while s(q, r) <= z, then is pushed with z = s(top, r), or -inf on an empty stack.  Position p belongs to the last
+ *     entry whose z < p: on an exact tie the smaller index keeps p.
+ *   Output: for p owned by q*, fl(f(q*) - c(q* - p)) with c(d) = (float)((double) a d d + (double) b d), the bounded call's cost
+ *     formula at any d; a line without a candidate gives -inf and no owner.
+ * The placement of (u, v) is (u*, v*), v* the owner in pass Y of column u and u* the owner in pass X of row v* at column u, or
+ * (-1, -1) when pass Y's column has no candidate.  On scores and weights where every operation is exact (small integers), the
+ * result equals sd_hog_distance_transform's at R >= max(w, h) bit for bit, placements included.  Each value depends on its plane
+ * and deformation alone: the same in any batch and in every run.  Lines of up to 32 positions keep their envelopes in shared
+ * memory, longer ones in the context's scratch (20 bytes per lane and position of the longest line; the grid is sized to keep
+ * it within 256 MB), so no map size is refused for lack of shared memory.  Null pointers, unaligned pointers, num_planes outside [1, SD_HOG_FILTER_MAX_BANK], a weight that
+ * is not finite, w0 <= 0 or w2 <= 0, or a grid smaller than 1 x 1 or with a negative offset is SD_ERR_INVALID before any work
+ * is queued (nothing is written). */
+SD_API int sd_hog_distance_transform_exact(sd_ctx* ctx, const sd_hog_grids* maps, int num_planes, const float* h_deformation,
+                                           float* d_values, int32_t* d_place /* or NULL */);
 /* A star model's geometry; its filters and deformations are the caller's (the correlate and transform calls take them). */
 typedef struct {
     int32_t num_components, num_parts;   /* Q >= 1, P in [1, SD_HOG_PART_MAX_PARTS], Q * P <= SD_HOG_FILTER_MAX_BANK */
@@ -652,6 +676,15 @@ SD_API int sd_hog_part_placements(sd_ctx* ctx, const float* d_parts, const sd_ho
                                   const sd_hog_part_model* model, const float* h_deformation, int max_displacement, int cell_size,
                                   const sd_hog_detection* d_det, const int32_t* d_count, int num_frames, int max_detections,
                                   sd_hog_part_placement* d_out /* num_frames x max_detections x P */);
+/* sd_hog_part_placements_mapped: the rows of sd_hog_part_placements, read from a transform's maps instead of recomputed.  d_values
+ * and d_place hold the transform's values and (u, v) placements of the part maps at the table's part_offset (floats; int32
+ * pairs at d_place + 2 part_offset): sd_hog_distance_transform_exact with out_offset = part_offset writes them.  Each part's
+ * term and placement are the maps' at its anchor, its box by the rule above.  Refusals, output and read-backs as
+ * sd_hog_part_placements (without h_deformation and max_displacement); d_place must be 8-byte aligned. */
+SD_API int sd_hog_part_placements_mapped(sd_ctx* ctx, const float* d_values, const int32_t* d_place, const sd_hog_part_map* d_maps,
+                                         int num_maps, const sd_hog_part_model* model, int cell_size, const sd_hog_detection* d_det,
+                                         const int32_t* d_count, int num_frames, int max_detections,
+                                         sd_hog_part_placement* d_out /* num_frames x max_detections x P */);
 
 /* ---- regressor: LinearRegressor<Solver> (regressors.hpp:318-400) ------------------------ */
 /* Solver::solve (regressors.hpp:199-234 == verbose_solver.hpp:53-111):

@@ -178,7 +178,8 @@ EXPORTS = [
     "sd_hog_dense_images", "sd_hog_dense_polar", "sd_hog_permutation", "sd_hog_glyphs", "sd_hog_render", "sd_hog_relayout",
     "sd_hog_pyramid_shape", "sd_hog_pyramid", "sd_hog_pyramid_images", "sd_hog_correlate", "sd_hog_detections",
     "sd_hog_windows", "sd_hog_box_windows", "sd_learn_squared_hinge", "sd_hog_train_filter", "sd_hog_train_filter_images",
-    "sd_hog_distance_transform", "sd_hog_part_scores", "sd_hog_part_placements",
+    "sd_hog_distance_transform", "sd_hog_distance_transform_exact", "sd_hog_part_scores", "sd_hog_part_placements",
+    "sd_hog_part_placements_mapped",
     "sd_learn", "sd_centre_features", "sd_learn_centred", "sd_learn_rank_revealing", "sd_gram", "sd_solve_gram", "sd_predict", "sd_test_residual", "sd_solver_timings", "sd_set_gram_mode", "sd_set_solver", "sd_solver_iterations",
     "sd_set_rank_diagnostic", "sd_last_rank",
     "sd_comm_get_unique_id", "sd_comm_create", "sd_comm_adopt", "sd_comm_destroy", "sd_comm_rank", "sd_comm_size",
@@ -253,6 +254,9 @@ def lib():
         l.sd_hog_train_filter_images.argtypes = [C.c_void_p, C.c_void_p, _i, C.c_void_p, _i, C.c_void_p, _i, _i, _i, _i, _i, _i, _i,
                                                  _i, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         l.sd_hog_distance_transform.argtypes = [C.c_void_p, C.c_void_p, _i, C.c_void_p, _i, C.c_void_p, C.c_void_p]
+        l.sd_hog_distance_transform_exact.argtypes = [C.c_void_p, C.c_void_p, _i, C.c_void_p, C.c_void_p, C.c_void_p]
+        l.sd_hog_part_placements_mapped.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _i, C.c_void_p, _i, C.c_void_p,
+                                                    C.c_void_p, _i, _i, C.c_void_p]
         l.sd_hog_part_scores.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _i, C.c_void_p, C.c_void_p]
         l.sd_hog_part_placements.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, _i, C.c_void_p, C.c_void_p, _i, _i, C.c_void_p,
                                              C.c_void_p, _i, _i, C.c_void_p]

@@ -1864,7 +1864,7 @@ def train_hog_filter(frames, box_frame, boxes, scales, filter_size, cell_size: i
 
 
 # ------------------------------------------------------------------------------------------------
-# deformable part models: bounded distance transforms, star-model scores and part placements
+# deformable part models: bounded and exact distance transforms, star-model scores and part placements
 # ------------------------------------------------------------------------------------------------
 PART_MAX_DISPLACEMENT = 32   # SD_HOG_PART_MAX_DISPLACEMENT
 PART_MAX_PARTS = 32          # SD_HOG_PART_MAX_PARTS
@@ -1874,11 +1874,11 @@ class HogPartModel:
     """A star model of Q components for vl_hog_part_detect: root (Q, dd, fh, fw) filters with bias (Q,), parts (Q, P, dd, pfh, pfw)
     filters scored at twice the root's resolution, anchors (Q, P, 2) int (ax, ay) in part-level cells relative to twice the root
     window's top-left cell, deformation (Q, P, 4) (w0, w1, w2, w3): a displacement (dx, dy) costs w0 dx^2 + w1 dx + w2 dy^2 + w3 dy,
-    pad = (pad_x, pad_y) of the root correlate, part_pad of the part correlate, and max_displacement R bounding |dx| and |dy|.
-    The filters are ones for the features they were trained on: a model of colour HOG (vl_hog_pyramid's multichannel and
+    pad = (pad_x, pad_y) of the root correlate, part_pad of the part correlate, and max_displacement R bounding |dx| and |dy|,
+    or None for the exact, unbounded transform of DPM (which needs w0 > 0 and w2 > 0).  The filters are ones for the features they were trained on: a model of colour HOG (vl_hog_pyramid's multichannel and
     bilinear_orientations) is scored by vl_hog_part_detect with the same values."""
 
-    def __init__(self, root, bias, parts, anchors, deformation, pad=(0, 0), part_pad=(0, 0), max_displacement: int = 4):
+    def __init__(self, root, bias, parts, anchors, deformation, pad=(0, 0), part_pad=(0, 0), max_displacement: Optional[int] = 4):
         self.root = _tensor(root).to(torch.float32).contiguous()
         self.bias = _tensor(bias).to(torch.float32).reshape(-1).contiguous()
         self.parts = _tensor(parts).to(torch.float32).contiguous()
@@ -1886,7 +1886,7 @@ class HogPartModel:
         self.deformation = np.ascontiguousarray(np.asarray(deformation, np.float32))
         self.pad = tuple(int(v) for v in pad)
         self.part_pad = tuple(int(v) for v in part_pad)
-        self.max_displacement = int(max_displacement)
+        self.max_displacement = None if max_displacement is None else int(max_displacement)
         if self.root.dim() != 4 or self.parts.dim() != 5:
             raise ValueError("root must be (Q, dd, fh, fw) and parts (Q, P, dd, pfh, pfw)")
         q, dd = self.root.shape[:2]
@@ -1933,13 +1933,15 @@ def _deformation(deformation, planes: int):
     return d, C.c_void_p(d.ctypes.data)
 
 
-def vl_hog_distance_transform(maps, deformation, max_displacement: int, ctx: Optional[Context] = None):
-    """The bounded generalised distance transform of score maps on the device (sd_hog_distance_transform):
-        D(v, u) = max over |dx|, |dy| <= R of s(v + dy, u + dx) - (w0 dx^2 + w1 dx + w2 dy^2 + w3 dy),
-    separably in float32 with the tie rule of include/sd_b200.h, and where that maximum is, (u + dx, v + dy).  maps: a
-    (N, P, h, w) float32 tensor, or a list of (P, h, w) maps of any sizes; deformation: (P, 4), plane k's (w0, w1, w2, w3);
-    R = max_displacement in [0, 32].  Returns (values, placements) in the shapes of maps, placements with a trailing (u, v)
-    axis of int32 ((-1, -1) where the rule places nothing)."""
+def vl_hog_distance_transform(maps, deformation, max_displacement: Optional[int] = None, ctx: Optional[Context] = None):
+    """The generalised distance transform of score maps on the device:
+        D(v, u) = max over (dx, dy) of s(v + dy, u + dx) - (w0 dx^2 + w1 dx + w2 dy^2 + w3 dy),
+    separably, and where that maximum is, (u + dx, v + dy).  max_displacement None: the exact, unbounded transform of DPM
+    (sd_hog_distance_transform_exact: lower envelopes in float64, finite scores only; w0 > 0 and w2 > 0); an integer R in
+    [0, 32]: |dx|, |dy| <= R in float32 (sd_hog_distance_transform).  The rules and tie breaks are in include/sd_b200.h.  maps:
+    a (N, P, h, w) float32 tensor, or a list of (P, h, w) maps of any sizes; deformation: (P, 4), plane k's (w0, w1, w2, w3).
+    Returns (values, placements) in the shapes of maps, placements with a trailing (u, v) axis of int32 ((-1, -1) where the
+    rule places nothing)."""
     ctx = ctx or default_context()
     dev = f"cuda:{ctx.device}"
     single = not isinstance(maps, (list, tuple))
@@ -1967,8 +1969,12 @@ def vl_hog_distance_transform(maps, deformation, max_displacement: int, ctx: Opt
         place = torch.empty((keep.numel(), 2), dtype=torch.int32, device=dev)
         table = _device_table([HogGridC(t.shape[2], t.shape[1], o, o) for t, o in zip(items, offs)], dev)
         g.d_features, g.count, g.width, g.height, g.d_grids = keep.data_ptr(), len(items), 0, 0, table.data_ptr()
-    _check(ctx.h, _capi.lib().sd_hog_distance_transform(ctx.h, C.byref(g), int(planes), d_ptr, int(max_displacement), ptr(values),
-                                                        ptr(place)))
+    lib = _capi.lib()
+    if max_displacement is None:
+        _check(ctx.h, lib.sd_hog_distance_transform_exact(ctx.h, C.byref(g), int(planes), d_ptr, ptr(values), ptr(place)))
+    else:
+        _check(ctx.h, lib.sd_hog_distance_transform(ctx.h, C.byref(g), int(planes), d_ptr, int(max_displacement), ptr(values),
+                                                    ptr(place)))
     if single:
         return values, place
     return ([values[o:o + t.numel()].view(t.shape) for t, o in zip(items, offs)],
@@ -2025,7 +2031,8 @@ def vl_hog_part_detect(frames, scales, model: HogPartModel, cell_size: int, num_
     both is computed once; root scales must be <= 2), vl_hog_correlate of the root filters (bias included) on the root levels and
     of all Q * P part filters on the part levels, each read in place; vl_hog_distance_transform of the part maps; the star
     model's scores (vl_hog_part_scores); sd_hog_detections over them with the root's filter size and pad, all components as one
-    class; and the part placements of every detection (sd_hog_part_placements).  One host read-back at the end.  frames,
+    class; and the part placements of every detection (sd_hog_part_placements, or with the model's max_displacement None, the
+    exact transform's placement maps read at the anchors by sd_hog_part_placements_mapped).  One host read-back at the end.  frames,
     multichannel and bilinear_orientations as vl_hog_pyramid takes them.  Returns HogPartDetections; detect_faces(frames,
     d.frame, boxes=d.boxes) takes the result as it is."""
     ctx = ctx or default_context()
@@ -2055,18 +2062,23 @@ def vl_hog_part_detect(frames, scales, model: HogPartModel, cell_size: int, num_
                                pad=model.part_pad, ctx=ctx) if plevels else []
     pmap = {key: sc for key, sc in zip(plevels, pscores) if sc.numel()}
     d, d_ptr = _deformation(model.deformation, q * p)
-    R = int(model.max_displacement)
+    R = model.max_displacement
     lib = _capi.lib()
     if pmap:
         stor = next(iter(pmap.values())).untyped_storage()
         raw = torch.empty(0, dtype=torch.float32, device=dev).set_(stor)
         values = torch.empty_like(raw)
+        pmaps = torch.empty((raw.numel() if R is None else 1, 2), dtype=torch.int32, device=dev)
         g = HogGridsC()
         gt = _device_table([HogGridC(sc.shape[2], sc.shape[1], sc.storage_offset(), sc.storage_offset()) for sc in pmap.values()], dev)
         g.d_features, g.count, g.width, g.height, g.d_grids = raw.data_ptr(), len(pmap), 0, 0, gt.data_ptr()
-        _check(ctx.h, lib.sd_hog_distance_transform(ctx.h, C.byref(g), q * p, d_ptr, R, ptr(values), None))
+        if R is None:
+            _check(ctx.h, lib.sd_hog_distance_transform_exact(ctx.h, C.byref(g), q * p, d_ptr, ptr(values), ptr(pmaps)))
+        else:
+            _check(ctx.h, lib.sd_hog_distance_transform(ctx.h, C.byref(g), q * p, d_ptr, int(R), ptr(values), None))
     else:
         raw = values = torch.zeros(1, dtype=torch.float32, device=dev)
+        pmaps = torch.zeros((1, 2), dtype=torch.int32, device=dev)
     mc, anchors = model._c(dev)
     md = int(max_detections)
     out = torch.empty((n, max(md, 1), len(HogDetectionC._fields_)), dtype=torch.int32, device=dev)
@@ -2093,8 +2105,12 @@ def vl_hog_part_detect(frames, scales, model: HogPartModel, cell_size: int, num_
     _check(ctx.h, lib.sd_hog_detections(ctx.h, ptr(total), ptr(score_table), len(kept), n, int(q), int(cell_size), int(fw), int(fh),
                                         model.pad[0], model.pad[1], float(threshold), float(overlap), int(max_candidates), md,
                                         ptr(out), ptr(count), ptr(above)))
-    _check(ctx.h, lib.sd_hog_part_placements(ctx.h, ptr(raw), ptr(table), len(kept), C.byref(mc), d_ptr, R, int(cell_size), ptr(out),
-                                             ptr(count), n, md, ptr(place)))
+    if R is None:
+        _check(ctx.h, lib.sd_hog_part_placements_mapped(ctx.h, ptr(values), ptr(pmaps), ptr(table), len(kept), C.byref(mc),
+                                                        int(cell_size), ptr(out), ptr(count), n, md, ptr(place)))
+    else:
+        _check(ctx.h, lib.sd_hog_part_placements(ctx.h, ptr(raw), ptr(table), len(kept), C.byref(mc), d_ptr, int(R), int(cell_size),
+                                                 ptr(out), ptr(count), n, md, ptr(place)))
     return _part_detections(_detections(out, count, above), place.cpu().numpy())
 
 

@@ -1,5 +1,6 @@
-// Deformable part models over HOG pyramids (sd_hog_distance_transform, sd_hog_part_scores, sd_hog_part_placements): the bounded
-// generalised distance transform of part score maps, the star model's score maps, and the part boxes of each detection.
+// Deformable part models over HOG pyramids (sd_hog_distance_transform, sd_hog_distance_transform_exact, sd_hog_part_scores,
+// sd_hog_part_placements, sd_hog_part_placements_mapped): the bounded and the exact generalised distance transforms of part score
+// maps, the star model's score maps, and the part boxes of each detection.
 //
 //   dt_tile_kernel        one CTA per 32 x 32 output tile of one plane: the tile's rows with R rows of halo above and below and
 //                         R columns either side are staged in shared memory, pass X runs over every staged row (32 columns),
@@ -8,10 +9,19 @@
 //   part_place_kernel     one warp per (detection, part): the rule of dt_tile_kernel at the one anchor, through dt_take again,
 //                         so that the placement is bit for bit the transform's.
 //
+//   dt_exact_kernel<X>    (sd_hog_distance_transform_exact) one warp per block of 32 rows of one plane, a row per lane: the
+//                         block is staged through shared memory 32 columns at a time, so every global access is a whole row
+//                         segment; each lane builds its row's lower envelope and then writes the row's values.
+//   dt_exact_kernel<Y>    one warp per block of 32 adjacent columns, a column per lane: every step reads and writes 32
+//                         consecutive floats, in place on pass X's output.
+//   part_mapped_kernel    (sd_hog_part_placements_mapped) one thread per (detection, part): the transform's value and
+//                         placement at the anchor.
+//
 // Every kernel walks a flat list of work items with a grid-stride loop over blockIdx.x; no count is bound by gridDim.y / z.
 // There are no atomics: each output element is written by one thread.
 //
-// Scratch (SD_WS_PARTS): the cost tables, the per-map first tiles of a table route, and the placements' per-detection map index.
+// Scratch (SD_WS_PARTS): the cost tables or deformations, the per-map first tiles or line blocks of a table route, the
+// placements' per-detection map index, and the envelopes of lines too long for shared memory.
 #include "sd_internal.cuh"
 
 #include <algorithm>
@@ -136,6 +146,156 @@ __global__ void __launch_bounds__(kThreads) dt_tile_kernel(const __grid_constant
     }
 }
 
+// ---- the exact transform --------------------------------------------------------------------------------------------------------
+// The header's rule, in its operation order: every double operation is an explicit _rn intrinsic, so nvcc contracts nothing
+// into an FMA and tests/hog_dt_exact_ref.py reproduces each rounding.
+
+constexpr int kExactWarps = 4;        // warps per CTA of the exact passes
+constexpr int kEnvShared = 32;        // lines of at most this many positions keep their envelopes in shared memory
+constexpr int kTileStride = 33;       // pass X's staging tiles: 32 x 32 with a padded row, conflict-free either way
+constexpr int kEnvBytes = 20;         // per envelope entry: z (double), index, score, pass X's placement (int32 each)
+
+// cost of displacement d: (float)((double) w0 d d + (double) w1 d), the bounded call's cost-table formula
+__device__ __forceinline__ float dt_exact_cost(double a, double b, int d)
+{
+    const double x = (double)d;
+    return __double2float_rn(__dadd_rn(__dmul_rn(__dmul_rn(a, x), x), __dmul_rn(b, x)));
+}
+
+// the first position r (> q) owns against q: p* = (((f(q) - f(r)) + a (r - q)(r + q)) + b (r - q)) / ((a + a)(r - q))
+__device__ __forceinline__ double dt_exact_meet(int q, float fq, int r, float fr, double a, double b)
+{
+    const double dq = (double)(r - q), sq = (double)((long long)(r - q) * (long long)(r + q));
+    const double num = __dadd_rn(__dadd_rn(__dsub_rn((double)fq, (double)fr), __dmul_rn(a, sq)), __dmul_rn(b, dq));
+    return __ddiv_rn(num, __dmul_rn(__dadd_rn(a, a), dq));
+}
+
+struct ExactArgs {
+    const float* in;              // pass X: the maps at each grid's offset; pass Y: d_values at out_offset
+    float* out;                   // d_values
+    int* place;                   // d_place as int32 (u, v) pairs, or null; pass X leaves each row's owner in u
+    const sd_hog_grid* grids;     // null: equally sized maps
+    int width, height;            // equally sized maps
+    int num_maps, P;
+    const float* deformation;     // [P][4]
+    const long long* item0;       // table route: each map's first line block
+    long long total_items;
+    unsigned char* env;           // scratch route: nmax entries per lane of every warp of the grid; null: shared memory
+    int nmax;                     // the longest line of the pass
+};
+
+// One pass over every line of every plane: kY = false, rows (pass X); kY = true, columns (pass Y).  A lane's envelope is
+// entries [0, cnt): owner index v, its score f, and z, the point past which it owns (z[0] = -inf); the entries of a warp are
+// interleaved, entry i of lane l at i * 32 + l.
+template <bool kY>
+__global__ void __launch_bounds__(kExactWarps * 32) dt_exact_kernel(const __grid_constant__ ExactArgs a)
+{
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const size_t tile_bytes = kY ? 0 : 2 * 32 * kTileStride * sizeof(float);
+    unsigned char* wsm = smem + (size_t)wid * (tile_bytes + (a.env ? 0 : (size_t)kEnvBytes * a.nmax * 32));
+    float* tile = reinterpret_cast<float*>(wsm);                 // pass X: 32 x 32 scores, then 32 x 32 owners
+    int* otile = reinterpret_cast<int*>(tile + 32 * kTileStride);
+    const long long gw = (long long)blockIdx.x * kExactWarps + wid;
+    unsigned char* env = a.env ? a.env + (size_t)gw * kEnvBytes * a.nmax * 32 : wsm + tile_bytes;
+    double* ez = reinterpret_cast<double*>(env) + lane;
+    int* ev = reinterpret_cast<int*>(env + (size_t)8 * a.nmax * 32) + lane;
+    float* ef = reinterpret_cast<float*>(ev + a.nmax * 32);
+    int* ex = ev + 2 * a.nmax * 32;
+
+    for (long long it = gw; it < a.total_items; it += (long long)gridDim.x * kExactWarps) {
+        int m, w, h;
+        long long ibase, obase, local;
+        if (a.grids) {
+            m = sd_find_last_le(0, a.num_maps - 1, it, [&](int i) { return __ldg(a.item0 + i); });
+            const sd_hog_grid g = a.grids[m];
+            w = g.width; h = g.height; obase = g.out_offset; ibase = kY ? g.out_offset : g.offset;
+            local = it - __ldg(a.item0 + m);
+        } else {
+            w = a.width; h = a.height;
+            const long long per = (long long)a.P * (((kY ? w : h) + 31) / 32);
+            m = (int)(it / per);
+            local = it - (long long)m * per;
+            ibase = obase = (long long)m * a.P * w * h;
+        }
+        const int n = kY ? h : w, lines = kY ? w : h, blocks = (lines + 31) / 32;
+        const int k = (int)(local / blocks), l0 = (int)(local - (long long)k * blocks) * 32, line = l0 + lane;
+        const bool live = line < lines;
+        const long long plane = (long long)k * w * h;
+        const float* src = a.in + ibase + plane;
+        float* dst = a.out + obase + plane;
+        int* place = a.place ? a.place + 2 * (obase + plane) : nullptr;
+        const double wa = (double)__ldg(a.deformation + 4 * k + (kY ? 2 : 0)), wb = (double)__ldg(a.deformation + 4 * k + (kY ? 3 : 1));
+        // position i of this lane's line, as a float offset from the plane
+        auto at = [&](int i) { return kY ? (long long)i * w + line : (long long)line * w + i; };
+
+        // the envelope, candidates in ascending position
+        int cnt = 0;
+        for (int i0 = 0; i0 < n; i0 += 32) {
+            const int len = min(32, n - i0);
+            if (!kY) {
+                __syncwarp();
+                for (int r = 0; r < 32 && l0 + r < lines; ++r)
+                    if (lane < len) tile[r * kTileStride + lane] = src[(long long)(l0 + r) * w + i0 + lane];
+                __syncwarp();
+            }
+            if (!live) continue;
+            for (int j = 0; j < len; ++j) {
+                const int q = i0 + j;
+                const float fq = kY ? src[at(q)] : tile[lane * kTileStride + j];
+                if (!isfinite(fq)) continue;
+                double s = -INFINITY;
+                while (cnt > 0) {
+                    s = dt_exact_meet(ev[(cnt - 1) * 32], ef[(cnt - 1) * 32], q, fq, wa, wb);
+                    if (s > ez[(cnt - 1) * 32]) break;
+                    --cnt;
+                    s = -INFINITY;
+                }
+                ez[cnt * 32] = s;
+                ev[cnt * 32] = q;
+                ef[cnt * 32] = fq;
+                if (kY && place) ex[cnt * 32] = place[2 * at(q)];
+                ++cnt;
+            }
+        }
+
+        // the values: position p belongs to the last entry whose z is below p
+        int e = 0;
+        for (int i0 = 0; i0 < n; i0 += 32) {
+            const int len = min(32, n - i0);
+            if (!kY) __syncwarp();                                // every lane is done reading the tiles
+            if (live)
+                for (int j = 0; j < len; ++j) {
+                    const int p = i0 + j;
+                    float val = -INFINITY;
+                    int q = -1;
+                    if (cnt > 0) {
+                        while (e + 1 < cnt && ez[(e + 1) * 32] < (double)p) ++e;
+                        q = ev[e * 32];
+                        val = __fsub_rn(ef[e * 32], dt_exact_cost(wa, wb, q - p));
+                    }
+                    if (kY) {
+                        dst[at(p)] = val;
+                        if (place) reinterpret_cast<int2*>(place)[at(p)] = q < 0 ? make_int2(-1, -1) : make_int2(ex[e * 32], q);
+                    } else {
+                        tile[lane * kTileStride + j] = val;
+                        otile[lane * kTileStride + j] = q;
+                    }
+                }
+            if (!kY) {
+                __syncwarp();
+                for (int r = 0; r < 32 && l0 + r < lines; ++r)
+                    if (lane < len) {
+                        const long long o = (long long)(l0 + r) * w + i0 + lane;
+                        dst[o] = tile[r * kTileStride + lane];
+                        if (place) place[2 * o] = otile[r * kTileStride + lane];
+                    }
+                __syncwarp();
+            }
+        }
+    }
+}
+
 // ---- the star model's scores --------------------------------------------------------------------------------------------------
 
 struct ScoreArgs {
@@ -250,6 +410,51 @@ __global__ void __launch_bounds__(kPlaceWarps * 32) part_place_kernel(const __gr
     }
 }
 
+struct MappedArgs {
+    const float* values;          // the transform's values and (u, v) placements, at the table's part_offset
+    const int2* place;
+    const sd_hog_part_map* maps;
+    const int32_t* anchors;
+    const sd_hog_detection* det;
+    const int32_t* count;
+    const int32_t* slot_map;
+    sd_hog_part_placement* out;
+    int num_frames, max_det, P, cell, pfw, pfh, pad_x, pad_y, part_pad_x, part_pad_y;
+};
+
+__global__ void __launch_bounds__(kThreads) part_mapped_kernel(const __grid_constant__ MappedArgs a)
+{
+    const long long items = (long long)a.num_frames * a.max_det * a.P;
+    for (long long it = (long long)blockIdx.x * kThreads + threadIdx.x; it < items; it += (long long)gridDim.x * kThreads) {
+        const long long slot = it / a.P;
+        const int p = (int)(it - slot * a.P);
+        const int f = (int)(slot / a.max_det), k = (int)(slot - (long long)f * a.max_det);
+        if (k >= __ldg(a.count + f)) continue;
+        const sd_hog_detection det = a.det[slot];
+        const sd_hog_part_map d = a.maps[__ldg(a.slot_map + slot)];
+        const int kp = det.filter * a.P + p;
+        const int2 an = __ldg(reinterpret_cast<const int2*>(a.anchors) + kp);
+        const long long u0 = 2LL * (det.cell_x - a.pad_x) + an.x + a.part_pad_x, v0 = 2LL * (det.cell_y - a.pad_y) + an.y + a.part_pad_y;
+        sd_hog_part_placement r;
+        r.u = r.v = -1;
+        r.term = -INFINITY;
+        r.x = r.y = r.w = r.h = 0;
+        if (u0 >= 0 && u0 < d.part_width && v0 >= 0 && v0 < d.part_height) {
+            const long long o = d.part_offset + ((long long)kp * d.part_height + v0) * d.part_width + u0;
+            const int2 pl = a.place[o];
+            r.term = a.values[o];
+            if (pl.x >= 0) {
+                r.u = pl.x;
+                r.v = pl.y;
+                const sd_box64 b = sd_window_box(r.u, r.v, a.part_pad_x, a.part_pad_y, a.pfw, a.pfh, a.cell, d.frame_w, d.frame_h,
+                                                 d.part_level_w, d.part_level_h);
+                r.x = (int)b.x0; r.y = (int)b.y0; r.w = (int)(b.x1 - b.x0); r.h = (int)(b.y1 - b.y0);
+            }
+        }
+        a.out[it] = r;
+    }
+}
+
 // cost tables of num_planes deformations: cx[d] = (float)((double)w0 d^2 + (double)w1 d), cy alike with w2, w3
 bool cost_tables(const float* h_def, int num_planes, int R, std::vector<float>& costs)
 {
@@ -290,6 +495,67 @@ int part_tiles(sd_ctx* ctx, const std::vector<sd_hog_part_map>& table, int Q, st
     }
     *total = tiles;
     return SD_OK;
+}
+
+// The checks both placement calls make of their table and detections, with the detections read back once: slot_map receives
+// each detection's table entry, *work the number of detections.
+int placement_slots(sd_ctx* ctx, const sd_hog_part_map* d_maps, int num_maps, const sd_hog_part_model* model, int cell_size,
+                    const sd_hog_detection* d_det, const int32_t* d_count, int num_frames, int max_detections,
+                    std::vector<int32_t>& slot_map, long long* work)
+{
+    const int Q = model->num_components;
+    std::vector<sd_hog_part_map> table;
+    if (num_maps > 0)
+        if (const int rc = sd_fetch_table(ctx, d_maps, num_maps, table)) return rc;
+    std::vector<long long> tile0;
+    long long tiles = 0;
+    if (const int rc = part_tiles(ctx, table, Q, tile0, &tiles)) return rc;
+    std::map<std::pair<int, int>, int> index;
+    for (int i = 0; i < num_maps; ++i) {
+        const sd_hog_part_map& d = table[i];
+        SD_REQUIRE(ctx, d.frame >= 0 && d.frame < num_frames, "a map's frame is out of range");
+        SD_REQUIRE(ctx, d.frame_w >= 1 && d.frame_h >= 1 && d.part_level_w >= 1 && d.part_level_h >= 1,
+                   "a map's frame or part level is smaller than 1 x 1");
+        SD_REQUIRE(ctx, index.emplace(std::make_pair(d.frame, d.level), i).second, "two maps share one (frame, level)");
+        SD_REQUIRE(ctx, sd_window_boxes_fit_int32(d.part_width, d.part_height, model->part_pad_x, model->part_pad_y, model->part_w,
+                                                  model->part_h, cell_size, d.frame_w, d.frame_h, d.part_level_w, d.part_level_h),
+                   "a map's part boxes do not fit in int32");
+    }
+    // the detections, read back once: each must come from a map of the table
+    const size_t slots = (size_t)num_frames * max_detections;
+    std::vector<int32_t> count(num_frames);
+    std::vector<sd_hog_detection> det(slots);
+    SD_CUDA(ctx, cudaMemcpyAsync(count.data(), d_count, sizeof(int32_t) * num_frames, cudaMemcpyDeviceToHost, ctx->stream));
+    SD_CUDA(ctx, cudaMemcpyAsync(det.data(), d_det, sizeof(sd_hog_detection) * slots, cudaMemcpyDeviceToHost, ctx->stream));
+    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    slot_map.assign(slots, 0);
+    *work = 0;
+    for (int f = 0; f < num_frames; ++f) {
+        SD_REQUIRE(ctx, count[f] >= 0 && count[f] <= max_detections, "a frame's detection count is outside [0, max_detections]");
+        for (int k = 0; k < count[f]; ++k) {
+            const sd_hog_detection& r = det[(size_t)f * max_detections + k];
+            const auto it = index.find(std::make_pair(f, (int)r.level));
+            SD_REQUIRE(ctx, it != index.end(), "a detection's (frame, level) is not in the table");
+            const sd_hog_part_map& d = table[it->second];
+            SD_REQUIRE(ctx, r.filter >= 0 && r.filter < Q && r.cell_x >= 0 && r.cell_x < d.width && r.cell_y >= 0 && r.cell_y < d.height,
+                       "a detection's filter or score position is not one of its map");
+            slot_map[(size_t)f * max_detections + k] = it->second;
+            ++*work;
+        }
+    }
+    return SD_OK;
+}
+
+// the first line block of each map of a table, in pass X (rows) or pass Y (columns)
+long long exact_items(const std::vector<sd_hog_grid>& table, int P, bool columns, std::vector<long long>& item0)
+{
+    long long items = 0;
+    item0.resize(table.size());
+    for (size_t i = 0; i < table.size(); ++i) {
+        item0[i] = items;
+        items += (long long)P * sd_div_up(columns ? table[i].width : table[i].height, 32);
+    }
+    return items;
 }
 
 }  // namespace
@@ -414,47 +680,13 @@ int sd_hog_part_placements(sd_ctx* ctx, const float* d_parts, const sd_hog_part_
     const int Q = model->num_components, P = model->num_parts, R = max_displacement;
     std::vector<float> costs;
     SD_REQUIRE(ctx, cost_tables(h_deformation, Q * P, R, costs), "a cost table entry is not finite");
-
-    std::vector<sd_hog_part_map> table;
-    if (num_maps > 0)
-        if (const int rc = sd_fetch_table(ctx, d_maps, num_maps, table)) return rc;
-    std::vector<long long> tile0;
-    long long tiles = 0;
-    if (const int rc = part_tiles(ctx, table, Q, tile0, &tiles)) return rc;
-    std::map<std::pair<int, int>, int> index;
-    for (int i = 0; i < num_maps; ++i) {
-        const sd_hog_part_map& d = table[i];
-        SD_REQUIRE(ctx, d.frame >= 0 && d.frame < num_frames, "a map's frame is out of range");
-        SD_REQUIRE(ctx, d.frame_w >= 1 && d.frame_h >= 1 && d.part_level_w >= 1 && d.part_level_h >= 1,
-                   "a map's frame or part level is smaller than 1 x 1");
-        SD_REQUIRE(ctx, index.emplace(std::make_pair(d.frame, d.level), i).second, "two maps share one (frame, level)");
-        SD_REQUIRE(ctx, sd_window_boxes_fit_int32(d.part_width, d.part_height, model->part_pad_x, model->part_pad_y, model->part_w,
-                                                  model->part_h, cell_size, d.frame_w, d.frame_h, d.part_level_w, d.part_level_h),
-                   "a map's part boxes do not fit in int32");
-    }
-    // the detections, read back once: each must come from a map of the table
-    const size_t slots = (size_t)num_frames * max_detections;
-    std::vector<int32_t> count(num_frames);
-    std::vector<sd_hog_detection> det(slots);
-    SD_CUDA(ctx, cudaMemcpyAsync(count.data(), d_count, sizeof(int32_t) * num_frames, cudaMemcpyDeviceToHost, ctx->stream));
-    SD_CUDA(ctx, cudaMemcpyAsync(det.data(), d_det, sizeof(sd_hog_detection) * slots, cudaMemcpyDeviceToHost, ctx->stream));
-    SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    std::vector<int32_t> slot_map(slots, 0);
+    std::vector<int32_t> slot_map;
     long long work = 0;
-    for (int f = 0; f < num_frames; ++f) {
-        SD_REQUIRE(ctx, count[f] >= 0 && count[f] <= max_detections, "a frame's detection count is outside [0, max_detections]");
-        for (int k = 0; k < count[f]; ++k) {
-            const sd_hog_detection& r = det[(size_t)f * max_detections + k];
-            const auto it = index.find(std::make_pair(f, (int)r.level));
-            SD_REQUIRE(ctx, it != index.end(), "a detection's (frame, level) is not in the table");
-            const sd_hog_part_map& d = table[it->second];
-            SD_REQUIRE(ctx, r.filter >= 0 && r.filter < Q && r.cell_x >= 0 && r.cell_x < d.width && r.cell_y >= 0 && r.cell_y < d.height,
-                       "a detection's filter or score position is not one of its map");
-            slot_map[(size_t)f * max_detections + k] = it->second;
-            ++work;
-        }
-    }
+    if (const int rc = placement_slots(ctx, d_maps, num_maps, model, cell_size, d_det, d_count, num_frames, max_detections, slot_map,
+                                       &work))
+        return rc;
     if (work == 0) return SD_OK;
+    const size_t slots = slot_map.size();
 
     const size_t cost_bytes = sd_round16(sizeof(float) * costs.size());
     unsigned char* ws = static_cast<unsigned char*>(sd_workspace(ctx, SD_WS_PARTS, cost_bytes + sizeof(int32_t) * slots));
@@ -484,6 +716,136 @@ int sd_hog_part_placements(sd_ctx* ctx, const float* d_parts, const sd_hog_part_
     const int smem = kPlaceWarps * 2 * (2 * R + 1) * (int)sizeof(float);
     part_place_kernel<<<grid, kPlaceWarps * 32, smem, ctx->stream>>>(a);
     SD_LAUNCH_CHECK(ctx, "part_place_kernel");
+    return SD_OK;
+}
+
+int sd_hog_distance_transform_exact(sd_ctx* ctx, const sd_hog_grids* maps, int num_planes, const float* h_deformation, float* d_values,
+                                    int32_t* d_place)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, maps && h_deformation && d_values, "null argument");
+    SD_REQUIRE(ctx, maps->count >= 0, "negative map count");
+    SD_REQUIRE(ctx, maps->count == 0 || (maps->d_features && sd_aligned(maps->d_features, 4)), "maps must be non-null and 4-byte aligned");
+    SD_REQUIRE(ctx, sd_aligned(d_values, 4) && sd_aligned(d_place, 8), "values must be 4-byte aligned and placements 8-byte aligned");
+    SD_REQUIRE(ctx, num_planes >= 1 && num_planes <= SD_HOG_FILTER_MAX_BANK, "num_planes must be in [1, SD_HOG_FILTER_MAX_BANK]");
+    for (int i = 0; i < 4 * num_planes; ++i)
+        SD_REQUIRE(ctx, std::isfinite(h_deformation[i]) && (i % 2 == 1 || h_deformation[i] > 0),
+                   "every deformation weight must be finite, with w0 > 0 and w2 > 0");
+    if (maps->count == 0) return SD_OK;
+    int max_w = 0, max_h = 0;
+    std::vector<sd_hog_grid> table;
+    if (const int rc = sd_read_hog_grids(ctx, __func__, maps, &max_w, &max_h, maps->d_grids ? &table : nullptr)) return rc;
+    std::vector<long long> item0[2];
+    long long items[2];
+    for (int y = 0; y < 2; ++y)
+        items[y] = maps->d_grids ? exact_items(table, num_planes, y == 1, item0[y])
+                                 : (long long)maps->count * num_planes * sd_div_up(y ? maps->width : maps->height, 32);
+    if (items[0] == 0) return SD_OK;
+
+    // scratch: the deformations, each pass's first line blocks, then the envelopes of a pass whose lines do not fit in shared
+    // memory (kEnvBytes per position of the longest line, for each lane of each warp of the grid; at most kEnvBudget bytes
+    // unless one CTA needs more)
+    constexpr size_t kEnvBudget = size_t(256) << 20;
+    const int nmax[2] = {max_w, max_h};
+    int grid[2];
+    size_t env_at = sd_round16(sizeof(float) * 4 * num_planes), items_at[2];
+    for (int y = 0; y < 2; ++y) {
+        items_at[y] = env_at;
+        env_at += sd_round16(sizeof(long long) * item0[y].size());
+    }
+    size_t env_bytes = 0;
+    for (int y = 0; y < 2; ++y) {
+        const size_t per_cta = (size_t)kExactWarps * 32 * kEnvBytes * nmax[y];
+        long long ctas = std::min<long long>(sd_div_up(items[y], kExactWarps), 8LL * ctx->sm_count);
+        if (nmax[y] > kEnvShared) {
+            ctas = std::max<long long>(1, std::min<long long>(ctas, (long long)(kEnvBudget / per_cta)));
+            env_bytes = std::max(env_bytes, (size_t)ctas * per_cta);
+        }
+        grid[y] = (int)ctas;
+    }
+    unsigned char* ws = static_cast<unsigned char*>(sd_workspace(ctx, SD_WS_PARTS, env_at + env_bytes));
+    if (!ws) return SD_ERR_CUDA;
+    SD_CUDA(ctx, cudaMemcpyAsync(ws, h_deformation, sizeof(float) * 4 * num_planes, cudaMemcpyHostToDevice, ctx->stream));
+    for (int y = 0; y < 2; ++y)
+        if (!item0[y].empty())
+            SD_CUDA(ctx, cudaMemcpyAsync(ws + items_at[y], item0[y].data(), sizeof(long long) * item0[y].size(), cudaMemcpyHostToDevice,
+                                         ctx->stream));
+    for (int y = 0; y < 2; ++y) {
+        ExactArgs a;
+        memset(&a, 0, sizeof(a));
+        a.in = y ? d_values : maps->d_features;
+        a.out = d_values;
+        a.place = d_place;
+        a.grids = maps->d_grids;
+        a.width = maps->width;
+        a.height = maps->height;
+        a.num_maps = maps->count;
+        a.P = num_planes;
+        a.deformation = reinterpret_cast<const float*>(ws);
+        a.item0 = reinterpret_cast<const long long*>(ws + items_at[y]);
+        a.total_items = items[y];
+        a.nmax = nmax[y];
+        a.env = nmax[y] > kEnvShared ? ws + env_at : nullptr;
+        const int smem = kExactWarps * ((y ? 0 : 2 * 32 * kTileStride * (int)sizeof(float)) + (a.env ? 0 : kEnvBytes * 32 * nmax[y]));
+        if (y) {
+            SD_CUDA(ctx, cudaFuncSetAttribute(dt_exact_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            dt_exact_kernel<true><<<grid[y], kExactWarps * 32, smem, ctx->stream>>>(a);
+            SD_LAUNCH_CHECK(ctx, "dt_exact_kernel<Y>");
+        } else {
+            SD_CUDA(ctx, cudaFuncSetAttribute(dt_exact_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            dt_exact_kernel<false><<<grid[y], kExactWarps * 32, smem, ctx->stream>>>(a);
+            SD_LAUNCH_CHECK(ctx, "dt_exact_kernel<X>");
+        }
+    }
+    return SD_OK;
+}
+
+int sd_hog_part_placements_mapped(sd_ctx* ctx, const float* d_values, const int32_t* d_place, const sd_hog_part_map* d_maps,
+                                  int num_maps, const sd_hog_part_model* model, int cell_size, const sd_hog_detection* d_det,
+                                  const int32_t* d_count, int num_frames, int max_detections, sd_hog_part_placement* d_out)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    if (const int rc = check_model(ctx, model)) return rc;
+    SD_REQUIRE(ctx, d_det && d_count && d_out && (num_maps == 0 || (d_values && d_place && d_maps)), "null argument");
+    SD_REQUIRE(ctx, sd_aligned(d_values, 4) && sd_aligned(d_place, 8) && sd_aligned(d_maps, 8) && sd_aligned(d_det, 4) &&
+                        sd_aligned(d_count, 4) && sd_aligned(d_out, 4),
+               "values, detections, counts and output must be 4-byte aligned, the placements and the map table 8-byte aligned");
+    SD_REQUIRE(ctx, num_maps >= 0, "negative map count");
+    SD_REQUIRE(ctx, num_frames >= 1, "num_frames must be >= 1");
+    SD_REQUIRE(ctx, max_detections >= 1 && max_detections <= SD_HOG_DETECT_MAX_CANDIDATES,
+               "max_detections must be in [1, SD_HOG_DETECT_MAX_CANDIDATES]");
+    SD_REQUIRE(ctx, cell_size >= 1 && cell_size <= kDenseMaxCell, "cell_size must be in [1,32]");
+    std::vector<int32_t> slot_map;
+    long long work = 0;
+    if (const int rc = placement_slots(ctx, d_maps, num_maps, model, cell_size, d_det, d_count, num_frames, max_detections, slot_map,
+                                       &work))
+        return rc;
+    if (work == 0) return SD_OK;
+    const size_t slots = slot_map.size();
+    int32_t* ws = static_cast<int32_t*>(sd_workspace(ctx, SD_WS_PARTS, sizeof(int32_t) * slots));
+    if (!ws) return SD_ERR_CUDA;
+    SD_CUDA(ctx, cudaMemcpyAsync(ws, slot_map.data(), sizeof(int32_t) * slots, cudaMemcpyHostToDevice, ctx->stream));
+    MappedArgs a;
+    memset(&a, 0, sizeof(a));
+    a.values = d_values;
+    a.place = reinterpret_cast<const int2*>(d_place);
+    a.maps = d_maps;
+    a.anchors = model->d_anchors;
+    a.det = d_det;
+    a.count = d_count;
+    a.slot_map = ws;
+    a.out = d_out;
+    a.num_frames = num_frames;
+    a.max_det = max_detections;
+    a.P = model->num_parts;
+    a.cell = cell_size;
+    a.pfw = model->part_w; a.pfh = model->part_h;
+    a.pad_x = model->pad_x; a.pad_y = model->pad_y;
+    a.part_pad_x = model->part_pad_x; a.part_pad_y = model->part_pad_y;
+    const long long items = (long long)slots * model->num_parts;
+    const int grid = (int)std::min<long long>((items + kThreads - 1) / kThreads, 16LL * ctx->sm_count);
+    part_mapped_kernel<<<grid, kThreads, 0, ctx->stream>>>(a);
+    SD_LAUNCH_CHECK(ctx, "part_mapped_kernel");
     return SD_OK;
 }
 

@@ -503,7 +503,9 @@ inline std::vector<std::vector<hog_detection>> vl_hog_detect(const std::vector<c
 // A star model for vl_hog_part_detect (include/sd_b200.h, sd_hog_part_model): Q root filters with their bias, and per component
 // P part filters scored at twice the root's resolution, in the shell's filter layout (dd * fh rows of fw floats); anchors[q][p]
 // = (ax, ay) in part-level cells relative to twice the root window's top-left cell; deformation[q][p] = (w0, w1, w2, w3), a
-// displacement (dx, dy) costing w0 dx^2 + w1 dx + w2 dy^2 + w3 dy; the root and part pads; R = max_displacement.
+// displacement (dx, dy) costing w0 dx^2 + w1 dx + w2 dy^2 + w3 dy; the root and part pads; R = max_displacement bounding |dx|
+// and |dy|, or, with unbounded, the exact transform of DPM (sd_hog_distance_transform_exact: no bound, w0 > 0 and w2 > 0;
+// max_displacement is then ignored).
 struct hog_part_model {
     std::vector<cv::Mat> root;
     std::vector<float> bias;
@@ -512,6 +514,7 @@ struct hog_part_model {
     std::vector<std::vector<std::array<float, 4>>> deformation;
     int pad_x = 0, pad_y = 0, part_pad_x = 0, part_pad_y = 0;
     int max_displacement = 4;
+    bool unbounded = false;
 };
 
 // One part of a detection: its box in frame pixels (empty where it has no placement), its placement (u, v) in part score
@@ -529,7 +532,7 @@ struct hog_part_detection {
 // A star-model detector over image pyramids: vl_hog_pyramid over the root scales and their doubles (a scale present in both is
 // computed once; root scales must be in (0, 2]), vl_hog_correlate of the roots and of all Q * P parts, then on the device
 // sd_hog_distance_transform, sd_hog_part_scores, sd_hog_detections (the root's filter size and pad, all components as one
-// class) and sd_hog_part_placements.  multichannel and bilinear_orientations as vl_hog_pyramid takes them: a model of colour
+// class) and sd_hog_part_placements; an unbounded model takes sd_hog_distance_transform_exact and sd_hog_part_placements_mapped.  multichannel and bilinear_orientations as vl_hog_pyramid takes them: a model of colour
 // HOG is scored with the values it was built for.  Returns one list per frame, in the rule's order; each detection's box is
 // what detect_faces takes.  Throws std::runtime_error for a model of inconsistent shapes and where those calls refuse.
 inline std::vector<std::vector<hog_part_detection>> vl_hog_part_detect(const std::vector<cv::Mat>& images, const std::vector<double>& scales,
@@ -597,7 +600,7 @@ inline std::vector<std::vector<hog_part_detection>> vl_hog_part_detect(const std
         part_maps.empty() ? std::vector<cv::Mat>() : vl_hog_correlate(part_maps, part_filters, variant, num_bins, {}, model.part_pad_x, model.part_pad_y);
     sd_ctx* ctx = sd_b200::context();
     // the part score maps on the device, their transform at the same offsets
-    sd_b200::DeviceBuffer d_raw, d_values, d_grids;
+    sd_b200::DeviceBuffer d_raw, d_values, d_place, d_grids;
     std::vector<cv::Mat> pplanes;
     std::vector<int> pslot(part_scores.size(), -1);   // each part level's place among the maps with scores
     for (size_t k = 0; k < part_scores.size(); ++k)
@@ -614,6 +617,7 @@ inline std::vector<std::vector<hog_part_detection>> vl_hog_part_detect(const std
     }
     d_raw.allocate(static_cast<size_t>(std::max<int64_t>(raw_floats, 1)) * sizeof(float));
     d_values.allocate(static_cast<size_t>(std::max<int64_t>(raw_floats, 1)) * sizeof(float));
+    if (model.unbounded) d_place.allocate(static_cast<size_t>(std::max<int64_t>(raw_floats, 1)) * 2 * sizeof(int32_t));
     if (!grids.empty()) {
         d_grids.allocate(grids.size() * sizeof(sd_hog_grid));
         sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_grids.as<sd_hog_grid>(), grids.data(), grids.size() * sizeof(sd_hog_grid)), "vl_hog_part_detect upload");
@@ -621,8 +625,12 @@ inline std::vector<std::vector<hog_part_detection>> vl_hog_part_detect(const std
         g.d_features = d_raw.as<float>();
         g.count = static_cast<int32_t>(grids.size());
         g.d_grids = d_grids.as<sd_hog_grid>();
-        sd_b200::check(ctx, sd_hog_distance_transform(ctx, &g, Q * P, deformation.data(), model.max_displacement, d_values.as<float>(), nullptr),
-                       "sd_hog_distance_transform");
+        if (model.unbounded)
+            sd_b200::check(ctx, sd_hog_distance_transform_exact(ctx, &g, Q * P, deformation.data(), d_values.as<float>(), d_place.as<int32_t>()),
+                           "sd_hog_distance_transform_exact");
+        else
+            sd_b200::check(ctx, sd_hog_distance_transform(ctx, &g, Q * P, deformation.data(), model.max_displacement, d_values.as<float>(), nullptr),
+                           "sd_hog_distance_transform");
     }
     // the root scores and the star model's scores at the same offsets
     std::vector<cv::Mat> planes;
@@ -683,9 +691,14 @@ inline std::vector<std::vector<hog_part_detection>> vl_hog_part_detect(const std
     sd_b200::check(ctx, sd_hog_detections(ctx, d_total.as<float>(), d_maps.as<sd_hog_score_map>(), nm, n, Q, cell_size, m.filter_w, m.filter_h,
                                           m.pad_x, m.pad_y, threshold, overlap, max_candidates, max_detections, d_out.as<sd_hog_detection>(),
                                           d_count.as<int32_t>(), nullptr), "sd_hog_detections");
-    sd_b200::check(ctx, sd_hog_part_placements(ctx, d_raw.as<float>(), d_table.as<sd_hog_part_map>(), nm, &m, deformation.data(),
-                                               model.max_displacement, cell_size, d_out.as<sd_hog_detection>(), d_count.as<int32_t>(), n,
-                                               max_detections, d_parts.as<sd_hog_part_placement>()), "sd_hog_part_placements");
+    if (model.unbounded)
+        sd_b200::check(ctx, sd_hog_part_placements_mapped(ctx, d_values.as<float>(), d_place.as<int32_t>(), d_table.as<sd_hog_part_map>(), nm, &m,
+                                                          cell_size, d_out.as<sd_hog_detection>(), d_count.as<int32_t>(), n, max_detections,
+                                                          d_parts.as<sd_hog_part_placement>()), "sd_hog_part_placements_mapped");
+    else
+        sd_b200::check(ctx, sd_hog_part_placements(ctx, d_raw.as<float>(), d_table.as<sd_hog_part_map>(), nm, &m, deformation.data(),
+                                                   model.max_displacement, cell_size, d_out.as<sd_hog_detection>(), d_count.as<int32_t>(), n,
+                                                   max_detections, d_parts.as<sd_hog_part_placement>()), "sd_hog_part_placements");
     std::vector<sd_hog_part_placement> parts(slots * P);
     sd_b200::check(ctx, sd_memcpy_d2h(ctx, parts.data(), d_parts.as<void>(), parts.size() * sizeof(sd_hog_part_placement)), "vl_hog_part_detect download");
     std::vector<sd_hog_detection> out;
