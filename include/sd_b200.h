@@ -287,10 +287,30 @@ SD_API int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cel
  * votes, the first on a tie.  The levels go through context scratch one slice of the batch at a time, as in sd_hog_pyramid.
  * Null pointers, a dtype other than SD_HOG_U8, channels outside [1, 16], bilinear_orientations outside {0, 1}, num_scales < 1,
  * an invalid scale or configuration, a frame smaller than 1 x 1, or a negative offset or stride is SD_ERR_INVALID before any
- * work is queued (d_out is not written). */
+ * work is queued (d_out is not written).  sd_hog_pyramid_float (below) takes float frames. */
 SD_API int sd_hog_pyramid_images(sd_ctx* ctx, const sd_hog_images* images, const double* h_scales, int num_scales,
                                  int cell_size, int num_bins, int variant, int bilinear_orientations,
                                  float* d_out, const int64_t* d_out_offset);
+/* sd_hog_pyramid_float: sd_hog_pyramid_images of float frames (dtype SD_HOG_F32, d_data 4-byte aligned) with 1..16 channels, in
+ * any layout an sd_hog_images describes.  Level sizes, empty levels, limits, output layout, offsets, scratch slices and refusals
+ * are sd_hog_pyramid_images'; a dtype other than SD_HOG_F32 or an unaligned buffer is refused as well.  Each channel is resized
+ * on its own by cv::resize INTER_LINEAR's float rule, per axis of n_in -> n_out px:
+ *   - a level of the frame's own size is a bit copy of it (NaN payloads and -0 included);
+ *   - scale = 1 / (n_out / n_in) in double, f = (float)((d + 0.5) * scale - 0.5), s = floor(f), f -= s (in float);
+ *   - columns: s < 0 gives s = 0, f = 0, and s >= W - 1 gives s = W - 1, f = 0.  The row value is S[s] * (1 - f) at s = W - 1
+ *     and S[s] * (1 - f) + S[s + 1] * f otherwise: a tap of weight 0 is read and multiplied (inf * 0 is NaN, as in cv2);
+ *   - rows: f is not zeroed at the borders; y0 = clamp(s, 0, H - 1), y1 = clamp(s + 1, 0, H - 1), and the value is
+ *     t(y0) * (1 - f) + t(y1) * f;
+ *   - every product and sum is rounded on its own (no FMA), and there is no special case at exact 2x.
+ * That is cv::resize of float frames with IPP off, bit for bit, at every level except exact 2x downscales on both axes, where
+ * cv::resize switches to INTER_AREA: there it is equal at 4 channels, equal at 1 channel except on the last w mod 4 columns,
+ * and within one rounding (relative difference at most 2.4e-7) elsewhere.  IPP's own arithmetic differs from both.  Each
+ * level's features are bit for bit sd_hog_dense_images' of the resized float level with the same channels and
+ * bilinear_orientations.  Channels and their range are taken as given: VLFeat's normalisation epsilon makes the features of
+ * frames in [0, 1] and in [0, 255] differ. */
+SD_API int sd_hog_pyramid_float(sd_ctx* ctx, const sd_hog_images* images, const double* h_scales, int num_scales,
+                                int cell_size, int num_bins, int variant, int bilinear_orientations,
+                                float* d_out, const int64_t* d_out_offset);
 
 /* ---- dense HOG of a caller's gradient fields: vl_hog_put_polar_field + vl_hog_extract (hog.c:746-845, :857-1062) ----------
  * Each field is a modulus and an angle per pixel, e.g. the gradient of another operator, colour gradients combined by the
@@ -559,6 +579,13 @@ SD_API int sd_hog_train_filter_images(sd_ctx* ctx, const sd_hog_images* images, 
                                       int num_boxes, const double* h_scales, int num_scales, int cell_size, int num_bins, int variant,
                                       int filter_w, int filter_h, int pad_x, int pad_y, const sd_hog_train_param* p, float* d_filter,
                                       float* h_bias, sd_hog_train_report* h_rounds, sd_hog_window* h_negatives, int* h_num_negatives);
+/* sd_hog_train_filter_float: sd_hog_train_filter_images with the same arguments, rule, report and output, on float frames
+ * (dtype SD_HOG_F32, 4-byte aligned) whose pyramids are sd_hog_pyramid_float's; a filter trained so is scored on
+ * sd_hog_pyramid_float's features.  A dtype other than SD_HOG_F32 or an unaligned buffer is SD_ERR_INVALID as well. */
+SD_API int sd_hog_train_filter_float(sd_ctx* ctx, const sd_hog_images* images, int bilinear_orientations, const sd_hog_box* h_boxes,
+                                     int num_boxes, const double* h_scales, int num_scales, int cell_size, int num_bins, int variant,
+                                     int filter_w, int filter_h, int pad_x, int pad_y, const sd_hog_train_param* p, float* d_filter,
+                                     float* h_bias, sd_hog_train_report* h_rounds, sd_hog_window* h_negatives, int* h_num_negatives);
 
 /* ---- deformable part models: bounded distance transforms, star-model scores and the part boxes of each detection -----------
  * A star model has Q components.  Component q is a root filter (filter_w x filter_h cells) scored on a level of scale s, and P

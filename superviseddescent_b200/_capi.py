@@ -176,8 +176,9 @@ EXPORTS = [
     "sd_memcpy2d_h2d", "sd_memcpy2d_d2h", "sd_memcpy2d_d2d",
     "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_bgr2gray", "sd_upload_frames", "sd_hog_dense_shape", "sd_hog_dense",
     "sd_hog_dense_images", "sd_hog_dense_polar", "sd_hog_permutation", "sd_hog_glyphs", "sd_hog_render", "sd_hog_relayout",
-    "sd_hog_pyramid_shape", "sd_hog_pyramid", "sd_hog_pyramid_images", "sd_hog_correlate", "sd_hog_detections",
+    "sd_hog_pyramid_shape", "sd_hog_pyramid", "sd_hog_pyramid_images", "sd_hog_pyramid_float", "sd_hog_correlate", "sd_hog_detections",
     "sd_hog_windows", "sd_hog_box_windows", "sd_learn_squared_hinge", "sd_hog_train_filter", "sd_hog_train_filter_images",
+    "sd_hog_train_filter_float",
     "sd_hog_distance_transform", "sd_hog_distance_transform_exact", "sd_hog_part_scores", "sd_hog_part_placements",
     "sd_hog_part_placements_mapped",
     "sd_learn", "sd_centre_features", "sd_learn_centred", "sd_learn_rank_revealing", "sd_gram", "sd_solve_gram", "sd_predict", "sd_test_residual", "sd_solver_timings", "sd_set_gram_mode", "sd_set_solver", "sd_solver_iterations",
@@ -241,6 +242,7 @@ def lib():
         l.sd_hog_pyramid_shape.argtypes = [_i, _i, C.c_double, _i, _i, _i, _ip, _ip, _ip, _ip, _ip]
         l.sd_hog_pyramid.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_double), _i, _i, _i, _i, C.c_void_p, C.c_void_p]
         l.sd_hog_pyramid_images.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_double), _i, _i, _i, _i, _i, C.c_void_p, C.c_void_p]
+        l.sd_hog_pyramid_float.argtypes = l.sd_hog_pyramid_images.argtypes
         l.sd_hog_correlate.argtypes = [C.c_void_p, C.c_void_p, _i, _i, C.c_void_p, _i, _i, _i, C.c_void_p, _i, _i, C.c_void_p]
         l.sd_hog_detections.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, _i, _i, _i, _i, _i, _i, _i, _i, C.c_float, C.c_double,
                                         _i, _i, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -253,6 +255,7 @@ def lib():
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         l.sd_hog_train_filter_images.argtypes = [C.c_void_p, C.c_void_p, _i, C.c_void_p, _i, C.c_void_p, _i, _i, _i, _i, _i, _i, _i,
                                                  _i, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        l.sd_hog_train_filter_float.argtypes = l.sd_hog_train_filter_images.argtypes
         l.sd_hog_distance_transform.argtypes = [C.c_void_p, C.c_void_p, _i, C.c_void_p, _i, C.c_void_p, C.c_void_p]
         l.sd_hog_distance_transform_exact.argtypes = [C.c_void_p, C.c_void_p, _i, C.c_void_p, C.c_void_p, C.c_void_p]
         l.sd_hog_part_placements_mapped.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _i, C.c_void_p, _i, C.c_void_p,

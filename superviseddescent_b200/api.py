@@ -527,14 +527,17 @@ def vl_hog(images, cell_size: int, num_bins: int, variant: int = 1, bilinear_ori
                                                                                      int(variant), bil, ptr(out), ptr(offsets))))
 
 
-def _hog_images(images, channels_last: bool, ctx: Context, check):
+def _hog_images(images, channels_last: bool, ctx: Context, check, float_only: bool = False):
     """The frames of vl_hog, or of the multichannel=True route of the sliding-window calls -> (what owns their device bytes,
     their HogImagesC, [(H, W)] per frame).  A batch is read through its strides (a CUDA tensor in place, a host one after one
     copy); a list of frames is packed end to end in one device buffer after check(W, H) has accepted every size, with a
-    descriptor table when the sizes differ.  An empty list gives (None, None, [])."""
+    descriptor table when the sizes differ.  An empty list gives (None, None, []).  float_only: frames of another dtype than
+    float32 are refused before any upload."""
     dev = f"cuda:{ctx.device}"
 
     def dtype_of(t):
+        if float_only and t.dtype != torch.float32:
+            raise ValueError("float_frames=True takes float32 frames")
         if t.dtype not in _VL_HOG_DTYPES:
             raise ValueError("frames must be uint8 or float32")
         return _VL_HOG_DTYPES[t.dtype]
@@ -1542,8 +1545,19 @@ def hog_pyramid_shape(width: int, height: int, scale: float, cell_size: int, num
     return (lw, lh), (d, h, w)
 
 
+def _window_frames(frames, ctx: Context, check, multichannel: bool, bilinear_orientations: bool, float_frames: bool):
+    """The frames of vl_hog_pyramid and train_hog_filter -> (owner, batch, sizes): _hog_images' (channels last) with
+    multichannel, _grey_frames' without.  bilinear_orientations and float_frames need multichannel, and float_frames float32
+    frames."""
+    if bilinear_orientations and not multichannel:
+        raise ValueError("bilinear_orientations needs multichannel=True (grey frames pass as they are)")
+    if float_frames and not multichannel:
+        raise ValueError("float_frames needs multichannel=True (float frames keep their channels)")
+    return _hog_images(frames, True, ctx, check, float_frames) if multichannel else _grey_frames(frames, ctx, check)
+
+
 def vl_hog_pyramid(frames, scales, cell_size: int, num_bins: int, variant: int = 1, ctx: Optional[Context] = None,
-                   multichannel: bool = False, bilinear_orientations: bool = False):
+                   multichannel: bool = False, bilinear_orientations: bool = False, float_frames: bool = False):
     """Dense HOG of every frame at every scale in one call (sd_hog_pyramid): level s of a W x H frame is the frame resized by
     cv::resize INTER_LINEAR to floor(W * s + 0.5) x floor(H * s + 0.5), and its features are hog_dense's of that level.
 
@@ -1551,21 +1565,21 @@ def vl_hog_pyramid(frames, scales, cell_size: int, num_bins: int, variant: int =
     (sd_hog_pyramid_images): frames are uint8, channels last -- a host or CUDA (count, H, W) or (count, H, W, C) array or tensor
     (CUDA tensors read in place through their strides), or a list of (H, W) or (H, W, C) frames of any sizes with one C -- each
     channel is resized on its own, and at each pixel the channel with the largest gradient votes, as vl_hog does;
-    bilinear_orientations (multichannel only): every pixel votes into its two nearest orientation bins.  Returns (features,
+    bilinear_orientations (multichannel only): every pixel votes into its two nearest orientation bins.  float_frames
+    (multichannel only, sd_hog_pyramid_float): the frames are float32 in the same layouts, each channel resized by
+    cv::resize's float INTER_LINEAR rule (include/sd_b200.h), its values and range taken as given.  Returns (features,
     sizes): features[f][s] is a (dd, hogH, hogW) float32 CUDA view into one buffer, or None for an empty level (smaller than
     4 px or than half a cell); sizes[f][s] = (level_w, level_h)."""
     ctx = ctx or default_context()
     scales = [float(s) for s in scales]
     if not scales:
         raise ValueError("vl_hog_pyramid needs at least one scale")
-    if bilinear_orientations and not multichannel:
-        raise ValueError("bilinear_orientations needs multichannel=True (grey frames pass as they are)")
 
     def check(w, h):
         for s in scales:
             hog_pyramid_shape(w, h, s, cell_size, num_bins, variant)
 
-    keep, ib, sizes = _hog_images(frames, True, ctx, check) if multichannel else _grey_frames(frames, ctx, check)
+    keep, ib, sizes = _window_frames(frames, ctx, check, multichannel, bilinear_orientations, float_frames)
     if not sizes:
         return [], []
     levels = [[hog_pyramid_shape(w, h, s, cell_size, num_bins, variant) for s in scales] for h, w in sizes]
@@ -1574,8 +1588,9 @@ def vl_hog_pyramid(frames, scales, cell_size: int, num_bins: int, variant: int =
     d_off = torch.tensor(offsets, dtype=torch.int64, device=dev)
     h_scales = (C.c_double * len(scales))(*scales)
     if multichannel:
-        _check(ctx.h, _capi.lib().sd_hog_pyramid_images(ctx.h, C.byref(ib), h_scales, len(scales), int(cell_size), int(num_bins),
-                                                        int(variant), int(bool(bilinear_orientations)), ptr(out), ptr(d_off)))
+        call = _capi.lib().sd_hog_pyramid_float if float_frames else _capi.lib().sd_hog_pyramid_images
+        _check(ctx.h, call(ctx.h, C.byref(ib), h_scales, len(scales), int(cell_size), int(num_bins), int(variant),
+                           int(bool(bilinear_orientations)), ptr(out), ptr(d_off)))
     else:
         _check(ctx.h, _capi.lib().sd_hog_pyramid(ctx.h, C.byref(ib), h_scales, len(scales), int(cell_size), int(num_bins),
                                                  int(variant), ptr(out), ptr(d_off)))
@@ -1625,14 +1640,15 @@ cell (n, 2) int32 (the score position x, y in its level), and above (num_frames,
 
 def vl_hog_detect(frames, scales, filters, cell_size: int, num_bins: int, threshold: float, variant: int = 1, bias=None, pad=(0, 0),
                   overlap: float = 0.5, max_candidates: int = 4096, max_detections: int = 256,
-                  ctx: Optional[Context] = None, multichannel: bool = False, bilinear_orientations: bool = False) -> HogDetections:
+                  ctx: Optional[Context] = None, multichannel: bool = False, bilinear_orientations: bool = False,
+                  float_frames: bool = False) -> HogDetections:
     """A sliding-window detector over image pyramids: vl_hog_pyramid of every frame at every scale, vl_hog_correlate of the
     filter bank on every level (read in place), and one sd_hog_detections call over all score maps: the scores above threshold,
     their boxes in frame pixels, the first max_candidates of each frame by score, and greedy non-maximum suppression at IoU
-    overlap over all filters as one class, up to max_detections per frame.  frames, scales, filters, bias, pad, multichannel
-    and bilinear_orientations as vl_hog_pyramid and vl_hog_correlate take them; filters trained with multichannel or
-    bilinear_orientations are scored with the same.  Returns HogDetections; detect_faces(frames, d.frame, boxes=d.boxes) takes
-    the result as it is."""
+    overlap over all filters as one class, up to max_detections per frame.  frames, scales, filters, bias, pad, multichannel,
+    bilinear_orientations and float_frames as vl_hog_pyramid and vl_hog_correlate take them; filters trained with
+    multichannel, bilinear_orientations or float_frames are scored with the same.  Returns HogDetections;
+    detect_faces(frames, d.frame, boxes=d.boxes) takes the result as it is."""
     ctx = ctx or default_context()
     f = _tensor(filters)
     if f.dim() != 4:
@@ -1640,7 +1656,7 @@ def vl_hog_detect(frames, scales, filters, cell_size: int, num_bins: int, thresh
     q, _, fh, fw = f.shape
     pad_x, pad_y = (int(p) for p in pad)
     feats, levels = vl_hog_pyramid(frames, scales, cell_size, num_bins, variant, ctx=ctx, multichannel=multichannel,
-                                   bilinear_orientations=bilinear_orientations)
+                                   bilinear_orientations=bilinear_orientations, float_frames=float_frames)
     n = len(feats)
     if n == 0:
         return _detections(None, None, None)[0]
@@ -1798,20 +1814,21 @@ array of the negative cache in slot order (frame, level, x, y), and report, one 
 sd_hog_train_report, the solve as an SvmReport, or None when the round's solve was skipped; times_ms, the round's phases in
 milliseconds, and gathered_bytes).  positive_overlap reaches the library as a float: the positives are hog_box_windows(...,
 positive_overlap=float(np.float32(positive_overlap))).  The filter is one for the features it was trained on: one trained with
-multichannel or bilinear_orientations is scored by vl_hog_detect with the same values."""
+multichannel, bilinear_orientations or float_frames is scored by vl_hog_detect with the same values."""
 
 
 def train_hog_filter(frames, box_frame, boxes, scales, filter_size, cell_size: int, num_bins: int, variant: int = 1, pad=(0, 0),
                      lam: float = 0.01, positive_overlap: float = 0.5, negative_overlap: float = 0.3, flip_positives: bool = False,
                      rounds: int = 3, negatives_per_frame: int = 32, mine_overlap: float = 0.5, max_negatives: int = 8192,
                      max_iterations: int = 50, ctx: Optional[Context] = None, multichannel: bool = False,
-                     bilinear_orientations: bool = False) -> HogFilter:
+                     bilinear_orientations: bool = False, float_frames: bool = False) -> HogFilter:
     """Train a HOG filter for vl_hog_detect (sd_hog_train_filter): each box's best window as a positive (hog_box_windows, with
     its mirror if flip_positives), round 0 with the mean positive minus its mean as the filter, then `rounds` rounds of
     hard-negative mining at the margin (threshold -1) and a squared-hinge SVM (learn_squared_hinge) each.  frames,
-    multichannel and bilinear_orientations as vl_hog_pyramid takes them (multichannel: sd_hog_train_filter_images); box_frame
-    (n,) and boxes (n, 4) (x, y, w, h) in the layout of HogDetections.  vl_hog_detect(frames, scales, hf.filter[None], ...,
-    bias=[hf.bias]) with the same multichannel and bilinear_orientations takes the result as it is."""
+    multichannel, bilinear_orientations and float_frames as vl_hog_pyramid takes them (multichannel:
+    sd_hog_train_filter_images, with float_frames sd_hog_train_filter_float); box_frame (n,) and boxes (n, 4) (x, y, w, h) in
+    the layout of HogDetections.  vl_hog_detect(frames, scales, hf.filter[None], ..., bias=[hf.bias]) with the same
+    multichannel, bilinear_orientations and float_frames takes the result as it is."""
     ctx = ctx or default_context()
     dd = _hog_dims(num_bins, variant)
     fw, fh = (int(v) for v in filter_size)
@@ -1819,14 +1836,12 @@ def train_hog_filter(frames, box_frame, boxes, scales, filter_size, cell_size: i
     scales = [float(s) for s in scales]
     if not scales:
         raise ValueError("train_hog_filter needs at least one scale")
-    if bilinear_orientations and not multichannel:
-        raise ValueError("bilinear_orientations needs multichannel=True (grey frames pass as they are)")
 
     def check(w, h):
         for s in scales:
             hog_pyramid_shape(w, h, s, cell_size, num_bins, variant)
 
-    keep, ib, sizes = _hog_images(frames, True, ctx, check) if multichannel else _grey_frames(frames, ctx, check)
+    keep, ib, sizes = _window_frames(frames, ctx, check, multichannel, bilinear_orientations, float_frames)
     if not sizes:
         raise ValueError("train_hog_filter needs at least one frame")
     bf = np.asarray(box_frame, np.int64).reshape(-1)
@@ -1848,7 +1863,8 @@ def train_hog_filter(frames, box_frame, boxes, scales, filter_size, cell_size: i
     rest = (hb, nb, sc, len(scales), int(cell_size), int(num_bins), int(variant), fw, fh, pad_x, pad_y, C.byref(prm), ptr(filt),
             C.byref(bias), reps, negs, C.byref(nn))
     if multichannel:
-        _check(ctx.h, lib.sd_hog_train_filter_images(ctx.h, C.byref(ib), int(bool(bilinear_orientations)), *rest))
+        call = lib.sd_hog_train_filter_float if float_frames else lib.sd_hog_train_filter_images
+        _check(ctx.h, call(ctx.h, C.byref(ib), int(bool(bilinear_orientations)), *rest))
     else:
         _check(ctx.h, lib.sd_hog_train_filter(ctx.h, C.byref(ib), *rest))
     S = len(scales)
@@ -1875,8 +1891,8 @@ class HogPartModel:
     filters scored at twice the root's resolution, anchors (Q, P, 2) int (ax, ay) in part-level cells relative to twice the root
     window's top-left cell, deformation (Q, P, 4) (w0, w1, w2, w3): a displacement (dx, dy) costs w0 dx^2 + w1 dx + w2 dy^2 + w3 dy,
     pad = (pad_x, pad_y) of the root correlate, part_pad of the part correlate, and max_displacement R bounding |dx| and |dy|,
-    or None for the exact, unbounded transform of DPM (which needs w0 > 0 and w2 > 0).  The filters are ones for the features they were trained on: a model of colour HOG (vl_hog_pyramid's multichannel and
-    bilinear_orientations) is scored by vl_hog_part_detect with the same values."""
+    or None for the exact, unbounded transform of DPM (which needs w0 > 0 and w2 > 0).  The filters are ones for the features they were trained on: a model of colour HOG (vl_hog_pyramid's multichannel,
+    bilinear_orientations and float_frames) is scored by vl_hog_part_detect with the same values."""
 
     def __init__(self, root, bias, parts, anchors, deformation, pad=(0, 0), part_pad=(0, 0), max_displacement: Optional[int] = 4):
         self.root = _tensor(root).to(torch.float32).contiguous()
@@ -2026,14 +2042,14 @@ score positions ((-1, -1) for none) and part_scores (n, P) float32, each part's 
 def vl_hog_part_detect(frames, scales, model: HogPartModel, cell_size: int, num_bins: int, threshold: float, variant: int = 1,
                        overlap: float = 0.5, max_candidates: int = 4096, max_detections: int = 256,
                        ctx: Optional[Context] = None, multichannel: bool = False,
-                       bilinear_orientations: bool = False) -> HogPartDetections:
+                       bilinear_orientations: bool = False, float_frames: bool = False) -> HogPartDetections:
     """A star-model detector over image pyramids: one vl_hog_pyramid over the root scales and their doubles (a scale present in
     both is computed once; root scales must be <= 2), vl_hog_correlate of the root filters (bias included) on the root levels and
     of all Q * P part filters on the part levels, each read in place; vl_hog_distance_transform of the part maps; the star
     model's scores (vl_hog_part_scores); sd_hog_detections over them with the root's filter size and pad, all components as one
     class; and the part placements of every detection (sd_hog_part_placements, or with the model's max_displacement None, the
     exact transform's placement maps read at the anchors by sd_hog_part_placements_mapped).  One host read-back at the end.  frames,
-    multichannel and bilinear_orientations as vl_hog_pyramid takes them.  Returns HogPartDetections; detect_faces(frames,
+    multichannel, bilinear_orientations and float_frames as vl_hog_pyramid takes them.  Returns HogPartDetections; detect_faces(frames,
     d.frame, boxes=d.boxes) takes the result as it is."""
     ctx = ctx or default_context()
     dev = f"cuda:{ctx.device}"
@@ -2047,7 +2063,7 @@ def vl_hog_part_detect(frames, scales, model: HogPartModel, cell_size: int, num_
     every = list(dict.fromkeys(scales + [2 * s for s in scales]))
     ri, pi = [every.index(s) for s in scales], [every.index(2 * s) for s in scales]
     feats, levels = vl_hog_pyramid(frames, every, cell_size, num_bins, variant, ctx=ctx, multichannel=multichannel,
-                                   bilinear_orientations=bilinear_orientations)
+                                   bilinear_orientations=bilinear_orientations, float_frames=float_frames)
     n = len(feats)
     if n == 0:
         return _part_detections(_detections(None, None, None), np.zeros((0, 1, p, len(HogPartPlacementC._fields_)), np.int32))

@@ -259,13 +259,21 @@ struct HogResizeTap {
 __device__ __forceinline__ int clip_index(int x, int a, int b) { return x >= a ? (x < b ? x : b - 1) : a; }
 __device__ __forceinline__ short sat_short(int v) { return (short)(v > 32767 ? 32767 : (v < -32768 ? -32768 : v)); }
 
-__device__ __forceinline__ HogResizeTap hog_resize_tap(int t, int dst, int src)
+// The source coordinate of output coordinate t, split into s = floor(f) (returned) and the fraction *f, both rules' first step
+__device__ __forceinline__ int hog_resize_coord(int t, int dst, int src, float* frac)
 {
     const double inv_scale = __ddiv_rn((double)dst, (double)src);
     const double scale = __ddiv_rn(1.0, inv_scale);
-    float f = (float)__dadd_rn(__dmul_rn((double)t + 0.5, scale), -0.5);
+    const float f = (float)__dadd_rn(__dmul_rn((double)t + 0.5, scale), -0.5);
     const int s = (int)floorf(f);
-    f = __fsub_rn(f, (float)s);
+    *frac = __fsub_rn(f, (float)s);
+    return s;
+}
+
+__device__ __forceinline__ HogResizeTap hog_resize_tap(int t, int dst, int src)
+{
+    float f;
+    const int s = hog_resize_coord(t, dst, src, &f);
     int sx = s;
     float fx = f;
     if (sx < 0) { fx = 0.f; sx = 0; }
@@ -288,6 +296,40 @@ __device__ __forceinline__ HogResizeTap hog_resize_tap(int t, int dst, int src)
 __device__ __forceinline__ int hog_resize_out(int yb, int t0, int t1)
 {
     return (((((int)(short)yb) * (t0 >> 4)) >> 16) + (((yb >> 16) * (t1 >> 4)) >> 16) + 2) >> 2;
+}
+
+// ---- cv::resize INTER_LINEAR of float pixels, the float pyramid's levels (sd_hog_pyramid_float): the coordinate of
+//      hog_resize_coord; column taps sx (clamped as above, its fraction then 0) and xw = the fraction's float bits; row taps y0,
+//      y1 as above and yw = the unclamped fraction's float bits.  Every product and sum rounded on its own (no FMA). -----------
+__device__ __forceinline__ HogResizeTap hog_resize_tap_f32(int t, int dst, int src)
+{
+    float f;
+    const int s = hog_resize_coord(t, dst, src, &f);
+    int sx = s;
+    float fx = f;
+    if (sx < 0) { fx = 0.f; sx = 0; }
+    if (sx >= src - 1) { fx = 0.f; sx = src - 1; }
+    HogResizeTap r;
+    r.sx = sx;
+    r.xw = __float_as_int(fx);
+    r.y0 = clip_index(s, 0, src);
+    r.y1 = clip_index(s + 1, 0, src);
+    r.yw = __float_as_int(f);
+    return r;
+}
+
+// One source row's value at column taps (sx, fx): S[sx] (1 - fx) + S[sx + 1] fx, or S[sx] (1 - fx) alone at the last column.
+// A tap of weight 0 is still read and multiplied, so inf * 0 gives NaN as in cv::resize.
+__device__ __forceinline__ float hog_resize_row_f32(const float* row, long long ps, int sx, float fx, int last)
+{
+    const float a = __fmul_rn(__ldg(row + sx * ps), __fsub_rn(1.f, fx));
+    return sx == last ? a : __fadd_rn(a, __fmul_rn(__ldg(row + (sx + 1) * ps), fx));
+}
+
+// The vertical step: t0 (1 - fy) + t1 fy
+__device__ __forceinline__ float hog_resize_out_f32(float fy, float t0, float t1)
+{
+    return __fadd_rn(__fmul_rn(t0, __fsub_rn(1.f, fy)), __fmul_rn(t1, fy));
 }
 
 // ---- TMA staging: one thread copies the box at (x, y, z) of a 3-D tensor map (`bytes` bytes; x a multiple of 16, bytes

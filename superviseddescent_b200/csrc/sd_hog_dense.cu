@@ -668,9 +668,10 @@ __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_kernel(cons
     }
 }
 
-// ---- the pyramid of 8-bit frames with C channels (sd_hog_pyramid_images): each channel resized on its own by the rule above,
-//      every level written interleaved ((H, W, C), rows at a pitch of C * w rounded up to 16 bytes) into scratch, then all of
-//      them through hog_images_kernel as one batch of sd_hog_image descriptors
+// ---- the pyramid of 8-bit or float frames with C channels (sd_hog_pyramid_images, sd_hog_pyramid_float): each channel
+//      resized on its own by the rule of its type (hog_resize_tap, hog_resize_tap_f32), every level written interleaved ((H, W,
+//      C) elements of the frames' type, rows at a pitch of C * w elements rounded up to 16 bytes) into scratch, then all of them
+//      through hog_images_kernel as one batch of sd_hog_image descriptors
 struct PyrImageLevel {
     long long src;               // element offset of the frame's pixel (0, 0, 0) from the batch's data
     long long rs, ps, chs;       // the frame's row, pixel and channel strides in elements
@@ -682,7 +683,7 @@ struct PyrImageLevel {
 };
 
 struct ResizeImagesArgs {
-    const uint8_t* images;
+    const void* images;
     uint8_t* scratch;
     const PyrImageLevel* levels;
     int count, channels;
@@ -691,9 +692,11 @@ struct ResizeImagesArgs {
 };
 
 // One CTA per kResizeW x kResizeH pixel tile of one level, as hog_pyramid_resize_kernel: the taps of its columns and rows once,
-// then every channel of every pixel with the channel fastest, so that a warp writes consecutive bytes of the level.
+// then every channel of every pixel with the channel fastest, so that a warp writes consecutive elements of the level.
+template <class T>
 __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kernel(const __grid_constant__ ResizeImagesArgs a)
 {
+    constexpr bool f32 = std::is_same<T, float>::value;
     __shared__ int s_sx[kResizeW], s_xw[kResizeW], s_y0[kResizeH], s_y1[kResizeH], s_yw[kResizeH];
     const int b = blockIdx.x, tid = threadIdx.x, C = a.channels;
     const int lo = sd_find_last_le(0, a.count - 1, b, [&](int i) { return a.levels[i].tile0; });
@@ -701,20 +704,20 @@ __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kern
     const int t = b - L.tile0, ty = t / L.tiles_x;
     const int x0 = (t - ty * L.tiles_x) * kResizeW, y0 = ty * kResizeH;
     if (t == 0 && tid == 0) a.level_offset[lo] = a.out_offset[L.slot];
-    const uint8_t* __restrict__ src = a.images + L.src;
+    const T* __restrict__ src = static_cast<const T*>(a.images) + L.src;
     uint8_t* __restrict__ dst = a.scratch + L.dst;
     const bool copy = L.w == L.W && L.h == L.H;
     if (!copy) {
         if (tid < kResizeW) {
             if (x0 + tid < L.w) {
-                const HogResizeTap r = hog_resize_tap(x0 + tid, L.w, L.W);
+                const HogResizeTap r = f32 ? hog_resize_tap_f32(x0 + tid, L.w, L.W) : hog_resize_tap(x0 + tid, L.w, L.W);
                 s_sx[tid] = r.sx;
                 s_xw[tid] = r.xw;
             }
         } else if (tid < kResizeW + kResizeH) {
             const int i = tid - kResizeW;
             if (y0 + i < L.h) {
-                const HogResizeTap r = hog_resize_tap(y0 + i, L.h, L.H);
+                const HogResizeTap r = f32 ? hog_resize_tap_f32(y0 + i, L.h, L.H) : hog_resize_tap(y0 + i, L.h, L.H);
                 s_y0[i] = r.y0;
                 s_y1[i] = r.y1;
                 s_yw[i] = r.yw;
@@ -728,19 +731,32 @@ __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kern
         const int c = j / C, ch = j - c * C;
         const int x = x0 + c, y = y0 + r;
         if (x >= L.w || y >= L.h) continue;
-        const uint8_t* s = src + ch * L.chs;
-        int v;
-        if (copy) {
-            v = __ldg(s + y * L.rs + x * L.ps);
+        const T* s = src + ch * L.chs;
+        if constexpr (f32) {
+            float v;
+            if (copy) {
+                v = __ldg(s + y * L.rs + x * L.ps);   // a bit copy: no arithmetic touches the value
+            } else {
+                const int sx = s_sx[c];
+                const float fx = __int_as_float(s_xw[c]);
+                v = hog_resize_out_f32(__int_as_float(s_yw[r]), hog_resize_row_f32(s + s_y0[r] * L.rs, L.ps, sx, fx, L.W - 1),
+                                       hog_resize_row_f32(s + s_y1[r] * L.rs, L.ps, sx, fx, L.W - 1));
+            }
+            reinterpret_cast<float*>(dst + (long long)y * L.pitch)[x * C + ch] = v;
         } else {
-            const int sx = s_sx[c], sx1 = min(sx + 1, L.W - 1);   // a clamped tap has zero weight
-            const int ax = (short)s_xw[c], bx = s_xw[c] >> 16;
-            const uint8_t* r0 = s + s_y0[r] * L.rs;
-            const uint8_t* r1 = s + s_y1[r] * L.rs;
-            v = hog_resize_out(s_yw[r], (int)__ldg(r0 + sx * L.ps) * ax + (int)__ldg(r0 + sx1 * L.ps) * bx,
-                               (int)__ldg(r1 + sx * L.ps) * ax + (int)__ldg(r1 + sx1 * L.ps) * bx);
+            int v;
+            if (copy) {
+                v = __ldg(s + y * L.rs + x * L.ps);
+            } else {
+                const int sx = s_sx[c], sx1 = min(sx + 1, L.W - 1);   // a clamped tap has zero weight
+                const int ax = (short)s_xw[c], bx = s_xw[c] >> 16;
+                const uint8_t* r0 = s + s_y0[r] * L.rs;
+                const uint8_t* r1 = s + s_y1[r] * L.rs;
+                v = hog_resize_out(s_yw[r], (int)__ldg(r0 + sx * L.ps) * ax + (int)__ldg(r0 + sx1 * L.ps) * bx,
+                                   (int)__ldg(r1 + sx * L.ps) * ax + (int)__ldg(r1 + sx1 * L.ps) * bx);
+            }
+            dst[(long long)y * L.pitch + x * C + ch] = (uint8_t)v;
         }
-        dst[(long long)y * L.pitch + x * C + ch] = (uint8_t)v;
     }
 }
 
@@ -799,6 +815,124 @@ uint8_t* pyramid_scratch(sd_ctx* ctx, long long bytes, const Level* levels, cons
         return nullptr;
     return ws;
 }
+
+// sd_hog_pyramid_images (T = uint8_t) and sd_hog_pyramid_float (T = float) past their null and dtype checks: the arguments'
+// other checks, the frame table, every non-empty level and the slices, with levels of T at a pitch of C * w * sizeof(T) bytes
+// rounded up to 16.  fn names the entry point in errors.
+#define PYR_REQUIRE(cond, msg)                                                         \
+    do {                                                                               \
+        if (!(cond)) return sd_fail(ctx, SD_ERR_INVALID, "%s: %s", fn, msg);           \
+    } while (0)
+template <class T>
+int pyramid_images(sd_ctx* ctx, const char* fn, const sd_hog_images* images, const double* h_scales, int num_scales, int cell_size,
+                   int num_bins, int variant, int bilinear_orientations, float* d_out, const int64_t* d_out_offset)
+{
+    constexpr int es = (int)sizeof(T);
+    PYR_REQUIRE(images->channels >= 1 && images->channels <= kDenseMaxChannels, "channels must be in [1,16]");
+    PYR_REQUIRE(bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
+    if (const int rc = sd_hog_check_config(ctx, fn, variant, num_bins, cell_size)) return rc;
+    PYR_REQUIRE(num_scales >= 1, "num_scales must be at least 1");
+    for (int s = 0; s < num_scales; ++s)
+        PYR_REQUIRE(h_scales[s] > 0.0 && h_scales[s] <= 4.0, "every scale must be finite and in (0, 4]");
+    PYR_REQUIRE(images->count >= 0, "negative frame count");
+    const int count = images->count, C = images->channels;
+    if (count == 0) return SD_OK;
+    PYR_REQUIRE(images->d_data, "null argument");
+    PYR_REQUIRE(es == 1 || (reinterpret_cast<uintptr_t>(images->d_data) & 3) == 0, "float frames must be 4-byte aligned");
+    PYR_REQUIRE((long long)count * num_scales <= INT_MAX, "too many levels");
+
+    // the frames: the batch's, or the descriptor table read back once
+    std::vector<sd_hog_image> fr;
+    if (images->d_frames) {
+        if (const int rc = sd_fetch_table(ctx, images->d_frames, count, fr)) return rc;
+    } else {
+        PYR_REQUIRE(images->image_stride >= 0, "negative image stride");
+        fr.assign(count, images->frame);
+        for (int i = 0; i < count; ++i) fr[i].offset += (int64_t)i * images->image_stride;
+    }
+    // every non-empty level of every frame, in the order of the caller's slots
+    std::vector<PyrImageLevel> lv;
+    std::vector<int> first(count + 1, 0);
+    for (int f = 0; f < count; ++f) {
+        const sd_hog_image& d = fr[f];
+        if (d.width < 1 || d.height < 1 || d.offset < 0 || d.row_stride < 0 || d.pixel_stride < 0 || d.channel_stride < 0)
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d (%d x %d) is smaller than 1 x 1 or has a negative offset or stride",
+                           fn, f, d.width, d.height);
+        first[f] = (int)lv.size();
+        for (int s = 0; s < num_scales; ++s) {
+            PyrImageLevel L{};
+            int hw, hh, dd;
+            if (!pyramid_level(d.width, d.height, h_scales[s], &L.w, &L.h))
+                return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d at scale %g is larger than 2^28 px per side", fn, f, h_scales[s]);
+            if (!dense_shape(L.w, L.h, cell_size, num_bins, variant, &hw, &hh, &dd)) continue;
+            if ((long long)L.w * C * es > INT_MAX - 15) return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d: level too large", fn, f);
+            L.src = d.offset;
+            L.rs = d.row_stride; L.ps = d.pixel_stride; L.chs = d.channel_stride;
+            L.W = d.width; L.H = d.height;
+            L.pitch = dense_align(L.w * C * es, 16);
+            L.tiles_x = sd_div_up(L.w, kResizeW);
+            L.slot = f * num_scales + s;
+            lv.push_back(L);
+        }
+    }
+    first[count] = (int)lv.size();
+    if (lv.empty()) return SD_OK;
+
+    // one 8-bit channel, nearest bins, contiguous rows: sd_hog_pyramid computes the same levels (as sd_hog_dense_images routes
+    // to sd_hog_dense)
+    const sd_hog_image& f0 = images->frame;
+    if (es == 1 && C == 1 && !bilinear_orientations && !images->d_frames && f0.pixel_stride == 1 && f0.row_stride >= f0.width &&
+        f0.row_stride <= INT_MAX && (count == 1 || images->image_stride > 0)) {
+        sd_image_batch ib{};
+        ib.d_data = static_cast<const uint8_t*>(images->d_data) + f0.offset;
+        ib.width = f0.width; ib.height = f0.height; ib.row_stride = (int32_t)f0.row_stride;
+        ib.image_stride = images->image_stride;
+        ib.count = count;
+        return sd_hog_pyramid(ctx, &ib, h_scales, num_scales, cell_size, num_bins, variant, d_out, d_out_offset);
+    }
+
+    const bool bil = bilinear_orientations != 0;
+    const ImagesKernel kern = bil ? images_kernel<T, true>(num_bins) : images_kernel<T, false>(num_bins);
+    ImageArgs a;
+    memset(&a, 0, sizeof(a));
+    a.channels = C;
+    a.out = d_out;
+    a.variant = variant; a.cs = cell_size; a.K = num_bins; a.dd = sd_hog_dd(num_bins, variant);
+    a.tile = images_tile(kern, cell_size, num_bins, bil);
+    a.span = cell_size * (a.tile + 3) + 4;
+    a.pi_k = 3.141592653589793 / (double)num_bins;    // VL_PI / numOrientations (hog.c:677)
+    hog_orientations(num_bins, a.orient);
+    const DenseSmem lay = dense_smem_layout(a.span, 0, num_bins, dense_cells(a.tile), bil);
+    return pyramid_slices(ctx, fn, lv, first, count, cell_size, [&](int l0, int n, long long bytes, int tiles, int max_w, int max_h) -> int {
+        std::vector<sd_hog_image> desc(n);
+        for (int i = 0; i < n; ++i) {
+            const PyrImageLevel& L = lv[l0 + i];
+            desc[i] = sd_hog_image{L.w, L.h, L.dst / es, L.pitch / es, C, 1};   // elements of T
+        }
+        PyrImageLevel* d_lv;
+        sd_hog_image* d_desc;
+        int64_t* d_off;
+        uint8_t* ws = pyramid_scratch(ctx, bytes, lv.data() + l0, desc, &d_lv, &d_desc, &d_off);
+        if (!ws) return SD_ERR_CUDA;
+
+        ResizeImagesArgs r;
+        r.images = images->d_data;
+        r.scratch = ws;
+        r.levels = d_lv;
+        r.count = n;
+        r.channels = C;
+        r.out_offset = d_out_offset;
+        r.level_offset = d_off;
+        hog_pyramid_resize_images_kernel<T><<<(unsigned)tiles, kResizeThreads, 0, ctx->stream>>>(r);
+        SD_LAUNCH_CHECK(ctx, "hog_pyramid_resize_images_kernel");
+
+        a.data = ws;
+        a.frames = d_desc;
+        a.out_offset = d_off;
+        return launch_dense(ctx, fn, "hog_images_kernel", kern, a, n, max_w, max_h, lay.total);
+    });
+}
+#undef PYR_REQUIRE
 
 }  // namespace
 
@@ -962,108 +1096,18 @@ int sd_hog_pyramid_images(sd_ctx* ctx, const sd_hog_images* images, const double
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, images && h_scales && d_out && d_out_offset, "null argument");
     SD_REQUIRE(ctx, images->dtype == SD_HOG_U8, "dtype must be SD_HOG_U8: the levels are resized by the 8-bit rule");
-    SD_REQUIRE(ctx, images->channels >= 1 && images->channels <= kDenseMaxChannels, "channels must be in [1,16]");
-    SD_REQUIRE(ctx, bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
-    if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins, cell_size)) return rc;
-    SD_REQUIRE(ctx, num_scales >= 1, "num_scales must be at least 1");
-    for (int s = 0; s < num_scales; ++s)
-        SD_REQUIRE(ctx, h_scales[s] > 0.0 && h_scales[s] <= 4.0, "every scale must be finite and in (0, 4]");
-    SD_REQUIRE(ctx, images->count >= 0, "negative frame count");
-    const int count = images->count, C = images->channels;
-    if (count == 0) return SD_OK;
-    SD_REQUIRE(ctx, images->d_data, "null argument");
-    SD_REQUIRE(ctx, (long long)count * num_scales <= INT_MAX, "too many levels");
+    return pyramid_images<uint8_t>(ctx, __func__, images, h_scales, num_scales, cell_size, num_bins, variant, bilinear_orientations,
+                                   d_out, d_out_offset);
+}
 
-    // the frames: the batch's, or the descriptor table read back once
-    std::vector<sd_hog_image> fr;
-    if (images->d_frames) {
-        if (const int rc = sd_fetch_table(ctx, images->d_frames, count, fr)) return rc;
-    } else {
-        SD_REQUIRE(ctx, images->image_stride >= 0, "negative image stride");
-        fr.assign(count, images->frame);
-        for (int i = 0; i < count; ++i) fr[i].offset += (int64_t)i * images->image_stride;
-    }
-    // every non-empty level of every frame, in the order of the caller's slots
-    std::vector<PyrImageLevel> lv;
-    std::vector<int> first(count + 1, 0);
-    for (int f = 0; f < count; ++f) {
-        const sd_hog_image& d = fr[f];
-        if (d.width < 1 || d.height < 1 || d.offset < 0 || d.row_stride < 0 || d.pixel_stride < 0 || d.channel_stride < 0)
-            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d (%d x %d) is smaller than 1 x 1 or has a negative offset or stride",
-                           __func__, f, d.width, d.height);
-        first[f] = (int)lv.size();
-        for (int s = 0; s < num_scales; ++s) {
-            PyrImageLevel L{};
-            int hw, hh, dd;
-            if (!pyramid_level(d.width, d.height, h_scales[s], &L.w, &L.h))
-                return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d at scale %g is larger than 2^28 px per side", __func__, f, h_scales[s]);
-            if (!dense_shape(L.w, L.h, cell_size, num_bins, variant, &hw, &hh, &dd)) continue;
-            if ((long long)L.w * C > INT_MAX - 15) return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d: level too large", __func__, f);
-            L.src = d.offset;
-            L.rs = d.row_stride; L.ps = d.pixel_stride; L.chs = d.channel_stride;
-            L.W = d.width; L.H = d.height;
-            L.pitch = dense_align(L.w * C, 16);
-            L.tiles_x = sd_div_up(L.w, kResizeW);
-            L.slot = f * num_scales + s;
-            lv.push_back(L);
-        }
-    }
-    first[count] = (int)lv.size();
-    if (lv.empty()) return SD_OK;
-
-    // one channel, nearest bins, contiguous rows: sd_hog_pyramid computes the same levels (as sd_hog_dense_images routes to
-    // sd_hog_dense)
-    const sd_hog_image& f0 = images->frame;
-    if (C == 1 && !bilinear_orientations && !images->d_frames && f0.pixel_stride == 1 && f0.row_stride >= f0.width &&
-        f0.row_stride <= INT_MAX && (count == 1 || images->image_stride > 0)) {
-        sd_image_batch ib{};
-        ib.d_data = static_cast<const uint8_t*>(images->d_data) + f0.offset;
-        ib.width = f0.width; ib.height = f0.height; ib.row_stride = (int32_t)f0.row_stride;
-        ib.image_stride = images->image_stride;
-        ib.count = count;
-        return sd_hog_pyramid(ctx, &ib, h_scales, num_scales, cell_size, num_bins, variant, d_out, d_out_offset);
-    }
-
-    const bool bil = bilinear_orientations != 0;
-    const ImagesKernel kern = bil ? images_kernel<uint8_t, true>(num_bins) : images_kernel<uint8_t, false>(num_bins);
-    ImageArgs a;
-    memset(&a, 0, sizeof(a));
-    a.channels = C;
-    a.out = d_out;
-    a.variant = variant; a.cs = cell_size; a.K = num_bins; a.dd = sd_hog_dd(num_bins, variant);
-    a.tile = images_tile(kern, cell_size, num_bins, bil);
-    a.span = cell_size * (a.tile + 3) + 4;
-    a.pi_k = 3.141592653589793 / (double)num_bins;    // VL_PI / numOrientations (hog.c:677)
-    hog_orientations(num_bins, a.orient);
-    const DenseSmem lay = dense_smem_layout(a.span, 0, num_bins, dense_cells(a.tile), bil);
-    return pyramid_slices(ctx, __func__, lv, first, count, cell_size, [&](int l0, int n, long long bytes, int tiles, int max_w, int max_h) -> int {
-        std::vector<sd_hog_image> desc(n);
-        for (int i = 0; i < n; ++i) {
-            const PyrImageLevel& L = lv[l0 + i];
-            desc[i] = sd_hog_image{L.w, L.h, L.dst, L.pitch, C, 1};
-        }
-        PyrImageLevel* d_lv;
-        sd_hog_image* d_desc;
-        int64_t* d_off;
-        uint8_t* ws = pyramid_scratch(ctx, bytes, lv.data() + l0, desc, &d_lv, &d_desc, &d_off);
-        if (!ws) return SD_ERR_CUDA;
-
-        ResizeImagesArgs r;
-        r.images = static_cast<const uint8_t*>(images->d_data);
-        r.scratch = ws;
-        r.levels = d_lv;
-        r.count = n;
-        r.channels = C;
-        r.out_offset = d_out_offset;
-        r.level_offset = d_off;
-        hog_pyramid_resize_images_kernel<<<(unsigned)tiles, kResizeThreads, 0, ctx->stream>>>(r);
-        SD_LAUNCH_CHECK(ctx, "hog_pyramid_resize_images_kernel");
-
-        a.data = ws;
-        a.frames = d_desc;
-        a.out_offset = d_off;
-        return launch_dense(ctx, "sd_hog_pyramid_images", "hog_images_kernel", kern, a, n, max_w, max_h, lay.total);
-    });
+int sd_hog_pyramid_float(sd_ctx* ctx, const sd_hog_images* images, const double* h_scales, int num_scales, int cell_size,
+                         int num_bins, int variant, int bilinear_orientations, float* d_out, const int64_t* d_out_offset)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, images && h_scales && d_out && d_out_offset, "null argument");
+    SD_REQUIRE(ctx, images->dtype == SD_HOG_F32, "dtype must be SD_HOG_F32: the levels are resized by the float rule");
+    return pyramid_images<float>(ctx, __func__, images, h_scales, num_scales, cell_size, num_bins, variant, bilinear_orientations,
+                                 d_out, d_out_offset);
 }
 
 int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size, int num_bins, int variant,

@@ -791,6 +791,46 @@ int train_filter(sd_ctx* ctx, const char* fn, const TrainFrames& src, const sd_h
     return SD_OK;
 }
 
+// sd_hog_train_filter_images and sd_hog_train_filter_float past their null and dtype checks: a frame source over an
+// sd_hog_images whose slices' pyramids are pyramid's (sd_hog_pyramid_images or sd_hog_pyramid_float).  fn names the entry point.
+using ImagesPyramid = int (*)(sd_ctx*, const sd_hog_images*, const double*, int, int, int, int, int, float*, const int64_t*);
+int train_filter_images(sd_ctx* ctx, const char* fn, ImagesPyramid pyramid, const sd_hog_images* images, int bilinear_orientations,
+                        const sd_hog_box* h_boxes, int num_boxes, const double* h_scales, int num_scales, int cell_size, int num_bins,
+                        int variant, int filter_w, int filter_h, int pad_x, int pad_y, const sd_hog_train_param* p, float* d_filter,
+                        float* h_bias, sd_hog_train_report* h_rounds, sd_hog_window* h_negatives, int* h_num_negatives)
+{
+    TRAIN_REQUIRE(images->channels >= 1 && images->channels <= 16, "channels must be in [1,16]");
+    TRAIN_REQUIRE(bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
+    TRAIN_REQUIRE(images->count < 1 || images->d_data, "null argument");
+    TrainFrames src;
+    src.count = images->count;
+    src.sizes = [&](std::vector<FrameSize>& sizes) -> int {
+        std::vector<sd_hog_image> fr;
+        if (images->d_frames) {
+            if (const int rc = sd_fetch_table(ctx, images->d_frames, images->count, fr)) return rc;
+        } else {
+            TRAIN_REQUIRE(images->image_stride >= 0, "negative image stride");
+            fr.assign(images->count, images->frame);
+        }
+        for (int f = 0; f < images->count; ++f) {
+            const sd_hog_image& d = fr[f];
+            if (d.offset < 0 || d.row_stride < 0 || d.pixel_stride < 0 || d.channel_stride < 0)
+                return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d has a negative offset or stride", fn, f);
+            sizes.push_back({d.width, d.height});
+        }
+        return SD_OK;
+    };
+    src.pyramid = [&](int f0, int f1, float* d_out, const int64_t* d_off) {
+        sd_hog_images sub = *images;
+        sub.count = f1 - f0;
+        if (images->d_frames) sub.d_frames = images->d_frames + f0;
+        else sub.frame.offset += (int64_t)f0 * images->image_stride;
+        return pyramid(ctx, &sub, h_scales, num_scales, cell_size, num_bins, variant, bilinear_orientations, d_out, d_off);
+    };
+    return train_filter(ctx, fn, src, h_boxes, num_boxes, h_scales, num_scales, cell_size, num_bins, variant, filter_w, filter_h,
+                        pad_x, pad_y, p, d_filter, h_bias, h_rounds, h_negatives, h_num_negatives);
+}
+
 #undef TRAIN_REQUIRE
 
 }  // namespace
@@ -838,36 +878,24 @@ int sd_hog_train_filter_images(sd_ctx* ctx, const sd_hog_images* images, int bil
     SD_REQUIRE(ctx, images && h_scales && p && d_filter && h_bias && h_rounds && h_num_negatives && (num_boxes == 0 || h_boxes),
                "null argument");
     SD_REQUIRE(ctx, images->dtype == SD_HOG_U8, "dtype must be SD_HOG_U8: the levels are resized by the 8-bit rule");
-    SD_REQUIRE(ctx, images->channels >= 1 && images->channels <= 16, "channels must be in [1,16]");
-    SD_REQUIRE(ctx, bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
-    SD_REQUIRE(ctx, images->count < 1 || images->d_data, "null argument");
-    TrainFrames src;
-    src.count = images->count;
-    src.sizes = [&](std::vector<FrameSize>& sizes) -> int {
-        std::vector<sd_hog_image> fr;
-        if (images->d_frames) {
-            if (const int rc = sd_fetch_table(ctx, images->d_frames, images->count, fr)) return rc;
-        } else {
-            if (images->image_stride < 0) return sd_fail(ctx, SD_ERR_INVALID, "sd_hog_train_filter_images: negative image stride");
-            fr.assign(images->count, images->frame);
-        }
-        for (int f = 0; f < images->count; ++f) {
-            const sd_hog_image& d = fr[f];
-            if (d.offset < 0 || d.row_stride < 0 || d.pixel_stride < 0 || d.channel_stride < 0)
-                return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d has a negative offset or stride", "sd_hog_train_filter_images", f);
-            sizes.push_back({d.width, d.height});
-        }
-        return SD_OK;
-    };
-    src.pyramid = [&](int f0, int f1, float* d_out, const int64_t* d_off) {
-        sd_hog_images sub = *images;
-        sub.count = f1 - f0;
-        if (images->d_frames) sub.d_frames = images->d_frames + f0;
-        else sub.frame.offset += (int64_t)f0 * images->image_stride;
-        return sd_hog_pyramid_images(ctx, &sub, h_scales, num_scales, cell_size, num_bins, variant, bilinear_orientations, d_out, d_off);
-    };
-    return train_filter(ctx, __func__, src, h_boxes, num_boxes, h_scales, num_scales, cell_size, num_bins, variant, filter_w, filter_h,
-                        pad_x, pad_y, p, d_filter, h_bias, h_rounds, h_negatives, h_num_negatives);
+    return train_filter_images(ctx, __func__, sd_hog_pyramid_images, images, bilinear_orientations, h_boxes, num_boxes, h_scales,
+                               num_scales, cell_size, num_bins, variant, filter_w, filter_h, pad_x, pad_y, p, d_filter, h_bias,
+                               h_rounds, h_negatives, h_num_negatives);
+}
+
+int sd_hog_train_filter_float(sd_ctx* ctx, const sd_hog_images* images, int bilinear_orientations, const sd_hog_box* h_boxes,
+                              int num_boxes, const double* h_scales, int num_scales, int cell_size, int num_bins, int variant,
+                              int filter_w, int filter_h, int pad_x, int pad_y, const sd_hog_train_param* p, float* d_filter,
+                              float* h_bias, sd_hog_train_report* h_rounds, sd_hog_window* h_negatives, int* h_num_negatives)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, images && h_scales && p && d_filter && h_bias && h_rounds && h_num_negatives && (num_boxes == 0 || h_boxes),
+               "null argument");
+    SD_REQUIRE(ctx, images->dtype == SD_HOG_F32, "dtype must be SD_HOG_F32: the levels are resized by the float rule");
+    SD_REQUIRE(ctx, (reinterpret_cast<uintptr_t>(images->d_data) & 3) == 0, "float frames must be 4-byte aligned");
+    return train_filter_images(ctx, __func__, sd_hog_pyramid_float, images, bilinear_orientations, h_boxes, num_boxes, h_scales,
+                               num_scales, cell_size, num_bins, variant, filter_w, filter_h, pad_x, pad_y, p, d_filter, h_bias,
+                               h_rounds, h_negatives, h_num_negatives);
 }
 
 }  // extern "C"

@@ -117,16 +117,13 @@ inline std::vector<int64_t> pack_planes(sd_ctx* ctx, const std::vector<cv::Mat>&
     return start;
 }
 
-// 8UC1 or 8UC3 (B,G,R) frames, all of one type, on the device with their channels kept, interleaved as OpenCV holds them:
-// packed end to end into buf (row steps dropped), one descriptor per frame in table
-inline sd_hog_images upload_channels(sd_ctx* ctx, const std::vector<cv::Mat>& images, sd_b200::DeviceBuffer& buf,
-                                     sd_b200::DeviceBuffer& table, const char* what)
+// Frames of one type with C channels of elem bytes each (checked by the caller) on the device, interleaved as OpenCV holds
+// them: packed end to end into buf (row steps dropped), one descriptor per frame in table
+inline sd_hog_images upload_interleaved(sd_ctx* ctx, const std::vector<cv::Mat>& images, size_t elem, int dtype,
+                                        sd_b200::DeviceBuffer& buf, sd_b200::DeviceBuffer& table, const char* what)
 {
     const int n = static_cast<int>(images.size()), C = images[0].channels();
-    for (const cv::Mat& m : images)
-        if (m.type() != images[0].type() || (m.type() != CV_8UC1 && m.type() != CV_8UC3))
-            throw std::runtime_error(std::string(what) + ": frames must be all CV_8UC1 or all CV_8UC3");
-    const std::vector<int64_t> start = pack_planes(ctx, images, static_cast<size_t>(C), buf, what);
+    const std::vector<int64_t> start = pack_planes(ctx, images, elem * static_cast<size_t>(C), buf, what);
     std::vector<sd_hog_image> desc;
     for (int i = 0; i < n; ++i)
         desc.push_back(sd_hog_image{images[i].cols, images[i].rows, start[i] * C, static_cast<int64_t>(images[i].cols) * C, C, 1});
@@ -134,11 +131,31 @@ inline sd_hog_images upload_channels(sd_ctx* ctx, const std::vector<cv::Mat>& im
     sd_b200::check(ctx, sd_memcpy_h2d(ctx, table.as<sd_hog_image>(), desc.data(), desc.size() * sizeof(sd_hog_image)), what);
     sd_hog_images batch{};
     batch.d_data = buf.as<void>();
-    batch.dtype = SD_HOG_U8;
+    batch.dtype = dtype;
     batch.channels = C;
     batch.count = n;
     batch.d_frames = table.as<sd_hog_image>();
     return batch;
+}
+
+// 8UC1 or 8UC3 (B,G,R) frames, all of one type, on the device with their channels kept (upload_interleaved)
+inline sd_hog_images upload_channels(sd_ctx* ctx, const std::vector<cv::Mat>& images, sd_b200::DeviceBuffer& buf,
+                                     sd_b200::DeviceBuffer& table, const char* what)
+{
+    for (const cv::Mat& m : images)
+        if (m.type() != images[0].type() || (m.type() != CV_8UC1 && m.type() != CV_8UC3))
+            throw std::runtime_error(std::string(what) + ": frames must be all CV_8UC1 or all CV_8UC3");
+    return upload_interleaved(ctx, images, 1, SD_HOG_U8, buf, table, what);
+}
+
+// 32FC1 or 32FC3 frames, all of one type, on the device as float channels (upload_interleaved), for the float pyramid
+inline sd_hog_images upload_float_channels(sd_ctx* ctx, const std::vector<cv::Mat>& images, sd_b200::DeviceBuffer& buf,
+                                           sd_b200::DeviceBuffer& table, const char* what)
+{
+    for (const cv::Mat& m : images)
+        if (m.type() != images[0].type() || (m.type() != CV_32FC1 && m.type() != CV_32FC3))
+            throw std::runtime_error(std::string(what) + ": float frames must be all CV_32FC1 or all CV_32FC3");
+    return upload_interleaved(ctx, images, sizeof(float), SD_HOG_F32, buf, table, what);
 }
 
 }  // namespace hog_batch
@@ -343,15 +360,18 @@ inline std::vector<cv::Mat> hog_dense(const std::vector<cv::Mat>& images, VlHogV
 // level.  Returns, per frame, one Mat per scale as hog_dense returns it (dd * hogH rows of hogW columns), or an empty Mat for
 // an empty level (smaller than 4 px or than half a cell).  multichannel: frames keep their channels (8-bit, one channel count;
 // 8UC3 is B,G,R as given) and go through sd_hog_pyramid_images, where the channel with the largest gradient votes at each
-// pixel; bilinear_orientations (multichannel only): every pixel votes into its two nearest orientation bins.  Throws
-// std::runtime_error for no scales, a scale outside (0, 4], or a configuration that sd_hog_pyramid_shape refuses.
+// pixel; bilinear_orientations (multichannel only): every pixel votes into its two nearest orientation bins.  float_frames
+// (multichannel only): the frames are CV_32FC1 or CV_32FC3 and go through sd_hog_pyramid_float, each channel resized by
+// cv::resize's float rule, values and range as given.  Throws std::runtime_error for no scales, a scale outside (0, 4], or a
+// configuration that sd_hog_pyramid_shape refuses.
 inline std::vector<std::vector<cv::Mat>> vl_hog_pyramid(const std::vector<cv::Mat>& images, const std::vector<double>& scales,
                                                         VlHogVariant variant, int cell_size, int num_bins, bool multichannel = false,
-                                                        bool bilinear_orientations = false)
+                                                        bool bilinear_orientations = false, bool float_frames = false)
 {
     if (images.empty()) return {};
     if (scales.empty()) throw std::runtime_error("vl_hog_pyramid: no scales");
     if (bilinear_orientations && !multichannel) throw std::runtime_error("vl_hog_pyramid: bilinear_orientations needs multichannel");
+    if (float_frames && !multichannel) throw std::runtime_error("vl_hog_pyramid: float_frames needs multichannel");
     sd_ctx* ctx = sd_b200::context();
     const int n = static_cast<int>(images.size()), S = static_cast<int>(scales.size());
     hog_batch::Results res;
@@ -364,7 +384,11 @@ inline std::vector<std::vector<cv::Mat>> vl_hog_pyramid(const std::vector<cv::Ma
             res.add(dd * h, w);
         }
     sd_b200::DeviceBuffer buf, table;
-    if (multichannel) {
+    if (float_frames) {
+        const sd_hog_images batch = hog_batch::upload_float_channels(ctx, images, buf, table, "vl_hog_pyramid upload");
+        sd_b200::check(ctx, sd_hog_pyramid_float(ctx, &batch, scales.data(), S, cell_size, num_bins, variant, bilinear_orientations ? 1 : 0,
+                                                 res.out(), res.offsets(ctx, "vl_hog_pyramid")), "sd_hog_pyramid_float");
+    } else if (multichannel) {
         const sd_hog_images batch = hog_batch::upload_channels(ctx, images, buf, table, "vl_hog_pyramid upload");
         sd_b200::check(ctx, sd_hog_pyramid_images(ctx, &batch, scales.data(), S, cell_size, num_bins, variant, bilinear_orientations ? 1 : 0,
                                                   res.out(), res.offsets(ctx, "vl_hog_pyramid")), "sd_hog_pyramid_images");
@@ -443,17 +467,19 @@ inline hog_detection to_hog_detection(const sd_hog_detection& r) { return {cv::R
 // A sliding-window detector over image pyramids: vl_hog_pyramid of every frame, vl_hog_correlate of the filter bank on every
 // level, then sd_hog_detections over all score maps (the scores above threshold, their boxes in frame pixels, the first
 // max_candidates of each frame by score, and greedy non-maximum suppression at IoU overlap over all filters as one class).
-// Arguments as vl_hog_pyramid and vl_hog_correlate take them; filters trained with multichannel or bilinear_orientations are
-// scored with the same.  Returns one list per frame, in the rule's order (include/sd_b200.h); each box is what detect_faces
+// Arguments as vl_hog_pyramid and vl_hog_correlate take them; filters trained with multichannel, bilinear_orientations or
+// float_frames are scored with the same.  Returns one list per frame, in the rule's order (include/sd_b200.h); each box is what detect_faces
 // takes.  Throws std::runtime_error where those calls or sd_hog_detections refuse.
 inline std::vector<std::vector<hog_detection>> vl_hog_detect(const std::vector<cv::Mat>& images, const std::vector<double>& scales,
                                                              const std::vector<cv::Mat>& filters, VlHogVariant variant, int cell_size,
                                                              int num_bins, const std::vector<float>& bias, int pad_x, int pad_y,
                                                              float threshold, double overlap, int max_candidates, int max_detections,
-                                                             bool multichannel = false, bool bilinear_orientations = false)
+                                                             bool multichannel = false, bool bilinear_orientations = false,
+                                                             bool float_frames = false)
 {
     if (images.empty()) return {};
-    const std::vector<std::vector<cv::Mat>> pyr = vl_hog_pyramid(images, scales, variant, cell_size, num_bins, multichannel, bilinear_orientations);
+    const std::vector<std::vector<cv::Mat>> pyr = vl_hog_pyramid(images, scales, variant, cell_size, num_bins, multichannel, bilinear_orientations,
+                                                                 float_frames);
     const int dd = sd_b200::hog_dimension(variant, num_bins);
     const int Q = static_cast<int>(filters.size());
     if (Q < 1 || filters[0].rows % dd) throw std::runtime_error("vl_hog_detect: no filters, or filters not dd * fh rows");
@@ -532,14 +558,14 @@ struct hog_part_detection {
 // A star-model detector over image pyramids: vl_hog_pyramid over the root scales and their doubles (a scale present in both is
 // computed once; root scales must be in (0, 2]), vl_hog_correlate of the roots and of all Q * P parts, then on the device
 // sd_hog_distance_transform, sd_hog_part_scores, sd_hog_detections (the root's filter size and pad, all components as one
-// class) and sd_hog_part_placements; an unbounded model takes sd_hog_distance_transform_exact and sd_hog_part_placements_mapped.  multichannel and bilinear_orientations as vl_hog_pyramid takes them: a model of colour
+// class) and sd_hog_part_placements; an unbounded model takes sd_hog_distance_transform_exact and sd_hog_part_placements_mapped.  multichannel, bilinear_orientations and float_frames as vl_hog_pyramid takes them: a model of colour
 // HOG is scored with the values it was built for.  Returns one list per frame, in the rule's order; each detection's box is
 // what detect_faces takes.  Throws std::runtime_error for a model of inconsistent shapes and where those calls refuse.
 inline std::vector<std::vector<hog_part_detection>> vl_hog_part_detect(const std::vector<cv::Mat>& images, const std::vector<double>& scales,
                                                                        const hog_part_model& model, VlHogVariant variant, int cell_size,
                                                                        int num_bins, float threshold, double overlap, int max_candidates,
                                                                        int max_detections, bool multichannel = false,
-                                                                       bool bilinear_orientations = false)
+                                                                       bool bilinear_orientations = false, bool float_frames = false)
 {
     if (images.empty()) return {};
     const int dd = sd_b200::hog_dimension(variant, num_bins);
@@ -569,7 +595,8 @@ inline std::vector<std::vector<hog_part_detection>> vl_hog_part_detect(const std
     for (double s : scales)
         if (std::find(every.begin(), every.end(), 2 * s) == every.end()) every.push_back(2 * s);
     auto index = [&every](double s) { return static_cast<int>(std::find(every.begin(), every.end(), s) - every.begin()); };
-    const std::vector<std::vector<cv::Mat>> pyr = vl_hog_pyramid(images, every, variant, cell_size, num_bins, multichannel, bilinear_orientations);
+    const std::vector<std::vector<cv::Mat>> pyr = vl_hog_pyramid(images, every, variant, cell_size, num_bins, multichannel, bilinear_orientations,
+                                                                 float_frames);
     const int n = static_cast<int>(images.size());
     std::vector<cv::Mat> root_maps;
     std::vector<std::array<int, 2>> root_of;   // (frame, scale index)
@@ -729,23 +756,25 @@ struct hog_filter {
 
 // Trains a HOG filter for vl_hog_detect with a squared-hinge SVM and hard-negative mining (sd_hog_train_filter; the rule is in
 // include/sd_b200.h).  images: 8UC1 or 8UC3 (B,G,R) frames of any sizes; box k, boxes[k] in frame pixels, belongs to frame
-// box_frame[k]; frames without a box are pure negative frames.  multichannel and bilinear_orientations as vl_hog_pyramid takes
-// them (sd_hog_train_filter_images); vl_hog_detect scores the filter with the same values.  Throws std::runtime_error where
-// sd_hog_train_filter refuses.
+// box_frame[k]; frames without a box are pure negative frames.  multichannel, bilinear_orientations and float_frames as
+// vl_hog_pyramid takes them (sd_hog_train_filter_images, with float_frames sd_hog_train_filter_float on CV_32FC1 or CV_32FC3
+// frames); vl_hog_detect scores the filter with the same values.  Throws std::runtime_error where sd_hog_train_filter refuses.
 inline hog_filter train_hog_filter(const std::vector<cv::Mat>& images, const std::vector<int>& box_frame, const std::vector<cv::Rect>& boxes,
                                    const std::vector<double>& scales, VlHogVariant variant, int cell_size, int num_bins, int filter_w,
                                    int filter_h, int pad_x, int pad_y, const sd_hog_train_param& params, bool multichannel = false,
-                                   bool bilinear_orientations = false)
+                                   bool bilinear_orientations = false, bool float_frames = false)
 {
     if (images.empty()) throw std::runtime_error("train_hog_filter: no frames");
     if (box_frame.size() != boxes.size()) throw std::runtime_error("train_hog_filter: box_frame and boxes differ in length");
     if (params.rounds < 0 || params.max_negatives < 1) throw std::runtime_error("train_hog_filter: rounds < 0 or max_negatives < 1");
     if (bilinear_orientations && !multichannel) throw std::runtime_error("train_hog_filter: bilinear_orientations needs multichannel");
+    if (float_frames && !multichannel) throw std::runtime_error("train_hog_filter: float_frames needs multichannel");
     sd_ctx* ctx = sd_b200::context();
     sd_b200::DeviceBuffer buf, table;
     sd_image_batch grey{};
     sd_hog_images colour{};
-    if (multichannel) colour = hog_batch::upload_channels(ctx, images, buf, table, "train_hog_filter upload");
+    if (float_frames) colour = hog_batch::upload_float_channels(ctx, images, buf, table, "train_hog_filter upload");
+    else if (multichannel) colour = hog_batch::upload_channels(ctx, images, buf, table, "train_hog_filter upload");
     else grey = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), buf, "train_hog_filter upload");
     std::vector<sd_hog_box> hb;
     for (size_t k = 0; k < boxes.size(); ++k)
@@ -758,10 +787,11 @@ inline hog_filter train_hog_filter(const std::vector<cv::Mat>& images, const std
     int num_negatives = 0;
     const int nb = static_cast<int>(hb.size()), S = static_cast<int>(scales.size());
     if (multichannel)
-        sd_b200::check(ctx, sd_hog_train_filter_images(ctx, &colour, bilinear_orientations ? 1 : 0, hb.data(), nb, scales.data(), S, cell_size,
-                                                       num_bins, variant, filter_w, filter_h, pad_x, pad_y, &params, d_filter.as<float>(),
-                                                       &out.bias, out.rounds.data(), out.negatives.data(), &num_negatives),
-                       "sd_hog_train_filter_images");
+        sd_b200::check(ctx, (float_frames ? sd_hog_train_filter_float : sd_hog_train_filter_images)(
+                                ctx, &colour, bilinear_orientations ? 1 : 0, hb.data(), nb, scales.data(), S, cell_size, num_bins, variant,
+                                filter_w, filter_h, pad_x, pad_y, &params, d_filter.as<float>(), &out.bias, out.rounds.data(),
+                                out.negatives.data(), &num_negatives),
+                       float_frames ? "sd_hog_train_filter_float" : "sd_hog_train_filter_images");
     else
         sd_b200::check(ctx, sd_hog_train_filter(ctx, &grey, hb.data(), nb, scales.data(), S, cell_size, num_bins, variant, filter_w, filter_h,
                                                 pad_x, pad_y, &params, d_filter.as<float>(), &out.bias, out.rounds.data(),

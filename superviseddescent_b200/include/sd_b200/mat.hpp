@@ -25,6 +25,7 @@
 #define CV_8UC1 0
 #define CV_8UC3 16
 #define CV_32FC1 5
+#define CV_32FC3 21
 
 namespace cv {
 
@@ -72,7 +73,7 @@ public:
     }
 
     int type() const { return type_; }
-    int channels() const { return type_ == CV_8UC3 ? 3 : 1; }
+    int channels() const { return type_ == CV_8UC3 || type_ == CV_32FC3 ? 3 : 1; }
     bool empty() const { return data_ == nullptr || rows == 0 || cols == 0; }
     bool isContinuous() const { return step_ == static_cast<size_t>(cols) * elem_size(type_); }
     size_t step() const { return step_; }
@@ -126,7 +127,7 @@ public:
     template <class T> T* end() { return ptr<T>(0) + static_cast<size_t>(rows) * cols; }
 
 private:
-    static size_t elem_size(int type) { return type == CV_32FC1 ? 4 : (type == CV_8UC3 ? 3 : 1); }
+    static size_t elem_size(int type) { return type == CV_32FC1 ? 4 : type == CV_8UC3 ? 3 : type == CV_32FC3 ? 12 : 1; }
     int type_ = CV_32FC1;
     size_t step_ = 0;
     unsigned char* data_ = nullptr;
