@@ -115,6 +115,13 @@ typedef struct {
     const sd_frame* d_frames;
 } sd_image_batch;
 
+/* A left-right mirrored sample: OR-ed into a sample's frame index in d_image_index of sd_hog_batch / sd_hog_debug and in
+ * sd_level_frames.d_sample_frame of sd_train_level, sd_apply_level and sd_level_chunk_rows (both routes).  The sample is then a
+ * sample of its frame's mirror, read in place (see sd_hog_batch).  A flag bit rather than a field, so that no struct and no
+ * signature changes.  Every other call that takes frame indices (sd_detect_faces_*'s face_frame, the dense, pyramid and window
+ * calls) treats a flagged index as out of range. */
+#define SD_SAMPLE_MIRRORED (1 << 30)
+
 /* One host frame (sd_detect_faces_host, sd_upload_frames): 8UC1, or 8UC3 with interleaved B,G,R (converted exactly as
  * sd_bgr2gray does). */
 typedef struct {
@@ -163,6 +170,11 @@ SD_API int sd_hog_feature_length(int num_landmarks, const sd_hog_param* p);
  * image index out of range raises a flag on the device that the NEXT synchronising call on the context reports as
  * SD_ERR_INVALID: sd_sync, sd_hog_debug, sd_detect_batch_device / _host.
  * For sample i: image = images[d_image_index ? d_image_index[i] : i], landmarks = d_x[i, 0:2L].
+ * Mirrored samples: d_image_index[i] = frame | SD_SAMPLE_MIRRORED makes sample i a sample of the frame's left-right mirror
+ * M[y][u] = f[y][W - 1 - u] (cv::flip(f, 1)), with its landmarks in M's coordinates.  Every result -- feature rows, and
+ * sd_hog_debug's centre, half size, resized patch and bins -- is bit for bit what the call gives with M passed as a frame of
+ * its own; no copy of M is made (the kernel reads f's window right to left).  W is the frame's width (the batch's width or
+ * d_frames[frame].width), not its ROI's.  A flagged index whose frame is out of range raises the same flag as an unflagged one.
  * Writes the reference's feature row (per landmark [dim][cell col][cell row], then bias 1)
  * to d_A[i*ld .. i*ld + D).  Columns [D, ld) are left untouched.  hog.c:174-204,595-728,857-1062
  * run fused with the crop / zero-pad / cv::resize glue of adaptive_vlhog.hpp:123-176.
@@ -873,7 +885,10 @@ SD_API int sd_subtract_templates(sd_ctx* ctx, float* d_A, int64_t lda, const flo
  *     Frames that break these rules are SD_ERR_INVALID before any work is queued.  Every rank passes its own frames.
  *   - d_sample_frame (device, N ints, may be NULL = frame i): sample i reads frame d_sample_frame[i].  An index out of range raises
  *     the projection's status flag (reported by the next synchronising call, as for sd_hog_batch); on the host route the sample
- *     then reads frame 0. */
+ *     then reads frame 0.  frame | SD_SAMPLE_MIRRORED makes sample i a mirrored sample of the frame (as in sd_hog_batch), on
+ *     either route: X, lambda and x_next are bit for bit those of the same call with the mirror passed as a frame of its own.  On
+ *     the host route the gather plans the frame's window of a mirrored patch, and samples of one frame, mirrored or not, share
+ *     one region of it. */
 typedef struct {
     const sd_image_batch* images;      /* frames resident on the device, or NULL */
     const sd_host_frame* host_frames;  /* frames in pinned host memory, or NULL */

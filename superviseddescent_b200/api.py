@@ -617,6 +617,10 @@ class _PinnedBuffer:
             pass
 
 
+# sd_level_frames / sd_hog_batch: OR-ed into a sample's frame index, the sample is a sample of the frame's left-right mirror
+SAMPLE_MIRRORED = 1 << 30
+
+
 class HogTransform:
     """Projection functor h.  images: (count, H, W) uint8 (8UC1) or (count, H, W, 3) uint8 (8UC3, B G R: converted
     once on the device as adaptive_vlhog.hpp:114-120 does per call), on host or device, or a list of such frames of any
@@ -624,7 +628,11 @@ class HogTransform:
 
     A list may name one frame several times (rcr-train makes 11 samples per photo): entries that are the same object or share
     data pointer, shape and strides are one frame, held once.  image_index (optional, N ints): sample i reads images[image_index[i]]
-    (default: sample i reads images[i]).  Host frames whose grey bytes fit in DEVICE_FRAME_SHARE of the free device memory are
+    (default: sample i reads images[i]).  mirrored (optional, N bools, one per sample as image_index): sample i is a sample of the
+    left-right mirror of its frame (np.fliplr, cv::flip(f, 1)), with its landmarks in the mirror's coordinates (mirror_landmarks);
+    the frame is still held once and read right to left, and every row is bit for bit that of the mirror passed as a frame of
+    its own.  The flags hold wherever the transform's sample map is used: __call__ and debug without a training_index, into
+    without an image_index, and the optimiser's train / test / predict.  Host frames whose grey bytes fit in DEVICE_FRAME_SHARE of the free device memory are
     uploaded when the transform is first used; larger sets stay in host memory and the optimiser gathers them level by level.
     Frames the levels can read in place (pinned and aligned, sd_host_frame_in_place) are read at every level, so changing them
     after the first use changes the result; the others are copied once, on first use, into one pinned buffer.  Until the first
@@ -632,13 +640,13 @@ class HogTransform:
 
     __call__(parameters, regressor_level, training_index) keeps the reference's meaning
     (adaptive_vlhog.hpp:109) but takes ALL rows at once: parameters is (N, 2L) and training_index an
-    optional (N,) int array of indices into images (default: the sample -> frame map above).  A single (2L,) row
+    optional (N,) int array of indices into images (default: the sample -> frame map above), read unmirrored.  A single (2L,) row
     with an int training_index is accepted too (predict()'s call shape, superviseddescent.hpp:332).
     """
 
     def __init__(self, images, hog_params: Sequence[HoGParam], model_landmarks_list: Sequence[str],
                  right_eye_identifiers: Sequence[str], left_eye_identifiers: Sequence[str], ctx: Optional[Context] = None,
-                 image_index=None):
+                 image_index=None, mirrored=None):
         self.ctx = ctx or default_context()
         self.hog_params = list(hog_params)
         self.norm = InterEyeDistanceNormalisation(model_landmarks_list, right_eye_identifiers, left_eye_identifiers)
@@ -660,6 +668,13 @@ class HogTransform:
             sample = (self._list_frame[idx] if self._list_frame is not None else idx).astype(np.int32)
         else:
             sample = self._list_frame
+        if mirrored is not None:
+            flags = np.ascontiguousarray(mirrored, dtype=bool).ravel()
+            n_samples = idx.size if image_index is not None else n_list
+            if flags.size != n_samples:
+                raise ValueError(f"mirrored has {flags.size} entries for {n_samples} samples")
+            base = sample if sample is not None else np.arange(n_samples, dtype=np.int32)
+            sample = np.where(flags, base | np.int32(SAMPLE_MIRRORED), base).astype(np.int32)
         self._sample_frame = None if sample is None else torch.from_numpy(np.ascontiguousarray(sample, dtype=np.int32)).to(f"cuda:{self.ctx.device}")
 
     @staticmethod
@@ -1205,6 +1220,59 @@ def perturb(facebox, translation_x: float, translation_y: float, scaling: float 
     if rc != 0:
         raise SdError(rc, "sd_perturb_box")
     return tuple(int(v) for v in out)
+
+
+# ibug-68's left-right pairs (1-based ids): jaw 1-17, brows 18-27, nose 32-36, eyes 37-48, outer lip 49-60, inner lip 61-68.  Every
+# other id (9, 28-31, 34, 52, 58, 63, 67) is its own mirror.
+IBUG68_MIRROR_PAIRS = (tuple((i, 18 - i) for i in range(1, 9)) + tuple((i, 45 - i) for i in range(18, 23)) + ((32, 36), (33, 35))
+                       + ((37, 46), (38, 45), (39, 44), (40, 43), (41, 48), (42, 47))
+                       + ((49, 55), (50, 54), (51, 53), (56, 60), (57, 59)) + ((61, 65), (62, 64), (66, 68)))
+_IBUG68_MIRROR = {**{a: b for a, b in IBUG68_MIRROR_PAIRS}, **{b: a for a, b in IBUG68_MIRROR_PAIRS}}
+
+
+def mirror_permutation(landmark_ids: Sequence[str]) -> np.ndarray:
+    """The left-right correspondence of a model's landmark list under ibug-68 ids (the rcr_22 and ibug-68 lists use them): perm[l]
+    is the position of landmark l's mirror partner in the list.  Raises ValueError when an id is not an ibug-68 id or its partner
+    is not in the list.  A caller with another id scheme passes its own permutation to mirror_landmarks."""
+    ids = [str(i) for i in landmark_ids]
+    pos = {v: k for k, v in enumerate(ids)}
+    perm = np.empty(len(ids), dtype=np.int64)
+    for k, v in enumerate(ids):
+        try:
+            n = int(v)
+        except ValueError:
+            raise ValueError(f"mirror_permutation: landmark id {v!r} is not an ibug-68 id") from None
+        if not 1 <= n <= 68:
+            raise ValueError(f"mirror_permutation: landmark id {v!r} is not an ibug-68 id")
+        partner = str(_IBUG68_MIRROR.get(n, n))
+        if partner not in pos:
+            raise ValueError(f"mirror_permutation: the mirror partner {partner} of landmark {v} is not in the list")
+        perm[k] = pos[partner]
+    return perm
+
+
+def mirror_landmarks(x, frame_width, perm) -> np.ndarray:
+    """Landmarks of the left-right mirrored frames: x is (N, 2L) float32 rows [x_0 .. x_{L-1}, y_0 .. y_{L-1}] (or one (2L,) row),
+    frame_width one width or one per row, perm a landmark permutation (mirror_permutation).  x'[l] = W - 1 - x[perm[l]] and
+    y'[l] = y[perm[l]], in float32: the pixel at column u of a frame is at column W - 1 - u of its mirror (np.fliplr, cv::flip)."""
+    x = np.asarray(x, dtype=np.float32)
+    single = x.ndim == 1
+    x = np.atleast_2d(x)
+    perm = np.asarray(perm, dtype=np.int64)
+    L = x.shape[1] // 2
+    if x.shape[1] != 2 * L or perm.shape != (L,):
+        raise ValueError("mirror_landmarks: x must be (N, 2L) and perm (L,)")
+    w = np.broadcast_to(np.asarray(frame_width, dtype=np.float32).reshape(-1, 1), (x.shape[0], 1))
+    out = np.empty_like(x)
+    out[:, :L] = (w - np.float32(1)) - x[:, perm]
+    out[:, L:] = x[:, L + perm]
+    return out[0] if single else out
+
+
+def mirror_box(box, frame_width: int):
+    """The box (x, y, w, h) of a frame as a box of its left-right mirror: (W - x - w, y, w, h)."""
+    x, y, w, h = (int(v) for v in box)
+    return (int(frame_width) - x - w, y, w, h)
 
 
 def calculate_normalised_landmark_errors(predictions, groundtruth, model_landmarks: Sequence[str], right_eye_identifiers: Sequence[str],

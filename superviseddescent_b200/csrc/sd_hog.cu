@@ -177,10 +177,19 @@ constexpr int kTmaClasses = 8;
 __host__ __device__ constexpr int hog_tma_box(int c) { return c == 0 ? 32 : c == 1 ? 48 : c == 2 ? 64 : c == 3 ? 80 : c == 4 ? 96 : c == 5 ? 112 : c == 6 ? 128 : 160; }
 struct HogMaps { CUtensorMap m[kTmaClasses]; };
 
+// Whether sample i is a sample of its frame's mirror (CTA-uniform).  Only the MIR instantiations, launched for an index that
+// may carry SD_SAMPLE_MIRRORED, ask; the others compile to the unmirrored kernel.  hog_patch_kernel asks again where it needs
+// the answer instead of keeping a flag live through S1, which would push the compiled-in schedules past 32 registers.
+template <bool MIR>
+__device__ __forceinline__ bool hog_sample_mirrored(const HogArgs& a, int sample)
+{
+    return MIR && sd_sample_is_mirrored(a.image_index[sample]);
+}
+
 // NT threads per CTA.  The compiled-in schedules fit 32 registers without spills, so an SM holds 2048 / NT CTAs where shared
 // memory allows; the run-time ones (NT = 256) spill at that bound and keep the compiler's choice (a minimum of 0 CTAs per SM
 // sets no bound).
-template <int KT, int NCT, int CST, int NT>
+template <int KT, int NCT, int CST, int NT, bool MIR>
 __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(const __grid_constant__ HogArgs a, const __grid_constant__ HogMaps maps)
 {
     // whole warps, and at least one row group of the fs <= 64 resize (NT / fs >= 1)
@@ -217,6 +226,7 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
     const int cx = __float2int_rn(row[lm]);
     const int cy = __float2int_rn(row[lm + a.L]);
     int img_idx = a.image_index ? a.image_index[sample] : sample;
+    if (MIR) img_idx = sd_sample_frame_of(img_idx);
     if (img_idx < 0 || img_idx >= a.image_count) {
         img_idx = 0;
         if (tid == 0 && a.status) atomicOr(a.status, 2);
@@ -242,8 +252,11 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
     }
 
     // ---- S1: zero-padded crop + fixed-point bilinear resize.  The P x P source window is staged in shared memory with its
-    //      zero padding materialised, then resampled from there: one output row per warp pass, lanes along x.
-    const int x0 = cx - half, y0 = cy - half;
+    //      zero padding materialised, then resampled from there: one output row per warp pass, lanes along x.  A mirrored
+    //      sample's centre cx is a column of the mirror M; its window is the frame's window starting at x0 (sd_window_x0), which
+    //      is staged by the same route as any other and then reversed row by row in shared memory, so that from then on column
+    //      c of the staged window is M's column c and the resize, and everything after it, runs on M's window unchanged.
+    const int x0 = sd_window_x0(cx, half, W, hog_sample_mirrored<MIR>(a, sample)), y0 = cy - half;
     uint8_t* s_stage = smem + lay.bin;                             // [bin | r1 | vote] are dead until S2
     const int stage_cap = lay.stage_end - lay.bin;
     // TMA route: whole frames resident and describable by a tensor map; the smallest box class that covers the window and
@@ -327,6 +340,21 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
             }
             __syncthreads();                                       // tables (and the load loops' stores) visible
             if (tma_box) hog_tma_wait(s_mbar);
+            if (hog_sample_mirrored<MIR>(a, sample)) {
+                // swap columns c and P - 1 - c of every staged row (P is even), a row per warp, lanes along the row; the resize's
+                // clamped tap P - 1 + 1 (weight 0) may still read the unreversed byte past the window
+#pragma unroll 1
+                for (int r = warp; r < P; r += kWarps) {
+                    uint8_t* q = s_stage + r * pitch + shiftb;
+#pragma unroll 1
+                    for (int c = lane; c < half; c += 32) {
+                        const uint8_t u = q[c], v = q[P - 1 - c];
+                        q[c] = v;
+                        q[P - 1 - c] = u;
+                    }
+                }
+                __syncthreads();
+            }
             if (fs <= 64) {
                 // a thread keeps TWO adjacent output columns (their taps and weights stay in registers) and walks down the
                 // rows: NT / ceil(fs / 2) row groups, the rest of the threads idle.  When the four taps of the pair lie in the
@@ -387,7 +415,9 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
                 }
             }
         } else {
-            // window too large for the staging area: sample straight from global memory with full checks
+            // window too large for the staging area: sample straight from global memory with full checks; a mirrored sample's
+            // column u of M's window is column P - 1 - u of the frame's
+            const bool mirrored = hog_sample_mirrored<MIR>(a, sample);
             __syncthreads();                                       // tables visible
             for (int dy = warp; dy < fs; dy += kWarps) {
                 const int4 yt = s_tab[dy];
@@ -398,7 +428,8 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
                     int p[4];
 #pragma unroll
                     for (int q = 0; q < 4; ++q) {
-                        const int ix = x0 + sx + (q & 1), iy = (q & 2) ? iy1 : iy0;
+                        const int u = sx + (q & 1);
+                        const int ix = mirrored ? x0 + P - 1 - u : x0 + u, iy = (q & 2) ? iy1 : iy0;
                         int v = 0;
                         if ((q & 1) && xa.y == 0) { p[q] = 0; continue; }
                         if ((unsigned)ix < (unsigned)W && (unsigned)iy < (unsigned)H) {
@@ -595,7 +626,22 @@ __global__ void __launch_bounds__(kHogThreads) hog_normalise_kernel(const NormAr
     }
 }
 
-int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x,
+// the hog_patch_kernel instantiation of a configuration and its threads per CTA: a compiled-in schedule (DESIGN §4.1) or a run-time one
+template <bool MIR>
+decltype(&hog_patch_kernel<0, 0, 0, kHogThreads, MIR>) pick_hog_kernel(int K, int nc, int cs, int* threads)
+{
+    *threads = kHogThreads;
+    if (nc == 5 && (K == 4 || K == 9)) {
+#define SD_HOG_PICK(KK, CC, TT) if (K == KK && cs == CC) { *threads = TT; return hog_patch_kernel<KK, 5, CC, TT, MIR>; }
+        SD_HOG_PICK(4, 11, 224) SD_HOG_PICK(4, 10, 160) SD_HOG_PICK(4, 8, 160) SD_HOG_PICK(4, 6, 128)
+        SD_HOG_PICK(9, 11, 256) SD_HOG_PICK(9, 10, 160) SD_HOG_PICK(9, 8, 160) SD_HOG_PICK(9, 6, 128)
+#undef SD_HOG_PICK
+    }
+    return K == 4 ? hog_patch_kernel<4, 0, 0, kHogThreads, MIR> : K == 9 ? hog_patch_kernel<9, 0, 0, kHogThreads, MIR>
+                                                                       : hog_patch_kernel<0, 0, 0, kHogThreads, MIR>;
+}
+
+int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, bool mirrors, const float* d_x,
                int64_t ldx, int N, int L, const sd_normalisation* eyes, const sd_hog_param* p, float* d_A,
                int64_t ld, int32_t* d_geometry, uint8_t* d_patches, int8_t* d_bins)
 {
@@ -680,17 +726,11 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
         }
     }
 
-    auto kern = hog_patch_kernel<0, 0, 0, kHogThreads>;
+    // an index that may carry SD_SAMPLE_MIRRORED takes the MIR instantiations; without one (or for detect's face_frame) the
+    // launch is the unmirrored kernel
     int threads = kHogThreads;
-    if (a.K == 4) kern = hog_patch_kernel<4, 0, 0, kHogThreads>;
-    else if (a.K == 9) kern = hog_patch_kernel<9, 0, 0, kHogThreads>;
-    if (a.nc == 5 && (a.K == 4 || a.K == 9)) {
-        // the compiled-in schedules and their threads per CTA (DESIGN §4.1)
-#define SD_HOG_PICK(KK, CC, TT) if (a.K == KK && a.cs == CC) { kern = hog_patch_kernel<KK, 5, CC, TT>; threads = TT; }
-        SD_HOG_PICK(4, 11, 224) SD_HOG_PICK(4, 10, 160) SD_HOG_PICK(4, 8, 160) SD_HOG_PICK(4, 6, 128)
-        SD_HOG_PICK(9, 11, 256) SD_HOG_PICK(9, 10, 160) SD_HOG_PICK(9, 8, 160) SD_HOG_PICK(9, 6, 128)
-#undef SD_HOG_PICK
-    }
+    const auto kern = mirrors && d_image_index ? pick_hog_kernel<true>(a.K, a.nc, a.cs, &threads)
+                                               : pick_hog_kernel<false>(a.K, a.nc, a.cs, &threads);
     SD_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
     // Default shared-memory carve-out: the maximum one ran the four detect levels no faster (5.84 ms both, 4096 faces, one
     // H100 80GB HBM3 at a 400 W power limit; measured at 256 threads, when registers, not shared memory, bounded the CTAs per
@@ -707,6 +747,16 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
 }
 
 }  // namespace
+
+int sd_hog_batch_unmirrored(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int64_t ldx,
+                            int num_samples, int num_landmarks, const sd_normalisation* eyes, const sd_hog_param* p, float* d_A,
+                            int64_t ld)
+{
+    if (num_samples == 0) return SD_OK;
+    SD_REQUIRE(ctx, d_A, "null output");
+    return launch_hog(ctx, images, d_image_index, false, d_x, ldx, num_samples, num_landmarks, eyes, p, d_A, ld, nullptr, nullptr,
+                      nullptr);
+}
 
 namespace {
 // cv::cvtColor(BGR2GRAY), 8-bit, OpenCV >= 3 fixed point (15-bit coefficients): HBM-bound, 3 bytes read + 1 written per
@@ -758,7 +808,7 @@ int sd_hog_batch(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_ima
     if (!ctx) return SD_ERR_INVALID;
     if (num_samples == 0) return SD_OK;
     SD_REQUIRE(ctx, d_A, "null output");
-    return launch_hog(ctx, images, d_image_index, d_x, ldx, num_samples, num_landmarks, eyes, p, d_A, ld,
+    return launch_hog(ctx, images, d_image_index, true, d_x, ldx, num_samples, num_landmarks, eyes, p, d_A, ld,
                       nullptr, nullptr, nullptr);
 }
 
@@ -767,7 +817,7 @@ int sd_hog_debug(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_ima
                  const sd_hog_param* p, int32_t* d_geometry, uint8_t* d_patches, int8_t* d_bins)
 {
     if (!ctx) return SD_ERR_INVALID;
-    return launch_hog(ctx, images, d_image_index, d_x, ldx, num_samples, num_landmarks, eyes, p, nullptr, 0,
+    return launch_hog(ctx, images, d_image_index, true, d_x, ldx, num_samples, num_landmarks, eyes, p, nullptr, 0,
                       d_geometry, d_patches, d_bins);
 }
 

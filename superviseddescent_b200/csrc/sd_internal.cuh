@@ -216,6 +216,11 @@ int syrk_upper(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ
                bool big, bool unbiased, const sd_row_filter* rows = nullptr);
 bool syrk_is_big(int K, int64_t MI, int64_t NJ);
 
+// sd_hog_batch for callers whose index is not a sample map (detect's face_frame): an SD_SAMPLE_MIRRORED bit there is an index
+// out of range, as it always was (sd_hog.cu)
+int sd_hog_batch_unmirrored(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int64_t ldx,
+                            int num_samples, int num_landmarks, const sd_normalisation* eyes, const sd_hog_param* p, float* d_A,
+                            int64_t ld);
 int sd_check_hog_status(sd_ctx* ctx, const char* what);   // sd_api.cu: synchronises, reports and clears the projection's flags
 // the grids of an sd_hog_grids call, validated; per-grid descriptors are read back once into *table (if given) (sd_hog_render.cu)
 int sd_read_hog_grids(sd_ctx* ctx, const char* fn, const sd_hog_grids* grids, int* max_w, int* max_h, std::vector<sd_hog_grid>* table);
@@ -364,6 +369,18 @@ __device__ __forceinline__ int sd_patch_half(const float* __restrict__ row, int 
     }
     return half;
 }
+
+// A sample's frame index with its SD_SAMPLE_MIRRORED bit (include/sd_b200.h): the frame it reads and whether it is mirrored.
+// A negative index is neither decoded nor mirrored: it stays out of range, as before.  The HOG kernel (sd_hog.cu) and the
+// host-frame gather (sd_train.cu, device and host side) all decode it here.
+__host__ __device__ __forceinline__ bool sd_sample_is_mirrored(int32_t v) { return v >= 0 && (v & SD_SAMPLE_MIRRORED) != 0; }
+__host__ __device__ __forceinline__ int sd_sample_frame_of(int32_t v) { return sd_sample_is_mirrored(v) ? v & ~SD_SAMPLE_MIRRORED : v; }
+
+// First column, in frame f of width W, of the P = 2 half wide window of a patch centred at column cx (cvRound of the landmark).
+// Unmirrored: cx - half.  Mirrored, cx is a column of the mirror M[y][u] = f[y][W - 1 - u], whose window [cx - half, cx + half)
+// is f's window [W - cx - half, W - cx + half) read right to left.  hog_patch_kernel and roi_plan_kernel both call it, so the
+// region a training gather plans is the region the kernel reads.
+__device__ __forceinline__ int sd_window_x0(int cx, int half, int W, bool mirrored) { return mirrored ? W - cx - half : cx - half; }
 
 // cv::cvtColor(BGR2GRAY) of one 8-bit pixel, OpenCV >= 3 fixed point (15-bit coefficients, SURVEY.md 8c).  The only spelling of
 // the conversion: bgr2gray_kernel (sd_hog.cu) and the colour ROI gather (sd_model.cu) both call it.

@@ -162,7 +162,7 @@ int detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, 
     float* cur = xa;
     float* nxt = xb;
     for (int s = 0; s < m->num_levels; ++s) {               // superviseddescent.hpp:326-342
-        int rc = sd_hog_batch(ctx, images, d_image_index, cur, P, count, L, &m->norm, &m->hog[s], A, ld);
+        int rc = sd_hog_batch_unmirrored(ctx, images, d_image_index, cur, P, count, L, &m->norm, &m->hog[s], A, ld);
         if (rc) return rc;
         rc = sd_cascade_update(ctx, A, ld, count, m->rows[s], m->d_weights[s], P, cur, &m->norm, nxt);
         if (rc) return rc;

@@ -69,6 +69,7 @@ struct HostGather {
     GatherRec* d_rec;                     // grey records [0, F), colour records [F, 2F)
     sd_roi* d_roi;                        // per sample: its frame's region
     sd_frame* d_dims;                     // per sample: its frame's size
+    int32_t* d_hidx;                      // per sample: its HOG index into its batch, with its mirrored bit (NULL: none is mirrored)
     uint8_t* d_miss;                      // per sample: a patch read outside the region (must never be raised)
     GatherTotals* d_tot;
     int guess = 0;                        // samples the next batch starts from (gather_hog_rows)
@@ -81,7 +82,7 @@ constexpr int kLayoutThreads = 1024;
 // frame of sample s, as the HOG kernel resolves an image index: an index out of range raises the status flag and reads frame 0
 __device__ __forceinline__ int sample_frame(const int32_t* __restrict__ idx, int s, int F, int* status)
 {
-    int f = idx[s];
+    int f = sd_sample_frame_of(idx[s]);
     if (f < 0 || f >= F) {
         if (status) atomicOr(status, 2);
         f = 0;
@@ -89,25 +90,31 @@ __device__ __forceinline__ int sample_frame(const int32_t* __restrict__ idx, int
     return f;
 }
 
-// One block per sample: the union of [cvRound(x_l) - half, cvRound(x_l) + half) over its L patches, merged into its frame's slot.
+// One block per sample: the union of the windows of its L patches in its frame, [x0, x0 + 2 half) x [cy - half, cy + half) with
+// x0 = sd_window_x0 (cvRound(x_l) - half, or the frame's window of a mirrored patch), merged into its frame's slot.
 __global__ void __launch_bounds__(kPlanThreads) roi_plan_kernel(const float* __restrict__ x, int L, const int32_t* __restrict__ idx,
-                                                                int F, const sd_eyes_dev eyes, float rel, int fixed_half,
-                                                                int2* __restrict__ lo, int2* __restrict__ hi, int* status)
+                                                                int F, const FrameDev* __restrict__ fr, const sd_eyes_dev eyes,
+                                                                float rel, int fixed_half, int2* __restrict__ lo, int2* __restrict__ hi,
+                                                                int* status)
 {
     const int s = blockIdx.x;
     const float* __restrict__ row = x + (long long)s * 2 * L;
-    __shared__ int s_half;
+    __shared__ int s_half, s_frame, s_width, s_mirrored;
     __shared__ int s_box[4][kPlanThreads / 32];
     if (threadIdx.x == 0) {
         bool degenerate;
         s_half = sd_patch_half(row, L, eyes, rel, fixed_half, &degenerate);   // the HOG kernel flags a degenerate sample itself
+        s_frame = sample_frame(idx, s, F, status);
+        s_width = fr[s_frame].width;
+        s_mirrored = sd_sample_is_mirrored(idx[s]);
     }
     __syncthreads();
     int x0 = INT_MAX, y0 = INT_MAX, x1 = INT_MIN, y1 = INT_MIN;
     for (int l = threadIdx.x; l < L; l += kPlanThreads) {
         const int cx = __float2int_rn(row[l]), cy = __float2int_rn(row[l + L]);
-        x0 = min(x0, cx - s_half); y0 = min(y0, cy - s_half);
-        x1 = max(x1, cx + s_half); y1 = max(y1, cy + s_half);
+        const int wx = sd_window_x0(cx, s_half, s_width, s_mirrored);
+        x0 = min(x0, wx); y0 = min(y0, cy - s_half);
+        x1 = max(x1, wx + 2 * s_half); y1 = max(y1, cy + s_half);
     }
     for (int o = 16; o > 0; o >>= 1) {
         x0 = min(x0, __shfl_xor_sync(0xffffffffu, x0, o)); y0 = min(y0, __shfl_xor_sync(0xffffffffu, y0, o));
@@ -120,7 +127,7 @@ __global__ void __launch_bounds__(kPlanThreads) roi_plan_kernel(const float* __r
         for (int k = 1; k < kPlanThreads / 32; ++k) {
             x0 = min(x0, s_box[0][k]); y0 = min(y0, s_box[1][k]); x1 = max(x1, s_box[2][k]); y1 = max(y1, s_box[3][k]);
         }
-        const int f = sample_frame(idx, s, F, status);
+        const int f = s_frame;
         atomicMin(&lo[f].x, x0); atomicMin(&lo[f].y, y0);
         atomicMax(&hi[f].x, x1); atomicMax(&hi[f].y, y1);
     }
@@ -128,12 +135,13 @@ __global__ void __launch_bounds__(kPlanThreads) roi_plan_kernel(const float* __r
 
 // One block over all frames: every touched union is clipped to its frame, its x aligned down to 16 pixels and its width bounded by
 // row_stride / channels (as detect's face_roi does), laid out at an exclusive scan of the region bytes, given a gather record, and
-// its slot emptied for the next batch.  Then each of the batch's n samples receives its frame's region and size.
+// its slot emptied for the next batch.  Then each of the batch's n samples receives its frame's region and size, and, when some
+// sample is mirrored (hidx), its index into the batch with its mirrored bit.
 __global__ void __launch_bounds__(kLayoutThreads) gather_layout_kernel(const FrameDev* __restrict__ fr, int F, int2* __restrict__ lo,
                                                                        int2* __restrict__ hi, sd_roi* __restrict__ froi,
                                                                        GatherRec* __restrict__ rec, const int32_t* __restrict__ idx, int n,
                                                                        sd_roi* __restrict__ roi, sd_frame* __restrict__ dims,
-                                                                       GatherTotals* __restrict__ tot)
+                                                                       int32_t* __restrict__ hidx, GatherTotals* __restrict__ tot)
 {
     __shared__ long long s_scan[kLayoutThreads / 32];
     __shared__ long long s_base, s_pcie;
@@ -200,6 +208,7 @@ __global__ void __launch_bounds__(kLayoutThreads) gather_layout_kernel(const Fra
         const int f = sample_frame(idx, s, F, nullptr);        // roi_plan_kernel has flagged a bad index
         roi[s] = froi[f];
         dims[s] = sd_frame{fr[f].width, fr[f].height, 0, 0, 0};
+        if (hidx) hidx[s] = sd_sample_is_mirrored(idx[s]) ? s | SD_SAMPLE_MIRRORED : s;
     }
     if (tid == 0) *tot = GatherTotals{s_base, s_pcie, s_ng, s_nc};
 }
@@ -224,7 +233,12 @@ int gather_prepare(sd_ctx* ctx, HostGather& g, const sd_level_frames& src, int N
         SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     }
     std::vector<char> used(F, 0);
-    for (int s = 0; s < N; ++s) used[idx[s] >= 0 && idx[s] < F ? idx[s] : 0] = 1;
+    bool mirrored = false;
+    for (int s = 0; s < N; ++s) {
+        const int f = sd_sample_frame_of(idx[s]);
+        used[f >= 0 && f < F ? f : 0] = 1;
+        mirrored = mirrored || sd_sample_is_mirrored(idx[s]);
+    }
     std::vector<FrameDev> fr(F);
     PinnedRange last;
     size_t largest = 0;
@@ -250,8 +264,9 @@ int gather_prepare(sd_ctx* ctx, HostGather& g, const sd_level_frames& src, int N
     const size_t b_fr = sd_round16(F * sizeof(FrameDev)), b_lo = sd_round16(F * sizeof(int2)), b_froi = sd_round16(F * sizeof(sd_roi));
     const size_t b_rec = sd_round16(2 * F * sizeof(GatherRec)), b_roi = sd_round16(n * sizeof(sd_roi)), b_dims = sd_round16(n * sizeof(sd_frame));
     const size_t b_idx = src.d_sample_frame ? 0 : sd_round16(n * sizeof(int32_t));
-    uint8_t* t = (uint8_t*)sd_workspace(ctx, SD_WS_GATHER,
-                                        b_fr + 2 * b_lo + b_froi + b_rec + b_roi + b_dims + b_idx + sd_round16(n) + sizeof(GatherTotals));
+    const size_t b_hidx = mirrored ? sd_round16(n * sizeof(int32_t)) : 0;
+    uint8_t* t = (uint8_t*)sd_workspace(ctx, SD_WS_GATHER, b_fr + 2 * b_lo + b_froi + b_rec + b_roi + b_dims + b_idx + b_hidx +
+                                                               sd_round16(n) + sizeof(GatherTotals));
     if (!t) return SD_ERR_CUDA;
     g.d_fr = (FrameDev*)t;                      t += b_fr;
     g.d_lo = (int2*)t;                          t += b_lo;
@@ -261,6 +276,7 @@ int gather_prepare(sd_ctx* ctx, HostGather& g, const sd_level_frames& src, int N
     g.d_roi = (sd_roi*)t;                       t += b_roi;
     g.d_dims = (sd_frame*)t;                    t += b_dims;
     int32_t* d_idx = (int32_t*)t;               t += b_idx;
+    g.d_hidx = b_hidx ? (int32_t*)t : nullptr;  t += b_hidx;
     g.d_miss = t;                               t += sd_round16(n);
     g.d_tot = (GatherTotals*)t;
     g.num_frames = F;
@@ -311,11 +327,12 @@ int gather_hog_rows(sd_ctx* ctx, HostGather& g, const float* d_x, int r0, int ro
         int nb = g.guess < rows - b0 ? g.guess : rows - b0;
         GatherTotals t;
         for (;;) {
-            roi_plan_kernel<<<nb, kPlanThreads, 0, ctx->copy_stream>>>(d_x + (int64_t)s0 * P, L, g.d_sample_frame + s0, g.num_frames, eyes_dev,
-                                                                       p->relative_patch_size, fixed_half, g.d_lo, g.d_hi, status);
+            roi_plan_kernel<<<nb, kPlanThreads, 0, ctx->copy_stream>>>(d_x + (int64_t)s0 * P, L, g.d_sample_frame + s0, g.num_frames, g.d_fr,
+                                                                       eyes_dev, p->relative_patch_size, fixed_half, g.d_lo, g.d_hi, status);
             SD_LAUNCH_CHECK(ctx, "roi_plan_kernel");
             gather_layout_kernel<<<1, kLayoutThreads, 0, ctx->copy_stream>>>(g.d_fr, g.num_frames, g.d_lo, g.d_hi, g.d_froi, g.d_rec,
-                                                                            g.d_sample_frame + s0, nb, g.d_roi + s0, g.d_dims + s0, g.d_tot);
+                                                                            g.d_sample_frame + s0, nb, g.d_roi + s0, g.d_dims + s0,
+                                                                            g.d_hidx ? g.d_hidx + s0 : nullptr, g.d_tot);
             SD_LAUNCH_CHECK(ctx, "gather_layout_kernel");
             SD_CUDA(ctx, cudaMemcpyAsync(&t, g.d_tot, sizeof(t), cudaMemcpyDeviceToHost, ctx->copy_stream));
             SD_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
@@ -340,7 +357,7 @@ int gather_hog_rows(sd_ctx* ctx, HostGather& g, const float* d_x, int r0, int ro
         ib.d_roi = g.d_roi + s0;
         ib.d_roi_miss = g.d_miss + s0;
         ib.d_frames = g.d_dims + s0;
-        rc = sd_hog_batch(ctx, &ib, nullptr, d_x + (int64_t)s0 * P, P, nb, L, eyes, p, d_chunk + (int64_t)b0 * ld, ld);
+        rc = sd_hog_batch(ctx, &ib, g.d_hidx ? g.d_hidx + s0 : nullptr, d_x + (int64_t)s0 * P, P, nb, L, eyes, p, d_chunk + (int64_t)b0 * ld, ld);
         if (rc) return rc;
         SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[buf], ctx->stream));
         ctx->gathered_bytes += t.pcie;

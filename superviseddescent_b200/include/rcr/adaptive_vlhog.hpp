@@ -163,10 +163,19 @@ inline sd_hog_images upload_float_channels(sd_ctx* ctx, const std::vector<cv::Ma
 class HogTransform {
 public:
     // Do not call with `images` that are temporaries (the reference holds a const&, adaptive_vlhog.hpp:188).
+    // mirrored (optional, one entry per image entry, i.e. per sample): entry i is a sample of the left-right mirror of its photo
+    // (cv::flip(image, 1)), with its landmarks in the mirror's coordinates (rcr::mirror_landmarks).  The photo is still held once
+    // -- a mirrored shallow copy shares its frame -- and read right to left (SD_SAMPLE_MIRRORED): rows, weights and predictions are
+    // bit for bit those of a flipped deep copy.
     HogTransform(const std::vector<cv::Mat>& images, std::vector<HoGParam> hog_params, std::vector<std::string> modelLandmarksList,
-                 std::vector<std::string> rightEyeIdentifiers, std::vector<std::string> leftEyeIdentifiers)
+                 std::vector<std::string> rightEyeIdentifiers, std::vector<std::string> leftEyeIdentifiers,
+                 std::vector<bool> mirrored = {})
         : images(images), hog_params(hog_params), modelLandmarksList(modelLandmarksList), rightEyeIdentifiers(rightEyeIdentifiers),
-          leftEyeIdentifiers(leftEyeIdentifiers), dev(std::make_shared<DeviceImages>()) {}
+          leftEyeIdentifiers(leftEyeIdentifiers), mirrored(mirrored), dev(std::make_shared<DeviceImages>())
+    {
+        if (!this->mirrored.empty() && this->mirrored.size() != images.size())
+            throw std::runtime_error("HogTransform: mirrored needs one entry per image");
+    }
 
     int feature_length(size_t level) const
     {
@@ -183,7 +192,7 @@ public:
         sd_b200::DeviceBuffer dx, dA(static_cast<size_t>(D) * sizeof(float)), didx(sizeof(int32_t));
         sd_b200::upload(parameters, dx, parameters.cols);
         // an index outside images stays out of range, and the projection reports it
-        const int32_t idx = trainingIndex >= 0 && trainingIndex < static_cast<int>(dev->frame_of.size()) ? dev->frame_of[trainingIndex] : -1;
+        const int32_t idx = trainingIndex >= 0 && trainingIndex < static_cast<int>(dev->frame_of.size()) ? sample_index(trainingIndex) : -1;
         sd_b200::check(ctx, sd_memcpy_h2d(ctx, didx.as<int32_t>(), &idx, sizeof(idx)), "HogTransform");
         const sd_normalisation nrm = eyes();
         const sd_hog_param p = hog_params[regressorLevel].c();
@@ -255,6 +264,12 @@ public:
     }
 
 private:
+    // the frame image entry i reads, with SD_SAMPLE_MIRRORED when the entry is mirrored
+    int32_t sample_index(size_t i) const
+    {
+        return dev->frame_of[i] | (!mirrored.empty() && mirrored[i] ? SD_SAMPLE_MIRRORED : 0);
+    }
+
     struct DeviceImages {
         std::vector<sd_host_frame> frames;   // the distinct frames (on the host route: where the levels read them)
         std::vector<int32_t> frame_of;        // images[i] -> distinct frame
@@ -287,8 +302,10 @@ private:
             frames.push_back(f);
             grey += static_cast<size_t>(f.height) * ((static_cast<size_t>(f.width) + 15) / 16 * 16);
         }
+        std::vector<int32_t> index(all.size());
+        for (size_t i = 0; i < all.size(); ++i) index[i] = sample_index(i);
         dev->index.allocate(all.size() * sizeof(int32_t));
-        sd_b200::check(ctx, sd_memcpy_h2d(ctx, dev->index.as<int32_t>(), dev->frame_of.data(), all.size() * sizeof(int32_t)), "HogTransform upload");
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, dev->index.as<int32_t>(), index.data(), all.size() * sizeof(int32_t)), "HogTransform upload");
         sd_b200::check(ctx, sd_sync(ctx), "HogTransform upload");
         size_t free_bytes = 0, total = 0;
         sd_b200::check(ctx, sd_device_memory(ctx, &free_bytes, &total), "sd_device_memory");
@@ -327,6 +344,7 @@ private:
     std::vector<std::string> modelLandmarksList;
     std::vector<std::string> rightEyeIdentifiers;
     std::vector<std::string> leftEyeIdentifiers;
+    std::vector<bool> mirrored;          // per image entry: a sample of the photo's mirror (empty: none)
     std::shared_ptr<DeviceImages> dev;   // shared between the copies the optimiser makes of this functor
 };
 

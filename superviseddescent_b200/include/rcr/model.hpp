@@ -23,6 +23,58 @@ inline cv::Mat align_mean(cv::Mat mean, cv::Rect facebox, float scaling_x = 1.0f
     return aligned;
 }
 
+// ---- mirrored samples (the landmark correspondence of a left-right flip; Python: mirror_permutation / mirror_landmarks / mirror_box)
+// perm[l] = the position of landmark l's mirror partner in the list, under ibug-68 ids (the rcr_22 and ibug-68 lists use them):
+// the pairs 1-17 .. 8-10, 18-27 .. 22-23, 32-36, 33-35, 37-46, 38-45, 39-44, 40-43, 41-48, 42-47, 49-55, 50-54, 51-53, 56-60,
+// 57-59, 61-65, 62-64, 66-68; every other id is its own mirror.  Throws when an id is not an ibug-68 id or its partner is not in
+// the list; a caller with another id scheme passes its own permutation to mirror_landmarks.
+inline std::vector<int> mirror_permutation(const std::vector<std::string>& landmark_ids)
+{
+    static const int pairs[][2] = {{1, 17}, {2, 16}, {3, 15}, {4, 14}, {5, 13}, {6, 12}, {7, 11}, {8, 10}, {18, 27}, {19, 26},
+                                   {20, 25}, {21, 24}, {22, 23}, {32, 36}, {33, 35}, {37, 46}, {38, 45}, {39, 44}, {40, 43},
+                                   {41, 48}, {42, 47}, {49, 55}, {50, 54}, {51, 53}, {56, 60}, {57, 59}, {61, 65}, {62, 64}, {66, 68}};
+    int partner[69];
+    for (int i = 0; i <= 68; ++i) partner[i] = i;
+    for (const auto& p : pairs) { partner[p[0]] = p[1]; partner[p[1]] = p[0]; }
+    std::vector<int> perm(landmark_ids.size());
+    for (size_t k = 0; k < landmark_ids.size(); ++k) {
+        const std::string& id = landmark_ids[k];
+        int n = 0;
+        bool digits = !id.empty() && id.size() <= 2;
+        for (char c : id) digits = digits && c >= '0' && c <= '9';
+        if (digits) n = std::stoi(id);
+        if (!digits || n < 1 || n > 68) throw std::runtime_error("mirror_permutation: landmark id " + id + " is not an ibug-68 id");
+        const std::string want = std::to_string(partner[n]);
+        size_t j = 0;
+        while (j < landmark_ids.size() && landmark_ids[j] != want) ++j;
+        if (j == landmark_ids.size()) throw std::runtime_error("mirror_permutation: the mirror partner " + want + " of landmark " + id + " is not in the list");
+        perm[k] = static_cast<int>(j);
+    }
+    return perm;
+}
+
+// Landmark rows [x_0 .. x_{L-1}, y_0 .. y_{L-1}] (CV_32FC1, one per row) of left-right mirrored frames: x'[l] = W - 1 - x[perm[l]],
+// y'[l] = y[perm[l]], in float, with frame_width[r] the width of row r's frame (one entry: the same width for every row).
+inline cv::Mat mirror_landmarks(cv::Mat x, const std::vector<int>& frame_width, const std::vector<int>& perm)
+{
+    const int L = x.cols / 2;
+    if (x.cols != 2 * L || static_cast<int>(perm.size()) != L || frame_width.empty() ||
+        (frame_width.size() != 1 && static_cast<int>(frame_width.size()) != x.rows))
+        throw std::runtime_error("mirror_landmarks: x must be N x 2L, perm L long and frame_width 1 or N long");
+    cv::Mat out(x.rows, x.cols, CV_32FC1);
+    for (int r = 0; r < x.rows; ++r) {
+        const float w1 = static_cast<float>(frame_width[frame_width.size() == 1 ? 0 : r]) - 1.0f;
+        for (int l = 0; l < L; ++l) {
+            out.at<float>(r, l) = w1 - x.at<float>(r, perm[l]);
+            out.at<float>(r, L + l) = x.at<float>(r, L + perm[l]);
+        }
+    }
+    return out;
+}
+
+// a box of a frame of width W as a box of its left-right mirror: (W - x - w, y, w, h)
+inline cv::Rect mirror_box(cv::Rect box, int frame_width) { return cv::Rect(frame_width - box.x - box.width, box.y, box.width, box.height); }
+
 class InterEyeDistanceNormalisation {
 public:
     InterEyeDistanceNormalisation() = default;
