@@ -5,9 +5,9 @@
 Workload: --frames B,G,R frames of 1280 x 720 per call, cell size 8, K = 9, UoCTTI, 21 levels at 2^(-l/5), l = 0 .. 20.  The
 grey pyramid reads the frames' grey conversion (done once, outside the timing); the colour pyramid reads the interleaved
 frames in place.  Per frame, with CUDA events: the grey and the colour pyramid alternated in one run; the colour pyramid with
-bilinear orientations; and, from a torch.profiler pass of its own after the timed runs, the colour pyramid's resize
-(hog_pyramid_resize_images_kernel) and HOG (hog_images_kernel) launches, and the grey pyramid's (hog_pyramid_resize_kernel,
-hog_dense_kernel).  Then vl_hog_detect end to end (host clock around a synchronised call, read-back included), grey against
+bilinear orientations; and, from torch.profiler passes after the timed runs, one per pyramid because both resize with
+hog_pyramid_resize_images_kernel, each pyramid's resize launches and HOG launches (hog_dense_kernel for the grey pyramid,
+hog_images_kernel for the colour one).  Then vl_hog_detect end to end (host clock around a synchronised call, read-back included), grey against
 colour, with Q = 2 (a 6 x 6-cell filter and its mirror).  The card's name, power limit and clock are read in the same run.
 One JSON line per measurement; nothing is written into the tree.
 """
@@ -121,20 +121,20 @@ def main():
     emit({"measure": "colour_over_grey", "ratio_of_medians": statistics.median(times["colour"]) / statistics.median(times["grey"]),
           "bilinear_over_grey": statistics.median(times["colour_bilinear"]) / statistics.median(times["grey"])})
 
-    # per-launch kernel times: a profiler pass of its own
+    # per-launch kernel times: a profiler pass of its own for each pyramid, whose resize launches share a kernel name
     from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(3):
-            grey_call()
-            colour_call()
-        torch.cuda.synchronize()
-    per_kernel = {}
-    for e in prof.key_averages():
-        for name in ("hog_pyramid_resize_images_kernel", "hog_pyramid_resize_kernel", "hog_images_kernel", "hog_dense_kernel"):
-            if name in e.key and e.device_type.name == "CUDA":
-                t = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0)
-                per_kernel[name] = per_kernel.get(name, 0.0) + t / 3 / n          # us per frame
-    emit({"measure": "pyramid_kernels_us_per_frame", **per_kernel})
+    for route, call in (("grey", grey_call), ("colour", colour_call)):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(3):
+                call()
+            torch.cuda.synchronize()
+        per_kernel = {}
+        for e in prof.key_averages():
+            for name in ("hog_pyramid_resize_images_kernel", "hog_images_kernel", "hog_dense_kernel"):
+                if name in e.key and e.device_type.name == "CUDA":
+                    t = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0)
+                    per_kernel[name] = per_kernel.get(name, 0.0) + t / 3 / n      # us per frame
+        emit({"measure": f"pyramid_{route}_kernels_us_per_frame", **per_kernel})
 
     # vl_hog_detect end to end, grey against colour, Q = 2
     rng = np.random.default_rng(2)

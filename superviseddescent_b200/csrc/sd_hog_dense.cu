@@ -20,6 +20,11 @@
 // Every histogram depends only on the frame's pixels and is summed in a fixed order (the order of the landmark-patch
 // kernel's two vote passes), so the result does not depend on the tiling, on the batch, or on the run.  A frame of
 // fs x fs pixels gives, bit for bit, the features the patch kernel computes from the same fs x fs patch.
+//
+// Pyramids (sd_hog_pyramid, sd_hog_pyramid_images, sd_hog_pyramid_float and the filter trainer's slices) are one routine,
+// sd_hog_pyramid_frames, on a host list of frames that each entry point reads once by its own rules: per slice of frames, every
+// level resized into scratch by hog_pyramid_resize_images_kernel, then one dense pass over the levels, hog_dense_kernel for
+// batches that sd_hog_dense takes (8-bit grey, nearest bins) and hog_images_kernel for the others.
 #include "sd_internal.cuh"
 #include "sd_hog_common.cuh"
 
@@ -459,6 +464,12 @@ ImagesKernel images_kernel(int K)
     return K == 4 ? hog_images_kernel<4, Pix, BIL> : K == 9 ? hog_images_kernel<9, Pix, BIL> : hog_images_kernel<0, Pix, BIL>;
 }
 
+ImagesKernel images_kernel(int dtype, bool bil, int K)
+{
+    return dtype == SD_HOG_U8 ? (bil ? images_kernel<uint8_t, true>(K) : images_kernel<uint8_t, false>(K))
+                              : (bil ? images_kernel<float, true>(K) : images_kernel<float, false>(K));
+}
+
 template <bool BIL>
 PolarKernel polar_kernel(int K)
 {
@@ -580,10 +591,11 @@ int launch_dense(sd_ctx* ctx, const char* fn, const char* name, void (*kern)(Arg
     return SD_OK;
 }
 
-// ---- the pyramid (sd_hog_pyramid): every level of every frame resized into scratch (hog_pyramid_resize_kernel), then all of
-//      them through hog_dense_kernel as one batch of sd_frame descriptors (the load-loop route: the levels differ in size).
-//      The batch is cut into slices whose levels fit kPyramidSliceBytes (one frame at least), so the scratch is bounded by
-//      the slice, not by the batch.
+// ---- the pyramid (sd_hog_pyramid, sd_hog_pyramid_images, sd_hog_pyramid_float): every level of every frame resized into
+//      scratch, each channel on its own by the rule of the frames' type (hog_resize_tap, hog_resize_tap_f32) and written
+//      interleaved ((H, W, C) elements of that type, rows at a pitch of C * w elements rounded up to 16 bytes), then all of them
+//      through one dense pass.  The batch is cut into slices whose levels fit kPyramidSliceBytes (one frame at least), so the
+//      scratch is bounded by the slice, not by the batch.
 constexpr int kResizeW = 64, kResizeH = 16, kResizeThreads = 256;   // output pixels of a resize CTA
 constexpr size_t kPyramidSliceBytes = size_t(64) << 20;
 constexpr double kPyramidMaxSide = 1 << 28;                          // px per side of a level
@@ -600,86 +612,14 @@ bool pyramid_level(int width, int height, double scale, int* lw, int* lh)
     return true;
 }
 
-struct PyrLevel {
-    long long src, dst;          // byte offsets of the frame's first pixel from the batch's data, of the level's from the scratch
-    int W, H, rs;                // the frame: size and row stride
-    int w, h, pitch;             // the level: size and row stride
-    int tile0, tiles_x;          // the level's first CTA of the resize launch, and its CTAs per row of tiles
-    int slot;                    // frame * num_scales + scale: the caller's output offset of the level
-};
-
-struct ResizeArgs {
-    const uint8_t* images;
-    uint8_t* scratch;
-    const PyrLevel* levels;
-    int count;
-    const int64_t* out_offset;   // the caller's, per slot
-    int64_t* level_offset;       // per level: the caller's offset of its slot (the dense kernel's out_offset)
-};
-
-// One CTA per kResizeW x kResizeH tile of one level: the taps of its columns and rows (hog_resize_tap), then cv::resize's two
-// fixed-point passes per pixel, the source read through L1.  A level of the frame's own size is copied.
-__global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_kernel(const __grid_constant__ ResizeArgs a)
-{
-    __shared__ int s_sx[kResizeW], s_xw[kResizeW], s_y0[kResizeH], s_y1[kResizeH], s_yw[kResizeH];
-    const int b = blockIdx.x, tid = threadIdx.x;
-    const int lo = sd_find_last_le(0, a.count - 1, b, [&](int i) { return a.levels[i].tile0; });   // the level of tile b
-    const PyrLevel L = a.levels[lo];
-    const int t = b - L.tile0, ty = t / L.tiles_x;
-    const int x0 = (t - ty * L.tiles_x) * kResizeW, y0 = ty * kResizeH;
-    if (t == 0 && tid == 0) a.level_offset[lo] = a.out_offset[L.slot];
-    const uint8_t* __restrict__ src = a.images + L.src;
-    uint8_t* __restrict__ dst = a.scratch + L.dst;
-    const bool copy = L.w == L.W && L.h == L.H;
-    if (!copy) {
-        if (tid < kResizeW) {
-            if (x0 + tid < L.w) {
-                const HogResizeTap r = hog_resize_tap(x0 + tid, L.w, L.W);
-                s_sx[tid] = r.sx;
-                s_xw[tid] = r.xw;
-            }
-        } else if (tid < kResizeW + kResizeH) {
-            const int i = tid - kResizeW;
-            if (y0 + i < L.h) {
-                const HogResizeTap r = hog_resize_tap(y0 + i, L.h, L.H);
-                s_y0[i] = r.y0;
-                s_y1[i] = r.y1;
-                s_yw[i] = r.yw;
-            }
-        }
-        __syncthreads();
-    }
-    for (int i = tid; i < kResizeW * kResizeH; i += kResizeThreads) {
-        const int r = i / kResizeW, c = i - r * kResizeW;
-        const int x = x0 + c, y = y0 + r;
-        if (x >= L.w || y >= L.h) continue;
-        int v;
-        if (copy) {
-            v = __ldg(src + (long long)y * L.rs + x);
-        } else {
-            const int sx = s_sx[c], sx1 = min(sx + 1, L.W - 1);   // a clamped tap has zero weight
-            const int ax = (short)s_xw[c], bx = s_xw[c] >> 16;
-            const uint8_t* r0 = src + (long long)s_y0[r] * L.rs;
-            const uint8_t* r1 = src + (long long)s_y1[r] * L.rs;
-            v = hog_resize_out(s_yw[r], (int)__ldg(r0 + sx) * ax + (int)__ldg(r0 + sx1) * bx,
-                               (int)__ldg(r1 + sx) * ax + (int)__ldg(r1 + sx1) * bx);
-        }
-        dst[(long long)y * L.pitch + x] = (uint8_t)v;
-    }
-}
-
-// ---- the pyramid of 8-bit or float frames with C channels (sd_hog_pyramid_images, sd_hog_pyramid_float): each channel
-//      resized on its own by the rule of its type (hog_resize_tap, hog_resize_tap_f32), every level written interleaved ((H, W,
-//      C) elements of the frames' type, rows at a pitch of C * w elements rounded up to 16 bytes) into scratch, then all of them
-//      through hog_images_kernel as one batch of sd_hog_image descriptors
 struct PyrImageLevel {
     long long src;               // element offset of the frame's pixel (0, 0, 0) from the batch's data
     long long rs, ps, chs;       // the frame's row, pixel and channel strides in elements
     long long dst;               // byte offset of the level from the scratch
     int W, H;                    // the frame
     int w, h, pitch;             // the level: size and row stride in bytes
-    int tile0, tiles_x;
-    int slot;
+    int tile0, tiles_x;          // the level's first CTA of the resize launch, and its CTAs per row of tiles
+    int slot;                    // the level's index in the caller's output offsets
 };
 
 struct ResizeImagesArgs {
@@ -687,18 +627,21 @@ struct ResizeImagesArgs {
     uint8_t* scratch;
     const PyrImageLevel* levels;
     int count, channels;
-    const int64_t* out_offset;
-    int64_t* level_offset;
+    const int64_t* out_offset;   // the caller's, per slot
+    int64_t* level_offset;       // per level: the caller's offset of its slot (the dense kernel's out_offset)
 };
 
-// One CTA per kResizeW x kResizeH pixel tile of one level, as hog_pyramid_resize_kernel: the taps of its columns and rows once,
-// then every channel of every pixel with the channel fastest, so that a warp writes consecutive elements of the level.
-template <class T>
+// One CTA per kResizeW x kResizeH pixel tile of one level: the taps of its columns and rows once, then cv::resize's two passes
+// for every channel of every pixel with the channel fastest, so that a warp writes consecutive elements of the level, the
+// source read through L1.  A level of the frame's own size is copied.  kC = 1: 8-bit frames of one channel, contiguous pixels
+// (pixel stride 1), frames and levels of fewer than 2^31 bytes, the grey pyramid's: the pixel loop is spared two divisions by
+// a run-time count and takes every offset in 32 bits.  kC = 0: any channel count, strides and sizes.
+template <class T, int kC>
 __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kernel(const __grid_constant__ ResizeImagesArgs a)
 {
     constexpr bool f32 = std::is_same<T, float>::value;
     __shared__ int s_sx[kResizeW], s_xw[kResizeW], s_y0[kResizeH], s_y1[kResizeH], s_yw[kResizeH];
-    const int b = blockIdx.x, tid = threadIdx.x, C = a.channels;
+    const int b = blockIdx.x, tid = threadIdx.x, C = kC > 0 ? kC : a.channels;
     const int lo = sd_find_last_le(0, a.count - 1, b, [&](int i) { return a.levels[i].tile0; });
     const PyrImageLevel L = a.levels[lo];
     const int t = b - L.tile0, ty = t / L.tiles_x;
@@ -744,29 +687,53 @@ __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kern
             }
             reinterpret_cast<float*>(dst + (long long)y * L.pitch)[x * C + ch] = v;
         } else {
+            using Off = typename std::conditional<kC == 1, int, long long>::type;   // offsets within the frame and the level
+            const Off rs = (Off)L.rs, ps = kC == 1 ? 1 : (Off)L.ps;
             int v;
             if (copy) {
-                v = __ldg(s + y * L.rs + x * L.ps);
+                v = __ldg(s + (Off)y * rs + x * ps);
             } else {
                 const int sx = s_sx[c], sx1 = min(sx + 1, L.W - 1);   // a clamped tap has zero weight
                 const int ax = (short)s_xw[c], bx = s_xw[c] >> 16;
-                const uint8_t* r0 = s + s_y0[r] * L.rs;
-                const uint8_t* r1 = s + s_y1[r] * L.rs;
-                v = hog_resize_out(s_yw[r], (int)__ldg(r0 + sx * L.ps) * ax + (int)__ldg(r0 + sx1 * L.ps) * bx,
-                                   (int)__ldg(r1 + sx * L.ps) * ax + (int)__ldg(r1 + sx1 * L.ps) * bx);
+                const uint8_t* r0 = s + (Off)s_y0[r] * rs;
+                const uint8_t* r1 = s + (Off)s_y1[r] * rs;
+                v = hog_resize_out(s_yw[r], (int)__ldg(r0 + sx * ps) * ax + (int)__ldg(r0 + sx1 * ps) * bx,
+                                   (int)__ldg(r1 + sx * ps) * ax + (int)__ldg(r1 + sx1 * ps) * bx);
             }
-            dst[(long long)y * L.pitch + x * C + ch] = (uint8_t)v;
+            dst[(Off)y * L.pitch + x * C + ch] = (uint8_t)v;
         }
     }
 }
 
-// Queues the levels of a pyramid one slice of whole frames at a time, the frames' levels fitting kPyramidSliceBytes (one
-// frame at least), so the scratch is bounded by the slice and not by the batch.  lv: every non-empty level (PyrLevel or
-// PyrImageLevel), frame f's at lv[first[f] .. first[f + 1]).  Per slice it places the levels in scratch (dst, tile0) and calls
-// run(l0, n, bytes, tiles, max_w, max_h): its first level, level count, scratch bytes, resize CTAs and largest cell grid.
-template <class Level, class Run>
-int pyramid_slices(sd_ctx* ctx, const char* fn, std::vector<Level>& lv, const std::vector<int>& first, int count, int cell_size, Run run)
+// The scratch of one slice: [levels (bytes, 16-byte aligned) | level table | the dense kernel's descriptors | per-level
+// output offsets], the two tables uploaded.  Returns the scratch, or nullptr (the context holds the error).
+template <class Desc>
+uint8_t* pyramid_scratch(sd_ctx* ctx, long long bytes, const PyrImageLevel* levels, const std::vector<Desc>& desc,
+                         PyrImageLevel** d_lv, Desc** d_desc, int64_t** d_off)
 {
+    const size_t n = desc.size();
+    const size_t pix = sd_round16((size_t)bytes), lv_bytes = sizeof(PyrImageLevel) * n, desc_bytes = sizeof(Desc) * n;
+    uint8_t* ws = static_cast<uint8_t*>(sd_workspace(ctx, SD_WS_PYRAMID, pix + lv_bytes + desc_bytes + sizeof(int64_t) * n));
+    if (!ws) return nullptr;
+    *d_lv = reinterpret_cast<PyrImageLevel*>(ws + pix);
+    *d_desc = reinterpret_cast<Desc*>(ws + pix + lv_bytes);
+    *d_off = reinterpret_cast<int64_t*>(ws + pix + lv_bytes + desc_bytes);
+    if (sd_check_cuda(ctx, cudaMemcpyAsync(*d_lv, levels, lv_bytes, cudaMemcpyHostToDevice, ctx->stream), "pyramid levels") ||
+        sd_check_cuda(ctx, cudaMemcpyAsync(*d_desc, desc.data(), desc_bytes, cudaMemcpyHostToDevice, ctx->stream), "pyramid levels"))
+        return nullptr;
+    return ws;
+}
+
+// Queues the levels of a pyramid one slice of whole frames at a time, the frames' levels fitting kPyramidSliceBytes (one
+// frame at least).  lv: every non-empty level, frame f's at lv[first[f] .. first[f + 1]).  Per slice it places the levels in
+// scratch (dst, tile0), uploads them with the dense kernel's descriptor desc_of(level) of each, resizes them in one launch and
+// calls dense(n, scratch, d_desc, d_off, max_w, max_h): its level count, the descriptors and per-level output offsets in
+// scratch, and its largest cell grid.
+template <class DescOf, class Dense>
+int pyramid_slices(sd_ctx* ctx, const char* fn, const HogPyramidFrames& src, std::vector<PyrImageLevel>& lv,
+                   const std::vector<int>& first, int count, int cell_size, const int64_t* d_out_offset, DescOf desc_of, Dense dense)
+{
+    using Desc = decltype(desc_of(lv[0]));
     for (int f0 = 0; f0 < count;) {
         size_t bytes = 0;
         int f1 = f0;
@@ -781,8 +748,10 @@ int pyramid_slices(sd_ctx* ctx, const char* fn, std::vector<Level>& lv, const st
         if (n == 0) continue;
         long long pos = 0;
         int tiles = 0, max_w = 0, max_h = 0;
+        bool grey = src.dtype == SD_HOG_U8 && src.channels == 1;   // hog_pyramid_resize_images_kernel's kC = 1
+        std::vector<Desc> desc(n);
         for (int i = 0; i < n; ++i) {
-            Level& L = lv[l0 + i];
+            PyrImageLevel& L = lv[l0 + i];
             L.dst = pos;
             L.tile0 = tiles;
             if ((long long)tiles + (long long)L.tiles_x * sd_div_up(L.h, kResizeH) > INT_MAX)
@@ -791,74 +760,144 @@ int pyramid_slices(sd_ctx* ctx, const char* fn, std::vector<Level>& lv, const st
             pos += (long long)L.pitch * L.h;
             max_w = std::max(max_w, (L.w + cell_size / 2) / cell_size);
             max_h = std::max(max_h, (L.h + cell_size / 2) / cell_size);
+            desc[i] = desc_of(L);
+            grey = grey && L.ps == 1 && (long long)(L.H - 1) * L.rs + L.W <= INT_MAX && (long long)L.pitch * L.h <= INT_MAX;
         }
-        if (const int rc = run(l0, n, pos, tiles, max_w, max_h)) return rc;
+        PyrImageLevel* d_lv;
+        Desc* d_desc;
+        int64_t* d_off;
+        uint8_t* ws = pyramid_scratch(ctx, pos, lv.data() + l0, desc, &d_lv, &d_desc, &d_off);
+        if (!ws) return SD_ERR_CUDA;
+
+        ResizeImagesArgs r;
+        r.images = src.data;
+        r.scratch = ws;
+        r.levels = d_lv;
+        r.count = n;
+        r.channels = src.channels;
+        r.out_offset = d_out_offset;
+        r.level_offset = d_off;
+        const auto resize = grey ? hog_pyramid_resize_images_kernel<uint8_t, 1>
+                            : src.dtype == SD_HOG_F32 ? hog_pyramid_resize_images_kernel<float, 0> : hog_pyramid_resize_images_kernel<uint8_t, 0>;
+        resize<<<(unsigned)tiles, kResizeThreads, 0, ctx->stream>>>(r);
+        SD_LAUNCH_CHECK(ctx, "hog_pyramid_resize_images_kernel");
+        if (const int rc = dense(n, ws, d_desc, d_off, max_w, max_h)) return rc;
     }
     return SD_OK;
 }
 
-// The scratch of one slice: [levels (bytes, 16-byte aligned) | level table | the dense kernel's descriptors | per-level
-// output offsets], the two tables uploaded.  Returns the scratch, or nullptr (the context holds the error).
-template <class Level, class Desc>
-uint8_t* pyramid_scratch(sd_ctx* ctx, long long bytes, const Level* levels, const std::vector<Desc>& desc, Level** d_lv,
-                         Desc** d_desc, int64_t** d_off)
-{
-    const size_t n = desc.size();
-    const size_t pix = sd_round16((size_t)bytes), lv_bytes = sizeof(Level) * n, desc_bytes = sizeof(Desc) * n;
-    uint8_t* ws = static_cast<uint8_t*>(sd_workspace(ctx, SD_WS_PYRAMID, pix + lv_bytes + desc_bytes + sizeof(int64_t) * n));
-    if (!ws) return nullptr;
-    *d_lv = reinterpret_cast<Level*>(ws + pix);
-    *d_desc = reinterpret_cast<Desc*>(ws + pix + lv_bytes);
-    *d_off = reinterpret_cast<int64_t*>(ws + pix + lv_bytes + desc_bytes);
-    if (sd_check_cuda(ctx, cudaMemcpyAsync(*d_lv, levels, lv_bytes, cudaMemcpyHostToDevice, ctx->stream), "pyramid levels") ||
-        sd_check_cuda(ctx, cudaMemcpyAsync(*d_desc, desc.data(), desc_bytes, cudaMemcpyHostToDevice, ctx->stream), "pyramid levels"))
-        return nullptr;
-    return ws;
-}
-
-// sd_hog_pyramid_images (T = uint8_t) and sd_hog_pyramid_float (T = float) past their null and dtype checks: the arguments'
-// other checks, the frame table, every non-empty level and the slices, with levels of T at a pitch of C * w * sizeof(T) bytes
-// rounded up to 16.  fn names the entry point in errors.
+// The argument checks the pyramid entry points share, in their order (fn names the entry point in messages): channels,
+// orientation assignment, configuration, scales, frame count, data, alignment of float frames and the number of levels.
+// A call without frames passes once its count is checked.
 #define PYR_REQUIRE(cond, msg)                                                         \
     do {                                                                               \
         if (!(cond)) return sd_fail(ctx, SD_ERR_INVALID, "%s: %s", fn, msg);           \
     } while (0)
-template <class T>
-int pyramid_images(sd_ctx* ctx, const char* fn, const sd_hog_images* images, const double* h_scales, int num_scales, int cell_size,
-                   int num_bins, int variant, int bilinear_orientations, float* d_out, const int64_t* d_out_offset)
+int pyramid_check(sd_ctx* ctx, const char* fn, int channels, int bilinear_orientations, int cell_size, int num_bins, int variant,
+                  const double* h_scales, int num_scales, int count, const void* d_data, bool f32)
 {
-    constexpr int es = (int)sizeof(T);
-    PYR_REQUIRE(images->channels >= 1 && images->channels <= kDenseMaxChannels, "channels must be in [1,16]");
+    PYR_REQUIRE(channels >= 1 && channels <= kDenseMaxChannels, "channels must be in [1,16]");
     PYR_REQUIRE(bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
     if (const int rc = sd_hog_check_config(ctx, fn, variant, num_bins, cell_size)) return rc;
     PYR_REQUIRE(num_scales >= 1, "num_scales must be at least 1");
     for (int s = 0; s < num_scales; ++s)
         PYR_REQUIRE(h_scales[s] > 0.0 && h_scales[s] <= 4.0, "every scale must be finite and in (0, 4]");
-    PYR_REQUIRE(images->count >= 0, "negative frame count");
-    const int count = images->count, C = images->channels;
+    PYR_REQUIRE(count >= 0, "negative frame count");
     if (count == 0) return SD_OK;
-    PYR_REQUIRE(images->d_data, "null argument");
-    PYR_REQUIRE(es == 1 || (reinterpret_cast<uintptr_t>(images->d_data) & 3) == 0, "float frames must be 4-byte aligned");
+    PYR_REQUIRE(d_data, "null argument");
+    PYR_REQUIRE(!f32 || sd_aligned(d_data, 4), "float frames must be 4-byte aligned");
     PYR_REQUIRE((long long)count * num_scales <= INT_MAX, "too many levels");
+    return SD_OK;
+}
 
-    // the frames: the batch's, or the descriptor table read back once
-    std::vector<sd_hog_image> fr;
+// contiguous 8-bit grey frames of one size, nearest bins: hog_dense_kernel's frames, whose features it computes bit for bit
+// as hog_images_kernel does (sd_hog_dense_images and sd_hog_pyramid_images run it there)
+bool grey_batch(const sd_hog_images* images, int bilinear_orientations)
+{
+    const sd_hog_image& f = images->frame;
+    return images->dtype == SD_HOG_U8 && images->channels == 1 && !bilinear_orientations && !images->d_frames &&
+           f.pixel_stride == 1 && f.row_stride >= f.width && f.row_stride <= INT_MAX && (images->count == 1 || images->image_stride > 0);
+}
+
+// sd_hog_pyramid_images and sd_hog_pyramid_float past their null and dtype checks
+int pyramid_images(sd_ctx* ctx, const char* fn, const sd_hog_images* images, const double* h_scales, int num_scales, int cell_size,
+                   int num_bins, int variant, int bilinear_orientations, float* d_out, const int64_t* d_out_offset)
+{
+    if (const int rc = pyramid_check(ctx, fn, images->channels, bilinear_orientations, cell_size, num_bins, variant, h_scales,
+                                     num_scales, images->count, images->d_data, images->dtype == SD_HOG_F32))
+        return rc;
+    if (images->count == 0) return SD_OK;
+    HogPyramidFrames fr;
+    if (const int rc = sd_hog_read_image_frames(ctx, fn, images, bilinear_orientations, &fr)) return rc;
+    return sd_hog_pyramid_frames(ctx, fn, fr, 0, images->count, h_scales, num_scales, cell_size, num_bins, variant, d_out, d_out_offset);
+}
+#undef PYR_REQUIRE
+
+}  // namespace
+
+int sd_hog_read_grey_frames(sd_ctx* ctx, const char* fn, const sd_image_batch* images, HogPyramidFrames* out)
+{
+    const int count = images->count;
+    std::vector<sd_frame> fr;
     if (images->d_frames) {
         if (const int rc = sd_fetch_table(ctx, images->d_frames, count, fr)) return rc;
     } else {
-        PYR_REQUIRE(images->image_stride >= 0, "negative image stride");
+        if (!(count == 1 || images->image_stride > 0)) return sd_fail(ctx, SD_ERR_INVALID, "%s: bad strides", fn);
+        fr.assign(count, sd_frame{images->width, images->height, images->row_stride, 0, 0});
+        for (int i = 0; i < count; ++i) fr[i].offset = (int64_t)i * images->image_stride;
+    }
+    out->data = images->d_data;
+    out->dtype = SD_HOG_U8;
+    out->channels = 1;
+    out->bilinear = 0;
+    out->grey_kernel = 1;
+    out->frames.resize(count);
+    for (int f = 0; f < count; ++f) {
+        const sd_frame& d = fr[f];
+        if (d.width < 1 || d.height < 1 || d.row_stride < d.width || d.offset < 0)
+            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d (%d x %d, row stride %d, offset %lld) is not a frame", fn, f, d.width,
+                           d.height, d.row_stride, (long long)d.offset);
+        out->frames[f] = sd_hog_image{d.width, d.height, d.offset, d.row_stride, 1, 0};
+    }
+    return SD_OK;
+}
+
+int sd_hog_read_image_frames(sd_ctx* ctx, const char* fn, const sd_hog_images* images, int bilinear_orientations, HogPyramidFrames* out)
+{
+    const int count = images->count;
+    std::vector<sd_hog_image>& fr = out->frames;
+    if (images->d_frames) {
+        if (const int rc = sd_fetch_table(ctx, images->d_frames, count, fr)) return rc;
+    } else {
+        if (images->image_stride < 0) return sd_fail(ctx, SD_ERR_INVALID, "%s: negative image stride", fn);
         fr.assign(count, images->frame);
         for (int i = 0; i < count; ++i) fr[i].offset += (int64_t)i * images->image_stride;
     }
-    // every non-empty level of every frame, in the order of the caller's slots
-    std::vector<PyrImageLevel> lv;
-    std::vector<int> first(count + 1, 0);
     for (int f = 0; f < count; ++f) {
         const sd_hog_image& d = fr[f];
         if (d.width < 1 || d.height < 1 || d.offset < 0 || d.row_stride < 0 || d.pixel_stride < 0 || d.channel_stride < 0)
             return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d (%d x %d) is smaller than 1 x 1 or has a negative offset or stride",
                            fn, f, d.width, d.height);
-        first[f] = (int)lv.size();
+    }
+    out->data = images->d_data;
+    out->dtype = images->dtype;
+    out->channels = images->channels;
+    out->bilinear = bilinear_orientations;
+    out->grey_kernel = grey_batch(images, bilinear_orientations);
+    return SD_OK;
+}
+
+int sd_hog_pyramid_frames(sd_ctx* ctx, const char* fn, const HogPyramidFrames& src, int f0, int f1, const double* h_scales,
+                          int num_scales, int cell_size, int num_bins, int variant, float* d_out, const int64_t* d_out_offset)
+{
+    const int C = src.channels, es = src.dtype == SD_HOG_F32 ? 4 : 1, count = f1 - f0;
+    // every non-empty level of every frame, in the order of the caller's slots
+    std::vector<PyrImageLevel> lv;
+    std::vector<int> first(count + 1, 0);
+    for (int i = 0; i < count; ++i) {
+        const int f = f0 + i;
+        const sd_hog_image& d = src.frames[f];
+        first[i] = (int)lv.size();
         for (int s = 0; s < num_scales; ++s) {
             PyrImageLevel L{};
             int hw, hh, dd;
@@ -871,70 +910,51 @@ int pyramid_images(sd_ctx* ctx, const char* fn, const sd_hog_images* images, con
             L.W = d.width; L.H = d.height;
             L.pitch = dense_align(L.w * C * es, 16);
             L.tiles_x = sd_div_up(L.w, kResizeW);
-            L.slot = f * num_scales + s;
+            L.slot = i * num_scales + s;
             lv.push_back(L);
         }
     }
     first[count] = (int)lv.size();
     if (lv.empty()) return SD_OK;
 
-    // one 8-bit channel, nearest bins, contiguous rows: sd_hog_pyramid computes the same levels (as sd_hog_dense_images routes
-    // to sd_hog_dense)
-    const sd_hog_image& f0 = images->frame;
-    if (es == 1 && C == 1 && !bilinear_orientations && !images->d_frames && f0.pixel_stride == 1 && f0.row_stride >= f0.width &&
-        f0.row_stride <= INT_MAX && (count == 1 || images->image_stride > 0)) {
-        sd_image_batch ib{};
-        ib.d_data = static_cast<const uint8_t*>(images->d_data) + f0.offset;
-        ib.width = f0.width; ib.height = f0.height; ib.row_stride = (int32_t)f0.row_stride;
-        ib.image_stride = images->image_stride;
-        ib.count = count;
-        return sd_hog_pyramid(ctx, &ib, h_scales, num_scales, cell_size, num_bins, variant, d_out, d_out_offset);
+    const int dd = sd_hog_dd(num_bins, variant);
+    if (src.grey_kernel) {   // sd_frame descriptors, staged by the load loop: the levels differ in size
+        DenseArgs a = dense_args(nullptr, nullptr, cell_size, num_bins, variant, dd, d_out, nullptr);
+        const DenseSmem lay = dense_smem_layout(a.span, a.pitch, num_bins, dense_cells(a.tile));
+        CUtensorMap map;                             // not read
+        memset(&map, 0, sizeof(map));
+        return pyramid_slices(
+            ctx, fn, src, lv, first, count, cell_size, d_out_offset,
+            [](const PyrImageLevel& L) { return sd_frame{L.w, L.h, L.pitch, 0, L.dst}; },
+            [&](int n, uint8_t* ws, const sd_frame* d_desc, const int64_t* d_off, int max_w, int max_h) {
+                a.images = ws;
+                a.frames = d_desc;
+                a.out_offset = d_off;
+                return launch_dense(ctx, fn, "hog_dense_kernel", dense_kernel(num_bins), a, n, max_w, max_h, lay.total, map);
+            });
     }
-
-    const bool bil = bilinear_orientations != 0;
-    const ImagesKernel kern = bil ? images_kernel<T, true>(num_bins) : images_kernel<T, false>(num_bins);
+    const bool bil = src.bilinear != 0;
+    const ImagesKernel kern = images_kernel(src.dtype, bil, num_bins);
     ImageArgs a;
     memset(&a, 0, sizeof(a));
     a.channels = C;
     a.out = d_out;
-    a.variant = variant; a.cs = cell_size; a.K = num_bins; a.dd = sd_hog_dd(num_bins, variant);
+    a.variant = variant; a.cs = cell_size; a.K = num_bins; a.dd = dd;
     a.tile = images_tile(kern, cell_size, num_bins, bil);
     a.span = cell_size * (a.tile + 3) + 4;
     a.pi_k = 3.141592653589793 / (double)num_bins;    // VL_PI / numOrientations (hog.c:677)
     hog_orientations(num_bins, a.orient);
     const DenseSmem lay = dense_smem_layout(a.span, 0, num_bins, dense_cells(a.tile), bil);
-    return pyramid_slices(ctx, fn, lv, first, count, cell_size, [&](int l0, int n, long long bytes, int tiles, int max_w, int max_h) -> int {
-        std::vector<sd_hog_image> desc(n);
-        for (int i = 0; i < n; ++i) {
-            const PyrImageLevel& L = lv[l0 + i];
-            desc[i] = sd_hog_image{L.w, L.h, L.dst / es, L.pitch / es, C, 1};   // elements of T
-        }
-        PyrImageLevel* d_lv;
-        sd_hog_image* d_desc;
-        int64_t* d_off;
-        uint8_t* ws = pyramid_scratch(ctx, bytes, lv.data() + l0, desc, &d_lv, &d_desc, &d_off);
-        if (!ws) return SD_ERR_CUDA;
-
-        ResizeImagesArgs r;
-        r.images = images->d_data;
-        r.scratch = ws;
-        r.levels = d_lv;
-        r.count = n;
-        r.channels = C;
-        r.out_offset = d_out_offset;
-        r.level_offset = d_off;
-        hog_pyramid_resize_images_kernel<T><<<(unsigned)tiles, kResizeThreads, 0, ctx->stream>>>(r);
-        SD_LAUNCH_CHECK(ctx, "hog_pyramid_resize_images_kernel");
-
-        a.data = ws;
-        a.frames = d_desc;
-        a.out_offset = d_off;
-        return launch_dense(ctx, fn, "hog_images_kernel", kern, a, n, max_w, max_h, lay.total);
-    });
+    return pyramid_slices(
+        ctx, fn, src, lv, first, count, cell_size, d_out_offset,
+        [&](const PyrImageLevel& L) { return sd_hog_image{L.w, L.h, L.dst / es, L.pitch / es, C, 1}; },   // elements of the type
+        [&](int n, uint8_t* ws, const sd_hog_image* d_desc, const int64_t* d_off, int max_w, int max_h) {
+            a.data = ws;
+            a.frames = d_desc;
+            a.out_offset = d_off;
+            return launch_dense(ctx, fn, "hog_images_kernel", kern, a, n, max_w, max_h, lay.total);
+        });
 }
-#undef PYR_REQUIRE
-
-}  // namespace
 
 extern "C" {
 
@@ -1011,83 +1031,14 @@ int sd_hog_pyramid(sd_ctx* ctx, const sd_image_batch* images, const double* h_sc
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, images && h_scales && d_out && d_out_offset, "null argument");
     SD_REQUIRE(ctx, !images->d_roi, "a batch with regions of interest has no whole frames");
-    if (const int rc = sd_hog_check_config(ctx, __func__, variant, num_bins, cell_size)) return rc;
-    SD_REQUIRE(ctx, num_scales >= 1, "num_scales must be at least 1");
-    for (int s = 0; s < num_scales; ++s)
-        SD_REQUIRE(ctx, h_scales[s] > 0.0 && h_scales[s] <= 4.0, "every scale must be finite and in (0, 4]");
-    SD_REQUIRE(ctx, images->count >= 0, "negative frame count");
-    const int count = images->count;
-    if (count == 0) return SD_OK;
-    SD_REQUIRE(ctx, images->d_data, "null argument");
-    SD_REQUIRE(ctx, (long long)count * num_scales <= INT_MAX, "too many levels");
-
-    // the frames: the batch's, or the descriptor table read back once
-    std::vector<sd_frame> fr;
-    if (images->d_frames) {
-        if (const int rc = sd_fetch_table(ctx, images->d_frames, count, fr)) return rc;
-    } else {
-        SD_REQUIRE(ctx, count == 1 || images->image_stride > 0, "bad strides");
-        fr.assign(count, sd_frame{images->width, images->height, images->row_stride, 0, 0});
-        for (int i = 0; i < count; ++i) fr[i].offset = (int64_t)i * images->image_stride;
-    }
-    // every level of every frame, in the order of the caller's slots; empty levels are left out
-    std::vector<PyrLevel> lv;
-    std::vector<int> first(count + 1, 0);           // frame f's levels are lv[first[f] .. first[f + 1])
-    for (int f = 0; f < count; ++f) {
-        const sd_frame& d = fr[f];
-        if (d.width < 1 || d.height < 1 || d.row_stride < d.width || d.offset < 0)
-            return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d (%d x %d, row stride %d, offset %lld) is not a frame", __func__, f,
-                           d.width, d.height, d.row_stride, (long long)d.offset);
-        first[f] = (int)lv.size();
-        for (int s = 0; s < num_scales; ++s) {
-            PyrLevel L{};
-            int hw, hh, dd;
-            if (!pyramid_level(d.width, d.height, h_scales[s], &L.w, &L.h))
-                return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d at scale %g is larger than 2^28 px per side", __func__, f, h_scales[s]);
-            if (!dense_shape(L.w, L.h, cell_size, num_bins, variant, &hw, &hh, &dd)) continue;
-            L.src = d.offset;
-            L.W = d.width; L.H = d.height; L.rs = d.row_stride;
-            L.pitch = dense_align(L.w, 16);
-            L.tiles_x = sd_div_up(L.w, kResizeW);
-            L.slot = f * num_scales + s;
-            lv.push_back(L);
-        }
-    }
-    first[count] = (int)lv.size();
-    if (lv.empty()) return SD_OK;
-
-    const int dd = sd_hog_dd(num_bins, variant);
-    DenseArgs a = dense_args(nullptr, nullptr, cell_size, num_bins, variant, dd, d_out, nullptr);
-    const DenseSmem lay = dense_smem_layout(a.span, a.pitch, num_bins, dense_cells(a.tile));
-    CUtensorMap map;                                 // not read: levels of different sizes are staged by the load loop
-    memset(&map, 0, sizeof(map));
-    return pyramid_slices(ctx, __func__, lv, first, count, cell_size, [&](int l0, int n, long long bytes, int tiles, int max_w, int max_h) -> int {
-        std::vector<sd_frame> desc(n);
-        for (int i = 0; i < n; ++i) {
-            const PyrLevel& L = lv[l0 + i];
-            desc[i] = sd_frame{L.w, L.h, L.pitch, 0, L.dst};
-        }
-        PyrLevel* d_lv;
-        sd_frame* d_desc;
-        int64_t* d_off;
-        uint8_t* ws = pyramid_scratch(ctx, bytes, lv.data() + l0, desc, &d_lv, &d_desc, &d_off);
-        if (!ws) return SD_ERR_CUDA;
-
-        ResizeArgs r;
-        r.images = images->d_data;
-        r.scratch = ws;
-        r.levels = d_lv;
-        r.count = n;
-        r.out_offset = d_out_offset;
-        r.level_offset = d_off;
-        hog_pyramid_resize_kernel<<<(unsigned)tiles, kResizeThreads, 0, ctx->stream>>>(r);
-        SD_LAUNCH_CHECK(ctx, "hog_pyramid_resize_kernel");
-
-        a.images = ws;
-        a.frames = d_desc;
-        a.out_offset = d_off;
-        return launch_dense(ctx, "sd_hog_pyramid", "hog_dense_kernel", dense_kernel(num_bins), a, n, max_w, max_h, lay.total, map);
-    });
+    if (const int rc = pyramid_check(ctx, __func__, 1, 0, cell_size, num_bins, variant, h_scales, num_scales, images->count,
+                                     images->d_data, false))
+        return rc;
+    if (images->count == 0) return SD_OK;
+    HogPyramidFrames fr;
+    if (const int rc = sd_hog_read_grey_frames(ctx, __func__, images, &fr)) return rc;
+    return sd_hog_pyramid_frames(ctx, __func__, fr, 0, images->count, h_scales, num_scales, cell_size, num_bins, variant, d_out,
+                                 d_out_offset);
 }
 
 int sd_hog_pyramid_images(sd_ctx* ctx, const sd_hog_images* images, const double* h_scales, int num_scales, int cell_size,
@@ -1096,8 +1047,8 @@ int sd_hog_pyramid_images(sd_ctx* ctx, const sd_hog_images* images, const double
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, images && h_scales && d_out && d_out_offset, "null argument");
     SD_REQUIRE(ctx, images->dtype == SD_HOG_U8, "dtype must be SD_HOG_U8: the levels are resized by the 8-bit rule");
-    return pyramid_images<uint8_t>(ctx, __func__, images, h_scales, num_scales, cell_size, num_bins, variant, bilinear_orientations,
-                                   d_out, d_out_offset);
+    return pyramid_images(ctx, __func__, images, h_scales, num_scales, cell_size, num_bins, variant, bilinear_orientations, d_out,
+                          d_out_offset);
 }
 
 int sd_hog_pyramid_float(sd_ctx* ctx, const sd_hog_images* images, const double* h_scales, int num_scales, int cell_size,
@@ -1106,8 +1057,8 @@ int sd_hog_pyramid_float(sd_ctx* ctx, const sd_hog_images* images, const double*
     if (!ctx) return SD_ERR_INVALID;
     SD_REQUIRE(ctx, images && h_scales && d_out && d_out_offset, "null argument");
     SD_REQUIRE(ctx, images->dtype == SD_HOG_F32, "dtype must be SD_HOG_F32: the levels are resized by the float rule");
-    return pyramid_images<float>(ctx, __func__, images, h_scales, num_scales, cell_size, num_bins, variant, bilinear_orientations,
-                                 d_out, d_out_offset);
+    return pyramid_images(ctx, __func__, images, h_scales, num_scales, cell_size, num_bins, variant, bilinear_orientations, d_out,
+                          d_out_offset);
 }
 
 int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size, int num_bins, int variant,
@@ -1137,9 +1088,8 @@ int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size,
     }
 
     // 8-bit grey frames with contiguous rows: the staged (TMA) kernel of sd_hog_dense computes the same features
-    const sd_hog_image& fr = images->frame;
-    if (images->dtype == SD_HOG_U8 && images->channels == 1 && !bilinear_orientations && !images->d_frames && fr.pixel_stride == 1 &&
-        fr.row_stride >= fr.width && fr.row_stride <= INT_MAX && (count == 1 || images->image_stride > 0)) {
+    if (grey_batch(images, bilinear_orientations)) {
+        const sd_hog_image& fr = images->frame;
         sd_image_batch ib{};
         ib.d_data = static_cast<const uint8_t*>(images->d_data) + fr.offset;
         ib.width = fr.width; ib.height = fr.height; ib.row_stride = (int32_t)fr.row_stride;
@@ -1160,8 +1110,7 @@ int sd_hog_dense_images(sd_ctx* ctx, const sd_hog_images* images, int cell_size,
     a.out_stride = (long long)dd * max_w * max_h;
     a.variant = variant; a.cs = cell_size; a.K = num_bins; a.dd = dd;
     const bool bil = bilinear_orientations != 0;
-    const ImagesKernel kern = images->dtype == SD_HOG_U8 ? (bil ? images_kernel<uint8_t, true>(num_bins) : images_kernel<uint8_t, false>(num_bins))
-                                                         : (bil ? images_kernel<float, true>(num_bins) : images_kernel<float, false>(num_bins));
+    const ImagesKernel kern = images_kernel(images->dtype, bil, num_bins);
     a.tile = images_tile(kern, cell_size, num_bins, bil);
     a.span = cell_size * (a.tile + 3) + 4;
     a.pi_k = 3.141592653589793 / (double)num_bins;    // VL_PI / numOrientations (hog.c:677)

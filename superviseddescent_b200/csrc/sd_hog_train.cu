@@ -1,7 +1,7 @@
 // Training HOG filters for the sliding-window detector (sd_hog_windows, sd_hog_box_windows, sd_learn_squared_hinge,
 // sd_hog_train_filter): the feature rows of score positions, the window that covers a ground-truth box, a squared-hinge
-// linear SVM on the learn path, and the hard-negative mining loop that composes them with sd_hog_pyramid, sd_hog_correlate
-// and sd_hog_detections.
+// linear SVM on the learn path, and the hard-negative mining loop that composes them with the pyramid routine
+// (sd_hog_pyramid_frames), sd_hog_correlate and sd_hog_detections.
 //
 // The window gather is one CTA per row: its threads walk the row's columns in order, so the stores of a row are coalesced and
 // the loads of one (channel, dy) run of fw cells are consecutive floats of the map.  The SVM's kernels are the margins (one
@@ -14,7 +14,6 @@
 #include <cfloat>
 #include <cmath>
 #include <cstring>
-#include <functional>
 #include <set>
 #include <tuple>
 #include <vector>
@@ -415,30 +414,23 @@ int sd_learn_squared_hinge(sd_ctx* ctx, const float* d_A, int64_t lda, const flo
 
 namespace {
 
-// The trainer's frames, the one thing its two entry points differ in: their count, each one's size (read once, after the
-// arguments are checked) and the pyramids of frames [f0, f1) into d_out at sd_hog_pyramid's per-level offsets d_off.
-struct FrameSize { int width, height; };
-struct TrainFrames {
-    int count;
-    std::function<int(std::vector<FrameSize>&)> sizes;
-    std::function<int(int f0, int f1, float* d_out, const int64_t* d_off)> pyramid;
-};
-
 #define TRAIN_REQUIRE(cond, msg)                                                   \
     do {                                                                           \
         if (!(cond)) return sd_fail(ctx, SD_ERR_INVALID, "%s: %s", fn, msg);       \
     } while (0)
 
-// sd_hog_train_filter's rule (include/sd_b200.h) on the frames of src; fn names the entry point in messages
-int train_filter(sd_ctx* ctx, const char* fn, const TrainFrames& src, const sd_hog_box* h_boxes, int num_boxes, const double* h_scales,
-                 int num_scales, int cell_size, int num_bins, int variant, int filter_w, int filter_h, int pad_x, int pad_y,
-                 const sd_hog_train_param* p, float* d_filter, float* h_bias, sd_hog_train_report* h_rounds, sd_hog_window* h_negatives,
-                 int* h_num_negatives)
+// sd_hog_train_filter's rule (include/sd_b200.h) on the 8-bit grey frames of grey (sd_hog_train_filter), or else on those of
+// images with bilinear_orientations (sd_hog_train_filter_images, sd_hog_train_filter_float); fn names the entry point in messages
+int train_filter(sd_ctx* ctx, const char* fn, const sd_image_batch* grey, const sd_hog_images* images, int bilinear_orientations,
+                 const sd_hog_box* h_boxes, int num_boxes, const double* h_scales, int num_scales, int cell_size, int num_bins, int variant,
+                 int filter_w, int filter_h, int pad_x, int pad_y, const sd_hog_train_param* p, float* d_filter, float* h_bias,
+                 sd_hog_train_report* h_rounds, sd_hog_window* h_negatives, int* h_num_negatives)
 {
     if (const int rc = sd_hog_check_config(ctx, fn, variant, num_bins, cell_size)) return rc;
     if (const int rc = sd_hog_check_filter(ctx, fn, filter_w, filter_h, pad_x, pad_y)) return rc;
     TRAIN_REQUIRE(sd_aligned(d_filter, 4), "the filter must be 4-byte aligned");
-    TRAIN_REQUIRE(num_scales >= 1 && src.count >= 1 && num_boxes >= 0, "need at least one scale and one frame");
+    const int F = grey ? grey->count : images->count, S = num_scales;
+    TRAIN_REQUIRE(num_scales >= 1 && F >= 1 && num_boxes >= 0, "need at least one scale and one frame");
     for (int s = 0; s < num_scales; ++s)
         TRAIN_REQUIRE(h_scales[s] > 0.0 && h_scales[s] <= 4.0, "every scale must be finite and in (0, 4]");
     TRAIN_REQUIRE(p->lambda > 0.f && std::isfinite(p->lambda), "lambda must be positive and finite");
@@ -451,14 +443,14 @@ int train_filter(sd_ctx* ctx, const char* fn, const TrainFrames& src, const sd_h
     const int dd = sd_hog_dd(num_bins, variant);
     const int D = dd * filter_w * filter_h + 1;
     TRAIN_REQUIRE(D <= SD_HOG_TRAIN_MAX_DIM, "dd * filter_h * filter_w + 1 exceeds SD_HOG_TRAIN_MAX_DIM");
-    const int F = src.count, S = num_scales;
 
-    // the frames' sizes and level tables
-    std::vector<FrameSize> frames;
-    if (const int rc = src.sizes(frames)) return rc;
+    // the frames, read once, and their level tables
+    HogPyramidFrames fr;
+    if (const int rc = grey ? sd_hog_read_grey_frames(ctx, fn, grey, &fr) : sd_hog_read_image_frames(ctx, fn, images, bilinear_orientations, &fr))
+        return rc;
+    const std::vector<sd_hog_image>& frames = fr.frames;
     std::vector<std::vector<Level>> lv(F);
     for (int f = 0; f < F; ++f) {
-        TRAIN_REQUIRE(frames[f].width >= 1 && frames[f].height >= 1, "every frame must be at least 1 x 1");
         if (level_table(frames[f].width, frames[f].height, h_scales, S, cell_size, num_bins, variant, &lv[f]))
             return sd_fail(ctx, SD_ERR_INVALID, "%s: invalid pyramid level", fn);
     }
@@ -476,10 +468,10 @@ int train_filter(sd_ctx* ctx, const char* fn, const TrainFrames& src, const sd_h
     int unassigned = 0;
     for (int b = 0; b < num_boxes; ++b) {
         const sd_hog_box& q = h_boxes[b];
-        const FrameSize& fr = frames[q.frame];
+        const sd_hog_image& d = frames[q.frame];
         sd_hog_window wv;
         double iou;
-        best_window(lv[q.frame], fr.width, fr.height, cell_size, filter_w, filter_h, pad_x, pad_y, p->positive_overlap,
+        best_window(lv[q.frame], d.width, d.height, cell_size, filter_w, filter_h, pad_x, pad_y, p->positive_overlap,
                     sd_box64{q.x, q.y, (int64_t)q.x + q.w, (int64_t)q.y + q.h}, &wv, &iou);
         if (wv.grid < 0) {
             ++unassigned;
@@ -610,7 +602,9 @@ int train_filter(sd_ctx* ctx, const char* fn, const TrainFrames& src, const sd_h
             }
         if (grids.empty()) return SD_OK;
         SD_CUDA(ctx, cudaMemcpyAsync(d_off, off.data(), sizeof(int64_t) * off.size(), cudaMemcpyHostToDevice, ctx->stream));
-        return timed(&sd_hog_train_report::pyramid_ms, [&] { return src.pyramid(f0, f1, d_feat, d_off); });
+        return timed(&sd_hog_train_report::pyramid_ms, [&] {
+            return sd_hog_pyramid_frames(ctx, fn, fr, f0, f1, h_scales, S, cell_size, num_bins, variant, d_feat, d_off);
+        });
     };
     // gather windows (frame, level, x, y, flip) of the resident slice into rows dest[i] of d_rows
     auto gather = [&](int f0, const std::vector<sd_hog_window>& w, const std::vector<int>& dest) -> int {
@@ -791,46 +785,6 @@ int train_filter(sd_ctx* ctx, const char* fn, const TrainFrames& src, const sd_h
     return SD_OK;
 }
 
-// sd_hog_train_filter_images and sd_hog_train_filter_float past their null and dtype checks: a frame source over an
-// sd_hog_images whose slices' pyramids are pyramid's (sd_hog_pyramid_images or sd_hog_pyramid_float).  fn names the entry point.
-using ImagesPyramid = int (*)(sd_ctx*, const sd_hog_images*, const double*, int, int, int, int, int, float*, const int64_t*);
-int train_filter_images(sd_ctx* ctx, const char* fn, ImagesPyramid pyramid, const sd_hog_images* images, int bilinear_orientations,
-                        const sd_hog_box* h_boxes, int num_boxes, const double* h_scales, int num_scales, int cell_size, int num_bins,
-                        int variant, int filter_w, int filter_h, int pad_x, int pad_y, const sd_hog_train_param* p, float* d_filter,
-                        float* h_bias, sd_hog_train_report* h_rounds, sd_hog_window* h_negatives, int* h_num_negatives)
-{
-    TRAIN_REQUIRE(images->channels >= 1 && images->channels <= 16, "channels must be in [1,16]");
-    TRAIN_REQUIRE(bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
-    TRAIN_REQUIRE(images->count < 1 || images->d_data, "null argument");
-    TrainFrames src;
-    src.count = images->count;
-    src.sizes = [&](std::vector<FrameSize>& sizes) -> int {
-        std::vector<sd_hog_image> fr;
-        if (images->d_frames) {
-            if (const int rc = sd_fetch_table(ctx, images->d_frames, images->count, fr)) return rc;
-        } else {
-            TRAIN_REQUIRE(images->image_stride >= 0, "negative image stride");
-            fr.assign(images->count, images->frame);
-        }
-        for (int f = 0; f < images->count; ++f) {
-            const sd_hog_image& d = fr[f];
-            if (d.offset < 0 || d.row_stride < 0 || d.pixel_stride < 0 || d.channel_stride < 0)
-                return sd_fail(ctx, SD_ERR_INVALID, "%s: frame %d has a negative offset or stride", fn, f);
-            sizes.push_back({d.width, d.height});
-        }
-        return SD_OK;
-    };
-    src.pyramid = [&](int f0, int f1, float* d_out, const int64_t* d_off) {
-        sd_hog_images sub = *images;
-        sub.count = f1 - f0;
-        if (images->d_frames) sub.d_frames = images->d_frames + f0;
-        else sub.frame.offset += (int64_t)f0 * images->image_stride;
-        return pyramid(ctx, &sub, h_scales, num_scales, cell_size, num_bins, variant, bilinear_orientations, d_out, d_off);
-    };
-    return train_filter(ctx, fn, src, h_boxes, num_boxes, h_scales, num_scales, cell_size, num_bins, variant, filter_w, filter_h,
-                        pad_x, pad_y, p, d_filter, h_bias, h_rounds, h_negatives, h_num_negatives);
-}
-
 #undef TRAIN_REQUIRE
 
 }  // namespace
@@ -846,27 +800,9 @@ int sd_hog_train_filter(sd_ctx* ctx, const sd_image_batch* images, const sd_hog_
     SD_REQUIRE(ctx, images && h_scales && p && d_filter && h_bias && h_rounds && h_num_negatives && (num_boxes == 0 || h_boxes),
                "null argument");
     SD_REQUIRE(ctx, !images->d_roi, "a batch with regions of interest has no whole frames");
-    TrainFrames src;
-    src.count = images->count;
-    src.sizes = [&](std::vector<FrameSize>& sizes) -> int {
-        std::vector<sd_frame> fr;
-        if (images->d_frames) {
-            if (const int rc = sd_fetch_table(ctx, images->d_frames, images->count, fr)) return rc;
-        } else {
-            fr.assign(images->count, sd_frame{images->width, images->height, images->row_stride, 0, 0});
-        }
-        for (const sd_frame& d : fr) sizes.push_back({d.width, d.height});
-        return SD_OK;
-    };
-    src.pyramid = [&](int f0, int f1, float* d_out, const int64_t* d_off) {
-        sd_image_batch sub = *images;
-        sub.count = f1 - f0;
-        if (images->d_frames) sub.d_frames = images->d_frames + f0;
-        else sub.d_data = images->d_data + (int64_t)f0 * images->image_stride;
-        return sd_hog_pyramid(ctx, &sub, h_scales, num_scales, cell_size, num_bins, variant, d_out, d_off);
-    };
-    return train_filter(ctx, __func__, src, h_boxes, num_boxes, h_scales, num_scales, cell_size, num_bins, variant, filter_w, filter_h,
-                        pad_x, pad_y, p, d_filter, h_bias, h_rounds, h_negatives, h_num_negatives);
+    SD_REQUIRE(ctx, images->count < 1 || images->d_data, "null argument");
+    return train_filter(ctx, __func__, images, nullptr, 0, h_boxes, num_boxes, h_scales, num_scales, cell_size, num_bins, variant,
+                        filter_w, filter_h, pad_x, pad_y, p, d_filter, h_bias, h_rounds, h_negatives, h_num_negatives);
 }
 
 int sd_hog_train_filter_images(sd_ctx* ctx, const sd_hog_images* images, int bilinear_orientations, const sd_hog_box* h_boxes,
@@ -878,9 +814,12 @@ int sd_hog_train_filter_images(sd_ctx* ctx, const sd_hog_images* images, int bil
     SD_REQUIRE(ctx, images && h_scales && p && d_filter && h_bias && h_rounds && h_num_negatives && (num_boxes == 0 || h_boxes),
                "null argument");
     SD_REQUIRE(ctx, images->dtype == SD_HOG_U8, "dtype must be SD_HOG_U8: the levels are resized by the 8-bit rule");
-    return train_filter_images(ctx, __func__, sd_hog_pyramid_images, images, bilinear_orientations, h_boxes, num_boxes, h_scales,
-                               num_scales, cell_size, num_bins, variant, filter_w, filter_h, pad_x, pad_y, p, d_filter, h_bias,
-                               h_rounds, h_negatives, h_num_negatives);
+    SD_REQUIRE(ctx, images->channels >= 1 && images->channels <= 16, "channels must be in [1,16]");
+    SD_REQUIRE(ctx, bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
+    SD_REQUIRE(ctx, images->count < 1 || images->d_data, "null argument");
+    return train_filter(ctx, __func__, nullptr, images, bilinear_orientations, h_boxes, num_boxes, h_scales, num_scales, cell_size,
+                        num_bins, variant, filter_w, filter_h, pad_x, pad_y, p, d_filter, h_bias, h_rounds, h_negatives,
+                        h_num_negatives);
 }
 
 int sd_hog_train_filter_float(sd_ctx* ctx, const sd_hog_images* images, int bilinear_orientations, const sd_hog_box* h_boxes,
@@ -893,9 +832,12 @@ int sd_hog_train_filter_float(sd_ctx* ctx, const sd_hog_images* images, int bili
                "null argument");
     SD_REQUIRE(ctx, images->dtype == SD_HOG_F32, "dtype must be SD_HOG_F32: the levels are resized by the float rule");
     SD_REQUIRE(ctx, (reinterpret_cast<uintptr_t>(images->d_data) & 3) == 0, "float frames must be 4-byte aligned");
-    return train_filter_images(ctx, __func__, sd_hog_pyramid_float, images, bilinear_orientations, h_boxes, num_boxes, h_scales,
-                               num_scales, cell_size, num_bins, variant, filter_w, filter_h, pad_x, pad_y, p, d_filter, h_bias,
-                               h_rounds, h_negatives, h_num_negatives);
+    SD_REQUIRE(ctx, images->channels >= 1 && images->channels <= 16, "channels must be in [1,16]");
+    SD_REQUIRE(ctx, bilinear_orientations == 0 || bilinear_orientations == 1, "bilinear_orientations must be 0 or 1");
+    SD_REQUIRE(ctx, images->count < 1 || images->d_data, "null argument");
+    return train_filter(ctx, __func__, nullptr, images, bilinear_orientations, h_boxes, num_boxes, h_scales, num_scales, cell_size,
+                        num_bins, variant, filter_w, filter_h, pad_x, pad_y, p, d_filter, h_bias, h_rounds, h_negatives,
+                        h_num_negatives);
 }
 
 }  // extern "C"

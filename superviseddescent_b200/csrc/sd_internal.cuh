@@ -225,6 +225,23 @@ int sd_check_hog_status(sd_ctx* ctx, const char* what);   // sd_api.cu: synchron
 // the grids of an sd_hog_grids call, validated; per-grid descriptors are read back once into *table (if given) (sd_hog_render.cu)
 int sd_read_hog_grids(sd_ctx* ctx, const char* fn, const sd_hog_grids* grids, int* max_w, int* max_h, std::vector<sd_hog_grid>* table);
 
+// The frames of a HOG pyramid, read once on the host (sd_hog_dense.cu): frame f's element (x, y, c) of type dtype is at data
+// + frames[f].offset + y * row_stride + x * pixel_stride + c * channel_stride.  grey_kernel: the levels go through the
+// 8-bit grey kernel of sd_hog_dense (one 8-bit channel, nearest bins) rather than that of sd_hog_dense_images.
+struct HogPyramidFrames {
+    const void* data;
+    int dtype, channels, bilinear, grey_kernel;
+    std::vector<sd_hog_image> frames;
+};
+// The frames of an 8-bit grey batch (the rules of sd_hog_pyramid) and of an sd_hog_images (those of sd_hog_pyramid_images),
+// the descriptor table read back once; SD_ERR_INVALID names fn and the frame that breaks them.  The callers have checked the
+// other arguments and count >= 1.
+int sd_hog_read_grey_frames(sd_ctx* ctx, const char* fn, const sd_image_batch* images, HogPyramidFrames* out);
+int sd_hog_read_image_frames(sd_ctx* ctx, const char* fn, const sd_hog_images* images, int bilinear_orientations, HogPyramidFrames* out);
+// sd_hog_pyramid of frames [f0, f1) of fr: level s of frame f0 + i at d_out + d_out_offset[i * num_scales + s]
+int sd_hog_pyramid_frames(sd_ctx* ctx, const char* fn, const HogPyramidFrames& fr, int f0, int f1, const double* h_scales,
+                          int num_scales, int cell_size, int num_bins, int variant, float* d_out, const int64_t* d_out_offset);
+
 // The learn path of sd_learn_centred in two steps (sd_linalg.cu), so that a training level can add its rows chunk by chunk
 // (sd_train.cu).  The Gram lives in the context's workspace (D x sd_learn_ldg floats).
 inline int64_t sd_learn_ldg(int D, int M) { return ((int64_t)(D + M) + 3) / 4 * 4; }
