@@ -412,6 +412,23 @@ SD_API int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins,
                             const float* d_filters, int num_filters, int filter_w, int filter_h,
                             const float* d_bias /* num_filters floats or NULL */, int pad_x, int pad_y, float* d_scores);
 
+/* sd_hog_box_scores: a HOG filter's score at each of n boxes, asynchronous on the context's stream (e.g. to re-score another
+ * detector's boxes, or sd_track_faces's end-of-track test).  Box i = d_boxes[4 i .. 4 i + 3] = (x, y, w, h) in pixels of frame
+ * d_box_frame[i] of images (grey 8-bit, as for sd_hog_dense; no d_roi).  With e = (cvRound(w / (double) fw), cvRound(h / (double)
+ * fh)), one cell at the box's scale, its context rectangle (x - ex, y - ey, w + 2 ex, h + 2 ey) -- pixels outside the frame 0, as
+ * copyMakeBorder(BORDER_CONSTANT) -- is resized by cv::resize INTER_LINEAR's 8-bit rule (the pyramid levels' resize) to a crop of
+ * (fw + 2) cs x (fh + 2) cs px.  The crop's sd_hog_dense features ((fw + 2) x (fh + 2) cells, nearest bins) are scored by
+ * sd_hog_correlate with the [dd][fh][fw] filter, the bias and no pad: 3 x 3 scores, one cell of slack on every side.
+ * d_scores[i] is the largest of the 9 (a NaN score is never the largest; 9 NaNs give NaN), bit for bit that maximum.  The call
+ * reads the box and frame index tables (and d_frames, if any) back once.  Null pointers (d_box_frame and d_boxes may be NULL
+ * when n = 0), pointers that are not 4-byte aligned, n < 0, an invalid configuration (cell_size 1..32), filter sides outside
+ * sd_hog_correlate's limits, a crop of 3 px or less per side, a batch with d_roi or a frame smaller than 1 x 1 or with
+ * row_stride < width or a negative offset, a frame index out of range, or a box with w or h < 1 or whose context rectangle (its
+ * corners or its sides) does not fit in int32 is SD_ERR_INVALID before any work is queued (d_scores is not written). */
+SD_API int sd_hog_box_scores(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_box_frame, const int32_t* d_boxes, int n,
+                             const float* d_filter, int filter_w, int filter_h, float bias, int cell_size, int num_bins, int variant,
+                             float* d_scores);
+
 /* ---- detections from HOG filter scores: thresholded boxes in frame pixels and greedy non-maximum suppression ----------------
  * One score map of sd_hog_correlate's output: the [Q][height][width] scores of one pyramid level of one frame. */
 typedef struct {
@@ -1107,6 +1124,37 @@ SD_API int sd_detect_faces_host(sd_ctx* ctx, const sd_model* m, const sd_host_fr
  * in frame i), so a frame with several faces is resident once.  An index out of range is SD_ERR_INVALID. */
 SD_API int sd_detect_faces_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_face_frame,
                                   const float* d_x0, int num_faces, float* d_landmarks);
+
+/* ---- face tracking: one step of rcr-track's loop on the device ---------------------------------------------------------------
+ * sd_track_boxes: the face box of a set of landmarks, the inverse of align_mean at scaling 1 and translation 0.  For row t of
+ * d_landmarks (T x 2L, [x.., y..]): lx0, lx1 = min and max of its x, ly0, ly1 of its y, mx0, mx1, my0, my1 the same of the model's
+ * mean, and in double with every operation rounded on its own
+ *   w = (lx1 - lx0) / (mx1 - mx0),  h = (ly1 - ly0) / (my1 - my0),  bx = lx0 - (mx0 + 0.5) w,  by = ly0 - (my0 + 0.5) h,
+ * d_boxes[4 t ..] = (cvRound(bx), cvRound(by), cvRound(w), cvRound(h)) (ties to even).  d_valid[t] = 0 for a degenerate box: a
+ * value that is not finite or whose rounding does not fit in int32, or a rounded w or h below 1; its box is then (0, 0, 0, 0).
+ * align_mean of a valid box B at scaling 1 has B's enclosing box again, so box(align_mean(m, B)) == B for reasonable boxes.
+ * Asynchronous.  Null pointers or T < 0 is SD_ERR_INVALID. */
+SD_API int sd_track_boxes(sd_ctx* ctx, const sd_model* m, const float* d_landmarks, int T, int32_t* d_boxes, uint8_t* d_valid);
+/* sd_track_faces: one tracking step for T tracks, track t in frame images[d_track_frame[t]] (device frames as for
+ * sd_detect_faces_device, with or without d_frames) with the previous landmarks d_prev[t] (T x 2L).  Per track:
+ *   1. B = sd_track_boxes(prev).  A degenerate B ends the track: d_alive 0, d_landmarks = prev, box and score unspecified.
+ *   2. The cascade runs from align_mean(m, B) (on the device, bit for bit sd_align_mean's), so the landmarks are bit for bit
+ *      sd_detect_faces_device's from the box B.
+ *   3. B' = sd_track_boxes(new landmarks) goes to d_boxes[t] and its sd_hog_box_scores score with the filter to d_scores[t] (NaN
+ *      for a degenerate B' or one whose context rectangle does not fit in int32).  The track lives on (d_alive 1) iff B' is not
+ *      degenerate, score > threshold and no level of its cascade had an empty patch (inter-eye distance too small); such a
+ *      patch ends that track alone, where sd_detect_faces_device refuses the whole call.
+ * Every track is alive on entry; the caller drops dead tracks and starts new ones from sd_hog_detections boxes.  A track's
+ * results depend on its own inputs alone, whatever else shares the call.  Everything runs on the context's stream, with one
+ * status read-back after the cascade (as detect makes): a frame index out of range is SD_ERR_INVALID there, before any output
+ * is written, and the call clears the empty-patch flag it raised itself.  Null pointers, T < 0, a batch with d_roi, or a filter
+ * configuration sd_hog_box_scores refuses is SD_ERR_INVALID before any work is queued.  The frames must be valid as for
+ * sd_detect_faces_device (each at least 1 x 1, row_stride >= width, offset >= 0); like detect, the step does not read d_frames
+ * back to check them. */
+SD_API int sd_track_faces(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_track_frame,
+                          const float* d_prev, int T, const float* d_filter, int filter_w, int filter_h, float bias, int cell_size,
+                          int num_bins, int variant, float threshold, float* d_landmarks, int32_t* d_boxes, float* d_scores,
+                          uint8_t* d_alive);
 
 #ifdef __cplusplus
 }

@@ -193,6 +193,7 @@ EXPORTS = [
     "sd_model_get_mean", "sd_model_get_weights", "sd_model_landmark_id", "sd_align_mean",
     "sd_perturb_box", "sd_normalised_landmark_errors",
     "sd_detect_batch_device", "sd_detect_batch_host", "sd_detect_faces_host", "sd_detect_faces_device",
+    "sd_hog_box_scores", "sd_track_boxes", "sd_track_faces",
 ]
 
 _lib = None
@@ -263,6 +264,10 @@ def lib():
         l.sd_hog_part_scores.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _i, C.c_void_p, C.c_void_p]
         l.sd_hog_part_placements.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, _i, C.c_void_p, C.c_void_p, _i, _i, C.c_void_p,
                                              C.c_void_p, _i, _i, C.c_void_p]
+        _vp = C.c_void_p
+        l.sd_hog_box_scores.argtypes = [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, C.c_float, _i, _i, _i, _vp]
+        l.sd_track_boxes.argtypes = [_vp, _vp, _vp, _i, _vp, _vp]
+        l.sd_track_faces.argtypes = [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, C.c_float, _i, _i, _i, C.c_float, _vp, _vp, _vp, _vp]
         _lib = l
     return _lib
 

@@ -1427,6 +1427,35 @@ class detection_model:
         _check(self.ctx.h, _capi.lib().sd_detect_faces_device(self.ctx.h, self._m, C.byref(ib), ptr(idx), ptr(x0), n, ptr(out)))
         return out
 
+    def track_faces(self, frames, face_frame, previous, face_filter, filter_size, cell_size: int, num_bins: int, threshold: float,
+                    variant: int = 1) -> "TrackedFaces":
+        """One tracking step (sd_track_faces): track t lies in frames[face_frame[t]] and had the landmarks previous[t] ((T, 2L)).
+        Each track restarts the cascade from align_mean of track_boxes(previous), scores the box of its new landmarks with the
+        face filter (hog_box_scores) and stays alive while that box is valid, its score exceeds threshold and no cascade level had
+        an empty patch.  A dead track whose previous box was degenerate keeps its previous landmarks.  frames as hog_dense takes
+        them (a CUDA (count, H, W) uint8 tensor in place, or host frames uploaded with colour converted to grey); face_filter a
+        HogFilter of train_hog_filter (or a (filter, bias) pair) with filter_size = (fw, fh).  There is no tracker state: drop the
+        dead tracks and start new ones from vl_hog_detect boxes.  Returns TrackedFaces of CUDA tensors."""
+        ctx = self.ctx
+        dev = f"cuda:{ctx.device}"
+        keep, ib, _ = _grey_frames(frames, ctx, lambda w, h: None)
+        if ib is None:
+            raise ValueError("track_faces needs at least one frame")
+        P = 2 * self.num_landmarks
+        prev = _dev(previous, ctx).reshape(-1, P).contiguous()
+        T = prev.shape[0]
+        idx = _dev_int32(face_frame, dev).reshape(-1)
+        if idx.numel() != T:
+            raise ValueError("face_frame and previous must have one entry per track")
+        f, fw, fh = _box_filter(face_filter[0], filter_size, num_bins, variant, dev)
+        out = TrackedFaces(torch.empty((T, P), dtype=torch.float32, device=dev), torch.empty((T, 4), dtype=torch.int32, device=dev),
+                           torch.empty(T, dtype=torch.float32, device=dev), torch.empty(T, dtype=torch.uint8, device=dev))
+        _check(ctx.h, _capi.lib().sd_track_faces(ctx.h, self._m, C.byref(ib), ptr(idx), ptr(prev), T, ptr(f), fw, fh,
+                                                 C.c_float(float(face_filter[1])), int(cell_size), int(num_bins), int(variant),
+                                                 C.c_float(float(threshold)), ptr(out.landmarks), ptr(out.boxes), ptr(out.scores),
+                                                 ptr(out.alive)))
+        return out._replace(alive=out.alive.bool())
+
     def save(self, filename: str) -> None:
         _check(self.ctx.h, _capi.lib().sd_model_save(self.ctx.h, self._m, filename.encode()))
 
@@ -1437,6 +1466,66 @@ class detection_model:
                 self._m = None
         except Exception:
             pass
+
+
+TrackedFaces = collections.namedtuple("TrackedFaces", "landmarks boxes scores alive")
+TrackedFaces.__doc__ = """Result of detection_model.track_faces, CUDA tensors: landmarks (T, 2L) float32, boxes (T, 4) int32 (x, y, w, h:
+the track_boxes box of the new landmarks), scores (T,) float32 (its hog_box_scores score, NaN for a degenerate box) and alive (T,)
+bool."""
+
+
+def _dev_int32(a, dev) -> torch.Tensor:
+    return _tensor(np.asarray(a, dtype=np.int32) if not isinstance(a, torch.Tensor) else a).to(dev, torch.int32).contiguous()
+
+
+def _box_filter(filt, filter_size, num_bins: int, variant: int, dev):
+    """A (dd, fh, fw) or (1, dd, fh, fw) float32 filter -> (its contiguous device tensor, fw, fh), checked against filter_size."""
+    f = _tensor(filt).to(dev, torch.float32)
+    if f.dim() == 4 and f.shape[0] == 1:
+        f = f[0]
+    fw, fh = (int(v) for v in filter_size)
+    dd = _hog_dims(num_bins, variant)
+    if tuple(f.shape) != (dd, fh, fw):
+        raise ValueError(f"the filter must be ({dd}, {fh}, {fw}) for filter_size ({fw}, {fh}), got {tuple(f.shape)}")
+    return f.contiguous(), fw, fh
+
+
+def track_boxes(landmarks, model: detection_model):
+    """The face box of each row of landmarks ((T, 2L), [x.., y..]) under the model's mean (sd_track_boxes): the integer box B
+    whose align_mean has the landmarks' enclosing box, the inverse of align_mean at scaling 1 and translation 0.  Returns (boxes
+    (T, 4) int32, valid (T,) bool) CUDA tensors; an invalid (degenerate) row has the box (0, 0, 0, 0)."""
+    ctx = model.ctx
+    x = _dev(landmarks, ctx).reshape(-1, 2 * model.num_landmarks).contiguous()
+    T = x.shape[0]
+    boxes = torch.empty((T, 4), dtype=torch.int32, device=x.device)
+    valid = torch.empty(T, dtype=torch.uint8, device=x.device)
+    _check(ctx.h, _capi.lib().sd_track_boxes(ctx.h, model._m, ptr(x), T, ptr(boxes), ptr(valid)))
+    return boxes, valid.bool()
+
+
+def hog_box_scores(frames, box_frame, boxes, filter, bias: float, cell_size: int, num_bins: int, variant: int = 1,
+                   ctx: Optional[Context] = None) -> torch.Tensor:
+    """A HOG filter's score at each box (sd_hog_box_scores): box i ((x, y, w, h) of frames[box_frame[i]]) with one cell of
+    context on every side, zero outside the frame, resized by cv::resize INTER_LINEAR to (fw + 2) x (fh + 2) cells of cell_size
+    px, its hog_dense features scored by vl_hog_correlate with the filter ((dd, fh, fw)) and bias at every one of the 3 x 3
+    positions; the box's score is the largest (a NaN never is).  frames as hog_dense takes them.  Returns (n,) float32 on the
+    device."""
+    ctx = ctx or default_context()
+    dev = f"cuda:{ctx.device}"
+    keep, ib, _ = _grey_frames(frames, ctx, lambda w, h: None)
+    if ib is None:
+        raise ValueError("hog_box_scores needs at least one frame")
+    f = _tensor(filter)
+    f, fw, fh = _box_filter(f, (f.shape[-1], f.shape[-2]), num_bins, variant, dev)
+    bf = _dev_int32(box_frame, dev).reshape(-1)
+    bx = _dev_int32(boxes, dev).reshape(-1, 4)
+    n = bf.numel()
+    if bx.shape[0] != n:
+        raise ValueError("box_frame and boxes must have one entry per box")
+    out = torch.empty(n, dtype=torch.float32, device=dev)
+    _check(ctx.h, _capi.lib().sd_hog_box_scores(ctx.h, C.byref(ib), ptr(bf), ptr(bx), n, ptr(f), fw, fh, C.c_float(float(bias)),
+                                                int(cell_size), int(num_bins), int(variant), ptr(out)))
+    return out
 
 
 def load_detection_model(filename: str, ctx: Optional[Context] = None) -> detection_model:

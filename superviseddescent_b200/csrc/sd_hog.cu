@@ -61,9 +61,11 @@ struct HogArgs {
 // ---- per-sample geometry: IED -> half patch size (adaptive_vlhog.hpp:123) and the interpolation tables of cv::resize
 //      (INTER_LINEAR, 8U, 11-bit fixed point) for a P x P -> fs x fs resize, once per sample instead of once per thread of
 //      every one of its L patches.  One CTA per sample.  rtab[sample][0..4][fs]: x source index, x weights (2 x int16),
-//      y source index 0 / 1 (clamped), y weights (hog_resize_tap). ------------------------------------------------------
+//      y source index 0 / 1 (clamped), y weights (hog_resize_tap).  face_flag (optional): a degenerate sample also sets its
+//      own byte, so that a caller can drop that face alone (sd_track_faces). ----------------------------------------------
 __global__ void hog_geometry_kernel(const float* __restrict__ x, long long ldx, int N, int L, const sd_eyes_dev eyes, float rel,
-                                    int fixed_half, int fs, int* __restrict__ half_out, int* __restrict__ rtab, int* __restrict__ status)
+                                    int fixed_half, int fs, int* __restrict__ half_out, int* __restrict__ rtab, int* __restrict__ status,
+                                    uint8_t* __restrict__ face_flag)
 {
     const int i = blockIdx.x;
     if (i >= N) return;
@@ -71,7 +73,10 @@ __global__ void hog_geometry_kernel(const float* __restrict__ x, long long ldx, 
     if (threadIdx.x == 0) {
         bool degenerate;
         const int half = sd_patch_half(x + (long long)i * ldx, L, eyes, rel, fixed_half, &degenerate);
-        if (degenerate) atomicOr(status, 1);   // cv::resize would throw on the empty ROI; flag it and keep going
+        if (degenerate) {                      // cv::resize would throw on the empty ROI; flag it and keep going
+            atomicOr(status, 1);
+            if (face_flag) face_flag[i] = 1;
+        }
         half_out[i] = half;
         s_half = half;
     }
@@ -643,7 +648,7 @@ decltype(&hog_patch_kernel<0, 0, 0, kHogThreads, MIR>) pick_hog_kernel(int K, in
 
 int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, bool mirrors, const float* d_x,
                int64_t ldx, int N, int L, const sd_normalisation* eyes, const sd_hog_param* p, float* d_A,
-               int64_t ld, int32_t* d_geometry, uint8_t* d_patches, int8_t* d_bins)
+               int64_t ld, int32_t* d_geometry, uint8_t* d_patches, int8_t* d_bins, uint8_t* d_face_degenerate = nullptr)
 {
     SD_REQUIRE(ctx, images && images->d_data && d_x && p, "null argument");
     SD_REQUIRE(ctx, N >= 0 && L >= 1, "bad sample / landmark count");
@@ -706,7 +711,8 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
     if (!d_half) return SD_ERR_CUDA;
     int* d_rtab = d_half + N;
     float* d_btab = reinterpret_cast<float*>(d_rtab + (size_t)N * 5 * fs);
-    hog_geometry_kernel<<<N, 64, 0, ctx->stream>>>(d_x, ldx, N, L, eyes_dev, p->relative_patch_size, fixed_half, fs, d_half, d_rtab, a.status);
+    hog_geometry_kernel<<<N, 64, 0, ctx->stream>>>(d_x, ldx, N, L, eyes_dev, p->relative_patch_size, fixed_half, fs, d_half, d_rtab, a.status,
+                                                    d_face_degenerate);
     SD_LAUNCH_CHECK(ctx, "hog_geometry_kernel");
     hog_bintab_kernel<<<1, 256, 0, ctx->stream>>>(fs, a.nc, a.cs, lay.pw, d_btab);
     SD_LAUNCH_CHECK(ctx, "hog_bintab_kernel");
@@ -750,12 +756,12 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
 
 int sd_hog_batch_unmirrored(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int64_t ldx,
                             int num_samples, int num_landmarks, const sd_normalisation* eyes, const sd_hog_param* p, float* d_A,
-                            int64_t ld)
+                            int64_t ld, uint8_t* d_face_degenerate)
 {
     if (num_samples == 0) return SD_OK;
     SD_REQUIRE(ctx, d_A, "null output");
     return launch_hog(ctx, images, d_image_index, false, d_x, ldx, num_samples, num_landmarks, eyes, p, d_A, ld, nullptr, nullptr,
-                      nullptr);
+                      nullptr, d_face_degenerate);
 }
 
 namespace {

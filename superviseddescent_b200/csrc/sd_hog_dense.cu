@@ -629,16 +629,20 @@ struct ResizeImagesArgs {
     int count, channels;
     const int64_t* out_offset;   // the caller's, per slot
     int64_t* level_offset;       // per level: the caller's offset of its slot (the dense kernel's out_offset)
+    const int4* rect;            // kRect: per level, the origin (x, y) of its W x H source rectangle and the frame's size (z, w)
 };
 
 // One CTA per kResizeW x kResizeH pixel tile of one level: the taps of its columns and rows once, then cv::resize's two passes
 // for every channel of every pixel with the channel fastest, so that a warp writes consecutive elements of the level, the
 // source read through L1.  A level of the frame's own size is copied.  kC = 1: 8-bit frames of one channel, contiguous pixels
 // (pixel stride 1), frames and levels of fewer than 2^31 bytes, the grey pyramid's: the pixel loop is spared two divisions by
-// a run-time count and takes every offset in 32 bits.  kC = 0: any channel count, strides and sizes.
-template <class T, int kC>
+// a run-time count and takes every offset in 32 bits.  kC = 0: any channel count, strides and sizes.  kRect (8-bit grey only,
+// the box crops of sd_hog_box_scores): the level's W x H source is the rectangle at rect[level].(x, y) of a rect.z x rect.w
+// frame, its pixels outside the frame 0 (copyMakeBorder BORDER_CONSTANT); it writes no level offsets.
+template <class T, int kC, bool kRect = false>
 __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kernel(const __grid_constant__ ResizeImagesArgs a)
 {
+    static_assert(!kRect || (kC == 1 && std::is_same<T, uint8_t>::value), "source rectangles are 8-bit grey");
     constexpr bool f32 = std::is_same<T, float>::value;
     __shared__ int s_sx[kResizeW], s_xw[kResizeW], s_y0[kResizeH], s_y1[kResizeH], s_yw[kResizeH];
     const int b = blockIdx.x, tid = threadIdx.x, C = kC > 0 ? kC : a.channels;
@@ -646,7 +650,7 @@ __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kern
     const PyrImageLevel L = a.levels[lo];
     const int t = b - L.tile0, ty = t / L.tiles_x;
     const int x0 = (t - ty * L.tiles_x) * kResizeW, y0 = ty * kResizeH;
-    if (t == 0 && tid == 0) a.level_offset[lo] = a.out_offset[L.slot];
+    if (!kRect && t == 0 && tid == 0) a.level_offset[lo] = a.out_offset[L.slot];
     const T* __restrict__ src = static_cast<const T*>(a.images) + L.src;
     uint8_t* __restrict__ dst = a.scratch + L.dst;
     const bool copy = L.w == L.W && L.h == L.H;
@@ -675,7 +679,22 @@ __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kern
         const int x = x0 + c, y = y0 + r;
         if (x >= L.w || y >= L.h) continue;
         const T* s = src + ch * L.chs;
-        if constexpr (f32) {
+        if constexpr (kRect) {
+            const int4 R = a.rect[lo];
+            const auto px = [&](int u, int v) -> int {   // pixel (u, v) of the rectangle
+                const long long fx = (long long)R.x + u, fy = (long long)R.y + v;
+                return fx >= 0 && fx < R.z && fy >= 0 && fy < R.w ? (int)__ldg(s + fy * L.rs + fx) : 0;
+            };
+            int v;
+            if (copy) {
+                v = px(x, y);
+            } else {
+                const int sx = s_sx[c], sx1 = min(sx + 1, L.W - 1);
+                const int ax = (short)s_xw[c], bx = s_xw[c] >> 16;
+                v = hog_resize_out(s_yw[r], px(sx, s_y0[r]) * ax + px(sx1, s_y0[r]) * bx, px(sx, s_y1[r]) * ax + px(sx1, s_y1[r]) * bx);
+            }
+            dst[(long long)y * L.pitch + x] = (uint8_t)v;
+        } else if constexpr (f32) {
             float v;
             if (copy) {
                 v = __ldg(s + y * L.rs + x * L.ps);   // a bit copy: no arithmetic touches the value
@@ -703,6 +722,36 @@ __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kern
             dst[(Off)y * L.pitch + x * C + ch] = (uint8_t)v;
         }
     }
+}
+
+// The level of box i of sd_hog_box_crops: its context rectangle of its frame, resized to the crop size; a box whose d_ok byte is
+// 0 takes the 1 x 1 rectangle at (0, 0).  One thread per box.
+__global__ void hog_box_levels_kernel(const sd_image_batch images, const int32_t* __restrict__ box_frame, const int32_t* __restrict__ boxes,
+                                      const uint8_t* __restrict__ ok, int n, int fw, int fh, int cw, int ch, int pitch, int tiles_x,
+                                      int tiles_per_box, PyrImageLevel* __restrict__ levels, int4* __restrict__ rect)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int f = box_frame[i];
+    sd_frame d;
+    if (images.d_frames) {
+        d = images.d_frames[f];
+    } else {
+        d.width = images.width; d.height = images.height; d.row_stride = images.row_stride;
+        d.offset = (int64_t)f * images.image_stride;
+    }
+    int rx = 0, ry = 0, rw = 1, rh = 1;
+    if (!ok || ok[i]) sd_box_context(boxes[4 * i], boxes[4 * i + 1], boxes[4 * i + 2], boxes[4 * i + 3], fw, fh, &rx, &ry, &rw, &rh);
+    PyrImageLevel L{};
+    L.src = d.offset;
+    L.rs = d.row_stride; L.ps = 1; L.chs = 0;
+    L.dst = (long long)i * pitch * ch;
+    L.W = rw; L.H = rh;
+    L.w = cw; L.h = ch; L.pitch = pitch;
+    L.tile0 = i * tiles_per_box; L.tiles_x = tiles_x;
+    L.slot = i;
+    levels[i] = L;
+    rect[i] = make_int4(rx, ry, d.width, d.height);
 }
 
 // The scratch of one slice: [levels (bytes, 16-byte aligned) | level table | the dense kernel's descriptors | per-level
@@ -834,6 +883,33 @@ int pyramid_images(sd_ctx* ctx, const char* fn, const sd_hog_images* images, con
 #undef PYR_REQUIRE
 
 }  // namespace
+
+size_t sd_hog_box_table_bytes(int n) { return sd_round16(sizeof(PyrImageLevel) * (size_t)n) + sizeof(int4) * (size_t)n; }
+
+int sd_hog_box_crops(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_box_frame, const int32_t* d_boxes, const uint8_t* d_ok,
+                     int n, int fw, int fh, int cell_size, uint8_t* d_crops, int pitch, void* d_tables)
+{
+    if (n == 0) return SD_OK;
+    const int cw = (fw + 2) * cell_size, ch = (fh + 2) * cell_size;
+    const int tiles_x = sd_div_up(cw, kResizeW), tiles_per_box = tiles_x * sd_div_up(ch, kResizeH);
+    if ((long long)n * tiles_per_box > INT_MAX) return sd_fail(ctx, SD_ERR_INVALID, "sd_hog_box_scores: too many boxes for one launch");
+    PyrImageLevel* levels = static_cast<PyrImageLevel*>(d_tables);
+    int4* rect = reinterpret_cast<int4*>(static_cast<uint8_t*>(d_tables) + sd_round16(sizeof(PyrImageLevel) * (size_t)n));
+    hog_box_levels_kernel<<<sd_div_up(n, 128), 128, 0, ctx->stream>>>(*images, d_box_frame, d_boxes, d_ok, n, fw, fh, cw, ch, pitch,
+                                                                      tiles_x, tiles_per_box, levels, rect);
+    SD_LAUNCH_CHECK(ctx, "hog_box_levels_kernel");
+    ResizeImagesArgs r;
+    memset(&r, 0, sizeof(r));
+    r.images = images->d_data;
+    r.scratch = d_crops;
+    r.levels = levels;
+    r.count = n;
+    r.channels = 1;
+    r.rect = rect;
+    hog_pyramid_resize_images_kernel<uint8_t, 1, true><<<(unsigned)(n * tiles_per_box), kResizeThreads, 0, ctx->stream>>>(r);
+    SD_LAUNCH_CHECK(ctx, "hog_pyramid_resize_images_kernel");
+    return SD_OK;
+}
 
 int sd_hog_read_grey_frames(sd_ctx* ctx, const char* fn, const sd_image_batch* images, HogPyramidFrames* out)
 {

@@ -7,6 +7,7 @@
 
 #include <cstdarg>
 #include <cstdint>
+#include <cmath>
 #include <cstdio>
 #include <string>
 #include <vector>
@@ -30,6 +31,8 @@ enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_TRAIN_ROWS /* positive rows, negative cache and labels of sd_hog_train_filter (sd_hog_train.cu) */,
        SD_WS_TRAIN_SLICE /* one slice's pyramid, scores, tables and detections of sd_hog_train_filter (sd_hog_train.cu) */,
        SD_WS_PARTS /* cost tables, first tiles and detection map indices of the part-model calls (sd_hog_parts.cu) */,
+       SD_WS_BOXES /* crops, their level tables, features and scores of one slice of sd_hog_box_scores (sd_track.cu) */,
+       SD_WS_TRACK /* initial and new landmarks, patch flags and box flags of sd_track_faces (sd_track.cu) */,
        SD_WS_COUNT };
 
 // Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row
@@ -217,10 +220,44 @@ int syrk_upper(sd_ctx* ctx, const float* d_S, int64_t lds, int K, int MI, int NJ
 bool syrk_is_big(int K, int64_t MI, int64_t NJ);
 
 // sd_hog_batch for callers whose index is not a sample map (detect's face_frame): an SD_SAMPLE_MIRRORED bit there is an index
-// out of range, as it always was (sd_hog.cu)
+// out of range, as it always was (sd_hog.cu).  d_face_degenerate (optional): byte i is set to 1 when sample i's patch is empty,
+// beside the status word's flag; other bytes are not written.
 int sd_hog_batch_unmirrored(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int64_t ldx,
                             int num_samples, int num_landmarks, const sd_normalisation* eyes, const sd_hog_param* p, float* d_A,
-                            int64_t ld);
+                            int64_t ld, uint8_t* d_face_degenerate = nullptr);
+// The detect cascade of sd_detect_faces_device without its status read-back (sd_model.cu): d_face_degenerate as above, for
+// every level.  The model's mean on the device, 2L floats (sd_model.cu).
+int sd_detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_face_frame, const float* d_x0,
+                     int count, float* d_landmarks, uint8_t* d_face_degenerate);
+const float* sd_model_device_mean(const sd_model* m);
+// The crops of sd_hog_box_scores (sd_hog_dense.cu): box i's context rectangle (sd_box_context) of frame d_box_frame[i] resized
+// to (fw + 2) cs x (fh + 2) cs px at d_crops + i * pitch * (fh + 2) cs, rows pitch bytes apart.  d_ok (optional): a box whose
+// byte is 0 crops a 1 x 1 rectangle instead.  d_tables: sd_hog_box_table_bytes(n) bytes of device scratch.
+size_t sd_hog_box_table_bytes(int n);
+int sd_hog_box_crops(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_box_frame, const int32_t* d_boxes, const uint8_t* d_ok,
+                     int n, int fw, int fh, int cell_size, uint8_t* d_crops, int pitch, void* d_tables);
+
+// cvRound: to nearest, ties to even
+__host__ __device__ inline long long sd_cv_round(double v)
+{
+#ifdef __CUDA_ARCH__
+    return __double2ll_rn(v);
+#else
+    return std::llrint(v);
+#endif
+}
+// The context rectangle of box (x, y, w, h) under a filter of fw x fh cells (include/sd_b200.h, sd_hog_box_scores): one cell of
+// the box's scale on every side, e = (cvRound(w / fw), cvRound(h / fh)).  False for w or h < 1 or a rectangle whose corners do
+// not fit in int32 or whose sides do not.
+__host__ __device__ inline bool sd_box_context(int x, int y, int w, int h, int fw, int fh, int* rx, int* ry, int* rw, int* rh)
+{
+    if (w < 1 || h < 1) return false;
+    const long long ex = sd_cv_round((double)w / (double)fw), ey = sd_cv_round((double)h / (double)fh);
+    const long long x0 = (long long)x - ex, y0 = (long long)y - ey, ww = (long long)w + 2 * ex, hh = (long long)h + 2 * ey;
+    if (x0 < INT32_MIN || y0 < INT32_MIN || x0 + ww > INT32_MAX || y0 + hh > INT32_MAX || ww > INT32_MAX || hh > INT32_MAX) return false;
+    *rx = (int)x0; *ry = (int)y0; *rw = (int)ww; *rh = (int)hh;
+    return true;
+}
 int sd_check_hog_status(sd_ctx* ctx, const char* what);   // sd_api.cu: synchronises, reports and clears the projection's flags
 // the grids of an sd_hog_grids call, validated; per-grid descriptors are read back once into *table (if given) (sd_hog_render.cu)
 int sd_read_hog_grids(sd_ctx* ctx, const char* fn, const sd_hog_grids* grids, int* max_w, int* max_h, std::vector<sd_hog_grid>* table);

@@ -27,6 +27,7 @@ struct sd_model {
     std::vector<sd_regulariser> regs;
     std::vector<sd_hog_param> hog;
     std::vector<float> mean;
+    float* d_mean = nullptr;                      // device copy of the mean (sd_track_faces aligns it on the device)
     std::vector<std::string> ids, right_ids, left_ids;
     sd_normalisation norm{};
 };
@@ -135,6 +136,8 @@ int validate_and_upload(sd_ctx* ctx, sd_model* m)
     if (rc) return rc;
     m->device = ctx->device;
     m->d_weights.assign(m->num_levels, nullptr);
+    SD_CUDA(ctx, cudaMalloc(&m->d_mean, m->mean.size() * sizeof(float)));
+    SD_CUDA(ctx, cudaMemcpyAsync(m->d_mean, m->mean.data(), m->mean.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     for (int s = 0; s < m->num_levels; ++s) {
         const size_t bytes = m->weights[s].size() * sizeof(float);
         SD_CUDA(ctx, cudaMalloc(&m->d_weights[s], bytes));
@@ -145,7 +148,7 @@ int validate_and_upload(sd_ctx* ctx, sd_model* m)
 }
 
 int detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x0,
-                  int count, float* d_landmarks)
+                  int count, float* d_landmarks, uint8_t* d_face_degenerate = nullptr)
 {
     const int L = m->num_landmarks, P = 2 * L;
     if (count <= 0) return SD_OK;
@@ -162,7 +165,7 @@ int detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, 
     float* cur = xa;
     float* nxt = xb;
     for (int s = 0; s < m->num_levels; ++s) {               // superviseddescent.hpp:326-342
-        int rc = sd_hog_batch_unmirrored(ctx, images, d_image_index, cur, P, count, L, &m->norm, &m->hog[s], A, ld);
+        int rc = sd_hog_batch_unmirrored(ctx, images, d_image_index, cur, P, count, L, &m->norm, &m->hog[s], A, ld, d_face_degenerate);
         if (rc) return rc;
         rc = sd_cascade_update(ctx, A, ld, count, m->rows[s], m->d_weights[s], P, cur, &m->norm, nxt);
         if (rc) return rc;
@@ -790,6 +793,7 @@ void sd_model_destroy(sd_model* m)
     if (!m) return;
     cudaSetDevice(m->device);
     for (float* p : m->d_weights) if (p) cudaFree(p);
+    if (m->d_mean) cudaFree(m->d_mean);
     delete m;
 }
 
@@ -950,3 +954,11 @@ int sd_upload_frames(sd_ctx* ctx, const sd_host_frame* frames, int count, void* 
 }
 
 }  // extern "C"
+
+int sd_detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_face_frame, const float* d_x0,
+                     int count, float* d_landmarks, uint8_t* d_face_degenerate)
+{
+    return detect_device(ctx, m, images, d_face_frame, d_x0, count, d_landmarks, d_face_degenerate);
+}
+
+const float* sd_model_device_mean(const sd_model* m) { return m->d_mean; }

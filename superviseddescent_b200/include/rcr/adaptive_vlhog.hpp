@@ -819,6 +819,40 @@ inline hog_filter train_hog_filter(const std::vector<cv::Mat>& images, const std
     return out;
 }
 
+// A HOG filter's score at each box (sd_hog_box_scores; the rule is in include/sd_b200.h): box k, boxes[k] in pixels of frame
+// box_frame[k], with one cell of context on every side, zero outside the frame, is resized to (fw + 2) x (fh + 2) cells of
+// cell_size px and scored by the filter (dd * fh x fw CV_32FC1, hog_filter::filter's layout) and bias at each of the 3 x 3
+// positions; the box's score is the largest (a NaN never is).  images: 8UC1 or 8UC3 (B,G,R) frames of any sizes, uploaded as
+// grey.  Throws std::runtime_error where sd_hog_box_scores refuses.
+inline std::vector<float> hog_box_scores(const std::vector<cv::Mat>& images, const std::vector<int>& box_frame, const std::vector<cv::Rect>& boxes,
+                                         const cv::Mat& filter, float bias, VlHogVariant variant, int cell_size, int num_bins)
+{
+    if (images.empty()) throw std::runtime_error("hog_box_scores: no frames");
+    if (box_frame.size() != boxes.size()) throw std::runtime_error("hog_box_scores: box_frame and boxes differ in length");
+    const int dd = sd_b200::hog_dimension(variant, num_bins);
+    if (filter.type() != CV_32FC1 || filter.empty() || filter.rows % dd != 0)
+        throw std::runtime_error("hog_box_scores: the filter must be a CV_32FC1 Mat of dd * fh rows and fw columns");
+    const int n = static_cast<int>(boxes.size());
+    std::vector<float> out(n);
+    if (n == 0) return out;
+    sd_ctx* ctx = sd_b200::context();
+    sd_b200::DeviceBuffer buf, d_filter, d_boxes(static_cast<size_t>(n) * 5 * sizeof(int32_t)), d_scores(static_cast<size_t>(n) * sizeof(float));
+    const sd_image_batch batch = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), buf, "hog_box_scores upload");
+    sd_b200::upload(filter, d_filter, filter.cols);
+    std::vector<int32_t> table(static_cast<size_t>(n) * 5);   // [frame indices | boxes]
+    for (int k = 0; k < n; ++k) {
+        table[k] = box_frame[k];
+        const int32_t b[4] = {boxes[k].x, boxes[k].y, boxes[k].width, boxes[k].height};
+        std::memcpy(&table[n + 4 * k], b, sizeof(b));
+    }
+    sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_boxes.as<int32_t>(), table.data(), table.size() * sizeof(int32_t)), "hog_box_scores");
+    sd_b200::check(ctx, sd_hog_box_scores(ctx, &batch, d_boxes.as<int32_t>(), d_boxes.as<int32_t>() + n, n, d_filter.as<float>(), filter.cols,
+                                          filter.rows / dd, bias, cell_size, num_bins, variant, d_scores.as<float>()), "sd_hog_box_scores");
+    sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.data(), d_scores.as<float>(), out.size() * sizeof(float)), "hog_box_scores");
+    sd_b200::check(ctx, sd_sync(ctx), "hog_box_scores");
+    return out;
+}
+
 // VLFeat HOG of whole frames of one or more channels, 8-bit or float (vl_hog_new(variant, num_bins),
 // vl_hog_set_use_bilinear_orientation_assignments(bilinear_orientations), vl_hog_put_image(frame, channels, cell_size),
 // vl_hog_extract), in one batched call on the device (sd_hog_dense_images).  Each frame is the list of its channel planes --

@@ -108,6 +108,15 @@ private:
     std::vector<std::string> modelLandmarksList, rightEyeIdentifiers, leftEyeIdentifiers;
 };
 
+// One tracking step's result (detection_model::track): per track its new landmarks (1 x 2L), the box of those landmarks, that
+// box's face-filter score (NaN for a degenerate box) and whether the track is still alive.
+struct tracked_faces {
+    std::vector<cv::Mat> landmarks;
+    std::vector<cv::Rect> boxes;
+    std::vector<float> scores;
+    std::vector<bool> alive;
+};
+
 class detection_model {
 public:
     using model_type = superviseddescent::SupervisedDescentOptimiser<superviseddescent::LinearRegressor<superviseddescent::VerbosePartialPivLUSolver>, InterEyeDistanceNormalisation>;
@@ -183,6 +192,53 @@ public:
             throw std::runtime_error("detect: initialisations must be one 1 x 2L row per face");
         const cv::Mat x0 = initialisations.isContinuous() ? initialisations : initialisations.clone();
         return detect_faces(images, face_image, nullptr, x0.ptr<float>(0));
+    }
+
+    // One tracking step (sd_track_faces; the rule is in include/sd_b200.h): track t lies in images[face_frame[t]] and had the
+    // landmarks previous.row(t) (T x 2L, CV_32FC1).  Each track restarts the cascade from align_mean of the box of its previous
+    // landmarks (bit for bit detect() from that box), and its new landmarks' box is scored by the face filter; it stays alive
+    // while that box is valid, its score exceeds threshold and no cascade level had an empty patch.  A track whose previous box
+    // is degenerate dies and keeps its previous landmarks.  images: 8UC1 or 8UC3 (B,G,R) frames of any sizes, uploaded as grey
+    // (hog_batch::upload_grey).  There is no tracker state: drop the dead tracks and start new ones from vl_hog_detect boxes.
+    // Throws std::runtime_error where sd_track_faces refuses.
+    tracked_faces track(const std::vector<cv::Mat>& images, const std::vector<int>& face_frame, cv::Mat previous, const hog_filter& filter,
+                        VlHogVariant variant, int cell_size, int num_bins, float threshold)
+    {
+        const int P = 2 * sd_model_num_landmarks(handle.get()), T = static_cast<int>(face_frame.size());
+        if (images.empty()) throw std::runtime_error("track: no frames");
+        if (previous.rows != T || previous.cols != P || previous.type() != CV_32FC1)
+            throw std::runtime_error("track: previous must be one 1 x 2L CV_32FC1 row per track");
+        const int dd = sd_b200::hog_dimension(variant, num_bins);
+        if (filter.filter.type() != CV_32FC1 || filter.filter.empty() || filter.filter.rows % dd != 0)
+            throw std::runtime_error("track: the filter must be a CV_32FC1 Mat of dd * fh rows and fw columns");
+        tracked_faces out;
+        if (T == 0) return out;
+        sd_ctx* ctx = sd_b200::context();
+        sd_b200::DeviceBuffer buf, d_filter, d_prev, d_frame(static_cast<size_t>(T) * sizeof(int32_t));
+        sd_b200::DeviceBuffer d_lms(static_cast<size_t>(T) * P * sizeof(float)), d_boxes(static_cast<size_t>(T) * 4 * sizeof(int32_t));
+        sd_b200::DeviceBuffer d_scores(static_cast<size_t>(T) * sizeof(float)), d_alive(static_cast<size_t>(T));
+        const sd_image_batch batch = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), buf, "track upload");
+        sd_b200::upload(filter.filter, d_filter, filter.filter.cols);
+        sd_b200::upload(previous, d_prev, P);
+        const std::vector<int32_t> idx(face_frame.begin(), face_frame.end());
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_frame.as<int32_t>(), idx.data(), idx.size() * sizeof(int32_t)), "track");
+        sd_b200::check(ctx, sd_track_faces(ctx, handle.get(), &batch, d_frame.as<int32_t>(), d_prev.as<float>(), T, d_filter.as<float>(),
+                                           filter.filter.cols, filter.filter.rows / dd, filter.bias, cell_size, num_bins, variant, threshold,
+                                           d_lms.as<float>(), d_boxes.as<int32_t>(), d_scores.as<float>(), d_alive.as<uint8_t>()),
+                       "sd_track_faces");
+        std::vector<int32_t> boxes(static_cast<size_t>(T) * 4);
+        std::vector<uint8_t> alive(T);
+        out.scores.resize(T);
+        sd_b200::check(ctx, sd_memcpy_d2h(ctx, boxes.data(), d_boxes.as<int32_t>(), boxes.size() * sizeof(int32_t)), "track");
+        sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.scores.data(), d_scores.as<float>(), out.scores.size() * sizeof(float)), "track");
+        sd_b200::check(ctx, sd_memcpy_d2h(ctx, alive.data(), d_alive.as<uint8_t>(), alive.size()), "track");
+        const cv::Mat lms = sd_b200::download(d_lms.as<float>(), T, P, P);   // synchronises
+        for (int t = 0; t < T; ++t) {
+            out.landmarks.push_back(lms.row(t).clone());
+            out.boxes.push_back(cv::Rect(boxes[4 * t], boxes[4 * t + 1], boxes[4 * t + 2], boxes[4 * t + 3]));
+            out.alive.push_back(alive[t] != 0);
+        }
+        return out;
     }
 
     cv::Mat get_mean()
