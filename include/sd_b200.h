@@ -1156,6 +1156,49 @@ SD_API int sd_track_faces(sd_ctx* ctx, const sd_model* m, const sd_image_batch* 
                           int num_bins, int variant, float threshold, float* d_landmarks, int32_t* d_boxes, float* d_scores,
                           uint8_t* d_alive);
 
+/* The detector's side of sd_track_detect_faces: the pyramid scales, the filter's correlate pad and sd_hog_detections' threshold,
+ * suppression and bounds; track_overlap is the association's and the merge's IoU bound. */
+typedef struct {
+    const double* h_scales;     /* num_scales pyramid scales (host), as sd_hog_pyramid takes them */
+    int32_t num_scales;
+    int32_t pad_x, pad_y;       /* the filter's correlate pad, as sd_hog_correlate takes it */
+    float detect_threshold;     /* sd_hog_detections' threshold */
+    double nms_overlap;         /* sd_hog_detections' overlap */
+    double track_overlap;       /* in [0, 1]; 1 drops and merges nothing */
+    int32_t max_candidates, max_detections;
+} sd_track_detect_param;
+/* sd_track_detect_faces: one tracking step that also runs the sliding-window detector on the frames h_detect_frames lists, starts
+ * a track from every detection no live track covers, and merges tracks that meet on one face.  model, images, the T tracks,
+ * the filter ([dd][filter_h][filter_w] with its bias), cell_size, num_bins, variant and threshold are sd_track_faces's.  Output
+ * rows r < T + num_detect_frames * max_detections: d_landmarks (2L floats), d_boxes (4 int32), d_scores, d_alive, d_frame.
+ * Two boxes (x, y, w, h) overlap when (double)inter > track_overlap * (double)union, inter and union of their pixel rectangles in
+ * int64 (inter 0 when they do not meet).
+ *   1. Old rows t < T: landmarks, box, score and alive3[t] are bit for bit sd_track_faces's for track t; d_frame[t] =
+ *      d_track_frame[t].
+ *   2. Detections: for each listed frame, in list order, the detections sd_hog_detections gives over sd_hog_pyramid (h_scales)
+ *      and sd_hog_correlate (the filter, bias and pad) of that frame alone, with detect_threshold, nms_overlap, max_candidates
+ *      and max_detections: vl_hog_detect's detections of the same frame.
+ *   3. Association: a detection of frame f is dropped iff its box overlaps the box d_boxes[t] of an old row t of frame f with
+ *      alive3[t].
+ *   4. New rows T .. T + n - 1 (*h_num_new = n): the kept detections, frame by frame in list order, in detection order within a
+ *      frame.  Row r starts its cascade from align_mean(m, box) (landmarks bit for bit sd_detect_faces_device's from the box),
+ *      then takes its box, score and alive3 by rule 3 of sd_track_faces (an empty patch ends the row); d_frame[r] = its frame.
+ *   5. Merge: within each frame, the rows with alive3 in the order (old rows before new ones, score descending with -0 == +0,
+ *      row index ascending) are kept greedily: a row is kept unless a kept row before it overlaps it.  d_alive[r] = alive3[r]
+ *      and kept.  track_overlap = 1 merges and drops nothing.
+ * A row depends only on its own frame's inputs (the frame, its tracks, whether it is listed); every result is deterministic.
+ * Read-backs: sd_track_faces's status read-back, the frame table d_frames (only when a frame is listed) and the count n.  Null
+ * pointers, a listed frame out of range or listed twice, an overlap outside [0, 1], a NaN threshold or detect_threshold,
+ * max_candidates outside [1, SD_HOG_DETECT_MAX_CANDIDATES], max_detections outside [1, max_candidates], scales, pads or filter
+ * sides sd_hog_pyramid or sd_hog_correlate refuse, frames whose pyramid levels or boxes sd_hog_pyramid or sd_hog_detections
+ * refuse, more than INT32_MAX rows, and everything sd_track_faces refuses before its work are SD_ERR_INVALID before any work is
+ * queued, with nothing written.  A frame index out of range in d_track_frame is SD_ERR_INVALID as in sd_track_faces. */
+SD_API int sd_track_detect_faces(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_track_frame,
+                                 const float* d_prev, int T, const float* d_filter, int filter_w, int filter_h, float bias,
+                                 int cell_size, int num_bins, int variant, float threshold, const int32_t* h_detect_frames,
+                                 int num_detect_frames, const sd_track_detect_param* param, float* d_landmarks, int32_t* d_boxes,
+                                 float* d_scores, uint8_t* d_alive, int32_t* d_frame, int32_t* h_num_new);
+
 #ifdef __cplusplus
 }
 #endif

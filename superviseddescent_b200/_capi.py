@@ -85,6 +85,13 @@ class HogDetectionC(C.Structure):
                 ("filter", C.c_int32), ("level", C.c_int32), ("cell_x", C.c_int32), ("cell_y", C.c_int32)]
 
 
+class TrackDetectParamC(C.Structure):
+    """sd_track_detect_param: the detector's scales, pad, threshold, suppression and bounds, and the tracks' IoU bound."""
+    _fields_ = [("h_scales", C.c_void_p), ("num_scales", C.c_int32), ("pad_x", C.c_int32), ("pad_y", C.c_int32),
+                ("detect_threshold", C.c_float), ("nms_overlap", C.c_double), ("track_overlap", C.c_double),
+                ("max_candidates", C.c_int32), ("max_detections", C.c_int32)]
+
+
 class HogWindowC(C.Structure):
     """sd_hog_window: score position (x, y) of grid `grid`; flip = 1 reads the window of the mirrored image."""
     _fields_ = [("grid", C.c_int32), ("x", C.c_int32), ("y", C.c_int32), ("flip", C.c_int32)]
@@ -193,7 +200,7 @@ EXPORTS = [
     "sd_model_get_mean", "sd_model_get_weights", "sd_model_landmark_id", "sd_align_mean",
     "sd_perturb_box", "sd_normalised_landmark_errors",
     "sd_detect_batch_device", "sd_detect_batch_host", "sd_detect_faces_host", "sd_detect_faces_device",
-    "sd_hog_box_scores", "sd_track_boxes", "sd_track_faces",
+    "sd_hog_box_scores", "sd_track_boxes", "sd_track_faces", "sd_track_detect_faces",
 ]
 
 _lib = None
@@ -268,6 +275,8 @@ def lib():
         l.sd_hog_box_scores.argtypes = [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, C.c_float, _i, _i, _i, _vp]
         l.sd_track_boxes.argtypes = [_vp, _vp, _vp, _i, _vp, _vp]
         l.sd_track_faces.argtypes = [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, C.c_float, _i, _i, _i, C.c_float, _vp, _vp, _vp, _vp]
+        l.sd_track_detect_faces.argtypes = [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, C.c_float, _i, _i, _i, C.c_float, _vp, _i, _vp,
+                                            _vp, _vp, _vp, _vp, _vp, _vp]
         _lib = l
     return _lib
 

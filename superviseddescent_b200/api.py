@@ -1456,6 +1456,48 @@ class detection_model:
                                                  ptr(out.alive)))
         return out._replace(alive=out.alive.bool())
 
+    def track_and_detect(self, frames, face_frame, previous, face_filter, filter_size, cell_size: int, num_bins: int,
+                         threshold: float, scales, detect_frames, detect_threshold: float, variant: int = 1, pad=(0, 0),
+                         nms_overlap: float = 0.5, track_overlap: float = 0.5, max_candidates: int = 4096,
+                         max_detections: int = 16) -> "TrackStep":
+        """One tracking step that also detects (sd_track_detect_faces).  The T tracks (face_frame, previous) are stepped as
+        track_faces steps them.  On each frame of detect_frames (distinct frame indices, in the order given) the face filter runs
+        as vl_hog_detect runs it (scales, pad, detect_threshold, nms_overlap, max_candidates, max_detections); a detection is
+        dropped when a track of its frame alive after the step overlaps it by IoU > track_overlap, and every other one starts a
+        new row: detect_faces from its box, then scored and ended as a track.  Last, within each frame the alive rows are kept
+        greedily in the order (old rows first, score descending, row index) unless a kept row overlaps them by IoU >
+        track_overlap; track_overlap = 1 neither drops nor merges.  Returns TrackStep of CUDA tensors: rows 0..T-1 are the old
+        tracks, rows T.. the num_new new ones."""
+        ctx = self.ctx
+        dev = f"cuda:{ctx.device}"
+        keep, ib, _ = _grey_frames(frames, ctx, lambda w, h: None)
+        if ib is None:
+            raise ValueError("track_and_detect needs at least one frame")
+        P = 2 * self.num_landmarks
+        prev = _dev(previous, ctx).reshape(-1, P).contiguous()
+        T = prev.shape[0]
+        idx = _dev_int32(face_frame, dev).reshape(-1)
+        if idx.numel() != T:
+            raise ValueError("face_frame and previous must have one entry per track")
+        f, fw, fh = _box_filter(face_filter[0], filter_size, num_bins, variant, dev)
+        listed = np.ascontiguousarray(detect_frames, dtype=np.int32).ravel()
+        sc = np.ascontiguousarray(scales, dtype=np.float64).ravel()
+        pad_x, pad_y = (int(v) for v in pad)
+        param = _capi.TrackDetectParamC(sc.ctypes.data_as(C.c_void_p), sc.size, pad_x, pad_y, float(detect_threshold),
+                                        float(nms_overlap), float(track_overlap), int(max_candidates), int(max_detections))
+        R = T + listed.size * max(int(max_detections), 0)
+        out = TrackStep(torch.empty((R, P), dtype=torch.float32, device=dev), torch.empty((R, 4), dtype=torch.int32, device=dev),
+                        torch.empty(R, dtype=torch.float32, device=dev), torch.empty(R, dtype=torch.uint8, device=dev),
+                        torch.empty(R, dtype=torch.int32, device=dev), 0)
+        n = C.c_int32(0)
+        _check(ctx.h, _capi.lib().sd_track_detect_faces(ctx.h, self._m, C.byref(ib), ptr(idx), ptr(prev), T, ptr(f), fw, fh,
+                                                        C.c_float(float(face_filter[1])), int(cell_size), int(num_bins), int(variant),
+                                                        C.c_float(float(threshold)), _np_ptr(listed), listed.size, C.byref(param),
+                                                        ptr(out.landmarks), ptr(out.boxes), ptr(out.scores), ptr(out.alive),
+                                                        ptr(out.frame), C.byref(n)))
+        r = T + n.value
+        return TrackStep(out.landmarks[:r], out.boxes[:r], out.scores[:r], out.alive[:r].bool(), out.frame[:r], n.value)
+
     def save(self, filename: str) -> None:
         _check(self.ctx.h, _capi.lib().sd_model_save(self.ctx.h, self._m, filename.encode()))
 
@@ -1472,6 +1514,40 @@ TrackedFaces = collections.namedtuple("TrackedFaces", "landmarks boxes scores al
 TrackedFaces.__doc__ = """Result of detection_model.track_faces, CUDA tensors: landmarks (T, 2L) float32, boxes (T, 4) int32 (x, y, w, h:
 the track_boxes box of the new landmarks), scores (T,) float32 (its hog_box_scores score, NaN for a degenerate box) and alive (T,)
 bool."""
+
+TrackStep = collections.namedtuple("TrackStep", "landmarks boxes scores alive frame num_new")
+TrackStep.__doc__ = """Result of detection_model.track_and_detect: rows 0..T-1 are the old tracks, rows T..T+num_new-1 the new ones, as CUDA
+tensors landmarks (R, 2L) float32, boxes (R, 4) int32, scores (R,) float32, alive (R,) bool and frame (R,) int32; num_new an int."""
+
+
+class FaceTracker:
+    """The state of a multi-stream face tracker: the live rows' landmarks, frames and integer ids, and the next id.  Each step
+    is one track_and_detect call; frames holds one frame per stream, and a stream keeps its frame index from step to step.
+    Extra keyword arguments (variant, pad, nms_overlap, track_overlap, max_candidates, max_detections) go to track_and_detect."""
+
+    def __init__(self, model: detection_model, face_filter, filter_size, cell_size: int, num_bins: int, threshold: float, scales,
+                 detect_threshold: float, **options):
+        self.model = model
+        self.args = dict(face_filter=face_filter, filter_size=filter_size, cell_size=cell_size, num_bins=num_bins,
+                         threshold=threshold, scales=scales, detect_threshold=detect_threshold, **options)
+        dev = f"cuda:{model.ctx.device}"
+        self.landmarks = torch.empty((0, 2 * model.num_landmarks), dtype=torch.float32, device=dev)
+        self.frame = torch.empty(0, dtype=torch.int32, device=dev)
+        self.ids = torch.empty(0, dtype=torch.int64, device=dev)
+        self.next_id = 0
+
+    def step(self, frames, detect_frames=None):
+        """Steps every live track on frames and runs the detector on detect_frames (default: the frames without a live track).
+        Old rows keep their ids, new rows take fresh ids in row order, and the rows that are not alive are dropped.  Returns
+        (ids, frame, landmarks, boxes) of the live rows."""
+        if detect_frames is None:
+            live = set(self.frame.tolist())
+            detect_frames = [f for f in range(len(frames)) if f not in live]
+        r = self.model.track_and_detect(frames, self.frame, self.landmarks, detect_frames=detect_frames, **self.args)
+        ids = torch.cat([self.ids, torch.arange(self.next_id, self.next_id + r.num_new, device=self.ids.device)])
+        self.next_id += r.num_new
+        self.ids, self.frame, self.landmarks = ids[r.alive], r.frame[r.alive], r.landmarks[r.alive]
+        return self.ids, self.frame, self.landmarks, r.boxes[r.alive]
 
 
 def _dev_int32(a, dev) -> torch.Tensor:

@@ -360,6 +360,22 @@ int sd_hog_detections(sd_ctx* ctx, const float* d_scores, const sd_hog_score_map
     std::vector<sd_hog_score_map> table;
     if (num_maps > 0)
         if (const int rc = sd_fetch_table(ctx, d_maps, num_maps, table)) return rc;
+    return sd_hog_detections_table(ctx, d_scores, d_maps, table.data(), num_maps, num_frames, num_filters, cell_size, filter_w, filter_h,
+                                   pad_x, pad_y, threshold, overlap, max_candidates, max_detections, d_out, d_count, d_above);
+}
+
+}  // extern "C"
+
+#define DET_REQUIRE(cond, msg)                                                         \
+    do {                                                                               \
+        if (!(cond)) return sd_fail(ctx, SD_ERR_INVALID, "%s: %s", fn, msg);           \
+    } while (0)
+int sd_hog_detections_table(sd_ctx* ctx, const float* d_scores, const sd_hog_score_map* d_maps, const sd_hog_score_map* table,
+                            int num_maps, int num_frames, int num_filters, int cell_size, int filter_w, int filter_h, int pad_x,
+                            int pad_y, float threshold, double overlap, int max_candidates, int max_detections,
+                            sd_hog_detection* d_out, int32_t* d_count, int64_t* d_above)
+{
+    const char* fn = "sd_hog_detections";
     // per map: its first tile and first frame-local rank; the maps grouped by frame
     std::vector<int> ints(3 * (size_t)num_maps + num_frames + 1);
     int* tile0 = ints.data();
@@ -370,20 +386,20 @@ int sd_hog_detections(sd_ctx* ctx, const float* d_scores, const sd_hog_score_map
     long long tiles = 0;
     for (int i = 0; i < num_maps; ++i) {
         const sd_hog_score_map& m = table[i];
-        SD_REQUIRE(ctx, m.frame >= 0 && m.frame < num_frames, "a map's frame is out of range");
-        SD_REQUIRE(ctx, m.offset >= 0, "a map's offset is negative");
-        SD_REQUIRE(ctx, m.frame_w >= 1 && m.frame_h >= 1 && m.level_w >= 1 && m.level_h >= 1, "a map's frame or level is smaller than 1 x 1");
-        SD_REQUIRE(ctx, m.width >= 0 && m.height >= 0, "a map's size is negative");
+        DET_REQUIRE(m.frame >= 0 && m.frame < num_frames, "a map's frame is out of range");
+        DET_REQUIRE(m.offset >= 0, "a map's offset is negative");
+        DET_REQUIRE(m.frame_w >= 1 && m.frame_h >= 1 && m.level_w >= 1 && m.level_h >= 1, "a map's frame or level is smaller than 1 x 1");
+        DET_REQUIRE(m.width >= 0 && m.height >= 0, "a map's size is negative");
         const long long n = (long long)num_filters * m.width * m.height;
         tile0[i] = (int)tiles;
         tiles += (n + kTile - 1) / kTile;
-        SD_REQUIRE(ctx, tiles <= INT_MAX, "too many score tiles");
+        DET_REQUIRE(tiles <= INT_MAX, "too many score tiles");
         rank0[i] = (unsigned)frame_scores[m.frame];
         frame_scores[m.frame] += n;
-        SD_REQUIRE(ctx, frame_scores[m.frame] <= (long long)UINT_MAX, "more than 2^32 - 1 scores in one frame");
-        SD_REQUIRE(ctx, sd_window_boxes_fit_int32(m.width, m.height, pad_x, pad_y, filter_w, filter_h, cell_size, m.frame_w, m.frame_h,
-                                                  m.level_w, m.level_h),
-                   "a map's boxes do not fit in int32");
+        DET_REQUIRE(frame_scores[m.frame] <= (long long)UINT_MAX, "more than 2^32 - 1 scores in one frame");
+        DET_REQUIRE(sd_window_boxes_fit_int32(m.width, m.height, pad_x, pad_y, filter_w, filter_h, cell_size, m.frame_w, m.frame_h,
+                                              m.level_w, m.level_h),
+                    "a map's boxes do not fit in int32");
     }
     {
         std::vector<int> per(num_frames + 1, 0);
@@ -455,5 +471,4 @@ int sd_hog_detections(sd_ctx* ctx, const float* d_scores, const sd_hog_score_map
     SD_LAUNCH_CHECK(ctx, "det_nms_kernel");
     return SD_OK;
 }
-
-}  // extern "C"
+#undef DET_REQUIRE

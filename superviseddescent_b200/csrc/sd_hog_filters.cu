@@ -208,6 +208,17 @@ int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int va
     int max_w = 0, max_h = 0;
     std::vector<sd_hog_grid> table;
     if (const int rc = sd_read_hog_grids(ctx, __func__, maps, &max_w, &max_h, &table)) return rc;
+    return sd_hog_correlate_table(ctx, maps, table.data(), max_w, max_h, num_bins, variant, d_filters, num_filters, filter_w, filter_h,
+                                  d_bias, pad_x, pad_y, d_scores);
+}
+
+}  // extern "C"
+
+int sd_hog_correlate_table(sd_ctx* ctx, const sd_hog_grids* maps, const sd_hog_grid* table, int max_w, int max_h, int num_bins,
+                           int variant, const float* d_filters, int num_filters, int filter_w, int filter_h, const float* d_bias,
+                           int pad_x, int pad_y, float* d_scores)
+{
+    const int count = maps->count;
     const int dd = sd_hog_dd(num_bins, variant);
     const int QF = group_of(num_filters);
 
@@ -233,7 +244,7 @@ int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int va
             tile0[i] = (int)total;
             const int oh = sd_score_extent(table[i].height, pad_y, filter_h), ow = sd_score_extent(table[i].width, pad_x, filter_w);
             if (oh > 0 && ow > 0) total += (long long)sd_div_up(ow, kTileW) * sd_div_up(oh, kTileH);
-            SD_REQUIRE(ctx, total <= INT_MAX, "too many score tiles");
+            if (total > INT_MAX) return sd_fail(ctx, SD_ERR_INVALID, "sd_hog_correlate: too many score tiles");
         }
         if (total == 0) return SD_OK;
         int* d_tile0 = static_cast<int*>(sd_workspace(ctx, SD_WS_FILTERS, sizeof(int) * count));
@@ -249,7 +260,7 @@ int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int va
         a.tiles_x = sd_div_up(ow, kTileW);
         a.tiles = a.tiles_x * sd_div_up(oh, kTileH);
         total = (long long)a.tiles * count;
-        SD_REQUIRE(ctx, total <= INT_MAX, "too many score tiles");
+        if (total > INT_MAX) return sd_fail(ctx, SD_ERR_INVALID, "sd_hog_correlate: too many score tiles");
     }
 
     const CorrKernel kern = corr_kernel(QF);
@@ -258,5 +269,3 @@ int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins, int va
     SD_LAUNCH_CHECK(ctx, "hog_correlate_kernel");
     return SD_OK;
 }
-
-}  // extern "C"

@@ -33,6 +33,8 @@ enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_PARTS /* cost tables, first tiles and detection map indices of the part-model calls (sd_hog_parts.cu) */,
        SD_WS_BOXES /* crops, their level tables, features and scores of one slice of sd_hog_box_scores (sd_track.cu) */,
        SD_WS_TRACK /* initial and new landmarks, patch flags and box flags of sd_track_faces (sd_track.cu) */,
+       SD_WS_TRACK_DETECT /* one slice's pyramid, scores and tables, the detections, the frame groups and the new rows of
+                             sd_track_detect_faces (sd_track.cu) */,
        SD_WS_COUNT };
 
 // Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row
@@ -275,6 +277,16 @@ struct HogPyramidFrames {
 // other arguments and count >= 1.
 int sd_hog_read_grey_frames(sd_ctx* ctx, const char* fn, const sd_image_batch* images, HogPyramidFrames* out);
 int sd_hog_read_image_frames(sd_ctx* ctx, const char* fn, const sd_hog_images* images, int bilinear_orientations, HogPyramidFrames* out);
+// sd_hog_correlate and sd_hog_detections past their argument checks, with the descriptor table the caller built on the host
+// (table: maps->count grids, the largest max_w x max_h cells; num_maps score maps) instead of one read back from the device.
+// The results are those of the entry points for the same tables.
+int sd_hog_correlate_table(sd_ctx* ctx, const sd_hog_grids* maps, const sd_hog_grid* table, int max_w, int max_h, int num_bins,
+                           int variant, const float* d_filters, int num_filters, int filter_w, int filter_h, const float* d_bias,
+                           int pad_x, int pad_y, float* d_scores);
+int sd_hog_detections_table(sd_ctx* ctx, const float* d_scores, const sd_hog_score_map* d_maps, const sd_hog_score_map* table,
+                            int num_maps, int num_frames, int num_filters, int cell_size, int filter_w, int filter_h, int pad_x,
+                            int pad_y, float threshold, double overlap, int max_candidates, int max_detections,
+                            sd_hog_detection* d_out, int32_t* d_count, int64_t* d_above);
 // sd_hog_pyramid of frames [f0, f1) of fr: level s of frame f0 + i at d_out + d_out_offset[i * num_scales + s]
 int sd_hog_pyramid_frames(sd_ctx* ctx, const char* fn, const HogPyramidFrames& fr, int f0, int f1, const double* h_scales,
                           int num_scales, int cell_size, int num_bins, int variant, float* d_out, const int64_t* d_out_offset);

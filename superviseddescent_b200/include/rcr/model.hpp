@@ -117,6 +117,21 @@ struct tracked_faces {
     std::vector<bool> alive;
 };
 
+// The detector's side of detection_model::track_and_detect: sd_track_detect_param without its scales.
+struct track_detect_params {
+    int pad_x = 0, pad_y = 0;
+    float detect_threshold = 0.f;
+    double nms_overlap = 0.5, track_overlap = 0.5;
+    int max_candidates = 4096, max_detections = 16;
+};
+
+// One step of detection_model::track_and_detect: rows 0..T-1 are the old tracks, rows T.. the num_new new ones; frame[r] is the
+// frame row r lies in.
+struct track_step : tracked_faces {
+    std::vector<int> frame;
+    int num_new = 0;
+};
+
 class detection_model {
 public:
     using model_type = superviseddescent::SupervisedDescentOptimiser<superviseddescent::LinearRegressor<superviseddescent::VerbosePartialPivLUSolver>, InterEyeDistanceNormalisation>;
@@ -237,6 +252,69 @@ public:
             out.landmarks.push_back(lms.row(t).clone());
             out.boxes.push_back(cv::Rect(boxes[4 * t], boxes[4 * t + 1], boxes[4 * t + 2], boxes[4 * t + 3]));
             out.alive.push_back(alive[t] != 0);
+        }
+        return out;
+    }
+
+    // One tracking step that also detects (sd_track_detect_faces; the rule is in include/sd_b200.h): the tracks step as in
+    // track(), the face filter runs as vl_hog_detect on the frames detect_frames lists (distinct indices; the pyramid's scales),
+    // a detection that no alive track of its frame overlaps by IoU > params.track_overlap starts a new row from its box, and
+    // within each frame the alive rows are kept greedily (old rows first, then by score) unless a kept row overlaps them.  The
+    // frames are uploaded once (hog_batch::upload_grey).  previous may be empty when face_frame is.  Throws std::runtime_error
+    // where sd_track_detect_faces refuses.
+    track_step track_and_detect(const std::vector<cv::Mat>& images, const std::vector<int>& face_frame, cv::Mat previous,
+                                const hog_filter& filter, VlHogVariant variant, int cell_size, int num_bins, float threshold,
+                                const std::vector<double>& scales, const std::vector<int>& detect_frames, const track_detect_params& params)
+    {
+        const int P = 2 * sd_model_num_landmarks(handle.get()), T = static_cast<int>(face_frame.size());
+        if (images.empty()) throw std::runtime_error("track_and_detect: no frames");
+        if (T > 0 && (previous.rows != T || previous.cols != P || previous.type() != CV_32FC1))
+            throw std::runtime_error("track_and_detect: previous must be one 1 x 2L CV_32FC1 row per track");
+        const int dd = sd_b200::hog_dimension(variant, num_bins);
+        if (filter.filter.type() != CV_32FC1 || filter.filter.empty() || filter.filter.rows % dd != 0)
+            throw std::runtime_error("track_and_detect: the filter must be a CV_32FC1 Mat of dd * fh rows and fw columns");
+        if (params.max_detections < 1) throw std::runtime_error("track_and_detect: max_detections must be at least 1");
+        const size_t R = static_cast<size_t>(T) + detect_frames.size() * static_cast<size_t>(params.max_detections);
+        sd_ctx* ctx = sd_b200::context();
+        sd_b200::DeviceBuffer buf, d_filter, d_prev, d_face(static_cast<size_t>(T) * sizeof(int32_t) + 4);
+        sd_b200::DeviceBuffer d_lms(R * P * sizeof(float) + 4), d_boxes(R * 4 * sizeof(int32_t) + 4), d_scores(R * sizeof(float) + 4);
+        sd_b200::DeviceBuffer d_alive(R + 4), d_frame(R * sizeof(int32_t) + 4);
+        const sd_image_batch batch = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), buf, "track_and_detect upload");
+        sd_b200::upload(filter.filter, d_filter, filter.filter.cols);
+        if (T > 0) sd_b200::upload(previous, d_prev, P);
+        const std::vector<int32_t> idx(face_frame.begin(), face_frame.end()), listed(detect_frames.begin(), detect_frames.end());
+        if (T > 0) sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_face.as<int32_t>(), idx.data(), idx.size() * sizeof(int32_t)), "track_and_detect");
+        sd_track_detect_param p;
+        p.h_scales = scales.data();
+        p.num_scales = static_cast<int32_t>(scales.size());
+        p.pad_x = params.pad_x; p.pad_y = params.pad_y;
+        p.detect_threshold = params.detect_threshold;
+        p.nms_overlap = params.nms_overlap; p.track_overlap = params.track_overlap;
+        p.max_candidates = params.max_candidates; p.max_detections = params.max_detections;
+        int32_t num_new = 0;
+        sd_b200::check(ctx, sd_track_detect_faces(ctx, handle.get(), &batch, d_face.as<int32_t>(), d_prev.as<float>(), T, d_filter.as<float>(),
+                                                  filter.filter.cols, filter.filter.rows / dd, filter.bias, cell_size, num_bins, variant,
+                                                  threshold, listed.data(), static_cast<int>(listed.size()), &p, d_lms.as<float>(),
+                                                  d_boxes.as<int32_t>(), d_scores.as<float>(), d_alive.as<uint8_t>(), d_frame.as<int32_t>(),
+                                                  &num_new),
+                       "sd_track_detect_faces");
+        const int rows = T + num_new;
+        track_step out;
+        out.num_new = num_new;
+        if (rows == 0) return out;
+        std::vector<int32_t> boxes(static_cast<size_t>(rows) * 4), frame(rows);
+        std::vector<uint8_t> alive(rows);
+        out.scores.resize(rows);
+        sd_b200::check(ctx, sd_memcpy_d2h(ctx, boxes.data(), d_boxes.as<int32_t>(), boxes.size() * sizeof(int32_t)), "track_and_detect");
+        sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.scores.data(), d_scores.as<float>(), out.scores.size() * sizeof(float)), "track_and_detect");
+        sd_b200::check(ctx, sd_memcpy_d2h(ctx, alive.data(), d_alive.as<uint8_t>(), alive.size()), "track_and_detect");
+        sd_b200::check(ctx, sd_memcpy_d2h(ctx, frame.data(), d_frame.as<int32_t>(), frame.size() * sizeof(int32_t)), "track_and_detect");
+        const cv::Mat lms = sd_b200::download(d_lms.as<float>(), rows, P, P);   // synchronises
+        for (int r = 0; r < rows; ++r) {
+            out.landmarks.push_back(lms.row(r).clone());
+            out.boxes.push_back(cv::Rect(boxes[4 * r], boxes[4 * r + 1], boxes[4 * r + 2], boxes[4 * r + 3]));
+            out.alive.push_back(alive[r] != 0);
+            out.frame.push_back(frame[r]);
         }
         return out;
     }
