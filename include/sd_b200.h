@@ -323,6 +323,17 @@ SD_API int sd_hog_pyramid_images(sd_ctx* ctx, const sd_hog_images* images, const
 SD_API int sd_hog_pyramid_float(sd_ctx* ctx, const sd_hog_images* images, const double* h_scales, int num_scales,
                                 int cell_size, int num_bins, int variant, int bilinear_orientations,
                                 float* d_out, const int64_t* d_out_offset);
+/* Device colour frames -> one grey batch, so that a colour video is uploaded once for both the cascade (grey) and a colour filter
+ * (sd_track_faces_images).  bgr: an sd_hog_images batch of SD_HOG_U8 frames with 3 channels B, G, R, in any layout
+ * it describes and of any sizes.  The grey frames are laid out as sd_upload_frames lays them out (16-byte pitch, followed by the
+ * sd_frame table when the sizes differ), with the same size query (d_buf == NULL: *bytes receives the size, nothing else
+ * happens), and their pixels are bit for bit sd_upload_frames' of the same frames (sd_bgr2gray's fixed point).  That size is
+ * the sum over frames of height * roundup16(width) bytes, plus count * sizeof(sd_frame) when the sizes differ: a caller that
+ * knows its frames' sizes can compute it and skip the query, which has to read d_frames back.  The frame table of bgr (if any)
+ * is read back once per call.  Asynchronous on the context's stream once that read-back is done.  Null pointers, count < 1,
+ * a dtype other than SD_HOG_U8, channels other than 3, a frame smaller than 1 x 1 or with a negative offset or stride, an
+ * unaligned d_buf or a *bytes below the size query's are SD_ERR_INVALID before any work is queued (d_buf is not written). */
+SD_API int sd_bgr2gray_images(sd_ctx* ctx, const sd_hog_images* bgr, void* d_buf, size_t* bytes, sd_image_batch* out);
 
 /* ---- dense HOG of a caller's gradient fields: vl_hog_put_polar_field + vl_hog_extract (hog.c:746-845, :857-1062) ----------
  * Each field is a modulus and an angle per pixel, e.g. the gradient of another operator, colour gradients combined by the
@@ -425,6 +436,19 @@ SD_API int sd_hog_correlate(sd_ctx* ctx, const sd_hog_grids* maps, int num_bins,
  * sd_hog_correlate's limits, a crop of 3 px or less per side, a batch with d_roi or a frame smaller than 1 x 1 or with
  * row_stride < width or a negative offset, a frame index out of range, or a box with w or h < 1 or whose context rectangle (its
  * corners or its sides) does not fit in int32 is SD_ERR_INVALID before any work is queued (d_scores is not written). */
+/* sd_hog_box_scores_images: sd_hog_box_scores on frames that keep their channels, for filters trained on them
+ * (sd_hog_train_filter_images / _float).  Frames are an sd_hog_images batch in any layout it describes (1..16 channels, planar,
+ * interleaved or strided, equally sized or per-frame d_frames).  The context rectangle is sd_hog_box_scores'; each channel is cut
+ * from it (pixels outside the frame 0) and resized on its own to (fw + 2) cs x (fh + 2) cs px: SD_HOG_U8 frames by
+ * sd_hog_pyramid_images' 8-bit rule, SD_HOG_F32 frames by sd_hog_pyramid_float's float rule (a bit copy when the rectangle has the
+ * crop's size; a tap of weight 0 is read and multiplied, a pixel outside the frame being a tap holding +0.0f).  The crop's
+ * features are sd_hog_dense_images' with bilinear_orientations, scored and maximised as in sd_hog_box_scores.  One 8-bit channel
+ * with nearest bins gives sd_hog_box_scores' scores bit for bit.  Refusals are sd_hog_box_scores', plus those of
+ * sd_hog_pyramid_images / _float: a dtype other than SD_HOG_U8 or SD_HOG_F32, channels outside [1, 16], bilinear_orientations
+ * outside {0, 1}, an unaligned float buffer, a negative offset or stride; all before any work is queued, with nothing written. */
+SD_API int sd_hog_box_scores_images(sd_ctx* ctx, const sd_hog_images* images, int bilinear_orientations, const int32_t* d_box_frame,
+                                    const int32_t* d_boxes, int n, const float* d_filter, int filter_w, int filter_h, float bias,
+                                    int cell_size, int num_bins, int variant, float* d_scores);
 SD_API int sd_hog_box_scores(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_box_frame, const int32_t* d_boxes, int n,
                              const float* d_filter, int filter_w, int filter_h, float bias, int cell_size, int num_bins, int variant,
                              float* d_scores);
@@ -1198,6 +1222,30 @@ SD_API int sd_track_detect_faces(sd_ctx* ctx, const sd_model* m, const sd_image_
                                  int cell_size, int num_bins, int variant, float threshold, const int32_t* h_detect_frames,
                                  int num_detect_frames, const sd_track_detect_param* param, float* d_landmarks, int32_t* d_boxes,
                                  float* d_scores, uint8_t* d_alive, int32_t* d_frame, int32_t* h_num_new);
+
+/* The tracking steps on colour or float video: sd_track_faces and sd_track_detect_faces with the filter's frames kept as the filter
+ * was trained on them.  filter_images (an sd_hog_images batch as sd_hog_box_scores_images takes it) and bilinear_orientations
+ * follow images; every other argument and output is the grey step's.
+ *   - The cascade reads the grey batch images exactly as the grey step does, so the landmarks are bit for bit its.
+ *   - The keep-alive score of a box is sd_hog_box_scores_images' on filter_images.
+ *   - The detector (sd_track_detect_faces_images) runs sd_hog_pyramid_images (SD_HOG_U8) or sd_hog_pyramid_float (SD_HOG_F32) of
+ *     each listed frame of filter_images, then sd_hog_correlate and sd_hog_detections as the grey step does.
+ *   - Association, new rows and merge are the grey step's.
+ * Frame f of filter_images must have the width and height of frame f of images, and both batches the same count: boxes are in that
+ * shared pixel grid.  The call checks this on the host before any work, reading each frame table back once (the detector reuses
+ * filter_images' table), and refuses a mismatch with SD_ERR_INVALID.  Refusals are otherwise the grey step's plus
+ * sd_hog_box_scores_images'.  With filter_images the grey frames as one 8-bit channel and nearest bins, the results are the grey
+ * step's bit for bit. */
+SD_API int sd_track_faces_images(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const sd_hog_images* filter_images,
+                                 int bilinear_orientations, const int32_t* d_track_frame, const float* d_prev, int T,
+                                 const float* d_filter, int filter_w, int filter_h, float bias, int cell_size, int num_bins, int variant,
+                                 float threshold, float* d_landmarks, int32_t* d_boxes, float* d_scores, uint8_t* d_alive);
+SD_API int sd_track_detect_faces_images(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images,
+                                        const sd_hog_images* filter_images, int bilinear_orientations, const int32_t* d_track_frame,
+                                        const float* d_prev, int T, const float* d_filter, int filter_w, int filter_h, float bias,
+                                        int cell_size, int num_bins, int variant, float threshold, const int32_t* h_detect_frames,
+                                        int num_detect_frames, const sd_track_detect_param* param, float* d_landmarks,
+                                        int32_t* d_boxes, float* d_scores, uint8_t* d_alive, int32_t* d_frame, int32_t* h_num_new);
 
 #ifdef __cplusplus
 }

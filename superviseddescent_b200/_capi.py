@@ -201,6 +201,7 @@ EXPORTS = [
     "sd_perturb_box", "sd_normalised_landmark_errors",
     "sd_detect_batch_device", "sd_detect_batch_host", "sd_detect_faces_host", "sd_detect_faces_device",
     "sd_hog_box_scores", "sd_track_boxes", "sd_track_faces", "sd_track_detect_faces",
+    "sd_hog_box_scores_images", "sd_track_faces_images", "sd_track_detect_faces_images", "sd_bgr2gray_images",
 ]
 
 _lib = None
@@ -277,6 +278,10 @@ def lib():
         l.sd_track_faces.argtypes = [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, C.c_float, _i, _i, _i, C.c_float, _vp, _vp, _vp, _vp]
         l.sd_track_detect_faces.argtypes = [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, C.c_float, _i, _i, _i, C.c_float, _vp, _i, _vp,
                                             _vp, _vp, _vp, _vp, _vp, _vp]
+        l.sd_hog_box_scores_images.argtypes = [_vp, _vp, _i, _vp, _vp, _i, _vp, _i, _i, C.c_float, _i, _i, _i, _vp]
+        l.sd_track_faces_images.argtypes = l.sd_track_faces.argtypes[:3] + [_vp, _i] + l.sd_track_faces.argtypes[3:]
+        l.sd_track_detect_faces_images.argtypes = l.sd_track_detect_faces.argtypes[:3] + [_vp, _i] + l.sd_track_detect_faces.argtypes[3:]
+        l.sd_bgr2gray_images.argtypes = [_vp, _vp, _vp, _vp, _vp]
         _lib = l
     return _lib
 

@@ -26,7 +26,7 @@ import torch
 
 from . import _capi
 from ._capi import HogParam as HoGParam  # same field names as rcr::HoGParam
-from ._capi import HogBoxC, HogDetectionC, HogGridC, HogGridsC, HogImageC, HogImagesC, HogPartMapC, HogPartModelC, HogPartPlacementC, HogPolarFieldsC, HogScoreMapC, HogTrainParamC, HogTrainReportC, HogWindowC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, SvmReportC, ptr
+from ._capi import FrameC, HogBoxC, HogDetectionC, HogGridC, HogGridsC, HogImageC, HogImagesC, HogPartMapC, HogPartModelC, HogPartPlacementC, HogPolarFieldsC, HogScoreMapC, HogTrainParamC, HogTrainReportC, HogWindowC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, SvmReportC, ptr
 
 
 def _check(ctx, rc: int) -> None:
@@ -527,12 +527,12 @@ def vl_hog(images, cell_size: int, num_bins: int, variant: int = 1, bilinear_ori
                                                                                      int(variant), bil, ptr(out), ptr(offsets))))
 
 
-def _hog_images(images, channels_last: bool, ctx: Context, check, float_only: bool = False):
+def _hog_images(images, channels_last: bool, ctx: Context, check, float_only: bool = False, frames_out=None):
     """The frames of vl_hog, or of the multichannel=True route of the sliding-window calls -> (what owns their device bytes,
     their HogImagesC, [(H, W)] per frame).  A batch is read through its strides (a CUDA tensor in place, a host one after one
     copy); a list of frames is packed end to end in one device buffer after check(W, H) has accepted every size, with a
     descriptor table when the sizes differ.  An empty list gives (None, None, []).  float_only: frames of another dtype than
-    float32 are refused before any upload."""
+    float32 are refused before any upload.  frames_out (a list): receives each frame's HogImageC, offsets from the data."""
     dev = f"cuda:{ctx.device}"
 
     def dtype_of(t):
@@ -563,6 +563,8 @@ def _hog_images(images, channels_last: bool, ctx: Context, check, float_only: bo
         data, offsets = _pack(frames, dev)
         for (_, d), o in zip(descs, offsets):
             d.offset = o
+        if frames_out is not None:
+            frames_out.extend(d for _, d in descs)
         ib.channels, ib.count = descs[0][0], len(frames)
         keep = data
         if len(set(sizes)) == 1:
@@ -580,6 +582,10 @@ def _hog_images(images, channels_last: bool, ctx: Context, check, float_only: bo
         ib.channels, ib.frame = _vl_hog_frame(data, channels_last, True)
         ib.count, ib.image_stride = data.shape[0], data.stride(0)
         sizes = [(ib.frame.height, ib.frame.width)] * ib.count
+        if frames_out is not None:
+            f = ib.frame
+            frames_out.extend(HogImageC(f.width, f.height, f.offset + i * ib.image_stride, f.row_stride, f.pixel_stride, f.channel_stride)
+                              for i in range(ib.count))
     ib.d_data, ib.dtype = data.data_ptr(), dt
     return keep, ib, sizes
 
@@ -1428,19 +1434,23 @@ class detection_model:
         return out
 
     def track_faces(self, frames, face_frame, previous, face_filter, filter_size, cell_size: int, num_bins: int, threshold: float,
-                    variant: int = 1) -> "TrackedFaces":
+                    variant: int = 1, multichannel: bool = False, bilinear_orientations: bool = False, float_frames: bool = False,
+                    grey_frames=None) -> "TrackedFaces":
         """One tracking step (sd_track_faces): track t lies in frames[face_frame[t]] and had the landmarks previous[t] ((T, 2L)).
         Each track restarts the cascade from align_mean of track_boxes(previous), scores the box of its new landmarks with the
         face filter (hog_box_scores) and stays alive while that box is valid, its score exceeds threshold and no cascade level had
         an empty patch.  A dead track whose previous box was degenerate keeps its previous landmarks.  frames as hog_dense takes
         them (a CUDA (count, H, W) uint8 tensor in place, or host frames uploaded with colour converted to grey); face_filter a
         HogFilter of train_hog_filter (or a (filter, bias) pair) with filter_size = (fw, fh).  There is no tracker state: drop the
-        dead tracks and start new ones from vl_hog_detect boxes.  Returns TrackedFaces of CUDA tensors."""
+        dead tracks and start new ones from vl_hog_detect boxes.  Returns TrackedFaces of CUDA tensors.
+
+        multichannel, bilinear_orientations and float_frames as vl_hog_detect takes them: a filter trained on colour or float
+        frames (train_hog_filter with the same values) scores the boxes on the frames as given (sd_track_faces_images), while the
+        cascade reads grey frames: those of 8-bit B, G, R frames converted on the device after one upload, 8-bit grey frames as
+        they are, and for float frames or other channel counts grey_frames (frames as detect_faces takes them, of the same sizes)."""
         ctx = self.ctx
         dev = f"cuda:{ctx.device}"
-        keep, ib, _ = _grey_frames(frames, ctx, lambda w, h: None)
-        if ib is None:
-            raise ValueError("track_faces needs at least one frame")
+        keep, ib, hi = _track_frames(frames, ctx, multichannel, bilinear_orientations, float_frames, grey_frames, "track_faces")
         P = 2 * self.num_landmarks
         prev = _dev(previous, ctx).reshape(-1, P).contiguous()
         T = prev.shape[0]
@@ -1450,16 +1460,19 @@ class detection_model:
         f, fw, fh = _box_filter(face_filter[0], filter_size, num_bins, variant, dev)
         out = TrackedFaces(torch.empty((T, P), dtype=torch.float32, device=dev), torch.empty((T, 4), dtype=torch.int32, device=dev),
                            torch.empty(T, dtype=torch.float32, device=dev), torch.empty(T, dtype=torch.uint8, device=dev))
-        _check(ctx.h, _capi.lib().sd_track_faces(ctx.h, self._m, C.byref(ib), ptr(idx), ptr(prev), T, ptr(f), fw, fh,
-                                                 C.c_float(float(face_filter[1])), int(cell_size), int(num_bins), int(variant),
-                                                 C.c_float(float(threshold)), ptr(out.landmarks), ptr(out.boxes), ptr(out.scores),
-                                                 ptr(out.alive)))
+        lib = _capi.lib()
+        call, frames_args = ((lib.sd_track_faces, [C.byref(ib)]) if hi is None else
+                             (lib.sd_track_faces_images, [C.byref(ib), C.byref(hi), int(bool(bilinear_orientations))]))
+        _check(ctx.h, call(ctx.h, self._m, *frames_args, ptr(idx), ptr(prev), T, ptr(f), fw, fh, C.c_float(float(face_filter[1])),
+                           int(cell_size), int(num_bins), int(variant), C.c_float(float(threshold)), ptr(out.landmarks), ptr(out.boxes),
+                           ptr(out.scores), ptr(out.alive)))
         return out._replace(alive=out.alive.bool())
 
     def track_and_detect(self, frames, face_frame, previous, face_filter, filter_size, cell_size: int, num_bins: int,
                          threshold: float, scales, detect_frames, detect_threshold: float, variant: int = 1, pad=(0, 0),
                          nms_overlap: float = 0.5, track_overlap: float = 0.5, max_candidates: int = 4096,
-                         max_detections: int = 16) -> "TrackStep":
+                         max_detections: int = 16, multichannel: bool = False, bilinear_orientations: bool = False,
+                         float_frames: bool = False, grey_frames=None) -> "TrackStep":
         """One tracking step that also detects (sd_track_detect_faces).  The T tracks (face_frame, previous) are stepped as
         track_faces steps them.  On each frame of detect_frames (distinct frame indices, in the order given) the face filter runs
         as vl_hog_detect runs it (scales, pad, detect_threshold, nms_overlap, max_candidates, max_detections); a detection is
@@ -1467,12 +1480,12 @@ class detection_model:
         new row: detect_faces from its box, then scored and ended as a track.  Last, within each frame the alive rows are kept
         greedily in the order (old rows first, score descending, row index) unless a kept row overlaps them by IoU >
         track_overlap; track_overlap = 1 neither drops nor merges.  Returns TrackStep of CUDA tensors: rows 0..T-1 are the old
-        tracks, rows T.. the num_new new ones."""
+        tracks, rows T.. the num_new new ones.  multichannel, bilinear_orientations, float_frames and grey_frames as track_faces
+        takes them: with multichannel the box scores and the detector (vl_hog_detect(multichannel=True, ...)) read the frames as
+        given, the cascade their grey (sd_track_detect_faces_images)."""
         ctx = self.ctx
         dev = f"cuda:{ctx.device}"
-        keep, ib, _ = _grey_frames(frames, ctx, lambda w, h: None)
-        if ib is None:
-            raise ValueError("track_and_detect needs at least one frame")
+        keep, ib, hi = _track_frames(frames, ctx, multichannel, bilinear_orientations, float_frames, grey_frames, "track_and_detect")
         P = 2 * self.num_landmarks
         prev = _dev(previous, ctx).reshape(-1, P).contiguous()
         T = prev.shape[0]
@@ -1490,11 +1503,13 @@ class detection_model:
                         torch.empty(R, dtype=torch.float32, device=dev), torch.empty(R, dtype=torch.uint8, device=dev),
                         torch.empty(R, dtype=torch.int32, device=dev), 0)
         n = C.c_int32(0)
-        _check(ctx.h, _capi.lib().sd_track_detect_faces(ctx.h, self._m, C.byref(ib), ptr(idx), ptr(prev), T, ptr(f), fw, fh,
-                                                        C.c_float(float(face_filter[1])), int(cell_size), int(num_bins), int(variant),
-                                                        C.c_float(float(threshold)), _np_ptr(listed), listed.size, C.byref(param),
-                                                        ptr(out.landmarks), ptr(out.boxes), ptr(out.scores), ptr(out.alive),
-                                                        ptr(out.frame), C.byref(n)))
+        lib = _capi.lib()
+        call, frames_args = ((lib.sd_track_detect_faces, [C.byref(ib)]) if hi is None else
+                             (lib.sd_track_detect_faces_images, [C.byref(ib), C.byref(hi), int(bool(bilinear_orientations))]))
+        _check(ctx.h, call(ctx.h, self._m, *frames_args, ptr(idx), ptr(prev), T, ptr(f), fw, fh, C.c_float(float(face_filter[1])),
+                           int(cell_size), int(num_bins), int(variant), C.c_float(float(threshold)), _np_ptr(listed), listed.size,
+                           C.byref(param), ptr(out.landmarks), ptr(out.boxes), ptr(out.scores), ptr(out.alive), ptr(out.frame),
+                           C.byref(n)))
         r = T + n.value
         return TrackStep(out.landmarks[:r], out.boxes[:r], out.scores[:r], out.alive[:r].bool(), out.frame[:r], n.value)
 
@@ -1523,7 +1538,8 @@ tensors landmarks (R, 2L) float32, boxes (R, 4) int32, scores (R,) float32, aliv
 class FaceTracker:
     """The state of a multi-stream face tracker: the live rows' landmarks, frames and integer ids, and the next id.  Each step
     is one track_and_detect call; frames holds one frame per stream, and a stream keeps its frame index from step to step.
-    Extra keyword arguments (variant, pad, nms_overlap, track_overlap, max_candidates, max_detections) go to track_and_detect."""
+    Extra keyword arguments (variant, pad, nms_overlap, track_overlap, max_candidates, max_detections, and multichannel,
+    bilinear_orientations, float_frames for a filter trained on colour or float frames) go to track_and_detect."""
 
     def __init__(self, model: detection_model, face_filter, filter_size, cell_size: int, num_bins: int, threshold: float, scales,
                  detect_threshold: float, **options):
@@ -1536,18 +1552,73 @@ class FaceTracker:
         self.ids = torch.empty(0, dtype=torch.int64, device=dev)
         self.next_id = 0
 
-    def step(self, frames, detect_frames=None):
+    def step(self, frames, detect_frames=None, grey_frames=None):
         """Steps every live track on frames and runs the detector on detect_frames (default: the frames without a live track).
-        Old rows keep their ids, new rows take fresh ids in row order, and the rows that are not alive are dropped.  Returns
-        (ids, frame, landmarks, boxes) of the live rows."""
+        Old rows keep their ids, new rows take fresh ids in row order, and the rows that are not alive are dropped.  grey_frames:
+        the cascade's frames, for float frames (see track_faces).  Returns (ids, frame, landmarks, boxes) of the live rows."""
         if detect_frames is None:
             live = set(self.frame.tolist())
             detect_frames = [f for f in range(len(frames)) if f not in live]
-        r = self.model.track_and_detect(frames, self.frame, self.landmarks, detect_frames=detect_frames, **self.args)
+        extra = {} if grey_frames is None else {"grey_frames": grey_frames}
+        r = self.model.track_and_detect(frames, self.frame, self.landmarks, detect_frames=detect_frames, **extra, **self.args)
         ids = torch.cat([self.ids, torch.arange(self.next_id, self.next_id + r.num_new, device=self.ids.device)])
         self.next_id += r.num_new
         self.ids, self.frame, self.landmarks = ids[r.alive], r.frame[r.alive], r.landmarks[r.alive]
         return self.ids, self.frame, self.landmarks, r.boxes[r.alive]
+
+
+def _check_float_frames(hi, float_frames: bool) -> None:
+    """float32 frames are resized by the float rule, which float_frames=True selects (as vl_hog_pyramid refuses them without)."""
+    if hi.dtype == _VL_HOG_DTYPES[torch.float32] and not float_frames:
+        raise ValueError("float32 frames need float_frames=True")
+
+
+def _track_frames(frames, ctx: Context, multichannel: bool, bilinear_orientations: bool, float_frames: bool, grey_frames, fn: str):
+    """The frames of a tracking step -> (what owns their device bytes, the grey ImageBatchC the cascade reads, the HogImagesC the
+    filter reads or None for grey frames).  Without multichannel the frames are _grey_frames'.  With it they keep their channels
+    (_window_frames), and the cascade's grey frames come from grey_frames when given; else from the frames themselves: 8-bit
+    B, G, R frames through sd_bgr2gray_images (one upload), 8-bit grey frames read in place.  Other frames need grey_frames."""
+    none = lambda w, h: None
+    if not multichannel:
+        if grey_frames is not None:
+            raise ValueError("grey_frames needs multichannel=True (grey frames are the cascade's frames)")
+        keep, ib, _ = _window_frames(frames, ctx, none, False, bilinear_orientations, float_frames)
+        if ib is None:
+            raise ValueError(f"{fn} needs at least one frame")
+        return keep, ib, None
+    descs = []
+    keep, hi, sizes = _window_frames(frames, ctx, none, True, bilinear_orientations, float_frames, descs)
+    if hi is None:
+        raise ValueError(f"{fn} needs at least one frame")
+    _check_float_frames(hi, float_frames)
+    if grey_frames is not None:
+        gkeep, ib, _ = _grey_frames(grey_frames, ctx, none)
+        if ib is None:
+            raise ValueError("grey_frames holds no frame")
+        return (keep, gkeep), ib, hi
+    dev = f"cuda:{ctx.device}"
+    if hi.dtype == _VL_HOG_DTYPES[torch.uint8] and hi.channels == 3:
+        # sized by sd_bgr2gray_images' stated layout from the host sizes, so the frame table is read back by the conversion only
+        nbytes = C.c_size_t(sum(h * _round16(w) for h, w in sizes) + (0 if len(set(sizes)) == 1 else len(sizes) * C.sizeof(FrameC)))
+        buf = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        ib = ImageBatchC()
+        _check(ctx.h, _capi.lib().sd_bgr2gray_images(ctx.h, C.byref(hi), ptr(buf), C.byref(nbytes), C.byref(ib)))
+        return (keep, buf), ib, hi
+    if hi.dtype == _VL_HOG_DTYPES[torch.uint8] and hi.channels == 1:
+        if all(d.pixel_stride == 1 for d in descs):          # grey frames read in place, through their own descriptors
+            if not hi.d_frames:
+                f = hi.frame
+                return keep, ImageBatchC(C.c_void_p(hi.d_data + f.offset), f.width, f.height, f.row_stride, hi.image_stride, hi.count), hi
+            table = _device_table([FrameC(d.width, d.height, d.row_stride, 0, d.offset) for d in descs], dev)
+            ib = ImageBatchC()
+            ib.d_data, ib.count, ib.d_frames = hi.d_data, hi.count, table.data_ptr()
+            return (keep, table), ib, hi
+        # a batch whose grey pixels are not contiguous along rows (a strided view): one contiguous copy on the device
+        g = keep.reshape(keep.shape[:3]).contiguous()
+        n, h, w = g.shape
+        return (keep, g), ImageBatchC(C.c_void_p(g.data_ptr()), w, h, g.stride(1), g.stride(0), n), hi
+    raise ValueError(f"{fn}: the cascade reads grey 8-bit frames; pass them as grey_frames= for float frames or frames of "
+                     f"{hi.channels} channels")
 
 
 def _dev_int32(a, dev) -> torch.Tensor:
@@ -1580,17 +1651,22 @@ def track_boxes(landmarks, model: detection_model):
 
 
 def hog_box_scores(frames, box_frame, boxes, filter, bias: float, cell_size: int, num_bins: int, variant: int = 1,
-                   ctx: Optional[Context] = None) -> torch.Tensor:
+                   ctx: Optional[Context] = None, multichannel: bool = False, bilinear_orientations: bool = False,
+                   float_frames: bool = False) -> torch.Tensor:
     """A HOG filter's score at each box (sd_hog_box_scores): box i ((x, y, w, h) of frames[box_frame[i]]) with one cell of
     context on every side, zero outside the frame, resized by cv::resize INTER_LINEAR to (fw + 2) x (fh + 2) cells of cell_size
     px, its hog_dense features scored by vl_hog_correlate with the filter ((dd, fh, fw)) and bias at every one of the 3 x 3
-    positions; the box's score is the largest (a NaN never is).  frames as hog_dense takes them.  Returns (n,) float32 on the
-    device."""
+    positions; the box's score is the largest (a NaN never is).  frames as hog_dense takes them.  multichannel,
+    bilinear_orientations and float_frames as vl_hog_detect takes them (sd_hog_box_scores_images): each channel of the context
+    rectangle is resized on its own by the rule of the frames' dtype and the crop's features are vl_hog's.  Returns (n,) float32
+    on the device."""
     ctx = ctx or default_context()
     dev = f"cuda:{ctx.device}"
-    keep, ib, _ = _grey_frames(frames, ctx, lambda w, h: None)
+    keep, ib, sizes = _window_frames(frames, ctx, lambda w, h: None, multichannel, bilinear_orientations, float_frames)
     if ib is None:
         raise ValueError("hog_box_scores needs at least one frame")
+    if multichannel:
+        _check_float_frames(ib, float_frames)
     f = _tensor(filter)
     f, fw, fh = _box_filter(f, (f.shape[-1], f.shape[-2]), num_bins, variant, dev)
     bf = _dev_int32(box_frame, dev).reshape(-1)
@@ -1599,8 +1675,11 @@ def hog_box_scores(frames, box_frame, boxes, filter, bias: float, cell_size: int
     if bx.shape[0] != n:
         raise ValueError("box_frame and boxes must have one entry per box")
     out = torch.empty(n, dtype=torch.float32, device=dev)
-    _check(ctx.h, _capi.lib().sd_hog_box_scores(ctx.h, C.byref(ib), ptr(bf), ptr(bx), n, ptr(f), fw, fh, C.c_float(float(bias)),
-                                                int(cell_size), int(num_bins), int(variant), ptr(out)))
+    lib = _capi.lib()
+    call, frames_args = ((lib.sd_hog_box_scores_images, [C.byref(ib), int(bool(bilinear_orientations))]) if multichannel else
+                         (lib.sd_hog_box_scores, [C.byref(ib)]))
+    _check(ctx.h, call(ctx.h, *frames_args, ptr(bf), ptr(bx), n, ptr(f), fw, fh, C.c_float(float(bias)), int(cell_size), int(num_bins),
+                       int(variant), ptr(out)))
     return out
 
 
@@ -1778,7 +1857,7 @@ def hog_pyramid_shape(width: int, height: int, scale: float, cell_size: int, num
     return (lw, lh), (d, h, w)
 
 
-def _window_frames(frames, ctx: Context, check, multichannel: bool, bilinear_orientations: bool, float_frames: bool):
+def _window_frames(frames, ctx: Context, check, multichannel: bool, bilinear_orientations: bool, float_frames: bool, frames_out=None):
     """The frames of vl_hog_pyramid and train_hog_filter -> (owner, batch, sizes): _hog_images' (channels last) with
     multichannel, _grey_frames' without.  bilinear_orientations and float_frames need multichannel, and float_frames float32
     frames."""
@@ -1786,7 +1865,7 @@ def _window_frames(frames, ctx: Context, check, multichannel: bool, bilinear_ori
         raise ValueError("bilinear_orientations needs multichannel=True (grey frames pass as they are)")
     if float_frames and not multichannel:
         raise ValueError("float_frames needs multichannel=True (float frames keep their channels)")
-    return _hog_images(frames, True, ctx, check, float_frames) if multichannel else _grey_frames(frames, ctx, check)
+    return _hog_images(frames, True, ctx, check, float_frames, frames_out) if multichannel else _grey_frames(frames, ctx, check)
 
 
 def vl_hog_pyramid(frames, scales, cell_size: int, num_bins: int, variant: int = 1, ctx: Optional[Context] = None,

@@ -796,6 +796,34 @@ __global__ void bgr2gray_kernel(const uint8_t* __restrict__ bgr, int width, int 
         }
     }
 }
+
+// sd_bgr2gray_images: frame f0 + blockIdx.y of an sd_hog_images batch of B, G, R bytes (per-frame table src_frames, or equally sized
+// frames src_frame image_stride elements apart) into its grey frame (per-frame table dst_frames, or dst_image_stride bytes apart
+// at a pitch of dst_pitch).  The CTAs of a frame walk its rows, the threads a row's pixels.
+__global__ void bgr2gray_images_kernel(const uint8_t* __restrict__ src, const sd_hog_image* __restrict__ src_frames, sd_hog_image src_frame,
+                                       long long image_stride, int f0, uint8_t* __restrict__ dst, const sd_frame* __restrict__ dst_frames,
+                                       long long dst_image_stride, int dst_pitch)
+{
+    const int f = f0 + blockIdx.y;
+    sd_hog_image d;
+    if (src_frames) {
+        d = src_frames[f];
+    } else {
+        d = src_frame;
+        d.offset += (long long)f * image_stride;
+    }
+    const long long o = dst_frames ? dst_frames[f].offset : (long long)f * dst_image_stride;
+    const long long pitch = dst_frames ? dst_frames[f].row_stride : dst_pitch;
+    const long long cs = d.channel_stride;
+    for (int y = blockIdx.x; y < d.height; y += gridDim.x) {
+        const uint8_t* s = src + d.offset + (long long)y * d.row_stride;
+        uint8_t* g = dst + o + y * pitch;
+        for (int x = threadIdx.x; x < d.width; x += blockDim.x) {
+            const uint8_t* p = s + (long long)x * d.pixel_stride;
+            g[x] = (uint8_t)sd_bgr_to_gray(__ldg(p), __ldg(p + cs), __ldg(p + 2 * cs));
+        }
+    }
+}
 }  // namespace
 
 extern "C" {
@@ -841,6 +869,58 @@ int sd_bgr2gray(sd_ctx* ctx, const uint8_t* d_bgr, int width, int height, int64_
     bgr2gray_kernel<<<blocks, 256, 0, ctx->stream>>>(d_bgr, width, height, bgr_row_stride, bgr_image_stride, count, d_gray,
                                                      gray_row_stride, gray_image_stride, vec_ok);
     SD_LAUNCH_CHECK(ctx, "bgr2gray_kernel");
+    return SD_OK;
+}
+
+int sd_bgr2gray_images(sd_ctx* ctx, const sd_hog_images* bgr, void* d_buf, size_t* bytes, sd_image_batch* out)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, bgr && bytes && bgr->count >= 1 && bgr->d_data, "bad argument");
+    SD_REQUIRE(ctx, bgr->dtype == SD_HOG_U8 && bgr->channels == 3, "frames must be SD_HOG_U8 with 3 channels (B, G, R)");
+    const int count = bgr->count;
+    HogPyramidFrames fr;
+    if (const int rc = sd_hog_read_image_frames(ctx, __func__, bgr, 0, &fr)) return rc;
+    // sd_upload_frames' layout: grey frames at a 16-byte pitch, back to back, then the descriptors when the sizes differ
+    std::vector<sd_frame> desc(count);
+    bool uniform = true;
+    size_t gray = 0;
+    int max_h = 0;
+    for (int i = 0; i < count; ++i) {
+        const sd_hog_image& f = fr.frames[i];
+        desc[i] = sd_frame{f.width, f.height, (int32_t)sd_round16(f.width), 0, (int64_t)gray};
+        gray += (size_t)f.height * sd_round16(f.width);
+        uniform = uniform && f.width == fr.frames[0].width && f.height == fr.frames[0].height;
+        max_h = std::max(max_h, f.height);
+    }
+    const size_t need = gray + (uniform ? 0 : (size_t)count * sizeof(sd_frame));
+    if (!d_buf) {
+        *bytes = need;
+        return SD_OK;
+    }
+    SD_REQUIRE(ctx, out && sd_aligned(d_buf, 16) && *bytes >= need,
+               "d_buf must be 16-byte aligned and hold the size the query gives; out must not be NULL");
+    uint8_t* base = static_cast<uint8_t*>(d_buf);
+    const sd_frame* d_desc = uniform ? nullptr : reinterpret_cast<const sd_frame*>(base + gray);
+    if (!uniform)
+        SD_CUDA(ctx, cudaMemcpyAsync(base + gray, desc.data(), (size_t)count * sizeof(sd_frame), cudaMemcpyHostToDevice, ctx->stream));
+    const unsigned rows = (unsigned)std::min(max_h, 1024);
+    for (int f0 = 0; f0 < count; f0 += 65535) {
+        const dim3 grid(rows, (unsigned)std::min(count - f0, 65535));
+        bgr2gray_images_kernel<<<grid, 128, 0, ctx->stream>>>(static_cast<const uint8_t*>(bgr->d_data), bgr->d_frames, bgr->frame,
+                                                             bgr->image_stride, f0, base, d_desc, (long long)desc[0].row_stride * desc[0].height,
+                                                             desc[0].row_stride);
+        SD_LAUNCH_CHECK(ctx, "bgr2gray_images_kernel");
+    }
+    sd_image_batch ib{};
+    ib.d_data = base;
+    ib.count = count;
+    if (uniform) {
+        ib.width = desc[0].width; ib.height = desc[0].height; ib.row_stride = desc[0].row_stride;
+        ib.image_stride = (int64_t)desc[0].row_stride * desc[0].height;
+    } else {
+        ib.d_frames = d_desc;
+    }
+    *out = ib;
     return SD_OK;
 }
 

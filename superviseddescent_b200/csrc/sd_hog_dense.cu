@@ -636,13 +636,14 @@ struct ResizeImagesArgs {
 // for every channel of every pixel with the channel fastest, so that a warp writes consecutive elements of the level, the
 // source read through L1.  A level of the frame's own size is copied.  kC = 1: 8-bit frames of one channel, contiguous pixels
 // (pixel stride 1), frames and levels of fewer than 2^31 bytes, the grey pyramid's: the pixel loop is spared two divisions by
-// a run-time count and takes every offset in 32 bits.  kC = 0: any channel count, strides and sizes.  kRect (8-bit grey only,
-// the box crops of sd_hog_box_scores): the level's W x H source is the rectangle at rect[level].(x, y) of a rect.z x rect.w
-// frame, its pixels outside the frame 0 (copyMakeBorder BORDER_CONSTANT); it writes no level offsets.
+// a run-time count and takes every offset in 32 bits.  kC = 0: any channel count, strides and sizes.  kRect (the box crops of
+// sd_hog_box_scores and sd_hog_box_scores_images): the level's W x H source is the rectangle at rect[level].(x, y) of a rect.z x
+// rect.w frame, its pixels outside the frame 0 (copyMakeBorder BORDER_CONSTANT); it writes no level offsets.  A float
+// rectangle's pixel outside the frame is a tap holding +0.0f, read and multiplied like any other.
 template <class T, int kC, bool kRect = false>
 __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kernel(const __grid_constant__ ResizeImagesArgs a)
 {
-    static_assert(!kRect || (kC == 1 && std::is_same<T, uint8_t>::value), "source rectangles are 8-bit grey");
+    static_assert(kC != 1 || std::is_same<T, uint8_t>::value, "kC = 1 is 8-bit grey");
     constexpr bool f32 = std::is_same<T, float>::value;
     __shared__ int s_sx[kResizeW], s_xw[kResizeW], s_y0[kResizeH], s_y1[kResizeH], s_yw[kResizeH];
     const int b = blockIdx.x, tid = threadIdx.x, C = kC > 0 ? kC : a.channels;
@@ -680,20 +681,30 @@ __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kern
         if (x >= L.w || y >= L.h) continue;
         const T* s = src + ch * L.chs;
         if constexpr (kRect) {
+            using V = typename std::conditional<f32, float, int>::type;
             const int4 R = a.rect[lo];
-            const auto px = [&](int u, int v) -> int {   // pixel (u, v) of the rectangle
+            const auto px = [&](int u, int v) -> V {   // pixel (u, v) of the rectangle
                 const long long fx = (long long)R.x + u, fy = (long long)R.y + v;
-                return fx >= 0 && fx < R.z && fy >= 0 && fy < R.w ? (int)__ldg(s + fy * L.rs + fx) : 0;
+                if (!(fx >= 0 && fx < R.z && fy >= 0 && fy < R.w)) return V(0);
+                return (V)__ldg(s + fy * L.rs + (kC == 1 ? fx : fx * L.ps));
             };
-            int v;
+            V v;
             if (copy) {
                 v = px(x, y);
+            } else if constexpr (f32) {
+                const int sx = s_sx[c];
+                const float fx = __int_as_float(s_xw[c]);
+                const auto row_at = [&](int yy) {   // hog_resize_row_f32 of rectangle row yy
+                    const float t = __fmul_rn(px(sx, yy), __fsub_rn(1.f, fx));
+                    return sx == L.W - 1 ? t : __fadd_rn(t, __fmul_rn(px(sx + 1, yy), fx));
+                };
+                v = hog_resize_out_f32(__int_as_float(s_yw[r]), row_at(s_y0[r]), row_at(s_y1[r]));
             } else {
                 const int sx = s_sx[c], sx1 = min(sx + 1, L.W - 1);
                 const int ax = (short)s_xw[c], bx = s_xw[c] >> 16;
                 v = hog_resize_out(s_yw[r], px(sx, s_y0[r]) * ax + px(sx1, s_y0[r]) * bx, px(sx, s_y1[r]) * ax + px(sx1, s_y1[r]) * bx);
             }
-            dst[(long long)y * L.pitch + x] = (uint8_t)v;
+            reinterpret_cast<T*>(dst + (long long)y * L.pitch)[(long long)x * C + ch] = (T)v;
         } else if constexpr (f32) {
             float v;
             if (copy) {
@@ -724,27 +735,39 @@ __global__ void __launch_bounds__(kResizeThreads) hog_pyramid_resize_images_kern
     }
 }
 
+// Where hog_box_levels_kernel finds frame f: a grey batch's sd_frame table, an sd_hog_images table, or equally sized frames
+// (frame, offset advanced by image_stride elements per frame).
+struct BoxFrameTable {
+    const sd_frame* grey_frames;
+    const sd_hog_image* frames;
+    sd_hog_image frame;
+    long long image_stride;
+};
+
 // The level of box i of sd_hog_box_crops: its context rectangle of its frame, resized to the crop size; a box whose d_ok byte is
 // 0 takes the 1 x 1 rectangle at (0, 0).  One thread per box.
-__global__ void hog_box_levels_kernel(const sd_image_batch images, const int32_t* __restrict__ box_frame, const int32_t* __restrict__ boxes,
+__global__ void hog_box_levels_kernel(const BoxFrameTable t, const int32_t* __restrict__ box_frame, const int32_t* __restrict__ boxes,
                                       const uint8_t* __restrict__ ok, int n, int fw, int fh, int cw, int ch, int pitch, int tiles_x,
                                       int tiles_per_box, PyrImageLevel* __restrict__ levels, int4* __restrict__ rect)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int f = box_frame[i];
-    sd_frame d;
-    if (images.d_frames) {
-        d = images.d_frames[f];
+    sd_hog_image d;
+    if (t.grey_frames) {
+        const sd_frame g = t.grey_frames[f];
+        d = sd_hog_image{g.width, g.height, g.offset, g.row_stride, 1, 0};
+    } else if (t.frames) {
+        d = t.frames[f];
     } else {
-        d.width = images.width; d.height = images.height; d.row_stride = images.row_stride;
-        d.offset = (int64_t)f * images.image_stride;
+        d = t.frame;
+        d.offset += (long long)f * t.image_stride;
     }
     int rx = 0, ry = 0, rw = 1, rh = 1;
     if (!ok || ok[i]) sd_box_context(boxes[4 * i], boxes[4 * i + 1], boxes[4 * i + 2], boxes[4 * i + 3], fw, fh, &rx, &ry, &rw, &rh);
     PyrImageLevel L{};
     L.src = d.offset;
-    L.rs = d.row_stride; L.ps = 1; L.chs = 0;
+    L.rs = d.row_stride; L.ps = d.pixel_stride; L.chs = d.channel_stride;
     L.dst = (long long)i * pitch * ch;
     L.W = rw; L.H = rh;
     L.w = cw; L.h = ch; L.pitch = pitch;
@@ -886,7 +909,7 @@ int pyramid_images(sd_ctx* ctx, const char* fn, const sd_hog_images* images, con
 
 size_t sd_hog_box_table_bytes(int n) { return sd_round16(sizeof(PyrImageLevel) * (size_t)n) + sizeof(int4) * (size_t)n; }
 
-int sd_hog_box_crops(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_box_frame, const int32_t* d_boxes, const uint8_t* d_ok,
+int sd_hog_box_crops(sd_ctx* ctx, const BoxFrames& src, const int32_t* d_box_frame, const int32_t* d_boxes, const uint8_t* d_ok,
                      int n, int fw, int fh, int cell_size, uint8_t* d_crops, int pitch, void* d_tables)
 {
     if (n == 0) return SD_OK;
@@ -895,18 +918,34 @@ int sd_hog_box_crops(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d
     if ((long long)n * tiles_per_box > INT_MAX) return sd_fail(ctx, SD_ERR_INVALID, "sd_hog_box_scores: too many boxes for one launch");
     PyrImageLevel* levels = static_cast<PyrImageLevel*>(d_tables);
     int4* rect = reinterpret_cast<int4*>(static_cast<uint8_t*>(d_tables) + sd_round16(sizeof(PyrImageLevel) * (size_t)n));
-    hog_box_levels_kernel<<<sd_div_up(n, 128), 128, 0, ctx->stream>>>(*images, d_box_frame, d_boxes, d_ok, n, fw, fh, cw, ch, pitch,
-                                                                      tiles_x, tiles_per_box, levels, rect);
+    BoxFrameTable t{};
+    if (src.grey) {
+        t.grey_frames = src.grey->d_frames;
+        t.frame = sd_hog_image{src.grey->width, src.grey->height, 0, src.grey->row_stride, 1, 0};
+        t.image_stride = src.grey->image_stride;
+    } else {
+        t.frames = src.images->d_frames;
+        t.frame = src.images->frame;
+        t.image_stride = src.images->image_stride;
+    }
+    hog_box_levels_kernel<<<sd_div_up(n, 128), 128, 0, ctx->stream>>>(t, d_box_frame, d_boxes, d_ok, n, fw, fh, cw, ch, pitch, tiles_x,
+                                                                      tiles_per_box, levels, rect);
     SD_LAUNCH_CHECK(ctx, "hog_box_levels_kernel");
     ResizeImagesArgs r;
     memset(&r, 0, sizeof(r));
-    r.images = images->d_data;
+    r.images = src.data();
     r.scratch = d_crops;
     r.levels = levels;
     r.count = n;
-    r.channels = 1;
+    r.channels = src.channels();
     r.rect = rect;
-    hog_pyramid_resize_images_kernel<uint8_t, 1, true><<<(unsigned)(n * tiles_per_box), kResizeThreads, 0, ctx->stream>>>(r);
+    // kC = 1 for frames whose pixels are known to be contiguous bytes of one channel: a grey batch, or such an sd_hog_images batch
+    // of equally sized frames
+    const bool grey = src.grey || (src.dtype() == SD_HOG_U8 && src.channels() == 1 && !t.frames && t.frame.pixel_stride == 1);
+    const auto resize = grey ? hog_pyramid_resize_images_kernel<uint8_t, 1, true>
+                        : src.dtype() == SD_HOG_F32 ? hog_pyramid_resize_images_kernel<float, 0, true>
+                                                    : hog_pyramid_resize_images_kernel<uint8_t, 0, true>;
+    resize<<<(unsigned)(n * tiles_per_box), kResizeThreads, 0, ctx->stream>>>(r);
     SD_LAUNCH_CHECK(ctx, "hog_pyramid_resize_images_kernel");
     return SD_OK;
 }

@@ -232,11 +232,24 @@ int sd_hog_batch_unmirrored(sd_ctx* ctx, const sd_image_batch* images, const int
 int sd_detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_face_frame, const float* d_x0,
                      int count, float* d_landmarks, uint8_t* d_face_degenerate);
 const float* sd_model_device_mean(const sd_model* m);
-// The crops of sd_hog_box_scores (sd_hog_dense.cu): box i's context rectangle (sd_box_context) of frame d_box_frame[i] resized
-// to (fw + 2) cs x (fh + 2) cs px at d_crops + i * pitch * (fh + 2) cs, rows pitch bytes apart.  d_ok (optional): a box whose
-// byte is 0 crops a 1 x 1 rectangle instead.  d_tables: sd_hog_box_table_bytes(n) bytes of device scratch.
+// The frames whose boxes sd_hog_box_scores / sd_hog_box_scores_images score and on which the tracking step detects: an 8-bit grey
+// batch (grey, the grey entry points) or frames that keep their channels (images, with their orientation assignment).  Exactly
+// one of grey and images is set.
+struct BoxFrames {
+    const sd_image_batch* grey;
+    const sd_hog_images* images;
+    int bilinear;
+    int dtype() const { return grey ? SD_HOG_U8 : images->dtype; }
+    int channels() const { return grey ? 1 : images->channels; }
+    int count() const { return grey ? grey->count : images->count; }
+    const void* data() const { return grey ? static_cast<const void*>(grey->d_data) : images->d_data; }
+};
+// The crops of sd_hog_box_scores (sd_hog_dense.cu): box i's context rectangle (sd_box_context) of frame d_box_frame[i], each
+// channel resized on its own by the rule of the frames' dtype to (fw + 2) cs x (fh + 2) cs px, interleaved (channels last) at
+// d_crops + i * pitch * (fh + 2) cs bytes, rows pitch bytes apart.  d_ok (optional): a box whose byte is 0 crops a 1 x 1
+// rectangle instead.  d_tables: sd_hog_box_table_bytes(n) bytes of device scratch.
 size_t sd_hog_box_table_bytes(int n);
-int sd_hog_box_crops(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_box_frame, const int32_t* d_boxes, const uint8_t* d_ok,
+int sd_hog_box_crops(sd_ctx* ctx, const BoxFrames& src, const int32_t* d_box_frame, const int32_t* d_boxes, const uint8_t* d_ok,
                      int n, int fw, int fh, int cell_size, uint8_t* d_crops, int pitch, void* d_tables);
 
 // cvRound: to nearest, ties to even

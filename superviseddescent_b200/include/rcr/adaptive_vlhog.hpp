@@ -118,9 +118,10 @@ inline std::vector<int64_t> pack_planes(sd_ctx* ctx, const std::vector<cv::Mat>&
 }
 
 // Frames of one type with C channels of elem bytes each (checked by the caller) on the device, interleaved as OpenCV holds
-// them: packed end to end into buf (row steps dropped), one descriptor per frame in table
+// them: packed end to end into buf (row steps dropped), one descriptor per frame in table (and in *desc, if given)
 inline sd_hog_images upload_interleaved(sd_ctx* ctx, const std::vector<cv::Mat>& images, size_t elem, int dtype,
-                                        sd_b200::DeviceBuffer& buf, sd_b200::DeviceBuffer& table, const char* what)
+                                        sd_b200::DeviceBuffer& buf, sd_b200::DeviceBuffer& table, const char* what,
+                                        std::vector<sd_hog_image>* desc_out = nullptr)
 {
     const int n = static_cast<int>(images.size()), C = images[0].channels();
     const std::vector<int64_t> start = pack_planes(ctx, images, elem * static_cast<size_t>(C), buf, what);
@@ -135,17 +136,18 @@ inline sd_hog_images upload_interleaved(sd_ctx* ctx, const std::vector<cv::Mat>&
     batch.channels = C;
     batch.count = n;
     batch.d_frames = table.as<sd_hog_image>();
+    if (desc_out) *desc_out = desc;
     return batch;
 }
 
 // 8UC1 or 8UC3 (B,G,R) frames, all of one type, on the device with their channels kept (upload_interleaved)
 inline sd_hog_images upload_channels(sd_ctx* ctx, const std::vector<cv::Mat>& images, sd_b200::DeviceBuffer& buf,
-                                     sd_b200::DeviceBuffer& table, const char* what)
+                                     sd_b200::DeviceBuffer& table, const char* what, std::vector<sd_hog_image>* desc_out = nullptr)
 {
     for (const cv::Mat& m : images)
         if (m.type() != images[0].type() || (m.type() != CV_8UC1 && m.type() != CV_8UC3))
             throw std::runtime_error(std::string(what) + ": frames must be all CV_8UC1 or all CV_8UC3");
-    return upload_interleaved(ctx, images, 1, SD_HOG_U8, buf, table, what);
+    return upload_interleaved(ctx, images, 1, SD_HOG_U8, buf, table, what, desc_out);
 }
 
 // 32FC1 or 32FC3 frames, all of one type, on the device as float channels (upload_interleaved), for the float pyramid
@@ -156,6 +158,65 @@ inline sd_hog_images upload_float_channels(sd_ctx* ctx, const std::vector<cv::Ma
         if (m.type() != images[0].type() || (m.type() != CV_32FC1 && m.type() != CV_32FC3))
             throw std::runtime_error(std::string(what) + ": float frames must be all CV_32FC1 or all CV_32FC3");
     return upload_interleaved(ctx, images, sizeof(float), SD_HOG_F32, buf, table, what);
+}
+
+// The frames of a tracking step and of hog_box_scores: colour, the frames the filter reads, as vl_hog_pyramid uploads them
+// (multichannel: upload_channels; float_frames: upload_float_channels), and grey, the cascade's grey batch.  Without
+// multichannel both are the grey upload (upload_grey).  With it the grey frames are *grey_images (8UC1 / 8UC3, the sizes of
+// images) when given; else 8UC3 frames are converted on the device (sd_bgr2gray_images, so a colour frame is uploaded once)
+// and 8UC1 frames are read in place; float frames need grey_images.
+struct TrackFrames {
+    bool multichannel = false;
+    sd_image_batch grey{};
+    sd_hog_images colour{};
+    sd_b200::DeviceBuffer buf, table, grey_buf;
+};
+
+// sd_bgr2gray_images' size for frames of these sizes, by the layout include/sd_b200.h states (sd_upload_frames'): no read-back
+inline size_t bgr2gray_bytes(const std::vector<sd_hog_image>& desc)
+{
+    size_t bytes = 0;
+    bool uniform = true;
+    for (const sd_hog_image& d : desc) {
+        bytes += static_cast<size_t>(d.height) * ((static_cast<size_t>(d.width) + 15) / 16 * 16);
+        uniform = uniform && d.width == desc[0].width && d.height == desc[0].height;
+    }
+    return bytes + (uniform ? 0 : desc.size() * sizeof(sd_frame));
+}
+
+inline void upload_track_frames(sd_ctx* ctx, const std::vector<cv::Mat>& images, bool multichannel, bool bilinear_orientations,
+                                bool float_frames, const std::vector<cv::Mat>* grey_images, TrackFrames& out, const char* what)
+{
+    const std::string w(what);
+    if (bilinear_orientations && !multichannel) throw std::runtime_error(w + ": bilinear_orientations needs multichannel");
+    if (float_frames && !multichannel) throw std::runtime_error(w + ": float_frames needs multichannel");
+    if (grey_images && !multichannel) throw std::runtime_error(w + ": grey_images needs multichannel (grey frames are the cascade's)");
+    out.multichannel = multichannel;
+    if (!multichannel) {
+        out.grey = upload_grey(ctx, sd_b200::host_frames(images), out.buf, what);
+        return;
+    }
+    std::vector<sd_hog_image> desc;
+    out.colour = float_frames ? upload_float_channels(ctx, images, out.buf, out.table, what)
+                              : upload_channels(ctx, images, out.buf, out.table, what, &desc);
+    if (grey_images) {
+        if (grey_images->size() != images.size()) throw std::runtime_error(w + ": grey_images needs one frame per frame");
+        out.grey = upload_grey(ctx, sd_b200::host_frames(*grey_images), out.grey_buf, what);
+    } else if (float_frames) {
+        throw std::runtime_error(w + ": float frames need grey_images for the cascade");
+    } else if (images[0].type() == CV_8UC3) {
+        size_t bytes = bgr2gray_bytes(desc);
+        out.grey_buf.allocate(bytes);
+        sd_b200::check(ctx, sd_bgr2gray_images(ctx, &out.colour, out.grey_buf.as<void>(), &bytes, &out.grey), what);
+    } else {                                  // 8UC1: the grey batch is the uploaded frames, with its own sd_frame table
+        std::vector<sd_frame> grey;
+        for (const sd_hog_image& d : desc) grey.push_back(sd_frame{d.width, d.height, static_cast<int32_t>(d.row_stride), 0, d.offset});
+        out.grey_buf.allocate(grey.size() * sizeof(sd_frame));
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, out.grey_buf.as<void>(), grey.data(), grey.size() * sizeof(sd_frame)), what);
+        out.grey.d_data = static_cast<const uint8_t*>(out.colour.d_data);
+        out.grey.count = out.colour.count;
+        out.grey.d_frames = out.grey_buf.as<sd_frame>();
+    }
 }
 
 }  // namespace hog_batch
@@ -823,10 +884,15 @@ inline hog_filter train_hog_filter(const std::vector<cv::Mat>& images, const std
 // box_frame[k], with one cell of context on every side, zero outside the frame, is resized to (fw + 2) x (fh + 2) cells of
 // cell_size px and scored by the filter (dd * fh x fw CV_32FC1, hog_filter::filter's layout) and bias at each of the 3 x 3
 // positions; the box's score is the largest (a NaN never is).  images: 8UC1 or 8UC3 (B,G,R) frames of any sizes, uploaded as
-// grey.  Throws std::runtime_error where sd_hog_box_scores refuses.
+// grey.  multichannel, bilinear_orientations and float_frames as vl_hog_pyramid takes them (sd_hog_box_scores_images): a filter
+// trained on colour or float frames scores the boxes on the frames as given (8UC1 / 8UC3, or CV_32FC1 / CV_32FC3 with
+// float_frames).  Throws std::runtime_error where sd_hog_box_scores or sd_hog_box_scores_images refuses.
 inline std::vector<float> hog_box_scores(const std::vector<cv::Mat>& images, const std::vector<int>& box_frame, const std::vector<cv::Rect>& boxes,
-                                         const cv::Mat& filter, float bias, VlHogVariant variant, int cell_size, int num_bins)
+                                         const cv::Mat& filter, float bias, VlHogVariant variant, int cell_size, int num_bins,
+                                         bool multichannel = false, bool bilinear_orientations = false, bool float_frames = false)
 {
+    if (bilinear_orientations && !multichannel) throw std::runtime_error("hog_box_scores: bilinear_orientations needs multichannel");
+    if (float_frames && !multichannel) throw std::runtime_error("hog_box_scores: float_frames needs multichannel");
     if (images.empty()) throw std::runtime_error("hog_box_scores: no frames");
     if (box_frame.size() != boxes.size()) throw std::runtime_error("hog_box_scores: box_frame and boxes differ in length");
     const int dd = sd_b200::hog_dimension(variant, num_bins);
@@ -836,8 +902,12 @@ inline std::vector<float> hog_box_scores(const std::vector<cv::Mat>& images, con
     std::vector<float> out(n);
     if (n == 0) return out;
     sd_ctx* ctx = sd_b200::context();
-    sd_b200::DeviceBuffer buf, d_filter, d_boxes(static_cast<size_t>(n) * 5 * sizeof(int32_t)), d_scores(static_cast<size_t>(n) * sizeof(float));
-    const sd_image_batch batch = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), buf, "hog_box_scores upload");
+    sd_b200::DeviceBuffer buf, d_frames, d_filter, d_boxes(static_cast<size_t>(n) * 5 * sizeof(int32_t)), d_scores(static_cast<size_t>(n) * sizeof(float));
+    sd_image_batch batch{};
+    sd_hog_images colour{};
+    if (float_frames) colour = hog_batch::upload_float_channels(ctx, images, buf, d_frames, "hog_box_scores upload");
+    else if (multichannel) colour = hog_batch::upload_channels(ctx, images, buf, d_frames, "hog_box_scores upload");
+    else batch = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), buf, "hog_box_scores upload");
     sd_b200::upload(filter, d_filter, filter.cols);
     std::vector<int32_t> table(static_cast<size_t>(n) * 5);   // [frame indices | boxes]
     for (int k = 0; k < n; ++k) {
@@ -846,8 +916,13 @@ inline std::vector<float> hog_box_scores(const std::vector<cv::Mat>& images, con
         std::memcpy(&table[n + 4 * k], b, sizeof(b));
     }
     sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_boxes.as<int32_t>(), table.data(), table.size() * sizeof(int32_t)), "hog_box_scores");
-    sd_b200::check(ctx, sd_hog_box_scores(ctx, &batch, d_boxes.as<int32_t>(), d_boxes.as<int32_t>() + n, n, d_filter.as<float>(), filter.cols,
-                                          filter.rows / dd, bias, cell_size, num_bins, variant, d_scores.as<float>()), "sd_hog_box_scores");
+    if (multichannel)
+        sd_b200::check(ctx, sd_hog_box_scores_images(ctx, &colour, bilinear_orientations ? 1 : 0, d_boxes.as<int32_t>(), d_boxes.as<int32_t>() + n,
+                                                     n, d_filter.as<float>(), filter.cols, filter.rows / dd, bias, cell_size, num_bins, variant,
+                                                     d_scores.as<float>()), "sd_hog_box_scores_images");
+    else
+        sd_b200::check(ctx, sd_hog_box_scores(ctx, &batch, d_boxes.as<int32_t>(), d_boxes.as<int32_t>() + n, n, d_filter.as<float>(), filter.cols,
+                                              filter.rows / dd, bias, cell_size, num_bins, variant, d_scores.as<float>()), "sd_hog_box_scores");
     sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.data(), d_scores.as<float>(), out.size() * sizeof(float)), "hog_box_scores");
     sd_b200::check(ctx, sd_sync(ctx), "hog_box_scores");
     return out;

@@ -215,9 +215,13 @@ public:
     // while that box is valid, its score exceeds threshold and no cascade level had an empty patch.  A track whose previous box
     // is degenerate dies and keeps its previous landmarks.  images: 8UC1 or 8UC3 (B,G,R) frames of any sizes, uploaded as grey
     // (hog_batch::upload_grey).  There is no tracker state: drop the dead tracks and start new ones from vl_hog_detect boxes.
-    // Throws std::runtime_error where sd_track_faces refuses.
+    // multichannel, bilinear_orientations and float_frames as vl_hog_detect takes them (sd_track_faces_images): a filter trained
+    // on colour or float frames scores the boxes on the frames as given, while the cascade reads grey frames -- 8UC3 frames
+    // converted on the device after one upload, 8UC1 frames as they are, or *grey_images (needed for CV_32FC1 / CV_32FC3 frames;
+    // hog_batch::upload_track_frames).  Throws std::runtime_error where sd_track_faces or sd_track_faces_images refuses.
     tracked_faces track(const std::vector<cv::Mat>& images, const std::vector<int>& face_frame, cv::Mat previous, const hog_filter& filter,
-                        VlHogVariant variant, int cell_size, int num_bins, float threshold)
+                        VlHogVariant variant, int cell_size, int num_bins, float threshold, bool multichannel = false,
+                        bool bilinear_orientations = false, bool float_frames = false, const std::vector<cv::Mat>* grey_images = nullptr)
     {
         const int P = 2 * sd_model_num_landmarks(handle.get()), T = static_cast<int>(face_frame.size());
         if (images.empty()) throw std::runtime_error("track: no frames");
@@ -229,18 +233,26 @@ public:
         tracked_faces out;
         if (T == 0) return out;
         sd_ctx* ctx = sd_b200::context();
-        sd_b200::DeviceBuffer buf, d_filter, d_prev, d_frame(static_cast<size_t>(T) * sizeof(int32_t));
+        sd_b200::DeviceBuffer d_filter, d_prev, d_frame(static_cast<size_t>(T) * sizeof(int32_t));
         sd_b200::DeviceBuffer d_lms(static_cast<size_t>(T) * P * sizeof(float)), d_boxes(static_cast<size_t>(T) * 4 * sizeof(int32_t));
         sd_b200::DeviceBuffer d_scores(static_cast<size_t>(T) * sizeof(float)), d_alive(static_cast<size_t>(T));
-        const sd_image_batch batch = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), buf, "track upload");
+        hog_batch::TrackFrames fr;
+        hog_batch::upload_track_frames(ctx, images, multichannel, bilinear_orientations, float_frames, grey_images, fr, "track upload");
         sd_b200::upload(filter.filter, d_filter, filter.filter.cols);
         sd_b200::upload(previous, d_prev, P);
         const std::vector<int32_t> idx(face_frame.begin(), face_frame.end());
         sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_frame.as<int32_t>(), idx.data(), idx.size() * sizeof(int32_t)), "track");
-        sd_b200::check(ctx, sd_track_faces(ctx, handle.get(), &batch, d_frame.as<int32_t>(), d_prev.as<float>(), T, d_filter.as<float>(),
-                                           filter.filter.cols, filter.filter.rows / dd, filter.bias, cell_size, num_bins, variant, threshold,
-                                           d_lms.as<float>(), d_boxes.as<int32_t>(), d_scores.as<float>(), d_alive.as<uint8_t>()),
-                       "sd_track_faces");
+        if (multichannel)
+            sd_b200::check(ctx, sd_track_faces_images(ctx, handle.get(), &fr.grey, &fr.colour, bilinear_orientations ? 1 : 0, d_frame.as<int32_t>(),
+                                                      d_prev.as<float>(), T, d_filter.as<float>(), filter.filter.cols, filter.filter.rows / dd,
+                                                      filter.bias, cell_size, num_bins, variant, threshold, d_lms.as<float>(),
+                                                      d_boxes.as<int32_t>(), d_scores.as<float>(), d_alive.as<uint8_t>()),
+                           "sd_track_faces_images");
+        else
+            sd_b200::check(ctx, sd_track_faces(ctx, handle.get(), &fr.grey, d_frame.as<int32_t>(), d_prev.as<float>(), T, d_filter.as<float>(),
+                                               filter.filter.cols, filter.filter.rows / dd, filter.bias, cell_size, num_bins, variant, threshold,
+                                               d_lms.as<float>(), d_boxes.as<int32_t>(), d_scores.as<float>(), d_alive.as<uint8_t>()),
+                           "sd_track_faces");
         std::vector<int32_t> boxes(static_cast<size_t>(T) * 4);
         std::vector<uint8_t> alive(T);
         out.scores.resize(T);
@@ -260,11 +272,15 @@ public:
     // track(), the face filter runs as vl_hog_detect on the frames detect_frames lists (distinct indices; the pyramid's scales),
     // a detection that no alive track of its frame overlaps by IoU > params.track_overlap starts a new row from its box, and
     // within each frame the alive rows are kept greedily (old rows first, then by score) unless a kept row overlaps them.  The
-    // frames are uploaded once (hog_batch::upload_grey).  previous may be empty when face_frame is.  Throws std::runtime_error
-    // where sd_track_detect_faces refuses.
+    // frames are uploaded once (hog_batch::upload_grey).  previous may be empty when face_frame is.  multichannel,
+    // bilinear_orientations, float_frames and grey_images as track() takes them: the box scores and the detector
+    // (vl_hog_detect with the same options) read the frames as given, the cascade their grey (sd_track_detect_faces_images).
+    // Throws std::runtime_error where sd_track_detect_faces or sd_track_detect_faces_images refuses.
     track_step track_and_detect(const std::vector<cv::Mat>& images, const std::vector<int>& face_frame, cv::Mat previous,
                                 const hog_filter& filter, VlHogVariant variant, int cell_size, int num_bins, float threshold,
-                                const std::vector<double>& scales, const std::vector<int>& detect_frames, const track_detect_params& params)
+                                const std::vector<double>& scales, const std::vector<int>& detect_frames, const track_detect_params& params,
+                                bool multichannel = false, bool bilinear_orientations = false, bool float_frames = false,
+                                const std::vector<cv::Mat>* grey_images = nullptr)
     {
         const int P = 2 * sd_model_num_landmarks(handle.get()), T = static_cast<int>(face_frame.size());
         if (images.empty()) throw std::runtime_error("track_and_detect: no frames");
@@ -276,10 +292,12 @@ public:
         if (params.max_detections < 1) throw std::runtime_error("track_and_detect: max_detections must be at least 1");
         const size_t R = static_cast<size_t>(T) + detect_frames.size() * static_cast<size_t>(params.max_detections);
         sd_ctx* ctx = sd_b200::context();
-        sd_b200::DeviceBuffer buf, d_filter, d_prev, d_face(static_cast<size_t>(T) * sizeof(int32_t) + 4);
+        sd_b200::DeviceBuffer d_filter, d_prev, d_face(static_cast<size_t>(T) * sizeof(int32_t) + 4);
         sd_b200::DeviceBuffer d_lms(R * P * sizeof(float) + 4), d_boxes(R * 4 * sizeof(int32_t) + 4), d_scores(R * sizeof(float) + 4);
         sd_b200::DeviceBuffer d_alive(R + 4), d_frame(R * sizeof(int32_t) + 4);
-        const sd_image_batch batch = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), buf, "track_and_detect upload");
+        hog_batch::TrackFrames fr;
+        hog_batch::upload_track_frames(ctx, images, multichannel, bilinear_orientations, float_frames, grey_images, fr,
+                                       "track_and_detect upload");
         sd_b200::upload(filter.filter, d_filter, filter.filter.cols);
         if (T > 0) sd_b200::upload(previous, d_prev, P);
         const std::vector<int32_t> idx(face_frame.begin(), face_frame.end()), listed(detect_frames.begin(), detect_frames.end());
@@ -292,12 +310,21 @@ public:
         p.nms_overlap = params.nms_overlap; p.track_overlap = params.track_overlap;
         p.max_candidates = params.max_candidates; p.max_detections = params.max_detections;
         int32_t num_new = 0;
-        sd_b200::check(ctx, sd_track_detect_faces(ctx, handle.get(), &batch, d_face.as<int32_t>(), d_prev.as<float>(), T, d_filter.as<float>(),
-                                                  filter.filter.cols, filter.filter.rows / dd, filter.bias, cell_size, num_bins, variant,
-                                                  threshold, listed.data(), static_cast<int>(listed.size()), &p, d_lms.as<float>(),
-                                                  d_boxes.as<int32_t>(), d_scores.as<float>(), d_alive.as<uint8_t>(), d_frame.as<int32_t>(),
-                                                  &num_new),
-                       "sd_track_detect_faces");
+        if (multichannel)
+            sd_b200::check(ctx, sd_track_detect_faces_images(ctx, handle.get(), &fr.grey, &fr.colour, bilinear_orientations ? 1 : 0,
+                                                             d_face.as<int32_t>(), d_prev.as<float>(), T, d_filter.as<float>(), filter.filter.cols,
+                                                             filter.filter.rows / dd, filter.bias, cell_size, num_bins, variant, threshold,
+                                                             listed.data(), static_cast<int>(listed.size()), &p, d_lms.as<float>(),
+                                                             d_boxes.as<int32_t>(), d_scores.as<float>(), d_alive.as<uint8_t>(),
+                                                             d_frame.as<int32_t>(), &num_new),
+                           "sd_track_detect_faces_images");
+        else
+            sd_b200::check(ctx, sd_track_detect_faces(ctx, handle.get(), &fr.grey, d_face.as<int32_t>(), d_prev.as<float>(), T, d_filter.as<float>(),
+                                                      filter.filter.cols, filter.filter.rows / dd, filter.bias, cell_size, num_bins, variant,
+                                                      threshold, listed.data(), static_cast<int>(listed.size()), &p, d_lms.as<float>(),
+                                                      d_boxes.as<int32_t>(), d_scores.as<float>(), d_alive.as<uint8_t>(), d_frame.as<int32_t>(),
+                                                      &num_new),
+                           "sd_track_detect_faces");
         const int rows = T + num_new;
         track_step out;
         out.num_new = num_new;
