@@ -1247,6 +1247,58 @@ SD_API int sd_track_detect_faces_images(sd_ctx* ctx, const sd_model* m, const sd
                                         int num_detect_frames, const sd_track_detect_param* param, float* d_landmarks,
                                         int32_t* d_boxes, float* d_scores, uint8_t* d_alive, int32_t* d_frame, int32_t* h_num_new);
 
+/* ---- aligned face chips: a face's landmarks fitted to a template, its frame warped as cv::warpAffine does --------------------
+ * Fit.  Face i has the landmarks x = d_landmarks + i * ldl (2L floats, [x.., y..]); its n used landmarks k = h_landmark[j] have
+ * template points u_j = (h_template[2 j], h_template[2 j + 1]) in chip pixels.  The least-squares similarity
+ * T(u) = [[a, -b], [b, a]] u + t from template to landmarks (chip to frame) is, in double with every operation rounded on its own
+ * and every sum taken from 0 in list order (j ascending):
+ *   ubar = (sum u_j) / n, xbar = (sum x_j) / n, u~ = u - ubar, x~ = x - xbar,
+ *   den = sum (u~x u~x + u~y u~y), a = sum (u~x x~x + u~y x~y) / den, b = sum (u~x x~y - u~y x~x) / den,
+ *   tx = xbar_x - (a ubar_x - b ubar_y), ty = xbar_y - (b ubar_x + a ubar_y).
+ * chip_to_frame M = [a, -b, tx; b, a, ty]; frame_to_chip, its exact algebraic inverse, is [ia, ib, -(ia tx + ib ty); -ib, ia,
+ * ib tx - ia ty] with s = a a + b b, ia = a / s, ib = b / s.
+ * Warp: cv::warpAffine(frame, M, (width, height), INTER_LINEAR | WARP_INVERSE_MAP, BORDER_CONSTANT, 0), bit for bit.  For chip
+ * pixel (X, Y), with cvRound to nearest, ties to even:
+ *   adelta = cvRound(M00 X 1024), bdelta = cvRound(M10 X 1024), X0 = cvRound((M01 Y + M02) 1024) + 16, Y0 = cvRound((M11 Y + M12)
+ *   1024) + 16, Xs = (X0 + adelta) >> 5, Ys = (Y0 + bdelta) >> 5 (arithmetic shifts); the taps are (Xs >> 5, Ys >> 5) and its
+ *   right, lower and lower-right neighbours, fx = Xs & 31, fy = Ys & 31.  A tap outside the frame reads 0; every tap is read
+ *   and multiplied.  SD_HOG_U8: (S00 w0 + S01 w1 + S10 w2 + S11 w3 + 2^14) >> 15 with the integer weights w0 = (32 - fx)(32 - fy)
+ *   32, w1 = fx (32 - fy) 32, w2 = (32 - fx) fy 32, w3 = fx fy 32.  SD_HOG_F32: S00 w0 + S01 w1 + S10 w2 + S11 w3 in float, left
+ *   to right, each product and sum rounded on its own, with w0 = (1 - fx / 32)(1 - fy / 32) and so on (exact in float).
+ *   Each channel is warped on its own with the same taps.
+ * A face is invalid -- its chip all zeros, both transforms zeros, d_valid 0 -- when a used landmark is not finite, den == 0,
+ * a a + b b == 0, a value X0, Y0, adelta, bdelta, X0 + adelta or Y0 + bdelta of some chip pixel (or its cvRound argument) is not
+ * an int32, or, in a frame wider or taller than 32,767 px, a tap coordinate Xs >> 5 or Ys >> 5 is not an int16 (where cv2
+ * saturates).  Otherwise d_valid is 1. */
+typedef struct {
+    int32_t width, height;          /* chip size in px, >= 1 */
+    int32_t n;                      /* used landmarks, >= 2 */
+    const int32_t* h_landmark;      /* n distinct landmark indices in [0, L) (host) */
+    const double* h_template;       /* n template points (x, y) in chip pixels (host) */
+} sd_face_chip_param;
+/* sd_face_chip_template: host only.  The default template: landmark k = h_landmark[j] (or j for h_landmark == NULL, which takes
+ * n = L) of the model's mean m goes to h_template[2 j] = ((m_x[k] + 0.5 + padding) / (1 + 2 padding)) * width in double, each
+ * operation rounded on its own, and h_template[2 j + 1] alike with m_y and height: align_mean's unit box grown by padding on each
+ * side fills the chip.  Null pointers, width or height < 1, a padding that is not finite or <= -0.5, n < 1 (n != L without
+ * h_landmark) or an index out of range is SD_ERR_INVALID (h_template is not written). */
+SD_API int sd_face_chip_template(const sd_model* m, int width, int height, double padding, int n, const int32_t* h_landmark,
+                                 double* h_template);
+/* sd_face_chips: the aligned chip of each of num_faces faces, asynchronous on the context's stream.  Face i lies in frame
+ * d_face_frame[i] of frames (an sd_hog_images batch of SD_HOG_U8 or SD_HOG_F32 frames with 1..16 channels, in any layout it
+ * describes; its d_frames table, if any, is read back once).  Outputs, in the frames' dtype and as doubles:
+ *   d_chips          num_faces x height x width x channels, contiguous (channels last);
+ *   d_chip_to_frame  num_faces x 6 (M row-major), d_frame_to_chip num_faces x 6, d_valid num_faces bytes.
+ * One status read-back (after the fit, as the tracking step makes): a frame index out of range is SD_ERR_INVALID there, before
+ * any output is written.  Null pointers (the device pointers may be NULL when num_faces = 0), num_faces < 0, num_landmarks < 1,
+ * ldl < 2 num_landmarks, n < 2, a landmark index out of range or listed twice, a chip size below 1, of more than INT32_MAX
+ * pixels or taller than 1,048,560 px, chip bytes that overflow int64, unaligned float, double or landmark pointers, and the frames sd_hog_box_scores_images
+ * refuses (a dtype other than SD_HOG_U8 or SD_HOG_F32, channels outside [1, 16], count < 1, a frame smaller than 1 x 1 or with a
+ * negative offset or stride) are SD_ERR_INVALID before any work is queued, with nothing written.  Each face's results depend on
+ * its own landmarks and frame alone. */
+SD_API int sd_face_chips(sd_ctx* ctx, const sd_hog_images* frames, const int32_t* d_face_frame, const float* d_landmarks, int64_t ldl,
+                         int num_faces, int num_landmarks, const sd_face_chip_param* p, void* d_chips, double* d_chip_to_frame,
+                         double* d_frame_to_chip, uint8_t* d_valid);
+
 #ifdef __cplusplus
 }
 #endif

@@ -56,6 +56,11 @@ class HogImagesC(C.Structure):
                 ("frame", HogImageC), ("image_stride", C.c_int64), ("d_frames", C.c_void_p)]
 
 
+class FaceChipParamC(C.Structure):
+    """sd_face_chip_param: chip size, and the n landmark indices and template points (host) of the fit."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("n", C.c_int32), ("h_landmark", C.c_void_p), ("h_template", C.c_void_p)]
+
+
 class HogPolarFieldsC(C.Structure):
     """sd_hog_polar_fields: f32 modulus and angle fields on the device, one descriptor placing an element in both buffers."""
     _fields_ = [("d_modulus", C.c_void_p), ("d_angle", C.c_void_p), ("count", C.c_int32), ("frame", HogImageC),
@@ -202,6 +207,7 @@ EXPORTS = [
     "sd_detect_batch_device", "sd_detect_batch_host", "sd_detect_faces_host", "sd_detect_faces_device",
     "sd_hog_box_scores", "sd_track_boxes", "sd_track_faces", "sd_track_detect_faces",
     "sd_hog_box_scores_images", "sd_track_faces_images", "sd_track_detect_faces_images", "sd_bgr2gray_images",
+    "sd_face_chip_template", "sd_face_chips",
 ]
 
 _lib = None
@@ -282,6 +288,8 @@ def lib():
         l.sd_track_faces_images.argtypes = l.sd_track_faces.argtypes[:3] + [_vp, _i] + l.sd_track_faces.argtypes[3:]
         l.sd_track_detect_faces_images.argtypes = l.sd_track_detect_faces.argtypes[:3] + [_vp, _i] + l.sd_track_detect_faces.argtypes[3:]
         l.sd_bgr2gray_images.argtypes = [_vp, _vp, _vp, _vp, _vp]
+        l.sd_face_chip_template.argtypes = [_vp, _i, _i, C.c_double, _i, _vp, _vp]
+        l.sd_face_chips.argtypes = [_vp, _vp, _vp, _vp, C.c_int64, _i, _i, C.POINTER(FaceChipParamC), _vp, _vp, _vp, _vp]
         _lib = l
     return _lib
 

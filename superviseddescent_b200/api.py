@@ -26,7 +26,7 @@ import torch
 
 from . import _capi
 from ._capi import HogParam as HoGParam  # same field names as rcr::HoGParam
-from ._capi import FrameC, HogBoxC, HogDetectionC, HogGridC, HogGridsC, HogImageC, HogImagesC, HogPartMapC, HogPartModelC, HogPartPlacementC, HogPolarFieldsC, HogScoreMapC, HogTrainParamC, HogTrainReportC, HogWindowC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, SvmReportC, ptr
+from ._capi import FaceChipParamC, FrameC, HogBoxC, HogDetectionC, HogGridC, HogGridsC, HogImageC, HogImagesC, HogPartMapC, HogPartModelC, HogPartPlacementC, HogPolarFieldsC, HogScoreMapC, HogTrainParamC, HogTrainReportC, HogWindowC, HostFrameC, ImageBatchC, LevelFramesC, NormalisationC, RegulariserC, SdError, SvmReportC, ptr
 
 
 def _check(ctx, rc: int) -> None:
@@ -1681,6 +1681,69 @@ def hog_box_scores(frames, box_frame, boxes, filter, bias: float, cell_size: int
     _check(ctx.h, call(ctx.h, *frames_args, ptr(bf), ptr(bx), n, ptr(f), fw, fh, C.c_float(float(bias)), int(cell_size), int(num_bins),
                        int(variant), ptr(out)))
     return out
+
+
+FaceChips = collections.namedtuple("FaceChips", "chips chip_to_frame frame_to_chip valid")
+FaceChips.__doc__ = """Result of face_chips, CUDA tensors: chips (n, h, w, C) in the frames' dtype (channels last), chip_to_frame and
+frame_to_chip (n, 2, 3) float64 (the fitted similarity [a, -b, tx; b, a, ty] and its inverse) and valid (n,) bool.  An invalid
+face has a zero chip and zero transforms."""
+
+
+def _chip_size(size):
+    w, h = (int(size), int(size)) if np.isscalar(size) else (int(v) for v in size)
+    return w, h
+
+
+def face_chip_template(model: detection_model, size, padding: float = 0.25, landmarks=None) -> np.ndarray:
+    """The default template of face_chips (sd_face_chip_template): landmark k of the model's mean goes to ((m_x[k] + 0.5 +
+    padding) / (1 + 2 padding)) * width, and y alike with height, so align_mean's unit box grown by padding on each side fills a
+    chip of size ((w, h) or one side).  landmarks: the indices to place (default all).  Returns (n, 2) float64."""
+    w, h = _chip_size(size)
+    idx = None if landmarks is None else np.ascontiguousarray(landmarks, dtype=np.int32).ravel()
+    n = model.num_landmarks if idx is None else idx.size
+    out = np.empty((n, 2), dtype=np.float64)
+    rc = _capi.lib().sd_face_chip_template(model._m, w, h, C.c_double(float(padding)), n, None if idx is None else _np_ptr(idx),
+                                           _np_ptr(out))
+    if rc:
+        raise SdError(rc, "sd_face_chip_template: bad arguments (size >= 1, padding > -0.5 and finite, indices in range)")
+    return out
+
+
+def face_chips(frames, face_frame, landmarks, size, template, landmark_index=None, channels_last: bool = False,
+               ctx: Optional[Context] = None) -> FaceChips:
+    """Aligned face chips (sd_face_chips): for face i, the least-squares similarity from template ((n, 2) chip pixels) to its
+    landmarks landmark_index (default all) of landmarks[i] ((N, 2L) float32, [x.., y..]), and the chip of size ((w, h) or one
+    side) cut from frames[face_frame[i]] as cv2.warpAffine(frame, M, (w, h), INTER_LINEAR | WARP_INVERSE_MAP, BORDER_CONSTANT, 0)
+    does, bit for bit.  frames as vl_hog takes them (uint8 or float32, 1..16 channels; CUDA tensors read in place, host frames
+    uploaded once; channels_last for (H, W, C) frames); face_frame and landmarks may be CUDA tensors, e.g. a TrackStep's frame
+    and landmarks.  Returns FaceChips."""
+    ctx = ctx or default_context()
+    dev = f"cuda:{ctx.device}"
+    w, h = _chip_size(size)
+    keep, ib, _ = _hog_images(frames, channels_last, ctx, lambda fw, fh: None)
+    if ib is None:
+        raise ValueError("face_chips needs at least one frame")
+    ff = _dev_int32(face_frame, dev).reshape(-1)
+    x = _dev(landmarks, ctx)
+    if x.dim() != 2 or x.shape[1] % 2 or x.shape[0] != ff.numel():
+        raise ValueError("landmarks must be (N, 2L), one row per entry of face_frame")
+    if x.stride(1) != 1:
+        x = x.contiguous()
+    L = x.shape[1] // 2
+    idx = np.ascontiguousarray(np.arange(L) if landmark_index is None else landmark_index, dtype=np.int32).ravel()
+    tm = np.ascontiguousarray(template, dtype=np.float64)
+    if tm.shape != (idx.size, 2):
+        raise ValueError(f"template must be ({idx.size}, 2), one point per used landmark, got {tm.shape}")
+    n = ff.numel()
+    chips = torch.empty((n, h, w, ib.channels), dtype=torch.uint8 if ib.dtype == _VL_HOG_DTYPES[torch.uint8] else torch.float32,
+                        device=dev)
+    c2f = torch.empty((n, 2, 3), dtype=torch.float64, device=dev)
+    f2c = torch.empty((n, 2, 3), dtype=torch.float64, device=dev)
+    valid = torch.empty(n, dtype=torch.uint8, device=dev)
+    p = FaceChipParamC(w, h, idx.size, _np_ptr(idx), _np_ptr(tm))
+    _check(ctx.h, _capi.lib().sd_face_chips(ctx.h, C.byref(ib), ptr(ff), ptr(x), x.stride(0) if n else 2 * L, n, L, C.byref(p),
+                                            ptr(chips), ptr(c2f), ptr(f2c), ptr(valid)))
+    return FaceChips(chips, c2f, f2c, valid.bool())
 
 
 def load_detection_model(filename: str, ctx: Optional[Context] = None) -> detection_model:

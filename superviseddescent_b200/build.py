@@ -20,7 +20,7 @@ LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libsd_b200.so")
 
-SOURCES = ["sd_api.cu", "sd_hog.cu", "sd_hog_dense.cu", "sd_hog_render.cu", "sd_hog_filters.cu", "sd_hog_detect.cu", "sd_hog_train.cu", "sd_hog_parts.cu", "sd_linalg.cu", "sd_gram_tc.cu", "sd_model.cu", "sd_comm.cu", "sd_rank.cu", "sd_cg.cu", "sd_train.cu", "sd_track.cu"]
+SOURCES = ["sd_api.cu", "sd_hog.cu", "sd_hog_dense.cu", "sd_hog_render.cu", "sd_hog_filters.cu", "sd_hog_detect.cu", "sd_hog_train.cu", "sd_hog_parts.cu", "sd_linalg.cu", "sd_gram_tc.cu", "sd_model.cu", "sd_comm.cu", "sd_rank.cu", "sd_cg.cu", "sd_train.cu", "sd_track.cu", "sd_face_chips.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo",
          "-Xcompiler", "-fPIC,-fvisibility=hidden", "-I", os.path.join(ROOT, "include"), "-I", CSRC]

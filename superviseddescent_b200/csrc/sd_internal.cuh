@@ -35,6 +35,7 @@ enum { SD_WS_GRAM_EXT = 0, SD_WS_FEATURES, SD_WS_SCRATCH, SD_WS_TC_TILES,
        SD_WS_TRACK /* initial and new landmarks, patch flags and box flags of sd_track_faces (sd_track.cu) */,
        SD_WS_TRACK_DETECT /* one slice's pyramid, scores and tables, the detections, the frame groups and the new rows of
                              sd_track_detect_faces (sd_track.cu) */,
+       SD_WS_CHIPS /* per-face fits, the frame table, landmark indices and template of sd_face_chips (sd_face_chips.cu) */,
        SD_WS_COUNT };
 
 // Block-row ownership of the distributed factorisation: the matrix is cut into panels of SD_PANEL_ROWS rows (two 128-row

@@ -4,6 +4,7 @@
 // cereal archives (face_landmarks_model_rcr_22.bin loads unchanged).
 #pragma once
 
+#include <array>
 #include <string>
 #include <vector>
 
@@ -398,6 +399,78 @@ inline void save_detection_model(detection_model model, std::string filename)
 {
     sd_ctx* ctx = sd_b200::context();
     sd_b200::check(ctx, sd_model_save(ctx, model.native(), filename.c_str()), "save_detection_model");
+}
+
+// Aligned face chips (sd_face_chips; the rule is in include/sd_b200.h): chips[i] is cv::warpAffine(images[face_frame[i]], M_i,
+// (chip_width, chip_height), INTER_LINEAR | WARP_INVERSE_MAP, BORDER_CONSTANT, 0), bit for bit, with M_i = chip_to_frame[i] (row-major
+// 2 x 3) the least-squares similarity from the default template (sd_face_chip_template at padding) to landmarks.row(i).
+// frame_to_chip[i] is its inverse, and valid[i] is false for a face the rule calls invalid (a zero chip and zero transforms).
+struct face_chip_set {
+    std::vector<cv::Mat> chips;              // the images' type: CV_8UC1 / CV_8UC3 or CV_32FC1 / CV_32FC3
+    std::vector<std::array<double, 6>> chip_to_frame, frame_to_chip;
+    std::vector<bool> valid;
+};
+
+// images: all CV_8UC1, all CV_8UC3, all CV_32FC1 or all CV_32FC3, of any sizes; landmarks: one 1 x 2L CV_32FC1 row per face
+// (e.g. a track_step's landmarks stacked); landmark_ids: the landmarks to fit, by id (empty: all of the model's).  Throws
+// std::runtime_error where sd_face_chip_template or sd_face_chips refuses.
+inline face_chip_set face_chips(const std::vector<cv::Mat>& images, const std::vector<int>& face_frame, const cv::Mat& landmarks,
+                                const detection_model& model, int chip_width, int chip_height, double padding = 0.25,
+                                const std::vector<std::string>& landmark_ids = {})
+{
+    sd_model* m = model.native();
+    const int L = sd_model_num_landmarks(m), n = static_cast<int>(face_frame.size());
+    if (images.empty()) throw std::runtime_error("face_chips: no frames");
+    if (n > 0 && (landmarks.type() != CV_32FC1 || landmarks.cols != 2 * L || landmarks.rows != n))
+        throw std::runtime_error("face_chips: landmarks must be one 1 x 2L CV_32FC1 row per face");
+    std::vector<int32_t> idx;
+    for (const std::string& id : landmark_ids) {
+        int k = 0;
+        while (k < L && id != sd_model_landmark_id(m, k)) ++k;
+        if (k == L) throw std::runtime_error("face_chips: landmark id " + id + " is not one of the model's");
+        idx.push_back(k);
+    }
+    if (idx.empty())
+        for (int k = 0; k < L; ++k) idx.push_back(k);
+    std::vector<double> tmpl(2 * idx.size());
+    if (sd_face_chip_template(m, chip_width, chip_height, padding, static_cast<int>(idx.size()), idx.data(), tmpl.data()) != SD_OK)
+        throw std::runtime_error("face_chips: sd_face_chip_template refused the chip size, padding or landmarks");
+    sd_ctx* ctx = sd_b200::context();
+    const int type = images[0].type();
+    const bool is_float = type == CV_32FC1 || type == CV_32FC3;
+    sd_b200::DeviceBuffer buf, table;
+    const sd_hog_images frames = is_float ? hog_batch::upload_float_channels(ctx, images, buf, table, "face_chips upload")
+                                          : hog_batch::upload_channels(ctx, images, buf, table, "face_chips upload");
+    const size_t chip_bytes = static_cast<size_t>(chip_width) * chip_height * frames.channels * (is_float ? sizeof(float) : 1);
+    const size_t rows = static_cast<size_t>(n > 0 ? n : 1), P = 2 * static_cast<size_t>(L);
+    sd_b200::DeviceBuffer d_frame(rows * sizeof(int32_t)), d_lms(rows * P * sizeof(float)), d_chips(chip_bytes * rows),
+        d_c2f(rows * 6 * sizeof(double)), d_f2c(rows * 6 * sizeof(double)), d_valid(rows);
+    const std::vector<int32_t> ff(face_frame.begin(), face_frame.end());
+    if (n > 0) {
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_frame.as<int32_t>(), ff.data(), ff.size() * sizeof(int32_t)), "face_chips");
+        sd_b200::check(ctx, sd_memcpy2d_h2d(ctx, d_lms.as<float>(), P * sizeof(float), landmarks.ptr<float>(0), landmarks.step(),
+                                            P * sizeof(float), static_cast<size_t>(n)), "face_chips");
+    }
+    const sd_face_chip_param p{chip_width, chip_height, static_cast<int32_t>(idx.size()), idx.data(), tmpl.data()};
+    sd_b200::check(ctx, sd_face_chips(ctx, &frames, d_frame.as<int32_t>(), d_lms.as<float>(), static_cast<int64_t>(P), n, L, &p,
+                                      d_chips.as<void>(), d_c2f.as<double>(), d_f2c.as<double>(), d_valid.as<uint8_t>()), "sd_face_chips");
+    face_chip_set out;
+    out.chip_to_frame.resize(n);
+    out.frame_to_chip.resize(n);
+    std::vector<uint8_t> valid(n);
+    for (int i = 0; i < n; ++i) {
+        out.chips.emplace_back(chip_height, chip_width, type);
+        sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.chips[i].ptr<unsigned char>(0), d_chips.as<unsigned char>() + chip_bytes * i, chip_bytes),
+                       "face_chips");
+    }
+    if (n > 0) {
+        sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.chip_to_frame.data(), d_c2f.as<double>(), n * 6 * sizeof(double)), "face_chips");
+        sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.frame_to_chip.data(), d_f2c.as<double>(), n * 6 * sizeof(double)), "face_chips");
+        sd_b200::check(ctx, sd_memcpy_d2h(ctx, valid.data(), d_valid.as<uint8_t>(), valid.size()), "face_chips");
+    }
+    sd_b200::check(ctx, sd_sync(ctx), "face_chips");
+    for (int i = 0; i < n; ++i) out.valid.push_back(valid[i] != 0);
+    return out;
 }
 
 }  // namespace rcr
