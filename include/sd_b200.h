@@ -194,6 +194,36 @@ SD_API int sd_hog_debug(sd_ctx* ctx, const sd_image_batch* images, const int32_t
                         uint8_t* d_patches /* N*L*fs*fs or NULL */,
                         int8_t* d_bins /* N*L*fs*fs or NULL, -1 on border / zero gradient */);
 
+/* A sample warp: the sample is a sample of the virtual frame
+ *   V = cv::warpAffine(g, M, (width, height), INTER_LINEAR | WARP_INVERSE_MAP, BORDER_CONSTANT, 0),
+ * g its grey frame, M = m (row-major 2 x 3) mapping V's pixel (u, v) to the frame position (m[0] u + m[1] v + m[2],
+ * m[3] u + m[4] v + m[5]) -- the convention of sd_face_chips' chip_to_frame, whose rows can be used as warps.  Its landmarks are
+ * in V's coordinates.  V is never materialised: each patch's P x P window of V is computed from the frame by cv::warpAffine's
+ * fixed-point rule (10-bit coordinates, 1/32 px taps, 15-bit weights; a tap outside the frame reads 0), and a window pixel
+ * outside [0, width) x [0, height) is 0 (copyMakeBorder on V).  A warp is valid when its six values are finite, width and
+ * height are >= 1, every fixed-point value of every pixel of V fits int32 and, in a frame wider or taller than 32,767 px, every
+ * tap coordinate fits int16 (sd_face_chips' rule on V's corners: cv2's own failure domain). */
+typedef struct {
+    double m[6];
+    int32_t width, height;
+} sd_sample_warp;
+
+/* sd_hog_batch / sd_hog_debug on warped samples: sample i is a sample of the V of d_warp[i] (device memory, one entry per
+ * sample) over its frame images[d_image_index ? d_image_index[i] : i].  Every result -- feature rows, and sd_hog_debug's
+ * centre, half size, resized patch and bins -- is bit for bit what sd_hog_batch / sd_hog_debug give with V passed as a frame of
+ * its own; the identity warp at the frame's size gives the unwarped results.  An invalid warp, and an index carrying
+ * SD_SAMPLE_MIRRORED (the reflection [-1, 0, W - 1; 0, 1, 0] at the frame's size is the mirror), raise the projection's
+ * status flag, reported by the next synchronising call as SD_ERR_INVALID, as an index out of range is.  A batch with d_roi
+ * and a NULL d_warp are SD_ERR_INVALID before any work is queued. */
+SD_API int sd_hog_batch_warped(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index,
+                               const float* d_x, int64_t ldx, int num_samples, int num_landmarks,
+                               const sd_normalisation* eyes, const sd_hog_param* p, const sd_sample_warp* d_warp,
+                               float* d_A, int64_t ld);
+SD_API int sd_hog_debug_warped(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index,
+                               const float* d_x, int64_t ldx, int num_samples, int num_landmarks,
+                               const sd_normalisation* eyes, const sd_hog_param* p, const sd_sample_warp* d_warp,
+                               int32_t* d_geometry, uint8_t* d_patches, int8_t* d_bins);
+
 /* Colour frames: HogTransform::operator() converts 3-channel images with cv::cvtColor(BGR2GRAY) before anything else
  * (adaptive_vlhog.hpp:114-120).  Same conversion on the device, once per frame instead of once per call:
  *   gray = (3735 B + 19235 G + 9798 R + 2^14) >> 15      (OpenCV >= 3 fixed point; SURVEY.md 8c, pinned against cv2)
@@ -929,13 +959,20 @@ SD_API int sd_subtract_templates(sd_ctx* ctx, float* d_A, int64_t lda, const flo
  *     then reads frame 0.  frame | SD_SAMPLE_MIRRORED makes sample i a mirrored sample of the frame (as in sd_hog_batch), on
  *     either route: X, lambda and x_next are bit for bit those of the same call with the mirror passed as a frame of its own.  On
  *     the host route the gather plans the frame's window of a mirrored patch, and samples of one frame, mirrored or not, share
- *     one region of it. */
+ *     one region of it.
+ *   - d_sample_warp (device, N entries, may be NULL = no warp): sample i is a sample of the V of d_sample_warp[i] over its grey
+ *     frame (sd_sample_warp; on the host route colour frames are converted to grey first, so V is the warp of the grey frame),
+ *     on either route: X, lambda and x_next are bit for bit those of the same call with each V passed as a frame of its own.
+ *     With a warp table an index carrying SD_SAMPLE_MIRRORED is out of range, and an invalid warp raises the status flag.  On
+ *     the host route the gather plans a warped patch as the rectangle of frame pixels its taps read (bounded by the window's
+ *     corners: each fixed-point term is monotone), clipped to the frame. */
 typedef struct {
     const sd_image_batch* images;      /* frames resident on the device, or NULL */
     const sd_host_frame* host_frames;  /* frames in pinned host memory, or NULL */
     int32_t num_host_frames;
     const int32_t* d_sample_frame;     /* sample i reads frame d_sample_frame[i]; NULL = frame i, on either route */
     size_t stage_half_bytes;           /* host route: bytes per staging half; 0 = the library's default (48 MB) */
+    const sd_sample_warp* d_sample_warp;   /* sample i reads the V of d_sample_warp[i]; NULL = no warp, on either route */
 } sd_level_frames;
 /* sd_level_chunk_rows: the largest r <= N_local such that r rows of the caller's chunk buffer (r * ld * 4 bytes, with the update's
  * r * M * 8 bytes of partial sums) fit in free_bytes beside everything the level will still allocate with the context's current
@@ -1148,6 +1185,12 @@ SD_API int sd_detect_faces_host(sd_ctx* ctx, const sd_model* m, const sd_host_fr
  * in frame i), so a frame with several faces is resident once.  An index out of range is SD_ERR_INVALID. */
 SD_API int sd_detect_faces_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_face_frame,
                                   const float* d_x0, int num_faces, float* d_landmarks);
+/* sd_detect_faces_device on warped faces: face i is a face of the V of d_warp[i] (sd_sample_warp, device memory, one entry per
+ * face) over images[d_face_frame[i]] (d_face_frame may be NULL: frame i), and d_x0 / d_landmarks are in V's coordinates.  The
+ * landmarks are bit for bit sd_detect_faces_device's with each V passed as a frame of its own.  Refusals: detect's, a NULL
+ * d_warp or a batch with d_roi before any work is queued, and an invalid warp as an index out of range. */
+SD_API int sd_detect_faces_device_warped(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_face_frame,
+                                         const sd_sample_warp* d_warp, const float* d_x0, int num_faces, float* d_landmarks);
 
 /* ---- face tracking: one step of rcr-track's loop on the device ---------------------------------------------------------------
  * sd_track_boxes: the face box of a set of landmarks, the inverse of align_mean at scaling 1 and translation 0.  For row t of

@@ -155,10 +155,16 @@ class HostFrameC(C.Structure):
     _fields_ = [("h_data", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32), ("row_stride", C.c_int32), ("channels", C.c_int32)]
 
 
+class SampleWarpC(C.Structure):
+    """sd_sample_warp: a sample's V-to-frame matrix (row-major 2 x 3) and V's size."""
+    _fields_ = [("m", C.c_double * 6), ("width", C.c_int32), ("height", C.c_int32)]
+
+
 class LevelFramesC(C.Structure):
-    """sd_level_frames: where a cascade level's frames are (a device batch or host frames) and which frame each sample reads."""
+    """sd_level_frames: where a cascade level's frames are (a device batch or host frames), which frame each sample reads and,
+    optionally, each sample's warp."""
     _fields_ = [("images", C.POINTER(ImageBatchC)), ("host_frames", C.POINTER(HostFrameC)), ("num_host_frames", C.c_int32),
-                ("d_sample_frame", C.c_void_p), ("stage_half_bytes", C.c_size_t)]
+                ("d_sample_frame", C.c_void_p), ("stage_half_bytes", C.c_size_t), ("d_sample_warp", C.c_void_p)]
 
 
 # sd_project_fn(user, ctx, level, d_x, ldx, first_row, rows, d_out, ld) -> 0 or non-zero
@@ -186,7 +192,7 @@ EXPORTS = [
     "sd_ctx_create", "sd_ctx_destroy", "sd_last_error", "sd_sync", "sd_ctx_stream", "sd_version", "sd_launch_count", "sd_roi_fallback_count",
     "sd_malloc", "sd_free", "sd_host_alloc", "sd_host_free", "sd_memcpy_h2d", "sd_memcpy_d2h", "sd_memset",
     "sd_memcpy2d_h2d", "sd_memcpy2d_d2h", "sd_memcpy2d_d2d",
-    "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_bgr2gray", "sd_upload_frames", "sd_hog_dense_shape", "sd_hog_dense",
+    "sd_hog_feature_length", "sd_hog_batch", "sd_hog_debug", "sd_hog_batch_warped", "sd_hog_debug_warped", "sd_bgr2gray", "sd_upload_frames", "sd_hog_dense_shape", "sd_hog_dense",
     "sd_hog_dense_images", "sd_hog_dense_polar", "sd_hog_permutation", "sd_hog_glyphs", "sd_hog_render", "sd_hog_relayout",
     "sd_hog_pyramid_shape", "sd_hog_pyramid", "sd_hog_pyramid_images", "sd_hog_pyramid_float", "sd_hog_correlate", "sd_hog_detections",
     "sd_hog_windows", "sd_hog_box_windows", "sd_learn_squared_hinge", "sd_hog_train_filter", "sd_hog_train_filter_images",
@@ -204,7 +210,7 @@ EXPORTS = [
     "sd_model_num_landmarks", "sd_model_hog_param", "sd_model_regulariser", "sd_model_normalisation",
     "sd_model_get_mean", "sd_model_get_weights", "sd_model_landmark_id", "sd_align_mean",
     "sd_perturb_box", "sd_normalised_landmark_errors",
-    "sd_detect_batch_device", "sd_detect_batch_host", "sd_detect_faces_host", "sd_detect_faces_device",
+    "sd_detect_batch_device", "sd_detect_batch_host", "sd_detect_faces_host", "sd_detect_faces_device", "sd_detect_faces_device_warped",
     "sd_hog_box_scores", "sd_track_boxes", "sd_track_faces", "sd_track_detect_faces",
     "sd_hog_box_scores_images", "sd_track_faces_images", "sd_track_detect_faces_images", "sd_bgr2gray_images",
     "sd_face_chip_template", "sd_face_chips",

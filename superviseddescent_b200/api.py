@@ -626,6 +626,78 @@ class _PinnedBuffer:
 # sd_level_frames / sd_hog_batch: OR-ed into a sample's frame index, the sample is a sample of the frame's left-right mirror
 SAMPLE_MIRRORED = 1 << 30
 
+# sd_sample_warp as a numpy record (56 bytes, the C layout)
+_WARP_DTYPE = np.dtype([("m", "<f8", (6,)), ("width", "<i4"), ("height", "<i4")])
+
+
+def _warp_table(warps, warp_sizes, frame_sizes, dev) -> torch.Tensor:
+    """(N, 2, 3) V-to-frame matrices and (N, 2) (Wv, Hv) sizes (default: frame_sizes, the (N, 2) sizes of each sample's frame,
+    or None when they are not known) -> the device table of N sd_sample_warp records, as bytes."""
+    m = np.asarray(warps.cpu() if isinstance(warps, torch.Tensor) else warps, dtype=np.float64)
+    if m.ndim != 3 or m.shape[1:] != (2, 3):
+        raise ValueError(f"warps must be (N, 2, 3), got {m.shape}")
+    n = m.shape[0]
+    if warp_sizes is None:
+        if frame_sizes is None:
+            raise ValueError("warp_sizes is needed: the frames' sizes are not known here")
+        warp_sizes = frame_sizes
+    sz = np.asarray(warp_sizes.cpu() if isinstance(warp_sizes, torch.Tensor) else warp_sizes, dtype=np.int64)
+    sz = np.broadcast_to(sz, (n, 2)) if sz.shape == (2,) else sz
+    if sz.shape != (n, 2):
+        raise ValueError(f"warp_sizes must be (N, 2) (Wv, Hv) for {n} warps, got {sz.shape}")
+    rec = np.zeros(n, dtype=_WARP_DTYPE)
+    rec["m"] = m.reshape(n, 6)
+    rec["width"], rec["height"] = np.clip(sz[:, 0], -2 ** 31, 2 ** 31 - 1), np.clip(sz[:, 1], -2 ** 31, 2 ** 31 - 1)
+    return torch.from_numpy(rec.view(np.uint8).copy()).to(dev)
+
+
+def rotation_warp(centre, angle: float, scale: float = 1.0) -> np.ndarray:
+    """The V-to-frame matrix (2 x 3 float64) whose V is the frame rotated by angle degrees about centre and scaled by scale:
+    the inverse of cv2.getRotationMatrix2D(centre, angle, scale) (angle counter-clockwise, as cv2), in closed form.  Its V is
+    what cv2.warpAffine(frame, cv2.getRotationMatrix2D(centre, angle, scale), size) gives."""
+    cx, cy = float(centre[0]), float(centre[1])
+    a = math.radians(float(angle))
+    alpha, beta = math.cos(a) * float(scale), math.sin(a) * float(scale)
+    # getRotationMatrix2D: [[alpha, beta, (1 - alpha) cx - beta cy], [-beta, alpha, beta cx + (1 - alpha) cy]]
+    return invert_warp(np.array([[alpha, beta, (1 - alpha) * cx - beta * cy], [-beta, alpha, beta * cx + (1 - alpha) * cy]]))
+
+
+def invert_warp(M) -> np.ndarray:
+    """The exact algebraic inverse, in float64, of one (2, 3) affine matrix or of each of (N, 2, 3)."""
+    m = np.asarray(M, dtype=np.float64)
+    if m.shape[-2:] != (2, 3) or m.ndim not in (2, 3):
+        raise ValueError(f"invert_warp: M must be (2, 3) or (N, 2, 3), got {m.shape}")
+    a, b, c, d, e, f = (m[..., i // 3, i % 3] for i in range(6))
+    det = a * e - b * d
+    if np.any(det == 0) or not np.all(np.isfinite(det)):
+        raise ValueError("invert_warp: a matrix is singular or not finite")
+    ia, ib, id_, ie = e / det, -b / det, -d / det, a / det
+    out = np.empty_like(m)
+    out[..., 0, 0], out[..., 0, 1], out[..., 0, 2] = ia, ib, -(ia * c + ib * f)
+    out[..., 1, 0], out[..., 1, 1], out[..., 1, 2] = id_, ie, -(id_ * c + ie * f)
+    return out
+
+
+def warp_landmarks(x, M) -> np.ndarray:
+    """Landmarks x ((N, 2L) rows [x.., y..], or one (2L,) row) mapped through one (2, 3) matrix or one per row ((N, 2, 3)), in
+    float64, returned as float32: ground truth into a warp's V with invert_warp(warp), results back to the frame with the warp."""
+    x = np.asarray(x, dtype=np.float32)
+    single = x.ndim == 1
+    x = np.atleast_2d(x)
+    m = np.asarray(M, dtype=np.float64)
+    L = x.shape[1] // 2
+    if x.ndim != 2 or x.shape[1] != 2 * L or L < 1:
+        raise ValueError("warp_landmarks: x must be (N, 2L) or (2L,)")
+    if m.shape == (2, 3):
+        m = np.broadcast_to(m, (x.shape[0], 2, 3))
+    if m.shape != (x.shape[0], 2, 3):
+        raise ValueError(f"warp_landmarks: M must be (2, 3) or ({x.shape[0]}, 2, 3), got {m.shape}")
+    px, py = x[:, :L].astype(np.float64), x[:, L:].astype(np.float64)
+    out = np.empty_like(x)
+    out[:, :L] = m[:, 0, 0:1] * px + m[:, 0, 1:2] * py + m[:, 0, 2:3]
+    out[:, L:] = m[:, 1, 0:1] * px + m[:, 1, 1:2] * py + m[:, 1, 2:3]
+    return out[0] if single else out
+
 
 class HogTransform:
     """Projection functor h.  images: (count, H, W) uint8 (8UC1) or (count, H, W, 3) uint8 (8UC3, B G R: converted
@@ -637,7 +709,10 @@ class HogTransform:
     (default: sample i reads images[i]).  mirrored (optional, N bools, one per sample as image_index): sample i is a sample of the
     left-right mirror of its frame (np.fliplr, cv::flip(f, 1)), with its landmarks in the mirror's coordinates (mirror_landmarks);
     the frame is still held once and read right to left, and every row is bit for bit that of the mirror passed as a frame of
-    its own.  The flags hold wherever the transform's sample map is used: __call__ and debug without a training_index, into
+    its own.  warps (optional, (N, 2, 3) float64, one per sample as mirrored; not with mirrored): sample i is a sample of
+    V_i = cv2.warpAffine(grey frame, warps[i], warp_sizes[i], INTER_LINEAR | WARP_INVERSE_MAP) (sd_sample_warp; rotation_warp),
+    with its landmarks in V_i's coordinates; V_i is never built, and every row is bit for bit that of V_i passed as a frame of its
+    own.  warp_sizes ((N, 2) (Wv, Hv)) defaults to each sample's frame size.  The flags and warps hold wherever the transform's sample map is used: __call__ and debug without a training_index, into
     without an image_index, and the optimiser's train / test / predict.  Host frames whose grey bytes fit in DEVICE_FRAME_SHARE of the free device memory are
     uploaded when the transform is first used; larger sets stay in host memory and the optimiser gathers them level by level.
     Frames the levels can read in place (pinned and aligned, sd_host_frame_in_place) are read at every level, so changing them
@@ -652,7 +727,7 @@ class HogTransform:
 
     def __init__(self, images, hog_params: Sequence[HoGParam], model_landmarks_list: Sequence[str],
                  right_eye_identifiers: Sequence[str], left_eye_identifiers: Sequence[str], ctx: Optional[Context] = None,
-                 image_index=None, mirrored=None):
+                 image_index=None, mirrored=None, warps=None, warp_sizes=None):
         self.ctx = ctx or default_context()
         self.hog_params = list(hog_params)
         self.norm = InterEyeDistanceNormalisation(model_landmarks_list, right_eye_identifiers, left_eye_identifiers)
@@ -674,9 +749,21 @@ class HogTransform:
             sample = (self._list_frame[idx] if self._list_frame is not None else idx).astype(np.int32)
         else:
             sample = self._list_frame
+        n_samples = idx.size if image_index is not None else n_list
+        if mirrored is not None and warps is not None:
+            raise ValueError("HogTransform: mirrored and warps exclude each other (a mirror is the warp [-1, 0, W - 1; 0, 1, 0])")
+        self._sample_warp = None
+        if warps is not None:
+            base = sample if sample is not None else np.arange(n_samples, dtype=np.int32)
+            if self._frames is not None:
+                fsz = np.array([(r.width, r.height) for r, _ in self._frames], dtype=np.int64)[base]
+            else:
+                fsz = None if self._batch.d_frames else np.array([(self._batch.width, self._batch.height)] * n_samples, dtype=np.int64)
+            if len(np.asarray(warps.cpu() if isinstance(warps, torch.Tensor) else warps)) != n_samples:
+                raise ValueError(f"warps has {len(warps)} entries for {n_samples} samples")
+            self._sample_warp = _warp_table(warps, warp_sizes, fsz, f"cuda:{self.ctx.device}")
         if mirrored is not None:
             flags = np.ascontiguousarray(mirrored, dtype=bool).ravel()
-            n_samples = idx.size if image_index is not None else n_list
             if flags.size != n_samples:
                 raise ValueError(f"mirrored has {flags.size} entries for {n_samples} samples")
             base = sample if sample is not None else np.arange(n_samples, dtype=np.int32)
@@ -752,30 +839,47 @@ class HogTransform:
         """The sd_level_frames of n samples for sd_train_level / sd_apply_level: the device batch or the host frames, and the
         sample -> frame index.  It holds references to what it points at."""
         index = self.sample_frame(n)
-        f = LevelFramesC(d_sample_frame=ptr(index), stage_half_bytes=HOST_STAGE_HALF)
+        warp = self.sample_warp(n)
+        f = LevelFramesC(d_sample_frame=ptr(index), stage_half_bytes=HOST_STAGE_HALF, d_sample_warp=ptr(warp))
         if self.on_device():
             f.images = C.pointer(self._batch)
         else:
             f.host_frames, f.num_host_frames = self._host[0], len(self._host[0])
-        f.keep = (index, self._batch, self._host)
+        f.keep = (index, warp, self._batch, self._host)
         return f
+
+    def sample_warp(self, n: int) -> Optional[torch.Tensor]:
+        """The device table of the first n samples' sd_sample_warp records, as bytes (None: no warps)."""
+        if self._sample_warp is None:
+            return None
+        if n * _WARP_DTYPE.itemsize > self._sample_warp.numel():
+            raise ValueError(f"{n} samples but warps has {self._sample_warp.numel() // _WARP_DTYPE.itemsize}")
+        return self._sample_warp[:n * _WARP_DTYPE.itemsize]
 
     def feature_length(self, level: int) -> int:
         return _capi.lib().sd_hog_feature_length(self.num_landmarks, C.byref(self.hog_params[level]))
 
     def into(self, parameters: torch.Tensor, level: int, out: torch.Tensor, image_index: Optional[torch.Tensor] = None):
         """Writes the feature rows into out[:, :D] (out may be wider: extended [A | b] operand).  image_index: frames of batch()
-        (default: sample_frame)."""
+        (default: sample_frame, with the samples' warps)."""
+        n = parameters.shape[0]
+        warp = self.sample_warp(n) if image_index is None else None
+        if image_index is None:
+            image_index = self.sample_frame(n)
+        self._into(parameters, level, out, image_index, warp)
+
+    def _into(self, parameters: torch.Tensor, level: int, out: torch.Tensor, image_index, warp):
         ctx = self.ctx
         n = parameters.shape[0]
         eyes = self.norm.c()
         ib = self.batch()
-        if image_index is None:
-            image_index = self.sample_frame(n)
         idx_ptr = ptr(image_index) if image_index is not None else C.c_void_p(0)
-        _check(ctx.h, _capi.lib().sd_hog_batch(ctx.h, C.byref(ib), idx_ptr, ptr(parameters), C.c_int64(parameters.stride(0)),
-                                               n, self.num_landmarks, C.byref(eyes), C.byref(self.hog_params[level]),
-                                               ptr(out), C.c_int64(out.stride(0))))
+        args = (ctx.h, C.byref(ib), idx_ptr, ptr(parameters), C.c_int64(parameters.stride(0)), n, self.num_landmarks, C.byref(eyes),
+                C.byref(self.hog_params[level]))
+        if warp is not None:
+            _check(ctx.h, _capi.lib().sd_hog_batch_warped(*args, ptr(warp), ptr(out), C.c_int64(out.stride(0))))
+        else:
+            _check(ctx.h, _capi.lib().sd_hog_batch(*args, ptr(out), C.c_int64(out.stride(0))))
 
     def _frame_index(self, training_index, n: int, single: bool, device) -> Optional[torch.Tensor]:
         """training_index (indices into images) -> frames of batch()"""
@@ -794,9 +898,10 @@ class HogTransform:
         if single:
             x = x.reshape(1, -1)
         idx = self._frame_index(training_index, x.shape[0], single, x.device)
+        warp = self.sample_warp(x.shape[0]) if training_index is None and not single else None
         D = self.feature_length(regressor_level)
         out = torch.empty((x.shape[0], D), dtype=torch.float32, device=x.device)
-        self.into(x, regressor_level, out, idx)
+        self._into(x, regressor_level, out, idx, warp)
         return out[0] if single else out
 
     def debug(self, parameters, level: int, training_index=None):
@@ -811,10 +916,14 @@ class HogTransform:
         patches = torch.empty((n, L, fs, fs), dtype=torch.uint8, device=x.device)
         bins = torch.empty((n, L, fs, fs), dtype=torch.int8, device=x.device)
         idx = self._frame_index(training_index, n, False, x.device)
+        warp = self.sample_warp(n) if training_index is None else None
         eyes = self.norm.c()
         ib = self.batch()
-        _check(ctx.h, _capi.lib().sd_hog_debug(ctx.h, C.byref(ib), ptr(idx), ptr(x), C.c_int64(x.stride(0)), n, L,
-                                               C.byref(eyes), C.byref(p), ptr(geo), ptr(patches), ptr(bins)))
+        args = (ctx.h, C.byref(ib), ptr(idx), ptr(x), C.c_int64(x.stride(0)), n, L, C.byref(eyes), C.byref(p))
+        if warp is not None:
+            _check(ctx.h, _capi.lib().sd_hog_debug_warped(*args, ptr(warp), ptr(geo), ptr(patches), ptr(bins)))
+        else:
+            _check(ctx.h, _capi.lib().sd_hog_debug(*args, ptr(geo), ptr(patches), ptr(bins)))
         return geo, patches, bins
 
 
@@ -1382,12 +1491,19 @@ class detection_model:
             return self.detect_faces([image], [0], boxes=arg.reshape(1, 4))[0]
         return self.detect_faces([image], [0], initialisations=arg.reshape(1, -1))[0]
 
-    def detect_faces(self, frames, face_frame, boxes=None, initialisations=None) -> np.ndarray:
+    def detect_faces(self, frames, face_frame, boxes=None, initialisations=None, warps=None, warp_sizes=None) -> np.ndarray:
         """detect(image, facebox) / detect(image, initialisation) for any number of faces in host frames of any sizes
         (sd_detect_faces_host).  frames: a sequence of (H, W) grey or (H, W, 3) B,G,R uint8 numpy arrays or CPU tensors; face i
         lies in frames[face_frame[i]].  Give exactly one of boxes ((F, 4): x, y, w, h) and initialisations ((F, 2L), e.g. the
         previous video frame's landmarks).  A row pitch other than the row's bytes (strides[0]) is honoured; pinned frames with
-        16-byte aligned rows take the zero-copy region-of-interest route.  Returns (F, 2L) landmarks in the order of face_frame."""
+        16-byte aligned rows take the zero-copy region-of-interest route.  Returns (F, 2L) landmarks in the order of face_frame.
+
+        warps ((F, 2, 3) float64, optional): face i is a face of V_i = cv2.warpAffine(grey frame, warps[i], warp_sizes[i],
+        INTER_LINEAR | WARP_INVERSE_MAP) (default size: its frame's); boxes, initialisations and the landmarks are in V_i's
+        coordinates, bit for bit detect on V_i.  The referenced frames are uploaded once (sd_upload_frames) and the warped device
+        entry runs (sd_detect_faces_device_warped); V_i is never built."""
+        if warps is not None:
+            return self._detect_faces_warped(frames, face_frame, boxes, initialisations, warps, warp_sizes)
         recs, keep = [], []
         for f in frames:
             rec, a = _host_frame(f)
@@ -1403,6 +1519,38 @@ class detection_model:
         _check(self.ctx.h, _capi.lib().sd_detect_faces_host(self.ctx.h, self._m, table, len(recs), _np_ptr(idx), n, _np_ptr(b),
                                                             _np_ptr(x0), _np_ptr(out)))
         return out
+
+    def _detect_faces_warped(self, frames, face_frame, boxes, initialisations, warps, warp_sizes) -> np.ndarray:
+        idx = np.ascontiguousarray(face_frame, dtype=np.int64).ravel()
+        n = idx.size
+        P = 2 * self.num_landmarks
+        if (boxes is None) == (initialisations is None):
+            raise ValueError("detect_faces: give exactly one of boxes and initialisations")
+        if n == 0:
+            return np.empty((0, P), dtype=np.float32)
+        if idx.min() < 0 or idx.max() >= len(frames):
+            raise ValueError("detect_faces: a face refers to a frame that is not in the list")
+        used = np.unique(idx)
+        recs, keep = _host_frames([frames[f] for f in used])
+        dev, ib = _upload_host_frames(recs, self.ctx)
+        local = np.searchsorted(used, idx).astype(np.int32)
+        if initialisations is None:
+            mean = self.get_mean()
+            x0 = np.stack([align_mean(mean, b) for b in np.asarray(boxes, dtype=np.int64).reshape(n, 4)])
+        else:
+            x0 = np.ascontiguousarray(initialisations, dtype=np.float32).reshape(n, P)
+        sizes = np.array([(recs[k].width, recs[k].height) for k in local], dtype=np.int64)
+        d = f"cuda:{self.ctx.device}"
+        table = _warp_table(warps, warp_sizes, sizes, d)
+        if table.numel() != n * _WARP_DTYPE.itemsize:
+            raise ValueError(f"warps has {table.numel() // _WARP_DTYPE.itemsize} entries for {n} faces")
+        fi = torch.from_numpy(local).to(d)
+        xd = torch.from_numpy(np.ascontiguousarray(x0, dtype=np.float32)).to(d)
+        out = torch.empty((n, P), dtype=torch.float32, device=d)
+        _check(self.ctx.h, _capi.lib().sd_detect_faces_device_warped(self.ctx.h, self._m, C.byref(ib), ptr(fi), ptr(table), ptr(xd), n,
+                                                                     ptr(out)))
+        del dev, keep
+        return out.cpu().numpy()
 
     def detect_batch(self, images: np.ndarray, boxes: np.ndarray) -> np.ndarray:
         """Batched detect(image, facebox) with HOST buffers (copies are part of the call): (count, H, W) grey or
@@ -1422,14 +1570,23 @@ class detection_model:
                                                             out.ctypes.data_as(C.c_void_p)))
         return out
 
-    def detect_batch_device(self, images: torch.Tensor, x0: torch.Tensor, image_index=None) -> torch.Tensor:
+    def detect_batch_device(self, images: torch.Tensor, x0: torch.Tensor, image_index=None, warps=None, warp_sizes=None) -> torch.Tensor:
         """Batched detect(image, initialisation), frames and landmarks already resident in HBM.  Face i starts from x0[i] and
-        lies in images[image_index[i]] (default: images[i]), so a frame with several faces is resident once."""
+        lies in images[image_index[i]] (default: images[i]), so a frame with several faces is resident once.  warps ((n, 2, 3)
+        float64, optional; warp_sizes (n, 2), default the frames' size): face i is a face of the V of warps[i] as in detect_faces,
+        x0 and the result in V's coordinates."""
         n = x0.shape[0]
         h, w = images.shape[1], images.shape[2]
         ib = ImageBatchC(C.c_void_p(images.data_ptr()), w, h, images.stride(1), images.stride(0), images.shape[0])
         idx = None if image_index is None else torch.as_tensor(image_index, dtype=torch.int32).to(images.device).contiguous()
         out = torch.empty((n, 2 * self.num_landmarks), dtype=torch.float32, device=images.device)
+        if warps is not None:
+            table = _warp_table(warps, warp_sizes, np.array([(w, h)] * n, dtype=np.int64), images.device)
+            if table.numel() != n * _WARP_DTYPE.itemsize:
+                raise ValueError(f"warps has {table.numel() // _WARP_DTYPE.itemsize} entries for {n} faces")
+            _check(self.ctx.h, _capi.lib().sd_detect_faces_device_warped(self.ctx.h, self._m, C.byref(ib), ptr(idx), ptr(table), ptr(x0),
+                                                                         n, ptr(out)))
+            return out
         _check(self.ctx.h, _capi.lib().sd_detect_faces_device(self.ctx.h, self._m, C.byref(ib), ptr(idx), ptr(x0), n, ptr(out)))
         return out
 

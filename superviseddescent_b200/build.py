@@ -36,7 +36,7 @@ def _stale(target: str, deps) -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(LIBDIR, exist_ok=True)
     os.makedirs(OBJDIR, exist_ok=True)
-    headers = [os.path.join(CSRC, "sd_internal.cuh"), os.path.join(CSRC, "sd_hog_common.cuh"), os.path.join(ROOT, "include", "sd_b200.h")]
+    headers = [os.path.join(CSRC, "sd_internal.cuh"), os.path.join(CSRC, "sd_hog_common.cuh"), os.path.join(CSRC, "sd_warp.cuh"), os.path.join(ROOT, "include", "sd_b200.h")]
     jobs = []
     objs = []
     for src in SOURCES:

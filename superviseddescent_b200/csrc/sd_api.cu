@@ -82,6 +82,7 @@ int sd_check_hog_status(sd_ctx* ctx, const char* what)
     if (st) {
         SD_CUDA(ctx, cudaMemsetAsync(d, 0, sizeof(int), ctx->stream));
         if (st & 2) return sd_fail(ctx, SD_ERR_INVALID, "%s: image index out of range", what);
+        if (st & 4) return sd_fail(ctx, SD_ERR_INVALID, "%s: invalid sample warp (not finite, empty, or past cv::warpAffine's range)", what);
         if (st & 1) return sd_fail(ctx, SD_ERR_INVALID, "%s: empty HOG patch (inter-eye distance too small)", what);
     }
     return SD_OK;

@@ -6,6 +6,7 @@
 #include <cstring>
 
 #include "sd_internal.cuh"
+#include "sd_warp.cuh"
 
 namespace {
 
@@ -18,43 +19,6 @@ struct ChipFit {
     double m[6], inv[6];
     int32_t valid, frame;
 };
-
-// cvRound of v as an int64 when it fits int32, else false (NaN and infinities included)
-__device__ __forceinline__ bool round_int32(double v, long long* out)
-{
-    const double r = rint(v);
-    if (!(r >= (double)INT32_MIN && r <= (double)INT32_MAX)) return false;
-    *out = (long long)r;
-    return true;
-}
-
-__device__ __forceinline__ bool in_int32(long long v) { return v >= INT32_MIN && v <= INT32_MAX; }
-
-// Whether every fixed-point value of the warp of a w x h chip under M fits int32 and, for a frame wider or taller than 32,767 px,
-// every tap coordinate fits int16.  Each term is monotone in its own variable, so the corners X in {0, w - 1}, Y in {0, h - 1}
-// bound them all.
-__device__ bool chip_fits(const double* m, int w, int h, bool int16_taps)
-{
-    long long ad[2], bd[2], x0[2], y0[2];
-    for (int k = 0; k < 2; ++k) {
-        const double X = k ? (double)(w - 1) : 0.0, Y = k ? (double)(h - 1) : 0.0;
-        if (!round_int32(__dmul_rn(__dmul_rn(m[0], X), 1024.0), &ad[k]) ||
-            !round_int32(__dmul_rn(__dmul_rn(m[3], X), 1024.0), &bd[k]) ||
-            !round_int32(__dmul_rn(__dadd_rn(__dmul_rn(m[1], Y), m[2]), 1024.0), &x0[k]) ||
-            !round_int32(__dmul_rn(__dadd_rn(__dmul_rn(m[4], Y), m[5]), 1024.0), &y0[k]))
-            return false;
-        x0[k] += 16;
-        y0[k] += 16;
-        if (!in_int32(x0[k]) || !in_int32(y0[k])) return false;
-    }
-    for (int i = 0; i < 2; ++i)
-        for (int j = 0; j < 2; ++j) {
-            const long long sx = x0[i] + ad[j], sy = y0[i] + bd[j];
-            if (!in_int32(sx) || !in_int32(sy)) return false;
-            if (int16_taps && ((sx >> 10) < -32768 || (sx >> 10) > 32767 || (sy >> 10) < -32768 || (sy >> 10) > 32767)) return false;
-        }
-    return true;
-}
 
 __global__ void __launch_bounds__(kFitThreads) face_chip_fit_kernel(
     const int32_t* __restrict__ face_frame, const float* __restrict__ landmarks, int64_t ldl, int num_faces, int L,
@@ -98,7 +62,7 @@ __global__ void __launch_bounds__(kFitThreads) face_chip_fit_kernel(
         const double ty = __dsub_rn(my, __dadd_rn(__dmul_rn(b, ux), __dmul_rn(a, uy)));
         const double m[6] = {a, -b, tx, b, a, ty};
         const sd_hog_image& fr = frames[f];
-        if (s != 0 && chip_fits(m, w, h, fr.width > 32767 || fr.height > 32767)) {
+        if (s != 0 && sd_warp_fits(m, w, h, fr.width > 32767 || fr.height > 32767)) {
             const double ia = __ddiv_rn(a, s), ib = __ddiv_rn(b, s);
             const double inv[6] = {ia, ib, -__dadd_rn(__dmul_rn(ia, tx), __dmul_rn(ib, ty)),
                                    -ib, ia, __dsub_rn(__dmul_rn(ib, tx), __dmul_rn(ia, ty))};
@@ -115,22 +79,6 @@ __device__ __forceinline__ T tap(const T* __restrict__ src, const sd_hog_image& 
 {
     if (x < 0 || y < 0 || x >= fr.width || y >= fr.height) return T(0);
     return __ldg(src + fr.offset + (int64_t)y * fr.row_stride + (int64_t)x * fr.pixel_stride + (int64_t)c * fr.channel_stride);
-}
-
-__device__ __forceinline__ uint8_t blend(uint8_t s00, uint8_t s01, uint8_t s10, uint8_t s11, int fx, int fy)
-{
-    const int acc = (int)s00 * ((32 - fx) * (32 - fy) * 32) + (int)s01 * (fx * (32 - fy) * 32) + (int)s10 * ((32 - fx) * fy * 32) +
-                    (int)s11 * (fx * fy * 32);
-    return (uint8_t)min((acc + (1 << 14)) >> 15, 255);
-}
-
-__device__ __forceinline__ float blend(float s00, float s01, float s10, float s11, int fx, int fy)
-{
-    const float wx1 = fx * (1.0f / 32), wy1 = fy * (1.0f / 32), wx0 = 1.0f - wx1, wy0 = 1.0f - wy1;   // exact
-    float v = __fmul_rn(s00, __fmul_rn(wx0, wy0));
-    v = __fadd_rn(v, __fmul_rn(s01, __fmul_rn(wx1, wy0)));
-    v = __fadd_rn(v, __fmul_rn(s10, __fmul_rn(wx0, wy1)));
-    return __fadd_rn(v, __fmul_rn(s11, __fmul_rn(wx1, wy1)));
 }
 
 // CTA (tile x, tile y, face f0 + z): the tile's kTileH rows x kTileW columns x C channels of the chip, each output row of the tile
@@ -153,16 +101,18 @@ __global__ void __launch_bounds__(kWarpThreads) face_chip_warp_kernel(
         else valid[face] = (uint8_t)fit.valid;
     }
     if (ok) {
-        // the per-column and per-row terms, once per tile (valid faces fit int32: chip_fits)
+        // the per-column and per-row terms, once per tile (valid faces fit int32: sd_warp_fits)
         if (threadIdx.x < kTileW && threadIdx.x < tw) {
             const double X = (double)(tx0 + threadIdx.x);
-            s_ad[threadIdx.x] = (int)__double2ll_rn(__dmul_rn(__dmul_rn(fit.m[0], X), 1024.0));
-            s_bd[threadIdx.x] = (int)__double2ll_rn(__dmul_rn(__dmul_rn(fit.m[3], X), 1024.0));
+            const int2 d = sd_warp_col(fit.m, X);
+            s_ad[threadIdx.x] = d.x;
+            s_bd[threadIdx.x] = d.y;
         } else if (threadIdx.x >= 128 && threadIdx.x - 128 < th) {
             const int r = threadIdx.x - 128;
             const double Y = (double)(ty0 + r);
-            s_x0[r] = (int)__double2ll_rn(__dmul_rn(__dadd_rn(__dmul_rn(fit.m[1], Y), fit.m[2]), 1024.0)) + 16;
-            s_y0[r] = (int)__double2ll_rn(__dmul_rn(__dadd_rn(__dmul_rn(fit.m[4], Y), fit.m[5]), 1024.0)) + 16;
+            const int2 t = sd_warp_row(fit.m, Y);
+            s_x0[r] = t.x;
+            s_y0[r] = t.y;
         }
         __syncthreads();
     }
@@ -174,9 +124,7 @@ __global__ void __launch_bounds__(kWarpThreads) face_chip_warp_kernel(
         T v = T(0);
         if (ok) {
             const int sx = (s_x0[r] + s_ad[col]) >> 5, sy = (s_y0[r] + s_bd[col]) >> 5;
-            const int x = sx >> 5, y = sy >> 5;
-            v = blend(tap(src, fr, x, y, c), tap(src, fr, x + 1, y, c), tap(src, fr, x, y + 1, c), tap(src, fr, x + 1, y + 1, c),
-                      sx & 31, sy & 31);
+            v = sd_warp_sample<T>(sx, sy, [&](int x, int y) { return tap(src, fr, x, y, c); });
         }
         out[(size_t)r * w * C + q] = v;
     }

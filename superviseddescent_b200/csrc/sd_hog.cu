@@ -22,8 +22,10 @@
 // (fixed, deterministic tree here; raster order there): ~1e-7 relative.
 #include "sd_internal.cuh"
 #include "sd_hog_common.cuh"
+#include "sd_warp.cuh"
 
 #include <cmath>
+#include <type_traits>
 #include <cuda_pipeline.h>
 
 namespace {
@@ -62,10 +64,20 @@ struct HogArgs {
 //      (INTER_LINEAR, 8U, 11-bit fixed point) for a P x P -> fs x fs resize, once per sample instead of once per thread of
 //      every one of its L patches.  One CTA per sample.  rtab[sample][0..4][fs]: x source index, x weights (2 x int16),
 //      y source index 0 / 1 (clamped), y weights (hog_resize_tap).  face_flag (optional): a degenerate sample also sets its
-//      own byte, so that a caller can drop that face alone (sd_track_faces). ----------------------------------------------
+//      own byte, so that a caller can drop that face alone (sd_track_faces).  Warped launches (warp.in) also check each
+//      sample's warp here and copy it to warp.out, an invalid one (or one whose frame index is out of range) as a 0 x 0 V that
+//      the HOG kernel reads no pixel of. -----------------------------------------------------------------------------------------
+struct HogWarpCheck {
+    const sd_sample_warp* in;   // the caller's table, or NULL: no warp
+    sd_sample_warp* out;        // what hog_patch_kernel reads
+    const int* image_index;
+    int image_count, width, height;
+    const sd_frame* frames;
+};
+
 __global__ void hog_geometry_kernel(const float* __restrict__ x, long long ldx, int N, int L, const sd_eyes_dev eyes, float rel,
                                     int fixed_half, int fs, int* __restrict__ half_out, int* __restrict__ rtab, int* __restrict__ status,
-                                    uint8_t* __restrict__ face_flag)
+                                    uint8_t* __restrict__ face_flag, const HogWarpCheck warp)
 {
     const int i = blockIdx.x;
     if (i >= N) return;
@@ -79,6 +91,18 @@ __global__ void hog_geometry_kernel(const float* __restrict__ x, long long ldx, 
         }
         half_out[i] = half;
         s_half = half;
+        if (warp.in) {
+            sd_sample_warp w = warp.in[i];
+            const int f = warp.image_index ? warp.image_index[i] : i;   // a mirrored bit is out of range: no decoding
+            bool ok = f >= 0 && f < warp.image_count;                   // out of range: hog_patch_kernel flags it
+            if (ok) {
+                const int fw = warp.frames ? warp.frames[f].width : warp.width, fh = warp.frames ? warp.frames[f].height : warp.height;
+                ok = sd_warp_valid(w, fw, fh);
+                if (!ok) atomicOr(status, 4);
+            }
+            if (!ok) w.width = w.height = 0;
+            warp.out[i] = w;
+        }
     }
     __syncthreads();
     const int P = 2 * s_half;
@@ -181,6 +205,26 @@ __host__ __device__ inline HogSmem hog_smem_layout(int fs, int nc, int K)
 constexpr int kTmaClasses = 8;
 __host__ __device__ constexpr int hog_tma_box(int c) { return c == 0 ? 32 : c == 1 ? 48 : c == 2 ? 64 : c == 3 ? 80 : c == 4 ? 96 : c == 5 ? 112 : c == 6 ? 128 : 160; }
 struct HogMaps { CUtensorMap m[kTmaClasses]; };
+// The second parameter of hog_patch_kernel: the tensor maps, or in a warped launch (which loads no window) the checked warps.
+// A type rather than a third parameter, so that the unwarped instantiations keep their code.
+template <bool WARP> using HogSource = typename std::conditional<WARP, const sd_sample_warp*, HogMaps>::type;
+
+// Pixel (u, v) of the V of warp sw, computed from the four taps it reads in the frame (resident region rx, ry, rw, rh; a tap
+// outside the frame reads 0, one inside the frame but outside the region sets *miss): the unstaged route's window pixel.
+__device__ __noinline__ int hog_warp_pixel(const sd_sample_warp* __restrict__ sw, int u, int v, const uint8_t* __restrict__ img, int W,
+                                           int H, int rs, int rx, int ry, int rw, int rh, bool* miss)
+{
+    if ((unsigned)u >= (unsigned)sw->width || (unsigned)v >= (unsigned)sw->height) return 0;
+    const int2 d = sd_warp_col(sw->m, (double)u), r = sd_warp_row(sw->m, (double)v);
+    return sd_warp_sample<uint8_t>((r.x + d.x) >> 5, (r.y + d.y) >> 5, [&](int ix, int iy) -> uint8_t {
+        if ((unsigned)ix >= (unsigned)W || (unsigned)iy >= (unsigned)H) return 0;
+        if (ix < rx || ix >= rx + rw || iy < ry || iy >= ry + rh) {
+            *miss = true;
+            return 0;
+        }
+        return __ldg(img + (long long)(iy - ry) * rs + (ix - rx));
+    });
+}
 
 // Whether sample i is a sample of its frame's mirror (CTA-uniform).  Only the MIR instantiations, launched for an index that
 // may carry SD_SAMPLE_MIRRORED, ask; the others compile to the unmirrored kernel.  hog_patch_kernel asks again where it needs
@@ -193,9 +237,15 @@ __device__ __forceinline__ bool hog_sample_mirrored(const HogArgs& a, int sample
 
 // NT threads per CTA.  The compiled-in schedules fit 32 registers without spills, so an SM holds 2048 / NT CTAs where shared
 // memory allows; the run-time ones (NT = 256) spill at that bound and keep the compiler's choice (a minimum of 0 CTAs per SM
-// sets no bound).
-template <int KT, int NCT, int CST, int NT, bool MIR>
-__global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(const __grid_constant__ HogArgs a, const __grid_constant__ HogMaps maps)
+// sets no bound).  The WARP instantiations of the compiled-in schedules spill at 32 registers (the double-precision warp terms
+// and the tap arithmetic of S1) and are bounded at 1024 / NT CTAs per SM, 64 registers, instead (DESIGN §4.12).
+//
+// WARP: sample i is a sample of the V of warps[i] (sd_sample_warp; hog_geometry_kernel's checked copy, an invalid warp as a 0 x 0
+// V).  Only launches with a warp table take the WARP instantiations (MIR = false: a mirrored bit is an index out of range); in
+// the others `warps` is unused and the code is the unwarped kernel's.
+template <int KT, int NCT, int CST, int NT, bool MIR, bool WARP>
+__global__ void __launch_bounds__(NT, NCT > 0 ? (WARP ? 1024 : 2048) / NT : 0) hog_patch_kernel(const __grid_constant__ HogArgs a,
+                                                                                                 const __grid_constant__ HogSource<WARP> maps)
 {
     // whole warps, and at least one row group of the fs <= 64 resize (NT / fs >= 1)
     static_assert(NT % 32 == 0 && NT >= 64, "hog_patch_kernel needs whole warps and at least 64 threads");
@@ -273,7 +323,7 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
 #pragma unroll
     for (int c = kTmaClasses - 1; c >= 0; --c)
         if (c < a.tma_count && hog_tma_box(c) >= P + tma_shift && hog_tma_box(c) * hog_tma_box(c) <= stage_cap) tma_box = hog_tma_box(c);
-    if (tma_box > 0 && tid == 0) {
+    if constexpr (!WARP) if (tma_box > 0 && tid == 0) {
         // one elected thread: the box lands densely (pitch = box width); bytes outside the frame are zero-filled by the TMA,
         // which is exactly copyMakeBorder(..., BORDER_CONSTANT, 0) (adaptive_vlhog.hpp:136-147)
         int cls = 0;
@@ -302,10 +352,51 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
         // column c of the staged window sits at byte shiftb + c of its row
         const int shiftb = tma_box ? tma_shift : (vec16 ? ((x0 - rx) & 15) : (words ? ((x0 - rx) & 3) : 0));
         const int pitch = tma_box ? tma_box : ((P + 15 + 15) & ~15);
-        const bool staged = pitch * P <= stage_cap;
+        // A warped window is computed pixel by pixel, never loaded (the launch has no tensor maps: tma_box = 0), at byte shiftb of
+        // its staged rows as any window; its per-column and per-row terms (4 x P ints) follow the rows.  `if constexpr` keeps the
+        // unwarped instantiations' code as it was.
+        const bool staged = (pitch + (WARP ? 16 : 0)) * P <= stage_cap;
         bool miss = false;
         if (staged) {
-            if (tma_box) {
+            if constexpr (WARP) {
+                // cv::warpAffine's terms once per patch, as face_chip_warp_kernel does per tile: adelta / bdelta of each window
+                // column, X0 / Y0 of each window row (only inside V), then each window pixel from its four taps in the frame
+                const sd_sample_warp* __restrict__ warps = maps;                // a warped launch's second parameter
+                const sd_sample_warp* __restrict__ sw = warps + sample;
+                const int Wv = sw->width, Hv = sw->height;
+                int* s_wt = reinterpret_cast<int*>(s_stage + pitch * P);   // [adelta | bdelta | X0 | Y0], P each
+                for (int t = tid; t < P; t += NT) {
+                    if ((unsigned)(x0 + t) < (unsigned)Wv) {
+                        const int2 d = sd_warp_col(sw->m, (double)(x0 + t));
+                        s_wt[t] = d.x;
+                        s_wt[P + t] = d.y;
+                    }
+                    if ((unsigned)(y0 + t) < (unsigned)Hv) {
+                        const int2 r = sd_warp_row(sw->m, (double)(y0 + t));
+                        s_wt[2 * P + t] = r.x;
+                        s_wt[3 * P + t] = r.y;
+                    }
+                }
+                __syncthreads();
+                for (int r = warp; r < P; r += kWarps) {
+                    const bool rowin = (unsigned)(y0 + r) < (unsigned)Hv;
+                    const int X0 = s_wt[2 * P + r], Y0 = s_wt[3 * P + r];
+#pragma unroll 1
+                    for (int c = lane; c < P; c += 32) {
+                        uint8_t v = 0;
+                        if (rowin && (unsigned)(x0 + c) < (unsigned)Wv)
+                            v = sd_warp_sample<uint8_t>((X0 + s_wt[c]) >> 5, (Y0 + s_wt[P + c]) >> 5, [&](int ix, int iy) -> uint8_t {
+                                if ((unsigned)ix >= (unsigned)W || (unsigned)iy >= (unsigned)H) return 0;
+                                if (ix < rx || ix >= rx + rw || iy < ry || iy >= ry + rh) {
+                                    miss = true;                   // a frame pixel that was not uploaded
+                                    return 0;
+                                }
+                                return __ldg(img + (long long)(iy - ry) * rs + (ix - rx));
+                            });
+                        s_stage[r * pitch + shiftb + c] = v;
+                    }
+                }
+            } else if (tma_box) {
                 // nothing to do: the tile is in flight
             } else if (vec16) {
                 // 8 / 16 / 32 lanes per source row, one aligned uint4 each: ~P * nvec / 32 warp loads in total
@@ -437,6 +528,12 @@ __global__ void __launch_bounds__(NT, NCT > 0 ? 2048 / NT : 0) hog_patch_kernel(
                         const int ix = mirrored ? x0 + P - 1 - u : x0 + u, iy = (q & 2) ? iy1 : iy0;
                         int v = 0;
                         if ((q & 1) && xa.y == 0) { p[q] = 0; continue; }
+                        if constexpr (WARP) {
+                            // (ix, iy) is a pixel of V: its value from its four taps in the frame, 0 outside V
+                            const sd_sample_warp* __restrict__ warps = maps;        // a warped launch's second parameter
+                            p[q] = hog_warp_pixel(warps + sample, ix, iy, img, W, H, rs, rx, ry, rw, rh, &miss);
+                            continue;
+                        }
                         if ((unsigned)ix < (unsigned)W && (unsigned)iy < (unsigned)H) {
                             if (ix >= rx && ix < rx + rw && iy >= ry && iy < ry + rh) v = __ldg(img + (long long)(iy - ry) * rs + (ix - rx));
                             else miss = true;
@@ -632,22 +729,23 @@ __global__ void __launch_bounds__(kHogThreads) hog_normalise_kernel(const NormAr
 }
 
 // the hog_patch_kernel instantiation of a configuration and its threads per CTA: a compiled-in schedule (DESIGN §4.1) or a run-time one
-template <bool MIR>
-decltype(&hog_patch_kernel<0, 0, 0, kHogThreads, MIR>) pick_hog_kernel(int K, int nc, int cs, int* threads)
+template <bool MIR, bool WARP>
+decltype(&hog_patch_kernel<0, 0, 0, kHogThreads, MIR, WARP>) pick_hog_kernel(int K, int nc, int cs, int* threads)
 {
     *threads = kHogThreads;
     if (nc == 5 && (K == 4 || K == 9)) {
-#define SD_HOG_PICK(KK, CC, TT) if (K == KK && cs == CC) { *threads = TT; return hog_patch_kernel<KK, 5, CC, TT, MIR>; }
+#define SD_HOG_PICK(KK, CC, TT) if (K == KK && cs == CC) { *threads = TT; return hog_patch_kernel<KK, 5, CC, TT, MIR, WARP>; }
         SD_HOG_PICK(4, 11, 224) SD_HOG_PICK(4, 10, 160) SD_HOG_PICK(4, 8, 160) SD_HOG_PICK(4, 6, 128)
         SD_HOG_PICK(9, 11, 256) SD_HOG_PICK(9, 10, 160) SD_HOG_PICK(9, 8, 160) SD_HOG_PICK(9, 6, 128)
 #undef SD_HOG_PICK
     }
-    return K == 4 ? hog_patch_kernel<4, 0, 0, kHogThreads, MIR> : K == 9 ? hog_patch_kernel<9, 0, 0, kHogThreads, MIR>
-                                                                       : hog_patch_kernel<0, 0, 0, kHogThreads, MIR>;
+    return K == 4 ? hog_patch_kernel<4, 0, 0, kHogThreads, MIR, WARP> : K == 9 ? hog_patch_kernel<9, 0, 0, kHogThreads, MIR, WARP>
+                                                                             : hog_patch_kernel<0, 0, 0, kHogThreads, MIR, WARP>;
 }
 
-int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, bool mirrors, const float* d_x,
-               int64_t ldx, int N, int L, const sd_normalisation* eyes, const sd_hog_param* p, float* d_A,
+// d_warp (optional): the samples' warps (sd_hog_batch_warped); the launch then reads no mirrored bit
+int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, bool mirrors, const sd_sample_warp* d_warp,
+               const float* d_x, int64_t ldx, int N, int L, const sd_normalisation* eyes, const sd_hog_param* p, float* d_A,
                int64_t ld, int32_t* d_geometry, uint8_t* d_patches, int8_t* d_bins, uint8_t* d_face_degenerate = nullptr)
 {
     SD_REQUIRE(ctx, images && images->d_data && d_x && p, "null argument");
@@ -705,14 +803,20 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
 
     hog_orientations(a.K, a.orient);   // hog.c:195-204
 
-    // per-sample tables (half size, cv::resize taps) and the per-launch spatial binning table
-    const size_t geom_bytes = (size_t)N * sizeof(int) + (size_t)N * 5 * fs * sizeof(int) + (size_t)(a.nc * fs + 2 * a.nc) * sizeof(float);
+    // per-sample tables (half size, cv::resize taps), the per-launch spatial binning table and, warped, the checked warps
+    const size_t tab_bytes = (size_t)N * sizeof(int) + (size_t)N * 5 * fs * sizeof(int) + (size_t)(a.nc * fs + 2 * a.nc) * sizeof(float);
+    const size_t geom_bytes = d_warp ? sd_round16(tab_bytes) + (size_t)N * sizeof(sd_sample_warp) : tab_bytes;
     int* d_half = (int*)sd_workspace(ctx, SD_WS_GEOM, geom_bytes);
     if (!d_half) return SD_ERR_CUDA;
     int* d_rtab = d_half + N;
     float* d_btab = reinterpret_cast<float*>(d_rtab + (size_t)N * 5 * fs);
+    HogWarpCheck wc{};
+    if (d_warp) {
+        wc = HogWarpCheck{d_warp, reinterpret_cast<sd_sample_warp*>(reinterpret_cast<uint8_t*>(d_half) + sd_round16(tab_bytes)), d_image_index,
+                          images->count, images->width, images->height, images->d_frames};
+    }
     hog_geometry_kernel<<<N, 64, 0, ctx->stream>>>(d_x, ldx, N, L, eyes_dev, p->relative_patch_size, fixed_half, fs, d_half, d_rtab, a.status,
-                                                    d_face_degenerate);
+                                                    d_face_degenerate, wc);
     SD_LAUNCH_CHECK(ctx, "hog_geometry_kernel");
     hog_bintab_kernel<<<1, 256, 0, ctx->stream>>>(fs, a.nc, a.cs, lay.pw, d_btab);
     SD_LAUNCH_CHECK(ctx, "hog_bintab_kernel");
@@ -724,7 +828,7 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
     HogMaps maps;
     memset(&maps, 0, sizeof(maps));
     a.tma_count = 0;
-    if (!images->d_roi && (images->image_stride % 16) == 0 && (images->count == 1 || images->image_stride > 0)) {
+    if (!d_warp && !images->d_roi && (images->image_stride % 16) == 0 && (images->count == 1 || images->image_stride > 0)) {
         // classes are usable up to the first one that cannot be encoded
         for (int c = 0; c < kTmaClasses && hog_tma_box(c) <= 256; ++c) {
             if (!hog_frame_map(images, hog_tma_box(c), hog_tma_box(c), &maps.m[c])) break;
@@ -732,18 +836,23 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
         }
     }
 
-    // an index that may carry SD_SAMPLE_MIRRORED takes the MIR instantiations; without one (or for detect's face_frame) the
-    // launch is the unmirrored kernel
+    // a warp table takes the WARP instantiations; otherwise an index that may carry SD_SAMPLE_MIRRORED takes the MIR ones, and
+    // without one (or for detect's face_frame) the launch is the unmirrored kernel
     int threads = kHogThreads;
-    const auto kern = mirrors && d_image_index ? pick_hog_kernel<true>(a.K, a.nc, a.cs, &threads)
-                                               : pick_hog_kernel<false>(a.K, a.nc, a.cs, &threads);
-    SD_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
+    const auto launch = [&](auto kern, const auto& src) -> int {
+        SD_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
+        kern<<<(unsigned)blocks, threads, lay.total, ctx->stream>>>(a, src);
+        SD_LAUNCH_CHECK(ctx, "hog_patch_kernel");
+        return SD_OK;
+    };
     // Default shared-memory carve-out: the maximum one ran the four detect levels no faster (5.84 ms both, 4096 faces, one
     // H100 80GB HBM3 at a 400 W power limit; measured at 256 threads, when registers, not shared memory, bounded the CTAs per
     // SM at fs = 55 / 50 / 40).  With the default, every compiled schedule reaches the CTAs per SM that the thread and
     // shared-memory limits allow (DESIGN §4.1; counted per SM on an H100 and equal to cudaOccupancyMaxActiveBlocksPerMultiprocessor).
-    kern<<<(unsigned)blocks, threads, lay.total, ctx->stream>>>(a, maps);
-    SD_LAUNCH_CHECK(ctx, "hog_patch_kernel");
+    rc = d_warp ? launch(pick_hog_kernel<false, true>(a.K, a.nc, a.cs, &threads), wc.out)
+                : launch(mirrors && d_image_index ? pick_hog_kernel<true, false>(a.K, a.nc, a.cs, &threads)
+                                                  : pick_hog_kernel<false, false>(a.K, a.nc, a.cs, &threads), maps);
+    if (rc) return rc;
     if (!d_A) return SD_OK;
     auto norm = a.K == 4 ? hog_normalise_kernel<4> : a.K == 9 ? hog_normalise_kernel<9> : hog_normalise_kernel<0>;
     SD_CUDA(ctx, cudaFuncSetAttribute(norm, cudaFuncAttributeMaxDynamicSharedMemorySize, norm_smem));
@@ -756,11 +865,11 @@ int launch_hog(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image
 
 int sd_hog_batch_unmirrored(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int64_t ldx,
                             int num_samples, int num_landmarks, const sd_normalisation* eyes, const sd_hog_param* p, float* d_A,
-                            int64_t ld, uint8_t* d_face_degenerate)
+                            int64_t ld, uint8_t* d_face_degenerate, const sd_sample_warp* d_warp)
 {
     if (num_samples == 0) return SD_OK;
     SD_REQUIRE(ctx, d_A, "null output");
-    return launch_hog(ctx, images, d_image_index, false, d_x, ldx, num_samples, num_landmarks, eyes, p, d_A, ld, nullptr, nullptr,
+    return launch_hog(ctx, images, d_image_index, false, d_warp, d_x, ldx, num_samples, num_landmarks, eyes, p, d_A, ld, nullptr, nullptr,
                       nullptr, d_face_degenerate);
 }
 
@@ -842,8 +951,18 @@ int sd_hog_batch(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_ima
     if (!ctx) return SD_ERR_INVALID;
     if (num_samples == 0) return SD_OK;
     SD_REQUIRE(ctx, d_A, "null output");
-    return launch_hog(ctx, images, d_image_index, true, d_x, ldx, num_samples, num_landmarks, eyes, p, d_A, ld,
+    return launch_hog(ctx, images, d_image_index, true, nullptr, d_x, ldx, num_samples, num_landmarks, eyes, p, d_A, ld,
                       nullptr, nullptr, nullptr);
+}
+
+int sd_hog_batch_warped(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int64_t ldx,
+                        int num_samples, int num_landmarks, const sd_normalisation* eyes, const sd_hog_param* p,
+                        const sd_sample_warp* d_warp, float* d_A, int64_t ld)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, images && !images->d_roi, "a warped batch must hold whole frames (no d_roi)");
+    SD_REQUIRE(ctx, d_warp, "null warp table");
+    return sd_hog_batch_unmirrored(ctx, images, d_image_index, d_x, ldx, num_samples, num_landmarks, eyes, p, d_A, ld, nullptr, d_warp);
 }
 
 int sd_hog_debug(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x,
@@ -851,7 +970,18 @@ int sd_hog_debug(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_ima
                  const sd_hog_param* p, int32_t* d_geometry, uint8_t* d_patches, int8_t* d_bins)
 {
     if (!ctx) return SD_ERR_INVALID;
-    return launch_hog(ctx, images, d_image_index, true, d_x, ldx, num_samples, num_landmarks, eyes, p, nullptr, 0,
+    return launch_hog(ctx, images, d_image_index, true, nullptr, d_x, ldx, num_samples, num_landmarks, eyes, p, nullptr, 0,
+                      d_geometry, d_patches, d_bins);
+}
+
+int sd_hog_debug_warped(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int64_t ldx,
+                        int num_samples, int num_landmarks, const sd_normalisation* eyes, const sd_hog_param* p,
+                        const sd_sample_warp* d_warp, int32_t* d_geometry, uint8_t* d_patches, int8_t* d_bins)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, images && !images->d_roi, "a warped batch must hold whole frames (no d_roi)");
+    SD_REQUIRE(ctx, d_warp, "null warp table");
+    return launch_hog(ctx, images, d_image_index, false, d_warp, d_x, ldx, num_samples, num_landmarks, eyes, p, nullptr, 0,
                       d_geometry, d_patches, d_bins);
 }
 

@@ -224,14 +224,15 @@ bool syrk_is_big(int K, int64_t MI, int64_t NJ);
 
 // sd_hog_batch for callers whose index is not a sample map (detect's face_frame): an SD_SAMPLE_MIRRORED bit there is an index
 // out of range, as it always was (sd_hog.cu).  d_face_degenerate (optional): byte i is set to 1 when sample i's patch is empty,
-// beside the status word's flag; other bytes are not written.
+// beside the status word's flag; other bytes are not written.  d_warp (optional): sd_hog_batch_warped's warp table, here also
+// with a d_roi batch (the host-frame gather of sd_train.cu reads warped samples through its regions).
 int sd_hog_batch_unmirrored(sd_ctx* ctx, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x, int64_t ldx,
                             int num_samples, int num_landmarks, const sd_normalisation* eyes, const sd_hog_param* p, float* d_A,
-                            int64_t ld, uint8_t* d_face_degenerate = nullptr);
+                            int64_t ld, uint8_t* d_face_degenerate = nullptr, const sd_sample_warp* d_warp = nullptr);
 // The detect cascade of sd_detect_faces_device without its status read-back (sd_model.cu): d_face_degenerate as above, for
 // every level.  The model's mean on the device, 2L floats (sd_model.cu).
 int sd_detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_face_frame, const float* d_x0,
-                     int count, float* d_landmarks, uint8_t* d_face_degenerate);
+                     int count, float* d_landmarks, uint8_t* d_face_degenerate, const sd_sample_warp* d_warp = nullptr);
 const float* sd_model_device_mean(const sd_model* m);
 // The frames whose boxes sd_hog_box_scores / sd_hog_box_scores_images score and on which the tracking step detects: an 8-bit grey
 // batch (grey, the grey entry points) or frames that keep their channels (images, with their orientation assignment).  Exactly

@@ -148,7 +148,7 @@ int validate_and_upload(sd_ctx* ctx, sd_model* m)
 }
 
 int detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_image_index, const float* d_x0,
-                  int count, float* d_landmarks, uint8_t* d_face_degenerate = nullptr)
+                  int count, float* d_landmarks, uint8_t* d_face_degenerate = nullptr, const sd_sample_warp* d_warp = nullptr)
 {
     const int L = m->num_landmarks, P = 2 * L;
     if (count <= 0) return SD_OK;
@@ -165,7 +165,8 @@ int detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, 
     float* cur = xa;
     float* nxt = xb;
     for (int s = 0; s < m->num_levels; ++s) {               // superviseddescent.hpp:326-342
-        int rc = sd_hog_batch_unmirrored(ctx, images, d_image_index, cur, P, count, L, &m->norm, &m->hog[s], A, ld, d_face_degenerate);
+        int rc = sd_hog_batch_unmirrored(ctx, images, d_image_index, cur, P, count, L, &m->norm, &m->hog[s], A, ld, d_face_degenerate,
+                                         d_warp);
         if (rc) return rc;
         rc = sd_cascade_update(ctx, A, ld, count, m->rows[s], m->d_weights[s], P, cur, &m->norm, nxt);
         if (rc) return rc;
@@ -861,6 +862,18 @@ int sd_detect_faces_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch*
     return sd_check_hog_status(ctx, "detect");                // also reports a face index out of range
 }
 
+int sd_detect_faces_device_warped(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_face_frame,
+                                  const sd_sample_warp* d_warp, const float* d_x0, int num_faces, float* d_landmarks)
+{
+    if (!ctx) return SD_ERR_INVALID;
+    SD_REQUIRE(ctx, m && images && d_warp && d_x0 && d_landmarks && num_faces >= 0, "bad argument");
+    SD_REQUIRE(ctx, !images->d_roi, "a warped batch must hold whole frames (no d_roi)");
+    if (!d_face_frame) SD_REQUIRE(ctx, images->count >= num_faces, "fewer images than faces");
+    const int rc = detect_device(ctx, m, images, d_face_frame, d_x0, num_faces, d_landmarks, nullptr, d_warp);
+    if (rc) return rc;
+    return sd_check_hog_status(ctx, "detect");                // also reports a face index out of range or an invalid warp
+}
+
 int sd_detect_faces_host(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frames, int num_frames, const int32_t* h_face_frame,
                          int num_faces, const int32_t* h_boxes, const float* h_x0, float* h_landmarks)
 {
@@ -956,9 +969,9 @@ int sd_upload_frames(sd_ctx* ctx, const sd_host_frame* frames, int count, void* 
 }  // extern "C"
 
 int sd_detect_device(sd_ctx* ctx, const sd_model* m, const sd_image_batch* images, const int32_t* d_face_frame, const float* d_x0,
-                     int count, float* d_landmarks, uint8_t* d_face_degenerate)
+                     int count, float* d_landmarks, uint8_t* d_face_degenerate, const sd_sample_warp* d_warp)
 {
-    return detect_device(ctx, m, images, d_face_frame, d_x0, count, d_landmarks, d_face_degenerate);
+    return detect_device(ctx, m, images, d_face_frame, d_x0, count, d_landmarks, d_face_degenerate, d_warp);
 }
 
 const float* sd_model_device_mean(const sd_model* m) { return m->d_mean; }

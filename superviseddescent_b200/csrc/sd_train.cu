@@ -16,6 +16,7 @@
 // The HOG rows come from frames resident on the device, or from frames that stay in pinned host memory, gathered batch by batch
 // (gather_hog_rows); sd_level_frames says which.
 #include "sd_internal.cuh"
+#include "sd_warp.cuh"
 
 #include <climits>
 #include <cstring>
@@ -70,6 +71,7 @@ struct HostGather {
     sd_roi* d_roi;                        // per sample: its frame's region
     sd_frame* d_dims;                     // per sample: its frame's size
     int32_t* d_hidx;                      // per sample: its HOG index into its batch, with its mirrored bit (NULL: none is mirrored)
+    const sd_sample_warp* d_warp;         // the caller's per-sample warps (NULL: none)
     uint8_t* d_miss;                      // per sample: a patch read outside the region (must never be raised)
     GatherTotals* d_tot;
     int guess = 0;                        // samples the next batch starts from (gather_hog_rows)
@@ -79,10 +81,11 @@ struct HostGather {
 constexpr int kPlanThreads = 128;
 constexpr int kLayoutThreads = 1024;
 
-// frame of sample s, as the HOG kernel resolves an image index: an index out of range raises the status flag and reads frame 0
-__device__ __forceinline__ int sample_frame(const int32_t* __restrict__ idx, int s, int F, int* status)
+// frame of sample s, as the HOG kernel resolves an image index: an index out of range raises the status flag and reads frame 0.
+// With a warp table (warped) a mirrored bit is not decoded: the index is out of range.
+__device__ __forceinline__ int sample_frame(const int32_t* __restrict__ idx, int s, int F, int* status, bool warped)
 {
-    int f = sd_sample_frame_of(idx[s]);
+    int f = warped ? idx[s] : sd_sample_frame_of(idx[s]);
     if (f < 0 || f >= F) {
         if (status) atomicOr(status, 2);
         f = 0;
@@ -90,28 +93,60 @@ __device__ __forceinline__ int sample_frame(const int32_t* __restrict__ idx, int
     return f;
 }
 
+// The rectangle [x0, x1) x [y0, y1) of frame pixels that the taps of window [ua, ub) x [va, vb) of V (already clipped to V, not
+// empty) read under warp m: cv::warpAffine's fixed-point terms are each monotone in their own variable, so the window's corners
+// bound every tap, and each tap also reads the pixel right of and below it.
+__device__ __forceinline__ void warp_window_rect(const double* m, int ua, int ub, int va, int vb, int* x0, int* y0, int* x1, int* y1)
+{
+    const int2 ca = sd_warp_col(m, (double)ua), cb = sd_warp_col(m, (double)(ub - 1));
+    const int2 ra = sd_warp_row(m, (double)va), rb = sd_warp_row(m, (double)(vb - 1));
+    const int sx[4] = {ra.x + ca.x, ra.x + cb.x, rb.x + ca.x, rb.x + cb.x}, sy[4] = {ra.y + ca.y, ra.y + cb.y, rb.y + ca.y, rb.y + cb.y};
+    int xa = INT_MAX, xb = INT_MIN, ya = INT_MAX, yb = INT_MIN;
+    for (int k = 0; k < 4; ++k) {
+        xa = min(xa, sx[k] >> 10); xb = max(xb, sx[k] >> 10);
+        ya = min(ya, sy[k] >> 10); yb = max(yb, sy[k] >> 10);
+    }
+    *x0 = xa; *x1 = xb + 2; *y0 = ya; *y1 = yb + 2;
+}
+
 // One block per sample: the union of the windows of its L patches in its frame, [x0, x0 + 2 half) x [cy - half, cy + half) with
-// x0 = sd_window_x0 (cvRound(x_l) - half, or the frame's window of a mirrored patch), merged into its frame's slot.
+// x0 = sd_window_x0 (cvRound(x_l) - half, or the frame's window of a mirrored patch), merged into its frame's slot.  A warped
+// sample (warp != NULL) plans, per patch, the frame pixels its window of V reads (warp_window_rect); an invalid warp reads none
+// (the HOG kernel flags it and reads no pixel).
 __global__ void __launch_bounds__(kPlanThreads) roi_plan_kernel(const float* __restrict__ x, int L, const int32_t* __restrict__ idx,
                                                                 int F, const FrameDev* __restrict__ fr, const sd_eyes_dev eyes,
                                                                 float rel, int fixed_half, int2* __restrict__ lo, int2* __restrict__ hi,
-                                                                int* status)
+                                                                int* status, const sd_sample_warp* __restrict__ warp)
 {
     const int s = blockIdx.x;
     const float* __restrict__ row = x + (long long)s * 2 * L;
-    __shared__ int s_half, s_frame, s_width, s_mirrored;
+    __shared__ int s_half, s_frame, s_width, s_mirrored, s_warp_ok;
     __shared__ int s_box[4][kPlanThreads / 32];
     if (threadIdx.x == 0) {
         bool degenerate;
         s_half = sd_patch_half(row, L, eyes, rel, fixed_half, &degenerate);   // the HOG kernel flags a degenerate sample itself
-        s_frame = sample_frame(idx, s, F, status);
+        s_frame = sample_frame(idx, s, F, status, warp != nullptr);
         s_width = fr[s_frame].width;
-        s_mirrored = sd_sample_is_mirrored(idx[s]);
+        s_mirrored = !warp && sd_sample_is_mirrored(idx[s]);
+        if (warp) {
+            s_warp_ok = sd_warp_valid(warp[s], fr[s_frame].width, fr[s_frame].height);
+        }
     }
     __syncthreads();
     int x0 = INT_MAX, y0 = INT_MAX, x1 = INT_MIN, y1 = INT_MIN;
     for (int l = threadIdx.x; l < L; l += kPlanThreads) {
         const int cx = __float2int_rn(row[l]), cy = __float2int_rn(row[l + L]);
+        if (warp) {
+            if (!s_warp_ok) continue;
+            const sd_sample_warp& w = warp[s];
+            const int ua = max(cx - s_half, 0), ub = min(cx + s_half, w.width), va = max(cy - s_half, 0), vb = min(cy + s_half, w.height);
+            if (ua >= ub || va >= vb) continue;                   // the window lies outside V: zeros, no pixel read
+            int rx0, ry0, rx1, ry1;
+            warp_window_rect(w.m, ua, ub, va, vb, &rx0, &ry0, &rx1, &ry1);
+            x0 = min(x0, rx0); y0 = min(y0, ry0);
+            x1 = max(x1, rx1); y1 = max(y1, ry1);
+            continue;
+        }
         const int wx = sd_window_x0(cx, s_half, s_width, s_mirrored);
         x0 = min(x0, wx); y0 = min(y0, cy - s_half);
         x1 = max(x1, wx + 2 * s_half); y1 = max(y1, cy + s_half);
@@ -128,8 +163,10 @@ __global__ void __launch_bounds__(kPlanThreads) roi_plan_kernel(const float* __r
             x0 = min(x0, s_box[0][k]); y0 = min(y0, s_box[1][k]); x1 = max(x1, s_box[2][k]); y1 = max(y1, s_box[3][k]);
         }
         const int f = s_frame;
-        atomicMin(&lo[f].x, x0); atomicMin(&lo[f].y, y0);
-        atomicMax(&hi[f].x, x1); atomicMax(&hi[f].y, y1);
+        if (x0 <= x1) {                                       // a warped sample may read no pixel at all
+            atomicMin(&lo[f].x, x0); atomicMin(&lo[f].y, y0);
+            atomicMax(&hi[f].x, x1); atomicMax(&hi[f].y, y1);
+        }
     }
 }
 
@@ -141,7 +178,8 @@ __global__ void __launch_bounds__(kLayoutThreads) gather_layout_kernel(const Fra
                                                                        int2* __restrict__ hi, sd_roi* __restrict__ froi,
                                                                        GatherRec* __restrict__ rec, const int32_t* __restrict__ idx, int n,
                                                                        sd_roi* __restrict__ roi, sd_frame* __restrict__ dims,
-                                                                       int32_t* __restrict__ hidx, GatherTotals* __restrict__ tot)
+                                                                       int32_t* __restrict__ hidx, GatherTotals* __restrict__ tot,
+                                                                       bool warped)
 {
     __shared__ long long s_scan[kLayoutThreads / 32];
     __shared__ long long s_base, s_pcie;
@@ -205,7 +243,7 @@ __global__ void __launch_bounds__(kLayoutThreads) gather_layout_kernel(const Fra
         __syncthreads();
     }
     for (int s = tid; s < n; s += kLayoutThreads) {
-        const int f = sample_frame(idx, s, F, nullptr);        // roi_plan_kernel has flagged a bad index
+        const int f = sample_frame(idx, s, F, nullptr, warped);   // roi_plan_kernel has flagged a bad index
         roi[s] = froi[f];
         dims[s] = sd_frame{fr[f].width, fr[f].height, 0, 0, 0};
         if (hidx) hidx[s] = sd_sample_is_mirrored(idx[s]) ? s | SD_SAMPLE_MIRRORED : s;
@@ -234,10 +272,11 @@ int gather_prepare(sd_ctx* ctx, HostGather& g, const sd_level_frames& src, int N
     }
     std::vector<char> used(F, 0);
     bool mirrored = false;
+    const bool warped = src.d_sample_warp != nullptr;            // then a mirrored bit is an index out of range
     for (int s = 0; s < N; ++s) {
-        const int f = sd_sample_frame_of(idx[s]);
+        const int f = warped ? idx[s] : sd_sample_frame_of(idx[s]);
         used[f >= 0 && f < F ? f : 0] = 1;
-        mirrored = mirrored || sd_sample_is_mirrored(idx[s]);
+        mirrored = mirrored || (!warped && sd_sample_is_mirrored(idx[s]));
     }
     std::vector<FrameDev> fr(F);
     PinnedRange last;
@@ -281,6 +320,7 @@ int gather_prepare(sd_ctx* ctx, HostGather& g, const sd_level_frames& src, int N
     g.d_tot = (GatherTotals*)t;
     g.num_frames = F;
     g.d_sample_frame = b_idx ? d_idx : src.d_sample_frame;
+    g.d_warp = src.d_sample_warp;
     if (b_idx && N > 0)                                                                    // no index: sample i reads frame i
         SD_CUDA(ctx, cudaMemcpyAsync(d_idx, idx.data(), (size_t)N * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
     SD_CUDA(ctx, cudaMemcpyAsync(g.d_fr, fr.data(), F * sizeof(FrameDev), cudaMemcpyHostToDevice, ctx->stream));
@@ -328,11 +368,12 @@ int gather_hog_rows(sd_ctx* ctx, HostGather& g, const float* d_x, int r0, int ro
         GatherTotals t;
         for (;;) {
             roi_plan_kernel<<<nb, kPlanThreads, 0, ctx->copy_stream>>>(d_x + (int64_t)s0 * P, L, g.d_sample_frame + s0, g.num_frames, g.d_fr,
-                                                                       eyes_dev, p->relative_patch_size, fixed_half, g.d_lo, g.d_hi, status);
+                                                                       eyes_dev, p->relative_patch_size, fixed_half, g.d_lo, g.d_hi, status,
+                                                                       g.d_warp ? g.d_warp + s0 : nullptr);
             SD_LAUNCH_CHECK(ctx, "roi_plan_kernel");
             gather_layout_kernel<<<1, kLayoutThreads, 0, ctx->copy_stream>>>(g.d_fr, g.num_frames, g.d_lo, g.d_hi, g.d_froi, g.d_rec,
                                                                             g.d_sample_frame + s0, nb, g.d_roi + s0, g.d_dims + s0,
-                                                                            g.d_hidx ? g.d_hidx + s0 : nullptr, g.d_tot);
+                                                                            g.d_hidx ? g.d_hidx + s0 : nullptr, g.d_tot, g.d_warp != nullptr);
             SD_LAUNCH_CHECK(ctx, "gather_layout_kernel");
             SD_CUDA(ctx, cudaMemcpyAsync(&t, g.d_tot, sizeof(t), cudaMemcpyDeviceToHost, ctx->copy_stream));
             SD_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
@@ -357,7 +398,10 @@ int gather_hog_rows(sd_ctx* ctx, HostGather& g, const float* d_x, int r0, int ro
         ib.d_roi = g.d_roi + s0;
         ib.d_roi_miss = g.d_miss + s0;
         ib.d_frames = g.d_dims + s0;
-        rc = sd_hog_batch(ctx, &ib, g.d_hidx ? g.d_hidx + s0 : nullptr, d_x + (int64_t)s0 * P, P, nb, L, eyes, p, d_chunk + (int64_t)b0 * ld, ld);
+        rc = g.d_warp ? sd_hog_batch_unmirrored(ctx, &ib, nullptr, d_x + (int64_t)s0 * P, P, nb, L, eyes, p, d_chunk + (int64_t)b0 * ld, ld,
+                                                nullptr, g.d_warp + s0)
+                      : sd_hog_batch(ctx, &ib, g.d_hidx ? g.d_hidx + s0 : nullptr, d_x + (int64_t)s0 * P, P, nb, L, eyes, p,
+                                     d_chunk + (int64_t)b0 * ld, ld);
         if (rc) return rc;
         SD_CUDA(ctx, cudaEventRecord(ctx->stage_done[buf], ctx->stream));
         ctx->gathered_bytes += t.pcie;
@@ -390,6 +434,9 @@ int hog_rows(sd_ctx* ctx, const sd_level_frames& src, HostGather& g, const float
     const int P = 2 * L;
     const int32_t* idx = src.d_sample_frame;
     const sd_image_batch view = idx ? *src.images : batch_from(*src.images, r0);
+    if (src.d_sample_warp)
+        return sd_hog_batch_unmirrored(ctx, &view, idx ? idx + r0 : nullptr, d_x + (int64_t)r0 * P, P, rows, L, eyes, p, d_chunk, ld, nullptr,
+                                       src.d_sample_warp + r0);
     return sd_hog_batch(ctx, &view, idx ? idx + r0 : nullptr, d_x + (int64_t)r0 * P, P, rows, L, eyes, p, d_chunk, ld);
 }
 

@@ -228,14 +228,22 @@ public:
     // (cv::flip(image, 1)), with its landmarks in the mirror's coordinates (rcr::mirror_landmarks).  The photo is still held once
     // -- a mirrored shallow copy shares its frame -- and read right to left (SD_SAMPLE_MIRRORED): rows, weights and predictions are
     // bit for bit those of a flipped deep copy.
+    // warps (optional, one sd_sample_warp per image entry; not with mirrored): entry i is a sample of the virtual frame
+    // V = cv::warpAffine(grey photo, warps[i].m, (width, height), INTER_LINEAR | WARP_INVERSE_MAP) (rcr::rotation_warp,
+    // rcr::make_warp), with its landmarks in V's coordinates (rcr::warp_landmarks).  V is never built; rows, weights and predictions
+    // are bit for bit those of V passed as an image of its own.
     HogTransform(const std::vector<cv::Mat>& images, std::vector<HoGParam> hog_params, std::vector<std::string> modelLandmarksList,
                  std::vector<std::string> rightEyeIdentifiers, std::vector<std::string> leftEyeIdentifiers,
-                 std::vector<bool> mirrored = {})
+                 std::vector<bool> mirrored = {}, std::vector<sd_sample_warp> warps = {})
         : images(images), hog_params(hog_params), modelLandmarksList(modelLandmarksList), rightEyeIdentifiers(rightEyeIdentifiers),
-          leftEyeIdentifiers(leftEyeIdentifiers), mirrored(mirrored), dev(std::make_shared<DeviceImages>())
+          leftEyeIdentifiers(leftEyeIdentifiers), mirrored(mirrored), warps(warps), dev(std::make_shared<DeviceImages>())
     {
         if (!this->mirrored.empty() && this->mirrored.size() != images.size())
             throw std::runtime_error("HogTransform: mirrored needs one entry per image");
+        if (!this->warps.empty() && this->warps.size() != images.size())
+            throw std::runtime_error("HogTransform: warps needs one entry per image");
+        if (!this->warps.empty() && !this->mirrored.empty())
+            throw std::runtime_error("HogTransform: mirrored and warps exclude each other (a mirror is the warp [-1, 0, W - 1; 0, 1, 0])");
     }
 
     int feature_length(size_t level) const
@@ -257,7 +265,15 @@ public:
         sd_b200::check(ctx, sd_memcpy_h2d(ctx, didx.as<int32_t>(), &idx, sizeof(idx)), "HogTransform");
         const sd_normalisation nrm = eyes();
         const sd_hog_param p = hog_params[regressorLevel].c();
-        sd_b200::check(ctx, sd_hog_batch(ctx, &batch, didx.as<int32_t>(), dx.as<float>(), parameters.cols, 1, static_cast<int>(modelLandmarksList.size()),
+        const int L = static_cast<int>(modelLandmarksList.size());
+        if (!warps.empty() && idx >= 0) {
+            const sd_b200::DeviceBuffer dw(sizeof(sd_sample_warp));
+            sd_b200::check(ctx, sd_memcpy_h2d(ctx, dw.as<sd_sample_warp>(), &warps[trainingIndex], sizeof(sd_sample_warp)), "HogTransform");
+            sd_b200::check(ctx, sd_hog_batch_warped(ctx, &batch, didx.as<int32_t>(), dx.as<float>(), parameters.cols, 1, L, &nrm, &p,
+                                                    dw.as<sd_sample_warp>(), dA.as<float>(), D), "sd_hog_batch_warped");
+            return sd_b200::download(dA.as<float>(), 1, D, D);
+        }
+        sd_b200::check(ctx, sd_hog_batch(ctx, &batch, didx.as<int32_t>(), dx.as<float>(), parameters.cols, 1, L,
                                          &nrm, &p, dA.as<float>(), D), "sd_hog_batch");
         return sd_b200::download(dA.as<float>(), 1, D, D);
     }
@@ -300,6 +316,7 @@ public:
             f.images = &dev->batch;
         }
         f.d_sample_frame = dev->index.as<int32_t>();
+        f.d_sample_warp = warps.empty() ? nullptr : dev->warp.as<sd_sample_warp>();
         return f;
     }
     // number of distinct frames
@@ -335,6 +352,7 @@ private:
         std::vector<sd_host_frame> frames;   // the distinct frames (on the host route: where the levels read them)
         std::vector<int32_t> frame_of;        // images[i] -> distinct frame
         sd_b200::DeviceBuffer index;          // frame_of on the device
+        sd_b200::DeviceBuffer warp;           // the entries' warps on the device (when there are any)
         sd_b200::DeviceBuffer buf;            // device route: the grey frames
         sd_image_batch batch{};
         sd_b200::HostBuffer packed;           // host route: the frames that could not be read in place
@@ -367,6 +385,11 @@ private:
         for (size_t i = 0; i < all.size(); ++i) index[i] = sample_index(i);
         dev->index.allocate(all.size() * sizeof(int32_t));
         sd_b200::check(ctx, sd_memcpy_h2d(ctx, dev->index.as<int32_t>(), index.data(), all.size() * sizeof(int32_t)), "HogTransform upload");
+        if (!warps.empty()) {
+            dev->warp.allocate(warps.size() * sizeof(sd_sample_warp));
+            sd_b200::check(ctx, sd_memcpy_h2d(ctx, dev->warp.as<sd_sample_warp>(), warps.data(), warps.size() * sizeof(sd_sample_warp)),
+                           "HogTransform upload");
+        }
         sd_b200::check(ctx, sd_sync(ctx), "HogTransform upload");
         size_t free_bytes = 0, total = 0;
         sd_b200::check(ctx, sd_device_memory(ctx, &free_bytes, &total), "sd_device_memory");
@@ -406,6 +429,7 @@ private:
     std::vector<std::string> rightEyeIdentifiers;
     std::vector<std::string> leftEyeIdentifiers;
     std::vector<bool> mirrored;          // per image entry: a sample of the photo's mirror (empty: none)
+    std::vector<sd_sample_warp> warps;   // per image entry: the warp of its photo it samples (empty: none)
     std::shared_ptr<DeviceImages> dev;   // shared between the copies the optimiser makes of this functor
 };
 

@@ -76,6 +76,58 @@ inline cv::Mat mirror_landmarks(cv::Mat x, const std::vector<int>& frame_width, 
 // a box of a frame of width W as a box of its left-right mirror: (W - x - w, y, w, h)
 inline cv::Rect mirror_box(cv::Rect box, int frame_width) { return cv::Rect(frame_width - box.x - box.width, box.y, box.width, box.height); }
 
+// ---- warped samples (Python: rotation_warp / invert_warp / warp_landmarks).  A warp matrix is 2 x 3 doubles, row-major, mapping a
+// pixel of the virtual frame V to a position in its frame (include/sd_b200.h, sd_sample_warp); every helper computes in double with
+// each operation rounded on its own, in the order of the Python helper, so that both give the same bits.
+using warp_matrix = std::array<double, 6>;
+
+// A sample warp: M over a V of width x height
+inline sd_sample_warp make_warp(const warp_matrix& m, int width, int height)
+{
+    sd_sample_warp w{};
+    for (int k = 0; k < 6; ++k) w.m[k] = m[k];
+    w.width = width;
+    w.height = height;
+    return w;
+}
+
+// The exact algebraic inverse of M; throws when M is singular or not finite
+inline warp_matrix invert_warp(const warp_matrix& m)
+{
+    const double det = m[0] * m[4] - m[1] * m[3];
+    if (det == 0 || !std::isfinite(det)) throw std::runtime_error("invert_warp: the matrix is singular or not finite");
+    const double ia = m[4] / det, ib = -m[1] / det, id = -m[3] / det, ie = m[0] / det;
+    return warp_matrix{ia, ib, -(ia * m[2] + ib * m[5]), id, ie, -(id * m[2] + ie * m[5])};
+}
+
+// The V-to-frame matrix whose V is the frame rotated by angle degrees (counter-clockwise) about (cx, cy) and scaled by scale: the
+// inverse of cv::getRotationMatrix2D(centre, angle, scale).  Its V is what cv::warpAffine with that matrix gives.
+inline warp_matrix rotation_warp(double cx, double cy, double angle, double scale = 1.0)
+{
+    const double a = angle * (3.141592653589793 / 180.0);
+    const double alpha = std::cos(a) * scale, beta = std::sin(a) * scale;
+    return invert_warp(warp_matrix{alpha, beta, (1 - alpha) * cx - beta * cy, -beta, alpha, beta * cx + (1 - alpha) * cy});
+}
+
+// Landmark rows [x_0 .. x_{L-1}, y_0 .. y_{L-1}] (CV_32FC1, one per row) mapped through one matrix (m.size() == 1) or one per row,
+// in double, returned as float: ground truth into a warp's V with invert_warp, results back to the frame with the warp.
+inline cv::Mat warp_landmarks(cv::Mat x, const std::vector<warp_matrix>& m)
+{
+    const int L = x.cols / 2;
+    if (x.cols != 2 * L || L < 1 || m.empty() || (m.size() != 1 && static_cast<int>(m.size()) != x.rows))
+        throw std::runtime_error("warp_landmarks: x must be N x 2L and m 1 or N long");
+    cv::Mat out(x.rows, x.cols, CV_32FC1);
+    for (int r = 0; r < x.rows; ++r) {
+        const warp_matrix& w = m[m.size() == 1 ? 0 : r];
+        for (int l = 0; l < L; ++l) {
+            const double px = x.at<float>(r, l), py = x.at<float>(r, L + l);
+            out.at<float>(r, l) = static_cast<float>(w[0] * px + w[1] * py + w[2]);
+            out.at<float>(r, L + l) = static_cast<float>(w[3] * px + w[4] * py + w[5]);
+        }
+    }
+    return out;
+}
+
 class InterEyeDistanceNormalisation {
 public:
     InterEyeDistanceNormalisation() = default;
@@ -208,6 +260,32 @@ public:
             throw std::runtime_error("detect: initialisations must be one 1 x 2L row per face");
         const cv::Mat x0 = initialisations.isContinuous() ? initialisations : initialisations.clone();
         return detect_faces(images, face_image, nullptr, x0.ptr<float>(0));
+    }
+
+    // Warped faces (sd_detect_faces_device_warped): face i is a face of the virtual frame V_i = cv::warpAffine(grey
+    // images[face_image[i]], warps[i].m, (warps[i].width, warps[i].height), INTER_LINEAR | WARP_INVERSE_MAP) (rcr::make_warp,
+    // rcr::rotation_warp); its box and its landmarks are in V_i's coordinates, bit for bit detect() on V_i.  The frames are
+    // uploaded once (sd_upload_frames) and V_i is never built.  Returns one 1 x 2L row per face.
+    std::vector<cv::Mat> detect(const std::vector<cv::Mat>& images, const std::vector<int>& face_image, const std::vector<cv::Rect>& faceboxes,
+                                const std::vector<sd_sample_warp>& warps)
+    {
+        if (face_image.size() != faceboxes.size()) throw std::runtime_error("detect: face_image / faceboxes size mismatch");
+        const cv::Mat mean = get_mean();
+        cv::Mat x0(static_cast<int>(faceboxes.size()), mean.cols, CV_32FC1);
+        for (size_t i = 0; i < faceboxes.size(); ++i) {
+            const cv::Mat row = align_mean(mean, faceboxes[i]);
+            std::memcpy(x0.ptr<float>(static_cast<int>(i)), row.ptr<float>(0), sizeof(float) * mean.cols);
+        }
+        return detect_warped(images, face_image, x0, warps);
+    }
+
+    std::vector<cv::Mat> detect(const std::vector<cv::Mat>& images, const std::vector<int>& face_image, cv::Mat initialisations,
+                                const std::vector<sd_sample_warp>& warps)
+    {
+        const int P = 2 * sd_model_num_landmarks(handle.get());
+        if (initialisations.rows != static_cast<int>(face_image.size()) || initialisations.cols != P)
+            throw std::runtime_error("detect: initialisations must be one 1 x 2L row per face");
+        return detect_warped(images, face_image, initialisations.isContinuous() ? initialisations : initialisations.clone(), warps);
     }
 
     // One tracking step (sd_track_faces; the rule is in include/sd_b200.h): track t lies in images[face_frame[t]] and had the
@@ -359,6 +437,35 @@ public:
 private:
     friend detection_model load_detection_model(std::string filename);
     // sd_detect_faces_host: frames stay in host memory (Mat::step() is the row stride), landmarks come back in face order
+    std::vector<cv::Mat> detect_warped(const std::vector<cv::Mat>& images, const std::vector<int>& face_image, const cv::Mat& x0,
+                                       const std::vector<sd_sample_warp>& warps)
+    {
+        const size_t n = face_image.size();
+        if (warps.size() != n) throw std::runtime_error("detect: warps needs one entry per face");
+        std::vector<cv::Mat> out;
+        if (n == 0) return out;
+        for (int f : face_image)
+            if (f < 0 || f >= static_cast<int>(images.size())) throw std::runtime_error("detect: a face refers to a frame that is not in the list");
+        sd_ctx* ctx = sd_b200::context();
+        const int P = 2 * sd_model_num_landmarks(handle.get());
+        sd_b200::DeviceBuffer frames, didx(n * sizeof(int32_t)), dw(n * sizeof(sd_sample_warp)), dx0(n * P * sizeof(float)),
+            dout(n * P * sizeof(float));
+        const sd_image_batch batch = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), frames, "detect upload");
+        const std::vector<int32_t> idx(face_image.begin(), face_image.end());
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, didx.as<int32_t>(), idx.data(), n * sizeof(int32_t)), "detect");
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, dw.as<sd_sample_warp>(), warps.data(), n * sizeof(sd_sample_warp)), "detect");
+        sd_b200::check(ctx, sd_memcpy_h2d(ctx, dx0.as<float>(), x0.ptr<float>(0), n * P * sizeof(float)), "detect");
+        sd_b200::check(ctx, sd_detect_faces_device_warped(ctx, handle.get(), &batch, didx.as<int32_t>(), dw.as<sd_sample_warp>(), dx0.as<float>(),
+                                                          static_cast<int>(n), dout.as<float>()), "sd_detect_faces_device_warped");
+        const cv::Mat all = sd_b200::download(dout.as<float>(), static_cast<int>(n), P, P);
+        for (size_t i = 0; i < n; ++i) {
+            cv::Mat row(1, P, CV_32FC1);
+            std::memcpy(row.ptr<float>(0), all.ptr<float>(static_cast<int>(i)), sizeof(float) * P);
+            out.push_back(row);
+        }
+        return out;
+    }
+
     std::vector<cv::Mat> detect_faces(const std::vector<cv::Mat>& images, const std::vector<int>& face_image, const int32_t* boxes, const float* x0)
     {
         sd_ctx* ctx = sd_b200::context();
