@@ -339,26 +339,24 @@ def bgr2gray(images, ctx: Optional["Context"] = None) -> torch.Tensor:
 
 def _device_images(images, ctx: Context):
     """The images of a HogTransform -> (the device tensor that owns them, the ImageBatchC sd_hog_batch reads).  A CUDA tensor
-    (count, H, W) is used in place and (count, H, W, 3) converted by bgr2gray; a host (count, H, W) array or tensor is copied
-    in one piece.  Anything else from the host -- a list of (H, W) or (H, W, 3) frames of any sizes, or a (count, H, W, 3)
-    array -- is uploaded by sd_upload_frames."""
-    dev = f"cuda:{ctx.device}"
-    if isinstance(images, (list, tuple)):
-        frames = list(images)
-    else:
-        t = _tensor(images)
-        if t.dim() == 2:
-            t = t.unsqueeze(0)
-        if t.dtype != torch.uint8 or not (t.dim() == 3 or (t.dim() == 4 and t.shape[3] == 3)):
+    (count, H, W) is used in place (copied first when it is not contiguous) and (count, H, W, 3) converted by bgr2gray; a host
+    (count, H, W) array or tensor is copied in one piece.  Anything else from the host -- a list of (H, W) or (H, W, 3) frames of any sizes, or a (count, H, W, 3)
+    array -- is uploaded by sd_upload_frames (_grey_frames)."""
+    if not isinstance(images, (list, tuple)):
+        images = _tensor(images)
+        if images.dim() == 2:
+            images = images.unsqueeze(0)
+        if images.dtype != torch.uint8 or not (images.dim() == 3 or (images.dim() == 4 and images.shape[3] == 3)):
             raise ValueError("images must be (count, H, W) uint8, (count, H, W, 3) uint8, or a list of such frames of any sizes")
-        if t.is_cuda or t.dim() == 3:
-            t = t.to(dev)
-            t = (bgr2gray(t, ctx) if t.dim() == 4 else t).contiguous()
-            n, h, w = t.shape
-            return t, ImageBatchC(C.c_void_p(t.data_ptr()), w, h, t.stride(1), t.stride(0), n)
-        frames = list(t)
-    recs, keep = _host_frames(frames)                       # keep: the bytes stay alive until the upload returns
-    return _upload_host_frames(recs, ctx)
+        if images.dim() == 3:       # grey: from the host in one copy, however many frames; on the device, contiguous
+            images = images.to(f"cuda:{ctx.device}").contiguous()
+        elif images.is_cuda:
+            images = bgr2gray(images, ctx)
+    keep, ib, _ = _grey_frames(images, ctx, lambda w, h: None)
+    if ib is None:
+        # no frames: sd_upload_frames refuses an empty batch, so this call always raises its SdError
+        return _upload_host_frames([], ctx)
+    return keep, ib
 
 
 def _upload_host_frames(recs, ctx: Context):

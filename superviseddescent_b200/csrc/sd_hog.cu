@@ -1010,19 +1010,10 @@ int sd_bgr2gray_images(sd_ctx* ctx, const sd_hog_images* bgr, void* d_buf, size_
     const int count = bgr->count;
     HogPyramidFrames fr;
     if (const int rc = sd_hog_read_image_frames(ctx, __func__, bgr, 0, &fr)) return rc;
-    // sd_upload_frames' layout: grey frames at a 16-byte pitch, back to back, then the descriptors when the sizes differ
     std::vector<sd_frame> desc(count);
     bool uniform = true;
-    size_t gray = 0;
-    int max_h = 0;
-    for (int i = 0; i < count; ++i) {
-        const sd_hog_image& f = fr.frames[i];
-        desc[i] = sd_frame{f.width, f.height, (int32_t)sd_round16(f.width), 0, (int64_t)gray};
-        gray += (size_t)f.height * sd_round16(f.width);
-        uniform = uniform && f.width == fr.frames[0].width && f.height == fr.frames[0].height;
-        max_h = std::max(max_h, f.height);
-    }
-    const size_t need = gray + (uniform ? 0 : (size_t)count * sizeof(sd_frame));
+    const size_t gray = sd_gray_layout(fr.frames.data(), count, desc.data(), &uniform);
+    const size_t need = gray + (uniform ? 0 : (size_t)count * sizeof(sd_frame));   // the descriptors follow the grey frames
     if (!d_buf) {
         *bytes = need;
         return SD_OK;
@@ -1030,25 +1021,18 @@ int sd_bgr2gray_images(sd_ctx* ctx, const sd_hog_images* bgr, void* d_buf, size_
     SD_REQUIRE(ctx, out && sd_aligned(d_buf, 16) && *bytes >= need,
                "d_buf must be 16-byte aligned and hold the size the query gives; out must not be NULL");
     uint8_t* base = static_cast<uint8_t*>(d_buf);
-    const sd_frame* d_desc = uniform ? nullptr : reinterpret_cast<const sd_frame*>(base + gray);
+    const sd_image_batch ib = sd_gray_batch(base, desc.data(), count, uniform, reinterpret_cast<const sd_frame*>(base + gray));
     if (!uniform)
         SD_CUDA(ctx, cudaMemcpyAsync(base + gray, desc.data(), (size_t)count * sizeof(sd_frame), cudaMemcpyHostToDevice, ctx->stream));
+    int max_h = 0;
+    for (const sd_frame& d : desc) max_h = std::max(max_h, d.height);
     const unsigned rows = (unsigned)std::min(max_h, 1024);
     for (int f0 = 0; f0 < count; f0 += 65535) {
         const dim3 grid(rows, (unsigned)std::min(count - f0, 65535));
         bgr2gray_images_kernel<<<grid, 128, 0, ctx->stream>>>(static_cast<const uint8_t*>(bgr->d_data), bgr->d_frames, bgr->frame,
-                                                             bgr->image_stride, f0, base, d_desc, (long long)desc[0].row_stride * desc[0].height,
+                                                             bgr->image_stride, f0, base, ib.d_frames, (long long)desc[0].row_stride * desc[0].height,
                                                              desc[0].row_stride);
         SD_LAUNCH_CHECK(ctx, "bgr2gray_images_kernel");
-    }
-    sd_image_batch ib{};
-    ib.d_data = base;
-    ib.count = count;
-    if (uniform) {
-        ib.width = desc[0].width; ib.height = desc[0].height; ib.row_stride = desc[0].row_stride;
-        ib.image_stride = (int64_t)desc[0].row_stride * desc[0].height;
-    } else {
-        ib.d_frames = d_desc;
     }
     *out = ib;
     return SD_OK;

@@ -394,6 +394,41 @@ inline size_t sd_round16(size_t v) { return (v + 15) & ~(size_t)15; }
 // grey bytes of a frame at a 16-byte pitch: no region of it is larger
 inline size_t sd_gray_bytes(const sd_host_frame& f) { return (size_t)f.height * sd_round16(f.width); }
 
+// The grey batch layout of sd_upload_frames and sd_bgr2gray_images (and of detect's staging chunks): grey rows at a 16-byte
+// pitch, frames back to back from offset 0.  Equally sized frames are then a plain strided batch, which the HOG kernel stages
+// by TMA; otherwise each frame is read through its sd_frame descriptor, and the entry points place the descriptor table right
+// after the frames.  frames: n records with width and height (sd_host_frame, sd_hog_image).  Fills desc[0..n) and returns the
+// grey bytes; *uniform: all frames share one size.
+template <class Frame>
+size_t sd_gray_layout(const Frame* frames, int n, sd_frame* desc, bool* uniform)
+{
+    size_t off = 0;
+    *uniform = true;
+    for (int i = 0; i < n; ++i) {
+        const Frame& f = frames[i];
+        desc[i] = sd_frame{f.width, f.height, (int32_t)sd_round16(f.width), 0, (int64_t)off};
+        off += (size_t)f.height * desc[i].row_stride;
+        *uniform = *uniform && f.width == frames[0].width && f.height == frames[0].height;
+    }
+    return off;
+}
+
+// The batch sd_hog_batch reads for frames laid out by sd_gray_layout at d_gray; d_desc: the device copy of desc (read only when
+// the sizes differ).
+inline sd_image_batch sd_gray_batch(const uint8_t* d_gray, const sd_frame* desc, int n, bool uniform, const sd_frame* d_desc)
+{
+    sd_image_batch ib{};
+    ib.d_data = d_gray;
+    ib.count = n;
+    if (uniform) {
+        ib.width = desc[0].width; ib.height = desc[0].height; ib.row_stride = desc[0].row_stride;
+        ib.image_stride = (int64_t)desc[0].row_stride * desc[0].height;
+    } else {
+        ib.d_frames = d_desc;
+    }
+    return ib;
+}
+
 #ifdef __CUDACC__
 // The last index i in [lo, hi] whose start(i) <= t, for starts that ascend with i and start(lo) <= t: the grid, map or level that
 // work item t of a flattened launch belongs to.  start is the caller's load of a table entry.

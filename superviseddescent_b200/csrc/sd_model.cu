@@ -344,39 +344,7 @@ namespace {
 
 size_t bgr_bytes(const sd_host_frame& f) { return f.channels == 3 ? (size_t)f.height * sd_round16(3 * (size_t)f.width) : 0; }
 
-// ---- host frames -> grey device frames (sd_detect_faces_host's chunks, sd_upload_frames) --------------------------------
-// The device layout: grey rows at a 16-byte pitch, frames back to back from offset 0.  Equally sized frames are then a plain
-// strided batch, which the HOG kernel stages by TMA; otherwise each frame is read through its sd_frame descriptor.
-// Fills desc[0..n) and returns the grey bytes; *uniform: all frames share one size.
-size_t frame_layout(const sd_host_frame* frames, int n, sd_frame* desc, bool* uniform)
-{
-    size_t off = 0;
-    *uniform = true;
-    for (int i = 0; i < n; ++i) {
-        const sd_host_frame& f = frames[i];
-        desc[i] = sd_frame{f.width, f.height, (int32_t)sd_round16(f.width), 0, (int64_t)off};
-        off += sd_gray_bytes(f);
-        *uniform = *uniform && f.width == frames[0].width && f.height == frames[0].height;
-    }
-    return off;
-}
-
-// The batch sd_hog_batch reads for frames laid out by frame_layout at d_gray; d_desc: the device copy of desc (read only when
-// the sizes differ).
-sd_image_batch gray_batch(const uint8_t* d_gray, const sd_frame* desc, int n, bool uniform, const sd_frame* d_desc)
-{
-    sd_image_batch ib{};
-    ib.d_data = d_gray;
-    ib.count = n;
-    if (uniform) {
-        ib.width = desc[0].width; ib.height = desc[0].height; ib.row_stride = desc[0].row_stride;
-        ib.image_stride = (int64_t)desc[0].row_stride * desc[0].height;
-    } else {
-        ib.d_frames = d_desc;
-    }
-    return ib;
-}
-
+// ---- host frames -> grey device frames (sd_detect_faces_host's chunks, sd_upload_frames), laid out by sd_gray_layout -----
 // Copies frames[0..n) to the layout desc describes at d_gray, on the copy stream once free_ev (recorded on the compute stream:
 // nothing still reads the destination or d_bgr) has completed.  Grey frames go straight to their place; colour frames go as
 // B,G,R rows at a 16-byte pitch, back to back from d_bgr (bgr_bytes each), and the compute stream converts them into place
@@ -445,7 +413,7 @@ int detect_faces_full(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frame
     std::vector<char> uniform(nc);
     for (int c = 0; c < nc; ++c) {
         bool same = true;
-        bgr_at[c] = frame_layout(fr.data() + chunk_first[c], chunk_first[c + 1] - chunk_first[c], desc.data() + chunk_first[c], &same);
+        bgr_at[c] = sd_gray_layout(fr.data() + chunk_first[c], chunk_first[c + 1] - chunk_first[c], desc.data() + chunk_first[c], &same);
         uniform[c] = same;
     }
     std::vector<int> face_first(chunk_first.size(), count);   // first sorted face of each chunk
@@ -482,7 +450,7 @@ int detect_faces_full(sd_ctx* ctx, const sd_model* m, const sd_host_frame* frame
         uint8_t* stage = (uint8_t*)ctx->d_stage[buf];
         rc = upload_frames(ctx, fr.data() + u0, desc.data() + u0, u1 - u0, stage, stage + bgr_at[c], ctx->stage_done[buf], ctx->stage_ev[buf]);
         if (rc) return rc;
-        const sd_image_batch ib = gray_batch(stage, desc.data() + u0, u1 - u0, uniform[c], d_desc + u0);
+        const sd_image_batch ib = sd_gray_batch(stage, desc.data() + u0, u1 - u0, uniform[c], d_desc + u0);
         const int k0 = face_first[c], n = face_first[c + 1] - k0;
         rc = detect_device(ctx, m, &ib, d_idx + k0, d_x + (size_t)k0 * P, n, d_out + (size_t)k0 * P);
         if (rc) return rc;
@@ -940,7 +908,7 @@ int sd_upload_frames(sd_ctx* ctx, const sd_host_frame* frames, int count, void* 
     }
     std::vector<sd_frame> desc(count);
     bool uniform = true;
-    const size_t gray = frame_layout(frames, count, desc.data(), &uniform);
+    const size_t gray = sd_gray_layout(frames, count, desc.data(), &uniform);
     const size_t need = gray + (uniform ? 0 : (size_t)count * sizeof(sd_frame));   // the descriptors follow the grey frames
     if (!d_buf) { *bytes = need; return SD_OK; }
     SD_REQUIRE(ctx, out && (reinterpret_cast<uintptr_t>(d_buf) & 15) == 0 && *bytes >= need,
@@ -962,7 +930,7 @@ int sd_upload_frames(sd_ctx* ctx, const sd_host_frame* frames, int count, void* 
     if (!uniform)
         SD_CUDA(ctx, cudaMemcpyAsync(base + gray, desc.data(), (size_t)count * sizeof(sd_frame), cudaMemcpyHostToDevice, ctx->stream));
     SD_CUDA(ctx, cudaStreamSynchronize(ctx->stream));        // the caller may free or reuse the host frames
-    *out = gray_batch(base, desc.data(), count, uniform, reinterpret_cast<const sd_frame*>(base + gray));
+    *out = sd_gray_batch(base, desc.data(), count, uniform, reinterpret_cast<const sd_frame*>(base + gray));
     return SD_OK;
 }
 

@@ -140,36 +140,47 @@ inline sd_hog_images upload_interleaved(sd_ctx* ctx, const std::vector<cv::Mat>&
     return batch;
 }
 
-// 8UC1 or 8UC3 (B,G,R) frames, all of one type, on the device with their channels kept (upload_interleaved)
-inline sd_hog_images upload_channels(sd_ctx* ctx, const std::vector<cv::Mat>& images, sd_b200::DeviceBuffer& buf,
-                                     sd_b200::DeviceBuffer& table, const char* what, std::vector<sd_hog_image>* desc_out = nullptr)
+// The flags of a sliding-window call (vl_hog_pyramid, train_hog_filter, hog_box_scores, the tracking steps): bilinear_orientations
+// and float_frames need multichannel.  Throws std::runtime_error naming what.
+inline void check_window_flags(bool multichannel, bool bilinear_orientations, bool float_frames, const char* what)
 {
-    for (const cv::Mat& m : images)
-        if (m.type() != images[0].type() || (m.type() != CV_8UC1 && m.type() != CV_8UC3))
-            throw std::runtime_error(std::string(what) + ": frames must be all CV_8UC1 or all CV_8UC3");
-    return upload_interleaved(ctx, images, 1, SD_HOG_U8, buf, table, what, desc_out);
+    if (bilinear_orientations && !multichannel) throw std::runtime_error(std::string(what) + ": bilinear_orientations needs multichannel");
+    if (float_frames && !multichannel) throw std::runtime_error(std::string(what) + ": float_frames needs multichannel");
 }
 
-// 32FC1 or 32FC3 frames, all of one type, on the device as float channels (upload_interleaved), for the float pyramid
-inline sd_hog_images upload_float_channels(sd_ctx* ctx, const std::vector<cv::Mat>& images, sd_b200::DeviceBuffer& buf,
-                                           sd_b200::DeviceBuffer& table, const char* what)
+// The frames of a sliding-window call on the device: grey or colour as the call's flags select.
+struct WindowFrames {
+    sd_image_batch grey{};              // without multichannel
+    sd_hog_images colour{};             // with multichannel
+    sd_b200::DeviceBuffer buf, table;
+};
+
+// Checks the flags (check_window_flags) and uploads.  Without multichannel the frames (8UC1 / 8UC3 B,G,R) become the grey batch
+// (upload_grey).  With it they keep their channels (upload_interleaved, which fills *desc_out if given): all CV_8UC1 or all
+// CV_8UC3, or with float_frames all CV_32FC1 or all CV_32FC3.  Throws std::runtime_error naming what where either refuses.
+inline void upload_window_frames(sd_ctx* ctx, const std::vector<cv::Mat>& images, bool multichannel, bool bilinear_orientations,
+                                 bool float_frames, WindowFrames& out, const char* what, std::vector<sd_hog_image>* desc_out = nullptr)
 {
+    check_window_flags(multichannel, bilinear_orientations, float_frames, what);
+    if (!multichannel) {
+        out.grey = upload_grey(ctx, sd_b200::host_frames(images), out.buf, what);
+        return;
+    }
+    const int type1 = float_frames ? CV_32FC1 : CV_8UC1, type3 = float_frames ? CV_32FC3 : CV_8UC3;
     for (const cv::Mat& m : images)
-        if (m.type() != images[0].type() || (m.type() != CV_32FC1 && m.type() != CV_32FC3))
-            throw std::runtime_error(std::string(what) + ": float frames must be all CV_32FC1 or all CV_32FC3");
-    return upload_interleaved(ctx, images, sizeof(float), SD_HOG_F32, buf, table, what);
+        if (m.type() != images[0].type() || (m.type() != type1 && m.type() != type3))
+            throw std::runtime_error(std::string(what) + (float_frames ? ": float frames must be all CV_32FC1 or all CV_32FC3"
+                                                                       : ": frames must be all CV_8UC1 or all CV_8UC3"));
+    out.colour = upload_interleaved(ctx, images, float_frames ? sizeof(float) : 1, float_frames ? SD_HOG_F32 : SD_HOG_U8, out.buf,
+                                    out.table, what, desc_out);
 }
 
-// The frames of a tracking step and of hog_box_scores: colour, the frames the filter reads, as vl_hog_pyramid uploads them
-// (multichannel: upload_channels; float_frames: upload_float_channels), and grey, the cascade's grey batch.  Without
-// multichannel both are the grey upload (upload_grey).  With it the grey frames are *grey_images (8UC1 / 8UC3, the sizes of
-// images) when given; else 8UC3 frames are converted on the device (sd_bgr2gray_images, so a colour frame is uploaded once)
-// and 8UC1 frames are read in place; float frames need grey_images.
-struct TrackFrames {
-    bool multichannel = false;
-    sd_image_batch grey{};
-    sd_hog_images colour{};
-    sd_b200::DeviceBuffer buf, table, grey_buf;
+// The frames of a tracking step: colour, the frames the filter reads, and grey, the cascade's grey batch.  Without multichannel
+// grey is the window frames' grey batch.  With it the grey frames are *grey_images (8UC1 / 8UC3, the sizes of images) when
+// given; else 8UC3 frames are converted on the device (sd_bgr2gray_images, so a colour frame is uploaded once) and 8UC1 frames
+// are read in place; float frames need grey_images.
+struct TrackFrames : WindowFrames {
+    sd_b200::DeviceBuffer grey_buf;
 };
 
 // sd_bgr2gray_images' size for frames of these sizes, by the layout include/sd_b200.h states (sd_upload_frames'): no read-back
@@ -188,17 +199,11 @@ inline void upload_track_frames(sd_ctx* ctx, const std::vector<cv::Mat>& images,
                                 bool float_frames, const std::vector<cv::Mat>* grey_images, TrackFrames& out, const char* what)
 {
     const std::string w(what);
-    if (bilinear_orientations && !multichannel) throw std::runtime_error(w + ": bilinear_orientations needs multichannel");
-    if (float_frames && !multichannel) throw std::runtime_error(w + ": float_frames needs multichannel");
+    check_window_flags(multichannel, bilinear_orientations, float_frames, what);
     if (grey_images && !multichannel) throw std::runtime_error(w + ": grey_images needs multichannel (grey frames are the cascade's)");
-    out.multichannel = multichannel;
-    if (!multichannel) {
-        out.grey = upload_grey(ctx, sd_b200::host_frames(images), out.buf, what);
-        return;
-    }
     std::vector<sd_hog_image> desc;
-    out.colour = float_frames ? upload_float_channels(ctx, images, out.buf, out.table, what)
-                              : upload_channels(ctx, images, out.buf, out.table, what, &desc);
+    upload_window_frames(ctx, images, multichannel, bilinear_orientations, float_frames, out, what, &desc);
+    if (!multichannel) return;
     if (grey_images) {
         if (grey_images->size() != images.size()) throw std::runtime_error(w + ": grey_images needs one frame per frame");
         out.grey = upload_grey(ctx, sd_b200::host_frames(*grey_images), out.grey_buf, what);
@@ -473,8 +478,7 @@ inline std::vector<std::vector<cv::Mat>> vl_hog_pyramid(const std::vector<cv::Ma
 {
     if (images.empty()) return {};
     if (scales.empty()) throw std::runtime_error("vl_hog_pyramid: no scales");
-    if (bilinear_orientations && !multichannel) throw std::runtime_error("vl_hog_pyramid: bilinear_orientations needs multichannel");
-    if (float_frames && !multichannel) throw std::runtime_error("vl_hog_pyramid: float_frames needs multichannel");
+    hog_batch::check_window_flags(multichannel, bilinear_orientations, float_frames, "vl_hog_pyramid");
     sd_ctx* ctx = sd_b200::context();
     const int n = static_cast<int>(images.size()), S = static_cast<int>(scales.size());
     hog_batch::Results res;
@@ -486,20 +490,16 @@ inline std::vector<std::vector<cv::Mat>> vl_hog_pyramid(const std::vector<cv::Ma
                                          " or the configuration is invalid: scales in (0, 4], cell_size 1..32, num_bins 1..16");
             res.add(dd * h, w);
         }
-    sd_b200::DeviceBuffer buf, table;
-    if (float_frames) {
-        const sd_hog_images batch = hog_batch::upload_float_channels(ctx, images, buf, table, "vl_hog_pyramid upload");
-        sd_b200::check(ctx, sd_hog_pyramid_float(ctx, &batch, scales.data(), S, cell_size, num_bins, variant, bilinear_orientations ? 1 : 0,
-                                                 res.out(), res.offsets(ctx, "vl_hog_pyramid")), "sd_hog_pyramid_float");
-    } else if (multichannel) {
-        const sd_hog_images batch = hog_batch::upload_channels(ctx, images, buf, table, "vl_hog_pyramid upload");
-        sd_b200::check(ctx, sd_hog_pyramid_images(ctx, &batch, scales.data(), S, cell_size, num_bins, variant, bilinear_orientations ? 1 : 0,
-                                                  res.out(), res.offsets(ctx, "vl_hog_pyramid")), "sd_hog_pyramid_images");
-    } else {
-        const sd_image_batch batch = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), buf, "vl_hog_pyramid upload");
-        sd_b200::check(ctx, sd_hog_pyramid(ctx, &batch, scales.data(), S, cell_size, num_bins, variant, res.out(),
+    hog_batch::WindowFrames fr;
+    hog_batch::upload_window_frames(ctx, images, multichannel, bilinear_orientations, float_frames, fr, "vl_hog_pyramid upload");
+    if (multichannel)
+        sd_b200::check(ctx, (float_frames ? sd_hog_pyramid_float : sd_hog_pyramid_images)(
+                                ctx, &fr.colour, scales.data(), S, cell_size, num_bins, variant, bilinear_orientations ? 1 : 0, res.out(),
+                                res.offsets(ctx, "vl_hog_pyramid")),
+                       float_frames ? "sd_hog_pyramid_float" : "sd_hog_pyramid_images");
+    else
+        sd_b200::check(ctx, sd_hog_pyramid(ctx, &fr.grey, scales.data(), S, cell_size, num_bins, variant, res.out(),
                                            res.offsets(ctx, "vl_hog_pyramid")), "sd_hog_pyramid");
-    }
     const std::vector<cv::Mat> levels = res.download();
     std::vector<std::vector<cv::Mat>> out;
     for (int i = 0; i < n; ++i) out.emplace_back(levels.begin() + static_cast<size_t>(i) * S, levels.begin() + static_cast<size_t>(i + 1) * S);
@@ -870,15 +870,10 @@ inline hog_filter train_hog_filter(const std::vector<cv::Mat>& images, const std
     if (images.empty()) throw std::runtime_error("train_hog_filter: no frames");
     if (box_frame.size() != boxes.size()) throw std::runtime_error("train_hog_filter: box_frame and boxes differ in length");
     if (params.rounds < 0 || params.max_negatives < 1) throw std::runtime_error("train_hog_filter: rounds < 0 or max_negatives < 1");
-    if (bilinear_orientations && !multichannel) throw std::runtime_error("train_hog_filter: bilinear_orientations needs multichannel");
-    if (float_frames && !multichannel) throw std::runtime_error("train_hog_filter: float_frames needs multichannel");
+    hog_batch::check_window_flags(multichannel, bilinear_orientations, float_frames, "train_hog_filter");
     sd_ctx* ctx = sd_b200::context();
-    sd_b200::DeviceBuffer buf, table;
-    sd_image_batch grey{};
-    sd_hog_images colour{};
-    if (float_frames) colour = hog_batch::upload_float_channels(ctx, images, buf, table, "train_hog_filter upload");
-    else if (multichannel) colour = hog_batch::upload_channels(ctx, images, buf, table, "train_hog_filter upload");
-    else grey = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), buf, "train_hog_filter upload");
+    hog_batch::WindowFrames fr;
+    hog_batch::upload_window_frames(ctx, images, multichannel, bilinear_orientations, float_frames, fr, "train_hog_filter upload");
     std::vector<sd_hog_box> hb;
     for (size_t k = 0; k < boxes.size(); ++k)
         hb.push_back(sd_hog_box{box_frame[k], boxes[k].x, boxes[k].y, boxes[k].width, boxes[k].height});
@@ -891,12 +886,12 @@ inline hog_filter train_hog_filter(const std::vector<cv::Mat>& images, const std
     const int nb = static_cast<int>(hb.size()), S = static_cast<int>(scales.size());
     if (multichannel)
         sd_b200::check(ctx, (float_frames ? sd_hog_train_filter_float : sd_hog_train_filter_images)(
-                                ctx, &colour, bilinear_orientations ? 1 : 0, hb.data(), nb, scales.data(), S, cell_size, num_bins, variant,
+                                ctx, &fr.colour, bilinear_orientations ? 1 : 0, hb.data(), nb, scales.data(), S, cell_size, num_bins, variant,
                                 filter_w, filter_h, pad_x, pad_y, &params, d_filter.as<float>(), &out.bias, out.rounds.data(),
                                 out.negatives.data(), &num_negatives),
                        float_frames ? "sd_hog_train_filter_float" : "sd_hog_train_filter_images");
     else
-        sd_b200::check(ctx, sd_hog_train_filter(ctx, &grey, hb.data(), nb, scales.data(), S, cell_size, num_bins, variant, filter_w, filter_h,
+        sd_b200::check(ctx, sd_hog_train_filter(ctx, &fr.grey, hb.data(), nb, scales.data(), S, cell_size, num_bins, variant, filter_w, filter_h,
                                                 pad_x, pad_y, &params, d_filter.as<float>(), &out.bias, out.rounds.data(),
                                                 out.negatives.data(), &num_negatives), "sd_hog_train_filter");
     out.negatives.resize(static_cast<size_t>(num_negatives));
@@ -915,8 +910,7 @@ inline std::vector<float> hog_box_scores(const std::vector<cv::Mat>& images, con
                                          const cv::Mat& filter, float bias, VlHogVariant variant, int cell_size, int num_bins,
                                          bool multichannel = false, bool bilinear_orientations = false, bool float_frames = false)
 {
-    if (bilinear_orientations && !multichannel) throw std::runtime_error("hog_box_scores: bilinear_orientations needs multichannel");
-    if (float_frames && !multichannel) throw std::runtime_error("hog_box_scores: float_frames needs multichannel");
+    hog_batch::check_window_flags(multichannel, bilinear_orientations, float_frames, "hog_box_scores");
     if (images.empty()) throw std::runtime_error("hog_box_scores: no frames");
     if (box_frame.size() != boxes.size()) throw std::runtime_error("hog_box_scores: box_frame and boxes differ in length");
     const int dd = sd_b200::hog_dimension(variant, num_bins);
@@ -926,12 +920,9 @@ inline std::vector<float> hog_box_scores(const std::vector<cv::Mat>& images, con
     std::vector<float> out(n);
     if (n == 0) return out;
     sd_ctx* ctx = sd_b200::context();
-    sd_b200::DeviceBuffer buf, d_frames, d_filter, d_boxes(static_cast<size_t>(n) * 5 * sizeof(int32_t)), d_scores(static_cast<size_t>(n) * sizeof(float));
-    sd_image_batch batch{};
-    sd_hog_images colour{};
-    if (float_frames) colour = hog_batch::upload_float_channels(ctx, images, buf, d_frames, "hog_box_scores upload");
-    else if (multichannel) colour = hog_batch::upload_channels(ctx, images, buf, d_frames, "hog_box_scores upload");
-    else batch = hog_batch::upload_grey(ctx, sd_b200::host_frames(images), buf, "hog_box_scores upload");
+    sd_b200::DeviceBuffer d_filter, d_boxes(static_cast<size_t>(n) * 5 * sizeof(int32_t)), d_scores(static_cast<size_t>(n) * sizeof(float));
+    hog_batch::WindowFrames fr;
+    hog_batch::upload_window_frames(ctx, images, multichannel, bilinear_orientations, float_frames, fr, "hog_box_scores upload");
     sd_b200::upload(filter, d_filter, filter.cols);
     std::vector<int32_t> table(static_cast<size_t>(n) * 5);   // [frame indices | boxes]
     for (int k = 0; k < n; ++k) {
@@ -941,11 +932,11 @@ inline std::vector<float> hog_box_scores(const std::vector<cv::Mat>& images, con
     }
     sd_b200::check(ctx, sd_memcpy_h2d(ctx, d_boxes.as<int32_t>(), table.data(), table.size() * sizeof(int32_t)), "hog_box_scores");
     if (multichannel)
-        sd_b200::check(ctx, sd_hog_box_scores_images(ctx, &colour, bilinear_orientations ? 1 : 0, d_boxes.as<int32_t>(), d_boxes.as<int32_t>() + n,
+        sd_b200::check(ctx, sd_hog_box_scores_images(ctx, &fr.colour, bilinear_orientations ? 1 : 0, d_boxes.as<int32_t>(), d_boxes.as<int32_t>() + n,
                                                      n, d_filter.as<float>(), filter.cols, filter.rows / dd, bias, cell_size, num_bins, variant,
                                                      d_scores.as<float>()), "sd_hog_box_scores_images");
     else
-        sd_b200::check(ctx, sd_hog_box_scores(ctx, &batch, d_boxes.as<int32_t>(), d_boxes.as<int32_t>() + n, n, d_filter.as<float>(), filter.cols,
+        sd_b200::check(ctx, sd_hog_box_scores(ctx, &fr.grey, d_boxes.as<int32_t>(), d_boxes.as<int32_t>() + n, n, d_filter.as<float>(), filter.cols,
                                               filter.rows / dd, bias, cell_size, num_bins, variant, d_scores.as<float>()), "sd_hog_box_scores");
     sd_b200::check(ctx, sd_memcpy_d2h(ctx, out.data(), d_scores.as<float>(), out.size() * sizeof(float)), "hog_box_scores");
     sd_b200::check(ctx, sd_sync(ctx), "hog_box_scores");

@@ -545,9 +545,9 @@ inline face_chip_set face_chips(const std::vector<cv::Mat>& images, const std::v
     sd_ctx* ctx = sd_b200::context();
     const int type = images[0].type();
     const bool is_float = type == CV_32FC1 || type == CV_32FC3;
-    sd_b200::DeviceBuffer buf, table;
-    const sd_hog_images frames = is_float ? hog_batch::upload_float_channels(ctx, images, buf, table, "face_chips upload")
-                                          : hog_batch::upload_channels(ctx, images, buf, table, "face_chips upload");
+    hog_batch::WindowFrames fr;
+    hog_batch::upload_window_frames(ctx, images, true, false, is_float, fr, "face_chips upload");
+    const sd_hog_images& frames = fr.colour;
     const size_t chip_bytes = static_cast<size_t>(chip_width) * chip_height * frames.channels * (is_float ? sizeof(float) : 1);
     const size_t rows = static_cast<size_t>(n > 0 ? n : 1), P = 2 * static_cast<size_t>(L);
     sd_b200::DeviceBuffer d_frame(rows * sizeof(int32_t)), d_lms(rows * P * sizeof(float)), d_chips(chip_bytes * rows),

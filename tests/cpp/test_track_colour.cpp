@@ -124,6 +124,9 @@ int main(int argc, char** argv)
         }
         try { model.track(frames, face, previous, filter, VlHogVariantUoctti, cs, K, threshold, false, true); ++failures; std::printf("bilinear without multichannel not refused\n"); }
         catch (const std::runtime_error&) {}
+        // hog_box_scores refuses the flags before anything else, with no boxes too
+        try { rcr::hog_box_scores(frames, {}, {}, filter.filter, filter.bias, VlHogVariantUoctti, cs, K, false, true); ++failures; std::printf("hog_box_scores: bilinear without multichannel not refused\n"); }
+        catch (const std::runtime_error&) {}
     } catch (const std::exception& e) {
         std::printf("exception: %s\n", e.what());
         return 1;
